@@ -77,12 +77,12 @@ constexpr int kTilePixels = 256;    // fp32 kernel
 constexpr int kTcTilePixels = 128;  // tensor-core kernel
 // resident CTAs (one warpgroup and ~47 KB of shared memory each) per SM of the tensor-core kernel
 constexpr int kTcCtasPerSm = 4;
-// tensor-core partial: rows = accumulator rows that carry data (32 code-h, 32 code-l, 7 + 1 pose-h, 7 + 1 pose-l),
-// columns = B features (32 code, 7 pose/residual, 1 pad)
-constexpr int kTcRows = 80;
-constexpr int kTcCols = 40;
-// stored column-major with the row dimension padded to 96 (rows 80-95 are never read)
-constexpr int kTcRowsPad = 96;
+// tensor-core partial: the kernel's 64 x 56 accumulator D = A B^T, A rows = code-l 0-23 | code-h 0-31 | pose-h (7 + 1),
+// B columns = code-h 0-31 | pose-h (7 + 1) | code-l 24-31 | pose-l (7 + 1); see dfk_sfm_tc.cu for what each block holds
+constexpr int kTcRows = 64;
+constexpr int kTcCols = 56;
+// stored column-major ([column][row]); rows 0-23 of columns 40-55 (the dropped l*l terms) are never written or read
+constexpr int kTcRowsPad = kTcRows;
 constexpr int kTcPartialFloats = kTcRowsPad * kTcCols + 8;
 
 struct SfmLaunchPlan {

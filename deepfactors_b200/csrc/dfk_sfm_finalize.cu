@@ -14,7 +14,7 @@
 //
 // Two partial formats:
 //   fp32 kernel : G itself, row-major NFP x NFP (features: code 0..C-1, a C..C+5, r C+6), upper blocks valid
-//   tensor core : D = [h rows ; l rows] x h columns (kTcRows x kTcCols, stored column-major);  G = HH + LH + LH^T
+//   tensor core : D = A x B^T over split-tf32 h / l rows (kTcRows x kTcCols, stored column-major);  G = HH + LH + LH^T
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -29,9 +29,10 @@ constexpr int kFinUnroll = 4;
 
 __device__ __forceinline__ int packed_index(int i, int j, int NP) { return i * NP - (i * (i - 1)) / 2 + (j - i); }
 
-// partial row of the h / l part of feature f (tensor-core partial), C = 32
-__device__ __forceinline__ int tc_hrow(int f) { return f < 32 ? f : 64 + (f - 32); }
-__device__ __forceinline__ int tc_lrow(int f) { return f < 32 ? 32 + f : 72 + (f - 32); }
+// tensor-core partial (C = 32, column-major D of dfk_sfm_tc.cu), features f = code 0-31 | pose/residual 32-39:
+//   HH[i][j] = D[24 + i][j];  LH[i][j] = D[i][j] for i < 24, D[24 + j][16 + i] for i >= 24
+__device__ __forceinline__ int tc_hh(int i, int j) { return j * kTcRowsPad + 24 + i; }
+__device__ __forceinline__ int tc_lh(int i, int j) { return i < 24 ? j * kTcRowsPad + i : (16 + i) * kTcRowsPad + 24 + j; }
 
 template <int C, bool TC>
 __global__ void __launch_bounds__(kFinWarps * 32)
@@ -83,9 +84,9 @@ sfm_finalize_kernel(const SfmItemDev* __restrict__ items, const float* __restric
       fj = 0;
     }
     if constexpr (TC) {
-      off[q][0] = fj * kTcRowsPad + tc_hrow(fi);  // HH[i][j]   (partials are column-major: [col][row])
-      off[q][1] = fj * kTcRowsPad + tc_lrow(fi);  // LH[i][j]
-      off[q][2] = fi * kTcRowsPad + tc_lrow(fj);  // LH[j][i]
+      off[q][0] = tc_hh(fi, fj);  // HH[i][j]
+      off[q][1] = tc_lh(fi, fj);  // LH[i][j]
+      off[q][2] = tc_lh(fj, fi);  // LH[j][i]
     } else {
       off[q][0] = fi * NFP + fj;
     }

@@ -14,22 +14,26 @@
 //   memory, COALESCED (lane = 16-byte chunk lane&7 of pixel 4i + lane/8), scales them by the pixel's s (one shuffle),
 //   splits them into h / l and stores them K-major (pixels along K) into the CTA's operand buffer; each thread adds
 //   its own pixel's 7 pose / residual values.  Invalid pixels contribute exact zeros.  After one CTA barrier the
-//   warpgroup issues 16 x (wgmma.m64n48k8 + wgmma.m64n8k8) (K = 8 pixels each) and, without waiting, goes on with the
-//   next tile's gathers; it waits for the MMAs only before it overwrites the operand buffer.
+//   warpgroup issues 16 x wgmma.m64n56k8 (K = 8 pixels each) and, without waiting, goes on with the next tile's
+//   gathers; it waits for the MMAs only before it overwrites the operand buffer.
 //
-//   Operand buffer: 10 groups of 8 feature rows -- 0-3 code-l, 4-7 code-h, 8 pose-h (features 0-6, row 7 zero), 9 pose-l.
+//   Operand buffer: 10 groups of 8 feature rows --
+//     0-2 code-l 0-23 | 3-6 code-h 0-31 | 7 pose-h (features 0-6, row 7 zero) | 8 code-l 24-31 | 9 pose-l.
 //   Inside a group, the core matrix of pixels 4q..4q+3 sits at q * kLbo, feature row r of it at r * 16.  kLbo and kSbo
-//   carry 16 bytes of padding each, so the stores of a warp hit 32 different banks.
-//     accumulator 1 = A1 x B1: A1 = groups 0-7 (M = 64: code-l, code-h), B1 = groups 4-9 (N = 48: code-h, pose-h, pose-l).
-//       Besides HH and LH of the code rows it gives code-h x pose-l = (LH of the pose-l rows)^T; only the code-l x pose-l
-//       block (the dropped l*l terms) is unused.
-//     accumulator 2 = A2 x B2: A2 = groups 2-9 (M = 64), B2 = group 8 (N = 8: pose-h).  Only rows 48-63 (pose-h, pose-l:
-//       the 8 x 8 pose block of HH and LH) are used; wgmma has no M below 64, and at N = 8 the unused rows cost 1/7 of
-//       the tile's MMA work.
-//   The accumulators live in registers (24 + 4 floats per thread).  A chain is cut every kFlushTiles tiles and at item
+//   carry 16 bytes of padding each, so the code-h and pose stores of a warp hit 32 different banks (the code-l stores
+//   of groups 0 and 8 share banks: 2-way).
+//     D = A x B^T, A = groups 0-7 (M = 64: code-l 0-23, then all 40 h rows), B = groups 3-9 (N = 56: all 40 h rows, then
+//     code-l 24-31 and pose-l).  Both are contiguous, so one descriptor stride serves each.  With the 40 features
+//     f = code 0-31 | pose/residual 32-39:  HH[i][j] = D[24 + i][j];  LH[i][j] = D[i][j] for i < 24 and
+//     D[24 + j][16 + i] for i >= 24.  Only D[0-23][40-55] (l*l terms) is unused.
+//   The accumulator lives in registers (28 floats per thread).  A chain is cut every kFlushTiles tiles and at item
 //   boundaries: its fragments are added in round-to-nearest fp32 to the CTA's partial in global memory (single writer
-//   per address, program order), in the partial layout the finalize kernel reads (rows 0-31 code-h, 32-63 code-l,
-//   64-71 pose-h, 72-79 pose-l; columns 0-31 code, 32-39 pose).
+//   per address, program order), which is D itself, column-major (the finalize kernel reads it).
+//
+//   Input stream: the code-Jacobian rows, img0 and dpt0 are read once, through loads that do not allocate in L1 (L1 is
+//   left to the bilinear gathers of img1 / grad1, the only loads that reuse lines; the fused depth decode reads the code
+//   rows a first time through L1, so that the Gram's second read hits there).  Nothing is prefetched: on H100
+//   both a per-thread L2 prefetch of the pixel's code row and bulk L2 prefetches of a later tile made the kernel slower.
 //
 // The static tile->CTA assignment, the in-item tile permutation, the per-CTA partials and the wide deterministic
 // finalize are those of the fp32 kernel.
@@ -134,8 +138,30 @@ __device__ __forceinline__ void sts32(uint32_t addr, float v)
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v));
 }
 
+// read-once input stream (code-Jacobian rows, img0, dpt0): read-only path, no L1 allocation
+__device__ __forceinline__ float ld_stream(const float* p)
+{
+  float v;
+  asm("ld.global.nc.L1::no_allocate.f32 %0, [%1];" : "=f"(v) : "l"(p));
+  return v;
+}
+
 // 16 bytes of a code-Jacobian row; rows of items without the BULK flag are only 4-byte aligned
 __device__ __forceinline__ float4 load_chunk(const float* __restrict__ p, bool aligned16)
+{
+  if (aligned16) {
+    float4 v;
+    asm("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"
+        : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+        : "l"(p));
+    return v;
+  }
+  return make_float4(ld_stream(p), ld_stream(p + 1), ld_stream(p + 2), ld_stream(p + 3));
+}
+
+// the same 16 bytes through L1: the fused depth decode reads every chunk the Gram reads again a little later (the
+// no-allocate loads of load_chunk still hit lines that are in L1)
+__device__ __forceinline__ float4 load_chunk_l1(const float* __restrict__ p, bool aligned16)
 {
   if (aligned16) return __ldg(reinterpret_cast<const float4*>(p));
   return make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), __ldg(p + 3));
@@ -174,18 +200,16 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_items, int num_
   const uint32_t op = smem_u32(sm.op);
   // code-Jacobian stores: this lane holds features 4c..4c+3 of pixel 4 i8 + r of the warp's 32 pixels
   const int c = lane & 7, r = lane >> 3;
-  const uint32_t code_l = op + (uint32_t)(c >> 1) * kSbo + (uint32_t)(8 * warp) * kLbo + (uint32_t)(c & 1) * 64u +
-                          (uint32_t)r * 4u;
-  const uint32_t code_h = code_l + 4u * kSbo;
+  const uint32_t in_group = (uint32_t)(8 * warp) * kLbo + (uint32_t)(c & 1) * 64u + (uint32_t)r * 4u;
+  const uint32_t code_l = op + (uint32_t)((c >> 1) < 3 ? (c >> 1) : 8) * kSbo + in_group;
+  const uint32_t code_h = op + (uint32_t)(3 + (c >> 1)) * kSbo + in_group;
   // pose stores: this thread's own pixel
-  const uint32_t pose_h = op + 8u * kSbo + (uint32_t)(8 * warp + (lane >> 2)) * kLbo + (uint32_t)(lane & 3) * 4u;
-  const uint32_t pose_l = pose_h + kSbo;
+  const uint32_t pose_h = op + 7u * kSbo + (uint32_t)(8 * warp + (lane >> 2)) * kLbo + (uint32_t)(lane & 3) * 4u;
+  const uint32_t pose_l = pose_h + 2u * kSbo;
 
-  float acc1[24], acc2[4];
+  float acc[28];
 #pragma unroll
-  for (int q = 0; q < 24; ++q) acc1[q] = 0.0f;  // never read before a chain's first MMA overwrites them
-#pragma unroll
-  for (int q = 0; q < 4; ++q) acc2[q] = 0.0f;
+  for (int q = 0; q < 28; ++q) acc[q] = 0.0f;  // never read before a chain's first MMA overwrites them
   ItemSmem& I = sm.item[warp];
   int it = 0;
   int cur_item = -1;
@@ -203,22 +227,11 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_items, int num_
     if (fresh || chain_valid > 0) {
       const int m0 = 16 * warp + (lane >> 2);
 #pragma unroll
-      for (int q = 0; q < 24; ++q) {
+      for (int q = 0; q < 28; ++q) {
         const int m = m0 + 8 * ((q >> 1) & 1);
         const int n = 8 * (q >> 2) + 2 * (lane & 3) + (q & 1);
-        const float v = chain_valid > 0 ? acc1[q] : 0.0f;
-        if (n < 40)
-          put_partial(P + n * kTcRowsPad + ((m + 32) & 63), v, fresh);
-        else if (warp >= 2)  // code-h row m - 32 x pose-l column: LH of pose-l row n - 40, code column m - 32
-          put_partial(P + (m - 32) * kTcRowsPad + 72 + (n - 40), v, fresh);
-      }
-      if (warp == 3) {  // rows 48-55 pose-h, 56-63 pose-l x pose-h columns -> partial rows 64-79, columns 32-39
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int m = m0 + 8 * ((q >> 1) & 1);
-          const int n = 2 * (lane & 3) + (q & 1);
-          put_partial(P + (32 + n) * kTcRowsPad + m + 16, chain_valid > 0 ? acc2[q] : 0.0f, fresh);
-        }
+        if (n < 40 || m >= 24)  // D[0-23][40-55] holds only l*l terms
+          put_partial(P + n * kTcRowsPad + m, chain_valid > 0 ? acc[q] : 0.0f, fresh);
       }
     }
     if (item_end && tid == 0) reinterpret_cast<unsigned int*>(P)[kTcRowsPad * kTcCols] = inliers;
@@ -270,13 +283,10 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_items, int num_
     float feat[8];
     bool ok = false;
     if (blk_live) {
-#ifndef DFK_TC_NOPREFETCH
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(jac + joff));
-#endif
       const float xn = __ldg(I.ray_tab + pxx);
       const float yn = __ldg(I.ray_tab + W + py);
-      float d = __ldg(I.dpt0 + (size_t)py * I.dpt0_pitch + pxx);
-      const float i0 = __ldg(I.img0 + (size_t)py * I.img0_pitch + pxx);
+      float d = ld_stream(I.dpt0 + (size_t)py * I.dpt0_pitch + pxx);
+      const float i0 = ld_stream(I.img0 + (size_t)py * I.img0_pitch + pxx);
       if (fused) {
         // dpt0 is prx_orig: decode the depth from the pixel's code-Jacobian row -- same arithmetic as
         // update_depth_kernel (chunk fma chains, then the xor-butterfly over the 8 chunk sums, here ACROSS the 8
@@ -286,7 +296,7 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_items, int num_
 #pragma unroll
         for (int i8 = 0; i8 < 8; ++i8) {
           const uint32_t offk = __shfl_sync(0xffffffffu, joff, 4 * i8 + (lane >> 3));
-          float p = chunk_dot(load_chunk(jac + offk + 4 * (lane & 7), a16), cc);
+          float p = chunk_dot(load_chunk_l1(jac + offk + 4 * (lane & 7), a16), cc);
           p = __fadd_rn(p, __shfl_xor_sync(0xffffffffu, p, 4));
           p = __fadd_rn(p, __shfl_xor_sync(0xffffffffu, p, 2));
           p = __fadd_rn(p, __shfl_xor_sync(0xffffffffu, p, 1));
@@ -362,10 +372,10 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_items, int num_
       for (int kk = 0; kk < TILE / 8; ++kk) {
         const uint32_t k_off = (uint32_t)kk * 2u * kLbo;
         const bool accumulate = kk > 0 || chain_valid > 0;
-        wgmma_m64n48k8_tf32(acc1, make_wgmma_desc_kmajor(op + k_off, kLbo, kSbo),
-                            make_wgmma_desc_kmajor(op + 4u * kSbo + k_off, kLbo, kSbo), accumulate);
-        wgmma_m64n8k8_tf32(acc2, make_wgmma_desc_kmajor(op + 2u * kSbo + k_off, kLbo, kSbo),
-                           make_wgmma_desc_kmajor(op + 8u * kSbo + k_off, kLbo, kSbo), accumulate);
+#ifndef DFK_EXP_NOMMA  // experiment (wrong results): no MMA at all
+        wgmma_m64n56k8_tf32(acc, make_wgmma_desc_kmajor(op + k_off, kLbo, kSbo),
+                            make_wgmma_desc_kmajor(op + 3u * kSbo + k_off, kLbo, kSbo), accumulate);
+#endif
       }
       wgmma_commit();
     }

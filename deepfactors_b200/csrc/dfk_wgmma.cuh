@@ -1,5 +1,5 @@
 // dfk_wgmma.cuh -- inline-PTX wrappers for the Hopper warpgroup tensor-core path (sm_90a): the shared-memory matrix
-// descriptor, wgmma.mma_async m64n48k8 / m64n8k8 kind tf32 with both operands in shared memory, and the wgmma fences.
+// descriptor, wgmma.mma_async m64n56k8 kind tf32 with both operands in shared memory, and the wgmma fences.
 // Field layouts follow the PTX ISA chapter "Asynchronous Warpgroup Level Matrix Multiply-Accumulate".
 #pragma once
 
@@ -27,35 +27,24 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// D = A * B^T (+ D iff `accumulate`).  D 64 x N fp32 in registers (the warpgroup's accumulator fragment, N / 2 floats per
-// thread), A 64 x 8 and B N x 8 tf32 in shared memory (K-major).  Fragment: d[4 j + 2 h + b] holds row
+// D = A * B^T (+ D iff `accumulate`).  D 64 x 56 fp32 in registers (the warpgroup's accumulator fragment, 28 floats per
+// thread), A 64 x 8 and B 56 x 8 tf32 in shared memory (K-major).  Fragment: d[4 j + 2 h + b] holds row
 // 16 * warp + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + b.
-__device__ __forceinline__ void wgmma_m64n48k8_tf32(float (&d)[24], uint64_t a_desc, uint64_t b_desc, bool accumulate)
+__device__ __forceinline__ void wgmma_m64n56k8_tf32(float (&d)[28], uint64_t a_desc, uint64_t b_desc, bool accumulate)
 {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %26, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, "
-      "%24, %25, p, 1, 1;\n\t"
+      "setp.ne.b32 p, %30, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n56k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27}, "
+      "%28, %29, p, 1, 1;\n\t"
       "}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
         "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
-        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-      : "l"(a_desc), "l"(b_desc), "r"((uint32_t)accumulate)
-      : "memory");
-}
-
-__device__ __forceinline__ void wgmma_m64n8k8_tf32(float (&d)[4], uint64_t a_desc, uint64_t b_desc, bool accumulate)
-{
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n8k8.f32.tf32.tf32 {%0, %1, %2, %3}, %4, %5, p, 1, 1;\n\t"
-      "}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27])
       : "l"(a_desc), "l"(b_desc), "r"((uint32_t)accumulate)
       : "memory");
 }
