@@ -47,15 +47,17 @@ struct DfkContext {
   size_t items_cap = 0;
   float* partials_dev = nullptr;
   size_t partials_cap = 0;  // floats
-  // normalised ray tables of the tensor-core kernel: they depend on (fx, u0, width, fy, v0, height) only, so they are
+  // normalised ray tables of the RunStep kernels: they depend on (fx, u0, width, fy, v0, height) only, so they are
   // built once per camera level and reused by every later call (one launch less per evaluation in steady state)
   struct RayTab {
     float fx, fy, u0, v0;
     uint32_t w, h;
     float* dev;
+    bool built;  // the table kernel has been enqueued for it (an entry whose call failed before that stays false)
   };
   std::vector<RayTab> ray_cache;
-  bool ray_miss = false;  // build_items found a camera without a table: run the table kernel this call
+  std::vector<size_t> ray_pending;  // entries the current call uses that are not built yet: run the table kernel
+  bool ray_flush = false;           // a call missed on a full cache: empty it when the next call starts
   float* codes_dev = nullptr;  // fused depth decode: code_size floats per work item
   size_t codes_cap = 0;
   std::vector<float> codes_host;
@@ -295,9 +297,16 @@ cudaError_t ensure(T** ptr, size_t* cap, size_t need)
 }
 
 DfkStatus build_items(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_size, int tile_px, int max_ctas,
-                      bool want_ray_tabs, const float* codes_dev, SfmLaunchPlan* plan)
+                      const float* codes_dev, SfmLaunchPlan* plan)
 {
-  h->ray_miss = false;
+  h->ray_pending.clear();
+  // a caller cycling through more camera levels than the cache holds: start over (cudaFree synchronises).  Only here,
+  // between calls, so that no item of a call is left pointing at a freed table
+  if (h->ray_flush) {
+    for (auto& r : h->ray_cache) cudaFree(r.dev);
+    h->ray_cache.clear();
+    h->ray_flush = false;
+  }
   const DfkDenseSfmParams& sp = h->params.sfmparams;
   h->items_host.resize(n);
   uint32_t tile_cursor = 0;
@@ -346,26 +355,20 @@ DfkStatus build_items(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_
     }
     d.width = W; d.height = H; d.num_pixels = W * H;
     d.num_tiles = (d.num_pixels + tile_px - 1) / tile_px;
-    d.ray_tab = nullptr;
-    if (want_ray_tabs) {
-      for (const auto& r : h->ray_cache)
-        if (r.fx == d.fx && r.fy == d.fy && r.u0 == d.u0 && r.v0 == d.v0 && r.w == W && r.h == H) {
-          d.ray_tab = r.dev;
-          break;
-        }
-      if (!d.ray_tab) {
-        if (h->ray_cache.size() >= 256) {  // a caller cycling through cameras: start over (cudaFree synchronises)
-          for (auto& r : h->ray_cache) cudaFree(r.dev);
-          h->ray_cache.clear();
-        }
-        DfkContext::RayTab r{d.fx, d.fy, d.u0, d.v0, W, H, nullptr};
-        if (cudaMalloc((void**)&r.dev, sizeof(float) * ((size_t)W + H)) != cudaSuccess)
-          return fail(h, DFK_ERR_CUDA, "[SfmAligner::RunStep] scratch allocation failed");
-        h->ray_cache.push_back(r);
-        d.ray_tab = r.dev;
-        h->ray_miss = true;
-      }
+    size_t rt = 0;
+    for (const auto& r : h->ray_cache) {
+      if (r.fx == d.fx && r.fy == d.fy && r.u0 == d.u0 && r.v0 == d.v0 && r.w == W && r.h == H) break;
+      ++rt;
     }
+    if (rt == h->ray_cache.size()) {
+      if (rt >= 256) h->ray_flush = true;
+      DfkContext::RayTab r{d.fx, d.fy, d.u0, d.v0, W, H, nullptr, false};
+      if (cudaMalloc((void**)&r.dev, sizeof(float) * ((size_t)W + H)) != cudaSuccess)
+        return fail(h, DFK_ERR_CUDA, "[SfmAligner::RunStep] scratch allocation failed");
+      h->ray_cache.push_back(r);
+    }
+    d.ray_tab = h->ray_cache[rt].dev;
+    if (!h->ray_cache[rt].built) h->ray_pending.push_back(rt);
     d.tile_begin = tile_cursor;
     tile_cursor += d.num_tiles;
     d.perm_mul = perm_multiplier(d.num_tiles);
@@ -388,7 +391,6 @@ DfkStatus build_items(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_
   // which CTAs touch which item (CTA c owns global tiles [c*T/G, (c+1)*T/G))
   uint32_t partial_cursor = 0;
   int c = 0;
-  int max_per_item = 0;
   for (int i = 0; i < n; ++i) {
     SfmItemDev& d = h->items_host[i];
     const long long tb = d.tile_begin, te = tb + d.num_tiles;
@@ -399,10 +401,8 @@ DfkStatus build_items(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_
     d.num_ctas = (uint32_t)(last - first + 1);
     d.partial_begin = partial_cursor;
     partial_cursor += d.num_ctas;
-    max_per_item = std::max(max_per_item, (int)d.num_ctas);
   }
   plan->num_partials = (int)partial_cursor;
-  plan->max_ctas_per_item = max_per_item;
   return DFK_OK;
 }
 
@@ -475,8 +475,7 @@ DfkStatus run_batch(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_si
   }
   const int ctas_per_sm = tc ? kTcCtasPerSm : (wide ? 1 : sfm_fp32_ctas_per_sm(code_size));
   const int sms = (h->sm_limit > 0 && h->sm_limit < h->num_sms) ? h->sm_limit : h->num_sms;
-  DfkStatus st = build_items(h, items, n, code_size, tile_px, ctas_per_sm * sms,
-                             tc, h->codes_dev, &plan);
+  DfkStatus st = build_items(h, items, n, code_size, tile_px, ctas_per_sm * sms, h->codes_dev, &plan);
   if (st != DFK_OK) return st;
   if (any_fused)
     DFK_CUDA(h, cudaMemcpyAsync(h->codes_dev, h->codes_host.data(), sizeof(float) * (size_t)n * code_size,
@@ -489,20 +488,24 @@ DfkStatus run_batch(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_si
   DFK_CUDA(h, cudaMemcpyAsync(h->items_dev, h->items_host.data(), sizeof(SfmItemDev) * n, cudaMemcpyHostToDevice,
                               h->stream),
            "[SfmAligner::RunStep] work list upload failed");
+  if (!h->ray_pending.empty()) {  // the work list names a camera level the handle has no built table for yet
+    DFK_CUDA(h, launch_sfm_ray_tables(h->items_dev, n, h->stream), "[SfmAligner::RunStep] kernel launch failed");
+    for (size_t rt : h->ray_pending) h->ray_cache[rt].built = true;  // on the stream ahead of every later reader
+    h->launches += 1;
+  }
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   if (h->profiling) {
     DfkStatus ps = profile_events(h, &ev0, &ev1);
     if (ps != DFK_OK) return ps;
   }
   if (tc) {
-    DFK_CUDA(h, launch_sfm_tc(h->items_dev, plan, h->ray_miss, h->partials_dev, h->stream, ev0, ev1),
+    DFK_CUDA(h, launch_sfm_tc(h->items_dev, plan, h->partials_dev, h->stream, ev0, ev1),
              "[SfmAligner::RunStep] kernel launch failed");
-    if (h->ray_miss) h->launches += 1;  // ray-table kernel
   } else if (wide) {
     DFK_CUDA(h, launch_sfm_wide(code_size, h->items_dev, plan, h->partials_dev, h->stream, ev0, ev1),
              "[SfmAligner::RunStep] kernel launch failed");
   } else {
-    DFK_CUDA(h, launch_sfm_fp32(code_size, h->items_dev, plan, h->partials_dev, records_dev, h->stream, ev0, ev1),
+    DFK_CUDA(h, launch_sfm_fp32(code_size, h->items_dev, plan, h->partials_dev, h->stream, ev0, ev1),
              "[SfmAligner::RunStep] kernel launch failed");
   }
   DFK_CUDA(h, launch_sfm_finalize(code_size, tc, h->items_dev, n, h->partials_dev, records_dev, h->stream),

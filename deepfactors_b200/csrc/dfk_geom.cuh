@@ -74,12 +74,6 @@ __device__ __forceinline__ Warped warp_ray(float xn, float yn, float d, const fl
   return w;
 }
 
-struct Bilin {
-  int off;  // iy * pitch + ix (in pixels of the sampled image's own pitch unit)
-  int ix, iy;
-  float fu, fv;
-};
-
 __device__ __forceinline__ void bilin_setup(float u, float v, int& ix, int& iy, float& fu, float& fv)
 {
   const float flu = floorf(u), flv = floorf(v);

@@ -54,7 +54,6 @@ struct SfmItemDev {
   uint32_t dpt_out_pitch;
   const float* code;
   // normalised ray table of the item's camera level (device memory cached by the handle): xn[0..width), then yn[0..height)
-  // (tensor-core kernel)
   const float* ray_tab;
   // relative-pose Jacobians (warping.h:120-134), row-major 6x6; used by the finalize kernel
   float P0[36];
@@ -90,13 +89,14 @@ struct SfmLaunchPlan {
   int num_tiles = 0;
   int num_ctas = 0;
   int num_partials = 0;
-  int max_ctas_per_item = 0;
 };
 
 // dfk_sfm_fp32.cu
 cudaError_t launch_sfm_fp32(int code_size, const SfmItemDev* items_dev, const SfmLaunchPlan& plan,
-                            float* partials_dev, float* records_dev, cudaStream_t stream,
-                            cudaEvent_t ev_start = nullptr, cudaEvent_t ev_stop = nullptr);
+                            float* partials_dev, cudaStream_t stream, cudaEvent_t ev_start = nullptr,
+                            cudaEvent_t ev_stop = nullptr);
+// dfk_sfm_rays.cu : fills every item's ray_tab (all three RunStep kernels read it)
+cudaError_t launch_sfm_ray_tables(const SfmItemDev* items_dev, int num_items, cudaStream_t stream);
 cudaError_t launch_sfm_finalize(int code_size, bool tc, const SfmItemDev* items_dev, int num_items,
                                 const float* partials_dev, float* records_dev, cudaStream_t stream);
 // dfk_sfm_wide.cu : C = 64 / 128 (thread-owned 8x8 blocks); partial format = the fp32 kernel's
@@ -107,9 +107,8 @@ cudaError_t launch_sfm_wide(int code_size, const SfmItemDev* items_dev, const Sf
                             cudaEvent_t ev_stop = nullptr);
 // dfk_sfm_tc.cu
 bool sfm_tc_supported(int code_size);
-cudaError_t launch_sfm_tc(const SfmItemDev* items_dev, const SfmLaunchPlan& plan, bool build_ray_tables,
-                          float* partials_dev, cudaStream_t stream, cudaEvent_t ev_start = nullptr,
-                          cudaEvent_t ev_stop = nullptr);
+cudaError_t launch_sfm_tc(const SfmItemDev* items_dev, const SfmLaunchPlan& plan, float* partials_dev,
+                          cudaStream_t stream, cudaEvent_t ev_start = nullptr, cudaEvent_t ev_stop = nullptr);
 size_t sfm_partial_floats(int code_size);
 // resident CTAs per SM of the fp32 kernel: at C = 8 a CTA is 11 warps and ~60 KB of shared memory, two fit (the front-end
 // is latency-bound, so the second CTA nearly doubles the throughput); from C = 16 on the register budget allows one

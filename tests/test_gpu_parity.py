@@ -486,6 +486,30 @@ def test_error_reporting_is_loud(torch_mod):
                     dev["prx0_jac"], dev["grad1"])
 
 
+@pytest.mark.parametrize("cs", [8, 32])
+def test_sfm_failed_batch_leaves_no_unbuilt_ray_table(torch_mod, cs):
+    """a call that names a new camera level and then fails on a later item must not leave that level's ray table unbuilt
+    in the handle's cache: the next call on the level equals a fresh handle's, bit for bit"""
+    torch = torch_mod
+    from deepfactors_b200 import _lib
+    from deepfactors_b200.aligners import SfmAligner
+    pair = synth.make_pair(160, 120, cs, 1, seed=71, code_sigma=0.5)
+    L = pair.levels[0]
+    dev = upload_level(torch, L)
+    good = dict(pose0=pair.pose0, pose1=pair.pose1, cam=L.cam,
+                **{k: dev[k] for k in ("img0", "img1", "dpt0", "valid0", "prx0_jac", "grad1")})
+    al = SfmAligner(cs)
+    with pytest.raises(_lib.DfkError):  # img1 smaller than img0: rejected after the first item
+        al.RunStepBatch(al.make_work_items([good, dict(good, img1=dev["img1"][:100])]))
+    va, vb = torch.zeros_like(dev["valid0"]), torch.zeros_like(dev["valid0"])
+    got = al.RunStepBatch(al.make_work_items([dict(good, valid0=va)])).clone()
+    fresh = SfmAligner(cs)
+    want = fresh.RunStepBatch(fresh.make_work_items([dict(good, valid0=vb)])).clone()
+    torch.cuda.synchronize()
+    assert torch.equal(got, want)
+    assert torch.equal(va, vb)
+
+
 @pytest.mark.gpu
 def test_window_assembly_on_device_matches_host_mirror():
     """dfk_window_assemble (deterministic gather over the record buffer of a batch) == factors.WindowBlocks.pack on the

@@ -6,7 +6,7 @@ ROOT=$(cd "$(dirname "$0")/.." && pwd)
 OUT=$ROOT/tools/variants; mkdir -p $OUT/obj_$NAME
 cd $ROOT/deepfactors_b200/csrc
 ARCH="-gencode arch=compute_90a,code=sm_90a"
-for f in dfk_api dfk_sfm_fp32 dfk_sfm_tc dfk_sfm_wide dfk_sfm_finalize dfk_simple dfk_window dfk_depth dfk_sparse; do
+for f in dfk_api dfk_sfm_fp32 dfk_sfm_tc dfk_sfm_wide dfk_sfm_rays dfk_sfm_finalize dfk_simple dfk_window dfk_depth dfk_sparse; do
   if [ "$f" = "dfk_sfm_tc" ] || [ ! -f $OUT/obj_$NAME/$f.o ] || [ $f.cu -nt $OUT/obj_$NAME/$f.o ]; then
     if [ "$f" = "dfk_sfm_tc" ]; then X="$EXTRA"; else X=""; fi
     nvcc $ARCH -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -I../../include -I. $X -c $f.cu -o $OUT/obj_$NAME/$f.o &
