@@ -106,6 +106,7 @@ SYMBOLS = {
     "dfk_window_assemble": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dfk_se3_run_step": (C.c_int, [_H, _F, _CAM, _IMG, _IMG, _IMG, _IMG, _F, _F, _F, C.POINTER(C.c_uint64)]),
     "dfk_se3_track": (C.c_int, [_H, _F, C.POINTER(DfkTrackLevel), C.c_int, _F, _F, _F, _F, C.c_int]),
+    "dfk_se3_track_batch": (C.c_int, [_H, C.c_int, C.c_int, _F, C.POINTER(DfkTrackLevel), _F, _F, _F]),
     "dfk_se3_warp": (C.c_int, [_H, _F, _CAM, _IMG, _IMG, _IMG, _IMG, _F, C.POINTER(C.c_uint64)]),
     "dfk_depth_run_step": (C.c_int, [_H, _F, C.c_int, _IMG, _IMG, _IMG, _F, _F, _F, C.POINTER(C.c_uint64)]),
     "dfk_reprojection_linearize": (C.c_int, [_H, _F, _F, _F, C.c_int, _CAM, _IMG, _IMG, C.c_int, _F, _F, C.c_float,

@@ -512,6 +512,90 @@ class CameraTracker:
         self.history_ = hist[:total] if keep_history else None
         return pose
 
+    def TrackFrameBatch(self, keyframes, pyr_img1, pyr_grad1, poses_ck=None):
+        """The live frame (pyr_img1, pyr_grad1) tracked against every keyframe of `keyframes` at once
+        (dfk_se3_track_batch): one launch per Gauss-Newton iteration for all of them, one read-back.  `keyframes` is a
+        sequence of (pyr_img, pyr_dpt[, pose_wk]); `poses_ck` [N, 7] are the start poses, identity for every keyframe when
+        omitted (what Reset does before each TrackFrame in Relocalize / DetectLoop).  Keyframe n gives bit for bit what
+        SetKeyframe(keyframe n) + TrackFrame from poses_ck[n] gives.  Returns (poses_ck [N, 7], inlier_fractions [N],
+        errors [N]); the tracker's own keyframe, pose and statistics are left alone."""
+        poses = batch_start_poses(keyframes, self.config_.pyramid_levels, poses_ck)
+        n, L = poses.shape[0], self.config_.pyramid_levels
+        if len(pyr_img1) < L or len(pyr_grad1) < L:
+            raise ValueError(f"the live frame needs {L} pyramid levels")
+        self._hd.use_torch_stream()
+        levels = (DfkTrackLevel * (n * L))()
+        for k, kf in enumerate(keyframes):
+            for l in range(L):
+                lv = levels[k * L + l]
+                lv.cam = _cam(self.camera_pyr_[l])
+                lv.img0 = _image(kf[0][l])
+                lv.img1 = _image(pyr_img1[l])
+                lv.dpt0 = _image(kf[1][l])
+                lv.grad1 = _image(pyr_grad1[l], 2)
+                lv.iterations = int(self.config_.iterations_per_level[l])
+        frac = np.zeros(n, dtype=np.float32)
+        err = np.zeros(n, dtype=np.float32)
+        F = C.POINTER(C.c_float)
+        check(self._hd.h, lib().dfk_se3_track_batch(self._hd.h, n, L, poses.ctypes.data_as(F), levels,
+                                                    frac.ctypes.data_as(F), err.ctypes.data_as(F), None))
+        return poses, frac, err
+
+    def Relocalize(self, keyframes, pyr_img1, pyr_grad1):
+        """DeepFactors::Relocalize (core/deepfactors.cpp:713-743): track the live frame against every keyframe from
+        identity, keep the first keyframe with the strictly smallest error; when no error is finite, the first keyframe
+        at its own pose_wk (pose_ck = identity).  `keyframes` as in TrackFrameBatch; all of them are tracked in one
+        batched call.  Afterwards the tracker's keyframe is the winner and pose_ck_ its tracked pose, so the next
+        TrackFrame continues from there.  Returns (index, pose_wc, errors).
+
+        One deliberate difference: after the reference's loop GetError() / GetInliers() still hold the LAST keyframe
+        tracked, whichever won; here they report the winner's."""
+        poses, frac, err = self.TrackFrameBatch(keyframes, pyr_img1, pyr_grad1)
+        idx, pose_ck, pose_wc = relocalize_select(err, poses, [kf[2] if len(kf) > 2 else None for kf in keyframes])
+        kf = keyframes[idx]
+        self.kf_ = None  # SetKeyframe without the pose hand-over: pose_ck_ is set directly below
+        self.SetKeyframe(kf[0], kf[1], kf[2] if len(kf) > 2 else None)
+        self.pose_ck_ = pose_ck
+        self.inliers_ = float(frac[idx])
+        self.error_ = float(err[idx])
+        return idx, pose_wc, err
+
+
+def batch_start_poses(keyframes, pyramid_levels: int, poses_ck=None) -> np.ndarray:
+    """Argument checks of CameraTracker.TrackFrameBatch; returns the start poses as a fresh [N, 7] float32 array."""
+    n = len(keyframes)
+    if n < 1 or n > 65535:
+        raise ValueError(f"need 1 to 65535 keyframes, got {n}")
+    for k, kf in enumerate(keyframes):
+        if len(kf) not in (2, 3):
+            raise ValueError(f"keyframe {k} must be (pyr_img, pyr_dpt[, pose_wk])")
+        if len(kf[0]) < pyramid_levels or len(kf[1]) < pyramid_levels:
+            raise ValueError(f"keyframe {k} needs {pyramid_levels} pyramid levels of image and depth")
+    if poses_ck is None:
+        poses = np.tile(np.array([0, 0, 0, 1, 0, 0, 0], dtype=np.float32), (n, 1))
+    else:
+        poses = np.array(poses_ck, dtype=np.float32).reshape(-1, 7) if np.size(poses_ck) == 7 * n else None
+        if poses is None:
+            raise ValueError(f"poses_ck must be {n} x 7 floats")
+    return np.ascontiguousarray(poses)
+
+
+def relocalize_select(errors, poses_ck, poses_wk):
+    """The selection rule of DeepFactors::Relocalize (core/deepfactors.cpp:717-733): the first keyframe whose error is
+    strictly smaller than every earlier one (and than +inf), else keyframe 0 at its own pose_wk with pose_ck = identity.
+    poses_wk[k] may be None (identity).  Returns (index, pose_ck, pose_wc = pose_wk * pose_ck^-1, GetPoseEstimate)."""
+    from . import se3 as _se3
+    best, best_err = 0, float("inf")
+    for k, e in enumerate(np.asarray(errors, dtype=np.float64)):
+        if e < best_err:
+            best, best_err = k, float(e)
+    if best_err == float("inf"):  # nothing tracked: best_pose = keyframe 1's pose_wk in the reference
+        pose_ck = np.array([0, 0, 0, 1, 0, 0, 0], dtype=np.float32)
+    else:
+        pose_ck = np.asarray(poses_ck[best], dtype=np.float32).copy()
+    pose_wk = poses_wk[best] if poses_wk[best] is not None else np.array([0, 0, 0, 1, 0, 0, 0], dtype=np.float32)
+    return best, pose_ck, _se3.compose(np.asarray(pose_wk, np.float32), _se3.inverse(pose_ck))
+
 
 # ------------------------------------------------------------------------------------------- free functions
 _default_handle = {}

@@ -38,6 +38,17 @@ struct DfkContext {
   size_t track_cap = 0;              // floats
   float* track_host = nullptr;       // pinned mirror of track_dev + the last system (32)
   size_t track_host_cap = 0;
+  // dfk_se3_track_batch, apart from the single-problem buffers above so neither path disturbs the other:
+  //   batch_dev  [descriptors L x N (level-major) | poses 8 N | last systems 32 N]  (bytes; one H2D, one D2H per call)
+  //   batch_partials  N x stride x 32 floats,  batch_counters  N self-resetting tickets (zeroed on allocation)
+  unsigned char* batch_dev = nullptr;
+  size_t batch_cap = 0;
+  unsigned char* batch_host = nullptr;  // pinned mirror of batch_dev
+  size_t batch_host_cap = 0;
+  float* batch_partials = nullptr;
+  size_t batch_partials_cap = 0;  // floats
+  unsigned int* batch_counters = nullptr;
+  size_t batch_counters_cap = 0;
 
   float* sparse_dev = nullptr;       // dfk_reprojection_linearize: [query | train | rows | err2]
   size_t sparse_cap = 0;
@@ -587,6 +598,8 @@ DfkStatus dfk_destroy(DfkHandle h)
     cudaFree(h->track_dev);
     cudaFree(h->codes_dev);
     if (h->track_host) cudaFreeHost(h->track_host);
+    cudaFree(h->batch_dev); cudaFree(h->batch_partials); cudaFree(h->batch_counters);
+    if (h->batch_host) cudaFreeHost(h->batch_host);
     cudaFree(h->items_dev); cudaFree(h->partials_dev); cudaFree(h->records_dev);
     for (auto& r : h->ray_cache) cudaFree(r.dev);
     if (h->out_host) cudaFreeHost(h->out_host);
@@ -962,6 +975,113 @@ DfkStatus dfk_se3_track(DfkHandle h, float pose_ck[7], const DfkTrackLevel* leve
     }
     if (last_system) memcpy(last_system, host_sys, sizeof(float) * 29);
     if (history) memcpy(history, h->track_host + 8, sizeof(float) * 36 * (size_t)total_iters);
+    return DFK_OK;
+  } catch (...) {  // std::bad_alloc / std::length_error from host containers must not cross the C ABI
+    return oom(h);
+  }
+}
+
+DfkStatus dfk_se3_track_batch(DfkHandle h, int num_problems, int num_levels, float* poses_ck,
+                              const DfkTrackLevel* levels, float* inlier_fraction, float* error, float* last_systems)
+{
+  try {
+    if (!h) return DFK_ERR_INVALID_ARG;
+    if (!poses_ck || !levels || num_levels <= 0)
+      return fail(h, DFK_ERR_INVALID_ARG, "[CameraTracker::TrackFrame batch] null argument / no pyramid levels");
+    if (num_problems < 1 || num_problems > 65535)  // blockIdx.y of the step kernel is the problem
+      return fail(h, DFK_ERR_INVALID_ARG, "[CameraTracker::TrackFrame batch] number of problems must be in [1, 65535]");
+    const int N = num_problems, L = num_levels;
+    std::vector<Se3TrackDesc> descs((size_t)L * N);  // level-major: a launch reads the N descriptors of its level
+    std::vector<int> level_blocks(L, 0);             // grid width of a level: its largest problem
+    int stride = 1;                                  // partial rows per problem
+    for (int n = 0; n < N; ++n) {
+      for (int l = 0; l < L; ++l) {
+        const DfkTrackLevel& T = levels[(size_t)n * L + l];
+        const uint32_t W = T.img0.width, H = T.img0.height;
+        if (T.iterations < 0 || W == 0 || H == 0 || !img_ok(&T.img0, W, H, 1) || !img_ok(&T.img1, W, H, 1) ||
+            !img_ok(&T.dpt0, W, H, 1) || !img_ok(&T.grad1, W, H, 2) || !cam_ok(&T.cam, W, H))
+          return fail(h, DFK_ERR_INVALID_ARG,
+                      "[CameraTracker::TrackFrame batch] inconsistent image views / camera larger than them / "
+                      "negative iteration count at problem " + std::to_string(n) + " level " + std::to_string(l));
+        // the problems advance in lockstep, one launch per iteration for all of them
+        if (T.iterations != levels[l].iterations)
+          return fail(h, DFK_ERR_INVALID_ARG,
+                      "[CameraTracker::TrackFrame batch] problem " + std::to_string(n) + " has " +
+                          std::to_string(T.iterations) + " iterations at level " + std::to_string(l) +
+                          ", problem 0 has " + std::to_string(levels[l].iterations));
+        Se3TrackDesc& d = descs[(size_t)l * N + n];
+        d.pc = make_pixel_cam(poses_ck + 7 * (size_t)n, &T.cam, 1, 0.0f);  // q/t are overridden by the device pose
+        d.img0 = view_of(&T.img0); d.img1 = view_of(&T.img1); d.dpt0 = view_of(&T.dpt0); d.grad1 = view_of(&T.grad1);
+        d.width = (int)W;
+        d.height = (int)H;
+        d.nblocks = se3_step_blocks((int)W, (int)H);
+        d.grad_aligned = aligned(d.grad1.ptr, 8) && d.grad1.pitch % 2 == 0;
+        level_blocks[l] = std::max(level_blocks[l], d.nblocks);
+        stride = std::max(stride, d.nblocks);
+      }
+    }
+    DeviceGuard guard(h->device);
+    const size_t desc_bytes = (descs.size() * sizeof(Se3TrackDesc) + 15) & ~(size_t)15;
+    const size_t pose_bytes = sizeof(float) * 8 * (size_t)N, out_bytes = sizeof(float) * 32 * (size_t)N;
+    const size_t total = desc_bytes + pose_bytes + out_bytes;
+    DFK_CUDA(h, ensure(&h->batch_dev, &h->batch_cap, total),
+             "[CameraTracker::TrackFrame batch] scratch allocation failed");
+    DFK_CUDA(h, ensure(&h->batch_partials, &h->batch_partials_cap, (size_t)N * stride * 32),
+             "[CameraTracker::TrackFrame batch] scratch allocation failed");
+    if (h->batch_counters_cap < (size_t)N) {
+      DFK_CUDA(h, ensure(&h->batch_counters, &h->batch_counters_cap, (size_t)N),
+               "[CameraTracker::TrackFrame batch] scratch allocation failed");
+      DFK_CUDA(h, cudaMemsetAsync(h->batch_counters, 0, sizeof(unsigned int) * h->batch_counters_cap, h->stream),
+               "[CameraTracker::TrackFrame batch] memset failed");
+    }
+    if (h->batch_host_cap < total) {
+      if (h->batch_host) cudaFreeHost(h->batch_host);
+      h->batch_host = nullptr;
+      h->batch_host_cap = 0;
+      DFK_CUDA(h, cudaMallocHost((void**)&h->batch_host, total),
+               "[CameraTracker::TrackFrame batch] pinned allocation failed");
+      h->batch_host_cap = total;
+    }
+    // one upload: every level's descriptors and the start poses
+    memcpy(h->batch_host, descs.data(), descs.size() * sizeof(Se3TrackDesc));
+    float* host_poses = reinterpret_cast<float*>(h->batch_host + desc_bytes);
+    const float* host_outs = host_poses + 8 * (size_t)N;
+    for (int n = 0; n < N; ++n) {
+      memcpy(host_poses + 8 * (size_t)n, poses_ck + 7 * (size_t)n, sizeof(float) * 7);
+      host_poses[8 * (size_t)n + 7] = 0.0f;
+    }
+    DFK_CUDA(h, cudaMemcpyAsync(h->batch_dev, h->batch_host, desc_bytes + pose_bytes, cudaMemcpyHostToDevice, h->stream),
+             "[CameraTracker::TrackFrame batch] upload failed");
+    const Se3TrackDesc* descs_dev = reinterpret_cast<const Se3TrackDesc*>(h->batch_dev);
+    float* poses_dev = reinterpret_cast<float*>(h->batch_dev + desc_bytes);
+    float* outs_dev = poses_dev + 8 * (size_t)N;
+    DFK_CUDA(h, cudaMemsetAsync(outs_dev, 0, out_bytes, h->stream), "[CameraTracker::TrackFrame batch] memset failed");
+    for (int l = L - 1; l >= 0; --l) {  // coarse to fine (camera_tracker.cpp:48)
+      for (int k = 0; k < levels[l].iterations; ++k) {
+        DFK_CUDA(h, launch_se3_track_batch(descs_dev + (size_t)l * N, N, level_blocks[l], h->se3_huber_delta,
+                                           h->batch_partials, stride, h->batch_counters, outs_dev, poses_dev, h->stream),
+                 "[CameraTracker::TrackFrame batch] kernel launch failed");
+        h->launches += 1;
+      }
+    }
+    // one read-back: final poses and last evaluated systems
+    DFK_CUDA(h, cudaMemcpyAsync(host_poses, poses_dev, pose_bytes + out_bytes, cudaMemcpyDeviceToHost, h->stream),
+             "[CameraTracker::TrackFrame batch] read-back failed");
+    DFK_CUDA(h, cudaStreamSynchronize(h->stream), "[CameraTracker::TrackFrame batch] stream synchronize failed");
+    for (int n = 0; n < N; ++n) {
+      const float* sys = host_outs + 32 * (size_t)n;
+      memcpy(poses_ck + 7 * (size_t)n, host_poses + 8 * (size_t)n, sizeof(float) * 7);
+      // dfk_se3_track's rule: with no level-0 iteration the outputs keep their previous values
+      if (levels[0].iterations > 0) {
+        const DfkTrackLevel& T0 = levels[(size_t)n * L];
+        const uint32_t area = T0.img0.width * T0.img0.height;
+        uint32_t inl = 0;
+        memcpy(&inl, &sys[28], 4);
+        if (inlier_fraction) inlier_fraction[n] = area ? (float)inl / (float)area : 0.0f;
+        if (error) error[n] = inl != 0 ? sys[27] / (float)inl : INFINITY;
+      }
+      if (last_systems) memcpy(last_systems + 29 * (size_t)n, sys, sizeof(float) * 29);
+    }
     return DFK_OK;
   } catch (...) {  // std::bad_alloc / std::length_error from host containers must not cross the C ABI
     return oom(h);

@@ -130,6 +130,21 @@ cudaError_t launch_se3_step(const PixelCam& pc, float huber_delta, int width, in
                             float* out_dev /*29 floats: 21 JtJ, 6 Jtr, res, inliers bits*/, cudaStream_t s,
                             float* pose_dev = nullptr /*tracking mode: pose read from / updated in device memory*/,
                             float* history_dev = nullptr /*36 floats: the 29 above + the pose they were evaluated at*/);
+// One (problem, level) of dfk_se3_track_batch: what launch_se3_step takes for that level, and its block count.
+struct Se3TrackDesc {
+  PixelCam pc;  // q / t are overridden by the problem's device pose
+  View img0, img1, dpt0, grad1;
+  int width, height;
+  int nblocks;       // se3_step_blocks(width, height)
+  int grad_aligned;
+};
+// blocks of se3_step_kernel's grid for a level of this size (the batched kernel gives a problem exactly as many)
+int se3_step_blocks(int width, int height);
+// descs_dev: num_problems descriptors of one level.  Problem n: scratch rows [n * scratch_stride, + nblocks) (32 floats
+// each), counters[n] (zero, self-resetting), outs[32 n .. + 29) the last system, poses[8 n .. + 7) the pose, updated.
+cudaError_t launch_se3_track_batch(const Se3TrackDesc* descs_dev, int num_problems, int max_blocks, float huber_delta,
+                                   float* scratch, int scratch_stride, unsigned int* counters, float* outs, float* poses,
+                                   cudaStream_t s);
 cudaError_t launch_eval_error(const PixelCam& pc, float huber_delta, int width, int height, View img0, View img1,
                               View dpt0, float* scratch, unsigned int* counter, float* out_dev /*2*/, cudaStream_t s);
 cudaError_t launch_warp(const PixelCam& pc, int width, int height, View img0, View img1, View dpt0, float* img2,

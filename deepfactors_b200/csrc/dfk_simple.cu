@@ -28,10 +28,13 @@ constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 
 // Block-level reduction of NV floats + one counter, then last-block finalize.
-// out[0..NV) = sums, out[NV] = counter bits.  scratch: gridDim.x * 32 floats.  NV <= 31.
+// out[0..NV) = sums, out[NV] = counter bits.  scratch: nblocks * 32 floats.  NV <= 31.
+// `block` / `nblocks` are this block's index and the number of blocks that take part (blockIdx.x / gridDim.x for a
+// one-reduction grid; one row of a batched grid otherwise), so every reduction of the same size sums in the same order.
 template <int NV>
-__device__ __forceinline__ bool reduce_finalize(float (&v)[NV], unsigned int cnt, float* __restrict__ scratch,
-                                                unsigned int* __restrict__ counter, float* __restrict__ out)
+__device__ __forceinline__ bool reduce_finalize(float (&v)[NV], unsigned int cnt, int block, int nblocks,
+                                                float* __restrict__ scratch, unsigned int* __restrict__ counter,
+                                                float* __restrict__ out)
 {
   static_assert(NV <= 31, "one scratch row is 32 floats");
   __shared__ float red[kWarps][32];
@@ -52,19 +55,19 @@ __device__ __forceinline__ bool reduce_finalize(float (&v)[NV], unsigned int cnt
       float s = 0.0f;
 #pragma unroll
       for (int w = 0; w < kWarps; ++w) s += red[w][lane];
-      scratch[blockIdx.x * 32 + lane] = s;
+      scratch[block * 32 + lane] = s;
     } else {
       unsigned int c = 0;
 #pragma unroll
       for (int w = 0; w < kWarps; ++w) c += __float_as_uint(red[w][NV]);
-      scratch[blockIdx.x * 32 + NV] = __uint_as_float(c);
+      scratch[block * 32 + NV] = __uint_as_float(c);
     }
   }
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) {
     const unsigned int ticket = atomicAdd(counter, 1u);
-    is_last = (ticket == gridDim.x - 1);
+    is_last = (ticket == (unsigned int)nblocks - 1u);
   }
   __syncthreads();
   if (!is_last) return false;
@@ -73,7 +76,7 @@ __device__ __forceinline__ bool reduce_finalize(float (&v)[NV], unsigned int cnt
   float s = 0.0f;
   unsigned int c = 0;
   if (lane <= NV) {
-    for (int b = warp; b < (int)gridDim.x; b += kWarps) {
+    for (int b = warp; b < nblocks; b += kWarps) {
       const float x = __ldcg(&scratch[b * 32 + lane]);
       if (lane < NV) s += x;
       else c += __float_as_uint(x);
@@ -100,25 +103,18 @@ __device__ __forceinline__ bool reduce_finalize(float (&v)[NV], unsigned int cnt
 }
 
 // ------------------------------------------------------------------------------ SE3 RunStep
-__global__ void __launch_bounds__(kThreads)
-se3_step_kernel(PixelCam pc, float huber_delta, int width, int height, View img0, View img1, View dpt0, View grad1,
-                bool grad_aligned, float* __restrict__ scratch, unsigned int* __restrict__ counter,
-                float* __restrict__ out, float* pose_dev, float* __restrict__ history)
+// The per-pixel body of SE3Aligner::RunStep (lucas_kanade_se3.h:41-77): this thread's pixels first, first + stride, ...
+// of one problem, accumulated into acc (21 JtJ packed upper, 6 Jtr, 1 residual) and the inlier count.  Shared by the
+// single-problem and the batched kernel, so a problem gives the same sums whichever of the two evaluates it.
+__device__ __forceinline__ void se3_accumulate(const PixelCam& pc, float huber_delta, int width, int height, View img0,
+                                               View img1, View dpt0, View grad1, bool grad_aligned, int first,
+                                               int stride, float (&acc)[28], unsigned int& inl)
 {
-  // tracking mode (pose_dev != nullptr): the pose lives in device memory; the last block of the previous launch
-  // updated it, this launch reads it, and its own last block applies the next Gauss-Newton update.
-  if (pose_dev) {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) pc.q[k] = pose_dev[k];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) pc.t[k] = pose_dev[4 + k];
-  }
-  float acc[28];  // 21 JtJ (packed upper), 6 Jtr, 1 residual
 #pragma unroll
   for (int i = 0; i < 28; ++i) acc[i] = 0.0f;
-  unsigned int inl = 0;
+  inl = 0;
   const int area = width * height;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < area; i += gridDim.x * blockDim.x) {
+  for (int i = first; i < area; i += stride) {
     const int y = i / width, x = i - y * width;
     const float d = __ldg(dpt0.ptr + (size_t)y * dpt0.pitch + x);
     const Warped w = warp_pixel((float)x, (float)y, d, pc.q, pc.t, pc.fx, pc.fy, pc.u0, pc.v0, pc.border, pc.ulim,
@@ -149,28 +145,80 @@ se3_step_kernel(PixelCam pc, float huber_delta, int width, int height, View img0
       }
     }
   }
-  const bool last = reduce_finalize<28>(acc, inl, scratch, counter, out);
-  if (pose_dev && last) {
-    __syncthreads();  // out[0..28] was written by warp 0 of this block
-    if (threadIdx.x == 0) {
-      float pose[7];
+}
+
+// Tracking mode: the pose lives in device memory; the last block of the previous launch updated it, this launch
+// reads it, ...
+__device__ __forceinline__ void se3_load_pose(PixelCam& pc, const float* pose_dev)
+{
 #pragma unroll
-      for (int k = 0; k < 7; ++k) pose[k] = pose_dev[k];
-      if (history) {  // [29 system | 7 pose the system was evaluated at]
+  for (int k = 0; k < 4; ++k) pc.q[k] = pose_dev[k];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) pc.t[k] = pose_dev[4 + k];
+}
+
+// ... and its own last block applies the next Gauss-Newton update (a system that is not positive definite leaves the
+// pose alone).  Called by the last block of a problem only.
+__device__ __forceinline__ void se3_track_update(const float* out, float* pose_dev, float* __restrict__ history)
+{
+  __syncthreads();  // out[0..28] was written by warp 0 of this block
+  if (threadIdx.x == 0) {
+    float pose[7];
+#pragma unroll
+    for (int k = 0; k < 7; ++k) pose[k] = pose_dev[k];
+    if (history) {  // [29 system | 7 pose the system was evaluated at]
 #pragma unroll 1
-        for (int k = 0; k < 29; ++k) history[k] = out[k];
+      for (int k = 0; k < 29; ++k) history[k] = out[k];
 #pragma unroll
-        for (int k = 0; k < 7; ++k) history[29 + k] = pose[k];
-      }
-      float sys[27];
+      for (int k = 0; k < 7; ++k) history[29 + k] = pose[k];
+    }
+    float sys[27];
 #pragma unroll 1
-      for (int k = 0; k < 27; ++k) sys[k] = out[k];
-      if (gn_update_pose(sys, pose)) {
+    for (int k = 0; k < 27; ++k) sys[k] = out[k];
+    if (gn_update_pose(sys, pose)) {
 #pragma unroll
-        for (int k = 0; k < 7; ++k) pose_dev[k] = pose[k];
-      }
+      for (int k = 0; k < 7; ++k) pose_dev[k] = pose[k];
     }
   }
+}
+
+__global__ void __launch_bounds__(kThreads)
+se3_step_kernel(PixelCam pc, float huber_delta, int width, int height, View img0, View img1, View dpt0, View grad1,
+                bool grad_aligned, float* __restrict__ scratch, unsigned int* __restrict__ counter,
+                float* __restrict__ out, float* pose_dev, float* __restrict__ history)
+{
+  if (pose_dev) se3_load_pose(pc, pose_dev);  // tracking mode (pose_dev != nullptr)
+  float acc[28];
+  unsigned int inl;
+  se3_accumulate(pc, huber_delta, width, height, img0, img1, dpt0, grad1, grad_aligned,
+                 blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x, acc, inl);
+  const bool last = reduce_finalize<28>(acc, inl, blockIdx.x, gridDim.x, scratch, counter, out);
+  if (pose_dev && last) se3_track_update(out, pose_dev, history);
+}
+
+// N tracking problems advanced in lockstep, one Gauss-Newton iteration of every problem per launch.  Row blockIdx.y is
+// problem n; it uses the first d.nblocks blocks of the row (what se3_step_kernel's grid would be for that level), the
+// rest of the row returns at once and takes no ticket.  Problem n owns scratch rows [n * scratch_stride, +nblocks),
+// counters[n], out[32 n .. +29) and the pose poses[8 n .. +7); its last block updates that pose.
+__global__ void __launch_bounds__(kThreads)
+se3_track_batch_kernel(const Se3TrackDesc* __restrict__ descs, float huber_delta, float* __restrict__ scratch,
+                       int scratch_stride, unsigned int* __restrict__ counters, float* __restrict__ outs, float* poses)
+{
+  const int n = blockIdx.y;
+  const Se3TrackDesc& d = descs[n];
+  const int nblocks = d.nblocks;
+  if ((int)blockIdx.x >= nblocks) return;
+  float* pose_dev = poses + 8 * (size_t)n;
+  float* out = outs + 32 * (size_t)n;
+  PixelCam pc = d.pc;
+  se3_load_pose(pc, pose_dev);
+  float acc[28];
+  unsigned int inl;
+  se3_accumulate(pc, huber_delta, d.width, d.height, d.img0, d.img1, d.dpt0, d.grad1, d.grad_aligned != 0,
+                 blockIdx.x * blockDim.x + threadIdx.x, nblocks * blockDim.x, acc, inl);
+  const bool last = reduce_finalize<28>(acc, inl, blockIdx.x, nblocks, scratch + (size_t)n * scratch_stride * 32,
+                                        counters + n, out);
+  if (last) se3_track_update(out, pose_dev, nullptr);
 }
 
 // ------------------------------------------------------------------------------ EvaluateError
@@ -195,7 +243,7 @@ eval_error_kernel(PixelCam pc, float huber_delta, int width, int height, View im
     inl += 1;
     acc[0] = fmaf(diff, diff, acc[0]);
   }
-  reduce_finalize<1>(acc, inl, scratch, counter, out);
+  reduce_finalize<1>(acc, inl, blockIdx.x, gridDim.x, scratch, counter, out);
 }
 
 // ------------------------------------------------------------------------------ Warp
@@ -223,7 +271,7 @@ warp_kernel(PixelCam pc, int width, int height, View img0, View img1, View dpt0,
     }
     img2[(size_t)y * img2_pitch + x] = sampled;
   }
-  reduce_finalize<1>(acc, inl, scratch, counter, out);
+  reduce_finalize<1>(acc, inl, blockIdx.x, gridDim.x, scratch, counter, out);
 }
 
 // ------------------------------------------------------------------------------ SquaredError
@@ -238,7 +286,7 @@ squared_error_kernel(int width, int height, View a, View b, float* __restrict__ 
     const float d = __ldg(a.ptr + (size_t)y * a.pitch + x) - __ldg(b.ptr + (size_t)y * b.pitch + x);
     acc[0] = fmaf(d, d, acc[0]);
   }
-  reduce_finalize<1>(acc, 0u, scratch, counter, out);
+  reduce_finalize<1>(acc, 0u, blockIdx.x, gridDim.x, scratch, counter, out);
 }
 
 // ------------------------------------------------------------------------------ UpdateDepth
@@ -362,6 +410,18 @@ inline int grid_for(int area)
 }
 
 }  // namespace
+
+int se3_step_blocks(int width, int height) { return grid_for(width * height); }
+
+cudaError_t launch_se3_track_batch(const Se3TrackDesc* descs_dev, int num_problems, int max_blocks, float huber_delta,
+                                   float* scratch, int scratch_stride, unsigned int* counters, float* outs, float* poses,
+                                   cudaStream_t s)
+{
+  const dim3 grid((unsigned)max_blocks, (unsigned)num_problems);
+  se3_track_batch_kernel<<<grid, kThreads, 0, s>>>(descs_dev, huber_delta, scratch, scratch_stride, counters, outs,
+                                                   poses);
+  return cudaGetLastError();
+}
 
 cudaError_t launch_se3_step(const PixelCam& pc, float huber_delta, int width, int height, View img0, View img1,
                             View dpt0, View grad1, bool grad_aligned, float* scratch, unsigned int* counter,

@@ -26,6 +26,7 @@
 #ifndef DFK_FACADE_H_
 #define DFK_FACADE_H_
 
+#include <algorithm>
 #include <array>
 #include <cstddef>
 #include <cstdint>
@@ -435,6 +436,46 @@ public:
     detail::Check(h_.get(), dfk_se3_track(h_.get(), pose_ck.data(), lv.data(), static_cast<int>(lv.size()), &frac, &err,
                                           nullptr, nullptr, 0));
     return std::make_pair(frac, err);
+  }
+
+  // TrackLevels against many keyframes at once, the live frame (pyr_img1, pyr_grad1) shared: the loops of
+  // DeepFactors::Relocalize (core/deepfactors.cpp:713-743) and of LoopDetector::DetectLoop's geometry check
+  // (core/system/loop_detector.cpp:149-168) as ONE call.  kf_img_pyrs[n] / kf_dpt_pyrs[n] are keyframe n's pyramids,
+  // poses_ck[n] its start pose (identity = what Reset does), updated in place.  Every Gauss-Newton iteration is one launch
+  // for all keyframes.  Returns one {inliers / area, residual / inliers} per keyframe, bit for bit what TrackLevels gives
+  // for that keyframe alone.
+  template <typename SE3T, typename CamPyr, typename ImagePyrs0, typename ImagePyr1, typename DepthPyrs, typename GradPyr>
+  std::vector<std::pair<float, float>> TrackLevelsBatch(std::vector<SE3T>& poses_ck, const CamPyr& camera_pyr,
+                                                        const ImagePyrs0& kf_img_pyrs, const ImagePyr1& pyr_img1,
+                                                        const DepthPyrs& kf_dpt_pyrs, const GradPyr& pyr_grad1,
+                                                        const std::vector<int>& iterations_per_level)
+  {
+    const std::size_t n = poses_ck.size(), L = iterations_per_level.size();
+    if (kf_img_pyrs.size() != n || kf_dpt_pyrs.size() != n)
+      throw std::runtime_error("SE3Aligner::TrackLevelsBatch: one image and one depth pyramid per pose expected");
+    std::vector<DfkTrackLevel> lv(n * L);
+    std::vector<float> poses(n * 7);
+    for (std::size_t k = 0; k < n; ++k) {
+      for (std::size_t l = 0; l < L; ++l) {
+        DfkTrackLevel& t = lv[k * L + l];
+        t.cam = detail::Cam(camera_pyr[l]);
+        t.img0 = detail::View(kf_img_pyrs[k][l], 1);
+        t.img1 = detail::View(pyr_img1[l], 1);
+        t.dpt0 = detail::View(kf_dpt_pyrs[k][l], 1);
+        t.grad1 = detail::View(pyr_grad1[l], 2);
+        t.iterations = iterations_per_level[l];
+      }
+      std::copy(poses_ck[k].data(), poses_ck[k].data() + 7, poses.begin() + 7 * k);
+    }
+    std::vector<float> frac(n, 0.f), err(n, 0.f);
+    detail::Check(h_.get(), dfk_se3_track_batch(h_.get(), static_cast<int>(n), static_cast<int>(L), poses.data(),
+                                                lv.data(), frac.data(), err.data(), nullptr));
+    std::vector<std::pair<float, float>> stats(n);
+    for (std::size_t k = 0; k < n; ++k) {
+      std::copy(poses.begin() + 7 * k, poses.begin() + 7 * (k + 1), poses_ck[k].data());
+      stats[k] = std::make_pair(frac[k], err[k]);
+    }
+    return stats;
   }
 
 private:

@@ -283,6 +283,26 @@ DfkStatus dfk_se3_track(DfkHandle h, float pose_ck[7], const DfkTrackLevel* leve
                         float* inlier_fraction, float* error, float* last_system, float* history,
                         int history_capacity);
 
+/* One live frame tracked against many keyframes, the loop of DeepFactors::Relocalize (core/deepfactors.cpp:713-743:
+ * SetKeyframe + Reset + TrackFrame per keyframe of the map, keep the smallest GetError()) and of the geometry check in
+ * LoopDetector::DetectLoop (core/system/loop_detector.cpp:149-168: one TrackFrame per candidate keyframe, then
+ * GetInliers() / GetPoseEstimate()).  The reference tracks them one after another; here the num_problems problems
+ * advance in lockstep: every Gauss-Newton iteration is ONE launch for all of them, and there is one upload and one
+ * read-back per call.  Synchronous.
+ *   poses_ck         in/out, num_problems x 7 floats
+ *   levels           num_problems x num_levels, problem-major: problem n's pyramid is levels[n * num_levels ...],
+ *                    level 0 the finest.  Level sizes may differ between problems; the iteration count of a level
+ *                    must be the same for every problem (else DFK_ERR_INVALID_ARG).  1 <= num_problems <= 65535.
+ *   inlier_fraction  optional, num_problems floats
+ *   error            optional, num_problems floats
+ *   last_systems     optional, num_problems x 29 floats
+ * Problem n gives exactly what dfk_se3_track(h, poses_ck + 7n, levels + n * num_levels, num_levels, ...) gives, bit for
+ * bit, including its two rules: inlier_fraction / error are left untouched when level 0 has no iteration, and a system
+ * that is not positive definite leaves that problem's pose alone. */
+DfkStatus dfk_se3_track_batch(DfkHandle h, int num_problems, int num_levels, float* poses_ck,
+                              const DfkTrackLevel* levels, float* inlier_fraction, float* error,
+                              float* last_systems);
+
 /* SE3Aligner<float>::Warp (cu_se3aligner.h:58-63, cu_se3aligner.cpp:125-151): renders img1
  * into frame 0 (img2, 0 where invalid); residual = SIGNED sum(img0 - sampled) (:106). */
 DfkStatus dfk_se3_warp(DfkHandle h, const float se3[7], const DfkCamera* cam,

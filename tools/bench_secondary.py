@@ -9,6 +9,8 @@ One JSON line per case:
   * the synchronous per-call API (what a PhotometricFactor / CameraTracker pays per call, including the result
     read-back): SfmAligner::RunStep, EvaluateError, SE3Aligner::RunStep, UpdateDepth, SobelGradients,
     GaussianBlurDown at 640x480 -- wall clock per call.
+  * CameraTracker::TrackFrame (19 iterations) and Relocalize against K = 8 / 32 keyframes, per keyframe and batched --
+    wall clock per call, and for Relocalize the summed device time.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -148,6 +150,55 @@ def main():
     bytes_track = sum(iters[l] * (640 >> l) * (480 >> l) * 20 for l in range(3))
     timed("CameraTracker::TrackFrame 19 iterations, device-side loop (dfk_se3_track)", device_loop, bytes_track)
     timed("CameraTracker::TrackFrame 19 iterations, per-step API + host solve (reference structure)", host_loop, bytes_track)
+
+    # ---- DeepFactors::Relocalize: the same live frame tracked against K keyframes (deepfactors.cpp:713-743) ---------------
+    # K x (SetKeyframe + Reset + TrackFrame), what the reference does, against one Relocalize (dfk_se3_track_batch: one
+    # launch per iteration for all K keyframes).  Keyframes: the synthetic keyframe pyramid, every copy rolled by a
+    # different offset, each in its own buffers.
+    from torch.profiler import ProfilerActivity, profile
+
+    def device_us(fn, reps):  # summed device time (kernels, copies, memsets) per call, from a separate profiled run
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps):
+                fn()
+            torch.cuda.synchronize()
+        return sum(e.self_device_time_total for e in prof.key_averages()) / reps
+
+    for K in (8, 32):
+        kfs = []
+        for k in range(K):
+            sh = (7 * k) % 23 - 11
+            kfs.append(([torch.roll(x["img0"], shifts=sh >> l, dims=1).contiguous() for l, x in enumerate(lv)],
+                        [torch.roll(x["dpt0"], shifts=sh >> l, dims=1).contiguous() for l, x in enumerate(lv)]))
+
+        def per_keyframe():
+            errs = []
+            for kf in kfs:
+                trk.SetKeyframe(kf[0], kf[1])
+                trk.Reset()
+                trk.TrackFrame(img1s, grads)
+                errs.append(trk.GetError())
+            return errs
+
+        def relocalize():
+            return trk.Relocalize(kfs, img1s, grads)[2]
+
+        assert np.array_equal(np.asarray(per_keyframe(), np.float32), relocalize())  # same errors, bit for bit
+        reps = max(2, args.reps // 2)
+        for name, fn in (("K x CameraTracker::TrackFrame (dfk_se3_track per keyframe)", per_keyframe),
+                         ("one CameraTracker::Relocalize (dfk_se3_track_batch)", relocalize)):
+            for _ in range(3):
+                fn()
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            for _ in range(reps):
+                fn()
+            torch.cuda.synchronize()
+            us = (time.perf_counter() - t0) / reps * 1e6
+            print(json.dumps({"case": f"Relocalize 640x480 live frame vs K={K} keyframes, 3 levels x (10, 5, 4): {name}",
+                              "us_per_relocalisation": us, "device_us_per_relocalisation": device_us(fn, reps),
+                              "timing": "wall clock (synchronous); device time = summed kernel + copy time, "
+                                        "torch.profiler"}), flush=True)
 
 
 if __name__ == "__main__":
