@@ -61,6 +61,13 @@ class DfkTrackLevel(C.Structure):
                 ("iterations", C.c_int)]
 
 
+class DfkReprojectionItem(C.Structure):
+    _fields_ = [("pose0", C.c_float * 7), ("pose1", C.c_float * 7), ("cam", DfkCamera), ("prx_orig", DfkImage),
+                ("prx_jac", DfkImage), ("code", C.POINTER(C.c_float)), ("num_matches", C.c_int32),
+                ("query_xy", C.POINTER(C.c_float)), ("train_xy", C.POINTER(C.c_float)), ("cauchy_delta", C.c_float),
+                ("sigma", C.c_float)]
+
+
 class DfkWindowDesc(C.Structure):
     _fields_ = [("num_keyframes", C.c_int32), ("num_pairs", C.c_int32), ("num_items", C.c_int32), ("code_size", C.c_int32),
                 ("pair_k0", C.POINTER(C.c_int32)), ("pair_k1", C.POINTER(C.c_int32)), ("item_pair", C.POINTER(C.c_int32)),
@@ -111,6 +118,7 @@ SYMBOLS = {
     "dfk_depth_run_step": (C.c_int, [_H, _F, C.c_int, _IMG, _IMG, _IMG, _F, _F, _F, C.POINTER(C.c_uint64)]),
     "dfk_reprojection_linearize": (C.c_int, [_H, _F, _F, _F, C.c_int, _CAM, _IMG, _IMG, C.c_int, _F, _F, C.c_float,
                                              C.c_float, _F, _F]),
+    "dfk_reprojection_linearize_batch": (C.c_int, [_H, C.POINTER(DfkReprojectionItem), C.c_int, C.c_int, C.c_void_p]),
     "dfk_sparse_geometric_linearize": (C.c_int, [_H, _F, _F, _F, _F, C.c_int, _CAM, _IMG, _IMG, _IMG, _IMG, _IMG, C.c_int,
                                                  C.POINTER(C.c_int), C.c_float, _F, C.POINTER(C.c_int)]),
     "dfk_update_depth": (C.c_int, [_H, _F, C.c_int, _IMG, _IMG, C.c_float, _IMG]),

@@ -23,8 +23,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import (DfkCamera, DfkDenseSfmParams, DfkImage, DfkSfmAlignerParams, DfkSfmWorkItem, DfkTrackLevel, check,
-                   lib)
+from ._lib import (DfkCamera, DfkDenseSfmParams, DfkImage, DfkReprojectionItem, DfkSfmAlignerParams, DfkSfmWorkItem,
+                   DfkTrackLevel, check, lib)
 
 
 # ------------------------------------------------------------------------------------------- params
@@ -286,6 +286,43 @@ def ReprojectionLinearize(aligner, pose0, pose1, code0, cam, prx_orig, prx_jac, 
         q.ctypes.data_as(FP), t.ctypes.data_as(FP), C.c_float(cauchy_delta), C.c_float(sigma), rows.ctypes.data_as(FP),
         C.byref(tot)))
     return rows, float(tot.value)
+
+
+def ReprojectionLinearizeBatch(aligner, items: Sequence[dict], records: torch.Tensor | None = None) -> torch.Tensor:
+    """Many ReprojectionFactors linearised in one launch straight into normal-equation records
+    (dfk_reprojection_linearize_batch): items are dicts with the arguments of ReprojectionLinearize (pose0, pose1, code0,
+    cam, prx_orig, prx_jac, query_xy, train_xy, cauchy_delta, sigma).  Record i = [A^T A packed | -A^T b | b^T b | valid
+    matches] of factor i's rows, in the RunStep record layout, so it goes into Window.assemble as an unscaled record
+    (item size (0, 0)).  `records` may be a slice of a larger record buffer.  Asynchronous: returns a device tensor
+    [n, DFK_SFM_RECORD_FLOATS(CS)] on torch's current stream."""
+    aligner._hd.use_torch_stream()
+    cs, n = aligner.CS, len(items)
+    rec = _lib.record_floats(cs)
+    if records is None:
+        records = torch.empty((n, rec), dtype=torch.float32, device=f"cuda:{aligner._hd.device}")
+    if not (records.is_contiguous() and records.numel() >= n * rec):
+        raise ValueError(f"records must be a contiguous device tensor of at least {n} x {rec} floats")
+    arr = (DfkReprojectionItem * max(n, 1))()
+    keep = []  # the host arrays must outlive the ctypes pointers until the call returns
+    FP = C.POINTER(C.c_float)
+    for k, it in enumerate(items):
+        code = np.ascontiguousarray(it["code0"], dtype=np.float32)
+        if code.shape != (cs,):
+            raise ValueError(f"code0 must have {cs} entries")
+        q = np.ascontiguousarray(it["query_xy"], dtype=np.float32).reshape(-1, 2)
+        t = np.ascontiguousarray(it["train_xy"], dtype=np.float32).reshape(-1, 2)
+        if q.shape != t.shape:
+            raise ValueError("query_xy and train_xy must hold the same number of matches")
+        keep += [code, q, t]
+        w = arr[k]
+        w.pose0, w.pose1, w.cam = _pose(it["pose0"]), _pose(it["pose1"]), _cam(it["cam"])
+        w.prx_orig, w.prx_jac = _image(it["prx_orig"]), _image(it["prx_jac"], cs)
+        w.code, w.query_xy, w.train_xy = code.ctypes.data_as(FP), q.ctypes.data_as(FP), t.ctypes.data_as(FP)
+        w.num_matches = q.shape[0]
+        w.cauchy_delta, w.sigma = float(it["cauchy_delta"]), float(it["sigma"])
+    check(aligner.handle, lib().dfk_reprojection_linearize_batch(aligner.handle, arr, n, cs,
+                                                                 C.c_void_p(records.data_ptr())))
+    return records
 
 
 def SparseGeometricLinearize(aligner, pose0, pose1, code0, code1, cam, prx0_orig, prx0_jac, prx1_orig, prx1_jac, dpt_grad1,

@@ -54,6 +54,10 @@ struct DfkContext {
   size_t sparse_cap = 0;
   float* sparse_host = nullptr;      // pinned mirror
   size_t sparse_host_cap = 0;
+  // dfk_reprojection_linearize_batch: [descriptors | codes | query | train] (bytes), one H2D per call from rep_host
+  unsigned char* rep_dev = nullptr;
+  size_t rep_cap = 0;
+  std::vector<unsigned char> rep_host;
   SfmItemDev* items_dev = nullptr;
   size_t items_cap = 0;
   float* partials_dev = nullptr;
@@ -601,6 +605,7 @@ DfkStatus dfk_destroy(DfkHandle h)
     cudaFree(h->batch_dev); cudaFree(h->batch_partials); cudaFree(h->batch_counters);
     if (h->batch_host) cudaFreeHost(h->batch_host);
     cudaFree(h->items_dev); cudaFree(h->partials_dev); cudaFree(h->records_dev);
+    cudaFree(h->rep_dev);
     for (auto& r : h->ray_cache) cudaFree(r.dev);
     if (h->out_host) cudaFreeHost(h->out_host);
     if (h->records_host) cudaFreeHost(h->records_host);
@@ -1236,7 +1241,9 @@ DfkStatus dfk_window_create(DfkHandle h, const DfkWindowDesc* d, DfkWindow** out
       if (d->pair_k0[p] < 0 || d->pair_k0[p] >= K || d->pair_k1[p] < 0 || d->pair_k1[p] >= K)
         return fail(h, DFK_ERR_INVALID_ARG, "[Window] pair " + std::to_string(p) + " names a keyframe outside the window");
     for (int i = 0; i < n; ++i)
-      if (d->item_pair[i] < 0 || d->item_pair[i] >= P || d->item_width[i] <= 0 || d->item_height[i] <= 0)
+      // a record is scaled (W, H > 0: photometric) or unscaled (0, 0: reprojection)
+      if (d->item_pair[i] < 0 || d->item_pair[i] >= P ||
+          !((d->item_width[i] > 0 && d->item_height[i] > 0) || (d->item_width[i] == 0 && d->item_height[i] == 0)))
         return fail(h, DFK_ERR_INVALID_ARG, "[Window] record " + std::to_string(i) + " names a pair outside the window");
     // CSR lists in item order (the summation order of the gather kernel)
     std::vector<int> kf0_ptr(K + 1, 0), kf1_ptr(K + 1, 0), pair_ptr(P + 1, 0);
@@ -1611,6 +1618,80 @@ DfkStatus dfk_reprojection_linearize(DfkHandle h, const float pose0[7], const fl
     const float* e2 = h->sparse_host + n_in + 2 * M * RW;
     for (size_t i = 0; i < M; ++i) tot += e2[i];
     *total_err = tot;
+    return DFK_OK;
+  } catch (...) {
+    return oom(h);
+  }
+}
+
+DfkStatus dfk_reprojection_linearize_batch(DfkHandle h, const DfkReprojectionItem* items, int n, int code_size,
+                                           float* records_dev)
+{
+  try {
+    if (!h) return DFK_ERR_INVALID_ARG;
+    if (!items || n < 1 || !records_dev)
+      return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::linearize batch] null argument / empty batch");
+    if (!(code_size == 8 || code_size == 16 || code_size == 32 || code_size == 64 || code_size == 128))
+      return fail(h, DFK_ERR_UNSUPPORTED,
+                  "[ReprojectionFactor::linearize batch] code size not instantiated: " + std::to_string(code_size));
+    size_t total = 0;  // matches of the whole batch
+    for (int i = 0; i < n; ++i) {
+      const DfkReprojectionItem& it = items[i];
+      const std::string at = "[ReprojectionFactor::linearize batch] item " + std::to_string(i) + ": ";
+      if (!it.code || !it.query_xy || !it.train_xy) return fail(h, DFK_ERR_INVALID_ARG, at + "null argument");
+      if (it.num_matches < 1 || !(it.sigma > 0.0f))
+        return fail(h, DFK_ERR_INVALID_ARG, at + "no matches / non-positive sigma");
+      const uint32_t W = it.prx_orig.width, H = it.prx_orig.height;
+      if (W == 0 || H == 0 || !img_ok(&it.prx_orig, W, H, 1) || !img_ok(&it.prx_jac, W, H, code_size))
+        return fail(h, DFK_ERR_INVALID_ARG, at + "inconsistent image views");
+      total += (size_t)it.num_matches;
+    }
+    if (total > (size_t)INT32_MAX)
+      return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::linearize batch] more than 2^31 - 1 matches in one call");
+    DeviceGuard guard(h->device);
+    // one upload: [descriptors n | codes n x C | query 2 total | train 2 total]
+    const size_t desc_bytes = (sizeof(ReprojItemDev) * (size_t)n + 15) & ~(size_t)15;
+    const size_t code_bytes = sizeof(float) * (size_t)n * code_size;
+    const size_t match_bytes = sizeof(float) * 2 * total;
+    const size_t bytes = desc_bytes + code_bytes + 2 * match_bytes;
+    DFK_CUDA(h, ensure(&h->rep_dev, &h->rep_cap, bytes), "[ReprojectionFactor::linearize batch] scratch allocation failed");
+    h->rep_host.assign(bytes, 0);
+    ReprojItemDev* descs = reinterpret_cast<ReprojItemDev*>(h->rep_host.data());
+    float* codes = reinterpret_cast<float*>(h->rep_host.data() + desc_bytes);
+    float* query = reinterpret_cast<float*>(h->rep_host.data() + desc_bytes + code_bytes);
+    float* train = query + 2 * total;
+    const float* codes_dev = reinterpret_cast<const float*>(h->rep_dev + desc_bytes);
+    const float* query_dev = reinterpret_cast<const float*>(h->rep_dev + desc_bytes + code_bytes);
+    size_t begin = 0;
+    for (int i = 0; i < n; ++i) {
+      const DfkReprojectionItem& it = items[i];
+      ReprojItemDev& d = descs[i];
+      float p10[7];
+      relative_pose(it.pose1, it.pose0, p10, d.sp.P1, d.sp.P0);  // as dfk_reprojection_linearize
+      for (int k = 0; k < 4; ++k) d.sp.q[k] = p10[k];
+      for (int k = 0; k < 3; ++k) d.sp.t[k] = p10[4 + k];
+      quat_to_matrix(p10, d.sp.R);
+      d.sp.fx = it.cam.fx; d.sp.fy = it.cam.fy; d.sp.u0 = it.cam.u0; d.sp.v0 = it.cam.v0;
+      d.prx_orig = view_of(&it.prx_orig);
+      d.jac = view_of(&it.prx_jac);
+      d.code = codes_dev + (size_t)i * code_size;
+      d.width = (int)it.prx_orig.width;
+      d.height = (int)it.prx_orig.height;
+      d.num_matches = it.num_matches;
+      d.match_begin = (int)begin;
+      d.cauchy_delta = it.cauchy_delta;
+      d.sigma = it.sigma;
+      memcpy(codes + (size_t)i * code_size, it.code, sizeof(float) * code_size);
+      memcpy(query + 2 * begin, it.query_xy, sizeof(float) * 2 * it.num_matches);
+      memcpy(train + 2 * begin, it.train_xy, sizeof(float) * 2 * it.num_matches);
+      begin += (size_t)it.num_matches;
+    }
+    DFK_CUDA(h, cudaMemcpyAsync(h->rep_dev, h->rep_host.data(), bytes, cudaMemcpyHostToDevice, h->stream),
+             "[ReprojectionFactor::linearize batch] upload failed");
+    DFK_CUDA(h, launch_reprojection_records(code_size, reinterpret_cast<const ReprojItemDev*>(h->rep_dev), n, query_dev,
+                                            query_dev + 2 * total, h->params.sfmparams.avg_dpt, records_dev, h->stream),
+             "[ReprojectionFactor::linearize batch] kernel launch failed");
+    h->launches += 1;
     return DFK_OK;
   } catch (...) {
     return oom(h);

@@ -186,6 +186,19 @@ cudaError_t launch_reprojection_rows(const SparsePose& sp, const float* code_dev
                                      int width, int height, int num_matches, const float* query_dev, const float* train_dev,
                                      float cauchy_delta, float sigma, float avg_dpt, float* rows_dev, float* err2_dev,
                                      cudaStream_t s);
+// One factor of dfk_reprojection_linearize_batch: what launch_reprojection_rows takes for it.  Its matches are
+// query / train[match_begin, + num_matches); code points at its code_size floats in device scratch.
+struct ReprojItemDev {
+  SparsePose sp;
+  View prx_orig, jac;
+  const float* code;
+  int width, height;
+  int num_matches, match_begin;
+  float cauchy_delta, sigma;
+};
+// one CTA per item; records_dev: num_items records of DFK_SFM_RECORD_FLOATS(code_size) floats
+cudaError_t launch_reprojection_records(int code_size, const ReprojItemDev* items_dev, int num_items, const float* query_dev,
+                                        const float* train_dev, float avg_dpt, float* records_dev, cudaStream_t s);
 
 cudaError_t launch_sparse_geometric_rows(const SparsePose& sp, float cam_w, float cam_h, const float* code0_dev,
                                          const float* code1_dev, int code_size, View prx0, View jac0, View prx1, View jac1,

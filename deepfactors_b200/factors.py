@@ -85,9 +85,10 @@ def assemble_window(layout: WindowLayout, pairs: Sequence[Tuple[int, int]], JtJ,
 
     pairs[i] = (k0, k1): keyframe k0 is warped into frame k1 (pose0/code0 belong to k0, pose1 to k1).
     JtJ [n, NP, NP], Jtr [n, NP] in the aligner's column order [pose0 | pose1 | code0].  sizes[i] = (W, H) of the
-    level (for the residual rescale).  Works on numpy arrays or torch tensors (any device).
+    level (for the residual rescale); (0, 0) marks an unscaled record (a reprojection factor, whose residual b^T b enters f
+    as it is).  Works on numpy arrays or torch tensors (any device).
     Returns (H [dim, dim], g [dim], f) with g = -sum Jtr (photometric_factor.cpp:106) and f = sum of rescaled residuals
-    over items with overlap."""
+    over items with overlap plus the residuals of the unscaled records."""
     c, b = layout.code_size, layout.block
     is_torch = hasattr(JtJ, "detach")
     if is_torch:
@@ -109,15 +110,23 @@ def assemble_window(layout: WindowLayout, pairs: Sequence[Tuple[int, int]], JtJ,
             for lb, gb in loc:
                 H[ga, gb] += J64[i, la, lb]
         inl = int(inliers[i])
-        if inl > 0:
+        if is_unscaled(sizes[i]):
+            f += float(residual[i])
+        elif inl > 0:
             f += float(residual[i]) / inl * sizes[i][0] * sizes[i][1]
     return H, g, f
+
+
+def is_unscaled(size) -> bool:
+    """item size (0, 0): a record whose residual is not rescaled (dfk_reprojection_linearize_batch)"""
+    return size[0] == 0 and size[1] == 0
 
 
 @dataclass
 class WindowBlocks:
     """The packed block-sparse buffer dfk_window_assemble writes (include/dfk.h, SURVEY 8e): K diagonal blocks B x B,
-    K gradients B, P coupling blocks B x 6 ([pose0 | code0] of k0 x pose1 of k1), then f and the inlier total."""
+    K gradients B, P coupling blocks B x 6 ([pose0 | code0] of k0 x pose1 of k1), then f and the inlier total of the
+    photometric (scaled) records."""
     num_keyframes: int
     code_size: int
     pairs: Sequence[Tuple[int, int]]
@@ -140,7 +149,8 @@ class WindowBlocks:
 
     def pack(self, item_pair, JtJ, Jtr, residual, inliers, sizes):
         """Host mirror of dfk_window_assemble (numpy, float32 sums in item order): item i belongs to pair item_pair[i];
-        JtJ [n, NP, NP] dense, Jtr [n, NP], sizes[i] = (W, H).  Returns the flat buffer."""
+        JtJ [n, NP, NP] dense, Jtr [n, NP], sizes[i] = (W, H), or (0, 0) for an unscaled record: its residual is added
+        to f as it is and its inliers are left out of the inlier total.  Returns the flat buffer."""
         K, B, c = self.num_keyframes, self.B, self.code_size
         out = np.zeros(self.floats, dtype=np.float32)
         o_g, o_c, o_t = self.offsets()
@@ -160,6 +170,9 @@ class WindowBlocks:
             g[k1][:6] -= r[6:12]
             O[p] += H[np.ix_(loc0, np.arange(6, 12))]
             inl = int(inliers[i])
+            if is_unscaled(sizes[i]):
+                f += np.float32(residual[i])
+                continue
             if inl > 0:
                 f += np.float32(residual[i]) / np.float32(inl) * np.float32(sizes[i][0] * sizes[i][1])
             ninl += np.float32(inl)

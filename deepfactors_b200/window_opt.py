@@ -12,8 +12,11 @@ solves.  Here every heavy step of one iteration is ONE device operation over the
     assemble    block-sparse normal equations of the window, on the device               dfk_window_assemble
                 (+ one all-reduce across ranks when the pairs are sharded)
     solve       damped dense solve on the device (Cholesky, float64)                     torch.linalg
+    (links)     one batched launch over the stale reprojection links (global loop closures, use_reprojection),
+                straight into normal-equation records                                  dfk_reprojection_linearize_batch
     retract     pose: t += dt, R = exp(w) R (gtsam_traits.h:48-58); code += dc           (tiny, host)
-    accept      Levenberg-Marquardt on the rescaled residual energy f (what the factor's error() returns)
+    accept      Levenberg-Marquardt on the energy f: rescaled photometric residuals + b^T b of the links (what the
+                factors' error() return)
 
 The host side (cache, retraction, damping schedule) is plain Python / numpy; nothing here needs GTSAM.
 """
@@ -189,26 +192,51 @@ class WindowOptimizer:
         return poses, codes, trace
 
 
+@dataclass
+class ReprojectionLink:
+    """A reprojection factor between keyframes k0 -> k1 (ReprojectionFactor, reprojection_factor.cpp): matched keypoints
+    query_xy [M, 2] in k0 and train_xy [M, 2] in k1 (host), Cauchy delta and sigma.  A global loop closure is one link
+    each way with sigma = loop_sigma (mapper.cpp:367-376); use_reprojection adds them with rep_huber / rep_sigma
+    (mapper.cpp:314-325)."""
+    k0: int
+    k1: int
+    query_xy: np.ndarray
+    train_xy: np.ndarray
+    cauchy_delta: float
+    sigma: float
+
+
 class SfmWindowProblem:
     """The device pipeline of one linearisation, on SfmAligner + Window: keyframes hold their pyramids on the device
     (img, grad, prx_orig, prx_jac per level + the dpt / valid buffers the fused decode writes); `linearise` re-evaluates
-    the factors of the given pairs in one launch (depth decode fused in) and re-assembles the window."""
+    the factors of the given pairs in one launch (depth decode fused in) and re-assembles the window.
 
-    def __init__(self, aligner, cams, keyframes, pairs, allreduce: Optional[Callable] = None):
+    `links` (optional) are reprojection factors: they follow the photometric pairs in the window's pair list (same
+    variables pose0, pose1, code0, so the linearisation cache covers them), each owns one unscaled record at the end of
+    the record buffer, and the stale ones are re-linearised in one dfk_reprojection_linearize_batch launch."""
+
+    def __init__(self, aligner, cams, keyframes, pairs, allreduce: Optional[Callable] = None,
+                 links: Optional[Sequence[ReprojectionLink]] = None):
         import torch
         from . import _lib
         from .aligners import Window
         self.al = aligner
         self.cams = list(cams)
         self.kf = keyframes          # kf[k][l] = dict(img, grad, prx_orig, prx_jac, dpt, valid) of device tensors
-        self.pairs = [tuple(p) for p in pairs]
+        self.links = list(links or [])
+        self.num_photometric = len(pairs)
+        self.pairs = [tuple(p) for p in pairs] + [(int(ln.k0), int(ln.k1)) for ln in self.links]
         self.levels = len(self.cams)
         item_pair, sizes = [], []
-        for p in range(len(self.pairs)):
+        for p in range(self.num_photometric):
             for l in range(self.levels):
                 item_pair.append(p)
                 t = self.kf[self.pairs[p][0]][l]["img"]
                 sizes.append((int(t.shape[1]), int(t.shape[0])))
+        self.photometric_items = len(item_pair)
+        for j in range(len(self.links)):
+            item_pair.append(self.num_photometric + j)
+            sizes.append((0, 0))  # unscaled record: b^T b enters f as it is
         self.window = Window(aligner, len(keyframes), self.pairs, item_pair, sizes)
         self.layout = self.window.layout
         self.records = torch.zeros((len(item_pair), _lib.record_floats(aligner.CS)), dtype=torch.float32, device=self.kf[0][0]["img"].device)
@@ -225,16 +253,38 @@ class SfmWindowProblem:
                                   grad1=b["grad"], prx_orig=a["prx_orig"], code=codes[k0].astype(np.float32)))
         return items
 
+    def _link_items(self, poses, codes, todo):
+        items = []
+        for j in todo:
+            ln = self.links[j]
+            a = self.kf[ln.k0][0]
+            items.append(dict(pose0=poses[ln.k0].astype(np.float32), pose1=poses[ln.k1].astype(np.float32),
+                              code0=codes[ln.k0].astype(np.float32), cam=self.cams[0], prx_orig=a["prx_orig"],
+                              prx_jac=a["prx_jac"], query_xy=ln.query_xy, train_xy=ln.train_xy,
+                              cauchy_delta=ln.cauchy_delta, sigma=ln.sigma))
+        return items
+
     def linearise(self, poses, codes, todo):
         import torch
-        if todo:
-            work = self.al.make_work_items(self._items(poses, codes, todo))
-            if len(todo) == len(self.pairs):
-                self.al.RunStepBatch(work, self.records)
+        from .aligners import ReprojectionLinearizeBatch
+        photo = [p for p in todo if p < self.num_photometric]
+        links = [p - self.num_photometric for p in todo if p >= self.num_photometric]
+        if photo:
+            work = self.al.make_work_items(self._items(poses, codes, photo))
+            if len(photo) == self.num_photometric:
+                self.al.RunStepBatch(work, self.records[:self.photometric_items])
             else:
                 part = self.al.RunStepBatch(work)
-                rows = torch.as_tensor([p * self.levels + l for p in todo for l in range(self.levels)],
+                rows = torch.as_tensor([p * self.levels + l for p in photo for l in range(self.levels)],
                                        device=self.records.device)
+                self.records.index_copy_(0, rows, part)
+        if links:
+            items = self._link_items(poses, codes, links)
+            if len(links) == len(self.links):
+                ReprojectionLinearizeBatch(self.al, items, self.records[self.photometric_items:])
+            else:
+                part = ReprojectionLinearizeBatch(self.al, items)
+                rows = torch.as_tensor([self.photometric_items + j for j in links], device=self.records.device)
                 self.records.index_copy_(0, rows, part)
         buf = self.window.assemble(self.records)
         if self.allreduce is not None:

@@ -10,6 +10,9 @@
 //                          [pose_k (6) | code_k (C)] per keyframe; a pair (k0 -> k1) adds its pose0 / code0 blocks to
 //                          keyframe k0's diagonal block, pose1 to k1's, and the pose0-pose1 / pose1-code0 couplings off the
 //                          diagonal.  The buffer is what one NCCL all-reduce sums across ranks.
+//   LinearizeReprojectionBatch
+//                          many reprojection factors (loop closures, use_reprojection links) linearised in one launch
+//                          straight into device records [A^T A | -A^T b | b^T b | inliers] (WindowSystem::AddUnscaled).
 //   LinearizeReprojection / LinearizeSparseGeometric
 //                          the Jacobian rows of the two sparse factors (reprojection_factor.cpp:157-269,
 //                          sparse_geometric_factor.cpp:157-271), evaluated on the device from the keyframes' GPU buffers;
@@ -87,6 +90,21 @@ public:
   // pair (k0 -> k1): keyframe k0 is warped into frame k1 (pose0 / code0 belong to k0, pose1 to k1)
   void Add(int k0, int k1, const JTJJrReductionItem<float, 12 + CS>& sys, int width, int height)
   {
+    AddBlocks(k0, k1, sys);
+    if (sys.inliers > 0) f_ += static_cast<double>(sys.residual) / static_cast<double>(sys.inliers) * width * height;
+  }
+
+  // a reprojection factor (k0 -> k1) as a record of LinearizeReprojectionBatch: same blocks, its residual b^T b enters f
+  // as it is (no photometric rescale)
+  void AddUnscaled(int k0, int k1, const JTJJrReductionItem<float, 12 + CS>& sys)
+  {
+    AddBlocks(k0, k1, sys);
+    f_ += static_cast<double>(sys.residual);
+  }
+
+private:
+  void AddBlocks(int k0, int k1, const JTJJrReductionItem<float, 12 + CS>& sys)
+  {
     const int off[3] = {k0 * Block, k1 * Block, k0 * Block + 6};  // pose0, pose1, code0
     const int loc[3] = {0, 6, 12};
     const int len[3] = {6, 6, CS};
@@ -98,10 +116,8 @@ public:
             H(off[a] + r, off[b] + c) += static_cast<double>(sys.JtJ.toDenseMatrix(loc[a] + r, loc[b] + c));
       }
     }
-    if (sys.inliers > 0) f_ += static_cast<double>(sys.residual) / static_cast<double>(sys.inliers) * width * height;
   }
 
-private:
   int n_;
   std::vector<double> H_, g_;
   double f_;
@@ -136,6 +152,40 @@ SparseRows LinearizeReprojection(DfkHandle h, const SE3T& pose0, const SE3T& pos
   detail::Check(h, dfk_reprojection_linearize(h, pose0.data(), pose1.data(), code0.data(), CS, &c, &p, &j, num_matches,
                                               query_xy, train_xy, huber_delta, sigma, out.rows.data(), &out.total_err));
   return out;
+}
+
+// One factor of LinearizeReprojectionBatch: the arguments of LinearizeReprojection.  code0, query_xy and train_xy are
+// read when LinearizeReprojectionBatch is called (not kept).
+template <int CS, typename SE3T, typename CodeT, typename CamT, typename ImageBuffer>
+DfkReprojectionItem ReprojectionItem(const SE3T& pose0, const SE3T& pose1, const CodeT& code0, const CamT& cam,
+                                     const ImageBuffer& prx_orig, const ImageBuffer& prx_jac, int num_matches,
+                                     const float* query_xy, const float* train_xy, float huber_delta, float sigma)
+{
+  DfkReprojectionItem it{};
+  for (int k = 0; k < 7; ++k) {
+    it.pose0[k] = pose0.data()[k];
+    it.pose1[k] = pose1.data()[k];
+  }
+  it.cam = detail::Cam(cam);
+  it.prx_orig = detail::View(prx_orig, 1);
+  it.prx_jac = detail::View(prx_jac, CS);
+  it.code = code0.data();
+  it.num_matches = num_matches;
+  it.query_xy = query_xy;
+  it.train_xy = train_xy;
+  it.cauchy_delta = huber_delta;
+  it.sigma = sigma;
+  return it;
+}
+
+// Many ReprojectionFactors linearised in one launch into normal-equation records (dfk_reprojection_linearize_batch):
+// record i = [A^T A packed | -A^T b | b^T b | valid matches] of factor i's rows, in the RunStep record layout, at
+// records_dev + i * DFK_SFM_RECORD_FLOATS(CS) (DEVICE).  Asynchronous on the handle's stream; what a window adds with
+// WindowSystem::AddUnscaled, or dfk_window_assemble as an unscaled record (item size 0 x 0).
+template <int CS>
+void LinearizeReprojectionBatch(DfkHandle h, const std::vector<DfkReprojectionItem>& items, float* records_dev)
+{
+  detail::Check(h, dfk_reprojection_linearize_batch(h, items.data(), static_cast<int>(items.size()), CS, records_dev));
 }
 
 // SparseGeometricFactor::linearize (sparse_geometric_factor.cpp:157-271): 1 row per sampled point,

@@ -225,7 +225,8 @@ DfkStatus dfk_sfm_stream_wait(DfkHandle h, DfkSfmStream* s, uint64_t ticket, flo
  *   K diagonal blocks  B x B, row-major, full symmetric
  *   K gradients        B            (g = -sum Jtr)
  *   P coupling blocks  B x 6, row-major: rows = [pose0 | code0] of the pair's keyframe k0, columns = pose1 of its k1
- *   2 scalars          f = sum of rescaled residuals over items with overlap, total inliers (as a float)
+ *   2 scalars          f = sum of rescaled residuals over items with overlap + residuals of unscaled records,
+ *                      total inliers of the scaled (photometric) records (as a float)
  * Deterministic: every output element is summed by one thread in item order (a gather, no float atomics).
  */
 typedef struct DfkWindow DfkWindow;
@@ -237,8 +238,9 @@ typedef struct {
   const int32_t* pair_k0;  /* [num_pairs] keyframe (pose0 / code0) of every pair      (HOST arrays, copied) */
   const int32_t* pair_k1;  /* [num_pairs] frame (pose1)                                                      */
   const int32_t* item_pair;   /* [num_items] pair of every record                                            */
-  const int32_t* item_width;  /* [num_items] level size, for the residual rescale                            */
-  const int32_t* item_height;
+  const int32_t* item_width;  /* [num_items] level size, for the residual rescale; width = height = 0 marks an  */
+  const int32_t* item_height; /* UNSCALED record (dfk_reprojection_linearize_batch): its residual enters f as it is
+                                 and its inliers are left out of the inlier total                                */
 } DfkWindowDesc;
 DfkStatus dfk_window_create(DfkHandle h, const DfkWindowDesc* desc, DfkWindow** out);
 DfkStatus dfk_window_destroy(DfkHandle h, DfkWindow* w);
@@ -337,6 +339,33 @@ DfkStatus dfk_reprojection_linearize(DfkHandle h, const float pose0[7], const fl
                                      const DfkImage* prx_jac, int num_matches, const float* query_xy,
                                      const float* train_xy, float cauchy_delta, float sigma, float* rows,
                                      float* total_err);
+
+/* One ReprojectionFactor of a batch: the arguments of dfk_reprojection_linearize for one factor (k0 -> k1).  A global
+ * loop closure (DeepFactors::ProcessFrame -> Mapper::EnqueueLink(..., rep = true), core/deepfactors.cpp:274,
+ * mapper.cpp:367-376) and the use_reprojection links (mapper.cpp:314-325) are such factors. */
+typedef struct {
+  float pose0[7], pose1[7];
+  DfkCamera cam;                  /* level 0 (cam_pyr_[0], mapper.cpp:317) */
+  DfkImage prx_orig, prx_jac;     /* keyframe k0's level-0 DEVICE buffers */
+  const float* code;              /* HOST, code_size floats: code0 of k0 */
+  int32_t num_matches;
+  const float* query_xy;          /* HOST, 2 floats per match (keypoints in k0) */
+  const float* train_xy;          /* HOST, 2 floats per match (keypoints in k1) */
+  float cauchy_delta, sigma;      /* rep_huber, rep_sigma (or loop_sigma for a loop closure) */
+} DfkReprojectionItem;
+
+/* Batched ReprojectionFactor::linearize straight into normal-equation records: factor i's JacobianFactor [A | b] (the
+ * rows of dfk_reprojection_linearize, bit for bit) contributes H += A^T A, g += A^T b and 1/2 |b|^2 to the energy
+ * (reprojection_factor.cpp:148,254-268), so its record in the RunStep layout (DFK_SFM_RECORD_FLOATS) is
+ *   JtJ = A^T A (packed upper), Jtr = -A^T b, residual = b^T b, inliers = matches with a valid correspondence (u32 bits)
+ * and it enters dfk_window_assemble as an unscaled record (item_width = item_height = 0).  records_dev: DEVICE,
+ * n * DFK_SFM_RECORD_FLOATS(code_size) floats.  One launch, one CTA per factor, a fixed summation order per factor: a
+ * factor's record does not depend on the rest of the batch.  total_err (statistics only) is not computed.
+ * Asynchronous on the handle's stream (no host sync, no D2H); the host arrays may be freed when the call returns.
+ * Every item is validated before anything is enqueued (1 <= n, num_matches >= 1, sigma > 0, consistent views, non-NULL
+ * pointers); a rejected call writes nothing and dfk_last_error names the item. */
+DfkStatus dfk_reprojection_linearize_batch(DfkHandle h, const DfkReprojectionItem* items, int n, int code_size,
+                                           float* records_dev);
 
 /* SparseGeometricFactor::linearize (sources/core/gtsam/sparse_geometric_factor.cpp:157-271): the Jacobian rows of the
  * sparse depth-consistency factor between two keyframes, evaluated on the device from the keyframes' level-0 proximity /

@@ -11,11 +11,17 @@ One JSON line per case:
     GaussianBlurDown at 640x480 -- wall clock per call.
   * CameraTracker::TrackFrame (19 iterations) and Relocalize against K = 8 / 32 keyframes, per keyframe and batched --
     wall clock per call, and for Relocalize the summed device time.
+  * ReprojectionFactor linearisation of K = 32 / 400 factors x 1000 matches at C = 32 / 128: K synchronous
+    ReprojectionLinearize calls + the host A^T A (the only route before the batched call) against one
+    ReprojectionLinearizeBatch -- wall clock and summed device time; and one linearisation of the window200 window
+    (50 keyframes, 200 photometric pairs, 4 levels at 640x480, C = 32) without and with 400 reprojection links.
+Every line carries the card's name and power limit.  `--only reprojection` runs the reprojection cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
 
 import argparse
+import builtins
 import json
 import os
 import sys
@@ -28,6 +34,7 @@ sys.path.insert(0, ROOT)
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--only", choices=["reprojection"], default=None)
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -39,6 +46,18 @@ def main():
     torch.cuda.set_device(0)
     ppath = os.path.join(ROOT, "MEASURED_PEAKS.json")
     peak = float(json.load(open(ppath))["hbm_gbs"]) if os.path.exists(ppath) else 3350.0
+
+    props = torch.cuda.get_device_properties(0)
+    card = {"gpu": props.name, "power_limit_w": _power_limit_w()}
+    _print = builtins.print
+
+    def print(line, **kw):  # noqa: A001 -- every JSON line carries the card it was measured on
+        rec = json.loads(line)
+        rec.update(card)
+        _print(json.dumps(rec), **kw)
+
+    if args.only == "reprojection":
+        return reprojection_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -199,6 +218,127 @@ def main():
                               "us_per_relocalisation": us, "device_us_per_relocalisation": device_us(fn, reps),
                               "timing": "wall clock (synchronous); device time = summed kernel + copy time, "
                                         "torch.profiler"}), flush=True)
+
+    reprojection_cases(args, torch, print)
+
+
+def _power_limit_w():
+    import subprocess
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"],
+                             capture_output=True, text=True, timeout=30)
+        return float(out.stdout.strip().splitlines()[0])
+    except Exception:  # the number is still worth printing; the limit is then unknown
+        return None
+
+
+def _device_us(torch, fn, reps):
+    """summed device time (kernels, copies, memsets) per call, from a separate profiled run"""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            fn()
+        torch.cuda.synchronize()
+    return sum(e.self_device_time_total for e in prof.key_averages()) / reps
+
+
+def _wall_us(torch, fn, reps):
+    for _ in range(2):
+        fn()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(reps):
+        fn()
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t0) / reps * 1e6
+
+
+def reprojection_cases(args, torch, print):
+    """ReprojectionFactor linearisation: K x (dfk_reprojection_linearize + host A^T A) against one
+    dfk_reprojection_linearize_batch; and a window200 linearisation without / with 400 reprojection links."""
+    import numpy as np
+
+    from deepfactors_b200 import se3, synth
+    from deepfactors_b200.aligners import ReprojectionLinearize, ReprojectionLinearizeBatch, SfmAligner
+    dev = torch.device("cuda", 0)
+    M = 1000
+    rng = np.random.default_rng(3)
+
+    def matches(cam):  # keypoints of the keyframe and matched keypoints of the frame, ~1 px apart
+        q = np.stack([rng.uniform(4, cam.width - 5, M), rng.uniform(4, cam.height - 5, M)], axis=1).astype(np.float32)
+        return q, (q + rng.normal(0, 1.0, (M, 2))).astype(np.float32)
+
+    for cs in (32, 128):
+        L = synth.make_level(640, 480, cs, seed=12)
+        prx = torch.from_numpy(L.prx_orig).to(dev)
+        jac = torch.from_numpy(np.ascontiguousarray(L.prx_jac)).to(dev)
+        al = SfmAligner(cs)
+        for K in (32, 400):
+            items = []
+            for k in range(K):
+                q, t = matches(L.cam)
+                items.append(dict(pose0=se3.identity(), pose1=se3.make_pose([0.01 * (k % 5), -0.01, 0.0], [0.05, 0.0, 0.01 * (k % 3)],
+                                                                             np.float32),
+                                  code0=(rng.standard_normal(cs) * 0.1).astype(np.float32), cam=L.cam, prx_orig=prx,
+                                  prx_jac=jac, query_xy=q, train_xy=t, cauchy_delta=1.5, sigma=1.0))
+            rec = torch.empty((K, (12 + cs) * (13 + cs) // 2 + 14 + cs), dtype=torch.float32, device=dev)
+
+            def per_factor():  # rows to the host, then A^T A there (what a JacobianFactor costs the solver)
+                for it in items:
+                    rows, _ = ReprojectionLinearize(al, it["pose0"], it["pose1"], it["code0"], it["cam"], it["prx_orig"],
+                                                    it["prx_jac"], it["query_xy"], it["train_xy"], it["cauchy_delta"],
+                                                    it["sigma"])
+                    r = rows.astype(np.float64)
+                    r.T @ r
+
+            def batched():
+                ReprojectionLinearizeBatch(al, items, rec)
+
+            for name, fn, reps in ((f"K x ReprojectionLinearize + host A^T A", per_factor, 3 if K > 32 else 5),
+                                   (f"one ReprojectionLinearizeBatch", batched, max(5, args.reps))):
+                print(json.dumps({"case": f"ReprojectionFactor linearisation C={cs} K={K} factors x {M} matches: {name}",
+                                  "us_per_linearisation": _wall_us(torch, fn, reps),
+                                  "device_us_per_linearisation": _device_us(torch, fn, reps),
+                                  "host_syncs": K if fn is per_factor else 0,
+                                  "row_bytes_downloaded": K * 2 * M * (13 + cs) * 4 if fn is per_factor else 0,
+                                  "timing": "wall clock (synchronous); device time = summed kernel + copy time, "
+                                            "torch.profiler"}), flush=True)
+
+    # ---- window200 (bench.py --config window200): one linearisation of every factor, without and with 400 links --------
+    from deepfactors_b200.window_opt import ReprojectionLink, SfmWindowProblem
+    sys.path.insert(0, ROOT)
+    from bench import window_pairs
+    cs, levels, num_kf = 32, 4, 50
+    base = synth.make_pair(640, 480, cs, levels, seed=7)
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    shared = [dict(img=up(L.img0), grad=up(L.grad1), prx_orig=up(L.prx_orig), prx_jac=up(L.prx_jac)) for L in base.levels]
+    keyframes = [[dict(sh, dpt=torch.zeros_like(sh["img"]), valid=torch.zeros_like(sh["img"])) for sh in shared]
+                 for _ in range(num_kf)]
+    pairs = window_pairs(num_kf, 200)
+    cam0 = base.levels[0].cam
+    links = []
+    for j in range(400):
+        k0, k1 = (int(v) for v in rng.choice(num_kf, 2, replace=False))
+        q, t = matches(cam0)
+        links.append(ReprojectionLink(k0, k1, q, t, 1.5, 1.0))
+    al = SfmAligner(cs)
+    poses = np.stack([se3.make_pose([0.001 * (k % 7), 0.0, 0.0], [0.002 * (k % 5), 0.0, 0.0], np.float64)
+                      for k in range(num_kf)])
+    codes = np.zeros((num_kf, cs))
+    for n_links in (0, 400):
+        prob = SfmWindowProblem(al, [L.cam for L in base.levels], keyframes, pairs, links=links[:n_links] or None)
+        todo = list(range(len(prob.pairs)))
+
+        def lin():
+            prob.linearise(poses, codes, todo)
+
+        reps = max(5, args.reps // 2)
+        print(json.dumps({"case": f"window200 linearisation (50 keyframes, 200 pairs, 4 levels 640x480, C=32) + {n_links} "
+                                  f"reprojection links x {M} matches",
+                          "us_per_linearisation": _wall_us(torch, lin, reps),
+                          "device_us_per_linearisation": _device_us(torch, lin, reps),
+                          "timing": "wall clock to the end of the assembly (synchronised); device time = summed kernel + "
+                                    "copy time, torch.profiler"}), flush=True)
 
 
 if __name__ == "__main__":
