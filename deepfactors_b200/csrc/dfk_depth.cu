@@ -143,6 +143,11 @@ cudaError_t launch(const float* code_dev, int width, int height, View tgt, View 
 
 size_t depth_partial_floats(int code_size) { return (size_t)(code_size + 1) * (code_size + 2) / 2; }
 
+bool depth_supported(int code_size)
+{
+  return code_size == 8 || code_size == 16 || code_size == 32 || code_size == 64 || code_size == 128;
+}
+
 cudaError_t launch_depth_step(const float* code_dev, int code_size, int width, int height, View tgt, View prx_orig,
                               View jac, float avg_dpt, float* scratch, unsigned int* counter, float* out_dev, int blocks,
                               cudaStream_t s)

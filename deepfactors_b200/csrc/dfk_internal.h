@@ -171,12 +171,14 @@ struct WindowDev {
 cudaError_t launch_window_assemble(const WindowDev& w, const float* records_dev, float* out_dev, cudaStream_t stream);
 
 // dfk_depth.cu : DepthAligner::RunStep
+bool depth_supported(int code_size);
 size_t depth_partial_floats(int code_size);
 cudaError_t launch_depth_step(const float* code_dev, int code_size, int width, int height, View tgt, View prx_orig,
                               View jac, float avg_dpt, float* scratch /*blocks * depth_partial_floats*/,
                               unsigned int* counter, float* out_dev /*C(C+1)/2 + C + 2*/, int blocks, cudaStream_t s);
 
-// dfk_sparse.cu : ReprojectionFactor::linearize rows
+// dfk_sparse.cu : ReprojectionFactor::linearize rows (and records), SparseGeometricFactor::linearize rows
+bool sparse_supported(int code_size);
 struct SparsePose {
   float q[4], t[3], R[9];      // pose_10 = pose1^-1 * pose0
   float P0[36], P1[36];        // pose10_J_pose0 / pose10_J_pose1, row-major 6x6

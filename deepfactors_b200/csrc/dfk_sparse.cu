@@ -292,6 +292,11 @@ sparse_geometric_rows_kernel(SparsePose sp, float cam_w, float cam_h, const floa
 
 }  // namespace
 
+bool sparse_supported(int code_size)
+{
+  return code_size == 8 || code_size == 16 || code_size == 32 || code_size == 64 || code_size == 128;
+}
+
 cudaError_t launch_reprojection_rows(const SparsePose& sp, const float* code_dev, int code_size, View prx_orig, View jac,
                                      int width, int height, int num_matches, const float* query_dev, const float* train_dev,
                                      float cauchy_delta, float sigma, float avg_dpt, float* rows_dev, float* err2_dev,
