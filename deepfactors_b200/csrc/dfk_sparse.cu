@@ -135,8 +135,8 @@ struct RepCfg {
 };
 
 // One CTA per factor: the matches are walked in chunks of CH; every thread of the chunk writes one match's two rows into
-// shared memory, then every thread adds the chunk's rows, in match order (row 2i, then 2i + 1), into the Gram entries it
-// owns.  No atomics: a factor's record depends on that factor only.  The epilogue writes the RunStep record layout:
+// shared memory, then every thread sums the chunk's rows, in match order (row 2i, then 2i + 1), for the Gram entries it
+// owns and adds that chunk sum to its running totals.  No atomics: a factor's record depends on that factor only.  The epilogue writes the RunStep record layout:
 // JtJ = the (12+C) upper block of the Gram of [A | b], Jtr = -A^T b, residual = b^T b, inliers = valid matches.
 template <int C>
 __global__ void __launch_bounds__(RepCfg<C>::NT)
@@ -183,11 +183,18 @@ reprojection_records_kernel(const ReprojItemDev* __restrict__ items, const float
                                          it.cauchy_delta, it.sigma, avg_dpt, r0, r0 + RW, &e2);
     }
     inliers += __syncthreads_count(valid);  // also the barrier between the row writes and the Gram
+    // the chunk's rows are summed on their own and then added to the running total: an entry is a chain of 2 CH
+    // products plus one add per chunk, not one serial chain over all 2M rows (whose fp32 error grows with M)
+    float part[EPT];
+#pragma unroll
+    for (int k = 0; k < EPT; ++k) part[k] = 0.0f;
     for (int r = 0; r < 2 * cnt; ++r) {
       const float* row = rows + r * RW;
 #pragma unroll
-      for (int k = 0; k < EPT; ++k) acc[k] = fmaf(row[ea[k]], row[eb[k]], acc[k]);
+      for (int k = 0; k < EPT; ++k) part[k] = fmaf(row[ea[k]], row[eb[k]], part[k]);
     }
+#pragma unroll
+    for (int k = 0; k < EPT; ++k) acc[k] += part[k];
     __syncthreads();
   }
   float* rec = records + (size_t)blockIdx.x * REC;

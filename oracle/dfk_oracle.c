@@ -99,6 +99,7 @@ void dfko_sfm_run_step_f_omp(const float pose0[7], const float pose1[7], int cod
     acc.JtJ = scratch + (size_t)t * (NH + NP + 2);
     acc.Jtr = acc.JtJ + NH;
     acc.residual = 0; acc.inliers = 0;
+    acc.rows = NULL; acc.width = width; acc.y_begin = 0;
     const int y0 = (int)((long)height * t / nt), y1 = (int)((long)height * (t + 1) / nt);
     sfm_run_rows_f(y0, y1, 1, p10, P0, P1, code_size, &cam, width, img0, img0_pitch, img1, img1_pitch,
                    dpt0, dpt0_pitch, valid0, valid0_pitch, prx0_jac, jac_pitch, grad1, grad1_pitch, prm, &acc);

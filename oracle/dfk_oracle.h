@@ -100,6 +100,24 @@ void dfko_sfm_run_step_d(const float pose0[7], const float pose1[7], int code_si
                          const float* prx0_jac, size_t jac_pitch, const float* grad1, size_t grad1_pitch,
                          const DfkoSfmParams* params, int loop_order,
                          double* JtJ, double* Jtr, double* residual, uint64_t* inliers);
+/* The per-pixel rows the two entry points above sum, for image rows y_begin .. y_end-1: pixel (x, y) writes its
+ * Huber-weighted row [J (NP) | w*diff] at rows[((y - y_begin) * width + x) * (NP + 1)]; rows of invalid pixels are
+ * zero.  Same per-pixel function, so the rows summed in one precision give that precision's JtJ / Jtr up to the
+ * summation order.  valid0 as above (full image, only rows in the range are touched). */
+void dfko_sfm_pixel_rows_f(const float pose0[7], const float pose1[7], int code_size,
+                           const DfkoCamera* cam, int width, int height,
+                           const float* img0, size_t img0_pitch, const float* img1, size_t img1_pitch,
+                           const float* dpt0, size_t dpt0_pitch, float* valid0, size_t valid0_pitch,
+                           const float* prx0_jac, size_t jac_pitch, const float* grad1, size_t grad1_pitch,
+                           const DfkoSfmParams* params, int y_begin, int y_end,
+                           float* rows, float* residual, uint64_t* inliers);
+void dfko_sfm_pixel_rows_d(const float pose0[7], const float pose1[7], int code_size,
+                           const DfkoCamera* cam, int width, int height,
+                           const float* img0, size_t img0_pitch, const float* img1, size_t img1_pitch,
+                           const float* dpt0, size_t dpt0_pitch, float* valid0, size_t valid0_pitch,
+                           const float* prx0_jac, size_t jac_pitch, const float* grad1, size_t grad1_pitch,
+                           const DfkoSfmParams* params, int y_begin, int y_end,
+                           double* rows, double* residual, uint64_t* inliers);
 /* OpenMP row-major variant of the _f path: the multi-threaded CPU baseline. nthreads<=0 => all. */
 void dfko_sfm_run_step_f_omp(const float pose0[7], const float pose1[7], int code_size,
                              const DfkoCamera* cam, int width, int height,

@@ -183,6 +183,33 @@ def sfm_run_step(pose0, pose1, cam, img0, img1, dpt0, valid0, prx0_jac, grad1, p
     return StepResult(JtJ, Jtr, float(res.value), int(inl.value))
 
 
+def sfm_pixel_rows(pose0, pose1, cam, img0, img1, dpt0, valid0, prx0_jac, grad1, params=None, *, y_begin=0,
+                   y_end=None):
+    """The fp64 per-pixel rows that sfm_run_step(..., precision="f64") sums, for image rows y_begin .. y_end-1.
+    Returns (rows [(y_end - y_begin) * W, NP + 1] float64, row-major over the pixels: [J (NP) | w*diff], zero for an
+    invalid pixel; residual of the range; inliers of the range).  valid0: None or the full [H, W] mask (in/out)."""
+    params = params or default_params()
+    img0, img1, dpt0, prx0_jac, grad1 = map(_f32, (img0, img1, dpt0, prx0_jac, grad1))
+    H, W = img0.shape
+    Cs = prx0_jac.shape[2]
+    assert prx0_jac.shape[:2] == (H, W) and grad1.shape == (H, W, 2)
+    y_end = H if y_end is None else min(int(y_end), H)
+    y_begin = max(0, min(int(y_begin), y_end))
+    NP = 12 + Cs
+    pose0 = np.ascontiguousarray(pose0, dtype=np.float32)
+    pose1 = np.ascontiguousarray(pose1, dtype=np.float32)
+    c = _cam(cam)
+    inl = C.c_uint64(0)
+    res = C.c_double(0)
+    rows = np.empty(((y_end - y_begin) * W, NP + 1), dtype=np.float64)
+    vptr, vpitch = (None, C.c_size_t(0)) if valid0 is None else (_ptr(_f32(valid0)), _pitch(valid0))
+    lib().dfko_sfm_pixel_rows_d(_ptr(pose0), _ptr(pose1), C.c_int(Cs), C.byref(c), C.c_int(W), C.c_int(H),
+                                _ptr(img0), _pitch(img0), _ptr(img1), _pitch(img1), _ptr(dpt0), _pitch(dpt0), vptr,
+                                vpitch, _ptr(prx0_jac), _pitch(prx0_jac), _ptr(grad1), _pitch(grad1), C.byref(params),
+                                C.c_int(y_begin), C.c_int(y_end), _ptr(rows, C.c_double), C.byref(res), C.byref(inl))
+    return rows, float(res.value), int(inl.value)
+
+
 def sfm_evaluate_error(pose0, pose1, cam, img0, img1, dpt0, params=None, *, precision="f32"):
     params = params or default_params()
     img0, img1, dpt0 = map(_f32, (img0, img1, dpt0))

@@ -1,5 +1,6 @@
 """GPU tests at BASELINE.json's full sizes (640x480, 4-level pyramid, C=32) through size-independent
-properties -- the oracle would take too long here -- plus the C++ facade test binary:
+properties -- the fp64 comparison of every entry at these sizes is in test_gpu_system_accuracy.py -- plus the
+C++ facade test binary:
   * inliers == number of pixels flagged in valid0; valid0 idempotent (only ever set)
   * additivity: evaluating two complementary pixel sets (the other half made invalid through a negative
     depth) sums to the full evaluation, inliers exactly, JtJ/Jtr/residual to fp32 tolerance
