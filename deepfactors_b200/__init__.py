@@ -13,7 +13,7 @@ __all__ = ["aligners", "synth", "se3", "SfmAligner", "SE3Aligner"]
 _LAZY = {"SfmAligner": "aligners", "SE3Aligner": "aligners", "DepthAligner": "aligners", "Window": "aligners", "SfmAlignerParams": "aligners",
          "DenseSfmParams": "aligners", "UpdateDepth": "aligners", "SobelGradients": "aligners",
          "GaussianBlurDown": "aligners", "SquaredError": "aligners", "ReprojectionLinearize": "aligners",
-         "SparseGeometricLinearize": "aligners"}
+         "SparseGeometricLinearize": "aligners", "SparseGeometricLinearizeBatch": "aligners"}
 
 
 def __getattr__(name):

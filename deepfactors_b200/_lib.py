@@ -68,6 +68,13 @@ class DfkReprojectionItem(C.Structure):
                 ("sigma", C.c_float)]
 
 
+class DfkSparseGeometricItem(C.Structure):
+    _fields_ = [("pose0", C.c_float * 7), ("pose1", C.c_float * 7), ("cam", DfkCamera), ("prx0_orig", DfkImage),
+                ("prx0_jac", DfkImage), ("prx1_orig", DfkImage), ("prx1_jac", DfkImage), ("dpt_grad1", DfkImage),
+                ("code0", C.POINTER(C.c_float)), ("code1", C.POINTER(C.c_float)), ("num_points", C.c_int32),
+                ("points_xy", C.POINTER(C.c_int32)), ("huber_delta", C.c_float)]
+
+
 class DfkWindowDesc(C.Structure):
     _fields_ = [("num_keyframes", C.c_int32), ("num_pairs", C.c_int32), ("num_items", C.c_int32), ("code_size", C.c_int32),
                 ("pair_k0", C.POINTER(C.c_int32)), ("pair_k1", C.POINTER(C.c_int32)), ("item_pair", C.POINTER(C.c_int32)),
@@ -111,6 +118,9 @@ SYMBOLS = {
     "dfk_window_destroy": (C.c_int, [_H, C.c_void_p]),
     "dfk_window_floats": (C.c_size_t, [C.c_void_p]),
     "dfk_window_assemble": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dfk_window_create_geometric": (C.c_int, [_H, C.POINTER(DfkWindowDesc), C.c_int, C.POINTER(C.c_int32),
+                                              C.POINTER(C.c_int32), C.POINTER(C.c_void_p)]),
+    "dfk_window_assemble_geometric": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dfk_se3_run_step": (C.c_int, [_H, _F, _CAM, _IMG, _IMG, _IMG, _IMG, _F, _F, _F, C.POINTER(C.c_uint64)]),
     "dfk_se3_track": (C.c_int, [_H, _F, C.POINTER(DfkTrackLevel), C.c_int, _F, _F, _F, _F, C.c_int]),
     "dfk_se3_track_batch": (C.c_int, [_H, C.c_int, C.c_int, _F, C.POINTER(DfkTrackLevel), _F, _F, _F]),
@@ -121,6 +131,8 @@ SYMBOLS = {
     "dfk_reprojection_linearize_batch": (C.c_int, [_H, C.POINTER(DfkReprojectionItem), C.c_int, C.c_int, C.c_void_p]),
     "dfk_sparse_geometric_linearize": (C.c_int, [_H, _F, _F, _F, _F, C.c_int, _CAM, _IMG, _IMG, _IMG, _IMG, _IMG, C.c_int,
                                                  C.POINTER(C.c_int), C.c_float, _F, C.POINTER(C.c_int)]),
+    "dfk_sparse_geometric_linearize_batch": (C.c_int, [_H, C.POINTER(DfkSparseGeometricItem), C.c_int, C.c_int,
+                                                       C.c_void_p]),
     "dfk_update_depth": (C.c_int, [_H, _F, C.c_int, _IMG, _IMG, C.c_float, _IMG]),
     "dfk_sobel_gradients": (C.c_int, [_H, _IMG, _IMG]),
     "dfk_gaussian_blur_down": (C.c_int, [_H, _IMG, _IMG]),
@@ -156,4 +168,10 @@ def check(handle, status: int):
 
 def record_floats(code_size: int) -> int:
     npar = 12 + code_size
+    return npar * (npar + 1) // 2 + npar + 2
+
+
+def geo_record_floats(code_size: int) -> int:
+    """DFK_GEO_RECORD_FLOATS: a sparse geometric record over [pose0 | pose1 | code0 | code1]"""
+    npar = 12 + 2 * code_size
     return npar * (npar + 1) // 2 + npar + 2

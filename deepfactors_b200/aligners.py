@@ -23,7 +23,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import (DfkCamera, DfkDenseSfmParams, DfkImage, DfkReprojectionItem, DfkSfmAlignerParams, DfkSfmWorkItem,
+from ._lib import (DfkCamera, DfkDenseSfmParams, DfkImage, DfkReprojectionItem, DfkSfmAlignerParams, DfkSparseGeometricItem, DfkSfmWorkItem,
                    DfkTrackLevel, check, lib)
 
 
@@ -349,6 +349,44 @@ def SparseGeometricLinearize(aligner, pose0, pose1, code0, code1, cam, prx0_orig
     return rows, int(nv.value)
 
 
+def SparseGeometricLinearizeBatch(aligner, items: Sequence[dict], records: torch.Tensor | None = None) -> torch.Tensor:
+    """Many SparseGeometricFactors linearised in one launch straight into normal-equation records
+    (dfk_sparse_geometric_linearize_batch): items are dicts with the arguments of SparseGeometricLinearize (pose0, pose1,
+    code0, code1, cam, prx0_orig, prx0_jac, prx1_orig, prx1_jac, dpt_grad1, points_xy, huber_delta).  Record i =
+    [A^T A packed | -A^T b | b^T b | valid points] of factor i's rows over [pose0 | pose1 | code0 | code1]
+    (DFK_GEO_RECORD_FLOATS(CS) floats), which goes into Window.assemble(geo_records=...).  `records` may be a slice of a
+    larger record buffer.  Asynchronous: returns a device tensor [n, DFK_GEO_RECORD_FLOATS(CS)] on torch's current
+    stream."""
+    aligner._hd.use_torch_stream()
+    cs, n = aligner.CS, len(items)
+    rec = _lib.geo_record_floats(cs)
+    if records is None:
+        records = torch.empty((n, rec), dtype=torch.float32, device=f"cuda:{aligner._hd.device}")
+    if not (records.is_contiguous() and records.numel() >= n * rec):
+        raise ValueError(f"records must be a contiguous device tensor of at least {n} x {rec} floats")
+    arr = (DfkSparseGeometricItem * max(n, 1))()
+    keep = []  # the host arrays must outlive the ctypes pointers until the call returns
+    FP, IP = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+    for k, it in enumerate(items):
+        c0 = np.ascontiguousarray(it["code0"], dtype=np.float32)
+        c1 = np.ascontiguousarray(it["code1"], dtype=np.float32)
+        if c0.shape != (cs,) or c1.shape != (cs,):
+            raise ValueError(f"code0 and code1 must have {cs} entries")
+        pts = np.ascontiguousarray(it["points_xy"], dtype=np.int32).reshape(-1, 2)
+        keep += [c0, c1, pts]
+        w = arr[k]
+        w.pose0, w.pose1, w.cam = _pose(it["pose0"]), _pose(it["pose1"]), _cam(it["cam"])
+        w.prx0_orig, w.prx0_jac = _image(it["prx0_orig"]), _image(it["prx0_jac"], cs)
+        w.prx1_orig, w.prx1_jac = _image(it["prx1_orig"]), _image(it["prx1_jac"], cs)
+        w.dpt_grad1 = _image(it["dpt_grad1"], 2)
+        w.code0, w.code1, w.points_xy = c0.ctypes.data_as(FP), c1.ctypes.data_as(FP), pts.ctypes.data_as(IP)
+        w.num_points = pts.shape[0]
+        w.huber_delta = float(it["huber_delta"])
+    check(aligner.handle, lib().dfk_sparse_geometric_linearize_batch(aligner.handle, arr, n, cs,
+                                                                     C.c_void_p(records.data_ptr())))
+    return records
+
+
 # ------------------------------------------------------------------------------------------- DepthAligner
 class DepthAligner:
     """df::DepthAligner<float, CS> (sources/cuda/cu_depthaligner.h:38-54): code-only alignment of the decoded depth to a
@@ -385,12 +423,14 @@ class Window:
     what the factor graph does with the RunStep records of a window -- PhotometricFactor::linearize's block slicing,
     sign flip and residual rescale (sources/core/gtsam/photometric_factor.cpp:105-161,275-282) summed over the window's
     factors (one per pair and level, core/mapping/df_work.cpp:211-225).  `layout` (factors.WindowBlocks) describes the
-    buffer; it is the one buffer a multi-GPU Gauss-Newton step all-reduces."""
+    buffer; it is the one buffer a multi-GPU Gauss-Newton step all-reduces.  `geometric` lists the window's sparse
+    geometric links (k0, k1), one record each (SparseGeometricLinearizeBatch); their blocks follow the scalars."""
 
-    def __init__(self, aligner: "SfmAligner", num_keyframes: int, pairs, item_pair, item_sizes):
+    def __init__(self, aligner: "SfmAligner", num_keyframes: int, pairs, item_pair, item_sizes, geometric=()):
         from .factors import WindowBlocks
         self._al = aligner
-        self.layout = WindowBlocks(int(num_keyframes), aligner.CS, [tuple(map(int, p)) for p in pairs])
+        self.layout = WindowBlocks(int(num_keyframes), aligner.CS, [tuple(map(int, p)) for p in pairs],
+                                   [tuple(map(int, p)) for p in geometric])
         k0 = np.ascontiguousarray([p[0] for p in self.layout.pairs], dtype=np.int32)
         k1 = np.ascontiguousarray([p[1] for p in self.layout.pairs], dtype=np.int32)
         ip = np.ascontiguousarray(item_pair, dtype=np.int32)
@@ -401,19 +441,46 @@ class Window:
                                   k1.ctypes.data_as(I32), ip.ctypes.data_as(I32), iw.ctypes.data_as(I32),
                                   ih.ctypes.data_as(I32))
         self.w = C.c_void_p()
-        check(aligner.handle, lib().dfk_window_create(aligner.handle, C.byref(desc), C.byref(self.w)))
+        L = len(self.layout.geometric)
+        if L:
+            g0 = np.ascontiguousarray([p[0] for p in self.layout.geometric], dtype=np.int32)
+            g1 = np.ascontiguousarray([p[1] for p in self.layout.geometric], dtype=np.int32)
+            check(aligner.handle, lib().dfk_window_create_geometric(aligner.handle, C.byref(desc), L, g0.ctypes.data_as(I32),
+                                                                    g1.ctypes.data_as(I32), C.byref(self.w)))
+        else:
+            check(aligner.handle, lib().dfk_window_create(aligner.handle, C.byref(desc), C.byref(self.w)))
         self.num_items = len(ip)
         self.floats = int(lib().dfk_window_floats(self.w))
         assert self.floats == self.layout.floats
 
-    def assemble(self, records: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
-        """records: [num_items, REC] device tensor written by RunStepBatch.  Asynchronous on torch's current stream."""
+    def assemble(self, records: torch.Tensor, out: torch.Tensor | None = None,
+                 geo_records: torch.Tensor | None = None) -> torch.Tensor:
+        """records: [num_items, REC] device tensor written by RunStepBatch; geo_records: [num_links, GEO_REC] written by
+        SparseGeometricLinearizeBatch (required when the window has links).  Asynchronous on torch's current stream."""
         self._al._hd.use_torch_stream()
+        dev = torch.device(f"cuda:{self._al._hd.device}")
+
+        def need(t, n, what):  # the kernel reads / writes n floats of t on the handle's device
+            if not (t.dtype == torch.float32 and t.device == dev and t.is_contiguous() and t.numel() >= n):
+                raise ValueError(f"{what} must be a contiguous float32 tensor of at least {n} floats on {dev}")
+
+        rec = _lib.record_floats(self.layout.code_size)
+        need(records, self.num_items * rec, "records")
         if out is None:
             out = torch.empty(self.floats, dtype=torch.float32, device=records.device)
-        assert out.is_contiguous() and out.numel() >= self.floats and records.is_contiguous()
-        check(self._al.handle, lib().dfk_window_assemble(self._al.handle, self.w, C.c_void_p(records.data_ptr()),
-                                                         C.c_void_p(out.data_ptr())))
+        need(out, self.floats, "out")
+        if self.layout.geometric and geo_records is None:
+            raise ValueError("the window has geometric links: geo_records is required")
+        if geo_records is not None:
+            need(geo_records, len(self.layout.geometric) * _lib.geo_record_floats(self.layout.code_size), "geo_records")
+        if geo_records is None and not self.layout.geometric:
+            check(self._al.handle, lib().dfk_window_assemble(self._al.handle, self.w, C.c_void_p(records.data_ptr()),
+                                                             C.c_void_p(out.data_ptr())))
+            return out
+        geo = C.c_void_p(geo_records.data_ptr()) if geo_records is not None else None
+        check(self._al.handle, lib().dfk_window_assemble_geometric(self._al.handle, self.w,
+                                                                   C.c_void_p(records.data_ptr()), geo,
+                                                                   C.c_void_p(out.data_ptr())))
         return out
 
     def close(self):

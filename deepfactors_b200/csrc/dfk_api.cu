@@ -92,6 +92,10 @@ struct DfkContext {
   // dfk_reprojection_linearize_batch: [descriptors | codes | query | train] (bytes), one H2D per call from rep_host
   DeviceBuf<unsigned char> rep_dev;
   std::vector<unsigned char> rep_host;
+  // dfk_sparse_geometric_linearize_batch: [descriptors | codes | points] (bytes), one H2D per call from geo_host; apart
+  // from rep_dev so that batches of the two kinds enqueued back to back keep their own staging
+  DeviceBuf<unsigned char> geo_dev;
+  std::vector<unsigned char> geo_host;
   DeviceBuf<SfmItemDev> items_dev;
   DeviceBuf<float> partials_dev;
   // normalised ray tables of the RunStep kernels: they depend on (fx, u0, width, fy, v0, height) only, so they are
@@ -150,7 +154,9 @@ struct DfkSfmStream {
 struct DfkWindow {
   int device = 0;
   WindowDev dev{};
-  DeviceBuf<int> ints;      // one allocation: kf0_ptr | kf0_items | kf1_ptr | kf1_items | pair_ptr | pair_items
+  // one allocation: kf0_ptr | kf0_items | kf1_ptr | kf1_items | pair_ptr | pair_items | lk0_ptr | lk0_links |
+  // lk1_ptr | lk1_links
+  DeviceBuf<int> ints;
   DeviceBuf<float> areas;
   size_t floats = 0;
 };
@@ -1143,8 +1149,15 @@ DfkStatus dfk_squared_error(DfkHandle h, const DfkImage* a, const DfkImage* b, f
 
 DfkStatus dfk_window_create(DfkHandle h, const DfkWindowDesc* d, DfkWindow** out)
 {
+  return dfk_window_create_geometric(h, d, 0, nullptr, nullptr, out);
+}
+
+DfkStatus dfk_window_create_geometric(DfkHandle h, const DfkWindowDesc* d, int L, const int32_t* link_k0,
+                                      const int32_t* link_k1, DfkWindow** out)
+{
   return guarded(h, [&] {
-    if (!d || !out) return fail(h, DFK_ERR_INVALID_ARG, "[Window] null argument");
+    if (!d || !out || L < 0 || (L > 0 && (!link_k0 || !link_k1)))
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window] null argument");
     *out = nullptr;
     const int K = d->num_keyframes, P = d->num_pairs, n = d->num_items;
     if (K <= 0 || P <= 0 || n <= 0 || !d->pair_k0 || !d->pair_k1 || !d->item_pair || !d->item_width || !d->item_height)
@@ -1159,10 +1172,16 @@ DfkStatus dfk_window_create(DfkHandle h, const DfkWindowDesc* d, DfkWindow** out
       if (d->item_pair[i] < 0 || d->item_pair[i] >= P ||
           !((d->item_width[i] > 0 && d->item_height[i] > 0) || (d->item_width[i] == 0 && d->item_height[i] == 0)))
         return fail(h, DFK_ERR_INVALID_ARG, "[Window] record " + std::to_string(i) + " names a pair outside the window");
+    for (int l = 0; l < L; ++l) {
+      if (link_k0[l] < 0 || link_k0[l] >= K || link_k1[l] < 0 || link_k1[l] >= K)
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] link " + std::to_string(l) + " names a keyframe outside the window");
+      if (link_k0[l] == link_k1[l])
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] link " + std::to_string(l) + " ties a keyframe to itself");
+    }
     // one CSR list per key kind (keyframe k0, frame k1, pair): ptr[keys + 1], then the items of each key in item order
     // (the summation order of the gather kernel); returns where the list starts in blob
     std::vector<int> blob;
-    auto add_csr = [&](int keys, auto key_of) {
+    auto add_csr = [&](int keys, int n, auto key_of) {
       const size_t o = blob.size();
       blob.resize(o + keys + 1 + n, 0);
       int* ptr = blob.data() + o;
@@ -1172,9 +1191,11 @@ DfkStatus dfk_window_create(DfkHandle h, const DfkWindowDesc* d, DfkWindow** out
       for (int i = 0; i < n; ++i) ptr[keys + 1 + next[key_of(i)]++] = i;
       return o;
     };
-    const size_t o_kf0 = add_csr(K, [&](int i) { return d->pair_k0[d->item_pair[i]]; });
-    const size_t o_kf1 = add_csr(K, [&](int i) { return d->pair_k1[d->item_pair[i]]; });
-    const size_t o_pair = add_csr(P, [&](int i) { return d->item_pair[i]; });
+    const size_t o_kf0 = add_csr(K, n, [&](int i) { return d->pair_k0[d->item_pair[i]]; });
+    const size_t o_kf1 = add_csr(K, n, [&](int i) { return d->pair_k1[d->item_pair[i]]; });
+    const size_t o_pair = add_csr(P, n, [&](int i) { return d->item_pair[i]; });
+    const size_t o_lk0 = add_csr(K, L, [&](int l) { return link_k0[l]; });
+    const size_t o_lk1 = add_csr(K, L, [&](int l) { return link_k1[l]; });
     std::vector<float> areas(n);
     for (int i = 0; i < n; ++i) areas[i] = (float)d->item_width[i] * (float)d->item_height[i];
 
@@ -1193,8 +1214,11 @@ DfkStatus dfk_window_create(DfkHandle h, const DfkWindowDesc* d, DfkWindow** out
     w->dev.kf1_ptr = ints + o_kf1; w->dev.kf1_items = ints + o_kf1 + K + 1;
     w->dev.pair_ptr = ints + o_pair; w->dev.pair_items = ints + o_pair + P + 1;
     w->dev.item_area = w->areas.ptr;
+    w->dev.num_links = L;
+    w->dev.lk0_ptr = ints + o_lk0; w->dev.lk0_links = ints + o_lk0 + K + 1;
+    w->dev.lk1_ptr = ints + o_lk1; w->dev.lk1_links = ints + o_lk1 + K + 1;
     const size_t B = 6 + (size_t)d->code_size;
-    w->floats = (size_t)K * (B * B + B) + (size_t)P * 6 * B + 2;
+    w->floats = (size_t)K * (B * B + B) + (size_t)P * 6 * B + 2 + (size_t)L * B * B;
     *out = w.release();
     return DFK_OK;
   });
@@ -1215,8 +1239,26 @@ DfkStatus dfk_window_assemble(DfkHandle h, const DfkWindow* w, const float* reco
   return guarded(h, [&] {
     if (!w || !records_dev || !window_dev) return fail(h, DFK_ERR_INVALID_ARG, "[Window] null argument");
     if (w->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[Window] window and handle live on different devices");
+    if (w->dev.num_links > 0)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window] window has geometric links: assemble it with dfk_window_assemble_geometric");
     DeviceGuard guard(h->device);
-    DFK_CUDA(h, launch_window_assemble(w->dev, records_dev, window_dev, h->stream), "[Window] kernel launch failed");
+    DFK_CUDA(h, launch_window_assemble(w->dev, records_dev, nullptr, window_dev, h->stream), "[Window] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_assemble_geometric(DfkHandle h, const DfkWindow* w, const float* records_dev,
+                                        const float* geo_records_dev, float* window_dev)
+{
+  return guarded(h, [&] {
+    if (!w || !records_dev || !window_dev) return fail(h, DFK_ERR_INVALID_ARG, "[Window] null argument");
+    if (w->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[Window] window and handle live on different devices");
+    if (w->dev.num_links > 0 && !geo_records_dev)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window] window has geometric links but no geometric records");
+    DeviceGuard guard(h->device);
+    DFK_CUDA(h, launch_window_assemble(w->dev, records_dev, geo_records_dev, window_dev, h->stream),
+             "[Window] kernel launch failed");
     h->launches += 1;
     return DFK_OK;
   });
@@ -1584,6 +1626,78 @@ DfkStatus dfk_sparse_geometric_linearize(DfkHandle h, const float pose0[7], cons
       }
       *num_valid = nv;
     }
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_sparse_geometric_linearize_batch(DfkHandle h, const DfkSparseGeometricItem* items, int n, int code_size,
+                                               float* records_dev)
+{
+  return guarded(h, [&] {
+    if (!items || n < 1 || !records_dev)
+      return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::linearize batch] null argument / empty batch");
+    if (!sparse_supported(code_size))
+      return fail(h, DFK_ERR_UNSUPPORTED,
+                  "[SparseGeometricFactor::linearize batch] code size not instantiated: " + std::to_string(code_size));
+    size_t total = 0;  // points of the whole batch
+    for (int i = 0; i < n; ++i) {
+      const DfkSparseGeometricItem& it = items[i];
+      const std::string at = "[SparseGeometricFactor::linearize batch] item " + std::to_string(i) + ": ";
+      if (!it.code0 || !it.code1 || !it.points_xy) return fail(h, DFK_ERR_INVALID_ARG, at + "null argument");
+      if (it.num_points < 1 || !(it.huber_delta > 0.0f))
+        return fail(h, DFK_ERR_INVALID_ARG, at + "no points / non-positive huber delta");
+      const uint32_t W = it.prx0_orig.width, H = it.prx0_orig.height;
+      if (W == 0 || H == 0 || !img_ok(&it.prx0_orig, W, H, 1) || !img_ok(&it.prx0_jac, W, H, code_size) ||
+          !img_ok(&it.prx1_orig, W, H, 1) || !img_ok(&it.prx1_jac, W, H, code_size) || !img_ok(&it.dpt_grad1, W, H, 2))
+        return fail(h, DFK_ERR_INVALID_ARG, at + "inconsistent image views");
+      if (!cam_ok(&it.cam, W, H)) return fail(h, DFK_ERR_INVALID_ARG, at + "camera larger than the image views");
+      total += (size_t)it.num_points;
+    }
+    if (total > (size_t)INT32_MAX)
+      return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::linearize batch] more than 2^31 - 1 points in one call");
+    DeviceGuard guard(h->device);
+    // one upload: [descriptors n | codes n x 2C (code0, code1) | points 2 total]
+    const size_t desc_bytes = (sizeof(GeoItemDev) * (size_t)n + 15) & ~(size_t)15;
+    const size_t code_bytes = sizeof(float) * 2 * (size_t)n * code_size;
+    const size_t point_bytes = sizeof(int32_t) * 2 * total;
+    const size_t bytes = desc_bytes + code_bytes + point_bytes;
+    DFK_CUDA(h, h->geo_dev.ensure(bytes), "[SparseGeometricFactor::linearize batch] scratch allocation failed");
+    h->geo_host.assign(bytes, 0);
+    GeoItemDev* descs = reinterpret_cast<GeoItemDev*>(h->geo_host.data());
+    float* codes = reinterpret_cast<float*>(h->geo_host.data() + desc_bytes);
+    int32_t* points = reinterpret_cast<int32_t*>(h->geo_host.data() + desc_bytes + code_bytes);
+    const float* codes_dev = reinterpret_cast<const float*>(h->geo_dev.ptr + desc_bytes);
+    const int* points_dev = reinterpret_cast<const int*>(h->geo_dev.ptr + desc_bytes + code_bytes);
+    size_t begin = 0;
+    for (int i = 0; i < n; ++i) {
+      const DfkSparseGeometricItem& it = items[i];
+      GeoItemDev& d = descs[i];
+      set_relative_pose(d.sp, it.pose1, it.pose0, it.cam);  // as dfk_sparse_geometric_linearize
+      d.prx0 = view_of(&it.prx0_orig);
+      d.jac0 = view_of(&it.prx0_jac);
+      d.prx1 = view_of(&it.prx1_orig);
+      d.jac1 = view_of(&it.prx1_jac);
+      d.grad1 = view_of(&it.dpt_grad1);
+      d.code0 = codes_dev + 2 * (size_t)i * code_size;
+      d.code1 = d.code0 + code_size;
+      d.cam_w = it.cam.width;
+      d.cam_h = it.cam.height;
+      d.width = (int)it.prx0_orig.width;
+      d.height = (int)it.prx0_orig.height;
+      d.num_points = it.num_points;
+      d.point_begin = (int)begin;
+      d.huber_delta = it.huber_delta;
+      memcpy(codes + 2 * (size_t)i * code_size, it.code0, sizeof(float) * code_size);
+      memcpy(codes + (2 * (size_t)i + 1) * code_size, it.code1, sizeof(float) * code_size);
+      memcpy(points + 2 * begin, it.points_xy, sizeof(int32_t) * 2 * it.num_points);
+      begin += (size_t)it.num_points;
+    }
+    DFK_CUDA(h, cudaMemcpyAsync(h->geo_dev.ptr, h->geo_host.data(), bytes, cudaMemcpyHostToDevice, h->stream),
+             "[SparseGeometricFactor::linearize batch] upload failed");
+    DFK_CUDA(h, launch_sparse_geometric_records(code_size, reinterpret_cast<const GeoItemDev*>(h->geo_dev.ptr), n,
+                                                points_dev, h->params.sfmparams.avg_dpt, records_dev, h->stream),
+             "[SparseGeometricFactor::linearize batch] kernel launch failed");
+    h->launches += 1;
     return DFK_OK;
   });
 }

@@ -167,8 +167,15 @@ struct WindowDev {
   const int* pair_ptr;    // [P+1] items of pair p (its levels)
   const int* pair_items;
   const float* item_area; // [n] W * H of the item's level
+  int num_links;          // geometric links (k0 -> k1), one record of DFK_GEO_RECORD_FLOATS each
+  const int* lk0_ptr;     // [K+1] links whose k0 is k ...
+  const int* lk0_links;   // ... in link order
+  const int* lk1_ptr;     // [K+1] links whose k1 is k
+  const int* lk1_links;
 };
-cudaError_t launch_window_assemble(const WindowDev& w, const float* records_dev, float* out_dev, cudaStream_t stream);
+// geo_records_dev may be null when num_links == 0
+cudaError_t launch_window_assemble(const WindowDev& w, const float* records_dev, const float* geo_records_dev,
+                                   float* out_dev, cudaStream_t stream);
 
 // dfk_depth.cu : DepthAligner::RunStep
 bool depth_supported(int code_size);
@@ -206,6 +213,21 @@ cudaError_t launch_sparse_geometric_rows(const SparsePose& sp, float cam_w, floa
                                          const float* code1_dev, int code_size, View prx0, View jac0, View prx1, View jac1,
                                          View grad1, int width, int height, int num_points, const int* points_dev,
                                          float huber_delta, float avg_dpt, float* rows_dev, cudaStream_t s);
+// One factor of dfk_sparse_geometric_linearize_batch: what launch_sparse_geometric_rows takes for it.  Its points are
+// points[point_begin, + num_points); code0 / code1 point at its code_size floats each in device scratch.
+struct GeoItemDev {
+  SparsePose sp;
+  View prx0, jac0, prx1, jac1, grad1;
+  const float* code0;
+  const float* code1;
+  float cam_w, cam_h;
+  int width, height;
+  int num_points, point_begin;
+  float huber_delta;
+};
+// grid (num_items, 1 or 4 entry slices); records_dev: num_items records of DFK_GEO_RECORD_FLOATS(code_size) floats
+cudaError_t launch_sparse_geometric_records(int code_size, const GeoItemDev* items_dev, int num_items, const int* points_dev,
+                                            float avg_dpt, float* records_dev, cudaStream_t s);
 
 constexpr int kSimpleMaxBlocks = 1024;
 constexpr int kSimpleScratchFloats = kSimpleMaxBlocks * 32;

@@ -1,6 +1,7 @@
 // dfk_sparse.cu -- the sparse factors on the device: ReprojectionFactor::linearize
 // (sources/core/gtsam/reprojection_factor.cpp:157-269), the same factors batched straight into normal-equation records
-// (reprojection_records_kernel), and SparseGeometricFactor::linearize (second half of the file).
+// (reprojection_records_kernel), and SparseGeometricFactor::linearize (second half of the file), rows and records
+// (sparse_geometric_records_kernel).  Both records kernels share one Gram scaffold (gram_records).
 //
 // The reference evaluates this sparse keypoint factor on the CPU and, to read the code Jacobian at <= a few thousand
 // keypoints, forces a device -> host mirror of the keyframe's WHOLE level-0 code-Jacobian pyramid
@@ -122,45 +123,54 @@ reprojection_rows_kernel(SparsePose sp, const float* __restrict__ code, View prx
   err2[i] = e2;
 }
 
-// Geometry of the batched kernel: NT threads, CH matches per chunk (their 2 CH rows of RW floats are the dynamic shared
-// memory), EPT entries of the packed upper triangle of the augmented (13+C)^2 Gram per thread.
-template <int C>
-struct RepCfg {
-  static constexpr int RW = 13 + C;
-  static constexpr int NT = C >= 64 ? 256 : 128;
-  static constexpr int CH = C >= 64 ? 64 : 128;
+// Geometry of a batched records kernel: rows of RW floats, RPI rows per item (2 per reprojection match, 1 per geometric
+// point), NT threads, CH items per chunk (their RPI CH rows are the dynamic shared memory), NS CTAs per factor.  CTA s of
+// a factor owns the slice [s NT EPT, (s + 1) NT EPT) of the packed upper triangle of the augmented RW^2 Gram, EPT entries
+// per thread; every CTA of the factor recomputes the chunk rows itself.
+template <int RW_, int RPI_, int NT_, int CH_, int NS_>
+struct GramCfg {
+  static constexpr int RW = RW_, RPI = RPI_, NT = NT_, CH = CH_, NS = NS_;
   static constexpr int NE = RW * (RW + 1) / 2;
-  static constexpr int EPT = (NE + NT - 1) / NT;
-  static constexpr size_t SMEM = sizeof(float) * 2 * CH * RW;
+  static constexpr int EPT = (NE + NT * NS - 1) / (NT * NS);
+  static constexpr size_t SMEM = sizeof(float) * RPI * CH * RW;
 };
-
-// One CTA per factor: the matches are walked in chunks of CH; every thread of the chunk writes one match's two rows into
-// shared memory, then every thread sums the chunk's rows, in match order (row 2i, then 2i + 1), for the Gram entries it
-// owns and adds that chunk sum to its running totals.  No atomics: a factor's record depends on that factor only.  The epilogue writes the RunStep record layout:
-// JtJ = the (12+C) upper block of the Gram of [A | b], Jtr = -A^T b, residual = b^T b, inliers = valid matches.
 template <int C>
-__global__ void __launch_bounds__(RepCfg<C>::NT)
-reprojection_records_kernel(const ReprojItemDev* __restrict__ items, const float2* __restrict__ query,
-                            const float2* __restrict__ train, float avg_dpt, float* __restrict__ records)
+using RepCfg = GramCfg<13 + C, 2, C >= 64 ? 256 : 128, C >= 64 ? 64 : 128, 1>;
+// C = 128: 36315 entries, four CTAs of 256 x 36 per factor
+template <int C>
+using GeoCfg = GramCfg<13 + 2 * C, 1, C >= 32 ? 256 : 128, C >= 128 ? 64 : 128, C >= 128 ? 4 : 1>;
+
+// a factor's descriptor into shared memory, word by word; ends with the barrier that publishes it
+template <int NT, class Item>
+__device__ __forceinline__ void load_item(const Item* __restrict__ src_item, Item& it)
 {
-  using Cfg = RepCfg<C>;
-  constexpr int RW = Cfg::RW, NP = 12 + C, NH = NP * (NP + 1) / 2, REC = NH + NP + 2;
-  constexpr int NT = Cfg::NT, CH = Cfg::CH, EPT = Cfg::EPT;
-  extern __shared__ float rows[];  // [2 CH][RW]
-  __shared__ ReprojItemDev it;
-  {
-    static_assert(sizeof(ReprojItemDev) % 4 == 0, "descriptor copied as words");
-    const uint32_t* src = reinterpret_cast<const uint32_t*>(items + blockIdx.x);
-    uint32_t* dst = reinterpret_cast<uint32_t*>(&it);
-    for (int k = threadIdx.x; k < (int)(sizeof(ReprojItemDev) / 4); k += NT) dst[k] = src[k];
-  }
-  // the entries this thread owns: e = threadIdx.x + k NT of the packed upper triangle, (ea[k], eb[k]) in [0, RW)^2
+  static_assert(sizeof(Item) % 4 == 0, "descriptor copied as words");
+  const uint32_t* src = reinterpret_cast<const uint32_t*>(src_item);
+  uint32_t* dst = reinterpret_cast<uint32_t*>(&it);
+  for (int k = threadIdx.x; k < (int)(sizeof(Item) / 4); k += NT) dst[k] = src[k];
+  __syncthreads();
+}
+
+// The Gram scaffold of the batched kernels.  Factor blockIdx.x has M items; item_rows(i, rows) writes item i's RPI rows
+// and returns whether it is valid.  The items are walked in chunks of CH; every thread of the chunk writes one item's
+// rows into shared memory, then every thread sums the chunk's rows, in row order, for the Gram entries it owns and adds
+// that chunk sum to its running totals.  No atomics: a factor's record depends on that factor only, and each entry has
+// one owner whatever the grid.  The epilogue writes the RunStep record layout: JtJ = the (RW-1) upper block of the Gram
+// of [A | b], Jtr = -A^T b, residual = b^T b, inliers = valid items.
+template <class Cfg, class RowFn>
+__device__ __forceinline__ void gram_records(int M, float* __restrict__ records, RowFn item_rows)
+{
+  constexpr int RW = Cfg::RW, NP = RW - 1, NH = NP * (NP + 1) / 2, REC = NH + NP + 2;
+  constexpr int NT = Cfg::NT, CH = Cfg::CH, EPT = Cfg::EPT, RPI = Cfg::RPI;
+  extern __shared__ float rows[];  // [RPI CH][RW]
+  const int e0 = blockIdx.y * NT * EPT;  // first entry of this CTA's slice
+  // the entries this thread owns: e = e0 + threadIdx.x + k NT of the packed upper triangle, (ea[k], eb[k]) in [0, RW)^2
   int ea[EPT], eb[EPT];
   {
     int a = 0, first = 0;  // first = packed index of (a, a)
 #pragma unroll
     for (int k = 0; k < EPT; ++k) {
-      const int e = threadIdx.x + k * NT;
+      const int e = e0 + threadIdx.x + k * NT;
       while (a < RW - 1 && e >= first + (RW - a)) { first += RW - a; ++a; }
       ea[k] = e < Cfg::NE ? a : 0;
       eb[k] = e < Cfg::NE ? a + (e - first) : 0;
@@ -169,26 +179,18 @@ reprojection_records_kernel(const ReprojItemDev* __restrict__ items, const float
   float acc[EPT];
 #pragma unroll
   for (int k = 0; k < EPT; ++k) acc[k] = 0.0f;
-  __syncthreads();
-  const int M = it.num_matches;
   int inliers = 0;
   for (int base = 0; base < M; base += CH) {
     const int cnt = min(CH, M - base);
     bool valid = false;
-    if ((int)threadIdx.x < cnt) {
-      const int i = it.match_begin + base + threadIdx.x;
-      float* r0 = rows + 2 * threadIdx.x * RW;
-      float e2;
-      valid = reprojection_match_rows<C>(it.sp, it.code, it.prx_orig, it.jac, it.width, it.height, query[i], train[i],
-                                         it.cauchy_delta, it.sigma, avg_dpt, r0, r0 + RW, &e2);
-    }
+    if ((int)threadIdx.x < cnt) valid = item_rows(base + threadIdx.x, rows + RPI * threadIdx.x * RW);
     inliers += __syncthreads_count(valid);  // also the barrier between the row writes and the Gram
-    // the chunk's rows are summed on their own and then added to the running total: an entry is a chain of 2 CH
-    // products plus one add per chunk, not one serial chain over all 2M rows (whose fp32 error grows with M)
+    // the chunk's rows are summed on their own and then added to the running total: an entry is a chain of RPI CH
+    // products plus one add per chunk, not one serial chain over all rows (whose fp32 error grows with M)
     float part[EPT];
 #pragma unroll
     for (int k = 0; k < EPT; ++k) part[k] = 0.0f;
-    for (int r = 0; r < 2 * cnt; ++r) {
+    for (int r = 0; r < RPI * cnt; ++r) {
       const float* row = rows + r * RW;
 #pragma unroll
       for (int k = 0; k < EPT; ++k) part[k] = fmaf(row[ea[k]], row[eb[k]], part[k]);
@@ -200,13 +202,29 @@ reprojection_records_kernel(const ReprojItemDev* __restrict__ items, const float
   float* rec = records + (size_t)blockIdx.x * REC;
 #pragma unroll
   for (int k = 0; k < EPT; ++k) {
-    if ((int)threadIdx.x + k * NT >= Cfg::NE) break;
+    if (e0 + (int)threadIdx.x + k * NT >= Cfg::NE) break;
     const int a = ea[k], b = eb[k];
     if (b < NP) rec[a * NP - (a * (a - 1)) / 2 + (b - a)] = acc[k];  // JtJ
     else if (a < NP) rec[NH + a] = -acc[k];                          // Jtr = -A^T b
     else rec[NH + NP] = acc[k];                                      // residual = b^T b
   }
-  if (threadIdx.x == 0) rec[NH + NP + 1] = __uint_as_float((uint32_t)inliers);
+  if (threadIdx.x == 0 && blockIdx.y == 0) rec[NH + NP + 1] = __uint_as_float((uint32_t)inliers);
+}
+
+// One CTA per factor, two rows per match (row 2i, then 2i + 1).
+template <int C>
+__global__ void __launch_bounds__(RepCfg<C>::NT)
+reprojection_records_kernel(const ReprojItemDev* __restrict__ items, const float2* __restrict__ query,
+                            const float2* __restrict__ train, float avg_dpt, float* __restrict__ records)
+{
+  __shared__ ReprojItemDev it;
+  load_item<RepCfg<C>::NT>(items + blockIdx.x, it);
+  gram_records<RepCfg<C>>(it.num_matches, records, [&](int m, float* r0) {
+    const int i = it.match_begin + m;
+    float e2;
+    return reprojection_match_rows<C>(it.sp, it.code, it.prx_orig, it.jac, it.width, it.height, query[i], train[i],
+                                      it.cauchy_delta, it.sigma, avg_dpt, r0, r0 + 13 + C, &e2);
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -224,18 +242,17 @@ reprojection_records_kernel(const ReprojItemDev* __restrict__ items, const float
 //   everything * HuberWeight(err, huber_delta)                                                     :252-258
 // The decode and the validity chain use round-to-nearest intrinsics in the reference's operation order (as the dense
 // kernels do), so the set of valid rows and the nearest-neighbour pixels are those of the CPU evaluation.
+//
+// The per-point body: writes the point's row r (zero when the correspondence is invalid) and returns whether it is valid.
+// Shared by the single-factor kernel and the batched one, so the batched rows are those of dfk_sparse_geometric_linearize
+// by construction.
 template <int C>
-__global__ void __launch_bounds__(128)
-sparse_geometric_rows_kernel(SparsePose sp, float cam_w, float cam_h, const float* __restrict__ code0,
-                             const float* __restrict__ code1, View prx0, View jac0, View prx1, View jac1, View grad1, int width,
-                             int height, int num_points, const int2* __restrict__ points, float huber_delta, float avg_dpt,
-                             float* __restrict__ rows)
+__device__ __forceinline__ bool sparse_geometric_point_row(const SparsePose& sp, float cam_w, float cam_h,
+                                                           const float* __restrict__ code0, const float* __restrict__ code1,
+                                                           View prx0, View jac0, View prx1, View jac1, View grad1, int width,
+                                                           int height, int2 pt, float huber_delta, float avg_dpt, float* r)
 {
   constexpr int RW = 13 + 2 * C;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= num_points) return;
-  float* r = rows + (size_t)i * RW;
-  const int2 pt = points[i];
   bool valid = pt.x >= 0 && pt.y >= 0 && pt.x < width && pt.y < height;  // the reference would read out of bounds
   Warped w;
   w.valid = false;
@@ -252,7 +269,7 @@ sparse_geometric_rows_kernel(SparsePose sp, float cam_w, float cam_h, const floa
   }
   if (!valid) {
     for (int k = 0; k < RW; ++k) r[k] = 0.0f;
-    return;
+    return false;
   }
   const int nx = (int)w.u, ny = (int)w.v;  // pix1.cast<int>()
   const float* jr1 = jac1.ptr + (size_t)ny * jac1.pitch + (size_t)nx * C;
@@ -295,6 +312,35 @@ sparse_geometric_rows_kernel(SparsePose sp, float cam_w, float cam_h, const floa
     r[12 + C + k] = e1 * __ldg(jr1 + k);
   }
   r[12 + 2 * C] = err * hw;
+  return true;
+}
+
+template <int C>
+__global__ void __launch_bounds__(128)
+sparse_geometric_rows_kernel(SparsePose sp, float cam_w, float cam_h, const float* __restrict__ code0,
+                             const float* __restrict__ code1, View prx0, View jac0, View prx1, View jac1, View grad1, int width,
+                             int height, int num_points, const int2* __restrict__ points, float huber_delta, float avg_dpt,
+                             float* __restrict__ rows)
+{
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= num_points) return;
+  sparse_geometric_point_row<C>(sp, cam_w, cam_h, code0, code1, prx0, jac0, prx1, jac1, grad1, width, height, points[i],
+                                huber_delta, avg_dpt, rows + (size_t)i * (13 + 2 * C));
+}
+
+// Factor blockIdx.x, entry slice blockIdx.y (GeoCfg<C>::NS CTAs per factor), one row per point.
+template <int C>
+__global__ void __launch_bounds__(GeoCfg<C>::NT)
+sparse_geometric_records_kernel(const GeoItemDev* __restrict__ items, const int2* __restrict__ points, float avg_dpt,
+                                float* __restrict__ records)
+{
+  __shared__ GeoItemDev it;
+  load_item<GeoCfg<C>::NT>(items + blockIdx.x, it);
+  gram_records<GeoCfg<C>>(it.num_points, records, [&](int m, float* r) {
+    return sparse_geometric_point_row<C>(it.sp, it.cam_w, it.cam_h, it.code0, it.code1, it.prx0, it.jac0, it.prx1, it.jac1,
+                                         it.grad1, it.width, it.height, points[it.point_begin + m], it.huber_delta, avg_dpt,
+                                         r);
+  });
 }
 
 }  // namespace
@@ -377,6 +423,31 @@ cudaError_t launch_sparse_geometric_rows(const SparsePose& sp, float cam_w, floa
     default: return cudaErrorInvalidValue;
   }
 #undef DFK_SG
+  return cudaGetLastError();
+}
+
+cudaError_t launch_sparse_geometric_records(int code_size, const GeoItemDev* items_dev, int num_items, const int* points_dev,
+                                            float avg_dpt, float* records_dev, cudaStream_t s)
+{
+  const int2* pts = reinterpret_cast<const int2*>(points_dev);
+#define DFK_GR(CS)                                                                                                      \
+  case CS: {                                                                                                            \
+    cudaError_t e = cudaFuncSetAttribute(sparse_geometric_records_kernel<CS>,                                           \
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GeoCfg<CS>::SMEM);           \
+    if (e != cudaSuccess) return e;                                                                                     \
+    sparse_geometric_records_kernel<CS><<<dim3(num_items, GeoCfg<CS>::NS), GeoCfg<CS>::NT, GeoCfg<CS>::SMEM, s>>>(      \
+        items_dev, pts, avg_dpt, records_dev);                                                                          \
+    break;                                                                                                              \
+  }
+  switch (code_size) {
+    DFK_GR(8)
+    DFK_GR(16)
+    DFK_GR(32)
+    DFK_GR(64)
+    DFK_GR(128)
+    default: return cudaErrorInvalidValue;
+  }
+#undef DFK_GR
   return cudaGetLastError();
 }
 

@@ -17,7 +17,7 @@ aligners, so that a sharded evaluation can be reduced into one set of normal equ
 """
 from __future__ import annotations
 
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from typing import List, Sequence, Tuple
 
 import numpy as np
@@ -30,10 +30,28 @@ def record_layout(code_size: int) -> Tuple[int, int, int]:
     return n, nh, nh + n + 2
 
 
+def geo_record_layout(code_size: int) -> Tuple[int, int, int]:
+    """(NG, NH, record_floats) of a sparse geometric record over [pose0 | pose1 | code0 | code1] (DFK_GEO_RECORD_FLOATS)."""
+    n = 12 + 2 * code_size
+    nh = n * (n + 1) // 2
+    return n, nh, nh + n + 2
+
+
 def unpack_records(records, code_size: int):
     """records: [n, REC] float32 (numpy or torch, host or device) -> dense JtJ [n,NP,NP], Jtr [n,NP], residual [n],
     inliers [n] (int64), computed with the array library the input comes from."""
-    n, nh, rec = record_layout(code_size)
+    n, nh, _ = record_layout(code_size)
+    return _unpack(records, n, nh)
+
+
+def unpack_geometric_records(records, code_size: int):
+    """unpack_records for sparse geometric records: JtJ [n, NG, NG] over [pose0 | pose1 | code0 | code1], Jtr [n, NG],
+    residual [n], inliers [n] = valid points."""
+    n, nh, _ = geo_record_layout(code_size)
+    return _unpack(records, n, nh)
+
+
+def _unpack(records, n: int, nh: int):
     if hasattr(records, "detach"):  # torch
         import torch
         r = records
@@ -126,10 +144,12 @@ def is_unscaled(size) -> bool:
 class WindowBlocks:
     """The packed block-sparse buffer dfk_window_assemble writes (include/dfk.h, SURVEY 8e): K diagonal blocks B x B,
     K gradients B, P coupling blocks B x 6 ([pose0 | code0] of k0 x pose1 of k1), then f and the inlier total of the
-    photometric (scaled) records."""
+    photometric (scaled) records, then L link blocks B x B ([pose0 | code0] of k0 x [pose1 | code1] of k1), one per
+    sparse geometric link in `geometric`."""
     num_keyframes: int
     code_size: int
     pairs: Sequence[Tuple[int, int]]
+    geometric: Sequence[Tuple[int, int]] = field(default=())
 
     @property
     def B(self) -> int:
@@ -138,7 +158,7 @@ class WindowBlocks:
     @property
     def floats(self) -> int:
         K, P, B = self.num_keyframes, len(self.pairs), self.B
-        return K * (B * B + B) + P * 6 * B + 2
+        return K * (B * B + B) + P * 6 * B + 2 + len(self.geometric) * B * B
 
     def offsets(self):
         K, P, B = self.num_keyframes, len(self.pairs), self.B
@@ -147,10 +167,17 @@ class WindowBlocks:
         o_t = o_c + P * 6 * B
         return o_g, o_c, o_t
 
-    def pack(self, item_pair, JtJ, Jtr, residual, inliers, sizes):
+    @property
+    def geometric_offset(self) -> int:
+        """start of the link blocks, after f and the inlier total"""
+        return self.offsets()[2] + 2
+
+    def pack(self, item_pair, JtJ, Jtr, residual, inliers, sizes, geo=None):
         """Host mirror of dfk_window_assemble (numpy, float32 sums in item order): item i belongs to pair item_pair[i];
         JtJ [n, NP, NP] dense, Jtr [n, NP], sizes[i] = (W, H), or (0, 0) for an unscaled record: its residual is added
-        to f as it is and its inliers are left out of the inlier total.  Returns the flat buffer."""
+        to f as it is and its inliers are left out of the inlier total.  geo = (JtJ [L, NG, NG], Jtr [L, NG],
+        residual [L]) of the geometric links (dfk_window_assemble_geometric): after the items, the links where a
+        keyframe is k0, then those where it is k1, in link order.  Returns the flat buffer."""
         K, B, c = self.num_keyframes, self.B, self.code_size
         out = np.zeros(self.floats, dtype=np.float32)
         o_g, o_c, o_t = self.offsets()
@@ -176,6 +203,21 @@ class WindowBlocks:
             if inl > 0:
                 f += np.float32(residual[i]) / np.float32(inl) * np.float32(sizes[i][0] * sizes[i][1])
             ninl += np.float32(inl)
+        if self.geometric:
+            gJ, gr, gres = geo
+            loc1 = np.r_[6:12, 12 + c:12 + 2 * c]  # [pose1 | code1] rows of a geometric record
+            Lb = out[self.geometric_offset:].reshape(len(self.geometric), B, B)
+            for l, (k0, k1) in enumerate(self.geometric):
+                H = np.asarray(gJ[l], dtype=np.float32)
+                D[k0] += H[np.ix_(loc0, loc0)]
+                g[k0] -= np.asarray(gr[l], dtype=np.float32)[loc0]
+                Lb[l] = H[np.ix_(loc0, loc1)]
+            for l, (k0, k1) in enumerate(self.geometric):
+                H = np.asarray(gJ[l], dtype=np.float32)
+                D[k1] += H[np.ix_(loc1, loc1)]
+                g[k1] -= np.asarray(gr[l], dtype=np.float32)[loc1]
+            for l in range(len(self.geometric)):
+                f += np.float32(gres[l])
         out[o_t] = f
         out[o_t + 1] = ninl
         return out
@@ -200,6 +242,11 @@ class WindowBlocks:
         for p, (k0, k1) in enumerate(self.pairs):
             H[k0 * B:(k0 + 1) * B, k1 * B:k1 * B + 6] += O[p]
             H[k1 * B:k1 * B + 6, k0 * B:(k0 + 1) * B] += O[p].T if not is_torch else O[p].transpose(0, 1)
+        if self.geometric:
+            Lb = b64[self.geometric_offset:self.floats].reshape(len(self.geometric), B, B)
+            for l, (k0, k1) in enumerate(self.geometric):
+                H[k0 * B:(k0 + 1) * B, k1 * B:(k1 + 1) * B] += Lb[l]
+                H[k1 * B:(k1 + 1) * B, k0 * B:(k0 + 1) * B] += Lb[l].T if not is_torch else Lb[l].transpose(0, 1)
         g = b64[o_g:o_c].reshape(K * B)
         return H, g, float(b64[o_t]), float(b64[o_t + 1])
 

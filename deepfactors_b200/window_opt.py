@@ -14,6 +14,7 @@ solves.  Here every heavy step of one iteration is ONE device operation over the
     solve       damped dense solve on the device (Cholesky, float64)                     torch.linalg
     (links)     one batched launch over the stale reprojection links (global loop closures, use_reprojection),
                 straight into normal-equation records                                  dfk_reprojection_linearize_batch
+                and one over the stale sparse geometric links (use_geometric)          dfk_sparse_geometric_linearize_batch
     retract     pose: t += dt, R = exp(w) R (gtsam_traits.h:48-58); code += dc           (tiny, host)
     accept      Levenberg-Marquardt on the energy f: rescaled photometric residuals + b^T b of the links (what the
                 factors' error() return)
@@ -88,29 +89,37 @@ def damped_solve(H, g, lam: float, fixed: Sequence[int] = ()):
 
 class LinearisationCache:
     """photometric_factor.cpp:296-328 GetJacobiansIfNeeded for a whole window: a pair's factors are re-evaluated only when
-    pose0, pose1 or code0 moved by more than eps since the evaluation whose records are still in the record buffer."""
+    pose0, pose1 or code0 moved by more than eps since the evaluation whose records are still in the record buffer.
+    Geometric links (k0, k1) follow the pairs (link j is index len(pairs) + j); a link also depends on code1, so it is
+    stale when pose0, pose1, code0 or code1 moved."""
 
-    def __init__(self, pairs: Sequence[Tuple[int, int]], eps: float = 1e-6):
+    def __init__(self, pairs: Sequence[Tuple[int, int]], eps: float = 1e-6, geometric: Sequence[Tuple[int, int]] = ()):
         self.pairs = list(pairs)
+        self.geometric = [tuple(p) for p in geometric]
         self.eps = eps
-        self._at = [None] * len(self.pairs)  # (pose0, pose1, code0) the stored records were evaluated at
+        self.invalidate()
+
+    def _keys(self):
+        return [(k0, k1, False) for k0, k1 in self.pairs] + [(k0, k1, True) for k0, k1 in self.geometric]
 
     def stale(self, poses: np.ndarray, codes: np.ndarray) -> List[int]:
         out = []
-        for p, (k0, k1) in enumerate(self.pairs):
+        for p, (k0, k1, geo) in enumerate(self._keys()):
             at = self._at[p]
             if at is None or np.abs(at[0] - poses[k0]).max() > self.eps or np.abs(at[1] - poses[k1]).max() > self.eps or \
-                    np.abs(at[2] - codes[k0]).max() > self.eps:
+                    np.abs(at[2] - codes[k0]).max() > self.eps or (geo and np.abs(at[3] - codes[k1]).max() > self.eps):
                 out.append(p)
         return out
 
     def store(self, done: Sequence[int], poses: np.ndarray, codes: np.ndarray):
+        keys = self._keys()
         for p in done:
-            k0, k1 = self.pairs[p]
-            self._at[p] = (poses[k0].copy(), poses[k1].copy(), codes[k0].copy())
+            k0, k1, _ = keys[p]
+            # (pose0, pose1, code0, code1) the stored records were evaluated at
+            self._at[p] = (poses[k0].copy(), poses[k1].copy(), codes[k0].copy(), codes[k1].copy())
 
     def invalidate(self):
-        self._at = [None] * len(self.pairs)
+        self._at = [None] * (len(self.pairs) + len(self.geometric))
 
 
 def apply_update(poses: np.ndarray, codes: np.ndarray, dx: np.ndarray, code_size: int):
@@ -134,7 +143,7 @@ class WindowOptimizer:
         self.layout = layout
         self.linearise = linearise
         self.params = params or LMParams()
-        self.cache = LinearisationCache(layout.pairs, self.params.cache_eps)
+        self.cache = LinearisationCache(layout.pairs, self.params.cache_eps, layout.geometric)
 
     def _system(self, buf, codes):
         H, g, f, inl = self.layout.to_dense(buf)
@@ -206,6 +215,17 @@ class ReprojectionLink:
     sigma: float
 
 
+@dataclass
+class GeometricLink:
+    """A sparse geometric factor between keyframes k0 -> k1 (SparseGeometricFactor, sparse_geometric_factor.cpp): the
+    sampled pixels points_xy [M, 2] of k0 (host ints) and the Huber delta.  use_geometric adds one per new keyframe
+    connection and per enqueued link (mapper.cpp:328-337, 379-388)."""
+    k0: int
+    k1: int
+    points_xy: np.ndarray
+    huber_delta: float
+
+
 class SfmWindowProblem:
     """The device pipeline of one linearisation, on SfmAligner + Window: keyframes hold their pyramids on the device
     (img, grad, prx_orig, prx_jac per level + the dpt / valid buffers the fused decode writes); `linearise` re-evaluates
@@ -213,10 +233,15 @@ class SfmWindowProblem:
 
     `links` (optional) are reprojection factors: they follow the photometric pairs in the window's pair list (same
     variables pose0, pose1, code0, so the linearisation cache covers them), each owns one unscaled record at the end of
-    the record buffer, and the stale ones are re-linearised in one dfk_reprojection_linearize_batch launch."""
+    the record buffer, and the stale ones are re-linearised in one dfk_reprojection_linearize_batch launch.
+
+    `geometric` (optional) are sparse geometric links: keyframe k1 of each must carry kf[k1][0]["dpt_grad"], the Sobel
+    gradient of its level-0 depth (mapper.cpp:993-1000).  They own a record buffer of their own and a link block of the
+    window; link j is index len(self.pairs) + j of the cache, and the stale ones are re-linearised in one
+    dfk_sparse_geometric_linearize_batch launch."""
 
     def __init__(self, aligner, cams, keyframes, pairs, allreduce: Optional[Callable] = None,
-                 links: Optional[Sequence[ReprojectionLink]] = None):
+                 links: Optional[Sequence[ReprojectionLink]] = None, geometric: Optional[Sequence[GeometricLink]] = None):
         import torch
         from . import _lib
         from .aligners import Window
@@ -237,9 +262,17 @@ class SfmWindowProblem:
         for j in range(len(self.links)):
             item_pair.append(self.num_photometric + j)
             sizes.append((0, 0))  # unscaled record: b^T b enters f as it is
-        self.window = Window(aligner, len(keyframes), self.pairs, item_pair, sizes)
+        self.geometric = list(geometric or [])
+        for gl in self.geometric:
+            if "dpt_grad" not in self.kf[gl.k1][0]:
+                raise ValueError(f"keyframe {gl.k1} is k1 of a geometric link but carries no level-0 dpt_grad")
+        self.window = Window(aligner, len(keyframes), self.pairs, item_pair, sizes,
+                             [(int(gl.k0), int(gl.k1)) for gl in self.geometric])
         self.layout = self.window.layout
-        self.records = torch.zeros((len(item_pair), _lib.record_floats(aligner.CS)), dtype=torch.float32, device=self.kf[0][0]["img"].device)
+        dev = self.kf[0][0]["img"].device
+        self.records = torch.zeros((len(item_pair), _lib.record_floats(aligner.CS)), dtype=torch.float32, device=dev)
+        self.geo_records = torch.zeros((len(self.geometric), _lib.geo_record_floats(aligner.CS)), dtype=torch.float32,
+                                       device=dev) if self.geometric else None
         self.allreduce = allreduce
 
     def _items(self, poses, codes, todo):
@@ -264,9 +297,24 @@ class SfmWindowProblem:
                               cauchy_delta=ln.cauchy_delta, sigma=ln.sigma))
         return items
 
+    def _geo_items(self, poses, codes, todo):
+        items = []
+        for j in todo:
+            gl = self.geometric[j]
+            a, b = self.kf[gl.k0][0], self.kf[gl.k1][0]
+            items.append(dict(pose0=poses[gl.k0].astype(np.float32), pose1=poses[gl.k1].astype(np.float32),
+                              code0=codes[gl.k0].astype(np.float32), code1=codes[gl.k1].astype(np.float32),
+                              cam=self.cams[0], prx0_orig=a["prx_orig"], prx0_jac=a["prx_jac"], prx1_orig=b["prx_orig"],
+                              prx1_jac=b["prx_jac"], dpt_grad1=b["dpt_grad"], points_xy=gl.points_xy,
+                              huber_delta=gl.huber_delta))
+        return items
+
     def linearise(self, poses, codes, todo):
         import torch
-        from .aligners import ReprojectionLinearizeBatch
+        from .aligners import ReprojectionLinearizeBatch, SparseGeometricLinearizeBatch
+        P = len(self.pairs)
+        geo = [p - P for p in todo if p >= P]
+        todo = [p for p in todo if p < P]
         photo = [p for p in todo if p < self.num_photometric]
         links = [p - self.num_photometric for p in todo if p >= self.num_photometric]
         if photo:
@@ -286,7 +334,14 @@ class SfmWindowProblem:
                 part = ReprojectionLinearizeBatch(self.al, items)
                 rows = torch.as_tensor([self.photometric_items + j for j in links], device=self.records.device)
                 self.records.index_copy_(0, rows, part)
-        buf = self.window.assemble(self.records)
+        if geo:
+            items = self._geo_items(poses, codes, geo)
+            if len(geo) == len(self.geometric):
+                SparseGeometricLinearizeBatch(self.al, items, self.geo_records)
+            else:
+                part = SparseGeometricLinearizeBatch(self.al, items)
+                self.geo_records.index_copy_(0, torch.as_tensor(geo, device=self.geo_records.device), part)
+        buf = self.window.assemble(self.records, geo_records=self.geo_records)
         if self.allreduce is not None:
             self.allreduce(buf)
         return buf, None

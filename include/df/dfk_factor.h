@@ -13,6 +13,9 @@
 //   LinearizeReprojectionBatch
 //                          many reprojection factors (loop closures, use_reprojection links) linearised in one launch
 //                          straight into device records [A^T A | -A^T b | b^T b | inliers] (WindowSystem::AddUnscaled).
+//   LinearizeSparseGeometricBatch
+//                          many sparse geometric factors (use_geometric links) linearised in one launch into device
+//                          records over [pose0 | pose1 | code0 | code1] (WindowSystem::AddGeometric).
 //   LinearizeReprojection / LinearizeSparseGeometric
 //                          the Jacobian rows of the two sparse factors (reprojection_factor.cpp:157-269,
 //                          sparse_geometric_factor.cpp:157-271), evaluated on the device from the keyframes' GPU buffers;
@@ -99,6 +102,25 @@ public:
   void AddUnscaled(int k0, int k1, const JTJJrReductionItem<float, 12 + CS>& sys)
   {
     AddBlocks(k0, k1, sys);
+    f_ += static_cast<double>(sys.residual);
+  }
+
+  // a sparse geometric factor (k0 -> k1) as a record of LinearizeSparseGeometricBatch, variables [pose0 | pose1 | code0 |
+  // code1]: the blocks of all four (pose0 / code0 belong to k0, pose1 / code1 to k1) -- the HessianFactor over four
+  // keys that replaces the JacobianFactor -- and f += b^T b
+  void AddGeometric(int k0, int k1, const JTJJrReductionItem<float, 12 + 2 * CS>& sys)
+  {
+    const int off[4] = {k0 * Block, k1 * Block, k0 * Block + 6, k1 * Block + 6};  // pose0, pose1, code0, code1
+    const int loc[4] = {0, 6, 12, 12 + CS};
+    const int len[4] = {6, 6, CS, CS};
+    for (int a = 0; a < 4; ++a) {
+      for (int r = 0; r < len[a]; ++r) {
+        g_[off[a] + r] -= static_cast<double>(sys.Jtr[loc[a] + r]);
+        for (int b = 0; b < 4; ++b)
+          for (int c = 0; c < len[b]; ++c)
+            H(off[a] + r, off[b] + c) += static_cast<double>(sys.JtJ.toDenseMatrix(loc[a] + r, loc[b] + c));
+      }
+    }
     f_ += static_cast<double>(sys.residual);
   }
 
@@ -208,6 +230,45 @@ SparseRows LinearizeSparseGeometric(DfkHandle h, const SE3T& pose0, const SE3T& 
                                                   &p1, &j1, &g1, num_points, points_xy, huber_delta, out.rows.data(),
                                                   &out.num_valid));
   return out;
+}
+
+// One factor of LinearizeSparseGeometricBatch: the arguments of LinearizeSparseGeometric.  code0, code1 and points_xy
+// are read when LinearizeSparseGeometricBatch is called (not kept).
+template <int CS, typename SE3T, typename CodeT, typename CamT, typename ImageBuffer, typename GradBuffer>
+DfkSparseGeometricItem SparseGeometricItem(const SE3T& pose0, const SE3T& pose1, const CodeT& code0, const CodeT& code1,
+                                           const CamT& cam, const ImageBuffer& prx0_orig, const ImageBuffer& prx0_jac,
+                                           const ImageBuffer& prx1_orig, const ImageBuffer& prx1_jac,
+                                           const GradBuffer& dpt_grad1, int num_points, const int* points_xy,
+                                           float huber_delta)
+{
+  DfkSparseGeometricItem it{};
+  for (int k = 0; k < 7; ++k) {
+    it.pose0[k] = pose0.data()[k];
+    it.pose1[k] = pose1.data()[k];
+  }
+  it.cam = detail::Cam(cam);
+  it.prx0_orig = detail::View(prx0_orig, 1);
+  it.prx0_jac = detail::View(prx0_jac, CS);
+  it.prx1_orig = detail::View(prx1_orig, 1);
+  it.prx1_jac = detail::View(prx1_jac, CS);
+  it.dpt_grad1 = detail::View(dpt_grad1, 2);
+  it.code0 = code0.data();
+  it.code1 = code1.data();
+  it.num_points = num_points;
+  it.points_xy = points_xy;
+  it.huber_delta = huber_delta;
+  return it;
+}
+
+// Many SparseGeometricFactors linearised in one launch into normal-equation records
+// (dfk_sparse_geometric_linearize_batch): record i = [A^T A packed | -A^T b | b^T b | valid points] of factor i's rows
+// over [pose0 | pose1 | code0 | code1], at records_dev + i * DFK_GEO_RECORD_FLOATS(CS) (DEVICE).  Asynchronous on the
+// handle's stream; what a window adds with WindowSystem::AddGeometric, or dfk_window_assemble_geometric as a link.
+template <int CS>
+void LinearizeSparseGeometricBatch(DfkHandle h, const std::vector<DfkSparseGeometricItem>& items, float* records_dev)
+{
+  detail::Check(h, dfk_sparse_geometric_linearize_batch(h, items.data(), static_cast<int>(items.size()), CS,
+                                                        records_dev));
 }
 
 inline void ShardPairs(std::size_t num_pairs, int world_size, int rank, std::size_t* begin, std::size_t* end)

@@ -250,6 +250,22 @@ size_t dfk_window_floats(const DfkWindow* w);
  * floats (DEVICE), fully overwritten.  Asynchronous on the handle's stream, one launch. */
 DfkStatus dfk_window_assemble(DfkHandle h, const DfkWindow* w, const float* records_dev, float* window_dev);
 
+/* A window that also holds num_links sparse geometric links l = (link_k0[l] -> link_k1[l]) (HOST arrays, copied), one
+ * record of DFK_GEO_RECORD_FLOATS each (dfk_sparse_geometric_linearize_batch).  The buffer is the layout above with L
+ * link blocks appended after the two scalars, so no offset of the layout above moves:
+ *   L link blocks      B x B, row-major: rows = [pose | code] of the link's k0, columns = [pose | code] of its k1
+ * Link l adds its (pose0, code0) block to k0's diagonal block, its whole (pose1, code1) block to k1's, the matching
+ * parts of -Jtr to both gradients and its residual (b^T b) to f; it adds nothing to the inlier total.  An element sums
+ * the items in item order, then the links where its keyframe is k0, then those where it is k1, in link order.
+ * A link naming a keyframe outside the window or with k0 == k1 is rejected.  num_links = 0 is dfk_window_create. */
+DfkStatus dfk_window_create_geometric(DfkHandle h, const DfkWindowDesc* desc, int num_links, const int32_t* link_k0,
+                                      const int32_t* link_k1, DfkWindow** out);
+/* dfk_window_assemble for a window with links (dfk_window_assemble rejects such a window).  geo_records_dev: DEVICE,
+ * num_links records; it may be NULL only when the window has no links, and the buffer is then bit for bit the one
+ * dfk_window_assemble writes.  Asynchronous on the handle's stream, one launch. */
+DfkStatus dfk_window_assemble_geometric(DfkHandle h, const DfkWindow* w, const float* records_dev,
+                                        const float* geo_records_dev, float* window_dev);
+
 /* ------------------------------------------------------------------ SE3Aligner */
 
 /* SE3Aligner<float>::RunStep (cu_se3aligner.h:65-70, cu_se3aligner.cpp:153-176):
@@ -383,6 +399,35 @@ DfkStatus dfk_sparse_geometric_linearize(DfkHandle h, const float pose0[7], cons
                                          const DfkImage* prx0_jac, const DfkImage* prx1_orig, const DfkImage* prx1_jac,
                                          const DfkImage* dpt_grad1, int num_points, const int* points_xy, float huber_delta,
                                          float* rows, int* num_valid);
+
+/* One SparseGeometricFactor of a batch: the arguments of dfk_sparse_geometric_linearize for one factor (k0 -> k1), as
+ * Mapper adds them with use_geometric (mapper.cpp:328-337, 379-388). */
+typedef struct {
+  float pose0[7], pose1[7];
+  DfkCamera cam;                            /* level 0 */
+  DfkImage prx0_orig, prx0_jac;             /* keyframe k0, level 0, DEVICE */
+  DfkImage prx1_orig, prx1_jac, dpt_grad1;  /* keyframe k1, level 0, DEVICE; dpt_grad1 2 floats per pixel */
+  const float* code0;                       /* HOST, code_size floats */
+  const float* code1;                       /* HOST, code_size floats */
+  int32_t num_points;
+  const int32_t* points_xy;                 /* HOST, 2 ints per point */
+  float huber_delta;
+} DfkSparseGeometricItem;
+/* variables of a geometric record, in the JacobianFactor's key order [pose0 (6) | pose1 (6) | code0 (C) | code1 (C)] */
+#define DFK_GEO_NP(C) (12 + 2 * (C))
+#define DFK_GEO_RECORD_FLOATS(C) (DFK_GEO_NP(C) * (DFK_GEO_NP(C) + 1) / 2 + DFK_GEO_NP(C) + 2)
+
+/* Batched SparseGeometricFactor::linearize straight into normal-equation records: factor i's JacobianFactor [A | b] (the
+ * rows of dfk_sparse_geometric_linearize, bit for bit) gives the record
+ *   JtJ = A^T A (packed upper, DFK_GEO_NP(C) variables), Jtr = -A^T b, residual = b^T b, inliers = valid points (u32 bits)
+ * records_dev: DEVICE, n * DFK_GEO_RECORD_FLOATS(code_size) floats.  One launch; a factor's record is summed in a fixed
+ * order by CTAs of its own, so it does not depend on the rest of the batch.  avg_dpt is the handle's
+ * DenseSfmParams::avg_dpt.  Asynchronous on the handle's stream (no host sync, no D2H); the host arrays may be freed when
+ * the call returns.  Every item is validated before anything is enqueued (1 <= n, num_points >= 1, huber_delta > 0,
+ * consistent views, a camera no larger than the views, non-NULL pointers); a rejected call writes nothing and
+ * dfk_last_error names the item. */
+DfkStatus dfk_sparse_geometric_linearize_batch(DfkHandle h, const DfkSparseGeometricItem* items, int n, int code_size,
+                                               float* records_dev);
 
 /* ------------------------------------------------------------------ cu_image_proc free functions */
 

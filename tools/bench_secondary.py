@@ -15,7 +15,10 @@ One JSON line per case:
     ReprojectionLinearize calls + the host A^T A (the only route before the batched call) against one
     ReprojectionLinearizeBatch -- wall clock and summed device time; and one linearisation of the window200 window
     (50 keyframes, 200 photometric pairs, 4 levels at 640x480, C = 32) without and with 400 reprojection links.
-Every line carries the card's name and power limit.  `--only reprojection` runs the reprojection cases alone.
+  * SparseGeometricFactor linearisation of K = 32 / 200 factors x M = 500 / 3000 points at C = 32 / 128, 640x480
+    level 0: K synchronous SparseGeometricLinearize calls + the host A^T A against one SparseGeometricLinearizeBatch;
+    and one linearisation of the window200 window without and with 50 geometric links x 3000 points.
+Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` runs those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -34,7 +37,7 @@ sys.path.insert(0, ROOT)
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
-    ap.add_argument("--only", choices=["reprojection"], default=None)
+    ap.add_argument("--only", choices=["reprojection", "geometric"], default=None)
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -58,6 +61,8 @@ def main():
 
     if args.only == "reprojection":
         return reprojection_cases(args, torch, print)
+    if args.only == "geometric":
+        return geometric_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -220,6 +225,7 @@ def main():
                                         "torch.profiler"}), flush=True)
 
     reprojection_cases(args, torch, print)
+    geometric_cases(args, torch, print)
 
 
 def _power_limit_w():
@@ -335,6 +341,98 @@ def reprojection_cases(args, torch, print):
         reps = max(5, args.reps // 2)
         print(json.dumps({"case": f"window200 linearisation (50 keyframes, 200 pairs, 4 levels 640x480, C=32) + {n_links} "
                                   f"reprojection links x {M} matches",
+                          "us_per_linearisation": _wall_us(torch, lin, reps),
+                          "device_us_per_linearisation": _device_us(torch, lin, reps),
+                          "timing": "wall clock to the end of the assembly (synchronised); device time = summed kernel + "
+                                    "copy time, torch.profiler"}), flush=True)
+
+
+def geometric_cases(args, torch, print):
+    """SparseGeometricFactor linearisation: K x (dfk_sparse_geometric_linearize + host A^T A) against one
+    dfk_sparse_geometric_linearize_batch; and a window200 linearisation without / with 50 geometric links."""
+    import numpy as np
+
+    from deepfactors_b200 import _lib, se3, synth
+    from deepfactors_b200.aligners import SfmAligner, SparseGeometricLinearize, SparseGeometricLinearizeBatch
+    dev = torch.device("cuda", 0)
+    rng = np.random.default_rng(5)
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(dev)
+
+    def points(cam, m):
+        return np.stack([rng.integers(2, int(cam.width) - 2, m), rng.integers(2, int(cam.height) - 2, m)], 1).astype(np.int32)
+
+    for cs in (32, 128):
+        L0 = synth.make_level(640, 480, cs, seed=21)
+        L1 = synth.make_level(640, 480, cs, seed=22, phase=0.3)
+        dpt1 = (np.float32(2.0) / L1.prx_orig - np.float32(2.0)).astype(np.float32)
+        kf = dict(prx0_orig=up(L0.prx_orig), prx0_jac=up(L0.prx_jac), prx1_orig=up(L1.prx_orig), prx1_jac=up(L1.prx_jac),
+                  dpt_grad1=up(synth.sobel_np(dpt1)))
+        al = SfmAligner(cs)
+        for M in (500, 3000):
+            for K in (32, 200):
+                items = [dict(pose0=se3.identity(), pose1=se3.make_pose([0.01 * (k % 5), -0.01, 0.0],
+                                                                        [0.05, 0.0, 0.01 * (k % 3)], np.float32),
+                              code0=(rng.standard_normal(cs) * 0.1).astype(np.float32),
+                              code1=(rng.standard_normal(cs) * 0.1).astype(np.float32), cam=L0.cam,
+                              points_xy=points(L0.cam, M), huber_delta=0.1, **kf) for k in range(K)]
+                rec = torch.empty((K, _lib.geo_record_floats(cs)), dtype=torch.float32, device=dev)
+
+                def per_factor():  # rows to the host, then A^T A there (what a JacobianFactor costs the solver)
+                    for it in items:
+                        rows, _ = SparseGeometricLinearize(al, it["pose0"], it["pose1"], it["code0"], it["code1"], it["cam"],
+                                                           it["prx0_orig"], it["prx0_jac"], it["prx1_orig"], it["prx1_jac"],
+                                                           it["dpt_grad1"], it["points_xy"], it["huber_delta"])
+                        r = rows.astype(np.float64)
+                        r.T @ r
+
+                def batched():
+                    SparseGeometricLinearizeBatch(al, items, rec)
+
+                slow = 2 if K * M * cs > 32 * 3000 * 32 else 3
+                for name, fn, reps in (("K x SparseGeometricLinearize + host A^T A", per_factor, slow),
+                                       ("one SparseGeometricLinearizeBatch", batched, max(5, args.reps))):
+                    print(json.dumps({"case": f"SparseGeometricFactor linearisation 640x480 C={cs} K={K} factors x {M} "
+                                              f"points: {name}",
+                                      "us_per_linearisation": _wall_us(torch, fn, reps),
+                                      "device_us_per_linearisation": _device_us(torch, fn, max(1, reps // 2)),
+                                      "host_syncs": K if fn is per_factor else 0,
+                                      "row_bytes_downloaded": K * M * (13 + 2 * cs) * 4 if fn is per_factor else 0,
+                                      "timing": "wall clock (synchronous); device time = summed kernel + copy time, "
+                                                "torch.profiler"}), flush=True)
+        del kf, items, rec
+        torch.cuda.empty_cache()
+
+    # ---- window200 (bench.py --config window200): one linearisation of every factor, without and with 50 links --------
+    from deepfactors_b200.window_opt import GeometricLink, SfmWindowProblem
+    sys.path.insert(0, ROOT)
+    from bench import window_pairs
+    cs, levels, num_kf, M = 32, 4, 50, 3000
+    base = synth.make_pair(640, 480, cs, levels, seed=7)
+    shared = [dict(img=up(L.img0), grad=up(L.grad1), prx_orig=up(L.prx_orig), prx_jac=up(L.prx_jac)) for L in base.levels]
+    dpt = (np.float32(2.0) / base.levels[0].prx_orig - np.float32(2.0)).astype(np.float32)
+    shared[0]["dpt_grad"] = up(synth.sobel_np(dpt))  # Sobel of level-0 depth, computed once per keyframe
+    keyframes = [[dict(sh, dpt=torch.zeros_like(sh["img"]), valid=torch.zeros_like(sh["img"])) for sh in shared]
+                 for _ in range(num_kf)]
+    pairs = window_pairs(num_kf, 200)
+    cam0 = base.levels[0].cam
+    links = []
+    for j in range(50):
+        k0, k1 = (int(v) for v in rng.choice(num_kf, 2, replace=False))
+        links.append(GeometricLink(k0, k1, points(cam0, M), 0.1))
+    al = SfmAligner(cs)
+    poses = np.stack([se3.make_pose([0.001 * (k % 7), 0.0, 0.0], [0.002 * (k % 5), 0.0, 0.0], np.float64)
+                      for k in range(num_kf)])
+    codes = np.zeros((num_kf, cs))
+    for n_links in (0, 50):
+        prob = SfmWindowProblem(al, [L.cam for L in base.levels], keyframes, pairs, geometric=links[:n_links] or None)
+        todo = list(range(len(prob.pairs) + n_links))
+
+        def lin():
+            prob.linearise(poses, codes, todo)
+
+        reps = max(5, args.reps // 2)
+        print(json.dumps({"case": f"window200 linearisation (50 keyframes, 200 pairs, 4 levels 640x480, C=32) + {n_links} "
+                                  f"geometric links x {M} points",
                           "us_per_linearisation": _wall_us(torch, lin, reps),
                           "device_us_per_linearisation": _device_us(torch, lin, reps),
                           "timing": "wall clock to the end of the assembly (synchronised); device time = summed kernel + "
