@@ -390,11 +390,15 @@ def SparseGeometricLinearizeBatch(aligner, items: Sequence[dict], records: torch
 # ------------------------------------------------------------------------------------------- DepthAligner
 class DepthAligner:
     """df::DepthAligner<float, CS> (sources/cuda/cu_depthaligner.h:38-54): code-only alignment of the decoded depth to a
-    target depth map; the result is a JTJJrReductionItem over the CS code parameters."""
+    target depth map; the result is a JTJJrReductionItem over the CS code parameters.  The decode uses
+    params.sfmparams.avg_dpt (default 2, the value the reference hard-codes in this kernel)."""
 
-    def __init__(self, code_size: int, device=None):
+    def __init__(self, code_size: int, device=None, params: SfmAlignerParams | None = None):
         self.CS = int(code_size)
         self._hd = _Handle(device)
+        if params is not None:
+            cp = params.to_c()
+            check(self._hd.h, lib().dfk_sfm_set_params(self._hd.h, C.byref(cp)))
 
     @property
     def handle(self):

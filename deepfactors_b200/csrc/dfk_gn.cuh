@@ -18,7 +18,8 @@ namespace dfk {
 // so3 = SO3::exp(update.tail<3>()) * so3.  Eigen's LDLT is a robust Cholesky with symmetric (diagonal) pivoting that
 // still returns a solution for semi-definite / ill-conditioned systems: pivots not larger than the smallest normal
 // float contribute nothing (Eigen's LDLT::solve zeroes those components).  Same here, so a rank-deficient level moves
-// the pose where the reference moves it, and an all-zero system (no inliers) leaves it alone.
+// the pose where the reference moves it, and an all-zero system gives a zero step.  (The quaternion is still
+// renormalised; a tracker iteration without inliers skips this update altogether, se3_track_update in dfk_simple.cu.)
 __host__ __device__ inline void ldlt6_solve(float A[6][6] /* full symmetric, destroyed */, const float b[6], float x[6])
 {
   // Every array index below is a compile-time constant after unrolling (the pivot swap is a chain of predicated static

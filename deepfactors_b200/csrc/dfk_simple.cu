@@ -157,8 +157,10 @@ __device__ __forceinline__ void se3_load_pose(PixelCam& pc, const float* pose_de
   for (int k = 0; k < 3; ++k) pc.t[k] = pose_dev[4 + k];
 }
 
-// ... and its own last block applies the next Gauss-Newton update (a system that is not positive definite leaves the
-// pose alone).  Called by the last block of a problem only.
+// ... and its own last block applies the next Gauss-Newton update.  A system without inliers leaves the pose alone, bit
+// for bit, as the reference's tracker does (it skips the update when no pixel is valid): gn_update_pose would apply a
+// zero step and then renormalise the quaternion in fp32, which moves most unit quaternions by an ulp or so.  Called by
+// the last block of a problem only.
 __device__ __forceinline__ void se3_track_update(const float* out, float* pose_dev, float* __restrict__ history)
 {
   __syncthreads();  // out[0..28] was written by warp 0 of this block
@@ -172,6 +174,7 @@ __device__ __forceinline__ void se3_track_update(const float* out, float* pose_d
 #pragma unroll
       for (int k = 0; k < 7; ++k) history[29 + k] = pose[k];
     }
+    if (__float_as_uint(out[28]) == 0u) return;  // no inliers
     float sys[27];
 #pragma unroll 1
     for (int k = 0; k < 27; ++k) sys[k] = out[k];

@@ -60,6 +60,60 @@ void dfko_probe_pixel_d(double x, double y, double dpt, const DfkoCamera* cam, c
   dfko_probe_pixel_impl_d(x, y, dpt, cam, pose, border, min_dpt, avg_dpt, out);
 }
 
+/* ------------------------------------------------------------------ SE3Aligner::RunStep rows (fp64)
+ * The per-pixel rows [J (6) | w*diff] of dfko_se3_run_step_d for image rows y_begin .. y_end-1, row major: pixel (x, y)
+ * owns rows[((y - y_begin) * width + x) * 7 ...], zero for an invalid pixel.  valid_f32 != 0 takes the pixel set from
+ * the fp32 validity chain (the one the kernels and dfko_se3_run_step_f run) instead of the fp64 one, so that a pixel
+ * on the validity border is in or out exactly as it is for the kernel; its row is still evaluated in fp64, with pix1
+ * clamped below width - 1 / height - 1 so that the bilinear taps stay inside the image. */
+void dfko_se3_pixel_rows_d(const float se3[7], const DfkoCamera* camf, int width, int height,
+                           const float* img0, size_t img0_pitch, const float* img1, size_t img1_pitch,
+                           const float* dpt0, size_t dpt0_pitch, const float* grad1, size_t grad1_pitch,
+                           float huber_delta, int valid_f32, int y_begin, int y_end,
+                           double* rows, double* residual, uint64_t* inliers)
+{
+  double pose[7];
+  for (int i = 0; i < 7; ++i) pose[i] = (double)se3[i];
+  const Cam_d cam = cam_cast_d(camf);
+  const Cam_f cam32 = cam_cast_f(camf);
+  if (y_begin < 0) y_begin = 0;
+  if (y_end > height) y_end = height;
+  if (y_end < y_begin) y_end = y_begin;
+  for (size_t i = 0; i < (size_t)(y_end - y_begin) * (size_t)width * 7; ++i) rows[i] = 0;
+  double res = 0;
+  uint64_t inl = 0;
+  for (int y = y_begin; y < y_end; ++y)
+    for (int x = 0; x < width; ++x) {
+      const float d32 = dpt0[(size_t)y * dpt0_pitch + x];
+      Corr_d c = find_correspondence_d((double)x, (double)y, (double)d32, &cam, pose, 1, 0.0);
+      int valid = c.valid;
+      if (valid_f32) {
+        valid = find_correspondence_f((float)x, (float)y, d32, &cam32, se3, 1, 0.0f).valid;
+        if (valid) {
+          c.u = cam.fx * c.tpt[0] / c.tpt[2] + cam.u0;
+          c.v = cam.fy * c.tpt[1] / c.tpt[2] + cam.v0;
+          c.u = fmin(fmax(c.u, 0.0), cam.width - 1.0 - 1e-9);
+          c.v = fmin(fmax(c.v, 0.0), cam.height - 1.0 - 1e-9);
+        }
+      }
+      if (!valid) continue;
+      double A0[6], A1[6];
+      double* J = rows + ((size_t)(y - y_begin) * (size_t)width + (size_t)x) * 7;
+      corr_jac_pose_d(&c, &cam, A0, A1);
+      const double gx = bilinear_d(grad1, grad1_pitch, 2, 0, c.u, c.v);
+      const double gy = bilinear_d(grad1, grad1_pitch, 2, 1, c.u, c.v);
+      double diff = (double)img0[(size_t)y * img0_pitch + x] - bilinear_d(img1, img1_pitch, 1, 0, c.u, c.v);
+      const double w = huber_weight_d(diff, (double)huber_delta);
+      diff *= w;
+      for (int k = 0; k < 6; ++k) J[k] = ((-gx) * A0[k] + (-gy) * A1[k]) * w;
+      J[6] = diff;
+      inl += 1;
+      res += diff * diff;
+    }
+  *residual = res;
+  *inliers = inl;
+}
+
 /* ------------------------------------------------------------------ OpenMP CPU baseline */
 int dfko_omp_max_threads(void)
 {
@@ -198,6 +252,22 @@ void dfko_update_depth_f(const float* code, int code_size, int width, int height
       for (int k = 0; k < code_size; ++k) dot += jc[k] * code[k];
       const float prx = prx_orig[(size_t)y * prx_pitch + x] + dot;
       dpt_out[(size_t)y * dpt_pitch + x] = avg_dpt / prx - avg_dpt;
+    }
+}
+
+/* the same decode in fp64 (the truth UpdateDepth is checked against) */
+void dfko_update_depth_d(const float* code, int code_size, int width, int height,
+                         const float* prx_orig, size_t prx_pitch, const float* prx_jac, size_t jac_pitch,
+                         float avg_dpt, double* dpt_out, size_t dpt_pitch)
+{
+  const double avg = (double)avg_dpt;
+  for (int y = 0; y < height; ++y)
+    for (int x = 0; x < width; ++x) {
+      const float* jc = prx_jac + (size_t)y * jac_pitch + (size_t)x * code_size;
+      double dot = 0.0;
+      for (int k = 0; k < code_size; ++k) dot += (double)jc[k] * (double)code[k];
+      const double prx = (double)prx_orig[(size_t)y * prx_pitch + x] + dot;
+      dpt_out[(size_t)y * dpt_pitch + x] = avg / prx - avg;
     }
 }
 

@@ -166,6 +166,14 @@ void dfko_se3_run_step_d(const float se3[7], const DfkoCamera* cam, int width, i
                          const float* img0, size_t img0_pitch, const float* img1, size_t img1_pitch,
                          const float* dpt0, size_t dpt0_pitch, const float* grad1, size_t grad1_pitch,
                          float huber_delta, double* JtJ, double* Jtr, double* residual, uint64_t* inliers);
+/* Its fp64 per-pixel rows [J (6) | w*diff] for image rows y_begin .. y_end-1: pixel (x, y) owns
+ * rows[((y - y_begin) * width + x) * 7 ...], zero when invalid.  valid_f32 != 0: the pixel set of the fp32 validity
+ * chain (dfko_se3_run_step_f, the kernels) instead of the fp64 one. */
+void dfko_se3_pixel_rows_d(const float se3[7], const DfkoCamera* cam, int width, int height,
+                           const float* img0, size_t img0_pitch, const float* img1, size_t img1_pitch,
+                           const float* dpt0, size_t dpt0_pitch, const float* grad1, size_t grad1_pitch,
+                           float huber_delta, int valid_f32, int y_begin, int y_end,
+                           double* rows, double* residual, uint64_t* inliers);
 
 /* ---- SE3Aligner::Warp (cu_se3aligner.cpp:61-113,125-151): img2 = img1 warped into frame 0
  * (0 where invalid); residual = signed sum (img0 - sampled). */
@@ -182,6 +190,9 @@ void dfko_se3_warp_d(const float se3[7], const DfkoCamera* cam, int width, int h
 void dfko_update_depth_f(const float* code, int code_size, int width, int height,
                          const float* prx_orig, size_t prx_pitch, const float* prx_jac, size_t jac_pitch,
                          float avg_dpt, float* dpt_out, size_t dpt_pitch);
+void dfko_update_depth_d(const float* code, int code_size, int width, int height,
+                         const float* prx_orig, size_t prx_pitch, const float* prx_jac, size_t jac_pitch,
+                         float avg_dpt, double* dpt_out, size_t dpt_pitch);
 
 /* ---- DepthAligner::RunStep (cu_depthaligner.cpp:32-113): every pixel counts; JtJ packed upper C(C+1)/2, Jtr C.
  * avg_dpt is hard-coded to 2 in the reference kernel (:44); a parameter here. */
@@ -191,6 +202,14 @@ void dfko_depth_run_step_f(const float* code, int code_size, int width, int heig
 void dfko_depth_run_step_d(const float* code, int code_size, int width, int height, const float* tgt, size_t tgt_pitch,
                            const float* prx_orig, size_t prx_pitch, const float* prx_jac, size_t jac_pitch, float avg_dpt,
                            double* JtJ, double* Jtr, double* residual, uint64_t* inliers);
+/* Its per-pixel rows [J (C) | diff] for image rows y_begin .. y_end-1: pixel (x, y) owns
+ * rows[((y - y_begin) * width + x) * (C + 1) ...]. */
+void dfko_depth_pixel_rows_f(const float* code, int code_size, int width, int height, const float* tgt, size_t tgt_pitch,
+                             const float* prx_orig, size_t prx_pitch, const float* prx_jac, size_t jac_pitch,
+                             float avg_dpt, int y_begin, int y_end, float* rows);
+void dfko_depth_pixel_rows_d(const float* code, int code_size, int width, int height, const float* tgt, size_t tgt_pitch,
+                             const float* prx_orig, size_t prx_pitch, const float* prx_jac, size_t jac_pitch,
+                             float avg_dpt, int y_begin, int y_end, double* rows);
 
 /* ---- ReprojectionFactor::linearize rows (core/gtsam/reprojection_factor.cpp:157-269): rows_out is
  * (2 * num_matches) x (13 + C) row-major [J_pose0 | J_pose1 | J_code0 | b]; returns the sum of squared unweighted errors */

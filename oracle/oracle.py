@@ -250,6 +250,27 @@ def se3_run_step(se3, cam, img0, img1, dpt0, grad1, huber_delta=0.1, *, precisio
     return StepResult(JtJ, Jtr, float(res.value), int(inl.value))
 
 
+def se3_pixel_rows(se3, cam, img0, img1, dpt0, grad1, huber_delta=0.1, *, valid_f32=False, y_begin=0, y_end=None):
+    """The fp64 per-pixel rows that se3_run_step(..., precision="f64") sums, for image rows y_begin .. y_end-1.
+    Returns (rows [(y_end - y_begin) * W, 7] float64, row-major over the pixels: [J (6) | w*diff], zero for an invalid
+    pixel; residual of the range; inliers of the range).
+    valid_f32: take the pixel set from the fp32 validity chain (the kernels' and se3_run_step's f32 flavour)."""
+    img0, img1, dpt0, grad1 = map(_f32, (img0, img1, dpt0, grad1))
+    H, W = img0.shape
+    y_end = H if y_end is None else min(int(y_end), H)
+    y_begin = max(0, min(int(y_begin), y_end))
+    se3 = np.ascontiguousarray(se3, dtype=np.float32)
+    c = _cam(cam)
+    inl = C.c_uint64(0)
+    res = C.c_double(0)
+    rows = np.empty(((y_end - y_begin) * W, 7), dtype=np.float64)
+    lib().dfko_se3_pixel_rows_d(_ptr(se3), C.byref(c), C.c_int(W), C.c_int(H), _ptr(img0), _pitch(img0), _ptr(img1),
+                                _pitch(img1), _ptr(dpt0), _pitch(dpt0), _ptr(grad1), _pitch(grad1),
+                                C.c_float(huber_delta), C.c_int(1 if valid_f32 else 0), C.c_int(y_begin),
+                                C.c_int(y_end), _ptr(rows, C.c_double), C.byref(res), C.byref(inl))
+    return rows, float(res.value), int(inl.value)
+
+
 def se3_warp(se3, cam, img0, img1, dpt0, *, precision="f32"):
     img0, img1, dpt0 = map(_f32, (img0, img1, dpt0))
     H, W = img0.shape
@@ -298,15 +319,36 @@ def se3_track(pose_ck, cams, pyr_img0, pyr_img1, pyr_dpt0, pyr_grad1, iterations
     return pose, frac, err, hist
 
 
-def update_depth(code, prx_orig, prx_jac, avg_dpt=2.0):
+def update_depth(code, prx_orig, prx_jac, avg_dpt=2.0, *, precision="f32"):
+    """UpdateDepth on the CPU: dpt = avg / (prx_orig + prx_jac . code) - avg, in fp32 (reference-like) or fp64"""
     code = np.ascontiguousarray(code, dtype=np.float32)
     prx_orig, prx_jac = _f32(prx_orig), _f32(prx_jac)
     H, W = prx_orig.shape
-    out = np.zeros((H, W), dtype=np.float32)
-    lib().dfko_update_depth_f(_ptr(code), C.c_int(code.shape[0]), C.c_int(W), C.c_int(H), _ptr(prx_orig),
-                              _pitch(prx_orig), _ptr(prx_jac), _pitch(prx_jac), C.c_float(avg_dpt), _ptr(out),
-                              _pitch(out))
+    args = (_ptr(code), C.c_int(code.shape[0]), C.c_int(W), C.c_int(H), _ptr(prx_orig), _pitch(prx_orig),
+            _ptr(prx_jac), _pitch(prx_jac), C.c_float(avg_dpt))
+    if precision == "f64":
+        out = np.zeros((H, W), dtype=np.float64)
+        lib().dfko_update_depth_d(*args, _ptr(out, C.c_double), C.c_size_t(W))
+    else:
+        out = np.zeros((H, W), dtype=np.float32)
+        lib().dfko_update_depth_f(*args, _ptr(out), _pitch(out))
     return out
+
+
+def depth_pixel_rows(code, target_dpt, prx_orig, prx_jac, avg_dpt=2.0, *, y_begin=0, y_end=None):
+    """The fp64 per-pixel rows that depth_run_step(..., precision="f64") sums, for image rows y_begin .. y_end-1:
+    [(y_end - y_begin) * W, C + 1] float64, row-major over the pixels, [J (C) | diff]; every pixel counts."""
+    code = np.ascontiguousarray(code, dtype=np.float32)
+    tgt, prx_orig, prx_jac = _f32(target_dpt), _f32(prx_orig), _f32(prx_jac)
+    H, W = tgt.shape
+    Cs = code.shape[0]
+    y_end = H if y_end is None else min(int(y_end), H)
+    y_begin = max(0, min(int(y_begin), y_end))
+    rows = np.empty(((y_end - y_begin) * W, Cs + 1), dtype=np.float64)
+    lib().dfko_depth_pixel_rows_d(_ptr(code), C.c_int(Cs), C.c_int(W), C.c_int(H), _ptr(tgt), _pitch(tgt),
+                                  _ptr(prx_orig), _pitch(prx_orig), _ptr(prx_jac), _pitch(prx_jac), C.c_float(avg_dpt),
+                                  C.c_int(y_begin), C.c_int(y_end), _ptr(rows, C.c_double))
+    return rows
 
 
 def depth_run_step(code, target_dpt, prx_orig, prx_jac, avg_dpt=2.0, *, precision="f32") -> StepResult:

@@ -18,6 +18,12 @@ of these scales, the reference-like fp32 CPU path (one serial chain per entry) a
 the kernel bugs emulated in tests/test_system_accuracy.py (tf32 without its low part, the low part of code features
 24-31 lost, LH^T missing, a 128-pixel tile dropped, the code Jacobian rounded to tf32) at >= 3.6e-4 / 3.2e-6: the bars
 sit 4x or more below every one of them.
+
+The same bars apply to systems that reduce plain rows [J | r] with no expansion (E = I): RowGram builds H, Jtr and the
+scales S = sum |J|^T |J|, B_i = sum |J_i r| from any row set, se3_reference() does it for the tracker's SE3 step and
+depth_reference() for DepthAligner, from the oracle's fp64 per-pixel rows (entry names: SE3_NAMES, CODE_NAMES).
+UpdateDepth, a per-pixel decode, is held per pixel to UD_BAR times an error scale derived from its own roundings
+(update_depth_scale).  tests/test_tracker_depth_accuracy.py shows which emulated bugs these bars reject.
 """
 from __future__ import annotations
 
@@ -108,6 +114,100 @@ def _dense(JtJ, n):
     return H + np.triu(H, 1).T
 
 
+class RowGram:
+    """fp64 Gram of plain rows [J (n) | r], fed chunk by chunk: H = sum J^T J, Jtr = sum J r, residual = sum r^2, and the
+    scales S = sum |J|^T |J| and B_i = sum |J_i r| (the rows are what the kernel reduces, so E = I above)."""
+
+    def __init__(self, n):
+        self.n = n
+        self.G = np.zeros((n + 1, n + 1))
+        self.A = np.zeros((n, n))
+        self.B = np.zeros(n)
+
+    def add(self, X):
+        X = np.asarray(X, dtype=np.float64)
+        self.G += X.T @ X
+        a = np.abs(X[:, :self.n])
+        self.A += a.T @ a
+        self.B += (a * np.abs(X[:, self.n:])).sum(0)
+        return self
+
+    def reference(self, inliers, valid=None) -> Reference:
+        n = self.n
+        return Reference(self.G[:n, :n].copy(), self.G[:n, n].copy(), float(self.G[n, n]), int(inliers), self.A.copy(),
+                         self.B.copy(), valid)
+
+
+def se3_reference(se3, cam, img0, img1, dpt0, grad1, huber_delta=0.1, *, valid_f32=True,
+                  chunk_pixels=1 << 18) -> Reference:
+    """fp64 truth of one SE3Aligner::RunStep from the oracle's per-pixel rows.  valid_f32 (default): the pixel set of
+    the fp32 validity chain, which the kernels run -- so the system stays comparable entry by entry at poses where
+    fp32 and fp64 disagree on a border pixel (identity-like poses, small levels)."""
+    H_, W_ = img0.shape
+    g = RowGram(6)
+    inliers = 0
+    step = max(1, chunk_pixels // W_)
+    for y0 in range(0, H_, step):
+        X, _, n_ = orc.se3_pixel_rows(se3, cam, img0, img1, dpt0, grad1, huber_delta, valid_f32=valid_f32,
+                                      y_begin=y0, y_end=y0 + step)
+        g.add(X)
+        inliers += n_
+    return g.reference(inliers)
+
+
+def depth_reference(code, target_dpt, prx_orig, prx_jac, avg_dpt=2.0, *, chunk_pixels=1 << 16) -> Reference:
+    """fp64 truth of one DepthAligner::RunStep from the oracle's per-pixel rows (every pixel is an inlier)"""
+    H_, W_ = target_dpt.shape
+    g = RowGram(np.asarray(code).shape[0])
+    step = max(1, chunk_pixels // W_)
+    for y0 in range(0, H_, step):
+        g.add(orc.depth_pixel_rows(code, target_dpt, prx_orig, prx_jac, avg_dpt, y_begin=y0, y_end=y0 + step))
+    return g.reference(H_ * W_)
+
+
+# --------------------------------------------------------------------------------------------- UpdateDepth
+UD_BAR = 1e-6
+
+
+def update_depth_scale(code, prx_orig, prx_jac, avg_dpt, *, chunk_pixels=1 << 16):
+    """per-pixel error scale of the fp32 decode dpt = avg / (prx_orig + j . c) - avg, from its own roundings:
+
+        S_px = (avg / prx^2) (|prx_orig| + sum_k |j_k c_k|) + avg / |prx|
+
+    The first term carries the rounding of the dot product and of the add (each at most eps times the sum of the
+    magnitudes that went into it) through d dpt / d prx = -avg / prx^2; the second is the division and the final
+    subtraction (|dpt| <= avg / |prx| wherever 0 < prx < 1, the range a proximity lives in).
+
+    UpdateDepth is held to |dpt - dpt64| <= UD_BAR S_px = 1e-6 S_px, about 17 eps (eps = 2^-24).  Worst cases: a
+    serial fp32 chain over C terms errs by at most C eps of sum |j c| but, with the rounding errors independent and the
+    partial sums a random walk, typically by about 0.5 eps of it, and the worst of 1.2 M pixels by a few eps; a tree
+    (the vectorised kernel's lane split and shuffle sum) errs by log2(C) eps at most.  The add, division and
+    subtraction are one rounding each.  So a correct decode sits at a few eps, the bar leaves room for the serial
+    C = 256 generic kernel, and any lost term (one float4 lane dropped: 4 of C terms, about 3 % of sum |j c| at
+    C = 128) or a tf32-rounded operand (2^-11 relative per term, 4e-4 of sum |j c| / sqrt(C)) is far above it."""
+    code = np.asarray(code, dtype=np.float64)
+    H_, W_ = prx_orig.shape
+    ac = np.abs(code)
+    s = np.empty((H_, W_))
+    prx = np.empty((H_, W_))
+    step = max(1, chunk_pixels // W_)
+    for y0 in range(0, H_, step):
+        J = np.asarray(prx_jac[y0:y0 + step], dtype=np.float64)
+        po = np.asarray(prx_orig[y0:y0 + step], dtype=np.float64)
+        prx[y0:y0 + step] = po + J @ code
+        s[y0:y0 + step] = np.abs(po) + np.abs(J) @ ac
+    avg = float(avg_dpt)
+    return avg / prx ** 2 * s + avg / np.abs(prx)
+
+
+def update_depth_errors(got, ref64, scale):
+    """worst per-pixel ratio |got - ref64| / scale and where it is"""
+    r = np.abs(np.asarray(got, np.float64) - ref64) / scale
+    k = int(np.argmax(r))
+    return float(r.reshape(-1)[k]), np.unravel_index(k, r.shape)
+
+
+# --------------------------------------------------------------------------------------------- entry names
 def _name(i):
     if i >= 12:
         return f"code {i - 12}"
@@ -116,6 +216,11 @@ def _name(i):
 
 def _block(i):
     return "code" if i >= 12 else ("t0", "w0", "t1", "w1")[i // 3]
+
+
+SFM_NAMES = (_name, _block)
+SE3_NAMES = (lambda i: ("t", "w")[i // 3] + f" {i % 3}", lambda i: ("t", "w")[i // 3])
+CODE_NAMES = (lambda i: f"code {i}", lambda i: "code")
 
 
 def _ratio(err, scale):
@@ -139,13 +244,16 @@ def system_errors(got, ref, S, B):
     return dict(h=float(rh[k]), h_at=(int(iu[0][k]), int(iu[1][k])), jtr=float(rj[q]), jtr_at=q, res=rres, Hg=Hg)
 
 
-def assert_system_close(got, ref, S, B, what, *, h_bar=H_BAR, jtr_bar=JTR_BAR, res_bar=RES_BAR):
+def assert_system_close(got, ref, S, B, what, *, h_bar=H_BAR, jtr_bar=JTR_BAR, res_bar=RES_BAR, names=SFM_NAMES):
     """inliers exactly; max_ij |H - H64|_ij / S_ij <= h_bar (upper triangle); max_i |Jtr - Jtr64|_i / B_i <= jtr_bar;
-    residual to res_bar relative.  The message names the worst entry, its block, value and scale.  Returns the errors."""
+    residual to res_bar relative.  The message names the worst entry, its block, value and scale (names: SFM_NAMES for
+    the [pose0 | pose1 | code] system, SE3_NAMES for the tracker's [t | w], CODE_NAMES for DepthAligner's code-only
+    one).  Returns the errors."""
     assert int(got.inliers) == int(ref.inliers), f"{what}: inliers {got.inliers} != {ref.inliers}"
     e = system_errors(got, ref, S, B)
     i, j = e["h_at"]
     q = e["jtr_at"]
+    _name, _block = names
     msg = (f"{what}: worst H entry [{_block(i)}/{_block(j)}] ({_name(i)}, {_name(j)}): got {e['Hg'][i, j]:.9e} "
            f"ref {ref.H[i, j]:.9e} scale S {S[i, j]:.3e} -> {e['h']:.2e} (bar {h_bar:.0e}); "
            f"worst Jtr entry [{_block(q)}] ({_name(q)}): got {float(got.Jtr[q]):.9e} ref {ref.Jtr[q]:.9e} "
