@@ -265,6 +265,54 @@ class SfmAligner:
 
 
 # ------------------------------------------------------------------------------------------- sparse keypoint factor
+def _reprojection_item(it: dict, cs: int, keep: list) -> DfkReprojectionItem:
+    """one ReprojectionFactor's arguments as the C item; the host arrays go into `keep`, which must outlive the call"""
+    code = np.ascontiguousarray(it["code0"], dtype=np.float32)
+    if code.shape != (cs,):
+        raise ValueError(f"code0 must have {cs} entries")
+    q = np.ascontiguousarray(it["query_xy"], dtype=np.float32).reshape(-1, 2)
+    t = np.ascontiguousarray(it["train_xy"], dtype=np.float32).reshape(-1, 2)
+    if q.shape != t.shape:
+        raise ValueError("query_xy and train_xy must hold the same number of matches")
+    keep += [code, q, t]
+    FP = C.POINTER(C.c_float)
+    w = DfkReprojectionItem()
+    w.pose0, w.pose1, w.cam = _pose(it["pose0"]), _pose(it["pose1"]), _cam(it["cam"])
+    w.prx_orig, w.prx_jac = _image(it["prx_orig"]), _image(it["prx_jac"], cs)
+    w.code, w.query_xy, w.train_xy = code.ctypes.data_as(FP), q.ctypes.data_as(FP), t.ctypes.data_as(FP)
+    w.num_matches = q.shape[0]
+    w.cauchy_delta, w.sigma = float(it["cauchy_delta"]), float(it["sigma"])
+    return w
+
+
+def _geometric_item(it: dict, cs: int, keep: list) -> DfkSparseGeometricItem:
+    """one SparseGeometricFactor's arguments as the C item; the host arrays go into `keep`, which must outlive the call"""
+    c0 = np.ascontiguousarray(it["code0"], dtype=np.float32)
+    c1 = np.ascontiguousarray(it["code1"], dtype=np.float32)
+    if c0.shape != (cs,) or c1.shape != (cs,):
+        raise ValueError(f"code0 and code1 must have {cs} entries")
+    pts = np.ascontiguousarray(it["points_xy"], dtype=np.int32).reshape(-1, 2)
+    keep += [c0, c1, pts]
+    FP, IP = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+    w = DfkSparseGeometricItem()
+    w.pose0, w.pose1, w.cam = _pose(it["pose0"]), _pose(it["pose1"]), _cam(it["cam"])
+    w.prx0_orig, w.prx0_jac = _image(it["prx0_orig"]), _image(it["prx0_jac"], cs)
+    w.prx1_orig, w.prx1_jac = _image(it["prx1_orig"]), _image(it["prx1_jac"], cs)
+    w.dpt_grad1 = _image(it["dpt_grad1"], 2)
+    w.code0, w.code1, w.points_xy = c0.ctypes.data_as(FP), c1.ctypes.data_as(FP), pts.ctypes.data_as(IP)
+    w.num_points = pts.shape[0]
+    w.huber_delta = float(it["huber_delta"])
+    return w
+
+
+def _batch_records(aligner, n: int, rec: int, records: torch.Tensor | None) -> torch.Tensor:
+    if records is None:
+        return torch.empty((n, rec), dtype=torch.float32, device=f"cuda:{aligner._hd.device}")
+    if not (records.is_contiguous() and records.numel() >= n * rec):
+        raise ValueError(f"records must be a contiguous device tensor of at least {n} x {rec} floats")
+    return records
+
+
 def ReprojectionLinearize(aligner, pose0, pose1, code0, cam, prx_orig, prx_jac, query_xy, train_xy, cauchy_delta: float,
                           sigma: float):
     """ReprojectionFactor::linearize (sources/core/gtsam/reprojection_factor.cpp:157-269) with the rows gathered on the
@@ -272,18 +320,14 @@ def ReprojectionLinearize(aligner, pose0, pose1, code0, cam, prx_orig, prx_jac, 
     (host).  Returns (rows [2M, 13 + C] float32 = the blocks of the JacobianFactor [J_pose0 | J_pose1 | J_code0 | b],
     total_err)."""
     aligner._hd.use_torch_stream()
-    cs = aligner.CS
-    code = np.ascontiguousarray(code0, dtype=np.float32)
-    q = np.ascontiguousarray(query_xy, dtype=np.float32).reshape(-1, 2)
-    t = np.ascontiguousarray(train_xy, dtype=np.float32).reshape(-1, 2)
-    M = q.shape[0]
-    rows = np.zeros((2 * M, 13 + cs), dtype=np.float32)
+    cs, keep = aligner.CS, []
+    w = _reprojection_item(dict(pose0=pose0, pose1=pose1, code0=code0, cam=cam, prx_orig=prx_orig, prx_jac=prx_jac,
+                                query_xy=query_xy, train_xy=train_xy, cauchy_delta=cauchy_delta, sigma=sigma), cs, keep)
+    rows = np.zeros((2 * w.num_matches, 13 + cs), dtype=np.float32)
     tot = C.c_float(0)
-    FP = C.POINTER(C.c_float)
-    c, p, j = _cam(cam), _image(prx_orig), _image(prx_jac, cs)
     check(aligner.handle, lib().dfk_reprojection_linearize(
-        aligner.handle, _pose(pose0), _pose(pose1), code.ctypes.data_as(FP), cs, C.byref(c), C.byref(p), C.byref(j), M,
-        q.ctypes.data_as(FP), t.ctypes.data_as(FP), C.c_float(cauchy_delta), C.c_float(sigma), rows.ctypes.data_as(FP),
+        aligner.handle, w.pose0, w.pose1, w.code, cs, C.byref(w.cam), C.byref(w.prx_orig), C.byref(w.prx_jac),
+        w.num_matches, w.query_xy, w.train_xy, w.cauchy_delta, w.sigma, rows.ctypes.data_as(C.POINTER(C.c_float)),
         C.byref(tot)))
     return rows, float(tot.value)
 
@@ -296,30 +340,9 @@ def ReprojectionLinearizeBatch(aligner, items: Sequence[dict], records: torch.Te
     (item size (0, 0)).  `records` may be a slice of a larger record buffer.  Asynchronous: returns a device tensor
     [n, DFK_SFM_RECORD_FLOATS(CS)] on torch's current stream."""
     aligner._hd.use_torch_stream()
-    cs, n = aligner.CS, len(items)
-    rec = _lib.record_floats(cs)
-    if records is None:
-        records = torch.empty((n, rec), dtype=torch.float32, device=f"cuda:{aligner._hd.device}")
-    if not (records.is_contiguous() and records.numel() >= n * rec):
-        raise ValueError(f"records must be a contiguous device tensor of at least {n} x {rec} floats")
-    arr = (DfkReprojectionItem * max(n, 1))()
-    keep = []  # the host arrays must outlive the ctypes pointers until the call returns
-    FP = C.POINTER(C.c_float)
-    for k, it in enumerate(items):
-        code = np.ascontiguousarray(it["code0"], dtype=np.float32)
-        if code.shape != (cs,):
-            raise ValueError(f"code0 must have {cs} entries")
-        q = np.ascontiguousarray(it["query_xy"], dtype=np.float32).reshape(-1, 2)
-        t = np.ascontiguousarray(it["train_xy"], dtype=np.float32).reshape(-1, 2)
-        if q.shape != t.shape:
-            raise ValueError("query_xy and train_xy must hold the same number of matches")
-        keep += [code, q, t]
-        w = arr[k]
-        w.pose0, w.pose1, w.cam = _pose(it["pose0"]), _pose(it["pose1"]), _cam(it["cam"])
-        w.prx_orig, w.prx_jac = _image(it["prx_orig"]), _image(it["prx_jac"], cs)
-        w.code, w.query_xy, w.train_xy = code.ctypes.data_as(FP), q.ctypes.data_as(FP), t.ctypes.data_as(FP)
-        w.num_matches = q.shape[0]
-        w.cauchy_delta, w.sigma = float(it["cauchy_delta"]), float(it["sigma"])
+    cs, n, keep = aligner.CS, len(items), []
+    records = _batch_records(aligner, n, _lib.record_floats(cs), records)
+    arr = (DfkReprojectionItem * max(n, 1))(*[_reprojection_item(it, cs, keep) for it in items])
     check(aligner.handle, lib().dfk_reprojection_linearize_batch(aligner.handle, arr, n, cs,
                                                                  C.c_void_p(records.data_ptr())))
     return records
@@ -332,20 +355,16 @@ def SparseGeometricLinearize(aligner, pose0, pose1, code0, code1, cam, prx0_orig
     points_xy the sampled integer pixels [M, 2] (host).  Returns (rows [M, 13 + 2C] float32 = the blocks of the
     JacobianFactor [J_pose0 | J_pose1 | J_code0 | J_code1 | b], number of valid rows)."""
     aligner._hd.use_torch_stream()
-    cs = aligner.CS
-    c0 = np.ascontiguousarray(code0, dtype=np.float32)
-    c1 = np.ascontiguousarray(code1, dtype=np.float32)
-    pts = np.ascontiguousarray(points_xy, dtype=np.int32).reshape(-1, 2)
-    M = pts.shape[0]
-    rows = np.zeros((M, 13 + 2 * cs), dtype=np.float32)
+    cs, keep = aligner.CS, []
+    w = _geometric_item(dict(pose0=pose0, pose1=pose1, code0=code0, code1=code1, cam=cam, prx0_orig=prx0_orig,
+                             prx0_jac=prx0_jac, prx1_orig=prx1_orig, prx1_jac=prx1_jac, dpt_grad1=dpt_grad1,
+                             points_xy=points_xy, huber_delta=huber_delta), cs, keep)
+    rows = np.zeros((w.num_points, 13 + 2 * cs), dtype=np.float32)
     nv = C.c_int(0)
-    FP, IP = C.POINTER(C.c_float), C.POINTER(C.c_int)
-    c = _cam(cam)
-    i0, j0, i1, j1, g1 = _image(prx0_orig), _image(prx0_jac, cs), _image(prx1_orig), _image(prx1_jac, cs), _image(dpt_grad1, 2)
     check(aligner.handle, lib().dfk_sparse_geometric_linearize(
-        aligner.handle, _pose(pose0), _pose(pose1), c0.ctypes.data_as(FP), c1.ctypes.data_as(FP), cs, C.byref(c), C.byref(i0),
-        C.byref(j0), C.byref(i1), C.byref(j1), C.byref(g1), M, pts.ctypes.data_as(IP), C.c_float(huber_delta),
-        rows.ctypes.data_as(FP), C.byref(nv)))
+        aligner.handle, w.pose0, w.pose1, w.code0, w.code1, cs, C.byref(w.cam), C.byref(w.prx0_orig), C.byref(w.prx0_jac),
+        C.byref(w.prx1_orig), C.byref(w.prx1_jac), C.byref(w.dpt_grad1), w.num_points, w.points_xy, w.huber_delta,
+        rows.ctypes.data_as(C.POINTER(C.c_float)), C.byref(nv)))
     return rows, int(nv.value)
 
 
@@ -358,30 +377,9 @@ def SparseGeometricLinearizeBatch(aligner, items: Sequence[dict], records: torch
     larger record buffer.  Asynchronous: returns a device tensor [n, DFK_GEO_RECORD_FLOATS(CS)] on torch's current
     stream."""
     aligner._hd.use_torch_stream()
-    cs, n = aligner.CS, len(items)
-    rec = _lib.geo_record_floats(cs)
-    if records is None:
-        records = torch.empty((n, rec), dtype=torch.float32, device=f"cuda:{aligner._hd.device}")
-    if not (records.is_contiguous() and records.numel() >= n * rec):
-        raise ValueError(f"records must be a contiguous device tensor of at least {n} x {rec} floats")
-    arr = (DfkSparseGeometricItem * max(n, 1))()
-    keep = []  # the host arrays must outlive the ctypes pointers until the call returns
-    FP, IP = C.POINTER(C.c_float), C.POINTER(C.c_int32)
-    for k, it in enumerate(items):
-        c0 = np.ascontiguousarray(it["code0"], dtype=np.float32)
-        c1 = np.ascontiguousarray(it["code1"], dtype=np.float32)
-        if c0.shape != (cs,) or c1.shape != (cs,):
-            raise ValueError(f"code0 and code1 must have {cs} entries")
-        pts = np.ascontiguousarray(it["points_xy"], dtype=np.int32).reshape(-1, 2)
-        keep += [c0, c1, pts]
-        w = arr[k]
-        w.pose0, w.pose1, w.cam = _pose(it["pose0"]), _pose(it["pose1"]), _cam(it["cam"])
-        w.prx0_orig, w.prx0_jac = _image(it["prx0_orig"]), _image(it["prx0_jac"], cs)
-        w.prx1_orig, w.prx1_jac = _image(it["prx1_orig"]), _image(it["prx1_jac"], cs)
-        w.dpt_grad1 = _image(it["dpt_grad1"], 2)
-        w.code0, w.code1, w.points_xy = c0.ctypes.data_as(FP), c1.ctypes.data_as(FP), pts.ctypes.data_as(IP)
-        w.num_points = pts.shape[0]
-        w.huber_delta = float(it["huber_delta"])
+    cs, n, keep = aligner.CS, len(items), []
+    records = _batch_records(aligner, n, _lib.geo_record_floats(cs), records)
+    arr = (DfkSparseGeometricItem * max(n, 1))(*[_geometric_item(it, cs, keep) for it in items])
     check(aligner.handle, lib().dfk_sparse_geometric_linearize_batch(aligner.handle, arr, n, cs,
                                                                      C.c_void_p(records.data_ptr())))
     return records

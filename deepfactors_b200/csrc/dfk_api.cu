@@ -87,8 +87,9 @@ struct DfkContext {
   DeviceBuf<float> batch_partials;
   DeviceBuf<unsigned int> batch_counters;
 
-  DeviceBuf<float> sparse_dev;           // dfk_reprojection_linearize: [query | train | rows | err2]
-  PinnedBuf<float> sparse_host;          // mirror
+  // dfk_reprojection_linearize / dfk_sparse_geometric_linearize: [one item's staging block | rows (| err2)]
+  DeviceBuf<unsigned char> sparse_dev;
+  PinnedBuf<unsigned char> sparse_host;  // mirror
   // dfk_reprojection_linearize_batch: [descriptors | codes | query | train] (bytes), one H2D per call from rep_host
   DeviceBuf<unsigned char> rep_dev;
   std::vector<unsigned char> rep_host;
@@ -617,6 +618,128 @@ DfkStatus run_batch(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_si
   DFK_CUDA(h, launch_sfm_finalize(code_size, tc, items_dev, n, partials_dev, records_dev, h->stream),
            "[SfmAligner::RunStep] kernel launch failed");
   h->launches += 2;  // step kernel + finalize kernel
+  return DFK_OK;
+}
+
+// ---------------------------------------------------------------------------- sparse factors
+// A single call is a batch of one: the same checks, descriptors and staging.  Sparse<Item> is what the two factor kinds
+// stage differently: the argument check (the failure text, or null), the matches / points of a factor and the bytes each
+// takes, the codes per factor, and one factor's descriptor, codes and payload.
+template <class Item>
+struct Sparse;
+
+template <>
+struct Sparse<DfkReprojectionItem> {
+  using Dev = ReprojItemDev;
+  static constexpr int codes = 1;
+  static constexpr size_t unit_bytes = 4 * sizeof(float);  // payload: query 2 total | train 2 total
+  static constexpr const char* units = "matches";
+  static size_t count(const DfkReprojectionItem& it) { return (size_t)it.num_matches; }
+  static const char* error(const DfkReprojectionItem& it, int code_size)
+  {
+    if (!it.code || !it.query_xy || !it.train_xy) return "null argument";
+    if (it.num_matches < 1 || !(it.sigma > 0.0f)) return "no matches / non-positive sigma";
+    const uint32_t W = it.prx_orig.width, H = it.prx_orig.height;
+    if (W == 0 || H == 0 || !img_ok(&it.prx_orig, W, H, 1) || !img_ok(&it.prx_jac, W, H, code_size))
+      return "inconsistent image views";
+    return nullptr;
+  }
+  // begin: the factor's first match, total: the matches of the block
+  static void pack(const DfkReprojectionItem& it, int code_size, size_t begin, size_t total, Dev& d, float* code,
+                   const float* code_dev, unsigned char* payload)
+  {
+    d = Dev{{}, view_of(&it.prx_orig), view_of(&it.prx_jac), code_dev, (int)it.prx_orig.width, (int)it.prx_orig.height,
+            it.num_matches, (int)begin, it.cauchy_delta, it.sigma};
+    set_relative_pose(d.sp, it.pose1, it.pose0, it.cam);  // pose10_J_pose1, pose10_J_pose0 (:189-190)
+    memcpy(code, it.code, sizeof(float) * code_size);
+    float* query = reinterpret_cast<float*>(payload);
+    memcpy(query + 2 * begin, it.query_xy, sizeof(float) * 2 * it.num_matches);
+    memcpy(query + 2 * (total + begin), it.train_xy, sizeof(float) * 2 * it.num_matches);
+  }
+};
+
+template <>
+struct Sparse<DfkSparseGeometricItem> {
+  using Dev = GeoItemDev;
+  static constexpr int codes = 2;  // code0, code1
+  static constexpr size_t unit_bytes = 2 * sizeof(int32_t);  // payload: points 2 total
+  static constexpr const char* units = "points";
+  static size_t count(const DfkSparseGeometricItem& it) { return (size_t)it.num_points; }
+  static const char* error(const DfkSparseGeometricItem& it, int code_size)
+  {
+    if (!it.code0 || !it.code1 || !it.points_xy) return "null argument";
+    if (it.num_points < 1 || !(it.huber_delta > 0.0f)) return "no points / non-positive huber delta";
+    const uint32_t W = it.prx0_orig.width, H = it.prx0_orig.height;
+    if (W == 0 || H == 0 || !img_ok(&it.prx0_orig, W, H, 1) || !img_ok(&it.prx0_jac, W, H, code_size) ||
+        !img_ok(&it.prx1_orig, W, H, 1) || !img_ok(&it.prx1_jac, W, H, code_size) || !img_ok(&it.dpt_grad1, W, H, 2))
+      return "inconsistent image views";
+    // the nearest-neighbour lookups in keyframe 1 index with the camera's validity window
+    if (!cam_ok(&it.cam, W, H)) return "camera larger than the image views";
+    return nullptr;
+  }
+  static void pack(const DfkSparseGeometricItem& it, int code_size, size_t begin, size_t /*total*/, Dev& d, float* code,
+                   const float* code_dev, unsigned char* payload)
+  {
+    d = Dev{{}, view_of(&it.prx0_orig), view_of(&it.prx0_jac), view_of(&it.prx1_orig), view_of(&it.prx1_jac),
+            view_of(&it.dpt_grad1), code_dev, code_dev + code_size, it.cam.width, it.cam.height, (int)it.prx0_orig.width,
+            (int)it.prx0_orig.height, it.num_points, (int)begin, it.huber_delta};
+    set_relative_pose(d.sp, it.pose1, it.pose0, it.cam);  // pose10_J_pose1, pose10_J_pose0 (:176-178)
+    memcpy(code, it.code0, sizeof(float) * code_size);
+    memcpy(code + code_size, it.code1, sizeof(float) * code_size);
+    memcpy(reinterpret_cast<int32_t*>(payload) + 2 * begin, it.points_xy, sizeof(int32_t) * 2 * it.num_points);
+  }
+};
+
+// Host staging: the batches stage in pageable memory (cudaMemcpyAsync has read it when it returns, so the next batch may
+// refill it while the copy is still queued); the synchronous single calls in pinned memory, into which their rows return.
+cudaError_t host_block(std::vector<unsigned char>& v, size_t bytes, unsigned char** p)
+{
+  v.assign(bytes, 0);
+  *p = v.data();
+  return cudaSuccess;
+}
+cudaError_t host_block(PinnedBuf<unsigned char>& b, size_t bytes, unsigned char** p)
+{
+  const cudaError_t e = b.ensure(bytes);
+  *p = b.ptr;
+  return e;
+}
+
+struct Staged {
+  size_t bytes = 0;               // of the uploaded block; the caller's outputs may follow it
+  size_t total = 0;               // matches / points
+  const unsigned char* payload = nullptr;  // device address of the matches / points
+};
+
+// Checks the code size and items[0, n) (messages begin with `what`, a batch's name the item), then stages the factors in
+// one upload: [descriptors n | codes n x codes C | payload], packed in `host` and copied to `dev`, both grown by
+// out_bytes for the caller's outputs.
+template <class Item, class HostBuf>
+DfkStatus stage(DfkHandle h, const std::string& what, bool batch, const Item* items, int n, int code_size,
+                size_t out_bytes, HostBuf& host, DeviceBuf<unsigned char>& dev, Staged* st)
+{
+  using S = Sparse<Item>;
+  if (!sparse_supported(code_size))
+    return fail(h, DFK_ERR_UNSUPPORTED, what + "code size not instantiated: " + std::to_string(code_size));
+  for (int i = 0; i < n; ++i) {
+    if (const char* e = S::error(items[i], code_size))
+      return fail(h, DFK_ERR_INVALID_ARG, what + (batch ? "item " + std::to_string(i) + ": " : "") + e);
+    st->total += S::count(items[i]);
+  }
+  if (st->total > (size_t)INT32_MAX)
+    return fail(h, DFK_ERR_INVALID_ARG, what + "more than 2^31 - 1 " + S::units + " in one call");
+  const size_t desc_bytes = (sizeof(typename S::Dev) * (size_t)n + 15) & ~(size_t)15;
+  const size_t code_floats = (size_t)S::codes * code_size, payload = desc_bytes + sizeof(float) * n * code_floats;
+  st->bytes = payload + S::unit_bytes * st->total;
+  DFK_CUDA(h, dev.ensure(st->bytes + out_bytes), (what + "scratch allocation failed").c_str());
+  unsigned char* hb = nullptr;
+  DFK_CUDA(h, host_block(host, st->bytes + out_bytes, &hb), (what + "pinned allocation failed").c_str());
+  const float* codes_dev = reinterpret_cast<const float*>(dev.ptr + desc_bytes);
+  for (size_t i = 0, begin = 0; i < (size_t)n; begin += S::count(items[i]), ++i)
+    S::pack(items[i], code_size, begin, st->total, reinterpret_cast<typename S::Dev*>(hb)[i],
+            reinterpret_cast<float*>(hb + desc_bytes) + i * code_floats, codes_dev + i * code_floats, hb + payload);
+  DFK_CUDA(h, cudaMemcpyAsync(dev.ptr, hb, st->bytes, cudaMemcpyHostToDevice, h->stream), (what + "upload failed").c_str());
+  st->payload = dev.ptr + payload;
   return DFK_OK;
 }
 
@@ -1459,44 +1582,30 @@ DfkStatus dfk_reprojection_linearize(DfkHandle h, const float pose0[7], const fl
                                      float sigma, float* rows, float* total_err)
 {
   return guarded(h, [&] {
-    if (!pose0 || !pose1 || !code0 || !cam || !prx_orig || !prx_jac || !query_xy || !train_xy || !rows || !total_err)
+    if (!pose0 || !pose1 || !cam || !prx_orig || !prx_jac || !rows || !total_err)
       return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::linearize] null argument");
-    if (!sparse_supported(code_size))
-      return fail(h, DFK_ERR_UNSUPPORTED, "[ReprojectionFactor::linearize] code size not instantiated: " + std::to_string(code_size));
-    if (num_matches <= 0 || !(sigma > 0.0f))
-      return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::linearize] no matches / non-positive sigma");
-    const uint32_t W = prx_orig->width, H = prx_orig->height;
-    if (W == 0 || H == 0 || !img_ok(prx_orig, W, H, 1) || !img_ok(prx_jac, W, H, code_size))
-      return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::linearize] inconsistent image views");
+    DfkReprojectionItem it{{}, {}, *cam, *prx_orig, *prx_jac, code0, num_matches, query_xy, train_xy, cauchy_delta, sigma};
+    std::copy_n(pose0, 7, it.pose0);
+    std::copy_n(pose1, 7, it.pose1);
     DeviceGuard guard(h->device);
-    const size_t M = (size_t)num_matches, RW = 13 + (size_t)code_size;
-    const size_t n_in = 4 * M, n_out = 2 * M * RW + M;
-    DFK_CUDA(h, h->sparse_dev.ensure(n_in + n_out), "[ReprojectionFactor::linearize] scratch allocation failed");
-    DFK_CUDA(h, h->sparse_host.ensure(n_in + n_out), "[ReprojectionFactor::linearize] pinned allocation failed");
-    SparsePose sp;
-    set_relative_pose(sp, pose1, pose0, *cam);  // pose10_J_pose1, pose10_J_pose0 (:189-190)
-    float* host = h->sparse_host.ptr;
-    memcpy(host, query_xy, 2 * M * sizeof(float));
-    memcpy(host + 2 * M, train_xy, 2 * M * sizeof(float));
-    float* d_query = h->sparse_dev.ptr;
-    float* d_train = d_query + 2 * M;
-    float* d_rows = d_train + 2 * M;
-    float* d_err2 = d_rows + 2 * M * RW;
-    DFK_CUDA(h, cudaMemcpyAsync(h->code_dev.ptr, code0, sizeof(float) * code_size, cudaMemcpyHostToDevice, h->stream),
-             "[ReprojectionFactor::linearize] code upload failed");
-    DFK_CUDA(h, cudaMemcpyAsync(d_query, host, n_in * sizeof(float), cudaMemcpyHostToDevice, h->stream),
-             "[ReprojectionFactor::linearize] match upload failed");
-    DFK_CUDA(h, launch_reprojection_rows(sp, h->code_dev.ptr, code_size, view_of(prx_orig), view_of(prx_jac), (int)W,
-                                         (int)H, num_matches, d_query, d_train, cauchy_delta, sigma,
-                                         h->params.sfmparams.avg_dpt, d_rows, d_err2, h->stream),
+    // [the one item's staging | rows | err2], in scratch of its own: an earlier asynchronous batch may still be reading
+    // the batches' staging
+    const size_t M = (size_t)num_matches, RW = 13 + (size_t)code_size, n_out = 2 * M * RW + M;
+    Staged st;
+    DFK_TRY(stage(h, "[ReprojectionFactor::linearize] ", false, &it, 1, code_size, n_out * sizeof(float), h->sparse_host,
+                  h->sparse_dev, &st));
+    const float2* d_query = reinterpret_cast<const float2*>(st.payload);
+    float* d_rows = reinterpret_cast<float*>(h->sparse_dev.ptr + st.bytes);
+    DFK_CUDA(h, launch_reprojection_rows(code_size, *reinterpret_cast<const ReprojItemDev*>(h->sparse_host.ptr), d_query,
+                                         d_query + M, h->params.sfmparams.avg_dpt, d_rows, d_rows + 2 * M * RW, h->stream),
              "[ReprojectionFactor::linearize] kernel launch failed");
     h->launches += 1;
-    DFK_TRY(download(h, host + n_in, d_rows, n_out * sizeof(float), "[ReprojectionFactor::linearize] result download failed",
+    float* out = reinterpret_cast<float*>(h->sparse_host.ptr + st.bytes);
+    DFK_TRY(download(h, out, d_rows, n_out * sizeof(float), "[ReprojectionFactor::linearize] result download failed",
                      "[ReprojectionFactor::linearize] kernel launch failed"));
-    memcpy(rows, host + n_in, 2 * M * RW * sizeof(float));
+    memcpy(rows, out, 2 * M * RW * sizeof(float));
     float tot = 0.0f;  // Scalar total_err accumulated in match order (:179,242)
-    const float* e2 = host + n_in + 2 * M * RW;
-    for (size_t i = 0; i < M; ++i) tot += e2[i];
+    for (size_t i = 0; i < M; ++i) tot += out[2 * M * RW + i];
     *total_err = tot;
     return DFK_OK;
   });
@@ -1508,60 +1617,12 @@ DfkStatus dfk_reprojection_linearize_batch(DfkHandle h, const DfkReprojectionIte
   return guarded(h, [&] {
     if (!items || n < 1 || !records_dev)
       return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::linearize batch] null argument / empty batch");
-    if (!sparse_supported(code_size))
-      return fail(h, DFK_ERR_UNSUPPORTED,
-                  "[ReprojectionFactor::linearize batch] code size not instantiated: " + std::to_string(code_size));
-    size_t total = 0;  // matches of the whole batch
-    for (int i = 0; i < n; ++i) {
-      const DfkReprojectionItem& it = items[i];
-      const std::string at = "[ReprojectionFactor::linearize batch] item " + std::to_string(i) + ": ";
-      if (!it.code || !it.query_xy || !it.train_xy) return fail(h, DFK_ERR_INVALID_ARG, at + "null argument");
-      if (it.num_matches < 1 || !(it.sigma > 0.0f))
-        return fail(h, DFK_ERR_INVALID_ARG, at + "no matches / non-positive sigma");
-      const uint32_t W = it.prx_orig.width, H = it.prx_orig.height;
-      if (W == 0 || H == 0 || !img_ok(&it.prx_orig, W, H, 1) || !img_ok(&it.prx_jac, W, H, code_size))
-        return fail(h, DFK_ERR_INVALID_ARG, at + "inconsistent image views");
-      total += (size_t)it.num_matches;
-    }
-    if (total > (size_t)INT32_MAX)
-      return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::linearize batch] more than 2^31 - 1 matches in one call");
     DeviceGuard guard(h->device);
-    // one upload: [descriptors n | codes n x C | query 2 total | train 2 total]
-    const size_t desc_bytes = (sizeof(ReprojItemDev) * (size_t)n + 15) & ~(size_t)15;
-    const size_t code_bytes = sizeof(float) * (size_t)n * code_size;
-    const size_t match_bytes = sizeof(float) * 2 * total;
-    const size_t bytes = desc_bytes + code_bytes + 2 * match_bytes;
-    DFK_CUDA(h, h->rep_dev.ensure(bytes), "[ReprojectionFactor::linearize batch] scratch allocation failed");
-    h->rep_host.assign(bytes, 0);
-    ReprojItemDev* descs = reinterpret_cast<ReprojItemDev*>(h->rep_host.data());
-    float* codes = reinterpret_cast<float*>(h->rep_host.data() + desc_bytes);
-    float* query = reinterpret_cast<float*>(h->rep_host.data() + desc_bytes + code_bytes);
-    float* train = query + 2 * total;
-    const float* codes_dev = reinterpret_cast<const float*>(h->rep_dev.ptr + desc_bytes);
-    const float* query_dev = reinterpret_cast<const float*>(h->rep_dev.ptr + desc_bytes + code_bytes);
-    size_t begin = 0;
-    for (int i = 0; i < n; ++i) {
-      const DfkReprojectionItem& it = items[i];
-      ReprojItemDev& d = descs[i];
-      set_relative_pose(d.sp, it.pose1, it.pose0, it.cam);  // as dfk_reprojection_linearize
-      d.prx_orig = view_of(&it.prx_orig);
-      d.jac = view_of(&it.prx_jac);
-      d.code = codes_dev + (size_t)i * code_size;
-      d.width = (int)it.prx_orig.width;
-      d.height = (int)it.prx_orig.height;
-      d.num_matches = it.num_matches;
-      d.match_begin = (int)begin;
-      d.cauchy_delta = it.cauchy_delta;
-      d.sigma = it.sigma;
-      memcpy(codes + (size_t)i * code_size, it.code, sizeof(float) * code_size);
-      memcpy(query + 2 * begin, it.query_xy, sizeof(float) * 2 * it.num_matches);
-      memcpy(train + 2 * begin, it.train_xy, sizeof(float) * 2 * it.num_matches);
-      begin += (size_t)it.num_matches;
-    }
-    DFK_CUDA(h, cudaMemcpyAsync(h->rep_dev.ptr, h->rep_host.data(), bytes, cudaMemcpyHostToDevice, h->stream),
-             "[ReprojectionFactor::linearize batch] upload failed");
+    Staged st;
+    DFK_TRY(stage(h, "[ReprojectionFactor::linearize batch] ", true, items, n, code_size, 0, h->rep_host, h->rep_dev, &st));
+    const float2* query_dev = reinterpret_cast<const float2*>(st.payload);
     DFK_CUDA(h, launch_reprojection_records(code_size, reinterpret_cast<const ReprojItemDev*>(h->rep_dev.ptr), n,
-                                            query_dev, query_dev + 2 * total, h->params.sfmparams.avg_dpt, records_dev,
+                                            query_dev, query_dev + st.total, h->params.sfmparams.avg_dpt, records_dev,
                                             h->stream),
              "[ReprojectionFactor::linearize batch] kernel launch failed");
     h->launches += 1;
@@ -1576,56 +1637,31 @@ DfkStatus dfk_sparse_geometric_linearize(DfkHandle h, const float pose0[7], cons
                                          float* rows, int* num_valid)
 {
   return guarded(h, [&] {
-    if (!pose0 || !pose1 || !code0 || !code1 || !cam || !prx0_orig || !prx0_jac || !prx1_orig || !prx1_jac || !dpt_grad1 ||
-        !points_xy || !rows)
+    if (!pose0 || !pose1 || !cam || !prx0_orig || !prx0_jac || !prx1_orig || !prx1_jac || !dpt_grad1 || !rows)
       return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::linearize] null argument");
-    if (!sparse_supported(code_size))
-      return fail(h, DFK_ERR_UNSUPPORTED, "[SparseGeometricFactor::linearize] code size not instantiated: " + std::to_string(code_size));
-    if (num_points <= 0 || !(huber_delta > 0.0f))
-      return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::linearize] no points / non-positive huber delta");
-    const uint32_t W = prx0_orig->width, H = prx0_orig->height;
-    if (W == 0 || H == 0 || !img_ok(prx0_orig, W, H, 1) || !img_ok(prx0_jac, W, H, code_size) || !img_ok(prx1_orig, W, H, 1) ||
-        !img_ok(prx1_jac, W, H, code_size) || !img_ok(dpt_grad1, W, H, 2))
-      return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::linearize] inconsistent image views");
-    if (!cam_ok(cam, W, H))  // the nearest-neighbour lookups in keyframe 1 index with the camera's validity window
-      return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::linearize] camera larger than the image views");
+    DfkSparseGeometricItem it{{}, {}, *cam, *prx0_orig, *prx0_jac, *prx1_orig, *prx1_jac, *dpt_grad1, code0, code1,
+                              num_points, points_xy, huber_delta};
+    std::copy_n(pose0, 7, it.pose0);
+    std::copy_n(pose1, 7, it.pose1);
     DeviceGuard guard(h->device);
+    // [the one item's staging | rows], apart from the batches' staging
     const size_t M = (size_t)num_points, RW = 13 + 2 * (size_t)code_size;
-    const size_t n_in = 2 * M, n_out = M * RW;  // ints and floats are both 4 bytes
-    DFK_CUDA(h, h->sparse_dev.ensure(n_in + n_out), "[SparseGeometricFactor::linearize] scratch allocation failed");
-    DFK_CUDA(h, h->sparse_host.ensure(n_in + n_out), "[SparseGeometricFactor::linearize] pinned allocation failed");
-    SparsePose sp;
-    set_relative_pose(sp, pose1, pose0, *cam);  // pose10_J_pose1, pose10_J_pose0 (:176-178)
-    float* host = h->sparse_host.ptr;
-    memcpy(host, points_xy, 2 * M * sizeof(int));
-    float codes[256] = {0};  // code_dev holds 256 floats: code0 at 0, code1 at 128
-    memcpy(codes, code0, sizeof(float) * code_size);
-    memcpy(codes + 128, code1, sizeof(float) * code_size);
-    int* d_points = reinterpret_cast<int*>(h->sparse_dev.ptr);
-    float* d_rows = h->sparse_dev.ptr + n_in;
-    DFK_CUDA(h, cudaMemcpyAsync(h->code_dev.ptr, codes, sizeof(codes), cudaMemcpyHostToDevice, h->stream),
-             "[SparseGeometricFactor::linearize] code upload failed");
-    DFK_CUDA(h, cudaMemcpyAsync(d_points, host, n_in * sizeof(float), cudaMemcpyHostToDevice, h->stream),
-             "[SparseGeometricFactor::linearize] point upload failed");
-    DFK_CUDA(h, launch_sparse_geometric_rows(sp, cam->width, cam->height, h->code_dev.ptr, h->code_dev.ptr + 128, code_size,
-                                             view_of(prx0_orig), view_of(prx0_jac), view_of(prx1_orig), view_of(prx1_jac),
-                                             view_of(dpt_grad1), (int)W, (int)H, num_points, d_points, huber_delta,
-                                             h->params.sfmparams.avg_dpt, d_rows, h->stream),
+    Staged st;
+    DFK_TRY(stage(h, "[SparseGeometricFactor::linearize] ", false, &it, 1, code_size, M * RW * sizeof(float),
+                  h->sparse_host, h->sparse_dev, &st));
+    float* d_rows = reinterpret_cast<float*>(h->sparse_dev.ptr + st.bytes);
+    DFK_CUDA(h, launch_sparse_geometric_rows(code_size, *reinterpret_cast<const GeoItemDev*>(h->sparse_host.ptr),
+                                             reinterpret_cast<const int2*>(st.payload), h->params.sfmparams.avg_dpt,
+                                             d_rows, h->stream),
              "[SparseGeometricFactor::linearize] kernel launch failed");
     h->launches += 1;
-    DFK_TRY(download(h, host + n_in, d_rows, n_out * sizeof(float), "[SparseGeometricFactor::linearize] result download failed",
+    float* out = reinterpret_cast<float*>(h->sparse_host.ptr + st.bytes);
+    DFK_TRY(download(h, out, d_rows, M * RW * sizeof(float), "[SparseGeometricFactor::linearize] result download failed",
                      "[SparseGeometricFactor::linearize] kernel launch failed"));
-    memcpy(rows, host + n_in, n_out * sizeof(float));
-    if (num_valid) {
-      int nv = 0;
-      for (size_t i = 0; i < M; ++i) {
-        const float* r = rows + i * RW;
-        bool any = false;
-        for (size_t k = 0; k < RW && !any; ++k) any = r[k] != 0.0f;
-        nv += any ? 1 : 0;
-      }
-      *num_valid = nv;
-    }
+    memcpy(rows, out, M * RW * sizeof(float));
+    int nv = 0;  // rows that are not all zero
+    for (size_t i = 0; i < M; ++i) nv += std::any_of(out + i * RW, out + (i + 1) * RW, [](float v) { return v != 0.0f; });
+    if (num_valid) *num_valid = nv;
     return DFK_OK;
   });
 }
@@ -1636,66 +1672,13 @@ DfkStatus dfk_sparse_geometric_linearize_batch(DfkHandle h, const DfkSparseGeome
   return guarded(h, [&] {
     if (!items || n < 1 || !records_dev)
       return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::linearize batch] null argument / empty batch");
-    if (!sparse_supported(code_size))
-      return fail(h, DFK_ERR_UNSUPPORTED,
-                  "[SparseGeometricFactor::linearize batch] code size not instantiated: " + std::to_string(code_size));
-    size_t total = 0;  // points of the whole batch
-    for (int i = 0; i < n; ++i) {
-      const DfkSparseGeometricItem& it = items[i];
-      const std::string at = "[SparseGeometricFactor::linearize batch] item " + std::to_string(i) + ": ";
-      if (!it.code0 || !it.code1 || !it.points_xy) return fail(h, DFK_ERR_INVALID_ARG, at + "null argument");
-      if (it.num_points < 1 || !(it.huber_delta > 0.0f))
-        return fail(h, DFK_ERR_INVALID_ARG, at + "no points / non-positive huber delta");
-      const uint32_t W = it.prx0_orig.width, H = it.prx0_orig.height;
-      if (W == 0 || H == 0 || !img_ok(&it.prx0_orig, W, H, 1) || !img_ok(&it.prx0_jac, W, H, code_size) ||
-          !img_ok(&it.prx1_orig, W, H, 1) || !img_ok(&it.prx1_jac, W, H, code_size) || !img_ok(&it.dpt_grad1, W, H, 2))
-        return fail(h, DFK_ERR_INVALID_ARG, at + "inconsistent image views");
-      if (!cam_ok(&it.cam, W, H)) return fail(h, DFK_ERR_INVALID_ARG, at + "camera larger than the image views");
-      total += (size_t)it.num_points;
-    }
-    if (total > (size_t)INT32_MAX)
-      return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::linearize batch] more than 2^31 - 1 points in one call");
     DeviceGuard guard(h->device);
-    // one upload: [descriptors n | codes n x 2C (code0, code1) | points 2 total]
-    const size_t desc_bytes = (sizeof(GeoItemDev) * (size_t)n + 15) & ~(size_t)15;
-    const size_t code_bytes = sizeof(float) * 2 * (size_t)n * code_size;
-    const size_t point_bytes = sizeof(int32_t) * 2 * total;
-    const size_t bytes = desc_bytes + code_bytes + point_bytes;
-    DFK_CUDA(h, h->geo_dev.ensure(bytes), "[SparseGeometricFactor::linearize batch] scratch allocation failed");
-    h->geo_host.assign(bytes, 0);
-    GeoItemDev* descs = reinterpret_cast<GeoItemDev*>(h->geo_host.data());
-    float* codes = reinterpret_cast<float*>(h->geo_host.data() + desc_bytes);
-    int32_t* points = reinterpret_cast<int32_t*>(h->geo_host.data() + desc_bytes + code_bytes);
-    const float* codes_dev = reinterpret_cast<const float*>(h->geo_dev.ptr + desc_bytes);
-    const int* points_dev = reinterpret_cast<const int*>(h->geo_dev.ptr + desc_bytes + code_bytes);
-    size_t begin = 0;
-    for (int i = 0; i < n; ++i) {
-      const DfkSparseGeometricItem& it = items[i];
-      GeoItemDev& d = descs[i];
-      set_relative_pose(d.sp, it.pose1, it.pose0, it.cam);  // as dfk_sparse_geometric_linearize
-      d.prx0 = view_of(&it.prx0_orig);
-      d.jac0 = view_of(&it.prx0_jac);
-      d.prx1 = view_of(&it.prx1_orig);
-      d.jac1 = view_of(&it.prx1_jac);
-      d.grad1 = view_of(&it.dpt_grad1);
-      d.code0 = codes_dev + 2 * (size_t)i * code_size;
-      d.code1 = d.code0 + code_size;
-      d.cam_w = it.cam.width;
-      d.cam_h = it.cam.height;
-      d.width = (int)it.prx0_orig.width;
-      d.height = (int)it.prx0_orig.height;
-      d.num_points = it.num_points;
-      d.point_begin = (int)begin;
-      d.huber_delta = it.huber_delta;
-      memcpy(codes + 2 * (size_t)i * code_size, it.code0, sizeof(float) * code_size);
-      memcpy(codes + (2 * (size_t)i + 1) * code_size, it.code1, sizeof(float) * code_size);
-      memcpy(points + 2 * begin, it.points_xy, sizeof(int32_t) * 2 * it.num_points);
-      begin += (size_t)it.num_points;
-    }
-    DFK_CUDA(h, cudaMemcpyAsync(h->geo_dev.ptr, h->geo_host.data(), bytes, cudaMemcpyHostToDevice, h->stream),
-             "[SparseGeometricFactor::linearize batch] upload failed");
+    Staged st;
+    DFK_TRY(stage(h, "[SparseGeometricFactor::linearize batch] ", true, items, n, code_size, 0, h->geo_host, h->geo_dev,
+                  &st));
     DFK_CUDA(h, launch_sparse_geometric_records(code_size, reinterpret_cast<const GeoItemDev*>(h->geo_dev.ptr), n,
-                                                points_dev, h->params.sfmparams.avg_dpt, records_dev, h->stream),
+                                                reinterpret_cast<const int2*>(st.payload), h->params.sfmparams.avg_dpt,
+                                                records_dev, h->stream),
              "[SparseGeometricFactor::linearize batch] kernel launch failed");
     h->launches += 1;
     return DFK_OK;

@@ -184,19 +184,16 @@ cudaError_t launch_depth_step(const float* code_dev, int code_size, int width, i
                               View jac, float avg_dpt, float* scratch /*blocks * depth_partial_floats*/,
                               unsigned int* counter, float* out_dev /*C(C+1)/2 + C + 2*/, int blocks, cudaStream_t s);
 
-// dfk_sparse.cu : ReprojectionFactor::linearize rows (and records), SparseGeometricFactor::linearize rows
+// dfk_sparse.cu : ReprojectionFactor::linearize and SparseGeometricFactor::linearize, rows (one factor) and records (a
+// batch); the single call runs the batch's descriptor for one item
 bool sparse_supported(int code_size);
 struct SparsePose {
   float q[4], t[3], R[9];      // pose_10 = pose1^-1 * pose0
   float P0[36], P1[36];        // pose10_J_pose0 / pose10_J_pose1, row-major 6x6
   float fx, fy, u0, v0;
 };
-cudaError_t launch_reprojection_rows(const SparsePose& sp, const float* code_dev, int code_size, View prx_orig, View jac,
-                                     int width, int height, int num_matches, const float* query_dev, const float* train_dev,
-                                     float cauchy_delta, float sigma, float avg_dpt, float* rows_dev, float* err2_dev,
-                                     cudaStream_t s);
-// One factor of dfk_reprojection_linearize_batch: what launch_reprojection_rows takes for it.  Its matches are
-// query / train[match_begin, + num_matches); code points at its code_size floats in device scratch.
+// One ReprojectionFactor.  Its matches are query / train[match_begin, + num_matches); code points at its code_size floats
+// in device scratch.
 struct ReprojItemDev {
   SparsePose sp;
   View prx_orig, jac;
@@ -205,16 +202,15 @@ struct ReprojItemDev {
   int num_matches, match_begin;
   float cauchy_delta, sigma;
 };
+// rows_dev: 2 num_matches rows of 13 + code_size floats; err2_dev: num_matches squared errors
+cudaError_t launch_reprojection_rows(int code_size, const ReprojItemDev& item, const float2* query_dev,
+                                     const float2* train_dev, float avg_dpt, float* rows_dev, float* err2_dev, cudaStream_t s);
 // one CTA per item; records_dev: num_items records of DFK_SFM_RECORD_FLOATS(code_size) floats
-cudaError_t launch_reprojection_records(int code_size, const ReprojItemDev* items_dev, int num_items, const float* query_dev,
-                                        const float* train_dev, float avg_dpt, float* records_dev, cudaStream_t s);
+cudaError_t launch_reprojection_records(int code_size, const ReprojItemDev* items_dev, int num_items, const float2* query_dev,
+                                        const float2* train_dev, float avg_dpt, float* records_dev, cudaStream_t s);
 
-cudaError_t launch_sparse_geometric_rows(const SparsePose& sp, float cam_w, float cam_h, const float* code0_dev,
-                                         const float* code1_dev, int code_size, View prx0, View jac0, View prx1, View jac1,
-                                         View grad1, int width, int height, int num_points, const int* points_dev,
-                                         float huber_delta, float avg_dpt, float* rows_dev, cudaStream_t s);
-// One factor of dfk_sparse_geometric_linearize_batch: what launch_sparse_geometric_rows takes for it.  Its points are
-// points[point_begin, + num_points); code0 / code1 point at its code_size floats each in device scratch.
+// One SparseGeometricFactor.  Its points are points[point_begin, + num_points); code0 / code1 point at its code_size
+// floats each in device scratch.
 struct GeoItemDev {
   SparsePose sp;
   View prx0, jac0, prx1, jac1, grad1;
@@ -225,8 +221,11 @@ struct GeoItemDev {
   int num_points, point_begin;
   float huber_delta;
 };
+// rows_dev: num_points rows of 13 + 2 code_size floats
+cudaError_t launch_sparse_geometric_rows(int code_size, const GeoItemDev& item, const int2* points_dev, float avg_dpt,
+                                         float* rows_dev, cudaStream_t s);
 // grid (num_items, 1 or 4 entry slices); records_dev: num_items records of DFK_GEO_RECORD_FLOATS(code_size) floats
-cudaError_t launch_sparse_geometric_records(int code_size, const GeoItemDev* items_dev, int num_items, const int* points_dev,
+cudaError_t launch_sparse_geometric_records(int code_size, const GeoItemDev* items_dev, int num_items, const int2* points_dev,
                                             float avg_dpt, float* records_dev, cudaStream_t s);
 
 constexpr int kSimpleMaxBlocks = 1024;

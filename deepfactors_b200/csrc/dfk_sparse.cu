@@ -22,6 +22,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "dfk_geom.cuh"
 #include "dfk_internal.h"
 
@@ -29,16 +31,20 @@ namespace dfk {
 
 namespace {
 
-// The per-match body of ReprojectionFactor::linearize: writes match i's two rows r0, r1 (zero when the correspondence is
-// invalid) and its squared unweighted error; returns whether the correspondence is valid.  Shared by the single-factor
-// kernel and the batched one, so the batched rows are those of dfk_reprojection_linearize by construction.
+// The per-match body of ReprojectionFactor::linearize: writes the two rows r0, r1 of factor `it`'s match (q, tr) (zero
+// when the correspondence is invalid) and its squared unweighted error; returns whether the correspondence is valid.
+// Shared by the single-factor kernel and the batched one, so the batched rows are those of dfk_reprojection_linearize by
+// construction.
 template <int C>
-__device__ __forceinline__ bool reprojection_match_rows(const SparsePose& sp, const float* __restrict__ code, View prx_orig,
-                                                        View jac, int width, int height, float2 q, float2 tr,
-                                                        float cauchy_delta, float sigma, float avg_dpt, float* r0, float* r1,
-                                                        float* err2)
+__device__ __forceinline__ bool reprojection_match_rows(const ReprojItemDev& it, float2 q, float2 tr, float avg_dpt,
+                                                        float* r0, float* r1, float* err2)
 {
   constexpr int RW = 13 + C;
+  const SparsePose& sp = it.sp;
+  const float* __restrict__ code = it.code;
+  const View prx_orig = it.prx_orig, jac = it.jac;
+  const int width = it.width, height = it.height;
+  const float cauchy_delta = it.cauchy_delta, sigma = it.sigma;
   const int xi = (int)q.x, yi = (int)q.y;
   bool valid = xi >= 0 && yi >= 0 && xi < width && yi < height;  // the reference would read out of bounds
   float dpt0 = 0.f, X = 0.f, Y = 0.f, Z = 0.f, px = 0.f, py = 0.f, pz = 0.f, xn = 0.f, yn = 0.f;
@@ -107,20 +113,20 @@ __device__ __forceinline__ bool reprojection_match_rows(const SparsePose& sp, co
   return true;
 }
 
+// One thread per match of the single factor `it`: rows 2m and 2m + 1, err2[m].
 template <int C>
 __global__ void __launch_bounds__(128)
-reprojection_rows_kernel(SparsePose sp, const float* __restrict__ code, View prx_orig, View jac, int width, int height,
-                         int num_matches, const float2* __restrict__ query, const float2* __restrict__ train,
-                         float cauchy_delta, float sigma, float avg_dpt, float* __restrict__ rows, float* __restrict__ err2)
+reprojection_rows_kernel(const __grid_constant__ ReprojItemDev it, const float2* __restrict__ query,
+                         const float2* __restrict__ train, float avg_dpt, float* __restrict__ rows, float* __restrict__ err2)
 {
   constexpr int RW = 13 + C;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= num_matches) return;
-  float* r0 = rows + (size_t)(2 * i) * RW;
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= it.num_matches) return;
+  const int i = it.match_begin + m;
+  float* r0 = rows + (size_t)(2 * m) * RW;
   float e2;
-  reprojection_match_rows<C>(sp, code, prx_orig, jac, width, height, query[i], train[i], cauchy_delta, sigma, avg_dpt, r0,
-                             r0 + RW, &e2);
-  err2[i] = e2;
+  reprojection_match_rows<C>(it, query[i], train[i], avg_dpt, r0, r0 + RW, &e2);
+  err2[m] = e2;
 }
 
 // Geometry of a batched records kernel: rows of RW floats, RPI rows per item (2 per reprojection match, 1 per geometric
@@ -222,8 +228,7 @@ reprojection_records_kernel(const ReprojItemDev* __restrict__ items, const float
   gram_records<RepCfg<C>>(it.num_matches, records, [&](int m, float* r0) {
     const int i = it.match_begin + m;
     float e2;
-    return reprojection_match_rows<C>(it.sp, it.code, it.prx_orig, it.jac, it.width, it.height, query[i], train[i],
-                                      it.cauchy_delta, it.sigma, avg_dpt, r0, r0 + 13 + C, &e2);
+    return reprojection_match_rows<C>(it, query[i], train[i], avg_dpt, r0, r0 + 13 + C, &e2);
   });
 }
 
@@ -243,16 +248,20 @@ reprojection_records_kernel(const ReprojItemDev* __restrict__ items, const float
 // The decode and the validity chain use round-to-nearest intrinsics in the reference's operation order (as the dense
 // kernels do), so the set of valid rows and the nearest-neighbour pixels are those of the CPU evaluation.
 //
-// The per-point body: writes the point's row r (zero when the correspondence is invalid) and returns whether it is valid.
-// Shared by the single-factor kernel and the batched one, so the batched rows are those of dfk_sparse_geometric_linearize
-// by construction.
+// The per-point body: writes the row r of factor `it`'s point pt (zero when the correspondence is invalid) and returns
+// whether it is valid.  Shared by the single-factor kernel and the batched one, so the batched rows are those of
+// dfk_sparse_geometric_linearize by construction.
 template <int C>
-__device__ __forceinline__ bool sparse_geometric_point_row(const SparsePose& sp, float cam_w, float cam_h,
-                                                           const float* __restrict__ code0, const float* __restrict__ code1,
-                                                           View prx0, View jac0, View prx1, View jac1, View grad1, int width,
-                                                           int height, int2 pt, float huber_delta, float avg_dpt, float* r)
+__device__ __forceinline__ bool sparse_geometric_point_row(const GeoItemDev& it, int2 pt, float avg_dpt, float* r)
 {
   constexpr int RW = 13 + 2 * C;
+  const SparsePose& sp = it.sp;
+  const float cam_w = it.cam_w, cam_h = it.cam_h;
+  const float* __restrict__ code0 = it.code0;
+  const float* __restrict__ code1 = it.code1;
+  const View prx0 = it.prx0, jac0 = it.jac0, prx1 = it.prx1, jac1 = it.jac1, grad1 = it.grad1;
+  const int width = it.width, height = it.height;
+  const float huber_delta = it.huber_delta;
   bool valid = pt.x >= 0 && pt.y >= 0 && pt.x < width && pt.y < height;  // the reference would read out of bounds
   Warped w;
   w.valid = false;
@@ -315,17 +324,15 @@ __device__ __forceinline__ bool sparse_geometric_point_row(const SparsePose& sp,
   return true;
 }
 
+// One thread per point of the single factor `it`: row m.
 template <int C>
 __global__ void __launch_bounds__(128)
-sparse_geometric_rows_kernel(SparsePose sp, float cam_w, float cam_h, const float* __restrict__ code0,
-                             const float* __restrict__ code1, View prx0, View jac0, View prx1, View jac1, View grad1, int width,
-                             int height, int num_points, const int2* __restrict__ points, float huber_delta, float avg_dpt,
+sparse_geometric_rows_kernel(const __grid_constant__ GeoItemDev it, const int2* __restrict__ points, float avg_dpt,
                              float* __restrict__ rows)
 {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= num_points) return;
-  sparse_geometric_point_row<C>(sp, cam_w, cam_h, code0, code1, prx0, jac0, prx1, jac1, grad1, width, height, points[i],
-                                huber_delta, avg_dpt, rows + (size_t)i * (13 + 2 * C));
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= it.num_points) return;
+  sparse_geometric_point_row<C>(it, points[it.point_begin + m], avg_dpt, rows + (size_t)m * (13 + 2 * C));
 }
 
 // Factor blockIdx.x, entry slice blockIdx.y (GeoCfg<C>::NS CTAs per factor), one row per point.
@@ -337,118 +344,77 @@ sparse_geometric_records_kernel(const GeoItemDev* __restrict__ items, const int2
   __shared__ GeoItemDev it;
   load_item<GeoCfg<C>::NT>(items + blockIdx.x, it);
   gram_records<GeoCfg<C>>(it.num_points, records, [&](int m, float* r) {
-    return sparse_geometric_point_row<C>(it.sp, it.cam_w, it.cam_h, it.code0, it.code1, it.prx0, it.jac0, it.prx1, it.jac1,
-                                         it.grad1, it.width, it.height, points[it.point_begin + m], it.huber_delta, avg_dpt,
-                                         r);
+    return sparse_geometric_point_row<C>(it, points[it.point_begin + m], avg_dpt, r);
   });
+}
+
+// Calls f(std::integral_constant<int, C>{}) for the code sizes the sparse kernels are instantiated for.
+template <class F>
+cudaError_t with_sparse_code_size(int code_size, F&& f)
+{
+  switch (code_size) {
+    case 8: return f(std::integral_constant<int, 8>{});
+    case 16: return f(std::integral_constant<int, 16>{});
+    case 32: return f(std::integral_constant<int, 32>{});
+    case 64: return f(std::integral_constant<int, 64>{});
+    case 128: return f(std::integral_constant<int, 128>{});
+    default: return cudaErrorInvalidValue;
+  }
 }
 
 }  // namespace
 
 bool sparse_supported(int code_size)
 {
-  return code_size == 8 || code_size == 16 || code_size == 32 || code_size == 64 || code_size == 128;
+  return with_sparse_code_size(code_size, [](auto) { return cudaSuccess; }) == cudaSuccess;
 }
 
-cudaError_t launch_reprojection_rows(const SparsePose& sp, const float* code_dev, int code_size, View prx_orig, View jac,
-                                     int width, int height, int num_matches, const float* query_dev, const float* train_dev,
-                                     float cauchy_delta, float sigma, float avg_dpt, float* rows_dev, float* err2_dev,
-                                     cudaStream_t s)
+cudaError_t launch_reprojection_rows(int code_size, const ReprojItemDev& item, const float2* query_dev,
+                                     const float2* train_dev, float avg_dpt, float* rows_dev, float* err2_dev, cudaStream_t s)
 {
-  const int blocks = (num_matches + 127) / 128;
-  const float2* q = reinterpret_cast<const float2*>(query_dev);
-  const float2* t = reinterpret_cast<const float2*>(train_dev);
-#define DFK_SP(CS)                                                                                                      \
-  case CS:                                                                                                              \
-    reprojection_rows_kernel<CS><<<blocks, 128, 0, s>>>(sp, code_dev, prx_orig, jac, width, height, num_matches, q, t,   \
-                                                        cauchy_delta, sigma, avg_dpt, rows_dev, err2_dev);             \
-    break;
-  switch (code_size) {
-    DFK_SP(8)
-    DFK_SP(16)
-    DFK_SP(32)
-    DFK_SP(64)
-    DFK_SP(128)
-    default: return cudaErrorInvalidValue;
-  }
-#undef DFK_SP
-  return cudaGetLastError();
+  return with_sparse_code_size(code_size, [&](auto cs) {
+    reprojection_rows_kernel<cs.value><<<(item.num_matches + 127) / 128, 128, 0, s>>>(item, query_dev, train_dev, avg_dpt,
+                                                                                      rows_dev, err2_dev);
+    return cudaGetLastError();
+  });
 }
 
-cudaError_t launch_reprojection_records(int code_size, const ReprojItemDev* items_dev, int num_items, const float* query_dev,
-                                        const float* train_dev, float avg_dpt, float* records_dev, cudaStream_t s)
+cudaError_t launch_reprojection_records(int code_size, const ReprojItemDev* items_dev, int num_items, const float2* query_dev,
+                                        const float2* train_dev, float avg_dpt, float* records_dev, cudaStream_t s)
 {
-  const float2* q = reinterpret_cast<const float2*>(query_dev);
-  const float2* t = reinterpret_cast<const float2*>(train_dev);
-#define DFK_RR(CS)                                                                                                      \
-  case CS: {                                                                                                            \
-    cudaError_t e = cudaFuncSetAttribute(reprojection_records_kernel<CS>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
-                                         (int)RepCfg<CS>::SMEM);                                                        \
-    if (e != cudaSuccess) return e;                                                                                     \
-    reprojection_records_kernel<CS><<<num_items, RepCfg<CS>::NT, RepCfg<CS>::SMEM, s>>>(items_dev, q, t, avg_dpt,       \
-                                                                                       records_dev);                    \
-    break;                                                                                                              \
-  }
-  switch (code_size) {
-    DFK_RR(8)
-    DFK_RR(16)
-    DFK_RR(32)
-    DFK_RR(64)
-    DFK_RR(128)
-    default: return cudaErrorInvalidValue;
-  }
-#undef DFK_RR
-  return cudaGetLastError();
+  return with_sparse_code_size(code_size, [&](auto cs) {
+    using Cfg = RepCfg<cs.value>;
+    const cudaError_t e = cudaFuncSetAttribute(reprojection_records_kernel<cs.value>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
+    if (e != cudaSuccess) return e;
+    reprojection_records_kernel<cs.value><<<num_items, Cfg::NT, Cfg::SMEM, s>>>(items_dev, query_dev, train_dev, avg_dpt,
+                                                                               records_dev);
+    return cudaGetLastError();
+  });
 }
 
-cudaError_t launch_sparse_geometric_rows(const SparsePose& sp, float cam_w, float cam_h, const float* code0_dev,
-                                         const float* code1_dev, int code_size, View prx0, View jac0, View prx1, View jac1,
-                                         View grad1, int width, int height, int num_points, const int* points_dev,
-                                         float huber_delta, float avg_dpt, float* rows_dev, cudaStream_t s)
+cudaError_t launch_sparse_geometric_rows(int code_size, const GeoItemDev& item, const int2* points_dev, float avg_dpt,
+                                         float* rows_dev, cudaStream_t s)
 {
-  const int blocks = (num_points + 127) / 128;
-  const int2* pts = reinterpret_cast<const int2*>(points_dev);
-#define DFK_SG(CS)                                                                                                        \
-  case CS:                                                                                                                \
-    sparse_geometric_rows_kernel<CS><<<blocks, 128, 0, s>>>(sp, cam_w, cam_h, code0_dev, code1_dev, prx0, jac0, prx1, jac1, \
-                                                            grad1, width, height, num_points, pts, huber_delta, avg_dpt,  \
-                                                            rows_dev);                                                    \
-    break;
-  switch (code_size) {
-    DFK_SG(8)
-    DFK_SG(16)
-    DFK_SG(32)
-    DFK_SG(64)
-    DFK_SG(128)
-    default: return cudaErrorInvalidValue;
-  }
-#undef DFK_SG
-  return cudaGetLastError();
+  return with_sparse_code_size(code_size, [&](auto cs) {
+    sparse_geometric_rows_kernel<cs.value><<<(item.num_points + 127) / 128, 128, 0, s>>>(item, points_dev, avg_dpt,
+                                                                                         rows_dev);
+    return cudaGetLastError();
+  });
 }
 
-cudaError_t launch_sparse_geometric_records(int code_size, const GeoItemDev* items_dev, int num_items, const int* points_dev,
+cudaError_t launch_sparse_geometric_records(int code_size, const GeoItemDev* items_dev, int num_items, const int2* points_dev,
                                             float avg_dpt, float* records_dev, cudaStream_t s)
 {
-  const int2* pts = reinterpret_cast<const int2*>(points_dev);
-#define DFK_GR(CS)                                                                                                      \
-  case CS: {                                                                                                            \
-    cudaError_t e = cudaFuncSetAttribute(sparse_geometric_records_kernel<CS>,                                           \
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GeoCfg<CS>::SMEM);           \
-    if (e != cudaSuccess) return e;                                                                                     \
-    sparse_geometric_records_kernel<CS><<<dim3(num_items, GeoCfg<CS>::NS), GeoCfg<CS>::NT, GeoCfg<CS>::SMEM, s>>>(      \
-        items_dev, pts, avg_dpt, records_dev);                                                                          \
-    break;                                                                                                              \
-  }
-  switch (code_size) {
-    DFK_GR(8)
-    DFK_GR(16)
-    DFK_GR(32)
-    DFK_GR(64)
-    DFK_GR(128)
-    default: return cudaErrorInvalidValue;
-  }
-#undef DFK_GR
-  return cudaGetLastError();
+  return with_sparse_code_size(code_size, [&](auto cs) {
+    using Cfg = GeoCfg<cs.value>;
+    const cudaError_t e = cudaFuncSetAttribute(sparse_geometric_records_kernel<cs.value>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
+    if (e != cudaSuccess) return e;
+    sparse_geometric_records_kernel<cs.value><<<dim3(num_items, Cfg::NS), Cfg::NT, Cfg::SMEM, s>>>(items_dev, points_dev,
+                                                                                                   avg_dpt, records_dev);
+    return cudaGetLastError();
+  });
 }
 
 }  // namespace dfk

@@ -204,11 +204,11 @@ def test_reprojection_and_geometric_batches_back_to_back(torch_mod):
     assert np.array_equal(r2.cpu().numpy(), r_alone[::-1]) and np.array_equal(g2.cpu().numpy(), g_alone[:3])
 
 
-def test_rejected_calls_name_the_item_and_write_nothing(torch_mod):
+def test_rejected_calls_name_the_item_and_write_nothing(torch_mod, monkeypatch):
     import torch
-    from deepfactors_b200 import _lib
+    from deepfactors_b200 import _lib, aligners
     from deepfactors_b200._lib import DfkSparseGeometricItem
-    from deepfactors_b200.aligners import SfmAligner, _cam, _image, _pose
+    from deepfactors_b200.aligners import SfmAligner, SparseGeometricLinearize, _cam, _image, _pose
     cs = 8
     al = SfmAligner(cs)
     lib = _lib.lib()
@@ -268,6 +268,19 @@ def test_rejected_calls_name_the_item_and_write_nothing(torch_mod):
         st = fn()
         assert st == want, (k, st)
         assert words in lib.dfk_last_error(al.handle).decode(), (k, lib.dfk_last_error(al.handle))
+    # the single call checks its arguments as a batch item: a short code would make the C side read past the host
+    # array, so the call is refused before it reaches the linearise entry point
+    class NoLinearize:
+        def __getattr__(self, name):
+            assert "linearize" not in name, name
+            return getattr(lib, name)
+
+    monkeypatch.setattr(aligners, "lib", NoLinearize)
+    single = _args(fs[2])
+    for bad in (dict(code0=single["code0"][:cs - 1]), dict(code1=single["code1"][:cs - 1])):
+        with pytest.raises(ValueError):
+            SparseGeometricLinearize(al, **{**single, **bad})
+    monkeypatch.undo()
     torch.cuda.synchronize()
     assert (rec.cpu().numpy() == SENTINEL).all()
     assert call(items()) == _lib.DFK_OK  # and the handle still works

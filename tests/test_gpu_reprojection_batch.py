@@ -129,11 +129,11 @@ def test_a_factor_record_does_not_depend_on_the_batch(torch_mod, cs):
     assert (b[0] == SENTINEL).all() and (b[-1] == SENTINEL).all()
 
 
-def test_rejected_calls_name_the_item_and_write_nothing(torch_mod):
+def test_rejected_calls_name_the_item_and_write_nothing(torch_mod, monkeypatch):
     import torch
-    from deepfactors_b200 import _lib
+    from deepfactors_b200 import _lib, aligners
     from deepfactors_b200._lib import DfkReprojectionItem
-    from deepfactors_b200.aligners import SfmAligner, _cam, _image, _pose
+    from deepfactors_b200.aligners import ReprojectionLinearize, SfmAligner, _cam, _image, _pose
     cs = 8
     al = SfmAligner(cs)
     lib = _lib.lib()
@@ -186,6 +186,19 @@ def test_rejected_calls_name_the_item_and_write_nothing(torch_mod):
         st = fn()
         assert st == want, (k, st)
         assert words in lib.dfk_last_error(al.handle).decode(), (k, lib.dfk_last_error(al.handle))
+    # the single call checks its arguments as a batch item: a short code, or fewer train than query points, would make
+    # the C side read past the host arrays, so the call is refused before it reaches the linearise entry point
+    class NoLinearize:
+        def __getattr__(self, name):
+            assert "linearize" not in name, name
+            return getattr(lib, name)
+
+    monkeypatch.setattr(aligners, "lib", NoLinearize)
+    single = {k: v for k, v in fs[2].items() if k != "host"}
+    for bad in (dict(code0=single["code0"][:cs - 1]), dict(train_xy=single["train_xy"][:-1])):
+        with pytest.raises(ValueError):
+            ReprojectionLinearize(al, **{**single, **bad})
+    monkeypatch.undo()
     torch.cuda.synchronize()
     assert (rec.cpu().numpy() == SENTINEL).all()
     assert call(items()) == _lib.DFK_OK  # and the handle still works
