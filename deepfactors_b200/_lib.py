@@ -81,6 +81,10 @@ class DfkWindowDesc(C.Structure):
                 ("item_width", C.POINTER(C.c_int32)), ("item_height", C.POINTER(C.c_int32))]
 
 
+class DfkWindowSolveParams(C.Structure):
+    _fields_ = [("lambda_", C.c_double), ("code_prior_weight", C.c_double)]
+
+
 # every symbol include/dfk.h declares: (name, restype, argtypes)
 _F = C.POINTER(C.c_float)
 _IMG = C.POINTER(DfkImage)
@@ -121,6 +125,11 @@ SYMBOLS = {
     "dfk_window_create_geometric": (C.c_int, [_H, C.POINTER(DfkWindowDesc), C.c_int, C.POINTER(C.c_int32),
                                               C.POINTER(C.c_int32), C.POINTER(C.c_void_p)]),
     "dfk_window_assemble_geometric": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dfk_window_solver_create": (C.c_int, [_H, C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_void_p)]),
+    "dfk_window_solver_destroy": (C.c_int, [_H, C.c_void_p]),
+    "dfk_window_solver_tiles": (C.c_int, [_H, C.c_void_p, C.POINTER(C.c_size_t)]),
+    "dfk_window_solve": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.POINTER(DfkWindowSolveParams), C.POINTER(C.c_double),
+                                   C.c_void_p, C.c_void_p]),
     "dfk_se3_run_step": (C.c_int, [_H, _F, _CAM, _IMG, _IMG, _IMG, _IMG, _F, _F, _F, C.POINTER(C.c_uint64)]),
     "dfk_se3_track": (C.c_int, [_H, _F, C.POINTER(DfkTrackLevel), C.c_int, _F, _F, _F, _F, C.c_int]),
     "dfk_se3_track_batch": (C.c_int, [_H, C.c_int, C.c_int, _F, C.POINTER(DfkTrackLevel), _F, _F, _F]),

@@ -497,6 +497,69 @@ class Window:
             pass
 
 
+class WindowSolver:
+    """Damped block-sparse fp64 Cholesky of a Window's normal equations on the device (dfk_window_solve): the system
+    WindowOptimizer solves with to_dense + damped_solve, straight from the packed buffer.  `fixed` lists the window
+    variables k * B + r held at zero (e.g. range(6): the gauge keyframe's pose).  `tiles` is the number of structurally
+    nonzero B x B tiles of the factor, fill included."""
+
+    def __init__(self, window: Window, fixed=()):
+        self._win = window  # keeps the window (and its handle) alive
+        self._al = window._al
+        self.layout = window.layout
+        fx = np.ascontiguousarray([int(v) for v in fixed], dtype=np.int32)
+        self.fixed = tuple(int(v) for v in fx)
+        self.s = C.c_void_p()
+        check(self._al.handle, lib().dfk_window_solver_create(self._al.handle, window.w, len(fx),
+                                                              fx.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(self.s)))
+        tiles = C.c_size_t(0)
+        check(self._al.handle, lib().dfk_window_solver_tiles(self._al.handle, self.s, C.byref(tiles)))
+        self.tiles = int(tiles.value)
+
+    def solve(self, buf: torch.Tensor, lam: float, code_prior_weight: float = 0.0, codes=None,
+              dx: torch.Tensor | None = None, info: torch.Tensor | None = None):
+        """buf: the window buffer (contiguous float32 on the handle's device).  codes: [K, C] (host), required when
+        code_prior_weight > 0.  Returns (dx [K * B] float64, info [1] int32), device tensors written asynchronously on
+        torch's current stream; info = 0, or 1 + the first variable whose pivot was not positive (dx is then zero)."""
+        self._al._hd.use_torch_stream()
+        dev = torch.device(f"cuda:{self._al._hd.device}")
+        n = self.layout.num_keyframes * self.layout.B
+        if not (buf.dtype == torch.float32 and buf.device == dev and buf.is_contiguous()
+                and buf.numel() >= self.layout.floats):
+            raise ValueError(f"buf must be a contiguous float32 tensor of at least {self.layout.floats} floats on {dev}")
+        if dx is None:
+            dx = torch.empty(n, dtype=torch.float64, device=dev)
+        if not (dx.dtype == torch.float64 and dx.device == dev and dx.is_contiguous() and dx.numel() >= n):
+            raise ValueError(f"dx must be a contiguous float64 tensor of at least {n} entries on {dev}")
+        if info is None:
+            info = torch.empty(1, dtype=torch.int32, device=dev)
+        if not (info.dtype == torch.int32 and info.device == dev and info.numel() >= 1):
+            raise ValueError(f"info must be an int32 tensor on {dev}")
+        cp = None
+        if code_prior_weight > 0:
+            if codes is None:
+                raise ValueError("code_prior_weight > 0 needs the codes")
+            c64 = np.ascontiguousarray(codes, dtype=np.float64)
+            if c64.shape != (self.layout.num_keyframes, self.layout.code_size):
+                raise ValueError(f"codes must be [{self.layout.num_keyframes}, {self.layout.code_size}]")
+            cp = c64.ctypes.data_as(C.POINTER(C.c_double))
+        prm = _lib.DfkWindowSolveParams(float(lam), float(code_prior_weight))
+        check(self._al.handle, lib().dfk_window_solve(self._al.handle, self.s, C.c_void_p(buf.data_ptr()), C.byref(prm),
+                                                      cp, C.c_void_p(dx.data_ptr()), C.c_void_p(info.data_ptr())))
+        return dx, info
+
+    def close(self):
+        if getattr(self, "s", None):
+            lib().dfk_window_solver_destroy(self._al.handle, self.s)
+            self.s = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 # ------------------------------------------------------------------------------------------- SE3Aligner
 class SE3Aligner:
     """df::SE3Aligner<float> (sources/cuda/cu_se3aligner.h:38-86)."""

@@ -9,6 +9,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <memory>
 #include <new>
 #include <string>
@@ -160,6 +161,16 @@ struct DfkWindow {
   DeviceBuf<int> ints;
   DeviceBuf<float> areas;
   size_t floats = 0;
+  // host copy of the structure, for dfk_window_solver_create
+  std::vector<int> pair_k0, pair_k1, link_k0, link_k1;
+};
+
+// damped block-sparse Cholesky of one window (dfk_window_solver_create)
+struct DfkWindowSolver {
+  int device = 0;
+  int num_vars = 0, code_size = 0, num_keyframes = 0;
+  WindowSolverDev* dev = nullptr;
+  ~DfkWindowSolver() { window_solver_destroy(dev); }
 };
 
 namespace {
@@ -1342,6 +1353,10 @@ DfkStatus dfk_window_create_geometric(DfkHandle h, const DfkWindowDesc* d, int L
     w->dev.lk1_ptr = ints + o_lk1; w->dev.lk1_links = ints + o_lk1 + K + 1;
     const size_t B = 6 + (size_t)d->code_size;
     w->floats = (size_t)K * (B * B + B) + (size_t)P * 6 * B + 2 + (size_t)L * B * B;
+    w->pair_k0.assign(d->pair_k0, d->pair_k0 + P);
+    w->pair_k1.assign(d->pair_k1, d->pair_k1 + P);
+    w->link_k0.assign(link_k0, link_k0 + L);
+    w->link_k1.assign(link_k1, link_k1 + L);
     *out = w.release();
     return DFK_OK;
   });
@@ -1383,6 +1398,78 @@ DfkStatus dfk_window_assemble_geometric(DfkHandle h, const DfkWindow* w, const f
     DFK_CUDA(h, launch_window_assemble(w->dev, records_dev, geo_records_dev, window_dev, h->stream),
              "[Window] kernel launch failed");
     h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_solver_create(DfkHandle h, const DfkWindow* w, int num_fixed, const int32_t* fixed_vars,
+                                   DfkWindowSolver** out)
+{
+  return guarded(h, [&] {
+    if (!w || !out || num_fixed < 0 || (num_fixed > 0 && !fixed_vars))
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] null argument");
+    *out = nullptr;
+    if (w->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] window and handle live on different devices");
+    const int K = w->dev.num_keyframes, C = w->dev.code_size, n = K * (6 + C);
+    std::vector<int> fixed(fixed_vars, fixed_vars + num_fixed);
+    std::vector<char> seen(n, 0);
+    for (int q = 0; q < num_fixed; ++q) {
+      if (fixed[q] < 0 || fixed[q] >= n)
+        return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] fixed variable " + std::to_string(fixed[q]) +
+                                                " outside the window's " + std::to_string(n) + " variables");
+      if (seen[fixed[q]]++)
+        return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] fixed variable " + std::to_string(fixed[q]) + " listed twice");
+    }
+    DeviceGuard guard(h->device);
+    std::unique_ptr<DfkWindowSolver> s(new (std::nothrow) DfkWindowSolver());
+    if (!s) return oom(h);
+    s->device = h->device;
+    s->num_vars = n; s->code_size = C; s->num_keyframes = K;
+    DFK_CUDA(h, window_solver_create(K, C, w->pair_k0, w->pair_k1, w->link_k0, w->link_k1, fixed, &s->dev),
+             "[WindowSolver] workspace allocation failed");
+    *out = s.release();
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_solver_destroy(DfkHandle h, DfkWindowSolver* s)
+{
+  return guarded(h, [&] {
+    if (!s) return DFK_OK;
+    DeviceGuard guard(s->device);
+    delete s;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_solver_tiles(DfkHandle h, const DfkWindowSolver* s, size_t* tiles)
+{
+  return guarded(h, [&] {
+    if (!s || !tiles) return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] null argument");
+    *tiles = window_solver_tiles(s->dev);
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_solve(DfkHandle h, const DfkWindowSolver* s, const float* window_dev, const DfkWindowSolveParams* p,
+                           const double* codes, double* dx_dev, int32_t* info_dev)
+{
+  return guarded(h, [&] {
+    if (!s || !window_dev || !p || !dx_dev || !info_dev)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] null argument");
+    if (s->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] solver and handle live on different devices");
+    if (!(std::isfinite(p->lambda) && p->lambda >= 0.0))
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] lambda must be finite and >= 0");
+    if (!(std::isfinite(p->code_prior_weight) && p->code_prior_weight >= 0.0))
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] code_prior_weight must be finite and >= 0");
+    if (p->code_prior_weight > 0.0 && !codes)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] code_prior_weight > 0 needs the codes");
+    DeviceGuard guard(h->device);
+    DFK_CUDA(h, launch_window_solve(s->dev, window_dev, p->lambda, p->code_prior_weight, codes, dx_dev, info_dev,
+                                    h->stream, &h->launches),
+             "[WindowSolver] kernel launch failed");
     return DFK_OK;
   });
 }

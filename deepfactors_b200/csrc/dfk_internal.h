@@ -177,6 +177,21 @@ struct WindowDev {
 cudaError_t launch_window_assemble(const WindowDev& w, const float* records_dev, const float* geo_records_dev,
                                    float* out_dev, cudaStream_t stream);
 
+// dfk_window_solve.cu : damped block-sparse fp64 Cholesky of a window buffer.  The symbolic analysis and the workspace
+// (cudaMalloc, on the current device) belong to the solver; a solve allocates nothing.
+struct WindowSolverDev;
+// pairs / links: the window's keyframe lists; fixed_vars: distinct variable indices in [0, K (6 + C))
+cudaError_t window_solver_create(int num_keyframes, int code_size, const std::vector<int>& pair_k0,
+                                 const std::vector<int>& pair_k1, const std::vector<int>& link_k0,
+                                 const std::vector<int>& link_k1, const std::vector<int>& fixed_vars,
+                                 WindowSolverDev** out);
+void window_solver_destroy(WindowSolverDev* s);
+size_t window_solver_tiles(const WindowSolverDev* s);
+// codes_host: K * C doubles, read only when prior > 0; *launches += the kernels enqueued
+cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_dev, double lambda, double prior,
+                                const double* codes_host, double* dx_dev, int32_t* info_dev, cudaStream_t stream,
+                                uint64_t* launches);
+
 // dfk_depth.cu : DepthAligner::RunStep
 bool depth_supported(int code_size);
 size_t depth_partial_floats(int code_size);

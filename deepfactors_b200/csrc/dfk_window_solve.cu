@@ -1,0 +1,553 @@
+// dfk_window_solve.cu -- damped block-sparse fp64 Cholesky of a keyframe window's normal equations, straight from the
+// packed buffer of dfk_window_assemble[_geometric] (layout: include/dfk.h).
+//
+// The system is the one WindowOptimizer solves on torch (window_opt.py: WindowBlocks.to_dense, _system, damped_solve):
+// fp32 entries promoted to fp64 and summed in to_dense's order, the code prior w I / -w code, the fixed variables as
+// identity rows with a zero right-hand side, and lambda d + 1e-12 max|d| on the diagonal of the kept variables.
+//
+// Unit of sparsity: the B x B tile of a pair of keyframes (B = 6 + C).  The symbolic analysis (host, at create) marks the
+// lower tiles a pair or link touches and the fill of eliminating keyframes in index order, and stores them column by
+// column (tile 0 of a column is its diagonal tile).  One solve is, on the handle's stream:
+//   load           one launch, one CTA per tile: the tile's blocks summed in to_dense's order (+ prior, fixed rows,
+//                  damping; the diagonal CTAs also write the right-hand side)
+//   per column j   panel:  one CTA per nonzero tile (i, j).  Each refactors the diagonal tile in shared memory (its own
+//                          copy: no CTA waits for another), then solves X L_jj^T = A_ij in place; the diagonal CTA writes
+//                          L_jj to a slot of its own and y_j = L_jj^-1 g_j over g_j.
+//                  update: one CTA per target tile (i, k), j < k <= i, with (i, j) and (k, j) nonzero: A_ik -= L_ij L_kj^T
+//                          (DFMA, 16 x 16 threads with an M x M register tile each); a diagonal target also does
+//                          g_i -= L_ij y_j.
+//   per row j, descending   backward: one CTA per nonzero tile (j, i), i <= j.  Each solves L_jj^T x_j = y_j in shared
+//                          memory (again its own copy); the diagonal CTA writes dx_j, the others y_i -= L_ji^T x_j.
+// Every tile and every rhs block receives at most one update per launch and its updates in column order, every sum runs
+// in a fixed order and there are no atomics, so two solves of the same buffer are bit for bit equal.  Ordering comes from
+// stream order only: no CTA ever waits for another.
+#include <cuda_runtime.h>
+#include <math.h>
+#include <stdint.h>
+
+#include <algorithm>
+#include <memory>
+#include <set>
+#include <type_traits>
+#include <vector>
+
+#include "dfk_internal.h"
+
+namespace dfk {
+
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kSmemMax = 227 * 1024;  // opt-in dynamic shared memory per CTA on sm_90
+
+// contribution of one buffer block to a tile, in to_dense's order: kind in the low two bits
+enum : int { CONTRIB_PAIR = 0, CONTRIB_PAIR_T = 1, CONTRIB_LINK = 2, CONTRIB_LINK_T = 3 };
+
+struct SolveArgs {
+  const float* buf;
+  const double* codes;  // K * C, or null without prior
+  double* tiles;        // (num_tiles + K) tiles of B * B, row-major; slot num_tiles + j holds L_jj
+  double* rhs;          // K * B: g, then y, then (consumed) during the backward pass
+  double* dx;
+  int32_t* info;
+  const int* tile_row;
+  const int* tile_col;
+  const int* contrib_ptr;  // [num_tiles + 1]
+  const int* contrib;
+  const int* diag_tile;    // [K]
+  const unsigned char* fixed;  // [K * B]
+  int K, P;
+  int num_tiles;
+  double lambda, prior;
+};
+
+__device__ __forceinline__ size_t tile_off(int t, int B) { return (size_t)t * B * B; }
+
+// ------------------------------------------------------------------------------------------------------------- load
+// Value of H(row r of keyframe i, column c of keyframe j) before prior / damping: the diagonal block, then every
+// contribution in list order (to_dense: pairs in order, each one's block then its transpose, then links in order).
+template <int B>
+__device__ double tile_entry(const SolveArgs& a, int t, int r, int c)
+{
+  const size_t o_c = (size_t)a.K * (B * B + B), o_l = o_c + (size_t)a.P * B * 6 + 2;
+  const bool diag = a.tile_row[t] == a.tile_col[t];
+  double s = diag ? (double)a.buf[(size_t)a.tile_row[t] * B * B + r * B + c] : 0.0;
+  for (int q = a.contrib_ptr[t]; q < a.contrib_ptr[t + 1]; ++q) {
+    const int e = a.contrib[q], kind = e & 3, idx = e >> 2;
+    if (kind == CONTRIB_PAIR) {
+      if (c < 6) s += (double)a.buf[o_c + (size_t)idx * B * 6 + r * 6 + c];
+    } else if (kind == CONTRIB_PAIR_T) {
+      if (r < 6) s += (double)a.buf[o_c + (size_t)idx * B * 6 + c * 6 + r];
+    } else if (kind == CONTRIB_LINK) {
+      s += (double)a.buf[o_l + (size_t)idx * B * B + r * B + c];
+    } else {
+      s += (double)a.buf[o_l + (size_t)idx * B * B + c * B + r];
+    }
+  }
+  return s;
+}
+
+// diagonal entry (after the prior) of variable r of keyframe k
+template <int B>
+__device__ double diag_entry(const SolveArgs& a, int k, int r)
+{
+  double h = tile_entry<B>(a, a.diag_tile[k], r, r);
+  if (a.prior > 0.0 && r >= 6) h = __dadd_rn(h, a.prior);
+  return h;
+}
+
+template <int B>
+__global__ void __launch_bounds__(kThreads) window_solve_load_kernel(SolveArgs a)
+{
+  const int t = blockIdx.x;
+  const int i = a.tile_row[t], j = a.tile_col[t];
+  double* T = a.tiles + tile_off(t, B);
+  if (i != j) {
+    for (int e = threadIdx.x; e < B * B; e += blockDim.x) {
+      const int r = e / B, c = e - r * B;
+      const bool fx = a.fixed[i * B + r] | a.fixed[j * B + c];
+      T[e] = fx ? 0.0 : tile_entry<B>(a, t, r, c);
+    }
+    return;
+  }
+  // diagonal tile: max |d| over the kept variables of the whole window (every diagonal CTA computes it, max is exact)
+  __shared__ double red[kThreads / 32];
+  double m = 0.0;
+  for (int v = threadIdx.x; v < a.K * B; v += blockDim.x)
+    if (!a.fixed[v]) m = fmax(m, fabs(diag_entry<B>(a, v / B, v % B)));
+  for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = 0.0;
+  for (int w = 0; w < kThreads / 32; ++w) m = fmax(m, red[w]);
+  const double eps = __dmul_rn(1e-12, m);
+  for (int e = threadIdx.x; e < B * B; e += blockDim.x) {
+    const int r = e / B, c = e - r * B;
+    const bool fx = a.fixed[i * B + r] | a.fixed[i * B + c];
+    double h;
+    if (fx) {
+      h = r == c ? 1.0 : 0.0;
+    } else {
+      h = tile_entry<B>(a, t, r, c);
+      if (r == c) {
+        if (a.prior > 0.0 && r >= 6) h = __dadd_rn(h, a.prior);
+        h = __dadd_rn(h, __dadd_rn(__dmul_rn(a.lambda, h), eps));  // damped_solve: H + diag(lam d + 1e-12 max|d|)
+      }
+    }
+    T[e] = h;
+  }
+  for (int r = threadIdx.x; r < B; r += blockDim.x) {
+    double g = (double)a.buf[(size_t)a.K * B * B + (size_t)i * B + r];
+    if (a.prior > 0.0 && r >= 6) g = __dsub_rn(g, __dmul_rn(a.prior, a.codes[(size_t)i * (B - 6) + r - 6]));
+    a.rhs[(size_t)i * B + r] = a.fixed[i * B + r] ? 0.0 : g;
+  }
+  if (t == 0 && threadIdx.x == 0) *a.info = 0;
+}
+
+// ------------------------------------------------------------------------------------------------------------ panel
+// Rows of the TRSM that fit in shared memory next to L_jj (the whole tile for B <= 118, two passes at B = 134)
+template <int B>
+struct PanelCfg {
+  static constexpr int kRows = (kSmemMax - (B * B + B) * 8) / (B * 8) < B ? (kSmemMax - (B * B + B) * 8) / (B * 8) : B;
+  static constexpr int kSmem = (B * B + B + kRows * B) * 8;
+};
+
+// Cholesky of the lower triangle of L (row-major B x B, shared) in place; dg[c] = L_cc.  Returns the first column whose
+// pivot is not positive and finite, or -1.  Right-looking, two barriers per column.
+template <int B>
+__device__ int chol_shared(double* L, double* dg)
+{
+  int bad = -1;
+  for (int c = 0; c < B; ++c) {
+    const double p = L[c * B + c];
+    if (bad < 0 && !(p > 0.0 && p <= 1.7976931348623157e308)) bad = c;
+    const double d = sqrt(p);
+    for (int r = c + 1 + threadIdx.x; r < B; r += blockDim.x) L[r * B + c] = __ddiv_rn(L[r * B + c], d);
+    if (threadIdx.x == 0) dg[c] = d;
+    __syncthreads();
+    const int n = B - 1 - c;  // trailing rows c+1 .. B-1, lower triangle
+    for (int e = threadIdx.x; e < n * n; e += blockDim.x) {
+      const int r = c + 1 + e / n, m = c + 1 + e % n;
+      if (m <= r) L[r * B + m] = __fma_rn(-L[r * B + c], L[m * B + c], L[r * B + m]);
+    }
+    __syncthreads();
+  }
+  return bad;
+}
+
+// X L^T = X0 for `rows` rows of X (row-major, stride B, shared): forward substitution, two barriers per column
+template <int B>
+__device__ void trsm_rows(double* X, int rows, const double* L, const double* dg)
+{
+  for (int c = 0; c < B; ++c) {
+    for (int r = threadIdx.x; r < rows; r += blockDim.x) X[r * B + c] = __ddiv_rn(X[r * B + c], dg[c]);
+    __syncthreads();
+    const int n = B - 1 - c;
+    for (int e = threadIdx.x; e < rows * n; e += blockDim.x) {
+      const int r = e / n, m = c + 1 + e % n;
+      X[r * B + m] = __fma_rn(-X[r * B + c], L[m * B + c], X[r * B + m]);
+    }
+    __syncthreads();
+  }
+}
+
+template <int B>
+__global__ void __launch_bounds__(kThreads) window_solve_panel_kernel(SolveArgs a, int j, int col_begin)
+{
+  extern __shared__ double sm[];
+  double* L = sm;
+  double* dg = L + B * B;
+  double* X = dg + B;
+  const int t = col_begin + blockIdx.x;
+  const double* A = a.tiles + tile_off(col_begin, B);
+  for (int e = threadIdx.x; e < B * B; e += blockDim.x) L[e] = A[e];
+  __syncthreads();
+  const int bad = chol_shared<B>(L, dg);
+  if (t == col_begin) {
+    // diagonal: L_jj to its slot, y_j = L_jj^-1 g_j over g_j
+    double* Lj = a.tiles + tile_off(a.num_tiles + j, B);
+    for (int e = threadIdx.x; e < B * B; e += blockDim.x) {
+      const int r = e / B, c = e - r * B;
+      Lj[e] = c < r ? L[e] : (c == r ? dg[r] : 0.0);
+    }
+    double* g = a.rhs + (size_t)j * B;
+    for (int e = threadIdx.x; e < B; e += blockDim.x) X[e] = g[e];
+    __syncthreads();
+    trsm_rows<B>(X, 1, L, dg);
+    for (int e = threadIdx.x; e < B; e += blockDim.x) g[e] = X[e];
+    if (threadIdx.x == 0 && bad >= 0 && *a.info == 0) *a.info = 1 + j * B + bad;
+    return;
+  }
+  double* T = a.tiles + tile_off(t, B);
+  for (int r0 = 0; r0 < B; r0 += PanelCfg<B>::kRows) {
+    const int rows = min(PanelCfg<B>::kRows, B - r0);
+    for (int e = threadIdx.x; e < rows * B; e += blockDim.x) X[e] = T[(size_t)r0 * B + e];
+    __syncthreads();
+    trsm_rows<B>(X, rows, L, dg);
+    for (int e = threadIdx.x; e < rows * B; e += blockDim.x) T[(size_t)r0 * B + e] = X[e];
+    __syncthreads();
+  }
+}
+
+// ----------------------------------------------------------------------------------------------------------- update
+// Output sub-blocks of S x S (S a multiple of 16, NSUB x NSUB of them cover the tile), 16 x 16 threads with an M x M
+// register tile each, k in chunks of 16 staged through shared memory.
+template <int B>
+struct UpdCfg {
+  static constexpr int kSub = (B + 63) / 64;
+  static constexpr int S = (((B + kSub - 1) / kSub) + 15) / 16 * 16;
+  static constexpr int M = S / 16;
+  static constexpr int KC = 16;
+};
+
+struct UpdTask {
+  int target, a, b, rhs_row;  // rhs_row >= 0: diagonal target, also g_rhs_row -= L_a y_j
+};
+
+template <int B>
+__global__ void __launch_bounds__(kThreads) window_solve_update_kernel(SolveArgs a, const UpdTask* tasks, int j)
+{
+  using Cfg = UpdCfg<B>;
+  constexpr int S = Cfg::S, M = Cfg::M, KC = Cfg::KC;
+  __shared__ double As[KC][S + 1], Bs[KC][S + 1];
+  const UpdTask task = tasks[blockIdx.x];
+  double* T = a.tiles + tile_off(task.target, B);
+  const double* La = a.tiles + tile_off(task.a, B);
+  const double* Lb = a.tiles + tile_off(task.b, B);
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  for (int sr = 0; sr < Cfg::kSub; ++sr)
+    for (int sc = 0; sc < Cfg::kSub; ++sc) {
+      const int r0 = sr * S, c0 = sc * S;
+      double acc[M][M];
+#pragma unroll
+      for (int u = 0; u < M; ++u)
+#pragma unroll
+        for (int v = 0; v < M; ++v) acc[u][v] = 0.0;
+      for (int k0 = 0; k0 < B; k0 += KC) {
+        for (int e = threadIdx.x; e < S * KC; e += kThreads) {
+          const int rr = e / KC, kk = e % KC, k = k0 + kk;
+          As[kk][rr] = (r0 + rr < B && k < B) ? La[(r0 + rr) * B + k] : 0.0;
+          Bs[kk][rr] = (c0 + rr < B && k < B) ? Lb[(c0 + rr) * B + k] : 0.0;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int kk = 0; kk < KC; ++kk) {
+          double x[M], y[M];
+#pragma unroll
+          for (int u = 0; u < M; ++u) x[u] = As[kk][ty + 16 * u];
+#pragma unroll
+          for (int v = 0; v < M; ++v) y[v] = Bs[kk][tx + 16 * v];
+#pragma unroll
+          for (int u = 0; u < M; ++u)
+#pragma unroll
+            for (int v = 0; v < M; ++v) acc[u][v] = __fma_rn(x[u], y[v], acc[u][v]);
+        }
+        __syncthreads();
+      }
+#pragma unroll
+      for (int u = 0; u < M; ++u)
+#pragma unroll
+        for (int v = 0; v < M; ++v) {
+          const int r = r0 + ty + 16 * u, c = c0 + tx + 16 * v;
+          if (r < B && c < B) T[r * B + c] = __dsub_rn(T[r * B + c], acc[u][v]);
+        }
+    }
+  if (task.rhs_row >= 0) {
+    const double* y = a.rhs + (size_t)j * B;
+    double* g = a.rhs + (size_t)task.rhs_row * B;
+    for (int r = threadIdx.x; r < B; r += kThreads) {
+      double s = 0.0;
+      for (int m = 0; m < B; ++m) s = __fma_rn(La[r * B + m], y[m], s);
+      g[r] = __dsub_rn(g[r], s);
+    }
+  }
+}
+
+// --------------------------------------------------------------------------------------------------------- backward
+// launch for row j: CTA 0 writes dx_j; CTA q > 0 owns tile row_tiles[q - 1] = (j, i < j) and does y_i -= L_ji^T x_j
+template <int B>
+__global__ void __launch_bounds__(kThreads) window_solve_backward_kernel(SolveArgs a, const int* row_tiles, int j)
+{
+  extern __shared__ double sm[];
+  double* L = sm;        // L_jj, row-major
+  double* x = L + B * B;
+  const double* Lj = a.tiles + tile_off(a.num_tiles + j, B);
+  for (int e = threadIdx.x; e < B * B; e += blockDim.x) L[e] = Lj[e];
+  for (int e = threadIdx.x; e < B; e += blockDim.x) x[e] = a.rhs[(size_t)j * B + e];
+  __syncthreads();
+  // L^T x = y: for r = B-1 .. 0, x_r /= L_rr, then x_m -= L_rm x_r for m < r
+  for (int r = B - 1; r >= 0; --r) {
+    if (threadIdx.x == 0) x[r] = __ddiv_rn(x[r], L[r * B + r]);
+    __syncthreads();
+    for (int m = threadIdx.x; m < r; m += blockDim.x) x[m] = __fma_rn(-L[r * B + m], x[r], x[m]);
+    __syncthreads();
+  }
+  const bool ok = *a.info == 0;
+  if (blockIdx.x == 0) {
+    for (int r = threadIdx.x; r < B; r += blockDim.x)
+      a.dx[(size_t)j * B + r] = (ok && !a.fixed[j * B + r]) ? x[r] : 0.0;
+    return;
+  }
+  const int t = row_tiles[blockIdx.x - 1], i = a.tile_col[t];
+  const double* Lji = a.tiles + tile_off(t, B);
+  double* y = a.rhs + (size_t)i * B;
+  for (int c = threadIdx.x; c < B; c += blockDim.x) {
+    double s = 0.0;
+    for (int m = 0; m < B; ++m) s = __fma_rn(Lji[m * B + c], x[m], s);
+    y[c] = __dsub_rn(y[c], s);
+  }
+}
+
+template <class F>
+cudaError_t with_code_size(int code_size, F&& f)
+{
+  switch (code_size) {
+    case 8: return f(std::integral_constant<int, 14>{});
+    case 16: return f(std::integral_constant<int, 22>{});
+    case 32: return f(std::integral_constant<int, 38>{});
+    case 64: return f(std::integral_constant<int, 70>{});
+    case 128: return f(std::integral_constant<int, 134>{});
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+}  // namespace
+
+// --------------------------------------------------------------------------------------------------------- the plan
+struct WindowSolverDev {
+  int K = 0, C = 0, B = 0, P = 0, L = 0, num_tiles = 0;
+  std::vector<int> col_ptr;   // [K + 1] tiles of column j: [col_ptr[j], col_ptr[j+1]), the first one diagonal
+  std::vector<int> upd_ptr;   // [K + 1] update tasks of column j
+  std::vector<int> row_ptr;   // [K + 1] backward tiles of row j (off-diagonal, column order)
+  // device: one int allocation (tile_row | tile_col | contrib_ptr | contrib | diag_tile | row_tiles | tasks), the fixed
+  // mask, the codes, the tiles, the rhs
+  void* ints = nullptr;
+  unsigned char* fixed = nullptr;
+  double* codes = nullptr;
+  double* tiles = nullptr;
+  double* rhs = nullptr;
+  const int *tile_row = nullptr, *tile_col = nullptr, *contrib_ptr = nullptr, *contrib = nullptr, *diag_tile = nullptr,
+            *row_tiles = nullptr;
+  const UpdTask* tasks = nullptr;
+  ~WindowSolverDev()
+  {
+    cudaFree(ints);
+    cudaFree(fixed);
+    cudaFree(codes);
+    cudaFree(tiles);
+    cudaFree(rhs);
+  }
+};
+
+size_t window_solver_tiles(const WindowSolverDev* s) { return s ? (size_t)s->num_tiles : 0; }
+
+cudaError_t window_solver_create(int K, int C, const std::vector<int>& pair_k0, const std::vector<int>& pair_k1,
+                                 const std::vector<int>& link_k0, const std::vector<int>& link_k1,
+                                 const std::vector<int>& fixed_vars, WindowSolverDev** out)
+{
+  *out = nullptr;
+  const int B = 6 + C, P = (int)pair_k0.size(), L = (int)link_k0.size();
+  // ---- symbolic elimination in keyframe order: below[j] = rows i > j of the nonzero tiles of column j
+  std::vector<std::set<int>> below(K);
+  for (int p = 0; p < P; ++p)
+    if (pair_k0[p] != pair_k1[p]) below[std::min(pair_k0[p], pair_k1[p])].insert(std::max(pair_k0[p], pair_k1[p]));
+  for (int l = 0; l < L; ++l) below[std::min(link_k0[l], link_k1[l])].insert(std::max(link_k0[l], link_k1[l]));
+  for (int j = 0; j < K; ++j) {
+    for (auto ia = below[j].begin(); ia != below[j].end(); ++ia)
+      for (auto ib = below[j].begin(); ib != ia; ++ib) below[*ib].insert(*ia);  // (ia, ib) fills, ib < ia
+  }
+  auto s = std::make_unique<WindowSolverDev>();
+  s->K = K; s->C = C; s->B = B; s->P = P; s->L = L;
+  std::vector<int> tile_row, tile_col;
+  s->col_ptr.assign(K + 1, 0);
+  std::vector<std::vector<std::pair<int, int>>> col_index(K);  // (row, tile) per column, rows ascending
+  for (int j = 0; j < K; ++j) {
+    s->col_ptr[j] = (int)tile_row.size();
+    tile_row.push_back(j); tile_col.push_back(j);
+    col_index[j].push_back({j, s->col_ptr[j]});
+    for (int i : below[j]) {
+      col_index[j].push_back({i, (int)tile_row.size()});
+      tile_row.push_back(i); tile_col.push_back(j);
+    }
+  }
+  const int T = (int)tile_row.size();
+  s->num_tiles = T;
+  s->col_ptr[K] = T;
+  auto tile_of = [&](int i, int j) {  // i >= j, structurally nonzero: binary search of column j's rows
+    const auto& ci = col_index[j];
+    return std::lower_bound(ci.begin(), ci.end(), std::make_pair(i, -1))->second;
+  };
+  // ---- contributions per tile, in to_dense's order
+  std::vector<std::vector<int>> contrib(T);
+  for (int p = 0; p < P; ++p) {
+    const int k0 = pair_k0[p], k1 = pair_k1[p];
+    if (k0 == k1) {
+      contrib[tile_of(k0, k0)].push_back(p * 4 + CONTRIB_PAIR);
+      contrib[tile_of(k0, k0)].push_back(p * 4 + CONTRIB_PAIR_T);
+    } else if (k0 > k1) {
+      contrib[tile_of(k0, k1)].push_back(p * 4 + CONTRIB_PAIR);
+    } else {
+      contrib[tile_of(k1, k0)].push_back(p * 4 + CONTRIB_PAIR_T);
+    }
+  }
+  for (int l = 0; l < L; ++l) {
+    const int k0 = link_k0[l], k1 = link_k1[l];
+    if (k0 > k1) contrib[tile_of(k0, k1)].push_back(l * 4 + CONTRIB_LINK);
+    else contrib[tile_of(k1, k0)].push_back(l * 4 + CONTRIB_LINK_T);
+  }
+  // ---- update tasks per column, backward tiles per row
+  std::vector<UpdTask> tasks;
+  s->upd_ptr.assign(K + 1, 0);
+  std::vector<std::vector<int>> row_list(K);
+  for (int j = 0; j < K; ++j) {
+    s->upd_ptr[j] = (int)tasks.size();
+    const auto& ci = col_index[j];
+    for (size_t qa = 1; qa < ci.size(); ++qa) {
+      row_list[ci[qa].first].push_back(ci[qa].second);
+      for (size_t qb = 1; qb <= qa; ++qb)
+        tasks.push_back({tile_of(ci[qa].first, ci[qb].first), ci[qa].second, ci[qb].second, qa == qb ? ci[qa].first : -1});
+    }
+  }
+  s->upd_ptr[K] = (int)tasks.size();
+  s->row_ptr.assign(K + 1, 0);
+  std::vector<int> row_tiles;
+  for (int j = 0; j < K; ++j) {
+    s->row_ptr[j] = (int)row_tiles.size();
+    row_tiles.insert(row_tiles.end(), row_list[j].begin(), row_list[j].end());
+  }
+  s->row_ptr[K] = (int)row_tiles.size();
+  // ---- one int blob
+  std::vector<int> blob;
+  auto put = [&](const int* p, size_t n) {
+    const size_t o = blob.size();
+    blob.insert(blob.end(), p, p + n);
+    return o;
+  };
+  std::vector<int> cptr(T + 1, 0), cflat;
+  for (int t = 0; t < T; ++t) {
+    cptr[t] = (int)cflat.size();
+    cflat.insert(cflat.end(), contrib[t].begin(), contrib[t].end());
+  }
+  cptr[T] = (int)cflat.size();
+  std::vector<int> diag(K);
+  for (int j = 0; j < K; ++j) diag[j] = s->col_ptr[j];
+  const size_t o_tr = put(tile_row.data(), T), o_tc = put(tile_col.data(), T), o_cp = put(cptr.data(), T + 1);
+  const size_t o_cf = put(cflat.data(), cflat.size()), o_dg = put(diag.data(), K);
+  const size_t o_rt = put(row_tiles.data(), row_tiles.size());
+  blob.resize((blob.size() + 3) & ~(size_t)3, 0);  // UpdTask is 16-byte aligned
+  const size_t o_tk = put(reinterpret_cast<const int*>(tasks.data()), tasks.size() * 4);
+  std::vector<unsigned char> fixed((size_t)K * B, 0);
+  for (int v : fixed_vars) fixed[v] = 1;
+
+  cudaError_t e;
+  if ((e = cudaMalloc(&s->ints, std::max<size_t>(blob.size(), 1) * sizeof(int))) != cudaSuccess) return e;
+  if ((e = cudaMalloc((void**)&s->fixed, fixed.size())) != cudaSuccess) return e;
+  if ((e = cudaMalloc((void**)&s->codes, (size_t)K * C * sizeof(double))) != cudaSuccess) return e;
+  if ((e = cudaMalloc((void**)&s->tiles, (size_t)(T + K) * B * B * sizeof(double))) != cudaSuccess) return e;
+  if ((e = cudaMalloc((void**)&s->rhs, (size_t)K * B * sizeof(double))) != cudaSuccess) return e;
+  if ((e = cudaMemcpy(s->ints, blob.data(), blob.size() * sizeof(int), cudaMemcpyHostToDevice)) != cudaSuccess) return e;
+  if ((e = cudaMemcpy(s->fixed, fixed.data(), fixed.size(), cudaMemcpyHostToDevice)) != cudaSuccess) return e;
+  const int* ip = static_cast<const int*>(s->ints);
+  s->tile_row = ip + o_tr; s->tile_col = ip + o_tc; s->contrib_ptr = ip + o_cp; s->contrib = ip + o_cf;
+  s->diag_tile = ip + o_dg; s->row_tiles = ip + o_rt;
+  s->tasks = reinterpret_cast<const UpdTask*>(ip + o_tk);
+  // kernel attributes once, here: no runtime configuration call in a solve
+  e = with_code_size(C, [](auto bc) {
+    constexpr int Bv = bc.value;
+    cudaError_t r = cudaFuncSetAttribute(window_solve_panel_kernel<Bv>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         PanelCfg<Bv>::kSmem);
+    if (r != cudaSuccess) return r;
+    return cudaFuncSetAttribute(window_solve_backward_kernel<Bv>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (Bv * Bv + Bv) * 8);
+  });
+  if (e != cudaSuccess) return e;
+  *out = s.release();
+  return cudaSuccess;
+}
+
+void window_solver_destroy(WindowSolverDev* s) { delete s; }
+
+cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_dev, double lambda, double prior,
+                                const double* codes_host, double* dx_dev, int32_t* info_dev, cudaStream_t stream,
+                                uint64_t* launches)
+{
+  SolveArgs a{};
+  a.buf = window_dev;
+  a.codes = prior > 0.0 ? s->codes : nullptr;
+  a.tiles = s->tiles; a.rhs = s->rhs; a.dx = dx_dev; a.info = info_dev;
+  a.tile_row = s->tile_row; a.tile_col = s->tile_col; a.contrib_ptr = s->contrib_ptr; a.contrib = s->contrib;
+  a.diag_tile = s->diag_tile; a.fixed = s->fixed;
+  a.K = s->K; a.P = s->P; a.num_tiles = s->num_tiles;
+  a.lambda = lambda; a.prior = prior;
+  if (prior > 0.0) {
+    // pageable source: the copy is staged before the call returns, so the caller may reuse its array at once
+    cudaError_t e = cudaMemcpyAsync(s->codes, codes_host, (size_t)s->K * s->C * sizeof(double), cudaMemcpyHostToDevice,
+                                    stream);
+    if (e != cudaSuccess) return e;
+  }
+  return with_code_size(s->C, [&](auto bc) {
+    constexpr int Bv = bc.value;
+    uint64_t n = 0;
+    window_solve_load_kernel<Bv><<<s->num_tiles, kThreads, 0, stream>>>(a);
+    ++n;
+    for (int j = 0; j < s->K; ++j) {
+      const int c0 = s->col_ptr[j], nc = s->col_ptr[j + 1] - c0;
+      window_solve_panel_kernel<Bv><<<nc, kThreads, PanelCfg<Bv>::kSmem, stream>>>(a, j, c0);
+      ++n;
+      const int u0 = s->upd_ptr[j], nu = s->upd_ptr[j + 1] - u0;
+      if (nu > 0) {
+        window_solve_update_kernel<Bv><<<nu, kThreads, 0, stream>>>(a, s->tasks + u0, j);
+        ++n;
+      }
+    }
+    for (int j = s->K - 1; j >= 0; --j) {
+      const int r0 = s->row_ptr[j], nr = s->row_ptr[j + 1] - r0;
+      window_solve_backward_kernel<Bv><<<1 + nr, kThreads, (Bv * Bv + Bv) * 8, stream>>>(a, s->row_tiles + r0, j);
+      ++n;
+    }
+    *launches += n;
+    return cudaGetLastError();
+  });
+}
+
+}  // namespace dfk

@@ -12,6 +12,8 @@ solves.  Here every heavy step of one iteration is ONE device operation over the
     assemble    block-sparse normal equations of the window, on the device               dfk_window_assemble
                 (+ one all-reduce across ranks when the pairs are sharded)
     solve       damped dense solve on the device (Cholesky, float64)                     torch.linalg
+                or, with WindowOptimizer(solve=...), the damped block-sparse Cholesky      dfk_window_solve
+                straight from the window buffer (SfmWindowProblem.solve)
     (links)     one batched launch over the stale reprojection links (global loop closures, use_reprojection),
                 straight into normal-equation records                                  dfk_reprojection_linearize_batch
                 and one over the stale sparse geometric links (use_geometric)          dfk_sparse_geometric_linearize_batch
@@ -137,13 +139,27 @@ class WindowOptimizer:
     """Levenberg-Marquardt over the poses and codes of a keyframe window.
 
     `linearise(poses, codes, pairs_to_eval) -> (window_buffer, f)` is the device pipeline (see SfmWindowProblem below for
-    the one built on SfmAligner / Window); injected so that the host logic is testable without a GPU."""
+    the one built on SfmAligner / Window); injected so that the host logic is testable without a GPU.
 
-    def __init__(self, layout: WindowBlocks, linearise: Callable, params: Optional[LMParams] = None):
+    `solve(buf, lam, fixed, code_prior_weight, codes) -> dx (numpy float64) | None`, when given, replaces to_dense +
+    damped_solve: the loop then never builds H, reads f from the buffer's scalar slot (plus the host prior term) and
+    counts None (not positive definite) as a rejected step.  SfmWindowProblem.solve is the device one."""
+
+    def __init__(self, layout: WindowBlocks, linearise: Callable, params: Optional[LMParams] = None,
+                 solve: Optional[Callable] = None):
         self.layout = layout
         self.linearise = linearise
         self.params = params or LMParams()
+        self.solve = solve
         self.cache = LinearisationCache(layout.pairs, self.params.cache_eps, layout.geometric)
+
+    def _energy(self, buf, codes) -> float:
+        """f of _system without H: the buffer's scalar slot (what to_dense returns) plus the prior term"""
+        f = float(buf[self.layout.offsets()[2]])
+        w = self.params.code_prior_weight
+        if w > 0:
+            f += 0.5 * w * float((codes ** 2).sum())
+        return f
 
     def _system(self, buf, codes):
         H, g, f, inl = self.layout.to_dense(buf)
@@ -176,6 +192,8 @@ class WindowOptimizer:
         trace = LMTrace()
         fixed = list(range(6)) if prm.fix_first_pose else []
         lam = prm.lambda_init
+        if self.solve is not None:
+            return self._run_solve(poses, codes, trace, fixed, lam)
         buf = self._evaluate(poses, codes, trace)
         H, g, f = self._system(buf, codes)
         trace.energy.append(f)
@@ -195,6 +213,36 @@ class WindowOptimizer:
             else:
                 # H, g, f of the accepted point are still at hand; the record buffer (and with it the cache) now describes
                 # the rejected candidate, which the next candidate is compared against -- nothing to re-evaluate
+                lam = lam * prm.lambda_up
+                if lam > prm.lambda_max:
+                    break
+        return poses, codes, trace
+
+    def _run_solve(self, poses, codes, trace: LMTrace, fixed, lam):
+        """run() with the injected solve: the same schedule, on the buffer of the accepted point"""
+        prm = self.params
+        buf = self._evaluate(poses, codes, trace)
+        f = self._energy(buf, codes)
+        trace.energy.append(f)
+        for _ in range(prm.iterations):
+            dx = self.solve(buf, lam, fixed, prm.code_prior_weight, codes)
+            trace.lam.append(lam)
+            if dx is None:  # not positive definite at this damping: a rejected step, nothing re-linearised
+                trace.accepted.append(False)
+                lam = lam * prm.lambda_up
+                if lam > prm.lambda_max:
+                    break
+                continue
+            cand_p, cand_c = apply_update(poses, codes, np.asarray(dx, dtype=np.float64), self.layout.code_size)
+            cbuf = self._evaluate(cand_p, cand_c, trace)
+            cf = self._energy(cbuf, cand_c)
+            ok = np.isfinite(cf) and cf < f
+            trace.accepted.append(bool(ok))
+            if ok:
+                poses, codes, buf, f = cand_p, cand_c, cbuf, cf
+                trace.energy.append(f)
+                lam = max(lam * prm.lambda_down, 1e-12)
+            else:
                 lam = lam * prm.lambda_up
                 if lam > prm.lambda_max:
                     break
@@ -274,6 +322,24 @@ class SfmWindowProblem:
         self.geo_records = torch.zeros((len(self.geometric), _lib.geo_record_floats(aligner.CS)), dtype=torch.float32,
                                        device=dev) if self.geometric else None
         self.allreduce = allreduce
+        self._solvers = {}  # fixed variables -> WindowSolver, created on first use
+
+    def solve(self, buf, lam, fixed, code_prior_weight=0.0, codes=None):
+        """WindowOptimizer's `solve` on the device: dfk_window_solve of the window buffer, then one read-back of dx and
+        info together.  Returns dx (numpy float64), or None when the damped system is not positive definite."""
+        import torch
+        from .aligners import WindowSolver
+        key = tuple(int(v) for v in fixed)
+        if key not in self._solvers:
+            self._solvers[key] = WindowSolver(self.window, key)
+        n = self.layout.num_keyframes * self.layout.B
+        out = torch.empty(8 * n + 8, dtype=torch.uint8, device=buf.device)  # [dx float64 | info int32 | pad]
+        dx, info = out[:8 * n].view(torch.float64), out[8 * n:8 * n + 4].view(torch.int32)
+        self._solvers[key].solve(buf, lam, code_prior_weight, codes if code_prior_weight > 0 else None, dx=dx, info=info)
+        host = out.cpu().numpy()
+        if int(host[8 * n:8 * n + 4].view(np.int32)[0]) != 0:
+            return None
+        return host[:8 * n].view(np.float64).copy()
 
     def _items(self, poses, codes, todo):
         items = []

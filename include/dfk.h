@@ -266,6 +266,42 @@ DfkStatus dfk_window_create_geometric(DfkHandle h, const DfkWindowDesc* desc, in
 DfkStatus dfk_window_assemble_geometric(DfkHandle h, const DfkWindow* w, const float* records_dev,
                                         const float* geo_records_dev, float* window_dev);
 
+/* Damped block-sparse fp64 Cholesky solve of a window's normal equations, straight from its packed buffer.
+ *
+ * The system is the dense one the buffer stands for (fp32 entries promoted to fp64, every off-diagonal block mirrored):
+ *   1. with w = code_prior_weight > 0: + w I on every code block, - w code_k on every code gradient;
+ *   2. the fixed variables dropped (solved as identity rows with a zero right-hand side: dx = 0 there);
+ *   3. d = diag(H) over the kept variables, + lambda d + 1e-12 max|d| on that diagonal;
+ *   4. H dx = g.
+ * The unit of sparsity is the B x B tile of a pair of keyframes.  create runs the symbolic elimination in keyframe order
+ * (a tile (i, j), i >= j, is nonzero when i = j, when a pair or link joins i and j in either direction, or by fill) and
+ * allocates the workspace: (tiles + K) * B * B doubles for the factor, plus K * B doubles and K * C doubles.
+ * A solve is deterministic (two solves of the same buffer are bit for bit equal, on any handle of the same GPU model),
+ * asynchronous on the handle's stream, and allocates nothing: one load launch, a panel and an update launch per
+ * keyframe column, a backward launch per keyframe. */
+typedef struct DfkWindowSolver DfkWindowSolver;
+/* fixed_vars: HOST, num_fixed distinct window-variable indices k * B + r (e.g. 0..5 = the gauge keyframe's pose), copied.
+ * Out-of-range or duplicated indices are rejected. */
+DfkStatus dfk_window_solver_create(DfkHandle h, const DfkWindow* w, int num_fixed, const int32_t* fixed_vars,
+                                   DfkWindowSolver** out);
+/* h must not be NULL (like every entry point that takes a handle); s may be */
+DfkStatus dfk_window_solver_destroy(DfkHandle h, DfkWindowSolver* s);
+/* *tiles = the structurally nonzero B x B tiles of the lower factor, fill included */
+DfkStatus dfk_window_solver_tiles(DfkHandle h, const DfkWindowSolver* s, size_t* tiles);
+
+typedef struct {
+  double lambda;            /* LM damping, >= 0, finite */
+  double code_prior_weight; /* >= 0, finite; 0 = no prior */
+} DfkWindowSolveParams;
+
+/* window_dev: the packed buffer of dfk_window_assemble[_geometric] for this solver's window (DEVICE, fp32, read only).
+ * codes: HOST, K * C doubles, required iff code_prior_weight > 0 (read before the call returns).
+ * dx_dev: DEVICE, K * B doubles, fully written.  info_dev: DEVICE, one int32: 0, or 1 + the first variable (in
+ * elimination order) whose pivot was not positive and finite; dx is then all zero.
+ * Every argument is checked before anything is enqueued; a rejected call writes nothing. */
+DfkStatus dfk_window_solve(DfkHandle h, const DfkWindowSolver* s, const float* window_dev, const DfkWindowSolveParams* p,
+                           const double* codes, double* dx_dev, int32_t* info_dev);
+
 /* ------------------------------------------------------------------ SE3Aligner */
 
 /* SE3Aligner<float>::RunStep (cu_se3aligner.h:65-70, cu_se3aligner.cpp:153-176):

@@ -18,7 +18,12 @@ One JSON line per case:
   * SparseGeometricFactor linearisation of K = 32 / 200 factors x M = 500 / 3000 points at C = 32 / 128, 640x480
     level 0: K synchronous SparseGeometricLinearize calls + the host A^T A against one SparseGeometricLinearizeBatch;
     and one linearisation of the window200 window without and with 50 geometric links x 3000 points.
-Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` runs those cases alone.
+  * the window solve (`--only solve`): damped_solve(to_dense(buf)) on torch against dfk_window_solve (WindowSolver) on
+    random positive definite window buffers of window200 (50 keyframes, 200 pairs of bench.window_pairs) at C = 32 and
+    C = 128 and ba2k (200 keyframes, 2000 pairs) at C = 32 -- wall clock to a synchronise, the two alternated; then a
+    torch.profiler run of one device solve: device time, launches, and the fp64 flops of the fill pattern over it.
+Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` runs
+those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -37,7 +42,7 @@ sys.path.insert(0, ROOT)
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
-    ap.add_argument("--only", choices=["reprojection", "geometric"], default=None)
+    ap.add_argument("--only", choices=["reprojection", "geometric", "solve"], default=None)
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -63,6 +68,8 @@ def main():
         return reprojection_cases(args, torch, print)
     if args.only == "geometric":
         return geometric_cases(args, torch, print)
+    if args.only == "solve":
+        return solve_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -437,6 +444,92 @@ def geometric_cases(args, torch, print):
                           "device_us_per_linearisation": _device_us(torch, lin, reps),
                           "timing": "wall clock to the end of the assembly (synchronised); device time = summed kernel + "
                                     "copy time, torch.profiler"}), flush=True)
+
+
+
+def solve_fill(K, links):
+    """(tiles, fp64 flops) of the block Cholesky of a window whose keyframes are joined by `links`, eliminated in index
+    order (the symbolic analysis of dfk_window_solver_create): per column with n off-diagonal tiles, the diagonal
+    factor B^3 / 3, n triangular solves B^3 and n (n + 1) / 2 Schur updates 2 B^3, in units of B^3"""
+    below = [set() for _ in range(K)]
+    for a, b in links:
+        if a != b:
+            below[min(a, b)].add(max(a, b))
+    units = 0.0
+    for j in range(K):
+        rows = sorted(below[j])
+        for x in range(len(rows)):
+            for y in range(x):
+                below[rows[y]].add(rows[x])
+        n = len(rows)
+        units += 1.0 / 3.0 + n + n * (n + 1)
+    return K + sum(len(r) for r in below), units
+
+
+def solve_cases(args, torch, print):
+    import numpy as np
+    from bench import window_pairs
+    from deepfactors_b200.aligners import SfmAligner, Window, WindowSolver
+    from deepfactors_b200.window_opt import damped_solve
+    for name, K, P, cs in (("window200", 50, 200, 32), ("window200", 50, 200, 128), ("ba2k", 200, 2000, 32)):
+        pairs = window_pairs(K, P)
+        al = SfmAligner(cs)
+        win = Window(al, K, pairs, list(range(P)), [(0, 0)] * P)
+        lay = win.layout
+        NP = 12 + cs
+        rng = np.random.default_rng(1)
+        JtJ = np.empty((P, NP, NP), np.float32)
+        Jtr = np.empty((P, NP), np.float32)
+        for p in range(P):  # random Gram records: every block positive definite
+            A = rng.standard_normal((2 * NP, NP + 1)).astype(np.float32)
+            JtJ[p] = A[:, :NP].T @ A[:, :NP]
+            Jtr[p] = A[:, :NP].T @ A[:, NP]
+        buf = torch.from_numpy(lay.pack(list(range(P)), JtJ, Jtr, np.ones(P, np.float32), np.zeros(P), [(0, 0)] * P)).cuda()
+        fixed = tuple(range(6))
+        lam = 1e-4
+        sol = WindowSolver(win, fixed)
+        B = lay.B
+        tiles, units = solve_fill(K, pairs)
+        assert tiles == sol.tiles
+        flops = units * B ** 3
+
+        def run_torch():
+            H, g, _, _ = lay.to_dense(buf)
+            dx = damped_solve(H, g, lam, fixed)
+            torch.cuda.synchronize()
+            return dx
+
+        def run_dev():
+            dx, info = sol.solve(buf, lam)
+            torch.cuda.synchronize()
+            return dx, info
+
+        ref = run_torch()
+        dx, info = run_dev()
+        assert int(info.item()) == 0
+        err = float((dx - ref).abs().max() / ref.abs().max())
+        reps = min(args.reps, 5) if K > 100 else args.reps
+        tt, td = [], []
+        for _ in range(reps):  # alternated
+            t0 = time.perf_counter(); run_torch(); tt.append(time.perf_counter() - t0)
+            t0 = time.perf_counter(); run_dev(); td.append(time.perf_counter() - t0)
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            run_dev()
+        ev = [e for e in prof.events() if e.device_type.name == "CUDA" and "window_solve" in e.name]
+        dev_ms = sum(e.device_time for e in ev) / 1e3
+        per = {}
+        for e in ev:
+            k = e.name.split("window_solve_")[1].split("_kernel")[0]
+            per[k] = per.get(k, 0.0) + e.device_time / 1e3
+        print(json.dumps(dict(
+            case="window_solve", shape=name, K=K, pairs=P, C=cs, tiles=tiles, dense_tiles=K * (K + 1) // 2,
+            factor_mb=round((tiles + K) * B * B * 8 / 1e6, 1), dense_mb=round((K * B) ** 2 * 8 / 1e6, 1),
+            torch_ms_median=round(1e3 * float(np.median(tt)), 3), torch_ms_min=round(1e3 * min(tt), 3),
+            device_ms_median=round(1e3 * float(np.median(td)), 3), device_ms_min=round(1e3 * min(td), 3),
+            device_kernel_ms=round(dev_ms, 3), kernel_ms_by_kind={k: round(v, 3) for k, v in per.items()},
+            launches=len(ev), fill_gflop=round(flops / 1e9, 2), fp64_tflops=round(flops / (dev_ms * 1e-3) / 1e12, 3),
+            rel_diff_vs_torch=err, reps=reps)))
 
 
 if __name__ == "__main__":
