@@ -305,11 +305,17 @@ def _geometric_item(it: dict, cs: int, keep: list) -> DfkSparseGeometricItem:
     return w
 
 
+def _check_tensor(hd: _Handle, t: torch.Tensor, dtype: torch.dtype, n: int, what: str):
+    """a kernel reads or writes n elements of t, on the handle's device: refuse any other tensor before the C call"""
+    dev = torch.device("cuda", hd.device)
+    if not (t.dtype == dtype and t.device == dev and t.is_contiguous() and t.numel() >= n):
+        raise ValueError(f"{what} must be a contiguous {dtype} tensor of at least {n} entries on {dev}")
+
+
 def _batch_records(aligner, n: int, rec: int, records: torch.Tensor | None) -> torch.Tensor:
     if records is None:
         return torch.empty((n, rec), dtype=torch.float32, device=f"cuda:{aligner._hd.device}")
-    if not (records.is_contiguous() and records.numel() >= n * rec):
-        raise ValueError(f"records must be a contiguous device tensor of at least {n} x {rec} floats")
+    _check_tensor(aligner._hd, records, torch.float32, n * rec, "records")
     return records
 
 
@@ -442,15 +448,13 @@ class Window:
         desc = _lib.DfkWindowDesc(int(num_keyframes), len(k0), len(ip), aligner.CS, k0.ctypes.data_as(I32),
                                   k1.ctypes.data_as(I32), ip.ctypes.data_as(I32), iw.ctypes.data_as(I32),
                                   ih.ctypes.data_as(I32))
+        g0 = np.ascontiguousarray([p[0] for p in self.layout.geometric], dtype=np.int32)
+        g1 = np.ascontiguousarray([p[1] for p in self.layout.geometric], dtype=np.int32)
+        L = len(g0)
         self.w = C.c_void_p()
-        L = len(self.layout.geometric)
-        if L:
-            g0 = np.ascontiguousarray([p[0] for p in self.layout.geometric], dtype=np.int32)
-            g1 = np.ascontiguousarray([p[1] for p in self.layout.geometric], dtype=np.int32)
-            check(aligner.handle, lib().dfk_window_create_geometric(aligner.handle, C.byref(desc), L, g0.ctypes.data_as(I32),
-                                                                    g1.ctypes.data_as(I32), C.byref(self.w)))
-        else:
-            check(aligner.handle, lib().dfk_window_create(aligner.handle, C.byref(desc), C.byref(self.w)))
+        check(aligner.handle, lib().dfk_window_create_geometric(aligner.handle, C.byref(desc), L,
+                                                                g0.ctypes.data_as(I32) if L else None,
+                                                                g1.ctypes.data_as(I32) if L else None, C.byref(self.w)))
         self.num_items = len(ip)
         self.floats = int(lib().dfk_window_floats(self.w))
         assert self.floats == self.layout.floats
@@ -459,30 +463,21 @@ class Window:
                  geo_records: torch.Tensor | None = None) -> torch.Tensor:
         """records: [num_items, REC] device tensor written by RunStepBatch; geo_records: [num_links, GEO_REC] written by
         SparseGeometricLinearizeBatch (required when the window has links).  Asynchronous on torch's current stream."""
-        self._al._hd.use_torch_stream()
-        dev = torch.device(f"cuda:{self._al._hd.device}")
-
-        def need(t, n, what):  # the kernel reads / writes n floats of t on the handle's device
-            if not (t.dtype == torch.float32 and t.device == dev and t.is_contiguous() and t.numel() >= n):
-                raise ValueError(f"{what} must be a contiguous float32 tensor of at least {n} floats on {dev}")
-
-        rec = _lib.record_floats(self.layout.code_size)
-        need(records, self.num_items * rec, "records")
+        hd = self._al._hd
+        hd.use_torch_stream()
+        _check_tensor(hd, records, torch.float32, self.num_items * _lib.record_floats(self.layout.code_size), "records")
         if out is None:
             out = torch.empty(self.floats, dtype=torch.float32, device=records.device)
-        need(out, self.floats, "out")
+        _check_tensor(hd, out, torch.float32, self.floats, "out")
         if self.layout.geometric and geo_records is None:
             raise ValueError("the window has geometric links: geo_records is required")
+        geo = None
         if geo_records is not None:
-            need(geo_records, len(self.layout.geometric) * _lib.geo_record_floats(self.layout.code_size), "geo_records")
-        if geo_records is None and not self.layout.geometric:
-            check(self._al.handle, lib().dfk_window_assemble(self._al.handle, self.w, C.c_void_p(records.data_ptr()),
-                                                             C.c_void_p(out.data_ptr())))
-            return out
-        geo = C.c_void_p(geo_records.data_ptr()) if geo_records is not None else None
-        check(self._al.handle, lib().dfk_window_assemble_geometric(self._al.handle, self.w,
-                                                                   C.c_void_p(records.data_ptr()), geo,
-                                                                   C.c_void_p(out.data_ptr())))
+            _check_tensor(hd, geo_records, torch.float32,
+                          len(self.layout.geometric) * _lib.geo_record_floats(self.layout.code_size), "geo_records")
+            geo = C.c_void_p(geo_records.data_ptr())
+        check(hd.h, lib().dfk_window_assemble_geometric(hd.h, self.w, C.c_void_p(records.data_ptr()), geo,
+                                                        C.c_void_p(out.data_ptr())))
         return out
 
     def close(self):
@@ -521,20 +516,16 @@ class WindowSolver:
         """buf: the window buffer (contiguous float32 on the handle's device).  codes: [K, C] (host), required when
         code_prior_weight > 0.  Returns (dx [K * B] float64, info [1] int32), device tensors written asynchronously on
         torch's current stream; info = 0, or 1 + the first variable whose pivot was not positive (dx is then zero)."""
-        self._al._hd.use_torch_stream()
-        dev = torch.device(f"cuda:{self._al._hd.device}")
+        hd = self._al._hd
+        hd.use_torch_stream()
         n = self.layout.num_keyframes * self.layout.B
-        if not (buf.dtype == torch.float32 and buf.device == dev and buf.is_contiguous()
-                and buf.numel() >= self.layout.floats):
-            raise ValueError(f"buf must be a contiguous float32 tensor of at least {self.layout.floats} floats on {dev}")
+        _check_tensor(hd, buf, torch.float32, self.layout.floats, "buf")
         if dx is None:
-            dx = torch.empty(n, dtype=torch.float64, device=dev)
-        if not (dx.dtype == torch.float64 and dx.device == dev and dx.is_contiguous() and dx.numel() >= n):
-            raise ValueError(f"dx must be a contiguous float64 tensor of at least {n} entries on {dev}")
+            dx = torch.empty(n, dtype=torch.float64, device=buf.device)
+        _check_tensor(hd, dx, torch.float64, n, "dx")
         if info is None:
-            info = torch.empty(1, dtype=torch.int32, device=dev)
-        if not (info.dtype == torch.int32 and info.device == dev and info.numel() >= 1):
-            raise ValueError(f"info must be an int32 tensor on {dev}")
+            info = torch.empty(1, dtype=torch.int32, device=buf.device)
+        _check_tensor(hd, info, torch.int32, 1, "info")
         cp = None
         if code_prior_weight > 0:
             if codes is None:

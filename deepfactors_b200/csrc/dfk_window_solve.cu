@@ -1,7 +1,7 @@
 // dfk_window_solve.cu -- damped block-sparse fp64 Cholesky of a keyframe window's normal equations, straight from the
 // packed buffer of dfk_window_assemble[_geometric] (layout: include/dfk.h).
 //
-// The system is the one WindowOptimizer solves on torch (window_opt.py: WindowBlocks.to_dense, _system, damped_solve):
+// The system is the one WindowOptimizer solves on torch (window_opt.py: dense_solve = to_dense, prior, damped_solve):
 // fp32 entries promoted to fp64 and summed in to_dense's order, the code prior w I / -w code, the fixed variables as
 // identity rows with a zero right-hand side, and lambda d + 1e-12 max|d| on the diagonal of the kept variables.
 //

@@ -9,9 +9,9 @@ solves.  Here every heavy step of one iteration is ONE device operation over the
 
     linearise   one batched RunStep launch over all (pair, level) factors whose variables moved, with the depth decode
                 fused in (the code of keyframe k0 rides in the work item)               dfk_sfm_run_step_batch
-    assemble    block-sparse normal equations of the window, on the device               dfk_window_assemble
+    assemble    block-sparse normal equations of the window, on the device              dfk_window_assemble_geometric
                 (+ one all-reduce across ranks when the pairs are sharded)
-    solve       damped dense solve on the device (Cholesky, float64)                     torch.linalg
+    solve       damped dense solve on the device (dense_solve: Cholesky, float64)       torch.linalg
                 or, with WindowOptimizer(solve=...), the damped block-sparse Cholesky      dfk_window_solve
                 straight from the window buffer (SfmWindowProblem.solve)
     (links)     one batched launch over the stale reprojection links (global loop closures, use_reprojection),
@@ -25,6 +25,7 @@ The host side (cache, retraction, damping schedule) is plain Python / numpy; not
 """
 from __future__ import annotations
 
+import functools
 from dataclasses import dataclass, field
 from typing import Callable, List, Optional, Sequence, Tuple
 
@@ -89,6 +90,27 @@ def damped_solve(H, g, lam: float, fixed: Sequence[int] = ()):
     return dx
 
 
+def dense_solve(layout: WindowBlocks, buf, lam: float, fixed: Sequence[int], code_prior_weight: float, codes):
+    """WindowOptimizer's default solve: to_dense of the buffer plus the zero-code prior (w * I on every code block,
+    -w * code on its gradient), then damped_solve.  buf: numpy, or torch on any device (H is built and solved there).
+    Returns dx (numpy float64)."""
+    H, g, _, _ = layout.to_dense(buf)
+    w = code_prior_weight
+    if w > 0:
+        B = layout.B
+        for k in range(layout.num_keyframes):
+            sl = slice(k * B + 6, (k + 1) * B)
+            if hasattr(H, "detach"):
+                import torch
+                H[sl, sl] += w * torch.eye(B - 6, dtype=H.dtype, device=H.device)
+                g[sl] -= w * torch.as_tensor(codes[k], dtype=g.dtype, device=g.device)
+            else:
+                H[sl, sl] += w * np.eye(B - 6)
+                g[sl] -= w * codes[k]
+    dx = damped_solve(H, g, lam, fixed)
+    return dx.detach().cpu().numpy() if hasattr(dx, "detach") else dx
+
+
 class LinearisationCache:
     """photometric_factor.cpp:296-328 GetJacobiansIfNeeded for a whole window: a pair's factors are re-evaluated only when
     pose0, pose1 or code0 moved by more than eps since the evaluation whose records are still in the record buffer.
@@ -139,44 +161,28 @@ class WindowOptimizer:
     """Levenberg-Marquardt over the poses and codes of a keyframe window.
 
     `linearise(poses, codes, pairs_to_eval) -> (window_buffer, f)` is the device pipeline (see SfmWindowProblem below for
-    the one built on SfmAligner / Window); injected so that the host logic is testable without a GPU.
+    the one built on SfmAligner / Window); injected so that the host logic is testable without a GPU.  It must return a
+    buffer that its next call does not overwrite: the loop keeps the accepted point's buffer across a rejected candidate.
 
-    `solve(buf, lam, fixed, code_prior_weight, codes) -> dx (numpy float64) | None`, when given, replaces to_dense +
-    damped_solve: the loop then never builds H, reads f from the buffer's scalar slot (plus the host prior term) and
-    counts None (not positive definite) as a rejected step.  SfmWindowProblem.solve is the device one."""
+    `solve(buf, lam, fixed, code_prior_weight, codes) -> dx (numpy float64) | None` solves the damped system of a buffer;
+    None (not positive definite) counts as a rejected step.  The default is dense_solve; SfmWindowProblem.solve is the
+    block-sparse one on the device.  f is the buffer's scalar slot plus the host prior term."""
 
     def __init__(self, layout: WindowBlocks, linearise: Callable, params: Optional[LMParams] = None,
                  solve: Optional[Callable] = None):
         self.layout = layout
         self.linearise = linearise
         self.params = params or LMParams()
-        self.solve = solve
+        self.solve = solve or functools.partial(dense_solve, layout)
         self.cache = LinearisationCache(layout.pairs, self.params.cache_eps, layout.geometric)
 
     def _energy(self, buf, codes) -> float:
-        """f of _system without H: the buffer's scalar slot (what to_dense returns) plus the prior term"""
+        """f: the buffer's scalar slot (what to_dense returns) plus the prior term"""
         f = float(buf[self.layout.offsets()[2]])
         w = self.params.code_prior_weight
         if w > 0:
             f += 0.5 * w * float((codes ** 2).sum())
         return f
-
-    def _system(self, buf, codes):
-        H, g, f, inl = self.layout.to_dense(buf)
-        w = self.params.code_prior_weight
-        if w > 0:
-            B = self.layout.B
-            for k in range(self.layout.num_keyframes):
-                sl = slice(k * B + 6, (k + 1) * B)
-                if hasattr(H, "detach"):
-                    import torch
-                    H[sl, sl] += w * torch.eye(B - 6, dtype=H.dtype, device=H.device)
-                    g[sl] -= w * torch.as_tensor(codes[k], dtype=g.dtype, device=g.device)
-                else:
-                    H[sl, sl] += w * np.eye(B - 6)
-                    g[sl] -= w * codes[k]
-            f += 0.5 * w * float((codes ** 2).sum())
-        return H, g, f
 
     def _evaluate(self, poses, codes, trace: LMTrace):
         todo = self.cache.stale(poses, codes)
@@ -192,57 +198,26 @@ class WindowOptimizer:
         trace = LMTrace()
         fixed = list(range(6)) if prm.fix_first_pose else []
         lam = prm.lambda_init
-        if self.solve is not None:
-            return self._run_solve(poses, codes, trace, fixed, lam)
-        buf = self._evaluate(poses, codes, trace)
-        H, g, f = self._system(buf, codes)
-        trace.energy.append(f)
-        for _ in range(prm.iterations):
-            dx = damped_solve(H, g, lam, fixed)
-            dxh = dx.detach().cpu().numpy() if hasattr(dx, "detach") else np.asarray(dx)
-            cand_p, cand_c = apply_update(poses, codes, dxh, self.layout.code_size)
-            cbuf = self._evaluate(cand_p, cand_c, trace)
-            cH, cg, cf = self._system(cbuf, cand_c)
-            ok = np.isfinite(cf) and cf < f
-            trace.accepted.append(bool(ok))
-            trace.lam.append(lam)
-            if ok:
-                poses, codes, H, g, f = cand_p, cand_c, cH, cg, cf
-                trace.energy.append(f)
-                lam = max(lam * prm.lambda_down, 1e-12)
-            else:
-                # H, g, f of the accepted point are still at hand; the record buffer (and with it the cache) now describes
-                # the rejected candidate, which the next candidate is compared against -- nothing to re-evaluate
-                lam = lam * prm.lambda_up
-                if lam > prm.lambda_max:
-                    break
-        return poses, codes, trace
-
-    def _run_solve(self, poses, codes, trace: LMTrace, fixed, lam):
-        """run() with the injected solve: the same schedule, on the buffer of the accepted point"""
-        prm = self.params
         buf = self._evaluate(poses, codes, trace)
         f = self._energy(buf, codes)
         trace.energy.append(f)
         for _ in range(prm.iterations):
             dx = self.solve(buf, lam, fixed, prm.code_prior_weight, codes)
             trace.lam.append(lam)
-            if dx is None:  # not positive definite at this damping: a rejected step, nothing re-linearised
-                trace.accepted.append(False)
-                lam = lam * prm.lambda_up
-                if lam > prm.lambda_max:
-                    break
-                continue
-            cand_p, cand_c = apply_update(poses, codes, np.asarray(dx, dtype=np.float64), self.layout.code_size)
-            cbuf = self._evaluate(cand_p, cand_c, trace)
-            cf = self._energy(cbuf, cand_c)
-            ok = np.isfinite(cf) and cf < f
-            trace.accepted.append(bool(ok))
+            ok = False
+            if dx is not None:  # None: not positive definite at this damping, a rejected step with nothing re-linearised
+                cand_p, cand_c = apply_update(poses, codes, np.asarray(dx, dtype=np.float64), self.layout.code_size)
+                cbuf = self._evaluate(cand_p, cand_c, trace)
+                cf = self._energy(cbuf, cand_c)
+                ok = bool(np.isfinite(cf) and cf < f)
+            trace.accepted.append(ok)
             if ok:
                 poses, codes, buf, f = cand_p, cand_c, cbuf, cf
                 trace.energy.append(f)
                 lam = max(lam * prm.lambda_down, 1e-12)
             else:
+                # buf and f of the accepted point are still at hand; the record buffer (and with it the cache) now
+                # describes the rejected candidate, which the next candidate is compared against
                 lam = lam * prm.lambda_up
                 if lam > prm.lambda_max:
                     break
@@ -274,6 +249,45 @@ class GeometricLink:
     huber_delta: float
 
 
+@dataclass
+class _FactorKind:
+    """One kind of factor of a SfmWindowProblem.  Factor j joins keyframes ends[j], is index first + j of linearise's
+    `todo` and owns rows [j * rows, (j + 1) * rows) of `records`.  items(prob, j, kf0, kf1, pose0, pose1, code0, code1)
+    are factor j's batch items (float32 poses and codes); batch(aligner, items, records=None) linearises items in one
+    launch, into `records` when given."""
+    ends: List[Tuple[int, int]]
+    first: int
+    records: object
+    rows: int
+    items: Callable
+    batch: Callable
+
+
+def _photometric_items(prob, p, a, b, pose0, pose1, code0, code1):
+    """one RunStep work item per level, the depth decode of keyframe k0 fused in"""
+    return [dict(pose0=pose0, pose1=pose1, cam=prob.cams[l], img0=a[l]["img"], img1=b[l]["img"], dpt0=a[l]["dpt"],
+                 valid0=a[l]["valid"], prx0_jac=a[l]["prx_jac"], grad1=b[l]["grad"], prx_orig=a[l]["prx_orig"], code=code0)
+            for l in range(prob.levels)]
+
+
+def _reprojection_items(prob, j, a, b, pose0, pose1, code0, code1):
+    ln = prob.links[j]
+    return [dict(pose0=pose0, pose1=pose1, code0=code0, cam=prob.cams[0], prx_orig=a[0]["prx_orig"],
+                 prx_jac=a[0]["prx_jac"], query_xy=ln.query_xy, train_xy=ln.train_xy, cauchy_delta=ln.cauchy_delta,
+                 sigma=ln.sigma)]
+
+
+def _geometric_items(prob, j, a, b, pose0, pose1, code0, code1):
+    gl = prob.geometric[j]
+    return [dict(pose0=pose0, pose1=pose1, code0=code0, code1=code1, cam=prob.cams[0], prx0_orig=a[0]["prx_orig"],
+                 prx0_jac=a[0]["prx_jac"], prx1_orig=b[0]["prx_orig"], prx1_jac=b[0]["prx_jac"],
+                 dpt_grad1=b[0]["dpt_grad"], points_xy=gl.points_xy, huber_delta=gl.huber_delta)]
+
+
+def _run_step_batch(aligner, items, records=None):
+    return aligner.RunStepBatch(aligner.make_work_items(items), records)
+
+
 class SfmWindowProblem:
     """The device pipeline of one linearisation, on SfmAligner + Window: keyframes hold their pyramids on the device
     (img, grad, prx_orig, prx_jac per level + the dpt / valid buffers the fused decode writes); `linearise` re-evaluates
@@ -292,35 +306,42 @@ class SfmWindowProblem:
                  links: Optional[Sequence[ReprojectionLink]] = None, geometric: Optional[Sequence[GeometricLink]] = None):
         import torch
         from . import _lib
-        from .aligners import Window
+        from .aligners import ReprojectionLinearizeBatch, SparseGeometricLinearizeBatch, Window
         self.al = aligner
         self.cams = list(cams)
         self.kf = keyframes          # kf[k][l] = dict(img, grad, prx_orig, prx_jac, dpt, valid) of device tensors
         self.links = list(links or [])
-        self.num_photometric = len(pairs)
+        P = len(pairs)
         self.pairs = [tuple(p) for p in pairs] + [(int(ln.k0), int(ln.k1)) for ln in self.links]
         self.levels = len(self.cams)
         item_pair, sizes = [], []
-        for p in range(self.num_photometric):
+        for p in range(P):
             for l in range(self.levels):
                 item_pair.append(p)
                 t = self.kf[self.pairs[p][0]][l]["img"]
                 sizes.append((int(t.shape[1]), int(t.shape[0])))
-        self.photometric_items = len(item_pair)
         for j in range(len(self.links)):
-            item_pair.append(self.num_photometric + j)
+            item_pair.append(P + j)
             sizes.append((0, 0))  # unscaled record: b^T b enters f as it is
         self.geometric = list(geometric or [])
         for gl in self.geometric:
             if "dpt_grad" not in self.kf[gl.k1][0]:
                 raise ValueError(f"keyframe {gl.k1} is k1 of a geometric link but carries no level-0 dpt_grad")
-        self.window = Window(aligner, len(keyframes), self.pairs, item_pair, sizes,
-                             [(int(gl.k0), int(gl.k1)) for gl in self.geometric])
+        geo_ends = [(int(gl.k0), int(gl.k1)) for gl in self.geometric]
+        self.window = Window(aligner, len(keyframes), self.pairs, item_pair, sizes, geo_ends)
         self.layout = self.window.layout
         dev = self.kf[0][0]["img"].device
         self.records = torch.zeros((len(item_pair), _lib.record_floats(aligner.CS)), dtype=torch.float32, device=dev)
         self.geo_records = torch.zeros((len(self.geometric), _lib.geo_record_floats(aligner.CS)), dtype=torch.float32,
                                        device=dev) if self.geometric else None
+        L = P * self.levels
+        self._kinds = {  # in `todo` numbering: the photometric pairs, then the reprojection links, then the geometric links
+            "photometric": _FactorKind(self.pairs[:P], 0, self.records[:L], self.levels, _photometric_items,
+                                       _run_step_batch),
+            "reprojection": _FactorKind(self.pairs[P:], P, self.records[L:], 1, _reprojection_items,
+                                        ReprojectionLinearizeBatch),
+            "geometric": _FactorKind(geo_ends, len(self.pairs), self.geo_records, 1, _geometric_items,
+                                     SparseGeometricLinearizeBatch)}
         self.allreduce = allreduce
         self._solvers = {}  # fixed variables -> WindowSolver, created on first use
 
@@ -341,72 +362,28 @@ class SfmWindowProblem:
             return None
         return host[:8 * n].view(np.float64).copy()
 
-    def _items(self, poses, codes, todo):
-        items = []
-        for p in todo:
-            k0, k1 = self.pairs[p]
-            for l in range(self.levels):
-                a, b = self.kf[k0][l], self.kf[k1][l]
-                items.append(dict(pose0=poses[k0].astype(np.float32), pose1=poses[k1].astype(np.float32), cam=self.cams[l],
-                                  img0=a["img"], img1=b["img"], dpt0=a["dpt"], valid0=a["valid"], prx0_jac=a["prx_jac"],
-                                  grad1=b["grad"], prx_orig=a["prx_orig"], code=codes[k0].astype(np.float32)))
-        return items
-
-    def _link_items(self, poses, codes, todo):
+    def _items(self, kind, poses, codes, todo):
+        """the batch items of the factors `todo` of one kind (numbered within the kind) at these poses and codes"""
+        kd = self._kinds[kind]
         items = []
         for j in todo:
-            ln = self.links[j]
-            a = self.kf[ln.k0][0]
-            items.append(dict(pose0=poses[ln.k0].astype(np.float32), pose1=poses[ln.k1].astype(np.float32),
-                              code0=codes[ln.k0].astype(np.float32), cam=self.cams[0], prx_orig=a["prx_orig"],
-                              prx_jac=a["prx_jac"], query_xy=ln.query_xy, train_xy=ln.train_xy,
-                              cauchy_delta=ln.cauchy_delta, sigma=ln.sigma))
-        return items
-
-    def _geo_items(self, poses, codes, todo):
-        items = []
-        for j in todo:
-            gl = self.geometric[j]
-            a, b = self.kf[gl.k0][0], self.kf[gl.k1][0]
-            items.append(dict(pose0=poses[gl.k0].astype(np.float32), pose1=poses[gl.k1].astype(np.float32),
-                              code0=codes[gl.k0].astype(np.float32), code1=codes[gl.k1].astype(np.float32),
-                              cam=self.cams[0], prx0_orig=a["prx_orig"], prx0_jac=a["prx_jac"], prx1_orig=b["prx_orig"],
-                              prx1_jac=b["prx_jac"], dpt_grad1=b["dpt_grad"], points_xy=gl.points_xy,
-                              huber_delta=gl.huber_delta))
+            k0, k1 = kd.ends[j]
+            items += kd.items(self, j, self.kf[k0], self.kf[k1], poses[k0].astype(np.float32),
+                              poses[k1].astype(np.float32), codes[k0].astype(np.float32), codes[k1].astype(np.float32))
         return items
 
     def linearise(self, poses, codes, todo):
         import torch
-        from .aligners import ReprojectionLinearizeBatch, SparseGeometricLinearizeBatch
-        P = len(self.pairs)
-        geo = [p - P for p in todo if p >= P]
-        todo = [p for p in todo if p < P]
-        photo = [p for p in todo if p < self.num_photometric]
-        links = [p - self.num_photometric for p in todo if p >= self.num_photometric]
-        if photo:
-            work = self.al.make_work_items(self._items(poses, codes, photo))
-            if len(photo) == self.num_photometric:
-                self.al.RunStepBatch(work, self.records[:self.photometric_items])
-            else:
-                part = self.al.RunStepBatch(work)
-                rows = torch.as_tensor([p * self.levels + l for p in photo for l in range(self.levels)],
-                                       device=self.records.device)
-                self.records.index_copy_(0, rows, part)
-        if links:
-            items = self._link_items(poses, codes, links)
-            if len(links) == len(self.links):
-                ReprojectionLinearizeBatch(self.al, items, self.records[self.photometric_items:])
-            else:
-                part = ReprojectionLinearizeBatch(self.al, items)
-                rows = torch.as_tensor([self.photometric_items + j for j in links], device=self.records.device)
-                self.records.index_copy_(0, rows, part)
-        if geo:
-            items = self._geo_items(poses, codes, geo)
-            if len(geo) == len(self.geometric):
-                SparseGeometricLinearizeBatch(self.al, items, self.geo_records)
-            else:
-                part = SparseGeometricLinearizeBatch(self.al, items)
-                self.geo_records.index_copy_(0, torch.as_tensor(geo, device=self.geo_records.device), part)
+        for kind, kd in self._kinds.items():
+            sel = [p - kd.first for p in todo if kd.first <= p < kd.first + len(kd.ends)]
+            if not sel:
+                continue
+            items = self._items(kind, poses, codes, sel)
+            if len(sel) == len(kd.ends):  # the whole kind: straight into its records
+                kd.batch(self.al, items, kd.records)
+            else:  # some factors: one batch of their own, copied to their rows
+                rows = torch.as_tensor([j * kd.rows + r for j in sel for r in range(kd.rows)], device=kd.records.device)
+                kd.records.index_copy_(0, rows, kd.batch(self.al, items))
         buf = self.window.assemble(self.records, geo_records=self.geo_records)
         if self.allreduce is not None:
             self.allreduce(buf)

@@ -14,7 +14,7 @@ import pytest
 
 from deepfactors_b200 import factors, se3, synth
 from system_accuracy import Reference, assert_system_close
-from test_oracle_ref import _geometric_scene
+from test_oracle_ref import _geometric_scene, _keypoint_matches
 
 pytestmark = pytest.mark.gpu
 
@@ -280,6 +280,10 @@ def test_rejected_calls_name_the_item_and_write_nothing(torch_mod, monkeypatch):
     for bad in (dict(code0=single["code0"][:cs - 1]), dict(code1=single["code1"][:cs - 1])):
         with pytest.raises(ValueError):
             SparseGeometricLinearize(al, **{**single, **bad})
+    # records the kernel would write float32 rows into: big enough, but float64 or on the host
+    for wrong in (rec.double(), rec.cpu()):
+        with pytest.raises(ValueError):
+            aligners.SparseGeometricLinearizeBatch(al, [single], wrong)
     monkeypatch.undo()
     torch.cuda.synchronize()
     assert (rec.cpu().numpy() == SENTINEL).all()
@@ -321,7 +325,7 @@ def _window_poses():
                      se3.make_pose([-0.003, 0.002, 0.004], [-0.01, 0.012, -0.03], np.float64)])
 
 
-def test_window_with_geometric_links_on_device_equals_host_mirror(torch_mod):
+def test_geometric_link_window_on_device_equals_host_mirror(torch_mod):
     import torch
     from deepfactors_b200.aligners import SfmAligner, SparseGeometricLinearizeBatch
     from deepfactors_b200.window_opt import SfmWindowProblem
@@ -349,7 +353,7 @@ def test_window_with_geometric_links_on_device_equals_host_mirror(torch_mod):
     assert buf[o_t + 1] == float(inl.sum())  # links add no inliers
     assert abs(buf[o_t] - want[o_t]) <= 2e-6 * want[o_t]
     # the link records are those of SparseGeometricLinearizeBatch for the same arguments
-    direct = SparseGeometricLinearizeBatch(al, prob._geo_items(poses, codes, [0, 1, 2])).cpu().numpy()
+    direct = SparseGeometricLinearizeBatch(al, prob._items("geometric", poses, codes, [0, 1, 2])).cpu().numpy()
     assert np.array_equal(direct, grec)
     # bitwise reproducible, and a partial re-linearisation (one link) lands in the same place
     assert np.array_equal(prob.linearise(poses, codes, everything)[0].cpu().numpy(), buf)
@@ -372,6 +376,61 @@ def test_window_with_geometric_links_on_device_equals_host_mirror(torch_mod):
         fr += float(gres[l])
     assert np.abs(Hd - Hr).max() <= 2e-6 * np.abs(Hr).max()
     assert np.abs(gd - gr).max() <= 2e-6 * np.abs(gr).max() and abs(f - fr) <= 1e-5 * abs(fr)
+
+
+def test_window_relinearises_any_subset_of_its_factors_in_place(torch_mod):
+    """photometric pairs, reprojection links and geometric links in one window: with the records of the factors in
+    `todo` spoilt first, re-linearising any one factor, or every factor of one kind, at the same poses and codes writes
+    each record back to its own rows and leaves every other row alone.  Photometric pair p owns records rows
+    [p * levels, (p + 1) * levels), reprojection link j row len(pairs) * levels + j, geometric link j geo_records row j.
+    A link's record does not depend on its batch, and a batch of all photometric pairs is the one of the full
+    linearisation, so those come back bit for bit.  A batch of some photometric pairs sums their pixels in another
+    order; its records come back within 1e-5 of their largest entry, and another pair's record would not."""
+    import torch
+    from deepfactors_b200.aligners import SfmAligner
+    from deepfactors_b200.window_opt import ReprojectionLink, SfmWindowProblem
+    cs, levels = 8, 2
+    base, cams, keyframes = _window_scene(torch, cs, levels)
+    al = SfmAligner(cs)
+    L = base.levels[0]
+    ident = se3.identity(np.float64)
+    links = [ReprojectionLink(0, 2, *_keypoint_matches(L.cam, ident, ident, L.prx_orig, n=400, seed=31), 3.0, 1.5),
+             ReprojectionLink(2, 1, *_keypoint_matches(L.cam, ident, ident, L.prx_orig, n=300, seed=32), 2.0, 1.0)]
+    pairs = [(0, 1), (1, 2), (1, 0)]
+    geo = _geo_links(base)
+    prob = SfmWindowProblem(al, cams, keyframes, pairs, links=links, geometric=geo)
+    poses = _window_poses()
+    codes = np.random.default_rng(6).standard_normal((3, cs)) * 0.05
+    P, R, G = len(pairs), len(links), len(geo)
+    full = prob.linearise(poses, codes, list(range(P + R + G)))[0].cpu().numpy()
+    rec, grec = prob.records.cpu().numpy(), prob.geo_records.cpu().numpy()
+    assert np.isfinite(rec).all() and np.isfinite(grec).all()
+    assert np.abs(rec).max(1).min() > 0 and np.abs(grec).max(1).min() > 0
+    assert min(np.abs(rec[i] - rec[j]).max() / np.abs(rec[i]).max() for i in range(P * levels) for j in range(i)) > 1e-4
+
+    def rows(p):  # (records rows, geo_records rows) of factor p in `todo` numbering
+        if p < P:
+            return list(range(p * levels, (p + 1) * levels)), []
+        return ([P * levels + p - P], []) if p < P + R else ([], [p - P - R])
+
+    kinds = [list(range(P)), list(range(P, P + R)), list(range(P + R, P + R + G))]
+    for todo in [[p] for p in range(P + R + G)] + kinds:
+        spoilt = [r for p in todo for r in rows(p)[0]], [r for p in todo for r in rows(p)[1]]
+        r0, g0 = rec.copy(), grec.copy()
+        r0[spoilt[0]], g0[spoilt[1]] = np.nan, np.nan
+        prob.records.copy_(torch.from_numpy(r0))
+        prob.geo_records.copy_(torch.from_numpy(g0))
+        buf = prob.linearise(poses, codes, todo)[0].cpu().numpy()
+        got, ggot = prob.records.cpu().numpy(), prob.geo_records.cpu().numpy()
+        assert np.array_equal(ggot, grec), todo
+        if 0 < len([p for p in todo if p < P]) < P:
+            assert np.isfinite(got).all(), todo
+            assert (np.abs(got - rec).max(1) <= 1e-5 * np.abs(rec).max(1)).all(), todo
+            kept = np.setdiff1d(np.arange(len(rec)), spoilt[0])
+            assert np.array_equal(got[kept], rec[kept]), todo
+            assert np.abs(buf - full).max() <= 1e-5 * np.abs(full).max(), todo
+        else:
+            assert np.array_equal(got, rec) and np.array_equal(buf, full), todo
 
 
 def test_window_entry_points_reject_bad_links(torch_mod):

@@ -198,6 +198,10 @@ def test_rejected_calls_name_the_item_and_write_nothing(torch_mod, monkeypatch):
     for bad in (dict(code0=single["code0"][:cs - 1]), dict(train_xy=single["train_xy"][:-1])):
         with pytest.raises(ValueError):
             ReprojectionLinearize(al, **{**single, **bad})
+    # records the kernel would write float32 rows into: big enough, but float64 or on the host
+    for wrong in (rec.double(), rec.cpu()):
+        with pytest.raises(ValueError):
+            aligners.ReprojectionLinearizeBatch(al, [single], wrong)
     monkeypatch.undo()
     torch.cuda.synchronize()
     assert (rec.cpu().numpy() == SENTINEL).all()
@@ -228,7 +232,7 @@ def _links(base, delta=10.0, sigma=1.0):
     return [ReprojectionLink(0, 2, q02, t02, delta, sigma), ReprojectionLink(2, 0, q20, t20, delta, sigma)]
 
 
-def test_window_with_links_on_device_equals_host_mirror(torch_mod):
+def test_reprojection_link_window_on_device_equals_host_mirror(torch_mod):
     import torch
     from deepfactors_b200.aligners import SfmAligner
     from deepfactors_b200.window_opt import SfmWindowProblem
@@ -254,7 +258,7 @@ def test_window_with_links_on_device_equals_host_mirror(torch_mod):
     assert res[-2:].min() > 0 and abs(buf[o_t] - want[o_t]) <= 1e-6 * want[o_t]
     # the link records are those of ReprojectionLinearizeBatch for the same arguments
     from deepfactors_b200.aligners import ReprojectionLinearizeBatch
-    direct = ReprojectionLinearizeBatch(al, prob._link_items(poses, codes, [0, 1])).cpu().numpy()
+    direct = ReprojectionLinearizeBatch(al, prob._items("reprojection", poses, codes, [0, 1])).cpu().numpy()
     assert np.array_equal(direct, rec[-2:])
     # bitwise reproducible, and a partial re-linearisation (one link) lands in the same place
     assert np.array_equal(prob.linearise(poses, codes, everything)[0].cpu().numpy(), buf)

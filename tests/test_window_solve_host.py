@@ -65,12 +65,12 @@ def test_injected_solve_reproduces_the_default_trace_exactly():
         assert any(t0.accepted) and len(t0.energy) > 2
 
 
-def test_energy_from_the_buffer_is_to_dense_f_plus_the_prior():
+def test_energy_from_the_buffer_is_to_dense_f_plus_the_code_prior():
     wb, lin, poses, codes, _ = _problem()
     buf, _ = lin(poses, codes, [0, 1, 2])
     for w in (0.0, 0.5):
         opt = WindowOptimizer(wb, lin, LMParams(code_prior_weight=w))
-        assert opt._energy(buf, codes) == opt._system(buf, codes)[2]
+        assert opt._energy(buf, codes) == wb.to_dense(buf)[2] + 0.5 * w * float((codes ** 2).sum())
     assert WindowOptimizer(wb, lin)._energy(buf, codes) == wb.to_dense(buf)[2]
 
 
