@@ -570,9 +570,11 @@ DfkStatus run_batch(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_si
   if (!sfm_fp32_supported(code_size) && !wide)
     return fail(h, DFK_ERR_UNSUPPORTED,
                 "[SfmAligner::RunStep] no kernel instantiated for code size " + std::to_string(code_size));
-  bool tc = (h->gram_mode == DFK_GRAM_TF32X3) || (h->gram_mode == DFK_GRAM_AUTO && sfm_tc_supported(code_size));
+  const bool tc_ok = sfm_tc_supported(code_size) || sfm_tc_wide_supported(code_size);
+  bool tc = (h->gram_mode == DFK_GRAM_TF32X3) || (h->gram_mode == DFK_GRAM_AUTO && tc_ok);
   if (tc) {
-    // the tensor-core kernel gathers grad1 with 8-byte loads; odd layouts go to the fp32 kernel (AUTO) or fail (forced)
+    // the tensor-core kernels gather grad1 with 8-byte loads; odd layouts go to the fp32 / wide kernel (AUTO) or fail
+    // (forced)
     bool grads_ok = true;
     for (int i = 0; i < n && grads_ok; ++i)
       grads_ok = items[i].grad1.ptr && aligned(items[i].grad1.ptr, 8) && (items[i].grad1.pitch_bytes % 8 == 0);
@@ -582,27 +584,27 @@ DfkStatus run_batch(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_si
       tc = false;
     }
   }
-  if (tc && !sfm_tc_supported(code_size))
+  if (tc && !tc_ok)
     return fail(h, DFK_ERR_UNSUPPORTED,
                 "[SfmAligner::RunStep] tensor-core Gram path is not instantiated for code size " +
                     std::to_string(code_size));
   DeviceGuard guard(h->device);
   SfmLaunchPlan plan;
-  const int tile_px = tc ? kTcTilePixels : (wide ? sfm_wide_tile_pixels(code_size) : kTilePixels);
+  const int tile_px = tc ? sfm_tc_tile_pixels(code_size) : (wide ? sfm_wide_tile_pixels(code_size) : kTilePixels);
   bool any_fused = false;
   for (int i = 0; i < n; ++i) any_fused = any_fused || items[i].code != nullptr;
   if (any_fused) {
     DFK_CUDA(h, h->codes_dev.ensure((size_t)n * code_size), "[SfmAligner::RunStep] scratch allocation failed");
     h->codes_host.assign((size_t)n * code_size, 0.0f);
   }
-  const int ctas_per_sm = tc ? kTcCtasPerSm : (wide ? 1 : sfm_fp32_ctas_per_sm(code_size));
+  const int ctas_per_sm = tc ? sfm_tc_ctas_per_sm(code_size) : (wide ? 1 : sfm_fp32_ctas_per_sm(code_size));
   const int sms = (h->sm_limit > 0 && h->sm_limit < h->num_sms) ? h->sm_limit : h->num_sms;
   DFK_TRY(build_items(h, items, n, code_size, tile_px, ctas_per_sm * sms, h->codes_dev.ptr, &plan));
   if (any_fused)
     DFK_CUDA(h, cudaMemcpyAsync(h->codes_dev.ptr, h->codes_host.data(), sizeof(float) * (size_t)n * code_size,
                                 cudaMemcpyHostToDevice, h->stream),
              "[SfmAligner::RunStep] code upload failed");
-  const size_t pfloats = tc ? (size_t)kTcPartialFloats : sfm_partial_floats(code_size);
+  const size_t pfloats = tc ? sfm_tc_partial_floats(code_size) : sfm_partial_floats(code_size);
   DFK_CUDA(h, h->items_dev.ensure((size_t)n), "[SfmAligner::RunStep] scratch allocation failed");
   DFK_CUDA(h, h->partials_dev.ensure((size_t)plan.num_partials * pfloats), "[SfmAligner::RunStep] scratch allocation failed");
   SfmItemDev* items_dev = h->items_dev.ptr;
@@ -616,7 +618,10 @@ DfkStatus run_batch(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_si
   }
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   if (h->profiling) DFK_TRY(profile_events(h, &ev0, &ev1));
-  if (tc) {
+  if (tc && wide) {
+    DFK_CUDA(h, launch_sfm_tc_wide(code_size, items_dev, plan, partials_dev, h->stream, ev0, ev1),
+             "[SfmAligner::RunStep] kernel launch failed");
+  } else if (tc) {
     DFK_CUDA(h, launch_sfm_tc(items_dev, plan, partials_dev, h->stream, ev0, ev1),
              "[SfmAligner::RunStep] kernel launch failed");
   } else if (wide) {

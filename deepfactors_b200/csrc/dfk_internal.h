@@ -73,16 +73,41 @@ struct SfmCfg {
 };
 
 constexpr int kTilePixels = 256;    // fp32 kernel
-constexpr int kTcTilePixels = 128;  // tensor-core kernel
-// resident CTAs (one warpgroup and ~47 KB of shared memory each) per SM of the tensor-core kernel
-constexpr int kTcCtasPerSm = 4;
-// tensor-core partial: the kernel's 64 x 56 accumulator D = A B^T, A rows = code-l 0-23 | code-h 0-31 | pose-h (7 + 1),
-// B columns = code-h 0-31 | pose-h (7 + 1) | code-l 24-31 | pose-l (7 + 1); see dfk_sfm_tc.cu for what each block holds
-constexpr int kTcRows = 64;
-constexpr int kTcCols = 56;
-// stored column-major ([column][row]); rows 0-23 of columns 40-55 (the dropped l*l terms) are never written or read
+
+// Tensor-core partial of code size C (32: dfk_sfm_tc.cu; 64, 128: dfk_sfm_tc_wide.cu).  Features f = code 0..C-1 |
+// pose/residual C..C+6 | zero C+7 (F = C + 8), each split into h (tf32) and l.  The first S = C - 8 code features have
+// their l rows in A, the last 8 code features and the pose/zero group in B:
+//   A rows    = code-l 0..S-1 | h 0..F-1                        (M = 2C)
+//   B columns = h 0..F-1 | code-l S..C-1 | pose-l (7 + zero)    (N = C + 24)
+// The accumulator D = A B^T is stored column-major ([column][row]), then the inlier count:
+//   HH[i][j] = D[S + i][j];   LH[i][j] = D[i][j] for i < S,  D[S + j][16 + i] for i >= S.
+// Rows 0..S-1 of columns F..N-1 hold only l*l terms and are never written or read.
+template <int C>
+struct TcCfg {
+  static constexpr int S = C - 8;
+  static constexpr int F = C + 8;
+  static constexpr int ROWS = 2 * C;
+  static constexpr int COLS = C + 24;
+  static constexpr int PARTIAL_FLOATS = ROWS * COLS + 8;
+  static constexpr int INLIERS = ROWS * COLS;  // offset of the inlier count (u32)
+  __host__ __device__ static constexpr int hh(int i, int j) { return j * ROWS + S + i; }
+  __host__ __device__ static constexpr int lh(int i, int j) { return i < S ? j * ROWS + i : (16 + i) * ROWS + S + j; }
+};
+
+// tiles of 128 pixels: K of the wgmma chain per tile
+constexpr int sfm_tc_tile_pixels(int) { return 128; }
+// resident CTAs per SM: C = 32 one warpgroup and ~47 KB of shared memory; C = 64 one warpgroup, ~85 KB;
+// C = 128 two warpgroups, ~163 KB
+constexpr int sfm_tc_ctas_per_sm(int code_size) { return code_size <= 32 ? 4 : (code_size <= 64 ? 2 : 1); }
+constexpr size_t sfm_tc_partial_floats(int code_size) { return (size_t)(2 * code_size) * (code_size + 24) + 8; }
+
+// the C = 32 kernel's names for the above
+constexpr int kTcTilePixels = sfm_tc_tile_pixels(32);
+constexpr int kTcCtasPerSm = sfm_tc_ctas_per_sm(32);
+constexpr int kTcRows = TcCfg<32>::ROWS;
+constexpr int kTcCols = TcCfg<32>::COLS;
 constexpr int kTcRowsPad = kTcRows;
-constexpr int kTcPartialFloats = kTcRowsPad * kTcCols + 8;
+constexpr int kTcPartialFloats = TcCfg<32>::PARTIAL_FLOATS;
 
 struct SfmLaunchPlan {
   int num_items = 0;
@@ -105,10 +130,14 @@ bool sfm_wide_supported(int code_size);
 cudaError_t launch_sfm_wide(int code_size, const SfmItemDev* items_dev, const SfmLaunchPlan& plan,
                             float* partials_dev, cudaStream_t stream, cudaEvent_t ev_start = nullptr,
                             cudaEvent_t ev_stop = nullptr);
-// dfk_sfm_tc.cu
+// dfk_sfm_tc.cu (C = 32) and dfk_sfm_tc_wide.cu (C = 64, 128)
 bool sfm_tc_supported(int code_size);
 cudaError_t launch_sfm_tc(const SfmItemDev* items_dev, const SfmLaunchPlan& plan, float* partials_dev,
                           cudaStream_t stream, cudaEvent_t ev_start = nullptr, cudaEvent_t ev_stop = nullptr);
+bool sfm_tc_wide_supported(int code_size);
+cudaError_t launch_sfm_tc_wide(int code_size, const SfmItemDev* items_dev, const SfmLaunchPlan& plan,
+                               float* partials_dev, cudaStream_t stream, cudaEvent_t ev_start = nullptr,
+                               cudaEvent_t ev_stop = nullptr);
 size_t sfm_partial_floats(int code_size);
 // resident CTAs per SM of the fp32 kernel: at C = 8 a CTA is 11 warps and ~60 KB of shared memory, two fit (the front-end
 // is latency-bound, so the second CTA nearly doubles the throughput); from C = 16 on the register budget allows one

@@ -14,7 +14,7 @@
 //
 // Two partial formats:
 //   fp32 kernel : G itself, row-major NFP x NFP (features: code 0..C-1, a C..C+5, r C+6), upper blocks valid
-//   tensor core : D = A x B^T over split-tf32 h / l rows (kTcRows x kTcCols, stored column-major);  G = HH + LH + LH^T
+//   tensor core : D = A x B^T over split-tf32 h / l rows (TcCfg<C>, stored column-major);  G = HH + LH + LH^T
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -29,11 +29,6 @@ constexpr int kFinUnroll = 4;
 
 __device__ __forceinline__ int packed_index(int i, int j, int NP) { return i * NP - (i * (i - 1)) / 2 + (j - i); }
 
-// tensor-core partial (C = 32, column-major D of dfk_sfm_tc.cu), features f = code 0-31 | pose/residual 32-39:
-//   HH[i][j] = D[24 + i][j];  LH[i][j] = D[i][j] for i < 24, D[24 + j][16 + i] for i >= 24
-__device__ __forceinline__ int tc_hh(int i, int j) { return j * kTcRowsPad + 24 + i; }
-__device__ __forceinline__ int tc_lh(int i, int j) { return i < 24 ? j * kTcRowsPad + i : (16 + i) * kTcRowsPad + 24 + j; }
-
 template <int C, bool TC>
 __global__ void __launch_bounds__(kFinWarps * 32)
 sfm_finalize_kernel(const SfmItemDev* __restrict__ items, const float* __restrict__ partials,
@@ -46,8 +41,9 @@ sfm_finalize_kernel(const SfmItemDev* __restrict__ items, const float* __restric
   constexpr int REC = NH + NP + 2;
   constexpr int NE = (C + 7 > 49) ? (C + 7) : 49;  // entries per unit (code row: <= C+7, pose unit: 49)
   constexpr int EPL = (NE + 31) / 32;              // entries per lane
-  constexpr int PSTRIDE = TC ? kTcPartialFloats : Cfg::PARTIAL_FLOATS;
-  constexpr int INL_OFF = TC ? kTcRowsPad * kTcCols : NFP * NFP;
+  using Tc = TcCfg<C>;
+  constexpr int PSTRIDE = TC ? Tc::PARTIAL_FLOATS : Cfg::PARTIAL_FLOATS;
+  constexpr int INL_OFF = TC ? Tc::INLIERS : NFP * NFP;
   constexpr int NOFF = TC ? 3 : 1;
   __shared__ float red[kFinWarps][EPL * 32];
   __shared__ unsigned int red_inl[kFinWarps];
@@ -84,9 +80,9 @@ sfm_finalize_kernel(const SfmItemDev* __restrict__ items, const float* __restric
       fj = 0;
     }
     if constexpr (TC) {
-      off[q][0] = tc_hh(fi, fj);  // HH[i][j]
-      off[q][1] = tc_lh(fi, fj);  // LH[i][j]
-      off[q][2] = tc_lh(fj, fi);  // LH[j][i]
+      off[q][0] = Tc::hh(fi, fj);  // HH[i][j]
+      off[q][1] = Tc::lh(fi, fj);  // LH[i][j]
+      off[q][2] = Tc::lh(fj, fi);  // LH[j][i]
     } else {
       off[q][0] = fi * NFP + fj;
     }
@@ -225,8 +221,12 @@ cudaError_t launch_sfm_finalize(int code_size, bool tc, const SfmItemDev* items_
                                 const float* partials_dev, float* records_dev, cudaStream_t stream)
 {
   if (tc) {
-    if (code_size != 32) return cudaErrorInvalidValue;
-    return launch_fin<32, true>(items_dev, num_items, partials_dev, records_dev, stream);
+    switch (code_size) {
+      case 32: return launch_fin<32, true>(items_dev, num_items, partials_dev, records_dev, stream);
+      case 64: return launch_fin<64, true>(items_dev, num_items, partials_dev, records_dev, stream);
+      case 128: return launch_fin<128, true>(items_dev, num_items, partials_dev, records_dev, stream);
+      default: return cudaErrorInvalidValue;
+    }
   }
   switch (code_size) {
     case 8: return launch_fin<8, false>(items_dev, num_items, partials_dev, records_dev, stream);

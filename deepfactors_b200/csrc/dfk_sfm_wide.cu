@@ -15,8 +15,9 @@
 //     pixels so two stages fit.  This file writes the reduced row m = w * [ e*jc (C) | a (6) | diff ]
 //     pixel-major and compacted into M[pixel][NFP].
 //   * Gram threads: for every valid pixel of their split, 2+2 LDS.128 and 64 FMA.
-// This is the first correct path for these sizes: CUDA-core bound (9.8 kFMA per pixel at C = 128), the
-// tensor-core formulation of dfk_sfm_tc.cu is the follow-up.
+// CUDA-core bound (9.8 kFMA per pixel at C = 128).  DFK_GRAM_AUTO runs these sizes on the tensor-core kernel
+// (dfk_sfm_tc_wide.cu); this one is the DFK_GRAM_FP32 engine and AUTO's engine for grad1 rows the tensor-core
+// kernel cannot gather (not 8-byte aligned).
 #include <cuda_runtime.h>
 #include <stdint.h>
 

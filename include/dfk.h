@@ -91,8 +91,10 @@ typedef struct {
 /* How the (6+C)x(6+C) Gauss-Newton Gram is accumulated.
  *   DFK_GRAM_FP32     CUDA-core FFMA, fp32 products and sums (any supported code size)
  *   DFK_GRAM_TF32X3   wgmma tensor cores, split-precision tf32 (hi*hi + lo*hi + hi*lo),
- *                     fp32 accumulate in registers; code size >= 32 only
- *   DFK_GRAM_AUTO     tensor cores where available for the code size, else FP32 */
+ *                     fp32 accumulate in registers; code sizes 32, 64 and 128, grad1 rows
+ *                     8-byte aligned (else DFK_ERR_UNSUPPORTED)
+ *   DFK_GRAM_AUTO     tensor cores for code sizes 32, 64 and 128, else FP32; FP32 also for a
+ *                     batch whose grad1 rows are not 8-byte aligned */
 typedef enum { DFK_GRAM_AUTO = 0, DFK_GRAM_FP32 = 1, DFK_GRAM_TF32X3 = 2 } DfkGramMode;
 
 /* ------------------------------------------------------------------ lifetime / config */

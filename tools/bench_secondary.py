@@ -115,8 +115,10 @@ def main():
     batched(160, 120, 8, 256)
     batched(640, 480, 32, 8, "fp32")
     batched(640, 480, 32, 8, "tf32x3")
-    batched(640, 480, 64, 4)
-    batched(640, 480, 128, 3)
+    batched(640, 480, 64, 4, "fp32")
+    batched(640, 480, 64, 4, "tf32x3")
+    batched(640, 480, 128, 3, "fp32")
+    batched(640, 480, 128, 3, "tf32x3")
 
     # ---- synchronous per-call API at 640x480 ---------------------------------------------------------------
     pair = synth.make_pair(640, 480, 32, 1, seed=7)
