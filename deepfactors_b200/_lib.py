@@ -125,6 +125,12 @@ SYMBOLS = {
     "dfk_window_create_geometric": (C.c_int, [_H, C.POINTER(DfkWindowDesc), C.c_int, C.POINTER(C.c_int32),
                                               C.POINTER(C.c_int32), C.POINTER(C.c_void_p)]),
     "dfk_window_assemble_geometric": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dfk_window_create_frames": (C.c_int, [_H, C.POINTER(DfkWindowDesc), C.c_int, C.POINTER(C.c_int32),
+                                           C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_void_p)]),
+    "dfk_window_marginalize_frames": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.c_void_p,
+                                                C.c_void_p]),
+    "dfk_window_add_priors": (C.c_int, [_H, C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p,
+                                        C.c_void_p]),
     "dfk_window_solver_create": (C.c_int, [_H, C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_void_p)]),
     "dfk_window_solver_destroy": (C.c_int, [_H, C.c_void_p]),
     "dfk_window_solver_tiles": (C.c_int, [_H, C.c_void_p, C.POINTER(C.c_size_t)]),
@@ -184,3 +190,9 @@ def geo_record_floats(code_size: int) -> int:
     """DFK_GEO_RECORD_FLOATS: a sparse geometric record over [pose0 | pose1 | code0 | code1]"""
     npar = 12 + 2 * code_size
     return npar * (npar + 1) // 2 + npar + 2
+
+
+def prior_doubles(code_size: int) -> int:
+    """DFK_PRIOR_DOUBLES: a linear keyframe prior [G (B x B) | g (B) | f0], B = 6 + code_size"""
+    b = 6 + code_size
+    return b * b + b + 1

@@ -432,13 +432,16 @@ class Window:
     sign flip and residual rescale (sources/core/gtsam/photometric_factor.cpp:105-161,275-282) summed over the window's
     factors (one per pair and level, core/mapping/df_work.cpp:211-225).  `layout` (factors.WindowBlocks) describes the
     buffer; it is the one buffer a multi-GPU Gauss-Newton step all-reduces.  `geometric` lists the window's sparse
-    geometric links (k0, k1), one record each (SparseGeometricLinearizeBatch); their blocks follow the scalars."""
+    geometric links (k0, k1), one record each (SparseGeometricLinearizeBatch); their blocks follow the scalars.
+    `num_frames` tracked frames (pose-only variables, dfk_window_create_frames): a pair (k, K + f) is frame f's one
+    photometric pair; the frames' blocks follow the links'."""
 
-    def __init__(self, aligner: "SfmAligner", num_keyframes: int, pairs, item_pair, item_sizes, geometric=()):
+    def __init__(self, aligner: "SfmAligner", num_keyframes: int, pairs, item_pair, item_sizes, geometric=(),
+                 num_frames: int = 0):
         from .factors import WindowBlocks
         self._al = aligner
         self.layout = WindowBlocks(int(num_keyframes), aligner.CS, [tuple(map(int, p)) for p in pairs],
-                                   [tuple(map(int, p)) for p in geometric])
+                                   [tuple(map(int, p)) for p in geometric], int(num_frames))
         k0 = np.ascontiguousarray([p[0] for p in self.layout.pairs], dtype=np.int32)
         k1 = np.ascontiguousarray([p[1] for p in self.layout.pairs], dtype=np.int32)
         ip = np.ascontiguousarray(item_pair, dtype=np.int32)
@@ -452,9 +455,10 @@ class Window:
         g1 = np.ascontiguousarray([p[1] for p in self.layout.geometric], dtype=np.int32)
         L = len(g0)
         self.w = C.c_void_p()
-        check(aligner.handle, lib().dfk_window_create_geometric(aligner.handle, C.byref(desc), L,
-                                                                g0.ctypes.data_as(I32) if L else None,
-                                                                g1.ctypes.data_as(I32) if L else None, C.byref(self.w)))
+        check(aligner.handle, lib().dfk_window_create_frames(aligner.handle, C.byref(desc), L,
+                                                             g0.ctypes.data_as(I32) if L else None,
+                                                             g1.ctypes.data_as(I32) if L else None, int(num_frames),
+                                                             C.byref(self.w)))
         self.num_items = len(ip)
         self.floats = int(lib().dfk_window_floats(self.w))
         assert self.floats == self.layout.floats
@@ -480,6 +484,44 @@ class Window:
                                                         C.c_void_p(out.data_ptr())))
         return out
 
+    def marginalize_frames(self, records: torch.Tensor, frames, priors: torch.Tensor | None = None,
+                           info: torch.Tensor | None = None):
+        """dfk_window_marginalize_frames: the linear prior each listed frame leaves on its keyframe (the Schur complement
+        of the frame's pose in its pair's records, undamped).  records: [num_items, REC] on the device.  Returns
+        (priors [n, DFK_PRIOR_DOUBLES] float64, info [n] int32), device tensors written asynchronously on torch's
+        current stream; info[i] = 0, or 1 + the row of the frame block whose pivot failed (prior i is then zero)."""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        _check_tensor(hd, records, torch.float32, self.num_items * _lib.record_floats(self.layout.code_size), "records")
+        fr = np.ascontiguousarray([int(f) for f in frames], dtype=np.int32)
+        n, pd = len(fr), _lib.prior_doubles(self.layout.code_size)
+        if priors is None:
+            priors = torch.empty((n, pd), dtype=torch.float64, device=records.device)
+        _check_tensor(hd, priors, torch.float64, n * pd, "priors")
+        if info is None:
+            info = torch.empty(n, dtype=torch.int32, device=records.device)
+        _check_tensor(hd, info, torch.int32, n, "info")
+        check(hd.h, lib().dfk_window_marginalize_frames(hd.h, self.w, C.c_void_p(records.data_ptr()), n,
+                                                        fr.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                        C.c_void_p(priors.data_ptr()), C.c_void_p(info.data_ptr())))
+        return priors, info
+
+    def add_priors(self, buf: torch.Tensor, prior_kf, priors: torch.Tensor, delta: torch.Tensor) -> torch.Tensor:
+        """dfk_window_add_priors, in place on an assembled buffer: prior i (a row of `priors`, [m, DFK_PRIOR_DOUBLES]
+        float64 on the device) on keyframe prior_kf[i] at delta[i] ([m, B] float64 on the device) = Local(x0_i, x).
+        With sharded pairs, call it after the all-reduce.  Asynchronous on torch's current stream."""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        kf = np.ascontiguousarray([int(k) for k in prior_kf], dtype=np.int32)
+        m, B = len(kf), self.layout.B
+        _check_tensor(hd, buf, torch.float32, self.floats, "buf")
+        _check_tensor(hd, priors, torch.float64, m * _lib.prior_doubles(self.layout.code_size), "priors")
+        _check_tensor(hd, delta, torch.float64, m * B, "delta")
+        check(hd.h, lib().dfk_window_add_priors(hd.h, self.w, m, kf.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                C.c_void_p(priors.data_ptr()), C.c_void_p(delta.data_ptr()),
+                                                C.c_void_p(buf.data_ptr())))
+        return buf
+
     def close(self):
         if getattr(self, "w", None):
             lib().dfk_window_destroy(self._al.handle, self.w)
@@ -496,7 +538,8 @@ class WindowSolver:
     """Damped block-sparse fp64 Cholesky of a Window's normal equations on the device (dfk_window_solve): the system
     WindowOptimizer solves with to_dense + damped_solve, straight from the packed buffer.  `fixed` lists the window
     variables k * B + r held at zero (e.g. range(6): the gauge keyframe's pose).  `tiles` is the number of structurally
-    nonzero B x B tiles of the factor, fill included."""
+    nonzero B x B tiles of the factor, fill included.  With tracked frames dx has K * B + 6 F entries (frame f's pose
+    at K * B + 6 f)."""
 
     def __init__(self, window: Window, fixed=()):
         self._win = window  # keeps the window (and its handle) alive
@@ -514,11 +557,11 @@ class WindowSolver:
     def solve(self, buf: torch.Tensor, lam: float, code_prior_weight: float = 0.0, codes=None,
               dx: torch.Tensor | None = None, info: torch.Tensor | None = None):
         """buf: the window buffer (contiguous float32 on the handle's device).  codes: [K, C] (host), required when
-        code_prior_weight > 0.  Returns (dx [K * B] float64, info [1] int32), device tensors written asynchronously on
+        code_prior_weight > 0.  Returns (dx [K * B + 6 F] float64, info [1] int32), device tensors written asynchronously on
         torch's current stream; info = 0, or 1 + the first variable whose pivot was not positive (dx is then zero)."""
         hd = self._al._hd
         hd.use_torch_stream()
-        n = self.layout.num_keyframes * self.layout.B
+        n = self.layout.dim
         _check_tensor(hd, buf, torch.float32, self.layout.floats, "buf")
         if dx is None:
             dx = torch.empty(n, dtype=torch.float64, device=buf.device)

@@ -100,6 +100,8 @@ struct DfkContext {
   std::vector<unsigned char> geo_host;
   DeviceBuf<SfmItemDev> items_dev;
   DeviceBuf<float> partials_dev;
+  // dfk_window_marginalize_frames / dfk_window_add_priors: the call's index lists (one pageable H2D per call)
+  DeviceBuf<int> window_lists;
   // normalised ray tables of the RunStep kernels: they depend on (fx, u0, width, fy, v0, height) only, so they are
   // built once per camera level and reused by every later call (one launch less per evaluation in steady state)
   struct RayTab {
@@ -1294,8 +1296,14 @@ DfkStatus dfk_window_create(DfkHandle h, const DfkWindowDesc* d, DfkWindow** out
 DfkStatus dfk_window_create_geometric(DfkHandle h, const DfkWindowDesc* d, int L, const int32_t* link_k0,
                                       const int32_t* link_k1, DfkWindow** out)
 {
+  return dfk_window_create_frames(h, d, L, link_k0, link_k1, 0, out);
+}
+
+DfkStatus dfk_window_create_frames(DfkHandle h, const DfkWindowDesc* d, int L, const int32_t* link_k0,
+                                   const int32_t* link_k1, int F, DfkWindow** out)
+{
   return guarded(h, [&] {
-    if (!d || !out || L < 0 || (L > 0 && (!link_k0 || !link_k1)))
+    if (!d || !out || L < 0 || F < 0 || (L > 0 && (!link_k0 || !link_k1)))
       return fail(h, DFK_ERR_INVALID_ARG, "[Window] null argument");
     *out = nullptr;
     const int K = d->num_keyframes, P = d->num_pairs, n = d->num_items;
@@ -1303,14 +1311,29 @@ DfkStatus dfk_window_create_geometric(DfkHandle h, const DfkWindowDesc* d, int L
       return fail(h, DFK_ERR_INVALID_ARG, "[Window] empty window / null index array");
     if (!dfk_sfm_supports_code_size(d->code_size))
       return fail(h, DFK_ERR_UNSUPPORTED, "[Window] no RunStep kernel for code size " + std::to_string(d->code_size));
-    for (int p = 0; p < P; ++p)
-      if (d->pair_k0[p] < 0 || d->pair_k0[p] >= K || d->pair_k1[p] < 0 || d->pair_k1[p] >= K)
+    // pair_k1 in [K, K + F): frame pair_k1 - K, which must be k1 of exactly this one pair
+    std::vector<int> frame_pair(F, -1);
+    for (int p = 0; p < P; ++p) {
+      if (d->pair_k0[p] < 0 || d->pair_k0[p] >= K || d->pair_k1[p] < 0 || d->pair_k1[p] >= K + F)
         return fail(h, DFK_ERR_INVALID_ARG, "[Window] pair " + std::to_string(p) + " names a keyframe outside the window");
+      if (d->pair_k1[p] >= K) {
+        if (frame_pair[d->pair_k1[p] - K] >= 0)
+          return fail(h, DFK_ERR_INVALID_ARG, "[Window] frame " + std::to_string(d->pair_k1[p] - K) +
+                                                  " is k1 of more than one pair");
+        frame_pair[d->pair_k1[p] - K] = p;
+      }
+    }
+    for (int f = 0; f < F; ++f)
+      if (frame_pair[f] < 0)
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] frame " + std::to_string(f) + " is k1 of no pair");
     for (int i = 0; i < n; ++i)
       // a record is scaled (W, H > 0: photometric) or unscaled (0, 0: reprojection)
       if (d->item_pair[i] < 0 || d->item_pair[i] >= P ||
           !((d->item_width[i] > 0 && d->item_height[i] > 0) || (d->item_width[i] == 0 && d->item_height[i] == 0)))
         return fail(h, DFK_ERR_INVALID_ARG, "[Window] record " + std::to_string(i) + " names a pair outside the window");
+    for (int i = 0; i < n; ++i)
+      if (d->pair_k1[d->item_pair[i]] >= K && d->item_width[i] == 0)
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] record " + std::to_string(i) + " of a frame pair is unscaled");
     for (int l = 0; l < L; ++l) {
       if (link_k0[l] < 0 || link_k0[l] >= K || link_k1[l] < 0 || link_k1[l] >= K)
         return fail(h, DFK_ERR_INVALID_ARG, "[Window] link " + std::to_string(l) + " names a keyframe outside the window");
@@ -1318,23 +1341,29 @@ DfkStatus dfk_window_create_geometric(DfkHandle h, const DfkWindowDesc* d, int L
         return fail(h, DFK_ERR_INVALID_ARG, "[Window] link " + std::to_string(l) + " ties a keyframe to itself");
     }
     // one CSR list per key kind (keyframe k0, frame k1, pair): ptr[keys + 1], then the items of each key in item order
-    // (the summation order of the gather kernel); returns where the list starts in blob
+    // (the summation order of the gather kernel); an item whose key is outside [0, keys) is in no list.  Returns where
+    // the list starts in blob
     std::vector<int> blob;
     auto add_csr = [&](int keys, int n, auto key_of) {
       const size_t o = blob.size();
       blob.resize(o + keys + 1 + n, 0);
       int* ptr = blob.data() + o;
-      for (int i = 0; i < n; ++i) ptr[key_of(i) + 1] += 1;
+      for (int i = 0; i < n; ++i)
+        if (key_of(i) < keys) ptr[key_of(i) + 1] += 1;
       for (int k = 0; k < keys; ++k) ptr[k + 1] += ptr[k];
       std::vector<int> next(ptr, ptr + keys);
-      for (int i = 0; i < n; ++i) ptr[keys + 1 + next[key_of(i)]++] = i;
+      for (int i = 0; i < n; ++i)
+        if (key_of(i) < keys) ptr[keys + 1 + next[key_of(i)]++] = i;
       return o;
     };
     const size_t o_kf0 = add_csr(K, n, [&](int i) { return d->pair_k0[d->item_pair[i]]; });
+    // a frame pair's pose1 is the frame's: its items go to the frame's block, not to a keyframe's
     const size_t o_kf1 = add_csr(K, n, [&](int i) { return d->pair_k1[d->item_pair[i]]; });
     const size_t o_pair = add_csr(P, n, [&](int i) { return d->item_pair[i]; });
     const size_t o_lk0 = add_csr(K, L, [&](int l) { return link_k0[l]; });
     const size_t o_lk1 = add_csr(K, L, [&](int l) { return link_k1[l]; });
+    const size_t o_fr = blob.size();
+    blob.insert(blob.end(), frame_pair.begin(), frame_pair.end());
     std::vector<float> areas(n);
     for (int i = 0; i < n; ++i) areas[i] = (float)d->item_width[i] * (float)d->item_height[i];
 
@@ -1356,8 +1385,10 @@ DfkStatus dfk_window_create_geometric(DfkHandle h, const DfkWindowDesc* d, int L
     w->dev.num_links = L;
     w->dev.lk0_ptr = ints + o_lk0; w->dev.lk0_links = ints + o_lk0 + K + 1;
     w->dev.lk1_ptr = ints + o_lk1; w->dev.lk1_links = ints + o_lk1 + K + 1;
+    w->dev.num_frames = F;
+    w->dev.frame_pair = ints + o_fr;
     const size_t B = 6 + (size_t)d->code_size;
-    w->floats = (size_t)K * (B * B + B) + (size_t)P * 6 * B + 2 + (size_t)L * B * B;
+    w->floats = (size_t)K * (B * B + B) + (size_t)P * 6 * B + 2 + (size_t)L * B * B + (size_t)F * 42;
     w->pair_k0.assign(d->pair_k0, d->pair_k0 + P);
     w->pair_k1.assign(d->pair_k1, d->pair_k1 + P);
     w->link_k0.assign(link_k0, link_k0 + L);
@@ -1407,6 +1438,67 @@ DfkStatus dfk_window_assemble_geometric(DfkHandle h, const DfkWindow* w, const f
   });
 }
 
+DfkStatus dfk_window_marginalize_frames(DfkHandle h, const DfkWindow* w, const float* records_dev, int n,
+                                        const int32_t* frames_host, double* priors_dev, int32_t* info_dev)
+{
+  return guarded(h, [&] {
+    if (!w || !records_dev || n < 0 || (n > 0 && (!frames_host || !priors_dev || !info_dev)))
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::MarginalizeFrames] null argument");
+    if (w->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::MarginalizeFrames] window and handle live on different devices");
+    for (int i = 0; i < n; ++i)
+      if (frames_host[i] < 0 || frames_host[i] >= w->dev.num_frames)
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window::MarginalizeFrames] frame " + std::to_string(frames_host[i]) +
+                                                " is not a frame of the window");
+    if (n == 0) return DFK_OK;
+    DeviceGuard guard(h->device);
+    const char* what = "[Window::MarginalizeFrames] index upload failed";
+    DFK_CUDA(h, h->window_lists.ensure(n), what);
+    // pageable source: staged before the call returns
+    DFK_CUDA(h, cudaMemcpyAsync(h->window_lists.ptr, frames_host, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream),
+             what);
+    DFK_CUDA(h, launch_window_marginalize_frames(w->dev, records_dev, n, h->window_lists.ptr, priors_dev, info_dev,
+                                                 h->stream),
+             "[Window::MarginalizeFrames] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_add_priors(DfkHandle h, const DfkWindow* w, int m, const int32_t* prior_kf_host,
+                                const double* priors_dev, const double* delta_dev, float* window_dev)
+{
+  return guarded(h, [&] {
+    if (!w || !window_dev || m < 0 || (m > 0 && (!prior_kf_host || !priors_dev || !delta_dev)))
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddPriors] null argument");
+    if (w->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddPriors] window and handle live on different devices");
+    const int K = w->dev.num_keyframes;
+    for (int i = 0; i < m; ++i)
+      if (prior_kf_host[i] < 0 || prior_kf_host[i] >= K)
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddPriors] prior " + std::to_string(i) +
+                                                " names a keyframe outside the window");
+    if (m == 0) return DFK_OK;
+    // CSR of the priors per keyframe, in list order: ptr[K + 1] | indices[m]
+    std::vector<int> lists(K + 1 + m, 0);
+    for (int i = 0; i < m; ++i) lists[prior_kf_host[i] + 1] += 1;
+    for (int k = 0; k < K; ++k) lists[k + 1] += lists[k];
+    std::vector<int> next(lists.begin(), lists.begin() + K);
+    for (int i = 0; i < m; ++i) lists[K + 1 + next[prior_kf_host[i]]++] = i;
+    DeviceGuard guard(h->device);
+    const char* what = "[Window::AddPriors] index upload failed";
+    DFK_CUDA(h, h->window_lists.ensure(lists.size()), what);
+    DFK_CUDA(h, cudaMemcpyAsync(h->window_lists.ptr, lists.data(), sizeof(int) * lists.size(), cudaMemcpyHostToDevice,
+                                h->stream),
+             what);
+    DFK_CUDA(h, launch_window_add_priors(w->dev, m, h->window_lists.ptr, h->window_lists.ptr + K + 1, priors_dev,
+                                         delta_dev, window_dev, h->stream),
+             "[Window::AddPriors] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
 DfkStatus dfk_window_solver_create(DfkHandle h, const DfkWindow* w, int num_fixed, const int32_t* fixed_vars,
                                    DfkWindowSolver** out)
 {
@@ -1431,7 +1523,8 @@ DfkStatus dfk_window_solver_create(DfkHandle h, const DfkWindow* w, int num_fixe
     if (!s) return oom(h);
     s->device = h->device;
     s->num_vars = n; s->code_size = C; s->num_keyframes = K;
-    DFK_CUDA(h, window_solver_create(K, C, w->pair_k0, w->pair_k1, w->link_k0, w->link_k1, fixed, &s->dev),
+    DFK_CUDA(h, window_solver_create(K, C, w->dev.num_frames, w->pair_k0, w->pair_k1, w->link_k0, w->link_k1, fixed,
+                                     &s->dev),
              "[WindowSolver] workspace allocation failed");
     *out = s.release();
     return DFK_OK;

@@ -201,16 +201,26 @@ struct WindowDev {
   const int* lk0_links;   // ... in link order
   const int* lk1_ptr;     // [K+1] links whose k1 is k
   const int* lk1_links;
+  int num_frames;         // tracked frames (pose-only variables), frame f is pair_k1 = K + f of exactly one pair
+  const int* frame_pair;  // [F] the pair of frame f
 };
 // geo_records_dev may be null when num_links == 0
 cudaError_t launch_window_assemble(const WindowDev& w, const float* records_dev, const float* geo_records_dev,
                                    float* out_dev, cudaStream_t stream);
+// n frames frames_dev[i]: prior i (DFK_PRIOR_DOUBLES) = Schur complement of the frame's pose in its pair's items
+cudaError_t launch_window_marginalize_frames(const WindowDev& w, const float* records_dev, int n, const int* frames_dev,
+                                             double* priors_dev, int32_t* info_dev, cudaStream_t stream);
+// m priors on keyframes prior_kf (the CSR kf_ptr[K+1] / kf_priors of prior indices per keyframe, in list order)
+cudaError_t launch_window_add_priors(const WindowDev& w, int m, const int* kf_ptr_dev, const int* kf_priors_dev,
+                                     const double* priors_dev, const double* delta_dev, float* window_dev,
+                                     cudaStream_t stream);
 
 // dfk_window_solve.cu : damped block-sparse fp64 Cholesky of a window buffer.  The symbolic analysis and the workspace
 // (cudaMalloc, on the current device) belong to the solver; a solve allocates nothing.
 struct WindowSolverDev;
-// pairs / links: the window's keyframe lists; fixed_vars: distinct variable indices in [0, K (6 + C))
-cudaError_t window_solver_create(int num_keyframes, int code_size, const std::vector<int>& pair_k0,
+// pairs / links: the window's keyframe lists (a pair whose k1 is K + f belongs to frame f); fixed_vars: distinct
+// variable indices in [0, K (6 + C))
+cudaError_t window_solver_create(int num_keyframes, int code_size, int num_frames, const std::vector<int>& pair_k0,
                                  const std::vector<int>& pair_k1, const std::vector<int>& link_k0,
                                  const std::vector<int>& link_k1, const std::vector<int>& fixed_vars,
                                  WindowSolverDev** out);

@@ -13,14 +13,20 @@
 //                                                            photometric inliers
 //   [ L link blocks, B x B row-major ]                       geometric link l = (k0 -> k1): rows = k0's [pose0 | code0],
 //                                                            cols = k1's [pose1 | code1]
+//   [ F frame blocks, 6 x 6 ] [ F frame gradients, 6 ]       tracked frame f (a pose-only variable): pose1 x pose1 and
+//                                                            -Jtr(pose1) of its one pair (k0 -> K + f)
 // A pair (k0 -> k1) adds its pose0/code0 blocks to keyframe k0's diagonal block, pose1 x pose1 to k1's, and the
 // [pose0; code0] x pose1 coupling to its own block.  A geometric link (sparse_geometric_factor.cpp: keys pose0, pose1,
 // code0, code1) adds its (pose0, code0) block to k0's diagonal block, its whole (pose1, code1) block to k1's, and the
 // cross block to its own link block.
 //
 // Deterministic by construction: a GATHER, not a scatter -- every output element is owned by one thread, which sums the
-// contributions of its items in list order, then those of the links (no float atomics).  One launch: grid = K + P + L + 1
-// jobs.  Without links every element is the same chain of adds as in a photometric / reprojection-only window.
+// contributions of its items in list order, then those of the links (no float atomics).  One launch: grid = K + P + L + F
+// + 1 jobs.  Without links every element is the same chain of adds as in a photometric / reprojection-only window; a
+// frame pair's items are not in any keyframe's k1 list, so without frames nothing changes either.
+//
+// Also here: the marginalisation of frames into linear priors on their keyframe (the Schur complement of the frame's
+// pose, what ISAM2::marginalizeLeaves leaves for a leaf with one factor) and the addition of such priors to a window.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -105,6 +111,24 @@ window_assemble_kernel(WindowDev w, const float* __restrict__ records, const flo
       const int r = e / B, c = e - r * B;
       O[e] = rec_h(rec, link_row0(r), link_row1(c, C), NG);
     }
+  } else if (job < w.num_keyframes + w.num_pairs + w.num_links + w.num_frames) {
+    // ---- frame f: pose1 x pose1 block and -Jtr(pose1) of its one pair's items, in item order
+    const int f = job - w.num_keyframes - w.num_pairs - w.num_links;
+    float* Df = tail + 2 + (size_t)w.num_links * B * B + (size_t)f * 36;
+    float* gf = tail + 2 + (size_t)w.num_links * B * B + (size_t)w.num_frames * 36 + (size_t)f * 6;
+    const int p = w.frame_pair[f];
+    const int i0 = w.pair_ptr[p], i1 = w.pair_ptr[p + 1];
+    for (int e = threadIdx.x; e < 42; e += blockDim.x) {
+      float s = 0.0f;
+      if (e < 36) {
+        const int r = e / 6, c = e - r * 6;
+        for (int q = i0; q < i1; ++q) s += rec_h(records + (size_t)w.pair_items[q] * REC, 6 + r, 6 + c, NP);
+        Df[e] = s;
+      } else {
+        for (int q = i0; q < i1; ++q) s -= records[(size_t)w.pair_items[q] * REC + NH + 6 + (e - 36)];
+        gf[e - 36] = s;
+      }
+    }
   } else {
     // ---- energy: f = sum res / inliers * W * H over items with overlap (photometric_factor.cpp:275-282) + res of the
     // unscaled records (reprojection factors, error() = 1/2 |b|^2, reprojection_factor.cpp:148), photometric inliers
@@ -144,13 +168,205 @@ window_assemble_kernel(WindowDev w, const float* __restrict__ records, const flo
   }
 }
 
+// fixed-order block sum of one double per thread (lanes by xor butterfly, warps in index order); every thread gets it
+__device__ double block_sum(double v, double* red)
+{
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();  // red is free again
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.0;
+  for (int k = 0; k < (int)(blockDim.x >> 5); ++k) s += red[k];
+  return s;
+}
+
+constexpr int kMaxB = 6 + 128;
+
+// ---- marginalisation of frame frames[i] (one CTA each): the fp64 sums of its pair's items, in item order, over the
+// record rows a = [pose0 | code0] (keyframe k) and b = pose1 (the frame), then the Schur complement of b:
+//   G = H_aa - H_ab H_bb^-1 H_ab^T,  g = g_a - H_ab H_bb^-1 g_b,  f0 = f_p - g_b^T H_bb^-1 g_b
+// with H_bb = L L^T (6 x 6, undamped), Y = H_ab L^-T, z = L^-1 g_b: G = H_aa - Y Y^T, g = g_a - Y z, f0 = f_p - z^T z.
+// Prior i: [G (B x B row-major) | g (B) | f0].  A pivot of H_bb that is not positive and finite: info[i] = 1 + its
+// row, prior all zero.
+__global__ void __launch_bounds__(256)
+window_marginalize_kernel(WindowDev w, const float* __restrict__ records, const int* __restrict__ frames,
+                          double* __restrict__ priors, int32_t* __restrict__ info)
+{
+  const int C = w.code_size, B = 6 + C, NP = 12 + C;
+  const int NH = NP * (NP + 1) / 2, REC = NH + NP + 2;
+  __shared__ double Hab[kMaxB * 6], Y[kMaxB * 6], ga[kMaxB], Hbb[36], L[36], gb[6], z[6];
+  __shared__ int bad;
+  const int p = w.frame_pair[frames[blockIdx.x]];
+  const int i0 = w.pair_ptr[p], i1 = w.pair_ptr[p + 1];
+  double* G = priors + (size_t)blockIdx.x * (B * B + B + 1);
+  double* g = G + B * B;
+  for (int e = threadIdx.x; e < B * B; e += blockDim.x) {
+    const int r = e / B, c = e - r * B;
+    const int lr = r < 6 ? r : 6 + r, lc = c < 6 ? c : 6 + c;
+    double s = 0.0;
+    for (int q = i0; q < i1; ++q) s += (double)rec_h(records + (size_t)w.pair_items[q] * REC, lr, lc, NP);
+    G[e] = s;
+  }
+  for (int e = threadIdx.x; e < B * 6 + 36 + B + 6; e += blockDim.x) {
+    double s = 0.0;
+    if (e < B * 6) {
+      const int r = e / 6, c = e - r * 6, lr = r < 6 ? r : 6 + r;
+      for (int q = i0; q < i1; ++q) s += (double)rec_h(records + (size_t)w.pair_items[q] * REC, lr, 6 + c, NP);
+      Hab[e] = s;
+    } else if (e < B * 6 + 36) {
+      const int r = (e - B * 6) / 6, c = (e - B * 6) % 6;
+      for (int q = i0; q < i1; ++q) s += (double)rec_h(records + (size_t)w.pair_items[q] * REC, 6 + r, 6 + c, NP);
+      Hbb[e - B * 6] = s;
+    } else if (e < B * 7 + 36) {
+      const int r = e - B * 6 - 36, lr = r < 6 ? r : 6 + r;
+      for (int q = i0; q < i1; ++q) s -= (double)records[(size_t)w.pair_items[q] * REC + NH + lr];
+      ga[r] = s;
+    } else {
+      const int r = e - B * 7 - 36;
+      for (int q = i0; q < i1; ++q) s -= (double)records[(size_t)w.pair_items[q] * REC + NH + 6 + r];
+      gb[r] = s;
+    }
+  }
+  // f_p: the rescaled residuals of the items with overlap (the items of a frame pair are all scaled)
+  double fp = 0.0;
+  if (threadIdx.x == 0)
+    for (int q = i0; q < i1; ++q) {
+      const float* rec = records + (size_t)w.pair_items[q] * REC;
+      const uint32_t inl = __float_as_uint(rec[NH + NP + 1]);
+      if (inl > 0) fp += (double)rec[NH + NP] / (double)inl * (double)w.item_area[w.pair_items[q]];
+    }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int b = -1;
+    for (int c = 0; c < 6; ++c) {
+      double d = Hbb[c * 6 + c];
+      for (int m = 0; m < c; ++m) d = __fma_rn(-L[c * 6 + m], L[c * 6 + m], d);
+      if (b < 0 && !(d > 0.0 && d <= 1.7976931348623157e308)) b = c;
+      d = sqrt(d);
+      L[c * 6 + c] = d;
+      for (int r = c + 1; r < 6; ++r) {
+        double v = Hbb[r * 6 + c];
+        for (int m = 0; m < c; ++m) v = __fma_rn(-L[r * 6 + m], L[c * 6 + m], v);
+        L[r * 6 + c] = __ddiv_rn(v, d);
+      }
+    }
+    for (int c = 0; c < 6; ++c) {
+      double v = gb[c];
+      for (int m = 0; m < c; ++m) v = __fma_rn(-L[c * 6 + m], z[m], v);
+      z[c] = __ddiv_rn(v, L[c * 6 + c]);
+    }
+    bad = b;
+  }
+  __syncthreads();
+  if (bad >= 0) {
+    for (int e = threadIdx.x; e < B * B + B + 1; e += blockDim.x) G[e] = 0.0;
+    if (threadIdx.x == 0) info[blockIdx.x] = 1 + bad;
+    return;
+  }
+  for (int r = threadIdx.x; r < B; r += blockDim.x)  // Y L^T = H_ab, row by row
+    for (int c = 0; c < 6; ++c) {
+      double v = Hab[r * 6 + c];
+      for (int m = 0; m < c; ++m) v = __fma_rn(-Y[r * 6 + m], L[c * 6 + m], v);
+      Y[r * 6 + c] = __ddiv_rn(v, L[c * 6 + c]);
+    }
+  __syncthreads();
+  for (int e = threadIdx.x; e < B * B; e += blockDim.x) {
+    const int r = e / B, c = e - r * B;
+    double s = 0.0;
+    for (int m = 0; m < 6; ++m) s = __fma_rn(Y[r * 6 + m], Y[c * 6 + m], s);
+    G[e] = __dsub_rn(G[e], s);
+  }
+  for (int r = threadIdx.x; r < B; r += blockDim.x) {
+    double s = 0.0;
+    for (int m = 0; m < 6; ++m) s = __fma_rn(Y[r * 6 + m], z[m], s);
+    g[r] = __dsub_rn(ga[r], s);
+  }
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int m = 0; m < 6; ++m) s = __fma_rn(z[m], z[m], s);
+    g[B] = __dsub_rn(fp, s);
+    info[blockIdx.x] = 0;
+  }
+}
+
+// ---- priors into an assembled window, in place.  Prior i on keyframe k with delta_i = Local(x0_i, x):
+//   D_k += G,  g_k += g - G delta,  f += f0 - 2 g^T delta + delta^T G delta
+// CTA k < K: keyframe k's block and gradient, its priors in list order summed in fp64 onto the fp32 entry, rounded
+// once.  CTA K: f, every prior in list order (the inlier total is left alone).
+__global__ void __launch_bounds__(256)
+window_add_priors_kernel(WindowDev w, int m, const int* __restrict__ kf_ptr, const int* __restrict__ kf_priors,
+                         const double* __restrict__ priors, const double* __restrict__ delta, float* __restrict__ out)
+{
+  const int C = w.code_size, B = 6 + C, PD = B * B + B + 1;
+  const int K = w.num_keyframes;
+  if ((int)blockIdx.x < K) {
+    const int k = blockIdx.x, q0 = kf_ptr[k], q1 = kf_ptr[k + 1];
+    if (q0 == q1) return;
+    float* D = out + (size_t)k * B * B;
+    float* g = out + (size_t)K * B * B + (size_t)k * B;
+    for (int e = threadIdx.x; e < B * B + B; e += blockDim.x) {
+      if (e < B * B) {
+        double s = (double)D[e];
+        for (int q = q0; q < q1; ++q) s = __dadd_rn(s, priors[(size_t)kf_priors[q] * PD + e]);
+        D[e] = (float)s;
+      } else {
+        const int r = e - B * B;
+        double s = (double)g[r];
+        for (int q = q0; q < q1; ++q) {
+          const double* P = priors + (size_t)kf_priors[q] * PD;
+          const double* d = delta + (size_t)kf_priors[q] * B;
+          double gd = 0.0;
+          for (int c = 0; c < B; ++c) gd = __fma_rn(P[r * B + c], d[c], gd);
+          s = __dadd_rn(s, __dsub_rn(P[B * B + r], gd));
+        }
+        g[r] = (float)s;
+      }
+    }
+    return;
+  }
+  __shared__ double red[8];
+  float* tail = out + (size_t)K * (B * B + B) + (size_t)w.num_pairs * B * 6;
+  double s = (double)tail[0];
+  for (int i = 0; i < m; ++i) {
+    const double* P = priors + (size_t)i * PD;
+    const double* d = delta + (size_t)i * B;
+    double gd = 0.0, dGd = 0.0;
+    for (int r = threadIdx.x; r < B; r += blockDim.x) {
+      double Gd = 0.0;
+      for (int c = 0; c < B; ++c) Gd = __fma_rn(P[r * B + c], d[c], Gd);
+      gd = __fma_rn(P[B * B + r], d[r], gd);
+      dGd = __fma_rn(d[r], Gd, dGd);
+    }
+    gd = block_sum(gd, red);
+    dGd = block_sum(dGd, red);
+    s = __dadd_rn(s, __dadd_rn(__fma_rn(-2.0, gd, P[B * B + B]), dGd));
+  }
+  if (threadIdx.x == 0) tail[0] = (float)s;
+}
+
 }  // namespace
 
 cudaError_t launch_window_assemble(const WindowDev& w, const float* records_dev, const float* geo_records_dev,
                                    float* out_dev, cudaStream_t stream)
 {
-  window_assemble_kernel<<<w.num_keyframes + w.num_pairs + w.num_links + 1, 256, 0, stream>>>(w, records_dev,
-                                                                                             geo_records_dev, out_dev);
+  window_assemble_kernel<<<w.num_keyframes + w.num_pairs + w.num_links + w.num_frames + 1, 256, 0, stream>>>(
+      w, records_dev, geo_records_dev, out_dev);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_marginalize_frames(const WindowDev& w, const float* records_dev, int n, const int* frames_dev,
+                                             double* priors_dev, int32_t* info_dev, cudaStream_t stream)
+{
+  window_marginalize_kernel<<<n, 256, 0, stream>>>(w, records_dev, frames_dev, priors_dev, info_dev);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_add_priors(const WindowDev& w, int m, const int* kf_ptr_dev, const int* kf_priors_dev,
+                                     const double* priors_dev, const double* delta_dev, float* window_dev,
+                                     cudaStream_t stream)
+{
+  window_add_priors_kernel<<<w.num_keyframes + 1, 256, 0, stream>>>(w, m, kf_ptr_dev, kf_priors_dev, priors_dev,
+                                                                    delta_dev, window_dev);
   return cudaGetLastError();
 }
 

@@ -18,9 +18,17 @@
 //                          g_i -= L_ij y_j.
 //   per row j, descending   backward: one CTA per nonzero tile (j, i), i <= j.  Each solves L_jj^T x_j = y_j in shared
 //                          memory (again its own copy); the diagonal CTA writes dx_j, the others y_i -= L_ji^T x_j.
+//   frames         (windows with tracked frames) one launch, one CTA per frame: dx_f = S_f^-1 (g_f - O_f^T dx_k).
 // Every tile and every rhs block receives at most one update per launch and its updates in column order, every sum runs
 // in a fixed order and there are no atomics, so two solves of the same buffer are bit for bit equal.  Ordering comes from
 // stream order only: no CTA ever waits for another.
+//
+// Tracked frames are pose-only leaves with one pair to one keyframe k, so they are eliminated first, each into k's
+// diagonal tile by k's load CTA (frame order): S_f = D_f + diag(lambda d_f + eps) = L_f L_f^T (6 x 6, fp64), Y = O_f
+// L_f^-T with O_f's rows at fixed variables zero, z = L_f^-1 g_f; then T_kk -= Y Y^T and g_k -= Y z.  This creates no
+// fill, so the symbolic analysis ignores frame pairs.  L_f stays in the workspace for the frame launch; a frame pivot
+// that is not positive and finite is reported (by column 0's panel, as the first in elimination order) as
+// 1 + K B + 6 f + r.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -61,6 +69,18 @@ struct SolveArgs {
   double lambda, prior;
 };
 
+// the tracked frames of a window, a parameter of its own: only the kernels that handle frames take it, so those of a
+// window without frames keep SolveArgs' size and their register allocation
+struct FrameArgs {
+  int L, F;                     // links, tracked frames
+  const int* frame_ptr;         // [K + 1] frames of keyframe k: frame_list[frame_ptr[k] .. frame_ptr[k + 1])
+  const int* frame_list;
+  const int* frame_pair;        // [F]
+  const int* frame_kf;          // [F] keyframe of frame f (k0 of its pair)
+  double* frame_L;              // [F * 36] Cholesky factor of the damped S_f
+  int* frame_bad;               // [F] 0, or 1 + the row whose pivot failed
+};
+
 __device__ __forceinline__ size_t tile_off(int t, int B) { return (size_t)t * B * B; }
 
 // ------------------------------------------------------------------------------------------------------------- load
@@ -87,6 +107,13 @@ __device__ double tile_entry(const SolveArgs& a, int t, int r, int c)
   return s;
 }
 
+// buffer offsets of the frame blocks (6 x 6 each) and of the frame gradients
+template <int B>
+__device__ __forceinline__ size_t frame_block_off(const SolveArgs& a, const FrameArgs& fa)
+{
+  return (size_t)a.K * (B * B + B) + (size_t)a.P * B * 6 + 2 + (size_t)fa.L * B * B;
+}
+
 // diagonal entry (after the prior) of variable r of keyframe k
 template <int B>
 __device__ double diag_entry(const SolveArgs& a, int k, int r)
@@ -96,8 +123,69 @@ __device__ double diag_entry(const SolveArgs& a, int k, int r)
   return h;
 }
 
+// keyframe i's frames into its damped diagonal tile T and its rhs, in frame order (see the file comment).  Kept out
+// of the load kernel body for readability.
 template <int B>
-__global__ void __launch_bounds__(kThreads) window_solve_load_kernel(SolveArgs a)
+__device__ __forceinline__ void eliminate_frames(const SolveArgs& a, const FrameArgs& fa, int i, double* T, double eps)
+{
+  const size_t o_f = frame_block_off<B>(a, fa);
+  __syncthreads();  // every thread wrote its T / rhs entries
+  __shared__ double sL[36], sz[6], sY[B * 6];
+  for (int q = fa.frame_ptr[i]; q < fa.frame_ptr[i + 1]; ++q) {
+    const int f = fa.frame_list[q];
+    const float* O = a.buf + (size_t)a.K * (B * B + B) + (size_t)fa.frame_pair[f] * B * 6;
+    const float* Df = a.buf + o_f + (size_t)f * 36;
+    const float* gf = a.buf + o_f + (size_t)fa.F * 36 + (size_t)f * 6;
+    if (threadIdx.x == 0) {
+      int bad = -1;
+      for (int c = 0; c < 6; ++c) {
+        double d = (double)Df[c * 7];
+        d = __dadd_rn(d, __dadd_rn(__dmul_rn(a.lambda, d), eps));
+        for (int k = 0; k < c; ++k) d = __fma_rn(-sL[c * 6 + k], sL[c * 6 + k], d);
+        if (bad < 0 && !(d > 0.0 && d <= 1.7976931348623157e308)) bad = c;
+        d = sqrt(d);
+        sL[c * 6 + c] = d;
+        for (int r = c + 1; r < 6; ++r) {
+          double v = (double)Df[r * 6 + c];
+          for (int k = 0; k < c; ++k) v = __fma_rn(-sL[r * 6 + k], sL[c * 6 + k], v);
+          sL[r * 6 + c] = __ddiv_rn(v, d);
+        }
+        for (int r = 0; r < c; ++r) sL[r * 6 + c] = 0.0;
+      }
+      for (int c = 0; c < 6; ++c) {
+        double v = (double)gf[c];
+        for (int k = 0; k < c; ++k) v = __fma_rn(-sL[c * 6 + k], sz[k], v);
+        sz[c] = __ddiv_rn(v, sL[c * 6 + c]);
+      }
+      for (int e = 0; e < 36; ++e) fa.frame_L[(size_t)f * 36 + e] = sL[e];
+      fa.frame_bad[f] = bad + 1;
+    }
+    __syncthreads();
+    for (int r = threadIdx.x; r < B; r += blockDim.x)  // Y L^T = O, row by row; a fixed row of O counts as zero
+      for (int c = 0; c < 6; ++c) {
+        double v = a.fixed[i * B + r] ? 0.0 : (double)O[r * 6 + c];
+        for (int k = 0; k < c; ++k) v = __fma_rn(-sY[r * 6 + k], sL[c * 6 + k], v);
+        sY[r * 6 + c] = a.fixed[i * B + r] ? 0.0 : __ddiv_rn(v, sL[c * 6 + c]);
+      }
+    __syncthreads();
+    for (int e = threadIdx.x; e < B * B; e += blockDim.x) {
+      const int r = e / B, c = e - r * B;
+      double s = 0.0;
+      for (int k = 0; k < 6; ++k) s = __fma_rn(sY[r * 6 + k], sY[c * 6 + k], s);
+      T[e] = __dsub_rn(T[e], s);
+    }
+    for (int r = threadIdx.x; r < B; r += blockDim.x) {
+      double s = 0.0;
+      for (int k = 0; k < 6; ++k) s = __fma_rn(sY[r * 6 + k], sz[k], s);
+      a.rhs[(size_t)i * B + r] = __dsub_rn(a.rhs[(size_t)i * B + r], s);
+    }
+    __syncthreads();  // sL / sY are consumed
+  }
+}
+
+// kFrames = false (a window without frames) is the load kernel without any frame code: same registers, no stack
+template <int B, bool kFrames>
+__global__ void __launch_bounds__(kThreads) window_solve_load_kernel(SolveArgs a, FrameArgs fa)
 {
   const int t = blockIdx.x;
   const int i = a.tile_row[t], j = a.tile_col[t];
@@ -115,6 +203,9 @@ __global__ void __launch_bounds__(kThreads) window_solve_load_kernel(SolveArgs a
   double m = 0.0;
   for (int v = threadIdx.x; v < a.K * B; v += blockDim.x)
     if (!a.fixed[v]) m = fmax(m, fabs(diag_entry<B>(a, v / B, v % B)));
+  if constexpr (kFrames)
+    for (int v = threadIdx.x; v < fa.F * 6; v += blockDim.x)  // and over the frames' (never fixed)
+      m = fmax(m, fabs((double)a.buf[frame_block_off<B>(a, fa) + (v / 6) * 36 + (v % 6) * 7]));
   for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
   __syncthreads();
@@ -142,6 +233,7 @@ __global__ void __launch_bounds__(kThreads) window_solve_load_kernel(SolveArgs a
     a.rhs[(size_t)i * B + r] = a.fixed[i * B + r] ? 0.0 : g;
   }
   if (t == 0 && threadIdx.x == 0) *a.info = 0;
+  if constexpr (kFrames) eliminate_frames<B>(a, fa, i, T, eps);
 }
 
 // ------------------------------------------------------------------------------------------------------------ panel
@@ -192,7 +284,8 @@ __device__ void trsm_rows(double* X, int rows, const double* L, const double* dg
 }
 
 template <int B>
-__global__ void __launch_bounds__(kThreads) window_solve_panel_kernel(SolveArgs a, int j, int col_begin)
+__global__ void __launch_bounds__(kThreads) window_solve_panel_kernel(SolveArgs a, int j, int col_begin,
+                                                                       const int* frame_bad, int F)
 {
   extern __shared__ double sm[];
   double* L = sm;
@@ -215,6 +308,12 @@ __global__ void __launch_bounds__(kThreads) window_solve_panel_kernel(SolveArgs 
     __syncthreads();
     trsm_rows<B>(X, 1, L, dg);
     for (int e = threadIdx.x; e < B; e += blockDim.x) g[e] = X[e];
+    if (threadIdx.x == 0 && j == 0)  // the frames were eliminated first: the first failed frame pivot comes first
+      for (int f = 0; f < F; ++f)
+        if (frame_bad[f] != 0) {
+          *a.info = 1 + a.K * B + 6 * f + frame_bad[f] - 1;
+          break;
+        }
     if (threadIdx.x == 0 && bad >= 0 && *a.info == 0) *a.info = 1 + j * B + bad;
     return;
   }
@@ -338,6 +437,43 @@ __global__ void __launch_bounds__(kThreads) window_solve_backward_kernel(SolveAr
   }
 }
 
+// ----------------------------------------------------------------------------------------------------------- frames
+// one CTA of 32 threads per frame f of keyframe k: v = g_f - O_f^T dx_k (lane c < 6, rows in order, fixed rows skipped),
+// then dx_f = L_f^-T L_f^-1 v
+template <int B>
+__global__ void __launch_bounds__(32) window_solve_frames_kernel(SolveArgs a, FrameArgs fa)
+{
+  __shared__ double v[6];
+  const int f = blockIdx.x, p = fa.frame_pair[f];
+  const int k = fa.frame_kf[f];
+  const size_t o_f = frame_block_off<B>(a, fa);
+  if (threadIdx.x < 6) {
+    const int c = threadIdx.x;
+    const float* O = a.buf + (size_t)a.K * (B * B + B) + (size_t)p * B * 6;
+    double s = (double)a.buf[o_f + (size_t)fa.F * 36 + (size_t)f * 6 + c];
+    for (int r = 0; r < B; ++r)
+      if (!a.fixed[k * B + r]) s = __fma_rn(-(double)O[r * 6 + c], a.dx[(size_t)k * B + r], s);
+    v[c] = s;
+  }
+  __syncwarp();
+  if (threadIdx.x == 0) {
+    const double* L = fa.frame_L + (size_t)f * 36;
+    double y[6];
+    for (int c = 0; c < 6; ++c) {
+      double s = v[c];
+      for (int m = 0; m < c; ++m) s = __fma_rn(-L[c * 6 + m], y[m], s);
+      y[c] = __ddiv_rn(s, L[c * 6 + c]);
+    }
+    for (int c = 5; c >= 0; --c) {
+      double s = y[c];
+      for (int m = c + 1; m < 6; ++m) s = __fma_rn(-L[m * 6 + c], y[m], s);
+      y[c] = __ddiv_rn(s, L[c * 6 + c]);
+    }
+    const bool ok = *a.info == 0;
+    for (int c = 0; c < 6; ++c) a.dx[(size_t)a.K * B + 6 * f + c] = ok ? y[c] : 0.0;
+  }
+}
+
 template <class F>
 cudaError_t with_code_size(int code_size, F&& f)
 {
@@ -355,19 +491,23 @@ cudaError_t with_code_size(int code_size, F&& f)
 
 // --------------------------------------------------------------------------------------------------------- the plan
 struct WindowSolverDev {
-  int K = 0, C = 0, B = 0, P = 0, L = 0, num_tiles = 0;
+  int K = 0, C = 0, B = 0, P = 0, L = 0, F = 0, num_tiles = 0;
   std::vector<int> col_ptr;   // [K + 1] tiles of column j: [col_ptr[j], col_ptr[j+1]), the first one diagonal
   std::vector<int> upd_ptr;   // [K + 1] update tasks of column j
   std::vector<int> row_ptr;   // [K + 1] backward tiles of row j (off-diagonal, column order)
-  // device: one int allocation (tile_row | tile_col | contrib_ptr | contrib | diag_tile | row_tiles | tasks), the fixed
-  // mask, the codes, the tiles, the rhs
+  // device: one int allocation (tile_row | tile_col | contrib_ptr | contrib | diag_tile | row_tiles | frame_ptr |
+  // frame_list | frame_pair | frame_kf | tasks), the fixed mask, the codes, the tiles, the rhs, the frames' factors and
+  // pivot flags
   void* ints = nullptr;
   unsigned char* fixed = nullptr;
   double* codes = nullptr;
   double* tiles = nullptr;
   double* rhs = nullptr;
+  double* frame_L = nullptr;
+  int* frame_bad = nullptr;
   const int *tile_row = nullptr, *tile_col = nullptr, *contrib_ptr = nullptr, *contrib = nullptr, *diag_tile = nullptr,
-            *row_tiles = nullptr;
+            *row_tiles = nullptr, *frame_ptr = nullptr, *frame_list = nullptr, *frame_pair = nullptr,
+            *frame_kf = nullptr;
   const UpdTask* tasks = nullptr;
   ~WindowSolverDev()
   {
@@ -376,28 +516,32 @@ struct WindowSolverDev {
     cudaFree(codes);
     cudaFree(tiles);
     cudaFree(rhs);
+    cudaFree(frame_L);
+    cudaFree(frame_bad);
   }
 };
 
 size_t window_solver_tiles(const WindowSolverDev* s) { return s ? (size_t)s->num_tiles : 0; }
 
-cudaError_t window_solver_create(int K, int C, const std::vector<int>& pair_k0, const std::vector<int>& pair_k1,
+cudaError_t window_solver_create(int K, int C, int F, const std::vector<int>& pair_k0, const std::vector<int>& pair_k1,
                                  const std::vector<int>& link_k0, const std::vector<int>& link_k1,
                                  const std::vector<int>& fixed_vars, WindowSolverDev** out)
 {
   *out = nullptr;
   const int B = 6 + C, P = (int)pair_k0.size(), L = (int)link_k0.size();
-  // ---- symbolic elimination in keyframe order: below[j] = rows i > j of the nonzero tiles of column j
+  // ---- symbolic elimination in keyframe order: below[j] = rows i > j of the nonzero tiles of column j (a frame pair,
+  // k1 >= K, is eliminated at load: no tile, no fill)
   std::vector<std::set<int>> below(K);
   for (int p = 0; p < P; ++p)
-    if (pair_k0[p] != pair_k1[p]) below[std::min(pair_k0[p], pair_k1[p])].insert(std::max(pair_k0[p], pair_k1[p]));
+    if (pair_k0[p] != pair_k1[p] && pair_k1[p] < K)
+      below[std::min(pair_k0[p], pair_k1[p])].insert(std::max(pair_k0[p], pair_k1[p]));
   for (int l = 0; l < L; ++l) below[std::min(link_k0[l], link_k1[l])].insert(std::max(link_k0[l], link_k1[l]));
   for (int j = 0; j < K; ++j) {
     for (auto ia = below[j].begin(); ia != below[j].end(); ++ia)
       for (auto ib = below[j].begin(); ib != ia; ++ib) below[*ib].insert(*ia);  // (ia, ib) fills, ib < ia
   }
   auto s = std::make_unique<WindowSolverDev>();
-  s->K = K; s->C = C; s->B = B; s->P = P; s->L = L;
+  s->K = K; s->C = C; s->B = B; s->P = P; s->L = L; s->F = F;
   std::vector<int> tile_row, tile_col;
   s->col_ptr.assign(K + 1, 0);
   std::vector<std::vector<std::pair<int, int>>> col_index(K);  // (row, tile) per column, rows ascending
@@ -419,9 +563,14 @@ cudaError_t window_solver_create(int K, int C, const std::vector<int>& pair_k0, 
   };
   // ---- contributions per tile, in to_dense's order
   std::vector<std::vector<int>> contrib(T);
+  std::vector<int> frame_pair(F), frame_kf(F), frame_ptr(K + 1, 0), frame_list(F);
   for (int p = 0; p < P; ++p) {
     const int k0 = pair_k0[p], k1 = pair_k1[p];
-    if (k0 == k1) {
+    if (k1 >= K) {
+      frame_pair[k1 - K] = p;
+      frame_kf[k1 - K] = k0;
+      frame_ptr[k0 + 1] += 1;
+    } else if (k0 == k1) {
       contrib[tile_of(k0, k0)].push_back(p * 4 + CONTRIB_PAIR);
       contrib[tile_of(k0, k0)].push_back(p * 4 + CONTRIB_PAIR_T);
     } else if (k0 > k1) {
@@ -474,6 +623,13 @@ cudaError_t window_solver_create(int K, int C, const std::vector<int>& pair_k0, 
   const size_t o_tr = put(tile_row.data(), T), o_tc = put(tile_col.data(), T), o_cp = put(cptr.data(), T + 1);
   const size_t o_cf = put(cflat.data(), cflat.size()), o_dg = put(diag.data(), K);
   const size_t o_rt = put(row_tiles.data(), row_tiles.size());
+  for (int k = 0; k < K; ++k) frame_ptr[k + 1] += frame_ptr[k];
+  {
+    std::vector<int> next(frame_ptr.begin(), frame_ptr.end() - 1);
+    for (int f = 0; f < F; ++f) frame_list[next[frame_kf[f]]++] = f;
+  }
+  const size_t o_fp = put(frame_ptr.data(), K + 1), o_fl = put(frame_list.data(), F);
+  const size_t o_fr = put(frame_pair.data(), F), o_fk = put(frame_kf.data(), F);
   blob.resize((blob.size() + 3) & ~(size_t)3, 0);  // UpdTask is 16-byte aligned
   const size_t o_tk = put(reinterpret_cast<const int*>(tasks.data()), tasks.size() * 4);
   std::vector<unsigned char> fixed((size_t)K * B, 0);
@@ -485,11 +641,16 @@ cudaError_t window_solver_create(int K, int C, const std::vector<int>& pair_k0, 
   if ((e = cudaMalloc((void**)&s->codes, (size_t)K * C * sizeof(double))) != cudaSuccess) return e;
   if ((e = cudaMalloc((void**)&s->tiles, (size_t)(T + K) * B * B * sizeof(double))) != cudaSuccess) return e;
   if ((e = cudaMalloc((void**)&s->rhs, (size_t)K * B * sizeof(double))) != cudaSuccess) return e;
+  if (F > 0) {
+    if ((e = cudaMalloc((void**)&s->frame_L, (size_t)F * 36 * sizeof(double))) != cudaSuccess) return e;
+    if ((e = cudaMalloc((void**)&s->frame_bad, (size_t)F * sizeof(int))) != cudaSuccess) return e;
+  }
   if ((e = cudaMemcpy(s->ints, blob.data(), blob.size() * sizeof(int), cudaMemcpyHostToDevice)) != cudaSuccess) return e;
   if ((e = cudaMemcpy(s->fixed, fixed.data(), fixed.size(), cudaMemcpyHostToDevice)) != cudaSuccess) return e;
   const int* ip = static_cast<const int*>(s->ints);
   s->tile_row = ip + o_tr; s->tile_col = ip + o_tc; s->contrib_ptr = ip + o_cp; s->contrib = ip + o_cf;
   s->diag_tile = ip + o_dg; s->row_tiles = ip + o_rt;
+  s->frame_ptr = ip + o_fp; s->frame_list = ip + o_fl; s->frame_pair = ip + o_fr; s->frame_kf = ip + o_fk;
   s->tasks = reinterpret_cast<const UpdTask*>(ip + o_tk);
   // kernel attributes once, here: no runtime configuration call in a solve
   e = with_code_size(C, [](auto bc) {
@@ -518,6 +679,10 @@ cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_de
   a.tile_row = s->tile_row; a.tile_col = s->tile_col; a.contrib_ptr = s->contrib_ptr; a.contrib = s->contrib;
   a.diag_tile = s->diag_tile; a.fixed = s->fixed;
   a.K = s->K; a.P = s->P; a.num_tiles = s->num_tiles;
+  FrameArgs fa{};
+  fa.L = s->L; fa.F = s->F;
+  fa.frame_ptr = s->frame_ptr; fa.frame_list = s->frame_list; fa.frame_pair = s->frame_pair; fa.frame_kf = s->frame_kf;
+  fa.frame_L = s->frame_L; fa.frame_bad = s->frame_bad;
   a.lambda = lambda; a.prior = prior;
   if (prior > 0.0) {
     // pageable source: the copy is staged before the call returns, so the caller may reuse its array at once
@@ -528,11 +693,14 @@ cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_de
   return with_code_size(s->C, [&](auto bc) {
     constexpr int Bv = bc.value;
     uint64_t n = 0;
-    window_solve_load_kernel<Bv><<<s->num_tiles, kThreads, 0, stream>>>(a);
+    if (s->F > 0)
+      window_solve_load_kernel<Bv, true><<<s->num_tiles, kThreads, 0, stream>>>(a, fa);
+    else
+      window_solve_load_kernel<Bv, false><<<s->num_tiles, kThreads, 0, stream>>>(a, fa);
     ++n;
     for (int j = 0; j < s->K; ++j) {
       const int c0 = s->col_ptr[j], nc = s->col_ptr[j + 1] - c0;
-      window_solve_panel_kernel<Bv><<<nc, kThreads, PanelCfg<Bv>::kSmem, stream>>>(a, j, c0);
+      window_solve_panel_kernel<Bv><<<nc, kThreads, PanelCfg<Bv>::kSmem, stream>>>(a, j, c0, s->frame_bad, s->F);
       ++n;
       const int u0 = s->upd_ptr[j], nu = s->upd_ptr[j + 1] - u0;
       if (nu > 0) {
@@ -543,6 +711,10 @@ cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_de
     for (int j = s->K - 1; j >= 0; --j) {
       const int r0 = s->row_ptr[j], nr = s->row_ptr[j + 1] - r0;
       window_solve_backward_kernel<Bv><<<1 + nr, kThreads, (Bv * Bv + Bv) * 8, stream>>>(a, s->row_tiles + r0, j);
+      ++n;
+    }
+    if (s->F > 0) {
+      window_solve_frames_kernel<Bv><<<s->F, 32, 0, stream>>>(a, fa);
       ++n;
     }
     *launches += n;

@@ -145,11 +145,16 @@ class WindowBlocks:
     """The packed block-sparse buffer dfk_window_assemble writes (include/dfk.h, SURVEY 8e): K diagonal blocks B x B,
     K gradients B, P coupling blocks B x 6 ([pose0 | code0] of k0 x pose1 of k1), then f and the inlier total of the
     photometric (scaled) records, then L link blocks B x B ([pose0 | code0] of k0 x [pose1 | code1] of k1), one per
-    sparse geometric link in `geometric`."""
+    sparse geometric link in `geometric`, then F frame blocks 6 x 6 and F frame gradients 6 (dfk_window_create_frames).
+
+    Tracked frames are pose-only variables: a pair (k0, K + f) is frame f's one pair, its coupling block is [pose0 |
+    code0] of k0 x the frame's pose, and its pose1 parts go to frame f's block and gradient.  The dense system orders
+    the frames' variables after the keyframes': frame f at K * B + 6 f."""
     num_keyframes: int
     code_size: int
     pairs: Sequence[Tuple[int, int]]
     geometric: Sequence[Tuple[int, int]] = field(default=())
+    num_frames: int = 0
 
     @property
     def B(self) -> int:
@@ -158,7 +163,12 @@ class WindowBlocks:
     @property
     def floats(self) -> int:
         K, P, B = self.num_keyframes, len(self.pairs), self.B
-        return K * (B * B + B) + P * 6 * B + 2 + len(self.geometric) * B * B
+        return K * (B * B + B) + P * 6 * B + 2 + len(self.geometric) * B * B + 42 * self.num_frames
+
+    @property
+    def dim(self) -> int:
+        """variables of the dense system: K keyframes [pose | code], then F frame poses"""
+        return self.num_keyframes * self.B + 6 * self.num_frames
 
     def offsets(self):
         K, P, B = self.num_keyframes, len(self.pairs), self.B
@@ -172,18 +182,27 @@ class WindowBlocks:
         """start of the link blocks, after f and the inlier total"""
         return self.offsets()[2] + 2
 
+    @property
+    def frame_offset(self) -> int:
+        """start of the frame blocks (F x 36), followed by the frame gradients (F x 6)"""
+        return self.geometric_offset + len(self.geometric) * self.B * self.B
+
     def pack(self, item_pair, JtJ, Jtr, residual, inliers, sizes, geo=None):
         """Host mirror of dfk_window_assemble (numpy, float32 sums in item order): item i belongs to pair item_pair[i];
         JtJ [n, NP, NP] dense, Jtr [n, NP], sizes[i] = (W, H), or (0, 0) for an unscaled record: its residual is added
         to f as it is and its inliers are left out of the inlier total.  geo = (JtJ [L, NG, NG], Jtr [L, NG],
         residual [L]) of the geometric links (dfk_window_assemble_geometric): after the items, the links where a
-        keyframe is k0, then those where it is k1, in link order.  Returns the flat buffer."""
+        keyframe is k0, then those where it is k1, in link order.  A frame pair's pose1 parts go to its frame's block and
+        gradient.  Returns the flat buffer."""
         K, B, c = self.num_keyframes, self.B, self.code_size
         out = np.zeros(self.floats, dtype=np.float32)
         o_g, o_c, o_t = self.offsets()
         D = out[:o_g].reshape(K, B, B)
         g = out[o_g:o_c].reshape(K, B)
         O = out[o_c:o_t].reshape(len(self.pairs), B, 6)
+        F, o_f = self.num_frames, self.frame_offset
+        Df = out[o_f:o_f + 36 * F].reshape(F, 6, 6)
+        gf = out[o_f + 36 * F:o_f + 42 * F].reshape(F, 6)
         loc0 = np.r_[0:6, 12:12 + c]  # [pose0 | code0] rows of a record
         f = np.float32(0)
         ninl = np.float32(0)
@@ -192,9 +211,15 @@ class WindowBlocks:
             H = np.asarray(JtJ[i], dtype=np.float32)
             r = np.asarray(Jtr[i], dtype=np.float32)
             D[k0] += H[np.ix_(loc0, loc0)]
-            D[k1][:6, :6] += H[6:12, 6:12]
+            if k1 < K:
+                D[k1][:6, :6] += H[6:12, 6:12]
+            else:
+                Df[k1 - K] += H[6:12, 6:12]
             g[k0] -= r[loc0]
-            g[k1][:6] -= r[6:12]
+            if k1 < K:
+                g[k1][:6] -= r[6:12]
+            else:
+                gf[k1 - K] -= r[6:12]
             O[p] += H[np.ix_(loc0, np.arange(6, 12))]
             inl = int(inliers[i])
             if is_unscaled(sizes[i]):
@@ -206,7 +231,7 @@ class WindowBlocks:
         if self.geometric:
             gJ, gr, gres = geo
             loc1 = np.r_[6:12, 12 + c:12 + 2 * c]  # [pose1 | code1] rows of a geometric record
-            Lb = out[self.geometric_offset:].reshape(len(self.geometric), B, B)
+            Lb = out[self.geometric_offset:self.frame_offset].reshape(len(self.geometric), B, B)
             for l, (k0, k1) in enumerate(self.geometric):
                 H = np.asarray(gJ[l], dtype=np.float32)
                 D[k0] += H[np.ix_(loc0, loc0)]
@@ -224,30 +249,38 @@ class WindowBlocks:
 
     def to_dense(self, buf):
         """(H [dim, dim], g [dim], f, inliers) of the dense normal equations the buffer stands for (numpy float64, or
-        torch float64 on the buffer's device)."""
-        K, B = self.num_keyframes, self.B
+        torch float64 on the buffer's device); frame f's pose is variables K * B + 6 f ... + 6."""
+        K, B, F, n = self.num_keyframes, self.B, self.num_frames, self.dim
         o_g, o_c, o_t = self.offsets()
         is_torch = hasattr(buf, "detach")
         if is_torch:
             import torch
             b64 = buf.detach().to(torch.float64)
-            H = torch.zeros((K * B, K * B), dtype=torch.float64, device=buf.device)
+            H = torch.zeros((n, n), dtype=torch.float64, device=buf.device)
         else:
             b64 = np.asarray(buf, dtype=np.float64)
-            H = np.zeros((K * B, K * B))
+            H = np.zeros((n, n))
         D = b64[:o_g].reshape(K, B, B)
         for k in range(K):
             H[k * B:(k + 1) * B, k * B:(k + 1) * B] += D[k]
         O = b64[o_c:o_t].reshape(len(self.pairs), B, 6)
         for p, (k0, k1) in enumerate(self.pairs):
-            H[k0 * B:(k0 + 1) * B, k1 * B:k1 * B + 6] += O[p]
-            H[k1 * B:k1 * B + 6, k0 * B:(k0 + 1) * B] += O[p].T if not is_torch else O[p].transpose(0, 1)
+            v1 = k1 * B if k1 < K else K * B + 6 * (k1 - K)  # pose1: a keyframe's, or a frame's
+            H[k0 * B:(k0 + 1) * B, v1:v1 + 6] += O[p]
+            H[v1:v1 + 6, k0 * B:(k0 + 1) * B] += O[p].T if not is_torch else O[p].transpose(0, 1)
         if self.geometric:
-            Lb = b64[self.geometric_offset:self.floats].reshape(len(self.geometric), B, B)
+            Lb = b64[self.geometric_offset:self.frame_offset].reshape(len(self.geometric), B, B)
             for l, (k0, k1) in enumerate(self.geometric):
                 H[k0 * B:(k0 + 1) * B, k1 * B:(k1 + 1) * B] += Lb[l]
                 H[k1 * B:(k1 + 1) * B, k0 * B:(k0 + 1) * B] += Lb[l].T if not is_torch else Lb[l].transpose(0, 1)
         g = b64[o_g:o_c].reshape(K * B)
+        if F:
+            o_f = self.frame_offset
+            Df = b64[o_f:o_f + 36 * F].reshape(F, 6, 6)
+            for f in range(F):
+                H[K * B + 6 * f:K * B + 6 * f + 6, K * B + 6 * f:K * B + 6 * f + 6] += Df[f]
+            gf = b64[o_f + 36 * F:o_f + 42 * F].reshape(6 * F)
+            g = torch.cat([g, gf]) if is_torch else np.concatenate([g, gf])
         return H, g, float(b64[o_t]), float(b64[o_t + 1])
 
 

@@ -85,6 +85,27 @@ def retract(pose, delta, dtype=None) -> np.ndarray:
     return np.concatenate([q, p[4:7] + d[:3]]).astype(dtype or np.asarray(pose).dtype)
 
 
+def so3_log(q) -> np.ndarray:
+    """Sophus::SO3::log of a unit quaternion (x, y, z, w): the rotation vector omega with so3_exp(omega) = +-q."""
+    q = np.asarray(q, dtype=np.float64)
+    v, w = q[:3], float(q[3])
+    n = float(np.linalg.norm(v))
+    if n < 1e-10:
+        scale = 2.0 / w - (2.0 / 3.0) * n * n / (w * w * w)
+    else:
+        # atan of the half angle kept in (-pi/2, pi/2]: the shortest rotation for q and -q alike
+        scale = 2.0 * (np.arctan(n / w) if w != 0 else np.copysign(0.5 * np.pi, 1.0)) / n
+    return scale * v
+
+
+def local(pose0, pose, dtype=np.float64) -> np.ndarray:
+    """The inverse of retract (gtsam_traits.h:66-72): delta = [t - t0 | log(R R0^T)], so retract(pose0, delta) = pose."""
+    p0 = np.asarray(pose0, dtype=np.float64)
+    p = np.asarray(pose, dtype=np.float64)
+    q0i = np.array([-p0[0], -p0[1], -p0[2], p0[3]])
+    return np.concatenate([p[4:7] - p0[4:7], so3_log(quat_mul(p[:4], q0i))]).astype(dtype)
+
+
 def perturb(pose, idx: int, eps: float, dtype=None) -> np.ndarray:
     """tests/testing_utils.h:72-88 GetPerturbedPose."""
     d = np.zeros(6)

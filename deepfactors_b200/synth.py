@@ -64,8 +64,11 @@ def sobel_np(img: np.ndarray) -> np.ndarray:
 def _field(w, h, scale, phase):
     """sum of three sinusoids (periods 7..25 px at scale 1), values in [0, 1]"""
     y, x = np.mgrid[0:h, 0:w].astype(np.float64)
-    x = x * scale
-    y = y * scale
+    return _field_at(x * scale, y * scale, phase)
+
+
+def _field_at(x, y, phase):
+    """the field of _field at level-0 pixel coordinates (x, y) (any shape, not only the pixel grid)"""
     f = (np.sin(2 * np.pi * x / 25.0 + 0.3 + phase) * np.cos(2 * np.pi * y / 19.0 + 1.1 - 0.5 * phase)
          + 0.7 * np.sin(2 * np.pi * (x + 0.6 * y) / 13.0 + 2.0 + 0.7 * phase)
          + 0.5 * np.cos(2 * np.pi * (0.4 * x - y) / 7.0 + 0.5 + 1.3 * phase))
@@ -128,6 +131,20 @@ def make_level(w: int, h: int, code_size: int, *, scale: float = 1.0, seed: int 
     dpt0 = (np.float32(avg_dpt) / prx - np.float32(avg_dpt)).astype(np.float32)
     std0 = np.zeros((h, w), dtype=np.float32)
     return PairLevel(cam, img0, img1, grad1, prx_orig, prx_jac, dpt0, std0)
+
+
+def rotated_view(level: PairLevel, scale: float, omega, phase: float = 0.0) -> np.ndarray:
+    """img0 of a make_level level (pyramid scale `scale`, field phase `phase`) seen by a camera at the same centre
+    rotated by R = exp(omega): the view of a frame whose pose relative to the keyframe's is (R, 0).  A pure rotation
+    maps pixels by a homography whatever the depth, and img0 is an analytic field, so the view is exact (no resampling).
+    The frame's pose is pose0 retracted by [0, 0, 0, omega] (se3.retract)."""
+    cam = level.cam
+    R = se3.quat_to_matrix(se3.so3_exp(omega))
+    v, u = np.mgrid[0:level.height, 0:level.width].astype(np.float64)
+    d = np.stack([(u - cam.u0) / cam.fx, (v - cam.v0) / cam.fy, np.ones_like(u)], axis=-1) @ R.T  # R d, row-wise
+    x = cam.fx * d[..., 0] / d[..., 2] + cam.u0
+    y = cam.fy * d[..., 1] / d[..., 2] + cam.v0
+    return _field_at(x * scale, y * scale, phase)
 
 
 def make_pair(w: int = 640, h: int = 480, code_size: int = 32, levels: int = 4, *, seed: int = 0,

@@ -268,6 +268,38 @@ DfkStatus dfk_window_create_geometric(DfkHandle h, const DfkWindowDesc* desc, in
 DfkStatus dfk_window_assemble_geometric(DfkHandle h, const DfkWindow* w, const float* records_dev,
                                         const float* geo_records_dev, float* window_dev);
 
+/* Tracked frames (Mapper::EnqueueFrame): pose-only variables, one photometric factor keyframe -> frame each.
+ * A window of num_frames frames: a pair whose pair_k1 is K + f is frame f's pair (its pose1 is the frame's pose), and
+ * every frame must be k1 of exactly one pair, never k0, never in a link, and its pair's items must all be scaled
+ * (photometric, one per level).  The buffer is the layout above, links included, followed by
+ *   F frame blocks     6 x 6, row-major: pose1 x pose1 of the frame pair's items
+ *   F frame gradients  6            (-sum Jtr of pose1)
+ * so dfk_window_floats grows by 42 F and no offset above moves.  A frame pair's coupling block is its B x 6 block as
+ * for any pair (rows = k0's [pose | code], columns = the frame's pose); its items count toward f and the inlier total.
+ * Assemble with dfk_window_assemble_geometric (geo_records_dev NULL without links).  num_frames = 0 is
+ * dfk_window_create_geometric.  A rejected call writes nothing. */
+DfkStatus dfk_window_create_frames(DfkHandle h, const DfkWindowDesc* desc, int num_links, const int32_t* link_k0,
+                                   const int32_t* link_k1, int num_frames, DfkWindow** out);
+
+/* A linear prior on one keyframe's [pose | code] (B = 6 + C): [G (B x B row-major, symmetric) | g (B) | f0], doubles */
+#define DFK_PRIOR_DOUBLES(C) ((6 + (C)) * (6 + (C)) + (6 + (C)) + 1)
+/* Marginalise the frames frames_host[0..n) (HOST, copied) of window w: for each, the fp64 sums of its pair's items in
+ * item order give H_aa (k's [pose | code]), H_ab (x frame pose), H_bb (6 x 6), g_a, g_b (= -sum Jtr) and f_p (the
+ * items' rescaled residuals), and prior i (priors_dev + i * DFK_PRIOR_DOUBLES(C), DEVICE) is their Schur complement
+ *   G = H_aa - H_ab H_bb^-1 H_ab^T,  g = g_a - H_ab H_bb^-1 g_b,  f0 = f_p - g_b^T H_bb^-1 g_b
+ * at the point the records were evaluated at (H_bb undamped).  info_dev[i] (DEVICE int32) = 0, or 1 + the row of H_bb
+ * whose pivot was not positive and finite (prior i is then all zero).  One launch, one CTA per frame. */
+DfkStatus dfk_window_marginalize_frames(DfkHandle h, const DfkWindow* w, const float* records_dev, int n,
+                                        const int32_t* frames_host, double* priors_dev, int32_t* info_dev);
+/* Add m priors to an assembled window buffer in place.  Prior i (priors_dev, DEVICE, m * DFK_PRIOR_DOUBLES(C)) is on
+ * keyframe prior_kf_host[i] (HOST, copied) and delta_dev[i * B ..] (DEVICE, m * B doubles) = Local(x0_i, x) of that
+ * keyframe: [t - t0 | log(R R0^T) | c - c0].  It adds G to D_k, g - G delta to g_k and f0 - 2 g^T delta +
+ * delta^T G delta to f (buffer units: f is twice the factor-graph error); the inlier total is unchanged.  Every entry
+ * sums its keyframe's priors in list order in fp64 and is rounded once.  With sharded pairs, call it after the
+ * all-reduce (on every rank), or the priors are counted once per rank.  One launch. */
+DfkStatus dfk_window_add_priors(DfkHandle h, const DfkWindow* w, int m, const int32_t* prior_kf_host,
+                                const double* priors_dev, const double* delta_dev, float* window_dev);
+
 /* Damped block-sparse fp64 Cholesky solve of a window's normal equations, straight from its packed buffer.
  *
  * The system is the dense one the buffer stands for (fp32 entries promoted to fp64, every off-diagonal block mirrored):
@@ -280,7 +312,11 @@ DfkStatus dfk_window_assemble_geometric(DfkHandle h, const DfkWindow* w, const f
  * allocates the workspace: (tiles + K) * B * B doubles for the factor, plus K * B doubles and K * C doubles.
  * A solve is deterministic (two solves of the same buffer are bit for bit equal, on any handle of the same GPU model),
  * asynchronous on the handle's stream, and allocates nothing: one load launch, a panel and an update launch per
- * keyframe column, a backward launch per keyframe. */
+ * keyframe column, a backward launch per keyframe.
+ * A window with F tracked frames (dfk_window_create_frames) adds 6 F variables after the keyframes' (frame f at
+ * K B + 6 f); the system is the dense one with the frames' blocks, and d / max|d| of step 3 run over the frames too.
+ * Frames are leaves: each is eliminated first, into its keyframe's diagonal tile at load (no fill, the symbolic analysis
+ * ignores frame pairs), and its dx follows in one launch after the backward pass. */
 typedef struct DfkWindowSolver DfkWindowSolver;
 /* fixed_vars: HOST, num_fixed distinct window-variable indices k * B + r (e.g. 0..5 = the gauge keyframe's pose), copied.
  * Out-of-range or duplicated indices are rejected. */
@@ -298,8 +334,9 @@ typedef struct {
 
 /* window_dev: the packed buffer of dfk_window_assemble[_geometric] for this solver's window (DEVICE, fp32, read only).
  * codes: HOST, K * C doubles, required iff code_prior_weight > 0 (read before the call returns).
- * dx_dev: DEVICE, K * B doubles, fully written.  info_dev: DEVICE, one int32: 0, or 1 + the first variable (in
- * elimination order) whose pivot was not positive and finite; dx is then all zero.
+ * dx_dev: DEVICE, K * B + 6 F doubles, fully written.  info_dev: DEVICE, one int32: 0, or 1 + the first variable (in
+ * elimination order: the frames first, then the keyframes) whose pivot was not positive and finite; dx is then all
+ * zero.
  * Every argument is checked before anything is enqueued; a rejected call writes nothing. */
 DfkStatus dfk_window_solve(DfkHandle h, const DfkWindowSolver* s, const float* window_dev, const DfkWindowSolveParams* p,
                            const double* codes, double* dx_dev, int32_t* info_dev);

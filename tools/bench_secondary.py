@@ -22,6 +22,11 @@ One JSON line per case:
     random positive definite window buffers of window200 (50 keyframes, 200 pairs of bench.window_pairs) at C = 32 and
     C = 128 and ba2k (200 keyframes, 2000 pairs) at C = 32 -- wall clock to a synchronise, the two alternated; then a
     torch.profiler run of one device solve: device time, launches, and the fp64 flops of the fill pattern over it.
+  * tracked frames (`--only frames`): one window200 linearisation + dfk_window_solve (SfmWindowProblem.linearise +
+    .solve, 50 keyframes, 200 pairs, 4 levels 640x480, C = 32) without frames and with one frame per keyframe (50
+    frames, 200 more RunStep items in the same launch), the device solve alone for both, and one marginalisation of
+    the 50 frames (SfmWindowProblem.marginalize: their 200 items re-evaluated + dfk_window_marginalize_frames + the
+    read-back): wall clock to a synchronise and summed device time (torch.profiler, separate run).
 Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` runs
 those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
@@ -42,7 +47,7 @@ sys.path.insert(0, ROOT)
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
-    ap.add_argument("--only", choices=["reprojection", "geometric", "solve"], default=None)
+    ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames"], default=None)
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -70,6 +75,8 @@ def main():
         return geometric_cases(args, torch, print)
     if args.only == "solve":
         return solve_cases(args, torch, print)
+    if args.only == "frames":
+        return frames_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -447,6 +454,72 @@ def geometric_cases(args, torch, print):
                           "timing": "wall clock to the end of the assembly (synchronised); device time = summed kernel + "
                                     "copy time, torch.profiler"}), flush=True)
 
+
+def frames_cases(args, torch, print):
+    """window200 with and without one tracked frame per keyframe: linearisation + device solve, the solve alone, and the
+    marginalisation of the 50 frames"""
+    import numpy as np
+    from deepfactors_b200 import se3, synth
+    from deepfactors_b200.aligners import SfmAligner
+    from deepfactors_b200.window_opt import SfmWindowProblem, TrackedFrame
+    sys.path.insert(0, ROOT)
+    from bench import window_pairs
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
+    cs, levels, num_kf = 32, 4, 50
+    base = synth.make_pair(640, 480, cs, levels, seed=7)
+    shared = [dict(img=up(L.img0), grad=up(L.grad1), prx_orig=up(L.prx_orig), prx_jac=up(L.prx_jac)) for L in base.levels]
+    keyframes = [[dict(sh, dpt=torch.zeros_like(sh["img"]), valid=torch.zeros_like(sh["img"])) for sh in shared]
+                 for _ in range(num_kf)]
+    frame_levels = [dict(img=up(L.img1), grad=up(L.grad1)) for L in base.levels]
+    frames = [TrackedFrame(k, frame_levels) for k in range(num_kf)]
+    pairs = window_pairs(num_kf, 200)
+    cams = [L.cam for L in base.levels]
+    al = SfmAligner(cs)
+    poses = np.stack([se3.make_pose([0.001 * (k % 7), 0.0, 0.0], [0.002 * (k % 5), 0.0, 0.0], np.float64)
+                      for k in range(num_kf)])
+    fposes = np.stack([se3.make_pose([0.0, 0.001 * (k % 3), 0.0], [0.0, 0.002 * (k % 4), 0.0], np.float64)
+                       for k in range(num_kf)])
+    codes = np.zeros((num_kf, cs))
+    reps = max(5, args.reps // 2)
+    fixed = tuple(range(6))
+    for n_frames in (0, num_kf):
+        prob = SfmWindowProblem(al, cams, keyframes, pairs, frames=frames[:n_frames] or None)
+        todo = list(range(len(prob.pairs)))
+        fp = fposes[:n_frames] if n_frames else None
+        buf, _ = prob.linearise(poses, codes, todo, fp)
+
+        def lin_solve():
+            b, _ = prob.linearise(poses, codes, todo, fp)
+            prob.solve(b, 1e-4, fixed)
+
+        def solve():
+            prob.solve(buf, 1e-4, fixed)
+
+        assert prob.solve(buf, 1e-4, fixed) is not None
+        for what, fn in (("linearisation + device solve", lin_solve), ("device solve", solve)):
+            print(json.dumps({"case": f"window200 {what} (50 keyframes, 200 pairs, 4 levels 640x480, C=32) + "
+                                      f"{n_frames} tracked frames",
+                              "us_per_call": _wall_us(torch, fn, reps), "device_us_per_call": _device_us(torch, fn, reps),
+                              "timing": "wall clock to a synchronise (the solve reads dx back); device time = summed "
+                                        "kernel + copy time, torch.profiler"}), flush=True)
+        if n_frames:
+            which = list(range(n_frames))
+
+            def marg():
+                prob.marginalize(poses, codes, fposes, which)
+
+            from torch.profiler import ProfilerActivity, profile
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                marg()
+                torch.cuda.synchronize()
+            kern = sum(e.device_time for e in prof.events()
+                       if e.device_type.name == "CUDA" and "window_marginalize" in e.name)
+            print(json.dumps({"case": f"window200 marginalisation of {n_frames} tracked frames (their {n_frames * levels} "
+                                      "RunStep items re-evaluated + dfk_window_marginalize_frames + read-back)",
+                              "us_per_call": _wall_us(torch, marg, reps), "device_us_per_call": _device_us(torch, marg, reps),
+                              "marginalize_kernel_us": kern,
+                              "timing": "wall clock to a synchronise; device time = summed kernel + copy time, "
+                                        "torch.profiler"}), flush=True)
 
 
 def solve_fill(K, links):
