@@ -131,6 +131,14 @@ SYMBOLS = {
                                                 C.c_void_p]),
     "dfk_window_add_priors": (C.c_int, [_H, C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p,
                                         C.c_void_p]),
+    "dfk_window_create_priors": (C.c_int, [_H, C.POINTER(DfkWindowDesc), C.c_int, C.POINTER(C.c_int32),
+                                           C.POINTER(C.c_int32), C.c_int, C.c_int, C.POINTER(C.c_int32),
+                                           C.POINTER(C.c_int32), C.POINTER(C.c_void_p)]),
+    "dfk_window_add_keyframe_priors": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dfk_window_blanket": (C.c_int, [_H, C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "dfk_window_marginalize_keyframe": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_double,
+                                                  C.POINTER(C.c_double), C.c_void_p, C.c_void_p]),
     "dfk_window_solver_create": (C.c_int, [_H, C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_void_p)]),
     "dfk_window_solver_destroy": (C.c_int, [_H, C.c_void_p]),
     "dfk_window_solver_tiles": (C.c_int, [_H, C.c_void_p, C.POINTER(C.c_size_t)]),
@@ -196,3 +204,12 @@ def prior_doubles(code_size: int) -> int:
     """DFK_PRIOR_DOUBLES: a linear keyframe prior [G (B x B) | g (B) | f0], B = 6 + code_size"""
     b = 6 + code_size
     return b * b + b + 1
+
+
+def kf_prior_doubles(code_size: int, n: int) -> int:
+    """DFK_KF_PRIOR_DOUBLES: a keyframe prior over n keyframes [G (nB x nB) | g (nB) | f0], B = 6 + code_size"""
+    nb = n * (6 + code_size)
+    return nb * nb + nb + 1
+
+
+MAX_BLANKET = 16  # DFK_MAX_BLANKET

@@ -434,14 +434,16 @@ class Window:
     buffer; it is the one buffer a multi-GPU Gauss-Newton step all-reduces.  `geometric` lists the window's sparse
     geometric links (k0, k1), one record each (SparseGeometricLinearizeBatch); their blocks follow the scalars.
     `num_frames` tracked frames (pose-only variables, dfk_window_create_frames): a pair (k, K + f) is frame f's one
-    photometric pair; the frames' blocks follow the links'."""
+    photometric pair; the frames' blocks follow the links'.  `kf_priors` lists the keyframes of each keyframe prior
+    (dfk_window_create_priors, ascending lists); their prior blocks follow the frames'."""
 
     def __init__(self, aligner: "SfmAligner", num_keyframes: int, pairs, item_pair, item_sizes, geometric=(),
-                 num_frames: int = 0):
+                 num_frames: int = 0, kf_priors=()):
         from .factors import WindowBlocks
         self._al = aligner
         self.layout = WindowBlocks(int(num_keyframes), aligner.CS, [tuple(map(int, p)) for p in pairs],
-                                   [tuple(map(int, p)) for p in geometric], int(num_frames))
+                                   [tuple(map(int, p)) for p in geometric], int(num_frames),
+                                   [tuple(int(k) for k in p) for p in kf_priors])
         k0 = np.ascontiguousarray([p[0] for p in self.layout.pairs], dtype=np.int32)
         k1 = np.ascontiguousarray([p[1] for p in self.layout.pairs], dtype=np.int32)
         ip = np.ascontiguousarray(item_pair, dtype=np.int32)
@@ -455,10 +457,24 @@ class Window:
         g1 = np.ascontiguousarray([p[1] for p in self.layout.geometric], dtype=np.int32)
         L = len(g0)
         self.w = C.c_void_p()
-        check(aligner.handle, lib().dfk_window_create_frames(aligner.handle, C.byref(desc), L,
-                                                             g0.ctypes.data_as(I32) if L else None,
-                                                             g1.ctypes.data_as(I32) if L else None, int(num_frames),
-                                                             C.byref(self.w)))
+        kp = self.layout.kf_priors
+        if kp:
+            pp = np.ascontiguousarray(np.cumsum([0] + [len(p) for p in kp]), dtype=np.int32)
+            pk = np.ascontiguousarray([k for p in kp for k in p], dtype=np.int32)
+            check(aligner.handle, lib().dfk_window_create_priors(aligner.handle, C.byref(desc), L,
+                                                                 g0.ctypes.data_as(I32) if L else None,
+                                                                 g1.ctypes.data_as(I32) if L else None, int(num_frames),
+                                                                 len(kp), pp.ctypes.data_as(I32),
+                                                                 pk.ctypes.data_as(I32), C.byref(self.w)))
+        else:
+            check(aligner.handle, lib().dfk_window_create_frames(aligner.handle, C.byref(desc), L,
+                                                                 g0.ctypes.data_as(I32) if L else None,
+                                                                 g1.ctypes.data_as(I32) if L else None, int(num_frames),
+                                                                 C.byref(self.w)))
+        # doubles of each keyframe prior and of its deltas, and where each starts in the back-to-back buffers
+        self.kf_prior_sizes = [_lib.kf_prior_doubles(aligner.CS, len(p)) for p in kp]
+        self.kf_prior_doubles = int(sum(self.kf_prior_sizes))
+        self.kf_delta_doubles = int(sum(len(p) for p in kp)) * self.layout.B
         self.num_items = len(ip)
         self.floats = int(lib().dfk_window_floats(self.w))
         assert self.floats == self.layout.floats
@@ -521,6 +537,80 @@ class Window:
                                                 C.c_void_p(priors.data_ptr()), C.c_void_p(delta.data_ptr()),
                                                 C.c_void_p(buf.data_ptr())))
         return buf
+
+    def add_keyframe_priors(self, buf: torch.Tensor, priors: torch.Tensor, delta: torch.Tensor) -> torch.Tensor:
+        """dfk_window_add_keyframe_priors, in place on an assembled buffer: the window's keyframe priors back to back in
+        `priors` (float64 on the device, kf_prior_doubles entries) at `delta` (float64, kf_delta_doubles: Local(x0, x) of
+        every member, prior by prior).  With sharded pairs, call it after the all-reduce.  Asynchronous on torch's current
+        stream."""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        _check_tensor(hd, buf, torch.float32, self.floats, "buf")
+        if not self.layout.kf_priors:
+            return buf
+        _check_tensor(hd, priors, torch.float64, self.kf_prior_doubles, "priors")
+        _check_tensor(hd, delta, torch.float64, self.kf_delta_doubles, "delta")
+        check(hd.h, lib().dfk_window_add_keyframe_priors(hd.h, self.w, C.c_void_p(priors.data_ptr()),
+                                                         C.c_void_p(delta.data_ptr()), C.c_void_p(buf.data_ptr())))
+        return buf
+
+    def blanket(self, m: int):
+        """dfk_window_blanket: the ascending keyframes that share a factor with keyframe m"""
+        out = np.zeros(max(self.layout.num_keyframes, 1), dtype=np.int32)
+        n = C.c_int32(0)
+        check(self._al.handle, lib().dfk_window_blanket(self._al.handle, self.w, int(m),
+                                                        out.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(n)))
+        return [int(k) for k in out[:n.value]]
+
+    def marginalize_keyframe(self, records: torch.Tensor, m: int, geo_records: torch.Tensor | None = None,
+                             frame_priors: torch.Tensor | None = None, frame_delta: torch.Tensor | None = None,
+                             kf_priors: torch.Tensor | None = None, kf_delta: torch.Tensor | None = None,
+                             code_prior_weight: float = 0.0, code=None, prior: torch.Tensor | None = None,
+                             info: torch.Tensor | None = None):
+        """dfk_window_marginalize_keyframe: the keyframe prior over blanket(m) that eliminating keyframe m leaves (the
+        Schur complement of m's [pose | code], undamped, of every factor touching m).  records / geo_records: the
+        window's records on the device; frame_priors [r, DFK_PRIOR_DOUBLES] / frame_delta [r, B]: the frame priors on m
+        and their deltas; kf_priors / kf_delta: the window's keyframe priors as add_keyframe_priors takes them (needed
+        when one contains m); code_prior_weight / code (host, C): the zero-code prior on m.  Returns (prior
+        [DFK_KF_PRIOR_DOUBLES(C, n)] float64, info [1] int32), device tensors written asynchronously on torch's current
+        stream; info = 0, or 1 + the row of m's block whose pivot failed (the prior is then zero)."""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        cs, B = self.layout.code_size, self.layout.B
+        _check_tensor(hd, records, torch.float32, self.num_items * _lib.record_floats(cs), "records")
+        geo = None
+        if geo_records is not None:
+            _check_tensor(hd, geo_records, torch.float32, len(self.layout.geometric) * _lib.geo_record_floats(cs),
+                          "geo_records")
+            geo = C.c_void_p(geo_records.data_ptr())
+        r = 0
+        if frame_priors is not None:
+            r = frame_priors.numel() // _lib.prior_doubles(cs)
+            _check_tensor(hd, frame_priors, torch.float64, r * _lib.prior_doubles(cs), "frame_priors")
+            _check_tensor(hd, frame_delta, torch.float64, r * B, "frame_delta")
+        if kf_priors is not None:
+            _check_tensor(hd, kf_priors, torch.float64, self.kf_prior_doubles, "kf_priors")
+            _check_tensor(hd, kf_delta, torch.float64, self.kf_delta_doubles, "kf_delta")
+        n = len(self.blanket(m))
+        dev = records.device
+        if prior is None:
+            prior = torch.empty(_lib.kf_prior_doubles(cs, n), dtype=torch.float64, device=dev)
+        _check_tensor(hd, prior, torch.float64, _lib.kf_prior_doubles(cs, n), "prior")
+        if info is None:
+            info = torch.empty(1, dtype=torch.int32, device=dev)
+        _check_tensor(hd, info, torch.int32, 1, "info")
+        cp = None
+        if code_prior_weight > 0:
+            c64 = np.ascontiguousarray(code, dtype=np.float64).reshape(-1)
+            if c64.shape != (cs,):
+                raise ValueError(f"code must have {cs} entries")
+            cp = c64.ctypes.data_as(C.POINTER(C.c_double))
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        check(hd.h, lib().dfk_window_marginalize_keyframe(
+            hd.h, self.w, C.c_void_p(records.data_ptr()), geo, int(m), r, ptr(frame_priors) if r else None,
+            ptr(frame_delta) if r else None, ptr(kf_priors), ptr(kf_delta), float(code_prior_weight), cp,
+            C.c_void_p(prior.data_ptr()), C.c_void_p(info.data_ptr())))
+        return prior, info
 
     def close(self):
         if getattr(self, "w", None):

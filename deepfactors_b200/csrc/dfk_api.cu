@@ -102,6 +102,11 @@ struct DfkContext {
   DeviceBuf<float> partials_dev;
   // dfk_window_marginalize_frames / dfk_window_add_priors: the call's index lists (one pageable H2D per call)
   DeviceBuf<int> window_lists;
+  // dfk_window_marginalize_keyframe: the call's lists [refs | tile rows / cols | member locations | update tasks] (one
+  // pageable H2D per call), the code of m, and the local system's workspace (tiles, rhs, f)
+  DeviceBuf<int> marg_lists;
+  DeviceBuf<double> marg_code;
+  DeviceBuf<double> marg_dev;
   // normalised ray tables of the RunStep kernels: they depend on (fx, u0, width, fy, v0, height) only, so they are
   // built once per camera level and reused by every later call (one launch less per evaluation in steady state)
   struct RayTab {
@@ -163,8 +168,15 @@ struct DfkWindow {
   DeviceBuf<int> ints;
   DeviceBuf<float> areas;
   size_t floats = 0;
-  // host copy of the structure, for dfk_window_solver_create
-  std::vector<int> pair_k0, pair_k1, link_k0, link_k1;
+  // host copy of the structure, for dfk_window_solver_create and dfk_window_marginalize_keyframe
+  std::vector<int> pair_k0, pair_k1, link_k0, link_k1, item_pair;
+  // keyframe priors (dfk_window_create_priors): members prior_kf[prior_ptr[q] .. prior_ptr[q + 1]), the prior blocks
+  // (blk_i < blk_j) and their device lists (KfPriorDev)
+  std::vector<int> prior_ptr{0}, prior_kf, blk_i, blk_j;
+  std::vector<long long> prior_off;  // doubles: start of prior q in a priors buffer; back() = the buffer's size
+  DeviceBuf<int> kp_ints;
+  DeviceBuf<long long> kp_off;
+  KfPriorDev kp{};
 };
 
 // damped block-sparse Cholesky of one window (dfk_window_solver_create)
@@ -1302,8 +1314,16 @@ DfkStatus dfk_window_create_geometric(DfkHandle h, const DfkWindowDesc* d, int L
 DfkStatus dfk_window_create_frames(DfkHandle h, const DfkWindowDesc* d, int L, const int32_t* link_k0,
                                    const int32_t* link_k1, int F, DfkWindow** out)
 {
+  return dfk_window_create_priors(h, d, L, link_k0, link_k1, F, 0, nullptr, nullptr, out);
+}
+
+DfkStatus dfk_window_create_priors(DfkHandle h, const DfkWindowDesc* d, int L, const int32_t* link_k0,
+                                   const int32_t* link_k1, int F, int Q, const int32_t* prior_ptr,
+                                   const int32_t* prior_kf, DfkWindow** out)
+{
   return guarded(h, [&] {
-    if (!d || !out || L < 0 || F < 0 || (L > 0 && (!link_k0 || !link_k1)))
+    if (!d || !out || L < 0 || F < 0 || (L > 0 && (!link_k0 || !link_k1)) || Q < 0 ||
+        (Q > 0 && (!prior_ptr || !prior_kf)))
       return fail(h, DFK_ERR_INVALID_ARG, "[Window] null argument");
     *out = nullptr;
     const int K = d->num_keyframes, P = d->num_pairs, n = d->num_items;
@@ -1340,6 +1360,53 @@ DfkStatus dfk_window_create_frames(DfkHandle h, const DfkWindowDesc* d, int L, c
       if (link_k0[l] == link_k1[l])
         return fail(h, DFK_ERR_INVALID_ARG, "[Window] link " + std::to_string(l) + " ties a keyframe to itself");
     }
+    // keyframe priors: non-empty ascending lists of distinct keyframes of the window
+    if (Q > 0 && prior_ptr[0] != 0) return fail(h, DFK_ERR_INVALID_ARG, "[Window] prior_ptr[0] must be 0");
+    for (int q = 0; q < Q; ++q) {
+      if (prior_ptr[q + 1] <= prior_ptr[q])
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] keyframe prior " + std::to_string(q) + " has no keyframe");
+      for (int a = prior_ptr[q]; a < prior_ptr[q + 1]; ++a)
+        if (prior_kf[a] < 0 || prior_kf[a] >= K || (a > prior_ptr[q] && prior_kf[a] <= prior_kf[a - 1]))
+          return fail(h, DFK_ERR_INVALID_ARG, "[Window] keyframe prior " + std::to_string(q) +
+                                                  " is not an ascending list of distinct keyframes of the window");
+    }
+    const int M = Q > 0 ? prior_ptr[Q] : 0;  // members of all priors
+    // prior blocks: the distinct (i < j) of every prior, ascending; the entries of each keyframe and each block in
+    // prior order
+    std::vector<std::pair<int, int>> blocks;
+    for (int q = 0; q < Q; ++q)
+      for (int a = prior_ptr[q]; a < prior_ptr[q + 1]; ++a)
+        for (int c = a + 1; c < prior_ptr[q + 1]; ++c) blocks.push_back({prior_kf[a], prior_kf[c]});
+    std::sort(blocks.begin(), blocks.end());
+    blocks.erase(std::unique(blocks.begin(), blocks.end()), blocks.end());
+    const int NB = (int)blocks.size();
+    std::vector<std::vector<int>> kf_ent(K), blk_ent(NB);
+    for (int q = 0; q < Q; ++q)
+      for (int a = prior_ptr[q]; a < prior_ptr[q + 1]; ++a) {
+        kf_ent[prior_kf[a]].insert(kf_ent[prior_kf[a]].end(), {q, a - prior_ptr[q]});
+        for (int c = a + 1; c < prior_ptr[q + 1]; ++c) {
+          const int b = (int)(std::lower_bound(blocks.begin(), blocks.end(), std::make_pair(prior_kf[a], prior_kf[c])) -
+                              blocks.begin());
+          blk_ent[b].insert(blk_ent[b].end(), {q, a - prior_ptr[q], c - prior_ptr[q]});
+        }
+      }
+    std::vector<int> kp_blob(Q + 1, 0);  // mem_ptr
+    for (int q = 0; q < Q; ++q) kp_blob[q + 1] = prior_ptr[q + 1];
+    const size_t o_kfp = kp_blob.size();
+    kp_blob.push_back(0);
+    for (int k = 0; k < K; ++k) kp_blob.push_back(kp_blob[o_kfp + k] + (int)kf_ent[k].size() / 2);
+    const size_t o_bp = kp_blob.size();
+    kp_blob.push_back(0);
+    for (int b = 0; b < NB; ++b) kp_blob.push_back(kp_blob[o_bp + b] + (int)blk_ent[b].size() / 3);
+    kp_blob.resize((kp_blob.size() + 3) & ~(size_t)3, 0);  // int2 / int3 entries 16-byte aligned
+    const size_t o_ke = kp_blob.size();
+    for (int k = 0; k < K; ++k) kp_blob.insert(kp_blob.end(), kf_ent[k].begin(), kf_ent[k].end());
+    kp_blob.resize((kp_blob.size() + 3) & ~(size_t)3, 0);
+    const size_t o_be = kp_blob.size();
+    for (int b = 0; b < NB; ++b) kp_blob.insert(kp_blob.end(), blk_ent[b].begin(), blk_ent[b].end());
+    std::vector<long long> poff(Q + 1, 0);
+    for (int q = 0; q < Q; ++q)
+      poff[q + 1] = poff[q] + (long long)DFK_KF_PRIOR_DOUBLES(d->code_size, prior_ptr[q + 1] - prior_ptr[q]);
     // one CSR list per key kind (keyframe k0, frame k1, pair): ptr[keys + 1], then the items of each key in item order
     // (the summation order of the gather kernel); an item whose key is outside [0, keys) is in no list.  Returns where
     // the list starts in blob
@@ -1388,11 +1455,33 @@ DfkStatus dfk_window_create_frames(DfkHandle h, const DfkWindowDesc* d, int L, c
     w->dev.num_frames = F;
     w->dev.frame_pair = ints + o_fr;
     const size_t B = 6 + (size_t)d->code_size;
-    w->floats = (size_t)K * (B * B + B) + (size_t)P * 6 * B + 2 + (size_t)L * B * B + (size_t)F * 42;
+    const size_t block_off = (size_t)K * (B * B + B) + (size_t)P * 6 * B + 2 + (size_t)L * B * B + (size_t)F * 42;
+    w->floats = block_off + (size_t)NB * B * B;
     w->pair_k0.assign(d->pair_k0, d->pair_k0 + P);
     w->pair_k1.assign(d->pair_k1, d->pair_k1 + P);
     w->link_k0.assign(link_k0, link_k0 + L);
     w->link_k1.assign(link_k1, link_k1 + L);
+    w->item_pair.assign(d->item_pair, d->item_pair + n);
+    if (Q > 0) {
+      w->prior_ptr.assign(prior_ptr, prior_ptr + Q + 1);
+      w->prior_kf.assign(prior_kf, prior_kf + M);
+      for (const auto& b : blocks) {
+        w->blk_i.push_back(b.first);
+        w->blk_j.push_back(b.second);
+      }
+      w->prior_off = poff;
+      DFK_CUDA(h, w->kp_ints.ensure(kp_blob.size()), upload_failed);
+      DFK_CUDA(h, w->kp_off.ensure(poff.size()), upload_failed);
+      DFK_CUDA(h, cudaMemcpy(w->kp_ints.ptr, kp_blob.data(), kp_blob.size() * sizeof(int), cudaMemcpyHostToDevice),
+               upload_failed);
+      DFK_CUDA(h, cudaMemcpy(w->kp_off.ptr, poff.data(), poff.size() * sizeof(long long), cudaMemcpyHostToDevice),
+               upload_failed);
+      const int* kpi = w->kp_ints.ptr;
+      w->kp.num_priors = Q; w->kp.num_blocks = NB; w->kp.block_off = block_off;
+      w->kp.mem_ptr = kpi; w->kp.off = w->kp_off.ptr;
+      w->kp.kf_ptr = kpi + o_kfp; w->kp.kf_ent = reinterpret_cast<const int2*>(kpi + o_ke);
+      w->kp.blk_ptr = kpi + o_bp; w->kp.blk_ent = reinterpret_cast<const int3*>(kpi + o_be);
+    }
     *out = w.release();
     return DFK_OK;
   });
@@ -1418,6 +1507,10 @@ DfkStatus dfk_window_assemble(DfkHandle h, const DfkWindow* w, const float* reco
     DeviceGuard guard(h->device);
     DFK_CUDA(h, launch_window_assemble(w->dev, records_dev, nullptr, window_dev, h->stream), "[Window] kernel launch failed");
     h->launches += 1;
+    if (w->kp.num_blocks > 0)
+      DFK_CUDA(h, cudaMemsetAsync(window_dev + w->kp.block_off, 0, (w->floats - w->kp.block_off) * sizeof(float),
+                                  h->stream),
+               "[Window] kernel launch failed");
     return DFK_OK;
   });
 }
@@ -1434,6 +1527,10 @@ DfkStatus dfk_window_assemble_geometric(DfkHandle h, const DfkWindow* w, const f
     DFK_CUDA(h, launch_window_assemble(w->dev, records_dev, geo_records_dev, window_dev, h->stream),
              "[Window] kernel launch failed");
     h->launches += 1;
+    if (w->kp.num_blocks > 0)  // the prior blocks start at zero: dfk_window_add_keyframe_priors fills them
+      DFK_CUDA(h, cudaMemsetAsync(window_dev + w->kp.block_off, 0, (w->floats - w->kp.block_off) * sizeof(float),
+                                  h->stream),
+               "[Window] kernel launch failed");
     return DFK_OK;
   });
 }
@@ -1499,6 +1596,172 @@ DfkStatus dfk_window_add_priors(DfkHandle h, const DfkWindow* w, int m, const in
   });
 }
 
+DfkStatus dfk_window_add_keyframe_priors(DfkHandle h, const DfkWindow* w, const double* priors_dev,
+                                         const double* delta_dev, float* window_dev)
+{
+  return guarded(h, [&] {
+    if (!w || !window_dev) return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddKeyframePriors] null argument");
+    if (w->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddKeyframePriors] window and handle live on different devices");
+    if (w->kp.num_priors == 0) return DFK_OK;
+    if (!priors_dev || !delta_dev) return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddKeyframePriors] null argument");
+    DeviceGuard guard(h->device);
+    DFK_CUDA(h, launch_window_add_keyframe_priors(w->dev, w->kp, priors_dev, delta_dev, window_dev, h->stream),
+             "[Window::AddKeyframePriors] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+namespace {
+
+// N(m): the keyframes that share a pair, a link or a keyframe prior with m, ascending
+std::vector<int> window_blanket(const DfkWindow* w, int m)
+{
+  const int K = w->dev.num_keyframes;
+  std::vector<char> in(K, 0);
+  auto tie = [&](int a, int b) {
+    if (a < K && b < K && (a == m || b == m)) in[a] = in[b] = 1;
+  };
+  for (size_t p = 0; p < w->pair_k0.size(); ++p) tie(w->pair_k0[p], w->pair_k1[p]);
+  for (size_t l = 0; l < w->link_k0.size(); ++l) tie(w->link_k0[l], w->link_k1[l]);
+  for (size_t q = 0; q + 1 < w->prior_ptr.size(); ++q) {
+    const auto b = w->prior_kf.begin() + w->prior_ptr[q], e = w->prior_kf.begin() + w->prior_ptr[q + 1];
+    if (std::find(b, e, m) != e)
+      for (auto it = b; it != e; ++it) in[*it] = 1;
+  }
+  in[m] = 0;
+  std::vector<int> out;
+  for (int k = 0; k < K; ++k)
+    if (in[k]) out.push_back(k);
+  return out;
+}
+
+bool prior_contains(const DfkWindow* w, int q, int m)
+{
+  const auto b = w->prior_kf.begin() + w->prior_ptr[q], e = w->prior_kf.begin() + w->prior_ptr[q + 1];
+  return std::find(b, e, m) != e;
+}
+
+}  // namespace
+
+DfkStatus dfk_window_blanket(DfkHandle h, const DfkWindow* w, int m, int32_t* kf_out, int32_t* n)
+{
+  return guarded(h, [&] {
+    if (!w || !kf_out || !n) return fail(h, DFK_ERR_INVALID_ARG, "[Window::Blanket] null argument");
+    if (m < 0 || m >= w->dev.num_keyframes)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::Blanket] keyframe " + std::to_string(m) + " is not in the window");
+    const std::vector<int> nb = window_blanket(w, m);
+    std::copy(nb.begin(), nb.end(), kf_out);
+    *n = (int32_t)nb.size();
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_marginalize_keyframe(DfkHandle h, const DfkWindow* w, const float* records_dev,
+                                          const float* geo_records_dev, int m, int num_frame_priors,
+                                          const double* frame_priors_dev, const double* frame_delta_dev,
+                                          const double* kf_priors_dev, const double* kf_delta_dev,
+                                          double code_prior_weight, const double* code_m_host, double* prior_dev,
+                                          int32_t* info_dev)
+{
+  return guarded(h, [&] {
+    const char* what = "[Window::MarginalizeKeyframe] ";
+    auto bad = [&](DfkStatus s, const std::string& msg) { return fail(h, s, what + msg); };
+    if (!w || !records_dev || !prior_dev || !info_dev || num_frame_priors < 0 ||
+        (num_frame_priors > 0 && (!frame_priors_dev || !frame_delta_dev)))
+      return bad(DFK_ERR_INVALID_ARG, "null argument");
+    if (w->device != h->device) return bad(DFK_ERR_INVALID_ARG, "window and handle live on different devices");
+    const int K = w->dev.num_keyframes, C = w->dev.code_size, B = 6 + C;
+    if (m < 0 || m >= K) return bad(DFK_ERR_INVALID_ARG, "keyframe " + std::to_string(m) + " is not in the window");
+    if (w->dev.num_links > 0 && !geo_records_dev)
+      return bad(DFK_ERR_INVALID_ARG, "window has geometric links but no geometric records");
+    if (!(std::isfinite(code_prior_weight) && code_prior_weight >= 0.0))
+      return bad(DFK_ERR_INVALID_ARG, "code_prior_weight must be finite and >= 0");
+    if (code_prior_weight > 0.0 && !code_m_host) return bad(DFK_ERR_INVALID_ARG, "code_prior_weight > 0 needs m's code");
+    for (size_t p = 0; p < w->pair_k0.size(); ++p)
+      if (w->pair_k0[p] == m && w->pair_k1[p] >= K)
+        return bad(DFK_ERR_INVALID_ARG, "keyframe " + std::to_string(m) + " still has tracked frames: marginalise them first");
+    const int Q = w->kp.num_priors;
+    std::vector<int> kq;  // the keyframe priors that contain m
+    for (int q = 0; q < Q; ++q)
+      if (prior_contains(w, q, m)) kq.push_back(q);
+    if (!kq.empty() && (!kf_priors_dev || !kf_delta_dev))
+      return bad(DFK_ERR_INVALID_ARG, "keyframe priors contain m but none were given");
+    const std::vector<int> nb = window_blanket(w, m);
+    const int n = (int)nb.size();
+    if (n == 0) return bad(DFK_ERR_INVALID_ARG, "keyframe " + std::to_string(m) + " shares no factor with another");
+    if (n > DFK_MAX_BLANKET)
+      return bad(DFK_ERR_UNSUPPORTED, "blanket of " + std::to_string(n) + " keyframes (at most " +
+                                          std::to_string(DFK_MAX_BLANKET) + ")");
+    std::vector<int> loc(K, -1);
+    loc[m] = 0;
+    for (int i = 0; i < n; ++i) loc[nb[i]] = 1 + i;
+    // [refs | tile_row | tile_col | mem_loc | pad | update tasks]
+    std::vector<int> lists;
+    for (size_t i = 0; i < w->item_pair.size(); ++i) {
+      const int k0 = w->pair_k0[w->item_pair[i]], k1 = w->pair_k1[w->item_pair[i]];
+      if (k1 < K && (k0 == m || k1 == m)) lists.insert(lists.end(), {0, (int)i, loc[k0], loc[k1]});
+    }
+    for (size_t l = 0; l < w->link_k0.size(); ++l)
+      if (w->link_k0[l] == m || w->link_k1[l] == m)
+        lists.insert(lists.end(), {1, (int)l, loc[w->link_k0[l]], loc[w->link_k1[l]]});
+    for (int i = 0; i < num_frame_priors; ++i) lists.insert(lists.end(), {2, i, 0, 0});
+    for (int q : kq) lists.insert(lists.end(), {3, q, 0, 0});
+    const int num_refs = (int)lists.size() / 4;
+    const int T = n + 1 + n * (n + 1) / 2;
+    const size_t o_tr = lists.size();
+    for (int t = 0; t <= n; ++t) lists.push_back(t);
+    for (int I = 1; I <= n; ++I)
+      for (int J = 1; J <= I; ++J) lists.push_back(I);
+    const size_t o_tc = lists.size();
+    for (int t = 0; t <= n; ++t) lists.push_back(0);
+    for (int I = 1; I <= n; ++I)
+      for (int J = 1; J <= I; ++J) lists.push_back(J);
+    const size_t o_ml = lists.size();
+    for (int kf : w->prior_kf) lists.push_back(loc[kf]);
+    lists.resize((lists.size() + 3) & ~(size_t)3, 0);
+    const size_t o_tk = lists.size();
+    std::vector<int> tasks;
+    window_eliminate_first_tasks(n, tasks);
+    lists.insert(lists.end(), tasks.begin(), tasks.end());
+    const size_t ws = (size_t)(T + 1) * B * B + (size_t)(n + 1) * B + 1;
+
+    DeviceGuard guard(h->device);
+    const char* alloc = "[Window::MarginalizeKeyframe] scratch allocation failed";
+    DFK_CUDA(h, h->marg_lists.ensure(lists.size()), alloc);
+    DFK_CUDA(h, h->marg_dev.ensure(ws), alloc);
+    DFK_CUDA(h, h->marg_code.ensure(C), alloc);
+    // pageable sources: staged before the call returns
+    DFK_CUDA(h, cudaMemcpyAsync(h->marg_lists.ptr, lists.data(), lists.size() * sizeof(int), cudaMemcpyHostToDevice,
+                                h->stream), alloc);
+    if (code_prior_weight > 0.0)
+      DFK_CUDA(h, cudaMemcpyAsync(h->marg_code.ptr, code_m_host, C * sizeof(double), cudaMemcpyHostToDevice, h->stream),
+               alloc);
+    const int* li = h->marg_lists.ptr;
+    KfMargDev md{};
+    md.n = n;
+    md.num_refs = num_refs;
+    md.refs = reinterpret_cast<const KfMargRef*>(li);
+    md.tile_row = li + o_tr; md.tile_col = li + o_tc; md.mem_loc = li + o_ml;
+    md.records = records_dev; md.geo = geo_records_dev;
+    md.fpriors = frame_priors_dev; md.fdelta = frame_delta_dev;
+    md.kpriors = kf_priors_dev; md.kdelta = kf_delta_dev;
+    md.w = code_prior_weight; md.code = h->marg_code.ptr;
+    md.tiles = h->marg_dev.ptr;
+    md.rhs = md.tiles + (size_t)(T + 1) * B * B;
+    md.f = md.rhs + (size_t)(n + 1) * B;
+    md.info = info_dev;
+    const char* launch = "[Window::MarginalizeKeyframe] kernel launch failed";
+    DFK_CUDA(h, launch_window_marg_gather(w->dev, w->kp, md, T, h->stream), launch);
+    DFK_CUDA(h, launch_window_eliminate_first(C, n, md.tiles, md.rhs, info_dev, li + o_tk, (int)tasks.size() / 4,
+                                              h->stream), launch);
+    DFK_CUDA(h, launch_window_marg_finalize(C, md, T, prior_dev, h->stream), launch);
+    h->launches += 4;
+    return DFK_OK;
+  });
+}
+
 DfkStatus dfk_window_solver_create(DfkHandle h, const DfkWindow* w, int num_fixed, const int32_t* fixed_vars,
                                    DfkWindowSolver** out)
 {
@@ -1523,8 +1786,8 @@ DfkStatus dfk_window_solver_create(DfkHandle h, const DfkWindow* w, int num_fixe
     if (!s) return oom(h);
     s->device = h->device;
     s->num_vars = n; s->code_size = C; s->num_keyframes = K;
-    DFK_CUDA(h, window_solver_create(K, C, w->dev.num_frames, w->pair_k0, w->pair_k1, w->link_k0, w->link_k1, fixed,
-                                     &s->dev),
+    DFK_CUDA(h, window_solver_create(K, C, w->dev.num_frames, w->pair_k0, w->pair_k1, w->link_k0, w->link_k1, w->blk_i,
+                                     w->blk_j, w->kp.block_off, fixed, &s->dev),
              "[WindowSolver] workspace allocation failed");
     *out = s.release();
     return DFK_OK;

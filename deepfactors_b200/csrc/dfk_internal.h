@@ -214,23 +214,80 @@ cudaError_t launch_window_marginalize_frames(const WindowDev& w, const float* re
 cudaError_t launch_window_add_priors(const WindowDev& w, int m, const int* kf_ptr_dev, const int* kf_priors_dev,
                                      const double* priors_dev, const double* delta_dev, float* window_dev,
                                      cudaStream_t stream);
+// keyframe priors of a window (dfk_window_create_priors), a parameter of their own so that WindowDev and the assembly
+// kernel stay as they are.  Device lists built on the host at create.
+struct KfPriorDev {
+  int num_priors, num_blocks;
+  size_t block_off;          // floats: start of the prior blocks in the window buffer
+  const int* mem_ptr;        // [Q + 1] members of prior q: mem_ptr[q] .. mem_ptr[q + 1] (delta of q at mem_ptr[q] * B)
+  const long long* off;      // [Q] doubles: start of prior q in the priors buffer
+  const int* kf_ptr;         // [K + 1] (prior, position) entries of keyframe k, in prior order ...
+  const int2* kf_ent;        // ... (q, a): keyframe k is member a of prior q
+  const int* blk_ptr;        // [num_blocks + 1] entries of prior block b, in prior order ...
+  const int3* blk_ent;       // ... (q, a, c): the block is G_q's (a, c) block, a < c
+};
+cudaError_t launch_window_add_keyframe_priors(const WindowDev& w, const KfPriorDev& kp, const double* priors_dev,
+                                              const double* delta_dev, float* window_dev, cudaStream_t stream);
+// One factor of the local system of dfk_window_marginalize_keyframe (local keyframe 0 = m, 1..n = its blanket):
+//   kind 0: record item idx, its k0 / k1 are local l0 / l1 (-1: not a local keyframe)
+//   kind 1: geometric link idx, local l0 / l1
+//   kind 2: frame prior idx on m
+//   kind 3: keyframe prior idx of the window (its members' local indices: KfMargDev::mem_loc)
+struct KfMargRef {
+  int kind, idx, l0, l1;
+};
+struct KfMargDev {
+  int n;                      // blanket size; local system (1 + n) B
+  int num_refs;
+  const KfMargRef* refs;      // in summation order
+  const int* tile_row;        // [T] local tile t = (tile_row, tile_col): column 0 first (diagonal first), then 1..n
+  const int* tile_col;
+  const int* mem_loc;         // [members of all priors] local index of each member (indexed like KfPriorDev::mem_ptr)
+  const float* records;
+  const float* geo;
+  const double* fpriors;      // frame priors on m and their deltas
+  const double* fdelta;
+  const double* kpriors;      // the window's keyframe priors and their deltas
+  const double* kdelta;
+  double w;                   // zero-code prior weight, code of m (device)
+  const double* code;
+  double* tiles;              // [T + 1] local tiles B x B (slot T: L of m's block)
+  double* rhs;                // [(1 + n) B] g, local block 0 becomes z = L^-1 g_m
+  double* f;                  // [1]
+  int32_t* info;
+};
+// the local system's tiles, gradient and f: one launch, one CTA per tile + one
+cudaError_t launch_window_marg_gather(const WindowDev& w, const KfPriorDev& kp, const KfMargDev& md, int num_tiles,
+                                      cudaStream_t stream);
+// the prior out of the eliminated local system (after launch_window_eliminate_first): G from the tiles (I, J),
+// 1 <= J <= I <= n, g from rhs blocks 1..n, f0 = f - z^T z; all zero when md.info reports a failed pivot
+cudaError_t launch_window_marg_finalize(int code_size, const KfMargDev& md, int num_tiles, double* prior_dev,
+                                       cudaStream_t stream);
 
 // dfk_window_solve.cu : damped block-sparse fp64 Cholesky of a window buffer.  The symbolic analysis and the workspace
 // (cudaMalloc, on the current device) belong to the solver; a solve allocates nothing.
 struct WindowSolverDev;
 // pairs / links: the window's keyframe lists (a pair whose k1 is K + f belongs to frame f); fixed_vars: distinct
 // variable indices in [0, K (6 + C))
+// prior_i / prior_j: the window's prior blocks (i < j), at prior_off floats into the buffer
 cudaError_t window_solver_create(int num_keyframes, int code_size, int num_frames, const std::vector<int>& pair_k0,
                                  const std::vector<int>& pair_k1, const std::vector<int>& link_k0,
-                                 const std::vector<int>& link_k1, const std::vector<int>& fixed_vars,
-                                 WindowSolverDev** out);
+                                 const std::vector<int>& link_k1, const std::vector<int>& prior_i,
+                                 const std::vector<int>& prior_j, size_t prior_off,
+                                 const std::vector<int>& fixed_vars, WindowSolverDev** out);
 void window_solver_destroy(WindowSolverDev* s);
 size_t window_solver_tiles(const WindowSolverDev* s);
 // codes_host: K * C doubles, read only when prior > 0; *launches += the kernels enqueued
 cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_dev, double lambda, double prior,
                                 const double* codes_host, double* dx_dev, int32_t* info_dev, cudaStream_t stream,
                                 uint64_t* launches);
-
+// Elimination of local keyframe 0 from a local tile system laid out as KfMargDev (tiles 0..n = column 0, diagonal first,
+// then the lower tiles (I, J) of 1..n): the solve's panel launch of column 0 (L of block 0, z = L^-1 g_0, Y_I = H_I0
+// L^-T) and its update launch (H_IJ -= Y_I Y_J^T, g_I -= Y_I z).  info gets 0 or 1 + the failed row.
+cudaError_t launch_window_eliminate_first(int code_size, int n, double* tiles, double* rhs, int32_t* info,
+                                          const void* tasks_dev, int num_tasks, cudaStream_t stream);
+// update tasks of that elimination (16 bytes each), built on the host: (target, a, b, rhs_row)
+void window_eliminate_first_tasks(int n, std::vector<int>& out);
 // dfk_depth.cu : DepthAligner::RunStep
 bool depth_supported(int code_size);
 size_t depth_partial_floats(int code_size);

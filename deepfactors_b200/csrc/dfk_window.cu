@@ -26,7 +26,9 @@
 // frame pair's items are not in any keyframe's k1 list, so without frames nothing changes either.
 //
 // Also here: the marginalisation of frames into linear priors on their keyframe (the Schur complement of the frame's
-// pose, what ISAM2::marginalizeLeaves leaves for a leaf with one factor) and the addition of such priors to a window.
+// pose, what ISAM2::marginalizeLeaves leaves for a leaf with one factor) and the addition of such priors to a window;
+// and for sliding the window, the keyframe priors: their addition to a window, and the gather and the write-out of the
+// marginalisation of a keyframe (its elimination runs the solve's column-0 kernels, dfk_window_solve.cu).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -344,6 +346,256 @@ window_add_priors_kernel(WindowDev w, int m, const int* __restrict__ kf_ptr, con
   if (threadIdx.x == 0) tail[0] = (float)s;
 }
 
+// ---- keyframe priors into an assembled window, in place.  Prior q over keyframes kf_q (n_q of them) at delta_q:
+//   D_k += G_q(a, a),  prior block (i, j) += G_q(a, c),  g_k += (g_q - G_q delta_q)(a),
+//   f += f0_q - 2 g_q^T delta_q + delta_q^T G_q delta_q
+// (k = kf_q[a], i = kf_q[a], j = kf_q[c]).  CTA k < K: keyframe k's block and gradient; CTA K + b: prior block b; CTA
+// K + Qb: f.  Every entry sums its priors in prior order in fp64 onto its fp32 value and is rounded once.
+__device__ __forceinline__ const double* kf_prior(const KfPriorDev& kp, const double* priors, int q)
+{
+  return priors + kp.off[q];
+}
+
+__global__ void __launch_bounds__(256)
+window_add_kf_priors_kernel(WindowDev w, KfPriorDev kp, const double* __restrict__ priors,
+                            const double* __restrict__ delta, float* __restrict__ out)
+{
+  const int C = w.code_size, B = 6 + C, K = w.num_keyframes;
+  const int job = blockIdx.x;
+  if (job < K) {
+    const int k = job, q0 = kp.kf_ptr[k], q1 = kp.kf_ptr[k + 1];
+    if (q0 == q1) return;
+    float* D = out + (size_t)k * B * B;
+    float* g = out + (size_t)K * B * B + (size_t)k * B;
+    for (int e = threadIdx.x; e < B * B + B; e += blockDim.x) {
+      if (e < B * B) {
+        const int r = e / B, c = e - r * B;
+        double s = (double)D[e];
+        for (int q = q0; q < q1; ++q) {
+          const int p = kp.kf_ent[q].x, a = kp.kf_ent[q].y;
+          const size_t nB = (size_t)(kp.mem_ptr[p + 1] - kp.mem_ptr[p]) * B;
+          s = __dadd_rn(s, kf_prior(kp, priors, p)[(a * B + r) * nB + a * B + c]);
+        }
+        D[e] = (float)s;
+      } else {
+        const int r = e - B * B;
+        double s = (double)g[r];
+        for (int q = q0; q < q1; ++q) {
+          const int p = kp.kf_ent[q].x, a = kp.kf_ent[q].y;
+          const int nB = (kp.mem_ptr[p + 1] - kp.mem_ptr[p]) * B;
+          const double* G = kf_prior(kp, priors, p) + (size_t)(a * B + r) * nB;
+          const double* d = delta + (size_t)kp.mem_ptr[p] * B;
+          double gd = 0.0;
+          for (int c = 0; c < nB; ++c) gd = __fma_rn(G[c], d[c], gd);
+          s = __dadd_rn(s, __dsub_rn(kf_prior(kp, priors, p)[(size_t)nB * nB + a * B + r], gd));
+        }
+        g[r] = (float)s;
+      }
+    }
+    return;
+  }
+  if (job < K + kp.num_blocks) {
+    const int b = job - K;
+    float* O = out + kp.block_off + (size_t)b * B * B;
+    for (int e = threadIdx.x; e < B * B; e += blockDim.x) {
+      const int r = e / B, c = e - r * B;
+      double s = (double)O[e];
+      for (int q = kp.blk_ptr[b]; q < kp.blk_ptr[b + 1]; ++q) {
+        const int p = kp.blk_ent[q].x, a = kp.blk_ent[q].y, cc = kp.blk_ent[q].z;
+        const size_t nB = (size_t)(kp.mem_ptr[p + 1] - kp.mem_ptr[p]) * B;
+        s = __dadd_rn(s, kf_prior(kp, priors, p)[(a * B + r) * nB + cc * B + c]);
+      }
+      O[e] = (float)s;
+    }
+    return;
+  }
+  __shared__ double red[8];
+  float* tail = out + (size_t)K * (B * B + B) + (size_t)w.num_pairs * B * 6;
+  double s = (double)tail[0];
+  for (int p = 0; p < kp.num_priors; ++p) {
+    const int nB = (kp.mem_ptr[p + 1] - kp.mem_ptr[p]) * B;
+    const double* P = kf_prior(kp, priors, p);
+    const double* d = delta + (size_t)kp.mem_ptr[p] * B;
+    double gd = 0.0, dGd = 0.0;
+    for (int r = threadIdx.x; r < nB; r += blockDim.x) {
+      double Gd = 0.0;
+      for (int c = 0; c < nB; ++c) Gd = __fma_rn(P[(size_t)r * nB + c], d[c], Gd);
+      gd = __fma_rn(P[(size_t)nB * nB + r], d[r], gd);
+      dGd = __fma_rn(d[r], Gd, dGd);
+    }
+    gd = block_sum(gd, red);
+    dGd = block_sum(dGd, red);
+    s = __dadd_rn(s, __dadd_rn(__fma_rn(-2.0, gd, P[(size_t)nB * nB + nB]), dGd));
+  }
+  if (threadIdx.x == 0) tail[0] = (float)s;
+}
+
+// ---- marginalisation of a keyframe m: the local fp64 system over [m | N(m)] of the factors that touch m (KfMargDev).
+// CTA t < T: local tile t, each entry summing the refs in order; CTA T: the gradient (every thread its rows) and f
+// (block sums in ref order).
+// record rows of local keyframe X's variable r in a pair record (k0 / k1 local l0 / l1): up to two (a self pair)
+__device__ __forceinline__ int pair_rows(const KfMargRef& f, int X, int r, int* rows)
+{
+  int n = 0;
+  if (X == f.l0) rows[n++] = r < 6 ? r : 6 + r;
+  if (X == f.l1 && r < 6) rows[n++] = 6 + r;
+  return n;
+}
+
+__device__ __forceinline__ int member_pos(const KfPriorDev& kp, const KfMargDev& md, int p, int X)
+{
+  for (int a = kp.mem_ptr[p]; a < kp.mem_ptr[p + 1]; ++a)
+    if (md.mem_loc[a] == X) return a - kp.mem_ptr[p];
+  return -1;
+}
+
+__global__ void __launch_bounds__(256)
+window_marg_gather_kernel(WindowDev w, KfPriorDev kp, KfMargDev md, int num_tiles)
+{
+  const int C = w.code_size, B = 6 + C, NP = 12 + C;
+  const int NH = NP * (NP + 1) / 2, REC = NH + NP + 2;
+  const int NG = 12 + 2 * C, NHG = NG * (NG + 1) / 2, RECG = NHG + NG + 2;
+  const int PD = B * B + B + 1;
+  if ((int)blockIdx.x < num_tiles) {
+    const int t = blockIdx.x, I = md.tile_row[t], J = md.tile_col[t];
+    double* T = md.tiles + (size_t)t * B * B;
+    for (int e = threadIdx.x; e < B * B; e += blockDim.x) {
+      const int r = e / B, c = e - r * B;
+      double s = 0.0;
+      for (int q = 0; q < md.num_refs; ++q) {
+        const KfMargRef f = md.refs[q];
+        if (f.kind == 0) {
+          int ra[2], cb[2];
+          const int na = pair_rows(f, I, r, ra), nb = pair_rows(f, J, c, cb);
+          const float* rec = md.records + (size_t)f.idx * REC;
+          for (int u = 0; u < na; ++u)
+            for (int v = 0; v < nb; ++v) s += (double)rec_h(rec, ra[u], cb[v], NP);
+        } else if (f.kind == 1) {
+          const int ra = I == f.l0 ? link_row0(r) : (I == f.l1 ? link_row1(r, C) : -1);
+          const int cb = J == f.l0 ? link_row0(c) : (J == f.l1 ? link_row1(c, C) : -1);
+          if (ra >= 0 && cb >= 0) s += (double)rec_h(md.geo + (size_t)f.idx * RECG, ra, cb, NG);
+        } else if (f.kind == 2) {
+          if (I == 0 && J == 0) s += md.fpriors[(size_t)f.idx * PD + e];
+        } else {
+          const int a = member_pos(kp, md, f.idx, I), b = member_pos(kp, md, f.idx, J);
+          if (a >= 0 && b >= 0) {
+            const size_t nB = (size_t)(kp.mem_ptr[f.idx + 1] - kp.mem_ptr[f.idx]) * B;
+            s += md.kpriors[kp.off[f.idx] + (a * B + r) * nB + b * B + c];
+          }
+        }
+      }
+      if (I == 0 && J == 0 && r == c && r >= 6 && md.w > 0.0) s += md.w;
+      T[e] = s;
+    }
+    return;
+  }
+  // gradient of local variable (X, r), then f
+  const int N = (md.n + 1) * B;
+  for (int v = threadIdx.x; v < N; v += blockDim.x) {
+    const int X = v / B, r = v - X * B;
+    double s = 0.0;
+    for (int q = 0; q < md.num_refs; ++q) {
+      const KfMargRef f = md.refs[q];
+      if (f.kind == 0) {
+        int ra[2];
+        const int na = pair_rows(f, X, r, ra);
+        for (int u = 0; u < na; ++u) s -= (double)md.records[(size_t)f.idx * REC + NH + ra[u]];
+      } else if (f.kind == 1) {
+        const int ra = X == f.l0 ? link_row0(r) : (X == f.l1 ? link_row1(r, C) : -1);
+        if (ra >= 0) s -= (double)md.geo[(size_t)f.idx * RECG + NHG + ra];
+      } else if (f.kind == 2) {
+        if (X == 0) {
+          const double* P = md.fpriors + (size_t)f.idx * PD;
+          const double* d = md.fdelta + (size_t)f.idx * B;
+          double gd = 0.0;
+          for (int c = 0; c < B; ++c) gd = __fma_rn(P[r * B + c], d[c], gd);
+          s += P[B * B + r] - gd;
+        }
+      } else {
+        const int a = member_pos(kp, md, f.idx, X);
+        if (a >= 0) {
+          const int nB = (kp.mem_ptr[f.idx + 1] - kp.mem_ptr[f.idx]) * B;
+          const double* P = md.kpriors + kp.off[f.idx];
+          const double* d = md.kdelta + (size_t)kp.mem_ptr[f.idx] * B;
+          double gd = 0.0;
+          for (int c = 0; c < nB; ++c) gd = __fma_rn(P[(size_t)(a * B + r) * nB + c], d[c], gd);
+          s += P[(size_t)nB * nB + a * B + r] - gd;
+        }
+      }
+    }
+    if (X == 0 && r >= 6 && md.w > 0.0) s -= md.w * md.code[r - 6];
+    md.rhs[v] = s;
+  }
+  __shared__ double red[8];
+  double f = 0.0;  // thread 0's running sum; the block sums below are the same on every thread
+  for (int q = 0; q < md.num_refs; ++q) {
+    const KfMargRef fr = md.refs[q];
+    if (fr.kind == 0) {
+      if (threadIdx.x == 0) {
+        const float* rec = md.records + (size_t)fr.idx * REC;
+        const float area = w.item_area[fr.idx];
+        const uint32_t inl = __float_as_uint(rec[NH + NP + 1]);
+        if (area == 0.0f) f += (double)rec[NH + NP];
+        else if (inl > 0) f += (double)rec[NH + NP] / (double)inl * (double)area;
+      }
+    } else if (fr.kind == 1) {
+      if (threadIdx.x == 0) f += (double)md.geo[(size_t)fr.idx * RECG + NHG + NG];
+    } else {
+      const bool fp = fr.kind == 2;
+      const int nB = fp ? B : (kp.mem_ptr[fr.idx + 1] - kp.mem_ptr[fr.idx]) * B;
+      const double* P = fp ? md.fpriors + (size_t)fr.idx * PD : md.kpriors + kp.off[fr.idx];
+      const double* d = fp ? md.fdelta + (size_t)fr.idx * B : md.kdelta + (size_t)kp.mem_ptr[fr.idx] * B;
+      double gd = 0.0, dGd = 0.0;
+      for (int r = threadIdx.x; r < nB; r += blockDim.x) {
+        double Gd = 0.0;
+        for (int c = 0; c < nB; ++c) Gd = __fma_rn(P[(size_t)r * nB + c], d[c], Gd);
+        gd = __fma_rn(P[(size_t)nB * nB + r], d[r], gd);
+        dGd = __fma_rn(d[r], Gd, dGd);
+      }
+      gd = block_sum(gd, red);
+      dGd = block_sum(dGd, red);
+      f = __dadd_rn(f, __dadd_rn(__fma_rn(-2.0, gd, P[(size_t)nB * nB + nB]), dGd));
+    }
+  }
+  if (threadIdx.x == 0) {
+    if (md.w > 0.0) {
+      double cc = 0.0;
+      for (int c = 0; c < C; ++c) cc = __fma_rn(md.code[c], md.code[c], cc);
+      f = __fma_rn(md.w, cc, f);
+    }
+    *md.f = f;
+    *md.info = 0;  // the elimination's panel launch reports a failed pivot here
+  }
+}
+
+// ---- the prior out of the eliminated local system: CTA u < n(n+1)/2 writes tile (I, J) = G block (I-1, J-1) and its
+// transpose; the last CTA g (local blocks 1..n of the rhs) and f0 = f - z^T z.  A failed pivot: all zero.
+__global__ void __launch_bounds__(256)
+window_marg_finalize_kernel(int C, KfMargDev md, int num_tiles, double* __restrict__ prior)
+{
+  const int B = 6 + C, n = md.n, nB = n * B;
+  const bool bad = *md.info != 0;
+  const int u = blockIdx.x, nt = n * (n + 1) / 2;
+  if (u < nt) {
+    const int t = n + 1 + u, I = md.tile_row[t], J = md.tile_col[t];
+    const double* T = md.tiles + (size_t)t * B * B;
+    for (int e = threadIdx.x; e < B * B; e += blockDim.x) {
+      const int r = e / B, c = e - r * B;
+      if (I == J && r < c) continue;  // a diagonal tile: its lower triangle writes both halves
+      const double v = bad ? 0.0 : T[e];
+      prior[(size_t)((I - 1) * B + r) * nB + (J - 1) * B + c] = v;
+      prior[(size_t)((J - 1) * B + c) * nB + (I - 1) * B + r] = v;
+    }
+    return;
+  }
+  for (int v = threadIdx.x; v < nB; v += blockDim.x) prior[(size_t)nB * nB + v] = bad ? 0.0 : md.rhs[B + v];
+  if (threadIdx.x == 0) {
+    double zz = 0.0;
+    for (int r = 0; r < B; ++r) zz = __fma_rn(md.rhs[r], md.rhs[r], zz);
+    prior[(size_t)nB * nB + nB] = bad ? 0.0 : __dsub_rn(*md.f, zz);
+  }
+}
+
 }  // namespace
 
 cudaError_t launch_window_assemble(const WindowDev& w, const float* records_dev, const float* geo_records_dev,
@@ -367,6 +619,28 @@ cudaError_t launch_window_add_priors(const WindowDev& w, int m, const int* kf_pt
 {
   window_add_priors_kernel<<<w.num_keyframes + 1, 256, 0, stream>>>(w, m, kf_ptr_dev, kf_priors_dev, priors_dev,
                                                                     delta_dev, window_dev);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_add_keyframe_priors(const WindowDev& w, const KfPriorDev& kp, const double* priors_dev,
+                                              const double* delta_dev, float* window_dev, cudaStream_t stream)
+{
+  window_add_kf_priors_kernel<<<w.num_keyframes + kp.num_blocks + 1, 256, 0, stream>>>(w, kp, priors_dev, delta_dev,
+                                                                                       window_dev);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_marg_gather(const WindowDev& w, const KfPriorDev& kp, const KfMargDev& md, int num_tiles,
+                                      cudaStream_t stream)
+{
+  window_marg_gather_kernel<<<num_tiles + 1, 256, 0, stream>>>(w, kp, md, num_tiles);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_marg_finalize(int code_size, const KfMargDev& md, int num_tiles, double* prior_dev,
+                                       cudaStream_t stream)
+{
+  window_marg_finalize_kernel<<<md.n * (md.n + 1) / 2 + 1, 256, 0, stream>>>(code_size, md, num_tiles, prior_dev);
   return cudaGetLastError();
 }
 

@@ -19,6 +19,9 @@
 //   per row j, descending   backward: one CTA per nonzero tile (j, i), i <= j.  Each solves L_jj^T x_j = y_j in shared
 //                          memory (again its own copy); the diagonal CTA writes dx_j, the others y_i -= L_ji^T x_j.
 //   frames         (windows with tracked frames) one launch, one CTA per frame: dx_f = S_f^-1 (g_f - O_f^T dx_k).
+//   prior load     (windows with keyframe priors) right after the load: the prior blocks into their tiles.
+// The column-0 panel and update launches also eliminate a keyframe from the local system of
+// dfk_window_marginalize_keyframe (launch_window_eliminate_first).
 // Every tile and every rhs block receives at most one update per launch and its updates in column order, every sum runs
 // in a fixed order and there are no atomics, so two solves of the same buffer are bit for bit equal.  Ordering comes from
 // stream order only: no CTA ever waits for another.
@@ -234,6 +237,33 @@ __global__ void __launch_bounds__(kThreads) window_solve_load_kernel(SolveArgs a
   }
   if (t == 0 && threadIdx.x == 0) *a.info = 0;
   if constexpr (kFrames) eliminate_frames<B>(a, fa, i, T, eps);
+}
+
+// prior blocks of a window with keyframe priors: a second load launch, one CTA per tile that has prior blocks, so that
+// the load kernel of a window without them stays as it is.  Prior block (i, j), i < j, lands in lower tile (j, i)
+// transposed; the fp64 sum continues from the load kernel's value, blocks in order (to_dense: after the links), and a
+// fixed row or column stays zero.
+struct PriorLoadArgs {
+  const int* tiles;     // tiles with prior blocks
+  const int* blk_ptr;   // [tiles + 1] their prior blocks, ascending
+  const int* blk;
+  size_t off;           // floats: start of the prior blocks in the buffer
+};
+
+template <int B>
+__global__ void __launch_bounds__(kThreads) window_solve_prior_load_kernel(SolveArgs a, PriorLoadArgs pa)
+{
+  const int t = pa.tiles[blockIdx.x];
+  const int i = a.tile_row[t], j = a.tile_col[t];
+  double* T = a.tiles + tile_off(t, B);
+  for (int e = threadIdx.x; e < B * B; e += blockDim.x) {
+    const int r = e / B, c = e - r * B;
+    if (a.fixed[i * B + r] | a.fixed[j * B + c]) continue;
+    double s = T[e];
+    for (int q = pa.blk_ptr[blockIdx.x]; q < pa.blk_ptr[blockIdx.x + 1]; ++q)
+      s += (double)a.buf[pa.off + (size_t)pa.blk[q] * B * B + c * B + r];
+    T[e] = s;
+  }
 }
 
 // ------------------------------------------------------------------------------------------------------------ panel
@@ -492,6 +522,8 @@ cudaError_t with_code_size(int code_size, F&& f)
 // --------------------------------------------------------------------------------------------------------- the plan
 struct WindowSolverDev {
   int K = 0, C = 0, B = 0, P = 0, L = 0, F = 0, num_tiles = 0;
+  int prior_tiles = 0;        // tiles with prior blocks (0: no prior load launch)
+  PriorLoadArgs pa{};
   std::vector<int> col_ptr;   // [K + 1] tiles of column j: [col_ptr[j], col_ptr[j+1]), the first one diagonal
   std::vector<int> upd_ptr;   // [K + 1] update tasks of column j
   std::vector<int> row_ptr;   // [K + 1] backward tiles of row j (off-diagonal, column order)
@@ -525,10 +557,11 @@ size_t window_solver_tiles(const WindowSolverDev* s) { return s ? (size_t)s->num
 
 cudaError_t window_solver_create(int K, int C, int F, const std::vector<int>& pair_k0, const std::vector<int>& pair_k1,
                                  const std::vector<int>& link_k0, const std::vector<int>& link_k1,
+                                 const std::vector<int>& prior_i, const std::vector<int>& prior_j, size_t prior_off,
                                  const std::vector<int>& fixed_vars, WindowSolverDev** out)
 {
   *out = nullptr;
-  const int B = 6 + C, P = (int)pair_k0.size(), L = (int)link_k0.size();
+  const int B = 6 + C, P = (int)pair_k0.size(), L = (int)link_k0.size(), Q = (int)prior_i.size();
   // ---- symbolic elimination in keyframe order: below[j] = rows i > j of the nonzero tiles of column j (a frame pair,
   // k1 >= K, is eliminated at load: no tile, no fill)
   std::vector<std::set<int>> below(K);
@@ -536,6 +569,7 @@ cudaError_t window_solver_create(int K, int C, int F, const std::vector<int>& pa
     if (pair_k0[p] != pair_k1[p] && pair_k1[p] < K)
       below[std::min(pair_k0[p], pair_k1[p])].insert(std::max(pair_k0[p], pair_k1[p]));
   for (int l = 0; l < L; ++l) below[std::min(link_k0[l], link_k1[l])].insert(std::max(link_k0[l], link_k1[l]));
+  for (int q = 0; q < Q; ++q) below[prior_i[q]].insert(prior_j[q]);  // prior_i < prior_j
   for (int j = 0; j < K; ++j) {
     for (auto ia = below[j].begin(); ia != below[j].end(); ++ia)
       for (auto ib = below[j].begin(); ib != ia; ++ib) below[*ib].insert(*ia);  // (ia, ib) fills, ib < ia
@@ -584,6 +618,16 @@ cudaError_t window_solver_create(int K, int C, int F, const std::vector<int>& pa
     if (k0 > k1) contrib[tile_of(k0, k1)].push_back(l * 4 + CONTRIB_LINK);
     else contrib[tile_of(k1, k0)].push_back(l * 4 + CONTRIB_LINK_T);
   }
+  // prior blocks per tile (blocks ascending: in to_dense's order)
+  std::vector<std::vector<int>> pblk(T);
+  for (int q = 0; q < Q; ++q) pblk[tile_of(prior_j[q], prior_i[q])].push_back(q);
+  std::vector<int> ptiles, pptr(1, 0), pflat;
+  for (int t = 0; t < T; ++t)
+    if (!pblk[t].empty()) {
+      ptiles.push_back(t);
+      pflat.insert(pflat.end(), pblk[t].begin(), pblk[t].end());
+      pptr.push_back((int)pflat.size());
+    }
   // ---- update tasks per column, backward tiles per row
   std::vector<UpdTask> tasks;
   s->upd_ptr.assign(K + 1, 0);
@@ -630,6 +674,8 @@ cudaError_t window_solver_create(int K, int C, int F, const std::vector<int>& pa
   }
   const size_t o_fp = put(frame_ptr.data(), K + 1), o_fl = put(frame_list.data(), F);
   const size_t o_fr = put(frame_pair.data(), F), o_fk = put(frame_kf.data(), F);
+  const size_t o_pt = put(ptiles.data(), ptiles.size()), o_pp = put(pptr.data(), pptr.size());
+  const size_t o_pf = put(pflat.data(), pflat.size());
   blob.resize((blob.size() + 3) & ~(size_t)3, 0);  // UpdTask is 16-byte aligned
   const size_t o_tk = put(reinterpret_cast<const int*>(tasks.data()), tasks.size() * 4);
   std::vector<unsigned char> fixed((size_t)K * B, 0);
@@ -652,6 +698,8 @@ cudaError_t window_solver_create(int K, int C, int F, const std::vector<int>& pa
   s->diag_tile = ip + o_dg; s->row_tiles = ip + o_rt;
   s->frame_ptr = ip + o_fp; s->frame_list = ip + o_fl; s->frame_pair = ip + o_fr; s->frame_kf = ip + o_fk;
   s->tasks = reinterpret_cast<const UpdTask*>(ip + o_tk);
+  s->prior_tiles = (int)ptiles.size();
+  s->pa.tiles = ip + o_pt; s->pa.blk_ptr = ip + o_pp; s->pa.blk = ip + o_pf; s->pa.off = prior_off;
   // kernel attributes once, here: no runtime configuration call in a solve
   e = with_code_size(C, [](auto bc) {
     constexpr int Bv = bc.value;
@@ -698,6 +746,10 @@ cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_de
     else
       window_solve_load_kernel<Bv, false><<<s->num_tiles, kThreads, 0, stream>>>(a, fa);
     ++n;
+    if (s->prior_tiles > 0) {
+      window_solve_prior_load_kernel<Bv><<<s->prior_tiles, kThreads, 0, stream>>>(a, s->pa);
+      ++n;
+    }
     for (int j = 0; j < s->K; ++j) {
       const int c0 = s->col_ptr[j], nc = s->col_ptr[j + 1] - c0;
       window_solve_panel_kernel<Bv><<<nc, kThreads, PanelCfg<Bv>::kSmem, stream>>>(a, j, c0, s->frame_bad, s->F);
@@ -718,6 +770,38 @@ cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_de
       ++n;
     }
     *launches += n;
+    return cudaGetLastError();
+  });
+}
+
+// ----------------------------------------------------------------------------------- keyframe marginalisation
+// Local tile system (dfk_window_marginalize_keyframe): tiles 0..n are column 0 ((I, 0), diagonal first), tile n + 1 +
+// (I - 1) I / 2 + J - 1 is (I, J) for 1 <= J <= I <= n, slot T = n + 1 + n (n + 1) / 2 takes L_00.
+void window_eliminate_first_tasks(int n, std::vector<int>& out)
+{
+  out.clear();
+  for (int I = 1; I <= n; ++I)
+    for (int J = 1; J <= I; ++J) {
+      const UpdTask t{n + 1 + (I - 1) * I / 2 + J - 1, I, J, I == J ? I : -1};
+      out.insert(out.end(), {t.target, t.a, t.b, t.rhs_row});
+    }
+}
+
+cudaError_t launch_window_eliminate_first(int code_size, int n, double* tiles, double* rhs, int32_t* info,
+                                          const void* tasks_dev, int num_tasks, cudaStream_t stream)
+{
+  SolveArgs a{};
+  a.tiles = tiles; a.rhs = rhs; a.info = info;
+  a.K = n + 1;
+  a.num_tiles = n + 1 + n * (n + 1) / 2;
+  return with_code_size(code_size, [&](auto bc) {
+    constexpr int Bv = bc.value;
+    cudaError_t e = cudaFuncSetAttribute(window_solve_panel_kernel<Bv>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         PanelCfg<Bv>::kSmem);
+    if (e != cudaSuccess) return e;
+    window_solve_panel_kernel<Bv><<<n + 1, kThreads, PanelCfg<Bv>::kSmem, stream>>>(a, 0, 0, nullptr, 0);
+    if (num_tasks > 0)
+      window_solve_update_kernel<Bv><<<num_tasks, kThreads, 0, stream>>>(a, static_cast<const UpdTask*>(tasks_dev), 0);
     return cudaGetLastError();
   });
 }

@@ -149,21 +149,38 @@ class WindowBlocks:
 
     Tracked frames are pose-only variables: a pair (k0, K + f) is frame f's one pair, its coupling block is [pose0 |
     code0] of k0 x the frame's pose, and its pose1 parts go to frame f's block and gradient.  The dense system orders
-    the frames' variables after the keyframes': frame f at K * B + 6 f."""
+    the frames' variables after the keyframes': frame f at K * B + 6 f.
+
+    Keyframe priors (dfk_window_create_priors): kf_priors[q] is the ascending keyframe list of prior q, and the buffer
+    ends with one B x B prior block per distinct keyframe pair (i < j) of some prior (`prior_blocks`, ascending; rows =
+    keyframe i's [pose | code], columns = j's), at `prior_offset`.  pack leaves them zero; add_keyframe_priors fills
+    them."""
     num_keyframes: int
     code_size: int
     pairs: Sequence[Tuple[int, int]]
     geometric: Sequence[Tuple[int, int]] = field(default=())
     num_frames: int = 0
+    kf_priors: Sequence[Tuple[int, ...]] = field(default=())
 
     @property
     def B(self) -> int:
         return 6 + self.code_size
 
     @property
+    def prior_blocks(self) -> List[Tuple[int, int]]:
+        return sorted({(int(p[a]), int(p[c])) for p in self.kf_priors for a in range(len(p))
+                       for c in range(a + 1, len(p))})
+
+    @property
+    def prior_offset(self) -> int:
+        """start of the prior blocks, after the frames' blocks and gradients"""
+        return self.frame_offset + 42 * self.num_frames
+
+    @property
     def floats(self) -> int:
         K, P, B = self.num_keyframes, len(self.pairs), self.B
-        return K * (B * B + B) + P * 6 * B + 2 + len(self.geometric) * B * B + 42 * self.num_frames
+        return K * (B * B + B) + P * 6 * B + 2 + len(self.geometric) * B * B + 42 * self.num_frames + \
+            len(self.prior_blocks) * B * B
 
     @property
     def dim(self) -> int:
@@ -281,7 +298,45 @@ class WindowBlocks:
                 H[K * B + 6 * f:K * B + 6 * f + 6, K * B + 6 * f:K * B + 6 * f + 6] += Df[f]
             gf = b64[o_f + 36 * F:o_f + 42 * F].reshape(6 * F)
             g = torch.cat([g, gf]) if is_torch else np.concatenate([g, gf])
+        o_p = self.prior_offset
+        for b, (i, j) in enumerate(self.prior_blocks):
+            Pb = b64[o_p + b * B * B:o_p + (b + 1) * B * B].reshape(B, B)
+            H[i * B:(i + 1) * B, j * B:(j + 1) * B] += Pb
+            H[j * B:(j + 1) * B, i * B:(i + 1) * B] += Pb.T if not is_torch else Pb.transpose(0, 1)
         return H, g, float(b64[o_t]), float(b64[o_t + 1])
+
+    def add_keyframe_priors(self, buf, rows, deltas):
+        """Host mirror of dfk_window_add_keyframe_priors, in place on a numpy float32 buffer: rows[q] = keyframe prior q
+        [G | g | f0] over kf_priors[q], deltas[q] its n_q B deltas Local(x0, x).  Each entry sums its priors' terms in fp64
+        in prior order onto its float32 value, rounded once.  Returns buf."""
+        K, B = self.num_keyframes, self.B
+        o_g, _, o_t = self.offsets()
+        blocks = {ij: b for b, ij in enumerate(self.prior_blocks)}
+        acc = {}  # float offset of a B x B block or B gradient -> fp64 running value
+
+        def add(off, size, v):
+            if off not in acc:
+                acc[off] = np.asarray(buf[off:off + size], np.float64).copy()
+            acc[off] = acc[off] + v
+
+        fsum = np.float64(buf[o_t])
+        for q, kfs in enumerate(self.kf_priors):
+            n = len(kfs)
+            row = np.asarray(rows[q], np.float64)
+            d = np.asarray(deltas[q], np.float64).reshape(n * B)
+            G, g, f0 = row[:(n * B) ** 2].reshape(n * B, n * B), row[(n * B) ** 2:(n * B) ** 2 + n * B], row[-1]
+            gr = g - G @ d
+            for a, k in enumerate(kfs):
+                add(k * B * B, B * B, G[a * B:(a + 1) * B, a * B:(a + 1) * B].ravel())
+                add(o_g + k * B, B, gr[a * B:(a + 1) * B])
+                for c in range(a + 1, n):
+                    off = self.prior_offset + blocks[(int(k), int(kfs[c]))] * B * B
+                    add(off, B * B, G[a * B:(a + 1) * B, c * B:(c + 1) * B].ravel())
+            fsum = fsum + (f0 - 2 * g @ d + d @ G @ d)
+        for off, v in acc.items():
+            buf[off:off + v.size] = v.astype(np.float32)
+        buf[o_t] = np.float32(fsum)
+        return buf
 
 
 def shard_pairs(num_pairs: int, world_size: int, rank: int) -> range:

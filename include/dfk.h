@@ -300,6 +300,59 @@ DfkStatus dfk_window_marginalize_frames(DfkHandle h, const DfkWindow* w, const f
 DfkStatus dfk_window_add_priors(DfkHandle h, const DfkWindow* w, int m, const int32_t* prior_kf_host,
                                 const double* priors_dev, const double* delta_dev, float* window_dev);
 
+/* Sliding the window: keyframe priors.  Marginalising a keyframe m out of a window leaves a dense linear prior over its
+ * blanket N(m), the ascending list of the keyframes that share a factor with m (a pair in either direction, a reprojection
+ * or geometric link, or a keyframe prior that contains m).  A keyframe prior over the keyframes kf[0..n) (ascending) is
+ *   [G (nB x nB, symmetric, row-major) | g (nB) | f0]  doubles, rows / columns in the order of its keyframe list,
+ * a factor frozen at the point x0 it was made at: its energy at x is f0 - 2 g^T d + d^T G d, d = Local(x0, x) per member
+ * (buffer units, as for DFK_PRIOR_DOUBLES).  Like the frame priors it is never re-linearised. */
+#define DFK_KF_PRIOR_DOUBLES(C, n) \
+  ((size_t)(n) * (6 + (C)) * (size_t)(n) * (6 + (C)) + (size_t)(n) * (6 + (C)) + 1)
+/* the largest blanket dfk_window_marginalize_keyframe accepts */
+#define DFK_MAX_BLANKET 16
+/* A window that also holds num_kf_priors keyframe priors: prior i covers the keyframes prior_kf[prior_ptr[i] ..
+ * prior_ptr[i + 1]) (HOST arrays, copied; each list non-empty, ascending, distinct and inside the window).  The buffer is
+ * the dfk_window_create_frames layout followed by
+ *   Q prior blocks     B x B, row-major: rows = [pose | code] of keyframe i, columns = [pose | code] of keyframe j
+ * one per distinct keyframe pair (i < j) that occurs in some prior, in ascending (i, j) order, so no offset above moves.
+ * dfk_window_assemble_geometric zeroes the prior blocks; dfk_window_add_keyframe_priors fills them.  num_kf_priors = 0 is
+ * dfk_window_create_frames.  A rejected call writes nothing. */
+DfkStatus dfk_window_create_priors(DfkHandle h, const DfkWindowDesc* desc, int num_links, const int32_t* link_k0,
+                                   const int32_t* link_k1, int num_frames, int num_kf_priors, const int32_t* prior_ptr,
+                                   const int32_t* prior_kf, DfkWindow** out);
+/* Add the window's keyframe priors to an assembled buffer in place.  priors_dev: DEVICE, the priors in window order, each
+ * DFK_KF_PRIOR_DOUBLES(C, n_i) doubles, back to back.  delta_dev: DEVICE, n_i * B doubles per prior, back to back: Local(x0,
+ * x) of each member, [t - t0 | log(R R0^T) | c - c0].  G's diagonal blocks go to D_k, its off-diagonal blocks to the prior
+ * blocks, g - G delta to the gradients and f0 - 2 g^T delta + delta^T G delta to f; the inlier total is unchanged.  Every
+ * entry sums its terms in fp64 in prior order onto its fp32 value and is rounded once (no atomics).  With sharded pairs,
+ * call it after the all-reduce, on every rank.  One launch. */
+DfkStatus dfk_window_add_keyframe_priors(DfkHandle h, const DfkWindow* w, const double* priors_dev,
+                                         const double* delta_dev, float* window_dev);
+/* The blanket N(m) of keyframe m (a host query): kf_out (HOST, at least K - 1 entries) gets the ascending list, *n its
+ * length. */
+DfkStatus dfk_window_blanket(DfkHandle h, const DfkWindow* w, int m, int32_t* kf_out, int32_t* n);
+/* Marginalise keyframe m.  Forms in fp64 the joint system over [m | N(m)] of every factor that touches m, each entry
+ * summing, in this order: the records of m's pairs in item order (records_dev, as dfk_window_assemble reads them: -Jtr,
+ * residuals rescaled), m's geometric links in link order (geo_records_dev; NULL when the window has no links), the
+ * num_frame_priors frame priors on m (frame_priors_dev, DFK_PRIOR_DOUBLES(C) each, at frame_delta_dev, B doubles each),
+ * the window's keyframe priors that contain m (kf_priors_dev / kf_delta_dev as dfk_window_add_keyframe_priors takes them;
+ * NULL when the window has none), and with code_prior_weight w > 0 the zero-code prior on m (w I, -w c_m, w |c_m|^2;
+ * code_m_host: HOST, C doubles).  prior_dev (DEVICE, DFK_KF_PRIOR_DOUBLES(C, n)) gets the Schur complement of m's B
+ * variables, H_mm undamped, as a keyframe prior over N(m) at the point the records were evaluated at:
+ *   G = H_NN - H_Nm H_mm^-1 H_mN,  g = g_N - H_Nm H_mm^-1 g_m,  f0 = f - g_m^T H_mm^-1 g_m.
+ * info_dev (DEVICE int32) = 0, or 1 + the row of H_mm whose pivot was not positive and finite (the prior is then zero).
+ * A keyframe that still has tracked frames (marginalise them first), a blanket larger than DFK_MAX_BLANKET
+ * (DFK_ERR_UNSUPPORTED) and an empty blanket are rejected; a rejected call writes nothing.  Deterministic (two calls are
+ * bit for bit equal), asynchronous on the handle's stream, four launches.  The workspace, the lower B x B tiles of the
+ * local system plus one, (n + 2 + n (n + 1) / 2) B^2 + (n + 1) B + 1 doubles (38 MB at n = 16, C = 128), is the handle's
+ * grow-only scratch. */
+DfkStatus dfk_window_marginalize_keyframe(DfkHandle h, const DfkWindow* w, const float* records_dev,
+                                          const float* geo_records_dev, int m, int num_frame_priors,
+                                          const double* frame_priors_dev, const double* frame_delta_dev,
+                                          const double* kf_priors_dev, const double* kf_delta_dev,
+                                          double code_prior_weight, const double* code_m_host, double* prior_dev,
+                                          int32_t* info_dev);
+
 /* Damped block-sparse fp64 Cholesky solve of a window's normal equations, straight from its packed buffer.
  *
  * The system is the dense one the buffer stands for (fp32 entries promoted to fp64, every off-diagonal block mirrored):
@@ -316,7 +369,9 @@ DfkStatus dfk_window_add_priors(DfkHandle h, const DfkWindow* w, int m, const in
  * A window with F tracked frames (dfk_window_create_frames) adds 6 F variables after the keyframes' (frame f at
  * K B + 6 f); the system is the dense one with the frames' blocks, and d / max|d| of step 3 run over the frames too.
  * Frames are leaves: each is eliminated first, into its keyframe's diagonal tile at load (no fill, the symbolic analysis
- * ignores frame pairs), and its dx follows in one launch after the backward pass. */
+ * ignores frame pairs), and its dx follows in one launch after the backward pass.
+ * A window with keyframe priors (dfk_window_create_priors): every prior block is a nonzero tile of the symbolic analysis,
+ * like a link, and one more load launch adds the prior blocks to their tiles after the links, in to_dense's order. */
 typedef struct DfkWindowSolver DfkWindowSolver;
 /* fixed_vars: HOST, num_fixed distinct window-variable indices k * B + r (e.g. 0..5 = the gauge keyframe's pose), copied.
  * Out-of-range or duplicated indices are rejected. */

@@ -27,8 +27,11 @@ One JSON line per case:
     frames, 200 more RunStep items in the same launch), the device solve alone for both, and one marginalisation of
     the 50 frames (SfmWindowProblem.marginalize: their 200 items re-evaluated + dfk_window_marginalize_frames + the
     read-back): wall clock to a synchronise and summed device time (torch.profiler, separate run).
-Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` runs
-those cases alone.
+  * sliding the window (`--only slide`): window200 at C = 32 and 128, one keyframe marginalised
+    (dfk_window_marginalize_keyframe alone, and SfmWindowProblem.marginalize_keyframe with the re-evaluation of the
+    keyframe's factors), then the device solve of the 49-keyframe slid window with its keyframe prior and without.
+Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` /
+`--only frames` / `--only slide` runs those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -47,7 +50,7 @@ sys.path.insert(0, ROOT)
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
-    ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames"], default=None)
+    ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide"], default=None)
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -77,6 +80,8 @@ def main():
         return solve_cases(args, torch, print)
     if args.only == "frames":
         return frames_cases(args, torch, print)
+    if args.only == "slide":
+        return slide_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -520,6 +525,88 @@ def frames_cases(args, torch, print):
                               "marginalize_kernel_us": kern,
                               "timing": "wall clock to a synchronise; device time = summed kernel + copy time, "
                                         "torch.profiler"}), flush=True)
+
+
+def slide_cases(args, torch, print):
+    """window200 at C = 32 and 128: marginalising one keyframe (the device calls alone, and the whole
+    SfmWindowProblem.marginalize_keyframe with the re-evaluation of its factors), and the device solve of the 49-keyframe
+    window that slides past it, with its keyframe prior and without"""
+    import numpy as np
+    from deepfactors_b200 import se3, synth
+    from deepfactors_b200.aligners import SfmAligner
+    from deepfactors_b200.window_opt import SfmWindowProblem, drop_keyframe
+    sys.path.insert(0, ROOT)
+    from bench import window_pairs
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
+    levels, num_kf = 4, 50
+    reps = max(5, args.reps // 2)
+    for cs in (32, 128):
+        base = synth.make_pair(640, 480, cs, levels, seed=7)
+        shared = [dict(img=up(L.img0), grad=up(L.grad1), prx_orig=up(L.prx_orig), prx_jac=up(L.prx_jac))
+                  for L in base.levels]
+        keyframes = [[dict(sh, dpt=torch.zeros_like(sh["img"]), valid=torch.zeros_like(sh["img"])) for sh in shared]
+                     for _ in range(num_kf)]
+        pairs = window_pairs(num_kf, 200)
+        cams = [L.cam for L in base.levels]
+        al = SfmAligner(cs)
+        poses = np.stack([se3.make_pose([0.001 * (k % 7), 0.0, 0.0], [0.002 * (k % 5), 0.0, 0.0], np.float64)
+                          for k in range(num_kf)])
+        codes = np.zeros((num_kf, cs))
+        prob = SfmWindowProblem(al, cams, keyframes, pairs)
+        m = 0
+        nb = prob.window.blanket(m)
+        prob.linearise(poses, codes, list(range(len(prob.pairs))))
+        w = 1e-2
+
+        def dev_only():
+            prob.window.marginalize_keyframe(prob.records, m, code_prior_weight=w, code=codes[m])
+
+        def whole():
+            prob.marginalize_keyframe(poses, codes, m, code_prior_weight=w)
+
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            dev_only()
+            torch.cuda.synchronize()
+        import re
+        kern = {}  # kernel -> summed device time of one call
+        for e in prof.events():
+            k = re.search(r"(window_\w+_kernel)", e.name) if e.device_type.name == "CUDA" else None
+            if k:
+                kern[k.group(1)] = kern.get(k.group(1), 0.0) + e.device_time
+        items = sum(1 for p in pairs if m in p) * levels
+        print(json.dumps({"case": f"window200 C={cs}: marginalise keyframe {m} (blanket of {len(nb)}, {items} RunStep "
+                                  f"items), dfk_window_marginalize_keyframe alone",
+                          "us_per_call": _wall_us(torch, dev_only, reps),
+                          "device_us_per_call": _device_us(torch, dev_only, reps), "kernels_us": kern,
+                          "timing": "wall clock to a synchronise; device time = summed kernel + copy time, "
+                                    "torch.profiler"}), flush=True)
+        print(json.dumps({"case": f"window200 C={cs}: SfmWindowProblem.marginalize_keyframe of keyframe {m} (re-evaluation "
+                                  "of its factors + the device marginalisation + read-back)",
+                          "us_per_call": _wall_us(torch, whole, reps),
+                          "device_us_per_call": _device_us(torch, whole, reps),
+                          "timing": "wall clock to a synchronise; device time = summed kernel + copy time, "
+                                    "torch.profiler"}), flush=True)
+        prior = prob.marginalize_keyframe(poses, codes, m, code_prior_weight=w)
+        slid = prob.without_keyframe(m, prior)
+        bare = SfmWindowProblem(al, cams, keyframes[1:], [p for p in slid.pairs])
+        ps, cs_ = drop_keyframe(poses, codes, m)
+        fixed = tuple(range(6))
+        for name, pr in (("with its keyframe prior", slid), ("without the prior", bare)):
+            buf, _ = pr.linearise(ps, cs_, list(range(len(pr.pairs))))
+            assert pr.solve(buf, 1e-4, fixed) is not None
+
+            def solve():
+                pr.solve(buf, 1e-4, fixed)
+
+            print(json.dumps({"case": f"window200 C={cs}: device solve of the 49-keyframe slid window {name} "
+                                      f"({pr._solvers[fixed].tiles} tiles)",
+                              "us_per_call": _wall_us(torch, solve, reps),
+                              "device_us_per_call": _device_us(torch, solve, reps),
+                              "timing": "wall clock to a synchronise (the solve reads dx back); device time = summed "
+                                        "kernel + copy time, torch.profiler"}), flush=True)
+        del prob, slid, bare, keyframes, shared
+        torch.cuda.empty_cache()
 
 
 def solve_fill(K, links):
