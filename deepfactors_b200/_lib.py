@@ -75,6 +75,10 @@ class DfkSparseGeometricItem(C.Structure):
                 ("points_xy", C.POINTER(C.c_int32)), ("huber_delta", C.c_float)]
 
 
+class DfkDepthDecodeItem(C.Structure):
+    _fields_ = [("prx_orig", DfkImage), ("prx_jac", DfkImage), ("dpt", DfkImage), ("code", C.POINTER(C.c_float))]
+
+
 class DfkWindowDesc(C.Structure):
     _fields_ = [("num_keyframes", C.c_int32), ("num_pairs", C.c_int32), ("num_items", C.c_int32), ("code_size", C.c_int32),
                 ("pair_k0", C.POINTER(C.c_int32)), ("pair_k1", C.POINTER(C.c_int32)), ("item_pair", C.POINTER(C.c_int32)),
@@ -112,6 +116,7 @@ SYMBOLS = {
                                    _F, _F, _F, C.POINTER(C.c_uint64)]),
     "dfk_sfm_evaluate_error": (C.c_int, [_H, _F, _F, _CAM, _IMG, _IMG, _IMG, _IMG, _IMG, _F,
                                          C.POINTER(C.c_uint64)]),
+    "dfk_sfm_evaluate_error_batch": (C.c_int, [_H, C.POINTER(DfkSfmWorkItem), C.c_int, C.c_void_p]),
     "dfk_sfm_run_step_batch": (C.c_int, [_H, C.POINTER(DfkSfmWorkItem), C.c_int, C.c_int, C.c_void_p]),
     "dfk_sfm_run_step_batch_host": (C.c_int, [_H, C.POINTER(DfkSfmWorkItem), C.c_int, C.c_int, _F]),
     "dfk_sfm_stream_create": (C.c_int, [_H, C.c_int, C.c_int, C.c_size_t, C.c_int, C.POINTER(C.c_void_p)]),
@@ -156,7 +161,11 @@ SYMBOLS = {
                                                  C.POINTER(C.c_int), C.c_float, _F, C.POINTER(C.c_int)]),
     "dfk_sparse_geometric_linearize_batch": (C.c_int, [_H, C.POINTER(DfkSparseGeometricItem), C.c_int, C.c_int,
                                                        C.c_void_p]),
+    "dfk_reprojection_error_batch": (C.c_int, [_H, C.POINTER(DfkReprojectionItem), C.c_int, C.c_int, C.c_void_p]),
+    "dfk_sparse_geometric_error_batch": (C.c_int, [_H, C.POINTER(DfkSparseGeometricItem), C.c_int, C.c_int,
+                                                   C.c_void_p]),
     "dfk_update_depth": (C.c_int, [_H, _F, C.c_int, _IMG, _IMG, C.c_float, _IMG]),
+    "dfk_update_depth_batch": (C.c_int, [_H, C.POINTER(DfkDepthDecodeItem), C.c_int, C.c_int]),
     "dfk_sobel_gradients": (C.c_int, [_H, _IMG, _IMG]),
     "dfk_gaussian_blur_down": (C.c_int, [_H, _IMG, _IMG]),
     "dfk_build_image_pyramid": (C.c_int, [_H, _IMG, _IMG, C.c_int]),

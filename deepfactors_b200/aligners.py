@@ -23,7 +23,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import (DfkCamera, DfkDenseSfmParams, DfkImage, DfkReprojectionItem, DfkSfmAlignerParams, DfkSparseGeometricItem, DfkSfmWorkItem,
+from ._lib import (DfkCamera, DfkDenseSfmParams, DfkDepthDecodeItem, DfkImage, DfkReprojectionItem, DfkSfmAlignerParams, DfkSparseGeometricItem, DfkSfmWorkItem,
                    DfkTrackLevel, check, lib)
 
 
@@ -259,6 +259,42 @@ class SfmAligner:
         check(self._hd.h, st)
         return records
 
+    def EvaluateErrorBatch(self, work_items, out: torch.Tensor | None = None) -> torch.Tensor:
+        """Many EvaluateError items in one launch (dfk_sfm_evaluate_error_batch): work_items from make_work_items, without
+        the fused decode (no `code`: the depth is read from dpt0).  Asynchronous: returns a device tensor [n, 2] float32
+        on torch's current stream, row i = [residual | inliers as uint32 bits] (view column 1 as int32 for the count),
+        each bit for bit what EvaluateError gives for item i alone."""
+        self._hd.use_torch_stream()
+        n = len(work_items)
+        out = _batch_records(self, n, 2, out)
+        check(self._hd.h, lib().dfk_sfm_evaluate_error_batch(self._hd.h, work_items, n, C.c_void_p(out.data_ptr())))
+        return out
+
+    def UpdateDepthBatch(self, items):
+        """Many UpdateDepth calls in one launch (dfk_update_depth_batch): items are dicts with code (host, CS floats),
+        prx_orig, prx_jac and dpt (the output), e.g. one per (keyframe, level), or the array of make_depth_items.
+        avg_dpt is params.sfmparams.avg_dpt.  Item i is bit for bit UpdateDepth(code, prx_orig, prx_jac, avg_dpt, dpt).
+        Asynchronous."""
+        self._hd.use_torch_stream()
+        arr = items if isinstance(items, C.Array) else self.make_depth_items(items)
+        check(self._hd.h, lib().dfk_update_depth_batch(self._hd.h, arr, len(items), self.CS))
+
+    def make_depth_items(self, items: Sequence[dict]):
+        """the ctypes array of UpdateDepthBatch; a float32 C-contiguous code is referenced, not copied, so a caller may
+        build the array once and rewrite the codes in place"""
+        arr = (DfkDepthDecodeItem * max(len(items), 1))()
+        keep = []
+        for k, it in enumerate(items):
+            code = np.ascontiguousarray(it["code"], dtype=np.float32)
+            if code.shape != (self.CS,):
+                raise ValueError(f"code must have {self.CS} entries")
+            keep.append(code)
+            w = arr[k]
+            w.prx_orig, w.prx_jac, w.dpt = _image(it["prx_orig"]), _image(it["prx_jac"], self.CS), _image(it["dpt"])
+            w.code = code.ctypes.data_as(C.POINTER(C.c_float))
+        arr._keepalive = keep
+        return arr
+
     def unpack(self, records: torch.Tensor):
         r = records.detach().cpu().numpy()
         return [JTJJrReductionItem.from_record(r[i], self.CS) for i in range(r.shape[0])]
@@ -389,6 +425,47 @@ def SparseGeometricLinearizeBatch(aligner, items: Sequence[dict], records: torch
     check(aligner.handle, lib().dfk_sparse_geometric_linearize_batch(aligner.handle, arr, n, cs,
                                                                      C.c_void_p(records.data_ptr())))
     return records
+
+
+def make_reprojection_items(items: Sequence[dict], cs: int):
+    """the ctypes array of ReprojectionErrorBatch; a float32 C-contiguous code0 is referenced, not copied, so a caller
+    may build the array once and rewrite poses and codes in place"""
+    keep = []
+    arr = (DfkReprojectionItem * max(len(items), 1))(*[_reprojection_item(it, cs, keep) for it in items])
+    arr._keepalive = keep
+    return arr
+
+
+def make_geometric_items(items: Sequence[dict], cs: int):
+    """the ctypes array of SparseGeometricErrorBatch (code0 / code1 referenced as in make_reprojection_items)"""
+    keep = []
+    arr = (DfkSparseGeometricItem * max(len(items), 1))(*[_geometric_item(it, cs, keep) for it in items])
+    arr._keepalive = keep
+    return arr
+
+
+def ReprojectionErrorBatch(aligner, items, out: torch.Tensor | None = None) -> torch.Tensor:
+    """ReprojectionFactor::error of many factors in one launch (dfk_reprojection_error_batch): the items of
+    ReprojectionLinearizeBatch (dicts, or the array of make_reprojection_items).  Asynchronous: returns a device tensor [n, 2] float32, row i = [b^T b | valid matches as
+    uint32 bits], b^T b bit for bit the residual of factor i's ReprojectionLinearizeBatch record."""
+    aligner._hd.use_torch_stream()
+    cs, n = aligner.CS, len(items)
+    out = _batch_records(aligner, n, 2, out)
+    arr = items if isinstance(items, C.Array) else make_reprojection_items(items, cs)
+    check(aligner.handle, lib().dfk_reprojection_error_batch(aligner.handle, arr, n, cs, C.c_void_p(out.data_ptr())))
+    return out
+
+
+def SparseGeometricErrorBatch(aligner, items, out: torch.Tensor | None = None) -> torch.Tensor:
+    """SparseGeometricFactor::error of many factors in one launch (dfk_sparse_geometric_error_batch): the items of
+    SparseGeometricLinearizeBatch (dicts, or the array of make_geometric_items).  Asynchronous: returns a device tensor [n, 2] float32, row i = [b^T b | valid points
+    as uint32 bits], b^T b bit for bit the residual of factor i's SparseGeometricLinearizeBatch record."""
+    aligner._hd.use_torch_stream()
+    cs, n = aligner.CS, len(items)
+    out = _batch_records(aligner, n, 2, out)
+    arr = items if isinstance(items, C.Array) else make_geometric_items(items, cs)
+    check(aligner.handle, lib().dfk_sparse_geometric_error_batch(aligner.handle, arr, n, cs, C.c_void_p(out.data_ptr())))
+    return out
 
 
 # ------------------------------------------------------------------------------------------- DepthAligner

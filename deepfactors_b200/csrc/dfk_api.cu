@@ -87,6 +87,15 @@ struct DfkContext {
   PinnedBuf<unsigned char> batch_host;   // mirror of batch_dev
   DeviceBuf<float> batch_partials;
   DeviceBuf<unsigned int> batch_counters;
+  // dfk_sfm_evaluate_error_batch, apart from the single-call buffers: the descriptors (one H2D per call), the partials
+  // (one 32-float row per block of every item) and one self-resetting ticket per item (zeroed on allocation)
+  DeviceBuf<EvalErrorDesc> eval_descs;
+  std::vector<EvalErrorDesc> eval_host;
+  DeviceBuf<float> eval_partials;
+  DeviceBuf<unsigned int> eval_counters;
+  // dfk_update_depth_batch: [descriptors | codes] (bytes), one H2D per call from depth_host
+  DeviceBuf<unsigned char> depth_dev;
+  std::vector<unsigned char> depth_host;
 
   // dfk_reprojection_linearize / dfk_sparse_geometric_linearize: [one item's staging block | rows (| err2)]
   DeviceBuf<unsigned char> sparse_dev;
@@ -1030,6 +1039,57 @@ DfkStatus dfk_sfm_evaluate_error(DfkHandle h, const float pose0[7], const float 
   });
 }
 
+DfkStatus dfk_sfm_evaluate_error_batch(DfkHandle h, const DfkSfmWorkItem* items, int n, float* out_dev)
+{
+  return guarded(h, [&] {
+    if (!items || !out_dev || n < 1 || n > 65535)  // blockIdx.y of the kernel is the item
+      return fail(h, DFK_ERR_INVALID_ARG,
+                  "[SfmAligner::EvaluateError batch] null argument / number of items not in [1, 65535]");
+    h->eval_host.resize(n);
+    int max_blocks = 1, rows = 0;
+    for (int i = 0; i < n; ++i) {
+      const DfkSfmWorkItem& w = items[i];
+      const std::string at = " in work item " + std::to_string(i);
+      if (w.code)
+        return fail(h, DFK_ERR_INVALID_ARG,
+                    "[SfmAligner::EvaluateError batch] no fused depth decode: the depth is read from dpt0" + at);
+      const uint32_t W = w.img0.width, H = w.img0.height;
+      if (W == 0 || H == 0 || !img_ok(&w.img0, W, H, 1) || !img_ok(&w.img1, W, H, 1) || !img_ok(&w.dpt0, W, H, 1))
+        return fail(h, DFK_ERR_INVALID_ARG, "[SfmAligner::EvaluateError batch] inconsistent image views" + at);
+      if (!cam_ok(&w.cam, W, H))
+        return fail(h, DFK_ERR_INVALID_ARG,
+                    "[SfmAligner::EvaluateError batch] camera viewport larger than the image views" + at);
+      EvalErrorDesc& d = h->eval_host[i];
+      float p10[7];
+      relative_pose(w.pose1, w.pose0, p10, nullptr, nullptr);
+      d.pc = make_pixel_cam(p10, &w.cam, 1, 0.0f);  // as dfk_sfm_evaluate_error: border 1, min_dpt 0 (dense_sfm.h:91)
+      d.img0 = view_of(&w.img0); d.img1 = view_of(&w.img1); d.dpt0 = view_of(&w.dpt0);
+      d.width = (int)W;
+      d.height = (int)H;
+      d.nblocks = eval_error_blocks(d.width, d.height);
+      d.scratch_row = rows;
+      rows += d.nblocks;
+      max_blocks = std::max(max_blocks, d.nblocks);
+    }
+    DeviceGuard guard(h->device);
+    DFK_CUDA(h, h->eval_descs.ensure((size_t)n), "[SfmAligner::EvaluateError batch] scratch allocation failed");
+    DFK_CUDA(h, h->eval_partials.ensure((size_t)rows * 32), "[SfmAligner::EvaluateError batch] scratch allocation failed");
+    if (h->eval_counters.cap < (size_t)n) {
+      DFK_CUDA(h, h->eval_counters.ensure((size_t)n), "[SfmAligner::EvaluateError batch] scratch allocation failed");
+      DFK_CUDA(h, cudaMemsetAsync(h->eval_counters.ptr, 0, sizeof(unsigned int) * h->eval_counters.cap, h->stream),
+               "[SfmAligner::EvaluateError batch] memset failed");
+    }
+    DFK_CUDA(h, cudaMemcpyAsync(h->eval_descs.ptr, h->eval_host.data(), sizeof(EvalErrorDesc) * n,
+                                cudaMemcpyHostToDevice, h->stream),
+             "[SfmAligner::EvaluateError batch] upload failed");
+    DFK_CUDA(h, launch_eval_error_batch(h->eval_descs.ptr, n, max_blocks, h->params.sfmparams.huber_delta,
+                                        h->eval_partials.ptr, h->eval_counters.ptr, out_dev, h->stream),
+             "[SfmAligner::EvaluateError batch] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
 DfkStatus dfk_se3_run_step(DfkHandle h, const float se3[7], const DfkCamera* cam, const DfkImage* img0,
                            const DfkImage* img1, const DfkImage* dpt0, const DfkImage* grad1, float* JtJ, float* Jtr,
                            float* residual, uint64_t* inliers)
@@ -1235,6 +1295,54 @@ DfkStatus dfk_update_depth(DfkHandle h, const float* code, int code_size, const 
     DFK_CUDA(h, launch_update_depth(h->code_dev.ptr, code_size, (int)W, (int)H, view_of(prx_orig), view_of(prx_jac),
                                     avg_dpt, (float*)dpt_out->ptr, (uint32_t)(dpt_out->pitch_bytes / 4), h->stream),
              "[UpdateDepth] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_update_depth_batch(DfkHandle h, const DfkDepthDecodeItem* items, int n, int code_size)
+{
+  return guarded(h, [&] {
+    if (!items || n < 1 || n > 65535)  // blockIdx.y of the kernel is the item
+      return fail(h, DFK_ERR_INVALID_ARG, "[UpdateDepth batch] null argument / number of items not in [1, 65535]");
+    if (code_size < 1 || code_size > 256) return fail(h, DFK_ERR_UNSUPPORTED, "[UpdateDepth batch] code size out of range");
+    for (int i = 0; i < n; ++i) {
+      const DfkDepthDecodeItem& it = items[i];
+      const uint32_t W = it.dpt.width, H = it.dpt.height;
+      if (!it.code || W == 0 || H == 0 || !img_ok(&it.prx_orig, W, H, 1) || !img_ok(&it.prx_jac, W, H, code_size) ||
+          !img_ok(&it.dpt, W, H, 1))
+        return fail(h, DFK_ERR_INVALID_ARG,
+                    "[UpdateDepth batch] null code or inconsistent image views in item " + std::to_string(i));
+    }
+    DeviceGuard guard(h->device);
+    const size_t desc_bytes = (sizeof(DepthDecodeDesc) * (size_t)n + 15) & ~(size_t)15;
+    const size_t total = desc_bytes + sizeof(float) * (size_t)n * code_size;
+    DFK_CUDA(h, h->depth_dev.ensure(total), "[UpdateDepth batch] scratch allocation failed");
+    h->depth_host.assign(total, 0);
+    DepthDecodeDesc* descs = reinterpret_cast<DepthDecodeDesc*>(h->depth_host.data());
+    float* codes = reinterpret_cast<float*>(h->depth_host.data() + desc_bytes);
+    const float* codes_dev = reinterpret_cast<const float*>(h->depth_dev.ptr + desc_bytes);
+    int max_blocks = 1;
+    for (int i = 0; i < n; ++i) {
+      const DfkDepthDecodeItem& it = items[i];
+      DepthDecodeDesc& d = descs[i];
+      d.prx = view_of(&it.prx_orig);
+      d.jac = view_of(&it.prx_jac);
+      d.dpt = static_cast<float*>(it.dpt.ptr);
+      d.dpt_pitch = (uint32_t)(it.dpt.pitch_bytes / 4);
+      d.code = codes_dev + (size_t)i * code_size;
+      memcpy(codes + (size_t)i * code_size, it.code, sizeof(float) * code_size);
+      d.width = (int)it.dpt.width;
+      d.height = (int)it.dpt.height;
+      d.nblocks = update_depth_blocks(d.width, d.height);
+      d.vector = update_depth_vector(code_size, d.code, d.jac) ? 1 : 0;
+      max_blocks = std::max(max_blocks, d.nblocks);
+    }
+    DFK_CUDA(h, cudaMemcpyAsync(h->depth_dev.ptr, h->depth_host.data(), total, cudaMemcpyHostToDevice, h->stream),
+             "[UpdateDepth batch] upload failed");
+    DFK_CUDA(h, launch_update_depth_batch(code_size, reinterpret_cast<const DepthDecodeDesc*>(h->depth_dev.ptr), n,
+                                          max_blocks, h->params.sfmparams.avg_dpt, h->stream),
+             "[UpdateDepth batch] kernel launch failed");
     h->launches += 1;
     return DFK_OK;
   });
@@ -2128,6 +2236,41 @@ DfkStatus dfk_sparse_geometric_linearize_batch(DfkHandle h, const DfkSparseGeome
                                                 reinterpret_cast<const int2*>(st.payload), h->params.sfmparams.avg_dpt,
                                                 records_dev, h->stream),
              "[SparseGeometricFactor::linearize batch] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_reprojection_error_batch(DfkHandle h, const DfkReprojectionItem* items, int n, int code_size, float* out_dev)
+{
+  return guarded(h, [&] {
+    if (!items || n < 1 || !out_dev)
+      return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::error batch] null argument / empty batch");
+    DeviceGuard guard(h->device);
+    Staged st;
+    DFK_TRY(stage(h, "[ReprojectionFactor::error batch] ", true, items, n, code_size, 0, h->rep_host, h->rep_dev, &st));
+    const float2* query_dev = reinterpret_cast<const float2*>(st.payload);
+    DFK_CUDA(h, launch_reprojection_error(code_size, reinterpret_cast<const ReprojItemDev*>(h->rep_dev.ptr), n, query_dev,
+                                          query_dev + st.total, h->params.sfmparams.avg_dpt, out_dev, h->stream),
+             "[ReprojectionFactor::error batch] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_sparse_geometric_error_batch(DfkHandle h, const DfkSparseGeometricItem* items, int n, int code_size,
+                                           float* out_dev)
+{
+  return guarded(h, [&] {
+    if (!items || n < 1 || !out_dev)
+      return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::error batch] null argument / empty batch");
+    DeviceGuard guard(h->device);
+    Staged st;
+    DFK_TRY(stage(h, "[SparseGeometricFactor::error batch] ", true, items, n, code_size, 0, h->geo_host, h->geo_dev, &st));
+    DFK_CUDA(h, launch_sparse_geometric_error(code_size, reinterpret_cast<const GeoItemDev*>(h->geo_dev.ptr), n,
+                                              reinterpret_cast<const int2*>(st.payload), h->params.sfmparams.avg_dpt,
+                                              out_dev, h->stream),
+             "[SparseGeometricFactor::error batch] kernel launch failed");
     h->launches += 1;
     return DFK_OK;
   });

@@ -176,6 +176,35 @@ cudaError_t launch_se3_track_batch(const Se3TrackDesc* descs_dev, int num_proble
                                    cudaStream_t s);
 cudaError_t launch_eval_error(const PixelCam& pc, float huber_delta, int width, int height, View img0, View img1,
                               View dpt0, float* scratch, unsigned int* counter, float* out_dev /*2*/, cudaStream_t s);
+// One item of dfk_sfm_evaluate_error_batch: what launch_eval_error takes for it, its block count and its scratch rows.
+struct EvalErrorDesc {
+  PixelCam pc;
+  View img0, img1, dpt0;
+  int width, height;
+  int nblocks;      // eval_error_blocks(width, height)
+  int scratch_row;  // first of its nblocks scratch rows (32 floats each)
+};
+// blocks of eval_error_kernel's grid for an item of this size (the batched kernel gives an item exactly as many)
+int eval_error_blocks(int width, int height);
+// Item n: scratch rows [scratch_row, + nblocks), counters[n] (zero, self-resetting), outs[2 n .. + 2) = [residual |
+// inliers (u32 bits)].
+cudaError_t launch_eval_error_batch(const EvalErrorDesc* descs_dev, int num_items, int max_blocks, float huber_delta,
+                                    float* scratch, unsigned int* counters, float* outs, cudaStream_t s);
+// One item of dfk_update_depth_batch: what launch_update_depth takes for it, its block count and kernel body.
+struct DepthDecodeDesc {
+  View prx, jac;
+  float* dpt;
+  uint32_t dpt_pitch;
+  const float* code;  // code_size floats in device scratch
+  int width, height;
+  int nblocks;  // update_depth_blocks(width, height)
+  int vector;   // update_depth_vector(code_size, code, jac)
+};
+// launch_update_depth's grid for a level of this size, and whether it runs the vector kernel (else the generic one)
+int update_depth_blocks(int width, int height);
+bool update_depth_vector(int code_size, const float* code_dev, View jac);
+cudaError_t launch_update_depth_batch(int code_size, const DepthDecodeDesc* descs_dev, int num_items, int max_blocks,
+                                      float avg_dpt, cudaStream_t s);
 cudaError_t launch_warp(const PixelCam& pc, int width, int height, View img0, View img1, View dpt0, float* img2,
                         uint32_t img2_pitch, float* scratch, unsigned int* counter, float* out_dev /*2*/,
                         cudaStream_t s);
@@ -338,6 +367,12 @@ cudaError_t launch_sparse_geometric_rows(int code_size, const GeoItemDev& item, 
 // grid (num_items, 1 or 4 entry slices); records_dev: num_items records of DFK_GEO_RECORD_FLOATS(code_size) floats
 cudaError_t launch_sparse_geometric_records(int code_size, const GeoItemDev* items_dev, int num_items, const int2* points_dev,
                                             float avg_dpt, float* records_dev, cudaStream_t s);
+// error() of a batch: one CTA per item; out_dev: num_items x [b^T b | valid matches / points (u32 bits)], b^T b bit for
+// bit the residual of the item's record from launch_reprojection_records / launch_sparse_geometric_records
+cudaError_t launch_reprojection_error(int code_size, const ReprojItemDev* items_dev, int num_items, const float2* query_dev,
+                                      const float2* train_dev, float avg_dpt, float* out_dev, cudaStream_t s);
+cudaError_t launch_sparse_geometric_error(int code_size, const GeoItemDev* items_dev, int num_items, const int2* points_dev,
+                                          float avg_dpt, float* out_dev, cudaStream_t s);
 
 constexpr int kSimpleMaxBlocks = 1024;
 constexpr int kSimpleScratchFloats = kSimpleMaxBlocks * 32;

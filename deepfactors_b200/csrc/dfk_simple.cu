@@ -225,14 +225,30 @@ se3_track_batch_kernel(const Se3TrackDesc* __restrict__ descs, float huber_delta
 }
 
 // ------------------------------------------------------------------------------ EvaluateError
-__global__ void __launch_bounds__(kThreads)
-eval_error_kernel(PixelCam pc, float huber_delta, int width, int height, View img0, View img1, View dpt0,
-                  float* __restrict__ scratch, unsigned int* __restrict__ counter, float* __restrict__ out)
+// The grid a shared per-pixel body runs on: block() is this block's index and count() the number of blocks of the item,
+// read where the body needs them.  OneGrid is a kernel's whole grid, RowGrid the first `n` blocks of a batched row.
+struct OneGrid {
+  __device__ __forceinline__ unsigned int block() const { return blockIdx.x; }
+  __device__ __forceinline__ unsigned int count() const { return gridDim.x; }
+};
+struct RowGrid {
+  unsigned int n;
+  __device__ __forceinline__ unsigned int block() const { return blockIdx.x; }
+  __device__ __forceinline__ unsigned int count() const { return n; }
+};
+
+// The per-pixel body of DenseSfm_EvaluateError (dense_sfm.h:79-119) for one item on grid g: the Huber-weighted squared
+// error into acc[0] and the inlier count.  Shared by the single and the batched kernel, so an item gives the same sums
+// whichever of the two evaluates it.
+template <class Grid>
+__device__ __forceinline__ void eval_error_accumulate(Grid g, const PixelCam& pc, float huber_delta, int width,
+                                                      int height, View img0, View img1, View dpt0, float (&acc)[1],
+                                                      unsigned int& inl)
 {
-  float acc[1] = {0.0f};
-  unsigned int inl = 0;
+  acc[0] = 0.0f;
+  inl = 0;
   const int area = width * height;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < area; i += gridDim.x * blockDim.x) {
+  for (int i = g.block() * blockDim.x + threadIdx.x; i < area; i += g.count() * blockDim.x) {
     const int y = i / width, x = i - y * width;
     const float d = __ldg(dpt0.ptr + (size_t)y * dpt0.pitch + x);
     const Warped w = warp_pixel((float)x, (float)y, d, pc.q, pc.t, pc.fx, pc.fy, pc.u0, pc.v0, pc.border, pc.ulim,
@@ -246,7 +262,36 @@ eval_error_kernel(PixelCam pc, float huber_delta, int width, int height, View im
     inl += 1;
     acc[0] = fmaf(diff, diff, acc[0]);
   }
+}
+
+__global__ void __launch_bounds__(kThreads)
+eval_error_kernel(PixelCam pc, float huber_delta, int width, int height, View img0, View img1, View dpt0,
+                  float* __restrict__ scratch, unsigned int* __restrict__ counter, float* __restrict__ out)
+{
+  float acc[1];
+  unsigned int inl;
+  eval_error_accumulate(OneGrid{}, pc, huber_delta, width, height, img0, img1, dpt0, acc, inl);
   reduce_finalize<1>(acc, inl, blockIdx.x, gridDim.x, scratch, counter, out);
+}
+
+// N EvaluateError items in one launch.  Row blockIdx.y is item n; it uses the first d.nblocks blocks of the row (what
+// eval_error_kernel's grid would be for it), the rest of the row returns at once and takes no ticket.  Item n owns the
+// scratch rows [d.scratch_row, + nblocks), counters[n] and out[2 n .. + 2).
+__global__ void __launch_bounds__(kThreads)
+eval_error_batch_kernel(const EvalErrorDesc* __restrict__ descs, float huber_delta, float* __restrict__ scratch,
+                        unsigned int* __restrict__ counters, float* __restrict__ outs)
+{
+  const int n = blockIdx.y;
+  const EvalErrorDesc& d = descs[n];
+  const int nblocks = d.nblocks;
+  if ((int)blockIdx.x >= nblocks) return;
+  const PixelCam pc = d.pc;
+  float acc[1];
+  unsigned int inl;
+  eval_error_accumulate(RowGrid{(unsigned int)nblocks}, pc, huber_delta, d.width, d.height, d.img0, d.img1, d.dpt0, acc,
+                        inl);
+  reduce_finalize<1>(acc, inl, blockIdx.x, nblocks, scratch + (size_t)d.scratch_row * 32, counters + n,
+                     outs + 2 * (size_t)n);
 }
 
 // ------------------------------------------------------------------------------ Warp
@@ -295,10 +340,11 @@ squared_error_kernel(int width, int height, View a, View b, float* __restrict__ 
 // ------------------------------------------------------------------------------ UpdateDepth
 // LPP lanes cooperate on one pixel: lane `sub` owns float4 chunks sub, sub+LPP, ... of the C code
 // Jacobians, so a warp reads 32 consecutive float4 (512 contiguous bytes) per instruction.
-template <int C>
-__global__ void __launch_bounds__(kThreads)
-update_depth_kernel(const float* __restrict__ code, int width, int height, View prx, View jac, float avg_dpt,
-                    float* __restrict__ dpt, uint32_t dpt_pitch)
+// The body on grid g (OneGrid / RowGrid); shared by the single and the batched kernel.
+template <int C, class Grid>
+__device__ __forceinline__ void update_depth_pixels(Grid g, const float* __restrict__ code, int width, int height,
+                                                    View prx, View jac, float avg_dpt, float* __restrict__ dpt,
+                                                    uint32_t dpt_pitch)
 {
   constexpr int NV = C / 4;                  // float4 chunks per pixel
   constexpr int LPP = NV < 32 ? NV : 32;     // lanes per pixel
@@ -310,8 +356,8 @@ update_depth_kernel(const float* __restrict__ code, int width, int height, View 
 #pragma unroll
   for (int j = 0; j < CPL; ++j) cd[j] = __ldg(reinterpret_cast<const float4*>(code) + sub + j * LPP);
   const int area = width * height;
-  const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  const int warp_global = (g.block() * blockDim.x + threadIdx.x) >> 5;
+  const int nwarps = (g.count() * blockDim.x) >> 5;
   for (int base = warp_global * PPW; base < area; base += nwarps * PPW) {
     const int p = base + pw;
     float dot = 0.0f;
@@ -338,13 +384,22 @@ update_depth_kernel(const float* __restrict__ code, int width, int height, View 
   }
 }
 
-// generic (any C, any alignment) fallback: one thread per pixel
+template <int C>
 __global__ void __launch_bounds__(kThreads)
-update_depth_generic_kernel(const float* __restrict__ code, int C, int width, int height, View prx, View jac,
-                            float avg_dpt, float* __restrict__ dpt, uint32_t dpt_pitch)
+update_depth_kernel(const float* __restrict__ code, int width, int height, View prx, View jac, float avg_dpt,
+                    float* __restrict__ dpt, uint32_t dpt_pitch)
+{
+  update_depth_pixels<C>(OneGrid{}, code, width, height, prx, jac, avg_dpt, dpt, dpt_pitch);
+}
+
+// generic (any C, any alignment) fallback: one thread per pixel
+template <class Grid>
+__device__ __forceinline__ void update_depth_generic_pixels(Grid g, const float* __restrict__ code, int C, int width,
+                                                            int height, View prx, View jac, float avg_dpt,
+                                                            float* __restrict__ dpt, uint32_t dpt_pitch)
 {
   const int area = width * height;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < area; i += gridDim.x * blockDim.x) {
+  for (int i = g.block() * blockDim.x + threadIdx.x; i < area; i += g.count() * blockDim.x) {
     const int y = i / width, x = i - y * width;
     const float* row = jac.ptr + (size_t)y * jac.pitch + (size_t)x * C;
     float dot = 0.0f;
@@ -352,6 +407,34 @@ update_depth_generic_kernel(const float* __restrict__ code, int C, int width, in
     const float prxv = __ldg(prx.ptr + (size_t)y * prx.pitch + x) + dot;
     dpt[(size_t)y * dpt_pitch + x] = avg_dpt / prxv - avg_dpt;
   }
+}
+
+__global__ void __launch_bounds__(kThreads)
+update_depth_generic_kernel(const float* __restrict__ code, int C, int width, int height, View prx, View jac,
+                            float avg_dpt, float* __restrict__ dpt, uint32_t dpt_pitch)
+{
+  update_depth_generic_pixels(OneGrid{}, code, C, width, height, prx, jac, avg_dpt, dpt, dpt_pitch);
+}
+
+// N depth decodes in one launch.  Row blockIdx.y is item n; it uses the first d.nblocks blocks of the row (the grid
+// launch_update_depth gives the item) and runs the body launch_update_depth would pick for it: update_depth_kernel<C>'s
+// when d.vector is set, else the generic one's.  C = 0: code sizes without a vector kernel (generic only).
+template <int C>
+__global__ void __launch_bounds__(kThreads)
+update_depth_batch_kernel(const DepthDecodeDesc* __restrict__ descs, int code_size, float avg_dpt)
+{
+  const DepthDecodeDesc& d = descs[blockIdx.y];
+  const int nblocks = d.nblocks;
+  if ((int)blockIdx.x >= nblocks) return;
+  if constexpr (C > 0) {
+    if (d.vector) {
+      update_depth_pixels<C>(RowGrid{(unsigned int)nblocks}, d.code, d.width, d.height, d.prx, d.jac, avg_dpt, d.dpt,
+                             d.dpt_pitch);
+      return;
+    }
+  }
+  update_depth_generic_pixels(RowGrid{(unsigned int)nblocks}, d.code, code_size, d.width, d.height, d.prx, d.jac, avg_dpt,
+                              d.dpt, d.dpt_pitch);
 }
 
 // ------------------------------------------------------------------------------ Sobel
@@ -459,16 +542,56 @@ cudaError_t launch_squared_error(int width, int height, View a, View b, float* s
   return cudaGetLastError();
 }
 
-cudaError_t launch_update_depth(const float* code_dev, int code_size, int width, int height, View prx_orig, View jac,
-                                float avg_dpt, float* dpt, uint32_t dpt_pitch, cudaStream_t s)
+cudaError_t launch_eval_error_batch(const EvalErrorDesc* descs_dev, int num_items, int max_blocks, float huber_delta,
+                                    float* scratch, unsigned int* counters, float* outs, cudaStream_t s)
 {
-  const int area = width * height;
-  const bool aligned = (reinterpret_cast<uintptr_t>(jac.ptr) % 16 == 0) && (jac.pitch % 4 == 0) &&
-                       (reinterpret_cast<uintptr_t>(code_dev) % 16 == 0);
-  int blocks = (area + kThreads - 1) / kThreads;
+  const dim3 grid((unsigned)max_blocks, (unsigned)num_items);
+  eval_error_batch_kernel<<<grid, kThreads, 0, s>>>(descs_dev, huber_delta, scratch, counters, outs);
+  return cudaGetLastError();
+}
+
+int eval_error_blocks(int width, int height) { return grid_for(width * height); }
+
+int update_depth_blocks(int width, int height)
+{
+  int blocks = (width * height + kThreads - 1) / kThreads;
   const int cap = 8 * sfm_max_ctas();  // grid-stride loop: one full SM's worth (8 x 256 threads) of blocks per SM
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
+  return blocks;
+}
+
+bool update_depth_vector(int code_size, const float* code_dev, View jac)
+{
+  switch (code_size) {
+    case 4: case 8: case 16: case 32: case 64: case 128: break;
+    default: return false;
+  }
+  return (reinterpret_cast<uintptr_t>(jac.ptr) % 16 == 0) && (jac.pitch % 4 == 0) &&
+         (reinterpret_cast<uintptr_t>(code_dev) % 16 == 0);
+}
+
+cudaError_t launch_update_depth_batch(int code_size, const DepthDecodeDesc* descs_dev, int num_items, int max_blocks,
+                                      float avg_dpt, cudaStream_t s)
+{
+  const dim3 grid((unsigned)max_blocks, (unsigned)num_items);
+  switch (code_size) {
+    case 4: update_depth_batch_kernel<4><<<grid, kThreads, 0, s>>>(descs_dev, code_size, avg_dpt); break;
+    case 8: update_depth_batch_kernel<8><<<grid, kThreads, 0, s>>>(descs_dev, code_size, avg_dpt); break;
+    case 16: update_depth_batch_kernel<16><<<grid, kThreads, 0, s>>>(descs_dev, code_size, avg_dpt); break;
+    case 32: update_depth_batch_kernel<32><<<grid, kThreads, 0, s>>>(descs_dev, code_size, avg_dpt); break;
+    case 64: update_depth_batch_kernel<64><<<grid, kThreads, 0, s>>>(descs_dev, code_size, avg_dpt); break;
+    case 128: update_depth_batch_kernel<128><<<grid, kThreads, 0, s>>>(descs_dev, code_size, avg_dpt); break;
+    default: update_depth_batch_kernel<0><<<grid, kThreads, 0, s>>>(descs_dev, code_size, avg_dpt); break;
+  }
+  return cudaGetLastError();
+}
+
+cudaError_t launch_update_depth(const float* code_dev, int code_size, int width, int height, View prx_orig, View jac,
+                                float avg_dpt, float* dpt, uint32_t dpt_pitch, cudaStream_t s)
+{
+  const bool aligned = update_depth_vector(code_size, code_dev, jac);
+  const int blocks = update_depth_blocks(width, height);
 #define DFK_UD_CASE(CC)                                                                                       \
   case CC:                                                                                                    \
     if (aligned) {                                                                                            \

@@ -35,7 +35,8 @@ namespace {
 // when the correspondence is invalid) and its squared unweighted error; returns whether the correspondence is valid.
 // Shared by the single-factor kernel and the batched one, so the batched rows are those of dfk_reprojection_linearize by
 // construction.
-template <int C>
+// kJac = false writes b (r0[12 + C], r1[12 + C]) and err2 only, so the Jacobian work is dead code.
+template <int C, bool kJac = true>
 __device__ __forceinline__ bool reprojection_match_rows(const ReprojItemDev& it, float2 q, float2 tr, float avg_dpt,
                                                         float* r0, float* r1, float* err2)
 {
@@ -68,7 +69,12 @@ __device__ __forceinline__ bool reprojection_match_rows(const ReprojItemDev& it,
     valid = Z > 0.0f;  // depth > min_dpt (0); bounds are not checked (check_bounds = false)
   }
   if (!valid) {
-    for (int k = 0; k < RW; ++k) { r0[k] = 0.0f; r1[k] = 0.0f; }
+    if constexpr (kJac) {
+      for (int k = 0; k < RW; ++k) { r0[k] = 0.0f; r1[k] = 0.0f; }
+    } else {
+      r0[RW - 1] = 0.0f;
+      r1[RW - 1] = 0.0f;
+    }
     *err2 = 0.0f;
     return false;
   }
@@ -91,21 +97,23 @@ __device__ __forceinline__ bool reprojection_match_rows(const ReprojItemDev& it,
   // the reference (m_estimators.h:44-48): a match that lands exactly on its keypoint makes the whole factor NaN.
   const float a = cauchy_delta / err;
   const float w = fabsf(a) / sqrtf(2.0f) * sqrtf(logf(1.0f + 1.0f / a / a));
-  for (int j = 0; j < 6; ++j) {
-    float s00 = 0.f, s01 = 0.f, s10 = 0.f, s11 = 0.f;
-    for (int k = 0; k < 6; ++k) {
-      s00 += A0[k] * sp.P0[k * 6 + j];
-      s01 += A0[k] * sp.P1[k * 6 + j];
-      s10 += A1[k] * sp.P0[k * 6 + j];
-      s11 += A1[k] * sp.P1[k * 6 + j];
+  if constexpr (kJac) {
+    for (int j = 0; j < 6; ++j) {
+      float s00 = 0.f, s01 = 0.f, s10 = 0.f, s11 = 0.f;
+      for (int k = 0; k < 6; ++k) {
+        s00 += A0[k] * sp.P0[k * 6 + j];
+        s01 += A0[k] * sp.P1[k * 6 + j];
+        s10 += A1[k] * sp.P0[k * 6 + j];
+        s11 += A1[k] * sp.P1[k * 6 + j];
+      }
+      r0[j] = s00 * w / sigma; r0[6 + j] = s01 * w / sigma;
+      r1[j] = s10 * w / sigma; r1[6 + j] = s11 * w / sigma;
     }
-    r0[j] = s00 * w / sigma; r0[6 + j] = s01 * w / sigma;
-    r1[j] = s10 * w / sigma; r1[6 + j] = s11 * w / sigma;
-  }
-  for (int k = 0; k < C; ++k) {
-    const float jc = __ldg(jr + k);
-    r0[12 + k] = jd0 * jc * w / sigma;
-    r1[12 + k] = jd1 * jc * w / sigma;
+    for (int k = 0; k < C; ++k) {
+      const float jc = __ldg(jr + k);
+      r0[12 + k] = jd0 * jc * w / sigma;
+      r1[12 + k] = jd1 * jc * w / sigma;
+    }
   }
   r0[12 + C] = d0 * w / sigma;
   r1[12 + C] = d1 * w / sigma;
@@ -251,7 +259,8 @@ reprojection_records_kernel(const ReprojItemDev* __restrict__ items, const float
 // The per-point body: writes the row r of factor `it`'s point pt (zero when the correspondence is invalid) and returns
 // whether it is valid.  Shared by the single-factor kernel and the batched one, so the batched rows are those of
 // dfk_sparse_geometric_linearize by construction.
-template <int C>
+// kJac = false writes b (r[12 + 2 C]) only, so the Jacobian work is dead code.
+template <int C, bool kJac = true>
 __device__ __forceinline__ bool sparse_geometric_point_row(const GeoItemDev& it, int2 pt, float avg_dpt, float* r)
 {
   constexpr int RW = 13 + 2 * C;
@@ -277,7 +286,11 @@ __device__ __forceinline__ bool sparse_geometric_point_row(const GeoItemDev& it,
     valid = w.valid;
   }
   if (!valid) {
-    for (int k = 0; k < RW; ++k) r[k] = 0.0f;
+    if constexpr (kJac) {
+      for (int k = 0; k < RW; ++k) r[k] = 0.0f;
+    } else {
+      r[RW - 1] = 0.0f;
+    }
     return false;
   }
   const int nx = (int)w.u, ny = (int)w.v;  // pix1.cast<int>()
@@ -296,29 +309,31 @@ __device__ __forceinline__ bool sparse_geometric_point_row(const GeoItemDev& it,
 #pragma unroll
   for (int k = 0; k < 6; ++k) B[k] = T2[k] - (g0 * A0[k] + g1 * A1[k]);
   const float hw = huber_weight(err, huber_delta);
+  if constexpr (kJac) {
 #pragma unroll
-  for (int j = 0; j < 6; ++j) {
-    float s0 = 0.f, s1 = 0.f;
+    for (int j = 0; j < 6; ++j) {
+      float s0 = 0.f, s1 = 0.f;
 #pragma unroll
-    for (int k = 0; k < 6; ++k) {
-      s0 += B[k] * sp.P0[k * 6 + j];
-      s1 += B[k] * sp.P1[k * 6 + j];
+      for (int k = 0; k < 6; ++k) {
+        s0 += B[k] * sp.P0[k * 6 + j];
+        s1 += B[k] * sp.P1[k * 6 + j];
+      }
+      r[j] = s0 * hw;
+      r[6 + j] = s1 * hw;
     }
-    r[j] = s0 * hw;
-    r[6 + j] = s1 * hw;
-  }
-  // pix1_J_dpt = dCam * R * ray ; (R ray).z ; dpt_J_prx = -avg / prx^2
-  const float q0 = sp.R[0] * w.xn + sp.R[1] * w.yn + sp.R[2];
-  const float q1 = sp.R[3] * w.xn + sp.R[4] * w.yn + sp.R[5];
-  const float q2 = sp.R[6] * w.xn + sp.R[7] * w.yn + sp.R[8];
-  const float pr0 = avg_dpt / (avg_dpt + dpt0), dJ0 = -avg_dpt / (pr0 * pr0);
-  const float jd0 = (c00 * q0 + c02 * q2) * dJ0, jd1 = (c11 * q1 + c12 * q2) * dJ0;
-  const float e0 = (q2 * dJ0 - (g0 * jd0 + g1 * jd1)) * hw;
-  const float pr1 = avg_dpt / (avg_dpt + dpt1), dJ1 = -avg_dpt / (pr1 * pr1);
-  const float e1 = -dJ1 * hw;
-  for (int k = 0; k < C; ++k) {
-    r[12 + k] = e0 * __ldg(jr0 + k);
-    r[12 + C + k] = e1 * __ldg(jr1 + k);
+    // pix1_J_dpt = dCam * R * ray ; (R ray).z ; dpt_J_prx = -avg / prx^2
+    const float q0 = sp.R[0] * w.xn + sp.R[1] * w.yn + sp.R[2];
+    const float q1 = sp.R[3] * w.xn + sp.R[4] * w.yn + sp.R[5];
+    const float q2 = sp.R[6] * w.xn + sp.R[7] * w.yn + sp.R[8];
+    const float pr0 = avg_dpt / (avg_dpt + dpt0), dJ0 = -avg_dpt / (pr0 * pr0);
+    const float jd0 = (c00 * q0 + c02 * q2) * dJ0, jd1 = (c11 * q1 + c12 * q2) * dJ0;
+    const float e0 = (q2 * dJ0 - (g0 * jd0 + g1 * jd1)) * hw;
+    const float pr1 = avg_dpt / (avg_dpt + dpt1), dJ1 = -avg_dpt / (pr1 * pr1);
+    const float e1 = -dJ1 * hw;
+    for (int k = 0; k < C; ++k) {
+      r[12 + k] = e0 * __ldg(jr0 + k);
+      r[12 + C + k] = e1 * __ldg(jr1 + k);
+    }
   }
   r[12 + 2 * C] = err * hw;
   return true;
@@ -345,6 +360,75 @@ sparse_geometric_records_kernel(const GeoItemDev* __restrict__ items, const int2
   load_item<GeoCfg<C>::NT>(items + blockIdx.x, it);
   gram_records<GeoCfg<C>>(it.num_points, records, [&](int m, float* r) {
     return sparse_geometric_point_row<C>(it, points[it.point_begin + m], avg_dpt, r);
+  });
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The error() half of both factors: b^T b and the valid items of factor blockIdx.x, nothing else.  One CTA of Cfg::CH
+// threads per factor walks the items in the records kernel's chunks; thread t computes item base + t's b entries
+// (item_b(i, b), RPI of them, zero when invalid) into shared memory, then thread 0 sums the chunk's RPI cnt squares in
+// row order with the records kernel's fmaf chain and adds that chunk sum to the total.  That is exactly how gram_records
+// forms the (RW-1, RW-1) entry of the augmented Gram, so out[2 f] is bit for bit the residual of factor f's record.
+// out[2 f + 1] = valid items (u32 bits).
+template <class Cfg, class BFn>
+__device__ __forceinline__ void sparse_error(int M, float* __restrict__ out, BFn item_b)
+{
+  constexpr int RPI = Cfg::RPI, CH = Cfg::CH;
+  __shared__ float bs[RPI * CH];
+  float acc = 0.0f;
+  int inliers = 0;
+  for (int base = 0; base < M; base += CH) {
+    const int cnt = min(CH, M - base);
+    bool valid = false;
+    if ((int)threadIdx.x < cnt) {
+      float b[RPI];
+      valid = item_b(base + threadIdx.x, b);
+#pragma unroll
+      for (int r = 0; r < RPI; ++r) bs[RPI * threadIdx.x + r] = b[r];
+    }
+    inliers += __syncthreads_count(valid);
+    if (threadIdx.x == 0) {
+      float part = 0.0f;
+      for (int r = 0; r < RPI * cnt; ++r) part = fmaf(bs[r], bs[r], part);
+      acc += part;
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    out[2 * (size_t)blockIdx.x] = acc;
+    out[2 * (size_t)blockIdx.x + 1] = __uint_as_float((uint32_t)inliers);
+  }
+}
+
+template <int C>
+__global__ void __launch_bounds__(RepCfg<C>::CH)
+reprojection_error_kernel(const ReprojItemDev* __restrict__ items, const float2* __restrict__ query,
+                          const float2* __restrict__ train, float avg_dpt, float* __restrict__ out)
+{
+  __shared__ ReprojItemDev it;
+  load_item<RepCfg<C>::CH>(items + blockIdx.x, it);
+  sparse_error<RepCfg<C>>(it.num_matches, out, [&](int m, float (&b)[2]) {
+    const int i = it.match_begin + m;
+    float r[2][13 + C], e2;
+    const bool valid = reprojection_match_rows<C, false>(it, query[i], train[i], avg_dpt, r[0], r[1], &e2);
+    b[0] = r[0][12 + C];
+    b[1] = r[1][12 + C];
+    return valid;
+  });
+}
+
+template <int C>
+__global__ void __launch_bounds__(GeoCfg<C>::CH)
+sparse_geometric_error_kernel(const GeoItemDev* __restrict__ items, const int2* __restrict__ points, float avg_dpt,
+                              float* __restrict__ out)
+{
+  __shared__ GeoItemDev it;
+  load_item<GeoCfg<C>::CH>(items + blockIdx.x, it);
+  sparse_error<GeoCfg<C>>(it.num_points, out, [&](int m, float (&b)[1]) {
+    float r[13 + 2 * C];
+    const bool valid = sparse_geometric_point_row<C, false>(it, points[it.point_begin + m], avg_dpt, r);
+    b[0] = r[12 + 2 * C];
+    return valid;
   });
 }
 
@@ -413,6 +497,26 @@ cudaError_t launch_sparse_geometric_records(int code_size, const GeoItemDev* ite
     if (e != cudaSuccess) return e;
     sparse_geometric_records_kernel<cs.value><<<dim3(num_items, Cfg::NS), Cfg::NT, Cfg::SMEM, s>>>(items_dev, points_dev,
                                                                                                    avg_dpt, records_dev);
+    return cudaGetLastError();
+  });
+}
+
+cudaError_t launch_reprojection_error(int code_size, const ReprojItemDev* items_dev, int num_items, const float2* query_dev,
+                                      const float2* train_dev, float avg_dpt, float* out_dev, cudaStream_t s)
+{
+  return with_sparse_code_size(code_size, [&](auto cs) {
+    reprojection_error_kernel<cs.value><<<num_items, RepCfg<cs.value>::CH, 0, s>>>(items_dev, query_dev, train_dev,
+                                                                                 avg_dpt, out_dev);
+    return cudaGetLastError();
+  });
+}
+
+cudaError_t launch_sparse_geometric_error(int code_size, const GeoItemDev* items_dev, int num_items, const int2* points_dev,
+                                          float avg_dpt, float* out_dev, cudaStream_t s)
+{
+  return with_sparse_code_size(code_size, [&](auto cs) {
+    sparse_geometric_error_kernel<cs.value><<<num_items, GeoCfg<cs.value>::CH, 0, s>>>(items_dev, points_dev, avg_dpt,
+                                                                                     out_dev);
     return cudaGetLastError();
   });
 }

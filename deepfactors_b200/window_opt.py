@@ -23,6 +23,12 @@ solves.  Here every heavy step of one iteration is ONE device operation over the
     (slide)     a keyframe leaves the window: eliminated from the factors that touch it into a dense linear prior
                 over its blanket                                                        dfk_window_marginalize_keyframe
                 which the next window (without_keyframe) adds after the all-reduce      dfk_window_add_keyframe_priors
+    error       the window energy without linearising (SfmWindowProblem.error): every keyframe level decoded
+                into the problem's depth scratch in one launch                           dfk_update_depth_batch
+                every photometric and frame (pair, level) item's error in one launch      dfk_sfm_evaluate_error_batch
+                b^T b of every link, one launch per kind           dfk_reprojection_error_batch / dfk_sparse_geometric_error_batch
+                one read-back, summed on the host in fp64 with the priors; WindowOptimizer(error=...) then linearises
+                accepted points only
     retract     pose: t += dt, R = exp(w) R (gtsam_traits.h:48-58); code += dc           (tiny, host)
     accept      Levenberg-Marquardt on the energy f: rescaled photometric residuals + b^T b of the links (what the
                 factors' error() return)
@@ -31,6 +37,7 @@ The host side (cache, retraction, damping schedule) is plain Python / numpy; not
 """
 from __future__ import annotations
 
+import ctypes
 import functools
 from dataclasses import dataclass, field
 from typing import Callable, List, Optional, Sequence, Tuple
@@ -60,6 +67,54 @@ class LMTrace:
     accepted: List[bool] = field(default_factory=list)
     factors_relinearised: List[int] = field(default_factory=list)  # per linearisation: pairs that were re-evaluated
     frame_poses: Optional[np.ndarray] = None  # run(..., frame_poses): the frames' poses at the returned point
+    linearisations: int = 0       # calls of `linearise`
+    error_evaluations: int = 0    # calls of `error` (WindowOptimizer(error=...) only)
+
+
+@dataclass
+class WindowError:
+    """The parts of SfmWindowProblem.error's energy, each summed in fp64 in factor order (buffer units)."""
+    photometric: float = 0.0   # photometric and frame (pair, level) items: res / inliers * W * H, 0 without inliers
+    reprojection: float = 0.0  # b^T b of the reprojection links
+    geometric: float = 0.0     # b^T b of the sparse geometric links
+    priors: float = 0.0        # f0 - 2 g^T d + d^T G d of the frame priors, then of the keyframe priors
+    no_inliers: int = 0        # photometric and frame items without inliers (they add 0)
+    inliers: int = 0           # total inliers of the photometric and frame items
+
+    @property
+    def energy(self) -> float:
+        return self.photometric + self.reprojection + self.geometric + self.priors
+
+
+def prior_energy(row, delta) -> float:
+    """f0 - 2 g^T d + d^T G d of a linear prior row [G (n x n) | g (n) | f0] at d = delta (n), in fp64"""
+    d = np.asarray(delta, dtype=np.float64).ravel()
+    n = d.size
+    row = np.asarray(row, dtype=np.float64).ravel()
+    G, g, f0 = row[:n * n].reshape(n, n), row[n * n:n * n + n], float(row[n * n + n])
+    return f0 - 2.0 * float(g @ d) + float(d @ G @ d)
+
+
+def window_error_sum(dense, areas, reprojection, geometric, prior_terms) -> WindowError:
+    """The host half of SfmWindowProblem.error.  dense: [n, 2] float32 rows [residual | inliers as uint32 bits] of the
+    photometric and frame items (dfk_sfm_evaluate_error_batch) with their W * H in `areas`; reprojection / geometric:
+    [m, 2] rows [b^T b | valid (uint32 bits)] of the links; prior_terms: each prior's energy (prior_energy).  An item
+    without inliers adds 0, as in the window assembly (PhotometricFactor::error would return inf for it)."""
+    dense = np.ascontiguousarray(dense, dtype=np.float32).reshape(-1, 2)
+    res, inl = dense[:, 0].astype(np.float64), dense[:, 1].view(np.uint32).astype(np.int64)
+    out = WindowError()
+    for r, n, a in zip(res, inl, areas):
+        if n > 0:
+            out.photometric += float(r / n * a)
+    out.no_inliers = int((inl == 0).sum())
+    out.inliers = int(inl.sum())
+    for b in np.asarray(reprojection, dtype=np.float32).reshape(-1, 2)[:, 0]:
+        out.reprojection += float(b)
+    for b in np.asarray(geometric, dtype=np.float32).reshape(-1, 2)[:, 0]:
+        out.geometric += float(b)
+    for t in prior_terms:
+        out.priors += float(t)
+    return out
 
 
 def damped_solve(H, g, lam: float, fixed: Sequence[int] = ()):
@@ -191,23 +246,38 @@ class WindowOptimizer:
 
     With tracked frames (layout.num_frames > 0) run takes their poses, `linearise` is called as
     linearise(poses, codes, todo, frame_poses), dx carries the frames' steps after the keyframes' and the frames' final
-    poses come back on the trace (trace.frame_poses)."""
+    poses come back on the trace (trace.frame_poses).
+
+    `error(poses, codes[, frame_poses]) -> (E, breakdown)` (optional; SfmWindowProblem.error) is the energy at a point
+    without linearising it, in the units of the buffer's f.  With it the loop evaluates E at every candidate and
+    linearises only the points it accepts (the start point and every accepted step), so a rejected step costs one error
+    evaluation and leaves the record buffer and the cache at the accepted point.  f is then E plus the host prior term."""
 
     def __init__(self, layout: WindowBlocks, linearise: Callable, params: Optional[LMParams] = None,
-                 solve: Optional[Callable] = None):
+                 solve: Optional[Callable] = None, error: Optional[Callable] = None):
         self.layout = layout
         self.linearise = linearise
         self.params = params or LMParams()
         self.solve = solve or functools.partial(dense_solve, layout)
+        self.error = error
         self.cache = LinearisationCache(layout.pairs, self.params.cache_eps, layout.geometric)
+
+    def _code_prior(self, codes) -> float:
+        w = self.params.code_prior_weight
+        return 0.5 * w * float((codes ** 2).sum()) if w > 0 else 0.0
 
     def _energy(self, buf, codes) -> float:
         """f: the buffer's scalar slot (what to_dense returns) plus the prior term"""
         f = float(buf[self.layout.offsets()[2]])
-        w = self.params.code_prior_weight
-        if w > 0:
-            f += 0.5 * w * float((codes ** 2).sum())
+        if self.params.code_prior_weight > 0:
+            f += self._code_prior(codes)
         return f
+
+    def _error(self, poses, codes, trace: LMTrace, frame_poses=None) -> float:
+        """f from `error`: E plus the prior term"""
+        e, _ = self.error(poses, codes) if frame_poses is None else self.error(poses, codes, frame_poses)
+        trace.error_evaluations += 1
+        return float(e) + self._code_prior(codes)
 
     def _evaluate(self, poses, codes, trace: LMTrace, frame_poses=None):
         todo = self.cache.stale(poses, codes, frame_poses)
@@ -217,6 +287,7 @@ class WindowOptimizer:
             buf, _ = self.linearise(poses, codes, todo, frame_poses)
         self.cache.store(todo, poses, codes, frame_poses)
         trace.factors_relinearised.append(len(todo))
+        trace.linearisations += 1
         return buf
 
     def run(self, poses, codes, frame_poses=None) -> Tuple[np.ndarray, np.ndarray, LMTrace]:
@@ -230,7 +301,7 @@ class WindowOptimizer:
         fixed = list(range(6)) if prm.fix_first_pose else []
         lam = prm.lambda_init
         buf = self._evaluate(poses, codes, trace, frames)
-        f = self._energy(buf, codes)
+        f = self._energy(buf, codes) if self.error is None else self._error(poses, codes, trace, frames)
         trace.energy.append(f)
         for _ in range(prm.iterations):
             dx = self.solve(buf, lam, fixed, prm.code_prior_weight, codes)
@@ -243,17 +314,22 @@ class WindowOptimizer:
                     cand_f = None
                 else:
                     cand_p, cand_c, cand_f = apply_update(poses, codes, dx, self.layout.code_size, frames)
-                cbuf = self._evaluate(cand_p, cand_c, trace, cand_f)
-                cf = self._energy(cbuf, cand_c)
+                if self.error is None:
+                    cbuf = self._evaluate(cand_p, cand_c, trace, cand_f)
+                    cf = self._energy(cbuf, cand_c)
+                else:
+                    cf = self._error(cand_p, cand_c, trace, cand_f)
                 ok = bool(np.isfinite(cf) and cf < f)
             trace.accepted.append(ok)
             if ok:
+                if self.error is not None:  # only an accepted point is linearised
+                    cbuf = self._evaluate(cand_p, cand_c, trace, cand_f)
                 poses, codes, buf, f, frames = cand_p, cand_c, cbuf, cf, cand_f
                 trace.energy.append(f)
                 lam = max(lam * prm.lambda_down, 1e-12)
             else:
-                # buf and f of the accepted point are still at hand; the record buffer (and with it the cache) now
-                # describes the rejected candidate, which the next candidate is compared against
+                # buf and f of the accepted point are still at hand; without `error` the record buffer (and with it the
+                # cache) now describes the rejected candidate, which the next candidate is compared against
                 lam = lam * prm.lambda_up
                 if lam > prm.lambda_max:
                     break
@@ -386,6 +462,15 @@ def _geometric_items(prob, j, a, b, pose0, pose1, code0, code1):
     return [dict(pose0=pose0, pose1=pose1, code0=code0, code1=code1, cam=prob.cams[0], prx0_orig=a[0]["prx_orig"],
                  prx0_jac=a[0]["prx_jac"], prx1_orig=b[0]["prx_orig"], prx1_jac=b[0]["prx_jac"],
                  dpt_grad1=b[0]["dpt_grad"], points_xy=gl.points_xy, huber_delta=gl.huber_delta)]
+
+
+def _struct_floats(arr, name: str, count: int) -> np.ndarray:
+    """[len(arr), count] float32 numpy view of the float-array field `name` of every struct of a ctypes array: writing
+    the view rewrites the array in place"""
+    T = arr._type_
+    off = getattr(T, name).offset
+    raw = np.frombuffer(arr, dtype=np.uint8).reshape(len(arr), ctypes.sizeof(T))
+    return raw[:, off:off + 4 * count].view(np.float32)
 
 
 def _run_step_batch(aligner, items, records=None):
@@ -529,6 +614,112 @@ class SfmWindowProblem:
         return np.concatenate([np.concatenate([se3.local(pr.poses0[a], poses[k]), np.asarray(codes[k], np.float64) -
                                                np.asarray(pr.codes0[a], np.float64)])
                                for pr in self._kpriors for a, k in enumerate(pr.keyframes)])
+
+    def error(self, poses, codes, frame_poses=None):
+        """The window energy E at (poses, codes) without linearising: PhotometricFactor / ReprojectionFactor /
+        SparseGeometricFactor::error of every factor plus the priors, in the units of the buffer's f (WindowOptimizer adds
+        the code prior as for a linearisation).  Four launches and one read-back: every keyframe level decoded into depth
+        scratch owned by this problem (dfk_update_depth_batch; the keyframes' own dpt keeps the last linearised point),
+        the error of every photometric and frame (pair, level) item from that scratch (dfk_sfm_evaluate_error_batch), and
+        b^T b of the reprojection and the geometric links.  Summed on the host in fp64 (window_error_sum): an item with
+        inliers adds res / inliers * W * H, one without adds 0 (as in the assembly; PhotometricFactor::error would return
+        inf), a link its b^T b, a prior f0 - 2 g^T d + d^T G d at the d linearise uses.  The pixel validity rule is
+        EvaluateError's (border 1, min_dpt 0): E equals the linearisation's f when valid_border = 1 and min_dpt = 0.  With
+        sharded pairs, E covers this rank's items and every prior: sum the factor parts across ranks and add the priors
+        once.  Returns (E, WindowError)."""
+        from .aligners import ReprojectionErrorBatch, SparseGeometricErrorBatch
+        if self.frames and frame_poses is None:
+            raise ValueError("the window has tracked frames: error needs their poses")
+        st = self._err if getattr(self, "_err", None) is not None else self._error_state()
+        c32 = np.asarray(codes, dtype=np.float32)
+        st["depth_codes"][:] = np.repeat(c32, self.levels, axis=0)
+        self.al.UpdateDepthBatch(st["depth_items"])
+        allp = np.asarray(poses, dtype=np.float64)
+        if self.frames:
+            allp = np.concatenate([allp, np.asarray(frame_poses, dtype=np.float64).reshape(-1, 7)])
+        allp = allp.astype(np.float32)
+        out, nd, nr = st["out"], st["nd"], st["nr"]
+        if nd:
+            st["dense_p0"][:], st["dense_p1"][:] = allp[st["dense_k0"]], allp[st["dense_k1"]]
+            self.al.EvaluateErrorBatch(st["dense_items"], out[:nd])
+        for kind, fn, lo, hi in (("rep", ReprojectionErrorBatch, nd, nd + nr),
+                                 ("geo", SparseGeometricErrorBatch, nd + nr, out.shape[0])):
+            if hi > lo:
+                k0, k1 = st[kind + "_k0"], st[kind + "_k1"]
+                st[kind + "_p0"][:], st[kind + "_p1"][:] = allp[k0], allp[k1]
+                st[kind + "_code0"][:] = c32[k0]
+                if kind == "geo":
+                    st["geo_code1"][:] = c32[k1]
+                fn(self.al, st[kind + "_items"], out[lo:hi])
+        host = out.cpu().numpy()
+        terms = []
+        if self._mpriors:
+            terms += [prior_energy(pr.row, d) for pr, d in zip(self._mpriors, self._deltas(poses, codes))]
+        if self._kpriors:
+            d, at = self._kf_deltas(poses, codes), 0
+            for pr in self._kpriors:
+                n = len(pr.keyframes) * self.layout.B
+                terms.append(prior_energy(pr.row, d[at:at + n]))
+                at += n
+        ew = window_error_sum(host[:nd], st["areas"], host[nd:nd + nr], host[nd + nr:], terms)
+        return ew.energy, ew
+
+    def _error_state(self):
+        """what error() builds once: the depth scratch and the ctypes item arrays, whose poses and codes each call
+        rewrites in place through numpy views"""
+        import torch
+        from .aligners import make_geometric_items, make_reprojection_items
+        K, L, C, P, PF = len(self.kf), self.levels, self.al.CS, self._num_photometric, \
+            self._num_photometric + len(self.links)
+        st = {"dpt": [[torch.empty_like(self.kf[k][l]["dpt"]) for l in range(L)] for k in range(K)]}
+        st["depth_codes"] = np.zeros((K * L, C), dtype=np.float32)
+        st["depth_items"] = self.al.make_depth_items(
+            [dict(code=st["depth_codes"][k * L + l], prx_orig=self.kf[k][l]["prx_orig"], prx_jac=self.kf[k][l]["prx_jac"],
+                  dpt=st["dpt"][k][l]) for k in range(K) for l in range(L)])
+        zero = np.zeros(7, dtype=np.float32)
+        # the dense items in record order: the photometric pairs' levels, then the frame pairs'
+        ends = [(p, self.pairs[p]) for p in range(P)] + [(p, self.pairs[p]) for p in range(PF, len(self.pairs))]
+        dense, k0s, k1s, areas = [], [], [], []
+        for _, (a, b) in ends:
+            lv1 = self.kf[b] if b < K else self.frames[b - K].levels
+            for l in range(L):
+                img0 = self.kf[a][l]["img"]
+                dense.append(dict(pose0=zero, pose1=zero, cam=self.cams[l], img0=img0, img1=lv1[l]["img"],
+                                  dpt0=st["dpt"][a][l], valid0=self.kf[a][l]["valid"], prx0_jac=self.kf[a][l]["prx_jac"],
+                                  grad1=lv1[l]["grad"]))
+                k0s.append(a)
+                k1s.append(b)
+                areas.append(float(img0.shape[0] * img0.shape[1]))
+        st["nd"], st["areas"] = len(dense), areas
+        st["dense_k0"], st["dense_k1"] = np.asarray(k0s, dtype=np.int64), np.asarray(k1s, dtype=np.int64)
+        if dense:
+            st["dense_items"] = self.al.make_work_items(dense)
+            st["dense_p0"] = _struct_floats(st["dense_items"], "pose0", 7)
+            st["dense_p1"] = _struct_floats(st["dense_items"], "pose1", 7)
+        st["rep_k0"] = np.asarray([ln.k0 for ln in self.links], dtype=np.int64)
+        st["rep_k1"] = np.asarray([ln.k1 for ln in self.links], dtype=np.int64)
+        st["nr"] = len(self.links)
+        if self.links:
+            st["rep_code0"] = np.zeros((len(self.links), C), dtype=np.float32)
+            st["rep_items"] = make_reprojection_items(
+                [dict(it, code0=st["rep_code0"][j]) for j in range(len(self.links))
+                 for it in _reprojection_items(self, j, self.kf[self.links[j].k0], None, zero, zero, None, None)], C)
+            st["rep_p0"] = _struct_floats(st["rep_items"], "pose0", 7)
+            st["rep_p1"] = _struct_floats(st["rep_items"], "pose1", 7)
+        st["geo_k0"] = np.asarray([gl.k0 for gl in self.geometric], dtype=np.int64)
+        st["geo_k1"] = np.asarray([gl.k1 for gl in self.geometric], dtype=np.int64)
+        if self.geometric:
+            st["geo_code0"] = np.zeros((len(self.geometric), C), dtype=np.float32)
+            st["geo_code1"] = np.zeros((len(self.geometric), C), dtype=np.float32)
+            st["geo_items"] = make_geometric_items(
+                [dict(it, code0=st["geo_code0"][j], code1=st["geo_code1"][j]) for j, gl in enumerate(self.geometric)
+                 for it in _geometric_items(self, j, self.kf[gl.k0], self.kf[gl.k1], zero, zero, None, None)], C)
+            st["geo_p0"] = _struct_floats(st["geo_items"], "pose0", 7)
+            st["geo_p1"] = _struct_floats(st["geo_items"], "pose1", 7)
+        n = st["nd"] + st["nr"] + len(self.geometric)
+        st["out"] = torch.empty((max(n, 1), 2), dtype=torch.float32, device=self.records.device)[:n]
+        self._err = st
+        return st
 
     def linearise(self, poses, codes, todo, frame_poses=None):
         import torch

@@ -39,6 +39,12 @@
 
 #include "../dfk.h"
 
+// SfmAligner::EvaluateErrorBatch copies its results back with the CUDA runtime; it exists where the runtime's header does
+#if __has_include(<cuda_runtime_api.h>)
+#include <cuda_runtime_api.h>
+#define DFK_FACADE_CUDART 1
+#endif
+
 namespace df
 {
 
@@ -279,6 +285,50 @@ public:
     r.inliers = bits;
     return r;
   }
+
+#ifdef DFK_FACADE_CUDART
+  // extension: the work item of one EvaluateError call, for EvaluateErrorBatch
+  template <typename SE3T, typename CamT, typename ImageBuffer>
+  static DfkSfmWorkItem ErrorItem(const SE3T& pose0, const SE3T& pose1, const CamT& cam, const ImageBuffer& img0,
+                                  const ImageBuffer& img1, const ImageBuffer& dpt0)
+  {
+    DfkSfmWorkItem w{};
+    for (int k = 0; k < 7; ++k) {
+      w.pose0[k] = pose0.data()[k];
+      w.pose1[k] = pose1.data()[k];
+    }
+    w.cam = detail::Cam(cam);
+    w.img0 = detail::View(img0, 1); w.img1 = detail::View(img1, 1); w.dpt0 = detail::View(dpt0, 1);
+    return w;
+  }
+
+  // extension: EvaluateError of many (pair, level) items in one launch (dfk_sfm_evaluate_error_batch), the error() half
+  // of the PhotometricFactors of a window (photometric_factor.cpp:61-81); results in host memory after one synchronise.
+  // Item i is bit for bit EvaluateError of that item alone.
+  std::vector<ErrorReductionItem> EvaluateErrorBatch(const std::vector<DfkSfmWorkItem>& items)
+  {
+    std::vector<ErrorReductionItem> out(items.size());
+    if (items.empty()) return out;
+    const std::size_t bytes = sizeof(float) * 2 * items.size();
+    float* dev = nullptr;
+    if (cudaMalloc(reinterpret_cast<void**>(&dev), bytes) != cudaSuccess)
+      throw std::runtime_error("[SfmAligner::EvaluateErrorBatch] device allocation failed");
+    std::unique_ptr<float, cudaError_t (*)(void*)> guard(dev, cudaFree);
+    detail::Check(h_.get(), dfk_sfm_evaluate_error_batch(h_.get(), items.data(), static_cast<int>(items.size()), dev));
+    std::vector<float> host(2 * items.size());
+    cudaStream_t s = static_cast<cudaStream_t>(dfk_get_stream(h_.get()));
+    if (cudaMemcpyAsync(host.data(), dev, bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+        cudaStreamSynchronize(s) != cudaSuccess)
+      throw std::runtime_error("[SfmAligner::EvaluateErrorBatch] result download failed");
+    for (std::size_t i = 0; i < items.size(); ++i) {
+      out[i].residual = host[2 * i];
+      uint32_t bits;
+      std::memcpy(&bits, &host[2 * i + 1], 4);
+      out[i].inliers = bits;
+    }
+    return out;
+  }
+#endif
 
   void SetEvalThreadsBlocks(int threads, int blocks)
   {

@@ -193,6 +193,15 @@ DfkStatus dfk_sfm_run_step_batch(DfkHandle h, const DfkSfmWorkItem* items, int n
 DfkStatus dfk_sfm_run_step_batch_host(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_size,
                                       float* records_host);
 
+/* Batched SfmAligner::EvaluateError, the error() half of PhotometricFactor (photometric_factor.cpp:61-81, 197-219):
+ * n work items, the same DfkSfmWorkItem as dfk_sfm_run_step_batch, evaluated as dfk_sfm_evaluate_error evaluates one
+ * (border 1, min_dpt 0, the handle's huber_delta).  valid0, prx0_jac, grad1 and prx_orig are ignored; `code` must be
+ * NULL (the depth is read from dpt0; decode it first with dfk_update_depth_batch), else DFK_ERR_INVALID_ARG.
+ * out_dev: DEVICE, 2 floats per item, [residual | inliers (u32 bits)], each bit for bit what dfk_sfm_evaluate_error
+ * gives for that item alone, whatever else is in the batch.  1 <= n <= 65535.  One launch, asynchronous on the handle's
+ * stream (no host sync, no D2H); every item is validated before anything is enqueued. */
+DfkStatus dfk_sfm_evaluate_error_batch(DfkHandle h, const DfkSfmWorkItem* items, int n, float* out_dev);
+
 /* ------------------------------------------------------------------ streaming evaluation from HOST memory
  *
  * The reference's inputs live in host/device mirrored pyramids that are uploaded lazily, one synchronous copy at a
@@ -559,12 +568,37 @@ typedef struct {
 DfkStatus dfk_sparse_geometric_linearize_batch(DfkHandle h, const DfkSparseGeometricItem* items, int n, int code_size,
                                                float* records_dev);
 
+/* The error() half of the two sparse factors (ReprojectionFactor::error, reprojection_factor.cpp:97-154;
+ * SparseGeometricFactor::error, sparse_geometric_factor.cpp:85-142): the same items as the linearize batches, and per
+ * factor out_dev (DEVICE, 2 floats per factor) = [b^T b | valid matches / points (u32 bits)], where b is the last column of
+ * the factor's JacobianFactor [A | b].  b^T b is bit for bit the residual of the factor's record from the matching
+ * linearize batch, so it is twice the factor's error in the linearisation's units and follows the linearisation's
+ * validity rules (a point outside the views or behind the camera counts as invalid, not as an out-of-bounds read).  No
+ * Jacobian is formed.  One launch, one CTA per factor; asynchronous on the handle's stream; argument checks as for the
+ * linearize batches. */
+DfkStatus dfk_reprojection_error_batch(DfkHandle h, const DfkReprojectionItem* items, int n, int code_size,
+                                       float* out_dev);
+DfkStatus dfk_sparse_geometric_error_batch(DfkHandle h, const DfkSparseGeometricItem* items, int n, int code_size,
+                                           float* out_dev);
+
 /* ------------------------------------------------------------------ cu_image_proc free functions */
 
 /* df::UpdateDepth (cu_image_proc.h:41-44, cu_image_proc.cpp:248-277):
  * dpt = avg/(prx_orig + prx_jac . code) - avg.  code is HOST memory. Asynchronous. */
 DfkStatus dfk_update_depth(DfkHandle h, const float* code, int code_size, const DfkImage* prx_orig,
                            const DfkImage* prx_jac, float avg_dpt, const DfkImage* dpt_out);
+/* One depth decode of dfk_update_depth_batch, e.g. one (keyframe, level): dpt = avg/(prx_orig + prx_jac . code) - avg.
+ * code is a HOST pointer to code_size floats. */
+typedef struct {
+  DfkImage prx_orig, prx_jac;
+  DfkImage dpt; /* out */
+  const float* code;
+} DfkDepthDecodeItem;
+/* n dfk_update_depth calls in one launch (the per-level UpdateDepth loop of Mapper::BuildKeyframe, mapper.cpp:984-991, for
+ * many keyframes at once), avg_dpt = the handle's DenseSfmParams::avg_dpt.  Item i is bit for bit
+ * dfk_update_depth(h, items[i].code, code_size, &prx_orig, &prx_jac, avg_dpt, &dpt).  The codes go up in one copy.
+ * 1 <= n <= 65535.  Asynchronous on the handle's stream. */
+DfkStatus dfk_update_depth_batch(DfkHandle h, const DfkDepthDecodeItem* items, int n, int code_size);
 /* df::SobelGradients (cu_image_proc.h:27-29, cu_image_proc.cpp:57-113). Asynchronous. */
 DfkStatus dfk_sobel_gradients(DfkHandle h, const DfkImage* img, const DfkImage* grad);
 /* df::GaussianBlurDown (cu_image_proc.h:31-33, cu_image_proc.cpp:134-184). Asynchronous. */

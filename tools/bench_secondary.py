@@ -30,8 +30,14 @@ One JSON line per case:
   * sliding the window (`--only slide`): window200 at C = 32 and 128, one keyframe marginalised
     (dfk_window_marginalize_keyframe alone, and SfmWindowProblem.marginalize_keyframe with the re-evaluation of the
     keyframe's factors), then the device solve of the 49-keyframe slid window with its keyframe prior and without.
+  * the window energy without a linearisation (`--only error`): window200 at C = 32 and 128, every keyframe with a
+    code-Jacobian pyramid of its own: SfmWindowProblem.error against SfmWindowProblem.linearise with every factor
+    stale, dfk_update_depth_batch of the 200 keyframe levels against 200 dfk_update_depth calls, and a 10-iteration LM
+    from perturbed poses with the device solve, without and with `error` (its linearisation and error-evaluation
+    counts) -- wall clock to a synchronise and summed device time (torch.profiler, separate run); the byte model of
+    both paths is printed beside them.
 Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` /
-`--only frames` / `--only slide` runs those cases alone.
+`--only frames` / `--only slide` / `--only error` runs those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -50,7 +56,7 @@ sys.path.insert(0, ROOT)
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
-    ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide"], default=None)
+    ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error"], default=None)
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -82,6 +88,8 @@ def main():
         return frames_cases(args, torch, print)
     if args.only == "slide":
         return slide_cases(args, torch, print)
+    if args.only == "error":
+        return error_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -606,6 +614,103 @@ def slide_cases(args, torch, print):
                               "timing": "wall clock to a synchronise (the solve reads dx back); device time = summed "
                                         "kernel + copy time, torch.profiler"}), flush=True)
         del prob, slid, bare, keyframes, shared
+        torch.cuda.empty_cache()
+
+
+def error_cases(args, torch, print):
+    """window200 at C = 32 and 128: the window energy by SfmWindowProblem.error against a full linearisation, the batched
+    depth decode against one call per keyframe level, and LM without and with `error`"""
+    import numpy as np
+    from deepfactors_b200 import se3, synth
+    from deepfactors_b200.aligners import SfmAligner, UpdateDepth
+    from deepfactors_b200.window_opt import LMParams, SfmWindowProblem, WindowOptimizer
+    sys.path.insert(0, ROOT)
+    from bench import window_pairs
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
+    levels, num_kf = 4, 50
+    reps = max(5, args.reps // 2)
+    timing = "wall clock to a synchronise; device time = summed kernel + copy time, torch.profiler (separate run)"
+    for cs in (32, 128):
+        base = synth.make_pair(640, 480, cs, levels, seed=7)
+        shared = [dict(img=up(L.img0), grad=up(L.grad1), prx_orig=up(L.prx_orig)) for L in base.levels]
+        jac = [up(L.prx_jac) for L in base.levels]
+        gen = torch.Generator(device="cuda").manual_seed(cs)
+        # every keyframe its own code Jacobian (the byte model decodes 50 pyramids, not one cached in L2)
+        keyframes = [[dict(sh, prx_jac=j + 1e-3 * torch.randn(j.shape, device="cuda", generator=gen),
+                           dpt=torch.zeros_like(sh["img"]), valid=torch.zeros_like(sh["img"]))
+                      for sh, j in zip(shared, jac)] for _ in range(num_kf)]
+        pairs = window_pairs(num_kf, 200)
+        cams = [L.cam for L in base.levels]
+        al = SfmAligner(cs)
+        rng = np.random.default_rng(cs)
+        poses = np.stack([se3.make_pose(rng.standard_normal(3) * 0.003, rng.standard_normal(3) * 0.01, np.float64)
+                          for _ in range(num_kf)])
+        poses[0] = se3.identity(np.float64)
+        codes = np.zeros((num_kf, cs))
+        prob = SfmWindowProblem(al, cams, keyframes, pairs)
+        todo = list(range(len(prob.pairs)))
+        px = sum(int(L.img0.size) for L in base.levels)  # pixels of one pyramid
+        items = len(pairs) * levels
+        bytes_err = num_kf * px * (4 * cs + 8) + len(pairs) * px * 12
+        bytes_lin = len(pairs) * px * (4 * cs + 24)
+        E, parts = prob.error(poses, codes)
+        buf, _ = prob.linearise(poses, codes, todo)
+        f = float(buf[prob.layout.offsets()[2]])
+
+        def error():
+            prob.error(poses, codes)
+
+        def linearise():
+            prob.linearise(poses, codes, todo)
+            torch.cuda.synchronize()
+
+        for name, fn, nbytes in (("SfmWindowProblem.error (4 launches + 1 read-back)", error, bytes_err),
+                                 ("SfmWindowProblem.linearise, every factor stale", linearise, bytes_lin)):
+            wall = _wall_us(torch, fn, reps)
+            dev_us = _device_us(torch, fn, reps)
+            print(json.dumps({"case": f"window200 C={cs} ({num_kf} keyframes, {len(pairs)} pairs, {levels} levels 640x480, "
+                                      f"{items} items): {name}",
+                              "us_per_call": wall, "device_us_per_call": dev_us, "bytes_model": nbytes,
+                              "model_gbs_over_device_time": nbytes / dev_us / 1e3,
+                              "energy": E if fn is error else f, "timing": timing}), flush=True)
+        print(json.dumps({"case": f"window200 C={cs}: E against the linearisation's f (valid_border 2: the validity "
+                                  "rules differ at the border)", "E": E, "f": f, "parts": parts.__dict__}), flush=True)
+        dec = [dict(code=np.zeros(cs, np.float32), prx_orig=kf[l]["prx_orig"], prx_jac=kf[l]["prx_jac"],
+                    dpt=kf[l]["dpt"]) for kf in keyframes for l in range(levels)]
+        arr = al.make_depth_items(dec)
+
+        def batch():
+            al.UpdateDepthBatch(arr)
+
+        def single():
+            for it in dec:
+                UpdateDepth(it["code"], it["prx_orig"], it["prx_jac"], 2.0, it["dpt"])
+
+        for name, fn in (("one dfk_update_depth_batch", batch), (f"{len(dec)} dfk_update_depth calls", single)):
+            print(json.dumps({"case": f"window200 C={cs}: decode {len(dec)} keyframe levels, {name}",
+                              "us_per_call": _wall_us(torch, fn, reps), "device_us_per_call": _device_us(torch, fn, reps),
+                              "bytes_model": num_kf * px * (4 * cs + 8), "timing": timing}), flush=True)
+        prm = LMParams(iterations=10, lambda_init=1e-4)
+        for mode in ("linearise", "error"):
+            def lm():
+                p = SfmWindowProblem(al, cams, keyframes, pairs)
+                opt = WindowOptimizer(p.layout, p.linearise, prm, solve=p.solve,
+                                      error=p.error if mode == "error" else None)
+                return opt.run(poses, codes)
+
+            _, _, tr = lm()
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            _, _, tr = lm()
+            torch.cuda.synchronize()
+            wall = (time.perf_counter() - t0) * 1e6
+            dev_us = _device_us(torch, lm, 1)
+            print(json.dumps({"case": f"window200 C={cs}: 10-iteration LM from perturbed poses, device solve, "
+                                      f"{'with error()' if mode == 'error' else 'linearising every candidate'}",
+                              "us_total": wall, "device_us_total": dev_us, "linearisations": tr.linearisations,
+                              "error_evaluations": tr.error_evaluations, "accepted": tr.accepted,
+                              "energy_first_last": [tr.energy[0], tr.energy[-1]], "timing": timing}), flush=True)
+        del prob, keyframes, shared, jac, arr, dec
         torch.cuda.empty_cache()
 
 
