@@ -89,6 +89,43 @@ class DfkWindowSolveParams(C.Structure):
     _fields_ = [("lambda_", C.c_double), ("code_prior_weight", C.c_double)]
 
 
+class DfkWindowItemSlots(C.Structure):
+    _fields_ = [("pose0", C.c_int32), ("pose1", C.c_int32), ("code0", C.c_int32), ("code1", C.c_int32)]
+
+
+class DfkWindowProblemDesc(C.Structure):
+    _fields_ = [("window", C.c_void_p),
+                ("num_dense", C.c_int32), ("dense", C.POINTER(DfkSfmWorkItem)),
+                ("dense_slots", C.POINTER(DfkWindowItemSlots)),
+                ("num_reproj", C.c_int32), ("reproj", C.POINTER(DfkReprojectionItem)),
+                ("reproj_slots", C.POINTER(DfkWindowItemSlots)),
+                ("num_geo", C.c_int32), ("geo", C.POINTER(DfkSparseGeometricItem)),
+                ("geo_slots", C.POINTER(DfkWindowItemSlots)),
+                ("num_depth", C.c_int32), ("depth", C.POINTER(DfkDepthDecodeItem)),
+                ("depth_slots", C.POINTER(DfkWindowItemSlots)),
+                ("num_error", C.c_int32), ("error", C.POINTER(DfkSfmWorkItem)),
+                ("error_slots", C.POINTER(DfkWindowItemSlots)), ("error_depth", C.POINTER(C.c_int32)),
+                ("num_frame_priors", C.c_int32), ("frame_prior_kf", C.POINTER(C.c_int32)),
+                ("frame_prior_rows", C.POINTER(C.c_double)), ("frame_prior_x0", C.POINTER(C.c_double)),
+                ("kf_prior_rows", C.POINTER(C.c_double)), ("kf_prior_x0", C.POINTER(C.c_double)),
+                ("records_dev", C.c_void_p), ("geo_records_dev", C.c_void_p)]
+
+
+class DfkLMParams(C.Structure):
+    _fields_ = [("iterations", C.c_int32), ("lambda_init", C.c_double), ("lambda_up", C.c_double),
+                ("lambda_down", C.c_double), ("lambda_max", C.c_double), ("fix_first_pose", C.c_int32),
+                ("code_prior_weight", C.c_double), ("use_error", C.c_int32)]
+
+
+class DfkLMTrace(C.Structure):
+    _fields_ = [("energy", C.POINTER(C.c_double)), ("lambda_", C.POINTER(C.c_double)),
+                ("accepted", C.POINTER(C.c_int32)), ("num_energies", C.c_int32), ("num_steps", C.c_int32),
+                ("linearisations", C.c_int32), ("error_evaluations", C.c_int32)]
+
+
+WINDOW_ERROR_DOUBLES = 7  # DFK_WINDOW_ERROR_DOUBLES
+
+
 # every symbol include/dfk.h declares: (name, restype, argtypes)
 _F = C.POINTER(C.c_float)
 _IMG = C.POINTER(DfkImage)
@@ -149,6 +186,14 @@ SYMBOLS = {
     "dfk_window_solver_tiles": (C.c_int, [_H, C.c_void_p, C.POINTER(C.c_size_t)]),
     "dfk_window_solve": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.POINTER(DfkWindowSolveParams), C.POINTER(C.c_double),
                                    C.c_void_p, C.c_void_p]),
+    "dfk_window_problem_create": (C.c_int, [_H, C.POINTER(DfkWindowProblemDesc), C.POINTER(C.c_void_p)]),
+    "dfk_window_problem_destroy": (C.c_int, [_H, C.c_void_p]),
+    "dfk_window_problem_set_state": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dfk_window_problem_get_state": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dfk_window_problem_linearize": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
+    "dfk_window_problem_error": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
+    "dfk_window_problem_retract": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
+    "dfk_window_lm": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkLMParams), C.POINTER(DfkLMTrace)]),
     "dfk_se3_run_step": (C.c_int, [_H, _F, _CAM, _IMG, _IMG, _IMG, _IMG, _F, _F, _F, C.POINTER(C.c_uint64)]),
     "dfk_se3_track": (C.c_int, [_H, _F, C.POINTER(DfkTrackLevel), C.c_int, _F, _F, _F, _F, C.c_int]),
     "dfk_se3_track_batch": (C.c_int, [_H, C.c_int, C.c_int, _F, C.POINTER(DfkTrackLevel), _F, _F, _F]),

@@ -761,6 +761,142 @@ class WindowSolver:
             pass
 
 
+class WindowProblem:
+    """A window problem of the C ABI (dfk_window_problem_*): every work item of a window held on the device once, the
+    window's state (poses and codes, fp64) on the device, and the Levenberg-Marquardt loop as one call (dfk_window_lm).
+    Item arrays are the ctypes arrays of make_work_items / make_reprojection_items / make_geometric_items /
+    make_depth_items (their poses and codes are ignored); slots are [n, 4] ints (pose0, pose1, code0, code1; -1 where
+    unused); records / geo_records are the caller's record buffers, which linearize writes.  The problem keeps every
+    array it was given alive (the image views inside them must stay valid)."""
+
+    def __init__(self, window: Window, records: torch.Tensor, geo_records=None, dense=None, dense_slots=(),
+                 reproj=None, reproj_slots=(), geo=None, geo_slots=(), depth=None, depth_slots=(), error=None,
+                 error_slots=(), error_depth=(), frame_prior_kf=(), frame_prior_rows=None, frame_prior_x0=None,
+                 kf_prior_rows=None, kf_prior_x0=None):
+        self._win = window
+        self._al = window._al
+        self.layout = window.layout
+        keep = [records, geo_records, dense, reproj, geo, depth, error]
+        S = _lib.DfkWindowItemSlots
+
+        def slots(rows):
+            a = np.ascontiguousarray(np.asarray(rows, dtype=np.int32).reshape(-1, 4))
+            keep.append(a)
+            return len(a), (a.ctypes.data_as(C.POINTER(S)) if len(a) else None)
+
+        def f64(x):
+            if x is None:
+                return None
+            a = np.ascontiguousarray(np.asarray(x, dtype=np.float64).ravel())
+            keep.append(a)
+            return a.ctypes.data_as(C.POINTER(C.c_double))
+
+        def i32(x):
+            a = np.ascontiguousarray(np.asarray(x, dtype=np.int32).ravel())
+            keep.append(a)
+            return a.ctypes.data_as(C.POINTER(C.c_int32)) if a.size else None
+
+        nd, ds = slots(dense_slots)
+        nr, rs = slots(reproj_slots)
+        ng, gs = slots(geo_slots)
+        ndep, dps = slots(depth_slots)
+        ne, es = slots(error_slots)
+        mf = len(frame_prior_kf)
+        d = _lib.DfkWindowProblemDesc(
+            window.w, nd, dense if nd else None, ds, nr, reproj if nr else None, rs, ng, geo if ng else None, gs,
+            ndep, depth if ndep else None, dps, ne, error if ne else None, es, i32(error_depth), mf, i32(frame_prior_kf),
+            f64(frame_prior_rows), f64(frame_prior_x0), f64(kf_prior_rows), f64(kf_prior_x0),
+            C.c_void_p(records.data_ptr()), C.c_void_p(geo_records.data_ptr()) if geo_records is not None else None)
+        self._keep = keep
+        self.p = C.c_void_p()
+        self._al._hd.use_torch_stream()
+        check(self._al.handle, lib().dfk_window_problem_create(self._al.handle, C.byref(d), C.byref(self.p)))
+        L = self.layout
+        self.num_poses, self.num_codes = L.num_keyframes + L.num_frames, L.num_keyframes * L.code_size
+
+    def set_state(self, poses, codes):
+        """poses [(K + F), 7] (keyframes then frames), codes [K, C]: host arrays or device tensors (float64)"""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        args, keep = [], []
+        for x, n in ((poses, self.num_poses * 7), (codes, self.num_codes)):
+            if isinstance(x, torch.Tensor):
+                _check_tensor(hd, x, torch.float64, n, "state")
+                args.append(C.c_void_p(x.data_ptr()))
+            else:
+                a = np.ascontiguousarray(np.asarray(x, dtype=np.float64))
+                if a.size != n:
+                    raise ValueError(f"the state is {self.num_poses} poses and a [K, C] code array")
+                keep.append(a)
+                args.append(a.ctypes.data_as(C.c_void_p))
+        check(hd.h, lib().dfk_window_problem_set_state(hd.h, self.p, *args))
+
+    def get_state(self):
+        """(poses [(K + F), 7], codes [K, C]) float64 host arrays"""
+        self._al._hd.use_torch_stream()
+        P = np.zeros((self.num_poses, 7))
+        Q = np.zeros((self.layout.num_keyframes, self.layout.code_size))
+        check(self._al.handle, lib().dfk_window_problem_get_state(self._al.handle, self.p, P.ctypes.data_as(C.c_void_p),
+                                                                   Q.ctypes.data_as(C.c_void_p)))
+        check(self._al.handle, lib().dfk_synchronize(self._al.handle))
+        return P, Q
+
+    def linearize(self, out: torch.Tensor | None = None) -> torch.Tensor:
+        """dfk_window_problem_linearize: the window buffer at the state (asynchronous on torch's current stream)"""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        if out is None:
+            out = torch.empty(self._win.floats, dtype=torch.float32, device=f"cuda:{hd.device}")
+        _check_tensor(hd, out, torch.float32, self._win.floats, "out")
+        check(hd.h, lib().dfk_window_problem_linearize(hd.h, self.p, C.c_void_p(out.data_ptr())))
+        return out
+
+    def error(self, out: torch.Tensor | None = None) -> torch.Tensor:
+        """dfk_window_problem_error: [E | photometric | reprojection | geometric | priors | items without inliers |
+        inliers] float64 on the device (asynchronous)"""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        if out is None:
+            out = torch.empty(_lib.WINDOW_ERROR_DOUBLES, dtype=torch.float64, device=f"cuda:{hd.device}")
+        _check_tensor(hd, out, torch.float64, _lib.WINDOW_ERROR_DOUBLES, "out")
+        check(hd.h, lib().dfk_window_problem_error(hd.h, self.p, C.c_void_p(out.data_ptr())))
+        return out
+
+    def retract(self, dx: torch.Tensor):
+        """dfk_window_problem_retract: state <- retract(state, dx), dx [K B + 6 F] float64 on the device"""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        _check_tensor(hd, dx, torch.float64, self.layout.dim, "dx")
+        check(hd.h, lib().dfk_window_problem_retract(hd.h, self.p, C.c_void_p(dx.data_ptr())))
+
+    def lm(self, params, use_error: bool = False) -> dict:
+        """dfk_window_lm with window_opt.LMParams; returns the trace as a dict"""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        it = int(params.iterations)
+        prm = _lib.DfkLMParams(it, float(params.lambda_init), float(params.lambda_up), float(params.lambda_down),
+                               float(params.lambda_max), int(bool(params.fix_first_pose)),
+                               float(params.code_prior_weight), int(bool(use_error)))
+        e, lam, acc = np.zeros(it + 1), np.zeros(max(it, 1)), np.zeros(max(it, 1), dtype=np.int32)
+        tr = _lib.DfkLMTrace(e.ctypes.data_as(C.POINTER(C.c_double)), lam.ctypes.data_as(C.POINTER(C.c_double)),
+                             acc.ctypes.data_as(C.POINTER(C.c_int32)), 0, 0, 0, 0)
+        check(hd.h, lib().dfk_window_lm(hd.h, self.p, C.byref(prm), C.byref(tr)))
+        return dict(energy=e[:tr.num_energies].tolist(), lam=lam[:tr.num_steps].tolist(),
+                    accepted=[bool(a) for a in acc[:tr.num_steps]], linearisations=int(tr.linearisations),
+                    error_evaluations=int(tr.error_evaluations))
+
+    def close(self):
+        if getattr(self, "p", None):
+            lib().dfk_window_problem_destroy(self._al.handle, self.p)
+            self.p = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 # ------------------------------------------------------------------------------------------- SE3Aligner
 class SE3Aligner:
     """df::SE3Aligner<float> (sources/cuda/cu_se3aligner.h:38-86)."""

@@ -306,10 +306,11 @@ cudaError_t window_solver_create(int num_keyframes, int code_size, int num_frame
                                  const std::vector<int>& fixed_vars, WindowSolverDev** out);
 void window_solver_destroy(WindowSolverDev* s);
 size_t window_solver_tiles(const WindowSolverDev* s);
-// codes_host: K * C doubles, read only when prior > 0; *launches += the kernels enqueued
+// codes_host: K * C doubles, read only when prior > 0 (device memory when codes_on_device); *launches += the kernels
+// enqueued
 cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_dev, double lambda, double prior,
                                 const double* codes_host, double* dx_dev, int32_t* info_dev, cudaStream_t stream,
-                                uint64_t* launches);
+                                uint64_t* launches, bool codes_on_device = false);
 // Elimination of local keyframe 0 from a local tile system laid out as KfMargDev (tiles 0..n = column 0, diagonal first,
 // then the lower tiles (I, J) of 1..n): the solve's panel launch of column 0 (L of block 0, z = L^-1 g_0, Y_I = H_I0
 // L^-T) and its update launch (H_IJ -= Y_I Y_J^T, g_I -= Y_I z).  info gets 0 or 1 + the failed row.
@@ -373,6 +374,45 @@ cudaError_t launch_reprojection_error(int code_size, const ReprojItemDev* items_
                                       const float2* train_dev, float avg_dpt, float* out_dev, cudaStream_t s);
 cudaError_t launch_sparse_geometric_error(int code_size, const GeoItemDev* items_dev, int num_items, const int2* points_dev,
                                           float avg_dpt, float* out_dev, cudaStream_t s);
+
+// dfk_window_lm.cu : the window problem's loop kernels.  The state is [poses num_poses x 7 | codes K x C] doubles; a
+// slot int4 is (pose0, pose1, code0, code1).
+struct WindowReposeDev {
+  int code_size, num_poses;
+  const double* state;
+  SfmItemDev* dense;       const int4* dense_slots; int num_dense;  // q, t, R, P0, P1 and the fused-decode code
+  EvalErrorDesc* error;    const int4* error_slots; int num_error;  // pc.q, pc.t
+  ReprojItemDev* rep;      const int4* rep_slots;   int num_rep;    // sp and code
+  GeoItemDev* geo;         const int4* geo_slots;   int num_geo;    // sp, code0 and code1
+  DepthDecodeDesc* depth;  const int4* depth_slots; int num_depth;  // code (slot .z)
+};
+cudaError_t launch_window_repose(const WindowReposeDev& a, cudaStream_t stream);
+// out = retract(in, dx) for K keyframes (pose and code) and F frames (pose)
+cudaError_t launch_window_retract(const double* in, double* out, const double* dx, int K, int F, int C,
+                                  cudaStream_t stream);
+// delta row r = Local(x0 row r, keyframe ks[r]): [t - t0 | log(R R0^T) | c - c0], B doubles; x0 rows are [pose | code]
+cudaError_t launch_window_deltas(const double* state, int num_poses, int C, int n, const int* ks, const double* x0,
+                                 double* delta, cudaStream_t stream);
+struct WindowEnergyDev {
+  int B;
+  const float2* err_out;  // [num_error dense | num_rep | num_geo] rows [residual or b^T b | count (u32 bits)]
+  const double* areas;    // W * H of each dense error item
+  int num_error, num_rep, num_geo;
+  const float* buf_f;     // non-null: E is the window buffer's f (linearise mode), the error outputs are not read
+  int num_frame_priors;
+  const double* frame_rows;   // DFK_PRIOR_DOUBLES each
+  const double* frame_delta;  // B each
+  int num_kf_priors;
+  const double* kf_rows;      // back to back, prior q at kf_row_off[q]
+  const long long* kf_row_off;
+  const int* kf_mem_ptr;      // [Q + 1] members; deltas at kf_delta + mem_ptr[q] * B
+  const double* kf_delta;
+  const double* codes;        // K * C, for the code prior 1/2 w |c|^2
+  int num_codes;
+  double code_prior_weight;
+  double* out;  // [E | photometric | reprojection | geometric | priors | items without inliers | inliers | E + code prior]
+};
+cudaError_t launch_window_energy(const WindowEnergyDev& a, cudaStream_t stream);
 
 constexpr int kSimpleMaxBlocks = 1024;
 constexpr int kSimpleScratchFloats = kSimpleMaxBlocks * 32;

@@ -718,7 +718,7 @@ void window_solver_destroy(WindowSolverDev* s) { delete s; }
 
 cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_dev, double lambda, double prior,
                                 const double* codes_host, double* dx_dev, int32_t* info_dev, cudaStream_t stream,
-                                uint64_t* launches)
+                                uint64_t* launches, bool codes_on_device)
 {
   SolveArgs a{};
   a.buf = window_dev;
@@ -733,9 +733,10 @@ cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_de
   fa.frame_L = s->frame_L; fa.frame_bad = s->frame_bad;
   a.lambda = lambda; a.prior = prior;
   if (prior > 0.0) {
-    // pageable source: the copy is staged before the call returns, so the caller may reuse its array at once
-    cudaError_t e = cudaMemcpyAsync(s->codes, codes_host, (size_t)s->K * s->C * sizeof(double), cudaMemcpyHostToDevice,
-                                    stream);
+    // pageable source: the copy is staged before the call returns, so the caller may reuse its array at once.  A
+    // window problem passes its device state instead (a device-to-device copy on the stream)
+    cudaError_t e = cudaMemcpyAsync(s->codes, codes_host, (size_t)s->K * s->C * sizeof(double),
+                                    codes_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream);
     if (e != cudaSuccess) return e;
   }
   return with_code_size(s->C, [&](auto bc) {

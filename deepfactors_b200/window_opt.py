@@ -337,6 +337,38 @@ class WindowOptimizer:
         return poses, codes, trace
 
 
+class DeviceWindowOptimizer:
+    """WindowOptimizer's loop as one library call (dfk_window_lm on SfmWindowProblem.device_problem()): the state and
+    the accepted and candidate window buffers stay on the device, and each step reads back the solve's info and the
+    candidate's energy.  The policy is WindowOptimizer's with solve=prob.solve (and error=prob.error when
+    params.use_error), except that every linearisation re-evaluates every factor: an LM step moves every code, so the
+    linearisation cache would re-evaluate everything anyway.  run returns what WindowOptimizer.run returns.  A run
+    rewrites prob.records (see SfmWindowProblem.device_problem): invalidate the cache of a WindowOptimizer over the same
+    problem before its next run."""
+
+    def __init__(self, prob: "SfmWindowProblem", params: Optional[LMParams] = None, use_error: bool = False):
+        self.prob = prob
+        self.params = params or LMParams()
+        self.use_error = bool(use_error)
+        self.dev = prob.device_problem()
+
+    def run(self, poses, codes, frame_poses=None) -> Tuple[np.ndarray, np.ndarray, LMTrace]:
+        layout = self.prob.layout
+        K, F = layout.num_keyframes, layout.num_frames
+        frames = np.zeros((0, 7)) if frame_poses is None else np.asarray(frame_poses, np.float64).reshape(-1, 7)
+        if len(frames) != F:
+            raise ValueError(f"the window has {F} tracked frames: pass as many frame_poses")
+        self.dev.set_state(np.concatenate([np.asarray(poses, np.float64).reshape(-1, 7), frames]),
+                           np.asarray(codes, np.float64))
+        t = self.dev.lm(self.params, self.use_error)
+        p, c = self.dev.get_state()
+        n = len(self.prob.pairs) + len(self.prob.geometric)
+        trace = LMTrace(energy=t["energy"], lam=t["lam"], accepted=t["accepted"],
+                        factors_relinearised=[n] * t["linearisations"], frame_poses=p[K:] if F else None,
+                        linearisations=t["linearisations"], error_evaluations=t["error_evaluations"])
+        return p[:K], c, trace
+
+
 @dataclass
 class ReprojectionLink:
     """A reprojection factor between keyframes k0 -> k1 (ReprojectionFactor, reprojection_factor.cpp): matched keypoints
@@ -462,6 +494,22 @@ def _geometric_items(prob, j, a, b, pose0, pose1, code0, code1):
     return [dict(pose0=pose0, pose1=pose1, code0=code0, code1=code1, cam=prob.cams[0], prx0_orig=a[0]["prx_orig"],
                  prx0_jac=a[0]["prx_jac"], prx1_orig=b[0]["prx_orig"], prx1_jac=b[0]["prx_jac"],
                  dpt_grad1=b[0]["dpt_grad"], points_xy=gl.points_xy, huber_delta=gl.huber_delta)]
+
+
+def problem_slots(K: int, levels: int, pairs, num_photometric: int, links=(), geometric=()) -> dict:
+    """The state slots (pose0, pose1, code0, code1; -1 unused) of every item of SfmWindowProblem.device_problem: pairs
+    are the problem's pair list (photometric pairs, then one per reprojection link, then one (k, K + f) per tracked
+    frame); a pose slot >= K is frame slot - K.  dense: the photometric then the frame (pair, level) items in record
+    order; reproj / geo: one per link; depth: one decode per (keyframe, level); error: the dense items' error twins,
+    error_depth the decode each reads."""
+    P, PF = num_photometric, num_photometric + len(links)
+    ends = [tuple(pairs[p]) for p in list(range(P)) + list(range(PF, len(pairs)))]
+    return dict(dense=[(a, b, a, -1) for a, b in ends for _ in range(levels)],
+                reproj=[(int(ln.k0), int(ln.k1), int(ln.k0), -1) for ln in links],
+                geo=[(int(gl.k0), int(gl.k1), int(gl.k0), int(gl.k1)) for gl in geometric],
+                depth=[(-1, -1, k, -1) for k in range(K) for _ in range(levels)],
+                error=[(a, b, -1, -1) for a, b in ends for _ in range(levels)],
+                error_depth=[a * levels + l for a, b in ends for l in range(levels)])
 
 
 def _struct_floats(arr, name: str, count: int) -> np.ndarray:
@@ -720,6 +768,52 @@ class SfmWindowProblem:
         st["out"] = torch.empty((max(n, 1), 2), dtype=torch.float32, device=self.records.device)[:n]
         self._err = st
         return st
+
+    def device_problem(self):
+        """This window as one problem of the C ABI (aligners.WindowProblem, built once): the items linearise and error
+        use, each with the state slots it reads -- the photometric then the frame (pair, level) items (fused decode),
+        the reprojection links and the geometric links in record order, writing this problem's own record buffers (so
+        marginalize / marginalize_keyframe keep working), and error()'s depth decodes and error items -- and both prior
+        kinds with their frozen points.  DeviceWindowOptimizer runs on it.  A sharded window (allreduce) cannot.
+        The device problem writes self.records / self.geo_records: after a device run they hold its last linearised
+        point, so a WindowOptimizer over this problem that keeps running afterwards must start from an empty
+        linearisation cache (opt.cache.invalidate())."""
+        if self.allreduce is not None:
+            raise ValueError("a window with an all-reduce (sharded pairs) cannot run as one device problem")
+        if getattr(self, "_dev", None) is not None:
+            return self._dev
+        from .aligners import WindowProblem, make_geometric_items, make_reprojection_items
+        st = self._err if getattr(self, "_err", None) is not None else self._error_state()
+        K, L, C, P = len(self.kf), self.levels, self.al.CS, self._num_photometric
+        PF = P + len(self.links)
+        zero, zc = np.zeros(7, np.float32), np.zeros(C, np.float32)
+        dense = []
+        for p in list(range(P)) + list(range(PF, len(self.pairs))):
+            a, b = self.pairs[p]
+            lv1 = self.kf[b] if b < K else self.frames[b - K].levels
+            dense += _photometric_items(self, p, self.kf[a], lv1, zero, zero, zc, zc)
+        rep = [it for j, ln in enumerate(self.links)
+               for it in _reprojection_items(self, j, self.kf[ln.k0], None, zero, zero, zc, None)]
+        geo = [it for j, gl in enumerate(self.geometric)
+               for it in _geometric_items(self, j, self.kf[gl.k0], self.kf[gl.k1], zero, zero, zc, zc)]
+        kw = {}
+        if self._mpriors:
+            kw.update(frame_prior_kf=[pr.k for pr in self._mpriors],
+                      frame_prior_rows=np.stack([np.asarray(pr.row, np.float64) for pr in self._mpriors]),
+                      frame_prior_x0=np.stack([np.concatenate([pr.pose0, pr.code0]) for pr in self._mpriors]))
+        if self._kpriors:
+            kw.update(kf_prior_rows=np.concatenate([np.asarray(pr.row, np.float64).ravel() for pr in self._kpriors]),
+                      kf_prior_x0=np.stack([np.concatenate([pr.poses0[a], pr.codes0[a]])
+                                            for pr in self._kpriors for a in range(len(pr.keyframes))]))
+        sl = problem_slots(K, L, self.pairs, P, self.links, self.geometric)
+        self._dev = WindowProblem(
+            self.window, self.records, self.geo_records,
+            dense=self.al.make_work_items(dense) if dense else None, dense_slots=sl["dense"],
+            reproj=make_reprojection_items(rep, C) if rep else None, reproj_slots=sl["reproj"],
+            geo=make_geometric_items(geo, C) if geo else None, geo_slots=sl["geo"],
+            depth=st["depth_items"], depth_slots=sl["depth"],
+            error=st["dense_items"] if st["nd"] else None, error_slots=sl["error"], error_depth=sl["error_depth"], **kw)
+        return self._dev
 
     def linearise(self, poses, codes, todo, frame_poses=None):
         import torch

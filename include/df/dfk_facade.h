@@ -534,6 +534,111 @@ private:
 };
 
 // ---------------------------------------------------------------------------------------------
+// extension (no reference counterpart): a keyframe window problem and its Levenberg-Marquardt loop in the library
+// (dfk_window_problem_*, dfk_window_lm).  The reference's integrator restages every factor on every ISAM2 iteration
+// (mapper.cpp:518-519); here the items are staged once and only the state (poses and codes, fp64) changes.  RAII over
+// the C object; every call runs on the handle given at construction (e.g. SfmAligner<float, CS>::handle()), whose
+// sfmparams, Gram mode and SM limit at construction the problem keeps.  num_keyframes / num_frames are the window's.
+// ---------------------------------------------------------------------------------------------
+struct WindowError {  // window_opt.WindowError: each part summed in fp64 in factor order (buffer units)
+  double energy = 0.0, photometric = 0.0, reprojection = 0.0, geometric = 0.0, priors = 0.0;
+  int64_t no_inliers = 0, inliers = 0;
+};
+
+struct LMParams {  // window_opt.LMParams (the linearisation cache's eps has no counterpart: every factor is re-evaluated)
+  int iterations = 10;
+  double lambda_init = 1e-4, lambda_up = 10.0, lambda_down = 0.1, lambda_max = 1e6;
+  bool fix_first_pose = true;
+  double code_prior_weight = 0.0;
+  bool use_error = false;  // evaluate E at every candidate, linearise accepted points only
+};
+
+struct LMTrace {  // window_opt.LMTrace
+  std::vector<double> energy, lambda;
+  std::vector<bool> accepted;
+  int linearisations = 0, error_evaluations = 0;
+};
+
+template <int CS>
+class WindowProblem
+{
+public:
+  WindowProblem(DfkHandle h, const DfkWindowProblemDesc& desc, int num_keyframes, int num_frames)
+    : h_(h), K_(num_keyframes), F_(num_frames)
+  {
+    if (!h || num_keyframes < 1 || num_frames < 0)
+      throw std::invalid_argument("[WindowProblem] null handle / no keyframes / negative frame count");
+    detail::Check(h_, dfk_window_problem_create(h_, &desc, &p_));
+  }
+  ~WindowProblem() { dfk_window_problem_destroy(h_, p_); }
+  WindowProblem(const WindowProblem&) = delete;
+  WindowProblem& operator=(const WindowProblem&) = delete;
+
+  DfkWindowProblem* get() const { return p_; }
+
+  // poses: (K + F) x 7 (keyframes, then frames; Sophus::SE3 data() order), codes: K x CS, host
+  void SetState(const std::vector<double>& poses, const std::vector<double>& codes)
+  {
+    if (poses.size() != (size_t)(K_ + F_) * 7 || codes.size() != (size_t)K_ * CS)
+      throw std::invalid_argument("[WindowProblem] the state is (K + F) x 7 pose and K x CS code doubles");
+    detail::Check(h_, dfk_window_problem_set_state(h_, p_, poses.data(), codes.data()));
+    detail::Check(h_, dfk_synchronize(h_));  // the host vectors may go away when this returns
+  }
+  void GetState(std::vector<double>& poses, std::vector<double>& codes) const
+  {
+    poses.resize((size_t)(K_ + F_) * 7);
+    codes.resize((size_t)K_ * CS);
+    detail::Check(h_, dfk_window_problem_get_state(h_, p_, poses.data(), codes.data()));
+    detail::Check(h_, dfk_synchronize(h_));
+  }
+  // the window buffer at the state into window_dev (DEVICE, dfk_window_floats floats); asynchronous
+  void Linearize(float* window_dev) { detail::Check(h_, dfk_window_problem_linearize(h_, p_, window_dev)); }
+#ifdef DFK_FACADE_CUDART
+  // the energy at the state without linearising; synchronous (one small read-back with the CUDA runtime)
+  WindowError Error()
+  {
+    double* dev = nullptr;
+    if (cudaMalloc(&dev, sizeof(double) * DFK_WINDOW_ERROR_DOUBLES) != cudaSuccess)
+      throw std::runtime_error("[WindowProblem::Error] device allocation failed");
+    double o[DFK_WINDOW_ERROR_DOUBLES] = {};
+    DfkStatus st = dfk_window_problem_error(h_, p_, dev);
+    if (st == DFK_OK) st = dfk_synchronize(h_);
+    const cudaError_t e = st == DFK_OK ? cudaMemcpy(o, dev, sizeof(o), cudaMemcpyDeviceToHost) : cudaSuccess;
+    cudaFree(dev);
+    detail::Check(h_, st);
+    if (e != cudaSuccess) throw std::runtime_error("[WindowProblem::Error] result download failed");
+    WindowError r;
+    r.energy = o[0]; r.photometric = o[1]; r.reprojection = o[2]; r.geometric = o[3]; r.priors = o[4];
+    r.no_inliers = (int64_t)o[5]; r.inliers = (int64_t)o[6];
+    return r;
+  }
+#endif
+  // Levenberg-Marquardt from the state (dfk_window_lm); the state is the last accepted point afterwards
+  LMTrace Optimize(const LMParams& p)
+  {
+    if (p.iterations < 0) throw std::invalid_argument("[WindowProblem::Optimize] iterations < 0");
+    const DfkLMParams c{p.iterations, p.lambda_init, p.lambda_up, p.lambda_down, p.lambda_max, p.fix_first_pose ? 1 : 0,
+                        p.code_prior_weight, p.use_error ? 1 : 0};
+    std::vector<double> e(p.iterations + 1), lam(std::max(p.iterations, 1));
+    std::vector<int32_t> acc(std::max(p.iterations, 1));
+    DfkLMTrace t{e.data(), lam.data(), acc.data(), 0, 0, 0, 0};
+    detail::Check(h_, dfk_window_lm(h_, p_, &c, &t));
+    LMTrace r;
+    r.energy.assign(e.begin(), e.begin() + t.num_energies);
+    r.lambda.assign(lam.begin(), lam.begin() + t.num_steps);
+    for (int i = 0; i < t.num_steps; ++i) r.accepted.push_back(acc[i] != 0);
+    r.linearisations = t.linearisations;
+    r.error_evaluations = t.error_evaluations;
+    return r;
+  }
+
+private:
+  DfkHandle h_;
+  int K_, F_;
+  DfkWindowProblem* p_ = nullptr;
+};
+
+// ---------------------------------------------------------------------------------------------
 // cu_image_proc.h:27-44 free functions.  They use one process-wide handle (default stream semantics
 // of the reference); pass an explicit handle to run them on another stream.
 // ---------------------------------------------------------------------------------------------

@@ -612,6 +612,117 @@ DfkStatus dfk_build_image_pyramid(DfkHandle h, const DfkImage* imgs, const DfkIm
 /* df::SquaredError (cu_image_proc.h:35-39, cu_image_proc.cpp:190-242). Synchronous. */
 DfkStatus dfk_squared_error(DfkHandle h, const DfkImage* a, const DfkImage* b, float* out);
 
+/* ------------------------------------------------------------------ keyframe window problem (the LM loop on the device) */
+
+/* A window problem: the keyframe window's Levenberg-Marquardt loop in the library, with the window's state (poses and
+ * codes, fp64) on the device.  It holds every work item of a window once, validated and planned at create; between
+ * iterations only the pose- and code-dependent fields of the items change, and a device launch rewrites them from the
+ * state (bit for bit what the host staging of the batch calls computes from the same fp32-rounded poses and codes).
+ *
+ * State: K keyframe poses then F tracked-frame poses ((K + F) x 7, the pose convention above), then K codes (K x C).
+ * Every item names the state slots it reads (DfkWindowItemSlots): a pose slot s < K is keyframe s, s >= K is frame
+ * s - K; a code slot is a keyframe.  The pose and code fields of the template items are ignored.
+ *
+ * The descriptor describes a window in terms the ABI already has:
+ *   window          from any dfk_window_create*; the problem refers to it, so it must outlive the problem
+ *   dense           the photometric then the frame (pair, level) items in record order (DfkSfmWorkItem, fused depth
+ *                   decode: prx_orig required, dpt0 is the output), with slots (pose0, pose1, code0); record i of
+ *                   records_dev
+ *   reproj          the reprojection links (DfkReprojectionItem), slots (pose0, pose1, code0); record num_dense + j of
+ *                   records_dev (unscaled records, as the window expects them)
+ *   geo             the sparse geometric links (DfkSparseGeometricItem), slots (pose0, pose1, code0, code1); record j of
+ *                   geo_records_dev
+ *   depth           the depth decodes of the error path (DfkDepthDecodeItem, e.g. one per (keyframe, level)), slot
+ *                   code0; their dpt views give the size only: the problem decodes into depth scratch of its own
+ *   error           the error items (DfkSfmWorkItem without code), slots (pose0, pose1); error_depth[i] is the depth
+ *                   item whose decode item i reads (its dpt0 view is ignored)
+ *   frame priors    num_frame_priors DFK_PRIOR_DOUBLES(C) rows on keyframes frame_prior_kf, frozen at frame_prior_x0
+ *                   ([pose 7 | code C] doubles each)
+ *   keyframe priors the window's keyframe priors (dfk_window_create_priors) as dfk_window_add_keyframe_priors takes
+ *                   them, frozen at kf_prior_x0 ([pose 7 | code C] doubles per member, prior by prior)
+ * Every array is HOST memory and copied, except records_dev / geo_records_dev (DEVICE, the caller's record buffers,
+ * which linearize writes and which must outlive the problem).  The image views are the caller's and must outlive it.
+ * Create validates every item as the batch calls do, plans the RunStep launch and takes the handle's settings: its Gram
+ * mode, SM limit and every DenseSfmParams value (valid_border, min_dpt, avg_dpt, huber_delta) at create hold for every
+ * later call of the problem, for all its factor kinds; later dfk_sfm_set_params / dfk_sfm_set_gram_mode /
+ * dfk_set_sm_limit calls do not change it.  An error item must not ask for a fused decode (code NULL).  Create uploads the item arrays, which the problem owns with their code
+ * slots and ray tables (no pointer into the handle's shared scratch), creates the solver with the first pose fixed and
+ * allocates the depth scratch of the error path.  A rejected create writes nothing. */
+typedef struct DfkWindowProblem DfkWindowProblem;
+typedef struct {
+  int32_t pose0, pose1, code0, code1; /* state slots; -1 where an item kind does not read one */
+} DfkWindowItemSlots;
+typedef struct {
+  const DfkWindow* window;
+  int32_t num_dense;
+  const DfkSfmWorkItem* dense;
+  const DfkWindowItemSlots* dense_slots;
+  int32_t num_reproj;
+  const DfkReprojectionItem* reproj;
+  const DfkWindowItemSlots* reproj_slots;
+  int32_t num_geo;
+  const DfkSparseGeometricItem* geo;
+  const DfkWindowItemSlots* geo_slots;
+  int32_t num_depth;
+  const DfkDepthDecodeItem* depth;
+  const DfkWindowItemSlots* depth_slots;
+  int32_t num_error;
+  const DfkSfmWorkItem* error;
+  const DfkWindowItemSlots* error_slots;
+  const int32_t* error_depth;
+  int32_t num_frame_priors;
+  const int32_t* frame_prior_kf;
+  const double* frame_prior_rows;
+  const double* frame_prior_x0;
+  const double* kf_prior_rows;
+  const double* kf_prior_x0;
+  float* records_dev;
+  float* geo_records_dev;
+} DfkWindowProblemDesc;
+DfkStatus dfk_window_problem_create(DfkHandle h, const DfkWindowProblemDesc* desc, DfkWindowProblem** out);
+/* h must not be NULL; p may be */
+DfkStatus dfk_window_problem_destroy(DfkHandle h, DfkWindowProblem* p);
+/* poses: (K + F) x 7 doubles, codes: K x C doubles, host or device memory.  Asynchronous on the handle's stream. */
+DfkStatus dfk_window_problem_set_state(DfkHandle h, DfkWindowProblem* p, const double* poses, const double* codes);
+DfkStatus dfk_window_problem_get_state(DfkHandle h, const DfkWindowProblem* p, double* poses, double* codes);
+/* The window buffer at the state: every item re-posed from the state on the device, then the batches in the order of
+ * SfmWindowProblem.linearise with every factor stale -- the dense items in one RunStep launch (depth decode fused in),
+ * the reprojection links, the geometric links -- the assembly, and the frame and keyframe priors with their deltas
+ * Local(x0, x) formed on the device in fp64.  window_dev: DEVICE, dfk_window_floats() floats.  Asynchronous. */
+DfkStatus dfk_window_problem_linearize(DfkHandle h, DfkWindowProblem* p, float* window_dev);
+/* doubles of dfk_window_problem_error's output */
+#define DFK_WINDOW_ERROR_DOUBLES 7
+/* The window energy at the state without linearising (SfmWindowProblem.error): out_dev (DEVICE) = [E | photometric |
+ * reprojection | geometric | priors | items without inliers | total inliers], each part summed in fp64 in factor order.
+ * An item with inliers adds res / inliers * W * H, one without adds 0; a link its b^T b; a prior f0 - 2 g^T d + d^T G d.
+ * The keyframes' own depth and the records are not touched.  Asynchronous. */
+DfkStatus dfk_window_problem_error(DfkHandle h, DfkWindowProblem* p, double* out_dev);
+/* state <- retract(state, dx): t += dt, q = normalize(exp(w) q), c += dc, in fp64, for the keyframes and then the frames
+ * (dx_dev: DEVICE, K (6 + C) + 6 F doubles, the solve's layout).  Asynchronous. */
+DfkStatus dfk_window_problem_retract(DfkHandle h, DfkWindowProblem* p, const double* dx_dev);
+
+/* window_opt.LMParams; lambda_up and lambda_down finite and > 0 */
+typedef struct {
+  int32_t iterations;
+  double lambda_init, lambda_up, lambda_down, lambda_max;
+  int32_t fix_first_pose;   /* 1: variables 0..5 (keyframe 0's pose) are held */
+  double code_prior_weight; /* >= 0: adds 1/2 w |c|^2 to the energy and w I / -w c to the solve */
+  int32_t use_error;        /* 1: evaluate E at every candidate and linearise accepted points only */
+} DfkLMParams;
+/* window_opt.LMTrace; the caller's HOST arrays: energy iterations + 1 entries, lambda and accepted iterations each */
+typedef struct {
+  double* energy;           /* accepted energies, energy[0] = the start point's */
+  double* lambda;           /* the damping of every step */
+  int32_t* accepted;        /* 1 for an accepted step */
+  int32_t num_energies, num_steps, linearisations, error_evaluations;  /* out */
+} DfkLMTrace;
+/* Levenberg-Marquardt from the problem's state (window_opt.WindowOptimizer.run, the policy of its docstring); on return
+ * the state is the last accepted point, and the records describe the point last linearised (without use_error, the
+ * last candidate, accepted or not).  Every linearisation re-evaluates every factor (an LM step moves every code, so a
+ * linearisation cache would re-evaluate everything anyway).  The state and the accepted and candidate window buffers
+ * stay on the device; each step reads back the solve's info and the candidate's energy.  Synchronous. */
+DfkStatus dfk_window_lm(DfkHandle h, DfkWindowProblem* p, const DfkLMParams* params, DfkLMTrace* trace);
+
 #ifdef __cplusplus
 }
 #endif

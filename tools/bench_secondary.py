@@ -36,8 +36,11 @@ One JSON line per case:
     from perturbed poses with the device solve, without and with `error` (its linearisation and error-evaluation
     counts) -- wall clock to a synchronise and summed device time (torch.profiler, separate run); the byte model of
     both paths is printed beside them.
+  * the LM loop in the library (`--only lm`): window200 at C = 32 and 128, a 10-iteration LM by DeviceWindowOptimizer
+    (dfk_window_lm) against WindowOptimizer(solve=prob.solve) and WindowOptimizer(..., error=prob.error), alternated --
+    wall clock to a synchronise and summed device time (torch.profiler, separate run).
 Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` /
-`--only frames` / `--only slide` / `--only error` runs those cases alone.
+`--only frames` / `--only slide` / `--only error` / `--only lm` runs those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -56,7 +59,7 @@ sys.path.insert(0, ROOT)
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
-    ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error"], default=None)
+    ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error", "lm"], default=None)
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -90,6 +93,8 @@ def main():
         return slide_cases(args, torch, print)
     if args.only == "error":
         return error_cases(args, torch, print)
+    if args.only == "lm":
+        return lm_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -711,6 +716,72 @@ def error_cases(args, torch, print):
                               "error_evaluations": tr.error_evaluations, "accepted": tr.accepted,
                               "energy_first_last": [tr.energy[0], tr.energy[-1]], "timing": timing}), flush=True)
         del prob, keyframes, shared, jac, arr, dec
+        torch.cuda.empty_cache()
+
+
+def lm_cases(args, torch, print):
+    """window200 at C = 32 and 128: a 10-iteration LM as one library call (DeviceWindowOptimizer, dfk_window_lm) against
+    WindowOptimizer(solve=prob.solve) and WindowOptimizer(..., error=prob.error), alternated, from the same perturbed
+    start.  Each optimizer has its own SfmWindowProblem, built (and, for the device loop, device_problem() created) before
+    the timed runs: the setup is once per window, the loop once per window update."""
+    import numpy as np
+    from deepfactors_b200 import se3, synth
+    from deepfactors_b200.aligners import SfmAligner
+    from deepfactors_b200.window_opt import DeviceWindowOptimizer, LMParams, SfmWindowProblem, WindowOptimizer
+    sys.path.insert(0, ROOT)
+    from bench import window_pairs
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
+    levels, num_kf = 4, 50
+    reps = max(3, args.reps // 5)
+    timing = ("wall clock of one run() to a synchronise, median over the alternated repetitions; device time = summed "
+              "kernel + copy time of one run(), torch.profiler (separate run)")
+    for cs in (32, 128):
+        base = synth.make_pair(640, 480, cs, levels, seed=7)
+        shared = [dict(img=up(L.img0), grad=up(L.grad1), prx_orig=up(L.prx_orig)) for L in base.levels]
+        jac = [up(L.prx_jac) for L in base.levels]
+        gen = torch.Generator(device="cuda").manual_seed(cs)
+        keyframes = [[dict(sh, prx_jac=j + 1e-3 * torch.randn(j.shape, device="cuda", generator=gen),
+                           dpt=torch.zeros_like(sh["img"]), valid=torch.zeros_like(sh["img"]))
+                      for sh, j in zip(shared, jac)] for _ in range(num_kf)]
+        pairs = window_pairs(num_kf, 200)
+        cams = [L.cam for L in base.levels]
+        al = SfmAligner(cs)
+        rng = np.random.default_rng(cs)
+        poses = np.stack([se3.make_pose(rng.standard_normal(3) * 0.003, rng.standard_normal(3) * 0.01, np.float64)
+                          for _ in range(num_kf)])
+        poses[0] = se3.identity(np.float64)
+        codes = np.zeros((num_kf, cs))
+        prm = LMParams(iterations=10, lambda_init=1e-4)
+        runs = {}
+        for name in ("DeviceWindowOptimizer (dfk_window_lm)", "WindowOptimizer(solve=prob.solve)",
+                     "WindowOptimizer(solve=prob.solve, error=prob.error)"):
+            p = SfmWindowProblem(al, cams, keyframes, pairs)
+            if name.startswith("Device"):
+                opt = DeviceWindowOptimizer(p, prm)
+                runs[name] = (lambda o=opt: o.run(poses, codes))
+            else:
+                err = p.error if "error=" in name else None
+                runs[name] = (lambda p=p, err=err: WindowOptimizer(p.layout, p.linearise, prm, solve=p.solve,
+                                                                   error=err).run(poses, codes))
+        traces, walls = {}, {n: [] for n in runs}
+        for name, fn in runs.items():  # warm-up: module loads, allocations, the solver's workspace
+            _, _, traces[name] = fn()
+        torch.cuda.synchronize()
+        for _ in range(reps):
+            for name, fn in runs.items():
+                t0 = time.perf_counter()
+                fn()
+                torch.cuda.synchronize()
+                walls[name].append((time.perf_counter() - t0) * 1e6)
+        for name, fn in runs.items():
+            tr = traces[name]
+            print(json.dumps({"case": f"window200 C={cs} ({num_kf} keyframes, {len(pairs)} pairs, {levels} levels "
+                                      f"640x480): 10-iteration LM, {name}",
+                              "us_total": float(np.median(walls[name])), "us_runs": walls[name],
+                              "device_us_total": _device_us(torch, fn, 1), "linearisations": tr.linearisations,
+                              "error_evaluations": tr.error_evaluations, "accepted": tr.accepted,
+                              "energy_first_last": [tr.energy[0], tr.energy[-1]], "timing": timing}), flush=True)
+        del runs, keyframes, shared, jac
         torch.cuda.empty_cache()
 
 
