@@ -123,6 +123,17 @@ class DfkLMTrace(C.Structure):
                 ("linearisations", C.c_int32), ("error_evaluations", C.c_int32)]
 
 
+class DfkLevelSchedule(C.Structure):
+    _fields_ = [("num_levels", C.c_int32), ("iters", C.POINTER(C.c_int32)), ("dense_level", C.POINTER(C.c_int32)),
+                ("error_pair", C.POINTER(C.c_int32)), ("error_level", C.POINTER(C.c_int32)), ("num_pairs", C.c_int32),
+                ("pair_steps_done", C.POINTER(C.c_int32)), ("pair_remove_after", C.POINTER(C.c_uint8))]
+
+
+class DfkLevelTrace(C.Structure):
+    _fields_ = [("switch_energy", C.POINTER(C.c_double)), ("pair_levels", C.POINTER(C.c_int32)),
+                ("pair_steps_done", C.POINTER(C.c_int32)), ("num_switches", C.c_int32)]
+
+
 WINDOW_ERROR_DOUBLES = 7  # DFK_WINDOW_ERROR_DOUBLES
 
 
@@ -194,6 +205,9 @@ SYMBOLS = {
     "dfk_window_problem_error": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
     "dfk_window_problem_retract": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
     "dfk_window_lm": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkLMParams), C.POINTER(DfkLMTrace)]),
+    "dfk_window_problem_set_active": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dfk_window_lm_levels": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkLMParams), C.POINTER(DfkLevelSchedule),
+                                       C.POINTER(DfkLMTrace), C.POINTER(DfkLevelTrace)]),
     "dfk_se3_run_step": (C.c_int, [_H, _F, _CAM, _IMG, _IMG, _IMG, _IMG, _F, _F, _F, C.POINTER(C.c_uint64)]),
     "dfk_se3_track": (C.c_int, [_H, _F, C.POINTER(DfkTrackLevel), C.c_int, _F, _F, _F, _F, C.c_int]),
     "dfk_se3_track_batch": (C.c_int, [_H, C.c_int, C.c_int, _F, C.POINTER(DfkTrackLevel), _F, _F, _F]),

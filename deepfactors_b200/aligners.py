@@ -524,6 +524,7 @@ class Window:
         k0 = np.ascontiguousarray([p[0] for p in self.layout.pairs], dtype=np.int32)
         k1 = np.ascontiguousarray([p[1] for p in self.layout.pairs], dtype=np.int32)
         ip = np.ascontiguousarray(item_pair, dtype=np.int32)
+        self.item_pair = ip.copy()
         iw = np.ascontiguousarray([s[0] for s in item_sizes], dtype=np.int32)
         ih = np.ascontiguousarray([s[1] for s in item_sizes], dtype=np.int32)
         I32 = C.POINTER(C.c_int32)
@@ -813,6 +814,7 @@ class WindowProblem:
         check(self._al.handle, lib().dfk_window_problem_create(self._al.handle, C.byref(d), C.byref(self.p)))
         L = self.layout
         self.num_poses, self.num_codes = L.num_keyframes + L.num_frames, L.num_keyframes * L.code_size
+        self.num_dense, self.num_error = nd, ne
 
     def set_state(self, poses, codes):
         """poses [(K + F), 7] (keyframes then frames), codes [K, C]: host arrays or device tensors (float64)"""
@@ -884,6 +886,62 @@ class WindowProblem:
         return dict(energy=e[:tr.num_energies].tolist(), lam=lam[:tr.num_steps].tolist(),
                     accepted=[bool(a) for a in acc[:tr.num_steps]], linearisations=int(tr.linearisations),
                     error_evaluations=int(tr.error_evaluations))
+
+    def set_active(self, dense_active, error_active=None):
+        """dfk_window_problem_set_active: bool masks over the dense and the error items (error_active None: the dense
+        mask, which needs as many error items as dense items)"""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        d = np.ascontiguousarray(np.asarray(dense_active, dtype=bool).astype(np.uint8).ravel())
+        e = None if error_active is None else np.ascontiguousarray(np.asarray(error_active, bool).astype(np.uint8).ravel())
+        if d.size != self.num_dense or (e is not None and e.size != self.num_error) or \
+                (e is None and self.num_error != self.num_dense):
+            raise ValueError(f"masks of {self.num_dense} dense and {self.num_error} error items expected (error_active "
+                             "may be None only with as many error as dense items)")
+        check(hd.h, lib().dfk_window_problem_set_active(hd.h, self.p, d.ctypes.data_as(C.c_void_p),
+                                                         None if e is None else e.ctypes.data_as(C.c_void_p)))
+
+    def lm_levels(self, params, schedule, use_error: bool = False) -> dict:
+        """dfk_window_lm_levels with window_opt.LMParams and window_opt.LevelSchedule; returns dfk_window_lm's trace
+        dict plus switch_energy, pair_levels (per step, per pair; -1 = off) and pair_steps_done"""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        it = int(params.iterations)
+        prm = _lib.DfkLMParams(it, float(params.lambda_init), float(params.lambda_up), float(params.lambda_down),
+                               float(params.lambda_max), int(bool(params.fix_first_pose)),
+                               float(params.code_prior_weight), int(bool(use_error)))
+        P = len(schedule.steps_done)
+        # the C call reads num_dense / num_error / num_pairs entries: wrong lengths are rejected here
+        ln = lambda x: len(np.ravel(x))
+        if ln(schedule.item_level) != self.num_dense or ln(schedule.item_pair) != self.num_dense or \
+                ln(schedule.remove_after) != P or \
+                any(x is not None and ln(x) != self.num_error for x in (schedule.error_pair, schedule.error_level)):
+            raise ValueError(f"a schedule of {self.num_dense} dense items, {self.num_error} error items and "
+                             f"{P} pairs expected")
+        # the device takes each dense item's pair from the window: the schedule's pairing must be the same
+        ids = self._win.item_pair[:self.num_dense]
+        if not np.array_equal(np.searchsorted(np.unique(ids), ids), np.asarray(schedule.item_pair)):
+            raise ValueError("schedule.item_pair is not the window's pairing of the dense items (the distinct window "
+                             "pairs of the dense items in window order)")
+        i32 = lambda x: np.ascontiguousarray(np.asarray(x, dtype=np.int32).ravel())
+        iters, dl, steps = i32(schedule.iters), i32(schedule.item_level), i32(schedule.steps_done)
+        rem = np.ascontiguousarray(np.asarray(schedule.remove_after, dtype=bool).astype(np.uint8).ravel())
+        ep = None if schedule.error_pair is None else i32(schedule.error_pair)
+        el = None if schedule.error_level is None else i32(schedule.error_level)
+        ip = lambda a: None if a is None else a.ctypes.data_as(C.POINTER(C.c_int32))
+        sc = _lib.DfkLevelSchedule(len(iters), ip(iters), ip(dl), ip(ep), ip(el), P, ip(steps),
+                                   rem.ctypes.data_as(C.POINTER(C.c_uint8)) if rem.size else None)
+        e, lam, acc = np.zeros(it + 1), np.zeros(max(it, 1)), np.zeros(max(it, 1), dtype=np.int32)
+        sw, lv, done = np.zeros(max(it, 1)), np.zeros(max(it * P, 1), dtype=np.int32), np.zeros(max(P, 1), np.int32)
+        tr = _lib.DfkLMTrace(e.ctypes.data_as(C.POINTER(C.c_double)), lam.ctypes.data_as(C.POINTER(C.c_double)),
+                             acc.ctypes.data_as(C.POINTER(C.c_int32)), 0, 0, 0, 0)
+        lt = _lib.DfkLevelTrace(sw.ctypes.data_as(C.POINTER(C.c_double)), ip(lv), ip(done), 0)
+        check(hd.h, lib().dfk_window_lm_levels(hd.h, self.p, C.byref(prm), C.byref(sc), C.byref(tr), C.byref(lt)))
+        n = tr.num_steps
+        return dict(energy=e[:tr.num_energies].tolist(), lam=lam[:n].tolist(), accepted=[bool(a) for a in acc[:n]],
+                    linearisations=int(tr.linearisations), error_evaluations=int(tr.error_evaluations),
+                    switch_energy=sw[:lt.num_switches].tolist(),
+                    pair_levels=[lv[s * P:(s + 1) * P].tolist() for s in range(n)], pair_steps_done=done[:P].tolist())
 
     def close(self):
         if getattr(self, "p", None):

@@ -17,6 +17,7 @@
 
 #include "dfk.h"
 #include "dfk_internal.h"
+#include "dfk_levels.h"
 #include "dfk_lm.h"
 #include "dfk_se3.cuh"
 
@@ -379,6 +380,8 @@ uint32_t perm_multiplier(uint32_t n)
   return m % n == 0 ? 1 : m;
 }
 
+void plan_tiles(SfmItemDev* items, int n, int max_ctas, SfmLaunchPlan* plan);
+
 DfkStatus build_items(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_size, int tile_px, int max_ctas,
                       const float* codes_dev, SfmLaunchPlan* plan)
 {
@@ -391,7 +394,6 @@ DfkStatus build_items(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_
   }
   const DfkDenseSfmParams& sp = h->params.sfmparams;
   h->items_host.resize(n);
-  uint32_t tile_cursor = 0;
   for (int i = 0; i < n; ++i) {
     const DfkSfmWorkItem& w = items[i];
     SfmItemDev& d = h->items_host[i];
@@ -446,8 +448,6 @@ DfkStatus build_items(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_
     }
     d.ray_tab = h->ray_cache[rt].dev.ptr;
     if (!h->ray_cache[rt].built) h->ray_pending.push_back(rt);
-    d.tile_begin = tile_cursor;
-    tile_cursor += d.num_tiles;
     d.perm_mul = perm_multiplier(d.num_tiles);
     d.mag_tiles = (uint32_t)((1ull << 32) / d.num_tiles);
     d.mag_width = (uint32_t)((1ull << 32) / W);
@@ -459,6 +459,19 @@ DfkStatus build_items(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_
     if (aligned(d.grad1, 8) && d.grad1_pitch % 2 == 0) d.flags |= ITEM_FLAG_GRAD_ALIGNED;
     if (fused) d.flags |= ITEM_FLAG_FUSED_DEPTH;
   }
+  plan_tiles(h->items_host.data(), n, max_ctas, plan);
+  return DFK_OK;
+}
+
+// the tile plan of items whose num_tiles are set: their global tile ranges back to back, and which CTAs (and partial
+// slots) each one's tiles fall to when CTA c of the grid owns global tiles [c T / G, (c + 1) T / G)
+void plan_tiles(SfmItemDev* items, int n, int max_ctas, SfmLaunchPlan* plan)
+{
+  uint32_t tile_cursor = 0;
+  for (int i = 0; i < n; ++i) {
+    items[i].tile_begin = tile_cursor;
+    tile_cursor += items[i].num_tiles;
+  }
   const int T = (int)tile_cursor;
   int G = std::min(max_ctas, T);
   if (G < 1) G = 1;
@@ -469,7 +482,7 @@ DfkStatus build_items(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_
   uint32_t partial_cursor = 0;
   int c = 0;
   for (int i = 0; i < n; ++i) {
-    SfmItemDev& d = h->items_host[i];
+    SfmItemDev& d = items[i];
     const long long tb = d.tile_begin, te = tb + d.num_tiles;
     while ((long long)(c + 1) * T / G <= tb) ++c;  // first CTA whose range ends after tb
     int first = c, last = c;
@@ -480,7 +493,6 @@ DfkStatus build_items(DfkHandle h, const DfkSfmWorkItem* items, int n, int code_
     partial_cursor += d.num_ctas;
   }
   plan->num_partials = (int)partial_cursor;
-  return DFK_OK;
 }
 
 constexpr size_t kMaxEventPairs = 8192;
@@ -777,6 +789,22 @@ struct DfkWindowProblem {
   DeviceBuf<double> dx;
   DeviceBuf<unsigned char> small;  // [energy 8 doubles | info int32]
   PinnedBuf<unsigned char> small_host;
+  // active subsets (dfk_window_problem_set_active): the create-time dense and error items with their slots and areas
+  // are the templates a mask selects from; the selected items go to arrays of their own, so the full arrays stay as
+  // create planned them and an all-active mask runs exactly the create-time launches
+  std::vector<SfmItemDev> dense_tmpl;
+  std::vector<EvalErrorDesc> err_tmpl;
+  std::vector<int4> slots_tmpl;      // dense | error
+  std::vector<double> areas_tmpl;
+  bool sub_dense = false, sub_err = false;
+  int nda = 0, nea = 0;              // active dense / error items while sub_dense / sub_err
+  SfmLaunchPlan sub_plan;
+  DeviceBuf<SfmItemDev> dense_sub;
+  DeviceBuf<EvalErrorDesc> err_sub;
+  DeviceBuf<int4> sub_slots;         // dense [0, nd) | error [nd, nd + ne)
+  DeviceBuf<double> areas_sub;
+  DeviceBuf<int> rec_src;            // record slot i <- subset record rec_src[i], -1: zeros
+  DeviceBuf<float> sub_records;
   ~DfkWindowProblem()
   {
     window_solver_destroy(solver[0]);
@@ -798,6 +826,12 @@ WindowReposeDev repose_args(const DfkWindowProblem* p, const double* state)
   a.state = state;
   a.dense = p->dense.ptr; a.dense_slots = sl; a.num_dense = p->nd;
   a.error = p->err.ptr; a.error_slots = sl + p->nd; a.num_error = p->ne;
+  if (p->sub_dense) {
+    a.dense = p->dense_sub.ptr; a.dense_slots = p->sub_slots.ptr; a.num_dense = p->nda;
+  }
+  if (p->sub_err) {
+    a.error = p->err_sub.ptr; a.error_slots = p->sub_slots.ptr + p->nd; a.num_error = p->nea;
+  }
   a.rep = reinterpret_cast<ReprojItemDev*>(p->rep.ptr); a.rep_slots = sl + p->nd + p->ne; a.num_rep = p->nr;
   a.geo = reinterpret_cast<GeoItemDev*>(p->geo.ptr); a.geo_slots = sl + p->nd + p->ne + p->nr; a.num_geo = p->ng;
   a.depth = reinterpret_cast<DepthDecodeDesc*>(p->depth.ptr); a.depth_slots = sl + p->nd + p->ne + p->nr + p->ng;
@@ -821,7 +855,18 @@ DfkStatus problem_linearize(DfkHandle h, DfkWindowProblem* p, const double* stat
   DFK_CUDA(h, launch_window_repose(repose_args(p, state), h->stream), what);
   h->launches += 1;
   const float avg = p->avg_dpt;
-  if (p->nd > 0) {
+  if (p->sub_dense) {  // the active items only, then every record slot from the subset's records or zeros
+    if (p->nda > 0) {
+      DFK_CUDA(h, h->partials_dev.ensure((size_t)p->sub_plan.num_partials * p->step.pfloats),
+               "[WindowProblem::linearize] scratch allocation failed");
+      DFK_TRY(launch_step(h, p->step, p->C, p->dense_sub.ptr, p->nda, p->sub_plan, h->partials_dev.ptr,
+                          p->sub_records.ptr));
+    }
+    DFK_CUDA(h, launch_window_scatter_records(p->sub_records.ptr, p->rec_src.ptr, p->nd, DFK_SFM_RECORD_FLOATS(p->C),
+                                              p->records, h->stream),
+             what);
+    h->launches += 1;
+  } else if (p->nd > 0) {
     DFK_CUDA(h, h->partials_dev.ensure((size_t)p->plan.num_partials * p->step.pfloats),
              "[WindowProblem::linearize] scratch allocation failed");
     DFK_TRY(launch_step(h, p->step, p->C, p->dense.ptr, p->nd, p->plan, h->partials_dev.ptr, p->records));
@@ -867,8 +912,8 @@ WindowEnergyDev energy_args(const DfkWindowProblem* p, const double* state, doub
   WindowEnergyDev a{};
   a.B = p->B;
   a.err_out = reinterpret_cast<const float2*>(p->err_out.ptr);
-  a.areas = p->areas.ptr;
-  a.num_error = p->ne; a.num_rep = p->nr; a.num_geo = p->ng;
+  a.areas = p->sub_err ? p->areas_sub.ptr : p->areas.ptr;
+  a.num_error = p->sub_err ? p->nea : p->ne; a.num_rep = p->nr; a.num_geo = p->ng;
   a.num_frame_priors = p->mf; a.frame_rows = p->frows.ptr; a.frame_delta = p->delta.ptr;
   a.num_kf_priors = p->w->kp.num_priors; a.kf_rows = p->kfrows.ptr; a.kf_row_off = p->w->kp.off;
   a.kf_mem_ptr = p->w->kp.mem_ptr; a.kf_delta = p->delta.ptr + (size_t)p->mf * p->B;
@@ -893,35 +938,188 @@ DfkStatus problem_error(DfkHandle h, DfkWindowProblem* p, const double* state, d
     h->launches += 1;
   }
   float* out = p->err_out.ptr;
-  if (p->ne > 0) {
+  // with an active subset only its items are evaluated, and their rows come first (energy_args reads as many)
+  const int ne = p->sub_err ? p->nea : p->ne;
+  if (ne > 0) {
     const char* sw = "[WindowProblem::error] scratch allocation failed";
     DFK_CUDA(h, h->eval_partials.ensure((size_t)p->err_rows * 32), sw);
     if (h->eval_counters.cap < (size_t)p->ne) {
       DFK_CUDA(h, h->eval_counters.ensure((size_t)p->ne), sw);
       DFK_CUDA(h, cudaMemsetAsync(h->eval_counters.ptr, 0, sizeof(unsigned int) * h->eval_counters.cap, h->stream), sw);
     }
-    DFK_CUDA(h, launch_eval_error_batch(p->err.ptr, p->ne, p->err_max_blocks, p->huber_delta,
-                                        h->eval_partials.ptr, h->eval_counters.ptr, out, h->stream),
+    DFK_CUDA(h, launch_eval_error_batch(p->sub_err ? p->err_sub.ptr : p->err.ptr, ne, p->err_max_blocks,
+                                        p->huber_delta, h->eval_partials.ptr, h->eval_counters.ptr, out, h->stream),
              what);
     h->launches += 1;
   }
   if (p->nr > 0) {
     const float2* q = reinterpret_cast<const float2*>(p->rep_payload);
     DFK_CUDA(h, launch_reprojection_error(p->C, reinterpret_cast<const ReprojItemDev*>(p->rep.ptr), p->nr, q,
-                                          q + p->rep_total, avg, out + 2 * (size_t)p->ne, h->stream),
+                                          q + p->rep_total, avg, out + 2 * (size_t)ne, h->stream),
              what);
     h->launches += 1;
   }
   if (p->ng > 0) {
     DFK_CUDA(h, launch_sparse_geometric_error(p->C, reinterpret_cast<const GeoItemDev*>(p->geo.ptr), p->ng,
                                               reinterpret_cast<const int2*>(p->geo_payload), avg,
-                                              out + 2 * (size_t)(p->ne + p->nr), h->stream),
+                                              out + 2 * (size_t)(ne + p->nr), h->stream),
              what);
     h->launches += 1;
   }
   DFK_TRY(problem_deltas(h, p, state));
   DFK_CUDA(h, launch_window_energy(energy_args(p, state, w), h->stream), what);
   h->launches += 1;
+  return DFK_OK;
+}
+
+// the active subsets of a validated mask (em: one byte per error item): the selected templates, their slots and the
+// subset's tile plan, uploaded on the stream behind every launch still reading the previous ones.  The subset arrays
+// are allocated once at full size, so no later mask reallocates an array a queued launch reads
+DfkStatus problem_set_active(DfkHandle h, DfkWindowProblem* p, const uint8_t* dm, const uint8_t* em)
+{
+  const char* amsg = "[WindowProblem::set_active] allocation failed";
+  const char* umsg = "[WindowProblem::set_active] upload failed";
+  const int nd = p->nd, ne = p->ne;
+  const bool all_d = std::all_of(dm, dm + nd, [](uint8_t v) { return v != 0; });
+  const bool all_e = std::all_of(em, em + ne, [](uint8_t v) { return v != 0; });
+  if (!all_d || !all_e) {
+    DFK_CUDA(h, p->sub_slots.ensure((size_t)std::max(nd + ne, 1)), amsg);
+    if (!all_d) {
+      DFK_CUDA(h, p->dense_sub.ensure((size_t)std::max(nd, 1)), amsg);
+      DFK_CUDA(h, p->rec_src.ensure((size_t)nd), amsg);
+      DFK_CUDA(h, p->sub_records.ensure((size_t)nd * DFK_SFM_RECORD_FLOATS(p->C)), amsg);
+    }
+    if (!all_e) {
+      DFK_CUDA(h, p->err_sub.ensure((size_t)std::max(ne, 1)), amsg);
+      DFK_CUDA(h, p->areas_sub.ensure((size_t)std::max(ne, 1)), amsg);
+    }
+  }
+  if (!all_d) {
+    std::vector<SfmItemDev> items;
+    std::vector<int4> sl;
+    std::vector<int> src(nd, -1);
+    for (int i = 0; i < nd; ++i)
+      if (dm[i]) {
+        src[i] = (int)items.size();
+        items.push_back(p->dense_tmpl[i]);
+        sl.push_back(p->slots_tmpl[i]);
+      }
+    plan_tiles(items.data(), (int)items.size(), p->step.max_ctas, &p->sub_plan);
+    if (!items.empty()) {
+      DFK_CUDA(h, cudaMemcpyAsync(p->dense_sub.ptr, items.data(), sizeof(SfmItemDev) * items.size(),
+                                  cudaMemcpyHostToDevice, h->stream),
+               umsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->sub_slots.ptr, sl.data(), sizeof(int4) * sl.size(), cudaMemcpyHostToDevice,
+                                  h->stream),
+               umsg);
+    }
+    DFK_CUDA(h, cudaMemcpyAsync(p->rec_src.ptr, src.data(), sizeof(int) * nd, cudaMemcpyHostToDevice, h->stream), umsg);
+    p->nda = (int)items.size();
+  }
+  if (!all_e) {
+    std::vector<EvalErrorDesc> items;
+    std::vector<int4> sl;
+    std::vector<double> areas;
+    for (int i = 0; i < ne; ++i)
+      if (em[i]) {
+        items.push_back(p->err_tmpl[i]);
+        sl.push_back(p->slots_tmpl[nd + i]);
+        areas.push_back(p->areas_tmpl[i]);
+      }
+    if (!items.empty()) {
+      DFK_CUDA(h, cudaMemcpyAsync(p->err_sub.ptr, items.data(), sizeof(EvalErrorDesc) * items.size(),
+                                  cudaMemcpyHostToDevice, h->stream),
+               umsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->sub_slots.ptr + nd, sl.data(), sizeof(int4) * sl.size(), cudaMemcpyHostToDevice,
+                                  h->stream),
+               umsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->areas_sub.ptr, areas.data(), sizeof(double) * areas.size(),
+                                  cudaMemcpyHostToDevice, h->stream),
+               umsg);
+    }
+    p->nea = (int)items.size();
+  }
+  p->sub_dense = !all_d;
+  p->sub_err = !all_e;
+  return DFK_OK;
+}
+
+// dfk_window_lm's device half (the Ops of dfk_lm.h / dfk_levels.h): the state, buffers and solve of a problem
+struct ProblemLMOps {
+  DfkHandle h;
+  DfkWindowProblem* p;
+  const DfkLMParams* prm;
+  WindowSolverDev* solver;
+  size_t nf, f_off;
+  double w;
+  int cand() const { return 1 - p->cur; }
+  float* buf(bool c) const { return p->bufs.ptr + (size_t)(c ? 1 - p->acc : p->acc) * nf; }
+  DfkStatus linearize(bool c) { return problem_linearize(h, p, p->st(c ? cand() : p->cur), buf(c)); }
+  DfkStatus energy(bool c, double* f)
+  {
+    const double* s = p->st(c ? cand() : p->cur);
+    if (prm->use_error) {
+      DFK_TRY(problem_error(h, p, s, w));
+    } else {
+      WindowEnergyDev a = energy_args(p, s, w);
+      a.buf_f = buf(c) + f_off;
+      a.num_frame_priors = a.num_kf_priors = 0;
+      DFK_CUDA(h, launch_window_energy(a, h->stream), "[WindowLM] kernel launch failed");
+      h->launches += 1;
+    }
+    DFK_TRY(download(h, p->small_host.ptr, p->energy(), 8 * sizeof(double), "[WindowLM] read-back failed",
+                     "[WindowLM] kernel failed"));
+    *f = reinterpret_cast<const double*>(p->small_host.ptr)[7];
+    return DFK_OK;
+  }
+  DfkStatus solve(double lam, int* info)
+  {
+    DFK_CUDA(h, launch_window_solve(solver, buf(false), lam, w, p->st(p->cur) + (size_t)(p->K + p->F) * 7, p->dx.ptr,
+                                    p->info(), h->stream, &h->launches, true),
+             "[WindowLM] solve launch failed");
+    DFK_TRY(download(h, p->small_host.ptr, p->info(), sizeof(int32_t), "[WindowLM] read-back failed",
+                     "[WindowLM] solve failed"));
+    *info = *reinterpret_cast<const int32_t*>(p->small_host.ptr);
+    return DFK_OK;
+  }
+  DfkStatus retract()
+  {
+    DFK_CUDA(h, launch_window_retract(p->st(p->cur), p->st(cand()), p->dx.ptr, p->K, p->F, p->C, h->stream),
+             "[WindowLM] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  }
+  void accept()
+  {
+    p->cur = cand();
+    p->acc = 1 - p->acc;
+  }
+};
+
+// dfk_window_lm's checks of the parameters and trace, and the solver, buffers and Ops of a run
+DfkStatus lm_setup(DfkHandle h, DfkWindowProblem* p, const DfkLMParams* prm, DfkLMTrace* tr, const char* name,
+                   ProblemLMOps* ops)
+{
+  const std::string what = std::string("[") + name + "] ";
+  if (!p || !prm || !tr || !tr->energy || (prm->iterations > 0 && (!tr->lambda || !tr->accepted)))
+    return fail(h, DFK_ERR_INVALID_ARG, what + "null argument");
+  if (p->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, what + "problem and handle live on different devices");
+  if (prm->iterations < 0 || !(std::isfinite(prm->lambda_init) && prm->lambda_init >= 0.0) ||
+      !(std::isfinite(prm->code_prior_weight) && prm->code_prior_weight >= 0.0))
+    return fail(h, DFK_ERR_INVALID_ARG, what + "iterations < 0, or lambda_init / code_prior_weight not finite and >= 0");
+  if (!(std::isfinite(prm->lambda_up) && prm->lambda_up > 0.0) ||
+      !(std::isfinite(prm->lambda_down) && prm->lambda_down > 0.0) || std::isnan(prm->lambda_max))
+    return fail(h, DFK_ERR_INVALID_ARG, what + "lambda_up / lambda_down must be finite and > 0, lambda_max a number");
+  const int fix = prm->fix_first_pose ? 1 : 0;
+  const std::string amsg = what + "allocation failed";
+  if (!p->solver[fix])
+    DFK_CUDA(h, window_solver_create(p->K, p->C, p->F, p->w->pair_k0, p->w->pair_k1, p->w->link_k0, p->w->link_k1,
+                                     p->w->blk_i, p->w->blk_j, p->w->kp.block_off, std::vector<int>(), &p->solver[0]),
+             amsg.c_str());
+  const size_t nf = p->w->floats, f_off = (size_t)p->K * p->B * (p->B + 1) + (size_t)p->w->dev.num_pairs * 6 * p->B;
+  DFK_CUDA(h, p->bufs.ensure(2 * nf), amsg.c_str());
+  DFK_CUDA(h, p->dx.ensure((size_t)p->K * p->B + 6 * (size_t)p->F), amsg.c_str());
+  *ops = ProblemLMOps{h, p, prm, p->solver[fix], nf, f_off, prm->code_prior_weight};
   return DFK_OK;
 }
 
@@ -2529,6 +2727,7 @@ DfkStatus dfk_window_problem_create(DfkHandle h, const DfkWindowProblemDesc* d, 
         }
         it.ray_tab = p->rays[r].ptr;
       }
+      p->dense_tmpl = items;
       DFK_CUDA(h, p->dense.ensure(nd), amsg);
       DFK_CUDA(h, cudaMemcpyAsync(p->dense.ptr, items.data(), sizeof(SfmItemDev) * nd, cudaMemcpyHostToDevice, h->stream),
                "[WindowProblem] upload failed");
@@ -2620,6 +2819,8 @@ DfkStatus dfk_window_problem_create(DfkHandle h, const DfkWindowProblemDesc* d, 
                "[WindowProblem] upload failed");
       DFK_CUDA(h, cudaMemcpyAsync(p->areas.ptr, areas.data(), sizeof(double) * ne, cudaMemcpyHostToDevice, h->stream),
                "[WindowProblem] upload failed");
+      p->err_tmpl = descs;
+      p->areas_tmpl = areas;
     }
     DFK_CUDA(h, p->err_out.ensure(std::max<size_t>(1, 2 * (size_t)(ne + nr + ng))), amsg);
     // ---- slots, in the repose kernel's order
@@ -2629,6 +2830,7 @@ DfkStatus dfk_window_problem_create(DfkHandle h, const DfkWindowProblemDesc* d, 
     };
     push(d->dense_slots, nd); push(d->error_slots, ne); push(d->reproj_slots, nr); push(d->geo_slots, ng);
     push(d->depth_slots, ndep);
+    p->slots_tmpl.assign(slots.begin(), slots.begin() + nd + ne);
     if (!slots.empty()) {
       DFK_CUDA(h, p->slots.ensure(slots.size()), amsg);
       DFK_CUDA(h, cudaMemcpyAsync(p->slots.ptr, slots.data(), sizeof(int4) * slots.size(), cudaMemcpyHostToDevice,
@@ -2775,77 +2977,88 @@ DfkStatus dfk_window_problem_retract(DfkHandle h, DfkWindowProblem* p, const dou
 DfkStatus dfk_window_lm(DfkHandle h, DfkWindowProblem* p, const DfkLMParams* prm, DfkLMTrace* tr)
 {
   return guarded(h, [&] {
-    if (!p || !prm || !tr || !tr->energy || (prm->iterations > 0 && (!tr->lambda || !tr->accepted)))
-      return fail(h, DFK_ERR_INVALID_ARG, "[WindowLM] null argument");
-    if (p->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[WindowLM] problem and handle live on different devices");
-    if (prm->iterations < 0 || !(std::isfinite(prm->lambda_init) && prm->lambda_init >= 0.0) ||
-        !(std::isfinite(prm->code_prior_weight) && prm->code_prior_weight >= 0.0))
-      return fail(h, DFK_ERR_INVALID_ARG, "[WindowLM] iterations < 0, or lambda_init / code_prior_weight not finite and >= 0");
-    if (!(std::isfinite(prm->lambda_up) && prm->lambda_up > 0.0) ||
-        !(std::isfinite(prm->lambda_down) && prm->lambda_down > 0.0) || std::isnan(prm->lambda_max))
-      return fail(h, DFK_ERR_INVALID_ARG, "[WindowLM] lambda_up / lambda_down must be finite and > 0, lambda_max a number");
     DeviceGuard guard(h->device);
-    const int fix = prm->fix_first_pose ? 1 : 0;
-    const char* amsg = "[WindowLM] allocation failed";
-    if (!p->solver[fix])
-      DFK_CUDA(h, window_solver_create(p->K, p->C, p->F, p->w->pair_k0, p->w->pair_k1, p->w->link_k0, p->w->link_k1,
-                                       p->w->blk_i, p->w->blk_j, p->w->kp.block_off, std::vector<int>(), &p->solver[0]),
-               amsg);
-    const size_t nf = p->w->floats, f_off = (size_t)p->K * p->B * (p->B + 1) + (size_t)p->w->dev.num_pairs * 6 * p->B;
-    DFK_CUDA(h, p->bufs.ensure(2 * nf), amsg);
-    DFK_CUDA(h, p->dx.ensure((size_t)p->K * p->B + 6 * (size_t)p->F), amsg);
-    const double w = prm->code_prior_weight;
-    struct Ops {
-      DfkHandle h;
-      DfkWindowProblem* p;
-      const DfkLMParams* prm;
-      WindowSolverDev* solver;
-      size_t nf, f_off;
-      double w;
-      int cand() const { return 1 - p->cur; }
-      float* buf(bool c) const { return p->bufs.ptr + (size_t)(c ? 1 - p->acc : p->acc) * nf; }
-      DfkStatus linearize(bool c) { return problem_linearize(h, p, p->st(c ? cand() : p->cur), buf(c)); }
-      DfkStatus energy(bool c, double* f)
-      {
-        const double* s = p->st(c ? cand() : p->cur);
-        if (prm->use_error) {
-          DFK_TRY(problem_error(h, p, s, w));
-        } else {
-          WindowEnergyDev a = energy_args(p, s, w);
-          a.buf_f = buf(c) + f_off;
-          a.num_frame_priors = a.num_kf_priors = 0;
-          DFK_CUDA(h, launch_window_energy(a, h->stream), "[WindowLM] kernel launch failed");
-          h->launches += 1;
-        }
-        DFK_TRY(download(h, p->small_host.ptr, p->energy(), 8 * sizeof(double), "[WindowLM] read-back failed",
-                         "[WindowLM] kernel failed"));
-        *f = reinterpret_cast<const double*>(p->small_host.ptr)[7];
-        return DFK_OK;
-      }
-      DfkStatus solve(double lam, int* info)
-      {
-        DFK_CUDA(h, launch_window_solve(solver, buf(false), lam, w, p->st(p->cur) + (size_t)(p->K + p->F) * 7, p->dx.ptr,
-                                        p->info(), h->stream, &h->launches, true),
-                 "[WindowLM] solve launch failed");
-        DFK_TRY(download(h, p->small_host.ptr, p->info(), sizeof(int32_t), "[WindowLM] read-back failed",
-                         "[WindowLM] solve failed"));
-        *info = *reinterpret_cast<const int32_t*>(p->small_host.ptr);
-        return DFK_OK;
-      }
-      DfkStatus retract()
-      {
-        DFK_CUDA(h, launch_window_retract(p->st(p->cur), p->st(cand()), p->dx.ptr, p->K, p->F, p->C, h->stream),
-                 "[WindowLM] kernel launch failed");
-        h->launches += 1;
-        return DFK_OK;
-      }
-      void accept()
-      {
-        p->cur = cand();
-        p->acc = 1 - p->acc;
-      }
-    } ops{h, p, prm, p->solver[fix], nf, f_off, w};
+    ProblemLMOps ops;
+    DFK_TRY(lm_setup(h, p, prm, tr, "WindowLM", &ops));
     return lm_run(*prm, ops, tr);
+  });
+}
+
+DfkStatus dfk_window_problem_set_active(DfkHandle h, DfkWindowProblem* p, const uint8_t* dense_active,
+                                        const uint8_t* error_active)
+{
+  return guarded(h, [&] {
+    const char* what = "[WindowProblem::set_active] ";
+    if (!p || (p->nd > 0 && !dense_active) || (!error_active && p->ne != p->nd))
+      return fail(h, DFK_ERR_INVALID_ARG, std::string(what) +
+                                              "null argument (error_active may be NULL only when num_error == num_dense)");
+    if (p->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] problem and handle live on different devices");
+    DeviceGuard guard(h->device);
+    return problem_set_active(h, p, dense_active, error_active ? error_active : dense_active);
+  });
+}
+
+DfkStatus dfk_window_lm_levels(DfkHandle h, DfkWindowProblem* p, const DfkLMParams* prm, const DfkLevelSchedule* sc,
+                               DfkLMTrace* tr, DfkLevelTrace* lt)
+{
+  return guarded(h, [&] {
+    const std::string what = "[WindowLMLevels] ";
+    if (!p || !sc) return fail(h, DFK_ERR_INVALID_ARG, what + "null argument");
+    const int nd = p->nd, ne = p->ne, L = sc->num_levels;
+    if (L < 1 || !sc->iters || (nd > 0 && !sc->dense_level) || sc->num_pairs < 0 ||
+        (sc->num_pairs > 0 && !sc->pair_steps_done))
+      return fail(h, DFK_ERR_INVALID_ARG, what + "num_levels < 1, or null iters / dense_level / pair_steps_done");
+    if (ne > 0 && ne != nd && (!sc->error_pair || !sc->error_level))
+      return fail(h, DFK_ERR_INVALID_ARG, what + "error_pair and error_level are required when num_error != num_dense");
+    for (int l = 0; l < L; ++l)
+      if (sc->iters[l] < 0) return fail(h, DFK_ERR_INVALID_ARG, what + "iters[" + std::to_string(l) + "] < 0");
+    // the schedule's pairs: the distinct window pairs of the dense items, in window order
+    std::vector<int> dpair(nd), ids;
+    for (int i = 0; i < nd; ++i) ids.push_back(p->w->item_pair[i]);
+    std::sort(ids.begin(), ids.end());
+    ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
+    if ((int)ids.size() != sc->num_pairs)
+      return fail(h, DFK_ERR_INVALID_ARG, what + "num_pairs " + std::to_string(sc->num_pairs) + ", but the dense items" +
+                                              " cover " + std::to_string(ids.size()) + " pairs");
+    for (int i = 0; i < nd; ++i)
+      dpair[i] = (int)(std::lower_bound(ids.begin(), ids.end(), p->w->item_pair[i]) - ids.begin());
+    for (int i = 0; i < nd; ++i)
+      if (sc->dense_level[i] < 0 || sc->dense_level[i] >= L)
+        return fail(h, DFK_ERR_INVALID_ARG, what + "dense item " + std::to_string(i) + ": level outside [0, num_levels)");
+    std::vector<int> epair(ne), elevel(ne);
+    for (int i = 0; i < ne; ++i) {
+      epair[i] = sc->error_pair ? sc->error_pair[i] : dpair[i];
+      elevel[i] = sc->error_level ? sc->error_level[i] : sc->dense_level[i];
+      if (epair[i] < 0 || epair[i] >= sc->num_pairs || elevel[i] < 0 || elevel[i] >= L)
+        return fail(h, DFK_ERR_INVALID_ARG, what + "error item " + std::to_string(i) +
+                                                ": pair or level out of range");
+    }
+    for (int q = 0; q < sc->num_pairs; ++q)
+      if (sc->pair_steps_done[q] < 0)
+        return fail(h, DFK_ERR_INVALID_ARG, what + "pair_steps_done[" + std::to_string(q) + "] < 0");
+    DeviceGuard guard(h->device);
+    struct LevelOps : ProblemLMOps {
+      const DfkLevelSchedule* sc;
+      const std::vector<int>* dpair;
+      const std::vector<int>* epair;
+      const std::vector<int>* elevel;
+      std::vector<uint8_t> dm, em;
+      DfkStatus set_levels(const int* lvl)
+      {
+        for (size_t i = 0; i < dm.size(); ++i) dm[i] = lvl[(*dpair)[i]] == sc->dense_level[i];
+        for (size_t i = 0; i < em.size(); ++i) em[i] = lvl[(*epair)[i]] == (*elevel)[i];
+        return problem_set_active(h, p, dm.data(), em.data());
+      }
+    } ops;
+    DFK_TRY(lm_setup(h, p, prm, tr, "WindowLMLevels", &ops));
+    ops.sc = sc;
+    ops.dpair = &dpair;
+    ops.epair = &epair;
+    ops.elevel = &elevel;
+    ops.dm.assign(nd, 1);
+    ops.em.assign(ne, 1);
+    return lm_levels_run(*prm, *sc, ops, tr, lt);
   });
 }
 

@@ -413,6 +413,9 @@ struct WindowEnergyDev {
   double* out;  // [E | photometric | reprojection | geometric | priors | items without inliers | inliers | E + code prior]
 };
 cudaError_t launch_window_energy(const WindowEnergyDev& a, cudaStream_t stream);
+// records slot i (i < n, rf floats each) <- sub record src[i], or zeros where src[i] < 0 (an inactive item)
+cudaError_t launch_window_scatter_records(const float* sub, const int* src, int n, int rf, float* records,
+                                          cudaStream_t stream);
 
 constexpr int kSimpleMaxBlocks = 1024;
 constexpr int kSimpleScratchFloats = kSimpleMaxBlocks * 32;

@@ -10,6 +10,8 @@
 //   deltas    Local(x0, x) = [t - t0 | log(R R0^T) | c - c0] of every frame prior and every keyframe-prior member
 //   energy    one CTA: the window energy from the error outputs (each part summed sequentially in factor order, as
 //             window_error_sum does) or from the buffer's f, plus the prior terms and the code prior
+//   scatter   with an active subset (dfk_window_problem_set_active): the subset's records into their slots, zeros
+//             into the inactive items' slots
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -243,7 +245,30 @@ __global__ void __launch_bounds__(kEnergyThreads) window_energy_kernel(WindowEne
   o[7] = __dadd_rn(E, cp);
 }
 
+// one CTA per record slot i: the active subset's record src[i], or an all-zero record for an inactive item (src[i] < 0)
+__global__ void __launch_bounds__(256) window_scatter_records_kernel(const float* __restrict__ sub,
+                                                                     const int* __restrict__ src, int rf,
+                                                                     float* __restrict__ records)
+{
+  const int s = src[blockIdx.x];
+  float* o = records + (size_t)blockIdx.x * rf;
+  if (s < 0) {
+    for (int k = threadIdx.x; k < rf; k += blockDim.x) o[k] = 0.0f;
+    return;
+  }
+  const float* in = sub + (size_t)s * rf;
+  for (int k = threadIdx.x; k < rf; k += blockDim.x) o[k] = in[k];
+}
+
 }  // namespace
+
+cudaError_t launch_window_scatter_records(const float* sub, const int* src, int n, int rf, float* records,
+                                          cudaStream_t stream)
+{
+  if (n == 0) return cudaSuccess;
+  window_scatter_records_kernel<<<n, 256, 0, stream>>>(sub, src, rf, records);
+  return cudaGetLastError();
+}
 
 cudaError_t launch_window_repose(const WindowReposeDev& a, cudaStream_t stream)
 {

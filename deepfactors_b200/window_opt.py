@@ -69,6 +69,95 @@ class LMTrace:
     frame_poses: Optional[np.ndarray] = None  # run(..., frame_poses): the frames' poses at the returned point
     linearisations: int = 0       # calls of `linearise`
     error_evaluations: int = 0    # calls of `error` (WindowOptimizer(error=...) only)
+    # run(..., schedule=...) only: the energy every level switch re-linearised to, the level of every pair at every
+    # step (-1: inactive) and every pair's position at the end (LevelSchedule.steps_done of a continuing schedule)
+    switch_energy: List[float] = field(default_factory=list)
+    pair_levels: List[List[int]] = field(default_factory=list)
+    pair_steps_done: List[int] = field(default_factory=list)
+
+
+def level_at(iters: Sequence[int], s: int, remove_after: bool = False) -> int:
+    """The active level of a pair after s steps of its schedule (-1: inactive): level len(iters) - 1 for its first
+    iters[-1] + 1 steps, then each finer level l for iters[l] + 1 steps; afterwards level 0, or -1 with remove_after"""
+    for l in range(len(iters) - 1, -1, -1):
+        if s < iters[l] + 1:
+            return l
+        s -= iters[l] + 1
+    return -1 if remove_after else 0
+
+
+def level_start(iters: Sequence[int], l: int) -> int:
+    """the position of the first step at level l"""
+    return sum(int(iters[m]) + 1 for m in range(l + 1, len(iters)))
+
+
+@dataclass
+class LevelSchedule:
+    """The coarse-to-fine schedule of WindowOptimizer.run(schedule=...) and dfk_window_lm_levels (the reference's
+    OptimizePhoto works, df_work.cpp:100-225, with pho_iters = iters).  The schedule's pairs are the window pairs of the
+    dense items (photometric, then frame pairs, in window order); item_pair / item_level give every dense item's pair
+    and pyramid level.  Error items are the dense items' twins unless error_pair / error_level say otherwise.  steps_done
+    is each pair's position (0 for a new pair; trace.pair_steps_done continues a schedule), remove_after marks the pairs
+    that leave once their schedule has run out (mapper.cpp:306-311: the backward direction of a new connection)."""
+    iters: Sequence[int]
+    item_level: Sequence[int]
+    item_pair: Sequence[int]
+    steps_done: Sequence[int]
+    remove_after: Sequence[bool]
+    error_pair: Optional[Sequence[int]] = None
+    error_level: Optional[Sequence[int]] = None
+
+    def levels(self, pos: Sequence[int]) -> List[int]:
+        return [level_at(self.iters, int(s), bool(r)) for s, r in zip(pos, self.remove_after)]
+
+    def masks(self, lvl: Sequence[int]):
+        """(dense mask, error mask or None) of the pair levels lvl"""
+        dm = np.asarray([lvl[q] == l for q, l in zip(self.item_pair, self.item_level)], dtype=bool)
+        if self.error_pair is None and self.error_level is None:
+            return dm, None
+        ep = self.item_pair if self.error_pair is None else self.error_pair
+        el = self.item_level if self.error_level is None else self.error_level
+        return dm, np.asarray([lvl[q] == l for q, l in zip(ep, el)], dtype=bool)
+
+
+class OptimizeWork:
+    """A transliteration of the reference's OptimizeWork for one pair (df_work.cpp:100-190): the readable statement of
+    the per-pair rule level_at / WindowOptimizer.run(schedule=...) implement.  Per mapping step the mapper calls
+    bookkeeping (the factor the pair holds: constructed at a level start, removed after remove_after), then update
+    (the counter), and signal_no_relinearize when ISAM2 relinearised nothing (mapper.cpp:440-538)."""
+
+    def __init__(self, iters: Sequence[int], remove_after: bool = False):
+        self.iters, self.orig = list(iters), list(iters)
+        self.active_level = len(iters) - 1
+        self.first, self.remove, self.remove_after = True, False, remove_after
+        self.factor: Optional[int] = None  # the level of the PhotometricFactor in the graph
+
+    def is_new_level_start(self) -> bool:
+        return self.active_level >= 0 and self.iters[self.active_level] == self.orig[self.active_level]
+
+    def bookkeeping(self) -> Optional[int]:
+        if self.remove:
+            self.factor = None
+            self.active_level = -2
+        if self.first or (self.active_level >= 0 and self.is_new_level_start()):
+            self.first = False
+            self.factor = self.active_level
+        return self.factor
+
+    def update(self):
+        if self.active_level >= 0:
+            self.iters[self.active_level] -= 1
+            if self.iters[self.active_level] < 0:
+                self.active_level -= 1
+        if self.remove_after and self.active_level < 0:
+            self.remove = True
+
+    def signal_no_relinearize(self):
+        if not self.first:
+            self.active_level -= 1
+
+    def finished(self) -> bool:
+        return self.active_level == (-2 if self.remove_after else -1)
 
 
 @dataclass
@@ -95,12 +184,17 @@ def prior_energy(row, delta) -> float:
     return f0 - 2.0 * float(g @ d) + float(d @ G @ d)
 
 
-def window_error_sum(dense, areas, reprojection, geometric, prior_terms) -> WindowError:
+def window_error_sum(dense, areas, reprojection, geometric, prior_terms, active=None) -> WindowError:
     """The host half of SfmWindowProblem.error.  dense: [n, 2] float32 rows [residual | inliers as uint32 bits] of the
     photometric and frame items (dfk_sfm_evaluate_error_batch) with their W * H in `areas`; reprojection / geometric:
     [m, 2] rows [b^T b | valid (uint32 bits)] of the links; prior_terms: each prior's energy (prior_energy).  An item
-    without inliers adds 0, as in the window assembly (PhotometricFactor::error would return inf for it)."""
+    without inliers adds 0, as in the window assembly (PhotometricFactor::error would return inf for it).  active
+    (optional, n bools): the inactive rows are skipped, counted neither as items without inliers nor in the inliers."""
     dense = np.ascontiguousarray(dense, dtype=np.float32).reshape(-1, 2)
+    areas = list(areas)
+    if active is not None:
+        keep = np.asarray(active, dtype=bool)
+        dense, areas = dense[keep], [a for a, k in zip(areas, keep) if k]
     res, inl = dense[:, 0].astype(np.float64), dense[:, 1].view(np.uint32).astype(np.int64)
     out = WindowError()
     for r, n, a in zip(res, inl, areas):
@@ -251,16 +345,32 @@ class WindowOptimizer:
     `error(poses, codes[, frame_poses]) -> (E, breakdown)` (optional; SfmWindowProblem.error) is the energy at a point
     without linearising it, in the units of the buffer's f.  With it the loop evaluates E at every candidate and
     linearises only the points it accepts (the start point and every accepted step), so a rejected step costs one error
-    evaluation and leaves the record buffer and the cache at the accepted point.  f is then E plus the host prior term."""
+    evaluation and leaves the record buffer and the cache at the accepted point.  f is then E plus the host prior term.
+    The masks of SfmWindowProblem.set_active hold for every run until the next set_active call, also for a run
+    without a schedule.
+
+    run(..., schedule=LevelSchedule) optimises coarse to fine: the policy of dfk_levels.h, with `set_active(dense_mask,
+    error_mask)` (SfmWindowProblem.set_active) making the levels of the pairs the active items.  Every step moves every
+    active pair one position along its schedule (level_at); when lambda would exceed lambda_max every pair above level 0
+    jumps to its next finer level and lambda restarts (the run ends only when no pair is above level 0); whenever a
+    level changes, the accepted point is re-linearised under the new masks and its energy becomes f."""
 
     def __init__(self, layout: WindowBlocks, linearise: Callable, params: Optional[LMParams] = None,
-                 solve: Optional[Callable] = None, error: Optional[Callable] = None):
+                 solve: Optional[Callable] = None, error: Optional[Callable] = None,
+                 set_active: Optional[Callable] = None):
         self.layout = layout
         self.linearise = linearise
         self.params = params or LMParams()
         self.solve = solve or functools.partial(dense_solve, layout)
         self.error = error
+        self.set_active = set_active
         self.cache = LinearisationCache(layout.pairs, self.params.cache_eps, layout.geometric)
+
+    def _set_levels(self, schedule: "LevelSchedule", lvl):
+        """the masks of the pair levels lvl (set_active(dense_mask, error_mask)); the records of the items that were
+        off are zero, so the cache starts over"""
+        self.set_active(*schedule.masks(lvl))
+        self.cache.invalidate()
 
     def _code_prior(self, codes) -> float:
         w = self.params.code_prior_weight
@@ -290,7 +400,8 @@ class WindowOptimizer:
         trace.linearisations += 1
         return buf
 
-    def run(self, poses, codes, frame_poses=None) -> Tuple[np.ndarray, np.ndarray, LMTrace]:
+    def run(self, poses, codes, frame_poses=None, schedule: Optional[LevelSchedule] = None
+            ) -> Tuple[np.ndarray, np.ndarray, LMTrace]:
         prm = self.params
         poses = np.asarray(poses, dtype=np.float64).copy()
         codes = np.asarray(codes, dtype=np.float64).copy()
@@ -300,10 +411,18 @@ class WindowOptimizer:
         trace = LMTrace()
         fixed = list(range(6)) if prm.fix_first_pose else []
         lam = prm.lambda_init
+        if schedule is not None:
+            if self.set_active is None:
+                raise ValueError("run(schedule=...) needs WindowOptimizer(..., set_active=...), e.g. prob.set_active")
+            pos = [int(v) for v in schedule.steps_done]
+            lvl = schedule.levels(pos)
+            self._set_levels(schedule, lvl)
         buf = self._evaluate(poses, codes, trace, frames)
         f = self._energy(buf, codes) if self.error is None else self._error(poses, codes, trace, frames)
         trace.energy.append(f)
-        for _ in range(prm.iterations):
+        for it in range(prm.iterations):
+            if schedule is not None:
+                trace.pair_levels.append(list(lvl))
             dx = self.solve(buf, lam, fixed, prm.code_prior_weight, codes)
             trace.lam.append(lam)
             ok = False
@@ -331,8 +450,28 @@ class WindowOptimizer:
                 # buf and f of the accepted point are still at hand; without `error` the record buffer (and with it the
                 # cache) now describes the rejected candidate, which the next candidate is compared against
                 lam = lam * prm.lambda_up
-                if lam > prm.lambda_max:
+                if lam > prm.lambda_max and schedule is None:
                     break
+            if schedule is None:
+                continue
+            pos = [p + 1 if l >= 0 else p for p, l in zip(pos, lvl)]
+            if not ok and lam > prm.lambda_max:  # stall: every pair above level 0 moves one level finer
+                now = schedule.levels(pos)
+                if not any(l > 0 for l in now):
+                    break
+                pos = [level_start(schedule.iters, l - 1) if l > 0 else p for p, l in zip(pos, now)]
+                lam = prm.lambda_init
+            if it + 1 == prm.iterations:
+                break
+            nxt = schedule.levels(pos)
+            if nxt != lvl:
+                lvl = nxt
+                self._set_levels(schedule, lvl)
+                buf = self._evaluate(poses, codes, trace, frames)
+                f = self._energy(buf, codes) if self.error is None else self._error(poses, codes, trace, frames)
+                trace.switch_energy.append(f)
+        if schedule is not None:
+            trace.pair_steps_done = pos
         trace.frame_poses = frames
         return poses, codes, trace
 
@@ -344,12 +483,16 @@ class DeviceWindowOptimizer:
     params.use_error), except that every linearisation re-evaluates every factor: an LM step moves every code, so the
     linearisation cache would re-evaluate everything anyway.  run returns what WindowOptimizer.run returns.  A run
     rewrites prob.records (see SfmWindowProblem.device_problem): invalidate the cache of a WindowOptimizer over the same
-    problem before its next run."""
+    problem before its next run.  With a schedule (LevelSchedule, e.g. prob.level_schedule(...)) run is
+    dfk_window_lm_levels, WindowOptimizer.run(schedule=...)'s policy; the device problem keeps the masks of the last
+    step."""
 
-    def __init__(self, prob: "SfmWindowProblem", params: Optional[LMParams] = None, use_error: bool = False):
+    def __init__(self, prob: "SfmWindowProblem", params: Optional[LMParams] = None, use_error: bool = False,
+                 schedule: Optional[LevelSchedule] = None):
         self.prob = prob
         self.params = params or LMParams()
         self.use_error = bool(use_error)
+        self.schedule = schedule
         self.dev = prob.device_problem()
 
     def run(self, poses, codes, frame_poses=None) -> Tuple[np.ndarray, np.ndarray, LMTrace]:
@@ -360,12 +503,19 @@ class DeviceWindowOptimizer:
             raise ValueError(f"the window has {F} tracked frames: pass as many frame_poses")
         self.dev.set_state(np.concatenate([np.asarray(poses, np.float64).reshape(-1, 7), frames]),
                            np.asarray(codes, np.float64))
-        t = self.dev.lm(self.params, self.use_error)
+        if self.schedule is None:
+            # a scheduled run leaves its last masks on the device problem: an unscheduled run uses every item
+            self.dev.set_active(np.ones(self.dev.num_dense, bool), np.ones(self.dev.num_error, bool))
+            t = self.dev.lm(self.params, self.use_error)
+        else:
+            t = self.dev.lm_levels(self.params, self.schedule, self.use_error)
         p, c = self.dev.get_state()
         n = len(self.prob.pairs) + len(self.prob.geometric)
         trace = LMTrace(energy=t["energy"], lam=t["lam"], accepted=t["accepted"],
                         factors_relinearised=[n] * t["linearisations"], frame_poses=p[K:] if F else None,
-                        linearisations=t["linearisations"], error_evaluations=t["error_evaluations"])
+                        linearisations=t["linearisations"], error_evaluations=t["error_evaluations"],
+                        switch_energy=t.get("switch_energy", []), pair_levels=t.get("pair_levels", []),
+                        pair_steps_done=t.get("pair_steps_done", []))
         return p[:K], c, trace
 
 
@@ -612,12 +762,43 @@ class SfmWindowProblem:
             "geometric": _FactorKind(geo_ends, len(self.pairs), self.geo_records, 0, 1, _geometric_items,
                                      SparseGeometricLinearizeBatch)}
         self.allreduce = allreduce
+        self._active = None  # set_active: the dense items' mask (None: every item active)
         self._solvers = {}  # fixed variables -> WindowSolver, created on first use
         self._prior_rows = torch.as_tensor(np.stack([np.asarray(pr.row, dtype=np.float64) for pr in self._mpriors]),
                                            device=dev) if self._mpriors else None
         self._kprior_rows = torch.as_tensor(np.concatenate([np.asarray(pr.row, dtype=np.float64).ravel()
                                                             for pr in self._kpriors]),
                                             device=dev) if self._kpriors else None
+
+    def set_active(self, mask, error_mask=None):
+        """Make only the dense items of `mask` (bools, record order: the photometric then the frame (pair, level)
+        items) active: linearise evaluates the active items only and writes all-zero records for the others, error
+        skips the inactive rows, and marginalize / marginalize_keyframe see the active factors.  The error items are
+        the dense items' twins, so error_mask, when given, must equal mask.  All true (or None) restores every item."""
+        m = None if mask is None else np.asarray(mask, dtype=bool).ravel()
+        nd = self._kinds["frame"].row0 + len(self._kinds["frame"].ends) * self.levels
+        if m is not None and m.size != nd:
+            raise ValueError(f"a mask of {nd} dense items expected")
+        if error_mask is not None and not np.array_equal(np.asarray(error_mask, dtype=bool).ravel(), m):
+            raise ValueError("the error items are the dense items' twins: their mask is the dense mask")
+        self._active = None if m is None or m.all() else m
+
+    def level_schedule(self, iters, steps_done=None, remove_after=None) -> LevelSchedule:
+        """The LevelSchedule of this window's photometric and frame pairs with pho_iters = iters: item (pair, l) has
+        level l; steps_done / remove_after per pair (photometric pairs, then frame pairs), default 0 / False."""
+        P, F = self._num_photometric, len(self.frames)
+        n = P + F
+        return LevelSchedule(iters=[int(v) for v in iters], item_level=[l for _ in range(n) for l in range(self.levels)],
+                             item_pair=[q for q in range(n) for _ in range(self.levels)],
+                             steps_done=[0] * n if steps_done is None else [int(v) for v in steps_done],
+                             remove_after=[False] * n if remove_after is None else [bool(v) for v in remove_after])
+
+    def _zero_inactive(self, records):
+        """the all-zero records of the inactive dense items"""
+        if self._active is not None:
+            import torch
+            off = torch.as_tensor(np.flatnonzero(~self._active), device=records.device)
+            records.index_fill_(0, off, 0.0)
 
     def solve(self, buf, lam, fixed, code_prior_weight=0.0, codes=None):
         """WindowOptimizer's `solve` on the device: dfk_window_solve of the window buffer, then one read-back of dx and
@@ -709,7 +890,7 @@ class SfmWindowProblem:
                 n = len(pr.keyframes) * self.layout.B
                 terms.append(prior_energy(pr.row, d[at:at + n]))
                 at += n
-        ew = window_error_sum(host[:nd], st["areas"], host[nd:nd + nr], host[nd + nr:], terms)
+        ew = window_error_sum(host[:nd], st["areas"], host[nd:nd + nr], host[nd + nr:], terms, self._active)
         return ew.energy, ew
 
     def _error_state(self):
@@ -891,6 +1072,7 @@ class SfmWindowProblem:
             rows = torch.as_tensor([kd.row0 + f * kd.rows + r for f in which for r in range(kd.rows)],
                                    device=records.device)
             records.index_copy_(0, rows, kd.batch(self.al, self._items("frame", poses, codes, which, frame_poses)))
+            self._zero_inactive(records)
         priors, info = self.window.marginalize_frames(records, which)
         rows, info = priors.cpu().numpy(), info.cpu().numpy()
         if np.any(info != 0):
@@ -910,12 +1092,20 @@ class SfmWindowProblem:
             sel = [p - kd.first for p in todo if kd.first <= p < kd.first + len(kd.ends)]
             if not sel:
                 continue
+            its = self._items(kind, poses, codes, sel, frame_poses)
+            rws = [kd.row0 + j * kd.rows + r for j in sel for r in range(kd.rows)]
+            if self._active is not None and kd.batch is _run_step_batch:  # the active (pair, level) items only
+                keep = [i for i, r in enumerate(rws) if self._active[r]]
+                its, rws = [its[i] for i in keep], [rws[i] for i in keep]
+                if not rws:
+                    continue
             target = swap.get(id(kd.base))
             base, items, rows = launches.setdefault(kd.batch, (kd.base if target is None else target, [], []))
-            items += self._items(kind, poses, codes, sel, frame_poses)
-            rows += [kd.row0 + j * kd.rows + r for j in sel for r in range(kd.rows)]
+            items += its
+            rows += rws
         for batch, (base, items, rows) in launches.items():
             if rows == list(range(rows[0], rows[0] + len(rows))):  # contiguous rows: straight into the records
                 batch(self.al, items, base[rows[0]:rows[0] + len(rows)])
             else:  # one batch of their own, copied to their rows
                 base.index_copy_(0, torch.as_tensor(rows, device=base.device), batch(self.al, items))
+        self._zero_inactive(self.records if records is None else records)

@@ -559,12 +559,25 @@ struct LMTrace {  // window_opt.LMTrace
   int linearisations = 0, error_evaluations = 0;
 };
 
+// window_opt.LevelSchedule in the C ABI's terms (DfkLevelSchedule): pairs are the distinct window pairs of the dense
+// items; error_pair / error_level empty: error item i follows dense item i; pair_remove_after empty: no pair leaves
+struct LevelSchedule {
+  std::vector<int32_t> iters, dense_level, error_pair, error_level, pair_steps_done;
+  std::vector<uint8_t> pair_remove_after;
+};
+
+struct LevelTrace {  // DfkLevelTrace
+  std::vector<double> switch_energy;
+  std::vector<std::vector<int32_t>> pair_levels;  // [step][pair], -1: off
+  std::vector<int32_t> pair_steps_done;
+};
+
 template <int CS>
 class WindowProblem
 {
 public:
   WindowProblem(DfkHandle h, const DfkWindowProblemDesc& desc, int num_keyframes, int num_frames)
-    : h_(h), K_(num_keyframes), F_(num_frames)
+    : h_(h), K_(num_keyframes), F_(num_frames), nd_(desc.num_dense), ne_(desc.num_error)
   {
     if (!h || num_keyframes < 1 || num_frames < 0)
       throw std::invalid_argument("[WindowProblem] null handle / no keyframes / negative frame count");
@@ -632,9 +645,55 @@ public:
     return r;
   }
 
+  // the active dense and error items (dfk_window_problem_set_active); error_active empty: the dense mask, which needs
+  // as many error as dense items.  The masks hold for Linearize, Error, Optimize and OptimizeLevels until the next call
+  void SetActive(const std::vector<uint8_t>& dense_active, const std::vector<uint8_t>& error_active = {})
+  {
+    if (dense_active.size() != (size_t)nd_ || (!error_active.empty() && error_active.size() != (size_t)ne_))
+      throw std::invalid_argument("[WindowProblem::SetActive] one byte per dense item and per error item");
+    detail::Check(h_, dfk_window_problem_set_active(h_, p_, dense_active.data(),
+                                                    error_active.empty() ? nullptr : error_active.data()));
+  }
+  // Levenberg-Marquardt coarse to fine (dfk_window_lm_levels); the problem keeps the masks of the last step
+  LMTrace OptimizeLevels(const LMParams& p, const LevelSchedule& s, LevelTrace* lt = nullptr)
+  {
+    if (p.iterations < 0) throw std::invalid_argument("[WindowProblem::OptimizeLevels] iterations < 0");
+    const size_t P = s.pair_steps_done.size();
+    if (s.iters.empty() || s.dense_level.size() != (size_t)nd_ ||
+        (!s.error_pair.empty() && s.error_pair.size() != (size_t)ne_) ||
+        (!s.error_level.empty() && s.error_level.size() != (size_t)ne_) ||
+        (!s.pair_remove_after.empty() && s.pair_remove_after.size() != P))
+      throw std::invalid_argument("[WindowProblem::OptimizeLevels] schedule arrays of the wrong length");
+    const DfkLMParams c{p.iterations, p.lambda_init, p.lambda_up, p.lambda_down, p.lambda_max, p.fix_first_pose ? 1 : 0,
+                        p.code_prior_weight, p.use_error ? 1 : 0};
+    const DfkLevelSchedule cs{(int32_t)s.iters.size(), s.iters.data(), s.dense_level.data(),
+                              s.error_pair.empty() ? nullptr : s.error_pair.data(),
+                              s.error_level.empty() ? nullptr : s.error_level.data(), (int32_t)P,
+                              s.pair_steps_done.data(), s.pair_remove_after.empty() ? nullptr : s.pair_remove_after.data()};
+    const int it = std::max(p.iterations, 1);
+    std::vector<double> e(p.iterations + 1), lam(it), sw(it);
+    std::vector<int32_t> acc(it), lv((size_t)it * std::max<size_t>(P, 1)), done(std::max<size_t>(P, 1));
+    DfkLMTrace t{e.data(), lam.data(), acc.data(), 0, 0, 0, 0};
+    DfkLevelTrace l{sw.data(), lv.data(), done.data(), 0};
+    detail::Check(h_, dfk_window_lm_levels(h_, p_, &c, &cs, &t, &l));
+    LMTrace r;
+    r.energy.assign(e.begin(), e.begin() + t.num_energies);
+    r.lambda.assign(lam.begin(), lam.begin() + t.num_steps);
+    for (int i = 0; i < t.num_steps; ++i) r.accepted.push_back(acc[i] != 0);
+    r.linearisations = t.linearisations;
+    r.error_evaluations = t.error_evaluations;
+    if (lt) {
+      lt->switch_energy.assign(sw.begin(), sw.begin() + l.num_switches);
+      lt->pair_levels.clear();
+      for (int i = 0; i < t.num_steps; ++i) lt->pair_levels.emplace_back(lv.begin() + i * P, lv.begin() + (i + 1) * P);
+      lt->pair_steps_done.assign(done.begin(), done.begin() + P);
+    }
+    return r;
+  }
+
 private:
   DfkHandle h_;
-  int K_, F_;
+  int K_, F_, nd_, ne_;
   DfkWindowProblem* p_ = nullptr;
 };
 

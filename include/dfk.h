@@ -644,7 +644,8 @@ DfkStatus dfk_squared_error(DfkHandle h, const DfkImage* a, const DfkImage* b, f
  * which linearize writes and which must outlive the problem).  The image views are the caller's and must outlive it.
  * Create validates every item as the batch calls do, plans the RunStep launch and takes the handle's settings: its Gram
  * mode, SM limit and every DenseSfmParams value (valid_border, min_dpt, avg_dpt, huber_delta) at create hold for every
- * later call of the problem, for all its factor kinds; later dfk_sfm_set_params / dfk_sfm_set_gram_mode /
+ * later call of the problem, for all its factor kinds (the RunStep kernel chosen at create also serves every active
+ * subset of dfk_window_problem_set_active); later dfk_sfm_set_params / dfk_sfm_set_gram_mode /
  * dfk_set_sm_limit calls do not change it.  An error item must not ask for a fused decode (code NULL).  Create uploads the item arrays, which the problem owns with their code
  * slots and ray tables (no pointer into the handle's shared scratch), creates the solver with the first pose fixed and
  * allocates the depth scratch of the error path.  A rejected create writes nothing. */
@@ -722,6 +723,54 @@ typedef struct {
  * linearisation cache would re-evaluate everything anyway).  The state and the accepted and candidate window buffers
  * stay on the device; each step reads back the solve's info and the candidate's energy.  Synchronous. */
 DfkStatus dfk_window_lm(DfkHandle h, DfkWindowProblem* p, const DfkLMParams* params, DfkLMTrace* trace);
+
+/* Active items (coarse to fine: one pyramid level per pair at a time, as the reference's OptimizePhoto holds one
+ * PhotometricFactor per pair).  dense_active: num_dense bytes, error_active: num_error bytes, both HOST memory and
+ * copied; error_active may be NULL only when num_error == num_dense, and then the dense mask is used.  Nonzero = active.
+ * After create every item is active.  With a mask:
+ *   linearize  the RunStep launch (depth decode fused in) covers the active dense items only, planned over them, so an
+ *              inactive item costs no tile; an inactive item's record is all zero (it adds nothing to f or the inliers)
+ *              and its dpt0 / valid0 are not written.  The links, the assembly and the priors are unchanged.  An
+ *              active item's record is bit for bit dfk_sfm_run_step_batch over the active items in record order.
+ *   error      only the active error items are evaluated; an inactive one adds 0 and is counted neither as an item
+ *              without inliers nor in the inlier total.
+ * The masks hold for every later linearize, error, dfk_window_lm and dfk_window_lm_levels call of the problem until the
+ * next set_active (dfk_window_lm_levels leaves those of its last step); all ones restores the create-time launches.
+ * The re-plan is host work ordered on the handle's stream (no synchronisation).  A rejected call writes nothing. */
+DfkStatus dfk_window_problem_set_active(DfkHandle h, DfkWindowProblem* p, const uint8_t* dense_active,
+                                        const uint8_t* error_active);
+
+/* The level schedule of dfk_window_lm_levels (window_opt.LevelSchedule), HOST arrays.  The schedule's pairs are the
+ * distinct window pairs of the dense items (the photometric, then the frame pairs), in window order; dense item i
+ * belongs to the window's item_pair[i].  Error items: with error_pair NULL (allowed when num_error == num_dense) error
+ * item i belongs to dense item i's pair; with error_level NULL (same condition) it has dense item i's level. */
+typedef struct {
+  int32_t num_levels;
+  const int32_t* iters;             /* [num_levels] >= 0: level l is active for iters[l] + 1 steps (pho_iters) */
+  const int32_t* dense_level;       /* [num_dense] in [0, num_levels) */
+  const int32_t* error_pair;        /* [num_error] schedule pair index, or NULL */
+  const int32_t* error_level;       /* [num_error] in [0, num_levels), or NULL */
+  int32_t num_pairs;                /* must equal the number of distinct pairs of the dense items */
+  const int32_t* pair_steps_done;   /* [num_pairs] >= 0: steps the pair has taken (0 for a new pair) */
+  const uint8_t* pair_remove_after; /* [num_pairs] nonzero: inactive once its schedule has run out; may be NULL */
+} DfkLevelSchedule;
+/* What dfk_window_lm_levels returns besides DfkLMTrace; the caller's HOST arrays, any may be NULL */
+typedef struct {
+  double* switch_energy;         /* [iterations]: the energy each switch re-linearised to */
+  int32_t* pair_levels;          /* [iterations x num_pairs]: the active level of every pair at every step, -1 = off */
+  int32_t* pair_steps_done;      /* [num_pairs] out: every pair's position, to continue its schedule in a later window */
+  int32_t num_switches;          /* out */
+} DfkLevelTrace;
+/* Levenberg-Marquardt with per-pair coarse-to-fine levels: the policy of dfk_levels.h (its header comment), with
+ * dfk_window_lm's accept / lambda rule and use_error.  A pair's position s is the number of steps it has taken: level
+ * num_levels - 1 for its first iters[num_levels - 1] + 1 steps, and so on down to level 0; after its schedule it stays
+ * at level 0, or becomes inactive with remove_after.  One LM iteration (accepted or rejected) is one step of every
+ * active pair.  When lambda would exceed lambda_max, every pair above level 0 jumps to the first step of the next finer
+ * level and lambda restarts at lambda_init; the run ends there only when no pair is above level 0.  Whenever the active
+ * set changes, the accepted point is re-linearised under the new mask (counted in trace->linearisations) and its energy
+ * becomes f.  On return the problem's mask is the one the last step used.  Synchronous. */
+DfkStatus dfk_window_lm_levels(DfkHandle h, DfkWindowProblem* p, const DfkLMParams* params,
+                               const DfkLevelSchedule* schedule, DfkLMTrace* trace, DfkLevelTrace* level_trace);
 
 #ifdef __cplusplus
 }

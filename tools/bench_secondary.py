@@ -39,8 +39,11 @@ One JSON line per case:
   * the LM loop in the library (`--only lm`): window200 at C = 32 and 128, a 10-iteration LM by DeviceWindowOptimizer
     (dfk_window_lm) against WindowOptimizer(solve=prob.solve) and WindowOptimizer(..., error=prob.error), alternated --
     wall clock to a synchronise and summed device time (torch.profiler, separate run).
+  * coarse to fine (`--only levels`): window200's 50 keyframes and 200 pairs at C = 32 and 128 with a 3-level pyramid
+    (640x480), a pho_iters = 4,8,15 schedule (dfk_window_lm_levels, 30 steps) against 30 all-level dfk_window_lm steps:
+    wall and device time, and from perturbations of increasing size the final pose error and the level-0 energy.
 Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` /
-`--only frames` / `--only slide` / `--only error` / `--only lm` runs those cases alone.
+`--only frames` / `--only slide` / `--only error` / `--only lm` / `--only levels` runs those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -59,7 +62,8 @@ sys.path.insert(0, ROOT)
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
-    ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error", "lm"], default=None)
+    ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error", "lm", "levels"],
+                    default=None)
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -95,6 +99,8 @@ def main():
         return error_cases(args, torch, print)
     if args.only == "lm":
         return lm_cases(args, torch, print)
+    if args.only == "levels":
+        return levels_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -782,6 +788,82 @@ def lm_cases(args, torch, print):
                               "error_evaluations": tr.error_evaluations, "accepted": tr.accepted,
                               "energy_first_last": [tr.energy[0], tr.energy[-1]], "timing": timing}), flush=True)
         del runs, keyframes, shared, jac
+        torch.cuda.empty_cache()
+
+
+def levels_cases(args, torch, print):
+    """Coarse to fine against all levels at once.  Every keyframe of the synthetic window holds the same pyramid, so the
+    identity poses are the scene's known solution; the starts perturb keyframes 1.. by increasing amounts.  pho_iters =
+    4,8,15 has three levels, so the window has three (640x480, 320x240, 160x120); the all-level loop takes as many LM
+    steps as the schedule has (30).  Reported per loop: wall time of one run to a synchronise (median of the alternated
+    repetitions), summed device time (torch.profiler, separate run), the final pose error against the identity (mean
+    translation norm and rotation angle over the keyframes) and the level-0 energy at the final point (the error of the
+    level-0 items alone, dfk_window_problem_error under a level-0 mask)."""
+    import numpy as np
+    from deepfactors_b200 import se3, synth
+    from deepfactors_b200.aligners import SfmAligner
+    from deepfactors_b200.window_opt import DeviceWindowOptimizer, LMParams, SfmWindowProblem
+    sys.path.insert(0, ROOT)
+    from bench import window_pairs
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
+    levels, num_kf, iters = 3, 50, (4, 8, 15)
+    steps = sum(i + 1 for i in iters)
+    reps = max(3, args.reps // 5)
+    timing = ("wall clock of one run() to a synchronise, median over the alternated repetitions; device time = summed "
+              "kernel + copy time of one run(), torch.profiler (separate run)")
+    for cs in (32, 128):
+        base = synth.make_pair(640, 480, cs, levels, seed=7)
+        shared = [dict(img=up(L.img0), grad=up(L.grad1), prx_orig=up(L.prx_orig)) for L in base.levels]
+        jac = [up(L.prx_jac) for L in base.levels]
+        gen = torch.Generator(device="cuda").manual_seed(cs)
+        keyframes = [[dict(sh, prx_jac=j + 1e-3 * torch.randn(j.shape, device="cuda", generator=gen),
+                           dpt=torch.zeros_like(sh["img"]), valid=torch.zeros_like(sh["img"]))
+                      for sh, j in zip(shared, jac)] for _ in range(num_kf)]
+        pairs = window_pairs(num_kf, 200)
+        cams = [L.cam for L in base.levels]
+        al = SfmAligner(cs)
+        prm = LMParams(iterations=steps, lambda_init=1e-4)
+        probs = {name: SfmWindowProblem(al, cams, keyframes, pairs) for name in ("levels", "all")}
+        sched = probs["levels"].level_schedule(iters)
+        opts = {"levels": DeviceWindowOptimizer(probs["levels"], prm, schedule=sched),
+                "all": DeviceWindowOptimizer(probs["all"], prm)}
+        level0 = np.asarray(sched.item_level) == 0
+        codes = np.zeros((num_kf, cs))
+        for scale in (0.003, 0.01, 0.03):
+            rng = np.random.default_rng(int(scale * 1e4))
+            poses = np.stack([se3.identity(np.float64)] + [
+                se3.make_pose(rng.standard_normal(3) * scale, rng.standard_normal(3) * scale * 3, np.float64)
+                for _ in range(num_kf - 1)])
+            runs = {n: (lambda o=o: o.run(poses, codes)) for n, o in opts.items()}
+            out = {n: fn() for n, fn in runs.items()}  # warm-up, and the result
+            torch.cuda.synchronize()
+            walls = {n: [] for n in runs}
+            for _ in range(reps):
+                for n, fn in runs.items():
+                    t0 = time.perf_counter()
+                    fn()
+                    torch.cuda.synchronize()
+                    walls[n].append((time.perf_counter() - t0) * 1e6)
+            for n, fn in runs.items():
+                p, c, tr = out[n]
+                dp = opts[n].dev
+                dp.set_state(p, c)
+                dp.set_active(level0)
+                e0 = float(dp.error().cpu()[0])
+                dp.set_active(np.ones(dp.num_dense, bool))
+                terr = float(np.mean(np.linalg.norm(p[:, 4:], axis=1)))
+                rerr = float(np.mean(2.0 * np.arccos(np.clip(np.abs(p[:, 3]), 0.0, 1.0))))
+                print(json.dumps({"case": f"window200 C={cs} ({num_kf} keyframes, {len(pairs)} pairs, {levels} levels "
+                                          f"640x480), start perturbed by {scale} rad / {3 * scale} m (std): "
+                                          + ("pho_iters 4,8,15 (dfk_window_lm_levels)" if n == "levels" else
+                                             f"{steps} all-level steps (dfk_window_lm)"),
+                                  "us_total": float(np.median(walls[n])), "us_runs": walls[n],
+                                  "device_us_total": _device_us(torch, fn, 1), "steps": len(tr.accepted),
+                                  "accepted": sum(tr.accepted), "switches": len(tr.switch_energy),
+                                  "linearisations": tr.linearisations, "level0_energy": e0,
+                                  "mean_translation_error_m": terr, "mean_rotation_error_rad": rerr,
+                                  "timing": timing}), flush=True)
+        del opts, probs, keyframes, shared, jac
         torch.cuda.empty_cache()
 
 
