@@ -134,6 +134,20 @@ class DfkLevelTrace(C.Structure):
                 ("pair_steps_done", C.POINTER(C.c_int32)), ("num_switches", C.c_int32)]
 
 
+class DfkFeatureSet(C.Structure):
+    _fields_ = [("keypoints", C.c_void_p), ("descriptors", C.c_void_p), ("num", C.c_int32),
+                ("descriptor_bytes", C.c_int32)]
+
+
+class DfkMatchItem(C.Structure):
+    _fields_ = [("query", DfkFeatureSet), ("train", DfkFeatureSet), ("cam", DfkCamera), ("max_dist", C.c_float),
+                ("max_iterations", C.c_int32), ("threshold", C.c_double), ("probability", C.c_double),
+                ("seed", C.c_uint64)]
+
+
+MATCH_MAX_QUERIES = 8192  # DFK_MATCH_MAX_QUERIES
+MATCH_MAX_ITERATIONS = 1000000  # DFK_MATCH_MAX_ITERATIONS
+
 WINDOW_ERROR_DOUBLES = 7  # DFK_WINDOW_ERROR_DOUBLES
 
 
@@ -223,6 +237,9 @@ SYMBOLS = {
     "dfk_reprojection_error_batch": (C.c_int, [_H, C.POINTER(DfkReprojectionItem), C.c_int, C.c_int, C.c_void_p]),
     "dfk_sparse_geometric_error_batch": (C.c_int, [_H, C.POINTER(DfkSparseGeometricItem), C.c_int, C.c_int,
                                                    C.c_void_p]),
+    "dfk_hamming_match_batch": (C.c_int, [_H, C.POINTER(DfkMatchItem), C.c_int, C.c_void_p]),
+    "dfk_reprojection_match_batch": (C.c_int, [_H, C.POINTER(DfkMatchItem), C.c_int, C.c_void_p, C.c_void_p,
+                                               C.c_void_p]),
     "dfk_update_depth": (C.c_int, [_H, _F, C.c_int, _IMG, _IMG, C.c_float, _IMG]),
     "dfk_update_depth_batch": (C.c_int, [_H, C.POINTER(DfkDepthDecodeItem), C.c_int, C.c_int]),
     "dfk_sobel_gradients": (C.c_int, [_H, _IMG, _IMG]),

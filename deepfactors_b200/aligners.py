@@ -456,6 +456,101 @@ def ReprojectionErrorBatch(aligner, items, out: torch.Tensor | None = None) -> t
     return out
 
 
+# ------------------------------------------------------------------------------------------- keypoint matching
+# the reference's rep_* options (deepfactors_options.h:93-101) and PruneMatchesEightPoint's probability (matching.h:48-50);
+# the threshold is the float option widened to double, as the reference passes it
+REP_MAX_DIST = 30.0
+REP_RANSAC_MAXITERS = 1000
+REP_RANSAC_THRESHOLD = float(np.float32(1e-4))
+REP_RANSAC_PROBABILITY = 0.99
+
+
+@dataclass
+class Features:
+    """A keyframe's keypoints and binary descriptors on the device (kf->features of the reference): keypoints [N, 2]
+    float32 (keypoints[i].pt at level 0), descriptors [N, D] uint8 with D = 32 (ORB) or 64 (BRISK)."""
+    keypoints: torch.Tensor
+    descriptors: torch.Tensor
+
+    @staticmethod
+    def from_host(keypoints, descriptors, device="cuda") -> "Features":
+        kp = np.ascontiguousarray(np.asarray(keypoints, np.float32).reshape(-1, 2))
+        d = np.ascontiguousarray(np.asarray(descriptors, np.uint8))
+        if d.ndim != 2 or d.shape[0] != kp.shape[0]:
+            raise ValueError("descriptors must be [N, D] with one row per keypoint")
+        return Features(torch.from_numpy(kp).to(device), torch.from_numpy(d).to(device))
+
+
+def _feature_set(hd: _Handle, f: Features) -> _lib.DfkFeatureSet:
+    kp, d = f.keypoints, f.descriptors
+    n = int(kp.shape[0]) if kp.dim() == 2 else -1
+    if kp.dim() != 2 or kp.shape[1] != 2 or d.dim() != 2 or d.shape[0] != n:
+        raise ValueError("features: keypoints must be [N, 2] and descriptors [N, D]")
+    _check_tensor(hd, kp, torch.float32, 2 * n, "keypoints")
+    _check_tensor(hd, d, torch.uint8, n * int(d.shape[1]), "descriptors")
+    return _lib.DfkFeatureSet(kp.data_ptr() if n else None, d.data_ptr() if n else None, n, int(d.shape[1]))
+
+
+def _match_item(hd: _Handle, it: dict) -> _lib.DfkMatchItem:
+    w = _lib.DfkMatchItem()
+    w.query, w.train = _feature_set(hd, it["query"]), _feature_set(hd, it["train"])
+    if it.get("cam") is not None:
+        w.cam = _cam(it["cam"])
+    w.max_dist = float(it.get("max_dist", REP_MAX_DIST))
+    w.max_iterations = int(it.get("max_iterations", REP_RANSAC_MAXITERS))
+    w.threshold = float(it.get("threshold", REP_RANSAC_THRESHOLD))
+    w.probability = float(it.get("probability", REP_RANSAC_PROBABILITY))
+    w.seed = int(it.get("seed", 0))
+    return w
+
+
+def match_offsets(items: Sequence[dict]) -> np.ndarray:
+    """[n + 1]: item i's rows of the match outputs are [offsets[i], offsets[i + 1]) (the prefix sum of the query counts)"""
+    return np.concatenate([[0], np.cumsum([int(it["query"].keypoints.shape[0]) for it in items])]).astype(np.int64)
+
+
+def HammingMatchBatch(aligner, items: Sequence[dict], out: torch.Tensor | None = None) -> torch.Tensor:
+    """cv::BFMatcher(NORM_HAMMING).match(query, train) of many factors in one launch (dfk_hamming_match_batch): items are
+    dicts with query / train (Features).  Asynchronous: returns a device tensor [sum of query counts, 2] int32, item i's
+    rows at match_offsets(items)[i], row q = (train index, Hamming distance), ties to the lowest train index, (-1, -1)
+    when the train set is empty."""
+    hd = aligner._hd
+    hd.use_torch_stream()
+    n = len(items)
+    arr = (_lib.DfkMatchItem * max(n, 1))(*[_match_item(hd, it) for it in items])
+    total = int(match_offsets(items)[-1])
+    if out is None:
+        out = torch.empty((max(total, 1), 2), dtype=torch.int32, device=f"cuda:{hd.device}")
+    _check_tensor(hd, out, torch.int32, 2 * total, "out")
+    check(hd.h, lib().dfk_hamming_match_batch(hd.h, arr, n, C.c_void_p(out.data_ptr())))
+    return out[:total]
+
+
+def ReprojectionMatchBatch(aligner, items: Sequence[dict]):
+    """The match lists of many ReprojectionFactors in four launches (dfk_reprojection_match_batch): Hamming matching,
+    eight-point RANSAC and distance pruning (reprojection_factor.cpp:56-65).  items are dicts with query / train
+    (Features), cam (level 0) and optionally max_dist, max_iterations, threshold, probability (the rep_* defaults above)
+    and seed (0).  Asynchronous: returns device tensors (matches [sum of query counts, 3] int32, counts [n] int32,
+    ransac [n, 3] int32): item i's list is matches[offsets[i] : offsets[i] + counts[i]] (offsets = match_offsets(items)),
+    rows (query index, train index, distance) sorted by (distance, query); ransac[i] = (selected hypothesis or -1, its
+    inliers, hypotheses evaluated)."""
+    hd = aligner._hd
+    hd.use_torch_stream()
+    n = len(items)
+    for it in items:
+        if it.get("cam") is None:
+            raise ValueError("ReprojectionMatchBatch: every item needs its level-0 camera")
+    arr = (_lib.DfkMatchItem * max(n, 1))(*[_match_item(hd, it) for it in items])
+    total = int(match_offsets(items)[-1])
+    dev = f"cuda:{hd.device}"
+    matches = torch.zeros((max(total, 1), 3), dtype=torch.int32, device=dev)  # rows past an item's count stay 0
+    counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    ransac = torch.empty((max(n, 1), 3), dtype=torch.int32, device=dev)
+    check(hd.h, lib().dfk_reprojection_match_batch(hd.h, arr, n, C.c_void_p(matches.data_ptr()),
+                                                   C.c_void_p(counts.data_ptr()), C.c_void_p(ransac.data_ptr())))
+    return matches[:total], counts[:n], ransac[:n]
+
+
 def SparseGeometricErrorBatch(aligner, items, out: torch.Tensor | None = None) -> torch.Tensor:
     """SparseGeometricFactor::error of many factors in one launch (dfk_sparse_geometric_error_batch): the items of
     SparseGeometricLinearizeBatch (dicts, or the array of make_geometric_items).  Asynchronous: returns a device tensor [n, 2] float32, row i = [b^T b | valid points

@@ -112,6 +112,11 @@ struct DfkContext {
   std::vector<unsigned char> geo_host;
   DeviceBuf<SfmItemDev> items_dev;
   DeviceBuf<float> partials_dev;
+  // dfk_hamming_match_batch / dfk_reprojection_match_batch: the item descriptors (one H2D per call) and the RANSAC
+  // scratch [matches (int2 per query) | hypothesis counts | selections (int3 per item)] (bytes)
+  DeviceBuf<MatchItemDev> match_items;
+  std::vector<MatchItemDev> match_host;
+  DeviceBuf<unsigned char> match_scratch;
   // dfk_window_marginalize_frames / dfk_window_add_priors: the call's index lists (one pageable H2D per call)
   DeviceBuf<int> window_lists;
   // dfk_window_marginalize_keyframe: the call's lists [refs | tile rows / cols | member locations | update tasks] (one
@@ -2525,6 +2530,128 @@ DfkStatus dfk_reprojection_linearize_batch(DfkHandle h, const DfkReprojectionIte
                                             h->stream),
              "[ReprojectionFactor::linearize batch] kernel launch failed");
     h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+namespace {
+
+// Validates and stages the items of a matching batch; max_n0 / total / hyp_total / max_iterations describe the batch.
+// ransac: the camera and RANSAC parameters are checked too.
+DfkStatus stage_match(DfkHandle h, const char* what, const DfkMatchItem* items, int n, bool ransac, int* max_n0,
+                      int* max_iterations, size_t* hyp_total)
+{
+  const std::string w(what);
+  if (!items || n < 1 || n > 65535)  // blockIdx.y of the kernels is the item
+    return fail(h, DFK_ERR_INVALID_ARG, w + "null argument / number of items not in [1, 65535]");
+  h->match_host.resize((size_t)n);
+  long long total = 0;
+  *max_n0 = 0;
+  *max_iterations = 0;
+  *hyp_total = 0;
+  for (int i = 0; i < n; ++i) {
+    const DfkMatchItem& it = items[i];
+    const std::string at = " in item " + std::to_string(i);
+    const DfkFeatureSet* sets[2] = {&it.query, &it.train};
+    for (const DfkFeatureSet* f : sets) {
+      if (f->descriptor_bytes != 32 && f->descriptor_bytes != 64)
+        return fail(h, DFK_ERR_UNSUPPORTED, w + "descriptor size " + std::to_string(f->descriptor_bytes) +
+                                                " (only 32, ORB, and 64, BRISK)" + at);
+      if (f->num < 0 || (f->num > 0 && (!f->keypoints || !f->descriptors)))
+        return fail(h, DFK_ERR_INVALID_ARG, w + "negative feature count or null feature arrays" + at);
+      if (((uintptr_t)f->descriptors & 15) != 0 || ((uintptr_t)f->keypoints & 3) != 0)
+        return fail(h, DFK_ERR_INVALID_ARG, w + "descriptors must be 16-byte aligned, keypoints 4-byte aligned" + at);
+    }
+    if (it.query.descriptor_bytes != it.train.descriptor_bytes)
+      return fail(h, DFK_ERR_INVALID_ARG, w + "query and train descriptors differ in size" + at);
+    if (it.query.num > DFK_MATCH_MAX_QUERIES)
+      return fail(h, DFK_ERR_INVALID_ARG, w + "more than DFK_MATCH_MAX_QUERIES query features" + at);
+    if (ransac) {
+      if (!(std::isfinite(it.cam.fx) && std::isfinite(it.cam.fy) && std::isfinite(it.cam.u0) &&
+            std::isfinite(it.cam.v0) && it.cam.fx != 0.0f && it.cam.fy != 0.0f))
+        return fail(h, DFK_ERR_INVALID_ARG, w + "camera needs finite intrinsics and fx, fy != 0" + at);
+      if (it.max_iterations < 1 || it.max_iterations > DFK_MATCH_MAX_ITERATIONS)
+        return fail(h, DFK_ERR_INVALID_ARG, w + "max_iterations not in [1, DFK_MATCH_MAX_ITERATIONS]" + at);
+      if (!(it.threshold > 0.0 && std::isfinite(it.threshold)) || !(it.probability > 0.0 && it.probability < 1.0) ||
+          !(it.max_dist >= 0.0f))
+        return fail(h, DFK_ERR_INVALID_ARG, w + "threshold must be finite and > 0, probability in (0, 1), max_dist >= 0" +
+                                                at);
+    }
+    MatchItemDev& d = h->match_host[(size_t)i];
+    d = MatchItemDev{};
+    d.kp0 = it.query.keypoints;
+    d.kp1 = it.train.keypoints;
+    d.d0 = it.query.descriptors;
+    d.d1 = it.train.descriptors;
+    d.n0 = it.query.num;
+    d.n1 = it.train.num;
+    d.words = it.query.descriptor_bytes / 4;
+    d.out_begin = (int)total;
+    total += it.query.num;
+    if (ransac) {
+      d.max_iterations = it.max_iterations;
+      d.hyp_begin = (int)*hyp_total;
+      *hyp_total += (size_t)(it.max_iterations + kMatchHyp - 1) / kMatchHyp * kMatchHyp;
+      d.fx = it.cam.fx; d.fy = it.cam.fy; d.u0 = it.cam.u0; d.v0 = it.cam.v0;
+      d.threshold = it.threshold;
+      d.probability = it.probability;
+      d.max_dist = it.max_dist;
+      d.seed = it.seed;
+      *max_iterations = std::max(*max_iterations, it.max_iterations);
+    }
+    *max_n0 = std::max(*max_n0, it.query.num);
+  }
+  if (total > INT32_MAX || *hyp_total > (size_t)INT32_MAX)
+    return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 queries or hypotheses in one call");
+  DFK_CUDA(h, h->match_items.ensure((size_t)n), (w + "scratch allocation failed").c_str());
+  DFK_CUDA(h, cudaMemcpyAsync(h->match_items.ptr, h->match_host.data(), sizeof(MatchItemDev) * (size_t)n,
+                              cudaMemcpyHostToDevice, h->stream),
+           (w + "upload failed").c_str());
+  return DFK_OK;
+}
+
+}  // namespace
+
+DfkStatus dfk_hamming_match_batch(DfkHandle h, const DfkMatchItem* items, int n, int32_t* matches_dev)
+{
+  return guarded(h, [&] {
+    const char* what = "[BFMatcher::match batch] ";
+    if (!matches_dev) return fail(h, DFK_ERR_INVALID_ARG, std::string(what) + "null output");
+    DeviceGuard guard(h->device);
+    int max_n0 = 0, max_it = 0;
+    size_t hyp = 0;
+    DFK_TRY(stage_match(h, what, items, n, false, &max_n0, &max_it, &hyp));
+    DFK_CUDA(h, launch_hamming_match(h->match_items.ptr, n, max_n0, reinterpret_cast<int2*>(matches_dev), h->stream),
+             "[BFMatcher::match batch] kernel launch failed");
+    h->launches += max_n0 > 0 ? 1 : 0;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_reprojection_match_batch(DfkHandle h, const DfkMatchItem* items, int n, int32_t* matches_dev,
+                                       int32_t* counts_dev, int32_t* ransac_dev)
+{
+  return guarded(h, [&] {
+    const char* what = "[ReprojectionFactor matches batch] ";
+    if (!matches_dev || !counts_dev) return fail(h, DFK_ERR_INVALID_ARG, std::string(what) + "null output");
+    DeviceGuard guard(h->device);
+    int max_n0 = 0, max_it = 0;
+    size_t hyp = 0;
+    DFK_TRY(stage_match(h, what, items, n, true, &max_n0, &max_it, &hyp));
+    size_t total = 0;
+    for (const MatchItemDev& d : h->match_host) total += (size_t)d.n0;
+    // [matches (int2 per query) | counts (int per hypothesis slot) | selections (int3 per item)], 16-byte aligned parts
+    const size_t b_match = (sizeof(int2) * total + 15) & ~(size_t)15;
+    const size_t b_count = (sizeof(int) * hyp + 15) & ~(size_t)15;
+    const size_t b_sel = sizeof(int3) * (size_t)n;
+    DFK_CUDA(h, h->match_scratch.ensure(b_match + b_count + b_sel + 16), "[ReprojectionFactor matches batch] scratch allocation failed");
+    unsigned char* base = h->match_scratch.ptr;
+    int3* sel = ransac_dev ? reinterpret_cast<int3*>(ransac_dev) : reinterpret_cast<int3*>(base + b_match + b_count);
+    DFK_CUDA(h, launch_reprojection_match(h->match_items.ptr, n, max_n0, max_it, reinterpret_cast<int2*>(base),
+                                          reinterpret_cast<int*>(base + b_match), sel,
+                                          reinterpret_cast<int3*>(matches_dev), counts_dev, h->stream),
+             "[ReprojectionFactor matches batch] kernel launch failed");
+    h->launches += 4;
     return DFK_OK;
   });
 }

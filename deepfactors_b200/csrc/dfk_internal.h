@@ -417,6 +417,31 @@ cudaError_t launch_window_energy(const WindowEnergyDev& a, cudaStream_t stream);
 cudaError_t launch_window_scatter_records(const float* sub, const int* src, int n, int rf, float* records,
                                           cudaStream_t stream);
 
+// one factor of dfk_hamming_match_batch / dfk_reprojection_match_batch (dfk_match.cu)
+struct MatchItemDev {
+  const float* kp0;
+  const float* kp1;       // [n, 2] keypoints
+  const uint8_t* d0;
+  const uint8_t* d1;      // [n, 4 * words] descriptors, 16-byte aligned
+  int n0, n1, words;
+  int out_begin;          // the item's segment of the match outputs: the prefix sum of n0
+  int hyp_begin;          // the item's segment of the per-hypothesis counts
+  int max_iterations;
+  double fx, fy, u0, v0;
+  double threshold, probability;
+  float max_dist;
+  uint64_t seed;
+};
+constexpr int kMatchHyp = 32;            // hypotheses per CTA of the RANSAC kernel
+constexpr int kMatchMaxQueries = 8192;   // query features per item (the compaction sorts them in shared memory)
+// matches_dev[out_begin + q] = (train, distance), (-1, -1) for an empty train set
+cudaError_t launch_hamming_match(const MatchItemDev* items_dev, int n, int max_n0, int2* matches_dev, cudaStream_t s);
+// matching, the hypotheses' inlier counts (counts_dev), the selection (select_dev: best, inliers, evaluated) and the
+// sorted, pruned lists (out_dev rows: query, train, distance; num_out_dev: their lengths)
+cudaError_t launch_reprojection_match(const MatchItemDev* items_dev, int n, int max_n0, int max_iterations,
+                                      int2* matches_dev, int* counts_dev, int3* select_dev, int3* out_dev,
+                                      int* num_out_dev, cudaStream_t s);
+
 constexpr int kSimpleMaxBlocks = 1024;
 constexpr int kSimpleScratchFloats = kSimpleMaxBlocks * 32;
 

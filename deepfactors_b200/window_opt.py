@@ -533,6 +533,51 @@ class ReprojectionLink:
     sigma: float
 
 
+REP_HUBER = 0.1  # rep_huber (deepfactors_options.h:97)
+REP_SIGMA = 1.0  # rep_sigma (deepfactors_options.h:99)
+
+
+def match_reprojection_links(aligner, features, connections, cam, cauchy_delta: float = REP_HUBER,
+                             sigma: float = REP_SIGMA, seed: int = 0, **options) -> List[ReprojectionLink]:
+    """The ReprojectionLinks of keyframe connections with their matches built on the device
+    (aligners.ReprojectionMatchBatch: Hamming matching, eight-point RANSAC, distance pruning).  features[k] is keyframe
+    k's aligners.Features, cam its level-0 camera, connections (k0, k1) pairs; each gives the factor k0 -> k1, then
+    k1 -> k0, as use_reprojection and a loop closure add them (mapper.cpp:314-325, 367-376; pass sigma = loop_sigma for
+    a loop closure).  options override the rep_* RANSAC defaults (max_dist, max_iterations, threshold, probability);
+    factor j of the batch has seed + j.  A factor without matches is dropped, as OptimizeRep::ConstructFactors does
+    (df_work.cpp:336).  The keypoints of every list are gathered on the device and read back once with the counts."""
+    import torch
+
+    from .aligners import ReprojectionMatchBatch, match_offsets
+
+    ends, items = [], []
+    for k0, k1 in connections:
+        for a, b in ((k0, k1), (k1, k0)):
+            items.append(dict(options, query=features[a], train=features[b], cam=cam, seed=seed + len(items)))
+            ends.append((a, b))
+    if not items:
+        return []
+    matches, counts, _ = ReprojectionMatchBatch(aligner, items)
+    off = match_offsets(items)
+    parts = [counts.view(torch.float32)]
+    for j, (a, b) in enumerate(ends):
+        rows = matches[off[j]:off[j + 1]].long()
+        if features[b].keypoints.shape[0] == 0:  # no train features: no matches, nothing to gather
+            rows = rows[:0]
+        parts += [features[a].keypoints[rows[:, 0]].reshape(-1), features[b].keypoints[rows[:, 1]].reshape(-1)]
+    host = torch.cat(parts).cpu().numpy()
+    num = host[:len(items)].view(np.int32)
+    links, pos = [], len(items)
+    for j, (a, b) in enumerate(ends):
+        seg = int(off[j + 1] - off[j]) if features[b].keypoints.shape[0] else 0
+        q = host[pos:pos + 2 * seg].reshape(-1, 2)[:num[j]]
+        t = host[pos + 2 * seg:pos + 4 * seg].reshape(-1, 2)[:num[j]]
+        pos += 4 * seg
+        if num[j] > 0:
+            links.append(ReprojectionLink(a, b, q.copy(), t.copy(), float(cauchy_delta), float(sigma)))
+    return links
+
+
 @dataclass
 class GeometricLink:
     """A sparse geometric factor between keyframes k0 -> k1 (SparseGeometricFactor, sparse_geometric_factor.cpp): the

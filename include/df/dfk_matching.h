@@ -1,0 +1,143 @@
+// dfk_matching.h -- the keypoint matching step of the reference's ReprojectionFactor (reprojection_factor.cpp:56-65)
+// on top of dfk_hamming_match_batch / dfk_reprojection_match_batch (include/dfk.h):
+//   df::Features                  the keypoints and descriptors of a keyframe, on the device (kf->features)
+//   df::DMatch                    cv::DMatch's members (queryIdx, trainIdx, distance)
+//   df::ReprojectionMatcher       owns a handle; MatchBatch / ReprojectionMatchesBatch run many factors in one call
+//     .ReprojectionMatches        the constructor's three steps for one factor (BFMatcher, PruneMatchesEightPoint,
+//                                 PruneMatchesByThreshold), as a std::vector<DMatch>
+//     .PruneMatchesEightPoint     BFMatcher + RANSAC: the inliers in match (query) order, as features/matching.cpp:75-128
+//   df::PruneMatchesByThreshold   features/matching.cpp:29-37 on the host: distance <= max_dist, sorted by (distance,
+//                                 queryIdx), the order the device lists have
+// The host-vector members copy their results back with the CUDA runtime; they exist where its header does.
+#ifndef DFK_MATCHING_H_
+#define DFK_MATCHING_H_
+
+#include <algorithm>
+#include <cstdint>
+#include <limits>
+#include <vector>
+
+#include "dfk_facade.h"
+
+namespace df
+{
+
+struct Features {
+  const float* keypoints = nullptr;      // DEVICE [num, 2], keypoints[i].pt at level 0
+  const uint8_t* descriptors = nullptr;  // DEVICE [num, descriptor_bytes], 16-byte aligned
+  int num = 0;
+  int descriptor_bytes = 32;             // 32 (ORB) or 64 (BRISK)
+  DfkFeatureSet View() const { return DfkFeatureSet{keypoints, descriptors, num, descriptor_bytes}; }
+};
+
+struct DMatch {
+  int queryIdx = -1, trainIdx = -1;
+  float distance = 0.0f;
+};
+
+// ReprojectionFactor's matching arguments: rep_max_dist, rep_ransac_maxiters, rep_ransac_threshold
+// (deepfactors_options.h:96-101) and PruneMatchesEightPoint's probability (matching.h:48-50)
+struct MatchParams {
+  float max_dist = 30.0f;
+  int max_iterations = 1000;
+  double threshold = 0.0001f;
+  double probability = 0.99;
+  uint64_t seed = 0;
+};
+
+// cv::DMatch::operator< orders by distance; ties here go to the lower queryIdx, as on the device
+inline std::vector<DMatch> PruneMatchesByThreshold(std::vector<DMatch> matches, float max_dist)
+{
+  std::sort(matches.begin(), matches.end(), [](const DMatch& a, const DMatch& b) {
+    return a.distance < b.distance || (a.distance == b.distance && a.queryIdx < b.queryIdx);
+  });
+  auto first_wrong = std::find_if(matches.begin(), matches.end(), [&](const DMatch& m) { return m.distance > max_dist; });
+  return std::vector<DMatch>(matches.begin(), first_wrong);
+}
+
+class ReprojectionMatcher
+{
+public:
+  ReprojectionMatcher() : h_(detail::MakeHandle()) {}
+
+  DfkHandle handle() const { return h_.get(); }
+  void SetStream(void* stream) { detail::Check(h_.get(), dfk_set_stream(h_.get(), stream)); }
+
+  template <typename CamT>
+  static DfkMatchItem Item(const Features& kf, const Features& fr, const CamT& cam, const MatchParams& p)
+  {
+    DfkMatchItem it{};
+    it.query = kf.View();
+    it.train = fr.View();
+    it.cam = detail::Cam(cam);
+    it.max_dist = p.max_dist;
+    it.max_iterations = p.max_iterations;
+    it.threshold = p.threshold;
+    it.probability = p.probability;
+    it.seed = p.seed;
+    return it;
+  }
+
+  // dfk_hamming_match_batch: DEVICE output, (train, distance) per query of every item
+  void MatchBatch(const std::vector<DfkMatchItem>& items, int32_t* matches_dev)
+  {
+    detail::Check(h_.get(), dfk_hamming_match_batch(h_.get(), items.data(), (int)items.size(), matches_dev));
+  }
+
+  // dfk_reprojection_match_batch: DEVICE outputs, (query, train, distance) rows, the counts, (best, inliers, evaluated)
+  void ReprojectionMatchesBatch(const std::vector<DfkMatchItem>& items, int32_t* matches_dev, int32_t* counts_dev,
+                                int32_t* ransac_dev = nullptr)
+  {
+    detail::Check(h_.get(), dfk_reprojection_match_batch(h_.get(), items.data(), (int)items.size(), matches_dev,
+                                                         counts_dev, ransac_dev));
+  }
+
+#ifdef DFK_FACADE_CUDART
+  // the three lines of ReprojectionFactor's constructor (reprojection_factor.cpp:56-65), for one factor
+  template <typename CamT>
+  std::vector<DMatch> ReprojectionMatches(const Features& kf, const Features& fr, const CamT& cam,
+                                          const MatchParams& p = MatchParams())
+  {
+    return Run(Item(kf, fr, cam, p));
+  }
+
+  // BFMatcher + PruneMatchesEightPoint (matching.cpp:75-128): the best hypothesis' inliers in match order
+  template <typename CamT>
+  std::vector<DMatch> PruneMatchesEightPoint(const Features& kf, const Features& fr, const CamT& cam,
+                                             const MatchParams& p = MatchParams())
+  {
+    DfkMatchItem it = Item(kf, fr, cam, p);
+    it.max_dist = std::numeric_limits<float>::infinity();
+    std::vector<DMatch> m = Run(it);
+    std::sort(m.begin(), m.end(), [](const DMatch& a, const DMatch& b) { return a.queryIdx < b.queryIdx; });
+    return m;
+  }
+
+private:
+  std::vector<DMatch> Run(const DfkMatchItem& it)
+  {
+    const size_t n0 = (size_t)std::max(it.query.num, 0);
+    int32_t* dev = nullptr;  // [n0 x 3 rows | count]
+    if (cudaMalloc(&dev, sizeof(int32_t) * (3 * n0 + 1)) != cudaSuccess)
+      throw std::runtime_error("[ReprojectionMatcher] device allocation failed");
+    std::unique_ptr<int32_t, void (*)(int32_t*)> guard(dev, [](int32_t* q) { cudaFree(q); });
+    std::vector<DfkMatchItem> items{it};
+    ReprojectionMatchesBatch(items, dev, dev + 3 * n0);
+    std::vector<int32_t> host(3 * n0 + 1);
+    if (cudaMemcpyAsync(host.data(), dev, host.size() * sizeof(int32_t), cudaMemcpyDeviceToHost,
+                        static_cast<cudaStream_t>(dfk_get_stream(h_.get()))) != cudaSuccess ||
+        cudaStreamSynchronize(static_cast<cudaStream_t>(dfk_get_stream(h_.get()))) != cudaSuccess)
+      throw std::runtime_error("[ReprojectionMatcher] result download failed");
+    std::vector<DMatch> out((size_t)host[3 * n0]);
+    for (size_t i = 0; i < out.size(); ++i) out[i] = DMatch{host[3 * i], host[3 * i + 1], (float)host[3 * i + 2]};
+    return out;
+  }
+#endif
+
+private:
+  detail::HandlePtr h_;
+};
+
+}  // namespace df
+
+#endif  // DFK_MATCHING_H_

@@ -581,6 +581,73 @@ DfkStatus dfk_reprojection_error_batch(DfkHandle h, const DfkReprojectionItem* i
 DfkStatus dfk_sparse_geometric_error_batch(DfkHandle h, const DfkSparseGeometricItem* items, int n, int code_size,
                                            float* out_dev);
 
+/* ------------------------------------------------------------------ keypoint matching of a reprojection factor */
+
+/* The features of one keyframe (df::Features, features/feature_detection.h: keypoints and descriptors of
+ * kf->features), on the device, so that every factor of the keyframe reads one upload. */
+typedef struct {
+  const float* keypoints;       /* DEVICE [num, 2]: keypoints[i].pt at level 0 */
+  const uint8_t* descriptors;   /* DEVICE [num, descriptor_bytes], rows back to back, 16-byte aligned */
+  int32_t num;                  /* >= 0 */
+  int32_t descriptor_bytes;     /* 32 (ORB, OrbDetector) or 64 (BRISK, BriskDetector); else DFK_ERR_UNSUPPORTED */
+} DfkFeatureSet;
+
+/* One factor k0 -> k1 of a matching batch: the arguments of ReprojectionFactor's constructor
+ * (reprojection_factor.cpp:56-65).  dfk_hamming_match_batch reads query and train only. */
+typedef struct {
+  DfkFeatureSet query;          /* k0: kf->features (<= DFK_MATCH_MAX_QUERIES features) */
+  DfkFeatureSet train;          /* k1: fr->features, same descriptor_bytes */
+  DfkCamera cam;                /* level 0: K of cam_.Matrix<double>() (:61-62); fx, fy != 0 */
+  float max_dist;               /* rep_max_dist (30) */
+  int32_t max_iterations;       /* rep_ransac_maxiters (1000), in [1, DFK_MATCH_MAX_ITERATIONS] */
+  double threshold;             /* rep_ransac_threshold (1e-4f), > 0 */
+  double probability;           /* 0.99 (matching.h:48-50), in (0, 1) */
+  uint64_t seed;                /* the item's sample generator (dfk_reprojection_match_batch) */
+} DfkMatchItem;
+#define DFK_MATCH_MAX_QUERIES 8192
+#define DFK_MATCH_MAX_ITERATIONS 1000000
+
+/* cv::BFMatcher(cv::NORM_HAMMING).match(kf desc, fr desc) (reprojection_factor.cpp:56-58) for every item: for query q
+ * of item i, matches_dev[o_i + q] = (argmin_j popcount(d0[q] ^ d1[j]), that distance), ties to the lowest j (as
+ * OpenCV), (-1, -1) when the train set is empty.  o_i = query.num of the items before i.  matches_dev: DEVICE, int32
+ * pairs, sum of query.num entries.  One launch (none when every query set is empty), one CTA per 128 queries of an item,
+ * train descriptors tiled through shared memory.  Asynchronous on the handle's stream.  Every item is validated before
+ * anything is enqueued (1 <= n <= 65535, descriptor sizes, non-NULL and aligned pointers); a rejected call writes
+ * nothing and dfk_last_error names the item. */
+DfkStatus dfk_hamming_match_batch(DfkHandle h, const DfkMatchItem* items, int n, int32_t* matches_dev);
+
+/* The match list of every item's ReprojectionFactor: its three steps (reprojection_factor.cpp:56-65) on the device.
+ *   1. matching      dfk_hamming_match_batch; the RANSAC runs over all query.num matches (a match per query)
+ *   2. RANSAC        PruneMatchesEightPoint (features/matching.cpp:75-128), opengv's EIGHTPT relative-pose RANSAC
+ *                    restated deterministically:
+ *      bearings      f = normalize([(u - u0) / fx, (v - v0) / fy, 1]) in fp64 for both views (matching.cpp:39-58)
+ *      samples       hypothesis h in [0, max_iterations) takes 8 distinct matches from splitmix64 of (seed, h): draw
+ *                    k = 0, 1, ... is r = mix(mix(seed + G (h + 1)) + G (k + 1)), index = ((r >> 32) * N) >> 32,
+ *                    G = 0x9E3779B97F4A7C15, mix = splitmix64's finaliser, repeats skipped; a hypothesis whose 8
+ *                    indices take more than 256 draws is invalid.  The batch position does not enter: an item's
+ *                    output depends on the item alone.
+ *      model (fp64)  E = null vector of the 8 x 9 system f1^T E f0 = 0 (Householder QR); invalid if the system has
+ *                    rank < 8.  E -> U diag(1, 1, 0) V^T, and of (U W V^T, +-u3), (U W^T V^T, +-u3) the one with the
+ *                    most sample points in front of both cameras, ties to the first (X1 = R X0 + t).
+ *      score (fp64)  opengv's: the midpoint triangulation reprojected into both views as unit vectors,
+ *                    (1 - f0 . p0) + (1 - f1 . p1); an inlier scores < threshold.  An invalid hypothesis has 0 inliers.
+ *      selection     the sequential adaptive loop: in order of h, strictly more inliers replace the best, then
+ *                    k = log(1 - p) / log(1 - w^8), w = best / N, 1 - w^8 clamped to [2^-52, 1 - 2^-52]; stop after
+ *                    h when h + 1 >= k, or at max_iterations.  Every hypothesis is scored on the device in parallel
+ *                    and the loop runs as a scan over the counts: its result is the sequential loop's.
+ *      fewer than 8 matches (or none with an inlier): the item yields no matches -- OptimizeRep::ConstructFactors
+ *                    drops such a factor (df_work.cpp:336).
+ *   3. pruning       PruneMatchesByThreshold (matching.cpp:29-37): the best hypothesis' inliers with distance
+ *                    <= max_dist, sorted by (distance, query index).  std::sort leaves equal distances unordered
+ *                    there; the order changes only the summation order of the factor's rows.
+ * Outputs (DEVICE, int32): matches_dev rows (query, train, distance), item i's list at row o_i (as in
+ * dfk_hamming_match_batch), its length in counts_dev[i]; ransac_dev (may be NULL) [n x 3] = (selected hypothesis or -1,
+ * its inlier count, hypotheses evaluated).  Four launches for the whole batch (matching, hypotheses, selection,
+ * compaction), no atomics: deterministic.  Asynchronous on the handle's stream; validation as dfk_hamming_match_batch,
+ * plus the camera and RANSAC parameters. */
+DfkStatus dfk_reprojection_match_batch(DfkHandle h, const DfkMatchItem* items, int n, int32_t* matches_dev,
+                                       int32_t* counts_dev, int32_t* ransac_dev);
+
 /* ------------------------------------------------------------------ cu_image_proc free functions */
 
 /* df::UpdateDepth (cu_image_proc.h:41-44, cu_image_proc.cpp:248-277):

@@ -42,8 +42,13 @@ One JSON line per case:
   * coarse to fine (`--only levels`): window200's 50 keyframes and 200 pairs at C = 32 and 128 with a 3-level pyramid
     (640x480), a pho_iters = 4,8,15 schedule (dfk_window_lm_levels, 30 steps) against 30 all-level dfk_window_lm steps:
     wall and device time, and from perturbations of increasing size the final pose error and the level-0 energy.
+  * keypoint matching of reprojection factors (`--only match`): one keyframe connection (4 back connections x 2
+    directions = 8 factors) at 500 ORB-sized and at 1000 BRISK-sized features, and 64 factors at 500: one
+    dfk_reprojection_match_batch (wall clock to a synchronise, and summed device time from a separate profiled run)
+    against cv2.BFMatcher plus the sequential C RANSAC of match_oracle on the host, factor by factor.
 Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` /
-`--only frames` / `--only slide` / `--only error` / `--only lm` / `--only levels` runs those cases alone.
+`--only frames` / `--only slide` / `--only error` / `--only lm` / `--only levels` / `--only match` runs those cases
+alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -62,7 +67,8 @@ sys.path.insert(0, ROOT)
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
-    ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error", "lm", "levels"],
+    ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error", "lm", "levels",
+                                           "match"],
                     default=None)
     args = ap.parse_args()
     import numpy as np
@@ -101,6 +107,8 @@ def main():
         return lm_cases(args, torch, print)
     if args.only == "levels":
         return levels_cases(args, torch, print)
+    if args.only == "match":
+        return match_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -865,6 +873,55 @@ def levels_cases(args, torch, print):
                                   "timing": timing}), flush=True)
         del opts, probs, keyframes, shared, jac
         torch.cuda.empty_cache()
+
+
+def match_cases(args, torch, print):
+    """dfk_reprojection_match_batch against cv2.BFMatcher + the sequential C RANSAC on the host (match_oracle)"""
+    import numpy as np
+
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from match_scenes import make_scene
+
+    from deepfactors_b200.aligners import Features, ReprojectionMatchBatch, SfmAligner
+    from match_oracle import match_oracle as mo
+    try:
+        import cv2
+        bf = cv2.BFMatcher(cv2.NORM_HAMMING)
+    except ImportError:  # the host leg then times the oracle's brute-force matcher instead
+        bf = None
+    al = SfmAligner(8)
+    for name, n, nb, factors in (("connection_orb500", 500, 32, 8), ("connection_brisk1000", 1000, 64, 8),
+                                 ("factors64_orb500", 500, 32, 64)):
+        scenes = [make_scene(n, 0.4, 0.5, 1000 + j, desc_bytes=nb, max_flips=40) for j in range(factors)]
+        items = [dict(query=Features.from_host(sc.kp0, sc.desc0), train=Features.from_host(sc.kp1, sc.desc1),
+                      cam=sc.cam, seed=j) for j, sc in enumerate(scenes)]
+
+        def device():
+            ReprojectionMatchBatch(al, items)
+
+        wall = _wall_us(torch, device, args.reps)
+        dev_us = _device_us(torch, device, args.reps)
+        _, counts, ransac = ReprojectionMatchBatch(al, items)
+        counts, ransac = counts.cpu().numpy(), ransac.cpu().numpy()
+        t0 = time.perf_counter()
+        kept = []
+        for j, sc in enumerate(scenes):
+            if bf is not None:
+                ms = bf.match(sc.desc0, sc.desc1)
+                m = np.full((n, 2), -1, np.int32)
+                for x in ms:
+                    m[x.queryIdx] = (x.trainIdx, int(round(x.distance)))
+            else:
+                m = mo.hamming(sc.desc0, sc.desc1)
+            r = mo.reprojection_match(mo.params(sc.cam, seed=j), sc.kp0, sc.desc0, sc.kp1, sc.desc1, m)
+            kept.append(len(r.rows))
+        host = (time.perf_counter() - t0) * 1e6
+        print(json.dumps({"case": f"match_{name}", "factors": factors, "features": n, "descriptor_bytes": nb,
+                          "device_wall_us": round(wall, 1), "device_time_us": round(dev_us, 1),
+                          "host_us": round(host, 1), "host_matcher": "cv2.BFMatcher" if bf else "oracle",
+                          "speedup_wall": round(host / wall, 1),
+                          "hypotheses_evaluated_mean": float(ransac[:, 2].mean()),
+                          "kept_equal_host": bool(list(counts) == kept)}))
 
 
 def solve_fill(K, links):
