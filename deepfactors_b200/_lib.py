@@ -148,6 +148,14 @@ class DfkMatchItem(C.Structure):
 MATCH_MAX_QUERIES = 8192  # DFK_MATCH_MAX_QUERIES
 MATCH_MAX_ITERATIONS = 1000000  # DFK_MATCH_MAX_ITERATIONS
 
+
+class DfkOrbItem(C.Structure):
+    _fields_ = [("image", DfkImage), ("nfeatures", C.c_int32), ("fast_threshold", C.c_int32),
+                ("capacity", C.c_int32)]
+
+
+ORB_MAX_SIDE = 16384  # DFK_ORB_MAX_SIDE
+
 WINDOW_ERROR_DOUBLES = 7  # DFK_WINDOW_ERROR_DOUBLES
 
 
@@ -240,6 +248,8 @@ SYMBOLS = {
     "dfk_hamming_match_batch": (C.c_int, [_H, C.POINTER(DfkMatchItem), C.c_int, C.c_void_p]),
     "dfk_reprojection_match_batch": (C.c_int, [_H, C.POINTER(DfkMatchItem), C.c_int, C.c_void_p, C.c_void_p,
                                                C.c_void_p]),
+    "dfk_orb_detect_batch": (C.c_int, [_H, C.POINTER(DfkOrbItem), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]),
     "dfk_update_depth": (C.c_int, [_H, _F, C.c_int, _IMG, _IMG, C.c_float, _IMG]),
     "dfk_update_depth_batch": (C.c_int, [_H, C.POINTER(DfkDepthDecodeItem), C.c_int, C.c_int]),
     "dfk_sobel_gradients": (C.c_int, [_H, _IMG, _IMG]),

@@ -551,6 +551,86 @@ def ReprojectionMatchBatch(aligner, items: Sequence[dict]):
     return matches[:total], counts[:n], ransac[:n]
 
 
+# ------------------------------------------------------------------------------------------- ORB features
+# the reference's rep_nfeatures (deepfactors_options.h) and cv::ORB's default FAST threshold
+REP_NFEATURES = 500
+ORB_FAST_THRESHOLD = 20
+
+
+@dataclass
+class OrbBatch:
+    """The device output of OrbDetectBatch: item i's rows are [offsets[i], offsets[i] + min(counts[i], capacity_i)),
+    in the detector's order (response descending, then y, then x).  keypoints [rows, 2] float32, descriptors [rows, 32]
+    uint8, angles [rows] float32 (degrees), responses [rows] float32, counts [n] int32 (the true counts)."""
+    keypoints: torch.Tensor
+    descriptors: torch.Tensor
+    angles: torch.Tensor
+    responses: torch.Tensor
+    counts: torch.Tensor
+    offsets: np.ndarray
+    capacities: np.ndarray
+
+    def host_counts(self) -> np.ndarray:
+        """The counts on the host (synchronises with the stream); raises when an image's count exceeds its capacity,
+        since its output then lacks the keypoints past the capacity"""
+        c = self.counts.cpu().numpy().astype(np.int64)
+        over = np.nonzero(c > self.capacities)[0]
+        if len(over):
+            i = int(over[0])
+            raise RuntimeError(f"OrbDetectBatch: image {i} has {int(c[i])} keypoints (ties at the cut) but capacity "
+                               f"{int(self.capacities[i])}; pass a larger capacity")
+        return c
+
+    def features(self) -> list:
+        """One Features per image (views into the batch's tensors), ready for HammingMatchBatch /
+        ReprojectionMatchBatch / window_opt.match_reprojection_links; one read-back of the counts"""
+        c = self.host_counts()
+        return [Features(self.keypoints[o:o + k], self.descriptors[o:o + k]) for o, k in zip(self.offsets[:-1], c)]
+
+
+def _orb_image(t: torch.Tensor) -> DfkImage:
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.uint8:
+        raise TypeError("OrbDetectBatch: images must be uint8 CUDA tensors")
+    if t.dim() != 2 or t.stride(1) != 1 or (t.shape[0] > 1 and t.stride(0) < t.shape[1]):
+        raise ValueError("OrbDetectBatch: an image must be [H, W] with unit column stride")
+    return DfkImage(C.c_void_p(t.data_ptr()), max(int(t.stride(0)), int(t.shape[1])), int(t.shape[1]),
+                    int(t.shape[0]))
+
+
+def OrbDetectBatch(aligner, images: Sequence[torch.Tensor], nfeatures: int = REP_NFEATURES,
+                   fast_threshold: int = ORB_FAST_THRESHOLD, capacity: int | None = None) -> OrbBatch:
+    """cv::ORB_create(nfeatures, 1.2, 1).detectAndCompute of many gray images in one call (dfk_orb_detect_batch): the
+    reference's OrbDetector with rep_nlevels = 1, bit for bit.  images: uint8 [H, W] CUDA tensors of any sizes (below
+    63 x 63 an image has no features).  nfeatures, fast_threshold and capacity (default 2 nfeatures: ties at the
+    response cut can add keypoints) are one value for all images or one per image.  Asynchronous: returns an OrbBatch
+    of device tensors; OrbBatch.features() splits it into per-image Features."""
+    hd = aligner._hd
+    hd.use_torch_stream()
+    n = len(images)
+    per = lambda v: [int(x) for x in (v if isinstance(v, (list, tuple, np.ndarray)) else [v] * n)]
+    nf, t = per(nfeatures), per(fast_threshold)
+    cap = per(capacity) if capacity is not None else [2 * x for x in nf]
+    if not (len(nf) == len(t) == len(cap) == n):
+        raise ValueError("OrbDetectBatch: per-image settings need one entry per image")
+    for im in images:
+        if im.device != torch.device("cuda", hd.device):
+            raise ValueError(f"OrbDetectBatch: images must be on cuda:{hd.device}")
+    arr = (_lib.DfkOrbItem * max(n, 1))(*[_lib.DfkOrbItem(_orb_image(im), a, b, c)
+                                          for im, a, b, c in zip(images, nf, t, cap)])
+    offsets = np.concatenate([[0], np.cumsum(cap)]).astype(np.int64)
+    rows = int(offsets[-1])
+    dev = f"cuda:{hd.device}"
+    kp = torch.zeros((max(rows, 1), 2), dtype=torch.float32, device=dev)  # rows past a count stay 0
+    desc = torch.zeros((max(rows, 1), 32), dtype=torch.uint8, device=dev)
+    ang = torch.zeros(max(rows, 1), dtype=torch.float32, device=dev)
+    resp = torch.zeros(max(rows, 1), dtype=torch.float32, device=dev)
+    counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    check(hd.h, lib().dfk_orb_detect_batch(hd.h, arr, n, C.c_void_p(kp.data_ptr()), C.c_void_p(desc.data_ptr()),
+                                           C.c_void_p(ang.data_ptr()), C.c_void_p(resp.data_ptr()),
+                                           C.c_void_p(counts.data_ptr())))
+    return OrbBatch(kp[:rows], desc[:rows], ang[:rows], resp[:rows], counts[:n], offsets, np.array(cap, np.int64))
+
+
 def SparseGeometricErrorBatch(aligner, items, out: torch.Tensor | None = None) -> torch.Tensor:
     """SparseGeometricFactor::error of many factors in one launch (dfk_sparse_geometric_error_batch): the items of
     SparseGeometricLinearizeBatch (dicts, or the array of make_geometric_items).  Asynchronous: returns a device tensor [n, 2] float32, row i = [b^T b | valid points

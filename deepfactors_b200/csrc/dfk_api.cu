@@ -19,6 +19,7 @@
 #include "dfk_internal.h"
 #include "dfk_levels.h"
 #include "dfk_lm.h"
+#include "dfk_orb_model.h"
 #include "dfk_se3.cuh"
 
 using namespace dfk;
@@ -117,6 +118,10 @@ struct DfkContext {
   DeviceBuf<MatchItemDev> match_items;
   std::vector<MatchItemDev> match_host;
   DeviceBuf<unsigned char> match_scratch;
+  // dfk_orb_detect_batch: the item descriptors (one H2D per call) and the detector's scratch (see the call)
+  DeviceBuf<OrbItemDev> orb_items;
+  std::vector<OrbItemDev> orb_host;
+  DeviceBuf<unsigned char> orb_scratch;
   // dfk_window_marginalize_frames / dfk_window_add_priors: the call's index lists (one pageable H2D per call)
   DeviceBuf<int> window_lists;
   // dfk_window_marginalize_keyframe: the call's lists [refs | tile rows / cols | member locations | update tasks] (one
@@ -2652,6 +2657,98 @@ DfkStatus dfk_reprojection_match_batch(DfkHandle h, const DfkMatchItem* items, i
                                           reinterpret_cast<int3*>(matches_dev), counts_dev, h->stream),
              "[ReprojectionFactor matches batch] kernel launch failed");
     h->launches += 4;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_orb_detect_batch(DfkHandle h, const DfkOrbItem* items, int n, float* keypoints_dev,
+                               uint8_t* descriptors_dev, float* angles_dev, float* responses_dev, int32_t* counts_dev)
+{
+  return guarded(h, [&] {
+    const std::string w = "[OrbDetector batch] ";
+    if (!items || n < 1 || n > 65535)  // gridDim.z of the FAST kernel is the item
+      return fail(h, DFK_ERR_INVALID_ARG, w + "null argument / number of items not in [1, 65535]");
+    if (!keypoints_dev || !descriptors_dev || !counts_dev)
+      return fail(h, DFK_ERR_INVALID_ARG, w + "null keypoint, descriptor or count output");
+    if (((uintptr_t)keypoints_dev & 3) || ((uintptr_t)descriptors_dev & 15) || ((uintptr_t)angles_dev & 3) ||
+        ((uintptr_t)responses_dev & 3) || ((uintptr_t)counts_dev & 3))
+      return fail(h, DFK_ERR_INVALID_ARG, w + "descriptors must be 16-byte aligned, the other outputs 4-byte aligned");
+    h->orb_host.resize((size_t)n);
+    long long rows = 0, segs = 0, corners = 0, map = 0, blur = 0;
+    int max_rw = 0, max_rh = 0, max_cc = 0, max_segs = 0, max_cap = 0, max_nf = 0;
+    for (int i = 0; i < n; ++i) {
+      const DfkOrbItem& it = items[i];
+      const std::string at = " in item " + std::to_string(i);
+      if (!it.image.ptr || it.image.width > DFK_ORB_MAX_SIDE || it.image.height > DFK_ORB_MAX_SIDE ||
+          it.image.pitch_bytes < it.image.width)
+        return fail(h, DFK_ERR_INVALID_ARG, w + "image needs a pointer, width and height <= DFK_ORB_MAX_SIDE and "
+                                                "pitch_bytes >= width" + at);
+      if (it.nfeatures < 1 || it.nfeatures > DFK_MATCH_MAX_QUERIES)
+        return fail(h, DFK_ERR_INVALID_ARG, w + "nfeatures not in [1, DFK_MATCH_MAX_QUERIES]" + at);
+      if (it.fast_threshold < 0 || it.fast_threshold > 255)
+        return fail(h, DFK_ERR_INVALID_ARG, w + "fast_threshold not in [0, 255]" + at);
+      if (it.capacity < it.nfeatures)
+        return fail(h, DFK_ERR_INVALID_ARG, w + "capacity < nfeatures" + at);
+      const bool big = it.image.width >= DFK_OM_MIN_SIZE && it.image.height >= DFK_OM_MIN_SIZE;
+      OrbItemDev& d = h->orb_host[(size_t)i];
+      d = OrbItemDev{};
+      d.img = static_cast<const uint8_t*>(it.image.ptr);
+      d.pitch = it.image.pitch_bytes;
+      d.rw = big ? (int)it.image.width - 2 * DFK_OM_EDGE : 0;
+      d.rh = big ? (int)it.image.height - 2 * DFK_OM_EDGE : 0;
+      d.tiles_x = (d.rw + kOrbTileW - 1) / kOrbTileW;
+      d.tiles_y = (d.rh + kOrbTileH - 1) / kOrbTileH;
+      d.nfeatures = it.nfeatures;
+      d.threshold = it.fast_threshold;
+      d.capacity = it.capacity;
+      d.out_begin = (int)std::min(rows, (long long)INT32_MAX);
+      d.map_begin = (size_t)map;
+      d.seg_begin = (int)std::min(segs, (long long)INT32_MAX);
+      d.corner_begin = (int)std::min(corners, (long long)INT32_MAX);
+      d.corner_cap = ((d.rw + 1) / 2) * ((d.rh + 1) / 2);  // one corner per 2 x 2 pixels at most survives NMS
+      d.blur_begin = (size_t)blur;
+      rows += it.capacity;
+      segs += (long long)d.rh * d.tiles_x;
+      corners += d.corner_cap;
+      map += (long long)d.rw * d.rh;
+      if (big) blur += (long long)(d.rw + 2 * DFK_OM_PATTERN_R) * (d.rh + 2 * DFK_OM_PATTERN_R);
+      max_rw = std::max(max_rw, d.rw);
+      max_rh = std::max(max_rh, d.rh);
+      max_cc = std::max(max_cc, d.corner_cap);
+      max_segs = std::max(max_segs, d.rh * d.tiles_x);
+      max_cap = std::max(max_cap, it.capacity);
+      max_nf = std::max(max_nf, it.nfeatures);
+    }
+    if (rows > INT32_MAX || corners > INT32_MAX || segs > INT32_MAX)
+      return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 output rows or scratch entries in one call");
+    DeviceGuard guard(h->device);
+    // one allocation: [hist | stats | segments | corner positions | keys | angles | row map | score maps | blurred
+    // images], 16-byte parts
+    auto part = [](size_t bytes) { return (bytes + 15) & ~(size_t)15; };
+    const size_t b_hist = part(sizeof(int) * 256 * (size_t)n), b_stats = part(sizeof(int) * 4 * (size_t)n);
+    const size_t b_seg = part(sizeof(int) * (size_t)segs), b_c = part(sizeof(uint32_t) * (size_t)corners);
+    const size_t b_rows = part(sizeof(int) * (size_t)rows), b_map = part((size_t)map), b_blur = part((size_t)blur);
+    DFK_CUDA(h, h->orb_items.ensure((size_t)n), "[OrbDetector batch] scratch allocation failed");
+    DFK_CUDA(h, h->orb_scratch.ensure(b_hist + b_stats + b_seg + 3 * b_c + b_rows + b_map + b_blur),
+             "[OrbDetector batch] scratch allocation failed");
+    unsigned char* p = h->orb_scratch.ptr;
+    OrbScratchDev s;
+    s.hist = reinterpret_cast<int*>(p);
+    s.stats = reinterpret_cast<int*>(p += b_hist);
+    s.seg = reinterpret_cast<int*>(p += b_stats);
+    s.pos = reinterpret_cast<uint32_t*>(p += b_seg);
+    s.key = reinterpret_cast<uint32_t*>(p += b_c);
+    s.angle = reinterpret_cast<float*>(p += b_c);
+    s.rows = reinterpret_cast<int*>(p += b_c);
+    s.map = p += b_rows;
+    s.blur = p + b_map;
+    DFK_CUDA(h, cudaMemcpyAsync(h->orb_items.ptr, h->orb_host.data(), sizeof(OrbItemDev) * (size_t)n,
+                                cudaMemcpyHostToDevice, h->stream),
+             "[OrbDetector batch] upload failed");
+    DFK_CUDA(h, launch_orb_detect(h->orb_items.ptr, n, s, max_rw, max_rh, max_cc, max_segs, max_cap, max_nf,
+                                  keypoints_dev, descriptors_dev, angles_dev, responses_dev, counts_dev, h->stream),
+             "[OrbDetector batch] kernel launch failed");
+    h->launches += max_rw > 0 ? 7 : 5;
     return DFK_OK;
   });
 }

@@ -442,6 +442,41 @@ cudaError_t launch_reprojection_match(const MatchItemDev* items_dev, int n, int 
                                       int2* matches_dev, int* counts_dev, int3* select_dev, int3* out_dev,
                                       int* num_out_dev, cudaStream_t s);
 
+// one image of dfk_orb_detect_batch (dfk_orb.cu).  The detector works on the region R = [31, W - 31) x [31, H - 31)
+// where keypoints may lie, rw x rh pixels (0 x 0 for an image below 63 x 63), cut into FAST tiles of 32 x 8 pixels;
+// a segment is one 32-pixel row of a tile, and segments in row-major order are R's raster order.
+struct OrbItemDev {
+  const uint8_t* img;
+  size_t pitch;
+  int rw, rh;             // the region R
+  int tiles_x, tiles_y;   // FAST tiles over R; tiles_x segments per row
+  int nfeatures, threshold, capacity;
+  int out_begin;          // the item's first output row: the prefix sum of the capacities
+  size_t map_begin;       // bytes of the NMS score map (rw * rh)
+  int seg_begin;          // segment counts / offsets (rh * tiles_x)
+  int corner_begin;       // corner list (corner_cap entries: at most one corner per 2 x 2 pixels survives NMS)
+  int corner_cap;
+  size_t blur_begin;      // bytes of the blurred image over R widened by 18 (the pattern's reach): (rw + 36) x (rh + 36)
+};
+// the batch's scratch, all of it in one grow-only allocation; hist is zeroed before the first kernel
+struct OrbScratchDev {
+  uint8_t* map;           // NMS'd FAST score + 1 per pixel of R, 0 for no keypoint
+  int* seg;               // per segment: its corner count, then its first corner's index
+  int* hist;              // [n, 256] FAST score histogram of the kept corners
+  int* stats;             // [n, 4]: corners, first-cut score threshold, candidates, 0
+  uint32_t* pos;          // corner (y << 16 | x), raster order
+  uint32_t* key;          // corner FAST score, then the response key of a candidate (0 for a non-candidate)
+  float* angle;           // candidate angle
+  int* rows;              // output row -> corner index
+  uint8_t* blur;          // the blurred images the descriptors sample
+};
+constexpr int kOrbTileW = 32, kOrbTileH = 8;
+constexpr int kOrbMaxSide = 16384;
+cudaError_t launch_orb_detect(const OrbItemDev* items_dev, int n, const OrbScratchDev& s, int max_rw, int max_rh,
+                              int max_corner_cap, int max_segs, int max_capacity, int max_nfeatures,
+                              float* keypoints, uint8_t* descriptors, float* angles, float* responses, int* counts,
+                              cudaStream_t stream);
+
 constexpr int kSimpleMaxBlocks = 1024;
 constexpr int kSimpleScratchFloats = kSimpleMaxBlocks * 32;
 

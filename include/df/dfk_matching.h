@@ -8,6 +8,8 @@
 //     .PruneMatchesEightPoint     BFMatcher + RANSAC: the inliers in match (query) order, as features/matching.cpp:75-128
 //   df::PruneMatchesByThreshold   features/matching.cpp:29-37 on the host: distance <= max_dist, sorted by (distance,
 //                                 queryIdx), the order the device lists have
+//   df::OrbDetector               the keypoints and descriptors themselves: OrbDetector(nfeatures, scale_factor, 1)
+//     .DetectAndCompute           of features/feature_detection.h for one device image or a batch (dfk_orb_detect_batch)
 // The host-vector members copy their results back with the CUDA runtime; they exist where its header does.
 #ifndef DFK_MATCHING_H_
 #define DFK_MATCHING_H_
@@ -135,6 +137,86 @@ private:
 #endif
 
 private:
+  detail::HandlePtr h_;
+};
+
+// The reference's OrbDetector (features/feature_detection.h) on the device: cv::ORB::create(nfeatures, scale_factor,
+// nlevels) with nlevels = 1 (rep_nlevels), through dfk_orb_detect_batch.  With one level cv::ORB ignores
+// scale_factor; any other nlevels is rejected.  Keypoints come in the device order (response descending, then y,
+// then x), as df::Features views.
+class OrbDetector
+{
+public:
+  explicit OrbDetector(int nfeatures = 500, float scale_factor = 1.2f, int nlevels = 1, int fast_threshold = 20)
+      : nfeatures_(nfeatures), fast_threshold_(fast_threshold), h_(detail::MakeHandle())
+  {
+    if (nlevels != 1) throw std::invalid_argument("[OrbDetector] only nlevels = 1 (one pyramid level) is supported");
+    (void)scale_factor;
+  }
+
+  DfkHandle handle() const { return h_.get(); }
+  void SetStream(void* stream) { detail::Check(h_.get(), dfk_set_stream(h_.get(), stream)); }
+  int nfeatures() const { return nfeatures_; }
+  // rows reserved per image: ties at the response cut can add keypoints past nfeatures
+  int capacity() const { return 2 * nfeatures_; }
+
+  DfkOrbItem Item(const DfkImage& image) const { return DfkOrbItem{image, nfeatures_, fast_threshold_, capacity()}; }
+
+  // dfk_orb_detect_batch into the caller's DEVICE buffers (rows at the prefix sums of the items' capacities)
+  void DetectBatch(const std::vector<DfkOrbItem>& items, float* keypoints_dev, uint8_t* descriptors_dev,
+                   float* angles_dev, float* responses_dev, int32_t* counts_dev)
+  {
+    detail::Check(h_.get(), dfk_orb_detect_batch(h_.get(), items.data(), (int)items.size(), keypoints_dev,
+                                                 descriptors_dev, angles_dev, responses_dev, counts_dev));
+  }
+
+#ifdef DFK_FACADE_CUDART
+  // FeatureDetector::DetectAndCompute for a device gray image: the features stay valid until the next detection
+  Features DetectAndCompute(const DfkImage& image) { return DetectAndCompute(std::vector<DfkImage>{image})[0]; }
+
+  // every image in one call; waits for the counts
+  std::vector<Features> DetectAndCompute(const std::vector<DfkImage>& images)
+  {
+    const size_t n = images.size(), rows = n * (size_t)capacity();
+    std::vector<DfkOrbItem> items;
+    for (const DfkImage& im : images) items.push_back(Item(im));
+    if (rows > rows_) {
+      out_.reset();
+      void* p = nullptr;  // [descriptors 32 per row | keypoints 2 floats per row | counts]
+      if (cudaMalloc(&p, rows * 40 + 4 * n + 16) != cudaSuccess)
+        throw std::runtime_error("[OrbDetector] device allocation failed");
+      out_.reset(static_cast<uint8_t*>(p));
+      rows_ = rows;
+    }
+    uint8_t* desc = out_.get();
+    float* kp = reinterpret_cast<float*>(desc + 32 * rows_);
+    int32_t* counts = reinterpret_cast<int32_t*>(kp + 2 * rows_);
+    DetectBatch(items, kp, desc, nullptr, nullptr, counts);
+    std::vector<int32_t> host(n);
+    const cudaStream_t s = static_cast<cudaStream_t>(dfk_get_stream(h_.get()));
+    if (cudaMemcpyAsync(host.data(), counts, n * sizeof(int32_t), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+        cudaStreamSynchronize(s) != cudaSuccess)
+      throw std::runtime_error("[OrbDetector] count download failed");
+    std::vector<Features> out(n);
+    for (size_t i = 0; i < n; ++i) {
+      if (host[i] > capacity())
+        throw std::runtime_error("[OrbDetector] more keypoints than the capacity (ties at the response cut)");
+      const size_t o = i * (size_t)capacity();
+      out[i] = Features{kp + 2 * o, desc + 32 * o, host[i], 32};
+    }
+    return out;
+  }
+
+private:
+  struct Free {
+    void operator()(uint8_t* p) const { cudaFree(p); }
+  };
+  std::unique_ptr<uint8_t, Free> out_;
+  size_t rows_ = 0;
+#endif
+
+private:
+  int nfeatures_, fast_threshold_;
   detail::HandlePtr h_;
 };
 

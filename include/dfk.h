@@ -648,6 +648,53 @@ DfkStatus dfk_hamming_match_batch(DfkHandle h, const DfkMatchItem* items, int n,
 DfkStatus dfk_reprojection_match_batch(DfkHandle h, const DfkMatchItem* items, int n, int32_t* matches_dev,
                                        int32_t* counts_dev, int32_t* ransac_dev);
 
+/* ------------------------------------------------------------------ ORB features of a keyframe or frame */
+
+/* One image of an ORB batch: the reference's OrbDetector (features/feature_detection.h), i.e.
+ * cv::ORB::create(nfeatures, scale_factor, 1): rep_nfeatures = 500, one pyramid level (rep_nlevels = 1, which makes
+ * scale_factor irrelevant), edgeThreshold = patchSize = 31, WTA_K = 2, HARRIS_SCORE. */
+typedef struct {
+  DfkImage image;               /* DEVICE uint8 gray image (outframe_gray of PreprocessImage), width and height <=
+                                   DFK_ORB_MAX_SIDE, pitch_bytes >= width; below 63 x 63 it has no features */
+  int32_t nfeatures;            /* in [1, DFK_MATCH_MAX_QUERIES] */
+  int32_t fast_threshold;       /* FAST threshold t in [0, 255] (cv::ORB's default 20) */
+  int32_t capacity;             /* output rows reserved for the image, >= nfeatures */
+} DfkOrbItem;
+#define DFK_ORB_MAX_SIDE 16384
+
+/* cv::ORB::detectAndCompute of every item with one pyramid level, bit for bit (DESIGN.md section 4.9):
+ *   1. FAST-9    a pixel whose 16-pixel circle of radius 3 lies inside the image is a corner when 9 contiguous circle
+ *                pixels are all > I + t or all < I - t; score = (the largest, over the 16 arcs of 9 and both signs, of
+ *                the arc's smallest difference) - 1.  A corner survives when its score is strictly greater than each
+ *                of its 8 neighbours' (a non-corner counts as 0): cv::FastFeatureDetector(t, true).
+ *   2. border    31 <= x < W - 31, 31 <= y < H - 31.
+ *   3. first cut KeyPointsFilter::retainBest(2 nfeatures) by FAST score: every corner scoring at least the
+ *                (2 nfeatures)-th largest score is kept, ties included.
+ *   4. Harris    integer a = sum Ix^2, b = sum Iy^2, c = sum Ix Iy over the 7 x 7 block around the corner, Ix, Iy
+ *                ORB's 3 x 3 derivatives; r = ((float)a b - (float)c c - 0.04f (a + b) (a + b)) s^4 in fp32 in that
+ *                order, s = 1 / (4 * 7 * 255).
+ *   5. second cut retainBest(nfeatures) by r, ties included: more than nfeatures keypoints can come out.
+ *   6. angle     the intensity centroid over the radius-15 disc (ORB's umax rows): integer moments m10, m01,
+ *                angle = cv::fastAtan2(m01, m10) in degrees, fp32.
+ *   7. rBRIEF    256 bits; bit j = B[c + rot(p0_j)] < B[c + rot(p1_j)], byte j / 8, bit j % 8.  B is the image
+ *                blurred by the 7-tap Gaussian of sigma 2 (fp64 taps of cv::getGaussianKernel(7, 2), separable, rows
+ *                first, rounded half to even); rot rounds (x cos - y sin, x sin + y cos) in fp32 with rint, cos and sin
+ *                of angle * (float)(pi / 180).  The pairs p are OpenCV's bit_pattern_31_.
+ *   8. order     by response descending, then y, then x (cv::ORB's own order is an artefact of std::nth_element).
+ * Outputs (DEVICE), item i's rows at o_i = the sum of the capacities of the items before i:
+ *   keypoints_dev   float [rows, 2]: the corner's integer (x, y), as KeyPoint::pt
+ *   descriptors_dev uint8 [rows, 32], 16-byte aligned: a slice (keypoints_dev + 2 o_i, descriptors_dev + 32 o_i,
+ *                   counts_dev[i]) is the DfkFeatureSet of the image
+ *   angles_dev      float [rows] degrees, may be NULL;  responses_dev float [rows], may be NULL
+ *   counts_dev      int32 [n]: the true count; when ties push it past capacity only the first capacity rows are written
+ * Rows past an item's count are not written.  Seven kernels and one memset for the whole batch; integer atomics only
+ * count, every position comes from a scan or a sort: deterministic, and an item's output depends on the item alone.
+ * Asynchronous on the handle's stream.  Every item is validated before anything is enqueued (1 <= n <= 65535, the
+ * image, nfeatures, fast_threshold, capacity, non-NULL and aligned pointers); a rejected call writes nothing and
+ * dfk_last_error names the item. */
+DfkStatus dfk_orb_detect_batch(DfkHandle h, const DfkOrbItem* items, int n, float* keypoints_dev,
+                               uint8_t* descriptors_dev, float* angles_dev, float* responses_dev, int32_t* counts_dev);
+
 /* ------------------------------------------------------------------ cu_image_proc free functions */
 
 /* df::UpdateDepth (cu_image_proc.h:41-44, cu_image_proc.cpp:248-277):

@@ -46,9 +46,13 @@ One JSON line per case:
     directions = 8 factors) at 500 ORB-sized and at 1000 BRISK-sized features, and 64 factors at 500: one
     dfk_reprojection_match_batch (wall clock to a synchronise, and summed device time from a separate profiled run)
     against cv2.BFMatcher plus the sequential C RANSAC of match_oracle on the host, factor by factor.
+  * ORB features (`--only orb`): 1, 8 and 64 gray images at 256x192 (the network's size) and at 640x480, 500
+    features each: one dfk_orb_detect_batch (OrbDetectBatch; wall clock to a synchronise, summed device time and the
+    time of each kernel from a separate profiled run) against cv2.ORB_create(500, 1.2, 1).detectAndCompute on the
+    host, one image at a time.
 Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` /
-`--only frames` / `--only slide` / `--only error` / `--only lm` / `--only levels` / `--only match` runs those cases
-alone.
+`--only frames` / `--only slide` / `--only error` / `--only lm` / `--only levels` / `--only match` / `--only orb` runs
+those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -68,7 +72,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error", "lm", "levels",
-                                           "match"],
+                                           "match", "orb"],
                     default=None)
     args = ap.parse_args()
     import numpy as np
@@ -109,6 +113,8 @@ def main():
         return levels_cases(args, torch, print)
     if args.only == "match":
         return match_cases(args, torch, print)
+    if args.only == "orb":
+        return orb_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -922,6 +928,62 @@ def match_cases(args, torch, print):
                           "speedup_wall": round(host / wall, 1),
                           "hypotheses_evaluated_mean": float(ransac[:, 2].mean()),
                           "kept_equal_host": bool(list(counts) == kept)}))
+
+
+def _kernel_name(key):
+    """orb_fast_kernel for 'dfk::(anonymous namespace)::orb_fast_kernel(...)'; other profiler keys as they are"""
+    import re
+    m = re.search(r"(\w+_kernel)\(", key)
+    return m.group(1) if m else key.strip()
+
+
+def orb_cases(args, torch, print):
+    """dfk_orb_detect_batch against cv2.ORB_create(500, 1.2, 1).detectAndCompute on the host, image by image"""
+    import numpy as np
+    from torch.profiler import ProfilerActivity, profile
+
+    from deepfactors_b200.aligners import OrbDetectBatch, SfmAligner
+    try:
+        import cv2
+    except ImportError:  # no host leg then
+        cv2 = None
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from orb_images import images
+    z = images()
+    al = SfmAligner(8)
+    for w, h in ((256, 192), (640, 480)):
+        base = [z[f"1047_{w}"], z[f"1052_{w}"]]
+        for n in (1, 8, 64):
+            rng = np.random.default_rng(n)
+            # the two test images, each copy with its own noise so that no two images of a batch are equal
+            imgs = [np.clip(base[i % 2].astype(np.int16) + rng.integers(-2, 3, base[0].shape), 0, 255).astype(np.uint8)
+                    for i in range(n)]
+            dev = [torch.from_numpy(im).cuda() for im in imgs]
+
+            def device():
+                OrbDetectBatch(al, dev, 500, 20)
+
+            wall = _wall_us(torch, device, args.reps)
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(args.reps):
+                    device()
+                torch.cuda.synchronize()
+            stages = {e.key: round(e.self_device_time_total / args.reps, 1) for e in prof.key_averages()
+                      if e.self_device_time_total > 0}
+            dev_us = sum(stages.values())
+            counts = OrbDetectBatch(al, dev, 500, 20).counts.cpu().numpy()
+            rec = {"case": f"orb_{w}x{h}_x{n}", "images": n, "width": w, "height": h, "nfeatures": 500,
+                   "device_wall_us": round(wall, 1), "device_time_us": round(dev_us, 1),
+                   "stages_us": {_kernel_name(k): v for k, v in stages.items()}}
+            if cv2 is not None:
+                orb = cv2.ORB_create(500, 1.2, 1)
+                orb.detectAndCompute(imgs[0], None)
+                t0 = time.perf_counter()
+                host_counts = [len(orb.detectAndCompute(im, None)[0]) for im in imgs]
+                host = (time.perf_counter() - t0) * 1e6
+                rec.update({"host_us": round(host, 1), "host": f"cv2 {cv2.__version__}, one image at a time",
+                            "speedup_wall": round(host / wall, 1), "counts_equal_host": host_counts == list(counts)})
+            print(json.dumps(rec))
 
 
 def solve_fill(K, links):
