@@ -1,0 +1,1365 @@
+// dfk_api_window.cu -- C ABI of libdfk.so (see include/dfk.h), keyframe window: the window (create, assemble, priors,
+// marginalisation, blanket), its solver, and the window problem with its Levenberg-Marquardt loops.
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include <string.h>
+
+#include <algorithm>
+#include <cmath>
+#include <memory>
+#include <new>
+#include <string>
+#include <vector>
+
+#include "dfk.h"
+#include "dfk_host.h"
+#include "dfk_internal.h"
+#include "dfk_levels.h"
+#include "dfk_lm.h"
+
+using namespace dfk;
+
+// CSR adjacency of a keyframe window on the device (dfk_window_create)
+struct DfkWindow {
+  int device = 0;
+  WindowDev dev{};
+  // one allocation: kf0_ptr | kf0_items | kf1_ptr | kf1_items | pair_ptr | pair_items | lk0_ptr | lk0_links |
+  // lk1_ptr | lk1_links
+  DeviceBuf<int> ints;
+  DeviceBuf<float> areas;
+  size_t floats = 0;
+  // host copy of the structure, for dfk_window_solver_create and dfk_window_marginalize_keyframe
+  std::vector<int> pair_k0, pair_k1, link_k0, link_k1, item_pair;
+  // keyframe priors (dfk_window_create_priors): members prior_kf[prior_ptr[q] .. prior_ptr[q + 1]), the prior blocks
+  // (blk_i < blk_j) and their device lists (KfPriorDev)
+  std::vector<int> prior_ptr{0}, prior_kf, blk_i, blk_j;
+  std::vector<long long> prior_off;  // doubles: start of prior q in a priors buffer; back() = the buffer's size
+  DeviceBuf<int> kp_ints;
+  DeviceBuf<long long> kp_off;
+  KfPriorDev kp{};
+};
+
+// damped block-sparse Cholesky of one window (dfk_window_solver_create)
+struct DfkWindowSolver {
+  int device = 0;
+  int num_vars = 0, code_size = 0, num_keyframes = 0;
+  WindowSolverDev* dev = nullptr;
+  ~DfkWindowSolver() { window_solver_destroy(dev); }
+};
+
+// ---------------------------------------------------------------------------------------------- window problem
+// One window's every work item, planned and uploaded once (dfk_window_problem_create); the loop kernels of
+// dfk_window_lm.cu re-pose them from the device state.  Everything the items point at that is not the caller's (code
+// slots, ray tables, depth scratch of the error path) belongs to the problem.
+struct DfkWindowProblem {
+  int device = 0;
+  const DfkWindow* w = nullptr;
+  int K = 0, F = 0, C = 0, B = 0;
+  float avg_dpt = 2.0f, huber_delta = 0.1f;  // the handle's sfmparams at create, like the dense items' (SfmItemDev)
+  int nd = 0, nr = 0, ng = 0, ndep = 0, ne = 0, mf = 0, nkm = 0;  // items of each kind, frame priors, kf-prior members
+  size_t S = 0;  // doubles of one state: (K + F) 7 + K C
+  StepKernel step;
+  SfmLaunchPlan plan;
+  DeviceBuf<SfmItemDev> dense;
+  DeviceBuf<float> dense_codes;
+  std::vector<DeviceBuf<float>> rays;
+  DeviceBuf<unsigned char> rep, geo;  // the sparse batches' staged blocks [descriptors | codes | payload]
+  std::vector<unsigned char> rep_host, geo_host;
+  const unsigned char* rep_payload = nullptr;
+  const unsigned char* geo_payload = nullptr;
+  size_t rep_total = 0;
+  DeviceBuf<EvalErrorDesc> err;
+  int err_max_blocks = 1, err_rows = 0;
+  DeviceBuf<unsigned char> depth;  // [descriptors | codes]
+  int depth_max_blocks = 1;
+  DeviceBuf<float> depth_scratch;
+  DeviceBuf<int4> slots;           // dense | error | reproj | geo | depth
+  DeviceBuf<double> areas;         // W * H of each error item
+  DeviceBuf<float> err_out;        // (ne + nr + ng) x 2
+  DeviceBuf<double> state;         // two states: [cur] the problem's, [1 - cur] an LM candidate
+  int cur = 0;
+  DeviceBuf<double> frows, kfrows, x0, delta;  // prior rows, frozen points (frame priors, then kf members), deltas
+  DeviceBuf<int> delta_kf;         // keyframe of every delta row
+  DeviceBuf<int> fp_lists;         // dfk_window_add_priors' CSR: ptr[K + 1] | prior indices
+  float* records = nullptr;
+  float* geo_records = nullptr;
+  WindowSolverDev* solver[2] = {nullptr, nullptr};  // [fix_first_pose]
+  DeviceBuf<float> bufs;           // the LM's accepted and candidate window buffers
+  int acc = 0;
+  DeviceBuf<double> dx;
+  DeviceBuf<unsigned char> small;  // [energy 8 doubles | info int32]
+  PinnedBuf<unsigned char> small_host;
+  // active subsets (dfk_window_problem_set_active): the create-time dense and error items with their slots and areas
+  // are the templates a mask selects from; the selected items go to arrays of their own, so the full arrays stay as
+  // create planned them and an all-active mask runs exactly the create-time launches
+  std::vector<SfmItemDev> dense_tmpl;
+  std::vector<EvalErrorDesc> err_tmpl;
+  std::vector<int4> slots_tmpl;      // dense | error
+  std::vector<double> areas_tmpl;
+  bool sub_dense = false, sub_err = false;
+  int nda = 0, nea = 0;              // active dense / error items while sub_dense / sub_err
+  SfmLaunchPlan sub_plan;
+  DeviceBuf<SfmItemDev> dense_sub;
+  DeviceBuf<EvalErrorDesc> err_sub;
+  DeviceBuf<int4> sub_slots;         // dense [0, nd) | error [nd, nd + ne)
+  DeviceBuf<double> areas_sub;
+  DeviceBuf<int> rec_src;            // record slot i <- subset record rec_src[i], -1: zeros
+  DeviceBuf<float> sub_records;
+  ~DfkWindowProblem()
+  {
+    window_solver_destroy(solver[0]);
+    window_solver_destroy(solver[1]);
+  }
+  double* st(int i) const { return state.ptr + (size_t)i * S; }
+  double* energy() const { return reinterpret_cast<double*>(small.ptr); }
+  int32_t* info() const { return reinterpret_cast<int32_t*>(small.ptr + 8 * sizeof(double)); }
+};
+
+namespace {
+
+// Appends one CSR list to blob: ptr[keys + 1], then the items of each key in item order (the summation order of the
+// gather kernels); an item whose key is outside [0, keys) is in no list.  Returns where the list starts in blob
+template <class KeyOf>
+size_t add_csr(std::vector<int>& blob, int keys, int n, KeyOf key_of)
+{
+  const size_t o = blob.size();
+  blob.resize(o + keys + 1 + n, 0);
+  int* ptr = blob.data() + o;
+  for (int i = 0; i < n; ++i)
+    if (key_of(i) < keys) ptr[key_of(i) + 1] += 1;
+  for (int k = 0; k < keys; ++k) ptr[k + 1] += ptr[k];
+  std::vector<int> next(ptr, ptr + keys);
+  for (int i = 0; i < n; ++i)
+    if (key_of(i) < keys) ptr[keys + 1 + next[key_of(i)]++] = i;
+  return o;
+}
+
+// The window buffer from the records: the assemble kernel, then the keyframe-prior blocks set to zero
+// (dfk_window_add_keyframe_priors fills them)
+DfkStatus assemble_window(DfkHandle h, const DfkWindow* w, const float* records, const float* geo_records, float* buf,
+                          const char* what)
+{
+  DFK_CUDA(h, launch_window_assemble(w->dev, records, geo_records, buf, h->stream), what);
+  h->launches += 1;
+  if (w->kp.num_blocks > 0)
+    DFK_CUDA(h, cudaMemsetAsync(buf + w->kp.block_off, 0, (w->floats - w->kp.block_off) * sizeof(float), h->stream), what);
+  return DFK_OK;
+}
+
+WindowReposeDev repose_args(const DfkWindowProblem* p, const double* state)
+{
+  const int4* sl = p->slots.ptr;
+  WindowReposeDev a{};
+  a.code_size = p->C;
+  a.num_poses = p->K + p->F;
+  a.state = state;
+  a.dense = p->dense.ptr; a.dense_slots = sl; a.num_dense = p->nd;
+  a.error = p->err.ptr; a.error_slots = sl + p->nd; a.num_error = p->ne;
+  if (p->sub_dense) {
+    a.dense = p->dense_sub.ptr; a.dense_slots = p->sub_slots.ptr; a.num_dense = p->nda;
+  }
+  if (p->sub_err) {
+    a.error = p->err_sub.ptr; a.error_slots = p->sub_slots.ptr + p->nd; a.num_error = p->nea;
+  }
+  a.rep = reinterpret_cast<ReprojItemDev*>(p->rep.ptr); a.rep_slots = sl + p->nd + p->ne; a.num_rep = p->nr;
+  a.geo = reinterpret_cast<GeoItemDev*>(p->geo.ptr); a.geo_slots = sl + p->nd + p->ne + p->nr; a.num_geo = p->ng;
+  a.depth = reinterpret_cast<DepthDecodeDesc*>(p->depth.ptr); a.depth_slots = sl + p->nd + p->ne + p->nr + p->ng;
+  a.num_depth = p->ndep;
+  return a;
+}
+
+DfkStatus problem_deltas(DfkHandle h, const DfkWindowProblem* p, const double* state)
+{
+  DFK_CUDA(h, launch_window_deltas(state, p->K + p->F, p->C, p->mf + p->nkm, p->delta_kf.ptr, p->x0.ptr, p->delta.ptr,
+                                   h->stream),
+           "[WindowProblem] kernel launch failed");
+  h->launches += (p->mf + p->nkm) > 0;
+  return DFK_OK;
+}
+
+// the window buffer at state `state` into buf (dfk_window_problem_linearize)
+DfkStatus problem_linearize(DfkHandle h, DfkWindowProblem* p, const double* state, float* buf)
+{
+  const char* what = "[WindowProblem::linearize] kernel launch failed";
+  DFK_CUDA(h, launch_window_repose(repose_args(p, state), h->stream), what);
+  h->launches += 1;
+  const float avg = p->avg_dpt;
+  if (p->sub_dense) {  // the active items only, then every record slot from the subset's records or zeros
+    if (p->nda > 0) {
+      DFK_CUDA(h, h->partials_dev.ensure((size_t)p->sub_plan.num_partials * p->step.pfloats),
+               "[WindowProblem::linearize] scratch allocation failed");
+      DFK_TRY(launch_step(h, p->step, p->C, p->dense_sub.ptr, p->nda, p->sub_plan, h->partials_dev.ptr,
+                          p->sub_records.ptr));
+    }
+    DFK_CUDA(h, launch_window_scatter_records(p->sub_records.ptr, p->rec_src.ptr, p->nd, DFK_SFM_RECORD_FLOATS(p->C),
+                                              p->records, h->stream),
+             what);
+    h->launches += 1;
+  } else if (p->nd > 0) {
+    DFK_CUDA(h, h->partials_dev.ensure((size_t)p->plan.num_partials * p->step.pfloats),
+             "[WindowProblem::linearize] scratch allocation failed");
+    DFK_TRY(launch_step(h, p->step, p->C, p->dense.ptr, p->nd, p->plan, h->partials_dev.ptr, p->records));
+  }
+  if (p->nr > 0) {
+    const float2* q = reinterpret_cast<const float2*>(p->rep_payload);
+    DFK_CUDA(h, launch_reprojection_records(p->C, reinterpret_cast<const ReprojItemDev*>(p->rep.ptr), p->nr, q,
+                                            q + p->rep_total, avg, p->records + (size_t)p->nd * DFK_SFM_RECORD_FLOATS(p->C),
+                                            h->stream),
+             what);
+    h->launches += 1;
+  }
+  if (p->ng > 0) {
+    DFK_CUDA(h, launch_sparse_geometric_records(p->C, reinterpret_cast<const GeoItemDev*>(p->geo.ptr), p->ng,
+                                                reinterpret_cast<const int2*>(p->geo_payload), avg, p->geo_records,
+                                                h->stream),
+             what);
+    h->launches += 1;
+  }
+  const DfkWindow* w = p->w;
+  DFK_TRY(assemble_window(h, w, p->records, p->ng > 0 ? p->geo_records : nullptr, buf, what));
+  DFK_TRY(problem_deltas(h, p, state));
+  if (p->mf > 0) {
+    DFK_CUDA(h, launch_window_add_priors(w->dev, p->mf, p->fp_lists.ptr, p->fp_lists.ptr + p->K + 1, p->frows.ptr,
+                                         p->delta.ptr, buf, h->stream),
+             what);
+    h->launches += 1;
+  }
+  if (w->kp.num_priors > 0) {
+    DFK_CUDA(h, launch_window_add_keyframe_priors(w->dev, w->kp, p->kfrows.ptr, p->delta.ptr + (size_t)p->mf * p->B, buf,
+                                                  h->stream),
+             what);
+    h->launches += 1;
+  }
+  return DFK_OK;
+}
+
+WindowEnergyDev energy_args(const DfkWindowProblem* p, const double* state, double w)
+{
+  WindowEnergyDev a{};
+  a.B = p->B;
+  a.err_out = reinterpret_cast<const float2*>(p->err_out.ptr);
+  a.areas = p->sub_err ? p->areas_sub.ptr : p->areas.ptr;
+  a.num_error = p->sub_err ? p->nea : p->ne; a.num_rep = p->nr; a.num_geo = p->ng;
+  a.num_frame_priors = p->mf; a.frame_rows = p->frows.ptr; a.frame_delta = p->delta.ptr;
+  a.num_kf_priors = p->w->kp.num_priors; a.kf_rows = p->kfrows.ptr; a.kf_row_off = p->w->kp.off;
+  a.kf_mem_ptr = p->w->kp.mem_ptr; a.kf_delta = p->delta.ptr + (size_t)p->mf * p->B;
+  a.codes = state + (size_t)(p->K + p->F) * 7;
+  a.num_codes = p->K * p->C;
+  a.code_prior_weight = w;
+  a.out = p->energy();
+  return a;
+}
+
+// the energy at `state` without linearising into p->energy() (E + 1/2 w |c|^2 in slot 7)
+DfkStatus problem_error(DfkHandle h, DfkWindowProblem* p, const double* state, double w)
+{
+  const char* what = "[WindowProblem::error] kernel launch failed";
+  DFK_CUDA(h, launch_window_repose(repose_args(p, state), h->stream), what);
+  h->launches += 1;
+  const float avg = p->avg_dpt;
+  if (p->ndep > 0) {
+    DFK_CUDA(h, launch_update_depth_batch(p->C, reinterpret_cast<const DepthDecodeDesc*>(p->depth.ptr), p->ndep,
+                                          p->depth_max_blocks, avg, h->stream),
+             what);
+    h->launches += 1;
+  }
+  float* out = p->err_out.ptr;
+  // with an active subset only its items are evaluated, and their rows come first (energy_args reads as many)
+  const int ne = p->sub_err ? p->nea : p->ne;
+  if (ne > 0) {
+    const char* sw = "[WindowProblem::error] scratch allocation failed";
+    DFK_CUDA(h, h->eval_partials.ensure((size_t)p->err_rows * 32), sw);
+    DFK_TRY(ensure_tickets(h, h->eval_counters, (size_t)p->ne, sw, sw));
+    DFK_CUDA(h, launch_eval_error_batch(p->sub_err ? p->err_sub.ptr : p->err.ptr, ne, p->err_max_blocks,
+                                        p->huber_delta, h->eval_partials.ptr, h->eval_counters.ptr, out, h->stream),
+             what);
+    h->launches += 1;
+  }
+  if (p->nr > 0) {
+    const float2* q = reinterpret_cast<const float2*>(p->rep_payload);
+    DFK_CUDA(h, launch_reprojection_error(p->C, reinterpret_cast<const ReprojItemDev*>(p->rep.ptr), p->nr, q,
+                                          q + p->rep_total, avg, out + 2 * (size_t)ne, h->stream),
+             what);
+    h->launches += 1;
+  }
+  if (p->ng > 0) {
+    DFK_CUDA(h, launch_sparse_geometric_error(p->C, reinterpret_cast<const GeoItemDev*>(p->geo.ptr), p->ng,
+                                              reinterpret_cast<const int2*>(p->geo_payload), avg,
+                                              out + 2 * (size_t)(ne + p->nr), h->stream),
+             what);
+    h->launches += 1;
+  }
+  DFK_TRY(problem_deltas(h, p, state));
+  DFK_CUDA(h, launch_window_energy(energy_args(p, state, w), h->stream), what);
+  h->launches += 1;
+  return DFK_OK;
+}
+
+// the active subsets of a validated mask (em: one byte per error item): the selected templates, their slots and the
+// subset's tile plan, uploaded on the stream behind every launch still reading the previous ones.  The subset arrays
+// are allocated once at full size, so no later mask reallocates an array a queued launch reads
+DfkStatus problem_set_active(DfkHandle h, DfkWindowProblem* p, const uint8_t* dm, const uint8_t* em)
+{
+  const char* amsg = "[WindowProblem::set_active] allocation failed";
+  const char* umsg = "[WindowProblem::set_active] upload failed";
+  const int nd = p->nd, ne = p->ne;
+  const bool all_d = std::all_of(dm, dm + nd, [](uint8_t v) { return v != 0; });
+  const bool all_e = std::all_of(em, em + ne, [](uint8_t v) { return v != 0; });
+  if (!all_d || !all_e) {
+    DFK_CUDA(h, p->sub_slots.ensure((size_t)std::max(nd + ne, 1)), amsg);
+    if (!all_d) {
+      DFK_CUDA(h, p->dense_sub.ensure((size_t)std::max(nd, 1)), amsg);
+      DFK_CUDA(h, p->rec_src.ensure((size_t)nd), amsg);
+      DFK_CUDA(h, p->sub_records.ensure((size_t)nd * DFK_SFM_RECORD_FLOATS(p->C)), amsg);
+    }
+    if (!all_e) {
+      DFK_CUDA(h, p->err_sub.ensure((size_t)std::max(ne, 1)), amsg);
+      DFK_CUDA(h, p->areas_sub.ensure((size_t)std::max(ne, 1)), amsg);
+    }
+  }
+  if (!all_d) {
+    std::vector<SfmItemDev> items;
+    std::vector<int4> sl;
+    std::vector<int> src(nd, -1);
+    for (int i = 0; i < nd; ++i)
+      if (dm[i]) {
+        src[i] = (int)items.size();
+        items.push_back(p->dense_tmpl[i]);
+        sl.push_back(p->slots_tmpl[i]);
+      }
+    plan_tiles(items.data(), (int)items.size(), p->step.max_ctas, &p->sub_plan);
+    if (!items.empty()) {
+      DFK_CUDA(h, cudaMemcpyAsync(p->dense_sub.ptr, items.data(), sizeof(SfmItemDev) * items.size(),
+                                  cudaMemcpyHostToDevice, h->stream),
+               umsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->sub_slots.ptr, sl.data(), sizeof(int4) * sl.size(), cudaMemcpyHostToDevice,
+                                  h->stream),
+               umsg);
+    }
+    DFK_CUDA(h, cudaMemcpyAsync(p->rec_src.ptr, src.data(), sizeof(int) * nd, cudaMemcpyHostToDevice, h->stream), umsg);
+    p->nda = (int)items.size();
+  }
+  if (!all_e) {
+    std::vector<EvalErrorDesc> items;
+    std::vector<int4> sl;
+    std::vector<double> areas;
+    for (int i = 0; i < ne; ++i)
+      if (em[i]) {
+        items.push_back(p->err_tmpl[i]);
+        sl.push_back(p->slots_tmpl[nd + i]);
+        areas.push_back(p->areas_tmpl[i]);
+      }
+    if (!items.empty()) {
+      DFK_CUDA(h, cudaMemcpyAsync(p->err_sub.ptr, items.data(), sizeof(EvalErrorDesc) * items.size(),
+                                  cudaMemcpyHostToDevice, h->stream),
+               umsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->sub_slots.ptr + nd, sl.data(), sizeof(int4) * sl.size(), cudaMemcpyHostToDevice,
+                                  h->stream),
+               umsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->areas_sub.ptr, areas.data(), sizeof(double) * areas.size(),
+                                  cudaMemcpyHostToDevice, h->stream),
+               umsg);
+    }
+    p->nea = (int)items.size();
+  }
+  p->sub_dense = !all_d;
+  p->sub_err = !all_e;
+  return DFK_OK;
+}
+
+// dfk_window_lm's device half (the Ops of dfk_lm.h / dfk_levels.h): the state, buffers and solve of a problem
+struct ProblemLMOps {
+  DfkHandle h;
+  DfkWindowProblem* p;
+  const DfkLMParams* prm;
+  WindowSolverDev* solver;
+  size_t nf, f_off;
+  double w;
+  int cand() const { return 1 - p->cur; }
+  float* buf(bool c) const { return p->bufs.ptr + (size_t)(c ? 1 - p->acc : p->acc) * nf; }
+  DfkStatus linearize(bool c) { return problem_linearize(h, p, p->st(c ? cand() : p->cur), buf(c)); }
+  DfkStatus energy(bool c, double* f)
+  {
+    const double* s = p->st(c ? cand() : p->cur);
+    if (prm->use_error) {
+      DFK_TRY(problem_error(h, p, s, w));
+    } else {
+      WindowEnergyDev a = energy_args(p, s, w);
+      a.buf_f = buf(c) + f_off;
+      a.num_frame_priors = a.num_kf_priors = 0;
+      DFK_CUDA(h, launch_window_energy(a, h->stream), "[WindowLM] kernel launch failed");
+      h->launches += 1;
+    }
+    DFK_TRY(download(h, p->small_host.ptr, p->energy(), 8 * sizeof(double), "[WindowLM] read-back failed",
+                     "[WindowLM] kernel failed"));
+    *f = reinterpret_cast<const double*>(p->small_host.ptr)[7];
+    return DFK_OK;
+  }
+  DfkStatus solve(double lam, int* info)
+  {
+    DFK_CUDA(h, launch_window_solve(solver, buf(false), lam, w, p->st(p->cur) + (size_t)(p->K + p->F) * 7, p->dx.ptr,
+                                    p->info(), h->stream, &h->launches, true),
+             "[WindowLM] solve launch failed");
+    DFK_TRY(download(h, p->small_host.ptr, p->info(), sizeof(int32_t), "[WindowLM] read-back failed",
+                     "[WindowLM] solve failed"));
+    *info = *reinterpret_cast<const int32_t*>(p->small_host.ptr);
+    return DFK_OK;
+  }
+  DfkStatus retract()
+  {
+    DFK_CUDA(h, launch_window_retract(p->st(p->cur), p->st(cand()), p->dx.ptr, p->K, p->F, p->C, h->stream),
+             "[WindowLM] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  }
+  void accept()
+  {
+    p->cur = cand();
+    p->acc = 1 - p->acc;
+  }
+};
+
+// dfk_window_lm's checks of the parameters and trace, and the solver, buffers and Ops of a run
+DfkStatus lm_setup(DfkHandle h, DfkWindowProblem* p, const DfkLMParams* prm, DfkLMTrace* tr, const char* name,
+                   ProblemLMOps* ops)
+{
+  const std::string what = std::string("[") + name + "] ";
+  if (!p || !prm || !tr || !tr->energy || (prm->iterations > 0 && (!tr->lambda || !tr->accepted)))
+    return fail(h, DFK_ERR_INVALID_ARG, what + "null argument");
+  if (p->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, what + "problem and handle live on different devices");
+  if (prm->iterations < 0 || !(std::isfinite(prm->lambda_init) && prm->lambda_init >= 0.0) ||
+      !(std::isfinite(prm->code_prior_weight) && prm->code_prior_weight >= 0.0))
+    return fail(h, DFK_ERR_INVALID_ARG, what + "iterations < 0, or lambda_init / code_prior_weight not finite and >= 0");
+  if (!(std::isfinite(prm->lambda_up) && prm->lambda_up > 0.0) ||
+      !(std::isfinite(prm->lambda_down) && prm->lambda_down > 0.0) || std::isnan(prm->lambda_max))
+    return fail(h, DFK_ERR_INVALID_ARG, what + "lambda_up / lambda_down must be finite and > 0, lambda_max a number");
+  const int fix = prm->fix_first_pose ? 1 : 0;
+  const std::string amsg = what + "allocation failed";
+  if (!p->solver[fix])
+    DFK_CUDA(h, window_solver_create(p->K, p->C, p->F, p->w->pair_k0, p->w->pair_k1, p->w->link_k0, p->w->link_k1,
+                                     p->w->blk_i, p->w->blk_j, p->w->kp.block_off, std::vector<int>(), &p->solver[0]),
+             amsg.c_str());
+  const size_t nf = p->w->floats, f_off = (size_t)p->K * p->B * (p->B + 1) + (size_t)p->w->dev.num_pairs * 6 * p->B;
+  DFK_CUDA(h, p->bufs.ensure(2 * nf), amsg.c_str());
+  DFK_CUDA(h, p->dx.ensure((size_t)p->K * p->B + 6 * (size_t)p->F), amsg.c_str());
+  *ops = ProblemLMOps{h, p, prm, p->solver[fix], nf, f_off, prm->code_prior_weight};
+  return DFK_OK;
+}
+
+bool slot_ok(int s, int lo, int hi) { return s >= lo && s < hi; }
+
+}  // namespace
+
+extern "C" {
+
+DfkStatus dfk_window_create(DfkHandle h, const DfkWindowDesc* d, DfkWindow** out)
+{
+  return dfk_window_create_geometric(h, d, 0, nullptr, nullptr, out);
+}
+
+DfkStatus dfk_window_create_geometric(DfkHandle h, const DfkWindowDesc* d, int L, const int32_t* link_k0,
+                                      const int32_t* link_k1, DfkWindow** out)
+{
+  return dfk_window_create_frames(h, d, L, link_k0, link_k1, 0, out);
+}
+
+DfkStatus dfk_window_create_frames(DfkHandle h, const DfkWindowDesc* d, int L, const int32_t* link_k0,
+                                   const int32_t* link_k1, int F, DfkWindow** out)
+{
+  return dfk_window_create_priors(h, d, L, link_k0, link_k1, F, 0, nullptr, nullptr, out);
+}
+
+DfkStatus dfk_window_create_priors(DfkHandle h, const DfkWindowDesc* d, int L, const int32_t* link_k0,
+                                   const int32_t* link_k1, int F, int Q, const int32_t* prior_ptr,
+                                   const int32_t* prior_kf, DfkWindow** out)
+{
+  return guarded(h, [&] {
+    if (!d || !out || L < 0 || F < 0 || (L > 0 && (!link_k0 || !link_k1)) || Q < 0 ||
+        (Q > 0 && (!prior_ptr || !prior_kf)))
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window] null argument");
+    *out = nullptr;
+    const int K = d->num_keyframes, P = d->num_pairs, n = d->num_items;
+    if (K <= 0 || P <= 0 || n <= 0 || !d->pair_k0 || !d->pair_k1 || !d->item_pair || !d->item_width || !d->item_height)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window] empty window / null index array");
+    if (!dfk_sfm_supports_code_size(d->code_size))
+      return fail(h, DFK_ERR_UNSUPPORTED, "[Window] no RunStep kernel for code size " + std::to_string(d->code_size));
+    // pair_k1 in [K, K + F): frame pair_k1 - K, which must be k1 of exactly this one pair
+    std::vector<int> frame_pair(F, -1);
+    for (int p = 0; p < P; ++p) {
+      if (d->pair_k0[p] < 0 || d->pair_k0[p] >= K || d->pair_k1[p] < 0 || d->pair_k1[p] >= K + F)
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] pair " + std::to_string(p) + " names a keyframe outside the window");
+      if (d->pair_k1[p] >= K) {
+        if (frame_pair[d->pair_k1[p] - K] >= 0)
+          return fail(h, DFK_ERR_INVALID_ARG, "[Window] frame " + std::to_string(d->pair_k1[p] - K) +
+                                                  " is k1 of more than one pair");
+        frame_pair[d->pair_k1[p] - K] = p;
+      }
+    }
+    for (int f = 0; f < F; ++f)
+      if (frame_pair[f] < 0)
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] frame " + std::to_string(f) + " is k1 of no pair");
+    for (int i = 0; i < n; ++i)
+      // a record is scaled (W, H > 0: photometric) or unscaled (0, 0: reprojection)
+      if (d->item_pair[i] < 0 || d->item_pair[i] >= P ||
+          !((d->item_width[i] > 0 && d->item_height[i] > 0) || (d->item_width[i] == 0 && d->item_height[i] == 0)))
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] record " + std::to_string(i) + " names a pair outside the window");
+    for (int i = 0; i < n; ++i)
+      if (d->pair_k1[d->item_pair[i]] >= K && d->item_width[i] == 0)
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] record " + std::to_string(i) + " of a frame pair is unscaled");
+    for (int l = 0; l < L; ++l) {
+      if (link_k0[l] < 0 || link_k0[l] >= K || link_k1[l] < 0 || link_k1[l] >= K)
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] link " + std::to_string(l) + " names a keyframe outside the window");
+      if (link_k0[l] == link_k1[l])
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] link " + std::to_string(l) + " ties a keyframe to itself");
+    }
+    // keyframe priors: non-empty ascending lists of distinct keyframes of the window
+    if (Q > 0 && prior_ptr[0] != 0) return fail(h, DFK_ERR_INVALID_ARG, "[Window] prior_ptr[0] must be 0");
+    for (int q = 0; q < Q; ++q) {
+      if (prior_ptr[q + 1] <= prior_ptr[q])
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window] keyframe prior " + std::to_string(q) + " has no keyframe");
+      for (int a = prior_ptr[q]; a < prior_ptr[q + 1]; ++a)
+        if (prior_kf[a] < 0 || prior_kf[a] >= K || (a > prior_ptr[q] && prior_kf[a] <= prior_kf[a - 1]))
+          return fail(h, DFK_ERR_INVALID_ARG, "[Window] keyframe prior " + std::to_string(q) +
+                                                  " is not an ascending list of distinct keyframes of the window");
+    }
+    const int M = Q > 0 ? prior_ptr[Q] : 0;  // members of all priors
+    // prior blocks: the distinct (i < j) of every prior, ascending; the entries of each keyframe and each block in
+    // prior order
+    std::vector<std::pair<int, int>> blocks;
+    for (int q = 0; q < Q; ++q)
+      for (int a = prior_ptr[q]; a < prior_ptr[q + 1]; ++a)
+        for (int c = a + 1; c < prior_ptr[q + 1]; ++c) blocks.push_back({prior_kf[a], prior_kf[c]});
+    std::sort(blocks.begin(), blocks.end());
+    blocks.erase(std::unique(blocks.begin(), blocks.end()), blocks.end());
+    const int NB = (int)blocks.size();
+    std::vector<std::vector<int>> kf_ent(K), blk_ent(NB);
+    for (int q = 0; q < Q; ++q)
+      for (int a = prior_ptr[q]; a < prior_ptr[q + 1]; ++a) {
+        kf_ent[prior_kf[a]].insert(kf_ent[prior_kf[a]].end(), {q, a - prior_ptr[q]});
+        for (int c = a + 1; c < prior_ptr[q + 1]; ++c) {
+          const int b = (int)(std::lower_bound(blocks.begin(), blocks.end(), std::make_pair(prior_kf[a], prior_kf[c])) -
+                              blocks.begin());
+          blk_ent[b].insert(blk_ent[b].end(), {q, a - prior_ptr[q], c - prior_ptr[q]});
+        }
+      }
+    std::vector<int> kp_blob(Q + 1, 0);  // mem_ptr
+    for (int q = 0; q < Q; ++q) kp_blob[q + 1] = prior_ptr[q + 1];
+    const size_t o_kfp = kp_blob.size();
+    kp_blob.push_back(0);
+    for (int k = 0; k < K; ++k) kp_blob.push_back(kp_blob[o_kfp + k] + (int)kf_ent[k].size() / 2);
+    const size_t o_bp = kp_blob.size();
+    kp_blob.push_back(0);
+    for (int b = 0; b < NB; ++b) kp_blob.push_back(kp_blob[o_bp + b] + (int)blk_ent[b].size() / 3);
+    kp_blob.resize((kp_blob.size() + 3) & ~(size_t)3, 0);  // int2 / int3 entries 16-byte aligned
+    const size_t o_ke = kp_blob.size();
+    for (int k = 0; k < K; ++k) kp_blob.insert(kp_blob.end(), kf_ent[k].begin(), kf_ent[k].end());
+    kp_blob.resize((kp_blob.size() + 3) & ~(size_t)3, 0);
+    const size_t o_be = kp_blob.size();
+    for (int b = 0; b < NB; ++b) kp_blob.insert(kp_blob.end(), blk_ent[b].begin(), blk_ent[b].end());
+    std::vector<long long> poff(Q + 1, 0);
+    for (int q = 0; q < Q; ++q)
+      poff[q + 1] = poff[q] + (long long)DFK_KF_PRIOR_DOUBLES(d->code_size, prior_ptr[q + 1] - prior_ptr[q]);
+    // one CSR list per key kind (keyframe k0, frame k1, pair, and the links' keyframes)
+    std::vector<int> blob;
+    const size_t o_kf0 = add_csr(blob, K, n, [&](int i) { return d->pair_k0[d->item_pair[i]]; });
+    // a frame pair's pose1 is the frame's: its items go to the frame's block, not to a keyframe's
+    const size_t o_kf1 = add_csr(blob, K, n, [&](int i) { return d->pair_k1[d->item_pair[i]]; });
+    const size_t o_pair = add_csr(blob, P, n, [&](int i) { return d->item_pair[i]; });
+    const size_t o_lk0 = add_csr(blob, K, L, [&](int l) { return link_k0[l]; });
+    const size_t o_lk1 = add_csr(blob, K, L, [&](int l) { return link_k1[l]; });
+    const size_t o_fr = blob.size();
+    blob.insert(blob.end(), frame_pair.begin(), frame_pair.end());
+    std::vector<float> areas(n);
+    for (int i = 0; i < n; ++i) areas[i] = (float)d->item_width[i] * (float)d->item_height[i];
+
+    DeviceGuard guard(h->device);
+    std::unique_ptr<DfkWindow> w(new (std::nothrow) DfkWindow());  // freed under the guard if the upload fails
+    if (!w) return oom(h);
+    w->device = h->device;
+    const char* upload_failed = "[Window] index upload failed";
+    DFK_CUDA(h, w->ints.ensure(blob.size()), upload_failed);
+    DFK_CUDA(h, w->areas.ensure(areas.size()), upload_failed);
+    DFK_CUDA(h, cudaMemcpy(w->ints.ptr, blob.data(), blob.size() * sizeof(int), cudaMemcpyHostToDevice), upload_failed);
+    DFK_CUDA(h, cudaMemcpy(w->areas.ptr, areas.data(), areas.size() * sizeof(float), cudaMemcpyHostToDevice), upload_failed);
+    const int* ints = w->ints.ptr;
+    w->dev.num_keyframes = K; w->dev.num_pairs = P; w->dev.num_items = n; w->dev.code_size = d->code_size;
+    w->dev.kf0_ptr = ints + o_kf0; w->dev.kf0_items = ints + o_kf0 + K + 1;
+    w->dev.kf1_ptr = ints + o_kf1; w->dev.kf1_items = ints + o_kf1 + K + 1;
+    w->dev.pair_ptr = ints + o_pair; w->dev.pair_items = ints + o_pair + P + 1;
+    w->dev.item_area = w->areas.ptr;
+    w->dev.num_links = L;
+    w->dev.lk0_ptr = ints + o_lk0; w->dev.lk0_links = ints + o_lk0 + K + 1;
+    w->dev.lk1_ptr = ints + o_lk1; w->dev.lk1_links = ints + o_lk1 + K + 1;
+    w->dev.num_frames = F;
+    w->dev.frame_pair = ints + o_fr;
+    const size_t B = 6 + (size_t)d->code_size;
+    const size_t block_off = (size_t)K * (B * B + B) + (size_t)P * 6 * B + 2 + (size_t)L * B * B + (size_t)F * 42;
+    w->floats = block_off + (size_t)NB * B * B;
+    w->pair_k0.assign(d->pair_k0, d->pair_k0 + P);
+    w->pair_k1.assign(d->pair_k1, d->pair_k1 + P);
+    w->link_k0.assign(link_k0, link_k0 + L);
+    w->link_k1.assign(link_k1, link_k1 + L);
+    w->item_pair.assign(d->item_pair, d->item_pair + n);
+    if (Q > 0) {
+      w->prior_ptr.assign(prior_ptr, prior_ptr + Q + 1);
+      w->prior_kf.assign(prior_kf, prior_kf + M);
+      for (const auto& b : blocks) {
+        w->blk_i.push_back(b.first);
+        w->blk_j.push_back(b.second);
+      }
+      w->prior_off = poff;
+      DFK_CUDA(h, w->kp_ints.ensure(kp_blob.size()), upload_failed);
+      DFK_CUDA(h, w->kp_off.ensure(poff.size()), upload_failed);
+      DFK_CUDA(h, cudaMemcpy(w->kp_ints.ptr, kp_blob.data(), kp_blob.size() * sizeof(int), cudaMemcpyHostToDevice),
+               upload_failed);
+      DFK_CUDA(h, cudaMemcpy(w->kp_off.ptr, poff.data(), poff.size() * sizeof(long long), cudaMemcpyHostToDevice),
+               upload_failed);
+      const int* kpi = w->kp_ints.ptr;
+      w->kp.num_priors = Q; w->kp.num_blocks = NB; w->kp.block_off = block_off;
+      w->kp.mem_ptr = kpi; w->kp.off = w->kp_off.ptr;
+      w->kp.kf_ptr = kpi + o_kfp; w->kp.kf_ent = reinterpret_cast<const int2*>(kpi + o_ke);
+      w->kp.blk_ptr = kpi + o_bp; w->kp.blk_ent = reinterpret_cast<const int3*>(kpi + o_be);
+    }
+    *out = w.release();
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_destroy(DfkHandle /*h*/, DfkWindow* w)
+{
+  if (!w) return DFK_OK;
+  DeviceGuard guard(w->device);
+  delete w;
+  return DFK_OK;
+}
+
+size_t dfk_window_floats(const DfkWindow* w) { return w ? w->floats : 0; }
+
+DfkStatus dfk_window_assemble(DfkHandle h, const DfkWindow* w, const float* records_dev, float* window_dev)
+{
+  return guarded(h, [&] {
+    if (!w || !records_dev || !window_dev) return fail(h, DFK_ERR_INVALID_ARG, "[Window] null argument");
+    if (w->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[Window] window and handle live on different devices");
+    if (w->dev.num_links > 0)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window] window has geometric links: assemble it with dfk_window_assemble_geometric");
+    DeviceGuard guard(h->device);
+    return assemble_window(h, w, records_dev, nullptr, window_dev, "[Window] kernel launch failed");
+  });
+}
+
+DfkStatus dfk_window_assemble_geometric(DfkHandle h, const DfkWindow* w, const float* records_dev,
+                                        const float* geo_records_dev, float* window_dev)
+{
+  return guarded(h, [&] {
+    if (!w || !records_dev || !window_dev) return fail(h, DFK_ERR_INVALID_ARG, "[Window] null argument");
+    if (w->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[Window] window and handle live on different devices");
+    if (w->dev.num_links > 0 && !geo_records_dev)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window] window has geometric links but no geometric records");
+    DeviceGuard guard(h->device);
+    return assemble_window(h, w, records_dev, geo_records_dev, window_dev, "[Window] kernel launch failed");
+  });
+}
+
+DfkStatus dfk_window_marginalize_frames(DfkHandle h, const DfkWindow* w, const float* records_dev, int n,
+                                        const int32_t* frames_host, double* priors_dev, int32_t* info_dev)
+{
+  return guarded(h, [&] {
+    if (!w || !records_dev || n < 0 || (n > 0 && (!frames_host || !priors_dev || !info_dev)))
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::MarginalizeFrames] null argument");
+    if (w->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::MarginalizeFrames] window and handle live on different devices");
+    for (int i = 0; i < n; ++i)
+      if (frames_host[i] < 0 || frames_host[i] >= w->dev.num_frames)
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window::MarginalizeFrames] frame " + std::to_string(frames_host[i]) +
+                                                " is not a frame of the window");
+    if (n == 0) return DFK_OK;
+    DeviceGuard guard(h->device);
+    const char* what = "[Window::MarginalizeFrames] index upload failed";
+    DFK_CUDA(h, h->window_lists.ensure(n), what);
+    // pageable source: staged before the call returns
+    DFK_CUDA(h, cudaMemcpyAsync(h->window_lists.ptr, frames_host, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream),
+             what);
+    DFK_CUDA(h, launch_window_marginalize_frames(w->dev, records_dev, n, h->window_lists.ptr, priors_dev, info_dev,
+                                                 h->stream),
+             "[Window::MarginalizeFrames] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_add_priors(DfkHandle h, const DfkWindow* w, int m, const int32_t* prior_kf_host,
+                                const double* priors_dev, const double* delta_dev, float* window_dev)
+{
+  return guarded(h, [&] {
+    if (!w || !window_dev || m < 0 || (m > 0 && (!prior_kf_host || !priors_dev || !delta_dev)))
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddPriors] null argument");
+    if (w->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddPriors] window and handle live on different devices");
+    const int K = w->dev.num_keyframes;
+    for (int i = 0; i < m; ++i)
+      if (prior_kf_host[i] < 0 || prior_kf_host[i] >= K)
+        return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddPriors] prior " + std::to_string(i) +
+                                                " names a keyframe outside the window");
+    if (m == 0) return DFK_OK;
+    // CSR of the priors per keyframe, in list order: ptr[K + 1] | indices[m]
+    std::vector<int> lists;
+    add_csr(lists, K, m, [&](int i) { return prior_kf_host[i]; });
+    DeviceGuard guard(h->device);
+    const char* what = "[Window::AddPriors] index upload failed";
+    DFK_CUDA(h, h->window_lists.ensure(lists.size()), what);
+    DFK_CUDA(h, cudaMemcpyAsync(h->window_lists.ptr, lists.data(), sizeof(int) * lists.size(), cudaMemcpyHostToDevice,
+                                h->stream),
+             what);
+    DFK_CUDA(h, launch_window_add_priors(w->dev, m, h->window_lists.ptr, h->window_lists.ptr + K + 1, priors_dev,
+                                         delta_dev, window_dev, h->stream),
+             "[Window::AddPriors] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_add_keyframe_priors(DfkHandle h, const DfkWindow* w, const double* priors_dev,
+                                         const double* delta_dev, float* window_dev)
+{
+  return guarded(h, [&] {
+    if (!w || !window_dev) return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddKeyframePriors] null argument");
+    if (w->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddKeyframePriors] window and handle live on different devices");
+    if (w->kp.num_priors == 0) return DFK_OK;
+    if (!priors_dev || !delta_dev) return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddKeyframePriors] null argument");
+    DeviceGuard guard(h->device);
+    DFK_CUDA(h, launch_window_add_keyframe_priors(w->dev, w->kp, priors_dev, delta_dev, window_dev, h->stream),
+             "[Window::AddKeyframePriors] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+namespace {
+
+// N(m): the keyframes that share a pair, a link or a keyframe prior with m, ascending
+std::vector<int> window_blanket(const DfkWindow* w, int m)
+{
+  const int K = w->dev.num_keyframes;
+  std::vector<char> in(K, 0);
+  auto tie = [&](int a, int b) {
+    if (a < K && b < K && (a == m || b == m)) in[a] = in[b] = 1;
+  };
+  for (size_t p = 0; p < w->pair_k0.size(); ++p) tie(w->pair_k0[p], w->pair_k1[p]);
+  for (size_t l = 0; l < w->link_k0.size(); ++l) tie(w->link_k0[l], w->link_k1[l]);
+  for (size_t q = 0; q + 1 < w->prior_ptr.size(); ++q) {
+    const auto b = w->prior_kf.begin() + w->prior_ptr[q], e = w->prior_kf.begin() + w->prior_ptr[q + 1];
+    if (std::find(b, e, m) != e)
+      for (auto it = b; it != e; ++it) in[*it] = 1;
+  }
+  in[m] = 0;
+  std::vector<int> out;
+  for (int k = 0; k < K; ++k)
+    if (in[k]) out.push_back(k);
+  return out;
+}
+
+bool prior_contains(const DfkWindow* w, int q, int m)
+{
+  const auto b = w->prior_kf.begin() + w->prior_ptr[q], e = w->prior_kf.begin() + w->prior_ptr[q + 1];
+  return std::find(b, e, m) != e;
+}
+
+}  // namespace
+
+DfkStatus dfk_window_blanket(DfkHandle h, const DfkWindow* w, int m, int32_t* kf_out, int32_t* n)
+{
+  return guarded(h, [&] {
+    if (!w || !kf_out || !n) return fail(h, DFK_ERR_INVALID_ARG, "[Window::Blanket] null argument");
+    if (m < 0 || m >= w->dev.num_keyframes)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::Blanket] keyframe " + std::to_string(m) + " is not in the window");
+    const std::vector<int> nb = window_blanket(w, m);
+    std::copy(nb.begin(), nb.end(), kf_out);
+    *n = (int32_t)nb.size();
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_marginalize_keyframe(DfkHandle h, const DfkWindow* w, const float* records_dev,
+                                          const float* geo_records_dev, int m, int num_frame_priors,
+                                          const double* frame_priors_dev, const double* frame_delta_dev,
+                                          const double* kf_priors_dev, const double* kf_delta_dev,
+                                          double code_prior_weight, const double* code_m_host, double* prior_dev,
+                                          int32_t* info_dev)
+{
+  return guarded(h, [&] {
+    const char* what = "[Window::MarginalizeKeyframe] ";
+    auto bad = [&](DfkStatus s, const std::string& msg) { return fail(h, s, what + msg); };
+    if (!w || !records_dev || !prior_dev || !info_dev || num_frame_priors < 0 ||
+        (num_frame_priors > 0 && (!frame_priors_dev || !frame_delta_dev)))
+      return bad(DFK_ERR_INVALID_ARG, "null argument");
+    if (w->device != h->device) return bad(DFK_ERR_INVALID_ARG, "window and handle live on different devices");
+    const int K = w->dev.num_keyframes, C = w->dev.code_size, B = 6 + C;
+    if (m < 0 || m >= K) return bad(DFK_ERR_INVALID_ARG, "keyframe " + std::to_string(m) + " is not in the window");
+    if (w->dev.num_links > 0 && !geo_records_dev)
+      return bad(DFK_ERR_INVALID_ARG, "window has geometric links but no geometric records");
+    if (!(std::isfinite(code_prior_weight) && code_prior_weight >= 0.0))
+      return bad(DFK_ERR_INVALID_ARG, "code_prior_weight must be finite and >= 0");
+    if (code_prior_weight > 0.0 && !code_m_host) return bad(DFK_ERR_INVALID_ARG, "code_prior_weight > 0 needs m's code");
+    for (size_t p = 0; p < w->pair_k0.size(); ++p)
+      if (w->pair_k0[p] == m && w->pair_k1[p] >= K)
+        return bad(DFK_ERR_INVALID_ARG, "keyframe " + std::to_string(m) + " still has tracked frames: marginalise them first");
+    const int Q = w->kp.num_priors;
+    std::vector<int> kq;  // the keyframe priors that contain m
+    for (int q = 0; q < Q; ++q)
+      if (prior_contains(w, q, m)) kq.push_back(q);
+    if (!kq.empty() && (!kf_priors_dev || !kf_delta_dev))
+      return bad(DFK_ERR_INVALID_ARG, "keyframe priors contain m but none were given");
+    const std::vector<int> nb = window_blanket(w, m);
+    const int n = (int)nb.size();
+    if (n == 0) return bad(DFK_ERR_INVALID_ARG, "keyframe " + std::to_string(m) + " shares no factor with another");
+    if (n > DFK_MAX_BLANKET)
+      return bad(DFK_ERR_UNSUPPORTED, "blanket of " + std::to_string(n) + " keyframes (at most " +
+                                          std::to_string(DFK_MAX_BLANKET) + ")");
+    std::vector<int> loc(K, -1);
+    loc[m] = 0;
+    for (int i = 0; i < n; ++i) loc[nb[i]] = 1 + i;
+    // [refs | tile_row | tile_col | mem_loc | pad | update tasks]
+    std::vector<int> lists;
+    for (size_t i = 0; i < w->item_pair.size(); ++i) {
+      const int k0 = w->pair_k0[w->item_pair[i]], k1 = w->pair_k1[w->item_pair[i]];
+      if (k1 < K && (k0 == m || k1 == m)) lists.insert(lists.end(), {0, (int)i, loc[k0], loc[k1]});
+    }
+    for (size_t l = 0; l < w->link_k0.size(); ++l)
+      if (w->link_k0[l] == m || w->link_k1[l] == m)
+        lists.insert(lists.end(), {1, (int)l, loc[w->link_k0[l]], loc[w->link_k1[l]]});
+    for (int i = 0; i < num_frame_priors; ++i) lists.insert(lists.end(), {2, i, 0, 0});
+    for (int q : kq) lists.insert(lists.end(), {3, q, 0, 0});
+    const int num_refs = (int)lists.size() / 4;
+    const int T = n + 1 + n * (n + 1) / 2;
+    const size_t o_tr = lists.size();
+    for (int t = 0; t <= n; ++t) lists.push_back(t);
+    for (int I = 1; I <= n; ++I)
+      for (int J = 1; J <= I; ++J) lists.push_back(I);
+    const size_t o_tc = lists.size();
+    for (int t = 0; t <= n; ++t) lists.push_back(0);
+    for (int I = 1; I <= n; ++I)
+      for (int J = 1; J <= I; ++J) lists.push_back(J);
+    const size_t o_ml = lists.size();
+    for (int kf : w->prior_kf) lists.push_back(loc[kf]);
+    lists.resize((lists.size() + 3) & ~(size_t)3, 0);
+    const size_t o_tk = lists.size();
+    std::vector<int> tasks;
+    window_eliminate_first_tasks(n, tasks);
+    lists.insert(lists.end(), tasks.begin(), tasks.end());
+    const size_t ws = (size_t)(T + 1) * B * B + (size_t)(n + 1) * B + 1;
+
+    DeviceGuard guard(h->device);
+    const char* alloc = "[Window::MarginalizeKeyframe] scratch allocation failed";
+    DFK_CUDA(h, h->marg_lists.ensure(lists.size()), alloc);
+    DFK_CUDA(h, h->marg_dev.ensure(ws), alloc);
+    DFK_CUDA(h, h->marg_code.ensure(C), alloc);
+    // pageable sources: staged before the call returns
+    DFK_CUDA(h, cudaMemcpyAsync(h->marg_lists.ptr, lists.data(), lists.size() * sizeof(int), cudaMemcpyHostToDevice,
+                                h->stream), alloc);
+    if (code_prior_weight > 0.0)
+      DFK_CUDA(h, cudaMemcpyAsync(h->marg_code.ptr, code_m_host, C * sizeof(double), cudaMemcpyHostToDevice, h->stream),
+               alloc);
+    const int* li = h->marg_lists.ptr;
+    KfMargDev md{};
+    md.n = n;
+    md.num_refs = num_refs;
+    md.refs = reinterpret_cast<const KfMargRef*>(li);
+    md.tile_row = li + o_tr; md.tile_col = li + o_tc; md.mem_loc = li + o_ml;
+    md.records = records_dev; md.geo = geo_records_dev;
+    md.fpriors = frame_priors_dev; md.fdelta = frame_delta_dev;
+    md.kpriors = kf_priors_dev; md.kdelta = kf_delta_dev;
+    md.w = code_prior_weight; md.code = h->marg_code.ptr;
+    md.tiles = h->marg_dev.ptr;
+    md.rhs = md.tiles + (size_t)(T + 1) * B * B;
+    md.f = md.rhs + (size_t)(n + 1) * B;
+    md.info = info_dev;
+    const char* launch = "[Window::MarginalizeKeyframe] kernel launch failed";
+    DFK_CUDA(h, launch_window_marg_gather(w->dev, w->kp, md, T, h->stream), launch);
+    DFK_CUDA(h, launch_window_eliminate_first(C, n, md.tiles, md.rhs, info_dev, li + o_tk, (int)tasks.size() / 4,
+                                              h->stream), launch);
+    DFK_CUDA(h, launch_window_marg_finalize(C, md, T, prior_dev, h->stream), launch);
+    h->launches += 4;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_solver_create(DfkHandle h, const DfkWindow* w, int num_fixed, const int32_t* fixed_vars,
+                                   DfkWindowSolver** out)
+{
+  return guarded(h, [&] {
+    if (!w || !out || num_fixed < 0 || (num_fixed > 0 && !fixed_vars))
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] null argument");
+    *out = nullptr;
+    if (w->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] window and handle live on different devices");
+    const int K = w->dev.num_keyframes, C = w->dev.code_size, n = K * (6 + C);
+    std::vector<int> fixed(fixed_vars, fixed_vars + num_fixed);
+    std::vector<char> seen(n, 0);
+    for (int q = 0; q < num_fixed; ++q) {
+      if (fixed[q] < 0 || fixed[q] >= n)
+        return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] fixed variable " + std::to_string(fixed[q]) +
+                                                " outside the window's " + std::to_string(n) + " variables");
+      if (seen[fixed[q]]++)
+        return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] fixed variable " + std::to_string(fixed[q]) + " listed twice");
+    }
+    DeviceGuard guard(h->device);
+    std::unique_ptr<DfkWindowSolver> s(new (std::nothrow) DfkWindowSolver());
+    if (!s) return oom(h);
+    s->device = h->device;
+    s->num_vars = n; s->code_size = C; s->num_keyframes = K;
+    DFK_CUDA(h, window_solver_create(K, C, w->dev.num_frames, w->pair_k0, w->pair_k1, w->link_k0, w->link_k1, w->blk_i,
+                                     w->blk_j, w->kp.block_off, fixed, &s->dev),
+             "[WindowSolver] workspace allocation failed");
+    *out = s.release();
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_solver_destroy(DfkHandle h, DfkWindowSolver* s)
+{
+  return guarded(h, [&] {
+    if (!s) return DFK_OK;
+    DeviceGuard guard(s->device);
+    delete s;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_solver_tiles(DfkHandle h, const DfkWindowSolver* s, size_t* tiles)
+{
+  return guarded(h, [&] {
+    if (!s || !tiles) return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] null argument");
+    *tiles = window_solver_tiles(s->dev);
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_solve(DfkHandle h, const DfkWindowSolver* s, const float* window_dev, const DfkWindowSolveParams* p,
+                           const double* codes, double* dx_dev, int32_t* info_dev)
+{
+  return guarded(h, [&] {
+    if (!s || !window_dev || !p || !dx_dev || !info_dev)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] null argument");
+    if (s->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] solver and handle live on different devices");
+    if (!(std::isfinite(p->lambda) && p->lambda >= 0.0))
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] lambda must be finite and >= 0");
+    if (!(std::isfinite(p->code_prior_weight) && p->code_prior_weight >= 0.0))
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] code_prior_weight must be finite and >= 0");
+    if (p->code_prior_weight > 0.0 && !codes)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] code_prior_weight > 0 needs the codes");
+    DeviceGuard guard(h->device);
+    DFK_CUDA(h, launch_window_solve(s->dev, window_dev, p->lambda, p->code_prior_weight, codes, dx_dev, info_dev,
+                                    h->stream, &h->launches),
+             "[WindowSolver] kernel launch failed");
+    return DFK_OK;
+  });
+}
+
+// ---------------------------------------------------------------------------------------------- window problem
+DfkStatus dfk_window_problem_create(DfkHandle h, const DfkWindowProblemDesc* d, DfkWindowProblem** out)
+{
+  return guarded(h, [&] {
+    const std::string what = "[WindowProblem] ";
+    if (!d || !out || !d->window) return fail(h, DFK_ERR_INVALID_ARG, what + "null argument");
+    *out = nullptr;
+    const DfkWindow* w = d->window;
+    if (w->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, what + "window and handle live on different devices");
+    const int K = w->dev.num_keyframes, F = w->dev.num_frames, C = w->dev.code_size, B = 6 + C, NP = K + F;
+    const int nd = d->num_dense, nr = d->num_reproj, ng = d->num_geo, ndep = d->num_depth, ne = d->num_error;
+    const int mf = d->num_frame_priors, nkm = (int)w->prior_kf.size();
+    if (nd < 0 || nr < 0 || ng < 0 || ndep < 0 || ne < 0 || mf < 0 || ne > 65535 || ndep > 65535)
+      return fail(h, DFK_ERR_INVALID_ARG, what + "negative item count / more than 65535 error or depth items");
+    if (nd + nr != w->dev.num_items || ng != w->dev.num_links)
+      return fail(h, DFK_ERR_INVALID_ARG, what + "the items do not match the window's records (" +
+                                              std::to_string(w->dev.num_items) + " records, " +
+                                              std::to_string(w->dev.num_links) + " links)");
+    if ((nd && (!d->dense || !d->dense_slots)) || (nr && (!d->reproj || !d->reproj_slots)) ||
+        (ng && (!d->geo || !d->geo_slots || !d->geo_records_dev)) || (ndep && (!d->depth || !d->depth_slots)) ||
+        (ne && (!d->error || !d->error_slots || !d->error_depth)) || !d->records_dev ||
+        (mf && (!d->frame_prior_kf || !d->frame_prior_rows || !d->frame_prior_x0)) ||
+        (w->kp.num_priors && (!d->kf_prior_rows || !d->kf_prior_x0)))
+      return fail(h, DFK_ERR_INVALID_ARG, what + "null argument");
+    // slots: pose slots name a keyframe or a frame, code slots a keyframe, an error item's depth slot a depth item.
+    // Every kind checks its fields in this order
+    enum { POSE0 = 1, POSE1 = 2, CODE0 = 4, CODE1 = 8, DEPTH = 16 };
+    const char* const field_name[5] = {"pose0", "pose1", "code0", "code1", "depth"};
+    const int field_end[5] = {NP, NP, K, K, ndep};
+    struct Kind {
+      const char* name;
+      const DfkWindowItemSlots* slots;
+      int n;
+      int fields;
+    };
+    const Kind kinds[] = {{"dense", d->dense_slots, nd, POSE0 | POSE1 | CODE0},
+                          {"reprojection", d->reproj_slots, nr, POSE0 | POSE1 | CODE0},
+                          {"geometric", d->geo_slots, ng, POSE0 | POSE1 | CODE0 | CODE1},
+                          {"depth", d->depth_slots, ndep, CODE0},
+                          {"error", d->error_slots, ne, POSE0 | POSE1 | DEPTH}};
+    for (const Kind& k : kinds)
+      for (int i = 0; i < k.n; ++i) {
+        const DfkWindowItemSlots& s = k.slots[i];
+        const int v[5] = {s.pose0, s.pose1, s.code0, s.code1, (k.fields & DEPTH) ? d->error_depth[i] : 0};
+        for (int f = 0; f < 5; ++f)
+          if ((k.fields >> f & 1) && !slot_ok(v[f], 0, field_end[f]))
+            return fail(h, DFK_ERR_INVALID_ARG, what + k.name + " item " + std::to_string(i) + ": " + field_name[f] +
+                                                    " slot out of range");
+      }
+    for (int i = 0; i < mf; ++i)
+      if (!slot_ok(d->frame_prior_kf[i], 0, K))
+        return fail(h, DFK_ERR_INVALID_ARG, what + "frame prior " + std::to_string(i) + " names a keyframe outside the window");
+    DeviceGuard guard(h->device);
+    std::unique_ptr<DfkWindowProblem> p(new (std::nothrow) DfkWindowProblem());
+    if (!p) return oom(h);
+    p->device = h->device; p->w = w;
+    p->K = K; p->F = F; p->C = C; p->B = B;
+    p->nd = nd; p->nr = nr; p->ng = ng; p->ndep = ndep; p->ne = ne; p->mf = mf; p->nkm = nkm;
+    p->S = (size_t)NP * 7 + (size_t)K * C;
+    p->avg_dpt = h->params.sfmparams.avg_dpt;
+    p->huber_delta = h->params.sfmparams.huber_delta;
+    p->records = d->records_dev; p->geo_records = d->geo_records_dev;
+    const char* amsg = "[WindowProblem] allocation failed";
+    const std::vector<float> zero_code(std::max(C, 1), 0.0f);
+    // ---- dense items: the batch's checks, kernel choice and tile plan, with a code slot of the problem's own each
+    if (nd > 0) {
+      std::vector<DfkSfmWorkItem> t(d->dense, d->dense + nd);
+      for (auto& it : t) it.code = zero_code.data();
+      DFK_TRY(choose_step_kernel(h, t.data(), nd, C, &p->step));
+      DFK_CUDA(h, p->dense_codes.ensure((size_t)nd * C), amsg);
+      std::vector<SfmItemDev> items(nd);
+      DFK_TRY(build_items(h, t.data(), nd, C, p->step.tile_px, p->step.max_ctas, p->dense_codes.ptr, items.data(),
+                          &p->plan));
+      // ray tables of its own, not the handle's cache: the cache may flush (and free) its tables
+      std::vector<const SfmItemDev*> owner;
+      for (auto& it : items) {
+        size_t r = 0;
+        for (; r < owner.size(); ++r) {
+          const SfmItemDev& o = *owner[r];
+          if (o.fx == it.fx && o.fy == it.fy && o.u0 == it.u0 && o.v0 == it.v0 && o.width == it.width &&
+              o.height == it.height)
+            break;
+        }
+        if (r == owner.size()) {
+          owner.push_back(&it);
+          p->rays.emplace_back();
+          DFK_CUDA(h, p->rays.back().ensure((size_t)it.width + it.height), amsg);
+        }
+        it.ray_tab = p->rays[r].ptr;
+      }
+      p->dense_tmpl = items;
+      DFK_CUDA(h, p->dense.ensure(nd), amsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->dense.ptr, items.data(), sizeof(SfmItemDev) * nd, cudaMemcpyHostToDevice, h->stream),
+               "[WindowProblem] upload failed");
+      DFK_CUDA(h, launch_sfm_ray_tables(p->dense.ptr, nd, h->stream), "[WindowProblem] kernel launch failed");
+      h->launches += 1;
+    }
+    // ---- sparse links: the batches' checks and staging, into blocks of the problem's own
+    if (nr > 0) {
+      std::vector<DfkReprojectionItem> t(d->reproj, d->reproj + nr);
+      for (auto& it : t) it.code = zero_code.data();
+      Staged st;
+      DFK_TRY(stage(h, what + "reprojection ", true, t.data(), nr, C, 0, p->rep_host, p->rep, &st));
+      p->rep_payload = st.payload;
+      p->rep_total = st.total;
+    }
+    if (ng > 0) {
+      std::vector<DfkSparseGeometricItem> t(d->geo, d->geo + ng);
+      for (auto& it : t) it.code0 = it.code1 = zero_code.data();
+      Staged st;
+      DFK_TRY(stage(h, what + "geometric ", true, t.data(), ng, C, 0, p->geo_host, p->geo, &st));
+      p->geo_payload = st.payload;
+    }
+    // ---- the error path: depth decodes into scratch of the problem's own, and the error items reading it
+    std::vector<size_t> dep_off(ndep + 1, 0);
+    for (int i = 0; i < ndep; ++i) {
+      const DfkDepthDecodeItem& it = d->depth[i];
+      const uint32_t W = it.dpt.width, H = it.dpt.height;
+      if (W == 0 || H == 0 || !img_ok(&it.prx_orig, W, H, 1) || !img_ok(&it.prx_jac, W, H, C))
+        return fail(h, DFK_ERR_INVALID_ARG, what + "inconsistent image views in depth item " + std::to_string(i));
+      dep_off[i + 1] = dep_off[i] + (((size_t)W * H + 3) & ~(size_t)3);
+    }
+    if (ndep > 0) {
+      DFK_CUDA(h, p->depth_scratch.ensure(dep_off[ndep]), amsg);
+      const size_t desc_bytes = (sizeof(DepthDecodeDesc) * (size_t)ndep + 15) & ~(size_t)15;
+      const size_t total = desc_bytes + sizeof(float) * (size_t)ndep * C;
+      DFK_CUDA(h, p->depth.ensure(total), amsg);
+      std::vector<unsigned char> hb(total, 0);
+      DepthDecodeDesc* descs = reinterpret_cast<DepthDecodeDesc*>(hb.data());
+      const float* codes_dev = reinterpret_cast<const float*>(p->depth.ptr + desc_bytes);
+      for (int i = 0; i < ndep; ++i) {
+        const DfkDepthDecodeItem& it = d->depth[i];
+        set_depth_decode_desc(descs[i], it, C, codes_dev + (size_t)i * C, p->depth_scratch.ptr + dep_off[i], it.dpt.width,
+                              &p->depth_max_blocks);
+      }
+      DFK_CUDA(h, cudaMemcpyAsync(p->depth.ptr, hb.data(), total, cudaMemcpyHostToDevice, h->stream),
+               "[WindowProblem] upload failed");
+    }
+    if (ne > 0) {
+      std::vector<EvalErrorDesc> descs(ne);
+      std::vector<double> areas(ne);
+      for (int i = 0; i < ne; ++i) {
+        const DfkSfmWorkItem& it = d->error[i];
+        const DfkDepthDecodeItem& dep = d->depth[d->error_depth[i]];
+        const DfkImage dpt{p->depth_scratch.ptr + dep_off[d->error_depth[i]], (size_t)dep.dpt.width * 4, dep.dpt.width,
+                           dep.dpt.height};
+        const uint32_t W = it.img0.width, H = it.img0.height;
+        if (it.code)
+          return fail(h, DFK_ERR_INVALID_ARG, what + "error item " + std::to_string(i) +
+                                                  ": no fused depth decode (the depth comes from its depth item)");
+        if (W == 0 || H == 0 || !img_ok(&it.img0, W, H, 1) || !img_ok(&it.img1, W, H, 1) || !img_ok(&dpt, W, H, 1))
+          return fail(h, DFK_ERR_INVALID_ARG, what + "inconsistent image views in error item " + std::to_string(i));
+        if (!cam_ok(&it.cam, W, H))
+          return fail(h, DFK_ERR_INVALID_ARG, what + "camera viewport larger than the image views in error item " +
+                                                  std::to_string(i));
+        const float ident[7] = {0, 0, 0, 1, 0, 0, 0};  // the repose kernel sets the relative pose
+        set_eval_error_desc(descs[i], it.cam, ident, it.img0, it.img1, dpt, &p->err_rows, &p->err_max_blocks);
+        areas[i] = (double)W * (double)H;
+      }
+      DFK_CUDA(h, p->err.ensure(ne), amsg);
+      DFK_CUDA(h, p->areas.ensure(ne), amsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->err.ptr, descs.data(), sizeof(EvalErrorDesc) * ne, cudaMemcpyHostToDevice, h->stream),
+               "[WindowProblem] upload failed");
+      DFK_CUDA(h, cudaMemcpyAsync(p->areas.ptr, areas.data(), sizeof(double) * ne, cudaMemcpyHostToDevice, h->stream),
+               "[WindowProblem] upload failed");
+      p->err_tmpl = descs;
+      p->areas_tmpl = areas;
+    }
+    DFK_CUDA(h, p->err_out.ensure(std::max<size_t>(1, 2 * (size_t)(ne + nr + ng))), amsg);
+    // ---- slots, in the repose kernel's order
+    std::vector<int4> slots;
+    auto push = [&](const DfkWindowItemSlots* s, int n) {
+      for (int i = 0; i < n; ++i) slots.push_back(make_int4(s[i].pose0, s[i].pose1, s[i].code0, s[i].code1));
+    };
+    push(d->dense_slots, nd); push(d->error_slots, ne); push(d->reproj_slots, nr); push(d->geo_slots, ng);
+    push(d->depth_slots, ndep);
+    p->slots_tmpl.assign(slots.begin(), slots.begin() + nd + ne);
+    if (!slots.empty()) {
+      DFK_CUDA(h, p->slots.ensure(slots.size()), amsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->slots.ptr, slots.data(), sizeof(int4) * slots.size(), cudaMemcpyHostToDevice,
+                                  h->stream),
+               "[WindowProblem] upload failed");
+    }
+    // ---- priors: rows, frozen points, the keyframe of every delta row, add_priors' lists
+    const size_t PD = DFK_PRIOR_DOUBLES(C), X = 7 + (size_t)C;
+    std::vector<int> dkf;
+    std::vector<double> x0;
+    if (mf > 0) {
+      DFK_CUDA(h, p->frows.ensure(mf * PD), amsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->frows.ptr, d->frame_prior_rows, sizeof(double) * mf * PD, cudaMemcpyHostToDevice,
+                                  h->stream),
+               "[WindowProblem] upload failed");
+      dkf.assign(d->frame_prior_kf, d->frame_prior_kf + mf);
+      x0.assign(d->frame_prior_x0, d->frame_prior_x0 + mf * X);
+      std::vector<int> lists;
+      add_csr(lists, K, mf, [&](int i) { return d->frame_prior_kf[i]; });
+      DFK_CUDA(h, p->fp_lists.ensure(lists.size()), amsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->fp_lists.ptr, lists.data(), sizeof(int) * lists.size(), cudaMemcpyHostToDevice,
+                                  h->stream),
+               "[WindowProblem] upload failed");
+    }
+    if (w->kp.num_priors > 0) {
+      const size_t kd = (size_t)w->prior_off.back();
+      DFK_CUDA(h, p->kfrows.ensure(kd), amsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->kfrows.ptr, d->kf_prior_rows, sizeof(double) * kd, cudaMemcpyHostToDevice, h->stream),
+               "[WindowProblem] upload failed");
+      dkf.insert(dkf.end(), w->prior_kf.begin(), w->prior_kf.end());
+      x0.insert(x0.end(), d->kf_prior_x0, d->kf_prior_x0 + nkm * X);
+    }
+    if (!dkf.empty()) {
+      DFK_CUDA(h, p->delta_kf.ensure(dkf.size()), amsg);
+      DFK_CUDA(h, p->x0.ensure(x0.size()), amsg);
+      DFK_CUDA(h, p->delta.ensure(dkf.size() * B), amsg);
+      DFK_CUDA(h, cudaMemcpyAsync(p->delta_kf.ptr, dkf.data(), sizeof(int) * dkf.size(), cudaMemcpyHostToDevice, h->stream),
+               "[WindowProblem] upload failed");
+      DFK_CUDA(h, cudaMemcpyAsync(p->x0.ptr, x0.data(), sizeof(double) * x0.size(), cudaMemcpyHostToDevice, h->stream),
+               "[WindowProblem] upload failed");
+    }
+    // ---- state (zero codes, identity poses until set_state), the gauge solver, the LM's small read-back block
+    DFK_CUDA(h, p->state.ensure(2 * p->S), amsg);
+    std::vector<double> init(2 * p->S, 0.0);
+    for (int s = 0; s < 2 * NP; ++s) init[(size_t)(s / NP) * p->S + (size_t)(s % NP) * 7 + 3] = 1.0;
+    DFK_CUDA(h, cudaMemcpyAsync(p->state.ptr, init.data(), sizeof(double) * init.size(), cudaMemcpyHostToDevice, h->stream),
+             "[WindowProblem] upload failed");
+    const std::vector<int> gauge{0, 1, 2, 3, 4, 5};
+    DFK_CUDA(h, window_solver_create(K, C, F, w->pair_k0, w->pair_k1, w->link_k0, w->link_k1, w->blk_i, w->blk_j,
+                                     w->kp.block_off, gauge, &p->solver[1]),
+             "[WindowProblem] solver workspace allocation failed");
+    DFK_CUDA(h, p->small.ensure(8 * sizeof(double) + 16), amsg);
+    DFK_CUDA(h, p->small_host.ensure(8 * sizeof(double) + 16), amsg);
+    DFK_CUDA(h, cudaStreamSynchronize(h->stream), "[WindowProblem] upload failed");  // the host staging is freed next
+    *out = p.release();
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_problem_destroy(DfkHandle h, DfkWindowProblem* p)
+{
+  return guarded(h, [&] {
+    if (!p) return DFK_OK;
+    DeviceGuard guard(p->device);
+    delete p;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_problem_set_state(DfkHandle h, DfkWindowProblem* p, const double* poses, const double* codes)
+{
+  return guarded(h, [&] {
+    if (!p || !poses || (!codes && p->K * p->C > 0)) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] null argument");
+    if (p->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] problem and handle live on different devices");
+    DeviceGuard guard(h->device);
+    const size_t np = (size_t)(p->K + p->F) * 7;
+    DFK_CUDA(h, cudaMemcpyAsync(p->st(p->cur), poses, sizeof(double) * np, cudaMemcpyDefault, h->stream),
+             "[WindowProblem] state copy failed");
+    if (p->K * p->C > 0)
+      DFK_CUDA(h, cudaMemcpyAsync(p->st(p->cur) + np, codes, sizeof(double) * (p->S - np), cudaMemcpyDefault, h->stream),
+               "[WindowProblem] state copy failed");
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_problem_get_state(DfkHandle h, const DfkWindowProblem* p, double* poses, double* codes)
+{
+  return guarded(h, [&] {
+    if (!p || !poses || (!codes && p->K * p->C > 0)) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] null argument");
+    if (p->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] problem and handle live on different devices");
+    DeviceGuard guard(h->device);
+    const size_t np = (size_t)(p->K + p->F) * 7;
+    DFK_CUDA(h, cudaMemcpyAsync(poses, p->st(p->cur), sizeof(double) * np, cudaMemcpyDefault, h->stream),
+             "[WindowProblem] state copy failed");
+    if (p->K * p->C > 0)
+      DFK_CUDA(h, cudaMemcpyAsync(codes, p->st(p->cur) + np, sizeof(double) * (p->S - np), cudaMemcpyDefault, h->stream),
+               "[WindowProblem] state copy failed");
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_problem_linearize(DfkHandle h, DfkWindowProblem* p, float* window_dev)
+{
+  return guarded(h, [&] {
+    if (!p || !window_dev) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem::linearize] null argument");
+    if (p->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] problem and handle live on different devices");
+    DeviceGuard guard(h->device);
+    return problem_linearize(h, p, p->st(p->cur), window_dev);
+  });
+}
+
+DfkStatus dfk_window_problem_error(DfkHandle h, DfkWindowProblem* p, double* out_dev)
+{
+  return guarded(h, [&] {
+    if (!p || !out_dev) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem::error] null argument");
+    if (p->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] problem and handle live on different devices");
+    DeviceGuard guard(h->device);
+    DFK_TRY(problem_error(h, p, p->st(p->cur), 0.0));
+    DFK_CUDA(h, cudaMemcpyAsync(out_dev, p->energy(), sizeof(double) * DFK_WINDOW_ERROR_DOUBLES, cudaMemcpyDeviceToDevice,
+                                h->stream),
+             "[WindowProblem::error] copy failed");
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_problem_retract(DfkHandle h, DfkWindowProblem* p, const double* dx_dev)
+{
+  return guarded(h, [&] {
+    if (!p || !dx_dev) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem::retract] null argument");
+    if (p->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] problem and handle live on different devices");
+    DeviceGuard guard(h->device);
+    // into the other state, which then becomes the problem's
+    DFK_CUDA(h, launch_window_retract(p->st(p->cur), p->st(1 - p->cur), dx_dev, p->K, p->F, p->C, h->stream),
+             "[WindowProblem::retract] kernel launch failed");
+    h->launches += 1;
+    p->cur = 1 - p->cur;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_lm(DfkHandle h, DfkWindowProblem* p, const DfkLMParams* prm, DfkLMTrace* tr)
+{
+  return guarded(h, [&] {
+    DeviceGuard guard(h->device);
+    ProblemLMOps ops;
+    DFK_TRY(lm_setup(h, p, prm, tr, "WindowLM", &ops));
+    return lm_run(*prm, ops, tr);
+  });
+}
+
+DfkStatus dfk_window_problem_set_active(DfkHandle h, DfkWindowProblem* p, const uint8_t* dense_active,
+                                        const uint8_t* error_active)
+{
+  return guarded(h, [&] {
+    const char* what = "[WindowProblem::set_active] ";
+    if (!p || (p->nd > 0 && !dense_active) || (!error_active && p->ne != p->nd))
+      return fail(h, DFK_ERR_INVALID_ARG, std::string(what) +
+                                              "null argument (error_active may be NULL only when num_error == num_dense)");
+    if (p->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] problem and handle live on different devices");
+    DeviceGuard guard(h->device);
+    return problem_set_active(h, p, dense_active, error_active ? error_active : dense_active);
+  });
+}
+
+DfkStatus dfk_window_lm_levels(DfkHandle h, DfkWindowProblem* p, const DfkLMParams* prm, const DfkLevelSchedule* sc,
+                               DfkLMTrace* tr, DfkLevelTrace* lt)
+{
+  return guarded(h, [&] {
+    const std::string what = "[WindowLMLevels] ";
+    if (!p || !sc) return fail(h, DFK_ERR_INVALID_ARG, what + "null argument");
+    const int nd = p->nd, ne = p->ne, L = sc->num_levels;
+    if (L < 1 || !sc->iters || (nd > 0 && !sc->dense_level) || sc->num_pairs < 0 ||
+        (sc->num_pairs > 0 && !sc->pair_steps_done))
+      return fail(h, DFK_ERR_INVALID_ARG, what + "num_levels < 1, or null iters / dense_level / pair_steps_done");
+    if (ne > 0 && ne != nd && (!sc->error_pair || !sc->error_level))
+      return fail(h, DFK_ERR_INVALID_ARG, what + "error_pair and error_level are required when num_error != num_dense");
+    for (int l = 0; l < L; ++l)
+      if (sc->iters[l] < 0) return fail(h, DFK_ERR_INVALID_ARG, what + "iters[" + std::to_string(l) + "] < 0");
+    // the schedule's pairs: the distinct window pairs of the dense items, in window order
+    std::vector<int> dpair(nd), ids;
+    for (int i = 0; i < nd; ++i) ids.push_back(p->w->item_pair[i]);
+    std::sort(ids.begin(), ids.end());
+    ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
+    if ((int)ids.size() != sc->num_pairs)
+      return fail(h, DFK_ERR_INVALID_ARG, what + "num_pairs " + std::to_string(sc->num_pairs) + ", but the dense items" +
+                                              " cover " + std::to_string(ids.size()) + " pairs");
+    for (int i = 0; i < nd; ++i)
+      dpair[i] = (int)(std::lower_bound(ids.begin(), ids.end(), p->w->item_pair[i]) - ids.begin());
+    for (int i = 0; i < nd; ++i)
+      if (sc->dense_level[i] < 0 || sc->dense_level[i] >= L)
+        return fail(h, DFK_ERR_INVALID_ARG, what + "dense item " + std::to_string(i) + ": level outside [0, num_levels)");
+    std::vector<int> epair(ne), elevel(ne);
+    for (int i = 0; i < ne; ++i) {
+      epair[i] = sc->error_pair ? sc->error_pair[i] : dpair[i];
+      elevel[i] = sc->error_level ? sc->error_level[i] : sc->dense_level[i];
+      if (epair[i] < 0 || epair[i] >= sc->num_pairs || elevel[i] < 0 || elevel[i] >= L)
+        return fail(h, DFK_ERR_INVALID_ARG, what + "error item " + std::to_string(i) +
+                                                ": pair or level out of range");
+    }
+    for (int q = 0; q < sc->num_pairs; ++q)
+      if (sc->pair_steps_done[q] < 0)
+        return fail(h, DFK_ERR_INVALID_ARG, what + "pair_steps_done[" + std::to_string(q) + "] < 0");
+    DeviceGuard guard(h->device);
+    struct LevelOps : ProblemLMOps {
+      const DfkLevelSchedule* sc;
+      const std::vector<int>* dpair;
+      const std::vector<int>* epair;
+      const std::vector<int>* elevel;
+      std::vector<uint8_t> dm, em;
+      DfkStatus set_levels(const int* lvl)
+      {
+        for (size_t i = 0; i < dm.size(); ++i) dm[i] = lvl[(*dpair)[i]] == sc->dense_level[i];
+        for (size_t i = 0; i < em.size(); ++i) em[i] = lvl[(*epair)[i]] == (*elevel)[i];
+        return problem_set_active(h, p, dm.data(), em.data());
+      }
+    } ops;
+    DFK_TRY(lm_setup(h, p, prm, tr, "WindowLMLevels", &ops));
+    ops.sc = sc;
+    ops.dpair = &dpair;
+    ops.epair = &epair;
+    ops.elevel = &elevel;
+    ops.dm.assign(nd, 1);
+    ops.em.assign(ne, 1);
+    return lm_levels_run(*prm, *sc, ops, tr, lt);
+  });
+}
+
+}  // extern "C"

@@ -6,7 +6,7 @@
 //   - a failed solve (info != 0) is a rejected step with nothing evaluated;
 //   - without use_error every candidate is linearised and its f is the linearisation's; with use_error the candidate's f
 //     is its error() and only the start point and accepted candidates are linearised.
-// `Ops` does the work (the device pipeline in dfk_api.cu, scripted values in the CPU test of this policy):
+// `Ops` does the work (the device pipeline in dfk_api_window.cu, scripted values in the CPU test of this policy):
 //   DfkStatus linearize(bool candidate)     linearise the accepted point (false) or the candidate (true)
 //   DfkStatus energy(bool candidate, double* f)  f of the point just linearised (use_error = 0) or its error() (1)
 //   DfkStatus solve(double lambda, int* info)    the damped step at the accepted point

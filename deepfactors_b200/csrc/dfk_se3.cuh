@@ -1,5 +1,5 @@
 // dfk_se3.cuh -- the fp32 relative pose of a work item (warping.h:98-137), one implementation for the host staging of
-// every batch (dfk_api.cu) and the device re-posing of a window problem (dfk_window_lm.cu).  Both must give the same
+// every batch (dfk_api.cu, dfk_host.h) and the device re-posing of a window problem (dfk_window_lm.cu).  Both must give the same
 // bits: on the device every product and sum is an explicitly rounded __fmul_rn / __fadd_rn / __fsub_rn, so nvcc cannot
 // contract a pair into an FMA; the host compiler targets x86-64 without FMA and does not reassociate, so the plain
 // operators there round each operation once in the same order.
