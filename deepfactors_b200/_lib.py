@@ -155,6 +155,13 @@ class DfkOrbItem(C.Structure):
 
 
 ORB_MAX_SIDE = 16384  # DFK_ORB_MAX_SIDE
+PREPROCESS_MAX_LEVELS = 15  # DFK_PREPROCESS_MAX_LEVELS
+
+
+class DfkPreprocessItem(C.Structure):
+    _fields_ = [("src", DfkImage), ("src_cam", DfkCamera), ("out_cam", DfkCamera), ("color", DfkImage),
+                ("gray", DfkImage), ("levels", C.POINTER(DfkImage)), ("grads", C.POINTER(DfkImage)),
+                ("normalize", C.c_int32)]
 
 WINDOW_ERROR_DOUBLES = 7  # DFK_WINDOW_ERROR_DOUBLES
 
@@ -256,6 +263,7 @@ SYMBOLS = {
     "dfk_gaussian_blur_down": (C.c_int, [_H, _IMG, _IMG]),
     "dfk_build_image_pyramid": (C.c_int, [_H, _IMG, _IMG, C.c_int]),
     "dfk_squared_error": (C.c_int, [_H, _IMG, _IMG, _F]),
+    "dfk_preprocess_batch": (C.c_int, [_H, C.POINTER(DfkPreprocessItem), C.c_int, C.c_int, C.c_void_p]),
 }
 
 _lib = None

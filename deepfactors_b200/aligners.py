@@ -631,6 +631,89 @@ def OrbDetectBatch(aligner, images: Sequence[torch.Tensor], nfeatures: int = REP
     return OrbBatch(kp[:rows], desc[:rows], ang[:rows], resp[:rows], counts[:n], offsets, np.array(cap, np.int64))
 
 
+# ------------------------------------------------------------------------------------------- frame preprocessing
+def resize_viewport(cam, w: int, h: int):
+    """PinholeCamera::ResizeViewport (pinhole_camera_impl.h:126-136) in the reference's fp32 arithmetic: the camera of a
+    frame of w x h pixels (orig_cam_ in PreprocessImage, deepfactors.cpp:638)"""
+    from .synth import Camera
+    return Camera(cam.fx, cam.fy, cam.u0, cam.v0, cam.width, cam.height).resized(int(w), int(h))
+
+
+@dataclass
+class PreprocessedFrame:
+    """One frame's output of PreprocessBatch, device tensors: color uint8 [H_o, W_o, 3] (kf->color_img) and gray uint8
+    [H_o, W_o] (OrbDetectBatch's image), or None when not asked for; levels float32 [h_l, w_l] (level 0 = f, or f'
+    when normalised) and grads float32 [h_l, w_l, 2] (or None); stats float64 [2] = (mu, sigma) of a normalised
+    frame, else None."""
+    color: torch.Tensor | None
+    gray: torch.Tensor | None
+    levels: list
+    grads: list | None
+    stats: torch.Tensor | None
+
+
+def _frame_view(t: torch.Tensor) -> DfkImage:
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.uint8:
+        raise TypeError("PreprocessBatch: frames must be uint8 CUDA tensors")
+    if t.dim() != 3 or t.shape[2] != 3 or t.stride(2) != 1 or t.stride(1) != 3:
+        raise ValueError("PreprocessBatch: a frame must be [H, W, 3] with interleaved contiguous pixels")
+    return DfkImage(C.c_void_p(t.data_ptr()), int(t.stride(0)), int(t.shape[1]), int(t.shape[0]))
+
+
+def pyramid_sizes(w: int, h: int, num_levels: int) -> list:
+    """(w, h) of each level: integer halving (camera_pyramid.h:43-44)"""
+    sizes = [(int(w), int(h))]
+    for _ in range(1, num_levels):
+        sizes.append((sizes[-1][0] // 2, sizes[-1][1] // 2))
+    return sizes[:num_levels]
+
+
+def PreprocessBatch(aligner, frames: Sequence[torch.Tensor], src_cams, out_cam, num_levels: int,
+                    normalize=False, color: bool = True, gray: bool = True, grads: bool = True) -> list:
+    """DeepFactors::PreprocessImage and the frame's image pyramid for many camera frames in one call
+    (dfk_preprocess_batch): the remap to out_cam, the gray and float conversion bit for bit cv::remap / cv::cvtColor /
+    convertTo, optionally the normalisation, then num_levels levels by GaussianBlurDown and their Sobel gradients.
+    frames: uint8 [H, W, 3] CUDA tensors of any sizes; src_cams: the camera of each frame at its size (one for all, or
+    one per frame; resize_viewport gives it); out_cam: the network camera, whose width x height is the output size;
+    normalize: one bool for all frames or one per frame.  Asynchronous: returns one PreprocessedFrame per frame."""
+    hd = aligner._hd
+    hd.use_torch_stream()
+    n = len(frames)
+    cams = list(src_cams) if isinstance(src_cams, (list, tuple)) else [src_cams] * n
+    norm = [bool(x) for x in normalize] if isinstance(normalize, (list, tuple, np.ndarray)) else [bool(normalize)] * n
+    if len(cams) != n or len(norm) != n:
+        raise ValueError("PreprocessBatch: per-frame settings need one entry per frame")
+    W, H = int(out_cam.width), int(out_cam.height)
+    if W != out_cam.width or H != out_cam.height or W < 1 or H < 1:
+        raise ValueError("PreprocessBatch: the output camera's size must be whole numbers >= 1")
+    dev = torch.device("cuda", hd.device)
+    for f in frames:
+        if f.device != dev:
+            raise ValueError(f"PreprocessBatch: frames must be on cuda:{hd.device}")
+    sizes = pyramid_sizes(W, H, num_levels)
+    stats = torch.zeros((max(n, 1), 2), dtype=torch.float64, device=dev) if any(norm) else None
+    out, items, keep = [], [], []
+    for i, f in enumerate(frames):
+        col = torch.empty((H, W, 3), dtype=torch.uint8, device=dev) if color else None
+        gr = torch.empty((H, W), dtype=torch.uint8, device=dev) if gray else None
+        lv = [torch.empty((h, w), dtype=torch.float32, device=dev) for w, h in sizes]
+        gd = [torch.empty((h, w, 2), dtype=torch.float32, device=dev) for w, h in sizes] if grads else None
+        la = (DfkImage * max(num_levels, 1))(*[_image(t) for t in lv])
+        ga = (DfkImage * max(num_levels, 1))(*[_image(t, 2) for t in gd]) if grads else None
+        keep += [la, ga]
+        items.append(_lib.DfkPreprocessItem(
+            _frame_view(f), _cam(cams[i]), _cam(out_cam),
+            DfkImage(C.c_void_p(col.data_ptr()), 3 * W, W, H) if color else DfkImage(),
+            DfkImage(C.c_void_p(gr.data_ptr()), W, W, H) if gray else DfkImage(),
+            C.cast(la, C.POINTER(DfkImage)) if num_levels > 0 else None,
+            C.cast(ga, C.POINTER(DfkImage)) if grads and num_levels > 0 else None, int(norm[i])))
+        out.append(PreprocessedFrame(col, gr, lv, gd, stats[i] if norm[i] else None))
+    arr = (_lib.DfkPreprocessItem * max(n, 1))(*items)
+    check(hd.h, lib().dfk_preprocess_batch(hd.h, arr, n, int(num_levels),
+                                           C.c_void_p(stats.data_ptr()) if stats is not None else None))
+    return out
+
+
 def SparseGeometricErrorBatch(aligner, items, out: torch.Tensor | None = None) -> torch.Tensor:
     """SparseGeometricFactor::error of many factors in one launch (dfk_sparse_geometric_error_batch): the items of
     SparseGeometricLinearizeBatch (dicts, or the array of make_geometric_items).  Asynchronous: returns a device tensor [n, 2] float32, row i = [b^T b | valid points

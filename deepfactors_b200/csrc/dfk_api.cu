@@ -965,6 +965,137 @@ DfkStatus dfk_squared_error(DfkHandle h, const DfkImage* a, const DfkImage* b, f
   });
 }
 
+static bool pp_cam_ok(const DfkCamera& c)
+{
+  return std::isfinite(c.fx) && std::isfinite(c.fy) && std::isfinite(c.u0) && std::isfinite(c.v0) && c.fx != 0.0f &&
+         c.fy != 0.0f;
+}
+
+// a uint8 view of w x h pixels with `channels` bytes each
+static bool pp_u8_ok(const DfkImage& im, uint32_t w, uint32_t h, uint32_t channels)
+{
+  return im.ptr && im.width == w && im.height == h && im.pitch_bytes >= (size_t)w * channels;
+}
+
+DfkStatus dfk_preprocess_batch(DfkHandle h, const DfkPreprocessItem* items, int n, int num_levels, double* stats_dev)
+{
+  return guarded(h, [&] {
+    const std::string w = "[PreprocessImage batch] ";
+    if (!items || n < 1 || n > 65535)  // gridDim.y / gridDim.z of the kernels is the item
+      return fail(h, DFK_ERR_INVALID_ARG, w + "null argument / number of items not in [1, 65535]");
+    if (num_levels < 0 || num_levels > DFK_PREPROCESS_MAX_LEVELS)
+      return fail(h, DFK_ERR_INVALID_ARG, w + "number of levels not in [0, DFK_PREPROCESS_MAX_LEVELS]");
+    if ((uintptr_t)stats_dev & 7) return fail(h, DFK_ERR_INVALID_ARG, w + "stats_dev must be 8-byte aligned");
+    const int L = num_levels;
+    // [item descriptors n | level descriptors L x n (level-major)], 16-byte parts
+    const size_t b_items = (sizeof(PpItemDev) * (size_t)n + 15) & ~(size_t)15;
+    h->pp_host.assign(b_items + sizeof(PyrLevelDev) * (size_t)L * n, 0);
+    PpItemDev* pp = reinterpret_cast<PpItemDev*>(h->pp_host.data());
+    PyrLevelDev* lv = reinterpret_cast<PyrLevelDev*>(h->pp_host.data() + b_items);
+    std::vector<int> max_w((size_t)L, 0), max_h((size_t)L, 0);
+    long long partials = 0;
+    int max_tiles = 0;
+    bool any_norm = false, any_grad = false;
+    for (int i = 0; i < n; ++i) {
+      const DfkPreprocessItem& it = items[i];
+      const std::string at = " in item " + std::to_string(i);
+      const DfkImage& s = it.src;
+      if (!s.ptr || s.width < 1 || s.height < 1 || s.width > DFK_ORB_MAX_SIDE || s.height > DFK_ORB_MAX_SIDE ||
+          s.pitch_bytes < 3 * (size_t)s.width)
+        return fail(h, DFK_ERR_INVALID_ARG, w + "source needs a pointer, width and height in [1, DFK_ORB_MAX_SIDE] and "
+                                                "pitch_bytes >= 3 width" + at);
+      if (!pp_cam_ok(it.src_cam) || !pp_cam_ok(it.out_cam))
+        return fail(h, DFK_ERR_INVALID_ARG, w + "camera intrinsics must be finite, with fx and fy != 0" + at);
+      const float cw = it.out_cam.width, ch = it.out_cam.height;
+      if (!(cw >= 1.0f && ch >= 1.0f && cw <= (float)DFK_ORB_MAX_SIDE && ch <= (float)DFK_ORB_MAX_SIDE) ||
+          cw != std::floor(cw) || ch != std::floor(ch))
+        return fail(h, DFK_ERR_INVALID_ARG, w + "output camera size must be whole numbers in [1, DFK_ORB_MAX_SIDE]" + at);
+      const uint32_t W = (uint32_t)cw, H = (uint32_t)ch;
+      if (it.color.ptr && !pp_u8_ok(it.color, W, H, 3))
+        return fail(h, DFK_ERR_INVALID_ARG, w + "color view is not W_o x H_o with pitch_bytes >= 3 W_o" + at);
+      if (it.gray.ptr && !pp_u8_ok(it.gray, W, H, 1))
+        return fail(h, DFK_ERR_INVALID_ARG, w + "gray view is not W_o x H_o with pitch_bytes >= W_o" + at);
+      if (it.normalize != 0 && it.normalize != 1) return fail(h, DFK_ERR_INVALID_ARG, w + "normalize not 0 or 1" + at);
+      if (L > 0 && !it.levels) return fail(h, DFK_ERR_INVALID_ARG, w + "null levels" + at);
+      uint32_t lw = W, lh = H;
+      for (int l = 0; l < L; ++l) {
+        if (l > 0) {
+          lw /= 2;
+          lh /= 2;
+        }
+        const std::string atl = " at level " + std::to_string(l) + at;
+        if (lw < 1 || lh < 1) return fail(h, DFK_ERR_INVALID_ARG, w + "level smaller than 1 x 1" + atl);
+        if (!img_ok(&it.levels[l], lw, lh, 1))
+          return fail(h, DFK_ERR_INVALID_ARG, w + "level view is not the halved size or not a float view" + atl);
+        if (it.grads && !img_ok(&it.grads[l], lw, lh, 2))
+          return fail(h, DFK_ERR_INVALID_ARG, w + "gradient view does not match its level" + atl);
+        PyrLevelDev& d = lv[(size_t)l * n + i];
+        d.img = static_cast<float*>(it.levels[l].ptr);
+        d.pitch = (uint32_t)(it.levels[l].pitch_bytes / 4);
+        d.w = (int)lw;
+        d.h = (int)lh;
+        d.grad = it.grads ? static_cast<float*>(it.grads[l].ptr) : nullptr;
+        d.grad_pitch = it.grads ? (uint32_t)(it.grads[l].pitch_bytes / 4) : 0u;
+        max_w[l] = std::max(max_w[l], (int)lw);
+        max_h[l] = std::max(max_h[l], (int)lh);
+      }
+      any_grad = any_grad || (L > 0 && it.grads);
+      PpItemDev& d = pp[i];
+      dfk_pm_map_init(&d.map, it.src_cam.fx, it.src_cam.fy, it.src_cam.u0, it.src_cam.v0, it.out_cam.fx,
+                      it.out_cam.fy, it.out_cam.u0, it.out_cam.v0);
+      d.src = static_cast<const uint8_t*>(s.ptr);
+      d.src_pitch = s.pitch_bytes;
+      d.sw = (int)s.width;
+      d.sh = (int)s.height;
+      d.w = (int)W;
+      d.h = (int)H;
+      d.tiles_x = (int)((W + DFK_PM_TILE_W - 1) / DFK_PM_TILE_W);
+      d.tiles = d.tiles_x * (int)((H + DFK_PM_TILE_H - 1) / DFK_PM_TILE_H);
+      d.color = static_cast<uint8_t*>(it.color.ptr);
+      d.color_pitch = it.color.pitch_bytes;
+      d.gray = static_cast<uint8_t*>(it.gray.ptr);
+      d.gray_pitch = it.gray.pitch_bytes;
+      d.level0 = L > 0 ? static_cast<float*>(it.levels[0].ptr) : nullptr;
+      d.level0_pitch = L > 0 ? (uint32_t)(it.levels[0].pitch_bytes / 4) : 0u;
+      d.normalize = it.normalize;
+      d.partial_begin = (int)std::min(partials, (long long)INT32_MAX);
+      d.stats = (it.normalize && stats_dev) ? stats_dev + 2 * (size_t)i : nullptr;
+      if (it.normalize) partials += d.tiles;
+      any_norm = any_norm || it.normalize;
+      max_tiles = std::max(max_tiles, d.tiles);
+    }
+    if (partials > INT32_MAX)
+      return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 tiles of normalising items in one call");
+    DeviceGuard guard(h->device);
+    DFK_CUDA(h, h->pp_dev.ensure(h->pp_host.size()), "[PreprocessImage batch] scratch allocation failed");
+    // [tile partials 2 each | moments 2 per item]
+    DFK_CUDA(h, h->pp_partials.ensure(2 * (size_t)partials + 2 * (size_t)n),
+             "[PreprocessImage batch] scratch allocation failed");
+    for (int i = 0; i < n; ++i) pp[i].moments = h->pp_partials.ptr + 2 * (size_t)partials + 2 * (size_t)i;
+    DFK_CUDA(h, cudaMemcpyAsync(h->pp_dev.ptr, h->pp_host.data(), h->pp_host.size(), cudaMemcpyHostToDevice, h->stream),
+             "[PreprocessImage batch] upload failed");
+    const PyrLevelDev* lv_dev = reinterpret_cast<const PyrLevelDev*>(h->pp_dev.ptr + b_items);
+    DFK_CUDA(h, launch_preprocess(reinterpret_cast<const PpItemDev*>(h->pp_dev.ptr), n, max_tiles, any_norm,
+                                  h->pp_partials.ptr, h->stream),
+             "[PreprocessImage batch] kernel launch failed");
+    h->launches += any_norm ? 3 : 1;
+    for (int l = 1; l < L; ++l) {
+      DFK_CUDA(h, launch_blur_down_batch(lv_dev + (size_t)(l - 1) * n, lv_dev + (size_t)l * n, n, max_w[l], max_h[l],
+                                         h->stream),
+               "Kernel launch failed (kernel_gaussian_blur_down)");
+      h->launches += 1;
+    }
+    if (any_grad) {
+      for (int l = 0; l < L; ++l) {
+        DFK_CUDA(h, launch_sobel_batch(lv_dev + (size_t)l * n, n, max_w[l], max_h[l], h->stream),
+                 "Kernel launch failed (kernel_sobel_gradients)");
+        h->launches += 1;
+      }
+    }
+    return DFK_OK;
+  });
+}
+
 // ---------------------------------------------------------------------------------------------- streaming from host
 DfkStatus dfk_sfm_stream_create(DfkHandle h, int code_size, int max_items, size_t max_bytes, int depth, DfkSfmStream** out)
 {

@@ -111,6 +111,11 @@ struct DfkContext {
   DeviceBuf<OrbItemDev> orb_items;
   std::vector<OrbItemDev> orb_host;
   DeviceBuf<unsigned char> orb_scratch;
+  // dfk_preprocess_batch: [item descriptors | pyramid level descriptors L x n] (bytes, one H2D per call from pp_host)
+  // and the normalising items' tile partials
+  DeviceBuf<unsigned char> pp_dev;
+  std::vector<unsigned char> pp_host;
+  DeviceBuf<double> pp_partials;
   // dfk_window_marginalize_frames / dfk_window_add_priors: the call's index lists (one pageable H2D per call)
   DeviceBuf<int> window_lists;
   // dfk_window_marginalize_keyframe: the call's lists [refs | tile rows / cols | member locations | update tasks] (one

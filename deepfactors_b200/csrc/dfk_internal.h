@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "dfk.h"
+#include "dfk_preprocess_model.h"
 
 namespace dfk {
 
@@ -476,6 +477,44 @@ cudaError_t launch_orb_detect(const OrbItemDev* items_dev, int n, const OrbScrat
                               int max_corner_cap, int max_segs, int max_capacity, int max_nfeatures,
                               float* keypoints, uint8_t* descriptors, float* angles, float* responses, int* counts,
                               cudaStream_t stream);
+
+// one frame of dfk_preprocess_batch (dfk_preprocess.cu): the output (w x h) is cut into tiles of DFK_PM_TILE_W x
+// DFK_PM_TILE_H pixels, one CTA each; pitches in bytes for the uint8 images, in floats for level 0
+struct PpItemDev {
+  DfkPmMap map;
+  const uint8_t* src;
+  size_t src_pitch;
+  int sw, sh;             // source size
+  int w, h;               // output size
+  int tiles_x, tiles;
+  uint8_t* color;         // null: not wanted
+  size_t color_pitch;
+  uint8_t* gray;          // null: not wanted
+  size_t gray_pitch;
+  float* level0;          // null: no levels
+  uint32_t level0_pitch;
+  int normalize;
+  int partial_begin;      // a normalising item's first tile partial (2 doubles each)
+  double* moments;        // (mu, sigma) of a normalising item in scratch
+  double* stats;          // the caller's stats row of a normalising item, or null
+};
+// grid (max_tiles, n); normalize: some item normalises (two more launches: the statistics, one CTA per item, then
+// level 0 rewritten as f')
+cudaError_t launch_preprocess(const PpItemDev* items_dev, int n, int max_tiles, bool normalize, double* partials,
+                              cudaStream_t s);
+// one level of one frame of a batched pyramid (dfk_simple.cu); pitches in floats, grad null: no gradient
+struct PyrLevelDev {
+  float* img;
+  uint32_t pitch;
+  int w, h;
+  float* grad;
+  uint32_t grad_pitch;
+};
+// out[i] = GaussianBlurDown(in[i]) and grad of lv[i] = SobelGradients(img of lv[i]) for the n frames of a level, bit for
+// bit launch_blur_down / launch_sobel on each frame alone; grid (max tiles x, max tiles y, n)
+cudaError_t launch_blur_down_batch(const PyrLevelDev* in_dev, const PyrLevelDev* out_dev, int n, int max_out_w,
+                                   int max_out_h, cudaStream_t s);
+cudaError_t launch_sobel_batch(const PyrLevelDev* lv_dev, int n, int max_w, int max_h, cudaStream_t s);
 
 constexpr int kSimpleMaxBlocks = 1024;
 constexpr int kSimpleScratchFloats = kSimpleMaxBlocks * 32;

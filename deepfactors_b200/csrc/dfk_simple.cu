@@ -440,12 +440,10 @@ update_depth_batch_kernel(const DepthDecodeDesc* __restrict__ descs, int code_si
 // ------------------------------------------------------------------------------ Sobel
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); }
 
-__global__ void __launch_bounds__(kThreads)
-sobel_kernel(int width, int height, View img, float* __restrict__ grad, uint32_t grad_pitch)
+// pixel (x, y) of SobelGradients; shared by the single and the batched kernel
+__device__ __forceinline__ void sobel_pixel(int x, int y, int width, int height, View img, float* __restrict__ grad,
+                                            uint32_t grad_pitch)
 {
-  const int x = blockIdx.x * 32 + (threadIdx.x & 31);
-  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
-  if (x >= width || y >= height) return;
   float p[3][3];
 #pragma unroll
   for (int py = -1; py <= 1; ++py)
@@ -467,13 +465,30 @@ sobel_kernel(int width, int height, View img, float* __restrict__ grad, uint32_t
   grad[(size_t)y * grad_pitch + 2 * x + 1] = sdy * 0.125f;
 }
 
-// ------------------------------------------------------------------------------ blur-down
 __global__ void __launch_bounds__(kThreads)
-blur_down_kernel(int in_w, int in_h, View in, int out_w, int out_h, float* __restrict__ out, uint32_t out_pitch)
+sobel_kernel(int width, int height, View img, float* __restrict__ grad, uint32_t grad_pitch)
 {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31);
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
-  if (x >= out_w || y >= out_h) return;
+  if (x >= width || y >= height) return;
+  sobel_pixel(x, y, width, height, img, grad, grad_pitch);
+}
+
+// the frames of one pyramid level, frame blockIdx.z; a frame without a gradient view returns
+__global__ void __launch_bounds__(kThreads) sobel_batch_kernel(const PyrLevelDev* __restrict__ lv)
+{
+  const PyrLevelDev d = lv[blockIdx.z];
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31);
+  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (!d.grad || x >= d.w || y >= d.h) return;
+  sobel_pixel(x, y, d.w, d.h, View{d.img, d.pitch}, d.grad, d.grad_pitch);
+}
+
+// ------------------------------------------------------------------------------ blur-down
+// output pixel (x, y) of GaussianBlurDown; shared by the single and the batched kernel
+__device__ __forceinline__ void blur_down_pixel(int x, int y, int in_w, int in_h, View in, float* __restrict__ out,
+                                                uint32_t out_pitch)
+{
   const float k1[5] = {1.f, 4.f, 6.f, 4.f, 1.f};
   float sum = 0.0f;
 #pragma unroll
@@ -486,6 +501,26 @@ blur_down_kernel(int in_w, int in_h, View in, int out_w, int out_h, float* __res
     }
   }
   out[(size_t)y * out_pitch + x] = sum * (1.0f / 256.0f);  // wall == 256 exactly
+}
+
+__global__ void __launch_bounds__(kThreads)
+blur_down_kernel(int in_w, int in_h, View in, int out_w, int out_h, float* __restrict__ out, uint32_t out_pitch)
+{
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31);
+  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= out_w || y >= out_h) return;
+  blur_down_pixel(x, y, in_w, in_h, in, out, out_pitch);
+}
+
+// out[z] = GaussianBlurDown(in[z]) for the frames of one pyramid level, frame blockIdx.z
+__global__ void __launch_bounds__(kThreads)
+blur_down_batch_kernel(const PyrLevelDev* __restrict__ in, const PyrLevelDev* __restrict__ out)
+{
+  const PyrLevelDev a = in[blockIdx.z], b = out[blockIdx.z];
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31);
+  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= b.w || y >= b.h) return;
+  blur_down_pixel(x, y, a.w, a.h, View{a.img, a.pitch}, b.img, b.pitch);
 }
 
 inline int grid_for(int area)
@@ -627,6 +662,21 @@ cudaError_t launch_blur_down(int in_w, int in_h, View in, int out_w, int out_h, 
 {
   dim3 grid((out_w + 31) / 32, (out_h + 7) / 8);
   blur_down_kernel<<<grid, kThreads, 0, s>>>(in_w, in_h, in, out_w, out_h, out, out_pitch);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_blur_down_batch(const PyrLevelDev* in_dev, const PyrLevelDev* out_dev, int n, int max_out_w,
+                                   int max_out_h, cudaStream_t s)
+{
+  const dim3 grid((max_out_w + 31) / 32, (max_out_h + 7) / 8, (unsigned)n);
+  blur_down_batch_kernel<<<grid, kThreads, 0, s>>>(in_dev, out_dev);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_sobel_batch(const PyrLevelDev* lv_dev, int n, int max_w, int max_h, cudaStream_t s)
+{
+  const dim3 grid((max_w + 31) / 32, (max_h + 7) / 8, (unsigned)n);
+  sobel_batch_kernel<<<grid, kThreads, 0, s>>>(lv_dev);
   return cudaGetLastError();
 }
 

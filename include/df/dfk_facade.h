@@ -87,6 +87,8 @@ inline DfkCamera Cam(const CamT& cam)
   return DfkCamera{static_cast<float>(cam.fx()), static_cast<float>(cam.fy()), static_cast<float>(cam.u0()),
                    static_cast<float>(cam.v0()), static_cast<float>(cam.width()), static_cast<float>(cam.height())};
 }
+// a DfkCamera passes through as it is
+inline DfkCamera Cam(const DfkCamera& cam) { return cam; }
 
 struct HandleDeleter {
   void operator()(DfkContext* h) const { dfk_destroy(h); }

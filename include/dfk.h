@@ -726,6 +726,65 @@ DfkStatus dfk_build_image_pyramid(DfkHandle h, const DfkImage* imgs, const DfkIm
 /* df::SquaredError (cu_image_proc.h:35-39, cu_image_proc.cpp:190-242). Synchronous. */
 DfkStatus dfk_squared_error(DfkHandle h, const DfkImage* a, const DfkImage* b, float* out);
 
+/* ------------------------------------------------------------------ camera frame preprocessing */
+
+/* One camera frame of dfk_preprocess_batch: DeepFactors::PreprocessImage (core/deepfactors.cpp:634-680) and the image
+ * pyramid of UploadLiveFrame / Frame::FillPyramids / Mapper::BuildKeyframe (deepfactors.cpp:616-630, mapper.cpp:935-949)
+ * for one frame. */
+typedef struct {
+  DfkImage src;           /* DEVICE uint8 x 3 interleaved camera frame, width x height in pixels, both in
+                             [1, DFK_ORB_MAX_SIDE], pitch_bytes >= 3 * width */
+  DfkCamera src_cam;      /* the camera at the source's size (orig_cam_ after ResizeViewport(cols, rows)); fx, fy
+                             finite and != 0, u0, v0 finite; its width and height are not used */
+  DfkCamera out_cam;      /* the network camera (netcfg_.camera); fx, fy finite and != 0, u0, v0 finite; width x height
+                             (whole numbers in [1, DFK_ORB_MAX_SIDE]) is the output size W_o x H_o */
+  DfkImage color;         /* out: DEVICE uint8 x 3, W_o x H_o, pitch_bytes >= 3 W_o (kf->color_img); ptr NULL: not
+                             wanted */
+  DfkImage gray;          /* out: DEVICE uint8, W_o x H_o, pitch_bytes >= W_o; ptr NULL: not wanted.  DfkOrbItem.image
+                             takes it as it is */
+  const DfkImage* levels; /* HOST array of num_levels DEVICE float views: level 0 is W_o x H_o, level l is
+                             (W_{l-1} / 2) x (H_{l-1} / 2) (integer halving, at least 1 x 1); NULL when num_levels = 0 */
+  const DfkImage* grads;  /* HOST array of num_levels DEVICE 2-float views of the levels' sizes, or NULL: no gradients */
+  int32_t normalize;      /* 1: normalise level 0 by the frame's mean and standard deviation (opts_.normalize_image);
+                             0: off (the reference's default) */
+} DfkPreprocessItem;
+
+/* For every item, each output pixel (j, r) of W_o x H_o (DESIGN.md section 4.10):
+ *   1. map       cv::initUndistortRectifyMap(K_in, no distortion, I, K_out, size, CV_32FC1) (deepfactors.cpp:641-645), fp64
+ *                without FMA contraction: K_in, K_out the pinhole matrices of src_cam and out_cam (fp32 widened),
+ *                iR = K_out^-1 as cv::Mat::inv(DECOMP_LU) gives it for 3 x 3 (1 / det3 times the adjugate);
+ *                x = (r iR01 + iR02) + j iR00, y = (r iR11 + iR12) + j iR10, w = (r iR21 + iR22) + j iR20,
+ *                u = (float)(fx_in (x (1 / w)) + u0_in), v = (float)(fy_in (y (1 / w)) + v0_in).
+ *   2. fixed     X = rint(u * 32) (fp32 product, half to even, saturated to int), x0 = X >> 5, tx = X & 31; same for Y.
+ *   3. weights   cv::remap's INTER_LINEAR table: f = t (1 / 32.f), (1 - f, f) per axis in fp32; tap (dy, dx) in the
+ *                order (0,0), (0,1), (1,0), (1,1) weighs rint((float)(wy_dy wx_dx) 32768); a sum != 32768 would be
+ *                fixed on the first largest (sum < 32768) or first smallest tap (it never is, for bilinear).
+ *   4. colour    cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) (deepfactors.cpp:648-650): per channel s = sum_k w_k
+ *                src(x0 + dx, y0 + dy), a tap outside the source reads 0, out = clamp((s + 2^14) >> 15, 0, 255).
+ *   5. gray      cv::cvtColor(COLOR_RGB2GRAY) on 8U (:653-654): g = (9798 c0 + 19235 c1 + 3735 c2 + 2^14) >> 15.
+ *                Channel 0 takes the R weight, as the reference calls it, whatever order the camera delivers.
+ *   6. float     convertTo(CV_32FC1, 1 / 255.0) (:657-658): f = (float)g * (float)(1 / 255.0).
+ *   7. normalise (normalize = 1; :660-665) mu = S1 / N, sigma = sqrt(max(S2 / N - mu^2, 0)), N = W_o H_o, S1 and S2
+ *                the fp64 sums of f and f^2 in a fixed order (32 x 8 pixel tiles in row-major order, a pairwise tree of
+ *                256 within a tile, the tile sums strided over 256 and the same tree); level 0 = (float)((f - mu) /
+ *                sigma).  cv::meanStdDev's own summation order is not reproducible, so mu and sigma agree with it to
+ *                1e-12 relative (the bound the tests check), not bit for bit.  sigma = 0 (a constant frame) is not
+ *                guarded, as in the reference: level 0 is then +-inf, or NaN where f = mu.
+ *   8. pyramid   levels[0] = f (or f'), levels[l] = GaussianBlurDown(levels[l-1]), grads[l] = SobelGradients(levels[l])
+ *                for every level, level 0 included (UploadLiveFrame skips it; dfk_build_image_pyramid does not); each
+ *                bit for bit dfk_gaussian_blur_down / dfk_sobel_gradients of that image alone.
+ * Steps 1-6 are bit for bit OpenCV 4.13.  stats_dev (DEVICE double [n, 2], may be NULL): row i = (mu, sigma) of a
+ * normalising item; rows of the other items are not written.  One kernel for steps 1-6 of every item, two more when an
+ * item normalises (the statistics, once per item, then level 0), then for the whole batch one blur-down launch per
+ * level past 0 and, when an item has gradients, one Sobel launch per level.  Deterministic; an item's output depends on
+ * the item alone.  Asynchronous on the handle's stream.  Every item is validated before anything is enqueued
+ * (1 <= n <= 65535, 0 <= num_levels <= DFK_PREPROCESS_MAX_LEVELS, at most 2^31 - 1 tiles of 32 x 8 output pixels over
+ * the normalising items, the views, sizes and cameras above, normalize 0 or 1, stats_dev 8-byte aligned); a rejected
+ * call writes nothing and dfk_last_error names the item. */
+DfkStatus dfk_preprocess_batch(DfkHandle h, const DfkPreprocessItem* items, int n, int num_levels, double* stats_dev);
+/* the most levels a frame of sides <= DFK_ORB_MAX_SIDE has: 16384, 8192, ..., 1 */
+#define DFK_PREPROCESS_MAX_LEVELS 15
+
 /* ------------------------------------------------------------------ keyframe window problem (the LM loop on the device) */
 
 /* A window problem: the keyframe window's Levenberg-Marquardt loop in the library, with the window's state (poses and

@@ -50,9 +50,15 @@ One JSON line per case:
     features each: one dfk_orb_detect_batch (OrbDetectBatch; wall clock to a synchronise, summed device time and the
     time of each kernel from a separate profiled run) against cv2.ORB_create(500, 1.2, 1).detectAndCompute on the
     host, one image at a time.
+  * frame preprocessing (`--only preprocess`): 1, 8 and 64 colour frames at 640x480 (the 2x pixel repeat of the two
+    test images, each copy with its own noise) to the network's 256x192 with 4 levels and gradients: one
+    dfk_preprocess_batch through PreprocessBatch (wall clock to a synchronise, output allocations included) and as a bare
+    C call on buffers and items built once (wall clock to a synchronise), summed device time and the time of each kernel
+    from a separate profiled run, against cv2.remap + cvtColor + the float conversion on the host (a numpy fp32 product,
+    bitwise convertTo; cv2's Python API has no convertTo), one frame at a time with the map computed once.
 Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` /
-`--only frames` / `--only slide` / `--only error` / `--only lm` / `--only levels` / `--only match` / `--only orb` runs
-those cases alone.
+`--only frames` / `--only slide` / `--only error` / `--only lm` / `--only levels` / `--only match` / `--only orb` /
+`--only preprocess` runs those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -72,7 +78,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error", "lm", "levels",
-                                           "match", "orb"],
+                                           "match", "orb", "preprocess"],
                     default=None)
     args = ap.parse_args()
     import numpy as np
@@ -115,6 +121,8 @@ def main():
         return match_cases(args, torch, print)
     if args.only == "orb":
         return orb_cases(args, torch, print)
+    if args.only == "preprocess":
+        return preprocess_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -984,6 +992,90 @@ def orb_cases(args, torch, print):
                 rec.update({"host_us": round(host, 1), "host": f"cv2 {cv2.__version__}, one image at a time",
                             "speedup_wall": round(host / wall, 1), "counts_equal_host": host_counts == list(counts)})
             print(json.dumps(rec))
+
+
+def preprocess_cases(args, torch, print):
+    """dfk_preprocess_batch against cv2.remap + cvtColor + convertTo on the host, frame by frame"""
+    import numpy as np
+    from torch.profiler import ProfilerActivity, profile
+
+    import ctypes
+
+    from deepfactors_b200 import _lib
+    from deepfactors_b200.aligners import PreprocessBatch, SfmAligner, resize_viewport
+    from deepfactors_b200.synth import Camera
+    cam4 = lambda c: (c.fx, c.fy, c.u0, c.v0)
+    try:
+        import cv2
+    except ImportError:  # no host leg then
+        cv2 = None
+    z = np.load(os.path.join(ROOT, "tests", "golden", "preprocess_frames.npz"))
+    base = [np.repeat(np.repeat(z[f"image_{k}"], 2, axis=0), 2, axis=1) for k in ("1047", "1052")]
+    src_cam = resize_viewport(Camera(525.0, 525.0, 319.5, 239.5, 640.0, 480.0), 640, 480)
+    out_cam = Camera.scenenet(256, 192)
+    levels = 4
+    al = SfmAligner(8)
+    for n in (1, 8, 64):
+        rng = np.random.default_rng(n)
+        frames = [np.clip(base[i % 2].astype(np.int16) + rng.integers(-2, 3, base[0].shape), 0, 255).astype(np.uint8)
+                  for i in range(n)]
+        dev = [torch.from_numpy(f).cuda() for f in frames]
+
+        def device():
+            PreprocessBatch(al, dev, src_cam, out_cam, levels)
+
+        wall = _wall_us(torch, device, args.reps)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.reps):
+                device()
+            torch.cuda.synchronize()
+        stages = {e.key: round(e.self_device_time_total / args.reps, 1) for e in prof.key_averages()
+                  if e.self_device_time_total > 0}
+        # the C call alone: output buffers and items built once, as a caller that keeps its buffers does
+        outs = PreprocessBatch(al, dev, src_cam, out_cam, levels)
+        keep, items = [], []
+        for f, o in zip(dev, outs):
+            la = (_lib.DfkImage * levels)(*[_lib.DfkImage(t.data_ptr(), 4 * t.shape[1], t.shape[1], t.shape[0])
+                                            for t in o.levels])
+            ga = (_lib.DfkImage * levels)(*[_lib.DfkImage(t.data_ptr(), 8 * t.shape[1], t.shape[1], t.shape[0])
+                                            for t in o.grads])
+            keep += [la, ga]
+            items.append(_lib.DfkPreprocessItem(
+                _lib.DfkImage(f.data_ptr(), 3 * 640, 640, 480), _lib.DfkCamera(*cam4(src_cam), 640, 480),
+                _lib.DfkCamera(*cam4(out_cam), 256, 192), _lib.DfkImage(o.color.data_ptr(), 3 * 256, 256, 192),
+                _lib.DfkImage(o.gray.data_ptr(), 256, 256, 192), ctypes.cast(la, ctypes.POINTER(_lib.DfkImage)),
+                ctypes.cast(ga, ctypes.POINTER(_lib.DfkImage)), 0))
+        arr = (_lib.DfkPreprocessItem * n)(*items)
+        L = _lib.lib()
+
+        def c_call():
+            _lib.check(al._hd.h, L.dfk_preprocess_batch(al._hd.h, arr, n, levels, None))
+
+        c_wall = _wall_us(torch, c_call, args.reps)
+        rec = {"case": f"preprocess_640x480_to_256x192_x{n}", "frames": n, "levels": levels, "grads": True,
+               "device_wall_us": round(wall, 1), "c_call_wall_us": round(c_wall, 1),
+               "device_time_us": round(sum(stages.values()), 1),
+               "stages_us": {_kernel_name(k): v for k, v in stages.items()}}
+        if cv2 is not None:
+            K = lambda c: np.array([[c.fx, 0, c.u0], [0, c.fy, c.v0], [0, 0, 1]], np.float64)
+            m1, m2 = cv2.initUndistortRectifyMap(K(src_cam), None, None, K(out_cam), (256, 192), cv2.CV_32FC1)
+
+            def host_chain(f):
+                gray = cv2.cvtColor(cv2.remap(f, m1, m2, cv2.INTER_LINEAR), cv2.COLOR_RGB2GRAY)
+                # cv2's Python API has no convertTo; this numpy fp32 product is bitwise what convertTo(CV_32FC1,
+                # 1 / 255.0) gives
+                return gray.astype(np.float32) * np.float32(1.0 / 255.0)
+
+            host_chain(frames[0])
+            t0 = time.perf_counter()
+            for f in frames:
+                host_chain(f)
+            host = (time.perf_counter() - t0) * 1e6
+            rec.update({"host_us": round(host, 1), "host_levels": 0,
+                        "host": f"cv2 {cv2.__version__} remap + cvtColor, then a numpy fp32 product (bitwise convertTo), "
+                                "one frame at a time, no pyramid",
+                        "speedup_wall": round(host / wall, 1)})
+        print(json.dumps(rec))
 
 
 def solve_fill(K, links):
