@@ -95,8 +95,10 @@ __device__ __forceinline__ bool reprojection_match_rows(const ReprojItemDev& it,
   const float err = sqrtf(d0 * d0 + d1 * d1);
   // CauchyWeight(x, delta): a = delta / x; abs(a) / sqrt(2) * sqrt(log(1 + 1 / a / a)).  NaN at err == 0 (a = inf), as in
   // the reference (m_estimators.h:44-48): a match that lands exactly on its keypoint makes the whole factor NaN.
+  // log1pf, not logf(1 + s): the reference's float 1 + 1 / a^2 rounds away the weight's digits once a >> 1 and gives
+  // w = 0 below err = delta / 4096 (the true weight tends to 1 / sqrt(2)); log1pf keeps it to fp32 accuracy.
   const float a = cauchy_delta / err;
-  const float w = fabsf(a) / sqrtf(2.0f) * sqrtf(logf(1.0f + 1.0f / a / a));
+  const float w = fabsf(a) / sqrtf(2.0f) * sqrtf(log1pf(1.0f / a / a));
   if constexpr (kJac) {
     for (int j = 0; j < 6; ++j) {
       float s00 = 0.f, s01 = 0.f, s10 = 0.f, s11 = 0.f;

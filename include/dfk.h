@@ -488,7 +488,12 @@ DfkStatus dfk_depth_run_step(DfkHandle h, const float* code, int code_size, cons
  *                         divided by sigma -- the blocks of gtsam::JacobianFactor(keys, Ab) (:255-268); zero rows for a
  *                         match whose point falls behind the camera (:204-212)
  *   total_err             out, sum of squared UNWEIGHTED reprojection errors (total_err_, :242,258)
- * avg_dpt is hard-coded to 2 there (:171); here it is the handle's DenseSfmParams::avg_dpt.  Synchronous. */
+ * avg_dpt is hard-coded to 2 there (:171); here it is the handle's DenseSfmParams::avg_dpt.
+ * The Cauchy weight is |a| / sqrt(2) * sqrt(log1p(1 / a^2)), a = cauchy_delta / err.  The reference's float
+ * log(1 + 1 / a^2) loses the weight as a grows and gives 0 below about err = cauchy_delta / 4096, so a near-exact match,
+ * or any match under a large cauchy_delta, drops out of H; this build keeps the weight to fp32 accuracy there (it tends
+ * to 1 / sqrt(2)).  A match exactly on its keypoint (err = 0) still gives NaN, as in the reference.  The same weight
+ * serves dfk_reprojection_linearize_batch and dfk_reprojection_error_batch.  Synchronous. */
 DfkStatus dfk_reprojection_linearize(DfkHandle h, const float pose0[7], const float pose1[7], const float* code0,
                                      int code_size, const DfkCamera* cam, const DfkImage* prx_orig,
                                      const DfkImage* prx_jac, int num_matches, const float* query_xy,

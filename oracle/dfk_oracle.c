@@ -25,6 +25,8 @@
 #define COS_ cosf
 #define FLOOR_ floorf
 #define FABS_ fabsf
+/* log(1 + s) of CauchyWeight as the reference writes it (m_estimators.h:44-48): 1 + s rounded in float */
+#define CAUCHY_LOG_(s) ((REAL)log((double)(R_(1) + (s))))
 #include "dfk_oracle_impl.inc"
 #undef REAL
 #undef ACC
@@ -34,6 +36,7 @@
 #undef COS_
 #undef FLOOR_
 #undef FABS_
+#undef CAUCHY_LOG_
 
 /* ------------------------------------------------------------------ double flavour */
 #define REAL double
@@ -44,6 +47,9 @@
 #define COS_ cos
 #define FLOOR_ floor
 #define FABS_ fabs
+/* the truth: log1p keeps the weight's digits when s = 1 / a^2 is far below 1 (a near-exact match, or a large delta),
+ * where 1 + s would round them away even in double (s = 1e-14 keeps two digits) */
+#define CAUCHY_LOG_(s) log1p(s)
 #include "dfk_oracle_impl.inc"
 #undef REAL
 #undef ACC
@@ -53,6 +59,7 @@
 #undef COS_
 #undef FLOOR_
 #undef FABS_
+#undef CAUCHY_LOG_
 
 void dfko_probe_pixel_d(double x, double y, double dpt, const DfkoCamera* cam, const double pose[7],
                         int border, double min_dpt, double avg_dpt, double out[17])
