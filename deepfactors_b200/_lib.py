@@ -163,6 +163,30 @@ class DfkPreprocessItem(C.Structure):
                 ("gray", DfkImage), ("levels", C.POINTER(DfkImage)), ("grads", C.POINTER(DfkImage)),
                 ("normalize", C.c_int32)]
 
+
+BOW_MAX_DEPTH = 16  # DFK_BOW_MAX_DEPTH
+BOW_MAX_NODES = 4194304  # DFK_BOW_MAX_NODES
+
+
+class DfkBowVocabularyDesc(C.Structure):
+    _fields_ = [("k", C.c_int32), ("L", C.c_int32), ("weighting", C.c_int32), ("scoring", C.c_int32),
+                ("descriptor_bytes", C.c_int32), ("num_nodes", C.c_int32), ("node_ids", C.c_void_p),
+                ("parent_ids", C.c_void_p), ("weights", C.c_void_p), ("descriptors", C.c_void_p),
+                ("num_words", C.c_int32), ("word_ids", C.c_void_p), ("word_nodes", C.c_void_p)]
+
+
+class DfkBowVector(C.Structure):
+    _fields_ = [("words", C.c_void_p), ("values", C.c_void_p), ("count", C.c_void_p), ("capacity", C.c_int32)]
+
+
+class DfkBowQuery(C.Structure):
+    _fields_ = [("vector", DfkBowVector), ("max_results", C.c_int32), ("max_id", C.c_int32)]
+
+
+class DfkBowScoreItem(C.Structure):
+    _fields_ = [("entry", C.c_int32), ("vector", DfkBowVector)]
+
+
 WINDOW_ERROR_DOUBLES = 7  # DFK_WINDOW_ERROR_DOUBLES
 
 
@@ -264,6 +288,18 @@ SYMBOLS = {
     "dfk_build_image_pyramid": (C.c_int, [_H, _IMG, _IMG, C.c_int]),
     "dfk_squared_error": (C.c_int, [_H, _IMG, _IMG, _F]),
     "dfk_preprocess_batch": (C.c_int, [_H, C.POINTER(DfkPreprocessItem), C.c_int, C.c_int, C.c_void_p]),
+    "dfk_bow_vocabulary_create": (C.c_int, [_H, C.POINTER(DfkBowVocabularyDesc), C.POINTER(C.c_void_p)]),
+    "dfk_bow_vocabulary_destroy": (C.c_int, [_H, C.c_void_p]),
+    "dfk_bow_transform_batch": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkFeatureSet), C.POINTER(C.c_int32), C.c_int,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dfk_bow_database_create": (C.c_int, [_H, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "dfk_bow_database_destroy": (C.c_int, [_H, C.c_void_p]),
+    "dfk_bow_database_clear": (C.c_int, [_H, C.c_void_p]),
+    "dfk_bow_database_size": (C.c_int, [_H, C.c_void_p, C.POINTER(C.c_int32)]),
+    "dfk_bow_database_add": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkBowVector), C.c_int, C.POINTER(C.c_int32)]),
+    "dfk_bow_database_query_batch": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkBowQuery), C.c_int, C.c_void_p, C.c_void_p,
+                                               C.c_void_p]),
+    "dfk_bow_score_batch": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkBowScoreItem), C.c_int, C.c_void_p]),
 }
 
 _lib = None

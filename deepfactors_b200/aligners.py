@@ -16,6 +16,9 @@ is no CPU or torch fallback.
 from __future__ import annotations
 
 import ctypes as C
+import gzip
+import os
+import re
 from dataclasses import dataclass, field
 from typing import Sequence
 
@@ -1417,6 +1420,378 @@ def relocalize_select(errors, poses_ck, poses_wk):
         pose_ck = np.asarray(poses_ck[best], dtype=np.float32).copy()
     pose_wk = poses_wk[best] if poses_wk[best] is not None else np.array([0, 0, 0, 1, 0, 0, 0], dtype=np.float32)
     return best, pose_ck, _se3.compose(np.asarray(pose_wk, np.float32), _se3.inverse(pose_ck))
+
+
+# ------------------------------------------------------------------------------------------- DBoW2 retrieval
+_BOW_NODE = re.compile(r'\{\s*nodeId\s*:\s*(\d+)\s*,\s*parentId\s*:\s*(\d+)\s*,\s*weight\s*:\s*([^,\s}]+)\s*,'
+                       r'\s*descriptor\s*:\s*"([^"]*)"\s*\}')
+_BOW_WORD = re.compile(r'\{\s*wordId\s*:\s*(\d+)\s*,\s*nodeId\s*:\s*(\d+)\s*\}')
+
+
+def parse_dbow2_vocabulary(text: str) -> dict:
+    """DBoW2's TemplatedVocabulary::save text (cv::FileStorage YAML) as the arrays of DfkBowVocabularyDesc: k, L,
+    weighting, scoring, descriptor_bytes, node_ids / parent_ids int32 [N], weights float64 [N] (float() rounds as strtod),
+    descriptors uint8 [N, D], word_ids / word_nodes int32 [W], all in file order.  A line break inside a quoted
+    descriptor, with or without a trailing backslash, reads as the writer meant it."""
+    text = re.sub(r'\\\r?\n\s*', '', text)  # an escaped line break joins the two lines
+
+    def head(key):
+        m = re.search(r'^\s*' + key + r'\s*:\s*(-?\d+)\s*$', text, re.M)
+        if not m:
+            raise ValueError(f"DBoW2 vocabulary: no {key}")
+        return int(m.group(1))
+
+    nodes = _BOW_NODE.findall(text)
+    words = _BOW_WORD.findall(text)
+    if not nodes or not words:
+        raise ValueError("DBoW2 vocabulary: no nodes or no words")
+    desc = [[int(t) for t in d.split()] for _, _, _, d in nodes]
+    D = len(desc[0])
+    if any(len(d) != D for d in desc):
+        raise ValueError("DBoW2 vocabulary: descriptors of different lengths")
+    return dict(k=head("k"), L=head("L"), weighting=head("weightingType"), scoring=head("scoringType"),
+                descriptor_bytes=D,
+                node_ids=np.array([int(n[0]) for n in nodes], np.int32),
+                parent_ids=np.array([int(n[1]) for n in nodes], np.int32),
+                weights=np.array([float(n[2]) for n in nodes], np.float64),
+                descriptors=np.array(desc, np.uint8).reshape(-1, D),
+                word_ids=np.array([int(w[0]) for w in words], np.int32),
+                word_nodes=np.array([int(w[1]) for w in words], np.int32))
+
+
+def load_dbow2_vocabulary(path) -> dict:
+    """parse_dbow2_vocabulary of a .yml or .yml.gz file; needs no OpenCV"""
+    path = os.fspath(path)
+    opener = gzip.open if path.endswith(".gz") else open
+    with opener(path, "rt", encoding="ascii") as f:
+        return parse_dbow2_vocabulary(f.read())
+
+
+class BowVocabulary:
+    """A DBoW2 vocabulary on the device (dfk_bow_vocabulary_create): a path or the dict of load_dbow2_vocabulary.  The
+    tree is validated when it is created; TF_IDF / L1_NORM only."""
+
+    def __init__(self, voc, device=None):
+        if not isinstance(voc, dict):
+            voc = load_dbow2_vocabulary(voc)
+        self.voc = voc
+        self._hd = _Handle(device)
+        arr = {k: np.ascontiguousarray(voc[k], dt) for k, dt in
+               (("node_ids", np.int32), ("parent_ids", np.int32), ("weights", np.float64), ("descriptors", np.uint8),
+                ("word_ids", np.int32), ("word_nodes", np.int32))}
+        d = _lib.DfkBowVocabularyDesc(int(voc["k"]), int(voc["L"]), int(voc["weighting"]), int(voc["scoring"]),
+                                      int(voc["descriptor_bytes"]), len(arr["node_ids"]), arr["node_ids"].ctypes.data,
+                                      arr["parent_ids"].ctypes.data, arr["weights"].ctypes.data,
+                                      arr["descriptors"].ctypes.data, len(arr["word_ids"]), arr["word_ids"].ctypes.data,
+                                      arr["word_nodes"].ctypes.data)
+        self._p = C.c_void_p()
+        check(self._hd.h, lib().dfk_bow_vocabulary_create(self._hd.h, C.byref(d), C.byref(self._p)))
+
+    @property
+    def descriptor_bytes(self) -> int:
+        return int(self.voc["descriptor_bytes"])
+
+    def close(self):
+        if getattr(self, "_p", None) and self._hd.h:
+            lib().dfk_bow_vocabulary_destroy(self._hd.h, self._p)
+            self._p = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+@dataclass
+class BowVector:
+    """A bag-of-words vector on the device (DfkBowVector): words int32 [capacity] ascending, values float64 [capacity],
+    count int32 [1] (a view into a transform's counts); only the first count rows hold the vector."""
+    words: torch.Tensor
+    values: torch.Tensor
+    count: torch.Tensor
+    capacity: int
+
+    def to_c(self) -> "_lib.DfkBowVector":
+        return _lib.DfkBowVector(self.words.data_ptr(), self.values.data_ptr(), self.count.data_ptr(), self.capacity)
+
+    def host(self):
+        """(words, values) on the host (synchronises)"""
+        c = int(self.count.item())
+        return self.words[:c].cpu().numpy(), self.values[:c].cpu().numpy()
+
+    @staticmethod
+    def from_host(words, values, device="cuda", capacity: int | None = None) -> "BowVector":
+        w = np.ascontiguousarray(words, np.int32)
+        v = np.ascontiguousarray(values, np.float64)
+        cap = len(w) if capacity is None else int(capacity)
+        tw = torch.zeros(max(cap, 1), dtype=torch.int32, device=device)
+        tv = torch.zeros(max(cap, 1), dtype=torch.float64, device=device)
+        tw[:len(w)] = torch.from_numpy(w).to(device)
+        tv[:len(v)] = torch.from_numpy(v).to(device)
+        return BowVector(tw, tv, torch.tensor([len(w)], dtype=torch.int32, device=device), cap)
+
+
+@dataclass
+class BowBatch:
+    """The device output of BowTransformBatch: item i's rows are [offsets[i], offsets[i] + capacities[i]); words int32,
+    values float64, feature_words int32 (the word of each descriptor, -1 when its weight is not > 0), counts int32 [n]."""
+    words: torch.Tensor
+    values: torch.Tensor
+    counts: torch.Tensor
+    feature_words: torch.Tensor
+    offsets: np.ndarray
+    capacities: np.ndarray
+
+    def vectors(self) -> list:
+        """one BowVector per item (views, no read-back): they feed BowDatabase.add / query / score as they are"""
+        return [BowVector(self.words[o:o + c], self.values[o:o + c], self.counts[i:i + 1], int(c))
+                for i, (o, c) in enumerate(zip(self.offsets[:-1], self.capacities))]
+
+
+def _descriptor_rows(d) -> torch.Tensor:
+    d = d.descriptors if isinstance(d, Features) else d
+    if not isinstance(d, torch.Tensor) or not d.is_cuda or d.dtype != torch.uint8 or d.dim() != 2 or \
+            (d.shape[0] > 1 and not d.is_contiguous()):
+        raise TypeError("BowTransformBatch: descriptors must be contiguous uint8 [N, D] CUDA tensors")
+    return d
+
+
+def BowTransformBatch(voc: BowVocabulary, descriptors: Sequence, capacities=None) -> BowBatch:
+    """voc_.transform(features, bow_vec) of many images in one call (dfk_bow_transform_batch), bit for bit DBoW2:
+    descriptors are uint8 [N, D] CUDA tensors (or Features), D the vocabulary's.  capacities (default N) reserve each
+    item's output rows.  Asynchronous: returns a BowBatch of device tensors."""
+    hd = voc._hd
+    hd.use_torch_stream()
+    rows = [_descriptor_rows(d) for d in descriptors]
+    n = len(rows)
+    caps = [int(r.shape[0]) for r in rows] if capacities is None else [int(c) for c in capacities]
+    if len(caps) != n:
+        raise ValueError("BowTransformBatch: one capacity per item")
+    sets = (_lib.DfkFeatureSet * max(n, 1))(*[_lib.DfkFeatureSet(None, r.data_ptr() if r.shape[0] else None,
+                                                                 int(r.shape[0]), int(r.shape[1])) for r in rows])
+    cap_arr = (C.c_int32 * max(n, 1))(*caps)
+    offsets = np.concatenate([[0], np.cumsum(caps)]).astype(np.int64)
+    total = int(offsets[-1])
+    dev = f"cuda:{hd.device}"
+    words = torch.zeros(max(total, 1), dtype=torch.int32, device=dev)
+    values = torch.zeros(max(total, 1), dtype=torch.float64, device=dev)
+    fw = torch.zeros(max(total, 1), dtype=torch.int32, device=dev)
+    counts = torch.zeros(max(n, 1), dtype=torch.int32, device=dev)
+    check(hd.h, lib().dfk_bow_transform_batch(hd.h, voc._p, sets, cap_arr, n, C.c_void_p(words.data_ptr()),
+                                              C.c_void_p(values.data_ptr()), C.c_void_p(counts.data_ptr()),
+                                              C.c_void_p(fw.data_ptr())))
+    return BowBatch(words, values, counts[:n], fw, offsets, np.array(caps, np.int64))
+
+
+@dataclass
+class BowQueryResult:
+    """BowDatabase.query's device output: query i's rows are [offsets[i], offsets[i] + min(counts[i], max_results[i]));
+    ids int32 entry ids, scores float64, best first; counts int32 [n] (DBoW2's ret.size() before the cut)."""
+    ids: torch.Tensor
+    scores: torch.Tensor
+    counts: torch.Tensor
+    offsets: np.ndarray
+    max_results: np.ndarray
+
+    def results(self) -> list:
+        """per query the list of (Id, Score), as DBoW2's QueryResults (one read-back)"""
+        c, ids, sc = self.counts.cpu().numpy(), self.ids.cpu().numpy(), self.scores.cpu().numpy()
+        return [[(int(ids[o + k]), float(sc[o + k])) for k in range(min(int(c[i]), int(m)))]
+                for i, (o, m) in enumerate(zip(self.offsets[:-1], self.max_results))]
+
+
+class BowDatabase:
+    """TemplatedDatabase(voc, false, 0) on the device (dfk_bow_database_*): add, query, score, clear, len."""
+
+    def __init__(self, voc: BowVocabulary):
+        self.voc = voc
+        self._hd = voc._hd
+        self._p = C.c_void_p()
+        check(self._hd.h, lib().dfk_bow_database_create(self._hd.h, voc._p, C.byref(self._p)))
+
+    def __len__(self) -> int:
+        n = C.c_int32()
+        check(self._hd.h, lib().dfk_bow_database_size(self._hd.h, self._p, C.byref(n)))
+        return int(n.value)
+
+    def clear(self):
+        check(self._hd.h, lib().dfk_bow_database_clear(self._hd.h, self._p))
+
+    def add(self, vectors: Sequence[BowVector]) -> int:
+        """adds the vectors in order (copied on the device, no read-back); returns the first entry id"""
+        self._hd.use_torch_stream()
+        n = len(vectors)
+        arr = (_lib.DfkBowVector * max(n, 1))(*[v.to_c() for v in vectors])
+        first = C.c_int32(-1)
+        check(self._hd.h, lib().dfk_bow_database_add(self._hd.h, self._p, arr, n, C.byref(first)))
+        return int(first.value)
+
+    def query(self, vectors: Sequence[BowVector], max_results=1, max_id=-1) -> BowQueryResult:
+        """db_.query(vec, ret, max_results, max_id) for every vector in one call (dfk_bow_database_query_batch);
+        max_results and max_id are one value for all or one per vector.  Asynchronous."""
+        self._hd.use_torch_stream()
+        n = len(vectors)
+        per = lambda v: [int(x) for x in (v if isinstance(v, (list, tuple, np.ndarray)) else [v] * n)]
+        mr, mi = per(max_results), per(max_id)
+        arr = (_lib.DfkBowQuery * max(n, 1))(*[_lib.DfkBowQuery(v.to_c(), a, b) for v, a, b in zip(vectors, mr, mi)])
+        offsets = np.concatenate([[0], np.cumsum(mr)]).astype(np.int64)
+        dev = f"cuda:{self._hd.device}"
+        ids = torch.full((max(int(offsets[-1]), 1),), -1, dtype=torch.int32, device=dev)
+        scores = torch.zeros(max(int(offsets[-1]), 1), dtype=torch.float64, device=dev)
+        counts = torch.zeros(max(n, 1), dtype=torch.int32, device=dev)
+        check(self._hd.h, lib().dfk_bow_database_query_batch(self._hd.h, self._p, arr, n, C.c_void_p(ids.data_ptr()),
+                                                             C.c_void_p(scores.data_ptr()),
+                                                             C.c_void_p(counts.data_ptr())))
+        return BowQueryResult(ids, scores, counts[:n], offsets, np.array(mr, np.int64))
+
+    def score(self, entries: Sequence[int], vectors: Sequence[BowVector]) -> torch.Tensor:
+        """voc_.score(entry's vector, vector) per pair (dfk_bow_score_batch): float64 [n] on the device"""
+        self._hd.use_torch_stream()
+        n = len(vectors)
+        arr = (_lib.DfkBowScoreItem * max(n, 1))(*[_lib.DfkBowScoreItem(int(e), v.to_c())
+                                                   for e, v in zip(entries, vectors)])
+        out = torch.zeros(max(n, 1), dtype=torch.float64, device=f"cuda:{self._hd.device}")
+        check(self._hd.h, lib().dfk_bow_score_batch(self._hd.h, self._p, arr, n, C.c_void_p(out.data_ptr())))
+        return out[:n]
+
+    def close(self):
+        if getattr(self, "_p", None) and self._hd.h:
+            lib().dfk_bow_database_destroy(self._hd.h, self._p)
+            self._p = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+# ------------------------------------------------------------------------------------------- LoopDetector
+@dataclass
+class LoopDetectorConfig:
+    """LoopDetectorConfig (core/system/loop_detector.h:44-53)"""
+    tracker_cfg: TrackerConfig = field(default_factory=TrackerConfig)
+    iters: Sequence[int] = (10, 5, 4)
+    min_similarity: float = 0.35
+    max_error: float = 0.5
+    max_dist: float = 0.1
+    max_candidates: int = 3
+    active_window: int = 5
+
+
+@dataclass
+class LoopInfo:
+    """LoopDetector::LoopInfo (loop_detector.h:73-78)"""
+    loop_id: int = 1
+    pose_wc: np.ndarray | None = None
+    detected: bool = False
+
+
+def _translation_dist(a, b) -> np.float32:
+    """(a.translation() - b.translation()).norm() in fp32 (poses: quaternion (x, y, z, w), translation)"""
+    d = np.asarray(a, np.float32)[4:7] - np.asarray(b, np.float32)[4:7]
+    return np.sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2], dtype=np.float32)
+
+
+def loop_candidates(results, curr_kf_id: int, active_window: int, min_similarity: float, entry_to_id=None) -> list:
+    """The candidate filter of LoopDetector::DetectLoop (loop_detector.cpp:117-139): results are the query's (Id, Score)
+    best first, keyframe id = entry_to_id(Id) (Id + 1 by default, as the reference assumes).  Skips the current
+    keyframe, ids > curr - active_window and Score < min_similarity.  The ids are size_t there, so curr - active_window
+    wraps when curr < active_window and then skips nothing; so does this."""
+    to_id = entry_to_id or (lambda e: e + 1)
+    thr = (int(curr_kf_id) - int(active_window)) % (1 << 64)
+    ms = float(np.float32(min_similarity))
+    out = []
+    for e, s in results:
+        kfid = int(to_id(e))
+        if kfid == curr_kf_id or kfid > thr or s < ms:
+            continue
+        out.append(kfid)
+    return out
+
+
+def loop_select(candidates, poses_wc, inliers, poses_wk, max_dist: float) -> LoopInfo:
+    """The geometry check's selection of LoopDetector::DetectLoop (loop_detector.cpp:146-184): per candidate its tracked
+    pose_wc, inlier fraction and pose_wk; skip inliers < 0.5, keep the strictly smallest translation distance, accept it
+    below max_dist."""
+    best_dist, best_id, best_pose = np.float32(np.inf), candidates[0], None
+    for cid, pwc, inl, pwk in zip(candidates, poses_wc, inliers, poses_wk):
+        dist = _translation_dist(pwc, pwk)
+        if np.float32(inl) < np.float32(0.5):
+            continue
+        if dist < best_dist:
+            best_dist, best_id, best_pose = dist, cid, pwc
+    if best_dist < np.float32(max_dist):
+        return LoopInfo(int(best_id), np.asarray(best_pose, np.float32), True)
+    return LoopInfo()
+
+
+def detect_local_loop(keyframe_poses, pose_cam, curr_kf_id: int, active_window: int, max_dist: float) -> int:
+    """LoopDetector::DetectLocalLoop (loop_detector.cpp:190-224), host only: keyframe_poses is (id, pose_wk) in the map's
+    order; the last active_window of them, newest first, the strictly closest by translation that is not the current
+    keyframe; its id when closer than max_dist, else 0."""
+    kp = list(keyframe_poses)
+    best_dist, best_id = np.float32(np.inf), (kp[-1][0] if kp else 0)
+    for kid, pwk in kp[::-1][:max(int(active_window), 0)]:
+        dist = _translation_dist(pose_cam, pwk)
+        if dist < best_dist and kid != curr_kf_id:
+            best_dist, best_id = dist, kid
+    if best_id != curr_kf_id and best_dist < np.float32(max_dist):
+        return int(best_id)
+    return 0
+
+
+class LoopDetector:
+    """df::LoopDetector (core/system/loop_detector.{h,cpp}) on the device: the vocabulary transform, the database and
+    its query run in libdfk.so (no descriptor leaves the device), the geometric check is one batched track of every
+    surviving candidate (CameraTracker.TrackFrameBatch).  Keyframes are passed as a mapping id -> (pyr_img, pyr_dpt,
+    pose_wk); entry e of the database is keyframe entry_to_id(e), e + 1 by default."""
+
+    def __init__(self, vocabulary, camera_pyr, config: LoopDetectorConfig | None = None, entry_to_id=None, device=None):
+        self.cfg_ = config or LoopDetectorConfig()
+        self.voc_ = vocabulary if isinstance(vocabulary, BowVocabulary) else BowVocabulary(vocabulary, device)
+        self.db_ = BowDatabase(self.voc_)
+        tc = self.cfg_.tracker_cfg
+        self.tracker_ = CameraTracker(camera_pyr, TrackerConfig(len(self.cfg_.iters), tuple(self.cfg_.iters),
+                                                                tc.huber_delta), device)
+        self.entry_to_id = entry_to_id or (lambda e: e + 1)
+        self.dmap_ = {}  # keyframe id -> (entry, BowVector)
+        self.last_min_score = None
+
+    def AddKeyframe(self, kf_id: int, descriptors) -> BowVector:
+        """transform the keyframe's descriptors and add them to the database (loop_detector.cpp:38-44)"""
+        vec = BowTransformBatch(self.voc_, [descriptors]).vectors()[0]
+        entry = self.db_.add([vec])
+        self.dmap_[kf_id] = (entry, vec)
+        return vec
+
+    def DetectLoop(self, pyr_img, pyr_grad, descriptors, curr_kf_id: int, keyframes) -> LoopInfo:
+        """LoopDetector::DetectLoop (loop_detector.cpp:96-185): transform, the score against the current keyframe
+        (kept in last_min_score; the reference only logs it), the query (max_id -1, max_candidates), the candidate
+        filter, one batched track of the survivors and the selection"""
+        vec = BowTransformBatch(self.voc_, [descriptors]).vectors()[0]
+        cur = self.dmap_.get(curr_kf_id)
+        score = self.db_.score([cur[0]], [vec]) if cur is not None else None
+        res = self.db_.query([vec], self.cfg_.max_candidates, -1).results()[0]
+        self.last_min_score = float(score.item()) if score is not None else None
+        cands = loop_candidates(res, curr_kf_id, self.cfg_.active_window, self.cfg_.min_similarity, self.entry_to_id)
+        if not cands:
+            return LoopInfo()
+        from . import se3 as _se3
+        kfs = [keyframes[c] for c in cands]
+        poses_ck, frac, _ = self.tracker_.TrackFrameBatch(kfs, pyr_img, pyr_grad)
+        ident = np.array([0, 0, 0, 1, 0, 0, 0], np.float32)
+        pwk = [np.asarray(kf[2], np.float32) if len(kf) > 2 and kf[2] is not None else ident for kf in kfs]
+        pwc = [_se3.compose(w, _se3.inverse(p)) for w, p in zip(pwk, poses_ck)]
+        return loop_select(cands, pwc, frac, pwk, self.cfg_.max_dist)
+
+    def DetectLocalLoop(self, keyframe_poses, pose_cam, curr_kf_id: int) -> int:
+        return detect_local_loop(keyframe_poses, pose_cam, curr_kf_id, self.cfg_.active_window, self.cfg_.max_dist)
+
+    def Reset(self):
+        self.db_.clear()
+        self.dmap_.clear()
 
 
 # ------------------------------------------------------------------------------------------- free functions

@@ -116,6 +116,12 @@ struct DfkContext {
   DeviceBuf<unsigned char> pp_dev;
   std::vector<unsigned char> pp_host;
   DeviceBuf<double> pp_partials;
+  // the dfk_bow_* calls: the call's descriptors (one H2D per call from bow_host), the transform's per-descriptor words
+  // when the caller passes none, and a query's [sums n x size | hits n x size] (bytes)
+  DeviceBuf<unsigned char> bow_dev;
+  std::vector<unsigned char> bow_host;
+  DeviceBuf<int32_t> bow_words;
+  DeviceBuf<unsigned char> bow_scratch;
   // dfk_window_marginalize_frames / dfk_window_add_priors: the call's index lists (one pageable H2D per call)
   DeviceBuf<int> window_lists;
   // dfk_window_marginalize_keyframe: the call's lists [refs | tile rows / cols | member locations | update tasks] (one

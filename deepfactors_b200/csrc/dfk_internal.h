@@ -516,6 +516,66 @@ cudaError_t launch_blur_down_batch(const PyrLevelDev* in_dev, const PyrLevelDev*
                                    int max_out_h, cudaStream_t s);
 cudaError_t launch_sobel_batch(const PyrLevelDev* lv_dev, int n, int max_w, int max_h, cudaStream_t s);
 
+// DBoW2 retrieval (dfk_bow.cu).  The vocabulary on the device, rows re-indexed breadth first so that a node's
+// children are consecutive rows: row 0 is the root, desc [rows, q] (q = descriptor_bytes / 16), child[row] = (first
+// child row, children; 0 for a leaf), word[row] = the leaf's word (-1 inside), word_weight [words].
+struct BowVocDev {
+  const uint4* desc;
+  const int2* child;
+  const int32_t* word;
+  const double* word_weight;
+  int q;
+};
+// one image of dfk_bow_transform_batch: its descriptor rows and its first output row
+struct BowItemDev {
+  const uint8_t* descriptors;
+  int num;
+  int out_begin;
+};
+// one vector of dfk_bow_database_add: copied to storage rows [offset, offset + count) as entry `entry`
+struct BowAddDev {
+  const int32_t* words;
+  const double* values;
+  const int32_t* count;
+  int capacity;
+  int entry;
+  long long offset;
+};
+// the database's storage: entry e's words and values start at offsets[e], counts[e] of them
+struct BowDbDev {
+  const int32_t* words;
+  const double* values;
+  const long long* offsets;
+  const int32_t* counts;
+  int size;
+};
+struct BowQueryDev {
+  const int32_t* words;
+  const double* values;
+  const int32_t* count;
+  int capacity;
+  int max_results;
+  int max_id;
+  int row_begin;
+};
+struct BowScoreDev {
+  const int32_t* words;
+  const double* values;
+  const int32_t* count;
+  int capacity;
+  int entry;
+};
+// the descent (grid (max_num / 8, n), none when max_num = 0) then the assembly (one CTA per item)
+cudaError_t launch_bow_transform(const BowVocDev& v, const BowItemDev* items_dev, int n, int max_num,
+                                 int32_t* feature_words, int32_t* words_out, double* values_out, int32_t* counts,
+                                 cudaStream_t s);
+cudaError_t launch_bow_add(const BowAddDev* adds_dev, int n, int32_t* st_words, double* st_values,
+                           long long* entry_offsets, int32_t* entry_counts, cudaStream_t s);
+// db.size >= 1; sums and hits [n, db.size]; max_cap the largest query capacity (its words and values in shared memory)
+cudaError_t launch_bow_query(const BowDbDev& db, const BowQueryDev* queries_dev, int n, int max_cap, double* sums,
+                             uint8_t* hits, int32_t* ids, double* scores, int32_t* counts, cudaStream_t s);
+cudaError_t launch_bow_score(const BowDbDev& db, const BowScoreDev* items_dev, int n, double* out, cudaStream_t s);
+
 constexpr int kSimpleMaxBlocks = 1024;
 constexpr int kSimpleScratchFloats = kSimpleMaxBlocks * 32;
 

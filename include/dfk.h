@@ -790,6 +790,140 @@ DfkStatus dfk_preprocess_batch(DfkHandle h, const DfkPreprocessItem* items, int 
 /* the most levels a frame of sides <= DFK_ORB_MAX_SIDE has: 16384, 8192, ..., 1 */
 #define DFK_PREPROCESS_MAX_LEVELS 15
 
+/* ------------------------------------------------------------------ loop-closure candidates (DBoW2 retrieval) */
+
+/* The bag-of-words retrieval of LoopDetector (core/system/loop_detector.cpp:38-44, 96-112): DBoW2 (commit 3924753)
+ * TemplatedVocabulary::transform / score and TemplatedDatabase::add / query with TF_IDF weighting and L1_NORM scoring,
+ * no direct index (TemplatedDatabase(voc, false, 0)).  DBoW2 is not vendored; this block is its specification
+ * (DESIGN.md section 4.11).  Every value is fp64 and every sum runs in the order stated; nothing is reassociated.
+ *   1. vocabulary  node 0 is the root and is not listed; the listed nodes have an id, a parent id, a weight (the idf)
+ *                  and a descriptor.  A node's children are in the order the nodes are listed.  A leaf is a node with no
+ *                  children; each word names one leaf.
+ *   2. word        of a descriptor: from the root, step to the child at the smallest Hamming distance (popcount over
+ *                  all descriptor_bytes), strict < in children order (a tie goes to the first child), until a leaf; the
+ *                  result is the leaf's word id and weight.
+ *   3. vector      a map ordered by word id.  Features in input order; one whose weight is > 0 is added, v[id] += w (the
+ *                  first occurrence inserts w, so a word seen n times holds w added n times in sequence, not n w); one
+ *                  whose weight is not > 0 is skipped.  Then L1 normalisation: norm = the sum of fabs(value) in
+ *                  ascending word order, from 0.0; if norm > 0 every value becomes value / norm.  (No division by the
+ *                  word count: L1 scoring normalises.)
+ *   4. database    add gives entry ids 0, 1, 2, ... in the order vectors are added; clear empties it.
+ *   5. query       (queryL1) for each query word in ascending order and each entry e holding it with e < max_id or
+ *                  max_id = -1: t = fabs(q - d) - fabs(q) - fabs(d) (q the query's value, d the entry's).  Per entry the
+ *                  first t initialises the sum, later ones are added in word order; only entries with a common word
+ *                  appear.  Sorted ascending by sum, cut to max_results, Score = -sum / 2.0.
+ *                  Deviation: DBoW2's std::sort leaves the order of equal sums unspecified; here equal sums go in
+ *                  ascending entry id.
+ *   6. score       (L1Scoring::score(a, b)) a and b merged in ascending word order; from 0.0, each common word adds
+ *                  fabs(vi - wi) - fabs(vi) - fabs(wi), vi from a and wi from b; the result is -score / 2.0.  This is not
+ *                  the query's operand order, and the two round differently.  Vectors with no common word score -0.0, bit
+ *                  for bit DBoW2's result.
+ * Only weighting TF_IDF (0) and scoring L1_NORM (0) are implemented; any other is DFK_ERR_UNSUPPORTED. */
+#define DFK_BOW_MAX_DEPTH 16
+#define DFK_BOW_MAX_NODES 4194304
+#define DFK_BOW_WEIGHTING_TF_IDF 0
+#define DFK_BOW_SCORING_L1 0
+
+/* A vocabulary as DBoW2's text format lists it.  All arrays are HOST memory, read during dfk_bow_vocabulary_create. */
+typedef struct {
+  int32_t k;                    /* branching factor, in [1, 32] */
+  int32_t L;                    /* depth levels, in [1, DFK_BOW_MAX_DEPTH] */
+  int32_t weighting;            /* weightingType: DFK_BOW_WEIGHTING_TF_IDF only */
+  int32_t scoring;              /* scoringType: DFK_BOW_SCORING_L1 only */
+  int32_t descriptor_bytes;     /* 32 (ORB), 48 (BRISK, the reference's small_voc) or 64 */
+  int32_t num_nodes;            /* N, the listed nodes (the root excluded), in [1, DFK_BOW_MAX_NODES] */
+  const int32_t* node_ids;      /* [N] in file order: a permutation of 1..N */
+  const int32_t* parent_ids;    /* [N] 0 (the root) or a listed id */
+  const double* weights;        /* [N] finite and >= 0 */
+  const uint8_t* descriptors;   /* [N, descriptor_bytes] */
+  int32_t num_words;            /* W >= 1 */
+  const int32_t* word_ids;      /* [W] a permutation of 0..W-1 */
+  const int32_t* word_nodes;    /* [W] the leaf each word names */
+} DfkBowVocabularyDesc;
+
+typedef struct DfkBowVocabulary DfkBowVocabulary;
+typedef struct DfkBowDatabase DfkBowDatabase;
+
+/* Validates the whole tree (the ids and word ids are permutations; every parent exists, there is no cycle and every
+ * node is reachable from the root; each node has <= k children and depth <= L; every leaf has exactly one word and no
+ * internal node has one; the weights are finite and >= 0) and uploads it re-indexed so that each node's children are
+ * consecutive rows in their original order.  Synchronous.  A rejected call creates nothing, and dfk_last_error names
+ * the node, word or field. */
+DfkStatus dfk_bow_vocabulary_create(DfkHandle h, const DfkBowVocabularyDesc* desc, DfkBowVocabulary** out);
+DfkStatus dfk_bow_vocabulary_destroy(DfkHandle h, DfkBowVocabulary* voc);
+
+/* A bag-of-words vector on the device: count (a DEVICE pointer, e.g. counts_dev + i of a transform) words in
+ * ascending order with their values.  Nothing of it is read on the host, so a transform's output feeds the database
+ * with no read-back. */
+typedef struct {
+  const int32_t* words;         /* DEVICE [capacity] */
+  const double* values;         /* DEVICE [capacity], 8-byte aligned */
+  const int32_t* count;         /* DEVICE: the word count; read as min(max(count, 0), capacity) */
+  int32_t capacity;             /* >= 0 */
+} DfkBowVector;
+
+/* Steps 2-3 for every item: item i is the descriptor rows of one image (keypoints is not read: a slice of the
+ * dfk_orb_detect_batch output passes as it is); descriptor_bytes must equal the vocabulary's, num in
+ * [0, DFK_MATCH_MAX_QUERIES], descriptors 16-byte aligned.  Outputs (DEVICE), item i's rows at o_i = the sum of the
+ * capacities before it (capacities HOST, capacities[i] >= num):
+ *   words_dev          int32, the vector's words ascending;  values_dev  fp64 (8-byte aligned), their values
+ *   counts_dev         int32 [n]: the vector's word count, so (words_dev + o_i, values_dev + o_i, counts_dev + i,
+ *                      capacities[i]) is the item's DfkBowVector
+ *   feature_words_dev  int32 (may be NULL): the word of each descriptor, -1 for one whose weight is not > 0
+ * Two launches for the whole batch (descent: one warp per descriptor; assembly: one CTA per item).  Deterministic, no
+ * floating-point atomics; an item's output depends on the item alone.  Asynchronous on the handle's stream.  Every item
+ * is validated before anything is enqueued (1 <= n <= 65535); a rejected call writes nothing and dfk_last_error names
+ * the item and field. */
+DfkStatus dfk_bow_transform_batch(DfkHandle h, const DfkBowVocabulary* voc, const DfkFeatureSet* items,
+                                  const int32_t* capacities, int n, int32_t* words_dev, double* values_dev,
+                                  int32_t* counts_dev, int32_t* feature_words_dev);
+
+/* An empty database (step 4).  Entries keep their words and values in device storage that grows only: an entry
+ * reserves the capacity of the vector it was added from, not its count, so a transform capacity of 2 x 500 rows costs
+ * 12 kB per entry however few words the image has (the slack is capacity - count rows of 12 bytes).  clear keeps the
+ * storage for reuse; destroy frees it. */
+DfkStatus dfk_bow_database_create(DfkHandle h, const DfkBowVocabulary* voc, DfkBowDatabase** out);
+DfkStatus dfk_bow_database_destroy(DfkHandle h, DfkBowDatabase* db);
+DfkStatus dfk_bow_database_clear(DfkHandle h, DfkBowDatabase* db);
+/* the number of entries, known on the host (no synchronisation) */
+DfkStatus dfk_bow_database_size(DfkHandle h, const DfkBowDatabase* db, int32_t* size);
+/* Adds n vectors in order as entries size, size + 1, ...; *first_entry (may be NULL) receives the first id.  One
+ * launch copies them on the device, ordered after earlier work on the handle's stream (a transform's output may be
+ * added before it has run).  1 <= n <= 65535 and at most 2^31 - 1 entries; a rejected call adds nothing. */
+DfkStatus dfk_bow_database_add(DfkHandle h, DfkBowDatabase* db, const DfkBowVector* vectors, int n,
+                               int32_t* first_entry);
+
+/* One query of dfk_bow_database_query_batch */
+typedef struct {
+  DfkBowVector vector;
+  int32_t max_results;          /* >= 1: the rows reserved for the query */
+  int32_t max_id;               /* -1 (every entry) or >= 0: entries e < max_id only */
+} DfkBowQuery;
+
+/* Step 5 for every query against the database.  Outputs (DEVICE), query i's rows at r_i = the sum of the max_results
+ * before it: ids_dev int32 entry ids and scores_dev fp64 Scores (8-byte aligned), best first; counts_dev int32 [n] =
+ * DBoW2's ret.size() before the cut, the number of entries with a common word.  Only min(count, max_results) rows are
+ * written.  Two launches (one warp per (query, entry) for the sums; the ranks of the sums, which place each row), plus a
+ * memset of counts_dev when the database is empty.  The query's words and values sit in shared memory, so a vector's
+ * capacity is at most DFK_MATCH_MAX_QUERIES.  Neither kernel indexes by word id, so a malformed vector cannot read out
+ * of bounds.  The ranks compare each hit with every other, so the work is n x size^2 comparisons: n x size <= 2^26
+ * (the sums' scratch) and n x size^2 <= 2^36 (one query against at most 262,144 entries; 10,000 entries take about
+ * 0.5 ms on an H100), and 1 <= n <= 65535; a rejected call writes nothing. */
+DfkStatus dfk_bow_database_query_batch(DfkHandle h, const DfkBowDatabase* db, const DfkBowQuery* queries, int n,
+                                       int32_t* ids_dev, double* scores_dev, int32_t* counts_dev);
+
+/* One score of dfk_bow_score_batch: score(the entry's vector, vector) */
+typedef struct {
+  int32_t entry;                /* in [0, size) */
+  DfkBowVector vector;
+} DfkBowScoreItem;
+
+/* Step 6 for every item: scores_dev[i] (DEVICE fp64, 8-byte aligned) = L1Scoring::score(a, b) with a the entry's
+ * vector and b the item's, the operand order of voc_.score(curr_kf->bow_vec, live) (loop_detector.cpp:107).  One launch,
+ * one warp per item.  1 <= n <= 65535; a rejected call writes nothing. */
+DfkStatus dfk_bow_score_batch(DfkHandle h, const DfkBowDatabase* db, const DfkBowScoreItem* items, int n,
+                              double* scores_dev);
+
 /* ------------------------------------------------------------------ keyframe window problem (the LM loop on the device) */
 
 /* A window problem: the keyframe window's Levenberg-Marquardt loop in the library, with the window's state (poses and

@@ -56,6 +56,12 @@ One JSON line per case:
     C call on buffers and items built once (wall clock to a synchronise), summed device time and the time of each kernel
     from a separate profiled run, against cv2.remap + cvtColor + the float conversion on the host (a numpy fp32 product,
     bitwise convertTo; cv2's Python API has no convertTo), one frame at a time with the map computed once.
+  * DBoW2 retrieval (`--only bow`): the bag-of-words transform of 1, 8 and 64 frames x 500 random descriptors with the
+    reference's small_voc (k 9, L 3, 48 bytes) and an ORB-SLAM-sized vocabulary (k 10, L 6, 32 bytes, random
+    centroids, 10^6 words): one dfk_bow_transform_batch (wall clock to a synchronise, and summed device time from a
+    separate profiled run) against the sequential C oracle (bow_oracle) on one host thread, frame by frame; and one
+    query of a 500-feature frame (max_results 20) against databases of 100, 1,000 and 10,000 entries.  The oracle's
+    query scans every entry (no inverted file), so its host time is an upper bound of DBoW2's.
 Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` /
 `--only frames` / `--only slide` / `--only error` / `--only lm` / `--only levels` / `--only match` / `--only orb` /
 `--only preprocess` runs those cases alone.
@@ -78,7 +84,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error", "lm", "levels",
-                                           "match", "orb", "preprocess"],
+                                           "match", "orb", "preprocess", "bow"],
                     default=None)
     args = ap.parse_args()
     import numpy as np
@@ -123,6 +129,8 @@ def main():
         return orb_cases(args, torch, print)
     if args.only == "preprocess":
         return preprocess_cases(args, torch, print)
+    if args.only == "bow":
+        return bow_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -992,6 +1000,78 @@ def orb_cases(args, torch, print):
                 rec.update({"host_us": round(host, 1), "host": f"cv2 {cv2.__version__}, one image at a time",
                             "speedup_wall": round(host / wall, 1), "counts_equal_host": host_counts == list(counts)})
             print(json.dumps(rec))
+
+
+def _full_voc(k: int, L: int, D: int, seed: int) -> dict:
+    """a complete k-ary tree of depth L listed breadth first, random centroids, leaf weights in (0.1, 3)"""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    sizes = [k ** d for d in range(1, L + 1)]
+    N = sum(sizes)
+    ids = np.arange(1, N + 1, dtype=np.int64)
+    parents = np.zeros(N, np.int64)
+    first = 0
+    for d, n in enumerate(sizes):
+        if d:
+            parents[first:first + n] = (first - sizes[d - 1]) + np.arange(n) // k + 1
+        first += n
+    leaves = ids[N - sizes[-1]:]
+    w = np.zeros(N)
+    w[N - sizes[-1]:] = rng.uniform(0.1, 3.0, sizes[-1])
+    return dict(k=k, L=L, weighting=0, scoring=0, descriptor_bytes=D, node_ids=ids.astype(np.int32),
+                parent_ids=parents.astype(np.int32), weights=w, descriptors=rng.integers(0, 256, (N, D), np.uint8),
+                word_ids=np.arange(len(leaves), dtype=np.int32), word_nodes=leaves.astype(np.int32))
+
+
+def bow_cases(args, torch, print):
+    """dfk_bow_transform_batch and dfk_bow_database_query_batch against the sequential C oracle on one host thread"""
+    import numpy as np
+
+    from bow_oracle import bow_oracle as bo
+    from deepfactors_b200 import aligners as A
+    vocs = {"small_voc": A.load_dbow2_vocabulary(os.path.join(ROOT, "tests", "golden", "dbow2_small_voc.yml.gz")),
+            "k10_L6": _full_voc(10, 6, 32, 0)}
+    for name, v in vocs.items():
+        gv, ov = A.BowVocabulary(v), bo.Vocabulary(v)
+        D = v["descriptor_bytes"]
+        for n in (1, 8, 64):
+            rng = np.random.default_rng(n)
+            sets = [rng.integers(0, 256, (500, D), np.uint8) for _ in range(n)]
+            dev = [torch.from_numpy(s).cuda() for s in sets]
+            fn = lambda: A.BowTransformBatch(gv, dev)
+            wall = _wall_us(torch, fn, args.reps)
+            dus = _device_us(torch, fn, args.reps)
+            t0 = time.perf_counter()
+            for s in sets:
+                ov.transform(s)
+            host = (time.perf_counter() - t0) * 1e6
+            print(json.dumps({"case": "bow_transform", "vocabulary": name, "words": len(v["word_ids"]), "frames": n,
+                              "features": 500, "device_wall_us": round(wall, 1), "device_us": round(dus, 1),
+                              "oracle_host_us": round(host, 1), "speedup_wall": round(host / wall, 1)}))
+    v = vocs["small_voc"]
+    gv, ov = A.BowVocabulary(v), bo.Vocabulary(v)
+    rng = np.random.default_rng(7)
+    images = [rng.integers(0, 256, (500, 48), np.uint8) for _ in range(100)]
+    b = A.BowTransformBatch(gv, [torch.from_numpy(s).cuda() for s in images])
+    vecs, ovecs = b.vectors(), [ov.transform(s)[1:] for s in images]
+    q = rng.integers(0, 256, (500, 48), np.uint8)
+    qv = A.BowTransformBatch(gv, [torch.from_numpy(q).cuda()]).vectors()
+    qo = ov.transform(q)[1:]
+    for entries in (100, 1000, 10000):
+        db, odb = A.BowDatabase(gv), bo.Database()
+        for s in range(0, entries, 100):
+            db.add(vecs[:min(100, entries - s)])
+        for e in range(entries):
+            odb.add(*ovecs[e % 100])
+        fn = lambda: db.query(qv, 20)
+        wall = _wall_us(torch, fn, args.reps)
+        dus = _device_us(torch, fn, args.reps)
+        t0 = time.perf_counter()
+        odb.query(*qo, 20)
+        host = (time.perf_counter() - t0) * 1e6
+        print(json.dumps({"case": "bow_query", "entries": entries, "max_results": 20, "device_wall_us": round(wall, 1),
+                          "device_us": round(dus, 1), "oracle_host_us": round(host, 1),
+                          "speedup_wall": round(host / wall, 1)}))
 
 
 def preprocess_cases(args, torch, print):
