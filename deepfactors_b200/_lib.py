@@ -155,6 +155,12 @@ class DfkOrbItem(C.Structure):
 
 
 ORB_MAX_SIDE = 16384  # DFK_ORB_MAX_SIDE
+ORB_MAX_LEVELS = 16  # DFK_ORB_MAX_LEVELS
+
+
+class DfkOrbPyramidItem(C.Structure):
+    _fields_ = [("image", DfkImage), ("nfeatures", C.c_int32), ("scale_factor", C.c_float), ("nlevels", C.c_int32),
+                ("fast_threshold", C.c_int32), ("capacity", C.c_int32)]
 PREPROCESS_MAX_LEVELS = 15  # DFK_PREPROCESS_MAX_LEVELS
 
 
@@ -281,6 +287,8 @@ SYMBOLS = {
                                                C.c_void_p]),
     "dfk_orb_detect_batch": (C.c_int, [_H, C.POINTER(DfkOrbItem), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p]),
+    "dfk_orb_detect_pyramid_batch": (C.c_int, [_H, C.POINTER(DfkOrbPyramidItem), C.c_int, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dfk_update_depth": (C.c_int, [_H, _F, C.c_int, _IMG, _IMG, C.c_float, _IMG]),
     "dfk_update_depth_batch": (C.c_int, [_H, C.POINTER(DfkDepthDecodeItem), C.c_int, C.c_int]),
     "dfk_sobel_gradients": (C.c_int, [_H, _IMG, _IMG]),

@@ -572,6 +572,7 @@ class OrbBatch:
     counts: torch.Tensor
     offsets: np.ndarray
     capacities: np.ndarray
+    _call = "OrbDetectBatch"  # the call named by host_counts' error
 
     def host_counts(self) -> np.ndarray:
         """The counts on the host (synchronises with the stream); raises when an image's count exceeds its capacity,
@@ -580,7 +581,7 @@ class OrbBatch:
         over = np.nonzero(c > self.capacities)[0]
         if len(over):
             i = int(over[0])
-            raise RuntimeError(f"OrbDetectBatch: image {i} has {int(c[i])} keypoints (ties at the cut) but capacity "
+            raise RuntimeError(f"{self._call}: image {i} has {int(c[i])} keypoints (ties at the cut) but capacity "
                                f"{int(self.capacities[i])}; pass a larger capacity")
         return c
 
@@ -632,6 +633,52 @@ def OrbDetectBatch(aligner, images: Sequence[torch.Tensor], nfeatures: int = REP
                                            C.c_void_p(ang.data_ptr()), C.c_void_p(resp.data_ptr()),
                                            C.c_void_p(counts.data_ptr())))
     return OrbBatch(kp[:rows], desc[:rows], ang[:rows], resp[:rows], counts[:n], offsets, np.array(cap, np.int64))
+
+
+@dataclass
+class OrbPyramidBatch(OrbBatch):
+    """The device output of OrbDetectPyramidBatch: OrbBatch's fields, item i's rows in level order (each level in the
+    one-level order), keypoints at level 0, plus octaves [rows] int32 (each row's level)."""
+    octaves: torch.Tensor = None
+    _call = "OrbDetectPyramidBatch"
+
+
+def OrbDetectPyramidBatch(aligner, images: Sequence[torch.Tensor], nfeatures: int = REP_NFEATURES,
+                          scale_factor: float = 1.2, nlevels: int = 8, fast_threshold: int = ORB_FAST_THRESHOLD,
+                          capacity: int | None = None) -> OrbPyramidBatch:
+    """cv::ORB_create(nfeatures, scale_factor, nlevels).detectAndCompute of many gray images in one call
+    (dfk_orb_detect_pyramid_batch): the reference's OrbDetector with rep_nlevels > 1, bit for bit.  images: uint8
+    [H, W] CUDA tensors of any sizes; every setting is one value for all images or one per image, capacity by default
+    2 nfeatures.  Asynchronous: returns an OrbPyramidBatch of device tensors; .features() feeds HammingMatchBatch,
+    ReprojectionMatchBatch, window_opt.match_reprojection_links and BowTransformBatch as OrbDetectBatch's does."""
+    hd = aligner._hd
+    hd.use_torch_stream()
+    n = len(images)
+    per = lambda v, f=int: [f(x) for x in (v if isinstance(v, (list, tuple, np.ndarray)) else [v] * n)]
+    nf, s, nl, t = per(nfeatures), per(scale_factor, float), per(nlevels), per(fast_threshold)
+    cap = per(capacity) if capacity is not None else [2 * x for x in nf]
+    if not (len(nf) == len(s) == len(nl) == len(t) == len(cap) == n):
+        raise ValueError("OrbDetectPyramidBatch: per-image settings need one entry per image")
+    for im in images:
+        if im.device != torch.device("cuda", hd.device):
+            raise ValueError(f"OrbDetectPyramidBatch: images must be on cuda:{hd.device}")
+    arr = (_lib.DfkOrbPyramidItem * max(n, 1))(*[_lib.DfkOrbPyramidItem(_orb_image(im), a, b, c, d, e)
+                                                 for im, a, b, c, d, e in zip(images, nf, s, nl, t, cap)])
+    offsets = np.concatenate([[0], np.cumsum(cap)]).astype(np.int64)
+    rows = int(offsets[-1])
+    dev = f"cuda:{hd.device}"
+    kp = torch.zeros((max(rows, 1), 2), dtype=torch.float32, device=dev)  # rows past a count stay 0
+    desc = torch.zeros((max(rows, 1), 32), dtype=torch.uint8, device=dev)
+    ang = torch.zeros(max(rows, 1), dtype=torch.float32, device=dev)
+    resp = torch.zeros(max(rows, 1), dtype=torch.float32, device=dev)
+    octv = torch.zeros(max(rows, 1), dtype=torch.int32, device=dev)
+    counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    check(hd.h, lib().dfk_orb_detect_pyramid_batch(hd.h, arr, n, C.c_void_p(kp.data_ptr()),
+                                                   C.c_void_p(desc.data_ptr()), C.c_void_p(ang.data_ptr()),
+                                                   C.c_void_p(resp.data_ptr()), C.c_void_p(octv.data_ptr()),
+                                                   C.c_void_p(counts.data_ptr())))
+    return OrbPyramidBatch(kp[:rows], desc[:rows], ang[:rows], resp[:rows], counts[:n], offsets,
+                           np.array(cap, np.int64), octv[:rows])
 
 
 # ------------------------------------------------------------------------------------------- frame preprocessing

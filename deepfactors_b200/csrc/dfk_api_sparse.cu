@@ -7,11 +7,13 @@
 #include <algorithm>
 #include <cmath>
 #include <string>
+#include <vector>
 
 #include "dfk.h"
 #include "dfk_host.h"
 #include "dfk_internal.h"
 #include "dfk_orb_model.h"
+#include "dfk_orb_pyramid_model.h"
 
 using namespace dfk;
 
@@ -193,6 +195,96 @@ DfkStatus dfk_reprojection_match_batch(DfkHandle h, const DfkMatchItem* items, i
   });
 }
 
+}  // extern "C"
+
+namespace {
+
+// The one-level detector's plan over its items (images, or (image, level) pairs of a pyramid): each item's
+// OrbItemDev and the scratch sizes and launch shape of the batch.
+struct OrbPlan {
+  long long rows = 0, segs = 0, corners = 0, map = 0, blur = 0;
+  int max_rw = 0, max_rh = 0, max_cc = 0, max_segs = 0, max_cap = 0, max_nf = 0;
+
+  // An item of w x h pixels (its image pointer is set by the caller); its rows follow the rows before it
+  void add(OrbItemDev& d, int w, int h, int nfeatures, int threshold, int capacity)
+  {
+    const bool big = w >= DFK_OM_MIN_SIZE && h >= DFK_OM_MIN_SIZE;
+    d = OrbItemDev{};
+    d.rw = big ? w - 2 * DFK_OM_EDGE : 0;
+    d.rh = big ? h - 2 * DFK_OM_EDGE : 0;
+    d.tiles_x = (d.rw + kOrbTileW - 1) / kOrbTileW;
+    d.tiles_y = (d.rh + kOrbTileH - 1) / kOrbTileH;
+    d.nfeatures = nfeatures;
+    d.threshold = threshold;
+    d.capacity = capacity;
+    d.out_begin = (int)std::min(rows, (long long)INT32_MAX);
+    d.map_begin = (size_t)map;
+    d.seg_begin = (int)std::min(segs, (long long)INT32_MAX);
+    d.corner_begin = (int)std::min(corners, (long long)INT32_MAX);
+    d.corner_cap = ((d.rw + 1) / 2) * ((d.rh + 1) / 2);  // one corner per 2 x 2 pixels at most survives NMS
+    d.blur_begin = (size_t)blur;
+    rows += capacity;
+    segs += (long long)d.rh * d.tiles_x;
+    corners += d.corner_cap;
+    map += (long long)d.rw * d.rh;
+    if (big) blur += (long long)(d.rw + 2 * DFK_OM_PATTERN_R) * (d.rh + 2 * DFK_OM_PATTERN_R);
+    max_rw = std::max(max_rw, d.rw);
+    max_rh = std::max(max_rh, d.rh);
+    max_cc = std::max(max_cc, d.corner_cap);
+    max_segs = std::max(max_segs, d.rh * d.tiles_x);
+    max_cap = std::max(max_cap, capacity);
+    max_nf = std::max(max_nf, nfeatures);
+  }
+  bool too_big() const { return rows > INT32_MAX || corners > INT32_MAX || segs > INT32_MAX; }
+
+  // one allocation for n items: [hist | stats | segments | corner positions | keys | angles | row map | score maps |
+  // blurred images], 16-byte parts
+  static size_t part(size_t bytes) { return (bytes + 15) & ~(size_t)15; }
+  size_t bytes(int n) const
+  {
+    return part(sizeof(int) * 256 * (size_t)n) + part(sizeof(int) * 4 * (size_t)n) + part(sizeof(int) * (size_t)segs) +
+           3 * part(sizeof(uint32_t) * (size_t)corners) + part(sizeof(int) * (size_t)rows) + part((size_t)map) +
+           part((size_t)blur);
+  }
+  OrbScratchDev layout(unsigned char* p, int n) const
+  {
+    const size_t b_c = part(sizeof(uint32_t) * (size_t)corners);
+    OrbScratchDev s;
+    s.hist = reinterpret_cast<int*>(p);
+    s.stats = reinterpret_cast<int*>(p += part(sizeof(int) * 256 * (size_t)n));
+    s.seg = reinterpret_cast<int*>(p += part(sizeof(int) * 4 * (size_t)n));
+    s.pos = reinterpret_cast<uint32_t*>(p += part(sizeof(int) * (size_t)segs));
+    s.key = reinterpret_cast<uint32_t*>(p += b_c);
+    s.angle = reinterpret_cast<float*>(p += b_c);
+    s.rows = reinterpret_cast<int*>(p += b_c);
+    s.map = p += part(sizeof(int) * (size_t)rows);
+    s.blur = p + part((size_t)map);
+    return s;
+  }
+  cudaError_t launch(const OrbItemDev* items_dev, int n, const OrbScratchDev& s, float* keypoints,
+                     uint8_t* descriptors, float* angles, float* responses, int* counts, cudaStream_t stream) const
+  {
+    return launch_orb_detect(items_dev, n, s, max_rw, max_rh, max_cc, max_segs, max_cap, max_nf, keypoints,
+                             descriptors, angles, responses, counts, stream);
+  }
+  int launches() const { return max_rw > 0 ? 7 : 5; }
+};
+
+// The checks an ORB item of either call shares; the failure text, or null
+const char* orb_item_error(const DfkImage& im, int nfeatures, int fast_threshold, int capacity)
+{
+  if (!im.ptr || im.width > DFK_ORB_MAX_SIDE || im.height > DFK_ORB_MAX_SIDE || im.pitch_bytes < im.width)
+    return "image needs a pointer, width and height <= DFK_ORB_MAX_SIDE and pitch_bytes >= width";
+  if (nfeatures < 1 || nfeatures > DFK_MATCH_MAX_QUERIES) return "nfeatures not in [1, DFK_MATCH_MAX_QUERIES]";
+  if (fast_threshold < 0 || fast_threshold > 255) return "fast_threshold not in [0, 255]";
+  if (capacity < nfeatures) return "capacity < nfeatures";
+  return nullptr;
+}
+
+}  // namespace
+
+extern "C" {
+
 DfkStatus dfk_orb_detect_batch(DfkHandle h, const DfkOrbItem* items, int n, float* keypoints_dev,
                                uint8_t* descriptors_dev, float* angles_dev, float* responses_dev, int32_t* counts_dev)
 {
@@ -206,81 +298,179 @@ DfkStatus dfk_orb_detect_batch(DfkHandle h, const DfkOrbItem* items, int n, floa
         ((uintptr_t)responses_dev & 3) || ((uintptr_t)counts_dev & 3))
       return fail(h, DFK_ERR_INVALID_ARG, w + "descriptors must be 16-byte aligned, the other outputs 4-byte aligned");
     h->orb_host.resize((size_t)n);
-    long long rows = 0, segs = 0, corners = 0, map = 0, blur = 0;
-    int max_rw = 0, max_rh = 0, max_cc = 0, max_segs = 0, max_cap = 0, max_nf = 0;
+    OrbPlan plan;
     for (int i = 0; i < n; ++i) {
       const DfkOrbItem& it = items[i];
-      const std::string at = " in item " + std::to_string(i);
-      if (!it.image.ptr || it.image.width > DFK_ORB_MAX_SIDE || it.image.height > DFK_ORB_MAX_SIDE ||
-          it.image.pitch_bytes < it.image.width)
-        return fail(h, DFK_ERR_INVALID_ARG, w + "image needs a pointer, width and height <= DFK_ORB_MAX_SIDE and "
-                                                "pitch_bytes >= width" + at);
-      if (it.nfeatures < 1 || it.nfeatures > DFK_MATCH_MAX_QUERIES)
-        return fail(h, DFK_ERR_INVALID_ARG, w + "nfeatures not in [1, DFK_MATCH_MAX_QUERIES]" + at);
-      if (it.fast_threshold < 0 || it.fast_threshold > 255)
-        return fail(h, DFK_ERR_INVALID_ARG, w + "fast_threshold not in [0, 255]" + at);
-      if (it.capacity < it.nfeatures)
-        return fail(h, DFK_ERR_INVALID_ARG, w + "capacity < nfeatures" + at);
-      const bool big = it.image.width >= DFK_OM_MIN_SIZE && it.image.height >= DFK_OM_MIN_SIZE;
+      if (const char* e = orb_item_error(it.image, it.nfeatures, it.fast_threshold, it.capacity))
+        return fail(h, DFK_ERR_INVALID_ARG, w + e + " in item " + std::to_string(i));
       OrbItemDev& d = h->orb_host[(size_t)i];
-      d = OrbItemDev{};
+      plan.add(d, (int)it.image.width, (int)it.image.height, it.nfeatures, it.fast_threshold, it.capacity);
       d.img = static_cast<const uint8_t*>(it.image.ptr);
       d.pitch = it.image.pitch_bytes;
-      d.rw = big ? (int)it.image.width - 2 * DFK_OM_EDGE : 0;
-      d.rh = big ? (int)it.image.height - 2 * DFK_OM_EDGE : 0;
-      d.tiles_x = (d.rw + kOrbTileW - 1) / kOrbTileW;
-      d.tiles_y = (d.rh + kOrbTileH - 1) / kOrbTileH;
-      d.nfeatures = it.nfeatures;
-      d.threshold = it.fast_threshold;
-      d.capacity = it.capacity;
-      d.out_begin = (int)std::min(rows, (long long)INT32_MAX);
-      d.map_begin = (size_t)map;
-      d.seg_begin = (int)std::min(segs, (long long)INT32_MAX);
-      d.corner_begin = (int)std::min(corners, (long long)INT32_MAX);
-      d.corner_cap = ((d.rw + 1) / 2) * ((d.rh + 1) / 2);  // one corner per 2 x 2 pixels at most survives NMS
-      d.blur_begin = (size_t)blur;
-      rows += it.capacity;
-      segs += (long long)d.rh * d.tiles_x;
-      corners += d.corner_cap;
-      map += (long long)d.rw * d.rh;
-      if (big) blur += (long long)(d.rw + 2 * DFK_OM_PATTERN_R) * (d.rh + 2 * DFK_OM_PATTERN_R);
-      max_rw = std::max(max_rw, d.rw);
-      max_rh = std::max(max_rh, d.rh);
-      max_cc = std::max(max_cc, d.corner_cap);
-      max_segs = std::max(max_segs, d.rh * d.tiles_x);
-      max_cap = std::max(max_cap, it.capacity);
-      max_nf = std::max(max_nf, it.nfeatures);
     }
-    if (rows > INT32_MAX || corners > INT32_MAX || segs > INT32_MAX)
+    if (plan.too_big())
       return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 output rows or scratch entries in one call");
     DeviceGuard guard(h->device);
-    // one allocation: [hist | stats | segments | corner positions | keys | angles | row map | score maps | blurred
-    // images], 16-byte parts
-    auto part = [](size_t bytes) { return (bytes + 15) & ~(size_t)15; };
-    const size_t b_hist = part(sizeof(int) * 256 * (size_t)n), b_stats = part(sizeof(int) * 4 * (size_t)n);
-    const size_t b_seg = part(sizeof(int) * (size_t)segs), b_c = part(sizeof(uint32_t) * (size_t)corners);
-    const size_t b_rows = part(sizeof(int) * (size_t)rows), b_map = part((size_t)map), b_blur = part((size_t)blur);
     DFK_CUDA(h, h->orb_items.ensure((size_t)n), "[OrbDetector batch] scratch allocation failed");
-    DFK_CUDA(h, h->orb_scratch.ensure(b_hist + b_stats + b_seg + 3 * b_c + b_rows + b_map + b_blur),
-             "[OrbDetector batch] scratch allocation failed");
-    unsigned char* p = h->orb_scratch.ptr;
-    OrbScratchDev s;
-    s.hist = reinterpret_cast<int*>(p);
-    s.stats = reinterpret_cast<int*>(p += b_hist);
-    s.seg = reinterpret_cast<int*>(p += b_stats);
-    s.pos = reinterpret_cast<uint32_t*>(p += b_seg);
-    s.key = reinterpret_cast<uint32_t*>(p += b_c);
-    s.angle = reinterpret_cast<float*>(p += b_c);
-    s.rows = reinterpret_cast<int*>(p += b_c);
-    s.map = p += b_rows;
-    s.blur = p + b_map;
+    DFK_CUDA(h, h->orb_scratch.ensure(plan.bytes(n)), "[OrbDetector batch] scratch allocation failed");
+    const OrbScratchDev s = plan.layout(h->orb_scratch.ptr, n);
     DFK_CUDA(h, cudaMemcpyAsync(h->orb_items.ptr, h->orb_host.data(), sizeof(OrbItemDev) * (size_t)n,
                                 cudaMemcpyHostToDevice, h->stream),
              "[OrbDetector batch] upload failed");
-    DFK_CUDA(h, launch_orb_detect(h->orb_items.ptr, n, s, max_rw, max_rh, max_cc, max_segs, max_cap, max_nf,
-                                  keypoints_dev, descriptors_dev, angles_dev, responses_dev, counts_dev, h->stream),
+    DFK_CUDA(h, plan.launch(h->orb_items.ptr, n, s, keypoints_dev, descriptors_dev, angles_dev, responses_dev,
+                            counts_dev, h->stream),
              "[OrbDetector batch] kernel launch failed");
-    h->launches += max_rw > 0 ? 7 : 5;
+    h->launches += plan.launches();
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_orb_detect_pyramid_batch(DfkHandle h, const DfkOrbPyramidItem* items, int n, float* keypoints_dev,
+                                       uint8_t* descriptors_dev, float* angles_dev, float* responses_dev,
+                                       int32_t* octaves_dev, int32_t* counts_dev)
+{
+  static_assert(kOrbMaxLevels == DFK_ORB_MAX_LEVELS && DFK_OPM_MAX_LEVELS == DFK_ORB_MAX_LEVELS, "level bound");
+  return guarded(h, [&] {
+    const std::string w = "[OrbDetector pyramid batch] ";
+    if (!items || n < 1 || n > 65535)  // gridDim.y of the gather kernel is the item
+      return fail(h, DFK_ERR_INVALID_ARG, w + "null argument / number of items not in [1, 65535]");
+    if (!keypoints_dev || !descriptors_dev || !counts_dev)
+      return fail(h, DFK_ERR_INVALID_ARG, w + "null keypoint, descriptor or count output");
+    if (((uintptr_t)keypoints_dev & 3) || ((uintptr_t)descriptors_dev & 15) || ((uintptr_t)angles_dev & 3) ||
+        ((uintptr_t)responses_dev & 3) || ((uintptr_t)octaves_dev & 3) || ((uintptr_t)counts_dev & 3))
+      return fail(h, DFK_ERR_INVALID_ARG, w + "descriptors must be 16-byte aligned, the other outputs 4-byte aligned");
+    // validation, and each item's levels: one one-level item per (image, level), level images for k >= 1 while they
+    // are at least 63 x 63 (a smaller level and every level after it has no features)
+    long long subs = 0, out_rows = 0;
+    for (int i = 0; i < n; ++i) {
+      const DfkOrbPyramidItem& it = items[i];
+      const std::string at = " in item " + std::to_string(i);
+      if (const char* e = orb_item_error(it.image, it.nfeatures, it.fast_threshold, it.capacity))
+        return fail(h, DFK_ERR_INVALID_ARG, w + e + at);
+      if (!(std::isfinite(it.scale_factor) && it.scale_factor > 1.0f))
+        return fail(h, DFK_ERR_INVALID_ARG, w + "scale_factor must be finite and > 1" + at);
+      if (it.nlevels < 1 || it.nlevels > DFK_ORB_MAX_LEVELS)
+        return fail(h, DFK_ERR_INVALID_ARG, w + "nlevels not in [1, DFK_ORB_MAX_LEVELS]" + at);
+      subs += it.nlevels;
+      out_rows += it.capacity;
+    }
+    if (subs > 65535)  // gridDim.z of the FAST kernel is the (image, level) item
+      return fail(h, DFK_ERR_INVALID_ARG, w + "more than 65535 levels over the items of one call");
+    if (out_rows > INT32_MAX) return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 output rows in one call");
+    std::vector<OrbItemDev>& sub = h->orb_host;
+    sub.resize((size_t)subs);
+    std::vector<OrbGatherDev> gather((size_t)n);
+    // the resize items by level, their source and destination as offsets into the level images until those are
+    // allocated (SIZE_MAX: the caller's image)
+    struct LevelJob {
+      OrbResizeDev r;
+      size_t src, dst;
+      const void* image;
+    };
+    std::vector<std::vector<LevelJob>> resize(DFK_ORB_MAX_LEVELS);
+    std::vector<size_t> sub_level((size_t)subs, SIZE_MAX);  // each (image, level)'s image, as above
+    OrbPlan plan;
+    size_t level_bytes = 0;
+    for (int i = 0, sb = 0; i < n; sb += items[i].nlevels, ++i) {
+      const DfkOrbPyramidItem& it = items[i];
+      int budget[DFK_ORB_MAX_LEVELS];
+      dfk_opm_budgets(it.nfeatures, it.scale_factor, it.nlevels, budget);
+      OrbGatherDev& g = gather[(size_t)i];
+      g = OrbGatherDev{};
+      g.sub_begin = sb;
+      g.nlevels = it.nlevels;
+      g.out_begin = i ? gather[(size_t)i - 1].out_begin + items[i - 1].capacity : 0;
+      g.capacity = it.capacity;
+      const int W = (int)it.image.width, H = (int)it.image.height;
+      int pw = W, ph = H;
+      for (int k = 0; k < it.nlevels; ++k) {
+        g.scale[k] = dfk_opm_level_scale(it.scale_factor, k);
+        const int lw = k ? dfk_opm_level_size(W, g.scale[k]) : W, lh = k ? dfk_opm_level_size(H, g.scale[k]) : H;
+        const bool built = lw >= DFK_OM_MIN_SIZE && lh >= DFK_OM_MIN_SIZE;
+        if (built && k) {
+          const size_t src = sub_level[(size_t)sb + k - 1];
+          const size_t src_pitch = src == SIZE_MAX ? it.image.pitch_bytes : (size_t)pw;
+          resize[(size_t)k].push_back(LevelJob{OrbResizeDev{nullptr, src_pitch, nullptr, pw, ph, lw, lh}, src,
+                                               level_bytes, it.image.ptr});
+          sub_level[(size_t)sb + k] = level_bytes;
+          level_bytes += (size_t)lw * lh;
+        }
+        // a level with no budget, or too small, is an empty item
+        const bool live = built && budget[k] > 0;
+        plan.add(sub[(size_t)sb + k], live ? lw : 0, live ? lh : 0, budget[k], it.fast_threshold, it.capacity);
+        sub[(size_t)sb + k].pitch = k && built ? (size_t)lw : it.image.pitch_bytes;
+        pw = lw;
+        ph = lh;
+      }
+    }
+    if (plan.too_big())
+      return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 staged rows or scratch entries in one call");
+    DeviceGuard guard(h->device);
+    // the detector's scratch, then [level images | staged keypoints | descriptors | angles | responses | counts]
+    const size_t srows = (size_t)plan.rows, b_det = plan.bytes((int)subs), b_lev = OrbPlan::part(level_bytes);
+    const size_t b_kp = OrbPlan::part(sizeof(float) * 2 * srows), b_desc = OrbPlan::part(32 * srows);
+    const size_t b_f = OrbPlan::part(sizeof(float) * srows), b_cnt = OrbPlan::part(sizeof(int) * (size_t)subs);
+    DFK_CUDA(h, h->orb_scratch.ensure(b_det + b_lev + b_kp + b_desc + 2 * b_f + b_cnt),
+             "[OrbDetector pyramid batch] scratch allocation failed");
+    unsigned char* base = h->orb_scratch.ptr;
+    const OrbScratchDev s = plan.layout(base, (int)subs);
+    unsigned char* levels = base + b_det;
+    float* st_kp = reinterpret_cast<float*>(levels + b_lev);
+    uint8_t* st_desc = reinterpret_cast<uint8_t*>(st_kp) + b_kp;
+    float* st_ang = reinterpret_cast<float*>(st_desc + b_desc);
+    float* st_resp = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(st_ang) + b_f);
+    int* st_cnt = reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(st_resp) + b_f);
+    auto level_ptr = [&](size_t off, const void* image) {
+      return off == SIZE_MAX ? static_cast<const uint8_t*>(image) : static_cast<const uint8_t*>(levels + off);
+    };
+    // one upload: [one-level items | gather items | resize items by level]
+    size_t nres = 0;
+    for (const auto& v : resize) nres += v.size();
+    const size_t b_sub = OrbPlan::part(sizeof(OrbItemDev) * (size_t)subs);
+    const size_t b_gat = OrbPlan::part(sizeof(OrbGatherDev) * (size_t)n);
+    std::vector<unsigned char>& host = h->orb_pyr_host;
+    host.assign(b_sub + b_gat + sizeof(OrbResizeDev) * nres, 0);
+    for (int i = 0, sb = 0; i < n; sb += items[i].nlevels, ++i)
+      for (int k = 0; k < items[i].nlevels; ++k)
+        sub[(size_t)sb + k].img = level_ptr(sub_level[(size_t)sb + k], items[i].image.ptr);
+    memcpy(host.data(), sub.data(), sizeof(OrbItemDev) * (size_t)subs);
+    memcpy(host.data() + b_sub, gather.data(), sizeof(OrbGatherDev) * (size_t)n);
+    OrbResizeDev* rh = reinterpret_cast<OrbResizeDev*>(host.data() + b_sub + b_gat);
+    for (const std::vector<LevelJob>& v : resize)
+      for (const LevelJob& job : v) {
+        *rh = job.r;
+        rh->src = level_ptr(job.src, job.image);
+        rh->dst = levels + job.dst;
+        ++rh;
+      }
+    DFK_CUDA(h, h->orb_pyr_dev.ensure(host.size()), "[OrbDetector pyramid batch] scratch allocation failed");
+    DFK_CUDA(h, cudaMemcpyAsync(h->orb_pyr_dev.ptr, host.data(), host.size(), cudaMemcpyHostToDevice, h->stream),
+             "[OrbDetector pyramid batch] upload failed");
+    const OrbItemDev* sub_dev = reinterpret_cast<const OrbItemDev*>(h->orb_pyr_dev.ptr);
+    const OrbGatherDev* gat_dev = reinterpret_cast<const OrbGatherDev*>(h->orb_pyr_dev.ptr + b_sub);
+    const OrbResizeDev* res_dev = reinterpret_cast<const OrbResizeDev*>(h->orb_pyr_dev.ptr + b_sub + b_gat);
+    // the chain of levels: level k of every image from its level k - 1
+    for (int k = 1, j = 0; k < DFK_ORB_MAX_LEVELS; ++k) {
+      const std::vector<LevelJob>& v = resize[(size_t)k];
+      if (v.empty()) continue;
+      int mw = 0, mh = 0;
+      for (const LevelJob& job : v) {
+        mw = std::max(mw, job.r.dw);
+        mh = std::max(mh, job.r.dh);
+      }
+      DFK_CUDA(h, launch_orb_resize_level(res_dev + j, (int)v.size(), mw, mh, h->stream),
+               "[OrbDetector pyramid batch] kernel launch failed");
+      j += (int)v.size();
+      h->launches += 1;
+    }
+    DFK_CUDA(h, plan.launch(sub_dev, (int)subs, s, st_kp, st_desc, st_ang, st_resp, st_cnt, h->stream),
+             "[OrbDetector pyramid batch] kernel launch failed");
+    h->launches += plan.launches();
+    const OrbStagingDev st{st_kp, st_desc, st_ang, st_resp, st_cnt};
+    DFK_CUDA(h, launch_orb_gather(gat_dev, n, sub_dev, st, plan.max_cap, keypoints_dev, descriptors_dev, angles_dev,
+                                  responses_dev, octaves_dev, counts_dev, h->stream),
+             "[OrbDetector pyramid batch] kernel launch failed");
+    h->launches += 1;
     return DFK_OK;
   });
 }

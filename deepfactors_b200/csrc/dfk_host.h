@@ -111,6 +111,10 @@ struct DfkContext {
   DeviceBuf<OrbItemDev> orb_items;
   std::vector<OrbItemDev> orb_host;
   DeviceBuf<unsigned char> orb_scratch;
+  // dfk_orb_detect_pyramid_batch: [one-level items | gather items | resize items] (bytes, one H2D per call from
+  // orb_pyr_host); its level images and staged rows follow the detector's scratch in orb_scratch
+  DeviceBuf<unsigned char> orb_pyr_dev;
+  std::vector<unsigned char> orb_pyr_host;
   // dfk_preprocess_batch: [item descriptors | pyramid level descriptors L x n] (bytes, one H2D per call from pp_host)
   // and the normalising items' tile partials
   DeviceBuf<unsigned char> pp_dev;

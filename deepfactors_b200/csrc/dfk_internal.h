@@ -478,6 +478,36 @@ cudaError_t launch_orb_detect(const OrbItemDev* items_dev, int n, const OrbScrat
                               float* keypoints, uint8_t* descriptors, float* angles, float* responses, int* counts,
                               cudaStream_t stream);
 
+// dfk_orb_detect_pyramid_batch (dfk_orb_pyramid.cu).  One level k >= 1 of one image: dst (dw x dh, pitch dw) is src
+// (sw x sh, the image's level k - 1) resized.
+struct OrbResizeDev {
+  const uint8_t* src;
+  size_t src_pitch;
+  uint8_t* dst;
+  int sw, sh, dw, dh;
+};
+constexpr int kOrbMaxLevels = 16;  // DFK_ORB_MAX_LEVELS
+// One image: its levels are the one-level items sub_begin .. sub_begin + nlevels - 1, whose rows and counts the
+// detector wrote to the staging arrays; the gather places them at out_begin in level order.
+struct OrbGatherDev {
+  int sub_begin, nlevels;
+  int out_begin, capacity;
+  float scale[kOrbMaxLevels];  // s_k
+};
+// The staged rows of the one-level items, indexed by their out_begin
+struct OrbStagingDev {
+  const float* keypoints;
+  const uint8_t* descriptors;
+  const float* angles;
+  const float* responses;
+  const int* counts;  // per one-level item
+};
+// one level of every image that has it: count resize items, max_w x max_h their largest output
+cudaError_t launch_orb_resize_level(const OrbResizeDev* items_dev, int count, int max_w, int max_h, cudaStream_t stream);
+cudaError_t launch_orb_gather(const OrbGatherDev* items_dev, int n, const OrbItemDev* subs_dev, const OrbStagingDev& st,
+                              int max_capacity, float* keypoints, uint8_t* descriptors, float* angles,
+                              float* responses, int32_t* octaves, int32_t* counts, cudaStream_t stream);
+
 // one frame of dfk_preprocess_batch (dfk_preprocess.cu): the output (w x h) is cut into tiles of DFK_PM_TILE_W x
 // DFK_PM_TILE_H pixels, one CTA each; pitches in bytes for the uint8 images, in floats for level 0
 struct PpItemDev {

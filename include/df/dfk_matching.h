@@ -10,6 +10,8 @@
 //                                 queryIdx), the order the device lists have
 //   df::OrbDetector               the keypoints and descriptors themselves: OrbDetector(nfeatures, scale_factor, 1)
 //     .DetectAndCompute           of features/feature_detection.h for one device image or a batch (dfk_orb_detect_batch)
+//   df::OrbPyramidDetector        OrbDetector(nfeatures, scale_factor, nlevels) with any nlevels (rep_nlevels > 1)
+//     .DetectAndCompute           likewise, through dfk_orb_detect_pyramid_batch
 // The host-vector members copy their results back with the CUDA runtime; they exist where its header does.
 #ifndef DFK_MATCHING_H_
 #define DFK_MATCHING_H_
@@ -217,6 +219,91 @@ private:
 
 private:
   int nfeatures_, fast_threshold_;
+  detail::HandlePtr h_;
+};
+
+// The reference's OrbDetector with a scale pyramid: cv::ORB::create(nfeatures, scale_factor, nlevels), 1 <= nlevels <=
+// DFK_ORB_MAX_LEVELS, scale_factor > 1, through dfk_orb_detect_pyramid_batch.  Keypoints come at level 0 in the
+// device order (levels ascending, each by response descending, then y, then x), as df::Features views.
+class OrbPyramidDetector
+{
+public:
+  explicit OrbPyramidDetector(int nfeatures = 500, float scale_factor = 1.2f, int nlevels = 8, int fast_threshold = 20)
+      : nfeatures_(nfeatures), nlevels_(nlevels), fast_threshold_(fast_threshold), scale_factor_(scale_factor),
+        h_(detail::MakeHandle())
+  {
+  }
+
+  DfkHandle handle() const { return h_.get(); }
+  void SetStream(void* stream) { detail::Check(h_.get(), dfk_set_stream(h_.get(), stream)); }
+  int nfeatures() const { return nfeatures_; }
+  int nlevels() const { return nlevels_; }
+  float scale_factor() const { return scale_factor_; }
+  // rows reserved per image: ties at the response cuts can add keypoints past nfeatures
+  int capacity() const { return 2 * nfeatures_; }
+
+  DfkOrbPyramidItem Item(const DfkImage& image) const
+  {
+    return DfkOrbPyramidItem{image, nfeatures_, scale_factor_, nlevels_, fast_threshold_, capacity()};
+  }
+
+  // dfk_orb_detect_pyramid_batch into the caller's DEVICE buffers (rows at the prefix sums of the items' capacities)
+  void DetectBatch(const std::vector<DfkOrbPyramidItem>& items, float* keypoints_dev, uint8_t* descriptors_dev,
+                   float* angles_dev, float* responses_dev, int32_t* octaves_dev, int32_t* counts_dev)
+  {
+    detail::Check(h_.get(), dfk_orb_detect_pyramid_batch(h_.get(), items.data(), (int)items.size(), keypoints_dev,
+                                                         descriptors_dev, angles_dev, responses_dev, octaves_dev,
+                                                         counts_dev));
+  }
+
+#ifdef DFK_FACADE_CUDART
+  // FeatureDetector::DetectAndCompute for a device gray image: the features stay valid until the next detection
+  Features DetectAndCompute(const DfkImage& image) { return DetectAndCompute(std::vector<DfkImage>{image})[0]; }
+
+  // every image in one call; waits for the counts
+  std::vector<Features> DetectAndCompute(const std::vector<DfkImage>& images)
+  {
+    const size_t n = images.size(), rows = n * (size_t)capacity();
+    std::vector<DfkOrbPyramidItem> items;
+    for (const DfkImage& im : images) items.push_back(Item(im));
+    if (rows > rows_) {
+      out_.reset();
+      void* p = nullptr;  // [descriptors 32 per row | keypoints 2 floats per row | counts]
+      if (cudaMalloc(&p, rows * 40 + 4 * n + 16) != cudaSuccess)
+        throw std::runtime_error("[OrbPyramidDetector] device allocation failed");
+      out_.reset(static_cast<uint8_t*>(p));
+      rows_ = rows;
+    }
+    uint8_t* desc = out_.get();
+    float* kp = reinterpret_cast<float*>(desc + 32 * rows_);
+    int32_t* counts = reinterpret_cast<int32_t*>(kp + 2 * rows_);
+    DetectBatch(items, kp, desc, nullptr, nullptr, nullptr, counts);
+    std::vector<int32_t> host(n);
+    const cudaStream_t s = static_cast<cudaStream_t>(dfk_get_stream(h_.get()));
+    if (cudaMemcpyAsync(host.data(), counts, n * sizeof(int32_t), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+        cudaStreamSynchronize(s) != cudaSuccess)
+      throw std::runtime_error("[OrbPyramidDetector] count download failed");
+    std::vector<Features> out(n);
+    for (size_t i = 0; i < n; ++i) {
+      if (host[i] > capacity())
+        throw std::runtime_error("[OrbPyramidDetector] more keypoints than the capacity (ties at the response cuts)");
+      const size_t o = i * (size_t)capacity();
+      out[i] = Features{kp + 2 * o, desc + 32 * o, host[i], 32};
+    }
+    return out;
+  }
+
+private:
+  struct Free {
+    void operator()(uint8_t* p) const { cudaFree(p); }
+  };
+  std::unique_ptr<uint8_t, Free> out_;
+  size_t rows_ = 0;
+#endif
+
+private:
+  int nfeatures_, nlevels_, fast_threshold_;
+  float scale_factor_;
   detail::HandlePtr h_;
 };
 

@@ -700,6 +700,42 @@ typedef struct {
 DfkStatus dfk_orb_detect_batch(DfkHandle h, const DfkOrbItem* items, int n, float* keypoints_dev,
                                uint8_t* descriptors_dev, float* angles_dev, float* responses_dev, int32_t* counts_dev);
 
+/* One image of an ORB pyramid batch: cv::ORB::create(nfeatures, scale_factor, nlevels) (the reference's OrbDetector
+ * with rep_nlevels > 1): firstLevel 0, edgeThreshold = patchSize = 31, WTA_K = 2, HARRIS_SCORE. */
+typedef struct {
+  DfkImage image;               /* as DfkOrbItem.image */
+  int32_t nfeatures;            /* in [1, DFK_MATCH_MAX_QUERIES], shared out among the levels */
+  float scale_factor;           /* s: finite, > 1 (cv::ORB's requirement) */
+  int32_t nlevels;              /* L in [1, DFK_ORB_MAX_LEVELS] */
+  int32_t fast_threshold;       /* in [0, 255] */
+  int32_t capacity;             /* output rows reserved for the image, >= nfeatures */
+} DfkOrbPyramidItem;
+#define DFK_ORB_MAX_LEVELS 16
+
+/* cv::ORB::detectAndCompute with L levels of every item, bit for bit (DESIGN.md section 4.9):
+ *   budgets  f = (float)(1 / s), d = nfeatures (1 - f) / (1 - (float)f^L) in fp32; levels 0 .. L - 2 get cvRound(d)
+ *            (d *= f after each), the last max(nfeatures - their sum, 0).
+ *   levels   level k has scale s_k = (float)pow(s, k) and size (cvRound((float)W / s_k), cvRound((float)H / s_k)); level
+ *            0 is the image, level k >= 1 is level k - 1 resized as cv::resize(level k - 1, size_k,
+ *            INTER_LINEAR_EXACT): per side, ratio = dst / src and t = (1 / ratio) (d + 0.5) - 0.5 in fp64, source
+ *            floor(t) with weight rint(256 (t - floor(t))) of the next pixel (clamped to the edge pixel outside), row
+ *            sums in 1/256, the column sum rounded once from 1/65536, half up.
+ *   detect   steps 1-7 of dfk_orb_detect_batch on each level with the level's budget.  A level below 63 x 63 (and every
+ *            level after it) has no features and is not built.
+ *   output   levels ascending, each in dfk_orb_detect_batch's order; a row's keypoint is the level's integer (x, y)
+ *            times s_k in fp32 (KeyPoint::pt at level 0; KeyPoint::size would be 31 s_k), its octave k.
+ * Outputs (DEVICE) as dfk_orb_detect_batch, item i's rows at o_i = the sum of the capacities of the items before i;
+ * octaves_dev int32 [rows], may be NULL.  counts_dev[i] is the true count, the sum of the levels' counts; when ties
+ * push it past capacity only the first capacity rows (lower levels first) are written.  One memset and seven kernels
+ * detect every (image, level) at once, one resize launch per level builds that level of every image, and a gather
+ * kernel places the rows; no floating-point atomics: deterministic, and an item's output depends on the item alone.
+ * With L = 1 the rows are dfk_orb_detect_batch's.  Asynchronous on the handle's stream.  Every item is validated
+ * before anything is enqueued (1 <= n, the sum of the items' levels <= 65535, and the fields above); a rejected call
+ * writes nothing and dfk_last_error names the item and the field. */
+DfkStatus dfk_orb_detect_pyramid_batch(DfkHandle h, const DfkOrbPyramidItem* items, int n, float* keypoints_dev,
+                                       uint8_t* descriptors_dev, float* angles_dev, float* responses_dev,
+                                       int32_t* octaves_dev, int32_t* counts_dev);
+
 /* ------------------------------------------------------------------ cu_image_proc free functions */
 
 /* df::UpdateDepth (cu_image_proc.h:41-44, cu_image_proc.cpp:248-277):

@@ -1,4 +1,5 @@
-/* dfk_orb_oracle.c -- CPU oracle of dfk_orb_detect_batch (include/dfk.h, DESIGN.md section 4.9).
+/* dfk_orb_oracle.c -- CPU oracle of dfk_orb_detect_batch and dfk_orb_detect_pyramid_batch (include/dfk.h, DESIGN.md
+ * section 4.9).
  *
  * TEST INFRASTRUCTURE ONLY.  One image at a time, the eight steps of the specification in order, sequentially:
  *   FAST-9 scores of every pixel, non-maximum suppression, the border, the first cut by FAST score, Harris responses,
@@ -11,6 +12,7 @@
 
 #include "dfk_orb_model.h"
 #include "dfk_orb_pattern.h"
+#include "dfk_orb_pyramid_model.h"
 
 static const int8_t kPattern[DFK_ORB_PATTERN_PAIRS * 4] = {DFK_ORB_PATTERN_DATA};
 
@@ -162,4 +164,84 @@ int dfko_detect(const uint8_t* img, int w, int h, int pitch, int nfeatures, int 
   free(score);
   free(c);
   return n;
+}
+
+/* ------------------------------------------------------------------ the scale pyramid (nlevels > 1) */
+
+/* dst (dw x dh, pitch dw) = src (sw x sh) resized as cv::resize(src, (dw, dh), INTER_LINEAR_EXACT) */
+void dfko_resize(const uint8_t* src, int sw, int sh, int spitch, uint8_t* dst, int dw, int dh)
+{
+  for (int y = 0; y < dh; ++y) {
+    int oy, cy;
+    dfk_opm_tap(y, sh, dh, &oy, &cy);
+    const int oy1 = oy + 1 < sh ? oy + 1 : sh - 1;
+    for (int x = 0; x < dw; ++x) {
+      int ox, cx;
+      dfk_opm_tap(x, sw, dw, &ox, &cx);
+      const int ox1 = ox + 1 < sw ? ox + 1 : sw - 1;
+      const uint8_t* r0 = src + (size_t)oy * spitch;
+      const uint8_t* r1 = src + (size_t)oy1 * spitch;
+      dst[(size_t)y * dw + x] = (uint8_t)dfk_opm_resize_px(r0[ox], r0[ox1], r1[ox], r1[ox1], cx, cy);
+    }
+  }
+}
+
+void dfko_budgets(int n, float s, int L, int32_t* out)
+{
+  int b[DFK_OPM_MAX_LEVELS];
+  dfk_opm_budgets(n, s, L, b);
+  for (int k = 0; k < L; ++k) out[k] = b[k];
+}
+
+/* The detector with L levels of scale factor s on one image: level k (made from level k - 1) runs dfko_detect with
+ * its budget, its rows follow the levels before it with the keypoints scaled to level 0 and octave k.  Writes
+ * min(total, capacity) rows and level_counts[L], and returns the total (-1 if out of memory). */
+int dfko_detect_pyramid(const uint8_t* img, int w, int h, int pitch, int nfeatures, float s, int L, int t, int capacity,
+                        float* keypoints, float* angles, float* responses, uint8_t* descriptors, int32_t* octaves,
+                        int32_t* level_counts)
+{
+  int budget[DFK_OPM_MAX_LEVELS];
+  dfk_opm_budgets(nfeatures, s, L, budget);
+  const uint8_t* prev = img;
+  int pw = w, ph = h, pp = pitch, total = 0;
+  uint8_t* owned = NULL;
+  for (int k = 0; k < L; ++k) {
+    const float scale = dfk_opm_level_scale(s, k);
+    const int lw = k ? dfk_opm_level_size(w, scale) : w, lh = k ? dfk_opm_level_size(h, scale) : h;
+    level_counts[k] = 0;
+    if (lw < DFK_OM_MIN_SIZE || lh < DFK_OM_MIN_SIZE) continue;  /* and so is every later level */
+    if (k) {
+      uint8_t* cur = (uint8_t*)malloc((size_t)lw * lh);
+      if (!cur) {
+        free(owned);
+        return -1;
+      }
+      dfko_resize(prev, pw, ph, pp, cur, lw, lh);
+      free(owned);
+      owned = cur;
+      prev = cur;
+      pw = lw;
+      ph = lh;
+      pp = lw;
+    }
+    if (budget[k] == 0) continue;
+    const int at = total < capacity ? total : capacity;
+    const int n = dfko_detect(prev, pw, ph, pp, budget[k], t, capacity - at, keypoints + 2 * (size_t)at,
+                              angles ? angles + at : NULL, responses ? responses + at : NULL,
+                              descriptors + 32 * (size_t)at);
+    if (n < 0) {
+      free(owned);
+      return -1;
+    }
+    const int rows = n < capacity - at ? n : capacity - at;
+    for (int i = 0; i < rows; ++i) {
+      keypoints[2 * (size_t)(at + i)] *= scale;
+      keypoints[2 * (size_t)(at + i) + 1] *= scale;
+      if (octaves) octaves[at + i] = k;
+    }
+    level_counts[k] = n;
+    total += n;
+  }
+  free(owned);
+  return total;
 }

@@ -50,6 +50,10 @@ One JSON line per case:
     features each: one dfk_orb_detect_batch (OrbDetectBatch; wall clock to a synchronise, summed device time and the
     time of each kernel from a separate profiled run) against cv2.ORB_create(500, 1.2, 1).detectAndCompute on the
     host, one image at a time.
+  * ORB features with a scale pyramid (`--only orb_pyramid`): 1, 8 and 64 gray images at 640x480, 500 features over 8
+    levels of 1.2: one dfk_orb_detect_pyramid_batch (OrbDetectPyramidBatch; wall clock to a synchronise, summed device
+    time and the time of each kernel from a separate profiled run) against the sequential C oracle (orb_oracle) and
+    cv2.ORB_create(500, 1.2, 8).detectAndCompute on the host, one image at a time.
   * frame preprocessing (`--only preprocess`): 1, 8 and 64 colour frames at 640x480 (the 2x pixel repeat of the two
     test images, each copy with its own noise) to the network's 256x192 with 4 levels and gradients: one
     dfk_preprocess_batch through PreprocessBatch (wall clock to a synchronise, output allocations included) and as a bare
@@ -64,7 +68,7 @@ One JSON line per case:
     query scans every entry (no inverted file), so its host time is an upper bound of DBoW2's.
 Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` /
 `--only frames` / `--only slide` / `--only error` / `--only lm` / `--only levels` / `--only match` / `--only orb` /
-`--only preprocess` runs those cases alone.
+`--only orb_pyramid` / `--only preprocess` runs those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -84,7 +88,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error", "lm", "levels",
-                                           "match", "orb", "preprocess", "bow"],
+                                           "match", "orb", "orb_pyramid", "preprocess", "bow"],
                     default=None)
     args = ap.parse_args()
     import numpy as np
@@ -127,6 +131,8 @@ def main():
         return match_cases(args, torch, print)
     if args.only == "orb":
         return orb_cases(args, torch, print)
+    if args.only == "orb_pyramid":
+        return orb_pyramid_cases(args, torch, print)
     if args.only == "preprocess":
         return preprocess_cases(args, torch, print)
     if args.only == "bow":
@@ -1000,6 +1006,61 @@ def orb_cases(args, torch, print):
                 rec.update({"host_us": round(host, 1), "host": f"cv2 {cv2.__version__}, one image at a time",
                             "speedup_wall": round(host / wall, 1), "counts_equal_host": host_counts == list(counts)})
             print(json.dumps(rec))
+
+
+def orb_pyramid_cases(args, torch, print):
+    """dfk_orb_detect_pyramid_batch against the C oracle and cv2.ORB_create(500, 1.2, 8) on the host, image by image"""
+    import numpy as np
+    from torch.profiler import ProfilerActivity, profile
+
+    from deepfactors_b200.aligners import OrbDetectPyramidBatch, SfmAligner
+    try:
+        import cv2
+    except ImportError:  # no cv2 leg then
+        cv2 = None
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from orb_images import images
+    from orb_oracle import orb_oracle as oo
+    z = images()
+    al = SfmAligner(8)
+    base = [z["1047_640"], z["1052_640"]]
+    for n in (1, 8, 64):
+        rng = np.random.default_rng(n)
+        imgs = [np.clip(base[i % 2].astype(np.int16) + rng.integers(-2, 3, base[0].shape), 0, 255).astype(np.uint8)
+                for i in range(n)]
+        dev = [torch.from_numpy(im).cuda() for im in imgs]
+
+        def device():
+            OrbDetectPyramidBatch(al, dev, 500, 1.2, 8, 20)
+
+        wall = _wall_us(torch, device, args.reps)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.reps):
+                device()
+            torch.cuda.synchronize()
+        stages = {}
+        for e in prof.key_averages():
+            if e.self_device_time_total > 0:
+                k = _kernel_name(e.key)
+                stages[k] = round(stages.get(k, 0.0) + e.self_device_time_total / args.reps, 1)
+        dev_us = sum(stages.values())
+        counts = OrbDetectPyramidBatch(al, dev, 500, 1.2, 8, 20).counts.cpu().numpy()
+        t0 = time.perf_counter()
+        oracle_counts = [oo.detect_pyramid(im, 500, 1.2, 8, 20, 1000).count for im in imgs]
+        oracle_us = (time.perf_counter() - t0) * 1e6
+        rec = {"case": f"orb_pyramid_640x480_x{n}", "images": n, "width": 640, "height": 480, "nfeatures": 500,
+               "scale_factor": 1.2, "nlevels": 8, "device_wall_us": round(wall, 1), "device_time_us": round(dev_us, 1),
+               "stages_us": stages, "host_oracle_us": round(oracle_us, 1),
+               "counts_equal_oracle": oracle_counts == list(counts)}
+        if cv2 is not None:
+            orb = cv2.ORB_create(500, 1.2, 8)
+            orb.detectAndCompute(imgs[0], None)
+            t0 = time.perf_counter()
+            host_counts = [len(orb.detectAndCompute(im, None)[0]) for im in imgs]
+            host = (time.perf_counter() - t0) * 1e6
+            rec.update({"host_us": round(host, 1), "host": f"cv2 {cv2.__version__}, one image at a time",
+                        "speedup_wall": round(host / wall, 1), "counts_equal_host": host_counts == list(counts)})
+        print(json.dumps(rec))
 
 
 def _full_voc(k: int, L: int, D: int, seed: int) -> dict:
