@@ -263,7 +263,9 @@ DfkStatus choose_step_kernel(DfkHandle h, const DfkSfmWorkItem* items, int n, in
   const int ctas_per_sm = tc ? sfm_tc_ctas_per_sm(code_size) : (wide ? 1 : sfm_fp32_ctas_per_sm(code_size));
   const int sms = (h->sm_limit > 0 && h->sm_limit < h->num_sms) ? h->sm_limit : h->num_sms;
   k->max_ctas = ctas_per_sm * sms;
-  k->pfloats = tc ? sfm_tc_partial_floats(code_size) : sfm_partial_floats(code_size);
+  // the wide tensor-core kernels write the raw split-tf32 product D; the C = 32 one combines it into G in the fp32
+  // kernels' format
+  k->pfloats = (tc && wide) ? sfm_tc_partial_floats(code_size) : sfm_partial_floats(code_size);
   return DFK_OK;
 }
 
@@ -286,7 +288,7 @@ DfkStatus launch_step(DfkHandle h, const StepKernel& k, int code_size, const Sfm
     DFK_CUDA(h, launch_sfm_fp32(code_size, items_dev, plan, partials_dev, h->stream, ev0, ev1),
              "[SfmAligner::RunStep] kernel launch failed");
   }
-  DFK_CUDA(h, launch_sfm_finalize(code_size, k.tc, items_dev, n, partials_dev, records_dev, h->stream),
+  DFK_CUDA(h, launch_sfm_finalize(code_size, k.tc && k.wide, items_dev, n, partials_dev, records_dev, h->stream),
            "[SfmAligner::RunStep] kernel launch failed");
   h->launches += 2;  // step kernel + finalize kernel
   return DFK_OK;

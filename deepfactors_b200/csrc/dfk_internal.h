@@ -75,7 +75,8 @@ struct SfmCfg {
 
 constexpr int kTilePixels = 256;    // fp32 kernel
 
-// Tensor-core partial of code size C (32: dfk_sfm_tc.cu; 64, 128: dfk_sfm_tc_wide.cu).  Features f = code 0..C-1 |
+// Tensor-core partial of the wide code sizes C = 64, 128 (dfk_sfm_tc_wide.cu; the C = 32 kernel combines the same D in
+// its flush and writes the fp32 kernel's partial, SfmCfg<32>).  Features f = code 0..C-1 |
 // pose/residual C..C+6 | zero C+7 (F = C + 8), each split into h (tf32) and l.  The first S = C - 8 code features have
 // their l rows in A, the last 8 code features and the pose/zero group in B:
 //   A rows    = code-l 0..S-1 | h 0..F-1                        (M = 2C)
@@ -105,10 +106,6 @@ constexpr size_t sfm_tc_partial_floats(int code_size) { return (size_t)(2 * code
 // the C = 32 kernel's names for the above
 constexpr int kTcTilePixels = sfm_tc_tile_pixels(32);
 constexpr int kTcCtasPerSm = sfm_tc_ctas_per_sm(32);
-constexpr int kTcRows = TcCfg<32>::ROWS;
-constexpr int kTcCols = TcCfg<32>::COLS;
-constexpr int kTcRowsPad = kTcRows;
-constexpr int kTcPartialFloats = TcCfg<32>::PARTIAL_FLOATS;
 
 struct SfmLaunchPlan {
   int num_items = 0;
@@ -123,7 +120,7 @@ cudaError_t launch_sfm_fp32(int code_size, const SfmItemDev* items_dev, const Sf
                             cudaEvent_t ev_stop = nullptr);
 // dfk_sfm_rays.cu : fills every item's ray_tab (all three RunStep kernels read it)
 cudaError_t launch_sfm_ray_tables(const SfmItemDev* items_dev, int num_items, cudaStream_t stream);
-cudaError_t launch_sfm_finalize(int code_size, bool tc, const SfmItemDev* items_dev, int num_items,
+cudaError_t launch_sfm_finalize(int code_size, bool tc_wide, const SfmItemDev* items_dev, int num_items,
                                 const float* partials_dev, float* records_dev, cudaStream_t stream);
 // dfk_sfm_wide.cu : C = 64 / 128 (thread-owned 8x8 blocks); partial format = the fp32 kernel's
 constexpr int sfm_wide_tile_pixels(int code_size) { return code_size >= 128 ? 64 : 128; }

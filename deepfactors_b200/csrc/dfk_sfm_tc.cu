@@ -27,8 +27,9 @@
 //     f = code 0-31 | pose/residual 32-39:  HH[i][j] = D[24 + i][j];  LH[i][j] = D[i][j] for i < 24 and
 //     D[24 + j][16 + i] for i >= 24.  Only D[0-23][40-55] (l*l terms) is unused.
 //   The accumulator lives in registers (28 floats per thread).  A chain is cut every kFlushTiles tiles and at item
-//   boundaries: its fragments are added in round-to-nearest fp32 to the CTA's partial in global memory (single writer
-//   per address, program order), which is D itself, column-major (the finalize kernel reads it).
+//   boundaries: its fragments are staged in the (then idle) operand buffer, combined into G = (HH + LH) + LH^T and added
+//   in round-to-nearest fp32 to the CTA's partial in global memory (single writer per address, program order), in the
+//   fp32 kernel's format (SfmCfg<32>: G row-major, upper triangle).
 //
 //   Input stream: the code-Jacobian rows, img0 and dpt0 are read once, through loads that do not allocate in L1 (L1 is
 //   left to the bilinear gathers of img1 / grad1, the only loads that reuse lines; the fused depth decode reads the code
@@ -66,17 +67,40 @@ constexpr uint32_t OP_BYTES = 10 * kSbo;
 #define DFK_FLUSH_TILES 8
 #endif
 constexpr int kFlushTiles = DFK_FLUSH_TILES;  // accumulation chain length (tiles)
+using Cfg = SfmCfg<C>;                         // the partial: G row-major NFP x NFP, then the inlier count
+// D (64 x 56) staged row-major at a flush; the odd row stride keeps the column reads of LH conflict-free
+constexpr int kDStride = 57;
+static_assert(64 * kDStride * 4 <= 7 * kSbo, "the staged D must leave row 7 of the pose groups alone");
+// LH[i][j] in the staged D
+__device__ __forceinline__ int lh(int i, int j) { return i < 24 ? i * kDStride + j : (24 + j) * kDStride + 16 + i; }
 
 struct Smem {
   alignas(128) unsigned char op[OP_BYTES];
   SfmItem<C> item[NWARP];
 };
 
+#ifdef DFK_EXP_CTA_CLOCKS
+// experiment (tools/cta_tail.py): per CTA of the last launch, %globaltimer at entry and exit, (tiles << 32 | tiles with
+// a valid pixel) and the SM it ran on
+constexpr int kClockCtas = 8192;
+__device__ unsigned long long g_cta_clocks[kClockCtas][4];
+__device__ __forceinline__ unsigned long long global_ns()
+{
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+#endif
+
 __global__ void __launch_bounds__(THREADS, kTcCtasPerSm)
 sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_tiles, float* __restrict__ partials)
 {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
+#ifdef DFK_EXP_CTA_CLOCKS
+  const unsigned long long t_entry = global_ns();
+  int valid_tiles = 0;
+#endif
   const int tid = threadIdx.x;
   const int warp = tid >> 5;
   const int lane = tid & 31;
@@ -85,9 +109,10 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_tiles, float* _
   const int ntiles = g_hi - g_lo;
   if (ntiles <= 0) return;
 
-  // row 7 of the pose groups is never written: zeros
-  for (int e = tid; e < (int)(OP_BYTES / 16); e += THREADS)
-    reinterpret_cast<float4*>(sm.op)[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+  // row 7 of the pose groups (7 and 9) is never written: zeros
+  if (tid < 64)
+    *reinterpret_cast<float4*>(sm.op + (tid < 32 ? 7 : 9) * kSbo + (tid & 31) * kLbo + 7 * 16) =
+        make_float4(0.f, 0.f, 0.f, 0.f);
   __syncthreads();
 
   const uint32_t op = smem_u32(sm.op);
@@ -111,23 +136,35 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_tiles, float* _
   bool fresh = true;
   unsigned int inliers = 0;
 
-  // close the chain: add the accumulators to the partial (the first chain of an item in this CTA stores).  The
-  // accumulators are only ever written by the MMAs (a chain's first MMA overwrites them), so ptxas can keep them in
-  // flight across the next tile's front-end
+  // close the chain: combine G = (HH + LH) + LH^T of the chain's accumulators and add it to the partial (the first
+  // chain of an item in this CTA stores).  D goes through the operand buffer, free once the chain's MMAs have completed;
+  // the next tile's operand stores rewrite every byte the MMAs read.  The accumulators are only ever written by the MMAs
+  // (a chain's first MMA overwrites them), so ptxas can keep them in flight across the next tile's front-end
   auto flush = [&](bool item_end) {
     wgmma_wait_all();
-    float* P = partials + (size_t)pslot * kTcPartialFloats;
-    if (fresh || chain_valid > 0) {
-      const int m0 = 16 * warp + (lane >> 2);
+    float* P = partials + (size_t)pslot * Cfg::PARTIAL_FLOATS;
+    if (fresh || chain_valid > 0) {  // uniform across the CTA, like all chain bookkeeping
+      const bool have = chain_valid > 0;
+      float* Ds = reinterpret_cast<float*>(sm.op);
+      if (have) {
+        __syncthreads();  // every warp's share of the chain's MMAs has completed
+        const int m0 = 16 * warp + (lane >> 2);
 #pragma unroll
-      for (int q = 0; q < 28; ++q) {
-        const int m = m0 + 8 * ((q >> 1) & 1);
-        const int n = 8 * (q >> 2) + 2 * (lane & 3) + (q & 1);
-        if (n < 40 || m >= 24)  // D[0-23][40-55] holds only l*l terms
-          put_partial(P + n * kTcRowsPad + m, chain_valid > 0 ? acc[q] : 0.0f, fresh);
+        for (int q = 0; q < 28; ++q)
+          Ds[(m0 + 8 * ((q >> 1) & 1)) * kDStride + 8 * (q >> 2) + 2 * (lane & 3) + (q & 1)] = acc[q];
+        __syncthreads();
       }
+      // entries (i, j), i <= j < NF, of the row-major NFP x NFP partial: the ones the finalize reads
+      for (int e = tid; e < Cfg::NFP * Cfg::NFP; e += THREADS) {
+        const int i = e / Cfg::NFP, j = e - Cfg::NFP * i;
+        if (i > j || j >= Cfg::NF) continue;
+        float g = 0.0f;
+        if (have) g = (Ds[(24 + i) * kDStride + j] + Ds[lh(i, j)]) + Ds[lh(j, i)];
+        put_partial(P + e, g, fresh);
+      }
+      if (have) __syncthreads();  // the staged D is read before the next tile's operand stores overwrite it
     }
-    if (item_end && tid == 0) reinterpret_cast<unsigned int*>(P)[kTcRowsPad * kTcCols] = inliers;
+    if (item_end && tid == 0) reinterpret_cast<unsigned int*>(P)[Cfg::NFP * Cfg::NFP] = inliers;
     fresh = false;
     chain_valid = 0;
     tiles_in_chain = 0;
@@ -247,8 +284,23 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_tiles, float* _
     chain_valid += nv;
     inliers += (unsigned)nv;
     ++tiles_in_chain;
+#ifdef DFK_EXP_CTA_CLOCKS
+    valid_tiles += nv > 0;
+#endif
   }
   flush(true);
+#ifdef DFK_EXP_CTA_CLOCKS
+  __syncthreads();
+  if (tid == 0 && blockIdx.x < kClockCtas) {
+    unsigned int smid;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+    unsigned long long* o = g_cta_clocks[blockIdx.x];
+    o[0] = t_entry;
+    o[1] = global_ns();
+    o[2] = ((unsigned long long)ntiles << 32) | (unsigned)valid_tiles;
+    o[3] = smid;
+  }
+#endif
 }
 
 }  // namespace
@@ -270,3 +322,13 @@ cudaError_t launch_sfm_tc(const SfmItemDev* items_dev, const SfmLaunchPlan& plan
 }
 
 }  // namespace dfk
+
+#ifdef DFK_EXP_CTA_CLOCKS
+// the per-CTA records of the last step kernel launch (n <= 8192 CTAs, 4 u64 each); synchronises the device
+extern "C" int dfk_exp_cta_clocks(unsigned long long* out, int n)
+{
+  if (n < 0 || n > dfk::kClockCtas) return -1;
+  if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+  return cudaMemcpyFromSymbol(out, dfk::g_cta_clocks, sizeof(unsigned long long) * 4 * (size_t)n) == cudaSuccess ? 0 : -1;
+}
+#endif
