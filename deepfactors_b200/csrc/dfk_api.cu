@@ -239,7 +239,7 @@ DfkStatus choose_step_kernel(DfkHandle h, const DfkSfmWorkItem* items, int n, in
   if (!sfm_fp32_supported(code_size) && !wide)
     return fail(h, DFK_ERR_UNSUPPORTED,
                 "[SfmAligner::RunStep] no kernel instantiated for code size " + std::to_string(code_size));
-  const bool tc_ok = sfm_tc_supported(code_size) || sfm_tc_wide_supported(code_size);
+  const bool tc_ok = sfm_tc_supported(code_size);
   bool tc = (h->gram_mode == DFK_GRAM_TF32X3) || (h->gram_mode == DFK_GRAM_AUTO && tc_ok);
   if (tc) {
     // the tensor-core kernels gather grad1 with 8-byte loads; odd layouts go to the fp32 / wide kernel (AUTO) or fail
@@ -259,13 +259,11 @@ DfkStatus choose_step_kernel(DfkHandle h, const DfkSfmWorkItem* items, int n, in
                     std::to_string(code_size));
   k->tc = tc;
   k->wide = wide;
-  k->tile_px = tc ? sfm_tc_tile_pixels(code_size) : (wide ? sfm_wide_tile_pixels(code_size) : kTilePixels);
+  k->tile_px = tc ? kSfmTcTilePixels : (wide ? sfm_wide_tile_pixels(code_size) : kTilePixels);
   const int ctas_per_sm = tc ? sfm_tc_ctas_per_sm(code_size) : (wide ? 1 : sfm_fp32_ctas_per_sm(code_size));
   const int sms = (h->sm_limit > 0 && h->sm_limit < h->num_sms) ? h->sm_limit : h->num_sms;
   k->max_ctas = ctas_per_sm * sms;
-  // the wide tensor-core kernels write the raw split-tf32 product D; the C = 32 one combines it into G in the fp32
-  // kernels' format
-  k->pfloats = (tc && wide) ? sfm_tc_partial_floats(code_size) : sfm_partial_floats(code_size);
+  k->pfloats = (tc && sfm_tc_writes_d(code_size)) ? sfm_tc_partial_floats(code_size) : sfm_partial_floats(code_size);
   return DFK_OK;
 }
 
@@ -275,11 +273,8 @@ DfkStatus launch_step(DfkHandle h, const StepKernel& k, int code_size, const Sfm
 {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   if (h->profiling) DFK_TRY(profile_events(h, &ev0, &ev1));
-  if (k.tc && k.wide) {
-    DFK_CUDA(h, launch_sfm_tc_wide(code_size, items_dev, plan, partials_dev, h->stream, ev0, ev1),
-             "[SfmAligner::RunStep] kernel launch failed");
-  } else if (k.tc) {
-    DFK_CUDA(h, launch_sfm_tc(items_dev, plan, partials_dev, h->stream, ev0, ev1),
+  if (k.tc) {
+    DFK_CUDA(h, launch_sfm_tc(code_size, items_dev, plan, partials_dev, h->stream, ev0, ev1),
              "[SfmAligner::RunStep] kernel launch failed");
   } else if (k.wide) {
     DFK_CUDA(h, launch_sfm_wide(code_size, items_dev, plan, partials_dev, h->stream, ev0, ev1),
@@ -288,7 +283,7 @@ DfkStatus launch_step(DfkHandle h, const StepKernel& k, int code_size, const Sfm
     DFK_CUDA(h, launch_sfm_fp32(code_size, items_dev, plan, partials_dev, h->stream, ev0, ev1),
              "[SfmAligner::RunStep] kernel launch failed");
   }
-  DFK_CUDA(h, launch_sfm_finalize(code_size, k.tc && k.wide, items_dev, n, partials_dev, records_dev, h->stream),
+  DFK_CUDA(h, launch_sfm_finalize(code_size, k.tc, items_dev, n, partials_dev, records_dev, h->stream),
            "[SfmAligner::RunStep] kernel launch failed");
   h->launches += 2;  // step kernel + finalize kernel
   return DFK_OK;

@@ -75,10 +75,9 @@ struct SfmCfg {
 
 constexpr int kTilePixels = 256;    // fp32 kernel
 
-// Tensor-core partial of the wide code sizes C = 64, 128 (dfk_sfm_tc_wide.cu; the C = 32 kernel combines the same D in
-// its flush and writes the fp32 kernel's partial, SfmCfg<32>).  Features f = code 0..C-1 |
-// pose/residual C..C+6 | zero C+7 (F = C + 8), each split into h (tf32) and l.  The first S = C - 8 code features have
-// their l rows in A, the last 8 code features and the pose/zero group in B:
+// Split-tf32 product of the tensor-core kernel (dfk_sfm_tc.cu), and its partial where sfm_tc_writes_d.  Features f =
+// code 0..C-1 | pose/residual C..C+6 | zero C+7 (F = C + 8), each split into h (tf32) and l.  The first S = C - 8 code
+// features have their l rows in A, the last 8 code features and the pose/zero group in B:
 //   A rows    = code-l 0..S-1 | h 0..F-1                        (M = 2C)
 //   B columns = h 0..F-1 | code-l S..C-1 | pose-l (7 + zero)    (N = C + 24)
 // The accumulator D = A B^T is stored column-major ([column][row]), then the inlier count:
@@ -97,15 +96,15 @@ struct TcCfg {
 };
 
 // tiles of 128 pixels: K of the wgmma chain per tile
-constexpr int sfm_tc_tile_pixels(int) { return 128; }
+constexpr int kSfmTcTilePixels = 128;
 // resident CTAs per SM: C = 32 one warpgroup and ~47 KB of shared memory; C = 64 one warpgroup, ~85 KB;
 // C = 128 two warpgroups, ~163 KB
 constexpr int sfm_tc_ctas_per_sm(int code_size) { return code_size <= 32 ? 4 : (code_size <= 64 ? 2 : 1); }
+// The partial a tensor-core launch writes, for its flush, the partial size and the finalize: D itself (TcCfg<C>,
+// sfm_tc_partial_floats) at C = 64, 128; at C = 32 the kernel combines G = HH + LH + LH^T in its flush and writes the
+// fp32 kernels' partial (SfmCfg<C>, sfm_partial_floats).
+__host__ __device__ constexpr bool sfm_tc_writes_d(int code_size) { return code_size > 32; }
 constexpr size_t sfm_tc_partial_floats(int code_size) { return (size_t)(2 * code_size) * (code_size + 24) + 8; }
-
-// the C = 32 kernel's names for the above
-constexpr int kTcTilePixels = sfm_tc_tile_pixels(32);
-constexpr int kTcCtasPerSm = sfm_tc_ctas_per_sm(32);
 
 struct SfmLaunchPlan {
   int num_items = 0;
@@ -120,7 +119,8 @@ cudaError_t launch_sfm_fp32(int code_size, const SfmItemDev* items_dev, const Sf
                             cudaEvent_t ev_stop = nullptr);
 // dfk_sfm_rays.cu : fills every item's ray_tab (all three RunStep kernels read it)
 cudaError_t launch_sfm_ray_tables(const SfmItemDev* items_dev, int num_items, cudaStream_t stream);
-cudaError_t launch_sfm_finalize(int code_size, bool tc_wide, const SfmItemDev* items_dev, int num_items,
+// tc: the partials are the tensor-core kernel's (sfm_tc_writes_d decides their format)
+cudaError_t launch_sfm_finalize(int code_size, bool tc, const SfmItemDev* items_dev, int num_items,
                                 const float* partials_dev, float* records_dev, cudaStream_t stream);
 // dfk_sfm_wide.cu : C = 64 / 128 (thread-owned 8x8 blocks); partial format = the fp32 kernel's
 constexpr int sfm_wide_tile_pixels(int code_size) { return code_size >= 128 ? 64 : 128; }
@@ -128,14 +128,10 @@ bool sfm_wide_supported(int code_size);
 cudaError_t launch_sfm_wide(int code_size, const SfmItemDev* items_dev, const SfmLaunchPlan& plan,
                             float* partials_dev, cudaStream_t stream, cudaEvent_t ev_start = nullptr,
                             cudaEvent_t ev_stop = nullptr);
-// dfk_sfm_tc.cu (C = 32) and dfk_sfm_tc_wide.cu (C = 64, 128)
+// dfk_sfm_tc.cu : C = 32, 64, 128
 bool sfm_tc_supported(int code_size);
-cudaError_t launch_sfm_tc(const SfmItemDev* items_dev, const SfmLaunchPlan& plan, float* partials_dev,
+cudaError_t launch_sfm_tc(int code_size, const SfmItemDev* items_dev, const SfmLaunchPlan& plan, float* partials_dev,
                           cudaStream_t stream, cudaEvent_t ev_start = nullptr, cudaEvent_t ev_stop = nullptr);
-bool sfm_tc_wide_supported(int code_size);
-cudaError_t launch_sfm_tc_wide(int code_size, const SfmItemDev* items_dev, const SfmLaunchPlan& plan,
-                               float* partials_dev, cudaStream_t stream, cudaEvent_t ev_start = nullptr,
-                               cudaEvent_t ev_stop = nullptr);
 size_t sfm_partial_floats(int code_size);
 // resident CTAs per SM of the fp32 kernel: at C = 8 a CTA is 11 warps and ~60 KB of shared memory, two fit (the front-end
 // is latency-bound, so the second CTA nearly doubles the throughput); from C = 16 on the register budget allows one

@@ -13,10 +13,10 @@
 // Record layout: [JtJ packed upper (NP(NP+1)/2) | Jtr (NP) | residual | inliers (u32 bits)].
 //
 // Two partial formats:
-//   fp32, wide and C = 32 tensor-core kernels : G itself, row-major NFP x NFP (features: code 0..C-1, a C..C+5,
-//                                               r C+6), upper blocks valid
-//   wide tensor-core kernels (C = 64, 128)     : D = A x B^T over split-tf32 h / l rows (TcCfg<C>, stored column-major);
-//                                               G = HH + LH + LH^T
+//   fp32 and wide kernels, tensor-core kernel at C = 32 : G itself, row-major NFP x NFP (features: code 0..C-1,
+//                                                         a C..C+5, r C+6), upper blocks valid
+//   tensor-core kernel at C = 64, 128 (sfm_tc_writes_d)  : D = A x B^T over split-tf32 h / l rows (TcCfg<C>, stored
+//                                                         column-major); G = HH + LH + LH^T
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -219,10 +219,10 @@ cudaError_t launch_fin(const SfmItemDev* items_dev, int num_items, const float* 
 
 }  // namespace
 
-cudaError_t launch_sfm_finalize(int code_size, bool tc_wide, const SfmItemDev* items_dev, int num_items,
+cudaError_t launch_sfm_finalize(int code_size, bool tc, const SfmItemDev* items_dev, int num_items,
                                 const float* partials_dev, float* records_dev, cudaStream_t stream)
 {
-  if (tc_wide) {
+  if (tc && sfm_tc_writes_d(code_size)) {
     switch (code_size) {
       case 64: return launch_fin<64, true>(items_dev, num_items, partials_dev, records_dev, stream);
       case 128: return launch_fin<128, true>(items_dev, num_items, partials_dev, records_dev, stream);

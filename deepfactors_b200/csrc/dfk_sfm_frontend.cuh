@@ -1,4 +1,5 @@
-// dfk_sfm_frontend.cuh -- what the three SfmAligner::RunStep kernels (dfk_sfm_tc.cu, dfk_sfm_fp32.cu, dfk_sfm_wide.cu)
+// dfk_sfm_frontend.cuh -- what the three SfmAligner::RunStep kernels (dfk_sfm_tc.cu: tensor cores, C = 32, 64, 128;
+// dfk_sfm_fp32.cu; dfk_sfm_wide.cu)
 // share in front of their Gram engines:
 //   * the per-item parameter block kept in shared memory (one per CTA, one per warp in the tensor-core kernel);
 //   * the static tile -> CTA assignment and the in-item tile permutation: tile k of an item is processed as

@@ -16,7 +16,7 @@
 //     pixel-major and compacted into M[pixel][NFP].
 //   * Gram threads: for every valid pixel of their split, 2+2 LDS.128 and 64 FMA.
 // CUDA-core bound (9.8 kFMA per pixel at C = 128).  DFK_GRAM_AUTO runs these sizes on the tensor-core kernel
-// (dfk_sfm_tc_wide.cu); this one is the DFK_GRAM_FP32 engine and AUTO's engine for grad1 rows the tensor-core
+// (dfk_sfm_tc.cu); this one is the DFK_GRAM_FP32 engine and AUTO's engine for grad1 rows the tensor-core
 // kernel cannot gather (not 8-byte aligned).
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """tools/cta_tail.py -- how evenly the C = 32 tensor-core step kernel's CTAs finish on bench.py's pair8 step.
 
-Needs a library built with the per-CTA clocks of sfm_step_tc_kernel:
+Needs a library built with the per-CTA clocks of sfm_step_tc_kernel (every code size records them):
     tools/build_variant.sh clocks "-DDFK_EXP_CTA_CLOCKS"
     DFK_LIB=tools/variants/libdfk_clocks.so python tools/cta_tail.py [--launches N] [--json OUT]
 
