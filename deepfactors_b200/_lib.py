@@ -170,6 +170,18 @@ class DfkPreprocessItem(C.Structure):
                 ("normalize", C.c_int32)]
 
 
+class DfkKeyframeMeshParams(C.Structure):
+    _fields_ = [("stdev_thresh", C.c_float), ("slt_thresh", C.c_float), ("crop_pix", C.c_int32),
+                ("draw_noisy_pixels", C.c_int32)]
+
+
+class DfkKeyframeMeshItem(C.Structure):
+    _fields_ = [("dpt", DfkImage), ("prx_orig", DfkImage), ("prx_jac", DfkImage), ("code", C.POINTER(C.c_float)),
+                ("std", DfkImage), ("valid", DfkImage), ("color", DfkImage), ("cam", DfkCamera),
+                ("pose_wk", C.c_float * 7), ("vertex_capacity", C.c_int32), ("triangle_capacity", C.c_int32),
+                ("depth_u16", DfkImage)]
+
+
 BOW_MAX_DEPTH = 16  # DFK_BOW_MAX_DEPTH
 BOW_MAX_NODES = 4194304  # DFK_BOW_MAX_NODES
 
@@ -296,6 +308,9 @@ SYMBOLS = {
     "dfk_build_image_pyramid": (C.c_int, [_H, _IMG, _IMG, C.c_int]),
     "dfk_squared_error": (C.c_int, [_H, _IMG, _IMG, _F]),
     "dfk_preprocess_batch": (C.c_int, [_H, C.POINTER(DfkPreprocessItem), C.c_int, C.c_int, C.c_void_p]),
+    "dfk_keyframe_mesh_batch": (C.c_int, [_H, C.POINTER(DfkKeyframeMeshItem), C.c_int, C.c_int,
+                                          C.POINTER(DfkKeyframeMeshParams), C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "dfk_bow_vocabulary_create": (C.c_int, [_H, C.POINTER(DfkBowVocabularyDesc), C.POINTER(C.c_void_p)]),
     "dfk_bow_vocabulary_destroy": (C.c_int, [_H, C.c_void_p]),
     "dfk_bow_transform_batch": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkFeatureSet), C.POINTER(C.c_int32), C.c_int,

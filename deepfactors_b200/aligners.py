@@ -764,6 +764,186 @@ def PreprocessBatch(aligner, frames: Sequence[torch.Tensor], src_cams, out_cam, 
     return out
 
 
+# ------------------------------------------------------------------------------------------- keyframe meshes
+@dataclass
+class KeyframeMeshParams:
+    """The keyframe renderer's parameters (gui/visualizer.cpp:657-661)."""
+    stdev_thresh: float = 4.2
+    slt_thresh: float = 0.0
+    crop_pix: int = 20
+    draw_noisy_pixels: bool = False
+
+    def to_c(self) -> "_lib.DfkKeyframeMeshParams":
+        return _lib.DfkKeyframeMeshParams(self.stdev_thresh, self.slt_thresh, int(self.crop_pix),
+                                          int(bool(self.draw_noisy_pixels)))
+
+
+@dataclass
+class KeyframeMesh:
+    """One keyframe's mesh: views into a KeyframeMeshes batch (None where the batch has no such output).  positions
+    and normals float32 [V, 3] in the world frame, colors uint8 [V, 3], pixels int32 [V] (y W + x), triangles int32
+    [T, 3] of item-local vertex indices.  overflow: the item's counts exceed its capacities, so it has no rows."""
+    positions: torch.Tensor
+    normals: torch.Tensor | None
+    colors: torch.Tensor | None
+    pixels: torch.Tensor | None
+    triangles: torch.Tensor | None
+    num_vertices: int
+    num_triangles: int
+    overflow: bool
+
+
+@dataclass
+class KeyframeMeshes:
+    """The device output of KeyframeMeshBatch: item i's vertex rows start at vertex_offsets[i] and its triangle rows at
+    triangle_offsets[i] (the capacities of the items before it); counts int32 [n, 2] holds each item's true vertex and
+    triangle counts; depth_u16[i] is item i's uint16 [H, W] depth image, or None."""
+    positions: torch.Tensor
+    normals: torch.Tensor | None
+    colors: torch.Tensor | None
+    pixels: torch.Tensor | None
+    triangles: torch.Tensor | None
+    counts: torch.Tensor
+    vertex_offsets: np.ndarray
+    triangle_offsets: np.ndarray
+    depth_u16: list
+
+    def meshes(self) -> list:
+        """One KeyframeMesh per item (one read-back of the counts)"""
+        c = self.counts.cpu().numpy().astype(np.int64)
+        out = []
+        for i, (nv, nt) in enumerate(c):
+            vo, to = int(self.vertex_offsets[i]), int(self.triangle_offsets[i])
+            over = nv > self.vertex_offsets[i + 1] - vo or nt > self.triangle_offsets[i + 1] - to
+            v, t = (0, 0) if over else (int(nv), int(nt))
+            sl = lambda a, o, k: None if a is None else a[o:o + k]
+            out.append(KeyframeMesh(sl(self.positions, vo, v), sl(self.normals, vo, v), sl(self.colors, vo, v),
+                                    sl(self.pixels, vo, v), sl(self.triangles, to, t), int(nv), int(nt), bool(over)))
+        return out
+
+
+def _u8_view(t: torch.Tensor, channels: int, what: str) -> DfkImage:
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.uint8:
+        raise TypeError(f"KeyframeMeshBatch: {what} must be a uint8 CUDA tensor")
+    if t.dim() != 3 or t.shape[2] != channels or t.stride(2) != 1 or t.stride(1) != channels:
+        raise ValueError(f"KeyframeMeshBatch: {what} must be [H, W, {channels}] with interleaved contiguous pixels")
+    return DfkImage(C.c_void_p(t.data_ptr()), int(t.stride(0)), int(t.shape[1]), int(t.shape[0]))
+
+
+def KeyframeMeshBatch(aligner, items: Sequence[dict], params: KeyframeMeshParams | None = None,
+                      code_size: int | None = None, normals: bool = True, pixels: bool = True,
+                      triangles: bool = True) -> KeyframeMeshes:
+    """What the keyframe renderer (gui/shaders/drawkf.geom) draws for many keyframes, as world-frame meshes, in one call
+    (dfk_keyframe_mesh_batch).  items are dicts with cam (the keyframe's camera, whose size is every view's), pose_wk
+    (7 floats), the depth as dpt (float32 [H, W], pyr_dpt level 0) or as prx_orig, prx_jac and a host code (decoded
+    bit for bit as UpdateDepthBatch decodes it, avg_dpt the aligner's), and optionally std (log-stdev), valid (float32
+    [H, W]), color (uint8 [H, W, 3]), vertex_capacity (default H W), triangle_capacity (default 2 H W) and depth_u16
+    (True: also return SaveKeyframes' uint16 depth image).  Colours are returned when every item has a color view.
+    code_size defaults to the aligner's.  Asynchronous: returns a KeyframeMeshes of device tensors."""
+    hd = aligner._hd
+    hd.use_torch_stream()
+    params = params or KeyframeMeshParams()
+    cs = int(code_size if code_size is not None else getattr(aligner, "CS", 0))
+    n = len(items)
+    dev = torch.device("cuda", hd.device)
+    arr = (_lib.DfkKeyframeMeshItem * max(n, 1))()
+    keep, u16s, vcap, tcap = [], [], [], []
+    with_colors = n > 0 and all(it.get("color") is not None for it in items)
+    for k, it in enumerate(items):
+        cam = it["cam"]
+        W, H = int(cam.width), int(cam.height)
+        a = arr[k]
+        a.cam = _cam(cam)
+        a.pose_wk = _pose(it["pose_wk"])
+        if it.get("dpt") is not None:
+            a.dpt = _image(it["dpt"])
+        else:
+            code = np.ascontiguousarray(it["code"], dtype=np.float32)
+            if code.shape != (cs,):
+                raise ValueError(f"KeyframeMeshBatch: item {k}'s code must have code_size = {cs} entries")
+            keep.append(code)
+            a.prx_orig, a.prx_jac = _image(it["prx_orig"]), _image(it["prx_jac"], cs)
+            a.code = code.ctypes.data_as(C.POINTER(C.c_float))
+        if it.get("std") is not None:
+            a.std = _image(it["std"])
+        if it.get("valid") is not None:
+            a.valid = _image(it["valid"])
+        if it.get("color") is not None:
+            a.color = _u8_view(it["color"], 3, "color")
+        vcap.append(int(it.get("vertex_capacity", W * H)))
+        tcap.append(int(it.get("triangle_capacity", 2 * W * H)))
+        a.vertex_capacity, a.triangle_capacity = vcap[-1], tcap[-1]
+        u16 = torch.empty((H, W), dtype=torch.uint16, device=dev) if it.get("depth_u16") else None
+        if u16 is not None:
+            a.depth_u16 = DfkImage(C.c_void_p(u16.data_ptr()), 2 * W, W, H)
+        u16s.append(u16)
+    vo = np.concatenate([[0], np.cumsum(vcap)]).astype(np.int64)
+    to = np.concatenate([[0], np.cumsum(tcap)]).astype(np.int64)
+    V, T = int(vo[-1]), int(to[-1])
+    pos = torch.zeros((max(V, 1), 3), dtype=torch.float32, device=dev)  # rows past a count stay 0
+    nrm = torch.zeros((max(V, 1), 3), dtype=torch.float32, device=dev) if normals else None
+    col = torch.zeros((max(V, 1), 3), dtype=torch.uint8, device=dev) if with_colors else None
+    pix = torch.zeros(max(V, 1), dtype=torch.int32, device=dev) if pixels else None
+    tri = torch.zeros((max(T, 1), 3), dtype=torch.int32, device=dev) if triangles else None
+    counts = torch.empty((max(n, 1), 2), dtype=torch.int32, device=dev)
+    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+    prm = params.to_c()
+    check(hd.h, lib().dfk_keyframe_mesh_batch(hd.h, arr, n, cs, C.byref(prm), ptr(pos), ptr(nrm), ptr(col), ptr(pix),
+                                              ptr(tri), ptr(counts)))
+    cut = lambda t, r: None if t is None else t[:r]
+    return KeyframeMeshes(pos[:V], cut(nrm, V), cut(col, V), cut(pix, V), cut(tri, T), counts[:n], vo, to, u16s)
+
+
+def write_ply(path, meshes: KeyframeMeshes, items=None) -> None:
+    """Writes the meshes of KeyframeMeshBatch to one binary little-endian PLY file: vertices x y z (nx ny nz when the
+    batch has normals, red green blue when it has colours), faces as `list uchar int vertex_indices` when it has
+    triangles.  items: the item indices to write (default all), concatenated in that order with their triangles'
+    indices offset by the vertices before them.  Raises when a written item overflowed its capacities."""
+    ms = meshes.meshes()
+    idx = range(len(ms)) if items is None else [int(i) for i in items]
+    for i in idx:
+        if ms[i].overflow:
+            raise RuntimeError(f"write_ply: item {i} has {ms[i].num_vertices} vertices and {ms[i].num_triangles} "
+                               "triangles, more than its capacities; call KeyframeMeshBatch again with larger ones")
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    if meshes.normals is not None:
+        fields += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
+    if meshes.colors is not None:
+        fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+    verts, faces, base = [], [], 0
+    for i in idx:
+        m = ms[i]
+        v = np.zeros(m.num_vertices, dtype=fields)
+        p = m.positions.cpu().numpy()
+        v["x"], v["y"], v["z"] = p[:, 0], p[:, 1], p[:, 2]
+        if m.normals is not None:
+            q = m.normals.cpu().numpy()
+            v["nx"], v["ny"], v["nz"] = q[:, 0], q[:, 1], q[:, 2]
+        if m.colors is not None:
+            c = m.colors.cpu().numpy()
+            v["red"], v["green"], v["blue"] = c[:, 0], c[:, 1], c[:, 2]
+        verts.append(v)
+        if m.triangles is not None:
+            f = np.zeros(m.num_triangles, dtype=[("n", "u1"), ("v", "<i4", (3,))])
+            f["n"] = 3
+            f["v"] = m.triangles.cpu().numpy().astype(np.int64) + base
+            faces.append(f)
+        base += m.num_vertices
+    vall = np.concatenate(verts) if verts else np.zeros(0, dtype=fields)
+    names = {"<f4": "float", "u1": "uchar"}
+    head = ["ply", "format binary_little_endian 1.0", f"element vertex {len(vall)}"]
+    head += [f"property {names[t]} {nm}" for nm, t in fields]
+    if meshes.triangles is not None:
+        fall = np.concatenate(faces) if faces else np.zeros(0, dtype=[("n", "u1"), ("v", "<i4", (3,))])
+        head += [f"element face {len(fall)}", "property list uchar int vertex_indices"]
+    head.append("end_header")
+    with open(path, "wb") as fh:
+        fh.write(("\n".join(head) + "\n").encode("ascii"))
+        fh.write(vall.tobytes())
+        if meshes.triangles is not None:
+            fh.write(fall.tobytes())
+
+
 def SparseGeometricErrorBatch(aligner, items, out: torch.Tensor | None = None) -> torch.Tensor:
     """SparseGeometricFactor::error of many factors in one launch (dfk_sparse_geometric_error_batch): the items of
     SparseGeometricLinearizeBatch (dicts, or the array of make_geometric_items).  Asynchronous: returns a device tensor [n, 2] float32, row i = [b^T b | valid points

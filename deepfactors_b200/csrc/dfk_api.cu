@@ -1093,6 +1093,162 @@ DfkStatus dfk_preprocess_batch(DfkHandle h, const DfkPreprocessItem* items, int 
   });
 }
 
+// the checks of one keyframe of dfk_keyframe_mesh_batch; the failure text (naming the field), or null
+static const char* mesh_item_error(const DfkKeyframeMeshItem& it, int code_size, bool colors, DfkStatus* status)
+{
+  *status = DFK_ERR_INVALID_ARG;
+  const float cw = it.cam.width, ch = it.cam.height;
+  if (!pp_cam_ok(it.cam)) return "cam: intrinsics must be finite, with fx and fy != 0";
+  if (!(cw >= 1.0f && ch >= 1.0f && cw <= (float)DFK_ORB_MAX_SIDE && ch <= (float)DFK_ORB_MAX_SIDE) ||
+      cw != std::floor(cw) || ch != std::floor(ch))
+    return "cam: width and height must be whole numbers in [1, DFK_ORB_MAX_SIDE]";
+  const uint32_t W = (uint32_t)cw, H = (uint32_t)ch;
+  if (it.dpt.ptr) {
+    if (it.prx_orig.ptr || it.prx_jac.ptr || it.code) return "dpt: set either dpt or (prx_orig, prx_jac, code), not both";
+    if (!img_ok(&it.dpt, W, H, 1)) return "dpt: not a W x H float view";
+  } else {
+    if (!it.code) return "dpt: no dpt and no code to decode";
+    if (code_size < 1 || code_size > 256) {
+      *status = DFK_ERR_UNSUPPORTED;
+      return "code_size: out of range for a decode";
+    }
+    if (!img_ok(&it.prx_orig, W, H, 1)) return "prx_orig: not a W x H float view";
+    if (!img_ok(&it.prx_jac, W, H, (uint32_t)code_size)) return "prx_jac: not a W x H view of code_size floats";
+  }
+  if (it.std.ptr && !img_ok(&it.std, W, H, 1)) return "std: not a W x H float view";
+  if (it.valid.ptr && !img_ok(&it.valid, W, H, 1)) return "valid: not a W x H float view";
+  if (it.color.ptr && !pp_u8_ok(it.color, W, H, 3)) return "color: not W x H with pitch_bytes >= 3 W";
+  if (colors && !it.color.ptr) return "color: colors_dev is given but the item has no color view";
+  const DfkImage& u = it.depth_u16;
+  if (u.ptr && (u.width != W || u.height != H || (u.pitch_bytes & 1) || u.pitch_bytes < 2 * (size_t)W))
+    return "depth_u16: not W x H with an even pitch_bytes >= 2 W";
+  for (int k = 0; k < 7; ++k)
+    if (!std::isfinite(it.pose_wk[k])) return "pose_wk: not finite";
+  if (it.vertex_capacity < 0 || it.triangle_capacity < 0) return "capacity: negative";
+  return nullptr;
+}
+
+DfkStatus dfk_keyframe_mesh_batch(DfkHandle h, const DfkKeyframeMeshItem* items, int n, int code_size,
+                                  const DfkKeyframeMeshParams* params, float* positions_dev, float* normals_dev,
+                                  uint8_t* colors_dev, int32_t* pixels_dev, int32_t* triangles_dev, int32_t* counts_dev)
+{
+  return guarded(h, [&] {
+    const std::string w = "[KeyframeMesh batch] ";
+    if (!items || !params || n < 1 || n > 65535)  // gridDim.y of the tile kernels is the item
+      return fail(h, DFK_ERR_INVALID_ARG, w + "null argument / number of items not in [1, 65535]");
+    if (!positions_dev || !counts_dev) return fail(h, DFK_ERR_INVALID_ARG, w + "null positions or counts output");
+    if (((uintptr_t)positions_dev & 3) || ((uintptr_t)normals_dev & 3) || ((uintptr_t)pixels_dev & 3) ||
+        ((uintptr_t)triangles_dev & 3) || ((uintptr_t)counts_dev & 3))
+      return fail(h, DFK_ERR_INVALID_ARG, w + "float and int32 outputs must be 4-byte aligned");
+    const DfkKeyframeMeshParams& prm = *params;
+    if (!std::isfinite(prm.stdev_thresh) || !std::isfinite(prm.slt_thresh))
+      return fail(h, DFK_ERR_INVALID_ARG, w + "params: stdev_thresh and slt_thresh must be finite");
+    if (prm.crop_pix < 0) return fail(h, DFK_ERR_INVALID_ARG, w + "params: crop_pix < 0");
+    if (prm.draw_noisy_pixels != 0 && prm.draw_noisy_pixels != 1)
+      return fail(h, DFK_ERR_INVALID_ARG, w + "params: draw_noisy_pixels not 0 or 1");
+    // sizes: segments and decoded pixels before each item, output rows
+    std::vector<long long> seg_at((size_t)n), dec_at((size_t)n);
+    long long segs = 0, dec_px = 0, vrows = 0, trows = 0;
+    int decodes = 0, max_tiles = 1;
+    for (int i = 0; i < n; ++i) {
+      const DfkKeyframeMeshItem& it = items[i];
+      DfkStatus st;
+      if (const char* e = mesh_item_error(it, code_size, colors_dev != nullptr, &st))
+        return fail(h, st, w + "item " + std::to_string(i) + ": " + e);
+      const long long W = (long long)it.cam.width, H = (long long)it.cam.height;
+      const long long tx = (W + kMeshTileW - 1) / kMeshTileW, ty = (H + kMeshTileH - 1) / kMeshTileH;
+      seg_at[(size_t)i] = segs;
+      dec_at[(size_t)i] = dec_px;
+      segs += H * tx;
+      if (!it.dpt.ptr) {
+        dec_px += (W * H + 3) & ~3LL;  // 16-byte aligned depths
+        decodes += 1;
+      }
+      vrows += it.vertex_capacity;
+      trows += it.triangle_capacity;
+      max_tiles = std::max(max_tiles, (int)(tx * ty));
+    }
+    if (vrows > INT32_MAX || trows > INT32_MAX)
+      return fail(h, DFK_ERR_INVALID_ARG, w + "capacity: more than 2^31 - 1 vertex or triangle rows in one call");
+    DeviceGuard guard(h->device);
+    // scratch [segment masks (uint3) | segment bases (int2) | decoded depths (float)], 16-byte parts
+    auto part = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    const size_t b_masks = part(sizeof(uint3) * (size_t)segs), b_bases = part(sizeof(int2) * (size_t)segs);
+    DFK_CUDA(h, h->mesh_scratch.ensure(b_masks + b_bases + sizeof(float) * (size_t)dec_px),
+             "[KeyframeMesh batch] scratch allocation failed");
+    uint3* masks = reinterpret_cast<uint3*>(h->mesh_scratch.ptr);
+    int2* bases = reinterpret_cast<int2*>(h->mesh_scratch.ptr + b_masks);
+    float* decoded = reinterpret_cast<float*>(h->mesh_scratch.ptr + b_masks + b_bases);
+    // descriptors [items | decode descriptors | codes], 16-byte parts, one upload
+    const size_t b_items = part(sizeof(MeshItemDev) * (size_t)n);
+    const size_t b_descs = part(sizeof(DepthDecodeDesc) * (size_t)decodes);
+    const size_t total = b_items + b_descs + sizeof(float) * (size_t)decodes * (size_t)std::max(code_size, 0);
+    DFK_CUDA(h, h->mesh_dev.ensure(total), "[KeyframeMesh batch] scratch allocation failed");
+    h->mesh_host.assign(total, 0);
+    MeshItemDev* md = reinterpret_cast<MeshItemDev*>(h->mesh_host.data());
+    DepthDecodeDesc* dd = reinterpret_cast<DepthDecodeDesc*>(h->mesh_host.data() + b_items);
+    float* codes = reinterpret_cast<float*>(h->mesh_host.data() + b_items + b_descs);
+    const float* codes_dev = reinterpret_cast<const float*>(h->mesh_dev.ptr + b_items + b_descs);
+    int dec = 0, max_blocks = 1;
+    long long v_begin = 0, t_begin = 0;
+    for (int i = 0; i < n; ++i) {
+      const DfkKeyframeMeshItem& it = items[i];
+      MeshItemDev& d = md[i];
+      d.w = (int)it.cam.width;
+      d.h = (int)it.cam.height;
+      if (it.dpt.ptr) {
+        d.dpt = view_of(&it.dpt);
+      } else {
+        float* out = decoded + dec_at[(size_t)i];
+        DfkDepthDecodeItem di{it.prx_orig, it.prx_jac, DfkImage{out, sizeof(float) * (size_t)d.w, (uint32_t)d.w,
+                                                                 (uint32_t)d.h}, it.code};
+        set_depth_decode_desc(dd[dec], di, code_size, codes_dev + (size_t)dec * code_size, out, (uint32_t)d.w,
+                              &max_blocks);
+        memcpy(codes + (size_t)dec * code_size, it.code, sizeof(float) * code_size);
+        dec += 1;
+        d.dpt = View{out, (uint32_t)d.w};
+      }
+      d.std = it.std.ptr ? view_of(&it.std) : View{nullptr, 0};
+      d.vld = it.valid.ptr ? view_of(&it.valid) : View{nullptr, 0};
+      d.color = static_cast<const uint8_t*>(it.color.ptr);
+      d.color_pitch = it.color.pitch_bytes;
+      d.depth_u16 = static_cast<uint16_t*>(it.depth_u16.ptr);
+      d.u16_pitch = it.depth_u16.pitch_bytes;
+      d.fx = it.cam.fx; d.fy = it.cam.fy; d.u0 = it.cam.u0; d.v0 = it.cam.v0;
+      for (int k = 0; k < 4; ++k) d.q[k] = it.pose_wk[k];
+      for (int k = 0; k < 3; ++k) d.t[k] = it.pose_wk[4 + k];
+      d.tiles_x = (d.w + kMeshTileW - 1) / kMeshTileW;
+      d.tiles = d.tiles_x * ((d.h + kMeshTileH - 1) / kMeshTileH);
+      d.seg_begin = seg_at[(size_t)i];
+      d.v_begin = v_begin;
+      d.t_begin = t_begin;
+      d.v_cap = it.vertex_capacity;
+      d.t_cap = it.triangle_capacity;
+      v_begin += it.vertex_capacity;
+      t_begin += it.triangle_capacity;
+    }
+    DFK_CUDA(h, cudaMemcpyAsync(h->mesh_dev.ptr, h->mesh_host.data(), total, cudaMemcpyHostToDevice, h->stream),
+             "[KeyframeMesh batch] upload failed");
+    if (decodes > 0) {
+      DFK_CUDA(h, launch_update_depth_batch(code_size, reinterpret_cast<const DepthDecodeDesc*>(h->mesh_dev.ptr + b_items),
+                                            decodes, max_blocks, h->params.sfmparams.avg_dpt, h->stream),
+               "[KeyframeMesh batch] depth decode launch failed");
+      h->launches += 1;
+    }
+    MeshParamsDev p;
+    p.tau = prm.stdev_thresh > 0.0f ? std::log((double)prm.stdev_thresh / std::sqrt(2.0)) : -INFINITY;
+    p.slt = prm.slt_thresh;
+    p.crop = prm.crop_pix;
+    p.draw_noisy = prm.draw_noisy_pixels;
+    const MeshOutDev o{positions_dev, normals_dev, colors_dev, pixels_dev, triangles_dev, counts_dev};
+    DFK_CUDA(h, launch_keyframe_mesh(reinterpret_cast<const MeshItemDev*>(h->mesh_dev.ptr), n, max_tiles, p, o, masks,
+                                     bases, h->stream),
+             "[KeyframeMesh batch] kernel launch failed");
+    h->launches += 3;
+    return DFK_OK;
+  });
+}
+
 // ---------------------------------------------------------------------------------------------- streaming from host
 DfkStatus dfk_sfm_stream_create(DfkHandle h, int code_size, int max_items, size_t max_bytes, int depth, DfkSfmStream** out)
 {

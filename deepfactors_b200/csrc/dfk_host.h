@@ -120,6 +120,11 @@ struct DfkContext {
   DeviceBuf<unsigned char> pp_dev;
   std::vector<unsigned char> pp_host;
   DeviceBuf<double> pp_partials;
+  // dfk_keyframe_mesh_batch: [item descriptors | decode descriptors | codes] (bytes, one H2D per call from mesh_host)
+  // and [segment masks | segment bases | decoded depths] (bytes)
+  DeviceBuf<unsigned char> mesh_dev;
+  std::vector<unsigned char> mesh_host;
+  DeviceBuf<unsigned char> mesh_scratch;
   // the dfk_bow_* calls: the call's descriptors (one H2D per call from bow_host), the transform's per-descriptor words
   // when the caller passes none, and a query's [sums n x size | hits n x size] (bytes)
   DeviceBuf<unsigned char> bow_dev;

@@ -599,6 +599,44 @@ cudaError_t launch_bow_query(const BowDbDev& db, const BowQueryDev* queries_dev,
                              uint8_t* hits, int32_t* ids, double* scores, int32_t* counts, cudaStream_t s);
 cudaError_t launch_bow_score(const BowDbDev& db, const BowScoreDev* items_dev, int n, double* out, cudaStream_t s);
 
+// One keyframe of dfk_keyframe_mesh_batch (dfk_mesh.cu).  Its W x H pixels are cut into tiles of kMeshTileW x
+// kMeshTileH, one CTA each; a segment is the kMeshTileW pixels of one row of a tile, and its three masks (vertex, T1, T2;
+// bit = x % 32) and two bases (the item's vertex and triangle rows before it, in row-major order) live at
+// seg_begin + y * tiles_x + x / 32.
+constexpr int kMeshTileW = 32;
+constexpr int kMeshTileH = 8;
+struct MeshItemDev {
+  View dpt;                   // the caller's depth, or its decode in scratch
+  View std, vld;              // ptr null: absent
+  const uint8_t* color;       // null: absent
+  size_t color_pitch;         // bytes
+  uint16_t* depth_u16;        // null: not wanted
+  size_t u16_pitch;           // bytes
+  float fx, fy, u0, v0;
+  float q[4], t[3];           // pose_wk
+  int w, h, tiles_x, tiles;
+  long long seg_begin;
+  long long v_begin, t_begin; // the item's first output rows
+  int v_cap, t_cap;
+};
+struct MeshParamsDev {
+  double tau;                 // log(stdev_thresh / sqrt 2), -inf for stdev_thresh <= 0
+  float slt;
+  int crop, draw_noisy;
+};
+struct MeshOutDev {
+  float* positions;
+  float* normals;
+  uint8_t* colors;
+  int32_t* pixels;
+  int32_t* triangles;
+  int32_t* counts;            // [2 n]: vertices, triangles
+};
+// classify (grid (max tiles, n)), scan (one CTA per item), write rows (grid (max tiles, n)); segs uint3 and bases int2
+// per segment, totals int2 per item (scratch)
+cudaError_t launch_keyframe_mesh(const MeshItemDev* items_dev, int n, int max_tiles, const MeshParamsDev& p,
+                                 const MeshOutDev& o, uint3* segs, int2* bases, cudaStream_t s);
+
 constexpr int kSimpleMaxBlocks = 1024;
 constexpr int kSimpleScratchFloats = kSimpleMaxBlocks * 32;
 

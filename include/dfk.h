@@ -826,6 +826,76 @@ DfkStatus dfk_preprocess_batch(DfkHandle h, const DfkPreprocessItem* items, int 
 /* the most levels a frame of sides <= DFK_ORB_MAX_SIDE has: 16384, 8192, ..., 1 */
 #define DFK_PREPROCESS_MAX_LEVELS 15
 
+/* ------------------------------------------------------------------ keyframe meshes (the dense map) */
+
+/* The keyframe renderer's parameters (gui/visualizer.cpp:657-661, the defaults in brackets). */
+typedef struct {
+  float stdev_thresh;          /* [4.2] a pixel with sqrt(2) exp(log-stdev) > stdev_thresh is noisy; finite */
+  float slt_thresh;            /* [0] a quad whose triangle normals meet the pixel's ray at |cos| < slt_thresh is
+                                  dropped; finite */
+  int32_t crop_pix;            /* [20] quads within crop_pix of the image edge are skipped; >= 0 */
+  int32_t draw_noisy_pixels;   /* [0] 1: noisy pixels stay valid and are coloured (255, 0, 0); 0 or 1 */
+} DfkKeyframeMeshParams;
+
+/* One keyframe of dfk_keyframe_mesh_batch.  W x H = cam.width x cam.height (whole numbers in [1, DFK_ORB_MAX_SIDE]) is
+ * the size of every view.  The depth is dpt, or the decode of (prx_orig, prx_jac, code): set exactly one of dpt.ptr
+ * and the three decode fields. */
+typedef struct {
+  DfkImage dpt;                /* DEVICE float depth (kf->pyr_dpt level 0), or ptr NULL: decode */
+  DfkImage prx_orig, prx_jac;  /* DEVICE float proximity and its code Jacobian (code_size floats per pixel) */
+  const float* code;           /* HOST code_size floats */
+  DfkImage std;                /* DEVICE float log-stdev (kf->pyr_stdev level 0); ptr NULL: no pixel is noisy */
+  DfkImage valid;              /* DEVICE float validity (kf->pyr_vld level 0); ptr NULL: every pixel passes */
+  DfkImage color;              /* DEVICE uint8 x 3 (kf->color_img, dfk_preprocess_batch's color), pitch_bytes >= 3 W;
+                                  ptr NULL: none (then colors_dev must be NULL) */
+  DfkCamera cam;               /* the keyframe's camera: fx, fy finite and != 0, u0, v0 finite */
+  float pose_wk[7];            /* kf->pose_wk: quaternion (x, y, z, w), translation; finite */
+  int32_t vertex_capacity;     /* output vertex rows reserved for the item, >= 0 */
+  int32_t triangle_capacity;   /* output triangle rows reserved for the item, >= 0 */
+  DfkImage depth_u16;          /* out: DEVICE uint16 W x H, pitch_bytes even and >= 2 W (SaveKeyframes' depth image);
+                                  ptr NULL: not wanted */
+} DfkKeyframeMeshItem;
+
+/* What drawkf.geom (gui/shaders/drawkf.geom) draws for each item, as a world-frame mesh (DESIGN.md section 4.12).
+ * Every value is fp32 without FMA contraction, except tau below.
+ *   depth      d = dpt, or bit for bit dfk_update_depth_batch's decode of the item (avg_dpt = the handle's
+ *              DenseSfmParams::avg_dpt), each pixel decoded once; 1 <= code_size <= 256 when an item decodes.
+ *   pixel      (x, y) is invalid when !(vld > 0) (a NaN vld included), d < 0.5 or d > 10 or d is NaN, or x < 4,
+ *              x > W - 4, y < 4 or y > H - 4 (:55-88).  It is noisy when (double)s > tau, s its log-stdev and
+ *              tau = log((double)stdev_thresh / sqrt(2.0)) in fp64 (-inf for stdev_thresh <= 0); a NaN s is not noisy.
+ *              A noisy pixel is invalid, or with draw_noisy_pixels stays valid with colour (255, 0, 0).  A pixel
+ *              outside the image has depth 0 and is invalid.
+ *   quad       at (x, y) for every pixel: skipped when x < crop, x > W - crop, y < crop or y > H - crop (:97-99).  Its
+ *              corners tr = (x, y), tl = (x - 1, y), br = (x, y + 1), bl = (x - 1, y + 1) lift to p = ((x - u0) / fx d,
+ *              (y - v0) / fy d, d); n1 = n(tr, tl, br), n2 = n(tl, bl, br) with n(a, b, c) = normalize(cross(c - a,
+ *              b - a)), r = normalize(((x - u0) / fx, (y - v0) / fy, 1)); dropped when |n1 . r| < slt_thresh or
+ *              |n2 . r| < slt_thresh (:113-125).  normalize divides each component by sqrtf((v.x v.x + v.y v.y) +
+ *              v.z v.z); dot products sum in the same order; a NaN fails every comparison.
+ *   triangles  T1 = (tr, tl, br) when tr, tl, br are valid; T2 = (br, tl, bl) when tl, br, bl are valid (:152-183); quads
+ *              in row-major order, T1 before T2; corners are item-local vertex indices.
+ *   vertices   the pixels that are a corner of an emitted triangle, in row-major order: position pose_wk * p;
+ *              colour the color bytes (or (255, 0, 0)); normal R_wk ((n1 + n2) 0.5) of the quad at the vertex's own
+ *              (x, y), not renormalised; pixel index y W + x.
+ *   u16        depth_u16 = cv::Mat::convertTo(CV_16UC1, 5000) of d (core/deepfactors.cpp:560): (float)(d * 5000),
+ *              rounded half to even, saturated to [0, 65535]; a NaN or a product beyond int32 gives 0 (cvRound on x86).
+ * Deviations from the shader: T2 keeps T1's winding (the strip flips it when tr is invalid); the normal is in the world
+ * frame (the shader's is in clip space, after mvp, :134-136); a NaN depth is invalid (the shader emits a NaN vertex).
+ * Outputs (DEVICE), item i's vertex rows at the sum of vertex_capacity over the items before it, its triangle rows
+ * likewise:
+ *   positions_dev  float [vertex rows, 3]            normals_dev  float [vertex rows, 3], may be NULL
+ *   colors_dev     uint8 [vertex rows, 3], may be NULL (then every item needs a color view)
+ *   pixels_dev     int32 [vertex rows], may be NULL  triangles_dev int32 [triangle rows, 3], may be NULL
+ *   counts_dev     int32 [n, 2]: the item's true vertex and triangle counts
+ * An item whose vertex or triangle count exceeds its capacity writes its two counts and nothing else (no rows, no
+ * depth_u16); the other items are unaffected.  Rows past a count are not written.  Three kernels over every (tile, item), after one depth
+ * decode launch when an item decodes; integer scans only: deterministic, and an item's output depends on the item
+ * alone.  Asynchronous on the handle's stream.  Every item is validated before anything is enqueued (1 <= n <= 65535,
+ * the sizes, views, camera, pose, capacities and their sums <= 2^31 - 1, the parameters, 4-byte aligned float and int
+ * outputs); a rejected call writes nothing and dfk_last_error names the item and the field. */
+DfkStatus dfk_keyframe_mesh_batch(DfkHandle h, const DfkKeyframeMeshItem* items, int n, int code_size,
+                                  const DfkKeyframeMeshParams* params, float* positions_dev, float* normals_dev,
+                                  uint8_t* colors_dev, int32_t* pixels_dev, int32_t* triangles_dev, int32_t* counts_dev);
+
 /* ------------------------------------------------------------------ loop-closure candidates (DBoW2 retrieval) */
 
 /* The bag-of-words retrieval of LoopDetector (core/system/loop_detector.cpp:38-44, 96-112): DBoW2 (commit 3924753)

@@ -66,9 +66,14 @@ One JSON line per case:
     separate profiled run) against the sequential C oracle (bow_oracle) on one host thread, frame by frame; and one
     query of a 500-feature frame (max_results 20) against databases of 100, 1,000 and 10,000 entries.  The oracle's
     query scans every entry (no inverted file), so its host time is an upper bound of DBoW2's.
+  * keyframe meshes (`--only mesh`): 1, 8 and 64 keyframes at 256x192 and 640x480 with log-stdev, validity and colour
+    views and the uint16 depth, from the depth and from the fused decode at C = 32: one dfk_keyframe_mesh_batch as a
+    bare C call on buffers and items built once (wall clock to a synchronise), summed device time and the time of each
+    kernel from a separate profiled run, the algorithmic bytes and achieved bandwidth over the device time, and the
+    sequential C oracle (mesh_oracle) on one host thread from the depth, keyframe by keyframe.
 Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` /
 `--only frames` / `--only slide` / `--only error` / `--only lm` / `--only levels` / `--only match` / `--only orb` /
-`--only orb_pyramid` / `--only preprocess` runs those cases alone.
+`--only orb_pyramid` / `--only preprocess` / `--only bow` / `--only mesh` runs those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -88,7 +93,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error", "lm", "levels",
-                                           "match", "orb", "orb_pyramid", "preprocess", "bow"],
+                                           "match", "orb", "orb_pyramid", "preprocess", "bow", "mesh"],
                     default=None)
     args = ap.parse_args()
     import numpy as np
@@ -137,6 +142,8 @@ def main():
         return preprocess_cases(args, torch, print)
     if args.only == "bow":
         return bow_cases(args, torch, print)
+    if args.only == "mesh":
+        return mesh_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -1302,6 +1309,111 @@ def solve_cases(args, torch, print):
             device_kernel_ms=round(dev_ms, 3), kernel_ms_by_kind={k: round(v, 3) for k, v in per.items()},
             launches=len(ev), fill_gflop=round(flops / 1e9, 2), fp64_tflops=round(flops / (dev_ms * 1e-3) / 1e12, 3),
             rel_diff_vs_torch=err, reps=reps)))
+
+
+def mesh_cases(args, torch, print):
+    """dfk_keyframe_mesh_batch from the depth and from the fused decode (C = 32) against the sequential C oracle"""
+    import ctypes
+    import numpy as np
+    from torch.profiler import ProfilerActivity, profile
+
+    from deepfactors_b200 import _lib
+    from deepfactors_b200.aligners import KeyframeMeshParams, SfmAligner
+    from mesh_oracle import mesh_oracle as mo
+    cs = 32
+    al = SfmAligner(cs)
+    prm = KeyframeMeshParams()
+    cparams = prm.to_c()
+    L = _lib.lib()
+    for w, h in ((256, 192), (640, 480)):
+        ys, xs = np.mgrid[0:h, 0:w].astype(np.float64)
+        for n in (1, 8, 64):
+            rng = np.random.default_rng(n)
+            items = (_lib.DfkKeyframeMeshItem * n)()
+            keep, host = [], []
+            for i in range(n):
+                prx = (0.5 + 0.1 * np.sin(xs / 17.0 + i) * np.cos(ys / 13.0)).astype(np.float32)
+                jac = (rng.standard_normal((h, w, cs)) * 1e-3).astype(np.float32)
+                std = rng.uniform(-2.0, 0.5, (h, w)).astype(np.float32)  # below the noise threshold: a dense mesh
+                col = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+                code = np.zeros(cs, np.float32)
+                t = {k: torch.from_numpy(v).cuda() for k, v in dict(prx=prx, jac=jac, std=std, col=col).items()}
+                t["vld"] = torch.ones((h, w), dtype=torch.float32, device="cuda")
+                t["dpt"] = torch.empty((h, w), dtype=torch.float32, device="cuda")
+                t["u16"] = torch.empty((h, w), dtype=torch.int16, device="cuda")
+                keep += [t, code]
+                a = items[i]
+                a.std = _lib.DfkImage(t["std"].data_ptr(), 4 * w, w, h)
+                a.valid = _lib.DfkImage(t["vld"].data_ptr(), 4 * w, w, h)
+                a.color = _lib.DfkImage(t["col"].data_ptr(), 3 * w, w, h)
+                a.cam = _lib.DfkCamera(0.9 * w, 0.9 * w, w / 2 - 0.5, h / 2 - 0.5, w, h)
+                a.pose_wk = (ctypes.c_float * 7)(0.01 * i, 0.0, 0.0, 1.0, 0.1 * i, 0.0, 0.0)
+                a.vertex_capacity, a.triangle_capacity = w * h, 2 * w * h
+                a.depth_u16 = _lib.DfkImage(t["u16"].data_ptr(), 2 * w, w, h)
+                host.append(dict(std=std, col=col, cam=(0.9 * w, 0.9 * w, w / 2 - 0.5, h / 2 - 0.5),
+                                 pose=np.frombuffer(a.pose_wk, np.float32).copy()))
+            # the decoded depths, by dfk_update_depth_batch, for the depth path and the oracle
+            dec = (_lib.DfkDepthDecodeItem * n)()
+            for i in range(n):
+                t = keep[2 * i]
+                dec[i].prx_orig = _lib.DfkImage(t["prx"].data_ptr(), 4 * w, w, h)
+                dec[i].prx_jac = _lib.DfkImage(t["jac"].data_ptr(), 4 * w * cs, w, h)
+                dec[i].dpt = _lib.DfkImage(t["dpt"].data_ptr(), 4 * w, w, h)
+                dec[i].code = keep[2 * i + 1].ctypes.data_as(ctypes.POINTER(ctypes.c_float))
+            al._hd.use_torch_stream()
+            _lib.check(al._hd.h, L.dfk_update_depth_batch(al._hd.h, dec, n, cs))
+            V, T = n * w * h, 2 * n * w * h
+            out = [torch.empty((V, 3), device="cuda"), torch.empty((V, 3), device="cuda"),
+                   torch.empty((V, 3), dtype=torch.uint8, device="cuda"), torch.empty(V, dtype=torch.int32, device="cuda"),
+                   torch.empty((T, 3), dtype=torch.int32, device="cuda"),
+                   torch.empty((n, 2), dtype=torch.int32, device="cuda")]
+            ptrs = [ctypes.c_void_p(o.data_ptr()) for o in out]
+            for source in ("depth", f"decode_c{cs}"):
+                for i in range(n):
+                    t, a = keep[2 * i], items[i]
+                    if source == "depth":
+                        a.dpt = _lib.DfkImage(t["dpt"].data_ptr(), 4 * w, w, h)
+                        a.prx_orig = a.prx_jac = _lib.DfkImage()
+                        a.code = None
+                    else:
+                        a.dpt = _lib.DfkImage()
+                        a.prx_orig, a.prx_jac, a.code = dec[i].prx_orig, dec[i].prx_jac, dec[i].code
+
+                def call():
+                    _lib.check(al._hd.h, L.dfk_keyframe_mesh_batch(al._hd.h, items, n, cs, ctypes.byref(cparams),
+                                                                    *ptrs))
+
+                wall = _wall_us(torch, call, args.reps)
+                with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                    for _ in range(args.reps):
+                        call()
+                    torch.cuda.synchronize()
+                stages = {_kernel_name(e.key): round(e.self_device_time_total / args.reps, 1) for e in prof.key_averages()
+                          if e.self_device_time_total > 0}
+                dev_us = sum(stages.values())
+                counts = out[5].cpu().numpy().astype(np.int64)
+                nv, nt = int(counts[:, 0].sum()), int(counts[:, 1].sum())
+                # algorithmic bytes: every input pixel read once (depth or proximity + C Jacobian floats, log-stdev,
+                # validity, colour), the uint16 depth written, and the rows (position, normal, colour, pixel; triangle)
+                px = n * w * h
+                src = 4 * px if source == "depth" else 4 * px * (1 + cs)
+                nbytes = src + px * (4 + 4 + 3 + 2) + nv * (12 + 12 + 3 + 4) + nt * 12
+                rec = {"case": f"keyframe_mesh_{w}x{h}_x{n}_{source}", "keyframes": n, "vertices": nv, "triangles": nt,
+                       "wall_us": round(wall, 1), "device_time_us": round(dev_us, 1), "stages_us": stages,
+                       "algorithmic_bytes": nbytes,
+                       "achieved_gbs": round(nbytes / (dev_us * 1e-6) / 1e9, 1) if dev_us > 0 else "not measured"}
+                if source == "depth":
+                    dpt = [keep[2 * i]["dpt"].cpu().numpy() for i in range(n)]
+                    t0 = time.perf_counter()
+                    for i in range(n):
+                        hd = host[i]
+                        mo.mesh(dpt[i], hd["cam"], hd["pose"], std=hd["std"], vld=np.ones((h, w), np.float32),
+                                color=hd["col"])
+                    rec["oracle_host_us"] = round((time.perf_counter() - t0) * 1e6, 1)
+                    rec["oracle_threads"] = 1
+                else:
+                    rec["oracle_host_us"] = "not measured (the oracle takes a decoded depth)"
+                print(json.dumps(rec), flush=True)
 
 
 if __name__ == "__main__":
