@@ -79,6 +79,10 @@ class DfkDepthDecodeItem(C.Structure):
     _fields_ = [("prx_orig", DfkImage), ("prx_jac", DfkImage), ("dpt", DfkImage), ("code", C.POINTER(C.c_float))]
 
 
+class DfkDepthPriorItem(C.Structure):
+    _fields_ = [("target_dpt", DfkImage), ("prx_orig", DfkImage), ("prx_jac", DfkImage), ("code", C.POINTER(C.c_float))]
+
+
 class DfkWindowDesc(C.Structure):
     _fields_ = [("num_keyframes", C.c_int32), ("num_pairs", C.c_int32), ("num_items", C.c_int32), ("code_size", C.c_int32),
                 ("pair_k0", C.POINTER(C.c_int32)), ("pair_k1", C.POINTER(C.c_int32)), ("item_pair", C.POINTER(C.c_int32)),
@@ -206,6 +210,7 @@ class DfkBowScoreItem(C.Structure):
 
 
 WINDOW_ERROR_DOUBLES = 7  # DFK_WINDOW_ERROR_DOUBLES
+WINDOW_ERROR_EX_DOUBLES = 8  # DFK_WINDOW_ERROR_EX_DOUBLES
 
 
 # every symbol include/dfk.h declares: (name, restype, argtypes)
@@ -275,6 +280,10 @@ SYMBOLS = {
     "dfk_window_problem_linearize": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
     "dfk_window_problem_error": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
     "dfk_window_problem_retract": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
+    "dfk_window_problem_error_ex": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
+    "dfk_window_problem_set_depth_priors": (C.c_int, [_H, C.c_void_p, C.c_int, C.POINTER(C.c_int32),
+                                                      C.POINTER(C.c_float), C.POINTER(C.c_int32),
+                                                      C.POINTER(DfkDepthPriorItem)]),
     "dfk_window_lm": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkLMParams), C.POINTER(DfkLMTrace)]),
     "dfk_window_problem_set_active": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dfk_window_lm_levels": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkLMParams), C.POINTER(DfkLevelSchedule),
@@ -284,6 +293,10 @@ SYMBOLS = {
     "dfk_se3_track_batch": (C.c_int, [_H, C.c_int, C.c_int, _F, C.POINTER(DfkTrackLevel), _F, _F, _F]),
     "dfk_se3_warp": (C.c_int, [_H, _F, _CAM, _IMG, _IMG, _IMG, _IMG, _F, C.POINTER(C.c_uint64)]),
     "dfk_depth_run_step": (C.c_int, [_H, _F, C.c_int, _IMG, _IMG, _IMG, _F, _F, _F, C.POINTER(C.c_uint64)]),
+    "dfk_depth_prior_linearize_batch": (C.c_int, [_H, C.POINTER(DfkDepthPriorItem), C.c_int, C.c_int, C.c_void_p]),
+    "dfk_depth_prior_error_batch": (C.c_int, [_H, C.POINTER(DfkDepthPriorItem), C.c_int, C.c_int, C.c_void_p]),
+    "dfk_window_add_depth_priors": (C.c_int, [_H, C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_float),
+                                              C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]),
     "dfk_reprojection_linearize": (C.c_int, [_H, _F, _F, _F, C.c_int, _CAM, _IMG, _IMG, C.c_int, _F, _F, C.c_float,
                                              C.c_float, _F, _F]),
     "dfk_reprojection_linearize_batch": (C.c_int, [_H, C.POINTER(DfkReprojectionItem), C.c_int, C.c_int, C.c_void_p]),
@@ -360,6 +373,11 @@ def geo_record_floats(code_size: int) -> int:
     """DFK_GEO_RECORD_FLOATS: a sparse geometric record over [pose0 | pose1 | code0 | code1]"""
     npar = 12 + 2 * code_size
     return npar * (npar + 1) // 2 + npar + 2
+
+
+def depth_record_floats(code_size: int) -> int:
+    """DFK_DEPTH_RECORD_FLOATS: a depth-prior record [JtJ packed upper | Jtr | residual | inliers]"""
+    return code_size * (code_size + 1) // 2 + code_size + 2
 
 
 def prior_doubles(code_size: int) -> int:

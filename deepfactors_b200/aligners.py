@@ -990,6 +990,52 @@ class DepthAligner:
         return JTJJrReductionItem(JtJ, Jtr, float(res.value), int(inl.value))
 
 
+def make_depth_prior_items(items: Sequence[dict], cs: int):
+    """the ctypes array of DepthPriorLinearizeBatch / DepthPriorErrorBatch: dicts with code (host, CS floats),
+    target_dpt, prx_orig and prx_jac (device views of one (keyframe, level)).  A float32 C-contiguous code is referenced,
+    not copied, so a caller may build the array once and rewrite the codes in place."""
+    arr = (_lib.DfkDepthPriorItem * max(len(items), 1))()
+    keep = []
+    for k, it in enumerate(items):
+        code = np.ascontiguousarray(it["code"], dtype=np.float32)
+        if code.shape != (cs,):
+            raise ValueError(f"code must have {cs} entries")
+        keep.append(code)
+        w = arr[k]
+        w.target_dpt, w.prx_orig = _image(it["target_dpt"]), _image(it["prx_orig"])
+        w.prx_jac = _image(it["prx_jac"], cs)
+        w.code = code.ctypes.data_as(C.POINTER(C.c_float))
+    arr._keepalive = keep
+    return arr
+
+
+def DepthPriorLinearizeBatch(aligner, items, records: torch.Tensor | None = None) -> torch.Tensor:
+    """DepthPriorFactor's per-level DepthAligner::RunStep for many (keyframe, level) items in one call
+    (dfk_depth_prior_linearize_batch): items are the dicts of make_depth_prior_items, or its array.  Record i =
+    [JtJ packed upper | Jtr | residual | inliers (uint32 bits) = W * H] (DFK_DEPTH_RECORD_FLOATS(CS)), item i's
+    DepthAligner.RunStep result, with the aligner's avg_dpt.  `records` may be a slice of a larger buffer.  Asynchronous:
+    returns a device tensor [n, DFK_DEPTH_RECORD_FLOATS(CS)] on torch's current stream."""
+    aligner._hd.use_torch_stream()
+    cs, n = aligner.CS, len(items)
+    records = _batch_records(aligner, n, _lib.depth_record_floats(cs), records)
+    arr = items if isinstance(items, C.Array) else make_depth_prior_items(items, cs)
+    check(aligner.handle, lib().dfk_depth_prior_linearize_batch(aligner.handle, arr, n, cs,
+                                                                C.c_void_p(records.data_ptr())))
+    return records
+
+
+def DepthPriorErrorBatch(aligner, items, out: torch.Tensor | None = None) -> torch.Tensor:
+    """DepthPriorFactor's sum diff^2 of many (keyframe, level) items in one call (dfk_depth_prior_error_batch): the items
+    of DepthPriorLinearizeBatch.  Asynchronous: returns a device tensor [n, 2] float32, row i = [sum diff^2 | W * H as
+    uint32 bits], the residual bit for bit the one of item i's DepthPriorLinearizeBatch record."""
+    aligner._hd.use_torch_stream()
+    cs, n = aligner.CS, len(items)
+    out = _batch_records(aligner, n, 2, out)
+    arr = items if isinstance(items, C.Array) else make_depth_prior_items(items, cs)
+    check(aligner.handle, lib().dfk_depth_prior_error_batch(aligner.handle, arr, n, cs, C.c_void_p(out.data_ptr())))
+    return out
+
+
 # ------------------------------------------------------------------------------------------- keyframe window
 class Window:
     """Device-side assembly of a keyframe window's block-sparse normal equations (dfk_window_* of include/dfk.h):
@@ -1102,6 +1148,28 @@ class Window:
         check(hd.h, lib().dfk_window_add_priors(hd.h, self.w, m, kf.ctypes.data_as(C.POINTER(C.c_int32)),
                                                 C.c_void_p(priors.data_ptr()), C.c_void_p(delta.data_ptr()),
                                                 C.c_void_p(buf.data_ptr())))
+        return buf
+
+    def add_depth_priors(self, buf: torch.Tensor, prior_kf, sigma, level_ptr, records: torch.Tensor) -> torch.Tensor:
+        """dfk_window_add_depth_priors, in place on an assembled buffer: depth prior i on keyframe prior_kf[i] with
+        standard deviation sigma[i] owns the rows [level_ptr[i], level_ptr[i + 1]) of `records` (DepthPriorLinearizeBatch's
+        records on the device): JtJ / sigma^2 to the keyframe's code block, -Jtr / sigma^2 to its code gradient,
+        residual / sigma^2 to f.  Asynchronous on torch's current stream."""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        kf = np.ascontiguousarray([int(k) for k in prior_kf], dtype=np.int32)
+        sg = np.ascontiguousarray([float(v) for v in sigma], dtype=np.float32)
+        lp = np.ascontiguousarray([int(v) for v in level_ptr], dtype=np.int32)
+        m = len(kf)
+        if sg.size != m or lp.size != m + 1:
+            raise ValueError("sigma needs one entry per prior and level_ptr one more")
+        _check_tensor(hd, buf, torch.float32, self.floats, "buf")
+        nrec = int(lp[-1]) if m else 0
+        _check_tensor(hd, records, torch.float32, nrec * _lib.depth_record_floats(self.layout.code_size), "records")
+        I32 = C.POINTER(C.c_int32)
+        check(hd.h, lib().dfk_window_add_depth_priors(hd.h, self.w, m, kf.ctypes.data_as(I32),
+                                                      sg.ctypes.data_as(C.POINTER(C.c_float)), lp.ctypes.data_as(I32),
+                                                      C.c_void_p(records.data_ptr()), C.c_void_p(buf.data_ptr())))
         return buf
 
     def add_keyframe_priors(self, buf: torch.Tensor, priors: torch.Tensor, delta: torch.Tensor) -> torch.Tensor:
@@ -1351,6 +1419,33 @@ class WindowProblem:
         _check_tensor(hd, out, torch.float64, _lib.WINDOW_ERROR_DOUBLES, "out")
         check(hd.h, lib().dfk_window_problem_error(hd.h, self.p, C.c_void_p(out.data_ptr())))
         return out
+
+    def error_ex(self, out: torch.Tensor | None = None) -> torch.Tensor:
+        """dfk_window_problem_error_ex: error()'s 7 doubles, then the depth-prior part of E (asynchronous)"""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        if out is None:
+            out = torch.empty(_lib.WINDOW_ERROR_EX_DOUBLES, dtype=torch.float64, device=f"cuda:{hd.device}")
+        _check_tensor(hd, out, torch.float64, _lib.WINDOW_ERROR_EX_DOUBLES, "out")
+        check(hd.h, lib().dfk_window_problem_error_ex(hd.h, self.p, C.c_void_p(out.data_ptr())))
+        return out
+
+    def set_depth_priors(self, prior_kf, sigma, level_ptr, items):
+        """dfk_window_problem_set_depth_priors: depth prior i on keyframe prior_kf[i] with standard deviation sigma[i]
+        owns items[level_ptr[i]:level_ptr[i + 1]] (dicts of target_dpt, prx_orig, prx_jac: one (keyframe, level) each;
+        their codes come from the problem's state).  The image views must outlive the problem."""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        kf = np.ascontiguousarray([int(k) for k in prior_kf], dtype=np.int32)
+        sg = np.ascontiguousarray([float(v) for v in sigma], dtype=np.float32)
+        lp = np.ascontiguousarray([int(v) for v in level_ptr], dtype=np.int32)
+        cs = self._al.CS
+        arr = make_depth_prior_items([dict(it, code=np.zeros(cs, np.float32)) for it in items], cs)
+        self._keep_depth = (arr, [it for it in items])
+        I32 = C.POINTER(C.c_int32)
+        check(hd.h, lib().dfk_window_problem_set_depth_priors(hd.h, self.p, len(kf), kf.ctypes.data_as(I32),
+                                                              sg.ctypes.data_as(C.POINTER(C.c_float)),
+                                                              lp.ctypes.data_as(I32), arr))
 
     def retract(self, dx: torch.Tensor):
         """dfk_window_problem_retract: state <- retract(state, dx), dx [K B + 6 F] float64 on the device"""

@@ -1438,4 +1438,41 @@ DfkStatus dfk_depth_run_step(DfkHandle h, const float* code, int code_size, cons
   });
 }
 
+namespace {
+
+DfkStatus depth_prior_batch(DfkHandle h, const char* what, const DfkDepthPriorItem* items, int n, int code_size,
+                            float* out_dev, bool gram)
+{
+  if (!out_dev) return fail(h, DFK_ERR_INVALID_ARG, std::string(what) + "null argument");
+  DeviceGuard guard(h->device);
+  int max_parts = 1, rows = 0;
+  DFK_TRY(stage_depth_prior(h, what, items, n, code_size, true, h->depth_prior_host, h->depth_prior_dev, &max_parts,
+                            &rows));
+  DFK_CUDA(h, h->depth_prior_partials.ensure((size_t)rows * depth_prior_partial_floats(code_size, gram)),
+           (std::string(what) + "scratch allocation failed").c_str());
+  DFK_CUDA(h, launch_depth_prior_batch(code_size, reinterpret_cast<const DepthPriorDesc*>(h->depth_prior_dev.ptr), n,
+                                       max_parts, h->params.sfmparams.avg_dpt, h->depth_prior_partials.ptr, out_dev, gram,
+                                       h->stream),
+           (std::string(what) + "kernel launch failed").c_str());
+  h->launches += 2;
+  return DFK_OK;
+}
+
+}  // namespace
+
+DfkStatus dfk_depth_prior_linearize_batch(DfkHandle h, const DfkDepthPriorItem* items, int n, int code_size,
+                                          float* records_dev)
+{
+  return guarded(h, [&] {
+    return depth_prior_batch(h, "[DepthPriorFactor::linearize batch] ", items, n, code_size, records_dev, true);
+  });
+}
+
+DfkStatus dfk_depth_prior_error_batch(DfkHandle h, const DfkDepthPriorItem* items, int n, int code_size, float* out_dev)
+{
+  return guarded(h, [&] {
+    return depth_prior_batch(h, "[DepthPriorFactor::error batch] ", items, n, code_size, out_dev, false);
+  });
+}
+
 }  // extern "C"

@@ -105,6 +105,15 @@ struct DfkWindowProblem {
   DeviceBuf<double> areas_sub;
   DeviceBuf<int> rec_src;            // record slot i <- subset record rec_src[i], -1: zeros
   DeviceBuf<float> sub_records;
+  // depth priors (dfk_window_problem_set_depth_priors): ndp priors over ndpi (keyframe, level) items, staged once
+  // ([descriptors | codes], the codes rewritten from the state before every batch), and the lists
+  // [add CSR ptr K + 1 | prior indices ndp | level_ptr ndp + 1 | sigma (float bits) ndp | keyframe of every item ndpi]
+  int ndp = 0, ndpi = 0, dp_max_parts = 1, dp_rows = 0;
+  size_t dp_code_off = 0, dp_lp = 0, dp_sg = 0, dp_kf = 0;
+  DeviceBuf<unsigned char> dp;
+  std::vector<unsigned char> dp_host;
+  DeviceBuf<int> dp_lists;
+  DeviceBuf<float> dp_partials, dp_records, dp_err;
   ~DfkWindowProblem()
   {
     window_solver_destroy(solver[0]);
@@ -113,6 +122,7 @@ struct DfkWindowProblem {
   double* st(int i) const { return state.ptr + (size_t)i * S; }
   double* energy() const { return reinterpret_cast<double*>(small.ptr); }
   int32_t* info() const { return reinterpret_cast<int32_t*>(small.ptr + 8 * sizeof(double)); }
+  double* depth_energy() const { return reinterpret_cast<double*>(small.ptr + 8 * sizeof(double) + 16); }
 };
 
 namespace {
@@ -166,6 +176,21 @@ WindowReposeDev repose_args(const DfkWindowProblem* p, const double* state)
   a.depth = reinterpret_cast<DepthDecodeDesc*>(p->depth.ptr); a.depth_slots = sl + p->nd + p->ne + p->nr + p->ng;
   a.num_depth = p->ndep;
   return a;
+}
+
+// the depth priors' batch at `state`: the items' codes from the state, then the records (gram) or the error rows
+DfkStatus problem_depth_priors(DfkHandle h, DfkWindowProblem* p, const double* state, bool gram, const char* what)
+{
+  const int* l = p->dp_lists.ptr;
+  float* codes = reinterpret_cast<float*>(p->dp.ptr + p->dp_code_off);
+  DFK_CUDA(h, launch_depth_prior_codes(state + (size_t)(p->K + p->F) * 7, l + p->dp_kf, p->ndpi, p->C, codes, h->stream),
+           what);
+  DFK_CUDA(h, launch_depth_prior_batch(p->C, reinterpret_cast<const DepthPriorDesc*>(p->dp.ptr), p->ndpi,
+                                       p->dp_max_parts, p->avg_dpt, p->dp_partials.ptr,
+                                       gram ? p->dp_records.ptr : p->dp_err.ptr, gram, h->stream),
+           what);
+  h->launches += 3;
+  return DFK_OK;
 }
 
 DfkStatus problem_deltas(DfkHandle h, const DfkWindowProblem* p, const double* state)
@@ -230,6 +255,15 @@ DfkStatus problem_linearize(DfkHandle h, DfkWindowProblem* p, const double* stat
              what);
     h->launches += 1;
   }
+  if (p->ndp > 0) {  // after the frame and keyframe priors, as SfmWindowProblem.linearise without an all-reduce
+    DFK_TRY(problem_depth_priors(h, p, state, true, what));
+    const int* l = p->dp_lists.ptr;
+    DFK_CUDA(h, launch_window_add_depth_priors(w->dev, p->ndp, l, l + p->K + 1, l + p->dp_lp,
+                                               reinterpret_cast<const float*>(l + p->dp_sg), p->dp_records.ptr, buf,
+                                               h->stream),
+             what);
+    h->launches += 1;
+  }
   return DFK_OK;
 }
 
@@ -246,6 +280,13 @@ WindowEnergyDev energy_args(const DfkWindowProblem* p, const double* state, doub
   a.codes = state + (size_t)(p->K + p->F) * 7;
   a.num_codes = p->K * p->C;
   a.code_prior_weight = w;
+  a.num_depth_priors = p->ndp;
+  if (p->ndp > 0) {
+    a.depth_err = reinterpret_cast<const float2*>(p->dp_err.ptr);
+    a.depth_level_ptr = p->dp_lists.ptr + p->dp_lp;
+    a.depth_sigma = reinterpret_cast<const float*>(p->dp_lists.ptr + p->dp_sg);
+    a.out_depth = p->depth_energy();
+  }
   a.out = p->energy();
   return a;
 }
@@ -289,6 +330,7 @@ DfkStatus problem_error(DfkHandle h, DfkWindowProblem* p, const double* state, d
              what);
     h->launches += 1;
   }
+  if (p->ndp > 0) DFK_TRY(problem_depth_priors(h, p, state, false, what));
   DFK_TRY(problem_deltas(h, p, state));
   DFK_CUDA(h, launch_window_energy(energy_args(p, state, w), h->stream), what);
   h->launches += 1;
@@ -713,6 +755,53 @@ DfkStatus dfk_window_add_priors(DfkHandle h, const DfkWindow* w, int m, const in
     DFK_CUDA(h, launch_window_add_priors(w->dev, m, h->window_lists.ptr, h->window_lists.ptr + K + 1, priors_dev,
                                          delta_dev, window_dev, h->stream),
              "[Window::AddPriors] kernel launch failed");
+    h->launches += 1;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_add_depth_priors(DfkHandle h, const DfkWindow* w, int m, const int32_t* prior_kf_host,
+                                      const float* sigma_host, const int32_t* level_ptr_host, const float* records_dev,
+                                      float* window_dev)
+{
+  return guarded(h, [&] {
+    if (!w || !window_dev || m < 0 || (m > 0 && (!prior_kf_host || !sigma_host || !level_ptr_host || !records_dev)))
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddDepthPriors] null argument");
+    if (w->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddDepthPriors] window and handle live on different devices");
+    if (!depth_supported(w->dev.code_size))
+      return fail(h, DFK_ERR_UNSUPPORTED, "[Window::AddDepthPriors] code size not instantiated by the depth prior");
+    const int K = w->dev.num_keyframes;
+    if (m > 0 && level_ptr_host[0] != 0)
+      return fail(h, DFK_ERR_INVALID_ARG, "[Window::AddDepthPriors] level_ptr[0] must be 0");
+    for (int i = 0; i < m; ++i) {
+      const std::string pre = "[Window::AddDepthPriors] prior " + std::to_string(i);
+      if (prior_kf_host[i] < 0 || prior_kf_host[i] >= K)
+        return fail(h, DFK_ERR_INVALID_ARG, pre + " names a keyframe outside the window");
+      if (!std::isfinite(sigma_host[i]) || !(sigma_host[i] > 0.0f))
+        return fail(h, DFK_ERR_INVALID_ARG, pre + ": sigma must be finite and > 0");
+      if (level_ptr_host[i + 1] <= level_ptr_host[i])
+        return fail(h, DFK_ERR_INVALID_ARG, pre + " has no records (level_ptr must increase)");
+    }
+    if (m == 0) return DFK_OK;
+    // [CSR of the priors per keyframe: ptr[K + 1] | indices m] | level_ptr[m + 1] | sigma[m] (float bits)
+    std::vector<int> lists;
+    add_csr(lists, K, m, [&](int i) { return prior_kf_host[i]; });
+    const size_t lp = lists.size();
+    lists.insert(lists.end(), level_ptr_host, level_ptr_host + m + 1);
+    const size_t sg = lists.size();
+    lists.resize(sg + m);
+    memcpy(lists.data() + sg, sigma_host, sizeof(float) * m);
+    DeviceGuard guard(h->device);
+    const char* what = "[Window::AddDepthPriors] index upload failed";
+    DFK_CUDA(h, h->window_lists.ensure(lists.size()), what);
+    DFK_CUDA(h, cudaMemcpyAsync(h->window_lists.ptr, lists.data(), sizeof(int) * lists.size(), cudaMemcpyHostToDevice,
+                                h->stream),
+             what);
+    const int* d = h->window_lists.ptr;
+    DFK_CUDA(h, launch_window_add_depth_priors(w->dev, m, d, d + K + 1, d + lp, reinterpret_cast<const float*>(d + sg),
+                                               records_dev, window_dev, h->stream),
+             "[Window::AddDepthPriors] kernel launch failed");
     h->launches += 1;
     return DFK_OK;
   });
@@ -1185,8 +1274,8 @@ DfkStatus dfk_window_problem_create(DfkHandle h, const DfkWindowProblemDesc* d, 
     DFK_CUDA(h, window_solver_create(K, C, F, w->pair_k0, w->pair_k1, w->link_k0, w->link_k1, w->blk_i, w->blk_j,
                                      w->kp.block_off, gauge, &p->solver[1]),
              "[WindowProblem] solver workspace allocation failed");
-    DFK_CUDA(h, p->small.ensure(8 * sizeof(double) + 16), amsg);
-    DFK_CUDA(h, p->small_host.ensure(8 * sizeof(double) + 16), amsg);
+    DFK_CUDA(h, p->small.ensure(9 * sizeof(double) + 16), amsg);  // energy | info | depth-prior energy
+    DFK_CUDA(h, p->small_host.ensure(9 * sizeof(double) + 16), amsg);
     DFK_CUDA(h, cudaStreamSynchronize(h->stream), "[WindowProblem] upload failed");  // the host staging is freed next
     *out = p.release();
     return DFK_OK;
@@ -1255,6 +1344,85 @@ DfkStatus dfk_window_problem_error(DfkHandle h, DfkWindowProblem* p, double* out
     DFK_CUDA(h, cudaMemcpyAsync(out_dev, p->energy(), sizeof(double) * DFK_WINDOW_ERROR_DOUBLES, cudaMemcpyDeviceToDevice,
                                 h->stream),
              "[WindowProblem::error] copy failed");
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_problem_error_ex(DfkHandle h, DfkWindowProblem* p, double* out_dev)
+{
+  return guarded(h, [&] {
+    if (!p || !out_dev) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem::error_ex] null argument");
+    if (p->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] problem and handle live on different devices");
+    DeviceGuard guard(h->device);
+    DFK_TRY(problem_error(h, p, p->st(p->cur), 0.0));
+    const char* what = "[WindowProblem::error_ex] copy failed";
+    DFK_CUDA(h, cudaMemcpyAsync(out_dev, p->energy(), sizeof(double) * DFK_WINDOW_ERROR_DOUBLES, cudaMemcpyDeviceToDevice,
+                                h->stream),
+             what);
+    if (p->ndp > 0)
+      DFK_CUDA(h, cudaMemcpyAsync(out_dev + DFK_WINDOW_ERROR_DOUBLES, p->depth_energy(), sizeof(double),
+                                  cudaMemcpyDeviceToDevice, h->stream),
+               what);
+    else
+      DFK_CUDA(h, cudaMemsetAsync(out_dev + DFK_WINDOW_ERROR_DOUBLES, 0, sizeof(double), h->stream), what);
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_problem_set_depth_priors(DfkHandle h, DfkWindowProblem* p, int m, const int32_t* prior_kf,
+                                              const float* sigma, const int32_t* level_ptr,
+                                              const DfkDepthPriorItem* items)
+{
+  return guarded(h, [&] {
+    const char* what = "[WindowProblem::set_depth_priors] ";
+    const std::string w(what);
+    if (!p || m < 0 || (m > 0 && (!prior_kf || !sigma || !level_ptr || !items)))
+      return fail(h, DFK_ERR_INVALID_ARG, w + "null argument");
+    if (p->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] problem and handle live on different devices");
+    if (m > 0 && level_ptr[0] != 0) return fail(h, DFK_ERR_INVALID_ARG, w + "level_ptr[0] must be 0");
+    for (int i = 0; i < m; ++i) {
+      const std::string pre = w + "prior " + std::to_string(i);
+      if (prior_kf[i] < 0 || prior_kf[i] >= p->K) return fail(h, DFK_ERR_INVALID_ARG, pre + " names a keyframe outside the window");
+      if (!std::isfinite(sigma[i]) || !(sigma[i] > 0.0f))
+        return fail(h, DFK_ERR_INVALID_ARG, pre + ": sigma must be finite and > 0");
+      if (level_ptr[i + 1] <= level_ptr[i] || level_ptr[i + 1] > 65535)
+        return fail(h, DFK_ERR_INVALID_ARG, pre + " has no items (level_ptr must increase) or more than 65535 in all");
+    }
+    DeviceGuard guard(h->device);
+    if (m == 0) {
+      p->ndp = p->ndpi = 0;
+      return DFK_OK;
+    }
+    const int n = level_ptr[m];
+    // the items' views are checked as the batch checks them; their codes come from the state (slot = prior_kf)
+    int max_parts = 1, rows = 0;
+    DFK_TRY(stage_depth_prior(h, what, items, n, p->C, false, p->dp_host, p->dp, &max_parts, &rows));
+    std::vector<int> lists;
+    add_csr(lists, p->K, m, [&](int i) { return prior_kf[i]; });
+    const size_t lp = lists.size();
+    lists.insert(lists.end(), level_ptr, level_ptr + m + 1);
+    const size_t sg = lists.size();
+    lists.resize(sg + m);
+    memcpy(lists.data() + sg, sigma, sizeof(float) * m);
+    const size_t kf = lists.size();
+    for (int i = 0; i < m; ++i)
+      for (int l = level_ptr[i]; l < level_ptr[i + 1]; ++l) lists.push_back(prior_kf[i]);
+    const char* amsg = "[WindowProblem::set_depth_priors] allocation failed";
+    DFK_CUDA(h, p->dp_lists.ensure(lists.size()), amsg);
+    DFK_CUDA(h, p->dp_partials.ensure((size_t)rows * depth_prior_partial_floats(p->C, true)), amsg);
+    DFK_CUDA(h, p->dp_records.ensure((size_t)n * DFK_DEPTH_RECORD_FLOATS(p->C)), amsg);
+    DFK_CUDA(h, p->dp_err.ensure((size_t)n * 2), amsg);
+    DFK_CUDA(h, cudaMemcpyAsync(p->dp_lists.ptr, lists.data(), sizeof(int) * lists.size(), cudaMemcpyHostToDevice,
+                                h->stream),
+             "[WindowProblem::set_depth_priors] upload failed");
+    p->ndp = m;
+    p->ndpi = n;
+    p->dp_max_parts = max_parts;
+    p->dp_rows = rows;
+    p->dp_code_off = (sizeof(DepthPriorDesc) * (size_t)n + 15) & ~(size_t)15;
+    p->dp_lp = lp;
+    p->dp_sg = sg;
+    p->dp_kf = kf;
     return DFK_OK;
   });
 }

@@ -89,6 +89,11 @@ struct DfkContext {
   // dfk_update_depth_batch: [descriptors | codes] (bytes), one H2D per call from depth_host
   DeviceBuf<unsigned char> depth_dev;
   std::vector<unsigned char> depth_host;
+  // dfk_depth_prior_linearize_batch / dfk_depth_prior_error_batch: [descriptors | codes] (bytes), one H2D per call from
+  // depth_prior_host, and the items' partial rows
+  DeviceBuf<unsigned char> depth_prior_dev;
+  std::vector<unsigned char> depth_prior_host;
+  DeviceBuf<float> depth_prior_partials;
 
   // dfk_reprojection_linearize / dfk_sparse_geometric_linearize: [one item's staging block | rows (| err2)]
   DeviceBuf<unsigned char> sparse_dev;
@@ -320,6 +325,55 @@ inline void set_depth_decode_desc(DepthDecodeDesc& d, const DfkDepthDecodeItem& 
   d.nblocks = update_depth_blocks(d.width, d.height);
   d.vector = update_depth_vector(code_size, d.code, d.jac) ? 1 : 0;
   *max_blocks = std::max(*max_blocks, d.nblocks);
+}
+
+// Checks and stages n depth-prior items in one upload, [descriptors n | codes n x C] packed in `host` and copied to
+// `dev` (codes: the items' HOST codes; with codes == false -- the window problem, which rewrites them from its state on
+// the device before every batch -- left zero and the items' code fields ignored).
+// *max_parts: the grid's partial blocks, *rows: the partial rows of the batch.
+inline DfkStatus stage_depth_prior(DfkHandle h, const char* what, const DfkDepthPriorItem* items, int n, int code_size,
+                                   bool codes, std::vector<unsigned char>& host, DeviceBuf<unsigned char>& dev,
+                                   int* max_parts, int* rows)
+{
+  const std::string w(what);
+  if (!items || n < 1 || n > 65535)  // blockIdx.y of the partial kernel is the item
+    return fail(h, DFK_ERR_INVALID_ARG, w + "null argument / number of items not in [1, 65535]");
+  if (!depth_supported(code_size))
+    return fail(h, DFK_ERR_UNSUPPORTED, w + "code size not instantiated: " + std::to_string(code_size));
+  for (int i = 0; i < n; ++i) {
+    const DfkDepthPriorItem& it = items[i];
+    const uint32_t W = it.target_dpt.width, H = it.target_dpt.height;
+    if ((codes && !it.code) || W == 0 || H == 0 || (uint64_t)W * H > (uint64_t)INT32_MAX ||
+        !img_ok(&it.target_dpt, W, H, 1) || !img_ok(&it.prx_orig, W, H, 1) || !img_ok(&it.prx_jac, W, H, code_size))
+      return fail(h, DFK_ERR_INVALID_ARG, w + "null code or inconsistent image views in item " + std::to_string(i));
+  }
+  const size_t desc_bytes = (sizeof(DepthPriorDesc) * (size_t)n + 15) & ~(size_t)15;
+  const size_t total = desc_bytes + sizeof(float) * (size_t)n * code_size;
+  DFK_CUDA(h, dev.ensure(total), (w + "scratch allocation failed").c_str());
+  host.assign(total, 0);
+  DepthPriorDesc* descs = reinterpret_cast<DepthPriorDesc*>(host.data());
+  float* code_host = reinterpret_cast<float*>(host.data() + desc_bytes);
+  const float* codes_dev = reinterpret_cast<const float*>(dev.ptr + desc_bytes);
+  *max_parts = 1;
+  *rows = 0;
+  for (int i = 0; i < n; ++i) {
+    const DfkDepthPriorItem& it = items[i];
+    DepthPriorDesc& d = descs[i];
+    d.tgt = view_of(&it.target_dpt);
+    d.prx = view_of(&it.prx_orig);
+    d.jac = view_of(&it.prx_jac);
+    d.code = codes_dev + (size_t)i * code_size;
+    d.width = (int)it.target_dpt.width;
+    d.height = (int)it.target_dpt.height;
+    d.parts = depth_prior_parts(d.width, d.height);
+    d.part0 = *rows;
+    *rows += d.parts;
+    *max_parts = std::max(*max_parts, d.parts);
+    if (codes) memcpy(code_host + (size_t)i * code_size, it.code, sizeof(float) * code_size);
+  }
+  DFK_CUDA(h, cudaMemcpyAsync(dev.ptr, host.data(), total, cudaMemcpyHostToDevice, h->stream),
+           (w + "upload failed").c_str());
+  return DFK_OK;
 }
 
 // n self-resetting tickets of a batched kernel: they must be zero when first used, so a buffer that grows is zeroed

@@ -319,6 +319,32 @@ cudaError_t launch_depth_step(const float* code_dev, int code_size, int width, i
                               View jac, float avg_dpt, float* scratch /*blocks * depth_partial_floats*/,
                               unsigned int* counter, float* out_dev /*C(C+1)/2 + C + 2*/, int blocks, cudaStream_t s);
 
+// dfk_depth_prior.cu : DepthPriorFactor, batched.  One item = one (keyframe, level) of a depth prior.
+struct DepthPriorDesc {
+  View tgt, prx, jac;
+  const float* code;  // code_size floats in device scratch
+  int width, height;
+  int parts;          // depth_prior_parts(width, height): partial rows of this item ...
+  int part0;          // ... from this row of the partial buffer
+};
+// partial rows of an item of this size (its own size alone decides, so a record never depends on the batch)
+int depth_prior_parts(int width, int height);
+// floats per partial row: the augmented Gram (gram) or diff^2 alone
+size_t depth_prior_partial_floats(int code_size, bool gram);
+// gram: n records of DFK_DEPTH_RECORD_FLOATS(code_size) into out_dev; else n rows [residual | inliers (u32 bits)].  Two
+// launches: the partial rows (grid max_parts x n), then one block per item sums them in partial order.
+cudaError_t launch_depth_prior_batch(int code_size, const DepthPriorDesc* descs_dev, int n, int max_parts, float avg_dpt,
+                                     float* partials, float* out_dev, bool gram, cudaStream_t s);
+// m depth priors (kf_ptr[K+1] / kf_priors: the CSR of prior indices per keyframe, in list order; level_ptr[m+1]: the
+// records of each prior; sigma[m]) into an assembled window buffer, in place
+// the codes of n depth-prior items from the state's codes (K x C doubles): item i reads keyframe item_kf[i], rounded to
+// fp32 (what the host staging of the batch does with the same codes), into codes_out (n x C floats)
+cudaError_t launch_depth_prior_codes(const double* state_codes, const int* item_kf, int n, int code_size,
+                                     float* codes_out, cudaStream_t s);
+cudaError_t launch_window_add_depth_priors(const WindowDev& w, int m, const int* kf_ptr_dev, const int* kf_priors_dev,
+                                           const int* level_ptr_dev, const float* sigma_dev, const float* records_dev,
+                                           float* window_dev, cudaStream_t stream);
+
 // dfk_sparse.cu : ReprojectionFactor::linearize and SparseGeometricFactor::linearize, rows (one factor) and records (a
 // batch); the single call runs the batch's descriptor for one item
 bool sparse_supported(int code_size);
@@ -404,6 +430,14 @@ struct WindowEnergyDev {
   const double* codes;        // K * C, for the code prior 1/2 w |c|^2
   int num_codes;
   double code_prior_weight;
+  // depth priors (dfk_window_problem_set_depth_priors), error mode only: prior q's items [level_ptr[q], level_ptr[q+1])
+  // of depth_err ([residual | W * H (u32 bits)] rows), weight 1 / sigma[q]^2; their sum goes to *out_depth and is added
+  // to E after the other parts
+  int num_depth_priors;
+  const float2* depth_err;
+  const int* depth_level_ptr;
+  const float* depth_sigma;
+  double* out_depth;
   double* out;  // [E | photometric | reprojection | geometric | priors | items without inliers | inliers | E + code prior]
 };
 cudaError_t launch_window_energy(const WindowEnergyDev& a, cudaStream_t stream);

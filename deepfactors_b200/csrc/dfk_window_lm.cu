@@ -239,6 +239,16 @@ __global__ void __launch_bounds__(kEnergyThreads) window_energy_kernel(WindowEne
     for (int i = 0; i < a.num_rep; ++i) rep = __dadd_rn(rep, (double)a.err_out[a.num_error + i].x);
     for (int i = 0; i < a.num_geo; ++i) geo = __dadd_rn(geo, (double)a.err_out[a.num_error + a.num_rep + i].x);
     E = __dadd_rn(__dadd_rn(__dadd_rn(phot, rep), geo), priors);
+    if (a.num_depth_priors > 0) {  // prior by prior, level by level, after the other parts (window_opt.WindowError)
+      double dep = 0.0;
+      for (int q = 0; q < a.num_depth_priors; ++q) {
+        const double s2 = __dmul_rn((double)a.depth_sigma[q], (double)a.depth_sigma[q]);
+        for (int l = a.depth_level_ptr[q]; l < a.depth_level_ptr[q + 1]; ++l)
+          dep = __dadd_rn(dep, __ddiv_rn((double)a.depth_err[l].x, s2));
+      }
+      *a.out_depth = dep;
+      E = __dadd_rn(E, dep);
+    }
   }
   double* o = a.out;
   o[0] = E; o[1] = phot; o[2] = rep; o[3] = geo; o[4] = priors; o[5] = no_inl; o[6] = inl;

@@ -338,6 +338,42 @@ class WindowBlocks:
         buf[o_t] = np.float32(fsum)
         return buf
 
+    def add_depth_priors(self, buf, prior_kf, sigma, level_ptr, records):
+        """Host mirror of dfk_window_add_depth_priors, in place on a numpy float32 buffer: depth prior i on keyframe
+        prior_kf[i] with standard deviation sigma[i] owns records[level_ptr[i]:level_ptr[i + 1]] (rows of
+        DFK_DEPTH_RECORD_FLOATS(C) floats: [JtJ packed upper | Jtr | residual | inliers]).  JtJ / sigma^2 goes to the
+        keyframe's code x code block (both triangles), -Jtr / sigma^2 to its code gradient and residual / sigma^2 to f.
+        Each entry sums its terms in fp64, in prior order then level order, onto its float32 value, rounded once.
+        Returns buf."""
+        K, B, c = self.num_keyframes, self.B, self.code_size
+        o_g, _, o_t = self.offsets()
+        nh = c * (c + 1) // 2
+        iu = np.triu_indices(c)
+        recs = np.asarray(records, np.float32).reshape(-1, nh + c + 2)
+        acc = {}  # keyframe -> (fp64 code block, fp64 code gradient)
+        fsum = np.float64(buf[o_t])
+        for i, k in enumerate(prior_kf):
+            k = int(k)
+            if k not in acc:
+                D = np.asarray(buf[k * B * B:(k + 1) * B * B], np.float64).reshape(B, B)[6:, 6:].copy()
+                acc[k] = (D, np.asarray(buf[o_g + k * B + 6:o_g + (k + 1) * B], np.float64).copy())
+            D, g = acc[k]
+            s2 = np.float64(np.float32(sigma[i])) * np.float64(np.float32(sigma[i]))
+            for r in recs[int(level_ptr[i]):int(level_ptr[i + 1])]:
+                J = np.zeros((c, c))
+                J[iu] = r[:nh].astype(np.float64)
+                J[(iu[1], iu[0])] = r[:nh].astype(np.float64)
+                D += J / s2
+                g -= r[nh:nh + c].astype(np.float64) / s2
+                fsum = fsum + np.float64(r[nh + c]) / s2
+        for k, (D, g) in acc.items():
+            blk = buf[k * B * B:(k + 1) * B * B].reshape(B, B)
+            blk[6:, 6:] = D.astype(np.float32)
+            buf[o_g + k * B + 6:o_g + (k + 1) * B] = g.astype(np.float32)
+        if len(prior_kf):
+            buf[o_t] = np.float32(fsum)
+        return buf
+
 
 def shard_pairs(num_pairs: int, world_size: int, rank: int) -> range:
     """Contiguous, balanced shard of the pair list for `rank` (sizes differ by at most one)."""

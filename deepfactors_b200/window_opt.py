@@ -20,6 +20,8 @@ solves.  Here every heavy step of one iteration is ONE device operation over the
     (frames)    tracked frames (Mapper::EnqueueFrame): pose-only variables with one photometric pair each, eliminated
                 first in the device solve; marginalised into linear keyframe priors     dfk_window_marginalize_frames
                 which later windows add after the all-reduce                            dfk_window_add_priors
+    (depth)     depth priors (DepthPriorFactor): one launch linearises every (prior, level) item, one adds them to the
+                buffer                            dfk_depth_prior_linearize_batch / dfk_window_add_depth_priors
     (slide)     a keyframe leaves the window: eliminated from the factors that touch it into a dense linear prior
                 over its blanket                                                        dfk_window_marginalize_keyframe
                 which the next window (without_keyframe) adds after the all-reduce      dfk_window_add_keyframe_priors
@@ -169,10 +171,12 @@ class WindowError:
     priors: float = 0.0        # f0 - 2 g^T d + d^T G d of the frame priors, then of the keyframe priors
     no_inliers: int = 0        # photometric and frame items without inliers (they add 0)
     inliers: int = 0           # total inliers of the photometric and frame items
+    depth: float = 0.0         # sum diff^2 / sigma^2 of the depth priors, prior by prior, level by level
 
     @property
     def energy(self) -> float:
-        return self.photometric + self.reprojection + self.geometric + self.priors
+        e = self.photometric + self.reprojection + self.geometric + self.priors
+        return e + self.depth if self.depth else e
 
 
 def prior_energy(row, delta) -> float:
@@ -622,6 +626,69 @@ class KeyframePrior:
     row: np.ndarray
 
 
+@dataclass
+class DepthPrior:
+    """DepthPriorFactor (sources/core/gtsam/depth_prior_factor.cpp:29-137): a unary factor on keyframe k's code that
+    pulls the depth decoded from it towards a measured depth map, with standard deviation sigma.  target_dpt[l] is the
+    target at pyramid level l (float32 device tensors [H_l, W_l], the keyframe's level sizes); make_depth_prior builds
+    them from level 0 as the factor's constructor does.  Its energy is 0.5 sum diff^2 / sigma^2 over every pixel of every
+    level (in buffer units, twice that); it has no active level: every level always counts."""
+    k: int
+    target_dpt: List[object]
+    sigma: float
+
+
+def depth_prior_sizes(width: int, height: int, levels: int) -> List[Tuple[int, int]]:
+    """(W_l, H_l) of a target pyramid: each level GaussianBlurDown's half of the one above (cu_image_proc.cpp:166-184)"""
+    out = [(int(width), int(height))]
+    for _ in range(1, levels):
+        out.append((out[-1][0] // 2, out[-1][1] // 2))
+    return out
+
+
+def make_depth_prior(k: int, target_dpt, sigma: float, levels: int) -> DepthPrior:
+    """A DepthPrior from a level-0 target depth (a float32 [H, W] device tensor): T_0 = target, T_l =
+    GaussianBlurDown(T_{l-1}) (the constructor, depth_prior_factor.cpp:29-53), in one dfk_build_image_pyramid call."""
+    import torch
+    from .aligners import BuildImagePyramid
+    t0 = target_dpt.contiguous()
+    sizes = depth_prior_sizes(t0.shape[1], t0.shape[0], levels)
+    pyr = [t0] + [torch.empty((h, w), dtype=torch.float32, device=t0.device) for w, h in sizes[1:]]
+    if levels > 1:
+        BuildImagePyramid(pyr)
+    return DepthPrior(int(k), pyr, float(sigma))
+
+
+def _depth_prior_items(prob, priors, codes):
+    """the (prior, level) items of `priors` at these codes, prior by prior, level by level"""
+    return [dict(code=np.asarray(codes[dp.k], np.float32), target_dpt=dp.target_dpt[l],
+                 prx_orig=prob.kf[dp.k][l]["prx_orig"], prx_jac=prob.kf[dp.k][l]["prx_jac"])
+            for dp in priors for l in range(prob.levels)]
+
+
+def depth_prior_rows(records, sigma, levels: int, code_size: int) -> np.ndarray:
+    """Depth priors as linear priors on their keyframe's [pose | code] (DFK_PRIOR_DOUBLES rows [G | g | f0], to be taken
+    at delta = 0): records [n * levels, DFK_DEPTH_RECORD_FLOATS] of n priors, each prior's levels summed in fp64 in level
+    order: G's code block = sum JtJ / sigma^2, g's code part = -sum Jtr / sigma^2, f0 = sum residual / sigma^2."""
+    C, B = code_size, 6 + code_size
+    nh = C * (C + 1) // 2
+    iu = np.triu_indices(C)
+    recs = np.asarray(records, np.float32).reshape(len(sigma), levels, nh + C + 2)
+    rows = np.zeros((len(sigma), B * B + B + 1))
+    for i, sg in enumerate(sigma):
+        s2 = np.float64(np.float32(sg)) * np.float64(np.float32(sg))
+        G, g, f0 = np.zeros((B, B)), np.zeros(B), np.float64(0.0)
+        for r in recs[i]:
+            J = np.zeros((C, C))
+            J[iu] = r[:nh].astype(np.float64)
+            J[(iu[1], iu[0])] = r[:nh].astype(np.float64)
+            G[6:, 6:] += J / s2
+            g[6:] -= r[nh:nh + C].astype(np.float64) / s2
+            f0 = f0 + np.float64(r[nh + C]) / s2
+        rows[i] = np.concatenate([G.ravel(), g, [f0]])
+    return rows
+
+
 def slide_factors(m: int, pairs, links=(), geometric=(), frames=(), priors=(), prior: Optional[KeyframePrior] = None):
     """The factors of a window without keyframe m, renumbered (keyframes above m move down by one): pairs and links that
     touch m are dropped, frames and the priors that do not contain m are kept, and the priors that contain m (frame priors
@@ -739,11 +806,19 @@ class SfmWindowProblem:
     levels; `linearise` then takes the frames' poses.  `priors` (optional) are MarginalPriors of frames marginalised
     out of an earlier window and KeyframePriors of keyframes marginalised out of it: `linearise` adds both kinds to the
     buffer after the all-reduce.  `marginalize` turns frames into MarginalPriors, `marginalize_keyframe` a keyframe into
-    a KeyframePrior, and `without_keyframe` builds the window that slides past it."""
+    a KeyframePrior, and `without_keyframe` builds the window that slides past it.
+
+    `depth_priors` (optional) are DepthPriors: `linearise` re-evaluates every (prior, level) item in one
+    dfk_depth_prior_linearize_batch launch and adds them with dfk_window_add_depth_priors after the assembly and before
+    the all-reduce on rank 0 only when the pairs are sharded, else after the frame and keyframe priors (the order of the
+    device problem); `error` adds their sum diff^2 / sigma^2 (WindowError.depth); `marginalize_keyframe` eliminates those
+    on m with the rest of its factors and `without_keyframe` drops them; `device_problem` hands them to the window
+    problem (dfk_window_problem_set_depth_priors), so DeviceWindowOptimizer runs such a window."""
 
     def __init__(self, aligner, cams, keyframes, pairs, allreduce: Optional[Callable] = None,
                  links: Optional[Sequence[ReprojectionLink]] = None, geometric: Optional[Sequence[GeometricLink]] = None,
-                 frames: Optional[Sequence[TrackedFrame]] = None, priors: Optional[Sequence] = None):
+                 frames: Optional[Sequence[TrackedFrame]] = None, priors: Optional[Sequence] = None,
+                 depth_priors: Optional[Sequence[DepthPrior]] = None):
         import torch
         from . import _lib
         from .aligners import ReprojectionLinearizeBatch, SparseGeometricLinearizeBatch, Window
@@ -755,6 +830,7 @@ class SfmWindowProblem:
         P, K = len(pairs), len(keyframes)
         self._num_photometric = P
         self.priors = list(priors or [])
+        self.depth_priors = list(depth_priors or [])
         self._mpriors = [pr for pr in self.priors if isinstance(pr, MarginalPrior)]
         self._kpriors = [pr for pr in self.priors if isinstance(pr, KeyframePrior)]
         for pr in self._mpriors:
@@ -763,6 +839,7 @@ class SfmWindowProblem:
         self.pairs = [tuple(p) for p in pairs] + [(int(ln.k0), int(ln.k1)) for ln in self.links] + \
             [(int(fr.k), K + f) for f, fr in enumerate(self.frames)]
         self.levels = len(self.cams)
+        self._check_depth_priors()
         item_pair, sizes = [], []
         for p in range(P):
             for l in range(self.levels):
@@ -814,6 +891,39 @@ class SfmWindowProblem:
         self._kprior_rows = torch.as_tensor(np.concatenate([np.asarray(pr.row, dtype=np.float64).ravel()
                                                             for pr in self._kpriors]),
                                             device=dev) if self._kpriors else None
+        nl = len(self.depth_priors) * self.levels
+        self.depth_records = torch.zeros((nl, _lib.depth_record_floats(aligner.CS)), dtype=torch.float32,
+                                         device=dev) if nl else None
+        self._depth_level_ptr = [i * self.levels for i in range(len(self.depth_priors) + 1)]
+
+    def _check_depth_priors(self):
+        K = len(self.kf)
+        for i, dp in enumerate(self.depth_priors):
+            if not 0 <= int(dp.k) < K:
+                raise ValueError(f"depth prior {i} on keyframe {dp.k}, outside the window")
+            if not (np.isfinite(dp.sigma) and dp.sigma > 0):
+                raise ValueError(f"depth prior {i}: sigma must be finite and > 0, got {dp.sigma}")
+            if len(dp.target_dpt) != self.levels:
+                raise ValueError(f"depth prior {i}: {len(dp.target_dpt)} target levels for a {self.levels}-level window")
+            for l, t in enumerate(dp.target_dpt):
+                want = tuple(self.kf[dp.k][l]["prx_orig"].shape[:2])
+                if tuple(t.shape[:2]) != want:
+                    raise ValueError(f"depth prior {i}: level {l} target is {tuple(t.shape[:2])}, keyframe {dp.k}'s "
+                                     f"level is {want}")
+
+    def _counts_depth_priors(self) -> bool:
+        """the sharding rule of dfk_window_add_depth_priors: on a sharded window only rank 0 adds the depth priors, before
+        the all-reduce, so each is counted once"""
+        if self.allreduce is None:
+            return True
+        import torch.distributed as dist
+        return not (dist.is_available() and dist.is_initialized()) or dist.get_rank() == 0
+
+    def _linearise_depth_priors(self, codes, records=None, priors=None):
+        """every (prior, level) item of `priors` (default: all) at `codes`, in one launch, into `records`"""
+        from .aligners import DepthPriorLinearizeBatch
+        items = _depth_prior_items(self, self.depth_priors if priors is None else priors, codes)
+        return DepthPriorLinearizeBatch(self.al, items, self.depth_records if records is None else records)
 
     def set_active(self, mask, error_mask=None):
         """Make only the dense items of `mask` (bools, record order: the photometric then the frame (pair, level)
@@ -936,7 +1046,21 @@ class SfmWindowProblem:
                 terms.append(prior_energy(pr.row, d[at:at + n]))
                 at += n
         ew = window_error_sum(host[:nd], st["areas"], host[nd:nd + nr], host[nd + nr:], terms, self._active)
+        if self.depth_priors and self._counts_depth_priors():
+            ew.depth = self._depth_error(codes)
         return ew.energy, ew
+
+    def _depth_error(self, codes) -> float:
+        """sum diff^2 / sigma^2 of the depth priors at `codes` (dfk_depth_prior_error_batch, one launch), summed in fp64
+        prior by prior, level by level"""
+        from .aligners import DepthPriorErrorBatch
+        res = DepthPriorErrorBatch(self.al, _depth_prior_items(self, self.depth_priors, codes)).cpu().numpy()[:, 0]
+        e = 0.0
+        for i, dp in enumerate(self.depth_priors):
+            s2 = np.float64(np.float32(dp.sigma)) * np.float64(np.float32(dp.sigma))
+            for l in range(self.levels):
+                e += float(np.float64(res[i * self.levels + l]) / s2)
+        return e
 
     def _error_state(self):
         """what error() builds once: the depth scratch and the ctypes item arrays, whose poses and codes each call
@@ -1039,6 +1163,10 @@ class SfmWindowProblem:
             geo=make_geometric_items(geo, C) if geo else None, geo_slots=sl["geo"],
             depth=st["depth_items"], depth_slots=sl["depth"],
             error=st["dense_items"] if st["nd"] else None, error_slots=sl["error"], error_depth=sl["error_depth"], **kw)
+        if self.depth_priors:
+            items = _depth_prior_items(self, self.depth_priors, np.zeros((len(self.kf), C)))
+            self._dev.set_depth_priors([dp.k for dp in self.depth_priors], [dp.sigma for dp in self.depth_priors],
+                                       self._depth_level_ptr, items)
         return self._dev
 
     def linearise(self, poses, codes, todo, frame_poses=None):
@@ -1047,7 +1175,10 @@ class SfmWindowProblem:
             raise ValueError("the window has tracked frames: linearise needs their poses")
         self._linearise_factors(poses, codes, todo, frame_poses)
         buf = self.window.assemble(self.records, geo_records=self.geo_records)
-        if self.allreduce is not None:
+        sharded = self.allreduce is not None
+        if sharded and self.depth_priors and self._counts_depth_priors():  # one rank, before the all-reduce
+            self._add_depth_priors(buf, codes)
+        if sharded:
             self.allreduce(buf)
         # after the all-reduce: every rank adds the priors once
         if self._mpriors:
@@ -1056,7 +1187,14 @@ class SfmWindowProblem:
         if self._kpriors:
             delta = torch.as_tensor(self._kf_deltas(poses, codes), device=buf.device)
             self.window.add_keyframe_priors(buf, self._kprior_rows, delta)
+        if not sharded and self.depth_priors:  # after the priors, the order of dfk_window_problem_linearize
+            self._add_depth_priors(buf, codes)
         return buf, None
+
+    def _add_depth_priors(self, buf, codes):
+        self._linearise_depth_priors(codes)
+        self.window.add_depth_priors(buf, [dp.k for dp in self.depth_priors], [dp.sigma for dp in self.depth_priors],
+                                     self._depth_level_ptr, self.depth_records)
 
     def marginalize_keyframe(self, poses, codes, m: int, frame_poses=None, code_prior_weight: float = 0.0
                              ) -> KeyframePrior:
@@ -1082,6 +1220,15 @@ class SfmWindowProblem:
         if fp:
             frows = torch.as_tensor(np.stack([np.asarray(pr.row, np.float64) for pr in fp]), device=dev)
             fdelta = torch.as_tensor(self._deltas(poses, codes, fp), device=dev)
+        dp = [d for d in self.depth_priors if d.k == m]
+        if dp:  # each a linear prior on m at delta 0, after m's frame priors
+            recs = self._linearise_depth_priors(codes, records=torch.empty(
+                (len(dp) * self.levels, self.depth_records.shape[1]), dtype=torch.float32, device=dev), priors=dp)
+            drows = torch.as_tensor(depth_prior_rows(recs.cpu().numpy(), [d.sigma for d in dp], self.levels,
+                                                     self.al.CS), device=dev)
+            dzero = torch.zeros((len(dp), self.layout.B), dtype=torch.float64, device=dev)
+            frows = drows if frows is None else torch.cat([frows, drows])
+            fdelta = dzero if fdelta is None else torch.cat([fdelta, dzero])
         if self._kpriors:
             krows = self._kprior_rows
             kdelta = torch.as_tensor(self._kf_deltas(poses, codes), device=dev)
@@ -1098,10 +1245,12 @@ class SfmWindowProblem:
         """The next window of a sliding window: keyframe m removed and the rest renumbered, the factors that touch m
         dropped, the priors that contain m replaced by `prior` (marginalize_keyframe's, old numbering), every other
         factor and prior renumbered (slide_factors).  drop_keyframe gives the matching poses and codes."""
+        import dataclasses
         pairs, links, geo, frames, priors = slide_factors(m, self.pairs[:self._num_photometric], self.links,
                                                           self.geometric, self.frames, self.priors, prior)
+        depth = [dataclasses.replace(dp, k=int(dp.k) - (int(dp.k) > m)) for dp in self.depth_priors if dp.k != m]
         return SfmWindowProblem(self.al, self.cams, self.kf[:m] + self.kf[m + 1:], pairs, self.allreduce, links, geo,
-                                frames, priors)
+                                frames, priors, depth)
 
     def marginalize(self, poses, codes, frame_poses, which) -> List[MarginalPrior]:
         """Marginalise the frames `which` at the current point (MarginalizeFrames): their pairs are re-evaluated at

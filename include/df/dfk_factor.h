@@ -16,6 +16,9 @@
 //   LinearizeSparseGeometricBatch
 //                          many sparse geometric factors (use_geometric links) linearised in one launch into device
 //                          records over [pose0 | pose1 | code0 | code1] (WindowSystem::AddGeometric).
+//   DepthPriorFactor       DepthPriorFactor (depth_prior_factor.cpp:29-137): a keyframe code's pull towards a measured depth
+//                          pyramid, every level linearised in one dfk_depth_prior_linearize_batch call
+//                          (WindowSystem::AddDepthPrior, or dfk_window_add_depth_priors on the device).
 //   LinearizeReprojection / LinearizeSparseGeometric
 //                          the Jacobian rows of the two sparse factors (reprojection_factor.cpp:157-269,
 //                          sparse_geometric_factor.cpp:157-271), evaluated on the device from the keyframes' GPU buffers;
@@ -26,6 +29,7 @@
 
 #include <cstddef>
 #include <limits>
+#include <utility>
 #include <vector>
 
 #include "dfk_facade.h"
@@ -122,6 +126,23 @@ public:
       }
     }
     f_ += static_cast<double>(sys.residual);
+  }
+
+  // one level's record of DepthPriorFactor::Linearize on keyframe k ([JtJ packed upper | Jtr | residual | inliers],
+  // DFK_DEPTH_RECORD_FLOATS(CS)): JtJ / sigma^2 to k's code block, -Jtr / sigma^2 to its code gradient and
+  // residual / sigma^2 to f (f is twice the factor-graph error, as everywhere in this system)
+  void AddDepthPrior(int k, const float* record, float sigma)
+  {
+    const double s2 = static_cast<double>(sigma) * static_cast<double>(sigma);
+    const int o = k * Block + 6;
+    int e = 0;
+    for (int i = 0; i < CS; ++i)
+      for (int j = i; j < CS; ++j, ++e) {
+        H(o + i, o + j) += static_cast<double>(record[e]) / s2;
+        if (j != i) H(o + j, o + i) += static_cast<double>(record[e]) / s2;
+      }
+    for (int i = 0; i < CS; ++i) g_[o + i] -= static_cast<double>(record[e + i]) / s2;
+    f_ += static_cast<double>(record[e + CS]) / s2;
   }
 
 private:
@@ -276,6 +297,65 @@ inline void ShardPairs(std::size_t num_pairs, int world_size, int rank, std::siz
   *begin = (num_pairs * static_cast<std::size_t>(rank)) / static_cast<std::size_t>(world_size);
   *end = (num_pairs * static_cast<std::size_t>(rank + 1)) / static_cast<std::size_t>(world_size);
 }
+
+// DepthPriorFactor (depth_prior_factor.cpp:29-137): keyframe `kf`'s code pulled towards a measured depth with standard
+// deviation sigma.  levels[l] = (target depth, proximity, code Jacobian) GPU views of level l; the target pyramid is the
+// caller's (the reference blurs it down once in its constructor: GaussianBlurDown, or dfk_build_image_pyramid).
+// Linearize runs RunAlignment (:107-121) as one dfk_depth_prior_linearize_batch over the levels: record l is level l's
+// DepthAligner::RunStep.  Error is the factor's error() (:62-76), 0.5 sum residual / sigma^2, from
+// dfk_depth_prior_error_batch.  Unlike the reference, neither touches the keyframe's own depth (UpdateKfDepth).
+template <int CS>
+class DepthPriorFactor
+{
+public:
+  struct Level {
+    DfkImage target_dpt, prx_orig, prx_jac;
+  };
+  template <typename ImageBuffer>
+  static Level MakeLevel(const ImageBuffer& target_dpt, const ImageBuffer& prx_orig, const ImageBuffer& prx_jac)
+  {
+    return Level{detail::View(target_dpt, 1), detail::View(prx_orig, 1), detail::View(prx_jac, CS)};
+  }
+
+  DepthPriorFactor(int kf, float sigma, std::vector<Level> levels) : kf_(kf), sigma_(sigma), levels_(std::move(levels)) {}
+  int keyframe() const { return kf_; }
+  float sigma() const { return sigma_; }
+  int num_levels() const { return static_cast<int>(levels_.size()); }
+
+  // the batch items at `code` (CS floats, read when the batch is called)
+  std::vector<DfkDepthPriorItem> Items(const float* code) const
+  {
+    std::vector<DfkDepthPriorItem> out;
+    for (const Level& l : levels_) out.push_back(DfkDepthPriorItem{l.target_dpt, l.prx_orig, l.prx_jac, code});
+    return out;
+  }
+  // records_dev: DEVICE, num_levels() * DFK_DEPTH_RECORD_FLOATS(CS) floats.  Asynchronous on the handle's stream.
+  void Linearize(DfkHandle h, const float* code, float* records_dev) const
+  {
+    const std::vector<DfkDepthPriorItem> it = Items(code);
+    detail::Check(h, dfk_depth_prior_linearize_batch(h, it.data(), num_levels(), CS, records_dev));
+  }
+  // the error rows [residual | W * H (u32 bits)] of every level into out_dev (DEVICE, 2 * num_levels() floats), each
+  // residual bit for bit the one of Linearize's record.  Asynchronous on the handle's stream.
+  void ErrorRows(DfkHandle h, const float* code, float* out_dev) const
+  {
+    const std::vector<DfkDepthPriorItem> it = Items(code);
+    detail::Check(h, dfk_depth_prior_error_batch(h, it.data(), num_levels(), CS, out_dev));
+  }
+  // error() from those rows copied to the host: 0.5 sum residual / sigma^2 over the levels
+  double Error(const float* rows_host) const
+  {
+    const double s2 = static_cast<double>(sigma_) * static_cast<double>(sigma_);
+    double e = 0.0;
+    for (std::size_t l = 0; l < levels_.size(); ++l) e += static_cast<double>(rows_host[2 * l]) / s2;
+    return 0.5 * e;
+  }
+
+private:
+  int kf_;
+  float sigma_;
+  std::vector<Level> levels_;
+};
 
 }  // namespace df
 

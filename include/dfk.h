@@ -476,6 +476,44 @@ DfkStatus dfk_depth_run_step(DfkHandle h, const float* code, int code_size, cons
                              const DfkImage* prx_orig, const DfkImage* prx_jac,
                              float* JtJ, float* Jtr, float* residual, uint64_t* inliers);
 
+/* DepthPriorFactor (sources/core/gtsam/depth_prior_factor.cpp:29-137), batched: a unary factor on one keyframe's code
+ * that pulls the depth decoded from it towards a measured depth map, one DepthAligner::RunStep per pyramid level
+ * (RunAlignment, :107-121).  One item is one (keyframe, level): the level's target depth (the factor's blurred-down
+ * target pyramid), the keyframe's proximity and code Jacobian at that level, and its code (HOST, code_size floats; all
+ * codes go up in one copy).  Pitched views are allowed and every item may have its own size. */
+typedef struct {
+  DfkImage target_dpt, prx_orig, prx_jac;
+  const float* code;
+} DfkDepthPriorItem;
+/* a record of dfk_depth_prior_linearize_batch: [JtJ packed upper C(C+1)/2 | Jtr C | residual | inliers (u32 bits)] */
+#define DFK_DEPTH_RECORD_FLOATS(C) ((C) * ((C) + 1) / 2 + (C) + 2)
+/* records_dev (DEVICE, n * DFK_DEPTH_RECORD_FLOATS(code_size) floats): record i is item i's dfk_depth_run_step result,
+ * JtJ / Jtr / residual = sum diff^2 / inliers = W * H, with the handle's avg_dpt.  code_size in {8, 16, 32, 64, 128}.
+ * The fp32 chunked Gram of dfk_depth_run_step over a grid of (item, partial); an item's partials are summed in a fixed
+ * order in fp64 and rounded once.  Deterministic, no atomics: two calls agree bit for bit and a record does not depend on
+ * the other items.  1 <= n <= 65535; a malformed item (NULL code, sizes that differ between its views, a bad pitch) is
+ * rejected with nothing written.  Asynchronous on the handle's stream, two launches. */
+DfkStatus dfk_depth_prior_linearize_batch(DfkHandle h, const DfkDepthPriorItem* items, int n, int code_size,
+                                          float* records_dev);
+/* out_dev (DEVICE, n x 2 floats): [residual | inliers (u32 bits)] of every item, the residual bit for bit the one of
+ * dfk_depth_prior_linearize_batch's record for the same item.  The same checks; asynchronous, two launches. */
+DfkStatus dfk_depth_prior_error_batch(DfkHandle h, const DfkDepthPriorItem* items, int n, int code_size,
+                                      float* out_dev);
+/* Add m depth priors to an assembled window buffer in place.  Prior i is on keyframe prior_kf_host[i] with standard
+ * deviation sigma_host[i] (finite, > 0) and owns the records [level_ptr_host[i], level_ptr_host[i + 1]) of records_dev
+ * (DEVICE, dfk_depth_prior_linearize_batch's records; level_ptr_host[0] = 0 and strictly increasing: every prior owns
+ * at least one record; HOST arrays copied).  It
+ * adds JtJ / sigma^2 to D_k's code x code sub-block (both triangles), -Jtr / sigma^2 to g_k's code part and
+ * residual / sigma^2 to f (buffer units: f is twice the factor-graph error 0.5 residual / sigma^2, see DESIGN's quirk on
+ * the constant of the reference's HessianFactor); the inlier total is unchanged.  Every entry sums its terms in fp64, in
+ * prior order and then level order, onto its fp32 value and is rounded once (no atomics).  Sharding rule: with sharded
+ * pairs, one rank (rank 0) linearises the depth priors and adds them to its buffer BEFORE the all-reduce, and the other
+ * ranks add none, so every prior is counted once and only one rank pays for its Gram.  A prior on a keyframe outside the
+ * window or with a bad sigma is rejected with nothing written; m = 0 writes nothing.  One launch. */
+DfkStatus dfk_window_add_depth_priors(DfkHandle h, const DfkWindow* w, int m, const int32_t* prior_kf_host,
+                                      const float* sigma_host, const int32_t* level_ptr_host, const float* records_dev,
+                                      float* window_dev);
+
 /* ------------------------------------------------------------------ sparse keypoint factor */
 
 /* ReprojectionFactor::linearize (sources/core/gtsam/reprojection_factor.cpp:157-269): the Jacobian rows of a keypoint
@@ -1119,6 +1157,26 @@ DfkStatus dfk_window_problem_error(DfkHandle h, DfkWindowProblem* p, double* out
 /* state <- retract(state, dx): t += dt, q = normalize(exp(w) q), c += dc, in fp64, for the keyframes and then the frames
  * (dx_dev: DEVICE, K (6 + C) + 6 F doubles, the solve's layout).  Asynchronous. */
 DfkStatus dfk_window_problem_retract(DfkHandle h, DfkWindowProblem* p, const double* dx_dev);
+/* Depth priors of the problem (DepthPriorFactor, dfk_depth_prior_linearize_batch).  Prior i is on keyframe prior_kf[i]
+ * with standard deviation sigma[i] (finite, > 0) and owns the items [level_ptr[i], level_ptr[i + 1]) of `items`
+ * (typically one per level; level_ptr[0] = 0, strictly increasing, level_ptr[m] <= 65535).  The items' code fields are
+ * ignored: an item reads its prior's keyframe code from the state, rounded to fp32, on the device.  HOST arrays,
+ * copied and validated as the batch validates them; the image views are the caller's and must outlive the problem.
+ * Call it after create and before the linearize it should affect; m = 0 removes them.  With depth priors:
+ *   linearize  after the frame and keyframe priors, one dfk_depth_prior_linearize_batch over every item into records
+ *              of the problem's own and one dfk_window_add_depth_priors
+ *   error      E gains the depth-prior part, sum residual / sigma^2 prior by prior and level by level in fp64 from one
+ *              dfk_depth_prior_error_batch, added after the other parts (dfk_window_problem_error_ex reports it)
+ *   LM         dfk_window_lm and dfk_window_lm_levels take them through linearize and error; they have no level, so
+ *              set_active and the level schedules leave them active
+ * A problem without depth priors computes bit for bit what it computed before.  A rejected call changes nothing. */
+DfkStatus dfk_window_problem_set_depth_priors(DfkHandle h, DfkWindowProblem* p, int m, const int32_t* prior_kf,
+                                              const float* sigma, const int32_t* level_ptr,
+                                              const DfkDepthPriorItem* items);
+/* doubles of dfk_window_problem_error_ex's output: dfk_window_problem_error's, then the depth-prior part */
+#define DFK_WINDOW_ERROR_EX_DOUBLES 8
+/* dfk_window_problem_error, plus out_dev[7] = the depth-prior part of E (0 without depth priors).  Asynchronous. */
+DfkStatus dfk_window_problem_error_ex(DfkHandle h, DfkWindowProblem* p, double* out_dev);
 
 /* window_opt.LMParams; lambda_up and lambda_down finite and > 0 */
 typedef struct {

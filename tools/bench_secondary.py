@@ -71,9 +71,12 @@ One JSON line per case:
     bare C call on buffers and items built once (wall clock to a synchronise), summed device time and the time of each
     kernel from a separate profiled run, the algorithmic bytes and achieved bandwidth over the device time, and the
     sequential C oracle (mesh_oracle) on one host thread from the depth, keyframe by keyframe.
+  * depth priors (`--only depth_prior`): 50 keyframes x 4 levels from 640x480 at C = 32 and 128, one
+    dfk_depth_prior_linearize_batch call (200 items) against the same 200 dfk_depth_run_step calls, and the error batch;
+    window200 with a depth prior on every keyframe, a 10-iteration DeviceWindowOptimizer run with and without them.
 Every line carries the card's name and power limit.  `--only reprojection` / `--only geometric` / `--only solve` /
 `--only frames` / `--only slide` / `--only error` / `--only lm` / `--only levels` / `--only match` / `--only orb` /
-`--only orb_pyramid` / `--only preprocess` / `--only bow` / `--only mesh` runs those cases alone.
+`--only orb_pyramid` / `--only preprocess` / `--only bow` / `--only mesh` / `--only depth_prior` runs those cases alone.
 Peak for the roofline fraction: MEASURED_PEAKS.json hbm_gbs (fallback 3350 GB/s, H100 SXM data sheet).
 """
 from __future__ import annotations
@@ -93,7 +96,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--only", choices=["reprojection", "geometric", "solve", "frames", "slide", "error", "lm", "levels",
-                                           "match", "orb", "orb_pyramid", "preprocess", "bow", "mesh"],
+                                           "match", "orb", "orb_pyramid", "preprocess", "bow", "mesh", "depth_prior"],
                     default=None)
     args = ap.parse_args()
     import numpy as np
@@ -144,6 +147,8 @@ def main():
         return bow_cases(args, torch, print)
     if args.only == "mesh":
         return mesh_cases(args, torch, print)
+    if args.only == "depth_prior":
+        return depth_prior_cases(args, torch, print)
 
     def upload(L):
         d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in dict(
@@ -340,6 +345,114 @@ def _wall_us(torch, fn, reps):
         fn()
     torch.cuda.synchronize()
     return (time.perf_counter() - t0) / reps * 1e6
+
+
+def depth_prior_cases(args, torch, print):
+    """50 keyframes x 4 levels (640x480 .. 80x60), random proximity, code Jacobian and target on the device: one
+    DepthPriorLinearizeBatch / DepthPriorErrorBatch call over the 200 items against the 200 synchronous
+    DepthAligner.RunStep calls the host loop makes; the records are checked against the single calls."""
+    import numpy as np
+
+    from deepfactors_b200.aligners import DepthAligner, DepthPriorErrorBatch, DepthPriorLinearizeBatch, SfmAligner
+    K, L = 50, 4
+    gen = torch.Generator(device="cuda").manual_seed(3)
+    for cs in (32, 128):
+        items = []
+        for k in range(K):
+            for l in range(L):
+                w, h = 640 >> l, 480 >> l
+                prx = 0.3 + 0.4 * torch.rand((h, w), device="cuda", generator=gen)
+                jac = 0.02 * torch.randn((h, w, cs), device="cuda", generator=gen)
+                tgt = 1.0 + 0.5 * torch.rand((h, w), device="cuda", generator=gen)
+                items.append(dict(code=(np.random.default_rng(k).standard_normal(cs) * 0.1).astype(np.float32),
+                                  target_dpt=tgt, prx_orig=prx, prx_jac=jac))
+        al, da = SfmAligner(cs), DepthAligner(cs)
+        from deepfactors_b200.aligners import make_depth_prior_items
+        arr = make_depth_prior_items(items, cs)
+        rec = DepthPriorLinearizeBatch(al, arr)
+        err = DepthPriorErrorBatch(al, arr)
+        torch.cuda.synchronize()
+        worst = 0.0
+        for i in (0, 1, 2, 3, len(items) - 1):  # the batch against the single call (different partial sums)
+            one = da.RunStep(items[i]["code"], items[i]["target_dpt"], items[i]["prx_orig"], items[i]["prx_jac"])
+            got = rec[i].cpu().numpy()[:cs * (cs + 1) // 2]
+            worst = max(worst, float(np.abs(got - one.JtJ).max() / np.abs(one.JtJ).max()))
+        batch_us = _wall_us(torch, lambda: DepthPriorLinearizeBatch(al, arr, rec), args.reps)
+        error_us = _wall_us(torch, lambda: DepthPriorErrorBatch(al, arr, err), args.reps)
+
+        def loop():
+            for it in items:
+                da.RunStep(it["code"], it["target_dpt"], it["prx_orig"], it["prx_jac"])
+        loop_us = _wall_us(torch, loop, max(2, args.reps // 4))
+        kern_us = _device_us(torch, lambda: DepthPriorLinearizeBatch(al, arr, rec), args.reps)
+        px = sum((640 >> l) * (480 >> l) for l in range(L)) * K
+        print(json.dumps({"case": "depth_prior", "code_size": cs, "keyframes": K, "levels": L, "items": K * L,
+                          "batch_us": batch_us, "batch_device_us": kern_us, "error_batch_us": error_us,
+                          "run_step_loop_us": loop_us, "speedup": loop_us / batch_us,
+                          "gflops_fp32": 2.0 * px * ((cs + 1) * (cs + 2) // 2) / (kern_us * 1e3),
+                          "max_rel_jtj_vs_single_call": worst}))
+        del items, arr, rec, err
+        torch.cuda.empty_cache()
+    depth_prior_lm_cases(args, torch, print)
+
+
+def depth_prior_lm_cases(args, torch, print):
+    """window200 at C = 32 and 128 with a depth prior on every keyframe (the target 2 % behind the scene's depth, sigma
+    0.1): a 10-iteration DeviceWindowOptimizer run with the depth priors against the same run without them, and against
+    WindowOptimizer(solve=prob.solve) with them, alternated from one perturbed start"""
+    import numpy as np
+    from deepfactors_b200 import se3, synth
+    from deepfactors_b200.aligners import SfmAligner
+    from deepfactors_b200.window_opt import (DeviceWindowOptimizer, LMParams, SfmWindowProblem, WindowOptimizer,
+                                             make_depth_prior)
+    from bench import window_pairs
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
+    levels, num_kf, reps = 4, 50, 3
+    for cs in (32, 128):
+        base = synth.make_pair(640, 480, cs, levels, seed=7)
+        shared = [dict(img=up(L.img0), grad=up(L.grad1), prx_orig=up(L.prx_orig)) for L in base.levels]
+        jac = [up(L.prx_jac) for L in base.levels]
+        gen = torch.Generator(device="cuda").manual_seed(cs)
+        keyframes = [[dict(sh, prx_jac=j + 1e-3 * torch.randn(j.shape, device="cuda", generator=gen),
+                           dpt=torch.zeros_like(sh["img"]), valid=torch.zeros_like(sh["img"]))
+                      for sh, j in zip(shared, jac)] for _ in range(num_kf)]
+        pairs, cams, al = window_pairs(num_kf, 200), [L.cam for L in base.levels], SfmAligner(cs)
+        target = up(base.levels[0].dpt0 * np.float32(1.02))
+        dps = [make_depth_prior(k, target, 0.1, levels) for k in range(num_kf)]
+        rng = np.random.default_rng(cs)
+        poses = np.stack([se3.make_pose(rng.standard_normal(3) * 0.003, rng.standard_normal(3) * 0.01, np.float64)
+                          for _ in range(num_kf)])
+        poses[0] = se3.identity(np.float64)
+        codes = np.zeros((num_kf, cs))
+        prm = LMParams(iterations=10, lambda_init=1e-4)
+        runs = {}
+        for name, dp in (("DeviceWindowOptimizer, depth priors", dps), ("DeviceWindowOptimizer, no depth priors", None),
+                         ("WindowOptimizer(solve=prob.solve), depth priors", dps)):
+            p = SfmWindowProblem(al, cams, keyframes, pairs, depth_priors=dp)
+            if name.startswith("Device"):
+                opt = DeviceWindowOptimizer(p, prm)
+                runs[name] = (lambda o=opt: o.run(poses, codes))
+            else:
+                runs[name] = (lambda p=p: WindowOptimizer(p.layout, p.linearise, prm, solve=p.solve).run(poses, codes))
+        traces, walls = {}, {n: [] for n in runs}
+        for name, fn in runs.items():
+            _, _, traces[name] = fn()
+        torch.cuda.synchronize()
+        for _ in range(reps):
+            for name, fn in runs.items():
+                t0 = time.perf_counter()
+                fn()
+                torch.cuda.synchronize()
+                walls[name].append((time.perf_counter() - t0) * 1e6)
+        for name, fn in runs.items():
+            tr = traces[name]
+            print(json.dumps({"case": f"window200 C={cs} ({num_kf} keyframes, {len(pairs)} pairs, {levels} levels "
+                                      f"640x480): 10-iteration LM, {name}",
+                              "us_total": float(np.median(walls[name])), "us_runs": walls[name],
+                              "linearisations": tr.linearisations, "accepted": tr.accepted,
+                              "energy_first_last": [tr.energy[0], tr.energy[-1]]}), flush=True)
+        del runs, keyframes, shared, jac, dps
+        torch.cuda.empty_cache()
 
 
 def reprojection_cases(args, torch, print):
