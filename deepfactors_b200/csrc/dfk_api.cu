@@ -622,7 +622,8 @@ DfkStatus dfk_sfm_evaluate_error_batch(DfkHandle h, const DfkSfmWorkItem* items,
     if (!items || !out_dev || n < 1 || n > 65535)  // blockIdx.y of the kernel is the item
       return fail(h, DFK_ERR_INVALID_ARG,
                   "[SfmAligner::EvaluateError batch] null argument / number of items not in [1, 65535]");
-    h->eval_host.resize(n);
+    Staging s(h->staging);
+    const Part<EvalErrorDesc> descs = s.add<EvalErrorDesc>(n);
     int max_blocks = 1, rows = 0;
     for (int i = 0; i < n; ++i) {
       const DfkSfmWorkItem& w = items[i];
@@ -638,17 +639,14 @@ DfkStatus dfk_sfm_evaluate_error_batch(DfkHandle h, const DfkSfmWorkItem* items,
                     "[SfmAligner::EvaluateError batch] camera viewport larger than the image views" + at);
       float p10[7];
       relative_pose(w.pose1, w.pose0, p10, nullptr, nullptr);
-      set_eval_error_desc(h->eval_host[i], w.cam, p10, w.img0, w.img1, w.dpt0, &rows, &max_blocks);
+      set_eval_error_desc(descs.at(s.host())[i], w.cam, p10, w.img0, w.img1, w.dpt0, &rows, &max_blocks);
     }
     DeviceGuard guard(h->device);
-    DFK_CUDA(h, h->eval_descs.ensure((size_t)n), "[SfmAligner::EvaluateError batch] scratch allocation failed");
     DFK_CUDA(h, h->eval_partials.ensure((size_t)rows * 32), "[SfmAligner::EvaluateError batch] scratch allocation failed");
     DFK_TRY(ensure_tickets(h, h->eval_counters, (size_t)n, "[SfmAligner::EvaluateError batch] scratch allocation failed",
                            "[SfmAligner::EvaluateError batch] memset failed"));
-    DFK_CUDA(h, cudaMemcpyAsync(h->eval_descs.ptr, h->eval_host.data(), sizeof(EvalErrorDesc) * n,
-                                cudaMemcpyHostToDevice, h->stream),
-             "[SfmAligner::EvaluateError batch] upload failed");
-    DFK_CUDA(h, launch_eval_error_batch(h->eval_descs.ptr, n, max_blocks, h->params.sfmparams.huber_delta,
+    DFK_TRY(s.upload(h, h->eval_descs, "[SfmAligner::EvaluateError batch] "));
+    DFK_CUDA(h, launch_eval_error_batch(descs.at(s.dev), n, max_blocks, h->params.sfmparams.huber_delta,
                                         h->eval_partials.ptr, h->eval_counters.ptr, out_dev, h->stream),
              "[SfmAligner::EvaluateError batch] kernel launch failed");
     h->launches += 1;
@@ -773,41 +771,40 @@ DfkStatus dfk_se3_track_batch(DfkHandle h, int num_problems, int num_levels, flo
       }
     }
     DeviceGuard guard(h->device);
-    const size_t desc_bytes = (descs.size() * sizeof(Se3TrackDesc) + 15) & ~(size_t)15;
-    const size_t pose_bytes = sizeof(float) * 8 * (size_t)N, out_bytes = sizeof(float) * 32 * (size_t)N;
-    const size_t total = desc_bytes + pose_bytes + out_bytes;
-    DFK_CUDA(h, h->batch_dev.ensure(total), "[CameraTracker::TrackFrame batch] scratch allocation failed");
+    Layout B;
+    const Part<Se3TrackDesc> descs_at = B.add<Se3TrackDesc>(descs.size());
+    const Part<float> poses_at = B.add<float>(8 * (size_t)N), outs_at = B.add<float>(32 * (size_t)N);
+    DFK_CUDA(h, h->batch_dev.ensure(B.bytes), "[CameraTracker::TrackFrame batch] scratch allocation failed");
     DFK_CUDA(h, h->batch_partials.ensure((size_t)N * stride * 32),
              "[CameraTracker::TrackFrame batch] scratch allocation failed");
     DFK_TRY(ensure_tickets(h, h->batch_counters, (size_t)N, "[CameraTracker::TrackFrame batch] scratch allocation failed",
                            "[CameraTracker::TrackFrame batch] memset failed"));
-    DFK_CUDA(h, h->batch_host.ensure(total), "[CameraTracker::TrackFrame batch] pinned allocation failed");
+    DFK_CUDA(h, h->batch_host.ensure(B.bytes), "[CameraTracker::TrackFrame batch] pinned allocation failed");
     // one upload: every level's descriptors and the start poses
-    memcpy(h->batch_host.ptr, descs.data(), descs.size() * sizeof(Se3TrackDesc));
-    float* host_poses = reinterpret_cast<float*>(h->batch_host.ptr + desc_bytes);
-    const float* host_outs = host_poses + 8 * (size_t)N;
+    memcpy(descs_at.at(h->batch_host.ptr), descs.data(), descs.size() * sizeof(Se3TrackDesc));
+    float* host_poses = poses_at.at(h->batch_host.ptr);
+    const float* host_outs = outs_at.at(h->batch_host.ptr);
     for (int n = 0; n < N; ++n) {
       memcpy(host_poses + 8 * (size_t)n, poses_ck + 7 * (size_t)n, sizeof(float) * 7);
       host_poses[8 * (size_t)n + 7] = 0.0f;
     }
-    DFK_CUDA(h, cudaMemcpyAsync(h->batch_dev.ptr, h->batch_host.ptr, desc_bytes + pose_bytes, cudaMemcpyHostToDevice,
-                                h->stream),
+    DFK_CUDA(h, cudaMemcpyAsync(h->batch_dev.ptr, h->batch_host.ptr, outs_at.off, cudaMemcpyHostToDevice, h->stream),
              "[CameraTracker::TrackFrame batch] upload failed");
-    const Se3TrackDesc* descs_dev = reinterpret_cast<const Se3TrackDesc*>(h->batch_dev.ptr);
-    float* poses_dev = reinterpret_cast<float*>(h->batch_dev.ptr + desc_bytes);
-    float* outs_dev = poses_dev + 8 * (size_t)N;
-    DFK_CUDA(h, cudaMemsetAsync(outs_dev, 0, out_bytes, h->stream), "[CameraTracker::TrackFrame batch] memset failed");
+    float* poses_dev = poses_at.at(h->batch_dev.ptr);
+    float* outs_dev = outs_at.at(h->batch_dev.ptr);
+    DFK_CUDA(h, cudaMemsetAsync(outs_dev, 0, B.bytes - outs_at.off, h->stream),
+             "[CameraTracker::TrackFrame batch] memset failed");
     for (int l = L - 1; l >= 0; --l) {  // coarse to fine (camera_tracker.cpp:48)
       for (int k = 0; k < levels[l].iterations; ++k) {
-        DFK_CUDA(h, launch_se3_track_batch(descs_dev + (size_t)l * N, N, level_blocks[l], h->se3_huber_delta,
-                                           h->batch_partials.ptr, stride, h->batch_counters.ptr, outs_dev, poses_dev,
-                                           h->stream),
+        DFK_CUDA(h, launch_se3_track_batch(descs_at.at(h->batch_dev.ptr) + (size_t)l * N, N, level_blocks[l],
+                                           h->se3_huber_delta, h->batch_partials.ptr, stride, h->batch_counters.ptr,
+                                           outs_dev, poses_dev, h->stream),
                  "[CameraTracker::TrackFrame batch] kernel launch failed");
         h->launches += 1;
       }
     }
     // one read-back: final poses and last evaluated systems
-    DFK_TRY(download(h, host_poses, poses_dev, pose_bytes + out_bytes, "[CameraTracker::TrackFrame batch] read-back failed",
+    DFK_TRY(download(h, host_poses, poses_dev, B.bytes - poses_at.off, "[CameraTracker::TrackFrame batch] read-back failed",
                      "[CameraTracker::TrackFrame batch] stream synchronize failed"));
     for (int n = 0; n < N; ++n) {
       memcpy(poses_ck + 7 * (size_t)n, host_poses + 8 * (size_t)n, sizeof(float) * 7);
@@ -878,24 +875,20 @@ DfkStatus dfk_update_depth_batch(DfkHandle h, const DfkDepthDecodeItem* items, i
                     "[UpdateDepth batch] null code or inconsistent image views in item " + std::to_string(i));
     }
     DeviceGuard guard(h->device);
-    const size_t desc_bytes = (sizeof(DepthDecodeDesc) * (size_t)n + 15) & ~(size_t)15;
-    const size_t total = desc_bytes + sizeof(float) * (size_t)n * code_size;
-    DFK_CUDA(h, h->depth_dev.ensure(total), "[UpdateDepth batch] scratch allocation failed");
-    h->depth_host.assign(total, 0);
-    DepthDecodeDesc* descs = reinterpret_cast<DepthDecodeDesc*>(h->depth_host.data());
-    float* codes = reinterpret_cast<float*>(h->depth_host.data() + desc_bytes);
-    const float* codes_dev = reinterpret_cast<const float*>(h->depth_dev.ptr + desc_bytes);
+    Staging s(h->staging);
+    const Part<DepthDecodeDesc> descs = s.add<DepthDecodeDesc>(n);
+    const Part<float> codes = s.add<float>((size_t)n * code_size);
+    DFK_TRY(s.grow(h, h->depth_dev, "[UpdateDepth batch] "));
     int max_blocks = 1;
     for (int i = 0; i < n; ++i) {
       const DfkDepthDecodeItem& it = items[i];
-      set_depth_decode_desc(descs[i], it, code_size, codes_dev + (size_t)i * code_size, static_cast<float*>(it.dpt.ptr),
-                            (uint32_t)(it.dpt.pitch_bytes / 4), &max_blocks);
-      memcpy(codes + (size_t)i * code_size, it.code, sizeof(float) * code_size);
+      set_depth_decode_desc(descs.at(s.host())[i], it, code_size, codes.at(s.dev) + (size_t)i * code_size,
+                            static_cast<float*>(it.dpt.ptr), (uint32_t)(it.dpt.pitch_bytes / 4), &max_blocks);
+      memcpy(codes.at(s.host()) + (size_t)i * code_size, it.code, sizeof(float) * code_size);
     }
-    DFK_CUDA(h, cudaMemcpyAsync(h->depth_dev.ptr, h->depth_host.data(), total, cudaMemcpyHostToDevice, h->stream),
-             "[UpdateDepth batch] upload failed");
-    DFK_CUDA(h, launch_update_depth_batch(code_size, reinterpret_cast<const DepthDecodeDesc*>(h->depth_dev.ptr), n,
-                                          max_blocks, h->params.sfmparams.avg_dpt, h->stream),
+    DFK_TRY(s.upload(h, h->depth_dev, "[UpdateDepth batch] "));
+    DFK_CUDA(h, launch_update_depth_batch(code_size, descs.at(s.dev), n, max_blocks, h->params.sfmparams.avg_dpt,
+                                          h->stream),
              "[UpdateDepth batch] kernel launch failed");
     h->launches += 1;
     return DFK_OK;
@@ -984,11 +977,10 @@ DfkStatus dfk_preprocess_batch(DfkHandle h, const DfkPreprocessItem* items, int 
       return fail(h, DFK_ERR_INVALID_ARG, w + "number of levels not in [0, DFK_PREPROCESS_MAX_LEVELS]");
     if ((uintptr_t)stats_dev & 7) return fail(h, DFK_ERR_INVALID_ARG, w + "stats_dev must be 8-byte aligned");
     const int L = num_levels;
-    // [item descriptors n | level descriptors L x n (level-major)], 16-byte parts
-    const size_t b_items = (sizeof(PpItemDev) * (size_t)n + 15) & ~(size_t)15;
-    h->pp_host.assign(b_items + sizeof(PyrLevelDev) * (size_t)L * n, 0);
-    PpItemDev* pp = reinterpret_cast<PpItemDev*>(h->pp_host.data());
-    PyrLevelDev* lv = reinterpret_cast<PyrLevelDev*>(h->pp_host.data() + b_items);
+    // [item descriptors n | level descriptors L x n (level-major)]
+    Staging up(h->staging);
+    const Part<PpItemDev> pp_at = up.add<PpItemDev>(n);
+    const Part<PyrLevelDev> lv_at = up.add<PyrLevelDev>((size_t)L * n);
     std::vector<int> max_w((size_t)L, 0), max_h((size_t)L, 0);
     long long partials = 0;
     int max_tiles = 0;
@@ -1026,7 +1018,7 @@ DfkStatus dfk_preprocess_batch(DfkHandle h, const DfkPreprocessItem* items, int 
           return fail(h, DFK_ERR_INVALID_ARG, w + "level view is not the halved size or not a float view" + atl);
         if (it.grads && !img_ok(&it.grads[l], lw, lh, 2))
           return fail(h, DFK_ERR_INVALID_ARG, w + "gradient view does not match its level" + atl);
-        PyrLevelDev& d = lv[(size_t)l * n + i];
+        PyrLevelDev& d = lv_at.at(up.host())[(size_t)l * n + i];
         d.img = static_cast<float*>(it.levels[l].ptr);
         d.pitch = (uint32_t)(it.levels[l].pitch_bytes / 4);
         d.w = (int)lw;
@@ -1037,7 +1029,7 @@ DfkStatus dfk_preprocess_batch(DfkHandle h, const DfkPreprocessItem* items, int 
         max_h[l] = std::max(max_h[l], (int)lh);
       }
       any_grad = any_grad || (L > 0 && it.grads);
-      PpItemDev& d = pp[i];
+      PpItemDev& d = pp_at.at(up.host())[i];
       dfk_pm_map_init(&d.map, it.src_cam.fx, it.src_cam.fy, it.src_cam.u0, it.src_cam.v0, it.out_cam.fx,
                       it.out_cam.fy, it.out_cam.u0, it.out_cam.v0);
       d.src = static_cast<const uint8_t*>(s.ptr);
@@ -1064,16 +1056,13 @@ DfkStatus dfk_preprocess_batch(DfkHandle h, const DfkPreprocessItem* items, int 
     if (partials > INT32_MAX)
       return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 tiles of normalising items in one call");
     DeviceGuard guard(h->device);
-    DFK_CUDA(h, h->pp_dev.ensure(h->pp_host.size()), "[PreprocessImage batch] scratch allocation failed");
     // [tile partials 2 each | moments 2 per item]
     DFK_CUDA(h, h->pp_partials.ensure(2 * (size_t)partials + 2 * (size_t)n),
              "[PreprocessImage batch] scratch allocation failed");
-    for (int i = 0; i < n; ++i) pp[i].moments = h->pp_partials.ptr + 2 * (size_t)partials + 2 * (size_t)i;
-    DFK_CUDA(h, cudaMemcpyAsync(h->pp_dev.ptr, h->pp_host.data(), h->pp_host.size(), cudaMemcpyHostToDevice, h->stream),
-             "[PreprocessImage batch] upload failed");
-    const PyrLevelDev* lv_dev = reinterpret_cast<const PyrLevelDev*>(h->pp_dev.ptr + b_items);
-    DFK_CUDA(h, launch_preprocess(reinterpret_cast<const PpItemDev*>(h->pp_dev.ptr), n, max_tiles, any_norm,
-                                  h->pp_partials.ptr, h->stream),
+    for (int i = 0; i < n; ++i) pp_at.at(up.host())[i].moments = h->pp_partials.ptr + 2 * ((size_t)partials + i);
+    DFK_TRY(up.upload(h, h->pp_dev, w));
+    const PyrLevelDev* lv_dev = lv_at.at(up.dev);
+    DFK_CUDA(h, launch_preprocess(pp_at.at(up.dev), n, max_tiles, any_norm, h->pp_partials.ptr, h->stream),
              "[PreprocessImage batch] kernel launch failed");
     h->launches += any_norm ? 3 : 1;
     for (int l = 1; l < L; ++l) {
@@ -1171,40 +1160,34 @@ DfkStatus dfk_keyframe_mesh_batch(DfkHandle h, const DfkKeyframeMeshItem* items,
     if (vrows > INT32_MAX || trows > INT32_MAX)
       return fail(h, DFK_ERR_INVALID_ARG, w + "capacity: more than 2^31 - 1 vertex or triangle rows in one call");
     DeviceGuard guard(h->device);
-    // scratch [segment masks (uint3) | segment bases (int2) | decoded depths (float)], 16-byte parts
-    auto part = [](size_t b) { return (b + 15) & ~(size_t)15; };
-    const size_t b_masks = part(sizeof(uint3) * (size_t)segs), b_bases = part(sizeof(int2) * (size_t)segs);
-    DFK_CUDA(h, h->mesh_scratch.ensure(b_masks + b_bases + sizeof(float) * (size_t)dec_px),
-             "[KeyframeMesh batch] scratch allocation failed");
-    uint3* masks = reinterpret_cast<uint3*>(h->mesh_scratch.ptr);
-    int2* bases = reinterpret_cast<int2*>(h->mesh_scratch.ptr + b_masks);
-    float* decoded = reinterpret_cast<float*>(h->mesh_scratch.ptr + b_masks + b_bases);
-    // descriptors [items | decode descriptors | codes], 16-byte parts, one upload
-    const size_t b_items = part(sizeof(MeshItemDev) * (size_t)n);
-    const size_t b_descs = part(sizeof(DepthDecodeDesc) * (size_t)decodes);
-    const size_t total = b_items + b_descs + sizeof(float) * (size_t)decodes * (size_t)std::max(code_size, 0);
-    DFK_CUDA(h, h->mesh_dev.ensure(total), "[KeyframeMesh batch] scratch allocation failed");
-    h->mesh_host.assign(total, 0);
-    MeshItemDev* md = reinterpret_cast<MeshItemDev*>(h->mesh_host.data());
-    DepthDecodeDesc* dd = reinterpret_cast<DepthDecodeDesc*>(h->mesh_host.data() + b_items);
-    float* codes = reinterpret_cast<float*>(h->mesh_host.data() + b_items + b_descs);
-    const float* codes_dev = reinterpret_cast<const float*>(h->mesh_dev.ptr + b_items + b_descs);
+    // scratch [segment masks | segment bases | decoded depths]
+    Layout S;
+    const Part<uint3> masks_at = S.add<uint3>((size_t)segs);
+    const Part<int2> bases_at = S.add<int2>((size_t)segs);
+    const Part<float> decoded_at = S.add<float>((size_t)dec_px);
+    DFK_CUDA(h, h->mesh_scratch.ensure(S.bytes), "[KeyframeMesh batch] scratch allocation failed");
+    // descriptors [items | decode descriptors | codes], one upload
+    Staging s(h->staging);
+    const Part<MeshItemDev> items_at = s.add<MeshItemDev>(n);
+    const Part<DepthDecodeDesc> descs_at = s.add<DepthDecodeDesc>(decodes);
+    const Part<float> codes_at = s.add<float>((size_t)decodes * (size_t)std::max(code_size, 0));
+    DFK_TRY(s.grow(h, h->mesh_dev, w));
     int dec = 0, max_blocks = 1;
     long long v_begin = 0, t_begin = 0;
     for (int i = 0; i < n; ++i) {
       const DfkKeyframeMeshItem& it = items[i];
-      MeshItemDev& d = md[i];
+      MeshItemDev& d = items_at.at(s.host())[i];
       d.w = (int)it.cam.width;
       d.h = (int)it.cam.height;
       if (it.dpt.ptr) {
         d.dpt = view_of(&it.dpt);
       } else {
-        float* out = decoded + dec_at[(size_t)i];
+        float* out = decoded_at.at(h->mesh_scratch.ptr) + dec_at[(size_t)i];
         DfkDepthDecodeItem di{it.prx_orig, it.prx_jac, DfkImage{out, sizeof(float) * (size_t)d.w, (uint32_t)d.w,
                                                                  (uint32_t)d.h}, it.code};
-        set_depth_decode_desc(dd[dec], di, code_size, codes_dev + (size_t)dec * code_size, out, (uint32_t)d.w,
-                              &max_blocks);
-        memcpy(codes + (size_t)dec * code_size, it.code, sizeof(float) * code_size);
+        set_depth_decode_desc(descs_at.at(s.host())[dec], di, code_size, codes_at.at(s.dev) + (size_t)dec * code_size,
+                              out, (uint32_t)d.w, &max_blocks);
+        memcpy(codes_at.at(s.host()) + (size_t)dec * code_size, it.code, sizeof(float) * code_size);
         dec += 1;
         d.dpt = View{out, (uint32_t)d.w};
       }
@@ -1227,11 +1210,10 @@ DfkStatus dfk_keyframe_mesh_batch(DfkHandle h, const DfkKeyframeMeshItem* items,
       v_begin += it.vertex_capacity;
       t_begin += it.triangle_capacity;
     }
-    DFK_CUDA(h, cudaMemcpyAsync(h->mesh_dev.ptr, h->mesh_host.data(), total, cudaMemcpyHostToDevice, h->stream),
-             "[KeyframeMesh batch] upload failed");
+    DFK_TRY(s.upload(h, h->mesh_dev, w));
     if (decodes > 0) {
-      DFK_CUDA(h, launch_update_depth_batch(code_size, reinterpret_cast<const DepthDecodeDesc*>(h->mesh_dev.ptr + b_items),
-                                            decodes, max_blocks, h->params.sfmparams.avg_dpt, h->stream),
+      DFK_CUDA(h, launch_update_depth_batch(code_size, descs_at.at(s.dev), decodes, max_blocks,
+                                            h->params.sfmparams.avg_dpt, h->stream),
                "[KeyframeMesh batch] depth decode launch failed");
       h->launches += 1;
     }
@@ -1241,8 +1223,8 @@ DfkStatus dfk_keyframe_mesh_batch(DfkHandle h, const DfkKeyframeMeshItem* items,
     p.crop = prm.crop_pix;
     p.draw_noisy = prm.draw_noisy_pixels;
     const MeshOutDev o{positions_dev, normals_dev, colors_dev, pixels_dev, triangles_dev, counts_dev};
-    DFK_CUDA(h, launch_keyframe_mesh(reinterpret_cast<const MeshItemDev*>(h->mesh_dev.ptr), n, max_tiles, p, o, masks,
-                                     bases, h->stream),
+    DFK_CUDA(h, launch_keyframe_mesh(items_at.at(s.dev), n, max_tiles, p, o, masks_at.at(h->mesh_scratch.ptr),
+                                     bases_at.at(h->mesh_scratch.ptr), h->stream),
              "[KeyframeMesh batch] kernel launch failed");
     h->launches += 3;
     return DFK_OK;
@@ -1445,13 +1427,12 @@ DfkStatus depth_prior_batch(DfkHandle h, const char* what, const DfkDepthPriorIt
 {
   if (!out_dev) return fail(h, DFK_ERR_INVALID_ARG, std::string(what) + "null argument");
   DeviceGuard guard(h->device);
-  int max_parts = 1, rows = 0;
-  DFK_TRY(stage_depth_prior(h, what, items, n, code_size, true, h->depth_prior_host, h->depth_prior_dev, &max_parts,
-                            &rows));
-  DFK_CUDA(h, h->depth_prior_partials.ensure((size_t)rows * depth_prior_partial_floats(code_size, gram)),
+  DepthPriorStaged st;
+  DFK_TRY(stage_depth_prior(h, what, items, n, code_size, true, h->staging, h->depth_prior_dev, &st));
+  DFK_CUDA(h, h->depth_prior_partials.ensure((size_t)st.rows * depth_prior_partial_floats(code_size, gram)),
            (std::string(what) + "scratch allocation failed").c_str());
-  DFK_CUDA(h, launch_depth_prior_batch(code_size, reinterpret_cast<const DepthPriorDesc*>(h->depth_prior_dev.ptr), n,
-                                       max_parts, h->params.sfmparams.avg_dpt, h->depth_prior_partials.ptr, out_dev, gram,
+  DFK_CUDA(h, launch_depth_prior_batch(code_size, st.descs.at(h->depth_prior_dev.ptr), n, st.max_parts,
+                                       h->params.sfmparams.avg_dpt, h->depth_prior_partials.ptr, out_dev, gram,
                                        h->stream),
            (std::string(what) + "kernel launch failed").c_str());
   h->launches += 2;

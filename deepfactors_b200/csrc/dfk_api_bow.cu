@@ -70,14 +70,6 @@ BowDbDev db_view(const DfkBowDatabase* db)
   return BowDbDev{db->words.ptr, db->values.ptr, db->offsets.ptr, db->counts.ptr, db->size};
 }
 
-// [n descriptors of T], 16-byte parts, into bow_host
-template <typename T>
-T* host_items(DfkHandle h, int n)
-{
-  h->bow_host.assign(sizeof(T) * (size_t)n, 0);
-  return reinterpret_cast<T*>(h->bow_host.data());
-}
-
 }  // namespace
 
 extern "C" {
@@ -172,36 +164,33 @@ DfkStatus dfk_bow_vocabulary_create(DfkHandle h, const DfkBowVocabularyDesc* d, 
     if (nchild[0] == 0) return fail(h, DFK_ERR_INVALID_ARG, w + "the root has no children");
     // the re-indexed tree
     const size_t rows = (size_t)N + 1;
-    auto part = [](size_t b) { return (b + 15) & ~(size_t)15; };
-    const size_t b_desc = part(rows * D), b_child = part(rows * sizeof(int2)), b_word = part(rows * sizeof(int32_t));
-    const size_t b_ww = part((size_t)W * sizeof(double));
-    std::vector<unsigned char> host(b_desc + b_child + b_word + b_ww, 0);
-    int2* child = reinterpret_cast<int2*>(host.data() + b_desc);
-    int32_t* word = reinterpret_cast<int32_t*>(host.data() + b_desc + b_child);
-    double* ww = reinterpret_cast<double*>(host.data() + b_desc + b_child + b_word);
+    std::vector<unsigned char> host;  // of its own: a tree blob is large, and made once per vocabulary
+    Staging s(host);
+    const Part<uint4> desc_at = s.add<uint4>(rows * D / 16);
+    const Part<int2> child_at = s.add<int2>(rows);
+    const Part<int32_t> word_at = s.add<int32_t>(rows);
+    const Part<double> ww_at = s.add<double>(W);
     for (size_t r = 0; r < rows; ++r) {
       const int id = order[r];
-      if (id > 0) memcpy(host.data() + r * D, d->descriptors + (size_t)at[(size_t)id] * D, (size_t)D);
+      if (id > 0) memcpy(desc_at.at(s.host()) + r * (D / 16), d->descriptors + (size_t)at[(size_t)id] * D, (size_t)D);
       const int nc = nchild[(size_t)id];
-      child[r] = make_int2(nc ? row[(size_t)kids[(size_t)first[(size_t)id]]] : 0, nc);
-      word[r] = id > 0 ? word_of[(size_t)id] : -1;
+      child_at.at(s.host())[r] = make_int2(nc ? row[(size_t)kids[(size_t)first[(size_t)id]]] : 0, nc);
+      word_at.at(s.host())[r] = id > 0 ? word_of[(size_t)id] : -1;
     }
-    for (int j = 0; j < W; ++j) ww[d->word_ids[j]] = d->weights[at[(size_t)d->word_nodes[j]]];
+    for (int j = 0; j < W; ++j) ww_at.at(s.host())[d->word_ids[j]] = d->weights[at[(size_t)d->word_nodes[j]]];
     DfkBowVocabulary* v = new DfkBowVocabulary;
     v->device = h->device;
     v->descriptor_bytes = D;
     v->num_words = W;
     DeviceGuard guard(h->device);
-    cudaError_t e = v->mem.ensure(host.size());
-    if (e == cudaSuccess) e = cudaMemcpy(v->mem.ptr, host.data(), host.size(), cudaMemcpyHostToDevice);
+    cudaError_t e = v->mem.ensure(s.bytes);
+    if (e == cudaSuccess) e = cudaMemcpy(v->mem.ptr, s.host(), s.bytes, cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {
       delete v;
       return cuda_fail(h, e, "[BowVocabulary] upload failed");
     }
     unsigned char* p = v->mem.ptr;
-    v->dev = BowVocDev{reinterpret_cast<const uint4*>(p), reinterpret_cast<const int2*>(p + b_desc),
-                       reinterpret_cast<const int32_t*>(p + b_desc + b_child),
-                       reinterpret_cast<const double*>(p + b_desc + b_child + b_word), D / 16};
+    v->dev = BowVocDev{desc_at.at(p), child_at.at(p), word_at.at(p), ww_at.at(p), D / 16};
     *out = v;
     return DFK_OK;
   });
@@ -229,7 +218,8 @@ DfkStatus dfk_bow_transform_batch(DfkHandle h, const DfkBowVocabulary* voc, cons
     if (!words_dev || !values_dev || !counts_dev || !aligned(words_dev, 4) || !aligned(values_dev, 8) ||
         !aligned(counts_dev, 4) || !aligned(feature_words_dev, 4))
       return fail(h, DFK_ERR_INVALID_ARG, w + "null or misaligned output");
-    BowItemDev* it = host_items<BowItemDev>(h, n);
+    Staging s(h->staging);
+    const Part<BowItemDev> items_at = s.add<BowItemDev>(n);
     long long rows = 0;
     int max_num = 0;
     for (int i = 0; i < n; ++i) {
@@ -242,7 +232,7 @@ DfkStatus dfk_bow_transform_batch(DfkHandle h, const DfkBowVocabulary* voc, cons
       if (f.num > 0 && (!f.descriptors || !aligned(f.descriptors, 16)))
         return fail(h, DFK_ERR_INVALID_ARG, w + "descriptors null or not 16-byte aligned" + at);
       if (capacities[i] < f.num) return fail(h, DFK_ERR_INVALID_ARG, w + "capacity < num" + at);
-      it[i] = BowItemDev{f.descriptors, f.num, (int)std::min(rows, (long long)INT32_MAX)};
+      items_at.at(s.host())[i] = BowItemDev{f.descriptors, f.num, (int)std::min(rows, (long long)INT32_MAX)};
       rows += capacities[i];
       max_num = std::max(max_num, f.num);
     }
@@ -253,11 +243,8 @@ DfkStatus dfk_bow_transform_batch(DfkHandle h, const DfkBowVocabulary* voc, cons
       DFK_CUDA(h, h->bow_words.ensure(std::max<size_t>((size_t)rows, 1)), "[BowVocabulary::transform batch] scratch allocation failed");
       fw = h->bow_words.ptr;
     }
-    DFK_CUDA(h, h->bow_dev.ensure(h->bow_host.size()), "[BowVocabulary::transform batch] scratch allocation failed");
-    DFK_CUDA(h, cudaMemcpyAsync(h->bow_dev.ptr, h->bow_host.data(), h->bow_host.size(), cudaMemcpyHostToDevice,
-                                h->stream),
-             "[BowVocabulary::transform batch] upload failed");
-    DFK_CUDA(h, launch_bow_transform(voc->dev, reinterpret_cast<const BowItemDev*>(h->bow_dev.ptr), n, max_num, fw,
+    DFK_TRY(s.upload(h, h->bow_dev, w));
+    DFK_CUDA(h, launch_bow_transform(voc->dev, items_at.at(s.dev), n, max_num, fw,
                                      words_dev, values_dev, counts_dev, h->stream),
              "[BowVocabulary::transform batch] kernel launch failed");
     h->launches += max_num > 0 ? 2 : 1;
@@ -314,14 +301,15 @@ DfkStatus dfk_bow_database_add(DfkHandle h, DfkBowDatabase* db, const DfkBowVect
     if (!db || !vectors || n < 1 || n > 65535)
       return fail(h, DFK_ERR_INVALID_ARG, w + "null argument / number of vectors not in [1, 65535]");
     if ((long long)db->size + n > INT32_MAX) return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 entries");
-    BowAddDev* a = host_items<BowAddDev>(h, n);
+    Staging s(h->staging);
+    const Part<BowAddDev> adds_at = s.add<BowAddDev>(n);
     long long used = db->used;
     for (int i = 0; i < n; ++i) {
       const DfkBowVector& v = vectors[i];
       if (!vector_ok(v))
         return fail(h, DFK_ERR_INVALID_ARG, w + "vector " + std::to_string(i) +
                                                 ": null or misaligned words, values or count, or capacity < 0");
-      a[i] = BowAddDev{v.words, v.values, v.count, v.capacity, db->size + i, used};
+      adds_at.at(s.host())[i] = BowAddDev{v.words, v.values, v.count, v.capacity, db->size + i, used};
       used += v.capacity;
     }
     DeviceGuard guard(h->device);
@@ -330,12 +318,9 @@ DfkStatus dfk_bow_database_add(DfkHandle h, DfkBowDatabase* db, const DfkBowVect
     DFK_CUDA(h, grow_keep(db->values, std::max<long long>(used, 1), db->used, h->stream), "[BowDatabase::add] storage allocation failed");
     DFK_CUDA(h, grow_keep(db->offsets, E, db->size, h->stream), "[BowDatabase::add] storage allocation failed");
     DFK_CUDA(h, grow_keep(db->counts, E, db->size, h->stream), "[BowDatabase::add] storage allocation failed");
-    DFK_CUDA(h, h->bow_dev.ensure(h->bow_host.size()), "[BowDatabase::add] scratch allocation failed");
-    DFK_CUDA(h, cudaMemcpyAsync(h->bow_dev.ptr, h->bow_host.data(), h->bow_host.size(), cudaMemcpyHostToDevice,
-                                h->stream),
-             "[BowDatabase::add] upload failed");
-    DFK_CUDA(h, launch_bow_add(reinterpret_cast<const BowAddDev*>(h->bow_dev.ptr), n, db->words.ptr, db->values.ptr,
-                               db->offsets.ptr, db->counts.ptr, h->stream),
+    DFK_TRY(s.upload(h, h->bow_dev, w));
+    DFK_CUDA(h, launch_bow_add(adds_at.at(s.dev), n, db->words.ptr, db->values.ptr, db->offsets.ptr, db->counts.ptr,
+                               h->stream),
              "[BowDatabase::add] kernel launch failed");
     h->launches += 1;
     if (first_entry) *first_entry = db->size;
@@ -360,7 +345,8 @@ DfkStatus dfk_bow_database_query_batch(DfkHandle h, const DfkBowDatabase* db, co
     // the ranks compare every hit with every other: n x size^2 comparisons, about 0.35 s at the bound on an H100
     if ((double)n * db->size * db->size > (double)(1LL << 36))
       return fail(h, DFK_ERR_INVALID_ARG, w + "queries x entries^2 > 2^36 (the ranking's comparisons)");
-    BowQueryDev* q = host_items<BowQueryDev>(h, n);
+    Staging s(h->staging);
+    const Part<BowQueryDev> queries_at = s.add<BowQueryDev>(n);
     long long rows = 0;
     int max_cap = 1;
     for (int i = 0; i < n; ++i) {
@@ -371,8 +357,8 @@ DfkStatus dfk_bow_database_query_batch(DfkHandle h, const DfkBowDatabase* db, co
         return fail(h, DFK_ERR_INVALID_ARG, w + "vector capacity > DFK_MATCH_MAX_QUERIES" + at);
       if (x.max_results < 1) return fail(h, DFK_ERR_INVALID_ARG, w + "max_results < 1" + at);
       if (x.max_id < -1) return fail(h, DFK_ERR_INVALID_ARG, w + "max_id < -1" + at);
-      q[i] = BowQueryDev{x.vector.words, x.vector.values, x.vector.count, x.vector.capacity, x.max_results, x.max_id,
-                         (int)std::min(rows, (long long)INT32_MAX)};
+      queries_at.at(s.host())[i] = BowQueryDev{x.vector.words, x.vector.values, x.vector.count, x.vector.capacity,
+                                               x.max_results, x.max_id, (int)std::min(rows, (long long)INT32_MAX)};
       rows += x.max_results;
       max_cap = std::max(max_cap, x.vector.capacity);
     }
@@ -382,15 +368,14 @@ DfkStatus dfk_bow_database_query_batch(DfkHandle h, const DfkBowDatabase* db, co
       DFK_CUDA(h, cudaMemsetAsync(counts_dev, 0, sizeof(int32_t) * (size_t)n, h->stream), "[BowDatabase::query batch] memset failed");
       return DFK_OK;
     }
-    const size_t cells = (size_t)n * db->size, b_sums = (sizeof(double) * cells + 15) & ~(size_t)15;
-    DFK_CUDA(h, h->bow_scratch.ensure(b_sums + cells), "[BowDatabase::query batch] scratch allocation failed");
-    DFK_CUDA(h, h->bow_dev.ensure(h->bow_host.size()), "[BowDatabase::query batch] scratch allocation failed");
-    DFK_CUDA(h, cudaMemcpyAsync(h->bow_dev.ptr, h->bow_host.data(), h->bow_host.size(), cudaMemcpyHostToDevice,
-                                h->stream),
-             "[BowDatabase::query batch] upload failed");
-    DFK_CUDA(h, launch_bow_query(db_view(db), reinterpret_cast<const BowQueryDev*>(h->bow_dev.ptr), n, max_cap,
-                                 reinterpret_cast<double*>(h->bow_scratch.ptr), h->bow_scratch.ptr + b_sums, ids_dev,
-                                 scores_dev, counts_dev, h->stream),
+    const size_t cells = (size_t)n * db->size;
+    Layout S;
+    const Part<double> sums_at = S.add<double>(cells);
+    const Part<unsigned char> hits_at = S.add<unsigned char>(cells);
+    DFK_CUDA(h, h->bow_scratch.ensure(S.bytes), "[BowDatabase::query batch] scratch allocation failed");
+    DFK_TRY(s.upload(h, h->bow_dev, w));
+    DFK_CUDA(h, launch_bow_query(db_view(db), queries_at.at(s.dev), n, max_cap, sums_at.at(h->bow_scratch.ptr),
+                                 hits_at.at(h->bow_scratch.ptr), ids_dev, scores_dev, counts_dev, h->stream),
              "[BowDatabase::query batch] kernel launch failed");
     h->launches += 2;
     return DFK_OK;
@@ -405,21 +390,18 @@ DfkStatus dfk_bow_score_batch(DfkHandle h, const DfkBowDatabase* db, const DfkBo
     if (!db || !items || n < 1 || n > 65535)
       return fail(h, DFK_ERR_INVALID_ARG, w + "null argument / number of items not in [1, 65535]");
     if (!scores_dev || !aligned(scores_dev, 8)) return fail(h, DFK_ERR_INVALID_ARG, w + "null or misaligned output");
-    BowScoreDev* s = host_items<BowScoreDev>(h, n);
+    Staging s(h->staging);
+    const Part<BowScoreDev> descs = s.add<BowScoreDev>(n);
     for (int i = 0; i < n; ++i) {
       const DfkBowScoreItem& x = items[i];
       const std::string at = " in item " + std::to_string(i);
       if (x.entry < 0 || x.entry >= db->size) return fail(h, DFK_ERR_INVALID_ARG, w + "entry not in [0, size)" + at);
       if (!vector_ok(x.vector)) return fail(h, DFK_ERR_INVALID_ARG, w + "null or misaligned vector" + at);
-      s[i] = BowScoreDev{x.vector.words, x.vector.values, x.vector.count, x.vector.capacity, x.entry};
+      descs.at(s.host())[i] = BowScoreDev{x.vector.words, x.vector.values, x.vector.count, x.vector.capacity, x.entry};
     }
     DeviceGuard guard(h->device);
-    DFK_CUDA(h, h->bow_dev.ensure(h->bow_host.size()), "[BowVocabulary::score batch] scratch allocation failed");
-    DFK_CUDA(h, cudaMemcpyAsync(h->bow_dev.ptr, h->bow_host.data(), h->bow_host.size(), cudaMemcpyHostToDevice,
-                                h->stream),
-             "[BowVocabulary::score batch] upload failed");
-    DFK_CUDA(h, launch_bow_score(db_view(db), reinterpret_cast<const BowScoreDev*>(h->bow_dev.ptr), n, scores_dev,
-                                 h->stream),
+    DFK_TRY(s.upload(h, h->bow_dev, w));
+    DFK_CUDA(h, launch_bow_score(db_view(db), descs.at(s.dev), n, scores_dev, h->stream),
              "[BowVocabulary::score batch] kernel launch failed");
     h->launches += 1;
     return DFK_OK;

@@ -62,7 +62,7 @@ DfkStatus dfk_reprojection_linearize_batch(DfkHandle h, const DfkReprojectionIte
       return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::linearize batch] null argument / empty batch");
     DeviceGuard guard(h->device);
     Staged st;
-    DFK_TRY(stage(h, "[ReprojectionFactor::linearize batch] ", true, items, n, code_size, 0, h->rep_host, h->rep_dev, &st));
+    DFK_TRY(stage(h, "[ReprojectionFactor::linearize batch] ", true, items, n, code_size, 0, h->staging, h->rep_dev, &st));
     const float2* query_dev = reinterpret_cast<const float2*>(st.payload);
     DFK_CUDA(h, launch_reprojection_records(code_size, reinterpret_cast<const ReprojItemDev*>(h->rep_dev.ptr), n,
                                             query_dev, query_dev + st.total, h->params.sfmparams.avg_dpt, records_dev,
@@ -75,15 +75,17 @@ DfkStatus dfk_reprojection_linearize_batch(DfkHandle h, const DfkReprojectionIte
 
 namespace {
 
-// Validates and stages the items of a matching batch; max_n0 / total / hyp_total / max_iterations describe the batch.
-// ransac: the camera and RANSAC parameters are checked too.
-DfkStatus stage_match(DfkHandle h, const char* what, const DfkMatchItem* items, int n, bool ransac, int* max_n0,
-                      int* max_iterations, size_t* hyp_total)
+// Validates and stages the items of a matching batch (*items_dev); max_n0 / queries / hyp_total / max_iterations
+// describe the batch.  ransac: the camera and RANSAC parameters are checked too.
+DfkStatus stage_match(DfkHandle h, const char* what, const DfkMatchItem* items, int n, bool ransac,
+                      const MatchItemDev** items_dev, int* max_n0, int* max_iterations, size_t* queries,
+                      size_t* hyp_total)
 {
   const std::string w(what);
   if (!items || n < 1 || n > 65535)  // blockIdx.y of the kernels is the item
     return fail(h, DFK_ERR_INVALID_ARG, w + "null argument / number of items not in [1, 65535]");
-  h->match_host.resize((size_t)n);
+  Staging s(h->staging);
+  const Part<MatchItemDev> descs = s.add<MatchItemDev>(n);
   long long total = 0;
   *max_n0 = 0;
   *max_iterations = 0;
@@ -116,8 +118,7 @@ DfkStatus stage_match(DfkHandle h, const char* what, const DfkMatchItem* items, 
         return fail(h, DFK_ERR_INVALID_ARG, w + "threshold must be finite and > 0, probability in (0, 1), max_dist >= 0" +
                                                 at);
     }
-    MatchItemDev& d = h->match_host[(size_t)i];
-    d = MatchItemDev{};
+    MatchItemDev& d = descs.at(s.host())[i];
     d.kp0 = it.query.keypoints;
     d.kp1 = it.train.keypoints;
     d.d0 = it.query.descriptors;
@@ -142,10 +143,9 @@ DfkStatus stage_match(DfkHandle h, const char* what, const DfkMatchItem* items, 
   }
   if (total > INT32_MAX || *hyp_total > (size_t)INT32_MAX)
     return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 queries or hypotheses in one call");
-  DFK_CUDA(h, h->match_items.ensure((size_t)n), (w + "scratch allocation failed").c_str());
-  DFK_CUDA(h, cudaMemcpyAsync(h->match_items.ptr, h->match_host.data(), sizeof(MatchItemDev) * (size_t)n,
-                              cudaMemcpyHostToDevice, h->stream),
-           (w + "upload failed").c_str());
+  *queries = (size_t)total;
+  DFK_TRY(s.upload(h, h->match_items, w));
+  *items_dev = descs.at(s.dev);
   return DFK_OK;
 }
 
@@ -157,10 +157,11 @@ DfkStatus dfk_hamming_match_batch(DfkHandle h, const DfkMatchItem* items, int n,
     const char* what = "[BFMatcher::match batch] ";
     if (!matches_dev) return fail(h, DFK_ERR_INVALID_ARG, std::string(what) + "null output");
     DeviceGuard guard(h->device);
+    const MatchItemDev* items_dev = nullptr;
     int max_n0 = 0, max_it = 0;
-    size_t hyp = 0;
-    DFK_TRY(stage_match(h, what, items, n, false, &max_n0, &max_it, &hyp));
-    DFK_CUDA(h, launch_hamming_match(h->match_items.ptr, n, max_n0, reinterpret_cast<int2*>(matches_dev), h->stream),
+    size_t total = 0, hyp = 0;
+    DFK_TRY(stage_match(h, what, items, n, false, &items_dev, &max_n0, &max_it, &total, &hyp));
+    DFK_CUDA(h, launch_hamming_match(items_dev, n, max_n0, reinterpret_cast<int2*>(matches_dev), h->stream),
              "[BFMatcher::match batch] kernel launch failed");
     h->launches += max_n0 > 0 ? 1 : 0;
     return DFK_OK;
@@ -174,20 +175,19 @@ DfkStatus dfk_reprojection_match_batch(DfkHandle h, const DfkMatchItem* items, i
     const char* what = "[ReprojectionFactor matches batch] ";
     if (!matches_dev || !counts_dev) return fail(h, DFK_ERR_INVALID_ARG, std::string(what) + "null output");
     DeviceGuard guard(h->device);
+    const MatchItemDev* items_dev = nullptr;
     int max_n0 = 0, max_it = 0;
-    size_t hyp = 0;
-    DFK_TRY(stage_match(h, what, items, n, true, &max_n0, &max_it, &hyp));
-    size_t total = 0;
-    for (const MatchItemDev& d : h->match_host) total += (size_t)d.n0;
-    // [matches (int2 per query) | counts (int per hypothesis slot) | selections (int3 per item)], 16-byte aligned parts
-    const size_t b_match = (sizeof(int2) * total + 15) & ~(size_t)15;
-    const size_t b_count = (sizeof(int) * hyp + 15) & ~(size_t)15;
-    const size_t b_sel = sizeof(int3) * (size_t)n;
-    DFK_CUDA(h, h->match_scratch.ensure(b_match + b_count + b_sel + 16), "[ReprojectionFactor matches batch] scratch allocation failed");
+    size_t total = 0, hyp = 0;
+    DFK_TRY(stage_match(h, what, items, n, true, &items_dev, &max_n0, &max_it, &total, &hyp));
+    // [matches (int2 per query) | counts (int per hypothesis slot) | selections (int3 per item)]
+    Layout L;
+    const Part<int2> match_at = L.add<int2>(total);
+    const Part<int> count_at = L.add<int>(hyp);
+    const Part<int3> sel_at = L.add<int3>(n);
+    DFK_CUDA(h, h->match_scratch.ensure(L.bytes), "[ReprojectionFactor matches batch] scratch allocation failed");
     unsigned char* base = h->match_scratch.ptr;
-    int3* sel = ransac_dev ? reinterpret_cast<int3*>(ransac_dev) : reinterpret_cast<int3*>(base + b_match + b_count);
-    DFK_CUDA(h, launch_reprojection_match(h->match_items.ptr, n, max_n0, max_it, reinterpret_cast<int2*>(base),
-                                          reinterpret_cast<int*>(base + b_match), sel,
+    int3* sel = ransac_dev ? reinterpret_cast<int3*>(ransac_dev) : sel_at.at(base);
+    DFK_CUDA(h, launch_reprojection_match(items_dev, n, max_n0, max_it, match_at.at(base), count_at.at(base), sel,
                                           reinterpret_cast<int3*>(matches_dev), counts_dev, h->stream),
              "[ReprojectionFactor matches batch] kernel launch failed");
     h->launches += 4;
@@ -237,29 +237,25 @@ struct OrbPlan {
   }
   bool too_big() const { return rows > INT32_MAX || corners > INT32_MAX || segs > INT32_MAX; }
 
-  // one allocation for n items: [hist | stats | segments | corner positions | keys | angles | row map | score maps |
-  // blurred images], 16-byte parts
-  static size_t part(size_t bytes) { return (bytes + 15) & ~(size_t)15; }
-  size_t bytes(int n) const
+  // The detector's scratch for n items, as parts of L: [hist | stats | segments | corner positions | keys | angles |
+  // row map | score maps | blurred images]
+  struct Parts {
+    Part<int> hist, stats, seg;
+    Part<uint32_t> pos, key;
+    Part<float> angle;
+    Part<int> rows;
+    Part<uint8_t> map, blur;
+    OrbScratchDev at(unsigned char* base) const
+    {
+      return OrbScratchDev{map.at(base), seg.at(base), hist.at(base), stats.at(base), pos.at(base), key.at(base),
+                           angle.at(base), rows.at(base), blur.at(base)};
+    }
+  };
+  Parts scratch(Layout& L, int n) const
   {
-    return part(sizeof(int) * 256 * (size_t)n) + part(sizeof(int) * 4 * (size_t)n) + part(sizeof(int) * (size_t)segs) +
-           3 * part(sizeof(uint32_t) * (size_t)corners) + part(sizeof(int) * (size_t)rows) + part((size_t)map) +
-           part((size_t)blur);
-  }
-  OrbScratchDev layout(unsigned char* p, int n) const
-  {
-    const size_t b_c = part(sizeof(uint32_t) * (size_t)corners);
-    OrbScratchDev s;
-    s.hist = reinterpret_cast<int*>(p);
-    s.stats = reinterpret_cast<int*>(p += part(sizeof(int) * 256 * (size_t)n));
-    s.seg = reinterpret_cast<int*>(p += part(sizeof(int) * 4 * (size_t)n));
-    s.pos = reinterpret_cast<uint32_t*>(p += part(sizeof(int) * (size_t)segs));
-    s.key = reinterpret_cast<uint32_t*>(p += b_c);
-    s.angle = reinterpret_cast<float*>(p += b_c);
-    s.rows = reinterpret_cast<int*>(p += b_c);
-    s.map = p += part(sizeof(int) * (size_t)rows);
-    s.blur = p + part((size_t)map);
-    return s;
+    return Parts{L.add<int>(256 * (size_t)n), L.add<int>(4 * (size_t)n), L.add<int>((size_t)segs),
+                   L.add<uint32_t>((size_t)corners), L.add<uint32_t>((size_t)corners), L.add<float>((size_t)corners),
+                   L.add<int>((size_t)rows), L.add<uint8_t>((size_t)map), L.add<uint8_t>((size_t)blur)};
   }
   cudaError_t launch(const OrbItemDev* items_dev, int n, const OrbScratchDev& s, float* keypoints,
                      uint8_t* descriptors, float* angles, float* responses, int* counts, cudaStream_t stream) const
@@ -281,6 +277,16 @@ const char* orb_item_error(const DfkImage& im, int nfeatures, int fast_threshold
   return nullptr;
 }
 
+// The size of level k of a pyramid item, and whether the level is built: at least DFK_OM_MIN_SIZE both ways.  The
+// built levels k >= 1 are the resize items; the call counts them with this before it stages them.
+bool orb_level(const DfkOrbPyramidItem& it, int k, int* lw, int* lh)
+{
+  const float scale = dfk_opm_level_scale(it.scale_factor, k);
+  *lw = k ? dfk_opm_level_size((int)it.image.width, scale) : (int)it.image.width;
+  *lh = k ? dfk_opm_level_size((int)it.image.height, scale) : (int)it.image.height;
+  return *lw >= DFK_OM_MIN_SIZE && *lh >= DFK_OM_MIN_SIZE;
+}
+
 }  // namespace
 
 extern "C" {
@@ -297,13 +303,14 @@ DfkStatus dfk_orb_detect_batch(DfkHandle h, const DfkOrbItem* items, int n, floa
     if (((uintptr_t)keypoints_dev & 3) || ((uintptr_t)descriptors_dev & 15) || ((uintptr_t)angles_dev & 3) ||
         ((uintptr_t)responses_dev & 3) || ((uintptr_t)counts_dev & 3))
       return fail(h, DFK_ERR_INVALID_ARG, w + "descriptors must be 16-byte aligned, the other outputs 4-byte aligned");
-    h->orb_host.resize((size_t)n);
+    Staging st(h->staging);
+    const Part<OrbItemDev> items_at = st.add<OrbItemDev>(n);
     OrbPlan plan;
     for (int i = 0; i < n; ++i) {
       const DfkOrbItem& it = items[i];
       if (const char* e = orb_item_error(it.image, it.nfeatures, it.fast_threshold, it.capacity))
         return fail(h, DFK_ERR_INVALID_ARG, w + e + " in item " + std::to_string(i));
-      OrbItemDev& d = h->orb_host[(size_t)i];
+      OrbItemDev& d = items_at.at(st.host())[i];
       plan.add(d, (int)it.image.width, (int)it.image.height, it.nfeatures, it.fast_threshold, it.capacity);
       d.img = static_cast<const uint8_t*>(it.image.ptr);
       d.pitch = it.image.pitch_bytes;
@@ -311,14 +318,12 @@ DfkStatus dfk_orb_detect_batch(DfkHandle h, const DfkOrbItem* items, int n, floa
     if (plan.too_big())
       return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 output rows or scratch entries in one call");
     DeviceGuard guard(h->device);
-    DFK_CUDA(h, h->orb_items.ensure((size_t)n), "[OrbDetector batch] scratch allocation failed");
-    DFK_CUDA(h, h->orb_scratch.ensure(plan.bytes(n)), "[OrbDetector batch] scratch allocation failed");
-    const OrbScratchDev s = plan.layout(h->orb_scratch.ptr, n);
-    DFK_CUDA(h, cudaMemcpyAsync(h->orb_items.ptr, h->orb_host.data(), sizeof(OrbItemDev) * (size_t)n,
-                                cudaMemcpyHostToDevice, h->stream),
-             "[OrbDetector batch] upload failed");
-    DFK_CUDA(h, plan.launch(h->orb_items.ptr, n, s, keypoints_dev, descriptors_dev, angles_dev, responses_dev,
-                            counts_dev, h->stream),
+    Layout S;
+    const OrbPlan::Parts scratch = plan.scratch(S, n);
+    DFK_CUDA(h, h->orb_scratch.ensure(S.bytes), "[OrbDetector batch] scratch allocation failed");
+    DFK_TRY(st.upload(h, h->orb_items, w));
+    DFK_CUDA(h, plan.launch(items_at.at(st.dev), n, scratch.at(h->orb_scratch.ptr), keypoints_dev, descriptors_dev,
+                            angles_dev, responses_dev, counts_dev, h->stream),
              "[OrbDetector batch] kernel launch failed");
     h->launches += plan.launches();
     return DFK_OK;
@@ -342,6 +347,7 @@ DfkStatus dfk_orb_detect_pyramid_batch(DfkHandle h, const DfkOrbPyramidItem* ite
     // validation, and each item's levels: one one-level item per (image, level), level images for k >= 1 while they
     // are at least 63 x 63 (a smaller level and every level after it has no features)
     long long subs = 0, out_rows = 0;
+    size_t nres = 0;  // levels k >= 1 that are built: the resize items
     for (int i = 0; i < n; ++i) {
       const DfkOrbPyramidItem& it = items[i];
       const std::string at = " in item " + std::to_string(i);
@@ -353,13 +359,18 @@ DfkStatus dfk_orb_detect_pyramid_batch(DfkHandle h, const DfkOrbPyramidItem* ite
         return fail(h, DFK_ERR_INVALID_ARG, w + "nlevels not in [1, DFK_ORB_MAX_LEVELS]" + at);
       subs += it.nlevels;
       out_rows += it.capacity;
+      for (int k = 1, lw, lh; k < it.nlevels; ++k) nres += orb_level(it, k, &lw, &lh);
     }
     if (subs > 65535)  // gridDim.z of the FAST kernel is the (image, level) item
       return fail(h, DFK_ERR_INVALID_ARG, w + "more than 65535 levels over the items of one call");
     if (out_rows > INT32_MAX) return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 output rows in one call");
-    std::vector<OrbItemDev>& sub = h->orb_host;
-    sub.resize((size_t)subs);
-    std::vector<OrbGatherDev> gather((size_t)n);
+    // one upload: [one-level items | gather items | resize items by level]
+    Staging up(h->staging);
+    const Part<OrbItemDev> sub_at = up.add<OrbItemDev>((size_t)subs);
+    const Part<OrbGatherDev> gat_at = up.add<OrbGatherDev>(n);
+    const Part<OrbResizeDev> res_at = up.add<OrbResizeDev>(nres);
+    OrbItemDev* sub = sub_at.at(up.host());
+    OrbGatherDev* gather = gat_at.at(up.host());
     // the resize items by level, their source and destination as offsets into the level images until those are
     // allocated (SIZE_MAX: the caller's image)
     struct LevelJob {
@@ -375,18 +386,16 @@ DfkStatus dfk_orb_detect_pyramid_batch(DfkHandle h, const DfkOrbPyramidItem* ite
       const DfkOrbPyramidItem& it = items[i];
       int budget[DFK_ORB_MAX_LEVELS];
       dfk_opm_budgets(it.nfeatures, it.scale_factor, it.nlevels, budget);
-      OrbGatherDev& g = gather[(size_t)i];
-      g = OrbGatherDev{};
+      OrbGatherDev& g = gather[i];
       g.sub_begin = sb;
       g.nlevels = it.nlevels;
       g.out_begin = i ? gather[(size_t)i - 1].out_begin + items[i - 1].capacity : 0;
       g.capacity = it.capacity;
-      const int W = (int)it.image.width, H = (int)it.image.height;
-      int pw = W, ph = H;
+      int pw = (int)it.image.width, ph = (int)it.image.height;
       for (int k = 0; k < it.nlevels; ++k) {
         g.scale[k] = dfk_opm_level_scale(it.scale_factor, k);
-        const int lw = k ? dfk_opm_level_size(W, g.scale[k]) : W, lh = k ? dfk_opm_level_size(H, g.scale[k]) : H;
-        const bool built = lw >= DFK_OM_MIN_SIZE && lh >= DFK_OM_MIN_SIZE;
+        int lw, lh;
+        const bool built = orb_level(it, k, &lw, &lh);
         if (built && k) {
           const size_t src = sub_level[(size_t)sb + k - 1];
           const size_t src_pitch = src == SIZE_MAX ? it.image.pitch_bytes : (size_t)pw;
@@ -407,35 +416,24 @@ DfkStatus dfk_orb_detect_pyramid_batch(DfkHandle h, const DfkOrbPyramidItem* ite
       return fail(h, DFK_ERR_INVALID_ARG, w + "more than 2^31 - 1 staged rows or scratch entries in one call");
     DeviceGuard guard(h->device);
     // the detector's scratch, then [level images | staged keypoints | descriptors | angles | responses | counts]
-    const size_t srows = (size_t)plan.rows, b_det = plan.bytes((int)subs), b_lev = OrbPlan::part(level_bytes);
-    const size_t b_kp = OrbPlan::part(sizeof(float) * 2 * srows), b_desc = OrbPlan::part(32 * srows);
-    const size_t b_f = OrbPlan::part(sizeof(float) * srows), b_cnt = OrbPlan::part(sizeof(int) * (size_t)subs);
-    DFK_CUDA(h, h->orb_scratch.ensure(b_det + b_lev + b_kp + b_desc + 2 * b_f + b_cnt),
-             "[OrbDetector pyramid batch] scratch allocation failed");
+    const size_t srows = (size_t)plan.rows;
+    Layout S;
+    const OrbPlan::Parts det = plan.scratch(S, (int)subs);
+    const Part<uint8_t> lev_at = S.add<uint8_t>(level_bytes);
+    const Part<float> kp_at = S.add<float>(2 * srows);
+    const Part<uint8_t> desc_at = S.add<uint8_t>(32 * srows);
+    const Part<float> ang_at = S.add<float>(srows), resp_at = S.add<float>(srows);
+    const Part<int> cnt_at = S.add<int>((size_t)subs);
+    DFK_CUDA(h, h->orb_scratch.ensure(S.bytes), "[OrbDetector pyramid batch] scratch allocation failed");
     unsigned char* base = h->orb_scratch.ptr;
-    const OrbScratchDev s = plan.layout(base, (int)subs);
-    unsigned char* levels = base + b_det;
-    float* st_kp = reinterpret_cast<float*>(levels + b_lev);
-    uint8_t* st_desc = reinterpret_cast<uint8_t*>(st_kp) + b_kp;
-    float* st_ang = reinterpret_cast<float*>(st_desc + b_desc);
-    float* st_resp = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(st_ang) + b_f);
-    int* st_cnt = reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(st_resp) + b_f);
+    unsigned char* levels = lev_at.at(base);
     auto level_ptr = [&](size_t off, const void* image) {
       return off == SIZE_MAX ? static_cast<const uint8_t*>(image) : static_cast<const uint8_t*>(levels + off);
     };
-    // one upload: [one-level items | gather items | resize items by level]
-    size_t nres = 0;
-    for (const auto& v : resize) nres += v.size();
-    const size_t b_sub = OrbPlan::part(sizeof(OrbItemDev) * (size_t)subs);
-    const size_t b_gat = OrbPlan::part(sizeof(OrbGatherDev) * (size_t)n);
-    std::vector<unsigned char>& host = h->orb_pyr_host;
-    host.assign(b_sub + b_gat + sizeof(OrbResizeDev) * nres, 0);
     for (int i = 0, sb = 0; i < n; sb += items[i].nlevels, ++i)
       for (int k = 0; k < items[i].nlevels; ++k)
         sub[(size_t)sb + k].img = level_ptr(sub_level[(size_t)sb + k], items[i].image.ptr);
-    memcpy(host.data(), sub.data(), sizeof(OrbItemDev) * (size_t)subs);
-    memcpy(host.data() + b_sub, gather.data(), sizeof(OrbGatherDev) * (size_t)n);
-    OrbResizeDev* rh = reinterpret_cast<OrbResizeDev*>(host.data() + b_sub + b_gat);
+    OrbResizeDev* rh = res_at.at(up.host());
     for (const std::vector<LevelJob>& v : resize)
       for (const LevelJob& job : v) {
         *rh = job.r;
@@ -443,12 +441,7 @@ DfkStatus dfk_orb_detect_pyramid_batch(DfkHandle h, const DfkOrbPyramidItem* ite
         rh->dst = levels + job.dst;
         ++rh;
       }
-    DFK_CUDA(h, h->orb_pyr_dev.ensure(host.size()), "[OrbDetector pyramid batch] scratch allocation failed");
-    DFK_CUDA(h, cudaMemcpyAsync(h->orb_pyr_dev.ptr, host.data(), host.size(), cudaMemcpyHostToDevice, h->stream),
-             "[OrbDetector pyramid batch] upload failed");
-    const OrbItemDev* sub_dev = reinterpret_cast<const OrbItemDev*>(h->orb_pyr_dev.ptr);
-    const OrbGatherDev* gat_dev = reinterpret_cast<const OrbGatherDev*>(h->orb_pyr_dev.ptr + b_sub);
-    const OrbResizeDev* res_dev = reinterpret_cast<const OrbResizeDev*>(h->orb_pyr_dev.ptr + b_sub + b_gat);
+    DFK_TRY(up.upload(h, h->orb_pyr_dev, w));
     // the chain of levels: level k of every image from its level k - 1
     for (int k = 1, j = 0; k < DFK_ORB_MAX_LEVELS; ++k) {
       const std::vector<LevelJob>& v = resize[(size_t)k];
@@ -458,17 +451,18 @@ DfkStatus dfk_orb_detect_pyramid_batch(DfkHandle h, const DfkOrbPyramidItem* ite
         mw = std::max(mw, job.r.dw);
         mh = std::max(mh, job.r.dh);
       }
-      DFK_CUDA(h, launch_orb_resize_level(res_dev + j, (int)v.size(), mw, mh, h->stream),
+      DFK_CUDA(h, launch_orb_resize_level(res_at.at(up.dev) + j, (int)v.size(), mw, mh, h->stream),
                "[OrbDetector pyramid batch] kernel launch failed");
       j += (int)v.size();
       h->launches += 1;
     }
-    DFK_CUDA(h, plan.launch(sub_dev, (int)subs, s, st_kp, st_desc, st_ang, st_resp, st_cnt, h->stream),
+    DFK_CUDA(h, plan.launch(sub_at.at(up.dev), (int)subs, det.at(base), kp_at.at(base), desc_at.at(base),
+                            ang_at.at(base), resp_at.at(base), cnt_at.at(base), h->stream),
              "[OrbDetector pyramid batch] kernel launch failed");
     h->launches += plan.launches();
-    const OrbStagingDev st{st_kp, st_desc, st_ang, st_resp, st_cnt};
-    DFK_CUDA(h, launch_orb_gather(gat_dev, n, sub_dev, st, plan.max_cap, keypoints_dev, descriptors_dev, angles_dev,
-                                  responses_dev, octaves_dev, counts_dev, h->stream),
+    const OrbStagingDev st{kp_at.at(base), desc_at.at(base), ang_at.at(base), resp_at.at(base), cnt_at.at(base)};
+    DFK_CUDA(h, launch_orb_gather(gat_at.at(up.dev), n, sub_at.at(up.dev), st, plan.max_cap, keypoints_dev,
+                                  descriptors_dev, angles_dev, responses_dev, octaves_dev, counts_dev, h->stream),
              "[OrbDetector pyramid batch] kernel launch failed");
     h->launches += 1;
     return DFK_OK;
@@ -519,7 +513,7 @@ DfkStatus dfk_sparse_geometric_linearize_batch(DfkHandle h, const DfkSparseGeome
       return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::linearize batch] null argument / empty batch");
     DeviceGuard guard(h->device);
     Staged st;
-    DFK_TRY(stage(h, "[SparseGeometricFactor::linearize batch] ", true, items, n, code_size, 0, h->geo_host, h->geo_dev,
+    DFK_TRY(stage(h, "[SparseGeometricFactor::linearize batch] ", true, items, n, code_size, 0, h->staging, h->geo_dev,
                   &st));
     DFK_CUDA(h, launch_sparse_geometric_records(code_size, reinterpret_cast<const GeoItemDev*>(h->geo_dev.ptr), n,
                                                 reinterpret_cast<const int2*>(st.payload), h->params.sfmparams.avg_dpt,
@@ -537,7 +531,7 @@ DfkStatus dfk_reprojection_error_batch(DfkHandle h, const DfkReprojectionItem* i
       return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::error batch] null argument / empty batch");
     DeviceGuard guard(h->device);
     Staged st;
-    DFK_TRY(stage(h, "[ReprojectionFactor::error batch] ", true, items, n, code_size, 0, h->rep_host, h->rep_dev, &st));
+    DFK_TRY(stage(h, "[ReprojectionFactor::error batch] ", true, items, n, code_size, 0, h->staging, h->rep_dev, &st));
     const float2* query_dev = reinterpret_cast<const float2*>(st.payload);
     DFK_CUDA(h, launch_reprojection_error(code_size, reinterpret_cast<const ReprojItemDev*>(h->rep_dev.ptr), n, query_dev,
                                           query_dev + st.total, h->params.sfmparams.avg_dpt, out_dev, h->stream),
@@ -555,7 +549,7 @@ DfkStatus dfk_sparse_geometric_error_batch(DfkHandle h, const DfkSparseGeometric
       return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::error batch] null argument / empty batch");
     DeviceGuard guard(h->device);
     Staged st;
-    DFK_TRY(stage(h, "[SparseGeometricFactor::error batch] ", true, items, n, code_size, 0, h->geo_host, h->geo_dev, &st));
+    DFK_TRY(stage(h, "[SparseGeometricFactor::error batch] ", true, items, n, code_size, 0, h->staging, h->geo_dev, &st));
     DFK_CUDA(h, launch_sparse_geometric_error(code_size, reinterpret_cast<const GeoItemDev*>(h->geo_dev.ptr), n,
                                               reinterpret_cast<const int2*>(st.payload), h->params.sfmparams.avg_dpt,
                                               out_dev, h->stream),

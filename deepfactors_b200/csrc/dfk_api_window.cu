@@ -108,8 +108,9 @@ struct DfkWindowProblem {
   // depth priors (dfk_window_problem_set_depth_priors): ndp priors over ndpi (keyframe, level) items, staged once
   // ([descriptors | codes], the codes rewritten from the state before every batch), and the lists
   // [add CSR ptr K + 1 | prior indices ndp | level_ptr ndp + 1 | sigma (float bits) ndp | keyframe of every item ndpi]
-  int ndp = 0, ndpi = 0, dp_max_parts = 1, dp_rows = 0;
-  size_t dp_code_off = 0, dp_lp = 0, dp_sg = 0, dp_kf = 0;
+  int ndp = 0, ndpi = 0;
+  DepthPriorStaged dp_st;
+  size_t dp_lp = 0, dp_sg = 0, dp_kf = 0;
   DeviceBuf<unsigned char> dp;
   std::vector<unsigned char> dp_host;
   DeviceBuf<int> dp_lists;
@@ -182,12 +183,11 @@ WindowReposeDev repose_args(const DfkWindowProblem* p, const double* state)
 DfkStatus problem_depth_priors(DfkHandle h, DfkWindowProblem* p, const double* state, bool gram, const char* what)
 {
   const int* l = p->dp_lists.ptr;
-  float* codes = reinterpret_cast<float*>(p->dp.ptr + p->dp_code_off);
-  DFK_CUDA(h, launch_depth_prior_codes(state + (size_t)(p->K + p->F) * 7, l + p->dp_kf, p->ndpi, p->C, codes, h->stream),
+  DFK_CUDA(h, launch_depth_prior_codes(state + (size_t)(p->K + p->F) * 7, l + p->dp_kf, p->ndpi, p->C,
+                                       p->dp_st.codes.at(p->dp.ptr), h->stream),
            what);
-  DFK_CUDA(h, launch_depth_prior_batch(p->C, reinterpret_cast<const DepthPriorDesc*>(p->dp.ptr), p->ndpi,
-                                       p->dp_max_parts, p->avg_dpt, p->dp_partials.ptr,
-                                       gram ? p->dp_records.ptr : p->dp_err.ptr, gram, h->stream),
+  DFK_CUDA(h, launch_depth_prior_batch(p->C, p->dp_st.descs.at(p->dp.ptr), p->ndpi, p->dp_st.max_parts, p->avg_dpt,
+                                       p->dp_partials.ptr, gram ? p->dp_records.ptr : p->dp_err.ptr, gram, h->stream),
            what);
   h->launches += 3;
   return DFK_OK;
@@ -784,22 +784,21 @@ DfkStatus dfk_window_add_depth_priors(DfkHandle h, const DfkWindow* w, int m, co
         return fail(h, DFK_ERR_INVALID_ARG, pre + " has no records (level_ptr must increase)");
     }
     if (m == 0) return DFK_OK;
-    // [CSR of the priors per keyframe: ptr[K + 1] | indices m] | level_ptr[m + 1] | sigma[m] (float bits)
-    std::vector<int> lists;
-    add_csr(lists, K, m, [&](int i) { return prior_kf_host[i]; });
-    const size_t lp = lists.size();
-    lists.insert(lists.end(), level_ptr_host, level_ptr_host + m + 1);
-    const size_t sg = lists.size();
-    lists.resize(sg + m);
-    memcpy(lists.data() + sg, sigma_host, sizeof(float) * m);
+    // [CSR of the priors per keyframe: ptr[K + 1] | indices m] | level_ptr[m + 1] | sigma[m]
+    std::vector<int> csr;
+    add_csr(csr, K, m, [&](int i) { return prior_kf_host[i]; });
+    Staging s(h->staging);
+    const Part<int> csr_at = s.add<int>(csr.size()), lp_at = s.add<int>(m + 1);
+    const Part<float> sg_at = s.add<float>(m);
+    memcpy(csr_at.at(s.host()), csr.data(), sizeof(int) * csr.size());
+    memcpy(lp_at.at(s.host()), level_ptr_host, sizeof(int) * (m + 1));
+    memcpy(sg_at.at(s.host()), sigma_host, sizeof(float) * m);
     DeviceGuard guard(h->device);
     const char* what = "[Window::AddDepthPriors] index upload failed";
-    DFK_CUDA(h, h->window_lists.ensure(lists.size()), what);
-    DFK_CUDA(h, cudaMemcpyAsync(h->window_lists.ptr, lists.data(), sizeof(int) * lists.size(), cudaMemcpyHostToDevice,
-                                h->stream),
-             what);
-    const int* d = h->window_lists.ptr;
-    DFK_CUDA(h, launch_window_add_depth_priors(w->dev, m, d, d + K + 1, d + lp, reinterpret_cast<const float*>(d + sg),
+    DFK_CUDA(h, h->window_lists.ensure(s.bytes / sizeof(int)), what);
+    DFK_CUDA(h, cudaMemcpyAsync(h->window_lists.ptr, s.host(), s.bytes, cudaMemcpyHostToDevice, h->stream), what);
+    int* d = h->window_lists.ptr;
+    DFK_CUDA(h, launch_window_add_depth_priors(w->dev, m, csr_at.at(d), csr_at.at(d) + K + 1, lp_at.at(d), sg_at.at(d),
                                                records_dev, window_dev, h->stream),
              "[Window::AddDepthPriors] kernel launch failed");
     h->launches += 1;
@@ -1170,18 +1169,16 @@ DfkStatus dfk_window_problem_create(DfkHandle h, const DfkWindowProblemDesc* d, 
     }
     if (ndep > 0) {
       DFK_CUDA(h, p->depth_scratch.ensure(dep_off[ndep]), amsg);
-      const size_t desc_bytes = (sizeof(DepthDecodeDesc) * (size_t)ndep + 15) & ~(size_t)15;
-      const size_t total = desc_bytes + sizeof(float) * (size_t)ndep * C;
-      DFK_CUDA(h, p->depth.ensure(total), amsg);
-      std::vector<unsigned char> hb(total, 0);
-      DepthDecodeDesc* descs = reinterpret_cast<DepthDecodeDesc*>(hb.data());
-      const float* codes_dev = reinterpret_cast<const float*>(p->depth.ptr + desc_bytes);
+      Staging s(h->staging);
+      const Part<DepthDecodeDesc> descs = s.add<DepthDecodeDesc>(ndep);
+      const Part<float> codes = s.add<float>((size_t)ndep * C);
+      DFK_CUDA(h, p->depth.ensure(s.bytes), amsg);
       for (int i = 0; i < ndep; ++i) {
         const DfkDepthDecodeItem& it = d->depth[i];
-        set_depth_decode_desc(descs[i], it, C, codes_dev + (size_t)i * C, p->depth_scratch.ptr + dep_off[i], it.dpt.width,
-                              &p->depth_max_blocks);
+        set_depth_decode_desc(descs.at(s.host())[i], it, C, codes.at(p->depth.ptr) + (size_t)i * C,
+                              p->depth_scratch.ptr + dep_off[i], it.dpt.width, &p->depth_max_blocks);
       }
-      DFK_CUDA(h, cudaMemcpyAsync(p->depth.ptr, hb.data(), total, cudaMemcpyHostToDevice, h->stream),
+      DFK_CUDA(h, cudaMemcpyAsync(p->depth.ptr, s.host(), s.bytes, cudaMemcpyHostToDevice, h->stream),
                "[WindowProblem] upload failed");
     }
     if (ne > 0) {
@@ -1395,8 +1392,8 @@ DfkStatus dfk_window_problem_set_depth_priors(DfkHandle h, DfkWindowProblem* p, 
     }
     const int n = level_ptr[m];
     // the items' views are checked as the batch checks them; their codes come from the state (slot = prior_kf)
-    int max_parts = 1, rows = 0;
-    DFK_TRY(stage_depth_prior(h, what, items, n, p->C, false, p->dp_host, p->dp, &max_parts, &rows));
+    DepthPriorStaged st;
+    DFK_TRY(stage_depth_prior(h, what, items, n, p->C, false, p->dp_host, p->dp, &st));
     std::vector<int> lists;
     add_csr(lists, p->K, m, [&](int i) { return prior_kf[i]; });
     const size_t lp = lists.size();
@@ -1409,7 +1406,7 @@ DfkStatus dfk_window_problem_set_depth_priors(DfkHandle h, DfkWindowProblem* p, 
       for (int l = level_ptr[i]; l < level_ptr[i + 1]; ++l) lists.push_back(prior_kf[i]);
     const char* amsg = "[WindowProblem::set_depth_priors] allocation failed";
     DFK_CUDA(h, p->dp_lists.ensure(lists.size()), amsg);
-    DFK_CUDA(h, p->dp_partials.ensure((size_t)rows * depth_prior_partial_floats(p->C, true)), amsg);
+    DFK_CUDA(h, p->dp_partials.ensure((size_t)st.rows * depth_prior_partial_floats(p->C, true)), amsg);
     DFK_CUDA(h, p->dp_records.ensure((size_t)n * DFK_DEPTH_RECORD_FLOATS(p->C)), amsg);
     DFK_CUDA(h, p->dp_err.ensure((size_t)n * 2), amsg);
     DFK_CUDA(h, cudaMemcpyAsync(p->dp_lists.ptr, lists.data(), sizeof(int) * lists.size(), cudaMemcpyHostToDevice,
@@ -1417,9 +1414,7 @@ DfkStatus dfk_window_problem_set_depth_priors(DfkHandle h, DfkWindowProblem* p, 
              "[WindowProblem::set_depth_priors] upload failed");
     p->ndp = m;
     p->ndpi = n;
-    p->dp_max_parts = max_parts;
-    p->dp_rows = rows;
-    p->dp_code_off = (sizeof(DepthPriorDesc) * (size_t)n + 15) & ~(size_t)15;
+    p->dp_st = st;
     p->dp_lp = lp;
     p->dp_sg = sg;
     p->dp_kf = kf;

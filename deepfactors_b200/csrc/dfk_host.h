@@ -1,5 +1,6 @@
-// dfk_host.h -- host-side pieces that the C ABI's units (dfk_api.cu, dfk_api_sparse.cu, dfk_api_window.cu) share:
-// scratch buffers, the handle, error reporting, argument checks, the dense RunStep planning and the sparse staging.
+// dfk_host.h -- host-side pieces that the C ABI's units (dfk_api.cu, dfk_api_sparse.cu, dfk_api_window.cu,
+// dfk_api_bow.cu) share: scratch buffers, the handle, error reporting, the blob layout and staging of every call's
+// upload (Layout, Staging), argument checks, the dense RunStep planning and the sparse staging.
 // Internal to libdfk.so.
 #pragma once
 
@@ -73,6 +74,10 @@ struct DfkContext {
   DeviceBuf<float> code_dev;             // 256 floats
   DeviceBuf<float> track_dev;            // dfk_se3_track: [pose 8 | per-iteration history 36 each]
   PinnedBuf<float> track_host;           // mirror of track_dev + the last system (32)
+  // The calls' staged blobs (see Staging) are laid out in `staging`, one pageable host buffer for every call:
+  // cudaMemcpyAsync from pageable memory has read it when it returns, so the next call may refill it while the copy is
+  // still queued.  Each call family uploads into a device buffer of its own, below.
+  std::vector<unsigned char> staging;
   // dfk_se3_track_batch, apart from the single-problem buffers above so neither path disturbs the other:
   //   batch_dev  [descriptors L x N (level-major) | poses 8 N | last systems 32 N]  (bytes; one H2D, one D2H per call)
   //   batch_partials  N x stride x 32 floats,  batch_counters  N self-resetting tickets (zeroed on allocation)
@@ -80,63 +85,50 @@ struct DfkContext {
   PinnedBuf<unsigned char> batch_host;   // mirror of batch_dev
   DeviceBuf<float> batch_partials;
   DeviceBuf<unsigned int> batch_counters;
-  // dfk_sfm_evaluate_error_batch, apart from the single-call buffers: the descriptors (one H2D per call), the partials
-  // (one 32-float row per block of every item) and one self-resetting ticket per item (zeroed on allocation)
-  DeviceBuf<EvalErrorDesc> eval_descs;
-  std::vector<EvalErrorDesc> eval_host;
+  // dfk_sfm_evaluate_error_batch, apart from the single-call buffers: the descriptors, the partials (one 32-float row per
+  // block of every item) and one self-resetting ticket per item (zeroed on allocation)
+  DeviceBuf<unsigned char> eval_descs;
   DeviceBuf<float> eval_partials;
   DeviceBuf<unsigned int> eval_counters;
-  // dfk_update_depth_batch: [descriptors | codes] (bytes), one H2D per call from depth_host
+  // dfk_update_depth_batch: [descriptors | codes]
   DeviceBuf<unsigned char> depth_dev;
-  std::vector<unsigned char> depth_host;
-  // dfk_depth_prior_linearize_batch / dfk_depth_prior_error_batch: [descriptors | codes] (bytes), one H2D per call from
-  // depth_prior_host, and the items' partial rows
+  // dfk_depth_prior_linearize_batch / dfk_depth_prior_error_batch: [descriptors | codes], and the items' partial rows
   DeviceBuf<unsigned char> depth_prior_dev;
-  std::vector<unsigned char> depth_prior_host;
   DeviceBuf<float> depth_prior_partials;
 
   // dfk_reprojection_linearize / dfk_sparse_geometric_linearize: [one item's staging block | rows (| err2)]
   DeviceBuf<unsigned char> sparse_dev;
   PinnedBuf<unsigned char> sparse_host;  // mirror
-  // dfk_reprojection_linearize_batch: [descriptors | codes | query | train] (bytes), one H2D per call from rep_host
+  // dfk_reprojection_linearize_batch: [descriptors | codes | query | train]
   DeviceBuf<unsigned char> rep_dev;
-  std::vector<unsigned char> rep_host;
-  // dfk_sparse_geometric_linearize_batch: [descriptors | codes | points] (bytes), one H2D per call from geo_host; apart
-  // from rep_dev so that batches of the two kinds enqueued back to back keep their own staging
+  // dfk_sparse_geometric_linearize_batch: [descriptors | codes | points]; apart from rep_dev so that batches of the two
+  // kinds enqueued back to back keep their own staging
   DeviceBuf<unsigned char> geo_dev;
-  std::vector<unsigned char> geo_host;
   DeviceBuf<SfmItemDev> items_dev;
   DeviceBuf<float> partials_dev;
-  // dfk_hamming_match_batch / dfk_reprojection_match_batch: the item descriptors (one H2D per call) and the RANSAC
-  // scratch [matches (int2 per query) | hypothesis counts | selections (int3 per item)] (bytes)
-  DeviceBuf<MatchItemDev> match_items;
-  std::vector<MatchItemDev> match_host;
+  // dfk_hamming_match_batch / dfk_reprojection_match_batch: the item descriptors and the RANSAC scratch [matches (int2
+  // per query) | hypothesis counts | selections (int3 per item)]
+  DeviceBuf<unsigned char> match_items;
   DeviceBuf<unsigned char> match_scratch;
-  // dfk_orb_detect_batch: the item descriptors (one H2D per call) and the detector's scratch (see the call)
-  DeviceBuf<OrbItemDev> orb_items;
-  std::vector<OrbItemDev> orb_host;
+  // dfk_orb_detect_batch: the item descriptors and the detector's scratch (OrbPlan::scratch)
+  DeviceBuf<unsigned char> orb_items;
   DeviceBuf<unsigned char> orb_scratch;
-  // dfk_orb_detect_pyramid_batch: [one-level items | gather items | resize items] (bytes, one H2D per call from
-  // orb_pyr_host); its level images and staged rows follow the detector's scratch in orb_scratch
+  // dfk_orb_detect_pyramid_batch: [one-level items | gather items | resize items]; its level images and staged rows
+  // follow the detector's scratch in orb_scratch
   DeviceBuf<unsigned char> orb_pyr_dev;
-  std::vector<unsigned char> orb_pyr_host;
-  // dfk_preprocess_batch: [item descriptors | pyramid level descriptors L x n] (bytes, one H2D per call from pp_host)
-  // and the normalising items' tile partials
+  // dfk_preprocess_batch: [item descriptors | pyramid level descriptors L x n], and the normalising items' tile partials
   DeviceBuf<unsigned char> pp_dev;
-  std::vector<unsigned char> pp_host;
   DeviceBuf<double> pp_partials;
-  // dfk_keyframe_mesh_batch: [item descriptors | decode descriptors | codes] (bytes, one H2D per call from mesh_host)
-  // and [segment masks | segment bases | decoded depths] (bytes)
+  // dfk_keyframe_mesh_batch: [item descriptors | decode descriptors | codes], and the scratch [segment masks | segment
+  // bases | decoded depths]
   DeviceBuf<unsigned char> mesh_dev;
-  std::vector<unsigned char> mesh_host;
   DeviceBuf<unsigned char> mesh_scratch;
-  // the dfk_bow_* calls: the call's descriptors (one H2D per call from bow_host), the transform's per-descriptor words
-  // when the caller passes none, and a query's [sums n x size | hits n x size] (bytes)
+  // the dfk_bow_* calls: the call's descriptors, the transform's per-descriptor words when the caller passes none, and a
+  // query's [sums n x size | hits n x size]
   DeviceBuf<unsigned char> bow_dev;
-  std::vector<unsigned char> bow_host;
   DeviceBuf<int32_t> bow_words;
   DeviceBuf<unsigned char> bow_scratch;
-  // dfk_window_marginalize_frames / dfk_window_add_priors: the call's index lists (one pageable H2D per call)
+  // dfk_window_marginalize_frames / _add_priors / _add_depth_priors: the call's index lists (one pageable H2D per call)
   DeviceBuf<int> window_lists;
   // dfk_window_marginalize_keyframe: the call's lists [refs | tile rows / cols | member locations | update tasks] (one
   // pageable H2D per call), the code of m, and the local system's workspace (tiles, rhs, f)
@@ -251,6 +243,60 @@ struct DeviceGuard {
   }
 };
 
+// ---------------------------------------------------------------------------- blobs of typed parts
+// A call's staged upload, or its scratch, is one blob of typed parts, each rounded up to 16 bytes: the kernels read
+// int2 / int3 / uint4 / double parts.  A Part is where one part starts; the same offset addresses it from the host
+// image and from the device copy.
+template <class T>
+struct Part {
+  size_t off = 0;
+  T* at(void* base) const { return reinterpret_cast<T*>(static_cast<unsigned char*>(base) + off); }
+};
+
+// The sizing pass: add() the parts in blob order; `bytes` is the blob's size
+struct Layout {
+  size_t bytes = 0;
+  template <class T>
+  Part<T> add(size_t count)
+  {
+    const Part<T> p{bytes};
+    bytes += (sizeof(T) * count + 15) & ~(size_t)15;
+    return p;
+  }
+};
+
+// A blob uploaded with one copy.  add() lays its parts out as Layout does and grows the host image, zeroed, in a
+// pageable buffer (the handle's `staging`, or one of the object the blob belongs to); upload() grows the device buffer
+// and copies.  Messages begin with `what`.
+struct Staging : Layout {
+  std::vector<unsigned char>& buf;
+  unsigned char* dev = nullptr;
+
+  explicit Staging(std::vector<unsigned char>& b) : buf(b) { buf.clear(); }
+  template <class T>
+  Part<T> add(size_t count)
+  {
+    const Part<T> p = Layout::add<T>(count);
+    buf.resize(bytes, 0);
+    return p;
+  }
+  unsigned char* host() { return buf.data(); }
+  // for parts that point into the device copy; after the call's checks, so that a rejected call allocates nothing
+  DfkStatus grow(DfkHandle h, DeviceBuf<unsigned char>& d, const std::string& what)
+  {
+    DFK_CUDA(h, d.ensure(bytes), (what + "scratch allocation failed").c_str());
+    dev = d.ptr;
+    return DFK_OK;
+  }
+  DfkStatus upload(DfkHandle h, DeviceBuf<unsigned char>& d, const std::string& what)
+  {
+    DFK_TRY(grow(h, d, what));
+    DFK_CUDA(h, cudaMemcpyAsync(dev, host(), bytes, cudaMemcpyHostToDevice, h->stream),
+             (what + "upload failed").c_str());
+    return DFK_OK;
+  }
+};
+
 // ---------------------------------------------------------------------------- validation helpers
 inline bool img_ok(const DfkImage* im, uint32_t w, uint32_t h, uint32_t floats_per_px)
 {
@@ -327,13 +373,19 @@ inline void set_depth_decode_desc(DepthDecodeDesc& d, const DfkDepthDecodeItem& 
   *max_blocks = std::max(*max_blocks, d.nblocks);
 }
 
+// A depth-prior batch as stage_depth_prior staged it
+struct DepthPriorStaged {
+  Part<DepthPriorDesc> descs;
+  Part<float> codes;
+  int max_parts = 1, rows = 0;  // the grid's partial blocks, the partial rows of the batch
+};
+
 // Checks and stages n depth-prior items in one upload, [descriptors n | codes n x C] packed in `host` and copied to
 // `dev` (codes: the items' HOST codes; with codes == false -- the window problem, which rewrites them from its state on
 // the device before every batch -- left zero and the items' code fields ignored).
-// *max_parts: the grid's partial blocks, *rows: the partial rows of the batch.
 inline DfkStatus stage_depth_prior(DfkHandle h, const char* what, const DfkDepthPriorItem* items, int n, int code_size,
                                    bool codes, std::vector<unsigned char>& host, DeviceBuf<unsigned char>& dev,
-                                   int* max_parts, int* rows)
+                                   DepthPriorStaged* st)
 {
   const std::string w(what);
   if (!items || n < 1 || n > 65535)  // blockIdx.y of the partial kernel is the item
@@ -347,33 +399,26 @@ inline DfkStatus stage_depth_prior(DfkHandle h, const char* what, const DfkDepth
         !img_ok(&it.target_dpt, W, H, 1) || !img_ok(&it.prx_orig, W, H, 1) || !img_ok(&it.prx_jac, W, H, code_size))
       return fail(h, DFK_ERR_INVALID_ARG, w + "null code or inconsistent image views in item " + std::to_string(i));
   }
-  const size_t desc_bytes = (sizeof(DepthPriorDesc) * (size_t)n + 15) & ~(size_t)15;
-  const size_t total = desc_bytes + sizeof(float) * (size_t)n * code_size;
-  DFK_CUDA(h, dev.ensure(total), (w + "scratch allocation failed").c_str());
-  host.assign(total, 0);
-  DepthPriorDesc* descs = reinterpret_cast<DepthPriorDesc*>(host.data());
-  float* code_host = reinterpret_cast<float*>(host.data() + desc_bytes);
-  const float* codes_dev = reinterpret_cast<const float*>(dev.ptr + desc_bytes);
-  *max_parts = 1;
-  *rows = 0;
+  Staging s(host);
+  st->descs = s.add<DepthPriorDesc>(n);
+  st->codes = s.add<float>((size_t)n * code_size);
+  DFK_TRY(s.grow(h, dev, w));
   for (int i = 0; i < n; ++i) {
     const DfkDepthPriorItem& it = items[i];
-    DepthPriorDesc& d = descs[i];
+    DepthPriorDesc& d = st->descs.at(s.host())[i];
     d.tgt = view_of(&it.target_dpt);
     d.prx = view_of(&it.prx_orig);
     d.jac = view_of(&it.prx_jac);
-    d.code = codes_dev + (size_t)i * code_size;
+    d.code = st->codes.at(s.dev) + (size_t)i * code_size;
     d.width = (int)it.target_dpt.width;
     d.height = (int)it.target_dpt.height;
     d.parts = depth_prior_parts(d.width, d.height);
-    d.part0 = *rows;
-    *rows += d.parts;
-    *max_parts = std::max(*max_parts, d.parts);
-    if (codes) memcpy(code_host + (size_t)i * code_size, it.code, sizeof(float) * code_size);
+    d.part0 = st->rows;
+    st->rows += d.parts;
+    st->max_parts = std::max(st->max_parts, d.parts);
+    if (codes) memcpy(st->codes.at(s.host()) + (size_t)i * code_size, it.code, sizeof(float) * code_size);
   }
-  DFK_CUDA(h, cudaMemcpyAsync(dev.ptr, host.data(), total, cudaMemcpyHostToDevice, h->stream),
-           (w + "upload failed").c_str());
-  return DFK_OK;
+  return s.upload(h, dev, w);
 }
 
 // n self-resetting tickets of a batched kernel: they must be zero when first used, so a buffer that grows is zeroed
@@ -471,8 +516,8 @@ struct Sparse<DfkSparseGeometricItem> {
   }
 };
 
-// Host staging: the batches stage in pageable memory (cudaMemcpyAsync has read it when it returns, so the next batch may
-// refill it while the copy is still queued); the synchronous single calls in pinned memory, into which their rows return.
+// Host staging: the batches stage in pageable memory (see DfkContext::staging), the synchronous single calls in pinned
+// memory, into which their rows return.
 inline cudaError_t host_block(std::vector<unsigned char>& v, size_t bytes, unsigned char** p)
 {
   v.assign(bytes, 0);
@@ -494,7 +539,7 @@ struct Staged {
 
 // Checks the code size and items[0, n) (messages begin with `what`, a batch's name the item), then stages the factors in
 // one upload: [descriptors n | codes n x codes C | payload], packed in `host` and copied to `dev`, both grown by
-// out_bytes for the caller's outputs.
+// out_bytes for the caller's outputs, which follow the upload.
 template <class Item, class HostBuf>
 DfkStatus stage(DfkHandle h, const std::string& what, bool batch, const Item* items, int n, int code_size,
                 size_t out_bytes, HostBuf& host, DeviceBuf<unsigned char>& dev, Staged* st)
@@ -509,17 +554,19 @@ DfkStatus stage(DfkHandle h, const std::string& what, bool batch, const Item* it
   }
   if (st->total > (size_t)INT32_MAX)
     return fail(h, DFK_ERR_INVALID_ARG, what + "more than 2^31 - 1 " + S::units + " in one call");
-  const size_t desc_bytes = (sizeof(typename S::Dev) * (size_t)n + 15) & ~(size_t)15;
-  const size_t code_floats = (size_t)S::codes * code_size, payload = desc_bytes + sizeof(float) * n * code_floats;
-  st->bytes = payload + S::unit_bytes * st->total;
+  const size_t code_floats = (size_t)S::codes * code_size;
+  Layout L;
+  const Part<typename S::Dev> descs = L.add<typename S::Dev>(n);
+  const Part<float> codes = L.add<float>(n * code_floats);
+  const Part<unsigned char> payload = L.add<unsigned char>(S::unit_bytes * st->total);
+  st->bytes = L.bytes;
   DFK_CUDA(h, dev.ensure(st->bytes + out_bytes), (what + "scratch allocation failed").c_str());
   unsigned char* hb = nullptr;
   DFK_CUDA(h, host_block(host, st->bytes + out_bytes, &hb), (what + "pinned allocation failed").c_str());
-  const float* codes_dev = reinterpret_cast<const float*>(dev.ptr + desc_bytes);
   for (size_t i = 0, begin = 0; i < (size_t)n; begin += S::count(items[i]), ++i)
-    S::pack(items[i], code_size, begin, st->total, reinterpret_cast<typename S::Dev*>(hb)[i],
-            reinterpret_cast<float*>(hb + desc_bytes) + i * code_floats, codes_dev + i * code_floats, hb + payload);
+    S::pack(items[i], code_size, begin, st->total, descs.at(hb)[i], codes.at(hb) + i * code_floats,
+            codes.at(dev.ptr) + i * code_floats, payload.at(hb));
   DFK_CUDA(h, cudaMemcpyAsync(dev.ptr, hb, st->bytes, cudaMemcpyHostToDevice, h->stream), (what + "upload failed").c_str());
-  st->payload = dev.ptr + payload;
+  st->payload = payload.at(dev.ptr);
   return DFK_OK;
 }
