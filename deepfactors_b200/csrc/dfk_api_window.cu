@@ -299,7 +299,7 @@ DfkStatus problem_error(DfkHandle h, DfkWindowProblem* p, const double* state, d
   h->launches += 1;
   const float avg = p->avg_dpt;
   if (p->ndep > 0) {
-    DFK_CUDA(h, launch_update_depth_batch(p->C, reinterpret_cast<const DepthDecodeDesc*>(p->depth.ptr), p->ndep,
+    DFK_CUDA(h, launch_update_depth(p->C, reinterpret_cast<const DepthDecodeDesc*>(p->depth.ptr), p->ndep,
                                           p->depth_max_blocks, avg, h->stream),
              what);
     h->launches += 1;
@@ -311,7 +311,7 @@ DfkStatus problem_error(DfkHandle h, DfkWindowProblem* p, const double* state, d
     const char* sw = "[WindowProblem::error] scratch allocation failed";
     DFK_CUDA(h, h->eval_partials.ensure((size_t)p->err_rows * 32), sw);
     DFK_TRY(ensure_tickets(h, h->eval_counters, (size_t)p->ne, sw, sw));
-    DFK_CUDA(h, launch_eval_error_batch(p->sub_err ? p->err_sub.ptr : p->err.ptr, ne, p->err_max_blocks,
+    DFK_CUDA(h, launch_eval_error(p->sub_err ? p->err_sub.ptr : p->err.ptr, ne, p->err_max_blocks,
                                         p->huber_delta, h->eval_partials.ptr, h->eval_counters.ptr, out, h->stream),
              what);
     h->launches += 1;

@@ -72,21 +72,20 @@ struct DfkContext {
   DeviceBuf<float> out_dev;              // 32 floats
   PinnedBuf<float> out_host;             // 32 floats
   DeviceBuf<float> code_dev;             // 256 floats
-  DeviceBuf<float> track_dev;            // dfk_se3_track: [pose 8 | per-iteration history 36 each]
-  PinnedBuf<float> track_host;           // mirror of track_dev + the last system (32)
   // The calls' staged blobs (see Staging) are laid out in `staging`, one pageable host buffer for every call:
   // cudaMemcpyAsync from pageable memory has read it when it returns, so the next call may refill it while the copy is
   // still queued.  Each call family uploads into a device buffer of its own, below.
   std::vector<unsigned char> staging;
-  // dfk_se3_track_batch, apart from the single-problem buffers above so neither path disturbs the other:
-  //   batch_dev  [descriptors L x N (level-major) | poses 8 N | last systems 32 N]  (bytes; one H2D, one D2H per call)
+  // dfk_se3_track and dfk_se3_track_batch:
+  //   batch_dev  [descriptors L x N (level-major) | poses 8 N | last systems 32 N | history 36 per iteration]  (bytes;
+  //   one H2D, one D2H per call)
   //   batch_partials  N x stride x 32 floats,  batch_counters  N self-resetting tickets (zeroed on allocation)
   DeviceBuf<unsigned char> batch_dev;
   PinnedBuf<unsigned char> batch_host;   // mirror of batch_dev
   DeviceBuf<float> batch_partials;
   DeviceBuf<unsigned int> batch_counters;
-  // dfk_sfm_evaluate_error_batch, apart from the single-call buffers: the descriptors, the partials (one 32-float row per
-  // block of every item) and one self-resetting ticket per item (zeroed on allocation)
+  // dfk_sfm_evaluate_error_batch: the descriptors, the partials (one 32-float row per block of every item) and one
+  // self-resetting ticket per item (zeroed on allocation)
   DeviceBuf<unsigned char> eval_descs;
   DeviceBuf<float> eval_partials;
   DeviceBuf<unsigned int> eval_counters;
@@ -351,7 +350,7 @@ inline void set_eval_error_desc(EvalErrorDesc& d, const DfkCamera& cam, const fl
   d.img0 = view_of(&img0); d.img1 = view_of(&img1); d.dpt0 = view_of(&dpt0);
   d.width = (int)img0.width;
   d.height = (int)img0.height;
-  d.nblocks = eval_error_blocks(d.width, d.height);
+  d.nblocks = grid_for(d.width * d.height);
   d.scratch_row = *rows;
   *rows += d.nblocks;
   *max_blocks = std::max(*max_blocks, d.nblocks);

@@ -148,65 +148,62 @@ struct View {
   const float* ptr;
   uint32_t pitch;  // floats
 };
-cudaError_t launch_se3_step(const PixelCam& pc, float huber_delta, int width, int height, View img0, View img1,
-                            View dpt0, View grad1, bool grad_aligned, float* scratch, unsigned int* counter,
-                            float* out_dev /*29 floats: 21 JtJ, 6 Jtr, res, inliers bits*/, cudaStream_t s,
-                            float* pose_dev = nullptr /*tracking mode: pose read from / updated in device memory*/,
-                            float* history_dev = nullptr /*36 floats: the 29 above + the pose they were evaluated at*/);
-// One (problem, level) of dfk_se3_track_batch: what launch_se3_step takes for that level, and its block count.
+// Blocks of a single-pass reduction over `area` pixels: one per 256 pixels, at least 1, at most kSimpleMaxBlocks (the
+// grid-stride loops take the rest).
+int grid_for(int area);
+// SE3 step, EvaluateError, UpdateDepth, and Sobel / blur-down (PyrLevelDev) have two launchers each: one item, whose
+// descriptor travels with the launch, and a batch, whose descriptors are in device memory (grid max_blocks x num_items).
+// Both run the same kernel, so an item gives the same bits either way.
+// One (problem, level) of SE3Aligner::RunStep / CameraTracker::TrackFrame.
 struct Se3TrackDesc {
-  PixelCam pc;  // q / t are overridden by the problem's device pose
+  PixelCam pc;  // q / t are overridden by the problem's device pose when tracking
   View img0, img1, dpt0, grad1;
   int width, height;
-  int nblocks;       // se3_step_blocks(width, height)
+  int nblocks;  // grid_for(width * height)
   int grad_aligned;
 };
-// blocks of se3_step_kernel's grid for a level of this size (the batched kernel gives a problem exactly as many)
-int se3_step_blocks(int width, int height);
-// descs_dev: num_problems descriptors of one level.  Problem n: scratch rows [n * scratch_stride, + nblocks) (32 floats
-// each), counters[n] (zero, self-resetting), outs[32 n .. + 29) the last system, poses[8 n .. + 7) the pose, updated.
-cudaError_t launch_se3_track_batch(const Se3TrackDesc* descs_dev, int num_problems, int max_blocks, float huber_delta,
-                                   float* scratch, int scratch_stride, unsigned int* counters, float* outs, float* poses,
-                                   cudaStream_t s);
-cudaError_t launch_eval_error(const PixelCam& pc, float huber_delta, int width, int height, View img0, View img1,
-                              View dpt0, float* scratch, unsigned int* counter, float* out_dev /*2*/, cudaStream_t s);
-// One item of dfk_sfm_evaluate_error_batch: what launch_eval_error takes for it, its block count and its scratch rows.
+// Problem n: scratch rows [n * scratch_stride, + nblocks) (32 floats each), counter n (zero, self-resetting), out[32 n ..
+// + 29) the system (21 JtJ, 6 Jtr, residual, inlier bits).  The pose is read from and updated in pose[8 n .. + 7)
+// (tracking; a batch always tracks), and history, if not null, receives the system and the pose it was evaluated at (36
+// floats).  A single problem with pose null is evaluated at d.pc's pose (RunStep).
+cudaError_t launch_se3_step(const Se3TrackDesc& d, float huber_delta, float* scratch, unsigned int* counter, float* out,
+                            float* pose, float* history, cudaStream_t s);
+cudaError_t launch_se3_step(const Se3TrackDesc* descs_dev, int num_problems, int max_blocks, float huber_delta,
+                            float* scratch, int scratch_stride, unsigned int* counters, float* outs, float* poses,
+                            cudaStream_t s);
+// One item of SfmAligner::EvaluateError: its block count and its scratch rows.
 struct EvalErrorDesc {
   PixelCam pc;
   View img0, img1, dpt0;
   int width, height;
-  int nblocks;      // eval_error_blocks(width, height)
+  int nblocks;      // grid_for(width * height)
   int scratch_row;  // first of its nblocks scratch rows (32 floats each)
 };
-// blocks of eval_error_kernel's grid for an item of this size (the batched kernel gives an item exactly as many)
-int eval_error_blocks(int width, int height);
-// Item n: scratch rows [scratch_row, + nblocks), counters[n] (zero, self-resetting), outs[2 n .. + 2) = [residual |
+// Item n: scratch rows [scratch_row, + nblocks), counter n (zero, self-resetting), out[2 n .. + 2) = [residual |
 // inliers (u32 bits)].
-cudaError_t launch_eval_error_batch(const EvalErrorDesc* descs_dev, int num_items, int max_blocks, float huber_delta,
-                                    float* scratch, unsigned int* counters, float* outs, cudaStream_t s);
-// One item of dfk_update_depth_batch: what launch_update_depth takes for it, its block count and kernel body.
+cudaError_t launch_eval_error(const EvalErrorDesc& d, float huber_delta, float* scratch, unsigned int* counter,
+                              float* out, cudaStream_t s);
+cudaError_t launch_eval_error(const EvalErrorDesc* descs_dev, int num_items, int max_blocks, float huber_delta,
+                              float* scratch, unsigned int* counters, float* outs, cudaStream_t s);
+// One depth decode (UpdateDepth): its block count and kernel body.
 struct DepthDecodeDesc {
   View prx, jac;
   float* dpt;
   uint32_t dpt_pitch;
-  const float* code;  // code_size floats in device scratch
+  const float* code;  // code_size floats in device memory
   int width, height;
   int nblocks;  // update_depth_blocks(width, height)
   int vector;   // update_depth_vector(code_size, code, jac)
 };
-// launch_update_depth's grid for a level of this size, and whether it runs the vector kernel (else the generic one)
+// The decode's grid for a level of this size, and whether it runs the vector body (else the generic one)
 int update_depth_blocks(int width, int height);
 bool update_depth_vector(int code_size, const float* code_dev, View jac);
-cudaError_t launch_update_depth_batch(int code_size, const DepthDecodeDesc* descs_dev, int num_items, int max_blocks,
-                                      float avg_dpt, cudaStream_t s);
+cudaError_t launch_update_depth(int code_size, const DepthDecodeDesc& d, float avg_dpt, cudaStream_t s);
+cudaError_t launch_update_depth(int code_size, const DepthDecodeDesc* descs_dev, int num_items, int max_blocks,
+                                float avg_dpt, cudaStream_t s);
 cudaError_t launch_warp(const PixelCam& pc, int width, int height, View img0, View img1, View dpt0, float* img2,
                         uint32_t img2_pitch, float* scratch, unsigned int* counter, float* out_dev /*2*/,
                         cudaStream_t s);
-cudaError_t launch_update_depth(const float* code_dev, int code_size, int width, int height, View prx_orig, View jac,
-                                float avg_dpt, float* dpt, uint32_t dpt_pitch, cudaStream_t s);
-cudaError_t launch_sobel(int width, int height, View img, float* grad, uint32_t grad_pitch, cudaStream_t s);
-cudaError_t launch_blur_down(int in_w, int in_h, View in, int out_w, int out_h, float* out, uint32_t out_pitch,
-                             cudaStream_t s);
 cudaError_t launch_squared_error(int width, int height, View a, View b, float* scratch, unsigned int* counter,
                                  float* out_dev, cudaStream_t s);
 // dfk_window.cu : block-sparse window assembly (gather over CSR lists built on the host by dfk_window_create)
@@ -559,7 +556,7 @@ struct PpItemDev {
 // level 0 rewritten as f')
 cudaError_t launch_preprocess(const PpItemDev* items_dev, int n, int max_tiles, bool normalize, double* partials,
                               cudaStream_t s);
-// one level of one frame of a batched pyramid (dfk_simple.cu); pitches in floats, grad null: no gradient
+// one level of one frame of a pyramid (dfk_simple.cu); pitches in floats, grad null: no gradient
 struct PyrLevelDev {
   float* img;
   uint32_t pitch;
@@ -567,11 +564,12 @@ struct PyrLevelDev {
   float* grad;
   uint32_t grad_pitch;
 };
-// out[i] = GaussianBlurDown(in[i]) and grad of lv[i] = SobelGradients(img of lv[i]) for the n frames of a level, bit for
-// bit launch_blur_down / launch_sobel on each frame alone; grid (max tiles x, max tiles y, n)
-cudaError_t launch_blur_down_batch(const PyrLevelDev* in_dev, const PyrLevelDev* out_dev, int n, int max_out_w,
-                                   int max_out_h, cudaStream_t s);
-cudaError_t launch_sobel_batch(const PyrLevelDev* lv_dev, int n, int max_w, int max_h, cudaStream_t s);
+// grad of lv = SobelGradients(img of lv), out = GaussianBlurDown(in); the batches take the n frames of one level
+cudaError_t launch_sobel(const PyrLevelDev& lv, cudaStream_t s);
+cudaError_t launch_sobel(const PyrLevelDev* lv_dev, int n, int max_w, int max_h, cudaStream_t s);
+cudaError_t launch_blur_down(const PyrLevelDev& in, const PyrLevelDev& out, cudaStream_t s);
+cudaError_t launch_blur_down(const PyrLevelDev* in_dev, const PyrLevelDev* out_dev, int n, int max_out_w,
+                             int max_out_h, cudaStream_t s);
 
 // DBoW2 retrieval (dfk_bow.cu).  The vocabulary on the device, rows re-indexed breadth first so that a node's
 // children are consecutive rows: row 0 is the root, desc [rows, q] (q = descriptor_bytes / 16), child[row] = (first

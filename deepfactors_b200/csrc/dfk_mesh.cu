@@ -1,7 +1,7 @@
 // dfk_mesh.cu -- dfk_keyframe_mesh_batch (include/dfk.h, DESIGN.md section 4.12): the keyframe renderer's geometry
 // (gui/shaders/drawkf.geom) as a world-frame mesh, and SaveKeyframes' uint16 depth, for many keyframes in one call.
 //
-// Three launches over every (tile, item); a depth the call decodes is already in scratch (update_depth_batch_kernel,
+// Three launches over every (tile, item); a depth the call decodes is already in scratch (update_depth_kernel,
 // enqueued by the call before these):
 //   classify  a 32 x 8 tile with a one-pixel halo: the pixel flags of 34 x 10 pixels, the triangle flags of the 33 x 9
 //             quads that touch the tile, then per pixel its own T1 / T2 flags and whether it is a corner of an emitted

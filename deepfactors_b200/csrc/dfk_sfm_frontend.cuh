@@ -151,7 +151,7 @@ __device__ __forceinline__ bool pixel_row(const SfmItem<MAXCODE>& I, uint32_t x,
   return true;
 }
 
-// fused depth decode from a staged code-Jacobian row: the arithmetic of update_depth_kernel (dfk_geom.cuh)
+// fused depth decode from a staged code-Jacobian row: the arithmetic of update_depth_kernel's vector body (dfk_geom.cuh)
 template <int C>
 __device__ __forceinline__ float staged_depth(const float* row, const float* code, float prx, float avg_dpt)
 {

@@ -339,7 +339,8 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_tiles, float* _
       const float i0 = ld_stream(I.img0 + (size_t)py * I.img0_pitch + pxx);
       if (fused) {
         // dpt0 is prx_orig: decode the depth from the pixel's code-Jacobian row with the arithmetic of
-        // update_depth_kernel, here across the 8 lanes (and the NCB registers) that hold the chunks of one pixel
+        // update_depth_kernel's vector body, here across the 8 lanes (and the NCB registers) that hold the chunks of
+        // one pixel
         float4 cc[NCB];
 #pragma unroll
         for (int cb = 0; cb < NCB; ++cb) cc[cb] = *reinterpret_cast<const float4*>(&I.code[32 * cb + 4 * (lane & 7)]);
