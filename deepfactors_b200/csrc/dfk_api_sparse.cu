@@ -34,12 +34,12 @@ DfkStatus dfk_reprojection_linearize(DfkHandle h, const float pose0[7], const fl
     // [the one item's staging | rows | err2], in scratch of its own: an earlier asynchronous batch may still be reading
     // the batches' staging
     const size_t M = (size_t)num_matches, RW = 13 + (size_t)code_size, n_out = 2 * M * RW + M;
-    Staged st;
+    Staged<DfkReprojectionItem> st;
     DFK_TRY(stage(h, "[ReprojectionFactor::linearize] ", false, &it, 1, code_size, n_out * sizeof(float), h->sparse_host,
                   h->sparse_dev, &st));
-    const float2* d_query = reinterpret_cast<const float2*>(st.payload);
+    const float2* d_query = st.payload.at(h->sparse_dev.ptr);
     float* d_rows = reinterpret_cast<float*>(h->sparse_dev.ptr + st.bytes);
-    DFK_CUDA(h, launch_reprojection_rows(code_size, *reinterpret_cast<const ReprojItemDev*>(h->sparse_host.ptr), d_query,
+    DFK_CUDA(h, launch_reprojection_rows(code_size, st.descs.at(h->sparse_host.ptr)[0], d_query,
                                          d_query + M, h->params.sfmparams.avg_dpt, d_rows, d_rows + 2 * M * RW, h->stream),
              "[ReprojectionFactor::linearize] kernel launch failed");
     h->launches += 1;
@@ -61,10 +61,10 @@ DfkStatus dfk_reprojection_linearize_batch(DfkHandle h, const DfkReprojectionIte
     if (!items || n < 1 || !records_dev)
       return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::linearize batch] null argument / empty batch");
     DeviceGuard guard(h->device);
-    Staged st;
+    Staged<DfkReprojectionItem> st;
     DFK_TRY(stage(h, "[ReprojectionFactor::linearize batch] ", true, items, n, code_size, 0, h->staging, h->rep_dev, &st));
-    const float2* query_dev = reinterpret_cast<const float2*>(st.payload);
-    DFK_CUDA(h, launch_reprojection_records(code_size, reinterpret_cast<const ReprojItemDev*>(h->rep_dev.ptr), n,
+    const float2* query_dev = st.payload.at(h->rep_dev.ptr);
+    DFK_CUDA(h, launch_reprojection_records(code_size, st.descs.at(h->rep_dev.ptr), n,
                                             query_dev, query_dev + st.total, h->params.sfmparams.avg_dpt, records_dev,
                                             h->stream),
              "[ReprojectionFactor::linearize batch] kernel launch failed");
@@ -485,12 +485,12 @@ DfkStatus dfk_sparse_geometric_linearize(DfkHandle h, const float pose0[7], cons
     DeviceGuard guard(h->device);
     // [the one item's staging | rows], apart from the batches' staging
     const size_t M = (size_t)num_points, RW = 13 + 2 * (size_t)code_size;
-    Staged st;
+    Staged<DfkSparseGeometricItem> st;
     DFK_TRY(stage(h, "[SparseGeometricFactor::linearize] ", false, &it, 1, code_size, M * RW * sizeof(float),
                   h->sparse_host, h->sparse_dev, &st));
     float* d_rows = reinterpret_cast<float*>(h->sparse_dev.ptr + st.bytes);
-    DFK_CUDA(h, launch_sparse_geometric_rows(code_size, *reinterpret_cast<const GeoItemDev*>(h->sparse_host.ptr),
-                                             reinterpret_cast<const int2*>(st.payload), h->params.sfmparams.avg_dpt,
+    DFK_CUDA(h, launch_sparse_geometric_rows(code_size, st.descs.at(h->sparse_host.ptr)[0],
+                                             st.payload.at(h->sparse_dev.ptr), h->params.sfmparams.avg_dpt,
                                              d_rows, h->stream),
              "[SparseGeometricFactor::linearize] kernel launch failed");
     h->launches += 1;
@@ -512,11 +512,11 @@ DfkStatus dfk_sparse_geometric_linearize_batch(DfkHandle h, const DfkSparseGeome
     if (!items || n < 1 || !records_dev)
       return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::linearize batch] null argument / empty batch");
     DeviceGuard guard(h->device);
-    Staged st;
+    Staged<DfkSparseGeometricItem> st;
     DFK_TRY(stage(h, "[SparseGeometricFactor::linearize batch] ", true, items, n, code_size, 0, h->staging, h->geo_dev,
                   &st));
-    DFK_CUDA(h, launch_sparse_geometric_records(code_size, reinterpret_cast<const GeoItemDev*>(h->geo_dev.ptr), n,
-                                                reinterpret_cast<const int2*>(st.payload), h->params.sfmparams.avg_dpt,
+    DFK_CUDA(h, launch_sparse_geometric_records(code_size, st.descs.at(h->geo_dev.ptr), n,
+                                                st.payload.at(h->geo_dev.ptr), h->params.sfmparams.avg_dpt,
                                                 records_dev, h->stream),
              "[SparseGeometricFactor::linearize batch] kernel launch failed");
     h->launches += 1;
@@ -530,10 +530,10 @@ DfkStatus dfk_reprojection_error_batch(DfkHandle h, const DfkReprojectionItem* i
     if (!items || n < 1 || !out_dev)
       return fail(h, DFK_ERR_INVALID_ARG, "[ReprojectionFactor::error batch] null argument / empty batch");
     DeviceGuard guard(h->device);
-    Staged st;
+    Staged<DfkReprojectionItem> st;
     DFK_TRY(stage(h, "[ReprojectionFactor::error batch] ", true, items, n, code_size, 0, h->staging, h->rep_dev, &st));
-    const float2* query_dev = reinterpret_cast<const float2*>(st.payload);
-    DFK_CUDA(h, launch_reprojection_error(code_size, reinterpret_cast<const ReprojItemDev*>(h->rep_dev.ptr), n, query_dev,
+    const float2* query_dev = st.payload.at(h->rep_dev.ptr);
+    DFK_CUDA(h, launch_reprojection_error(code_size, st.descs.at(h->rep_dev.ptr), n, query_dev,
                                           query_dev + st.total, h->params.sfmparams.avg_dpt, out_dev, h->stream),
              "[ReprojectionFactor::error batch] kernel launch failed");
     h->launches += 1;
@@ -548,10 +548,10 @@ DfkStatus dfk_sparse_geometric_error_batch(DfkHandle h, const DfkSparseGeometric
     if (!items || n < 1 || !out_dev)
       return fail(h, DFK_ERR_INVALID_ARG, "[SparseGeometricFactor::error batch] null argument / empty batch");
     DeviceGuard guard(h->device);
-    Staged st;
+    Staged<DfkSparseGeometricItem> st;
     DFK_TRY(stage(h, "[SparseGeometricFactor::error batch] ", true, items, n, code_size, 0, h->staging, h->geo_dev, &st));
-    DFK_CUDA(h, launch_sparse_geometric_error(code_size, reinterpret_cast<const GeoItemDev*>(h->geo_dev.ptr), n,
-                                              reinterpret_cast<const int2*>(st.payload), h->params.sfmparams.avg_dpt,
+    DFK_CUDA(h, launch_sparse_geometric_error(code_size, st.descs.at(h->geo_dev.ptr), n,
+                                              st.payload.at(h->geo_dev.ptr), h->params.sfmparams.avg_dpt,
                                               out_dev, h->stream),
              "[SparseGeometricFactor::error batch] kernel launch failed");
     h->launches += 1;

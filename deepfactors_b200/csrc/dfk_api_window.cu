@@ -23,10 +23,9 @@ using namespace dfk;
 struct DfkWindow {
   int device = 0;
   WindowDev dev{};
-  // one allocation: kf0_ptr | kf0_items | kf1_ptr | kf1_items | pair_ptr | pair_items | lk0_ptr | lk0_links |
-  // lk1_ptr | lk1_links
-  DeviceBuf<int> ints;
-  DeviceBuf<float> areas;
+  // one allocation: the CSR lists kf0 | kf1 | pair | lk0 | lk1 (ptr | items each), frame_pair, the item areas, and with
+  // keyframe priors their lists (KfPriorDev)
+  DeviceBuf<unsigned char> blob;
   size_t floats = 0;
   // host copy of the structure, for dfk_window_solver_create and dfk_window_marginalize_keyframe
   std::vector<int> pair_k0, pair_k1, link_k0, link_k1, item_pair;
@@ -34,8 +33,6 @@ struct DfkWindow {
   // (blk_i < blk_j) and their device lists (KfPriorDev)
   std::vector<int> prior_ptr{0}, prior_kf, blk_i, blk_j;
   std::vector<long long> prior_off;  // doubles: start of prior q in a priors buffer; back() = the buffer's size
-  DeviceBuf<int> kp_ints;
-  DeviceBuf<long long> kp_off;
   KfPriorDev kp{};
 };
 
@@ -60,35 +57,37 @@ struct DfkWindowProblem {
   size_t S = 0;  // doubles of one state: (K + F) 7 + K C
   StepKernel step;
   SfmLaunchPlan plan;
-  DeviceBuf<SfmItemDev> dense;
-  DeviceBuf<float> dense_codes;
+  // one allocation: the parts create uploads, then the scratch (from dense_codes on, never uploaded)
+  DeviceBuf<unsigned char> blob;
+  Part<SfmItemDev> dense;
+  Part<EvalErrorDesc> err;
+  Part<double> areas;  // W * H of each error item
+  Part<int4> dense_slots, err_slots, rep_slots, geo_slots, depth_slots;
+  Part<DepthDecodeDesc> depth;
+  Part<double> frows, kfrows, x0;  // prior rows, frozen points (frame priors, then kf members)
+  Part<int> fp_lists;              // dfk_window_add_priors' CSR: ptr[K + 1] | prior indices
+  Part<int> delta_kf;              // keyframe of every delta row
+  Part<double> state;              // two states: [cur] the problem's, [1 - cur] an LM candidate
+  Part<float> dense_codes, depth_codes;
+  Part<double> delta;
+  Part<float> err_out;             // (ne + nr + ng) x 2
+  Part<unsigned char> small;       // the LM's read-back block [energy 8 | info | depth-prior energy], mirrored in
+  Part<double> sm_energy, sm_depth_energy;  // small_host; these parts are offsets into it
+  Part<int32_t> sm_info;
+  PinnedBuf<unsigned char> small_host;
+  DeviceBuf<unsigned char> depth_scratch;  // the depth items' decoded depths, one part each
   std::vector<DeviceBuf<float>> rays;
-  DeviceBuf<unsigned char> rep, geo;  // the sparse batches' staged blocks [descriptors | codes | payload]
-  std::vector<unsigned char> rep_host, geo_host;
-  const unsigned char* rep_payload = nullptr;
-  const unsigned char* geo_payload = nullptr;
-  size_t rep_total = 0;
-  DeviceBuf<EvalErrorDesc> err;
-  int err_max_blocks = 1, err_rows = 0;
-  DeviceBuf<unsigned char> depth;  // [descriptors | codes]
-  int depth_max_blocks = 1;
-  DeviceBuf<float> depth_scratch;
-  DeviceBuf<int4> slots;           // dense | error | reproj | geo | depth
-  DeviceBuf<double> areas;         // W * H of each error item
-  DeviceBuf<float> err_out;        // (ne + nr + ng) x 2
-  DeviceBuf<double> state;         // two states: [cur] the problem's, [1 - cur] an LM candidate
+  DeviceBuf<unsigned char> rep, geo;  // the sparse batches' staged blocks
+  Staged<DfkReprojectionItem> rep_st;
+  Staged<DfkSparseGeometricItem> geo_st;
+  int err_max_blocks = 1, err_rows = 0, depth_max_blocks = 1;
   int cur = 0;
-  DeviceBuf<double> frows, kfrows, x0, delta;  // prior rows, frozen points (frame priors, then kf members), deltas
-  DeviceBuf<int> delta_kf;         // keyframe of every delta row
-  DeviceBuf<int> fp_lists;         // dfk_window_add_priors' CSR: ptr[K + 1] | prior indices
   float* records = nullptr;
   float* geo_records = nullptr;
   WindowSolverDev* solver[2] = {nullptr, nullptr};  // [fix_first_pose]
   DeviceBuf<float> bufs;           // the LM's accepted and candidate window buffers
   int acc = 0;
   DeviceBuf<double> dx;
-  DeviceBuf<unsigned char> small;  // [energy 8 doubles | info int32]
-  PinnedBuf<unsigned char> small_host;
   // active subsets (dfk_window_problem_set_active): the create-time dense and error items with their slots and areas
   // are the templates a mask selects from; the selected items go to arrays of their own, so the full arrays stay as
   // create planned them and an all-active mask runs exactly the create-time launches
@@ -107,42 +106,37 @@ struct DfkWindowProblem {
   DeviceBuf<float> sub_records;
   // depth priors (dfk_window_problem_set_depth_priors): ndp priors over ndpi (keyframe, level) items, staged once
   // ([descriptors | codes], the codes rewritten from the state before every batch), and the lists
-  // [add CSR ptr K + 1 | prior indices ndp | level_ptr ndp + 1 | sigma (float bits) ndp | keyframe of every item ndpi]
+  // [add CSR ptr K + 1 | prior indices ndp | level_ptr ndp + 1 | sigma ndp | keyframe of every item ndpi]
   int ndp = 0, ndpi = 0;
   DepthPriorStaged dp_st;
-  size_t dp_lp = 0, dp_sg = 0, dp_kf = 0;
-  DeviceBuf<unsigned char> dp;
-  std::vector<unsigned char> dp_host;
-  DeviceBuf<int> dp_lists;
+  DeviceBuf<unsigned char> dp, dp_lists;
+  Part<int> dp_csr, dp_level_ptr, dp_kf;
+  Part<float> dp_sigma;
   DeviceBuf<float> dp_partials, dp_records, dp_err;
   ~DfkWindowProblem()
   {
     window_solver_destroy(solver[0]);
     window_solver_destroy(solver[1]);
   }
-  double* st(int i) const { return state.ptr + (size_t)i * S; }
-  double* energy() const { return reinterpret_cast<double*>(small.ptr); }
-  int32_t* info() const { return reinterpret_cast<int32_t*>(small.ptr + 8 * sizeof(double)); }
-  double* depth_energy() const { return reinterpret_cast<double*>(small.ptr + 8 * sizeof(double) + 16); }
+  double* st(int i) const { return state.at(blob.ptr) + (size_t)i * S; }
+  double* energy() const { return sm_energy.at(small.at(blob.ptr)); }
+  int32_t* info() const { return sm_info.at(small.at(blob.ptr)); }
+  double* depth_energy() const { return sm_depth_energy.at(small.at(blob.ptr)); }
 };
 
 namespace {
 
-// Appends one CSR list to blob: ptr[keys + 1], then the items of each key in item order (the summation order of the
-// gather kernels); an item whose key is outside [0, keys) is in no list.  Returns where the list starts in blob
+// One CSR list into ptr[keys + 1 + n], zero: ptr[keys + 1], then the items of each key in item order (the summation
+// order of the gather kernels); an item whose key is outside [0, keys) is in no list
 template <class KeyOf>
-size_t add_csr(std::vector<int>& blob, int keys, int n, KeyOf key_of)
+void fill_csr(int* ptr, int keys, int n, KeyOf key_of)
 {
-  const size_t o = blob.size();
-  blob.resize(o + keys + 1 + n, 0);
-  int* ptr = blob.data() + o;
   for (int i = 0; i < n; ++i)
     if (key_of(i) < keys) ptr[key_of(i) + 1] += 1;
   for (int k = 0; k < keys; ++k) ptr[k + 1] += ptr[k];
   std::vector<int> next(ptr, ptr + keys);
   for (int i = 0; i < n; ++i)
     if (key_of(i) < keys) ptr[keys + 1 + next[key_of(i)]++] = i;
-  return o;
 }
 
 // The window buffer from the records: the assemble kernel, then the keyframe-prior blocks set to zero
@@ -159,31 +153,29 @@ DfkStatus assemble_window(DfkHandle h, const DfkWindow* w, const float* records,
 
 WindowReposeDev repose_args(const DfkWindowProblem* p, const double* state)
 {
-  const int4* sl = p->slots.ptr;
+  unsigned char* b = p->blob.ptr;
   WindowReposeDev a{};
   a.code_size = p->C;
   a.num_poses = p->K + p->F;
   a.state = state;
-  a.dense = p->dense.ptr; a.dense_slots = sl; a.num_dense = p->nd;
-  a.error = p->err.ptr; a.error_slots = sl + p->nd; a.num_error = p->ne;
+  a.dense = p->dense.at(b); a.dense_slots = p->dense_slots.at(b); a.num_dense = p->nd;
+  a.error = p->err.at(b); a.error_slots = p->err_slots.at(b); a.num_error = p->ne;
   if (p->sub_dense) {
     a.dense = p->dense_sub.ptr; a.dense_slots = p->sub_slots.ptr; a.num_dense = p->nda;
   }
   if (p->sub_err) {
     a.error = p->err_sub.ptr; a.error_slots = p->sub_slots.ptr + p->nd; a.num_error = p->nea;
   }
-  a.rep = reinterpret_cast<ReprojItemDev*>(p->rep.ptr); a.rep_slots = sl + p->nd + p->ne; a.num_rep = p->nr;
-  a.geo = reinterpret_cast<GeoItemDev*>(p->geo.ptr); a.geo_slots = sl + p->nd + p->ne + p->nr; a.num_geo = p->ng;
-  a.depth = reinterpret_cast<DepthDecodeDesc*>(p->depth.ptr); a.depth_slots = sl + p->nd + p->ne + p->nr + p->ng;
-  a.num_depth = p->ndep;
+  a.rep = p->rep_st.descs.at(p->rep.ptr); a.rep_slots = p->rep_slots.at(b); a.num_rep = p->nr;
+  a.geo = p->geo_st.descs.at(p->geo.ptr); a.geo_slots = p->geo_slots.at(b); a.num_geo = p->ng;
+  a.depth = p->depth.at(b); a.depth_slots = p->depth_slots.at(b); a.num_depth = p->ndep;
   return a;
 }
 
 // the depth priors' batch at `state`: the items' codes from the state, then the records (gram) or the error rows
 DfkStatus problem_depth_priors(DfkHandle h, DfkWindowProblem* p, const double* state, bool gram, const char* what)
 {
-  const int* l = p->dp_lists.ptr;
-  DFK_CUDA(h, launch_depth_prior_codes(state + (size_t)(p->K + p->F) * 7, l + p->dp_kf, p->ndpi, p->C,
+  DFK_CUDA(h, launch_depth_prior_codes(state + (size_t)(p->K + p->F) * 7, p->dp_kf.at(p->dp_lists.ptr), p->ndpi, p->C,
                                        p->dp_st.codes.at(p->dp.ptr), h->stream),
            what);
   DFK_CUDA(h, launch_depth_prior_batch(p->C, p->dp_st.descs.at(p->dp.ptr), p->ndpi, p->dp_st.max_parts, p->avg_dpt,
@@ -195,8 +187,9 @@ DfkStatus problem_depth_priors(DfkHandle h, DfkWindowProblem* p, const double* s
 
 DfkStatus problem_deltas(DfkHandle h, const DfkWindowProblem* p, const double* state)
 {
-  DFK_CUDA(h, launch_window_deltas(state, p->K + p->F, p->C, p->mf + p->nkm, p->delta_kf.ptr, p->x0.ptr, p->delta.ptr,
-                                   h->stream),
+  unsigned char* b = p->blob.ptr;
+  DFK_CUDA(h, launch_window_deltas(state, p->K + p->F, p->C, p->mf + p->nkm, p->delta_kf.at(b), p->x0.at(b),
+                                   p->delta.at(b), h->stream),
            "[WindowProblem] kernel launch failed");
   h->launches += (p->mf + p->nkm) > 0;
   return DFK_OK;
@@ -206,6 +199,7 @@ DfkStatus problem_deltas(DfkHandle h, const DfkWindowProblem* p, const double* s
 DfkStatus problem_linearize(DfkHandle h, DfkWindowProblem* p, const double* state, float* buf)
 {
   const char* what = "[WindowProblem::linearize] kernel launch failed";
+  unsigned char* b = p->blob.ptr;
   DFK_CUDA(h, launch_window_repose(repose_args(p, state), h->stream), what);
   h->launches += 1;
   const float avg = p->avg_dpt;
@@ -223,20 +217,18 @@ DfkStatus problem_linearize(DfkHandle h, DfkWindowProblem* p, const double* stat
   } else if (p->nd > 0) {
     DFK_CUDA(h, h->partials_dev.ensure((size_t)p->plan.num_partials * p->step.pfloats),
              "[WindowProblem::linearize] scratch allocation failed");
-    DFK_TRY(launch_step(h, p->step, p->C, p->dense.ptr, p->nd, p->plan, h->partials_dev.ptr, p->records));
+    DFK_TRY(launch_step(h, p->step, p->C, p->dense.at(b), p->nd, p->plan, h->partials_dev.ptr, p->records));
   }
   if (p->nr > 0) {
-    const float2* q = reinterpret_cast<const float2*>(p->rep_payload);
-    DFK_CUDA(h, launch_reprojection_records(p->C, reinterpret_cast<const ReprojItemDev*>(p->rep.ptr), p->nr, q,
-                                            q + p->rep_total, avg, p->records + (size_t)p->nd * DFK_SFM_RECORD_FLOATS(p->C),
-                                            h->stream),
+    const float2* q = p->rep_st.payload.at(p->rep.ptr);
+    DFK_CUDA(h, launch_reprojection_records(p->C, p->rep_st.descs.at(p->rep.ptr), p->nr, q, q + p->rep_st.total, avg,
+                                            p->records + (size_t)p->nd * DFK_SFM_RECORD_FLOATS(p->C), h->stream),
              what);
     h->launches += 1;
   }
   if (p->ng > 0) {
-    DFK_CUDA(h, launch_sparse_geometric_records(p->C, reinterpret_cast<const GeoItemDev*>(p->geo.ptr), p->ng,
-                                                reinterpret_cast<const int2*>(p->geo_payload), avg, p->geo_records,
-                                                h->stream),
+    DFK_CUDA(h, launch_sparse_geometric_records(p->C, p->geo_st.descs.at(p->geo.ptr), p->ng,
+                                                p->geo_st.payload.at(p->geo.ptr), avg, p->geo_records, h->stream),
              what);
     h->launches += 1;
   }
@@ -244,22 +236,22 @@ DfkStatus problem_linearize(DfkHandle h, DfkWindowProblem* p, const double* stat
   DFK_TRY(assemble_window(h, w, p->records, p->ng > 0 ? p->geo_records : nullptr, buf, what));
   DFK_TRY(problem_deltas(h, p, state));
   if (p->mf > 0) {
-    DFK_CUDA(h, launch_window_add_priors(w->dev, p->mf, p->fp_lists.ptr, p->fp_lists.ptr + p->K + 1, p->frows.ptr,
-                                         p->delta.ptr, buf, h->stream),
+    DFK_CUDA(h, launch_window_add_priors(w->dev, p->mf, p->fp_lists.at(b), p->fp_lists.at(b) + p->K + 1, p->frows.at(b),
+                                         p->delta.at(b), buf, h->stream),
              what);
     h->launches += 1;
   }
   if (w->kp.num_priors > 0) {
-    DFK_CUDA(h, launch_window_add_keyframe_priors(w->dev, w->kp, p->kfrows.ptr, p->delta.ptr + (size_t)p->mf * p->B, buf,
-                                                  h->stream),
+    DFK_CUDA(h, launch_window_add_keyframe_priors(w->dev, w->kp, p->kfrows.at(b), p->delta.at(b) + (size_t)p->mf * p->B,
+                                                  buf, h->stream),
              what);
     h->launches += 1;
   }
   if (p->ndp > 0) {  // after the frame and keyframe priors, as SfmWindowProblem.linearise without an all-reduce
     DFK_TRY(problem_depth_priors(h, p, state, true, what));
-    const int* l = p->dp_lists.ptr;
-    DFK_CUDA(h, launch_window_add_depth_priors(w->dev, p->ndp, l, l + p->K + 1, l + p->dp_lp,
-                                               reinterpret_cast<const float*>(l + p->dp_sg), p->dp_records.ptr, buf,
+    unsigned char* l = p->dp_lists.ptr;
+    DFK_CUDA(h, launch_window_add_depth_priors(w->dev, p->ndp, p->dp_csr.at(l), p->dp_csr.at(l) + p->K + 1,
+                                               p->dp_level_ptr.at(l), p->dp_sigma.at(l), p->dp_records.ptr, buf,
                                                h->stream),
              what);
     h->launches += 1;
@@ -269,22 +261,23 @@ DfkStatus problem_linearize(DfkHandle h, DfkWindowProblem* p, const double* stat
 
 WindowEnergyDev energy_args(const DfkWindowProblem* p, const double* state, double w)
 {
+  unsigned char* b = p->blob.ptr;
   WindowEnergyDev a{};
   a.B = p->B;
-  a.err_out = reinterpret_cast<const float2*>(p->err_out.ptr);
-  a.areas = p->sub_err ? p->areas_sub.ptr : p->areas.ptr;
+  a.err_out = reinterpret_cast<const float2*>(p->err_out.at(b));
+  a.areas = p->sub_err ? p->areas_sub.ptr : p->areas.at(b);
   a.num_error = p->sub_err ? p->nea : p->ne; a.num_rep = p->nr; a.num_geo = p->ng;
-  a.num_frame_priors = p->mf; a.frame_rows = p->frows.ptr; a.frame_delta = p->delta.ptr;
-  a.num_kf_priors = p->w->kp.num_priors; a.kf_rows = p->kfrows.ptr; a.kf_row_off = p->w->kp.off;
-  a.kf_mem_ptr = p->w->kp.mem_ptr; a.kf_delta = p->delta.ptr + (size_t)p->mf * p->B;
+  a.num_frame_priors = p->mf; a.frame_rows = p->frows.at(b); a.frame_delta = p->delta.at(b);
+  a.num_kf_priors = p->w->kp.num_priors; a.kf_rows = p->kfrows.at(b); a.kf_row_off = p->w->kp.off;
+  a.kf_mem_ptr = p->w->kp.mem_ptr; a.kf_delta = p->delta.at(b) + (size_t)p->mf * p->B;
   a.codes = state + (size_t)(p->K + p->F) * 7;
   a.num_codes = p->K * p->C;
   a.code_prior_weight = w;
   a.num_depth_priors = p->ndp;
   if (p->ndp > 0) {
     a.depth_err = reinterpret_cast<const float2*>(p->dp_err.ptr);
-    a.depth_level_ptr = p->dp_lists.ptr + p->dp_lp;
-    a.depth_sigma = reinterpret_cast<const float*>(p->dp_lists.ptr + p->dp_sg);
+    a.depth_level_ptr = p->dp_level_ptr.at(p->dp_lists.ptr);
+    a.depth_sigma = p->dp_sigma.at(p->dp_lists.ptr);
     a.out_depth = p->depth_energy();
   }
   a.out = p->energy();
@@ -295,38 +288,37 @@ WindowEnergyDev energy_args(const DfkWindowProblem* p, const double* state, doub
 DfkStatus problem_error(DfkHandle h, DfkWindowProblem* p, const double* state, double w)
 {
   const char* what = "[WindowProblem::error] kernel launch failed";
+  unsigned char* b = p->blob.ptr;
   DFK_CUDA(h, launch_window_repose(repose_args(p, state), h->stream), what);
   h->launches += 1;
   const float avg = p->avg_dpt;
   if (p->ndep > 0) {
-    DFK_CUDA(h, launch_update_depth(p->C, reinterpret_cast<const DepthDecodeDesc*>(p->depth.ptr), p->ndep,
-                                          p->depth_max_blocks, avg, h->stream),
-             what);
+    DFK_CUDA(h, launch_update_depth(p->C, p->depth.at(b), p->ndep, p->depth_max_blocks, avg, h->stream), what);
     h->launches += 1;
   }
-  float* out = p->err_out.ptr;
+  float* out = p->err_out.at(b);
   // with an active subset only its items are evaluated, and their rows come first (energy_args reads as many)
   const int ne = p->sub_err ? p->nea : p->ne;
   if (ne > 0) {
     const char* sw = "[WindowProblem::error] scratch allocation failed";
     DFK_CUDA(h, h->eval_partials.ensure((size_t)p->err_rows * 32), sw);
     DFK_TRY(ensure_tickets(h, h->eval_counters, (size_t)p->ne, sw, sw));
-    DFK_CUDA(h, launch_eval_error(p->sub_err ? p->err_sub.ptr : p->err.ptr, ne, p->err_max_blocks,
+    DFK_CUDA(h, launch_eval_error(p->sub_err ? p->err_sub.ptr : p->err.at(b), ne, p->err_max_blocks,
                                         p->huber_delta, h->eval_partials.ptr, h->eval_counters.ptr, out, h->stream),
              what);
     h->launches += 1;
   }
   if (p->nr > 0) {
-    const float2* q = reinterpret_cast<const float2*>(p->rep_payload);
-    DFK_CUDA(h, launch_reprojection_error(p->C, reinterpret_cast<const ReprojItemDev*>(p->rep.ptr), p->nr, q,
-                                          q + p->rep_total, avg, out + 2 * (size_t)ne, h->stream),
+    const float2* q = p->rep_st.payload.at(p->rep.ptr);
+    DFK_CUDA(h, launch_reprojection_error(p->C, p->rep_st.descs.at(p->rep.ptr), p->nr, q, q + p->rep_st.total, avg,
+                                          out + 2 * (size_t)ne, h->stream),
              what);
     h->launches += 1;
   }
   if (p->ng > 0) {
-    DFK_CUDA(h, launch_sparse_geometric_error(p->C, reinterpret_cast<const GeoItemDev*>(p->geo.ptr), p->ng,
-                                              reinterpret_cast<const int2*>(p->geo_payload), avg,
-                                              out + 2 * (size_t)(ne + p->nr), h->stream),
+    DFK_CUDA(h, launch_sparse_geometric_error(p->C, p->geo_st.descs.at(p->geo.ptr), p->ng,
+                                              p->geo_st.payload.at(p->geo.ptr), avg, out + 2 * (size_t)(ne + p->nr),
+                                              h->stream),
              what);
     h->launches += 1;
   }
@@ -432,9 +424,9 @@ struct ProblemLMOps {
       DFK_CUDA(h, launch_window_energy(a, h->stream), "[WindowLM] kernel launch failed");
       h->launches += 1;
     }
-    DFK_TRY(download(h, p->small_host.ptr, p->energy(), 8 * sizeof(double), "[WindowLM] read-back failed",
-                     "[WindowLM] kernel failed"));
-    *f = reinterpret_cast<const double*>(p->small_host.ptr)[7];
+    double* e = p->sm_energy.at(p->small_host.ptr);
+    DFK_TRY(download(h, e, p->energy(), 8 * sizeof(double), "[WindowLM] read-back failed", "[WindowLM] kernel failed"));
+    *f = e[7];
     return DFK_OK;
   }
   DfkStatus solve(double lam, int* info)
@@ -442,9 +434,9 @@ struct ProblemLMOps {
     DFK_CUDA(h, launch_window_solve(solver, buf(false), lam, w, p->st(p->cur) + (size_t)(p->K + p->F) * 7, p->dx.ptr,
                                     p->info(), h->stream, &h->launches, true),
              "[WindowLM] solve launch failed");
-    DFK_TRY(download(h, p->small_host.ptr, p->info(), sizeof(int32_t), "[WindowLM] read-back failed",
-                     "[WindowLM] solve failed"));
-    *info = *reinterpret_cast<const int32_t*>(p->small_host.ptr);
+    int32_t* i = p->sm_info.at(p->small_host.ptr);
+    DFK_TRY(download(h, i, p->info(), sizeof(int32_t), "[WindowLM] read-back failed", "[WindowLM] solve failed"));
+    *info = *i;
     return DFK_OK;
   }
   DfkStatus retract()
@@ -574,66 +566,77 @@ DfkStatus dfk_window_create_priors(DfkHandle h, const DfkWindowDesc* d, int L, c
     std::sort(blocks.begin(), blocks.end());
     blocks.erase(std::unique(blocks.begin(), blocks.end()), blocks.end());
     const int NB = (int)blocks.size();
-    std::vector<std::vector<int>> kf_ent(K), blk_ent(NB);
+    std::vector<std::vector<int2>> kf_ent(K);
+    std::vector<std::vector<int3>> blk_ent(NB);
+    size_t num_blk_ent = 0;
     for (int q = 0; q < Q; ++q)
       for (int a = prior_ptr[q]; a < prior_ptr[q + 1]; ++a) {
-        kf_ent[prior_kf[a]].insert(kf_ent[prior_kf[a]].end(), {q, a - prior_ptr[q]});
-        for (int c = a + 1; c < prior_ptr[q + 1]; ++c) {
+        kf_ent[prior_kf[a]].push_back(make_int2(q, a - prior_ptr[q]));
+        for (int c = a + 1; c < prior_ptr[q + 1]; ++c, ++num_blk_ent) {
           const int b = (int)(std::lower_bound(blocks.begin(), blocks.end(), std::make_pair(prior_kf[a], prior_kf[c])) -
                               blocks.begin());
-          blk_ent[b].insert(blk_ent[b].end(), {q, a - prior_ptr[q], c - prior_ptr[q]});
+          blk_ent[b].push_back(make_int3(q, a - prior_ptr[q], c - prior_ptr[q]));
         }
       }
-    std::vector<int> kp_blob(Q + 1, 0);  // mem_ptr
-    for (int q = 0; q < Q; ++q) kp_blob[q + 1] = prior_ptr[q + 1];
-    const size_t o_kfp = kp_blob.size();
-    kp_blob.push_back(0);
-    for (int k = 0; k < K; ++k) kp_blob.push_back(kp_blob[o_kfp + k] + (int)kf_ent[k].size() / 2);
-    const size_t o_bp = kp_blob.size();
-    kp_blob.push_back(0);
-    for (int b = 0; b < NB; ++b) kp_blob.push_back(kp_blob[o_bp + b] + (int)blk_ent[b].size() / 3);
-    kp_blob.resize((kp_blob.size() + 3) & ~(size_t)3, 0);  // int2 / int3 entries 16-byte aligned
-    const size_t o_ke = kp_blob.size();
-    for (int k = 0; k < K; ++k) kp_blob.insert(kp_blob.end(), kf_ent[k].begin(), kf_ent[k].end());
-    kp_blob.resize((kp_blob.size() + 3) & ~(size_t)3, 0);
-    const size_t o_be = kp_blob.size();
-    for (int b = 0; b < NB; ++b) kp_blob.insert(kp_blob.end(), blk_ent[b].begin(), blk_ent[b].end());
     std::vector<long long> poff(Q + 1, 0);
     for (int q = 0; q < Q; ++q)
       poff[q + 1] = poff[q] + (long long)DFK_KF_PRIOR_DOUBLES(d->code_size, prior_ptr[q + 1] - prior_ptr[q]);
-    // one CSR list per key kind (keyframe k0, frame k1, pair, and the links' keyframes)
-    std::vector<int> blob;
-    const size_t o_kf0 = add_csr(blob, K, n, [&](int i) { return d->pair_k0[d->item_pair[i]]; });
+    // one CSR list per key kind (keyframe k0, frame k1, pair, and the links' keyframes), frame_pair, the item areas
+    Staging s(h->staging);
+    const Part<int> kf0 = s.add<int>(K + 1 + n), kf1 = s.add<int>(K + 1 + n), pair = s.add<int>(P + 1 + n);
+    const Part<int> lk0 = s.add<int>(K + 1 + L), lk1 = s.add<int>(K + 1 + L), fr = s.add<int>(F);
+    const Part<float> areas = s.add<float>(n);
+    Part<int> mem_ptr, kf_ptr, blk_ptr;
+    Part<int2> kfe;
+    Part<int3> bke;
+    Part<long long> off;
+    if (Q > 0) {
+      mem_ptr = s.add<int>(Q + 1); kf_ptr = s.add<int>(K + 1); blk_ptr = s.add<int>(NB + 1);
+      kfe = s.add<int2>(M); bke = s.add<int3>(num_blk_ent); off = s.add<long long>(Q + 1);
+    }
+    unsigned char* hb = s.host();
+    fill_csr(kf0.at(hb), K, n, [&](int i) { return d->pair_k0[d->item_pair[i]]; });
     // a frame pair's pose1 is the frame's: its items go to the frame's block, not to a keyframe's
-    const size_t o_kf1 = add_csr(blob, K, n, [&](int i) { return d->pair_k1[d->item_pair[i]]; });
-    const size_t o_pair = add_csr(blob, P, n, [&](int i) { return d->item_pair[i]; });
-    const size_t o_lk0 = add_csr(blob, K, L, [&](int l) { return link_k0[l]; });
-    const size_t o_lk1 = add_csr(blob, K, L, [&](int l) { return link_k1[l]; });
-    const size_t o_fr = blob.size();
-    blob.insert(blob.end(), frame_pair.begin(), frame_pair.end());
-    std::vector<float> areas(n);
-    for (int i = 0; i < n; ++i) areas[i] = (float)d->item_width[i] * (float)d->item_height[i];
+    fill_csr(kf1.at(hb), K, n, [&](int i) { return d->pair_k1[d->item_pair[i]]; });
+    fill_csr(pair.at(hb), P, n, [&](int i) { return d->item_pair[i]; });
+    fill_csr(lk0.at(hb), K, L, [&](int l) { return link_k0[l]; });
+    fill_csr(lk1.at(hb), K, L, [&](int l) { return link_k1[l]; });
+    std::copy(frame_pair.begin(), frame_pair.end(), fr.at(hb));
+    for (int i = 0; i < n; ++i) areas.at(hb)[i] = (float)d->item_width[i] * (float)d->item_height[i];
+    if (Q > 0) {
+      std::copy(prior_ptr, prior_ptr + Q + 1, mem_ptr.at(hb));
+      int2* ke = kfe.at(hb);
+      for (int k = 0; k < K; ++k) {
+        kf_ptr.at(hb)[k + 1] = kf_ptr.at(hb)[k] + (int)kf_ent[k].size();
+        ke = std::copy(kf_ent[k].begin(), kf_ent[k].end(), ke);
+      }
+      int3* be = bke.at(hb);
+      for (int b = 0; b < NB; ++b) {
+        blk_ptr.at(hb)[b + 1] = blk_ptr.at(hb)[b] + (int)blk_ent[b].size();
+        be = std::copy(blk_ent[b].begin(), blk_ent[b].end(), be);
+      }
+      std::copy(poff.begin(), poff.end(), off.at(hb));
+    }
 
     DeviceGuard guard(h->device);
     std::unique_ptr<DfkWindow> w(new (std::nothrow) DfkWindow());  // freed under the guard if the upload fails
     if (!w) return oom(h);
     w->device = h->device;
     const char* upload_failed = "[Window] index upload failed";
-    DFK_CUDA(h, w->ints.ensure(blob.size()), upload_failed);
-    DFK_CUDA(h, w->areas.ensure(areas.size()), upload_failed);
-    DFK_CUDA(h, cudaMemcpy(w->ints.ptr, blob.data(), blob.size() * sizeof(int), cudaMemcpyHostToDevice), upload_failed);
-    DFK_CUDA(h, cudaMemcpy(w->areas.ptr, areas.data(), areas.size() * sizeof(float), cudaMemcpyHostToDevice), upload_failed);
-    const int* ints = w->ints.ptr;
+    // synchronous: the window may be used from any stream on its device
+    DFK_CUDA(h, w->blob.ensure(s.bytes), upload_failed);
+    DFK_CUDA(h, cudaMemcpy(w->blob.ptr, hb, s.bytes, cudaMemcpyHostToDevice), upload_failed);
+    unsigned char* b = w->blob.ptr;
     w->dev.num_keyframes = K; w->dev.num_pairs = P; w->dev.num_items = n; w->dev.code_size = d->code_size;
-    w->dev.kf0_ptr = ints + o_kf0; w->dev.kf0_items = ints + o_kf0 + K + 1;
-    w->dev.kf1_ptr = ints + o_kf1; w->dev.kf1_items = ints + o_kf1 + K + 1;
-    w->dev.pair_ptr = ints + o_pair; w->dev.pair_items = ints + o_pair + P + 1;
-    w->dev.item_area = w->areas.ptr;
+    w->dev.kf0_ptr = kf0.at(b); w->dev.kf0_items = kf0.at(b) + K + 1;
+    w->dev.kf1_ptr = kf1.at(b); w->dev.kf1_items = kf1.at(b) + K + 1;
+    w->dev.pair_ptr = pair.at(b); w->dev.pair_items = pair.at(b) + P + 1;
+    w->dev.item_area = areas.at(b);
     w->dev.num_links = L;
-    w->dev.lk0_ptr = ints + o_lk0; w->dev.lk0_links = ints + o_lk0 + K + 1;
-    w->dev.lk1_ptr = ints + o_lk1; w->dev.lk1_links = ints + o_lk1 + K + 1;
+    w->dev.lk0_ptr = lk0.at(b); w->dev.lk0_links = lk0.at(b) + K + 1;
+    w->dev.lk1_ptr = lk1.at(b); w->dev.lk1_links = lk1.at(b) + K + 1;
     w->dev.num_frames = F;
-    w->dev.frame_pair = ints + o_fr;
+    w->dev.frame_pair = fr.at(b);
     const size_t B = 6 + (size_t)d->code_size;
     const size_t block_off = (size_t)K * (B * B + B) + (size_t)P * 6 * B + 2 + (size_t)L * B * B + (size_t)F * 42;
     w->floats = block_off + (size_t)NB * B * B;
@@ -650,17 +653,10 @@ DfkStatus dfk_window_create_priors(DfkHandle h, const DfkWindowDesc* d, int L, c
         w->blk_j.push_back(b.second);
       }
       w->prior_off = poff;
-      DFK_CUDA(h, w->kp_ints.ensure(kp_blob.size()), upload_failed);
-      DFK_CUDA(h, w->kp_off.ensure(poff.size()), upload_failed);
-      DFK_CUDA(h, cudaMemcpy(w->kp_ints.ptr, kp_blob.data(), kp_blob.size() * sizeof(int), cudaMemcpyHostToDevice),
-               upload_failed);
-      DFK_CUDA(h, cudaMemcpy(w->kp_off.ptr, poff.data(), poff.size() * sizeof(long long), cudaMemcpyHostToDevice),
-               upload_failed);
-      const int* kpi = w->kp_ints.ptr;
       w->kp.num_priors = Q; w->kp.num_blocks = NB; w->kp.block_off = block_off;
-      w->kp.mem_ptr = kpi; w->kp.off = w->kp_off.ptr;
-      w->kp.kf_ptr = kpi + o_kfp; w->kp.kf_ent = reinterpret_cast<const int2*>(kpi + o_ke);
-      w->kp.blk_ptr = kpi + o_bp; w->kp.blk_ent = reinterpret_cast<const int3*>(kpi + o_be);
+      w->kp.mem_ptr = mem_ptr.at(b); w->kp.off = off.at(b);
+      w->kp.kf_ptr = kf_ptr.at(b); w->kp.kf_ent = kfe.at(b);
+      w->kp.blk_ptr = blk_ptr.at(b); w->kp.blk_ent = bke.at(b);
     }
     *out = w.release();
     return DFK_OK;
@@ -744,8 +740,8 @@ DfkStatus dfk_window_add_priors(DfkHandle h, const DfkWindow* w, int m, const in
                                                 " names a keyframe outside the window");
     if (m == 0) return DFK_OK;
     // CSR of the priors per keyframe, in list order: ptr[K + 1] | indices[m]
-    std::vector<int> lists;
-    add_csr(lists, K, m, [&](int i) { return prior_kf_host[i]; });
+    std::vector<int> lists(K + 1 + m, 0);
+    fill_csr(lists.data(), K, m, [&](int i) { return prior_kf_host[i]; });
     DeviceGuard guard(h->device);
     const char* what = "[Window::AddPriors] index upload failed";
     DFK_CUDA(h, h->window_lists.ensure(lists.size()), what);
@@ -785,12 +781,10 @@ DfkStatus dfk_window_add_depth_priors(DfkHandle h, const DfkWindow* w, int m, co
     }
     if (m == 0) return DFK_OK;
     // [CSR of the priors per keyframe: ptr[K + 1] | indices m] | level_ptr[m + 1] | sigma[m]
-    std::vector<int> csr;
-    add_csr(csr, K, m, [&](int i) { return prior_kf_host[i]; });
     Staging s(h->staging);
-    const Part<int> csr_at = s.add<int>(csr.size()), lp_at = s.add<int>(m + 1);
+    const Part<int> csr_at = s.add<int>(K + 1 + m), lp_at = s.add<int>(m + 1);
     const Part<float> sg_at = s.add<float>(m);
-    memcpy(csr_at.at(s.host()), csr.data(), sizeof(int) * csr.size());
+    fill_csr(csr_at.at(s.host()), K, m, [&](int i) { return prior_kf_host[i]; });
     memcpy(lp_at.at(s.host()), level_ptr_host, sizeof(int) * (m + 1));
     memcpy(sg_at.at(s.host()), sigma_host, sizeof(float) * m);
     DeviceGuard guard(h->device);
@@ -907,64 +901,58 @@ DfkStatus dfk_window_marginalize_keyframe(DfkHandle h, const DfkWindow* w, const
     std::vector<int> loc(K, -1);
     loc[m] = 0;
     for (int i = 0; i < n; ++i) loc[nb[i]] = 1 + i;
-    // [refs | tile_row | tile_col | mem_loc | pad | update tasks]
-    std::vector<int> lists;
+    std::vector<KfMargRef> refs;
     for (size_t i = 0; i < w->item_pair.size(); ++i) {
       const int k0 = w->pair_k0[w->item_pair[i]], k1 = w->pair_k1[w->item_pair[i]];
-      if (k1 < K && (k0 == m || k1 == m)) lists.insert(lists.end(), {0, (int)i, loc[k0], loc[k1]});
+      if (k1 < K && (k0 == m || k1 == m)) refs.push_back({0, (int)i, loc[k0], loc[k1]});
     }
     for (size_t l = 0; l < w->link_k0.size(); ++l)
-      if (w->link_k0[l] == m || w->link_k1[l] == m)
-        lists.insert(lists.end(), {1, (int)l, loc[w->link_k0[l]], loc[w->link_k1[l]]});
-    for (int i = 0; i < num_frame_priors; ++i) lists.insert(lists.end(), {2, i, 0, 0});
-    for (int q : kq) lists.insert(lists.end(), {3, q, 0, 0});
-    const int num_refs = (int)lists.size() / 4;
+      if (w->link_k0[l] == m || w->link_k1[l] == m) refs.push_back({1, (int)l, loc[w->link_k0[l]], loc[w->link_k1[l]]});
+    for (int i = 0; i < num_frame_priors; ++i) refs.push_back({2, i, 0, 0});
+    for (int q : kq) refs.push_back({3, q, 0, 0});
     const int T = n + 1 + n * (n + 1) / 2;
-    const size_t o_tr = lists.size();
-    for (int t = 0; t <= n; ++t) lists.push_back(t);
-    for (int I = 1; I <= n; ++I)
-      for (int J = 1; J <= I; ++J) lists.push_back(I);
-    const size_t o_tc = lists.size();
-    for (int t = 0; t <= n; ++t) lists.push_back(0);
-    for (int I = 1; I <= n; ++I)
-      for (int J = 1; J <= I; ++J) lists.push_back(J);
-    const size_t o_ml = lists.size();
-    for (int kf : w->prior_kf) lists.push_back(loc[kf]);
-    lists.resize((lists.size() + 3) & ~(size_t)3, 0);
-    const size_t o_tk = lists.size();
     std::vector<int> tasks;
     window_eliminate_first_tasks(n, tasks);
-    lists.insert(lists.end(), tasks.begin(), tasks.end());
-    const size_t ws = (size_t)(T + 1) * B * B + (size_t)(n + 1) * B + 1;
+    const bool code = code_prior_weight > 0.0;
+    // [refs | tile_row | tile_col | mem_loc | update tasks | code of m], and the workspace [tiles | rhs | f]
+    Staging s(h->staging);
+    const Part<KfMargRef> refs_at = s.add<KfMargRef>(refs.size());
+    const Part<int> tr = s.add<int>(T), tc = s.add<int>(T), ml = s.add<int>(w->prior_kf.size());
+    const Part<int> tk = s.add<int>(tasks.size());
+    const Part<double> code_at = s.add<double>(code ? C : 0);
+    unsigned char* hb = s.host();
+    std::copy(refs.begin(), refs.end(), refs_at.at(hb));
+    for (int t = 0; t <= n; ++t) tr.at(hb)[t] = t;  // tile_col 0
+    for (int I = 1, t = n + 1; I <= n; ++I)
+      for (int J = 1; J <= I; ++J, ++t) {
+        tr.at(hb)[t] = I;
+        tc.at(hb)[t] = J;
+      }
+    for (size_t a = 0; a < w->prior_kf.size(); ++a) ml.at(hb)[a] = loc[w->prior_kf[a]];
+    std::copy(tasks.begin(), tasks.end(), tk.at(hb));
+    if (code) memcpy(code_at.at(hb), code_m_host, C * sizeof(double));
+    Layout ws;
+    const Part<double> tiles = ws.add<double>((size_t)(T + 1) * B * B), rhs = ws.add<double>((size_t)(n + 1) * B);
+    const Part<double> f = ws.add<double>(1);
 
     DeviceGuard guard(h->device);
-    const char* alloc = "[Window::MarginalizeKeyframe] scratch allocation failed";
-    DFK_CUDA(h, h->marg_lists.ensure(lists.size()), alloc);
-    DFK_CUDA(h, h->marg_dev.ensure(ws), alloc);
-    DFK_CUDA(h, h->marg_code.ensure(C), alloc);
-    // pageable sources: staged before the call returns
-    DFK_CUDA(h, cudaMemcpyAsync(h->marg_lists.ptr, lists.data(), lists.size() * sizeof(int), cudaMemcpyHostToDevice,
-                                h->stream), alloc);
-    if (code_prior_weight > 0.0)
-      DFK_CUDA(h, cudaMemcpyAsync(h->marg_code.ptr, code_m_host, C * sizeof(double), cudaMemcpyHostToDevice, h->stream),
-               alloc);
-    const int* li = h->marg_lists.ptr;
+    DFK_CUDA(h, h->marg_dev.ensure(ws.bytes), "[Window::MarginalizeKeyframe] scratch allocation failed");
+    DFK_TRY(s.upload(h, h->marg_lists, what));  // pageable source: staged before the call returns
+    unsigned char* li = h->marg_lists.ptr;
     KfMargDev md{};
     md.n = n;
-    md.num_refs = num_refs;
-    md.refs = reinterpret_cast<const KfMargRef*>(li);
-    md.tile_row = li + o_tr; md.tile_col = li + o_tc; md.mem_loc = li + o_ml;
+    md.num_refs = (int)refs.size();
+    md.refs = refs_at.at(li);
+    md.tile_row = tr.at(li); md.tile_col = tc.at(li); md.mem_loc = ml.at(li);
     md.records = records_dev; md.geo = geo_records_dev;
     md.fpriors = frame_priors_dev; md.fdelta = frame_delta_dev;
     md.kpriors = kf_priors_dev; md.kdelta = kf_delta_dev;
-    md.w = code_prior_weight; md.code = h->marg_code.ptr;
-    md.tiles = h->marg_dev.ptr;
-    md.rhs = md.tiles + (size_t)(T + 1) * B * B;
-    md.f = md.rhs + (size_t)(n + 1) * B;
+    md.w = code_prior_weight; md.code = code_at.at(li);
+    md.tiles = tiles.at(h->marg_dev.ptr); md.rhs = rhs.at(h->marg_dev.ptr); md.f = f.at(h->marg_dev.ptr);
     md.info = info_dev;
     const char* launch = "[Window::MarginalizeKeyframe] kernel launch failed";
     DFK_CUDA(h, launch_window_marg_gather(w->dev, w->kp, md, T, h->stream), launch);
-    DFK_CUDA(h, launch_window_eliminate_first(C, n, md.tiles, md.rhs, info_dev, li + o_tk, (int)tasks.size() / 4,
+    DFK_CUDA(h, launch_window_eliminate_first(C, n, md.tiles, md.rhs, info_dev, tk.at(li), (int)tasks.size() / 4,
                                               h->stream), launch);
     DFK_CUDA(h, launch_window_marg_finalize(C, md, T, prior_dev, h->stream), launch);
     h->launches += 4;
@@ -1108,19 +1096,46 @@ DfkStatus dfk_window_problem_create(DfkHandle h, const DfkWindowProblemDesc* d, 
     p->huber_delta = h->params.sfmparams.huber_delta;
     p->records = d->records_dev; p->geo_records = d->geo_records_dev;
     const char* amsg = "[WindowProblem] allocation failed";
+    const size_t PD = DFK_PRIOR_DOUBLES(C), X = 7 + (size_t)C, nx = (size_t)mf + nkm;  // nx: frozen points
+    // ---- one allocation: the parts create uploads, staged in a host image of the problem's own (the sparse batches
+    // below stage through h->staging), then the scratch
+    std::vector<unsigned char> image;
+    Staging s(image);
+    p->dense = s.add<SfmItemDev>(nd);
+    p->err = s.add<EvalErrorDesc>(ne);
+    p->areas = s.add<double>(ne);
+    p->dense_slots = s.add<int4>(nd); p->err_slots = s.add<int4>(ne); p->rep_slots = s.add<int4>(nr);
+    p->geo_slots = s.add<int4>(ng); p->depth_slots = s.add<int4>(ndep);
+    p->depth = s.add<DepthDecodeDesc>(ndep);
+    p->frows = s.add<double>(mf * PD);
+    p->fp_lists = s.add<int>(mf > 0 ? K + 1 + mf : 0);
+    p->kfrows = s.add<double>(w->kp.num_priors > 0 ? (size_t)w->prior_off.back() : 0);
+    p->delta_kf = s.add<int>(nx);
+    p->x0 = s.add<double>(nx * X);
+    p->state = s.add<double>(2 * p->S);
+    Layout scratch{s.bytes};
+    p->dense_codes = scratch.add<float>((size_t)nd * C);
+    p->depth_codes = scratch.add<float>((size_t)ndep * C);  // the repose kernel writes them from the state
+    p->delta = scratch.add<double>(nx * B);
+    p->err_out = scratch.add<float>(std::max<size_t>(1, 2 * (size_t)(ne + nr + ng)));
+    Layout sm;
+    p->sm_energy = sm.add<double>(8); p->sm_info = sm.add<int32_t>(1); p->sm_depth_energy = sm.add<double>(1);
+    p->small = scratch.add<unsigned char>(sm.bytes);
+    DFK_CUDA(h, p->blob.ensure(scratch.bytes), amsg);
+    DFK_CUDA(h, p->small_host.ensure(sm.bytes), amsg);
+    unsigned char *const hb = s.host(), *const db = p->blob.ptr;
     const std::vector<float> zero_code(std::max(C, 1), 0.0f);
     // ---- dense items: the batch's checks, kernel choice and tile plan, with a code slot of the problem's own each
     if (nd > 0) {
       std::vector<DfkSfmWorkItem> t(d->dense, d->dense + nd);
       for (auto& it : t) it.code = zero_code.data();
       DFK_TRY(choose_step_kernel(h, t.data(), nd, C, &p->step));
-      DFK_CUDA(h, p->dense_codes.ensure((size_t)nd * C), amsg);
-      std::vector<SfmItemDev> items(nd);
-      DFK_TRY(build_items(h, t.data(), nd, C, p->step.tile_px, p->step.max_ctas, p->dense_codes.ptr, items.data(),
-                          &p->plan));
+      SfmItemDev* items = p->dense.at(hb);
+      DFK_TRY(build_items(h, t.data(), nd, C, p->step.tile_px, p->step.max_ctas, p->dense_codes.at(db), items, &p->plan));
       // ray tables of its own, not the handle's cache: the cache may flush (and free) its tables
       std::vector<const SfmItemDev*> owner;
-      for (auto& it : items) {
+      for (int i = 0; i < nd; ++i) {
+        SfmItemDev& it = items[i];
         size_t r = 0;
         for (; r < owner.size(); ++r) {
           const SfmItemDev& o = *owner[r];
@@ -1135,145 +1150,92 @@ DfkStatus dfk_window_problem_create(DfkHandle h, const DfkWindowProblemDesc* d, 
         }
         it.ray_tab = p->rays[r].ptr;
       }
-      p->dense_tmpl = items;
-      DFK_CUDA(h, p->dense.ensure(nd), amsg);
-      DFK_CUDA(h, cudaMemcpyAsync(p->dense.ptr, items.data(), sizeof(SfmItemDev) * nd, cudaMemcpyHostToDevice, h->stream),
-               "[WindowProblem] upload failed");
-      DFK_CUDA(h, launch_sfm_ray_tables(p->dense.ptr, nd, h->stream), "[WindowProblem] kernel launch failed");
-      h->launches += 1;
+      p->dense_tmpl.assign(items, items + nd);
     }
     // ---- sparse links: the batches' checks and staging, into blocks of the problem's own
     if (nr > 0) {
       std::vector<DfkReprojectionItem> t(d->reproj, d->reproj + nr);
       for (auto& it : t) it.code = zero_code.data();
-      Staged st;
-      DFK_TRY(stage(h, what + "reprojection ", true, t.data(), nr, C, 0, p->rep_host, p->rep, &st));
-      p->rep_payload = st.payload;
-      p->rep_total = st.total;
+      DFK_TRY(stage(h, what + "reprojection ", true, t.data(), nr, C, 0, h->staging, p->rep, &p->rep_st));
     }
     if (ng > 0) {
       std::vector<DfkSparseGeometricItem> t(d->geo, d->geo + ng);
       for (auto& it : t) it.code0 = it.code1 = zero_code.data();
-      Staged st;
-      DFK_TRY(stage(h, what + "geometric ", true, t.data(), ng, C, 0, p->geo_host, p->geo, &st));
-      p->geo_payload = st.payload;
+      DFK_TRY(stage(h, what + "geometric ", true, t.data(), ng, C, 0, h->staging, p->geo, &p->geo_st));
     }
     // ---- the error path: depth decodes into scratch of the problem's own, and the error items reading it
-    std::vector<size_t> dep_off(ndep + 1, 0);
+    Layout dl;
+    std::vector<Part<float>> dep(ndep);
     for (int i = 0; i < ndep; ++i) {
       const DfkDepthDecodeItem& it = d->depth[i];
       const uint32_t W = it.dpt.width, H = it.dpt.height;
       if (W == 0 || H == 0 || !img_ok(&it.prx_orig, W, H, 1) || !img_ok(&it.prx_jac, W, H, C))
         return fail(h, DFK_ERR_INVALID_ARG, what + "inconsistent image views in depth item " + std::to_string(i));
-      dep_off[i + 1] = dep_off[i] + (((size_t)W * H + 3) & ~(size_t)3);
+      dep[i] = dl.add<float>((size_t)W * H);
     }
     if (ndep > 0) {
-      DFK_CUDA(h, p->depth_scratch.ensure(dep_off[ndep]), amsg);
-      Staging s(h->staging);
-      const Part<DepthDecodeDesc> descs = s.add<DepthDecodeDesc>(ndep);
-      const Part<float> codes = s.add<float>((size_t)ndep * C);
-      DFK_CUDA(h, p->depth.ensure(s.bytes), amsg);
+      DFK_CUDA(h, p->depth_scratch.ensure(dl.bytes), amsg);
       for (int i = 0; i < ndep; ++i) {
         const DfkDepthDecodeItem& it = d->depth[i];
-        set_depth_decode_desc(descs.at(s.host())[i], it, C, codes.at(p->depth.ptr) + (size_t)i * C,
-                              p->depth_scratch.ptr + dep_off[i], it.dpt.width, &p->depth_max_blocks);
+        set_depth_decode_desc(p->depth.at(hb)[i], it, C, p->depth_codes.at(db) + (size_t)i * C,
+                              dep[i].at(p->depth_scratch.ptr), it.dpt.width, &p->depth_max_blocks);
       }
-      DFK_CUDA(h, cudaMemcpyAsync(p->depth.ptr, s.host(), s.bytes, cudaMemcpyHostToDevice, h->stream),
-               "[WindowProblem] upload failed");
     }
-    if (ne > 0) {
-      std::vector<EvalErrorDesc> descs(ne);
-      std::vector<double> areas(ne);
-      for (int i = 0; i < ne; ++i) {
-        const DfkSfmWorkItem& it = d->error[i];
-        const DfkDepthDecodeItem& dep = d->depth[d->error_depth[i]];
-        const DfkImage dpt{p->depth_scratch.ptr + dep_off[d->error_depth[i]], (size_t)dep.dpt.width * 4, dep.dpt.width,
-                           dep.dpt.height};
-        const uint32_t W = it.img0.width, H = it.img0.height;
-        if (it.code)
-          return fail(h, DFK_ERR_INVALID_ARG, what + "error item " + std::to_string(i) +
-                                                  ": no fused depth decode (the depth comes from its depth item)");
-        if (W == 0 || H == 0 || !img_ok(&it.img0, W, H, 1) || !img_ok(&it.img1, W, H, 1) || !img_ok(&dpt, W, H, 1))
-          return fail(h, DFK_ERR_INVALID_ARG, what + "inconsistent image views in error item " + std::to_string(i));
-        if (!cam_ok(&it.cam, W, H))
-          return fail(h, DFK_ERR_INVALID_ARG, what + "camera viewport larger than the image views in error item " +
-                                                  std::to_string(i));
-        const float ident[7] = {0, 0, 0, 1, 0, 0, 0};  // the repose kernel sets the relative pose
-        set_eval_error_desc(descs[i], it.cam, ident, it.img0, it.img1, dpt, &p->err_rows, &p->err_max_blocks);
-        areas[i] = (double)W * (double)H;
-      }
-      DFK_CUDA(h, p->err.ensure(ne), amsg);
-      DFK_CUDA(h, p->areas.ensure(ne), amsg);
-      DFK_CUDA(h, cudaMemcpyAsync(p->err.ptr, descs.data(), sizeof(EvalErrorDesc) * ne, cudaMemcpyHostToDevice, h->stream),
-               "[WindowProblem] upload failed");
-      DFK_CUDA(h, cudaMemcpyAsync(p->areas.ptr, areas.data(), sizeof(double) * ne, cudaMemcpyHostToDevice, h->stream),
-               "[WindowProblem] upload failed");
-      p->err_tmpl = descs;
-      p->areas_tmpl = areas;
+    for (int i = 0; i < ne; ++i) {
+      const DfkSfmWorkItem& it = d->error[i];
+      const DfkDepthDecodeItem& dep_it = d->depth[d->error_depth[i]];
+      const DfkImage dpt{dep[d->error_depth[i]].at(p->depth_scratch.ptr), (size_t)dep_it.dpt.width * 4,
+                         dep_it.dpt.width, dep_it.dpt.height};
+      const uint32_t W = it.img0.width, H = it.img0.height;
+      if (it.code)
+        return fail(h, DFK_ERR_INVALID_ARG, what + "error item " + std::to_string(i) +
+                                                ": no fused depth decode (the depth comes from its depth item)");
+      if (W == 0 || H == 0 || !img_ok(&it.img0, W, H, 1) || !img_ok(&it.img1, W, H, 1) || !img_ok(&dpt, W, H, 1))
+        return fail(h, DFK_ERR_INVALID_ARG, what + "inconsistent image views in error item " + std::to_string(i));
+      if (!cam_ok(&it.cam, W, H))
+        return fail(h, DFK_ERR_INVALID_ARG, what + "camera viewport larger than the image views in error item " +
+                                                std::to_string(i));
+      const float ident[7] = {0, 0, 0, 1, 0, 0, 0};  // the repose kernel sets the relative pose
+      set_eval_error_desc(p->err.at(hb)[i], it.cam, ident, it.img0, it.img1, dpt, &p->err_rows, &p->err_max_blocks);
+      p->areas.at(hb)[i] = (double)W * (double)H;
     }
-    DFK_CUDA(h, p->err_out.ensure(std::max<size_t>(1, 2 * (size_t)(ne + nr + ng))), amsg);
-    // ---- slots, in the repose kernel's order
-    std::vector<int4> slots;
-    auto push = [&](const DfkWindowItemSlots* s, int n) {
-      for (int i = 0; i < n; ++i) slots.push_back(make_int4(s[i].pose0, s[i].pose1, s[i].code0, s[i].code1));
+    p->err_tmpl.assign(p->err.at(hb), p->err.at(hb) + ne);
+    p->areas_tmpl.assign(p->areas.at(hb), p->areas.at(hb) + ne);
+    // ---- slots, one part per kind
+    auto put_slots = [&](Part<int4> to, const DfkWindowItemSlots* sl, int n) {
+      for (int i = 0; i < n; ++i) to.at(hb)[i] = make_int4(sl[i].pose0, sl[i].pose1, sl[i].code0, sl[i].code1);
     };
-    push(d->dense_slots, nd); push(d->error_slots, ne); push(d->reproj_slots, nr); push(d->geo_slots, ng);
-    push(d->depth_slots, ndep);
-    p->slots_tmpl.assign(slots.begin(), slots.begin() + nd + ne);
-    if (!slots.empty()) {
-      DFK_CUDA(h, p->slots.ensure(slots.size()), amsg);
-      DFK_CUDA(h, cudaMemcpyAsync(p->slots.ptr, slots.data(), sizeof(int4) * slots.size(), cudaMemcpyHostToDevice,
-                                  h->stream),
-               "[WindowProblem] upload failed");
-    }
-    // ---- priors: rows, frozen points, the keyframe of every delta row, add_priors' lists
-    const size_t PD = DFK_PRIOR_DOUBLES(C), X = 7 + (size_t)C;
-    std::vector<int> dkf;
-    std::vector<double> x0;
+    put_slots(p->dense_slots, d->dense_slots, nd); put_slots(p->err_slots, d->error_slots, ne);
+    put_slots(p->rep_slots, d->reproj_slots, nr); put_slots(p->geo_slots, d->geo_slots, ng);
+    put_slots(p->depth_slots, d->depth_slots, ndep);
+    p->slots_tmpl.assign(p->dense_slots.at(hb), p->dense_slots.at(hb) + nd);
+    p->slots_tmpl.insert(p->slots_tmpl.end(), p->err_slots.at(hb), p->err_slots.at(hb) + ne);
+    // ---- priors: rows, add_priors' lists, the keyframe of every delta row and the frozen points (frame priors, then
+    // keyframe-prior members)
     if (mf > 0) {
-      DFK_CUDA(h, p->frows.ensure(mf * PD), amsg);
-      DFK_CUDA(h, cudaMemcpyAsync(p->frows.ptr, d->frame_prior_rows, sizeof(double) * mf * PD, cudaMemcpyHostToDevice,
-                                  h->stream),
-               "[WindowProblem] upload failed");
-      dkf.assign(d->frame_prior_kf, d->frame_prior_kf + mf);
-      x0.assign(d->frame_prior_x0, d->frame_prior_x0 + mf * X);
-      std::vector<int> lists;
-      add_csr(lists, K, mf, [&](int i) { return d->frame_prior_kf[i]; });
-      DFK_CUDA(h, p->fp_lists.ensure(lists.size()), amsg);
-      DFK_CUDA(h, cudaMemcpyAsync(p->fp_lists.ptr, lists.data(), sizeof(int) * lists.size(), cudaMemcpyHostToDevice,
-                                  h->stream),
-               "[WindowProblem] upload failed");
+      memcpy(p->frows.at(hb), d->frame_prior_rows, sizeof(double) * mf * PD);
+      fill_csr(p->fp_lists.at(hb), K, mf, [&](int i) { return d->frame_prior_kf[i]; });
+      std::copy(d->frame_prior_kf, d->frame_prior_kf + mf, p->delta_kf.at(hb));
+      memcpy(p->x0.at(hb), d->frame_prior_x0, sizeof(double) * mf * X);
     }
     if (w->kp.num_priors > 0) {
-      const size_t kd = (size_t)w->prior_off.back();
-      DFK_CUDA(h, p->kfrows.ensure(kd), amsg);
-      DFK_CUDA(h, cudaMemcpyAsync(p->kfrows.ptr, d->kf_prior_rows, sizeof(double) * kd, cudaMemcpyHostToDevice, h->stream),
-               "[WindowProblem] upload failed");
-      dkf.insert(dkf.end(), w->prior_kf.begin(), w->prior_kf.end());
-      x0.insert(x0.end(), d->kf_prior_x0, d->kf_prior_x0 + nkm * X);
+      memcpy(p->kfrows.at(hb), d->kf_prior_rows, sizeof(double) * w->prior_off.back());
+      std::copy(w->prior_kf.begin(), w->prior_kf.end(), p->delta_kf.at(hb) + mf);
+      memcpy(p->x0.at(hb) + mf * X, d->kf_prior_x0, sizeof(double) * nkm * X);
     }
-    if (!dkf.empty()) {
-      DFK_CUDA(h, p->delta_kf.ensure(dkf.size()), amsg);
-      DFK_CUDA(h, p->x0.ensure(x0.size()), amsg);
-      DFK_CUDA(h, p->delta.ensure(dkf.size() * B), amsg);
-      DFK_CUDA(h, cudaMemcpyAsync(p->delta_kf.ptr, dkf.data(), sizeof(int) * dkf.size(), cudaMemcpyHostToDevice, h->stream),
-               "[WindowProblem] upload failed");
-      DFK_CUDA(h, cudaMemcpyAsync(p->x0.ptr, x0.data(), sizeof(double) * x0.size(), cudaMemcpyHostToDevice, h->stream),
-               "[WindowProblem] upload failed");
+    // ---- state (zero codes, identity poses until set_state)
+    for (int i = 0; i < 2 * NP; ++i) p->state.at(hb)[(size_t)(i / NP) * p->S + (size_t)(i % NP) * 7 + 3] = 1.0;
+    DFK_TRY(s.upload(h, p->blob, what));
+    if (nd > 0) {
+      DFK_CUDA(h, launch_sfm_ray_tables(p->dense.at(db), nd, h->stream), "[WindowProblem] kernel launch failed");
+      h->launches += 1;
     }
-    // ---- state (zero codes, identity poses until set_state), the gauge solver, the LM's small read-back block
-    DFK_CUDA(h, p->state.ensure(2 * p->S), amsg);
-    std::vector<double> init(2 * p->S, 0.0);
-    for (int s = 0; s < 2 * NP; ++s) init[(size_t)(s / NP) * p->S + (size_t)(s % NP) * 7 + 3] = 1.0;
-    DFK_CUDA(h, cudaMemcpyAsync(p->state.ptr, init.data(), sizeof(double) * init.size(), cudaMemcpyHostToDevice, h->stream),
-             "[WindowProblem] upload failed");
+    // ---- the gauge solver
     const std::vector<int> gauge{0, 1, 2, 3, 4, 5};
     DFK_CUDA(h, window_solver_create(K, C, F, w->pair_k0, w->pair_k1, w->link_k0, w->link_k1, w->blk_i, w->blk_j,
                                      w->kp.block_off, gauge, &p->solver[1]),
              "[WindowProblem] solver workspace allocation failed");
-    DFK_CUDA(h, p->small.ensure(9 * sizeof(double) + 16), amsg);  // energy | info | depth-prior energy
-    DFK_CUDA(h, p->small_host.ensure(9 * sizeof(double) + 16), amsg);
-    DFK_CUDA(h, cudaStreamSynchronize(h->stream), "[WindowProblem] upload failed");  // the host staging is freed next
+    DFK_CUDA(h, cudaStreamSynchronize(h->stream), "[WindowProblem] upload failed");
     *out = p.release();
     return DFK_OK;
   });
@@ -1393,30 +1355,28 @@ DfkStatus dfk_window_problem_set_depth_priors(DfkHandle h, DfkWindowProblem* p, 
     const int n = level_ptr[m];
     // the items' views are checked as the batch checks them; their codes come from the state (slot = prior_kf)
     DepthPriorStaged st;
-    DFK_TRY(stage_depth_prior(h, what, items, n, p->C, false, p->dp_host, p->dp, &st));
-    std::vector<int> lists;
-    add_csr(lists, p->K, m, [&](int i) { return prior_kf[i]; });
-    const size_t lp = lists.size();
-    lists.insert(lists.end(), level_ptr, level_ptr + m + 1);
-    const size_t sg = lists.size();
-    lists.resize(sg + m);
-    memcpy(lists.data() + sg, sigma, sizeof(float) * m);
-    const size_t kf = lists.size();
-    for (int i = 0; i < m; ++i)
-      for (int l = level_ptr[i]; l < level_ptr[i + 1]; ++l) lists.push_back(prior_kf[i]);
+    DFK_TRY(stage_depth_prior(h, what, items, n, p->C, false, h->staging, p->dp, &st));
+    // the lists, staged once the items' upload has read h->staging
+    Staging s(h->staging);
+    const Part<int> csr = s.add<int>(p->K + 1 + m), lp = s.add<int>(m + 1);
+    const Part<float> sg = s.add<float>(m);
+    const Part<int> kf = s.add<int>(n);
+    fill_csr(csr.at(s.host()), p->K, m, [&](int i) { return prior_kf[i]; });
+    memcpy(lp.at(s.host()), level_ptr, sizeof(int) * (m + 1));
+    memcpy(sg.at(s.host()), sigma, sizeof(float) * m);
+    for (int i = 0; i < m; ++i) std::fill(kf.at(s.host()) + level_ptr[i], kf.at(s.host()) + level_ptr[i + 1], prior_kf[i]);
     const char* amsg = "[WindowProblem::set_depth_priors] allocation failed";
-    DFK_CUDA(h, p->dp_lists.ensure(lists.size()), amsg);
+    DFK_CUDA(h, p->dp_lists.ensure(s.bytes), amsg);
     DFK_CUDA(h, p->dp_partials.ensure((size_t)st.rows * depth_prior_partial_floats(p->C, true)), amsg);
     DFK_CUDA(h, p->dp_records.ensure((size_t)n * DFK_DEPTH_RECORD_FLOATS(p->C)), amsg);
     DFK_CUDA(h, p->dp_err.ensure((size_t)n * 2), amsg);
-    DFK_CUDA(h, cudaMemcpyAsync(p->dp_lists.ptr, lists.data(), sizeof(int) * lists.size(), cudaMemcpyHostToDevice,
-                                h->stream),
-             "[WindowProblem::set_depth_priors] upload failed");
+    DFK_TRY(s.upload(h, p->dp_lists, w));
     p->ndp = m;
     p->ndpi = n;
     p->dp_st = st;
-    p->dp_lp = lp;
-    p->dp_sg = sg;
+    p->dp_csr = csr;
+    p->dp_level_ptr = lp;
+    p->dp_sigma = sg;
     p->dp_kf = kf;
     return DFK_OK;
   });

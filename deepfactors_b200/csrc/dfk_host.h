@@ -1,6 +1,6 @@
 // dfk_host.h -- host-side pieces that the C ABI's units (dfk_api.cu, dfk_api_sparse.cu, dfk_api_window.cu,
-// dfk_api_bow.cu) share: scratch buffers, the handle, error reporting, the blob layout and staging of every call's
-// upload (Layout, Staging), argument checks, the dense RunStep planning and the sparse staging.
+// dfk_api_bow.cu) share: scratch buffers, the handle, error reporting, the staging of every call's upload (Staging),
+// argument checks, the dense RunStep planning and the sparse staging.
 // Internal to libdfk.so.
 #pragma once
 
@@ -129,11 +129,10 @@ struct DfkContext {
   DeviceBuf<unsigned char> bow_scratch;
   // dfk_window_marginalize_frames / _add_priors / _add_depth_priors: the call's index lists (one pageable H2D per call)
   DeviceBuf<int> window_lists;
-  // dfk_window_marginalize_keyframe: the call's lists [refs | tile rows / cols | member locations | update tasks] (one
-  // pageable H2D per call), the code of m, and the local system's workspace (tiles, rhs, f)
-  DeviceBuf<int> marg_lists;
-  DeviceBuf<double> marg_code;
-  DeviceBuf<double> marg_dev;
+  // dfk_window_marginalize_keyframe: the call's staged [refs | tile rows / cols | member locations | update tasks | code
+  // of m] (one pageable H2D per call), and the local system's workspace [tiles | rhs | f]
+  DeviceBuf<unsigned char> marg_lists;
+  DeviceBuf<unsigned char> marg_dev;
   // normalised ray tables of the RunStep kernels: they depend on (fx, u0, width, fy, v0, height) only, so they are
   // built once per camera level and reused by every later call (one launch less per evaluation in steady state)
   struct RayTab {
@@ -242,29 +241,8 @@ struct DeviceGuard {
   }
 };
 
-// ---------------------------------------------------------------------------- blobs of typed parts
-// A call's staged upload, or its scratch, is one blob of typed parts, each rounded up to 16 bytes: the kernels read
-// int2 / int3 / uint4 / double parts.  A Part is where one part starts; the same offset addresses it from the host
-// image and from the device copy.
-template <class T>
-struct Part {
-  size_t off = 0;
-  T* at(void* base) const { return reinterpret_cast<T*>(static_cast<unsigned char*>(base) + off); }
-};
-
-// The sizing pass: add() the parts in blob order; `bytes` is the blob's size
-struct Layout {
-  size_t bytes = 0;
-  template <class T>
-  Part<T> add(size_t count)
-  {
-    const Part<T> p{bytes};
-    bytes += (sizeof(T) * count + 15) & ~(size_t)15;
-    return p;
-  }
-};
-
-// A blob uploaded with one copy.  add() lays its parts out as Layout does and grows the host image, zeroed, in a
+// ---------------------------------------------------------------------------- staged blobs
+// A blob uploaded with one copy (its parts: Part / Layout, dfk_internal.h).  add() lays its parts out as Layout does and grows the host image, zeroed, in a
 // pageable buffer (the handle's `staging`, or one of the object the blob belongs to); upload() grows the device buffer
 // and copies.  Messages begin with `what`.
 struct Staging : Layout {
@@ -449,15 +427,16 @@ DfkStatus launch_step(DfkHandle h, const StepKernel& k, int code_size, const Sfm
 // ---------------------------------------------------------------------------- sparse factors
 // A single call is a batch of one: the same checks, descriptors and staging.  Sparse<Item> is what the two factor kinds
 // stage differently: the argument check (the failure text, or null), the matches / points of a factor and the bytes each
-// takes, the codes per factor, and one factor's descriptor, codes and payload.
+// takes (in payload units), the codes per factor, and one factor's descriptor, codes and payload.
 template <class Item>
 struct Sparse;
 
 template <>
 struct Sparse<DfkReprojectionItem> {
   using Dev = ReprojItemDev;
+  using Unit = float2;
   static constexpr int codes = 1;
-  static constexpr size_t unit_bytes = 4 * sizeof(float);  // payload: query 2 total | train 2 total
+  static constexpr size_t units_per = 2;  // payload: query total | train total
   static constexpr const char* units = "matches";
   static size_t count(const DfkReprojectionItem& it) { return (size_t)it.num_matches; }
   static const char* error(const DfkReprojectionItem& it, int code_size)
@@ -471,23 +450,23 @@ struct Sparse<DfkReprojectionItem> {
   }
   // begin: the factor's first match, total: the matches of the block
   static void pack(const DfkReprojectionItem& it, int code_size, size_t begin, size_t total, Dev& d, float* code,
-                   const float* code_dev, unsigned char* payload)
+                   const float* code_dev, Unit* payload)
   {
     d = Dev{{}, view_of(&it.prx_orig), view_of(&it.prx_jac), code_dev, (int)it.prx_orig.width, (int)it.prx_orig.height,
             it.num_matches, (int)begin, it.cauchy_delta, it.sigma};
     set_relative_pose(d.sp, it.pose1, it.pose0, it.cam);  // pose10_J_pose1, pose10_J_pose0 (:189-190)
     memcpy(code, it.code, sizeof(float) * code_size);
-    float* query = reinterpret_cast<float*>(payload);
-    memcpy(query + 2 * begin, it.query_xy, sizeof(float) * 2 * it.num_matches);
-    memcpy(query + 2 * (total + begin), it.train_xy, sizeof(float) * 2 * it.num_matches);
+    memcpy(payload + begin, it.query_xy, sizeof(Unit) * it.num_matches);
+    memcpy(payload + total + begin, it.train_xy, sizeof(Unit) * it.num_matches);
   }
 };
 
 template <>
 struct Sparse<DfkSparseGeometricItem> {
   using Dev = GeoItemDev;
+  using Unit = int2;
   static constexpr int codes = 2;  // code0, code1
-  static constexpr size_t unit_bytes = 2 * sizeof(int32_t);  // payload: points 2 total
+  static constexpr size_t units_per = 1;  // payload: points total
   static constexpr const char* units = "points";
   static size_t count(const DfkSparseGeometricItem& it) { return (size_t)it.num_points; }
   static const char* error(const DfkSparseGeometricItem& it, int code_size)
@@ -503,7 +482,7 @@ struct Sparse<DfkSparseGeometricItem> {
     return nullptr;
   }
   static void pack(const DfkSparseGeometricItem& it, int code_size, size_t begin, size_t /*total*/, Dev& d, float* code,
-                   const float* code_dev, unsigned char* payload)
+                   const float* code_dev, Unit* payload)
   {
     d = Dev{{}, view_of(&it.prx0_orig), view_of(&it.prx0_jac), view_of(&it.prx1_orig), view_of(&it.prx1_jac),
             view_of(&it.dpt_grad1), code_dev, code_dev + code_size, it.cam.width, it.cam.height, (int)it.prx0_orig.width,
@@ -511,7 +490,7 @@ struct Sparse<DfkSparseGeometricItem> {
     set_relative_pose(d.sp, it.pose1, it.pose0, it.cam);  // pose10_J_pose1, pose10_J_pose0 (:176-178)
     memcpy(code, it.code0, sizeof(float) * code_size);
     memcpy(code + code_size, it.code1, sizeof(float) * code_size);
-    memcpy(reinterpret_cast<int32_t*>(payload) + 2 * begin, it.points_xy, sizeof(int32_t) * 2 * it.num_points);
+    memcpy(payload + begin, it.points_xy, sizeof(Unit) * it.num_points);
   }
 };
 
@@ -530,10 +509,14 @@ inline cudaError_t host_block(PinnedBuf<unsigned char>& b, size_t bytes, unsigne
   return e;
 }
 
+// A sparse batch as stage() staged it: [descriptors n | codes n x codes C | payload]
+template <class Item>
 struct Staged {
-  size_t bytes = 0;               // of the uploaded block; the caller's outputs may follow it
-  size_t total = 0;               // matches / points
-  const unsigned char* payload = nullptr;  // device address of the matches / points
+  Part<typename Sparse<Item>::Dev> descs;
+  Part<float> codes;
+  Part<typename Sparse<Item>::Unit> payload;  // the matches / points
+  size_t bytes = 0;  // of the uploaded block; the caller's outputs may follow it
+  size_t total = 0;  // matches / points
 };
 
 // Checks the code size and items[0, n) (messages begin with `what`, a batch's name the item), then stages the factors in
@@ -541,7 +524,7 @@ struct Staged {
 // out_bytes for the caller's outputs, which follow the upload.
 template <class Item, class HostBuf>
 DfkStatus stage(DfkHandle h, const std::string& what, bool batch, const Item* items, int n, int code_size,
-                size_t out_bytes, HostBuf& host, DeviceBuf<unsigned char>& dev, Staged* st)
+                size_t out_bytes, HostBuf& host, DeviceBuf<unsigned char>& dev, Staged<Item>* st)
 {
   using S = Sparse<Item>;
   if (!sparse_supported(code_size))
@@ -555,17 +538,16 @@ DfkStatus stage(DfkHandle h, const std::string& what, bool batch, const Item* it
     return fail(h, DFK_ERR_INVALID_ARG, what + "more than 2^31 - 1 " + S::units + " in one call");
   const size_t code_floats = (size_t)S::codes * code_size;
   Layout L;
-  const Part<typename S::Dev> descs = L.add<typename S::Dev>(n);
-  const Part<float> codes = L.add<float>(n * code_floats);
-  const Part<unsigned char> payload = L.add<unsigned char>(S::unit_bytes * st->total);
+  st->descs = L.add<typename S::Dev>(n);
+  st->codes = L.add<float>(n * code_floats);
+  st->payload = L.add<typename S::Unit>(S::units_per * st->total);
   st->bytes = L.bytes;
   DFK_CUDA(h, dev.ensure(st->bytes + out_bytes), (what + "scratch allocation failed").c_str());
   unsigned char* hb = nullptr;
   DFK_CUDA(h, host_block(host, st->bytes + out_bytes, &hb), (what + "pinned allocation failed").c_str());
   for (size_t i = 0, begin = 0; i < (size_t)n; begin += S::count(items[i]), ++i)
-    S::pack(items[i], code_size, begin, st->total, descs.at(hb)[i], codes.at(hb) + i * code_floats,
-            codes.at(dev.ptr) + i * code_floats, payload.at(hb));
+    S::pack(items[i], code_size, begin, st->total, st->descs.at(hb)[i], st->codes.at(hb) + i * code_floats,
+            st->codes.at(dev.ptr) + i * code_floats, st->payload.at(hb));
   DFK_CUDA(h, cudaMemcpyAsync(dev.ptr, hb, st->bytes, cudaMemcpyHostToDevice, h->stream), (what + "upload failed").c_str());
-  st->payload = payload.at(dev.ptr);
   return DFK_OK;
 }

@@ -12,6 +12,28 @@
 
 namespace dfk {
 
+// ---------------------------------------------------------------------------- blobs of typed parts
+// A call's staged upload, or its scratch, is one blob of typed parts, each rounded up to 16 bytes: the kernels read
+// int2 / int3 / uint4 / double parts.  A Part is where one part starts; the same offset addresses it from the host
+// image and from the device copy.
+template <class T>
+struct Part {
+  size_t off = 0;
+  T* at(void* base) const { return reinterpret_cast<T*>(static_cast<unsigned char*>(base) + off); }
+};
+
+// The sizing pass: add() the parts in blob order; `bytes` is the blob's size
+struct Layout {
+  size_t bytes = 0;
+  template <class T>
+  Part<T> add(size_t count)
+  {
+    const Part<T> p{bytes};
+    bytes += (sizeof(T) * count + 15) & ~(size_t)15;
+    return p;
+  }
+};
+
 // ----------------------------------------------------------------------------------------------
 // Device-side description of one (keyframe, frame, level) evaluation.  Built on the host by
 // dfk_api.cu from a DfkSfmWorkItem: the relative pose and its two 6x6 Jacobians are host work in

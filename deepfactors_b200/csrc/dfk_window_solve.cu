@@ -527,10 +527,10 @@ struct WindowSolverDev {
   std::vector<int> col_ptr;   // [K + 1] tiles of column j: [col_ptr[j], col_ptr[j+1]), the first one diagonal
   std::vector<int> upd_ptr;   // [K + 1] update tasks of column j
   std::vector<int> row_ptr;   // [K + 1] backward tiles of row j (off-diagonal, column order)
-  // device: one int allocation (tile_row | tile_col | contrib_ptr | contrib | diag_tile | row_tiles | frame_ptr |
-  // frame_list | frame_pair | frame_kf | tasks), the fixed mask, the codes, the tiles, the rhs, the frames' factors and
-  // pivot flags
-  void* ints = nullptr;
+  // device: one allocation, the uploaded lists (tile_row | tile_col | contrib_ptr | contrib | diag_tile | row_tiles |
+  // frame_ptr | frame_list | frame_pair | frame_kf | prior-load lists | tasks | fixed mask), then the workspace (codes |
+  // tiles | rhs | the frames' factors and pivot flags)
+  unsigned char* blob = nullptr;
   unsigned char* fixed = nullptr;
   double* codes = nullptr;
   double* tiles = nullptr;
@@ -541,16 +541,7 @@ struct WindowSolverDev {
             *row_tiles = nullptr, *frame_ptr = nullptr, *frame_list = nullptr, *frame_pair = nullptr,
             *frame_kf = nullptr;
   const UpdTask* tasks = nullptr;
-  ~WindowSolverDev()
-  {
-    cudaFree(ints);
-    cudaFree(fixed);
-    cudaFree(codes);
-    cudaFree(tiles);
-    cudaFree(rhs);
-    cudaFree(frame_L);
-    cudaFree(frame_bad);
-  }
+  ~WindowSolverDev() { cudaFree(blob); }
 };
 
 size_t window_solver_tiles(const WindowSolverDev* s) { return s ? (size_t)s->num_tiles : 0; }
@@ -649,57 +640,59 @@ cudaError_t window_solver_create(int K, int C, int F, const std::vector<int>& pa
     row_tiles.insert(row_tiles.end(), row_list[j].begin(), row_list[j].end());
   }
   s->row_ptr[K] = (int)row_tiles.size();
-  // ---- one int blob
-  std::vector<int> blob;
-  auto put = [&](const int* p, size_t n) {
-    const size_t o = blob.size();
-    blob.insert(blob.end(), p, p + n);
-    return o;
-  };
+  // ---- one allocation: the uploaded lists, then the workspace
   std::vector<int> cptr(T + 1, 0), cflat;
   for (int t = 0; t < T; ++t) {
     cptr[t] = (int)cflat.size();
     cflat.insert(cflat.end(), contrib[t].begin(), contrib[t].end());
   }
   cptr[T] = (int)cflat.size();
-  std::vector<int> diag(K);
-  for (int j = 0; j < K; ++j) diag[j] = s->col_ptr[j];
-  const size_t o_tr = put(tile_row.data(), T), o_tc = put(tile_col.data(), T), o_cp = put(cptr.data(), T + 1);
-  const size_t o_cf = put(cflat.data(), cflat.size()), o_dg = put(diag.data(), K);
-  const size_t o_rt = put(row_tiles.data(), row_tiles.size());
   for (int k = 0; k < K; ++k) frame_ptr[k + 1] += frame_ptr[k];
   {
     std::vector<int> next(frame_ptr.begin(), frame_ptr.end() - 1);
     for (int f = 0; f < F; ++f) frame_list[next[frame_kf[f]]++] = f;
   }
-  const size_t o_fp = put(frame_ptr.data(), K + 1), o_fl = put(frame_list.data(), F);
-  const size_t o_fr = put(frame_pair.data(), F), o_fk = put(frame_kf.data(), F);
-  const size_t o_pt = put(ptiles.data(), ptiles.size()), o_pp = put(pptr.data(), pptr.size());
-  const size_t o_pf = put(pflat.data(), pflat.size());
-  blob.resize((blob.size() + 3) & ~(size_t)3, 0);  // UpdTask is 16-byte aligned
-  const size_t o_tk = put(reinterpret_cast<const int*>(tasks.data()), tasks.size() * 4);
-  std::vector<unsigned char> fixed((size_t)K * B, 0);
-  for (int v : fixed_vars) fixed[v] = 1;
+  Layout lay;
+  const Part<int> tr = lay.add<int>(T), tc = lay.add<int>(T), cp = lay.add<int>(T + 1), cf = lay.add<int>(cflat.size());
+  const Part<int> dg = lay.add<int>(K), rt = lay.add<int>(row_tiles.size()), fp = lay.add<int>(K + 1), fl = lay.add<int>(F);
+  const Part<int> fr = lay.add<int>(F), fk = lay.add<int>(F), pt = lay.add<int>(ptiles.size()), pp = lay.add<int>(pptr.size());
+  const Part<int> pf = lay.add<int>(pflat.size());
+  const Part<UpdTask> tk = lay.add<UpdTask>(tasks.size());
+  const Part<unsigned char> fx = lay.add<unsigned char>((size_t)K * B);
+  const size_t uploaded = lay.bytes;
+  const Part<double> codes = lay.add<double>((size_t)K * C), tiles = lay.add<double>((size_t)(T + K) * B * B);
+  const Part<double> rhs = lay.add<double>((size_t)K * B), frame_L = lay.add<double>((size_t)F * 36);
+  const Part<int> frame_bad = lay.add<int>(F);
+  std::vector<unsigned char> host(uploaded, 0);
+  unsigned char* hb = host.data();
+  std::copy(tile_row.begin(), tile_row.end(), tr.at(hb));
+  std::copy(tile_col.begin(), tile_col.end(), tc.at(hb));
+  std::copy(cptr.begin(), cptr.end(), cp.at(hb));
+  std::copy(cflat.begin(), cflat.end(), cf.at(hb));
+  std::copy(s->col_ptr.begin(), s->col_ptr.end() - 1, dg.at(hb));  // the diagonal tile of column j is its first
+  std::copy(row_tiles.begin(), row_tiles.end(), rt.at(hb));
+  std::copy(frame_ptr.begin(), frame_ptr.end(), fp.at(hb));
+  std::copy(frame_list.begin(), frame_list.end(), fl.at(hb));
+  std::copy(frame_pair.begin(), frame_pair.end(), fr.at(hb));
+  std::copy(frame_kf.begin(), frame_kf.end(), fk.at(hb));
+  std::copy(ptiles.begin(), ptiles.end(), pt.at(hb));
+  std::copy(pptr.begin(), pptr.end(), pp.at(hb));
+  std::copy(pflat.begin(), pflat.end(), pf.at(hb));
+  std::copy(tasks.begin(), tasks.end(), tk.at(hb));
+  for (int v : fixed_vars) fx.at(hb)[v] = 1;
 
   cudaError_t e;
-  if ((e = cudaMalloc(&s->ints, std::max<size_t>(blob.size(), 1) * sizeof(int))) != cudaSuccess) return e;
-  if ((e = cudaMalloc((void**)&s->fixed, fixed.size())) != cudaSuccess) return e;
-  if ((e = cudaMalloc((void**)&s->codes, (size_t)K * C * sizeof(double))) != cudaSuccess) return e;
-  if ((e = cudaMalloc((void**)&s->tiles, (size_t)(T + K) * B * B * sizeof(double))) != cudaSuccess) return e;
-  if ((e = cudaMalloc((void**)&s->rhs, (size_t)K * B * sizeof(double))) != cudaSuccess) return e;
-  if (F > 0) {
-    if ((e = cudaMalloc((void**)&s->frame_L, (size_t)F * 36 * sizeof(double))) != cudaSuccess) return e;
-    if ((e = cudaMalloc((void**)&s->frame_bad, (size_t)F * sizeof(int))) != cudaSuccess) return e;
-  }
-  if ((e = cudaMemcpy(s->ints, blob.data(), blob.size() * sizeof(int), cudaMemcpyHostToDevice)) != cudaSuccess) return e;
-  if ((e = cudaMemcpy(s->fixed, fixed.data(), fixed.size(), cudaMemcpyHostToDevice)) != cudaSuccess) return e;
-  const int* ip = static_cast<const int*>(s->ints);
-  s->tile_row = ip + o_tr; s->tile_col = ip + o_tc; s->contrib_ptr = ip + o_cp; s->contrib = ip + o_cf;
-  s->diag_tile = ip + o_dg; s->row_tiles = ip + o_rt;
-  s->frame_ptr = ip + o_fp; s->frame_list = ip + o_fl; s->frame_pair = ip + o_fr; s->frame_kf = ip + o_fk;
-  s->tasks = reinterpret_cast<const UpdTask*>(ip + o_tk);
+  if ((e = cudaMalloc((void**)&s->blob, lay.bytes)) != cudaSuccess) return e;
+  if ((e = cudaMemcpy(s->blob, hb, uploaded, cudaMemcpyHostToDevice)) != cudaSuccess) return e;
+  unsigned char* b = s->blob;
+  s->tile_row = tr.at(b); s->tile_col = tc.at(b); s->contrib_ptr = cp.at(b); s->contrib = cf.at(b);
+  s->diag_tile = dg.at(b); s->row_tiles = rt.at(b);
+  s->frame_ptr = fp.at(b); s->frame_list = fl.at(b); s->frame_pair = fr.at(b); s->frame_kf = fk.at(b);
+  s->tasks = tk.at(b);
+  s->fixed = fx.at(b); s->codes = codes.at(b); s->tiles = tiles.at(b); s->rhs = rhs.at(b);
+  s->frame_L = frame_L.at(b); s->frame_bad = frame_bad.at(b);
   s->prior_tiles = (int)ptiles.size();
-  s->pa.tiles = ip + o_pt; s->pa.blk_ptr = ip + o_pp; s->pa.blk = ip + o_pf; s->pa.off = prior_off;
+  s->pa.tiles = pt.at(b); s->pa.blk_ptr = pp.at(b); s->pa.blk = pf.at(b); s->pa.off = prior_off;
   // kernel attributes once, here: no runtime configuration call in a solve
   e = with_code_size(C, [](auto bc) {
     constexpr int Bv = bc.value;
