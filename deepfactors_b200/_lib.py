@@ -93,6 +93,10 @@ class DfkWindowSolveParams(C.Structure):
     _fields_ = [("lambda_", C.c_double), ("code_prior_weight", C.c_double)]
 
 
+class DfkWindowUpdateParams(C.Structure):
+    _fields_ = [("code_prior_weight", C.c_double), ("diag_eps", C.c_double)]
+
+
 class DfkWindowItemSlots(C.Structure):
     _fields_ = [("pose0", C.c_int32), ("pose1", C.c_int32), ("code0", C.c_int32), ("code1", C.c_int32)]
 
@@ -273,6 +277,10 @@ SYMBOLS = {
     "dfk_window_solver_tiles": (C.c_int, [_H, C.c_void_p, C.POINTER(C.c_size_t)]),
     "dfk_window_solve": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.POINTER(DfkWindowSolveParams), C.POINTER(C.c_double),
                                    C.c_void_p, C.c_void_p]),
+    "dfk_window_solver_update": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.POINTER(DfkWindowUpdateParams),
+                                           C.POINTER(C.c_double), C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]),
+    "dfk_window_solver_create_from": (C.c_int, [_H, C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.c_void_p,
+                                                C.POINTER(C.c_void_p)]),
     "dfk_window_problem_create": (C.c_int, [_H, C.POINTER(DfkWindowProblemDesc), C.POINTER(C.c_void_p)]),
     "dfk_window_problem_destroy": (C.c_int, [_H, C.c_void_p]),
     "dfk_window_problem_set_state": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -1265,15 +1265,25 @@ class WindowSolver:
     nonzero B x B tiles of the factor, fill included.  With tracked frames dx has K * B + 6 F entries (frame f's pose
     at K * B + 6 f)."""
 
-    def __init__(self, window: Window, fixed=()):
+    def __init__(self, window: Window, fixed=(), _prev: "WindowSolver | None" = None):
         self._win = window  # keeps the window (and its handle) alive
         self._al = window._al
         self.layout = window.layout
         fx = np.ascontiguousarray([int(v) for v in fixed], dtype=np.int32)
         self.fixed = tuple(int(v) for v in fx)
         self.s = C.c_void_p()
-        check(self._al.handle, lib().dfk_window_solver_create(self._al.handle, window.w, len(fx),
-                                                              fx.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(self.s)))
+        self.info = None  # update()'s pivot report when the caller passes no info tensor
+        if _prev is None:
+            check(self._al.handle, lib().dfk_window_solver_create(self._al.handle, window.w, len(fx),
+                                                                  fx.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                                  C.byref(self.s)))
+        else:
+            # create_from copies the old solver's factor on the handle's stream: order it after torch's work, as
+            # update() does
+            self._al._hd.use_torch_stream()
+            check(self._al.handle, lib().dfk_window_solver_create_from(self._al.handle, window.w, len(fx),
+                                                                       fx.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                                       _prev.s, C.byref(self.s)))
         tiles = C.c_size_t(0)
         check(self._al.handle, lib().dfk_window_solver_tiles(self._al.handle, self.s, C.byref(tiles)))
         self.tiles = int(tiles.value)
@@ -1305,6 +1315,46 @@ class WindowSolver:
         check(self._al.handle, lib().dfk_window_solve(self._al.handle, self.s, C.c_void_p(buf.data_ptr()), C.byref(prm),
                                                       cp, C.c_void_p(dx.data_ptr()), C.c_void_p(info.data_ptr())))
         return dx, info
+
+    def update(self, buf: torch.Tensor, diag_eps: float, code_prior_weight: float = 0.0, codes=None,
+               dx: torch.Tensor | None = None, info: torch.Tensor | None = None):
+        """Incremental Gauss-Newton solve (dfk_window_solver_update): no lambda, diag_eps added to every kept diagonal
+        entry, and only the keyframe columns from the first one whose loaded system changed since the last update are
+        re-factorised.  Returns (dx, first_column): dx as solve() gives it, first_column = that column (K: nothing
+        changed).  The pivot report goes to `info` when given, else to self.info (0, or 1 + the failed variable; dx is
+        then zero).  Synchronises torch's current stream once when the solver has columns to reuse."""
+        hd = self._al._hd
+        hd.use_torch_stream()
+        n = self.layout.dim
+        _check_tensor(hd, buf, torch.float32, self.layout.floats, "buf")
+        if dx is None:
+            dx = torch.empty(n, dtype=torch.float64, device=buf.device)
+        _check_tensor(hd, dx, torch.float64, n, "dx")
+        if info is None:
+            if self.info is None:
+                self.info = torch.empty(1, dtype=torch.int32, device=buf.device)
+            info = self.info
+        _check_tensor(hd, info, torch.int32, 1, "info")
+        cp = None
+        if code_prior_weight > 0:
+            if codes is None:
+                raise ValueError("code_prior_weight > 0 needs the codes")
+            c64 = np.ascontiguousarray(codes, dtype=np.float64)
+            if c64.shape != (self.layout.num_keyframes, self.layout.code_size):
+                raise ValueError(f"codes must be [{self.layout.num_keyframes}, {self.layout.code_size}]")
+            cp = c64.ctypes.data_as(C.POINTER(C.c_double))
+        prm = _lib.DfkWindowUpdateParams(float(code_prior_weight), float(diag_eps))
+        j0 = C.c_int32(0)
+        check(self._al.handle, lib().dfk_window_solver_update(self._al.handle, self.s, C.c_void_p(buf.data_ptr()),
+                                                              C.byref(prm), cp, C.c_void_p(dx.data_ptr()),
+                                                              C.c_void_p(info.data_ptr()), C.byref(j0)))
+        return dx, int(j0.value)
+
+    def grown(self, window: Window, fixed=()) -> "WindowSolver":
+        """A solver for `window`, whose first keyframes are this solver's window's (same code size, the same fixed
+        variables among them), that takes over this solver's longest prefix of keyframe columns with an unchanged tile
+        pattern (dfk_window_solver_create_from).  This solver is left as it was."""
+        return WindowSolver(window, fixed, _prev=self)
 
     def close(self):
         if getattr(self, "s", None):

@@ -963,10 +963,24 @@ DfkStatus dfk_window_marginalize_keyframe(DfkHandle h, const DfkWindow* w, const
 DfkStatus dfk_window_solver_create(DfkHandle h, const DfkWindow* w, int num_fixed, const int32_t* fixed_vars,
                                    DfkWindowSolver** out)
 {
+  return dfk_window_solver_create_from(h, w, num_fixed, fixed_vars, nullptr, out);
+}
+
+DfkStatus dfk_window_solver_create_from(DfkHandle h, const DfkWindow* w, int num_fixed, const int32_t* fixed_vars,
+                                        const DfkWindowSolver* prev, DfkWindowSolver** out)
+{
   return guarded(h, [&] {
     if (!w || !out || num_fixed < 0 || (num_fixed > 0 && !fixed_vars))
       return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] null argument");
-    *out = nullptr;
+    if (prev && prev->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] previous solver and handle live on different devices");
+    if (prev && (prev->code_size != w->dev.code_size || prev->num_keyframes > w->dev.num_keyframes))
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] the window does not extend the previous solver's: " +
+                                              std::to_string(prev->num_keyframes) + " keyframes of code size " +
+                                              std::to_string(prev->code_size) + " need a prefix of " +
+                                              std::to_string(w->dev.num_keyframes) + " of size " +
+                                              std::to_string(w->dev.code_size));
+    if (!prev) *out = nullptr;
     if (w->device != h->device)
       return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] window and handle live on different devices");
     const int K = w->dev.num_keyframes, C = w->dev.code_size, n = K * (6 + C);
@@ -987,7 +1001,40 @@ DfkStatus dfk_window_solver_create(DfkHandle h, const DfkWindow* w, int num_fixe
     DFK_CUDA(h, window_solver_create(K, C, w->dev.num_frames, w->pair_k0, w->pair_k1, w->link_k0, w->link_k1, w->blk_i,
                                      w->blk_j, w->kp.block_off, fixed, &s->dev),
              "[WindowSolver] workspace allocation failed");
+    if (prev) {
+      if (!window_solver_extends(prev->dev, s->dev))
+        return fail(h, DFK_ERR_INVALID_ARG,
+                    "[WindowSolver] the window fixes other variables among the previous solver's keyframes");
+      int columns = 0;
+      DFK_CUDA(h, window_solver_adopt(s->dev, prev->dev, h->stream, &columns),
+               "[WindowSolver] copying the previous solver's factor failed");
+    }
     *out = s.release();
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_solver_update(DfkHandle h, DfkWindowSolver* s, const float* window_dev,
+                                   const DfkWindowUpdateParams* p, const double* codes, double* dx_dev,
+                                   int32_t* info_dev, int32_t* first_column)
+{
+  return guarded(h, [&] {
+    if (!s || !window_dev || !p || !dx_dev || !info_dev || !first_column)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] null argument");
+    if (s->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] solver and handle live on different devices");
+    if (!(std::isfinite(p->diag_eps) && p->diag_eps >= 0.0))
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] diag_eps must be finite and >= 0");
+    if (!(std::isfinite(p->code_prior_weight) && p->code_prior_weight >= 0.0))
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] code_prior_weight must be finite and >= 0");
+    if (p->code_prior_weight > 0.0 && !codes)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowSolver] code_prior_weight > 0 needs the codes");
+    DeviceGuard guard(h->device);
+    int j0 = 0;
+    DFK_CUDA(h, launch_window_solver_update(s->dev, window_dev, p->code_prior_weight, p->diag_eps, codes, dx_dev,
+                                            info_dev, h->stream, &h->launches, &j0),
+             "[WindowSolver] incremental update failed");
+    *first_column = j0;
     return DFK_OK;
   });
 }

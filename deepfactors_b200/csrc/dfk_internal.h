@@ -324,6 +324,20 @@ size_t window_solver_tiles(const WindowSolverDev* s);
 cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_dev, double lambda, double prior,
                                 const double* codes_host, double* dx_dev, int32_t* info_dev, cudaStream_t stream,
                                 uint64_t* launches, bool codes_on_device = false);
+// Gauss-Newton solve with an absolute diagonal term (dfk_window_solver_update): load into the new loaded set, compare it
+// column by column with the last update's, re-factorise from the first changed column j0 (*first_column; one 4-byte
+// read-back and stream synchronisation when the solver has a reusable prefix), replay the kept columns' updates onto
+// the rest, then the forward tail, the full backward pass and the frames.  The first call allocates the incremental
+// workspace.
+cudaError_t launch_window_solver_update(WindowSolverDev* s, const float* window_dev, double prior, double diag_eps,
+                                        const double* codes_host, double* dx_dev, int32_t* info_dev,
+                                        cudaStream_t stream, uint64_t* launches, int* first_column);
+// growth (dfk_window_solver_create_from): whether s's window can extend prev's (same code size, at least as many
+// keyframes, the same fixed variables among prev's), and s taking over prev's longest prefix of columns with the same
+// tile pattern (bounded by what prev holds from its last update): factor, stored loaded system and forward pass,
+// copied on the stream.  *columns = the prefix.
+bool window_solver_extends(const WindowSolverDev* prev, const WindowSolverDev* s);
+cudaError_t window_solver_adopt(WindowSolverDev* s, const WindowSolverDev* prev, cudaStream_t stream, int* columns);
 // Elimination of local keyframe 0 from a local tile system laid out as KfMargDev (tiles 0..n = column 0, diagonal first,
 // then the lower tiles (I, J) of 1..n): the solve's panel launch of column 0 (L of block 0, z = L^-1 g_0, Y_I = H_I0
 // L^-T) and its update launch (H_IJ -= Y_I Y_J^T, g_I -= Y_I z).  info gets 0 or 1 + the failed row.

@@ -33,6 +33,7 @@
 // that is not positive and finite is reported (by column 0's panel, as the first in elimination order) as
 // 1 + K B + 6 f + r.
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <math.h>
 #include <stdint.h>
 
@@ -70,6 +71,7 @@ struct SolveArgs {
   int K, P;
   int num_tiles;
   double lambda, prior;
+  double diag_eps;  // the incremental load's absolute diagonal term (window_solve_load_kernel<B, F, true>)
 };
 
 // the tracked frames of a window, a parameter of its own: only the kernels that handle frames take it, so those of a
@@ -186,8 +188,9 @@ __device__ __forceinline__ void eliminate_frames(const SolveArgs& a, const Frame
   }
 }
 
-// kFrames = false (a window without frames) is the load kernel without any frame code: same registers, no stack
-template <int B, bool kFrames>
+// kFrames = false (a window without frames) is the load kernel without any frame code: same registers, no stack.
+// kAbsEps (the incremental update): no lambda, and the diagonal term is a.diag_eps instead of 1e-12 max|d|.
+template <int B, bool kFrames, bool kAbsEps = false>
 __global__ void __launch_bounds__(kThreads) window_solve_load_kernel(SolveArgs a, FrameArgs fa)
 {
   const int t = blockIdx.x;
@@ -201,20 +204,25 @@ __global__ void __launch_bounds__(kThreads) window_solve_load_kernel(SolveArgs a
     }
     return;
   }
-  // diagonal tile: max |d| over the kept variables of the whole window (every diagonal CTA computes it, max is exact)
-  __shared__ double red[kThreads / 32];
-  double m = 0.0;
-  for (int v = threadIdx.x; v < a.K * B; v += blockDim.x)
-    if (!a.fixed[v]) m = fmax(m, fabs(diag_entry<B>(a, v / B, v % B)));
-  if constexpr (kFrames)
-    for (int v = threadIdx.x; v < fa.F * 6; v += blockDim.x)  // and over the frames' (never fixed)
-      m = fmax(m, fabs((double)a.buf[frame_block_off<B>(a, fa) + (v / 6) * 36 + (v % 6) * 7]));
-  for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
-  __syncthreads();
-  m = 0.0;
-  for (int w = 0; w < kThreads / 32; ++w) m = fmax(m, red[w]);
-  const double eps = __dmul_rn(1e-12, m);
+  double eps;
+  if constexpr (kAbsEps) {
+    eps = a.diag_eps;
+  } else {
+    // diagonal tile: max |d| over the kept variables of the whole window (every diagonal CTA computes it, max is exact)
+    __shared__ double red[kThreads / 32];
+    double m = 0.0;
+    for (int v = threadIdx.x; v < a.K * B; v += blockDim.x)
+      if (!a.fixed[v]) m = fmax(m, fabs(diag_entry<B>(a, v / B, v % B)));
+    if constexpr (kFrames)
+      for (int v = threadIdx.x; v < fa.F * 6; v += blockDim.x)  // and over the frames' (never fixed)
+        m = fmax(m, fabs((double)a.buf[frame_block_off<B>(a, fa) + (v / 6) * 36 + (v % 6) * 7]));
+    for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+    __syncthreads();
+    m = 0.0;
+    for (int w = 0; w < kThreads / 32; ++w) m = fmax(m, red[w]);
+    eps = __dmul_rn(1e-12, m);
+  }
   for (int e = threadIdx.x; e < B * B; e += blockDim.x) {
     const int r = e / B, c = e - r * B;
     const bool fx = a.fixed[i * B + r] | a.fixed[i * B + c];
@@ -225,7 +233,10 @@ __global__ void __launch_bounds__(kThreads) window_solve_load_kernel(SolveArgs a
       h = tile_entry<B>(a, t, r, c);
       if (r == c) {
         if (a.prior > 0.0 && r >= 6) h = __dadd_rn(h, a.prior);
-        h = __dadd_rn(h, __dadd_rn(__dmul_rn(a.lambda, h), eps));  // damped_solve: H + diag(lam d + 1e-12 max|d|)
+        if constexpr (kAbsEps)
+          h = __dadd_rn(h, eps);
+        else
+          h = __dadd_rn(h, __dadd_rn(__dmul_rn(a.lambda, h), eps));  // damped_solve: H + diag(lam d + 1e-12 max|d|)
       }
     }
     T[e] = h;
@@ -373,16 +384,15 @@ struct UpdTask {
   int target, a, b, rhs_row;  // rhs_row >= 0: diagonal target, also g_rhs_row -= L_a y_j
 };
 
+// T -= La Lb^T and, with g, g -= La y: one task's arithmetic, shared by the update launch of a column and the head
+// replay of an incremental update, so that both round alike.  Each thread reads and writes only its own entries of T
+// and g, so consecutive calls on one tile need no barrier between them.
 template <int B>
-__global__ void __launch_bounds__(kThreads) window_solve_update_kernel(SolveArgs a, const UpdTask* tasks, int j)
+__device__ __forceinline__ void update_tile(double* T, const double* La, const double* Lb, double* g, const double* y)
 {
   using Cfg = UpdCfg<B>;
   constexpr int S = Cfg::S, M = Cfg::M, KC = Cfg::KC;
   __shared__ double As[KC][S + 1], Bs[KC][S + 1];
-  const UpdTask task = tasks[blockIdx.x];
-  double* T = a.tiles + tile_off(task.target, B);
-  const double* La = a.tiles + tile_off(task.a, B);
-  const double* Lb = a.tiles + tile_off(task.b, B);
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   for (int sr = 0; sr < Cfg::kSub; ++sr)
     for (int sc = 0; sc < Cfg::kSub; ++sc) {
@@ -421,15 +431,21 @@ __global__ void __launch_bounds__(kThreads) window_solve_update_kernel(SolveArgs
           if (r < B && c < B) T[r * B + c] = __dsub_rn(T[r * B + c], acc[u][v]);
         }
     }
-  if (task.rhs_row >= 0) {
-    const double* y = a.rhs + (size_t)j * B;
-    double* g = a.rhs + (size_t)task.rhs_row * B;
+  if (g) {
     for (int r = threadIdx.x; r < B; r += kThreads) {
       double s = 0.0;
       for (int m = 0; m < B; ++m) s = __fma_rn(La[r * B + m], y[m], s);
       g[r] = __dsub_rn(g[r], s);
     }
   }
+}
+
+template <int B>
+__global__ void __launch_bounds__(kThreads) window_solve_update_kernel(SolveArgs a, const UpdTask* tasks, int j)
+{
+  const UpdTask task = tasks[blockIdx.x];
+  update_tile<B>(a.tiles + tile_off(task.target, B), a.tiles + tile_off(task.a, B), a.tiles + tile_off(task.b, B),
+                 task.rhs_row >= 0 ? a.rhs + (size_t)task.rhs_row * B : nullptr, a.rhs + (size_t)j * B);
 }
 
 // --------------------------------------------------------------------------------------------------------- backward
@@ -504,6 +520,95 @@ __global__ void __launch_bounds__(32) window_solve_frames_kernel(SolveArgs a, Fr
   }
 }
 
+// ------------------------------------------------------------------------------------------------------ incremental
+// The loaded system of an update (tiles 0 .. T-1 after the load launches, and the rhs blocks), one of two ping-pong sets
+// of the incremental workspace: the other holds the previous update's.
+struct LoadedSet {
+  double* tiles;
+  double* rhs;
+};
+
+// one CTA per keyframe column j: j0 = min(j0, j) when a tile of column j or rhs block j of `now` differs bit for bit
+// from `before`.  *j0 holds the reusable prefix before the launch; atomicMin makes the result independent of CTA order.
+__global__ void __launch_bounds__(kThreads) window_update_diff_kernel(LoadedSet now, LoadedSet before,
+                                                                      const int* diag_tile, int K, int T, int B,
+                                                                      int* j0)
+{
+  const int j = blockIdx.x;
+  const size_t t0 = (size_t)diag_tile[j] * B * B, t1 = (size_t)(j + 1 < K ? diag_tile[j + 1] : T) * B * B;
+  const unsigned long long* x = reinterpret_cast<const unsigned long long*>(now.tiles);
+  const unsigned long long* y = reinterpret_cast<const unsigned long long*>(before.tiles);
+  int diff = 0;
+  for (size_t e = t0 + threadIdx.x; e < t1; e += blockDim.x) diff |= x[e] != y[e];
+  const unsigned long long* gx = reinterpret_cast<const unsigned long long*>(now.rhs) + (size_t)j * B;
+  const unsigned long long* gy = reinterpret_cast<const unsigned long long*>(before.rhs) + (size_t)j * B;
+  for (int r = threadIdx.x; r < B; r += blockDim.x) diff |= gx[r] != gy[r];
+  if (__syncthreads_or(diff) && threadIdx.x == 0) atomicMin(j0, j);
+}
+
+// one CTA per tile t of the columns j0 .. K-1: the loaded tile (and, for a diagonal tile, the loaded rhs block) into the
+// working set, then the updates of the kept head columns j < j0 that target it, in column order, as their update
+// launches would apply them (update_tile, with y_j from the stored forward pass)
+template <int B>
+__global__ void __launch_bounds__(kThreads) window_update_replay_kernel(SolveArgs a, LoadedSet now, const double* ystore,
+                                                                        const int* rep_ptr, const UpdTask* rep_tasks,
+                                                                        int t_begin, int j0)
+{
+  const int t = t_begin + blockIdx.x;
+  const int i = a.tile_row[t];
+  const bool diag = i == a.tile_col[t];
+  double* T = a.tiles + tile_off(t, B);
+  const double* src = now.tiles + tile_off(t, B);
+  for (int e = threadIdx.x; e < B * B; e += blockDim.x) T[e] = src[e];
+  if (diag)
+    for (int r = threadIdx.x; r < B; r += blockDim.x) a.rhs[(size_t)i * B + r] = now.rhs[(size_t)i * B + r];
+  __syncthreads();
+  for (int q = rep_ptr[t]; q < rep_ptr[t + 1]; ++q) {
+    const UpdTask task = rep_tasks[q];
+    const int j = a.tile_col[task.a];
+    if (j >= j0) break;
+    update_tile<B>(T, a.tiles + tile_off(task.a, B), a.tiles + tile_off(task.b, B),
+                   task.rhs_row >= 0 ? a.rhs + (size_t)i * B : nullptr, ystore + (size_t)j * B);
+  }
+}
+
+// one CTA after the forward pass: the kept head's y_j (j < j0) back into the rhs for the backward pass, the new y_j
+// (j >= j0) into the store, and info as the panel launches of a full factorisation report it -- the first failed frame
+// pivot, else the first keyframe variable whose pivot failed.  A pivot p failed (!(p > 0 && p <= DBL_MAX)) exactly when
+// its stored diagonal sqrt(p) of L_jj is not positive and finite, so the kept columns need no record of their own.
+template <int B>
+__global__ void __launch_bounds__(kThreads) window_update_finish_kernel(SolveArgs a, double* ystore, const int* frame_bad,
+                                                                        int F, int j0)
+{
+  __shared__ int red[kThreads / 32];
+  const size_t split = (size_t)j0 * B, n = (size_t)a.K * B;
+  for (size_t v = threadIdx.x; v < split; v += blockDim.x) a.rhs[v] = ystore[v];
+  for (size_t v = split + threadIdx.x; v < n; v += blockDim.x) ystore[v] = a.rhs[v];
+  int first = INT_MAX;
+  for (int f = threadIdx.x; f < F; f += blockDim.x)
+    if (frame_bad[f] != 0) first = min(first, 6 * f + frame_bad[f] - 1);
+  for (int o = 16; o > 0; o >>= 1) first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = first;
+  __syncthreads();
+  int fr = INT_MAX;
+  for (int w = 0; w < kThreads / 32; ++w) fr = min(fr, red[w]);
+  __syncthreads();
+  first = INT_MAX;
+  for (int v = threadIdx.x; v < a.K * B; v += blockDim.x) {
+    const int j = v / B, r = v - j * B;
+    const double d = a.tiles[tile_off(a.num_tiles + j, B) + (size_t)r * B + r];
+    if (!(d > 0.0 && d <= 1.7976931348623157e308)) first = min(first, v);
+  }
+  for (int o = 16; o > 0; o >>= 1) first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = first;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int kf = INT_MAX;
+    for (int w = 0; w < kThreads / 32; ++w) kf = min(kf, red[w]);
+    *a.info = fr != INT_MAX ? 1 + a.K * B + fr : (kf != INT_MAX ? 1 + kf : 0);
+  }
+}
+
 template <class F>
 cudaError_t with_code_size(int code_size, F&& f)
 {
@@ -541,7 +646,25 @@ struct WindowSolverDev {
             *row_tiles = nullptr, *frame_ptr = nullptr, *frame_list = nullptr, *frame_pair = nullptr,
             *frame_kf = nullptr;
   const UpdTask* tasks = nullptr;
-  ~WindowSolverDev() { cudaFree(blob); }
+  // incremental updates (launch_window_solver_update): the update tasks grouped by target tile, in column order
+  const int* rep_ptr = nullptr;  // [num_tiles + 1]
+  const UpdTask* rep_tasks = nullptr;
+  std::vector<int> tile_row_h;   // host copies for window_solver_create_from
+  std::vector<unsigned char> fixed_h;
+  // the incremental workspace, allocated by the first update (or create_from): two loaded sets (the last update's and
+  // this one's, ping-pong), the forward pass's y, and j0
+  unsigned char* inc = nullptr;
+  LoadedSet loaded[2]{};
+  double* ystore = nullptr;
+  int* j0_dev = nullptr;
+  int cur = 0;               // loaded[cur]: the loaded system of the last update
+  mutable int reuse = 0;     // leading columns whose factor, y and stored loaded system are those of loaded[cur]
+  int j0_host = 0;
+  ~WindowSolverDev()
+  {
+    cudaFree(blob);
+    cudaFree(inc);
+  }
 };
 
 size_t window_solver_tiles(const WindowSolverDev* s) { return s ? (size_t)s->num_tiles : 0; }
@@ -658,6 +781,17 @@ cudaError_t window_solver_create(int K, int C, int F, const std::vector<int>& pa
   const Part<int> fr = lay.add<int>(F), fk = lay.add<int>(F), pt = lay.add<int>(ptiles.size()), pp = lay.add<int>(pptr.size());
   const Part<int> pf = lay.add<int>(pflat.size());
   const Part<UpdTask> tk = lay.add<UpdTask>(tasks.size());
+  // the same tasks grouped by target (column order within a target: tasks are listed column by column)
+  std::vector<int> rptr(T + 1, 0);
+  for (const UpdTask& u : tasks) ++rptr[u.target + 1];
+  for (int t = 0; t < T; ++t) rptr[t + 1] += rptr[t];
+  std::vector<UpdTask> rtasks(tasks.size());
+  {
+    std::vector<int> next(rptr.begin(), rptr.end() - 1);
+    for (const UpdTask& u : tasks) rtasks[next[u.target]++] = u;
+  }
+  const Part<int> rp = lay.add<int>(T + 1);
+  const Part<UpdTask> rk = lay.add<UpdTask>(rtasks.size());
   const Part<unsigned char> fx = lay.add<unsigned char>((size_t)K * B);
   const size_t uploaded = lay.bytes;
   const Part<double> codes = lay.add<double>((size_t)K * C), tiles = lay.add<double>((size_t)(T + K) * B * B);
@@ -679,7 +813,11 @@ cudaError_t window_solver_create(int K, int C, int F, const std::vector<int>& pa
   std::copy(pptr.begin(), pptr.end(), pp.at(hb));
   std::copy(pflat.begin(), pflat.end(), pf.at(hb));
   std::copy(tasks.begin(), tasks.end(), tk.at(hb));
+  std::copy(rptr.begin(), rptr.end(), rp.at(hb));
+  std::copy(rtasks.begin(), rtasks.end(), rk.at(hb));
   for (int v : fixed_vars) fx.at(hb)[v] = 1;
+  s->tile_row_h = tile_row;
+  s->fixed_h.assign(fx.at(hb), fx.at(hb) + (size_t)K * B);
 
   cudaError_t e;
   if ((e = cudaMalloc((void**)&s->blob, lay.bytes)) != cudaSuccess) return e;
@@ -689,6 +827,7 @@ cudaError_t window_solver_create(int K, int C, int F, const std::vector<int>& pa
   s->diag_tile = dg.at(b); s->row_tiles = rt.at(b);
   s->frame_ptr = fp.at(b); s->frame_list = fl.at(b); s->frame_pair = fr.at(b); s->frame_kf = fk.at(b);
   s->tasks = tk.at(b);
+  s->rep_ptr = rp.at(b); s->rep_tasks = rk.at(b);
   s->fixed = fx.at(b); s->codes = codes.at(b); s->tiles = tiles.at(b); s->rhs = rhs.at(b);
   s->frame_L = frame_L.at(b); s->frame_bad = frame_bad.at(b);
   s->prior_tiles = (int)ptiles.size();
@@ -713,6 +852,7 @@ cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_de
                                 const double* codes_host, double* dx_dev, int32_t* info_dev, cudaStream_t stream,
                                 uint64_t* launches, bool codes_on_device)
 {
+  s->reuse = 0;  // the factor is overwritten: a later incremental update starts over
   SolveArgs a{};
   a.buf = window_dev;
   a.codes = prior > 0.0 ? s->codes : nullptr;
@@ -766,6 +906,168 @@ cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_de
     *launches += n;
     return cudaGetLastError();
   });
+}
+
+// ------------------------------------------------------------------------------------------- incremental update
+namespace {
+
+cudaError_t ensure_incremental(WindowSolverDev* s)
+{
+  if (s->inc) return cudaSuccess;
+  const size_t K = s->K, B = s->B, T = s->num_tiles;
+  Layout lay;
+  const Part<double> t0 = lay.add<double>(T * B * B), r0 = lay.add<double>(K * B);
+  const Part<double> t1 = lay.add<double>(T * B * B), r1 = lay.add<double>(K * B);
+  const Part<double> ys = lay.add<double>(K * B);
+  const Part<int> j0 = lay.add<int>(1);
+  cudaError_t e = cudaMalloc((void**)&s->inc, lay.bytes);
+  if (e != cudaSuccess) return e;
+  s->loaded[0] = {t0.at(s->inc), r0.at(s->inc)};
+  s->loaded[1] = {t1.at(s->inc), r1.at(s->inc)};
+  s->ystore = ys.at(s->inc);
+  s->j0_dev = j0.at(s->inc);
+  return cudaSuccess;
+}
+
+}  // namespace
+
+cudaError_t launch_window_solver_update(WindowSolverDev* s, const float* window_dev, double prior, double diag_eps,
+                                        const double* codes_host, double* dx_dev, int32_t* info_dev,
+                                        cudaStream_t stream, uint64_t* launches, int* first_column)
+{
+  const int reuse = s->reuse;
+  s->reuse = 0;  // until this update completes
+  cudaError_t e = ensure_incremental(s);
+  if (e != cudaSuccess) return e;
+  SolveArgs a{};
+  a.buf = window_dev;
+  a.codes = prior > 0.0 ? s->codes : nullptr;
+  a.tiles = s->tiles; a.rhs = s->rhs; a.dx = dx_dev; a.info = info_dev;
+  a.tile_row = s->tile_row; a.tile_col = s->tile_col; a.contrib_ptr = s->contrib_ptr; a.contrib = s->contrib;
+  a.diag_tile = s->diag_tile; a.fixed = s->fixed;
+  a.K = s->K; a.P = s->P; a.num_tiles = s->num_tiles;
+  a.lambda = 0.0; a.prior = prior; a.diag_eps = diag_eps;
+  FrameArgs fa{};
+  fa.L = s->L; fa.F = s->F;
+  fa.frame_ptr = s->frame_ptr; fa.frame_list = s->frame_list; fa.frame_pair = s->frame_pair; fa.frame_kf = s->frame_kf;
+  fa.frame_L = s->frame_L; fa.frame_bad = s->frame_bad;
+  if (prior > 0.0) {
+    e = cudaMemcpyAsync(s->codes, codes_host, (size_t)s->K * s->C * sizeof(double), cudaMemcpyHostToDevice, stream);
+    if (e != cudaSuccess) return e;
+  }
+  const LoadedSet now = s->loaded[1 - s->cur], before = s->loaded[s->cur];
+  SolveArgs al = a;  // the load launches write the new loaded set
+  al.tiles = now.tiles; al.rhs = now.rhs;
+  uint64_t n = 0;
+  e = with_code_size(s->C, [&](auto bc) {
+    constexpr int Bv = bc.value;
+    if (s->F > 0)
+      window_solve_load_kernel<Bv, true, true><<<s->num_tiles, kThreads, 0, stream>>>(al, fa);
+    else
+      window_solve_load_kernel<Bv, false, true><<<s->num_tiles, kThreads, 0, stream>>>(al, fa);
+    ++n;
+    if (s->prior_tiles > 0) {
+      window_solve_prior_load_kernel<Bv><<<s->prior_tiles, kThreads, 0, stream>>>(al, s->pa);
+      ++n;
+    }
+    return cudaGetLastError();
+  });
+  if (e != cudaSuccess) return e;
+  int j0 = 0;
+  if (reuse > 0) {
+    // the first changed column decides how many column launches follow: the call's one synchronisation
+    s->j0_host = reuse;
+    if ((e = cudaMemcpyAsync(s->j0_dev, &s->j0_host, sizeof(int), cudaMemcpyHostToDevice, stream)) != cudaSuccess)
+      return e;
+    window_update_diff_kernel<<<reuse, kThreads, 0, stream>>>(now, before, s->diag_tile, s->K, s->num_tiles, s->B,
+                                                               s->j0_dev);
+    ++n;
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if ((e = cudaMemcpyAsync(&s->j0_host, s->j0_dev, sizeof(int), cudaMemcpyDeviceToHost, stream)) != cudaSuccess)
+      return e;
+    if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
+    j0 = s->j0_host;
+  }
+  s->cur = 1 - s->cur;  // this update's loaded system is the stored one from here on
+  e = with_code_size(s->C, [&](auto bc) {
+    constexpr int Bv = bc.value;
+    if (j0 < s->K) {
+      const int t0 = s->col_ptr[j0];
+      window_update_replay_kernel<Bv><<<s->num_tiles - t0, kThreads, 0, stream>>>(a, now, s->ystore, s->rep_ptr,
+                                                                                   s->rep_tasks, t0, j0);
+      ++n;
+    }
+    for (int j = j0; j < s->K; ++j) {
+      const int c0 = s->col_ptr[j], nc = s->col_ptr[j + 1] - c0;
+      window_solve_panel_kernel<Bv><<<nc, kThreads, PanelCfg<Bv>::kSmem, stream>>>(a, j, c0, s->frame_bad, s->F);
+      ++n;
+      const int u0 = s->upd_ptr[j], nu = s->upd_ptr[j + 1] - u0;
+      if (nu > 0) {
+        window_solve_update_kernel<Bv><<<nu, kThreads, 0, stream>>>(a, s->tasks + u0, j);
+        ++n;
+      }
+    }
+    window_update_finish_kernel<Bv><<<1, kThreads, 0, stream>>>(a, s->ystore, s->frame_bad, s->F, j0);
+    ++n;
+    for (int j = s->K - 1; j >= 0; --j) {
+      const int r0 = s->row_ptr[j], nr = s->row_ptr[j + 1] - r0;
+      window_solve_backward_kernel<Bv><<<1 + nr, kThreads, (Bv * Bv + Bv) * 8, stream>>>(a, s->row_tiles + r0, j);
+      ++n;
+    }
+    if (s->F > 0) {
+      window_solve_frames_kernel<Bv><<<s->F, 32, 0, stream>>>(a, fa);
+      ++n;
+    }
+    return cudaGetLastError();
+  });
+  *launches += n;
+  if (e != cudaSuccess) return e;
+  s->reuse = s->K;
+  *first_column = j0;
+  return cudaSuccess;
+}
+
+int window_solver_reusable_columns(const WindowSolverDev* prev, const WindowSolverDev* s)
+{
+  const int K = std::min(prev->K, s->K);
+  int j = 0;
+  for (; j < K; ++j) {
+    const int a0 = prev->col_ptr[j], a1 = prev->col_ptr[j + 1], b0 = s->col_ptr[j], b1 = s->col_ptr[j + 1];
+    if (a0 != b0 || a1 - a0 != b1 - b0 ||
+        !std::equal(prev->tile_row_h.begin() + a0, prev->tile_row_h.begin() + a1, s->tile_row_h.begin() + b0))
+      break;
+  }
+  return j;
+}
+
+bool window_solver_extends(const WindowSolverDev* prev, const WindowSolverDev* s)
+{
+  if (prev->C != s->C || prev->K > s->K) return false;
+  return std::equal(prev->fixed_h.begin(), prev->fixed_h.end(), s->fixed_h.begin());
+}
+
+cudaError_t window_solver_adopt(WindowSolverDev* s, const WindowSolverDev* prev, cudaStream_t stream, int* columns)
+{
+  const int p = std::min(window_solver_reusable_columns(prev, s), prev->reuse);
+  *columns = p;
+  if (p == 0) return cudaSuccess;
+  cudaError_t e = ensure_incremental(s);
+  if (e != cudaSuccess) return e;
+  const size_t BB = (size_t)s->B * s->B * sizeof(double), rows = (size_t)p * s->B * sizeof(double);
+  const size_t head = (size_t)s->col_ptr[p] * BB;  // the same tiles in both: columns < p are numbered alike
+  const LoadedSet& src = prev->loaded[prev->cur];
+  const LoadedSet& dst = s->loaded[s->cur];
+  const struct { void* d; const void* s; size_t n; } copies[] = {
+      {s->tiles, prev->tiles, head},
+      {s->tiles + (size_t)s->num_tiles * s->B * s->B, prev->tiles + (size_t)prev->num_tiles * prev->B * prev->B,
+       (size_t)p * BB},  // L_jj slots
+      {dst.tiles, src.tiles, head},
+      {dst.rhs, src.rhs, rows},
+      {s->ystore, prev->ystore, rows}};
+  for (const auto& c : copies)
+    if ((e = cudaMemcpyAsync(c.d, c.s, c.n, cudaMemcpyDeviceToDevice, stream)) != cudaSuccess) return e;
+  s->reuse = p;
+  return cudaSuccess;
 }
 
 // ----------------------------------------------------------------------------------- keyframe marginalisation

@@ -331,6 +331,240 @@ def apply_update(poses: np.ndarray, codes: np.ndarray, dx: np.ndarray, code_size
     return new_p, new_c, new_f
 
 
+def diag_eps_of(layout: WindowBlocks, buf, fixed: Sequence[int] = (), code_prior_weight: float = 0.0) -> float:
+    """1e-12 max|d| of a buffer's system over the kept variables, the code prior included (what damped_solve and
+    dfk_window_solve add to the diagonal): IncrementalOptimizer's fixed diag_eps"""
+    H, _, _, _ = layout.to_dense(buf)
+    d = np.array(H.diagonal().cpu().numpy() if hasattr(H, "detach") else np.diag(H), dtype=np.float64)
+    if code_prior_weight > 0:
+        B = layout.B
+        for k in range(layout.num_keyframes):
+            d[k * B + 6:(k + 1) * B] += code_prior_weight
+    keep = np.ones(d.size, dtype=bool)
+    keep[list(fixed)] = False
+    return 1e-12 * float(np.abs(d[keep]).max())
+
+
+def solver_columns(K: int, pairs, links=(), kf_priors=()) -> List[List[int]]:
+    """The tile pattern of the window solver's factor (dfk_window_solver_create's symbolic analysis): the rows i > j of
+    the nonzero tiles of every keyframe column j, fill included.  A frame pair (k1 >= K) makes no tile."""
+    below = [set() for _ in range(K)]
+    for a, b in list(pairs) + list(links):
+        if a != b and a < K and b < K:
+            below[min(a, b)].add(max(a, b))
+    for p in kf_priors:
+        p = sorted(int(v) for v in p)
+        for x in range(len(p)):
+            for y in range(x + 1, len(p)):
+                below[p[x]].add(p[y])
+    for j in range(K):
+        rows = sorted(below[j])
+        for x in range(len(rows)):
+            for y in range(x):
+                below[rows[y]].add(rows[x])
+    return [sorted(b) for b in below]
+
+
+def reusable_columns(old: WindowBlocks, new: WindowBlocks, old_fixed: Sequence[int] = (),
+                     new_fixed: Sequence[int] = ()) -> int:
+    """The growth rule of dfk_window_solver_create_from: the longest prefix of keyframe columns whose tile pattern the
+    grown window keeps.  Raises ValueError when `new` does not extend `old` (fewer keyframes, another code size, other
+    fixed variables among the old keyframes)."""
+    K0 = old.num_keyframes
+    if new.code_size != old.code_size or new.num_keyframes < K0:
+        raise ValueError("the window does not extend the old one")
+    n0 = K0 * old.B
+    if sorted(int(v) for v in old_fixed) != sorted(int(v) for v in new_fixed if int(v) < n0):
+        raise ValueError("the window fixes other variables among the old keyframes")
+    a = solver_columns(K0, old.pairs, old.geometric, old.kf_priors)
+    b = solver_columns(new.num_keyframes, new.pairs, new.geometric, new.kf_priors)
+    j = 0
+    while j < K0 and a[j] == b[j]:
+        j += 1
+    return j
+
+
+@dataclass
+class ISAM2Result:
+    """What one IncrementalOptimizer.update did (gtsam::ISAM2Result's counts)"""
+    variables_relinearized: int   # keys whose linearisation point moved (pose and code keys counted apart)
+    variables_reeliminated: int   # scalar variables re-factorised: (K - first_column) B + 6 F
+    factors_relinearised: int     # factors re-evaluated: the new ones and those that depend on a relinearised key
+    first_column: int             # the solver's first re-factorised keyframe column (K: none)
+
+
+class IncrementalOptimizer:
+    """The reference's mapping step (Mapper::MappingStep, one ISAM2::update per step) on the incremental window solver:
+    Gauss-Newton, Cholesky in keyframe order, relinearize_threshold / relinearize_skip as ISAM2Params.
+
+    Every key -- the pose and the code of each keyframe, the pose of each tracked frame -- has a linearisation point
+    theta_lin and the last full delta.  update() runs, in GTSAM's order:
+      1. every relinearize_skip-th update, the relinearisation check on the previous delta: a key with
+         max|delta_key| >= relinearize_threshold gets theta_lin <- theta_lin (+) delta_key;
+      2. linearise at theta_lin: the linearisation cache re-evaluates only the new factors and those that depend on a
+         relinearised key (every other key's theta_lin is unchanged bit for bit);
+      3. the incremental solve gives the full delta from theta_lin (re-factorising from the first changed column);
+      4. the estimate is theta_lin (+) delta (apply_update's retraction).
+    The check is GTSAM's full one (not the partial check), and back-substitution always runs in full.
+    MappingStep calls update with force_relinearize = true (mapper.cpp:520-521), which runs the check every step
+    whatever relinearizeSkip is: reproduce it with relinearize_skip = 1.  Its threshold is the float 0.05f
+    (0.0500000007 as a double); relinearize_threshold=float(np.float32(0.05)) reproduces that edge exactly.
+
+    `linearise(poses, codes, todo[, frame_poses]) -> (buf, _)` is WindowOptimizer's; `solve(buf, diag_eps, codes) ->
+    (dx, first_column)` the incremental solve (from_problem: WindowSolver.update).  diag_eps is fixed for the optimiser's
+    lifetime: 1e-12 max|d| of the first linearisation, so that later solves can reuse columns.  grow() adds keyframes,
+    factors and frames and carries the kept factors' cache entries over."""
+
+    def __init__(self, layout: WindowBlocks, linearise: Callable, solve: Callable, poses, codes, frame_poses=None,
+                 relinearize_threshold: float = 0.05, relinearize_skip: int = 1, code_prior_weight: float = 0.0,
+                 fix_first_pose: bool = True, cache_eps: float = 1e-6):
+        if relinearize_skip < 1:
+            raise ValueError("relinearize_skip must be >= 1")
+        self.relinearize_threshold = float(relinearize_threshold)
+        self.relinearize_skip = int(relinearize_skip)
+        self.code_prior_weight = float(code_prior_weight)
+        self.fixed = list(range(6)) if fix_first_pose else []
+        self.cache_eps = cache_eps
+        self.diag_eps: Optional[float] = None
+        self.update_count = 0
+        self._adopt(layout, linearise, solve)
+        self.cache = LinearisationCache(layout.pairs, cache_eps, layout.geometric)
+        self.lin_poses = np.asarray(poses, dtype=np.float64).copy()
+        self.lin_codes = np.asarray(codes, dtype=np.float64).copy()
+        self.lin_frames = np.asarray(frame_poses if frame_poses is not None else np.zeros((0, 7)),
+                                     dtype=np.float64).reshape(-1, 7).copy()
+        self._check_sizes()
+        self.delta = np.zeros(layout.dim)
+
+    @classmethod
+    def from_problem(cls, prob: "SfmWindowProblem", poses, codes, frame_poses=None, **kw) -> "IncrementalOptimizer":
+        """the optimiser of an SfmWindowProblem: its linearise, and WindowSolver.update on its window"""
+        opt = cls(prob.layout, prob.linearise, None, poses, codes, frame_poses, **kw)
+        opt._solver_of(prob.window, None)
+        return opt
+
+    def _adopt(self, layout, linearise, solve):
+        self.layout, self.linearise, self.solve = layout, linearise, solve
+
+    def _solver_of(self, window, prev):
+        from .aligners import WindowSolver
+        sol = WindowSolver(window, self.fixed) if prev is None else prev.grown(window, self.fixed)
+        self.solver = sol
+
+        def solve(buf, diag_eps, codes):
+            dx, j0 = sol.update(buf, diag_eps, self.code_prior_weight, codes if self.code_prior_weight > 0 else None)
+            if int(sol.info.cpu().item()) != 0:
+                raise RuntimeError(f"the window's system is not positive definite (variable {int(sol.info.item()) - 1})")
+            return dx.cpu().numpy(), j0
+        self.solve = solve
+
+    def _check_sizes(self):
+        K, F = self.layout.num_keyframes, self.layout.num_frames
+        if self.lin_poses.shape != (K, 7) or self.lin_codes.shape != (K, self.layout.code_size) or \
+                self.lin_frames.shape != (F, 7):
+            raise ValueError(f"the window has {K} keyframes of code size {self.layout.code_size} and {F} frames")
+
+    def _keys(self):
+        """(kind, index, slice of the delta) of every key: pose and code of each keyframe, then each frame's pose"""
+        K, B = self.layout.num_keyframes, self.layout.B
+        out = []
+        for k in range(K):
+            out += [("pose", k, slice(k * B, k * B + 6)), ("code", k, slice(k * B + 6, (k + 1) * B))]
+        return out + [("frame", f, slice(K * B + 6 * f, K * B + 6 * f + 6)) for f in range(self.layout.num_frames)]
+
+    def relinearize_keys(self) -> List[Tuple[str, int]]:
+        """the keys whose previous delta reaches the threshold (max |delta_key| >= relinearize_threshold)"""
+        return [(kind, i) for kind, i, sl in self._keys()
+                if np.abs(self.delta[sl]).max(initial=0.0) >= self.relinearize_threshold]
+
+    def estimate(self):
+        """theta_lin (+) delta: (poses, codes, frame_poses)"""
+        return apply_update(self.lin_poses, self.lin_codes, self.delta, self.layout.code_size, self.lin_frames)
+
+    def update(self) -> ISAM2Result:
+        self.update_count += 1
+        moved = []
+        if self.update_count % self.relinearize_skip == 0:
+            moved = self.relinearize_keys()
+            for kind, i, sl in self._keys():
+                if (kind, i) not in moved:
+                    continue
+                d = self.delta[sl]
+                if kind == "pose":
+                    self.lin_poses[i] = se3.retract(self.lin_poses[i], d, np.float64)
+                elif kind == "code":
+                    self.lin_codes[i] = self.lin_codes[i] + d
+                else:
+                    self.lin_frames[i] = se3.retract(self.lin_frames[i], d, np.float64)
+                self.delta[sl] = 0.0
+        frames = self.lin_frames if self.layout.num_frames else None
+        todo = self.cache.stale(self.lin_poses, self.lin_codes, frames)
+        if frames is None:
+            buf, _ = self.linearise(self.lin_poses, self.lin_codes, todo)
+        else:
+            buf, _ = self.linearise(self.lin_poses, self.lin_codes, todo, frames)
+        self.cache.store(todo, self.lin_poses, self.lin_codes, frames)
+        if self.diag_eps is None:
+            self.diag_eps = diag_eps_of(self.layout, buf, self.fixed, self.code_prior_weight)
+        dx, j0 = self.solve(buf, self.diag_eps, self.lin_codes)
+        self.delta = np.asarray(dx, dtype=np.float64).copy()
+        K, B = self.layout.num_keyframes, self.layout.B
+        return ISAM2Result(len(moved), (K - int(j0)) * B + 6 * self.layout.num_frames, len(todo), int(j0))
+
+    def grow(self, layout: WindowBlocks, linearise: Callable, poses, codes, frame_poses=None,
+             factor_of: Optional[Sequence[Optional[int]]] = None, frame_of: Optional[Sequence[Optional[int]]] = None,
+             window=None, solve: Optional[Callable] = None):
+        """Move to a grown window whose first keyframes are this one's (keyframes appended in index order, factors and
+        frames added or removed; no slide).  poses / codes: the new keyframes' initial estimates after the old ones'
+        (the old rows are ignored: the old keys keep theta_lin and delta); frame_poses: every frame's estimate, kept
+        frames' rows ignored.  factor_of[i] / frame_of[f]: the old index of new factor i (cache numbering) / frame f,
+        None for a new one (default: the old ones first, in order).  window: the new Window when the optimiser runs on
+        WindowSolver (from_problem): the solver grows from the old one (WindowSolver.grown); else `solve`."""
+        K0, B0 = self.layout.num_keyframes, self.layout.B
+        K, F = layout.num_keyframes, layout.num_frames
+        if layout.code_size != self.layout.code_size or K < K0:
+            raise ValueError("a grown window keeps the old keyframes first, with the same code size")
+        old_keys = len(self.cache._at)
+        factor_of = list(factor_of) if factor_of is not None else \
+            [i if i < old_keys else None for i in range(len(layout.pairs) + len(layout.geometric))]
+        frame_of = list(frame_of) if frame_of is not None else [f if f < len(self.lin_frames) else None for f in range(F)]
+        poses, codes = np.asarray(poses, np.float64), np.asarray(codes, np.float64)
+        lin_p = np.concatenate([self.lin_poses, poses[K0:K]]).reshape(K, 7)
+        lin_c = np.concatenate([self.lin_codes, codes[K0:K]]).reshape(K, layout.code_size)
+        fp = np.asarray(frame_poses if frame_poses is not None else np.zeros((0, 7)), np.float64).reshape(-1, 7)
+        lin_f = np.stack([self.lin_frames[o] if o is not None else fp[f] for f, o in enumerate(frame_of)]) \
+            if F else np.zeros((0, 7))
+        delta = np.zeros(layout.dim)
+        delta[:K0 * B0] = self.delta[:K0 * B0]
+        for f, o in enumerate(frame_of):
+            if o is not None:
+                delta[K * B0 + 6 * f:K * B0 + 6 * f + 6] = self.delta[K0 * B0 + 6 * o:K0 * B0 + 6 * o + 6]
+        cache = LinearisationCache(layout.pairs, self.cache_eps, layout.geometric)
+        for i, o in enumerate(factor_of):
+            if o is not None:
+                cache._at[i] = self.cache._at[o]
+        prev = getattr(self, "solver", None)
+        self._adopt(layout, linearise, solve)
+        self.cache, self.lin_poses, self.lin_codes, self.lin_frames, self.delta = cache, lin_p, lin_c, lin_f, delta
+        self._check_sizes()
+        if window is not None:
+            self._solver_of(window, prev)
+        elif solve is None:
+            raise ValueError("grow needs the new window (WindowSolver) or a solve")
+
+    def grow_problem(self, old: "SfmWindowProblem", prob: "SfmWindowProblem", poses, codes,
+                     frame_poses: Optional[np.ndarray], factor_of: Sequence[Optional[int]],
+                     frame_of: Sequence[Optional[int]]):
+        """grow() onto a grown SfmWindowProblem (from_problem's optimiser): the kept factors' records are copied from
+        the old problem (carry_records, which checks every kept factor's kind and ends) with their cache entries, and
+        the solver grows from the old window's.  factor_of and frame_of are required: SfmWindowProblem numbers its
+        factors by kind (photometric pairs, reprojection links, frame pairs, geometric links), so a new photometric
+        pair shifts every later factor and no positional default is right."""
+        factor_of, frame_of = list(factor_of), list(frame_of)
+        prob.carry_records(old, factor_of, frame_of)
+        self.grow(prob.layout, prob.linearise, poses, codes, frame_poses, factor_of, frame_of, window=prob.window)
+
+
 class WindowOptimizer:
     """Levenberg-Marquardt over the poses and codes of a keyframe window.
 
@@ -1251,6 +1485,40 @@ class SfmWindowProblem:
         depth = [dataclasses.replace(dp, k=int(dp.k) - (int(dp.k) > m)) for dp in self.depth_priors if dp.k != m]
         return SfmWindowProblem(self.al, self.cams, self.kf[:m] + self.kf[m + 1:], pairs, self.allreduce, links, geo,
                                 frames, priors, depth)
+
+    def carry_records(self, old: "SfmWindowProblem", factor_of: Sequence[Optional[int]],
+                      frame_of: Sequence[Optional[int]]):
+        """Copy the records of the factors this problem keeps from `old` (a grown map: IncrementalOptimizer.grow_problem).
+        factor_of[i]: the old `todo` index of this problem's factor i (photometric pairs, reprojection links, frame
+        pairs, geometric links), None for a new one; frame_of[f]: the old index of frame f, None for a new one.  A kept
+        factor must keep its kind and its ends (keyframes keep their indices; a frame pair's frame maps by frame_of):
+        anything else raises ValueError before a record is copied."""
+        import torch
+        K, K0 = len(self.kf), len(old.kf)
+        if len(factor_of) != len(self.pairs) + len(self.geometric) or len(frame_of) != len(self.frames):
+            raise ValueError("factor_of needs one entry per factor and frame_of one per frame")
+        copies = []
+        for kind, kd in self._kinds.items():
+            okd = old._kinds[kind]
+            src, dst = [], []
+            for j in range(len(kd.ends)):
+                o = factor_of[kd.first + j]
+                if o is None:
+                    continue
+                if not okd.first <= o < okd.first + len(okd.ends):
+                    raise ValueError(f"factor {kd.first + j} ({kind}) is old factor {o} of another kind")
+                (a, b), (oa, ob) = kd.ends[j], okd.ends[o - okd.first]
+                same = a == oa and (b == ob if b < K else ob >= K0 and frame_of[b - K] == ob - K0)
+                if not same:
+                    raise ValueError(f"factor {kd.first + j} ({kind}, ends {(a, b)}) is not old factor {o} "
+                                     f"(ends {(oa, ob)})")
+                src += range(okd.row0 + (o - okd.first) * okd.rows, okd.row0 + (o - okd.first + 1) * okd.rows)
+                dst += range(kd.row0 + j * kd.rows, kd.row0 + (j + 1) * kd.rows)
+            if dst:
+                copies.append((kd.base, okd.base, dst, src))
+        for base, obase, dst, src in copies:
+            dev = base.device
+            base.index_copy_(0, torch.as_tensor(dst, device=dev), obase.index_select(0, torch.as_tensor(src, device=dev)))
 
     def marginalize(self, poses, codes, frame_poses, which) -> List[MarginalPrior]:
         """Marginalise the frames `which` at the current point (MarginalizeFrames): their pairs are re-evaluated at

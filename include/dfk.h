@@ -405,6 +405,44 @@ typedef struct {
 DfkStatus dfk_window_solve(DfkHandle h, const DfkWindowSolver* s, const float* window_dev, const DfkWindowSolveParams* p,
                            const double* codes, double* dx_dev, int32_t* info_dev);
 
+/* Incremental Gauss-Newton solve (ISAM2's re-elimination of the changed part of the map, with a Cholesky factor in
+ * keyframe order).  The system is dfk_window_solve's with two changes: no lambda, and step 3 adds the caller's absolute
+ * diag_eps (>= 0, finite) to every kept diagonal entry, the frames' included, instead of 1e-12 max|d|.
+ * The solver keeps the loaded system of its last update: every tile after the load (blocks, frame elimination, keyframe
+ * priors, code prior, fixed rows, diag_eps) and every right-hand-side block, with the factor and the forward pass.  An
+ * update loads the buffer in one launch, finds the first keyframe column j0 whose loaded tiles or rhs block differ bit
+ * for bit from the stored ones, re-applies the kept columns' (< j0) updates to the reloaded tiles of columns >= j0 in
+ * column order with the factorisation's own arithmetic (one launch), re-factorises columns j0 .. K-1, and runs the
+ * backward pass in full and the frame launch.  dx and info are bit for bit those of a fresh solver's first update of
+ * the same buffer.  *first_column (HOST) = j0; K means nothing changed.  j0 comes back to the host in one 4-byte
+ * read-back (the number of column launches depends on it): that is the call's one stream synchronisation; a solver
+ * with nothing to reuse (fresh, or used by dfk_window_solve since its last update, which starts over at j0 = 0) skips
+ * it and stays asynchronous.  Launches: load (+ prior load), compare, replay, a panel and an update launch per column
+ * from j0, one finishing launch (info, forward pass store), a backward launch per keyframe, and the frames.
+ * info_dev reports a failed pivot exactly as dfk_window_solve does (dx is then zero).
+ * The first update allocates the incremental workspace: 2 (tiles B^2 + K B) + K B doubles (two loaded systems, the
+ * last one and the one being compared, and the forward pass), which roughly triples the solver's device memory. */
+typedef struct {
+  double code_prior_weight; /* >= 0, finite; 0 = no prior */
+  double diag_eps;          /* >= 0, finite: added to every kept diagonal entry */
+} DfkWindowUpdateParams;
+
+DfkStatus dfk_window_solver_update(DfkHandle h, DfkWindowSolver* s, const float* window_dev,
+                                   const DfkWindowUpdateParams* p, const double* codes, double* dx_dev,
+                                   int32_t* info_dev, int32_t* first_column);
+
+/* A solver for window w that takes over what prev holds (growth of the map: keyframes appended in index order, new
+ * pairs, links and tracked frames).  prev's K_old keyframes must be w's first K_old keyframes, with the same code size
+ * and the same fixed variables among them (fixed_vars as dfk_window_solver_create takes them); otherwise the call
+ * returns DFK_ERR_INVALID_ARG and writes nothing.  A slide renumbers keyframes and is not supported.  The symbolic
+ * analysis finds the longest prefix of keyframe columns whose tile pattern is unchanged: a column changes when it gains
+ * a tile, which happens to the column of every back connection or link of a new keyframe and to column j of a new
+ * link or pair (i, j), j < i, between old keyframes; the fill of those columns lands only in later columns.  That
+ * prefix's factor, stored loaded system and forward pass are copied (asynchronously, on the handle's stream), so the
+ * next update starts at the smaller of the prefix and the first changed column.  prev is left as it was. */
+DfkStatus dfk_window_solver_create_from(DfkHandle h, const DfkWindow* w, int num_fixed, const int32_t* fixed_vars,
+                                        const DfkWindowSolver* prev, DfkWindowSolver** out);
+
 /* ------------------------------------------------------------------ SE3Aligner */
 
 /* SE3Aligner<float>::RunStep (cu_se3aligner.h:65-70, cu_se3aligner.cpp:153-176):
