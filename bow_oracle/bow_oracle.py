@@ -43,6 +43,12 @@ def lib():
         L.dfkb_query.argtypes = [_P, _P, C.c_int, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P]
         L.dfkb_score.restype = C.c_double
         L.dfkb_score.argtypes = [_P, _P, C.c_int, _P, _P, C.c_int]
+        L.dfkb_train.restype = _P
+        L.dfkb_train.argtypes = [_P, C.c_int64, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_uint64]
+        L.dfkb_train_nodes.restype = C.c_int
+        L.dfkb_train_nodes.argtypes = [_P]
+        L.dfkb_train_get.argtypes = [_P, _P, _P, _P, _P]
+        L.dfkb_train_free.argtypes = [_P]
         _lib = L
     return _lib
 
@@ -126,3 +132,50 @@ def score(aw, av, bw, bv) -> float:
     """L1Scoring::score(a, b)"""
     aw, av, bw, bv = _a(aw, np.int32), _a(av, np.float64), _a(bw, np.int32), _a(bv, np.float64)
     return float(lib().dfkb_score(aw.ctypes.data, av.ctypes.data, len(aw), bw.ctypes.data, bv.ctypes.data, len(bw)))
+
+
+def save_order(parent_ids):
+    """DBoW2 save's node order from parent ids by id (index id - 1, children as consecutive ascending ids): a stack of
+    parents from the root; pop the last, list its children, push each that has children"""
+    parent_ids = np.asarray(parent_ids)
+    n = len(parent_ids)
+    kids = [[] for _ in range(n + 1)]
+    for i, p in enumerate(parent_ids):
+        kids[int(p)].append(i + 1)
+    order, stack = [], [0]
+    while stack:
+        p = stack.pop()
+        for c in kids[p]:
+            order.append(c)
+            if kids[c]:
+                stack.append(c)
+    return np.array(order, np.int64), kids
+
+
+def train(descriptors, image_offsets, k: int, L: int, seed: int):
+    """TemplatedVocabulary::create of the block in include/dfk.h, sequential and depth first: (the vocabulary dict of
+    load_dbow2_vocabulary in save order, stats dict)"""
+    d = _a(descriptors, np.uint8)
+    D = d.shape[1]
+    off = _a(image_offsets, np.int64)
+    p = lib().dfkb_train(d.ctypes.data, d.shape[0], D, off.ctypes.data, len(off) - 1, int(k), int(L),
+                         C.c_uint64(int(seed) & (2 ** 64 - 1)))
+    if not p:
+        raise MemoryError("bow oracle: out of memory")
+    try:
+        n = lib().dfkb_train_nodes(p)
+        par = np.zeros(n, np.int32)
+        wt = np.zeros(n, np.float64)
+        desc = np.zeros((n, D), np.uint8)
+        st = np.zeros(5 + 16, np.int32)
+        lib().dfkb_train_get(p, par.ctypes.data, wt.ctypes.data, desc.ctypes.data, st.ctypes.data)
+    finally:
+        lib().dfkb_train_free(p)
+    order, kids = save_order(par)
+    leaves = np.array([i for i in range(1, n + 1) if not kids[i]], np.int32)
+    voc = dict(k=int(k), L=int(L), weighting=0, scoring=0, descriptor_bytes=D, node_ids=order.astype(np.int32),
+               parent_ids=par[order - 1], weights=wt[order - 1], descriptors=desc[order - 1],
+               word_ids=np.arange(len(leaves), dtype=np.int32), word_nodes=leaves)
+    stats = dict(zip(("num_nodes", "num_words", "max_rounds", "capped_nodes", "empty_clusters"), map(int, st[:5])))
+    stats["level_max_rounds"] = [int(v) for v in st[5:]]
+    return voc, stats

@@ -11,6 +11,8 @@
 
 #include "dfk_bow_model.h"
 
+#define DFK_BOW_TRAIN_MAX_ROUNDS 1000 /* include/dfk.h */
+
 typedef struct {
   int n, d32;          /* listed nodes, descriptor words */
   int* first;          /* [n + 2]: children of node id p are kids[first[p] .. first[p + 1]) */
@@ -205,4 +207,268 @@ double dfkb_score(const int32_t* aw, const double* av, int an, const int32_t* bw
     }
   }
   return dfk_bow_final_score(score);
+}
+
+/* ---- vocabulary training: include/dfk.h's DBoW2 training block, followed literally -----------------------------
+ * TemplatedVocabulary::create as DBoW2 runs it: HKmeansStep one node at a time in its depth-first recursion, min_dist
+ * and its sums in double as DBoW2 keeps them, then createWords and setNodeWeights with a descent per descriptor.  The
+ * random draws are dfk_bow_model.h's per-node streams (the block's deviation 1). */
+typedef struct {
+  int n, cap, k, L, bytes, d32;
+  int32_t* parent;     /* [id] */
+  int32_t* first;      /* [id] first child id (children are consecutive ids) */
+  int32_t* nchild;     /* [id] */
+  uint64_t* key;       /* [id] */
+  double* weight;      /* [id] */
+  uint32_t* desc;      /* [id, d32] */
+  int32_t stats[5 + 16]; /* num_nodes, num_words, max_rounds, capped_nodes, empty_clusters, level_max_rounds[16] */
+  int failed;
+} Tree;
+
+static int tree_add(Tree* t, int parent, const uint32_t* d)
+{
+  if (t->n == t->cap) {
+    const int cap = t->cap ? 2 * t->cap : 1024;
+    t->parent = (int32_t*)realloc(t->parent, sizeof(int32_t) * (size_t)cap);
+    t->first = (int32_t*)realloc(t->first, sizeof(int32_t) * (size_t)cap);
+    t->nchild = (int32_t*)realloc(t->nchild, sizeof(int32_t) * (size_t)cap);
+    t->key = (uint64_t*)realloc(t->key, sizeof(uint64_t) * (size_t)cap);
+    t->weight = (double*)realloc(t->weight, sizeof(double) * (size_t)cap);
+    t->desc = (uint32_t*)realloc(t->desc, sizeof(uint32_t) * (size_t)cap * t->d32);
+    if (!t->parent || !t->first || !t->nchild || !t->key || !t->weight || !t->desc) {
+      t->failed = 1;
+      return -1;
+    }
+    t->cap = cap;
+  }
+  const int id = t->n++;
+  t->parent[id] = parent;
+  t->first[id] = 0;
+  t->nchild[id] = 0;
+  t->key[id] = 0;
+  t->weight[id] = 0.0;
+  memcpy(t->desc + (size_t)id * t->d32, d, sizeof(uint32_t) * t->d32);
+  return id;
+}
+
+static void hkmeans_step(Tree* t, const uint32_t* X, int parent, const int* idx, int m, int level)
+{
+  if (m == 0 || t->failed) return;
+  const int k = t->k, W = t->d32;
+  uint32_t* clusters = (uint32_t*)calloc((size_t)k * W, sizeof(uint32_t));
+  int* assoc = (int*)malloc(sizeof(int) * (size_t)m);
+  int* last = (int*)malloc(sizeof(int) * (size_t)m);
+  int* gsize = (int*)calloc((size_t)k, sizeof(int));
+  if (!clusters || !assoc || !last || !gsize) {
+    t->failed = 1;
+    return;
+  }
+  int nc = 0;
+  if (m <= k) {
+    for (int i = 0; i < m; ++i) {
+      memcpy(clusters + (size_t)i * W, X + (size_t)idx[i] * W, sizeof(uint32_t) * W);
+      assoc[i] = i;
+      gsize[i] = 1;
+    }
+    nc = m;
+  } else {
+    uint64_t s = t->key[parent];
+    /* initiateClustersKMpp */
+    double* min_dists = (double*)malloc(sizeof(double) * (size_t)m);
+    if (!min_dists) {
+      t->failed = 1;
+      return;
+    }
+    int ifeature = (int)dfk_bow_draw_index(&s, m);
+    memcpy(clusters, X + (size_t)idx[ifeature] * W, sizeof(uint32_t) * W);
+    nc = 1;
+    for (int i = 0; i < m; ++i) min_dists[i] = (double)dfk_bow_distance(X + (size_t)idx[i] * W, clusters, W);
+    while (nc < k) {
+      for (int i = 0; i < m; ++i)
+        if (min_dists[i] > 0) {
+          const double d = (double)dfk_bow_distance(X + (size_t)idx[i] * W, clusters + (size_t)(nc - 1) * W, W);
+          if (d < min_dists[i]) min_dists[i] = d;
+        }
+      double dist_sum = 0.0;
+      for (int i = 0; i < m; ++i) dist_sum += min_dists[i];
+      if (!(dist_sum > 0)) break;
+      const double cut = dfk_bow_draw_cut(&s, (int64_t)dist_sum);
+      double up = 0;
+      int i = 0;
+      for (; i < m; ++i) {
+        up += min_dists[i];
+        if (up >= cut) break;
+      }
+      ifeature = i == m ? m - 1 : i;
+      memcpy(clusters + (size_t)nc * W, X + (size_t)idx[ifeature] * W, sizeof(uint32_t) * W);
+      ++nc;
+    }
+    free(min_dists);
+    /* the rounds */
+    int* counts = (int*)malloc(sizeof(int) * (size_t)k * W * 32);
+    if (!counts) {
+      t->failed = 1;
+      return;
+    }
+    int rounds = 0, first_time = 1;
+    for (;;) {
+      if (!first_time) {
+        /* FBrisk::meanValue of each group */
+        memset(counts, 0, sizeof(int) * (size_t)k * W * 32);
+        for (int j = 0; j < m; ++j) {
+          const uint32_t* x = X + (size_t)idx[j] * W;
+          int* cc = counts + (size_t)assoc[j] * W * 32;
+          for (int b = 0; b < W * 32; ++b) cc[b] += (x[b / 32] >> (b % 32)) & 1u;
+        }
+        for (int c = 0; c < nc; ++c) {
+          uint32_t* mean = clusters + (size_t)c * W;
+          for (int b = 0; b < W * 32; ++b) {
+            if (b % 32 == 0) mean[b / 32] = 0;
+            if (counts[(size_t)c * W * 32 + b] > gsize[c] / 2) mean[b / 32] |= 1u << (b % 32);
+          }
+        }
+        memcpy(last, assoc, sizeof(int) * (size_t)m);
+      }
+      for (int c = 0; c < nc; ++c) gsize[c] = 0;
+      for (int j = 0; j < m; ++j) {
+        const uint32_t* x = X + (size_t)idx[j] * W;
+        int best = 0, bd = dfk_bow_distance(x, clusters, W);
+        for (int c = 1; c < nc; ++c) {
+          const int d = dfk_bow_distance(x, clusters + (size_t)c * W, W);
+          if (d < bd) {
+            bd = d;
+            best = c;
+          }
+        }
+        assoc[j] = best;
+        gsize[best]++;
+      }
+      ++rounds;
+      if (first_time) {
+        first_time = 0;
+        continue;
+      }
+      int same = 1;
+      for (int j = 0; j < m && same; ++j) same = assoc[j] == last[j];
+      if (same) break;
+      if (rounds == DFK_BOW_TRAIN_MAX_ROUNDS) {
+        t->stats[3]++;
+        break;
+      }
+    }
+    free(counts);
+    if (rounds > t->stats[2]) t->stats[2] = rounds;
+    if (rounds > t->stats[4 + level]) t->stats[4 + level] = rounds;
+    for (int c = 0; c < nc; ++c) t->stats[4] += gsize[c] == 0;
+  }
+  /* the children, one block of ids in cluster order */
+  const int first = t->n;
+  for (int c = 0; c < nc; ++c) {
+    const int id = tree_add(t, parent, clusters + (size_t)c * W);
+    if (id < 0) return;
+    t->key[id] = dfk_bow_child_key(t->key[parent], c);
+  }
+  t->first[parent] = first;
+  t->nchild[parent] = nc;
+  if (level < t->L) {
+    int* group = (int*)malloc(sizeof(int) * (size_t)m);
+    if (!group) {
+      t->failed = 1;
+      return;
+    }
+    for (int c = 0; c < nc; ++c) {
+      int g = 0;
+      for (int j = 0; j < m; ++j)
+        if (assoc[j] == c) group[g++] = idx[j];
+      if (g > 1) hkmeans_step(t, X, first + c, group, g, level + 1);
+    }
+    free(group);
+  }
+  free(clusters);
+  free(assoc);
+  free(last);
+  free(gsize);
+}
+
+void* dfkb_train(const uint8_t* desc, int64_t n, int bytes, const int64_t* offsets, int n_img, int k, int L,
+                 uint64_t seed)
+{
+  Tree* t = (Tree*)calloc(1, sizeof(Tree));
+  if (!t) return NULL;
+  t->k = k;
+  t->L = L;
+  t->bytes = bytes;
+  t->d32 = bytes / 4;
+  const uint32_t* X = (const uint32_t*)desc;
+  uint32_t zero[16] = {0};
+  tree_add(t, -1, zero);
+  t->key[0] = seed;
+  int* idx = (int*)malloc(sizeof(int) * (size_t)n);
+  if (!idx) return NULL;
+  for (int64_t i = 0; i < n; ++i) idx[i] = (int)i;
+  hkmeans_step(t, X, 0, idx, (int)n, 1);
+  free(idx);
+  if (t->failed) return NULL;
+  /* createWords: leaves in ascending id; setNodeWeights: N_i per word, one per image */
+  int* word = (int*)malloc(sizeof(int) * (size_t)t->n);
+  int nw = 0;
+  for (int id = 1; id < t->n; ++id) word[id] = t->nchild[id] == 0 ? nw++ : -1;
+  int* ni = (int*)calloc((size_t)nw + 1, sizeof(int));
+  int* seen = (int*)malloc(sizeof(int) * ((size_t)nw + 1));
+  for (int j = 0; j < nw; ++j) seen[j] = -1;
+  for (int img = 0; img < n_img; ++img)
+    for (int64_t f = offsets[img]; f < offsets[img + 1]; ++f) {
+      const uint32_t* x = X + (size_t)f * t->d32;
+      int id = 0;
+      do {
+        int best = t->first[id], bd = dfk_bow_distance(x, t->desc + (size_t)best * t->d32, t->d32);
+        for (int c = 1; c < t->nchild[id]; ++c) {
+          const int d = dfk_bow_distance(x, t->desc + (size_t)(t->first[id] + c) * t->d32, t->d32);
+          if (d < bd) {
+            bd = d;
+            best = t->first[id] + c;
+          }
+        }
+        id = best;
+      } while (t->nchild[id] > 0);
+      if (seen[word[id]] != img) {
+        seen[word[id]] = img;
+        ni[word[id]]++;
+      }
+    }
+  for (int id = 1; id < t->n; ++id)
+    if (word[id] >= 0 && ni[word[id]] > 0) t->weight[id] = log((double)n_img / (double)ni[word[id]]);
+  free(word);
+  free(ni);
+  free(seen);
+  t->stats[0] = t->n - 1;
+  t->stats[1] = nw;
+  return t;
+}
+
+/* the trained tree by id 1..n-1: parent, weight, descriptor; stats [5 + 16] */
+int dfkb_train_nodes(const void* p) { return ((const Tree*)p)->n - 1; }
+
+void dfkb_train_get(const void* p, int32_t* parent, double* weight, uint8_t* desc, int32_t* stats)
+{
+  const Tree* t = (const Tree*)p;
+  for (int id = 1; id < t->n; ++id) {
+    parent[id - 1] = t->parent[id];
+    weight[id - 1] = t->weight[id];
+    memcpy(desc + (size_t)(id - 1) * t->bytes, t->desc + (size_t)id * t->d32, (size_t)t->bytes);
+  }
+  memcpy(stats, t->stats, sizeof(t->stats));
+}
+
+void dfkb_train_free(void* p)
+{
+  Tree* t = (Tree*)p;
+  if (!t) return;
+  free(t->parent);
+  free(t->first);
+  free(t->nchild);
+  free(t->key);
+  free(t->weight);
+  free(t->desc);
+  free(t);
 }

@@ -213,6 +213,27 @@ class DfkBowScoreItem(C.Structure):
     _fields_ = [("entry", C.c_int32), ("vector", DfkBowVector)]
 
 
+BOW_TRAIN_MAX_ROUNDS = 1000  # DFK_BOW_TRAIN_MAX_ROUNDS
+BOW_TRAIN_MAX_DESCRIPTORS = 268435456  # DFK_BOW_TRAIN_MAX_DESCRIPTORS
+
+
+class DfkBowTrainDesc(C.Structure):
+    _fields_ = [("k", C.c_int32), ("L", C.c_int32), ("descriptor_bytes", C.c_int32), ("num_images", C.c_int32),
+                ("seed", C.c_uint64), ("num_descriptors", C.c_int64), ("descriptors_dev", C.c_void_p),
+                ("image_offsets", C.c_void_p)]
+
+
+class DfkBowTrainStats(C.Structure):
+    _fields_ = [("num_nodes", C.c_int32), ("num_words", C.c_int32), ("max_rounds", C.c_int32),
+                ("capped_nodes", C.c_int32), ("empty_clusters", C.c_int32),
+                ("level_max_rounds", C.c_int32 * BOW_MAX_DEPTH)]
+
+
+class DfkBowVocabularyShape(C.Structure):
+    _fields_ = [("k", C.c_int32), ("L", C.c_int32), ("weighting", C.c_int32), ("scoring", C.c_int32),
+                ("descriptor_bytes", C.c_int32), ("num_nodes", C.c_int32), ("num_words", C.c_int32)]
+
+
 WINDOW_ERROR_DOUBLES = 7  # DFK_WINDOW_ERROR_DOUBLES
 WINDOW_ERROR_EX_DOUBLES = 8  # DFK_WINDOW_ERROR_EX_DOUBLES
 
@@ -344,6 +365,10 @@ SYMBOLS = {
     "dfk_bow_database_query_batch": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkBowQuery), C.c_int, C.c_void_p, C.c_void_p,
                                                C.c_void_p]),
     "dfk_bow_score_batch": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkBowScoreItem), C.c_int, C.c_void_p]),
+    "dfk_bow_vocabulary_train": (C.c_int, [_H, C.POINTER(DfkBowTrainDesc), C.POINTER(DfkBowTrainStats),
+                                           C.POINTER(C.c_void_p)]),
+    "dfk_bow_vocabulary_export": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkBowVocabularyShape), C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

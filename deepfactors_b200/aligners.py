@@ -1841,7 +1841,10 @@ def load_dbow2_vocabulary(path) -> dict:
 
 class BowVocabulary:
     """A DBoW2 vocabulary on the device (dfk_bow_vocabulary_create): a path or the dict of load_dbow2_vocabulary.  The
-    tree is validated when it is created; TF_IDF / L1_NORM only."""
+    tree is validated when it is created; TF_IDF / L1_NORM only.  TrainVocabulary returns one too, with the training's
+    DfkBowTrainStats in .stats (None for a loaded vocabulary)."""
+
+    stats = None
 
     def __init__(self, voc, device=None):
         if not isinstance(voc, dict):
@@ -1863,6 +1866,10 @@ class BowVocabulary:
     def descriptor_bytes(self) -> int:
         return int(self.voc["descriptor_bytes"])
 
+    def export(self) -> dict:
+        """the vocabulary as dfk_bow_vocabulary_export lists it (DBoW2's save order, the ids it was created with)"""
+        return _export_vocabulary(self._hd, self._p)
+
     def close(self):
         if getattr(self, "_p", None) and self._hd.h:
             lib().dfk_bow_vocabulary_destroy(self._hd.h, self._p)
@@ -1873,6 +1880,78 @@ class BowVocabulary:
             self.close()
         except Exception:
             pass
+
+
+def format_dbow2_vocabulary(voc: dict) -> str:
+    """DBoW2's TemplatedVocabulary::save text (cv::FileStorage YAML) of a vocabulary dict (load_dbow2_vocabulary's keys),
+    in the layout of DBoW2's own files: nodes and words in the dict's order, each node on two lines.  Weights use
+    OpenCV's double format, "%d." for an integral value and "%.16e" otherwise, so strtod reads back the same double."""
+    def num(x):
+        x = float(x)
+        return f"{int(x)}." if x == int(x) and abs(x) < 2 ** 53 else f"{x:.16e}"
+
+    out = ["%YAML:1.0", "---", "vocabulary:", f"   k: {int(voc['k'])}", f"   L: {int(voc['L'])}",
+           f"   scoringType: {int(voc['scoring'])}", f"   weightingType: {int(voc['weighting'])}", "   nodes:"]
+    desc = np.asarray(voc["descriptors"], np.uint8)
+    for i, (nid, pid, w) in enumerate(zip(voc["node_ids"], voc["parent_ids"], voc["weights"])):
+        out.append(f"      - {{ nodeId:{int(nid)}, parentId:{int(pid)}, weight:{num(w)},")
+        out.append('          descriptor:"' + "".join(f"{int(b)} " for b in desc[i]) + '" }')
+    out.append("   words:")
+    for wid, nid in zip(voc["word_ids"], voc["word_nodes"]):
+        out.append(f"      - {{ wordId:{int(wid)}, nodeId:{int(nid)} }}")
+    return "\n".join(out) + "\n"
+
+
+def save_dbow2_vocabulary(path, voc) -> None:
+    """format_dbow2_vocabulary to a file (gzip when the path ends in .gz); voc is a dict or a BowVocabulary"""
+    voc = voc.voc if isinstance(voc, BowVocabulary) else voc
+    path = os.fspath(path)
+    opener = gzip.open if path.endswith(".gz") else open
+    with opener(path, "wt", encoding="ascii", newline="\n") as f:
+        f.write(format_dbow2_vocabulary(voc))
+
+
+def _export_vocabulary(hd, p) -> dict:
+    shape = _lib.DfkBowVocabularyShape()
+    check(hd.h, lib().dfk_bow_vocabulary_export(hd.h, p, C.byref(shape), None, None, None, None, None, None))
+    n, W, D = shape.num_nodes, shape.num_words, shape.descriptor_bytes
+    arr = dict(node_ids=np.zeros(n, np.int32), parent_ids=np.zeros(n, np.int32), weights=np.zeros(n, np.float64),
+               descriptors=np.zeros((n, D), np.uint8), word_ids=np.zeros(W, np.int32), word_nodes=np.zeros(W, np.int32))
+    check(hd.h, lib().dfk_bow_vocabulary_export(hd.h, p, C.byref(shape), *[a.ctypes.data for a in arr.values()]))
+    return dict(k=shape.k, L=shape.L, weighting=shape.weighting, scoring=shape.scoring, descriptor_bytes=D, **arr)
+
+
+def TrainVocabulary(descriptors, k: int = 10, L: int = 6, seed: int = 0, image_offsets=None,
+                    device=None) -> "BowVocabulary":
+    """TemplatedVocabulary(k, L, TF_IDF, L1_NORM).create(features) on the device (dfk_bow_vocabulary_train), with the
+    per-node random streams of include/dfk.h's training block.  descriptors: a list of per-image uint8 [n_i, D] CUDA
+    tensors (or Features), or one uint8 [N, D] CUDA tensor with image_offsets (int64 [num_images + 1]).  Returns a
+    BowVocabulary whose .voc is the vocabulary in DBoW2's save order and whose .stats holds DfkBowTrainStats."""
+    if image_offsets is None:
+        rows = [_descriptor_rows(d) for d in descriptors]
+        if not rows:
+            raise ValueError("TrainVocabulary: no images")
+        D = int(rows[0].shape[1])
+        offsets = np.concatenate([[0], np.cumsum([int(r.shape[0]) for r in rows])]).astype(np.int64)
+        flat = torch.cat([r.reshape(-1, D) for r in rows]).contiguous() if len(rows) > 1 else rows[0].contiguous()
+    else:
+        flat = _descriptor_rows(descriptors).contiguous()
+        D = int(flat.shape[1])
+        offsets = np.ascontiguousarray(image_offsets, np.int64)
+    dev = flat.device if device is None else device
+    hd = _Handle(dev)
+    hd.use_torch_stream()
+    d = _lib.DfkBowTrainDesc(int(k), int(L), D, len(offsets) - 1, int(seed) & (2 ** 64 - 1), int(flat.shape[0]),
+                             flat.data_ptr(), offsets.ctypes.data)
+    st = _lib.DfkBowTrainStats()
+    p = C.c_void_p()
+    check(hd.h, lib().dfk_bow_vocabulary_train(hd.h, C.byref(d), C.byref(st), C.byref(p)))
+    voc = BowVocabulary.__new__(BowVocabulary)
+    voc._hd, voc._p = hd, p
+    voc.voc = _export_vocabulary(hd, p)
+    voc.stats = {f: (list(getattr(st, f)) if f == "level_max_rounds" else int(getattr(st, f)))
+                 for f, _ in _lib.DfkBowTrainStats._fields_}
+    return voc
 
 
 @dataclass

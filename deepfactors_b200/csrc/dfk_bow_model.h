@@ -59,4 +59,50 @@ DFK_BOW_FN double dfk_bow_final_score(double sum)
   return -sum / 2.0;
 }
 
+/* ---- vocabulary training (include/dfk.h, the DBoW2 training block): each node's SplitMix64 stream */
+DFK_BOW_FN uint64_t dfk_bow_mix64(uint64_t z)
+{
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+DFK_BOW_FN uint64_t dfk_bow_next(uint64_t* s)
+{
+  *s += 0x9E3779B97F4A7C15ull;
+  return dfk_bow_mix64(*s);
+}
+
+DFK_BOW_FN uint64_t dfk_bow_child_key(uint64_t key, int i)
+{
+  return dfk_bow_mix64(key + (uint64_t)(i + 1) * 0xD1B54A32D192ED03ull);
+}
+
+/* the first centre's index in [0, m) */
+DFK_BOW_FN int64_t dfk_bow_draw_index(uint64_t* s, int64_t m)
+{
+  const uint64_t r = dfk_bow_next(s);
+#if defined(__CUDA_ARCH__)
+  return (int64_t)__umul64hi(r, (uint64_t)m);
+#else
+  return (int64_t)(((unsigned __int128)r * (uint64_t)m) >> 64);
+#endif
+}
+
+/* a cut in (0, dist_sum], dist_sum > 0 */
+DFK_BOW_FN double dfk_bow_draw_cut(uint64_t* s, int64_t dist_sum)
+{
+  double cut;
+  do {
+    cut = ((double)(dfk_bow_next(s) >> 11) * 0x1p-53) * (double)dist_sum;
+  } while (cut == 0.0);
+  return cut;
+}
+
+/* the least integer prefix sum that is >= cut (cut <= 2^53, so the ceiling is exact) */
+DFK_BOW_FN int64_t dfk_bow_cut_target(double cut)
+{
+  return (int64_t)ceil(cut);
+}
+
 #endif /* DFK_BOW_MODEL_H */

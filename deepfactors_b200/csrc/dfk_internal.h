@@ -667,6 +667,65 @@ cudaError_t launch_bow_query(const BowDbDev& db, const BowQueryDev* queries_dev,
                              uint8_t* hits, int32_t* ids, double* scores, int32_t* counts, cudaStream_t s);
 cudaError_t launch_bow_score(const BowDbDev& db, const BowScoreDev* items_dev, int n, double* out, cudaStream_t s);
 
+// DBoW2 vocabulary training (dfk_bow_train.cu), one tree level at a time.  A node of at most kBowTrainSmallMax
+// descriptors runs its whole k-means in one CTA; a larger one is cut into chunks of kBowTrainChunk descriptors, one CTA
+// each, for every step.  Rows are descriptor rows of the level's input (in) and output (out): a node's rows [begin,
+// begin + m) of `in` are its members in order, and the step writes them to the same rows of `out`, grouped by child in
+// cluster order and in their order within each group.
+constexpr int kBowTrainSmallMax = 2048;
+constexpr int kBowTrainSmallSplit = 256;  // the small nodes launch in two size classes, split here
+constexpr int kBowTrainChunk = 1024;
+struct BowTrainNode {
+  int begin, m;
+  unsigned long long key;
+};
+struct BowTrainLevel {
+  const BowTrainNode* nodes;  // [G]
+  const uint4* in;
+  uint4* out;
+  int* nc;                    // [G] children
+  int* rounds;                // [G] assignments made (0 when m <= k)
+  int* capped;                // [G] 1: stopped by DFK_BOW_TRAIN_MAX_ROUNDS
+  int* sizes;                 // [G, k] group sizes
+  uint4* centres;             // [G, k, q]
+  int k, q;
+};
+// the large nodes' state, j a large node, ch a chunk, r a row
+struct BowTrainLarge {
+  const int* node;            // [GL] its index in the level
+  const int2* chunk;          // [chunks] (j, first member within the node)
+  const int* chunk_first;     // [GL + 1]
+  unsigned long long* rng;    // [GL] the node's stream
+  int* seeding;               // [GL]
+  int* active;                // [GL] still assigning
+  int* changed;               // [GL] this round's assignment differs from the last
+  int* cut_chunk;             // [GL]
+  long long* cut_rem;         // [GL] the cut's target within cut_chunk
+  long long* chunk_sum;       // [chunks] sum of min_dist
+  int* chunk_counts;          // [chunks, k] members per cluster
+  int* chunk_base;            // [chunks, k] first output row per cluster
+  int* members;               // [GL, k]
+  int* bits;                  // [GL, k, 8 D] members with each bit set
+  int* min_dist;              // [rows]
+  unsigned char* assign;      // [rows]
+};
+// every small node of the level (small_idx [n_small], max_m their largest size): one launch
+cudaError_t launch_bow_train_small(const BowTrainLevel& lv, const int* small_idx, int n_small, int max_m,
+                                   cudaStream_t s);
+// the large nodes' seeding (1 + 3 (k - 1) launches), then `rounds` rounds of (assign, update), then the partition
+cudaError_t launch_bow_train_seed(const BowTrainLevel& lv, const BowTrainLarge& lg, int n_large, int chunks,
+                                  cudaStream_t s);
+cudaError_t launch_bow_train_rounds(const BowTrainLevel& lv, const BowTrainLarge& lg, int n_large, int chunks,
+                                    int rounds, cudaStream_t s);
+cudaError_t launch_bow_train_partition(const BowTrainLevel& lv, const BowTrainLarge& lg, int n_large, int chunks,
+                                       cudaStream_t s);
+// the level's centres to the tree's rows: node g's children to rows row_first[g] ...
+cudaError_t launch_bow_train_place(const BowTrainLevel& lv, int G, const int* row_first, uint4* tree_desc,
+                                   cudaStream_t s);
+// N_i: for each item, every word of its vector (words_out rows [out_begin, out_begin + counts[i])) counts once
+cudaError_t launch_bow_train_count(const BowItemDev* items_dev, int n, const int32_t* words_out,
+                                   const int32_t* counts, int32_t* word_images, cudaStream_t s);
+
 // One keyframe of dfk_keyframe_mesh_batch (dfk_mesh.cu).  Its W x H pixels are cut into tiles of kMeshTileW x
 // kMeshTileH, one CTA each; a segment is the kMeshTileW pixels of one row of a tile, and its three masks (vertex, T1, T2;
 // bit = x % 32) and two bases (the item's vertex and triangle rows before it, in row-major order) live at

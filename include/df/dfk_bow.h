@@ -2,7 +2,10 @@
 // (include/dfk.h, DBoW2 block): TF_IDF weighting, L1_NORM scoring, no direct index.
 //   df::BowVocabularyData          the arrays of DBoW2's vocabulary, in file order
 //     ::LoadText(std::istream&)    DBoW2's cv::FileStorage text format (uncompressed .yml)
+//     .SaveText(std::ostream&)     TemplatedVocabulary::save's text, which LoadText reads back
 //   df::BowVocabulary              owns a handle and the device tree
+//     (features, D, k, L, seed)    TemplatedVocabulary(k, L, TF_IDF, L1_NORM).create(features), on the device
+//     .Export()                    the tree in DBoW2's save order (dfk_bow_vocabulary_export)
 //     .transform(features, v)      voc_.transform(features, bow_vec) on DEVICE descriptors
 //     .transform(features[], v[])  many images in one call
 //   df::BowVector                  a bag-of-words vector on the device (owns its rows); Host() reads it back
@@ -15,10 +18,12 @@
 #include <cuda_runtime.h>
 
 #include <cctype>
+#include <cstdio>
 #include <cstdlib>
 #include <istream>
 #include <iterator>
 #include <map>
+#include <ostream>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -117,6 +122,30 @@ struct BowVocabularyData {
     return d;
   }
 
+  // TemplatedVocabulary::save's text in the layout of DBoW2's own files: nodes and words in this object's order, each
+  // node on two lines; weights in OpenCV's double format ("%d." when integral, "%.16e" otherwise), so strtod reads
+  // back the same double
+  void SaveText(std::ostream& out) const
+  {
+    char buf[64];
+    out << "%YAML:1.0\n---\nvocabulary:\n   k: " << k << "\n   L: " << L << "\n   scoringType: " << scoring
+        << "\n   weightingType: " << weighting << "\n   nodes:\n";
+    for (size_t i = 0; i < node_ids.size(); ++i) {
+      const double w = weights[i];
+      if (w == (double)(long long)w && w < 9007199254740992.0 && w > -9007199254740992.0)
+        std::snprintf(buf, sizeof buf, "%lld.", (long long)w);
+      else
+        std::snprintf(buf, sizeof buf, "%.16e", w);
+      out << "      - { nodeId:" << node_ids[i] << ", parentId:" << parent_ids[i] << ", weight:" << buf
+          << ",\n          descriptor:\"";
+      for (int b = 0; b < descriptor_bytes; ++b) out << (int)descriptors[i * (size_t)descriptor_bytes + b] << ' ';
+      out << "\" }\n";
+    }
+    out << "   words:\n";
+    for (size_t j = 0; j < word_ids.size(); ++j)
+      out << "      - { wordId:" << word_ids[j] << ", nodeId:" << word_nodes[j] << " }\n";
+  }
+
   DfkBowVocabularyDesc Desc() const
   {
     return DfkBowVocabularyDesc{k, L, weighting, scoring, descriptor_bytes, (int32_t)node_ids.size(), node_ids.data(),
@@ -188,6 +217,42 @@ public:
     const DfkBowVocabularyDesc desc = d.Desc();
     detail::Check(h_.get(), dfk_bow_vocabulary_create(h_.get(), &desc, &voc_));
   }
+  // TemplatedVocabulary(k, L, TF_IDF, L1_NORM).create(features) on the device (dfk_bow_vocabulary_train, with the
+  // per-node random streams of include/dfk.h's training block): descriptors_dev DEVICE [N, descriptor_bytes], 16-byte
+  // aligned, image j its rows [image_offsets[j], image_offsets[j + 1]).  Ordered after earlier work on the stream;
+  // synchronous.
+  BowVocabulary(const uint8_t* descriptors_dev, const std::vector<int64_t>& image_offsets, int descriptor_bytes, int k,
+                int L, uint64_t seed = 0)
+      : h_(detail::MakeHandle())
+  {
+    Train(descriptors_dev, image_offsets, descriptor_bytes, k, L, seed);
+  }
+  // the same from host features, one vector of descriptor_bytes-byte rows per image (DBoW2's getFeatures layout)
+  BowVocabulary(const std::vector<std::vector<uint8_t>>& features, int descriptor_bytes, int k, int L,
+                uint64_t seed = 0)
+      : h_(detail::MakeHandle())
+  {
+    std::vector<int64_t> off{0};
+    for (const auto& f : features) {
+      if (f.size() % (size_t)descriptor_bytes) throw std::invalid_argument("[BowVocabulary] a partial descriptor");
+      off.push_back(off.back() + (int64_t)(f.size() / descriptor_bytes));
+    }
+    void* dev = nullptr;
+    if (cudaMalloc(&dev, std::max<size_t>((size_t)off.back() * descriptor_bytes, 16)) != cudaSuccess)
+      throw std::runtime_error("[BowVocabulary] cudaMalloc failed");
+    size_t o = 0;
+    for (const auto& f : features) {
+      cudaMemcpy(static_cast<uint8_t*>(dev) + o, f.data(), f.size(), cudaMemcpyHostToDevice);
+      o += f.size();
+    }
+    try {
+      Train(static_cast<const uint8_t*>(dev), off, descriptor_bytes, k, L, seed);
+    } catch (...) {
+      cudaFree(dev);
+      throw;
+    }
+    cudaFree(dev);
+  }
   ~BowVocabulary() { dfk_bow_vocabulary_destroy(h_.get(), voc_); }
   BowVocabulary(const BowVocabulary&) = delete;
   BowVocabulary& operator=(const BowVocabulary&) = delete;
@@ -240,9 +305,45 @@ public:
   // voc_.score(a, b) with a = the database entry's vector (the reference scores curr_kf->bow_vec, a keyframe's)
   double score(const BowDatabase& db, int entry, const BowVector& b) const;
 
+  // the tree as DBoW2's save lists it, with the ids the vocabulary was created with (dfk_bow_vocabulary_export)
+  BowVocabularyData Export() const
+  {
+    DfkBowVocabularyShape sh{};
+    detail::Check(h_.get(), dfk_bow_vocabulary_export(h_.get(), voc_, &sh, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                                      nullptr));
+    BowVocabularyData d;
+    d.k = sh.k;
+    d.L = sh.L;
+    d.weighting = sh.weighting;
+    d.scoring = sh.scoring;
+    d.descriptor_bytes = sh.descriptor_bytes;
+    d.node_ids.resize((size_t)sh.num_nodes);
+    d.parent_ids.resize((size_t)sh.num_nodes);
+    d.weights.resize((size_t)sh.num_nodes);
+    d.descriptors.resize((size_t)sh.num_nodes * sh.descriptor_bytes);
+    d.word_ids.resize((size_t)sh.num_words);
+    d.word_nodes.resize((size_t)sh.num_words);
+    detail::Check(h_.get(), dfk_bow_vocabulary_export(h_.get(), voc_, &sh, d.node_ids.data(), d.parent_ids.data(),
+                                                      d.weights.data(), d.descriptors.data(), d.word_ids.data(),
+                                                      d.word_nodes.data()));
+    return d;
+  }
+  // what training found (zeros for a loaded vocabulary)
+  const DfkBowTrainStats& stats() const { return stats_; }
+
 private:
+  void Train(const uint8_t* descriptors_dev, const std::vector<int64_t>& image_offsets, int descriptor_bytes, int k,
+             int L, uint64_t seed)
+  {
+    if (image_offsets.size() < 2) throw std::invalid_argument("[BowVocabulary] no images");
+    const DfkBowTrainDesc d{k, L, descriptor_bytes, (int32_t)(image_offsets.size() - 1), seed, image_offsets.back(),
+                            descriptors_dev, image_offsets.data()};
+    detail::Check(h_.get(), dfk_bow_vocabulary_train(h_.get(), &d, &stats_, &voc_));
+  }
+
   detail::HandlePtr h_;
   DfkBowVocabulary* voc_ = nullptr;
+  DfkBowTrainStats stats_{};
 };
 
 class BowDatabase

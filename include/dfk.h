@@ -1106,6 +1106,103 @@ typedef struct {
 DfkStatus dfk_bow_score_batch(DfkHandle h, const DfkBowDatabase* db, const DfkBowScoreItem* items, int n,
                               double* scores_dev);
 
+/* ------------------------------------------------------------------ loop-closure vocabularies (DBoW2 training) */
+
+/* DBoW2 TemplatedVocabulary::create (HKmeansStep, initiateClustersKMpp, createWords, setNodeWeights) with TF_IDF
+ * weighting, L1_NORM scoring and the descriptor class FBrisk (core/system/fbrisk.cpp), for D = descriptor_bytes in
+ * {32, 48, 64}.  DBoW2 is not vendored; this block is its specification (DESIGN.md section 4.15).
+ *   input       images in order, each a run of D-byte descriptors; the descriptors are their concatenation, image after
+ *               image (getFeatures), N of them.
+ *   distance    popcount(a ^ b) over the D bytes (FBrisk::distance).
+ *   mean        of m descriptors (FBrisk::meanValue): bit b is set iff (the members with bit b set) > m / 2, integer
+ *               division; an empty cluster gets all zeros, one member copies itself.
+ *   step        HKmeansStep(node, descriptors in order, level), from (root, all N descriptors, level 1):
+ *                 m <= k: each descriptor is its own cluster, in order.
+ *                 m > k:  seed (below), then assign; then repeat "mean of each cluster, assign" until an assignment
+ *                         equals the previous one.  Assignment: the nearest centre, strict < in cluster order (a tie goes
+ *                         to the lower cluster).  The first assignment after seeding never counts as converged.
+ *               The node's children are created as one block of consecutive ids in cluster order (centre = descriptor);
+ *               then, only if level < L, the step recurses into each child in order whose group (its members in their
+ *               order in the node) holds more than one descriptor.  Node ids are therefore DBoW2's depth-first
+ *               numbering: the root is 0 and a node's children get the next free ids when the node is visited.
+ *   seeding     (initiateClustersKMpp) the first centre is the descriptor at draw_index(m); min_dist[i] = distance to
+ *               it.  Each later centre: min_dist[i] = min(min_dist[i], distance to the latest centre) where
+ *               min_dist[i] > 0; dist_sum = the sum of min_dist; if dist_sum = 0 seeding stops (the node has fewer than k
+ *               distinct descriptors and gets fewer than k children); otherwise cut = draw_cut(dist_sum) and the centre
+ *               is the first descriptor whose inclusive prefix sum of min_dist is >= cut.  DBoW2 keeps min_dist and the
+ *               sums in double; every value is an integer below 2^53, so the device's int64 sums are exact and equal.
+ *   words       the leaves in ascending node id (createWords).  Every training descriptor is then descended as in step
+ *               2 of the retrieval block; N_i = the images (empty images included) with a descriptor in word i.
+ *               weight = log((double)num_images / (double)N_i), or 0 when N_i = 0, computed on the host from the
+ *               device's integer counts; inner nodes weigh 0.
+ * Deviations from DBoW2:
+ *   1. random source.  DBoW2 draws from the process-wide rand() in the order of its depth-first recursion.  Here each
+ *      node has its own SplitMix64 stream, so the tree does not depend on the order nodes are trained in:
+ *        mix(z)        z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9; z = (z ^ (z >> 27)) * 0x94D049BB133111EB;
+ *                      return z ^ (z >> 31)   (uint64 arithmetic, wrapping)
+ *        next(s)       s += 0x9E3779B97F4A7C15; return mix(s)
+ *        key(root)     = seed;  key(child i of n, i from 0) = mix(key(n) + (i + 1) * 0xD1B54A32D192ED03)
+ *        a node's stream starts at s = key(node) and is used only when m > k:
+ *        draw_index(m) = the high 64 bits of next(s) * m (uint128 product)
+ *        draw_cut(t)   = ((double)(next(s) >> 11) * 0x1p-53) * (double)t, drawn again while it equals 0.0
+ *      The same seed gives the same tree on any device, handle or call.
+ *   2. round cap.  DBoW2 has no bound on its rounds, and ties could make an assignment cycle.  A node whose
+ *      DFK_BOW_TRAIN_MAX_ROUNDS-th assignment still differs from the one before stops with that assignment and the
+ *      centres it was made with, as if it had converged; DfkBowTrainStats::capped_nodes counts such nodes.
+ *   3. limits.  k in [2, 32] (the retrieval's descent has one lane per child), L in [1, DFK_BOW_MAX_DEPTH], D in
+ *      {32, 48, 64}, 1 <= N <= DFK_BOW_TRAIN_MAX_DESCRIPTORS, each image <= DFK_MATCH_MAX_QUERIES descriptors (the
+ *      transform's per-item bound, used by the idf pass).  A tree of more than DFK_BOW_MAX_NODES nodes is rejected
+ *      when it is found to be so (nothing is created). */
+#define DFK_BOW_TRAIN_MAX_ROUNDS 1000
+#define DFK_BOW_TRAIN_MAX_DESCRIPTORS 268435456
+
+typedef struct {
+  int32_t k;                    /* branching factor, in [2, 32] */
+  int32_t L;                    /* depth levels, in [1, DFK_BOW_MAX_DEPTH] */
+  int32_t descriptor_bytes;     /* 32, 48 or 64 */
+  int32_t num_images;           /* >= 1 */
+  uint64_t seed;                /* key of the root's stream */
+  int64_t num_descriptors;      /* N, in [1, DFK_BOW_TRAIN_MAX_DESCRIPTORS] */
+  const uint8_t* descriptors_dev;  /* DEVICE [N, descriptor_bytes], 16-byte aligned; not written */
+  const int64_t* image_offsets; /* HOST [num_images + 1]: image j is rows [offsets[j], offsets[j + 1]); 0 first, N
+                                   last, non-decreasing */
+} DfkBowTrainDesc;
+
+typedef struct {
+  int32_t num_nodes;            /* the nodes listed (the root excluded) */
+  int32_t num_words;
+  int32_t max_rounds;           /* the most assignments any node with m > k made (0 when there is none) */
+  int32_t capped_nodes;         /* nodes stopped by DFK_BOW_TRAIN_MAX_ROUNDS (deviation 2) */
+  int32_t empty_clusters;       /* children whose group is empty (leaves with N_i = 0 unless a descent reaches them) */
+  int32_t level_max_rounds[DFK_BOW_MAX_DEPTH];  /* [l]: the most assignments a node of level l + 1 (the root's is
+                                                   level 1) with m > k made; 0 past the deepest such level */
+} DfkBowTrainStats;
+
+/* Trains a vocabulary as specified above and returns it as dfk_bow_vocabulary_create would from the same tree listed
+ * in DBoW2's save order (it goes through the same validation).  Level-synchronous on the device: all nodes of a level go
+ * through together, a node of at most 2048 descriptors in one CTA, a larger one over many CTAs (DESIGN.md section
+ * 4.15).  Ordered after earlier work on the handle's stream (detector output from the same stream may be passed as it
+ * is); synchronous.  Every argument is checked before anything is enqueued; a rejected call creates nothing, and
+ * dfk_last_error names the field.  stats may be NULL. */
+DfkStatus dfk_bow_vocabulary_train(DfkHandle h, const DfkBowTrainDesc* desc, DfkBowTrainStats* stats,
+                                   DfkBowVocabulary** out);
+
+/* The sizes and scalars of a vocabulary, as DfkBowVocabularyDesc holds them */
+typedef struct {
+  int32_t k, L, weighting, scoring, descriptor_bytes, num_nodes, num_words;
+} DfkBowVocabularyShape;
+
+/* A vocabulary as DBoW2's save lists it, in caller HOST arrays of DfkBowVocabularyDesc's shape: node_ids,
+ * parent_ids, weights [num_nodes], descriptors [num_nodes, descriptor_bytes], word_ids, word_nodes [num_words].  The
+ * node order is save's: a stack of parents, starting with the root; pop the last, list its children in order, push each
+ * child that is not a leaf.  Words go in ascending word id.  Ids are the ones the vocabulary was created with (a
+ * trained one has DBoW2's), and weights are the listed ones: a vocabulary keeps its nodes' ids and weights on the host
+ * (12 bytes a node) and the rest of the tree is read back from the device (synchronous).  Pass every array NULL to read
+ * the shape alone, or none NULL. */
+DfkStatus dfk_bow_vocabulary_export(DfkHandle h, const DfkBowVocabulary* voc, DfkBowVocabularyShape* shape,
+                                    int32_t* node_ids, int32_t* parent_ids, double* weights, uint8_t* descriptors,
+                                    int32_t* word_ids, int32_t* word_nodes);
+
 /* ------------------------------------------------------------------ keyframe window problem (the LM loop on the device) */
 
 /* A window problem: the keyframe window's Levenberg-Marquardt loop in the library, with the window's state (poses and
