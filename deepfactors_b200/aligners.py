@@ -93,25 +93,26 @@ class JTJJrReductionItem:
 
 
 # ------------------------------------------------------------------------------------------- views
-def _image(t: torch.Tensor, floats_per_px: int = 1) -> DfkImage:
-    """vc::Image2DView over a torch CUDA tensor (no copy)."""
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32:
-        raise TypeError("expected a float32 CUDA tensor")
-    if floats_per_px == 1:
-        if t.dim() != 2 or t.stride(1) != 1:
-            raise ValueError("scalar image must be [H, W] with unit column stride")
+def _image(t: torch.Tensor, channels: int = 1, dtype: torch.dtype = torch.float32) -> DfkImage:
+    """vc::Image2DView over a torch CUDA tensor (no copy): [H, W] for one channel, else [H, W, channels] with
+    contiguous pixels, or for float32 also the reference's flat [H, W * channels] view.  Rows may be pitched."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != dtype:
+        raise TypeError(f"expected a {dtype} CUDA tensor")
+    if t.dim() == 3 and channels > 1:
+        if t.shape[2] != channels or t.stride(2) != 1 or t.stride(1) != channels:
+            raise ValueError(f"an image of {channels} channels must be [H, W, {channels}] with contiguous pixels")
+        w = t.shape[1]
+    elif t.dim() == 2 and (channels == 1 or dtype == torch.float32):
+        if t.stride(1) != 1 or t.shape[1] % channels != 0:
+            raise ValueError(f"a 2-D image must be [H, W * {channels}] with unit column stride")
+        w = t.shape[1] // channels
     else:
-        if t.dim() == 3:
-            if t.shape[2] != floats_per_px or t.stride(2) != 1 or t.stride(1) != floats_per_px:
-                raise ValueError("interleaved image must be [H, W, K] with contiguous pixels")
-        elif t.dim() == 2:  # the reference's (W*K) x H float-image view
-            if t.shape[1] % floats_per_px != 0 or t.stride(1) != 1:
-                raise ValueError("flat interleaved image must be [H, W*K]")
-        else:
-            raise ValueError("bad image rank")
-    h = t.shape[0]
-    w = t.shape[1] if (t.dim() == 3 or floats_per_px == 1) else t.shape[1] // floats_per_px
-    return DfkImage(C.c_void_p(t.data_ptr()), t.stride(0) * 4, w, h)
+        raise ValueError("bad image rank")
+    row = w * channels
+    if t.shape[0] > 1 and t.stride(0) < row:
+        raise ValueError("image rows overlap")
+    # a one-row view's row stride is arbitrary: its pitch is its row
+    return DfkImage(t.data_ptr(), max(t.stride(0), row) * t.element_size(), w, t.shape[0])
 
 
 def _cam(cam) -> DfkCamera:
@@ -125,12 +126,90 @@ def _pose(p) -> "C.Array":
     return (C.c_float * 7)(*a.tolist())
 
 
-class _Handle:
+def _ptr(a: np.ndarray):
+    """the typed pointer to a host array's data that a C argument or item field takes"""
+    return a.ctypes.data_as(C.POINTER(np.ctypeslib.as_ctypes_type(a.dtype)))
+
+
+def _host(keep: list, x, dtype, shape=None, what: str = "", null_if_empty: bool = False):
+    """x as a C-contiguous host array of `dtype` and its typed pointer (None for an empty array when null_if_empty).
+    The array goes into `keep`: a pointer stored in a C item does not hold its array, while one passed straight to a
+    call does.  `shape`, when given, is checked; `what` names x."""
+    a = np.ascontiguousarray(x, dtype=dtype)
+    if shape is not None and a.shape != tuple(shape):
+        raise ValueError(f"{what} must have {shape[0]} entries" if len(shape) == 1 else
+                         f"{what} must be [{', '.join(str(int(s)) for s in shape)}]")
+    keep.append(a)
+    return None if null_if_empty and a.size == 0 else _ptr(a)
+
+
+def _depth_prior_lists(prior_kf, sigma, level_ptr):
+    """(m, the host lists of m depth priors as C pointers: keyframes, sigmas, level offsets, the records they own):
+    prior i owns the records [level_ptr[i], level_ptr[i + 1])"""
+    kf, sg, lp = [int(k) for k in prior_kf], [float(v) for v in sigma], [int(v) for v in level_ptr]
+    m = len(kf)
+    if len(sg) != m or len(lp) != m + 1:
+        raise ValueError("sigma needs one entry per prior and level_ptr one more")
+    keep = []
+    return m, (_host(keep, kf, np.int32), _host(keep, sg, np.float32), _host(keep, lp, np.int32)), (lp[-1] if m else 0)
+
+
+def _code_prior(keep: list, weight: float, codes, shape, what: str):
+    """the fp64 codes a zero-code prior of `weight` reads: None when the weight is 0"""
+    if weight <= 0:
+        return None
+    if codes is None:
+        raise ValueError("code_prior_weight > 0 needs the codes")
+    return _host(keep, np.ravel(codes) if len(shape) == 1 else codes, np.float64, shape, what)
+
+
+def _per_item(value, n: int, cast, what: str) -> list:
+    """a setting given as one value for all n items or as one per item, as n values"""
+    vals = list(value) if isinstance(value, (list, tuple, np.ndarray)) else [value] * n
+    if len(vals) != n:
+        raise ValueError(f"{what}: per-item settings need one entry per item")
+    return [cast(v) for v in vals]
+
+
+def _items(T, fill, items, cs: int):
+    """The ctypes array of C items T that a batch call takes: `items` itself when it is one already (a make_*_items
+    array), else fill(item, cs, keep) of each dict, with the host arrays the items point at kept alive by the array.
+    The array has one entry per item, so its length is the item count."""
+    if isinstance(items, C.Array):
+        return items
+    keep = []
+    arr = (T * len(items))(*[fill(it, cs, keep) for it in items])
+    arr._keepalive = keep
+    return arr
+
+
+class _Owner:
+    """Owns one library object, held in the attribute that `_owned` names: close() frees it with _free, once, and so
+    does the collector."""
+    _owned = "_p"
+
+    def close(self):
+        p = getattr(self, self._owned, None)
+        if p:
+            self._free(p)
+            setattr(self, self._owned, None)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class _Handle(_Owner):
+    _owned = "h"
+
     def __init__(self, device=None):
         if not torch.cuda.is_available():
             raise RuntimeError("deepfactors_b200 needs a CUDA device (no CPU fallback)")
         dev = torch.cuda.current_device() if device is None else torch.device(device).index
         self.device = dev if dev is not None else torch.cuda.current_device()
+        self.dev = torch.device("cuda", self.device)
         torch.cuda.init()
         with torch.cuda.device(self.device):
             torch.zeros(1, device="cuda")  # make sure the primary context exists
@@ -139,21 +218,31 @@ class _Handle:
         if st != _lib.DFK_OK:
             raise _lib.DfkError(st, "dfk_create failed")
 
+    def _free(self, h):
+        lib().dfk_destroy(h)
+
     def use_torch_stream(self):
         """launch on torch's current stream (so torch-side events and allocations order correctly)"""
         s = torch.cuda.current_stream(self.device).cuda_stream
         check(self.h, lib().dfk_set_stream(self.h, C.c_void_p(s)))
 
-    def close(self):
-        if getattr(self, "h", None) is not None and self.h:
-            lib().dfk_destroy(self.h)
-            self.h = None
+    def call(self, name: str, *args, stream: bool = True):
+        """libdfk's `name`(handle, *args) on torch's current stream; raises DfkError on a bad status.  stream=False keeps
+        the handle's stream as it is, for calls that only set up or query host-side state."""
+        if stream:
+            self.use_torch_stream()
+        check(self.h, getattr(lib(), name)(self.h, *args))
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def buffer(self, t, dtype: torch.dtype, n: int, what: str, shape=None) -> torch.Tensor:
+        """The device buffer a kernel reads or writes n entries of: a new tensor of `shape` when t is None and the buffer
+        is an optional output, else t, refused before any C call unless it is a contiguous `dtype` tensor of at least n
+        entries on this handle's device."""
+        if t is None and shape is not None:
+            return torch.empty(shape, dtype=dtype, device=self.dev)
+        if not (isinstance(t, torch.Tensor) and t.dtype == dtype and t.device == self.dev and t.is_contiguous()
+                and t.numel() >= n):
+            raise ValueError(f"{what} must be a contiguous {dtype} tensor of at least {n} entries on {self.dev}")
+        return t
 
 
 # ------------------------------------------------------------------------------------------- SfmAligner
@@ -164,66 +253,59 @@ class SfmAligner:
         self.CS = int(code_size)
         self.params_ = params or SfmAlignerParams()
         self._hd = _Handle(device)
-        self._hd.use_torch_stream()
-        cp = self.params_.to_c()
-        check(self._hd.h, lib().dfk_sfm_set_params(self._hd.h, C.byref(cp)))
+        self._set_params()
         self.SetGramMode(gram_mode)
 
     @property
     def handle(self):
         return self._hd.h
 
+    def _set_params(self, stream: bool = True):
+        cp = self.params_.to_c()
+        self._hd.call("dfk_sfm_set_params", C.byref(cp), stream=stream)
+
     def SetSmLimit(self, num_sms: int):
         """size the persistent RunStep grids for `num_sms` SMs (0 = all): leaves room for a kernel on another stream, e.g.
         the window's all-reduce of the previous step (dfk_set_sm_limit)"""
-        check(self._hd.h, lib().dfk_set_sm_limit(self._hd.h, int(num_sms)))
+        self._hd.call("dfk_set_sm_limit", int(num_sms), stream=False)
 
     def SetGramMode(self, mode: str):
         m = {"auto": _lib.DFK_GRAM_AUTO, "fp32": _lib.DFK_GRAM_FP32, "tf32x3": _lib.DFK_GRAM_TF32X3}[mode]
-        check(self._hd.h, lib().dfk_sfm_set_gram_mode(self._hd.h, m))
+        self._hd.call("dfk_sfm_set_gram_mode", m, stream=False)
 
     def SetEvalThreadsBlocks(self, threads: int, blocks: int):
         self.params_.eval_threads, self.params_.eval_blocks = threads, blocks
-        cp = self.params_.to_c()
-        check(self._hd.h, lib().dfk_sfm_set_params(self._hd.h, C.byref(cp)))
+        self._set_params(stream=False)
 
     def SetStepThreadsBlocks(self, threads: int, blocks: int):
         self.params_.step_threads, self.params_.step_blocks = threads, blocks
-        cp = self.params_.to_c()
-        check(self._hd.h, lib().dfk_sfm_set_params(self._hd.h, C.byref(cp)))
+        self._set_params(stream=False)
 
     def RunStep(self, pose0, pose1, code0, cam, img0, img1, dpt0, std0, valid0, prx0_jac, grad1) -> JTJJrReductionItem:
         """cu_sfmaligner.h:76-86.  Synchronous, result by value."""
-        self._hd.use_torch_stream()
         n = 12 + self.CS
         JtJ = np.zeros(n * (n + 1) // 2, dtype=np.float32)
         Jtr = np.zeros(n, dtype=np.float32)
         res = C.c_float(0)
         inl = C.c_uint64(0)
-        code = None if code0 is None else np.ascontiguousarray(code0, dtype=np.float32)
-        F = C.POINTER(C.c_float)
+        code = None if code0 is None else _host([], code0, np.float32)
         i0, i1, d0 = _image(img0), _image(img1), _image(dpt0)
-        s0 = None if std0 is None else _image(std0)
+        s0 = None if std0 is None else C.byref(_image(std0))
         v0, jc, g1 = _image(valid0), _image(prx0_jac, self.CS), _image(grad1, 2)
         cc = _cam(cam)
-        st = lib().dfk_sfm_run_step(self._hd.h, _pose(pose0), _pose(pose1),
-                                    None if code is None else code.ctypes.data_as(F), self.CS, C.byref(cc),
-                                    C.byref(i0), C.byref(i1), C.byref(d0), None if s0 is None else C.byref(s0),
-                                    C.byref(v0), C.byref(jc), C.byref(g1),
-                                    JtJ.ctypes.data_as(F), Jtr.ctypes.data_as(F), C.byref(res), C.byref(inl))
-        check(self._hd.h, st)
+        self._hd.call("dfk_sfm_run_step", _pose(pose0), _pose(pose1), code, self.CS, C.byref(cc), C.byref(i0),
+                      C.byref(i1), C.byref(d0), s0, C.byref(v0), C.byref(jc), C.byref(g1), _ptr(JtJ), _ptr(Jtr),
+                      C.byref(res), C.byref(inl))
         return JTJJrReductionItem(JtJ, Jtr, float(res.value), int(inl.value))
 
     def EvaluateError(self, pose0, pose1, cam, img0, img1, dpt0, std0, grad1) -> CorrespondenceReductionItem:
         """cu_sfmaligner.h:67-74."""
-        self._hd.use_torch_stream()
         res = C.c_float(0)
         inl = C.c_uint64(0)
         i0, i1, d0 = _image(img0), _image(img1), _image(dpt0)
         cc = _cam(cam)
-        st = lib().dfk_sfm_evaluate_error(self._hd.h, _pose(pose0), _pose(pose1), C.byref(cc), C.byref(i0),
-                                          C.byref(i1), C.byref(d0), None, None, C.byref(res), C.byref(inl))
-        check(self._hd.h, st)
+        self._hd.call("dfk_sfm_evaluate_error", _pose(pose0), _pose(pose1), C.byref(cc), C.byref(i0), C.byref(i1),
+                      C.byref(d0), None, None, C.byref(res), C.byref(inl))
         return CorrespondenceReductionItem(float(res.value), int(inl.value))
 
     # ---- batched extension (one persistent launch for many (pair, level) items) -----------------
@@ -231,35 +313,14 @@ class SfmAligner:
         """items: dicts with pose0, pose1, cam, img0, img1, dpt0, valid0, prx0_jac, grad1; optionally prx_orig + code
         (fused depth decode: UpdateDepth(code, prx_orig, prx0_jac, avg_dpt, dpt0) happens inside the launch and dpt0
         becomes an output)."""
-        arr = (DfkSfmWorkItem * len(items))()
-        keep = []  # the code arrays must outlive the ctypes pointers
-        for k, it in enumerate(items):
-            w = arr[k]
-            w.pose0 = _pose(it["pose0"])
-            w.pose1 = _pose(it["pose1"])
-            w.cam = _cam(it["cam"])
-            w.img0, w.img1, w.dpt0 = _image(it["img0"]), _image(it["img1"]), _image(it["dpt0"])
-            w.valid0, w.prx0_jac, w.grad1 = _image(it["valid0"]), _image(it["prx0_jac"], self.CS), _image(it["grad1"], 2)
-            if it.get("code") is not None:
-                code = np.ascontiguousarray(it["code"], dtype=np.float32)
-                if code.shape != (self.CS,):
-                    raise ValueError(f"code must have {self.CS} entries")
-                keep.append(code)
-                w.prx_orig = _image(it["prx_orig"])
-                w.code = code.ctypes.data_as(C.POINTER(C.c_float))
-        arr._keepalive = keep
-        return arr
+        return _items(DfkSfmWorkItem, _work_item, items, self.CS)
 
     def RunStepBatch(self, work_items, records: torch.Tensor | None = None) -> torch.Tensor:
         """Asynchronous: returns a device tensor [n, DFK_SFM_RECORD_FLOATS(CS)] on torch's current stream."""
-        self._hd.use_torch_stream()
-        n = len(work_items)
-        rec = _lib.record_floats(self.CS)
-        if records is None:
-            records = torch.empty((n, rec), dtype=torch.float32, device=f"cuda:{self._hd.device}")
-        assert records.is_contiguous() and records.numel() >= n * rec
-        st = lib().dfk_sfm_run_step_batch(self._hd.h, work_items, n, self.CS, C.c_void_p(records.data_ptr()))
-        check(self._hd.h, st)
+        arr = _items(DfkSfmWorkItem, _work_item, work_items, self.CS)
+        n, rec = len(arr), _lib.record_floats(self.CS)
+        records = self._hd.buffer(records, torch.float32, n * rec, "records", (n, rec))
+        self._hd.call("dfk_sfm_run_step_batch", arr, n, self.CS, records.data_ptr())
         return records
 
     def EvaluateErrorBatch(self, work_items, out: torch.Tensor | None = None) -> torch.Tensor:
@@ -267,10 +328,10 @@ class SfmAligner:
         the fused decode (no `code`: the depth is read from dpt0).  Asynchronous: returns a device tensor [n, 2] float32
         on torch's current stream, row i = [residual | inliers as uint32 bits] (view column 1 as int32 for the count),
         each bit for bit what EvaluateError gives for item i alone."""
-        self._hd.use_torch_stream()
-        n = len(work_items)
-        out = _batch_records(self, n, 2, out)
-        check(self._hd.h, lib().dfk_sfm_evaluate_error_batch(self._hd.h, work_items, n, C.c_void_p(out.data_ptr())))
+        arr = _items(DfkSfmWorkItem, _work_item, work_items, self.CS)
+        n = len(arr)
+        out = self._hd.buffer(out, torch.float32, n * 2, "records", (n, 2))
+        self._hd.call("dfk_sfm_evaluate_error_batch", arr, n, out.data_ptr())
         return out
 
     def UpdateDepthBatch(self, items):
@@ -278,102 +339,88 @@ class SfmAligner:
         prx_orig, prx_jac and dpt (the output), e.g. one per (keyframe, level), or the array of make_depth_items.
         avg_dpt is params.sfmparams.avg_dpt.  Item i is bit for bit UpdateDepth(code, prx_orig, prx_jac, avg_dpt, dpt).
         Asynchronous."""
-        self._hd.use_torch_stream()
-        arr = items if isinstance(items, C.Array) else self.make_depth_items(items)
-        check(self._hd.h, lib().dfk_update_depth_batch(self._hd.h, arr, len(items), self.CS))
+        arr = self.make_depth_items(items)
+        self._hd.call("dfk_update_depth_batch", arr, len(arr), self.CS)
 
     def make_depth_items(self, items: Sequence[dict]):
         """the ctypes array of UpdateDepthBatch; a float32 C-contiguous code is referenced, not copied, so a caller may
         build the array once and rewrite the codes in place"""
-        arr = (DfkDepthDecodeItem * max(len(items), 1))()
-        keep = []
-        for k, it in enumerate(items):
-            code = np.ascontiguousarray(it["code"], dtype=np.float32)
-            if code.shape != (self.CS,):
-                raise ValueError(f"code must have {self.CS} entries")
-            keep.append(code)
-            w = arr[k]
-            w.prx_orig, w.prx_jac, w.dpt = _image(it["prx_orig"]), _image(it["prx_jac"], self.CS), _image(it["dpt"])
-            w.code = code.ctypes.data_as(C.POINTER(C.c_float))
-        arr._keepalive = keep
-        return arr
+        return _items(DfkDepthDecodeItem, _depth_item, items, self.CS)
 
     def unpack(self, records: torch.Tensor):
         r = records.detach().cpu().numpy()
         return [JTJJrReductionItem.from_record(r[i], self.CS) for i in range(r.shape[0])]
 
 
-# ------------------------------------------------------------------------------------------- sparse keypoint factor
+# ------------------------------------------------------------------------------------------- C items
+# Each fills one C item from a dict of its arguments; the host arrays it points at go into `keep`, which must outlive
+# every call that reads the item.
+def _work_item(it: dict, cs: int, keep: list) -> DfkSfmWorkItem:
+    w = DfkSfmWorkItem()
+    w.pose0, w.pose1, w.cam = _pose(it["pose0"]), _pose(it["pose1"]), _cam(it["cam"])
+    w.img0, w.img1, w.dpt0 = _image(it["img0"]), _image(it["img1"]), _image(it["dpt0"])
+    w.valid0, w.prx0_jac, w.grad1 = _image(it["valid0"]), _image(it["prx0_jac"], cs), _image(it["grad1"], 2)
+    if it.get("code") is not None:
+        w.prx_orig, w.code = _image(it["prx_orig"]), _host(keep, it["code"], np.float32, (cs,), "code")
+    return w
+
+
+def _depth_item(it: dict, cs: int, keep: list) -> DfkDepthDecodeItem:
+    return DfkDepthDecodeItem(_image(it["prx_orig"]), _image(it["prx_jac"], cs), _image(it["dpt"]),
+                              _host(keep, it["code"], np.float32, (cs,), "code"))
+
+
+def _depth_prior_item(it: dict, cs: int, keep: list) -> "_lib.DfkDepthPriorItem":
+    return _lib.DfkDepthPriorItem(_image(it["target_dpt"]), _image(it["prx_orig"]), _image(it["prx_jac"], cs),
+                                  _host(keep, it["code"], np.float32, (cs,), "code"))
+
+
 def _reprojection_item(it: dict, cs: int, keep: list) -> DfkReprojectionItem:
-    """one ReprojectionFactor's arguments as the C item; the host arrays go into `keep`, which must outlive the call"""
-    code = np.ascontiguousarray(it["code0"], dtype=np.float32)
-    if code.shape != (cs,):
-        raise ValueError(f"code0 must have {cs} entries")
-    q = np.ascontiguousarray(it["query_xy"], dtype=np.float32).reshape(-1, 2)
-    t = np.ascontiguousarray(it["train_xy"], dtype=np.float32).reshape(-1, 2)
+    """one ReprojectionFactor's arguments"""
+    q = np.asarray(it["query_xy"], dtype=np.float32).reshape(-1, 2)
+    t = np.asarray(it["train_xy"], dtype=np.float32).reshape(-1, 2)
     if q.shape != t.shape:
         raise ValueError("query_xy and train_xy must hold the same number of matches")
-    keep += [code, q, t]
-    FP = C.POINTER(C.c_float)
     w = DfkReprojectionItem()
     w.pose0, w.pose1, w.cam = _pose(it["pose0"]), _pose(it["pose1"]), _cam(it["cam"])
     w.prx_orig, w.prx_jac = _image(it["prx_orig"]), _image(it["prx_jac"], cs)
-    w.code, w.query_xy, w.train_xy = code.ctypes.data_as(FP), q.ctypes.data_as(FP), t.ctypes.data_as(FP)
+    w.code = _host(keep, it["code0"], np.float32, (cs,), "code0")
+    w.query_xy, w.train_xy = _host(keep, q, np.float32), _host(keep, t, np.float32)
     w.num_matches = q.shape[0]
     w.cauchy_delta, w.sigma = float(it["cauchy_delta"]), float(it["sigma"])
     return w
 
 
 def _geometric_item(it: dict, cs: int, keep: list) -> DfkSparseGeometricItem:
-    """one SparseGeometricFactor's arguments as the C item; the host arrays go into `keep`, which must outlive the call"""
-    c0 = np.ascontiguousarray(it["code0"], dtype=np.float32)
-    c1 = np.ascontiguousarray(it["code1"], dtype=np.float32)
-    if c0.shape != (cs,) or c1.shape != (cs,):
-        raise ValueError(f"code0 and code1 must have {cs} entries")
-    pts = np.ascontiguousarray(it["points_xy"], dtype=np.int32).reshape(-1, 2)
-    keep += [c0, c1, pts]
-    FP, IP = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+    """one SparseGeometricFactor's arguments"""
+    pts = np.asarray(it["points_xy"], dtype=np.int32).reshape(-1, 2)
     w = DfkSparseGeometricItem()
     w.pose0, w.pose1, w.cam = _pose(it["pose0"]), _pose(it["pose1"]), _cam(it["cam"])
     w.prx0_orig, w.prx0_jac = _image(it["prx0_orig"]), _image(it["prx0_jac"], cs)
     w.prx1_orig, w.prx1_jac = _image(it["prx1_orig"]), _image(it["prx1_jac"], cs)
     w.dpt_grad1 = _image(it["dpt_grad1"], 2)
-    w.code0, w.code1, w.points_xy = c0.ctypes.data_as(FP), c1.ctypes.data_as(FP), pts.ctypes.data_as(IP)
-    w.num_points = pts.shape[0]
+    w.code0 = _host(keep, it["code0"], np.float32, (cs,), "code0")
+    w.code1 = _host(keep, it["code1"], np.float32, (cs,), "code1")
+    w.points_xy, w.num_points = _host(keep, pts, np.int32), pts.shape[0]
     w.huber_delta = float(it["huber_delta"])
     return w
 
 
-def _check_tensor(hd: _Handle, t: torch.Tensor, dtype: torch.dtype, n: int, what: str):
-    """a kernel reads or writes n elements of t, on the handle's device: refuse any other tensor before the C call"""
-    dev = torch.device("cuda", hd.device)
-    if not (t.dtype == dtype and t.device == dev and t.is_contiguous() and t.numel() >= n):
-        raise ValueError(f"{what} must be a contiguous {dtype} tensor of at least {n} entries on {dev}")
-
-
-def _batch_records(aligner, n: int, rec: int, records: torch.Tensor | None) -> torch.Tensor:
-    if records is None:
-        return torch.empty((n, rec), dtype=torch.float32, device=f"cuda:{aligner._hd.device}")
-    _check_tensor(aligner._hd, records, torch.float32, n * rec, "records")
-    return records
-
-
+# ------------------------------------------------------------------------------------------- sparse keypoint factor
 def ReprojectionLinearize(aligner, pose0, pose1, code0, cam, prx_orig, prx_jac, query_xy, train_xy, cauchy_delta: float,
                           sigma: float):
     """ReprojectionFactor::linearize (sources/core/gtsam/reprojection_factor.cpp:157-269) with the rows gathered on the
     device: prx_orig / prx_jac are the keyframe's level-0 DEVICE buffers, query_xy / train_xy the matched keypoints [M, 2]
     (host).  Returns (rows [2M, 13 + C] float32 = the blocks of the JacobianFactor [J_pose0 | J_pose1 | J_code0 | b],
     total_err)."""
-    aligner._hd.use_torch_stream()
     cs, keep = aligner.CS, []
     w = _reprojection_item(dict(pose0=pose0, pose1=pose1, code0=code0, cam=cam, prx_orig=prx_orig, prx_jac=prx_jac,
                                 query_xy=query_xy, train_xy=train_xy, cauchy_delta=cauchy_delta, sigma=sigma), cs, keep)
     rows = np.zeros((2 * w.num_matches, 13 + cs), dtype=np.float32)
     tot = C.c_float(0)
-    check(aligner.handle, lib().dfk_reprojection_linearize(
-        aligner.handle, w.pose0, w.pose1, w.code, cs, C.byref(w.cam), C.byref(w.prx_orig), C.byref(w.prx_jac),
-        w.num_matches, w.query_xy, w.train_xy, w.cauchy_delta, w.sigma, rows.ctypes.data_as(C.POINTER(C.c_float)),
-        C.byref(tot)))
+    aligner._hd.call("dfk_reprojection_linearize", w.pose0, w.pose1, w.code, cs, C.byref(w.cam), C.byref(w.prx_orig),
+                     C.byref(w.prx_jac), w.num_matches, w.query_xy, w.train_xy, w.cauchy_delta, w.sigma, _ptr(rows),
+                     C.byref(tot))
     return rows, float(tot.value)
 
 
@@ -384,13 +431,8 @@ def ReprojectionLinearizeBatch(aligner, items: Sequence[dict], records: torch.Te
     matches] of factor i's rows, in the RunStep record layout, so it goes into Window.assemble as an unscaled record
     (item size (0, 0)).  `records` may be a slice of a larger record buffer.  Asynchronous: returns a device tensor
     [n, DFK_SFM_RECORD_FLOATS(CS)] on torch's current stream."""
-    aligner._hd.use_torch_stream()
-    cs, n, keep = aligner.CS, len(items), []
-    records = _batch_records(aligner, n, _lib.record_floats(cs), records)
-    arr = (DfkReprojectionItem * max(n, 1))(*[_reprojection_item(it, cs, keep) for it in items])
-    check(aligner.handle, lib().dfk_reprojection_linearize_batch(aligner.handle, arr, n, cs,
-                                                                 C.c_void_p(records.data_ptr())))
-    return records
+    return _factor_batch(aligner, "dfk_reprojection_linearize_batch", make_reprojection_items, items,
+                         _lib.record_floats(aligner.CS), records)
 
 
 def SparseGeometricLinearize(aligner, pose0, pose1, code0, code1, cam, prx0_orig, prx0_jac, prx1_orig, prx1_jac, dpt_grad1,
@@ -399,17 +441,15 @@ def SparseGeometricLinearize(aligner, pose0, pose1, code0, code1, cam, prx0_orig
     prx*_jac are the two keyframes' level-0 DEVICE buffers, dpt_grad1 keyframe 1's depth gradient [H, W, 2] (device),
     points_xy the sampled integer pixels [M, 2] (host).  Returns (rows [M, 13 + 2C] float32 = the blocks of the
     JacobianFactor [J_pose0 | J_pose1 | J_code0 | J_code1 | b], number of valid rows)."""
-    aligner._hd.use_torch_stream()
     cs, keep = aligner.CS, []
     w = _geometric_item(dict(pose0=pose0, pose1=pose1, code0=code0, code1=code1, cam=cam, prx0_orig=prx0_orig,
                              prx0_jac=prx0_jac, prx1_orig=prx1_orig, prx1_jac=prx1_jac, dpt_grad1=dpt_grad1,
                              points_xy=points_xy, huber_delta=huber_delta), cs, keep)
     rows = np.zeros((w.num_points, 13 + 2 * cs), dtype=np.float32)
     nv = C.c_int(0)
-    check(aligner.handle, lib().dfk_sparse_geometric_linearize(
-        aligner.handle, w.pose0, w.pose1, w.code0, w.code1, cs, C.byref(w.cam), C.byref(w.prx0_orig), C.byref(w.prx0_jac),
-        C.byref(w.prx1_orig), C.byref(w.prx1_jac), C.byref(w.dpt_grad1), w.num_points, w.points_xy, w.huber_delta,
-        rows.ctypes.data_as(C.POINTER(C.c_float)), C.byref(nv)))
+    aligner._hd.call("dfk_sparse_geometric_linearize", w.pose0, w.pose1, w.code0, w.code1, cs, C.byref(w.cam),
+                     C.byref(w.prx0_orig), C.byref(w.prx0_jac), C.byref(w.prx1_orig), C.byref(w.prx1_jac),
+                     C.byref(w.dpt_grad1), w.num_points, w.points_xy, w.huber_delta, _ptr(rows), C.byref(nv))
     return rows, int(nv.value)
 
 
@@ -421,42 +461,35 @@ def SparseGeometricLinearizeBatch(aligner, items: Sequence[dict], records: torch
     (DFK_GEO_RECORD_FLOATS(CS) floats), which goes into Window.assemble(geo_records=...).  `records` may be a slice of a
     larger record buffer.  Asynchronous: returns a device tensor [n, DFK_GEO_RECORD_FLOATS(CS)] on torch's current
     stream."""
-    aligner._hd.use_torch_stream()
-    cs, n, keep = aligner.CS, len(items), []
-    records = _batch_records(aligner, n, _lib.geo_record_floats(cs), records)
-    arr = (DfkSparseGeometricItem * max(n, 1))(*[_geometric_item(it, cs, keep) for it in items])
-    check(aligner.handle, lib().dfk_sparse_geometric_linearize_batch(aligner.handle, arr, n, cs,
-                                                                     C.c_void_p(records.data_ptr())))
+    return _factor_batch(aligner, "dfk_sparse_geometric_linearize_batch", make_geometric_items, items,
+                         _lib.geo_record_floats(aligner.CS), records)
+
+
+def _factor_batch(aligner, name: str, make, items, rec: int, records: torch.Tensor | None) -> torch.Tensor:
+    """the body of the factor batch calls: `name`(make(items), n, C, records), rec floats per record"""
+    arr = make(items, aligner.CS)
+    n = len(arr)
+    records = aligner._hd.buffer(records, torch.float32, n * rec, "records", (n, rec))
+    aligner._hd.call(name, arr, n, aligner.CS, records.data_ptr())
     return records
 
 
 def make_reprojection_items(items: Sequence[dict], cs: int):
     """the ctypes array of ReprojectionErrorBatch; a float32 C-contiguous code0 is referenced, not copied, so a caller
     may build the array once and rewrite poses and codes in place"""
-    keep = []
-    arr = (DfkReprojectionItem * max(len(items), 1))(*[_reprojection_item(it, cs, keep) for it in items])
-    arr._keepalive = keep
-    return arr
+    return _items(DfkReprojectionItem, _reprojection_item, items, cs)
 
 
 def make_geometric_items(items: Sequence[dict], cs: int):
     """the ctypes array of SparseGeometricErrorBatch (code0 / code1 referenced as in make_reprojection_items)"""
-    keep = []
-    arr = (DfkSparseGeometricItem * max(len(items), 1))(*[_geometric_item(it, cs, keep) for it in items])
-    arr._keepalive = keep
-    return arr
+    return _items(DfkSparseGeometricItem, _geometric_item, items, cs)
 
 
 def ReprojectionErrorBatch(aligner, items, out: torch.Tensor | None = None) -> torch.Tensor:
     """ReprojectionFactor::error of many factors in one launch (dfk_reprojection_error_batch): the items of
     ReprojectionLinearizeBatch (dicts, or the array of make_reprojection_items).  Asynchronous: returns a device tensor [n, 2] float32, row i = [b^T b | valid matches as
     uint32 bits], b^T b bit for bit the residual of factor i's ReprojectionLinearizeBatch record."""
-    aligner._hd.use_torch_stream()
-    cs, n = aligner.CS, len(items)
-    out = _batch_records(aligner, n, 2, out)
-    arr = items if isinstance(items, C.Array) else make_reprojection_items(items, cs)
-    check(aligner.handle, lib().dfk_reprojection_error_batch(aligner.handle, arr, n, cs, C.c_void_p(out.data_ptr())))
-    return out
+    return _factor_batch(aligner, "dfk_reprojection_error_batch", make_reprojection_items, items, 2, out)
 
 
 # ------------------------------------------------------------------------------------------- keypoint matching
@@ -489,8 +522,8 @@ def _feature_set(hd: _Handle, f: Features) -> _lib.DfkFeatureSet:
     n = int(kp.shape[0]) if kp.dim() == 2 else -1
     if kp.dim() != 2 or kp.shape[1] != 2 or d.dim() != 2 or d.shape[0] != n:
         raise ValueError("features: keypoints must be [N, 2] and descriptors [N, D]")
-    _check_tensor(hd, kp, torch.float32, 2 * n, "keypoints")
-    _check_tensor(hd, d, torch.uint8, n * int(d.shape[1]), "descriptors")
+    hd.buffer(kp, torch.float32, 2 * n, "keypoints")
+    hd.buffer(d, torch.uint8, n * int(d.shape[1]), "descriptors")
     return _lib.DfkFeatureSet(kp.data_ptr() if n else None, d.data_ptr() if n else None, n, int(d.shape[1]))
 
 
@@ -518,14 +551,11 @@ def HammingMatchBatch(aligner, items: Sequence[dict], out: torch.Tensor | None =
     rows at match_offsets(items)[i], row q = (train index, Hamming distance), ties to the lowest train index, (-1, -1)
     when the train set is empty."""
     hd = aligner._hd
-    hd.use_torch_stream()
     n = len(items)
     arr = (_lib.DfkMatchItem * max(n, 1))(*[_match_item(hd, it) for it in items])
     total = int(match_offsets(items)[-1])
-    if out is None:
-        out = torch.empty((max(total, 1), 2), dtype=torch.int32, device=f"cuda:{hd.device}")
-    _check_tensor(hd, out, torch.int32, 2 * total, "out")
-    check(hd.h, lib().dfk_hamming_match_batch(hd.h, arr, n, C.c_void_p(out.data_ptr())))
+    out = hd.buffer(out, torch.int32, 2 * total, "out", (max(total, 1), 2))
+    hd.call("dfk_hamming_match_batch", arr, n, out.data_ptr())
     return out[:total]
 
 
@@ -538,19 +568,16 @@ def ReprojectionMatchBatch(aligner, items: Sequence[dict]):
     rows (query index, train index, distance) sorted by (distance, query); ransac[i] = (selected hypothesis or -1, its
     inliers, hypotheses evaluated)."""
     hd = aligner._hd
-    hd.use_torch_stream()
     n = len(items)
     for it in items:
         if it.get("cam") is None:
             raise ValueError("ReprojectionMatchBatch: every item needs its level-0 camera")
     arr = (_lib.DfkMatchItem * max(n, 1))(*[_match_item(hd, it) for it in items])
     total = int(match_offsets(items)[-1])
-    dev = f"cuda:{hd.device}"
-    matches = torch.zeros((max(total, 1), 3), dtype=torch.int32, device=dev)  # rows past an item's count stay 0
-    counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
-    ransac = torch.empty((max(n, 1), 3), dtype=torch.int32, device=dev)
-    check(hd.h, lib().dfk_reprojection_match_batch(hd.h, arr, n, C.c_void_p(matches.data_ptr()),
-                                                   C.c_void_p(counts.data_ptr()), C.c_void_p(ransac.data_ptr())))
+    matches = torch.zeros((max(total, 1), 3), dtype=torch.int32, device=hd.dev)  # rows past an item's count stay 0
+    counts = torch.empty(max(n, 1), dtype=torch.int32, device=hd.dev)
+    ransac = torch.empty((max(n, 1), 3), dtype=torch.int32, device=hd.dev)
+    hd.call("dfk_reprojection_match_batch", arr, n, matches.data_ptr(), counts.data_ptr(), ransac.data_ptr())
     return matches[:total], counts[:n], ransac[:n]
 
 
@@ -593,12 +620,8 @@ class OrbBatch:
 
 
 def _orb_image(t: torch.Tensor) -> DfkImage:
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.uint8:
-        raise TypeError("OrbDetectBatch: images must be uint8 CUDA tensors")
-    if t.dim() != 2 or t.stride(1) != 1 or (t.shape[0] > 1 and t.stride(0) < t.shape[1]):
-        raise ValueError("OrbDetectBatch: an image must be [H, W] with unit column stride")
-    return DfkImage(C.c_void_p(t.data_ptr()), max(int(t.stride(0)), int(t.shape[1])), int(t.shape[1]),
-                    int(t.shape[0]))
+    """the view of a gray uint8 [H, W] image that the ORB detectors take"""
+    return _image(t, dtype=torch.uint8)
 
 
 def OrbDetectBatch(aligner, images: Sequence[torch.Tensor], nfeatures: int = REP_NFEATURES,
@@ -608,31 +631,32 @@ def OrbDetectBatch(aligner, images: Sequence[torch.Tensor], nfeatures: int = REP
     63 x 63 an image has no features).  nfeatures, fast_threshold and capacity (default 2 nfeatures: ties at the
     response cut can add keypoints) are one value for all images or one per image.  Asynchronous: returns an OrbBatch
     of device tensors; OrbBatch.features() splits it into per-image Features."""
-    hd = aligner._hd
-    hd.use_torch_stream()
-    n = len(images)
-    per = lambda v: [int(x) for x in (v if isinstance(v, (list, tuple, np.ndarray)) else [v] * n)]
-    nf, t = per(nfeatures), per(fast_threshold)
-    cap = per(capacity) if capacity is not None else [2 * x for x in nf]
-    if not (len(nf) == len(t) == len(cap) == n):
-        raise ValueError("OrbDetectBatch: per-image settings need one entry per image")
+    return _orb_detect(aligner, images, OrbBatch, _lib.DfkOrbItem, [(nfeatures, int), (fast_threshold, int)],
+                       capacity)
+
+
+def _orb_detect(aligner, images, result, T, settings, capacity):
+    """the body of OrbDetectBatch and OrbDetectPyramidBatch: items T(image, *settings, capacity), settings (value, type)
+    in T's field order, nfeatures first; a pyramid's result also has the octaves"""
+    hd, n, name, pyramid = aligner._hd, len(images), result._call, result is OrbPyramidBatch
+    cols = [_per_item(v, n, cast, name) for v, cast in settings]
+    cap = _per_item(capacity, n, int, name) if capacity is not None else [2 * x for x in cols[0]]
     for im in images:
-        if im.device != torch.device("cuda", hd.device):
-            raise ValueError(f"OrbDetectBatch: images must be on cuda:{hd.device}")
-    arr = (_lib.DfkOrbItem * max(n, 1))(*[_lib.DfkOrbItem(_orb_image(im), a, b, c)
-                                          for im, a, b, c in zip(images, nf, t, cap)])
+        if im.device != hd.dev:
+            raise ValueError(f"{name}: images must be on cuda:{hd.device}")
+    arr = (T * max(n, 1))(*[T(_orb_image(im), *row) for im, *row in zip(images, *cols, cap)])
     offsets = np.concatenate([[0], np.cumsum(cap)]).astype(np.int64)
     rows = int(offsets[-1])
-    dev = f"cuda:{hd.device}"
-    kp = torch.zeros((max(rows, 1), 2), dtype=torch.float32, device=dev)  # rows past a count stay 0
-    desc = torch.zeros((max(rows, 1), 32), dtype=torch.uint8, device=dev)
-    ang = torch.zeros(max(rows, 1), dtype=torch.float32, device=dev)
-    resp = torch.zeros(max(rows, 1), dtype=torch.float32, device=dev)
-    counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
-    check(hd.h, lib().dfk_orb_detect_batch(hd.h, arr, n, C.c_void_p(kp.data_ptr()), C.c_void_p(desc.data_ptr()),
-                                           C.c_void_p(ang.data_ptr()), C.c_void_p(resp.data_ptr()),
-                                           C.c_void_p(counts.data_ptr())))
-    return OrbBatch(kp[:rows], desc[:rows], ang[:rows], resp[:rows], counts[:n], offsets, np.array(cap, np.int64))
+    r = max(rows, 1)
+    outs = [torch.zeros((r, 2), dtype=torch.float32, device=hd.dev),  # rows past a count stay 0
+            torch.zeros((r, 32), dtype=torch.uint8, device=hd.dev), torch.zeros(r, dtype=torch.float32, device=hd.dev),
+            torch.zeros(r, dtype=torch.float32, device=hd.dev)] + \
+        ([torch.zeros(r, dtype=torch.int32, device=hd.dev)] if pyramid else [])
+    counts = torch.empty(max(n, 1), dtype=torch.int32, device=hd.dev)
+    hd.call("dfk_orb_detect_pyramid_batch" if pyramid else "dfk_orb_detect_batch", arr, n,
+            *[t.data_ptr() for t in outs], counts.data_ptr())
+    kp, desc, ang, resp, *octv = [t[:rows] for t in outs]
+    return result(kp, desc, ang, resp, counts[:n], offsets, np.array(cap, np.int64), *octv)
 
 
 @dataclass
@@ -651,34 +675,8 @@ def OrbDetectPyramidBatch(aligner, images: Sequence[torch.Tensor], nfeatures: in
     [H, W] CUDA tensors of any sizes; every setting is one value for all images or one per image, capacity by default
     2 nfeatures.  Asynchronous: returns an OrbPyramidBatch of device tensors; .features() feeds HammingMatchBatch,
     ReprojectionMatchBatch, window_opt.match_reprojection_links and BowTransformBatch as OrbDetectBatch's does."""
-    hd = aligner._hd
-    hd.use_torch_stream()
-    n = len(images)
-    per = lambda v, f=int: [f(x) for x in (v if isinstance(v, (list, tuple, np.ndarray)) else [v] * n)]
-    nf, s, nl, t = per(nfeatures), per(scale_factor, float), per(nlevels), per(fast_threshold)
-    cap = per(capacity) if capacity is not None else [2 * x for x in nf]
-    if not (len(nf) == len(s) == len(nl) == len(t) == len(cap) == n):
-        raise ValueError("OrbDetectPyramidBatch: per-image settings need one entry per image")
-    for im in images:
-        if im.device != torch.device("cuda", hd.device):
-            raise ValueError(f"OrbDetectPyramidBatch: images must be on cuda:{hd.device}")
-    arr = (_lib.DfkOrbPyramidItem * max(n, 1))(*[_lib.DfkOrbPyramidItem(_orb_image(im), a, b, c, d, e)
-                                                 for im, a, b, c, d, e in zip(images, nf, s, nl, t, cap)])
-    offsets = np.concatenate([[0], np.cumsum(cap)]).astype(np.int64)
-    rows = int(offsets[-1])
-    dev = f"cuda:{hd.device}"
-    kp = torch.zeros((max(rows, 1), 2), dtype=torch.float32, device=dev)  # rows past a count stay 0
-    desc = torch.zeros((max(rows, 1), 32), dtype=torch.uint8, device=dev)
-    ang = torch.zeros(max(rows, 1), dtype=torch.float32, device=dev)
-    resp = torch.zeros(max(rows, 1), dtype=torch.float32, device=dev)
-    octv = torch.zeros(max(rows, 1), dtype=torch.int32, device=dev)
-    counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
-    check(hd.h, lib().dfk_orb_detect_pyramid_batch(hd.h, arr, n, C.c_void_p(kp.data_ptr()),
-                                                   C.c_void_p(desc.data_ptr()), C.c_void_p(ang.data_ptr()),
-                                                   C.c_void_p(resp.data_ptr()), C.c_void_p(octv.data_ptr()),
-                                                   C.c_void_p(counts.data_ptr())))
-    return OrbPyramidBatch(kp[:rows], desc[:rows], ang[:rows], resp[:rows], counts[:n], offsets,
-                           np.array(cap, np.int64), octv[:rows])
+    return _orb_detect(aligner, images, OrbPyramidBatch, _lib.DfkOrbPyramidItem,
+                       [(nfeatures, int), (scale_factor, float), (nlevels, int), (fast_threshold, int)], capacity)
 
 
 # ------------------------------------------------------------------------------------------- frame preprocessing
@@ -702,14 +700,6 @@ class PreprocessedFrame:
     stats: torch.Tensor | None
 
 
-def _frame_view(t: torch.Tensor) -> DfkImage:
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.uint8:
-        raise TypeError("PreprocessBatch: frames must be uint8 CUDA tensors")
-    if t.dim() != 3 or t.shape[2] != 3 or t.stride(2) != 1 or t.stride(1) != 3:
-        raise ValueError("PreprocessBatch: a frame must be [H, W, 3] with interleaved contiguous pixels")
-    return DfkImage(C.c_void_p(t.data_ptr()), int(t.stride(0)), int(t.shape[1]), int(t.shape[0]))
-
-
 def pyramid_sizes(w: int, h: int, num_levels: int) -> list:
     """(w, h) of each level: integer halving (camera_pyramid.h:43-44)"""
     sizes = [(int(w), int(h))]
@@ -727,16 +717,13 @@ def PreprocessBatch(aligner, frames: Sequence[torch.Tensor], src_cams, out_cam, 
     one per frame; resize_viewport gives it); out_cam: the network camera, whose width x height is the output size;
     normalize: one bool for all frames or one per frame.  Asynchronous: returns one PreprocessedFrame per frame."""
     hd = aligner._hd
-    hd.use_torch_stream()
     n = len(frames)
-    cams = list(src_cams) if isinstance(src_cams, (list, tuple)) else [src_cams] * n
-    norm = [bool(x) for x in normalize] if isinstance(normalize, (list, tuple, np.ndarray)) else [bool(normalize)] * n
-    if len(cams) != n or len(norm) != n:
-        raise ValueError("PreprocessBatch: per-frame settings need one entry per frame")
+    cams = _per_item(src_cams, n, _cam, "PreprocessBatch")
+    norm = _per_item(normalize, n, bool, "PreprocessBatch")
     W, H = int(out_cam.width), int(out_cam.height)
     if W != out_cam.width or H != out_cam.height or W < 1 or H < 1:
         raise ValueError("PreprocessBatch: the output camera's size must be whole numbers >= 1")
-    dev = torch.device("cuda", hd.device)
+    dev = hd.dev
     for f in frames:
         if f.device != dev:
             raise ValueError(f"PreprocessBatch: frames must be on cuda:{hd.device}")
@@ -752,15 +739,13 @@ def PreprocessBatch(aligner, frames: Sequence[torch.Tensor], src_cams, out_cam, 
         ga = (DfkImage * max(num_levels, 1))(*[_image(t, 2) for t in gd]) if grads else None
         keep += [la, ga]
         items.append(_lib.DfkPreprocessItem(
-            _frame_view(f), _cam(cams[i]), _cam(out_cam),
-            DfkImage(C.c_void_p(col.data_ptr()), 3 * W, W, H) if color else DfkImage(),
-            DfkImage(C.c_void_p(gr.data_ptr()), W, W, H) if gray else DfkImage(),
+            _image(f, 3, torch.uint8), cams[i], _cam(out_cam),
+            _image(col, 3, torch.uint8) if color else DfkImage(), _image(gr, dtype=torch.uint8) if gray else DfkImage(),
             C.cast(la, C.POINTER(DfkImage)) if num_levels > 0 else None,
             C.cast(ga, C.POINTER(DfkImage)) if grads and num_levels > 0 else None, int(norm[i])))
         out.append(PreprocessedFrame(col, gr, lv, gd, stats[i] if norm[i] else None))
     arr = (_lib.DfkPreprocessItem * max(n, 1))(*items)
-    check(hd.h, lib().dfk_preprocess_batch(hd.h, arr, n, int(num_levels),
-                                           C.c_void_p(stats.data_ptr()) if stats is not None else None))
+    hd.call("dfk_preprocess_batch", arr, n, int(num_levels), stats.data_ptr() if stats is not None else None)
     return out
 
 
@@ -822,14 +807,6 @@ class KeyframeMeshes:
         return out
 
 
-def _u8_view(t: torch.Tensor, channels: int, what: str) -> DfkImage:
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.uint8:
-        raise TypeError(f"KeyframeMeshBatch: {what} must be a uint8 CUDA tensor")
-    if t.dim() != 3 or t.shape[2] != channels or t.stride(2) != 1 or t.stride(1) != channels:
-        raise ValueError(f"KeyframeMeshBatch: {what} must be [H, W, {channels}] with interleaved contiguous pixels")
-    return DfkImage(C.c_void_p(t.data_ptr()), int(t.stride(0)), int(t.shape[1]), int(t.shape[0]))
-
-
 def KeyframeMeshBatch(aligner, items: Sequence[dict], params: KeyframeMeshParams | None = None,
                       code_size: int | None = None, normals: bool = True, pixels: bool = True,
                       triangles: bool = True) -> KeyframeMeshes:
@@ -841,11 +818,10 @@ def KeyframeMeshBatch(aligner, items: Sequence[dict], params: KeyframeMeshParams
     (True: also return SaveKeyframes' uint16 depth image).  Colours are returned when every item has a color view.
     code_size defaults to the aligner's.  Asynchronous: returns a KeyframeMeshes of device tensors."""
     hd = aligner._hd
-    hd.use_torch_stream()
     params = params or KeyframeMeshParams()
     cs = int(code_size if code_size is not None else getattr(aligner, "CS", 0))
     n = len(items)
-    dev = torch.device("cuda", hd.device)
+    dev = hd.dev
     arr = (_lib.DfkKeyframeMeshItem * max(n, 1))()
     keep, u16s, vcap, tcap = [], [], [], []
     with_colors = n > 0 and all(it.get("color") is not None for it in items)
@@ -858,24 +834,20 @@ def KeyframeMeshBatch(aligner, items: Sequence[dict], params: KeyframeMeshParams
         if it.get("dpt") is not None:
             a.dpt = _image(it["dpt"])
         else:
-            code = np.ascontiguousarray(it["code"], dtype=np.float32)
-            if code.shape != (cs,):
-                raise ValueError(f"KeyframeMeshBatch: item {k}'s code must have code_size = {cs} entries")
-            keep.append(code)
+            a.code = _host(keep, it["code"], np.float32, (cs,), f"KeyframeMeshBatch: item {k}'s code")
             a.prx_orig, a.prx_jac = _image(it["prx_orig"]), _image(it["prx_jac"], cs)
-            a.code = code.ctypes.data_as(C.POINTER(C.c_float))
         if it.get("std") is not None:
             a.std = _image(it["std"])
         if it.get("valid") is not None:
             a.valid = _image(it["valid"])
         if it.get("color") is not None:
-            a.color = _u8_view(it["color"], 3, "color")
+            a.color = _image(it["color"], 3, torch.uint8)
         vcap.append(int(it.get("vertex_capacity", W * H)))
         tcap.append(int(it.get("triangle_capacity", 2 * W * H)))
         a.vertex_capacity, a.triangle_capacity = vcap[-1], tcap[-1]
         u16 = torch.empty((H, W), dtype=torch.uint16, device=dev) if it.get("depth_u16") else None
         if u16 is not None:
-            a.depth_u16 = DfkImage(C.c_void_p(u16.data_ptr()), 2 * W, W, H)
+            a.depth_u16 = _image(u16, dtype=torch.uint16)
         u16s.append(u16)
     vo = np.concatenate([[0], np.cumsum(vcap)]).astype(np.int64)
     to = np.concatenate([[0], np.cumsum(tcap)]).astype(np.int64)
@@ -886,10 +858,9 @@ def KeyframeMeshBatch(aligner, items: Sequence[dict], params: KeyframeMeshParams
     pix = torch.zeros(max(V, 1), dtype=torch.int32, device=dev) if pixels else None
     tri = torch.zeros((max(T, 1), 3), dtype=torch.int32, device=dev) if triangles else None
     counts = torch.empty((max(n, 1), 2), dtype=torch.int32, device=dev)
-    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
     prm = params.to_c()
-    check(hd.h, lib().dfk_keyframe_mesh_batch(hd.h, arr, n, cs, C.byref(prm), ptr(pos), ptr(nrm), ptr(col), ptr(pix),
-                                              ptr(tri), ptr(counts)))
+    hd.call("dfk_keyframe_mesh_batch", arr, n, cs, C.byref(prm),
+            *[None if t is None else t.data_ptr() for t in (pos, nrm, col, pix, tri, counts)])
     cut = lambda t, r: None if t is None else t[:r]
     return KeyframeMeshes(pos[:V], cut(nrm, V), cut(col, V), cut(pix, V), cut(tri, T), counts[:n], vo, to, u16s)
 
@@ -948,12 +919,7 @@ def SparseGeometricErrorBatch(aligner, items, out: torch.Tensor | None = None) -
     """SparseGeometricFactor::error of many factors in one launch (dfk_sparse_geometric_error_batch): the items of
     SparseGeometricLinearizeBatch (dicts, or the array of make_geometric_items).  Asynchronous: returns a device tensor [n, 2] float32, row i = [b^T b | valid points
     as uint32 bits], b^T b bit for bit the residual of factor i's SparseGeometricLinearizeBatch record."""
-    aligner._hd.use_torch_stream()
-    cs, n = aligner.CS, len(items)
-    out = _batch_records(aligner, n, 2, out)
-    arr = items if isinstance(items, C.Array) else make_geometric_items(items, cs)
-    check(aligner.handle, lib().dfk_sparse_geometric_error_batch(aligner.handle, arr, n, cs, C.c_void_p(out.data_ptr())))
-    return out
+    return _factor_batch(aligner, "dfk_sparse_geometric_error_batch", make_geometric_items, items, 2, out)
 
 
 # ------------------------------------------------------------------------------------------- DepthAligner
@@ -967,26 +933,21 @@ class DepthAligner:
         self._hd = _Handle(device)
         if params is not None:
             cp = params.to_c()
-            check(self._hd.h, lib().dfk_sfm_set_params(self._hd.h, C.byref(cp)))
+            self._hd.call("dfk_sfm_set_params", C.byref(cp), stream=False)
 
     @property
     def handle(self):
         return self._hd.h
 
     def RunStep(self, code, target_dpt, prx_orig, prx_jac) -> JTJJrReductionItem:
-        self._hd.use_torch_stream()
-        code = np.ascontiguousarray(code, dtype=np.float32)
-        if code.shape != (self.CS,):
-            raise ValueError(f"code must have {self.CS} entries")
+        code = _host([], code, np.float32, (self.CS,), "code")
         nh = self.CS * (self.CS + 1) // 2
         JtJ = np.zeros(nh, dtype=np.float32)
         Jtr = np.zeros(self.CS, dtype=np.float32)
         res, inl = C.c_float(0), C.c_uint64(0)
         t, p, j = _image(target_dpt), _image(prx_orig), _image(prx_jac, self.CS)
-        FP = C.POINTER(C.c_float)
-        check(self._hd.h, lib().dfk_depth_run_step(self._hd.h, code.ctypes.data_as(FP), self.CS, C.byref(t), C.byref(p),
-                                                  C.byref(j), JtJ.ctypes.data_as(FP), Jtr.ctypes.data_as(FP),
-                                                  C.byref(res), C.byref(inl)))
+        self._hd.call("dfk_depth_run_step", code, self.CS, C.byref(t), C.byref(p), C.byref(j), _ptr(JtJ), _ptr(Jtr),
+                      C.byref(res), C.byref(inl))
         return JTJJrReductionItem(JtJ, Jtr, float(res.value), int(inl.value))
 
 
@@ -994,19 +955,7 @@ def make_depth_prior_items(items: Sequence[dict], cs: int):
     """the ctypes array of DepthPriorLinearizeBatch / DepthPriorErrorBatch: dicts with code (host, CS floats),
     target_dpt, prx_orig and prx_jac (device views of one (keyframe, level)).  A float32 C-contiguous code is referenced,
     not copied, so a caller may build the array once and rewrite the codes in place."""
-    arr = (_lib.DfkDepthPriorItem * max(len(items), 1))()
-    keep = []
-    for k, it in enumerate(items):
-        code = np.ascontiguousarray(it["code"], dtype=np.float32)
-        if code.shape != (cs,):
-            raise ValueError(f"code must have {cs} entries")
-        keep.append(code)
-        w = arr[k]
-        w.target_dpt, w.prx_orig = _image(it["target_dpt"]), _image(it["prx_orig"])
-        w.prx_jac = _image(it["prx_jac"], cs)
-        w.code = code.ctypes.data_as(C.POINTER(C.c_float))
-    arr._keepalive = keep
-    return arr
+    return _items(_lib.DfkDepthPriorItem, _depth_prior_item, items, cs)
 
 
 def DepthPriorLinearizeBatch(aligner, items, records: torch.Tensor | None = None) -> torch.Tensor:
@@ -1015,29 +964,19 @@ def DepthPriorLinearizeBatch(aligner, items, records: torch.Tensor | None = None
     [JtJ packed upper | Jtr | residual | inliers (uint32 bits) = W * H] (DFK_DEPTH_RECORD_FLOATS(CS)), item i's
     DepthAligner.RunStep result, with the aligner's avg_dpt.  `records` may be a slice of a larger buffer.  Asynchronous:
     returns a device tensor [n, DFK_DEPTH_RECORD_FLOATS(CS)] on torch's current stream."""
-    aligner._hd.use_torch_stream()
-    cs, n = aligner.CS, len(items)
-    records = _batch_records(aligner, n, _lib.depth_record_floats(cs), records)
-    arr = items if isinstance(items, C.Array) else make_depth_prior_items(items, cs)
-    check(aligner.handle, lib().dfk_depth_prior_linearize_batch(aligner.handle, arr, n, cs,
-                                                                C.c_void_p(records.data_ptr())))
-    return records
+    return _factor_batch(aligner, "dfk_depth_prior_linearize_batch", make_depth_prior_items, items,
+                         _lib.depth_record_floats(aligner.CS), records)
 
 
 def DepthPriorErrorBatch(aligner, items, out: torch.Tensor | None = None) -> torch.Tensor:
     """DepthPriorFactor's sum diff^2 of many (keyframe, level) items in one call (dfk_depth_prior_error_batch): the items
     of DepthPriorLinearizeBatch.  Asynchronous: returns a device tensor [n, 2] float32, row i = [sum diff^2 | W * H as
     uint32 bits], the residual bit for bit the one of item i's DepthPriorLinearizeBatch record."""
-    aligner._hd.use_torch_stream()
-    cs, n = aligner.CS, len(items)
-    out = _batch_records(aligner, n, 2, out)
-    arr = items if isinstance(items, C.Array) else make_depth_prior_items(items, cs)
-    check(aligner.handle, lib().dfk_depth_prior_error_batch(aligner.handle, arr, n, cs, C.c_void_p(out.data_ptr())))
-    return out
+    return _factor_batch(aligner, "dfk_depth_prior_error_batch", make_depth_prior_items, items, 2, out)
 
 
 # ------------------------------------------------------------------------------------------- keyframe window
-class Window:
+class Window(_Owner):
     """Device-side assembly of a keyframe window's block-sparse normal equations (dfk_window_* of include/dfk.h):
     what the factor graph does with the RunStep records of a window -- PhotometricFactor::linearize's block slicing,
     sign flip and residual rescale (sources/core/gtsam/photometric_factor.cpp:105-161,275-282) summed over the window's
@@ -1047,69 +986,64 @@ class Window:
     `num_frames` tracked frames (pose-only variables, dfk_window_create_frames): a pair (k, K + f) is frame f's one
     photometric pair; the frames' blocks follow the links'.  `kf_priors` lists the keyframes of each keyframe prior
     (dfk_window_create_priors, ascending lists); their prior blocks follow the frames'."""
+    _owned = "w"
 
     def __init__(self, aligner: "SfmAligner", num_keyframes: int, pairs, item_pair, item_sizes, geometric=(),
                  num_frames: int = 0, kf_priors=()):
         from .factors import WindowBlocks
-        self._al = aligner
+        self._al, self._hd = aligner, aligner._hd
         self.layout = WindowBlocks(int(num_keyframes), aligner.CS, [tuple(map(int, p)) for p in pairs],
                                    [tuple(map(int, p)) for p in geometric], int(num_frames),
                                    [tuple(int(k) for k in p) for p in kf_priors])
-        k0 = np.ascontiguousarray([p[0] for p in self.layout.pairs], dtype=np.int32)
-        k1 = np.ascontiguousarray([p[1] for p in self.layout.pairs], dtype=np.int32)
-        ip = np.ascontiguousarray(item_pair, dtype=np.int32)
-        self.item_pair = ip.copy()
-        iw = np.ascontiguousarray([s[0] for s in item_sizes], dtype=np.int32)
-        ih = np.ascontiguousarray([s[1] for s in item_sizes], dtype=np.int32)
-        I32 = C.POINTER(C.c_int32)
-        desc = _lib.DfkWindowDesc(int(num_keyframes), len(k0), len(ip), aligner.CS, k0.ctypes.data_as(I32),
-                                  k1.ctypes.data_as(I32), ip.ctypes.data_as(I32), iw.ctypes.data_as(I32),
-                                  ih.ctypes.data_as(I32))
-        g0 = np.ascontiguousarray([p[0] for p in self.layout.geometric], dtype=np.int32)
-        g1 = np.ascontiguousarray([p[1] for p in self.layout.geometric], dtype=np.int32)
-        L = len(g0)
+        keep = []
+        i32 = lambda x, null_if_empty=False: _host(keep, x, np.int32, null_if_empty=null_if_empty)
+        self.item_pair = np.array(item_pair, dtype=np.int32)
+        self.num_items = len(self.item_pair)
+        L = self.layout
+        desc = _lib.DfkWindowDesc(int(num_keyframes), len(L.pairs), self.num_items, aligner.CS,
+                                  i32([p[0] for p in L.pairs]), i32([p[1] for p in L.pairs]), i32(self.item_pair),
+                                  i32([s[0] for s in item_sizes]), i32([s[1] for s in item_sizes]))
+        links = (len(L.geometric), i32([p[0] for p in L.geometric], True), i32([p[1] for p in L.geometric], True),
+                 int(num_frames))
         self.w = C.c_void_p()
-        kp = self.layout.kf_priors
+        kp = L.kf_priors
         if kp:
-            pp = np.ascontiguousarray(np.cumsum([0] + [len(p) for p in kp]), dtype=np.int32)
-            pk = np.ascontiguousarray([k for p in kp for k in p], dtype=np.int32)
-            check(aligner.handle, lib().dfk_window_create_priors(aligner.handle, C.byref(desc), L,
-                                                                 g0.ctypes.data_as(I32) if L else None,
-                                                                 g1.ctypes.data_as(I32) if L else None, int(num_frames),
-                                                                 len(kp), pp.ctypes.data_as(I32),
-                                                                 pk.ctypes.data_as(I32), C.byref(self.w)))
+            self._hd.call("dfk_window_create_priors", C.byref(desc), *links, len(kp),
+                          i32(np.cumsum([0] + [len(p) for p in kp])), i32([k for p in kp for k in p]), C.byref(self.w),
+                          stream=False)
         else:
-            check(aligner.handle, lib().dfk_window_create_frames(aligner.handle, C.byref(desc), L,
-                                                                 g0.ctypes.data_as(I32) if L else None,
-                                                                 g1.ctypes.data_as(I32) if L else None, int(num_frames),
-                                                                 C.byref(self.w)))
+            self._hd.call("dfk_window_create_frames", C.byref(desc), *links, C.byref(self.w), stream=False)
         # doubles of each keyframe prior and of its deltas, and where each starts in the back-to-back buffers
         self.kf_prior_sizes = [_lib.kf_prior_doubles(aligner.CS, len(p)) for p in kp]
         self.kf_prior_doubles = int(sum(self.kf_prior_sizes))
-        self.kf_delta_doubles = int(sum(len(p) for p in kp)) * self.layout.B
-        self.num_items = len(ip)
-        self.floats = int(lib().dfk_window_floats(self.w))
-        assert self.floats == self.layout.floats
+        self.kf_delta_doubles = int(sum(len(p) for p in kp)) * L.B
+        self.floats = int(lib().dfk_window_floats(self.w))  # takes no handle: a host-side query
+        assert self.floats == L.floats
+
+    def _free(self, w):
+        lib().dfk_window_destroy(self._al.handle, w)
+
+    def _records(self, records: torch.Tensor) -> torch.Tensor:
+        return self._hd.buffer(records, torch.float32, self.num_items * _lib.record_floats(self.layout.code_size),
+                               "records")
+
+    def _geo_records(self, geo_records: torch.Tensor | None):
+        """geo_records' pointer, or None"""
+        if geo_records is None:
+            return None
+        n = len(self.layout.geometric) * _lib.geo_record_floats(self.layout.code_size)
+        return self._hd.buffer(geo_records, torch.float32, n, "geo_records").data_ptr()
 
     def assemble(self, records: torch.Tensor, out: torch.Tensor | None = None,
                  geo_records: torch.Tensor | None = None) -> torch.Tensor:
         """records: [num_items, REC] device tensor written by RunStepBatch; geo_records: [num_links, GEO_REC] written by
         SparseGeometricLinearizeBatch (required when the window has links).  Asynchronous on torch's current stream."""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        _check_tensor(hd, records, torch.float32, self.num_items * _lib.record_floats(self.layout.code_size), "records")
-        if out is None:
-            out = torch.empty(self.floats, dtype=torch.float32, device=records.device)
-        _check_tensor(hd, out, torch.float32, self.floats, "out")
+        records = self._records(records)
+        out = self._hd.buffer(out, torch.float32, self.floats, "out", self.floats)
         if self.layout.geometric and geo_records is None:
             raise ValueError("the window has geometric links: geo_records is required")
-        geo = None
-        if geo_records is not None:
-            _check_tensor(hd, geo_records, torch.float32,
-                          len(self.layout.geometric) * _lib.geo_record_floats(self.layout.code_size), "geo_records")
-            geo = C.c_void_p(geo_records.data_ptr())
-        check(hd.h, lib().dfk_window_assemble_geometric(hd.h, self.w, C.c_void_p(records.data_ptr()), geo,
-                                                        C.c_void_p(out.data_ptr())))
+        self._hd.call("dfk_window_assemble_geometric", self.w, records.data_ptr(), self._geo_records(geo_records),
+                      out.data_ptr())
         return out
 
     def marginalize_frames(self, records: torch.Tensor, frames, priors: torch.Tensor | None = None,
@@ -1118,36 +1052,26 @@ class Window:
         of the frame's pose in its pair's records, undamped).  records: [num_items, REC] on the device.  Returns
         (priors [n, DFK_PRIOR_DOUBLES] float64, info [n] int32), device tensors written asynchronously on torch's
         current stream; info[i] = 0, or 1 + the row of the frame block whose pivot failed (prior i is then zero)."""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        _check_tensor(hd, records, torch.float32, self.num_items * _lib.record_floats(self.layout.code_size), "records")
-        fr = np.ascontiguousarray([int(f) for f in frames], dtype=np.int32)
+        records = self._records(records)
+        fr = [int(f) for f in frames]
         n, pd = len(fr), _lib.prior_doubles(self.layout.code_size)
-        if priors is None:
-            priors = torch.empty((n, pd), dtype=torch.float64, device=records.device)
-        _check_tensor(hd, priors, torch.float64, n * pd, "priors")
-        if info is None:
-            info = torch.empty(n, dtype=torch.int32, device=records.device)
-        _check_tensor(hd, info, torch.int32, n, "info")
-        check(hd.h, lib().dfk_window_marginalize_frames(hd.h, self.w, C.c_void_p(records.data_ptr()), n,
-                                                        fr.ctypes.data_as(C.POINTER(C.c_int32)),
-                                                        C.c_void_p(priors.data_ptr()), C.c_void_p(info.data_ptr())))
+        priors = self._hd.buffer(priors, torch.float64, n * pd, "priors", (n, pd))
+        info = self._hd.buffer(info, torch.int32, n, "info", n)
+        self._hd.call("dfk_window_marginalize_frames", self.w, records.data_ptr(), n, _host([], fr, np.int32),
+                      priors.data_ptr(), info.data_ptr())
         return priors, info
 
     def add_priors(self, buf: torch.Tensor, prior_kf, priors: torch.Tensor, delta: torch.Tensor) -> torch.Tensor:
         """dfk_window_add_priors, in place on an assembled buffer: prior i (a row of `priors`, [m, DFK_PRIOR_DOUBLES]
         float64 on the device) on keyframe prior_kf[i] at delta[i] ([m, B] float64 on the device) = Local(x0_i, x).
         With sharded pairs, call it after the all-reduce.  Asynchronous on torch's current stream."""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        kf = np.ascontiguousarray([int(k) for k in prior_kf], dtype=np.int32)
-        m, B = len(kf), self.layout.B
-        _check_tensor(hd, buf, torch.float32, self.floats, "buf")
-        _check_tensor(hd, priors, torch.float64, m * _lib.prior_doubles(self.layout.code_size), "priors")
-        _check_tensor(hd, delta, torch.float64, m * B, "delta")
-        check(hd.h, lib().dfk_window_add_priors(hd.h, self.w, m, kf.ctypes.data_as(C.POINTER(C.c_int32)),
-                                                C.c_void_p(priors.data_ptr()), C.c_void_p(delta.data_ptr()),
-                                                C.c_void_p(buf.data_ptr())))
+        kf = [int(k) for k in prior_kf]
+        m = len(kf)
+        self._hd.buffer(buf, torch.float32, self.floats, "buf")
+        self._hd.buffer(priors, torch.float64, m * _lib.prior_doubles(self.layout.code_size), "priors")
+        self._hd.buffer(delta, torch.float64, m * self.layout.B, "delta")
+        self._hd.call("dfk_window_add_priors", self.w, m, _host([], kf, np.int32), priors.data_ptr(), delta.data_ptr(),
+                      buf.data_ptr())
         return buf
 
     def add_depth_priors(self, buf: torch.Tensor, prior_kf, sigma, level_ptr, records: torch.Tensor) -> torch.Tensor:
@@ -1155,21 +1079,10 @@ class Window:
         standard deviation sigma[i] owns the rows [level_ptr[i], level_ptr[i + 1]) of `records` (DepthPriorLinearizeBatch's
         records on the device): JtJ / sigma^2 to the keyframe's code block, -Jtr / sigma^2 to its code gradient,
         residual / sigma^2 to f.  Asynchronous on torch's current stream."""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        kf = np.ascontiguousarray([int(k) for k in prior_kf], dtype=np.int32)
-        sg = np.ascontiguousarray([float(v) for v in sigma], dtype=np.float32)
-        lp = np.ascontiguousarray([int(v) for v in level_ptr], dtype=np.int32)
-        m = len(kf)
-        if sg.size != m or lp.size != m + 1:
-            raise ValueError("sigma needs one entry per prior and level_ptr one more")
-        _check_tensor(hd, buf, torch.float32, self.floats, "buf")
-        nrec = int(lp[-1]) if m else 0
-        _check_tensor(hd, records, torch.float32, nrec * _lib.depth_record_floats(self.layout.code_size), "records")
-        I32 = C.POINTER(C.c_int32)
-        check(hd.h, lib().dfk_window_add_depth_priors(hd.h, self.w, m, kf.ctypes.data_as(I32),
-                                                      sg.ctypes.data_as(C.POINTER(C.c_float)), lp.ctypes.data_as(I32),
-                                                      C.c_void_p(records.data_ptr()), C.c_void_p(buf.data_ptr())))
+        m, lists, nrec = _depth_prior_lists(prior_kf, sigma, level_ptr)
+        self._hd.buffer(buf, torch.float32, self.floats, "buf")
+        self._hd.buffer(records, torch.float32, nrec * _lib.depth_record_floats(self.layout.code_size), "records")
+        self._hd.call("dfk_window_add_depth_priors", self.w, m, *lists, records.data_ptr(), buf.data_ptr())
         return buf
 
     def add_keyframe_priors(self, buf: torch.Tensor, priors: torch.Tensor, delta: torch.Tensor) -> torch.Tensor:
@@ -1177,23 +1090,19 @@ class Window:
         `priors` (float64 on the device, kf_prior_doubles entries) at `delta` (float64, kf_delta_doubles: Local(x0, x) of
         every member, prior by prior).  With sharded pairs, call it after the all-reduce.  Asynchronous on torch's current
         stream."""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        _check_tensor(hd, buf, torch.float32, self.floats, "buf")
+        self._hd.buffer(buf, torch.float32, self.floats, "buf")
         if not self.layout.kf_priors:
             return buf
-        _check_tensor(hd, priors, torch.float64, self.kf_prior_doubles, "priors")
-        _check_tensor(hd, delta, torch.float64, self.kf_delta_doubles, "delta")
-        check(hd.h, lib().dfk_window_add_keyframe_priors(hd.h, self.w, C.c_void_p(priors.data_ptr()),
-                                                         C.c_void_p(delta.data_ptr()), C.c_void_p(buf.data_ptr())))
+        self._hd.buffer(priors, torch.float64, self.kf_prior_doubles, "priors")
+        self._hd.buffer(delta, torch.float64, self.kf_delta_doubles, "delta")
+        self._hd.call("dfk_window_add_keyframe_priors", self.w, priors.data_ptr(), delta.data_ptr(), buf.data_ptr())
         return buf
 
     def blanket(self, m: int):
         """dfk_window_blanket: the ascending keyframes that share a factor with keyframe m"""
         out = np.zeros(max(self.layout.num_keyframes, 1), dtype=np.int32)
         n = C.c_int32(0)
-        check(self._al.handle, lib().dfk_window_blanket(self._al.handle, self.w, int(m),
-                                                        out.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(n)))
+        self._hd.call("dfk_window_blanket", self.w, int(m), _ptr(out), C.byref(n), stream=False)
         return [int(k) for k in out[:n.value]]
 
     def marginalize_keyframe(self, records: torch.Tensor, m: int, geo_records: torch.Tensor | None = None,
@@ -1208,112 +1117,73 @@ class Window:
         when one contains m); code_prior_weight / code (host, C): the zero-code prior on m.  Returns (prior
         [DFK_KF_PRIOR_DOUBLES(C, n)] float64, info [1] int32), device tensors written asynchronously on torch's current
         stream; info = 0, or 1 + the row of m's block whose pivot failed (the prior is then zero)."""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        cs, B = self.layout.code_size, self.layout.B
-        _check_tensor(hd, records, torch.float32, self.num_items * _lib.record_floats(cs), "records")
-        geo = None
-        if geo_records is not None:
-            _check_tensor(hd, geo_records, torch.float32, len(self.layout.geometric) * _lib.geo_record_floats(cs),
-                          "geo_records")
-            geo = C.c_void_p(geo_records.data_ptr())
-        r = 0
+        hd, cs = self._hd, self.layout.code_size
+        records = self._records(records)
+        geo = self._geo_records(geo_records)
+        r, fp, fd = 0, None, None
         if frame_priors is not None:
             r = frame_priors.numel() // _lib.prior_doubles(cs)
-            _check_tensor(hd, frame_priors, torch.float64, r * _lib.prior_doubles(cs), "frame_priors")
-            _check_tensor(hd, frame_delta, torch.float64, r * B, "frame_delta")
+            fp = hd.buffer(frame_priors, torch.float64, r * _lib.prior_doubles(cs), "frame_priors").data_ptr()
+            fd = hd.buffer(frame_delta, torch.float64, r * self.layout.B, "frame_delta").data_ptr()
+        fp, fd = (fp, fd) if r else (None, None)
+        kp, kd = None, None
         if kf_priors is not None:
-            _check_tensor(hd, kf_priors, torch.float64, self.kf_prior_doubles, "kf_priors")
-            _check_tensor(hd, kf_delta, torch.float64, self.kf_delta_doubles, "kf_delta")
-        n = len(self.blanket(m))
-        dev = records.device
-        if prior is None:
-            prior = torch.empty(_lib.kf_prior_doubles(cs, n), dtype=torch.float64, device=dev)
-        _check_tensor(hd, prior, torch.float64, _lib.kf_prior_doubles(cs, n), "prior")
-        if info is None:
-            info = torch.empty(1, dtype=torch.int32, device=dev)
-        _check_tensor(hd, info, torch.int32, 1, "info")
-        cp = None
-        if code_prior_weight > 0:
-            c64 = np.ascontiguousarray(code, dtype=np.float64).reshape(-1)
-            if c64.shape != (cs,):
-                raise ValueError(f"code must have {cs} entries")
-            cp = c64.ctypes.data_as(C.POINTER(C.c_double))
-        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
-        check(hd.h, lib().dfk_window_marginalize_keyframe(
-            hd.h, self.w, C.c_void_p(records.data_ptr()), geo, int(m), r, ptr(frame_priors) if r else None,
-            ptr(frame_delta) if r else None, ptr(kf_priors), ptr(kf_delta), float(code_prior_weight), cp,
-            C.c_void_p(prior.data_ptr()), C.c_void_p(info.data_ptr())))
+            kp = hd.buffer(kf_priors, torch.float64, self.kf_prior_doubles, "kf_priors").data_ptr()
+            kd = hd.buffer(kf_delta, torch.float64, self.kf_delta_doubles, "kf_delta").data_ptr()
+        size = _lib.kf_prior_doubles(cs, len(self.blanket(m)))
+        prior = hd.buffer(prior, torch.float64, size, "prior", size)
+        info = hd.buffer(info, torch.int32, 1, "info", 1)
+        hd.call("dfk_window_marginalize_keyframe", self.w, records.data_ptr(), geo, int(m), r, fp, fd, kp, kd,
+                float(code_prior_weight), _code_prior([], code_prior_weight, code, (cs,), "code"), prior.data_ptr(),
+                info.data_ptr())
         return prior, info
 
-    def close(self):
-        if getattr(self, "w", None):
-            lib().dfk_window_destroy(self._al.handle, self.w)
-            self.w = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class WindowSolver:
+class WindowSolver(_Owner):
     """Damped block-sparse fp64 Cholesky of a Window's normal equations on the device (dfk_window_solve): the system
     WindowOptimizer solves with to_dense + damped_solve, straight from the packed buffer.  `fixed` lists the window
     variables k * B + r held at zero (e.g. range(6): the gauge keyframe's pose).  `tiles` is the number of structurally
     nonzero B x B tiles of the factor, fill included.  With tracked frames dx has K * B + 6 F entries (frame f's pose
     at K * B + 6 f)."""
+    _owned = "s"
 
     def __init__(self, window: Window, fixed=(), _prev: "WindowSolver | None" = None):
         self._win = window  # keeps the window (and its handle) alive
-        self._al = window._al
+        self._al, self._hd = window._al, window._hd
         self.layout = window.layout
-        fx = np.ascontiguousarray([int(v) for v in fixed], dtype=np.int32)
-        self.fixed = tuple(int(v) for v in fx)
+        self.fixed = tuple(int(v) for v in fixed)
+        fx = (len(self.fixed), _host([], self.fixed, np.int32))
         self.s = C.c_void_p()
         self.info = None  # update()'s pivot report when the caller passes no info tensor
         if _prev is None:
-            check(self._al.handle, lib().dfk_window_solver_create(self._al.handle, window.w, len(fx),
-                                                                  fx.ctypes.data_as(C.POINTER(C.c_int32)),
-                                                                  C.byref(self.s)))
+            self._hd.call("dfk_window_solver_create", window.w, *fx, C.byref(self.s), stream=False)
         else:
             # create_from copies the old solver's factor on the handle's stream: order it after torch's work, as
             # update() does
-            self._al._hd.use_torch_stream()
-            check(self._al.handle, lib().dfk_window_solver_create_from(self._al.handle, window.w, len(fx),
-                                                                       fx.ctypes.data_as(C.POINTER(C.c_int32)),
-                                                                       _prev.s, C.byref(self.s)))
+            self._hd.call("dfk_window_solver_create_from", window.w, *fx, _prev.s, C.byref(self.s))
         tiles = C.c_size_t(0)
-        check(self._al.handle, lib().dfk_window_solver_tiles(self._al.handle, self.s, C.byref(tiles)))
+        self._hd.call("dfk_window_solver_tiles", self.s, C.byref(tiles), stream=False)
         self.tiles = int(tiles.value)
+
+    def _free(self, s):
+        lib().dfk_window_solver_destroy(self._al.handle, s)
+
+    def _args(self, buf, weight, codes, dx, info):
+        """buf, the code prior, dx and info of solve and update, checked; dx and info allocated when not given"""
+        L, hd = self.layout, self._hd
+        buf = hd.buffer(buf, torch.float32, L.floats, "buf")
+        dx = hd.buffer(dx, torch.float64, L.dim, "dx", L.dim)
+        info = hd.buffer(info, torch.int32, 1, "info", 1)
+        return buf, _code_prior([], weight, codes, (L.num_keyframes, L.code_size), "codes"), dx, info
 
     def solve(self, buf: torch.Tensor, lam: float, code_prior_weight: float = 0.0, codes=None,
               dx: torch.Tensor | None = None, info: torch.Tensor | None = None):
         """buf: the window buffer (contiguous float32 on the handle's device).  codes: [K, C] (host), required when
         code_prior_weight > 0.  Returns (dx [K * B + 6 F] float64, info [1] int32), device tensors written asynchronously on
         torch's current stream; info = 0, or 1 + the first variable whose pivot was not positive (dx is then zero)."""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        n = self.layout.dim
-        _check_tensor(hd, buf, torch.float32, self.layout.floats, "buf")
-        if dx is None:
-            dx = torch.empty(n, dtype=torch.float64, device=buf.device)
-        _check_tensor(hd, dx, torch.float64, n, "dx")
-        if info is None:
-            info = torch.empty(1, dtype=torch.int32, device=buf.device)
-        _check_tensor(hd, info, torch.int32, 1, "info")
-        cp = None
-        if code_prior_weight > 0:
-            if codes is None:
-                raise ValueError("code_prior_weight > 0 needs the codes")
-            c64 = np.ascontiguousarray(codes, dtype=np.float64)
-            if c64.shape != (self.layout.num_keyframes, self.layout.code_size):
-                raise ValueError(f"codes must be [{self.layout.num_keyframes}, {self.layout.code_size}]")
-            cp = c64.ctypes.data_as(C.POINTER(C.c_double))
+        buf, cp, dx, info = self._args(buf, code_prior_weight, codes, dx, info)
         prm = _lib.DfkWindowSolveParams(float(lam), float(code_prior_weight))
-        check(self._al.handle, lib().dfk_window_solve(self._al.handle, self.s, C.c_void_p(buf.data_ptr()), C.byref(prm),
-                                                      cp, C.c_void_p(dx.data_ptr()), C.c_void_p(info.data_ptr())))
+        self._hd.call("dfk_window_solve", self.s, buf.data_ptr(), C.byref(prm), cp, dx.data_ptr(), info.data_ptr())
         return dx, info
 
     def update(self, buf: torch.Tensor, diag_eps: float, code_prior_weight: float = 0.0, codes=None,
@@ -1323,31 +1193,15 @@ class WindowSolver:
         re-factorised.  Returns (dx, first_column): dx as solve() gives it, first_column = that column (K: nothing
         changed).  The pivot report goes to `info` when given, else to self.info (0, or 1 + the failed variable; dx is
         then zero).  Synchronises torch's current stream once when the solver has columns to reuse."""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        n = self.layout.dim
-        _check_tensor(hd, buf, torch.float32, self.layout.floats, "buf")
-        if dx is None:
-            dx = torch.empty(n, dtype=torch.float64, device=buf.device)
-        _check_tensor(hd, dx, torch.float64, n, "dx")
         if info is None:
             if self.info is None:
-                self.info = torch.empty(1, dtype=torch.int32, device=buf.device)
+                self.info = torch.empty(1, dtype=torch.int32, device=self._hd.dev)
             info = self.info
-        _check_tensor(hd, info, torch.int32, 1, "info")
-        cp = None
-        if code_prior_weight > 0:
-            if codes is None:
-                raise ValueError("code_prior_weight > 0 needs the codes")
-            c64 = np.ascontiguousarray(codes, dtype=np.float64)
-            if c64.shape != (self.layout.num_keyframes, self.layout.code_size):
-                raise ValueError(f"codes must be [{self.layout.num_keyframes}, {self.layout.code_size}]")
-            cp = c64.ctypes.data_as(C.POINTER(C.c_double))
+        buf, cp, dx, info = self._args(buf, code_prior_weight, codes, dx, info)
         prm = _lib.DfkWindowUpdateParams(float(code_prior_weight), float(diag_eps))
         j0 = C.c_int32(0)
-        check(self._al.handle, lib().dfk_window_solver_update(self._al.handle, self.s, C.c_void_p(buf.data_ptr()),
-                                                              C.byref(prm), cp, C.c_void_p(dx.data_ptr()),
-                                                              C.c_void_p(info.data_ptr()), C.byref(j0)))
+        self._hd.call("dfk_window_solver_update", self.s, buf.data_ptr(), C.byref(prm), cp, dx.data_ptr(),
+                      info.data_ptr(), C.byref(j0))
         return dx, int(j0.value)
 
     def grown(self, window: Window, fixed=()) -> "WindowSolver":
@@ -1356,53 +1210,33 @@ class WindowSolver:
         pattern (dfk_window_solver_create_from).  This solver is left as it was."""
         return WindowSolver(window, fixed, _prev=self)
 
-    def close(self):
-        if getattr(self, "s", None):
-            lib().dfk_window_solver_destroy(self._al.handle, self.s)
-            self.s = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class WindowProblem:
+class WindowProblem(_Owner):
     """A window problem of the C ABI (dfk_window_problem_*): every work item of a window held on the device once, the
     window's state (poses and codes, fp64) on the device, and the Levenberg-Marquardt loop as one call (dfk_window_lm).
     Item arrays are the ctypes arrays of make_work_items / make_reprojection_items / make_geometric_items /
     make_depth_items (their poses and codes are ignored); slots are [n, 4] ints (pose0, pose1, code0, code1; -1 where
     unused); records / geo_records are the caller's record buffers, which linearize writes.  The problem keeps every
     array it was given alive (the image views inside them must stay valid)."""
+    _owned = "p"
 
     def __init__(self, window: Window, records: torch.Tensor, geo_records=None, dense=None, dense_slots=(),
                  reproj=None, reproj_slots=(), geo=None, geo_slots=(), depth=None, depth_slots=(), error=None,
                  error_slots=(), error_depth=(), frame_prior_kf=(), frame_prior_rows=None, frame_prior_x0=None,
                  kf_prior_rows=None, kf_prior_x0=None):
         self._win = window
-        self._al = window._al
-        self.layout = window.layout
+        self._al, self._hd = window._al, window._hd
+        self.layout = L = window.layout
+        records = self._hd.buffer(records, torch.float32, window.num_items * _lib.record_floats(L.code_size), "records")
+        geo_ptr = window._geo_records(geo_records)
         keep = [records, geo_records, dense, reproj, geo, depth, error]
-        S = _lib.DfkWindowItemSlots
 
         def slots(rows):
-            a = np.ascontiguousarray(np.asarray(rows, dtype=np.int32).reshape(-1, 4))
-            keep.append(a)
-            return len(a), (a.ctypes.data_as(C.POINTER(S)) if len(a) else None)
+            a = np.asarray(rows, dtype=np.int32).reshape(-1, 4)
+            return len(a), C.cast(_host(keep, a, np.int32), C.POINTER(_lib.DfkWindowItemSlots)) if len(a) else None
 
-        def f64(x):
-            if x is None:
-                return None
-            a = np.ascontiguousarray(np.asarray(x, dtype=np.float64).ravel())
-            keep.append(a)
-            return a.ctypes.data_as(C.POINTER(C.c_double))
-
-        def i32(x):
-            a = np.ascontiguousarray(np.asarray(x, dtype=np.int32).ravel())
-            keep.append(a)
-            return a.ctypes.data_as(C.POINTER(C.c_int32)) if a.size else None
-
+        f64 = lambda x: None if x is None else _host(keep, np.asarray(x, dtype=np.float64).ravel(), np.float64)
+        i32 = lambda x: _host(keep, np.ravel(x), np.int32, null_if_empty=True)
         nd, ds = slots(dense_slots)
         nr, rs = slots(reproj_slots)
         ng, gs = slots(geo_slots)
@@ -1412,137 +1246,103 @@ class WindowProblem:
         d = _lib.DfkWindowProblemDesc(
             window.w, nd, dense if nd else None, ds, nr, reproj if nr else None, rs, ng, geo if ng else None, gs,
             ndep, depth if ndep else None, dps, ne, error if ne else None, es, i32(error_depth), mf, i32(frame_prior_kf),
-            f64(frame_prior_rows), f64(frame_prior_x0), f64(kf_prior_rows), f64(kf_prior_x0),
-            C.c_void_p(records.data_ptr()), C.c_void_p(geo_records.data_ptr()) if geo_records is not None else None)
+            f64(frame_prior_rows), f64(frame_prior_x0), f64(kf_prior_rows), f64(kf_prior_x0), records.data_ptr(),
+            geo_ptr)
         self._keep = keep
         self.p = C.c_void_p()
-        self._al._hd.use_torch_stream()
-        check(self._al.handle, lib().dfk_window_problem_create(self._al.handle, C.byref(d), C.byref(self.p)))
-        L = self.layout
+        self._hd.call("dfk_window_problem_create", C.byref(d), C.byref(self.p))
         self.num_poses, self.num_codes = L.num_keyframes + L.num_frames, L.num_keyframes * L.code_size
         self.num_dense, self.num_error = nd, ne
 
+    def _free(self, p):
+        lib().dfk_window_problem_destroy(self._al.handle, p)
+
     def set_state(self, poses, codes):
         """poses [(K + F), 7] (keyframes then frames), codes [K, C]: host arrays or device tensors (float64)"""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        args, keep = [], []
+        args = []
         for x, n in ((poses, self.num_poses * 7), (codes, self.num_codes)):
             if isinstance(x, torch.Tensor):
-                _check_tensor(hd, x, torch.float64, n, "state")
-                args.append(C.c_void_p(x.data_ptr()))
+                args.append(self._hd.buffer(x, torch.float64, n, "state").data_ptr())
+            elif np.size(x) != n:
+                raise ValueError(f"the state is {self.num_poses} poses and a [K, C] code array")
             else:
-                a = np.ascontiguousarray(np.asarray(x, dtype=np.float64))
-                if a.size != n:
-                    raise ValueError(f"the state is {self.num_poses} poses and a [K, C] code array")
-                keep.append(a)
-                args.append(a.ctypes.data_as(C.c_void_p))
-        check(hd.h, lib().dfk_window_problem_set_state(hd.h, self.p, *args))
+                args.append(_host([], x, np.float64))
+        self._hd.call("dfk_window_problem_set_state", self.p, *args)
 
     def get_state(self):
         """(poses [(K + F), 7], codes [K, C]) float64 host arrays"""
-        self._al._hd.use_torch_stream()
         P = np.zeros((self.num_poses, 7))
         Q = np.zeros((self.layout.num_keyframes, self.layout.code_size))
-        check(self._al.handle, lib().dfk_window_problem_get_state(self._al.handle, self.p, P.ctypes.data_as(C.c_void_p),
-                                                                   Q.ctypes.data_as(C.c_void_p)))
-        check(self._al.handle, lib().dfk_synchronize(self._al.handle))
+        self._hd.call("dfk_window_problem_get_state", self.p, _ptr(P), _ptr(Q))
+        self._hd.call("dfk_synchronize")
         return P, Q
 
     def linearize(self, out: torch.Tensor | None = None) -> torch.Tensor:
         """dfk_window_problem_linearize: the window buffer at the state (asynchronous on torch's current stream)"""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        if out is None:
-            out = torch.empty(self._win.floats, dtype=torch.float32, device=f"cuda:{hd.device}")
-        _check_tensor(hd, out, torch.float32, self._win.floats, "out")
-        check(hd.h, lib().dfk_window_problem_linearize(hd.h, self.p, C.c_void_p(out.data_ptr())))
-        return out
+        return self._out("dfk_window_problem_linearize", out, torch.float32, self._win.floats)
 
     def error(self, out: torch.Tensor | None = None) -> torch.Tensor:
         """dfk_window_problem_error: [E | photometric | reprojection | geometric | priors | items without inliers |
         inliers] float64 on the device (asynchronous)"""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        if out is None:
-            out = torch.empty(_lib.WINDOW_ERROR_DOUBLES, dtype=torch.float64, device=f"cuda:{hd.device}")
-        _check_tensor(hd, out, torch.float64, _lib.WINDOW_ERROR_DOUBLES, "out")
-        check(hd.h, lib().dfk_window_problem_error(hd.h, self.p, C.c_void_p(out.data_ptr())))
-        return out
+        return self._out("dfk_window_problem_error", out, torch.float64, _lib.WINDOW_ERROR_DOUBLES)
 
     def error_ex(self, out: torch.Tensor | None = None) -> torch.Tensor:
         """dfk_window_problem_error_ex: error()'s 7 doubles, then the depth-prior part of E (asynchronous)"""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        if out is None:
-            out = torch.empty(_lib.WINDOW_ERROR_EX_DOUBLES, dtype=torch.float64, device=f"cuda:{hd.device}")
-        _check_tensor(hd, out, torch.float64, _lib.WINDOW_ERROR_EX_DOUBLES, "out")
-        check(hd.h, lib().dfk_window_problem_error_ex(hd.h, self.p, C.c_void_p(out.data_ptr())))
+        return self._out("dfk_window_problem_error_ex", out, torch.float64, _lib.WINDOW_ERROR_EX_DOUBLES)
+
+    def _out(self, name: str, out, dtype, n: int) -> torch.Tensor:
+        """`name`(problem, out) into n entries of `out`, allocated when not given"""
+        out = self._hd.buffer(out, dtype, n, "out", n)
+        self._hd.call(name, self.p, out.data_ptr())
         return out
 
     def set_depth_priors(self, prior_kf, sigma, level_ptr, items):
         """dfk_window_problem_set_depth_priors: depth prior i on keyframe prior_kf[i] with standard deviation sigma[i]
         owns items[level_ptr[i]:level_ptr[i + 1]] (dicts of target_dpt, prx_orig, prx_jac: one (keyframe, level) each;
         their codes come from the problem's state).  The image views must outlive the problem."""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        kf = np.ascontiguousarray([int(k) for k in prior_kf], dtype=np.int32)
-        sg = np.ascontiguousarray([float(v) for v in sigma], dtype=np.float32)
-        lp = np.ascontiguousarray([int(v) for v in level_ptr], dtype=np.int32)
+        m, lists, _ = _depth_prior_lists(prior_kf, sigma, level_ptr)
         cs = self._al.CS
         arr = make_depth_prior_items([dict(it, code=np.zeros(cs, np.float32)) for it in items], cs)
         self._keep_depth = (arr, [it for it in items])
-        I32 = C.POINTER(C.c_int32)
-        check(hd.h, lib().dfk_window_problem_set_depth_priors(hd.h, self.p, len(kf), kf.ctypes.data_as(I32),
-                                                              sg.ctypes.data_as(C.POINTER(C.c_float)),
-                                                              lp.ctypes.data_as(I32), arr))
+        self._hd.call("dfk_window_problem_set_depth_priors", self.p, m, *lists, arr)
 
     def retract(self, dx: torch.Tensor):
         """dfk_window_problem_retract: state <- retract(state, dx), dx [K B + 6 F] float64 on the device"""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        _check_tensor(hd, dx, torch.float64, self.layout.dim, "dx")
-        check(hd.h, lib().dfk_window_problem_retract(hd.h, self.p, C.c_void_p(dx.data_ptr())))
+        dx = self._hd.buffer(dx, torch.float64, self.layout.dim, "dx")
+        self._hd.call("dfk_window_problem_retract", self.p, dx.data_ptr())
 
     def lm(self, params, use_error: bool = False) -> dict:
         """dfk_window_lm with window_opt.LMParams; returns the trace as a dict"""
-        hd = self._al._hd
-        hd.use_torch_stream()
+        return self._lm("dfk_window_lm", params, use_error)
+
+    def _lm(self, name: str, params, use_error: bool, schedule=(), level_trace=()) -> dict:
+        """`name`(problem, LM params, *schedule, trace, *level_trace): the trace as lm's dict"""
         it = int(params.iterations)
         prm = _lib.DfkLMParams(it, float(params.lambda_init), float(params.lambda_up), float(params.lambda_down),
                                float(params.lambda_max), int(bool(params.fix_first_pose)),
                                float(params.code_prior_weight), int(bool(use_error)))
         e, lam, acc = np.zeros(it + 1), np.zeros(max(it, 1)), np.zeros(max(it, 1), dtype=np.int32)
-        tr = _lib.DfkLMTrace(e.ctypes.data_as(C.POINTER(C.c_double)), lam.ctypes.data_as(C.POINTER(C.c_double)),
-                             acc.ctypes.data_as(C.POINTER(C.c_int32)), 0, 0, 0, 0)
-        check(hd.h, lib().dfk_window_lm(hd.h, self.p, C.byref(prm), C.byref(tr)))
-        return dict(energy=e[:tr.num_energies].tolist(), lam=lam[:tr.num_steps].tolist(),
-                    accepted=[bool(a) for a in acc[:tr.num_steps]], linearisations=int(tr.linearisations),
-                    error_evaluations=int(tr.error_evaluations))
+        tr = _lib.DfkLMTrace(_ptr(e), _ptr(lam), _ptr(acc), 0, 0, 0, 0)
+        self._hd.call(name, self.p, C.byref(prm), *schedule, C.byref(tr), *level_trace)
+        n = tr.num_steps
+        return dict(energy=e[:tr.num_energies].tolist(), lam=lam[:n].tolist(), accepted=[bool(a) for a in acc[:n]],
+                    linearisations=int(tr.linearisations), error_evaluations=int(tr.error_evaluations))
 
     def set_active(self, dense_active, error_active=None):
         """dfk_window_problem_set_active: bool masks over the dense and the error items (error_active None: the dense
         mask, which needs as many error items as dense items)"""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        d = np.ascontiguousarray(np.asarray(dense_active, dtype=bool).astype(np.uint8).ravel())
-        e = None if error_active is None else np.ascontiguousarray(np.asarray(error_active, bool).astype(np.uint8).ravel())
+        d = np.asarray(dense_active, dtype=bool).ravel()
+        e = None if error_active is None else np.asarray(error_active, dtype=bool).ravel()
         if d.size != self.num_dense or (e is not None and e.size != self.num_error) or \
                 (e is None and self.num_error != self.num_dense):
             raise ValueError(f"masks of {self.num_dense} dense and {self.num_error} error items expected (error_active "
                              "may be None only with as many error as dense items)")
-        check(hd.h, lib().dfk_window_problem_set_active(hd.h, self.p, d.ctypes.data_as(C.c_void_p),
-                                                         None if e is None else e.ctypes.data_as(C.c_void_p)))
+        self._hd.call("dfk_window_problem_set_active", self.p, _host([], d, np.uint8),
+                      None if e is None else _host([], e, np.uint8))
 
     def lm_levels(self, params, schedule, use_error: bool = False) -> dict:
         """dfk_window_lm_levels with window_opt.LMParams and window_opt.LevelSchedule; returns dfk_window_lm's trace
         dict plus switch_energy, pair_levels (per step, per pair; -1 = off) and pair_steps_done"""
-        hd = self._al._hd
-        hd.use_torch_stream()
-        it = int(params.iterations)
-        prm = _lib.DfkLMParams(it, float(params.lambda_init), float(params.lambda_up), float(params.lambda_down),
-                               float(params.lambda_max), int(bool(params.fix_first_pose)),
-                               float(params.code_prior_weight), int(bool(use_error)))
         P = len(schedule.steps_done)
         # the C call reads num_dense / num_error / num_pairs entries: wrong lengths are rejected here
         ln = lambda x: len(np.ravel(x))
@@ -1556,36 +1356,19 @@ class WindowProblem:
         if not np.array_equal(np.searchsorted(np.unique(ids), ids), np.asarray(schedule.item_pair)):
             raise ValueError("schedule.item_pair is not the window's pairing of the dense items (the distinct window "
                              "pairs of the dense items in window order)")
-        i32 = lambda x: np.ascontiguousarray(np.asarray(x, dtype=np.int32).ravel())
-        iters, dl, steps = i32(schedule.iters), i32(schedule.item_level), i32(schedule.steps_done)
-        rem = np.ascontiguousarray(np.asarray(schedule.remove_after, dtype=bool).astype(np.uint8).ravel())
-        ep = None if schedule.error_pair is None else i32(schedule.error_pair)
-        el = None if schedule.error_level is None else i32(schedule.error_level)
-        ip = lambda a: None if a is None else a.ctypes.data_as(C.POINTER(C.c_int32))
-        sc = _lib.DfkLevelSchedule(len(iters), ip(iters), ip(dl), ip(ep), ip(el), P, ip(steps),
-                                   rem.ctypes.data_as(C.POINTER(C.c_uint8)) if rem.size else None)
-        e, lam, acc = np.zeros(it + 1), np.zeros(max(it, 1)), np.zeros(max(it, 1), dtype=np.int32)
+        keep = []
+        i32 = lambda x: None if x is None else _host(keep, np.ravel(x), np.int32)
+        rem = _host(keep, np.asarray(schedule.remove_after, dtype=bool).ravel(), np.uint8, null_if_empty=True)
+        sc = _lib.DfkLevelSchedule(ln(schedule.iters), i32(schedule.iters), i32(schedule.item_level),
+                                   i32(schedule.error_pair), i32(schedule.error_level), P, i32(schedule.steps_done), rem)
+        it = int(params.iterations)
         sw, lv, done = np.zeros(max(it, 1)), np.zeros(max(it * P, 1), dtype=np.int32), np.zeros(max(P, 1), np.int32)
-        tr = _lib.DfkLMTrace(e.ctypes.data_as(C.POINTER(C.c_double)), lam.ctypes.data_as(C.POINTER(C.c_double)),
-                             acc.ctypes.data_as(C.POINTER(C.c_int32)), 0, 0, 0, 0)
-        lt = _lib.DfkLevelTrace(sw.ctypes.data_as(C.POINTER(C.c_double)), ip(lv), ip(done), 0)
-        check(hd.h, lib().dfk_window_lm_levels(hd.h, self.p, C.byref(prm), C.byref(sc), C.byref(tr), C.byref(lt)))
-        n = tr.num_steps
-        return dict(energy=e[:tr.num_energies].tolist(), lam=lam[:n].tolist(), accepted=[bool(a) for a in acc[:n]],
-                    linearisations=int(tr.linearisations), error_evaluations=int(tr.error_evaluations),
-                    switch_energy=sw[:lt.num_switches].tolist(),
-                    pair_levels=[lv[s * P:(s + 1) * P].tolist() for s in range(n)], pair_steps_done=done[:P].tolist())
-
-    def close(self):
-        if getattr(self, "p", None):
-            lib().dfk_window_problem_destroy(self._al.handle, self.p)
-            self.p = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        lt = _lib.DfkLevelTrace(_ptr(sw), _ptr(lv), _ptr(done), 0)
+        out = self._lm("dfk_window_lm_levels", params, use_error, [C.byref(sc)], [C.byref(lt)])
+        n = len(out["lam"])
+        out.update(switch_energy=sw[:lt.num_switches].tolist(),
+                   pair_levels=[lv[s * P:(s + 1) * P].tolist() for s in range(n)], pair_steps_done=done[:P].tolist())
+        return out
 
 
 # ------------------------------------------------------------------------------------------- SE3Aligner
@@ -1594,37 +1377,30 @@ class SE3Aligner:
 
     def __init__(self, device=None):
         self._hd = _Handle(device)
-        self._hd.use_torch_stream()
         self.huber_delta_ = 0.1
 
     def SetHuberDelta(self, val: float):
         self.huber_delta_ = float(val)
-        check(self._hd.h, lib().dfk_se3_set_huber_delta(self._hd.h, C.c_float(val)))
+        self._hd.call("dfk_se3_set_huber_delta", C.c_float(val), stream=False)
 
     def RunStep(self, se3, cam, img0, img1, dpt0, grad1) -> JTJJrReductionItem:
-        self._hd.use_torch_stream()
         JtJ = np.zeros(21, dtype=np.float32)
         Jtr = np.zeros(6, dtype=np.float32)
         res = C.c_float(0)
         inl = C.c_uint64(0)
-        F = C.POINTER(C.c_float)
         i0, i1, d0, g1 = _image(img0), _image(img1), _image(dpt0), _image(grad1, 2)
         cc = _cam(cam)
-        st = lib().dfk_se3_run_step(self._hd.h, _pose(se3), C.byref(cc), C.byref(i0), C.byref(i1), C.byref(d0),
-                                    C.byref(g1), JtJ.ctypes.data_as(F), Jtr.ctypes.data_as(F), C.byref(res),
-                                    C.byref(inl))
-        check(self._hd.h, st)
+        self._hd.call("dfk_se3_run_step", _pose(se3), C.byref(cc), C.byref(i0), C.byref(i1), C.byref(d0), C.byref(g1),
+                      _ptr(JtJ), _ptr(Jtr), C.byref(res), C.byref(inl))
         return JTJJrReductionItem(JtJ, Jtr, float(res.value), int(inl.value))
 
     def Warp(self, se3, cam, img0, img1, dpt0, img2) -> CorrespondenceReductionItem:
-        self._hd.use_torch_stream()
         res = C.c_float(0)
         inl = C.c_uint64(0)
         i0, i1, d0, i2 = _image(img0), _image(img1), _image(dpt0), _image(img2)
         cc = _cam(cam)
-        st = lib().dfk_se3_warp(self._hd.h, _pose(se3), C.byref(cc), C.byref(i0), C.byref(i1), C.byref(d0),
-                                C.byref(i2), C.byref(res), C.byref(inl))
-        check(self._hd.h, st)
+        self._hd.call("dfk_se3_warp", _pose(se3), C.byref(cc), C.byref(i0), C.byref(i1), C.byref(d0), C.byref(i2),
+                      C.byref(res), C.byref(inl))
         return CorrespondenceReductionItem(float(res.value), int(inl.value))
 
 
@@ -1651,7 +1427,7 @@ class CameraTracker:
         self.config_ = config
         self.camera_pyr_ = list(camera_pyr)
         self._hd = _Handle(device)
-        check(self._hd.h, lib().dfk_se3_set_huber_delta(self._hd.h, C.c_float(config.huber_delta)))
+        self._hd.call("dfk_se3_set_huber_delta", C.c_float(config.huber_delta), stream=False)
         self.pose_ck_ = np.array([0, 0, 0, 1, 0, 0, 0], dtype=np.float32)
         self.kf_ = None
         self.inliers_ = 0.0
@@ -1683,26 +1459,15 @@ class CameraTracker:
     def TrackFrame(self, pyr_img1, pyr_grad1, keep_history: bool = False):
         if self.kf_ is None:
             raise RuntimeError("Calling CameraTracker::TrackFrame before a keyframe was set")
-        self._hd.use_torch_stream()
         n = self.config_.pyramid_levels
-        levels = (DfkTrackLevel * n)()
-        for l in range(n):
-            levels[l].cam = _cam(self.camera_pyr_[l])
-            levels[l].img0 = _image(self.kf_[0][l])
-            levels[l].img1 = _image(pyr_img1[l])
-            levels[l].dpt0 = _image(self.kf_[1][l])
-            levels[l].grad1 = _image(pyr_grad1[l], 2)
-            levels[l].iterations = int(self.config_.iterations_per_level[l])
+        levels = self._levels([self.kf_], pyr_img1, pyr_grad1)
         total = int(sum(self.config_.iterations_per_level))
         pose = np.ascontiguousarray(self.pose_ck_, dtype=np.float32).copy()
         frac, err = C.c_float(0), C.c_float(0)
         last = np.zeros(29, dtype=np.float32)
         hist = np.zeros((max(total, 1), 36), dtype=np.float32) if keep_history else None
-        F = C.POINTER(C.c_float)
-        st = lib().dfk_se3_track(self._hd.h, pose.ctypes.data_as(F), levels, n, C.byref(frac), C.byref(err),
-                                 last.ctypes.data_as(F), hist.ctypes.data_as(F) if keep_history else None,
-                                 total if keep_history else 0)
-        check(self._hd.h, st)
+        self._hd.call("dfk_se3_track", _ptr(pose), levels, n, C.byref(frac), C.byref(err), _ptr(last),
+                      _ptr(hist) if keep_history else None, total if keep_history else 0)
         self.pose_ck_ = pose
         self.inliers_ = float(frac.value)
         self.error_ = float(err.value)
@@ -1720,23 +1485,18 @@ class CameraTracker:
         n, L = poses.shape[0], self.config_.pyramid_levels
         if len(pyr_img1) < L or len(pyr_grad1) < L:
             raise ValueError(f"the live frame needs {L} pyramid levels")
-        self._hd.use_torch_stream()
-        levels = (DfkTrackLevel * (n * L))()
-        for k, kf in enumerate(keyframes):
-            for l in range(L):
-                lv = levels[k * L + l]
-                lv.cam = _cam(self.camera_pyr_[l])
-                lv.img0 = _image(kf[0][l])
-                lv.img1 = _image(pyr_img1[l])
-                lv.dpt0 = _image(kf[1][l])
-                lv.grad1 = _image(pyr_grad1[l], 2)
-                lv.iterations = int(self.config_.iterations_per_level[l])
+        levels = self._levels(keyframes, pyr_img1, pyr_grad1)
         frac = np.zeros(n, dtype=np.float32)
         err = np.zeros(n, dtype=np.float32)
-        F = C.POINTER(C.c_float)
-        check(self._hd.h, lib().dfk_se3_track_batch(self._hd.h, n, L, poses.ctypes.data_as(F), levels,
-                                                    frac.ctypes.data_as(F), err.ctypes.data_as(F), None))
+        self._hd.call("dfk_se3_track_batch", n, L, _ptr(poses), levels, _ptr(frac), _ptr(err), None)
         return poses, frac, err
+
+    def _levels(self, keyframes, pyr_img1, pyr_grad1):
+        """the DfkTrackLevel of every (keyframe, level), keyframe by keyframe: the live frame against the keyframe"""
+        L, its = self.config_.pyramid_levels, self.config_.iterations_per_level
+        return (DfkTrackLevel * (len(keyframes) * L))(*[
+            DfkTrackLevel(_cam(self.camera_pyr_[l]), _image(kf[0][l]), _image(pyr_img1[l]), _image(kf[1][l]),
+                          _image(pyr_grad1[l], 2), int(its[l])) for kf in keyframes for l in range(L)])
 
     def Relocalize(self, keyframes, pyr_img1, pyr_grad1):
         """DeepFactors::Relocalize (core/deepfactors.cpp:713-743): track the live frame against every keyframe from
@@ -1839,7 +1599,7 @@ def load_dbow2_vocabulary(path) -> dict:
         return parse_dbow2_vocabulary(f.read())
 
 
-class BowVocabulary:
+class BowVocabulary(_Owner):
     """A DBoW2 vocabulary on the device (dfk_bow_vocabulary_create): a path or the dict of load_dbow2_vocabulary.  The
     tree is validated when it is created; TF_IDF / L1_NORM only.  TrainVocabulary returns one too, with the training's
     DfkBowTrainStats in .stats (None for a loaded vocabulary)."""
@@ -1860,7 +1620,7 @@ class BowVocabulary:
                                       arr["descriptors"].ctypes.data, len(arr["word_ids"]), arr["word_ids"].ctypes.data,
                                       arr["word_nodes"].ctypes.data)
         self._p = C.c_void_p()
-        check(self._hd.h, lib().dfk_bow_vocabulary_create(self._hd.h, C.byref(d), C.byref(self._p)))
+        self._hd.call("dfk_bow_vocabulary_create", C.byref(d), C.byref(self._p), stream=False)
 
     @property
     def descriptor_bytes(self) -> int:
@@ -1870,16 +1630,8 @@ class BowVocabulary:
         """the vocabulary as dfk_bow_vocabulary_export lists it (DBoW2's save order, the ids it was created with)"""
         return _export_vocabulary(self._hd, self._p)
 
-    def close(self):
-        if getattr(self, "_p", None) and self._hd.h:
-            lib().dfk_bow_vocabulary_destroy(self._hd.h, self._p)
-            self._p = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def _free(self, p):
+        lib().dfk_bow_vocabulary_destroy(self._hd.h, p)
 
 
 def format_dbow2_vocabulary(voc: dict) -> str:
@@ -1913,11 +1665,11 @@ def save_dbow2_vocabulary(path, voc) -> None:
 
 def _export_vocabulary(hd, p) -> dict:
     shape = _lib.DfkBowVocabularyShape()
-    check(hd.h, lib().dfk_bow_vocabulary_export(hd.h, p, C.byref(shape), None, None, None, None, None, None))
+    hd.call("dfk_bow_vocabulary_export", p, C.byref(shape), None, None, None, None, None, None, stream=False)
     n, W, D = shape.num_nodes, shape.num_words, shape.descriptor_bytes
     arr = dict(node_ids=np.zeros(n, np.int32), parent_ids=np.zeros(n, np.int32), weights=np.zeros(n, np.float64),
                descriptors=np.zeros((n, D), np.uint8), word_ids=np.zeros(W, np.int32), word_nodes=np.zeros(W, np.int32))
-    check(hd.h, lib().dfk_bow_vocabulary_export(hd.h, p, C.byref(shape), *[a.ctypes.data for a in arr.values()]))
+    hd.call("dfk_bow_vocabulary_export", p, C.byref(shape), *[a.ctypes.data for a in arr.values()], stream=False)
     return dict(k=shape.k, L=shape.L, weighting=shape.weighting, scoring=shape.scoring, descriptor_bytes=D, **arr)
 
 
@@ -1940,12 +1692,11 @@ def TrainVocabulary(descriptors, k: int = 10, L: int = 6, seed: int = 0, image_o
         offsets = np.ascontiguousarray(image_offsets, np.int64)
     dev = flat.device if device is None else device
     hd = _Handle(dev)
-    hd.use_torch_stream()
     d = _lib.DfkBowTrainDesc(int(k), int(L), D, len(offsets) - 1, int(seed) & (2 ** 64 - 1), int(flat.shape[0]),
                              flat.data_ptr(), offsets.ctypes.data)
     st = _lib.DfkBowTrainStats()
     p = C.c_void_p()
-    check(hd.h, lib().dfk_bow_vocabulary_train(hd.h, C.byref(d), C.byref(st), C.byref(p)))
+    hd.call("dfk_bow_vocabulary_train", C.byref(d), C.byref(st), C.byref(p))
     voc = BowVocabulary.__new__(BowVocabulary)
     voc._hd, voc._p = hd, p
     voc.voc = _export_vocabulary(hd, p)
@@ -2013,7 +1764,6 @@ def BowTransformBatch(voc: BowVocabulary, descriptors: Sequence, capacities=None
     descriptors are uint8 [N, D] CUDA tensors (or Features), D the vocabulary's.  capacities (default N) reserve each
     item's output rows.  Asynchronous: returns a BowBatch of device tensors."""
     hd = voc._hd
-    hd.use_torch_stream()
     rows = [_descriptor_rows(d) for d in descriptors]
     n = len(rows)
     caps = [int(r.shape[0]) for r in rows] if capacities is None else [int(c) for c in capacities]
@@ -2024,14 +1774,12 @@ def BowTransformBatch(voc: BowVocabulary, descriptors: Sequence, capacities=None
     cap_arr = (C.c_int32 * max(n, 1))(*caps)
     offsets = np.concatenate([[0], np.cumsum(caps)]).astype(np.int64)
     total = int(offsets[-1])
-    dev = f"cuda:{hd.device}"
-    words = torch.zeros(max(total, 1), dtype=torch.int32, device=dev)
-    values = torch.zeros(max(total, 1), dtype=torch.float64, device=dev)
-    fw = torch.zeros(max(total, 1), dtype=torch.int32, device=dev)
-    counts = torch.zeros(max(n, 1), dtype=torch.int32, device=dev)
-    check(hd.h, lib().dfk_bow_transform_batch(hd.h, voc._p, sets, cap_arr, n, C.c_void_p(words.data_ptr()),
-                                              C.c_void_p(values.data_ptr()), C.c_void_p(counts.data_ptr()),
-                                              C.c_void_p(fw.data_ptr())))
+    words = torch.zeros(max(total, 1), dtype=torch.int32, device=hd.dev)
+    values = torch.zeros(max(total, 1), dtype=torch.float64, device=hd.dev)
+    fw = torch.zeros(max(total, 1), dtype=torch.int32, device=hd.dev)
+    counts = torch.zeros(max(n, 1), dtype=torch.int32, device=hd.dev)
+    hd.call("dfk_bow_transform_batch", voc._p, sets, cap_arr, n, words.data_ptr(), values.data_ptr(), counts.data_ptr(),
+            fw.data_ptr())
     return BowBatch(words, values, counts[:n], fw, offsets, np.array(caps, np.int64))
 
 
@@ -2052,70 +1800,57 @@ class BowQueryResult:
                 for i, (o, m) in enumerate(zip(self.offsets[:-1], self.max_results))]
 
 
-class BowDatabase:
+class BowDatabase(_Owner):
     """TemplatedDatabase(voc, false, 0) on the device (dfk_bow_database_*): add, query, score, clear, len."""
 
     def __init__(self, voc: BowVocabulary):
         self.voc = voc
         self._hd = voc._hd
         self._p = C.c_void_p()
-        check(self._hd.h, lib().dfk_bow_database_create(self._hd.h, voc._p, C.byref(self._p)))
+        self._hd.call("dfk_bow_database_create", voc._p, C.byref(self._p), stream=False)
+
+    def _free(self, p):
+        lib().dfk_bow_database_destroy(self._hd.h, p)
 
     def __len__(self) -> int:
         n = C.c_int32()
-        check(self._hd.h, lib().dfk_bow_database_size(self._hd.h, self._p, C.byref(n)))
+        self._hd.call("dfk_bow_database_size", self._p, C.byref(n), stream=False)
         return int(n.value)
 
     def clear(self):
-        check(self._hd.h, lib().dfk_bow_database_clear(self._hd.h, self._p))
+        self._hd.call("dfk_bow_database_clear", self._p, stream=False)
 
     def add(self, vectors: Sequence[BowVector]) -> int:
         """adds the vectors in order (copied on the device, no read-back); returns the first entry id"""
-        self._hd.use_torch_stream()
         n = len(vectors)
         arr = (_lib.DfkBowVector * max(n, 1))(*[v.to_c() for v in vectors])
         first = C.c_int32(-1)
-        check(self._hd.h, lib().dfk_bow_database_add(self._hd.h, self._p, arr, n, C.byref(first)))
+        self._hd.call("dfk_bow_database_add", self._p, arr, n, C.byref(first))
         return int(first.value)
 
     def query(self, vectors: Sequence[BowVector], max_results=1, max_id=-1) -> BowQueryResult:
         """db_.query(vec, ret, max_results, max_id) for every vector in one call (dfk_bow_database_query_batch);
         max_results and max_id are one value for all or one per vector.  Asynchronous."""
-        self._hd.use_torch_stream()
         n = len(vectors)
-        per = lambda v: [int(x) for x in (v if isinstance(v, (list, tuple, np.ndarray)) else [v] * n)]
-        mr, mi = per(max_results), per(max_id)
+        mr, mi = _per_item(max_results, n, int, "BowDatabase.query"), _per_item(max_id, n, int, "BowDatabase.query")
         arr = (_lib.DfkBowQuery * max(n, 1))(*[_lib.DfkBowQuery(v.to_c(), a, b) for v, a, b in zip(vectors, mr, mi)])
         offsets = np.concatenate([[0], np.cumsum(mr)]).astype(np.int64)
-        dev = f"cuda:{self._hd.device}"
+        dev = self._hd.dev
         ids = torch.full((max(int(offsets[-1]), 1),), -1, dtype=torch.int32, device=dev)
         scores = torch.zeros(max(int(offsets[-1]), 1), dtype=torch.float64, device=dev)
         counts = torch.zeros(max(n, 1), dtype=torch.int32, device=dev)
-        check(self._hd.h, lib().dfk_bow_database_query_batch(self._hd.h, self._p, arr, n, C.c_void_p(ids.data_ptr()),
-                                                             C.c_void_p(scores.data_ptr()),
-                                                             C.c_void_p(counts.data_ptr())))
+        self._hd.call("dfk_bow_database_query_batch", self._p, arr, n, ids.data_ptr(), scores.data_ptr(),
+                      counts.data_ptr())
         return BowQueryResult(ids, scores, counts[:n], offsets, np.array(mr, np.int64))
 
     def score(self, entries: Sequence[int], vectors: Sequence[BowVector]) -> torch.Tensor:
         """voc_.score(entry's vector, vector) per pair (dfk_bow_score_batch): float64 [n] on the device"""
-        self._hd.use_torch_stream()
         n = len(vectors)
         arr = (_lib.DfkBowScoreItem * max(n, 1))(*[_lib.DfkBowScoreItem(int(e), v.to_c())
                                                    for e, v in zip(entries, vectors)])
-        out = torch.zeros(max(n, 1), dtype=torch.float64, device=f"cuda:{self._hd.device}")
-        check(self._hd.h, lib().dfk_bow_score_batch(self._hd.h, self._p, arr, n, C.c_void_p(out.data_ptr())))
+        out = torch.zeros(max(n, 1), dtype=torch.float64, device=self._hd.dev)
+        self._hd.call("dfk_bow_score_batch", self._p, arr, n, out.data_ptr())
         return out[:n]
-
-    def close(self):
-        if getattr(self, "_p", None) and self._hd.h:
-            lib().dfk_bow_database_destroy(self._hd.h, self._p)
-            self._p = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 # ------------------------------------------------------------------------------------------- LoopDetector
@@ -2253,50 +1988,42 @@ def _free_handle(device=None) -> _Handle:
     dev = torch.cuda.current_device() if device is None else torch.device(device).index
     if dev not in _default_handle:
         _default_handle[dev] = _Handle(dev)
-    hd = _default_handle[dev]
-    hd.use_torch_stream()
-    return hd
+    return _default_handle[dev]
 
 
 def UpdateDepth(code, prx_orig, prx_jac, avg_dpt, dpt_out):
     """df::UpdateDepth (cu_image_proc.cpp:266-277): dpt = avg/(prx_orig + prx_jac.code) - avg."""
     hd = _free_handle(dpt_out.device)
-    code = np.ascontiguousarray(code, dtype=np.float32)
-    cs = int(code.shape[0])
+    cs = int(np.shape(code)[0])
     p, j, d = _image(prx_orig), _image(prx_jac, cs), _image(dpt_out)
-    st = lib().dfk_update_depth(hd.h, code.ctypes.data_as(C.POINTER(C.c_float)), cs, C.byref(p), C.byref(j),
-                                C.c_float(avg_dpt), C.byref(d))
-    check(hd.h, st)
+    hd.call("dfk_update_depth", _host([], code, np.float32), cs, C.byref(p), C.byref(j), C.c_float(avg_dpt),
+            C.byref(d))
 
 
 def SobelGradients(img, grad):
     """df::SobelGradients (cu_image_proc.cpp:95-113)."""
-    hd = _free_handle(img.device)
     i, g = _image(img), _image(grad, 2)
-    check(hd.h, lib().dfk_sobel_gradients(hd.h, C.byref(i), C.byref(g)))
+    _free_handle(img.device).call("dfk_sobel_gradients", C.byref(i), C.byref(g))
 
 
 def GaussianBlurDown(inp, out):
     """df::GaussianBlurDown (cu_image_proc.cpp:166-184)."""
-    hd = _free_handle(inp.device)
     i, o = _image(inp), _image(out)
-    check(hd.h, lib().dfk_gaussian_blur_down(hd.h, C.byref(i), C.byref(o)))
+    _free_handle(inp.device).call("dfk_gaussian_blur_down", C.byref(i), C.byref(o))
 
 
 def BuildImagePyramid(imgs, grads=None):
     """imgs[0] given; fills imgs[1:] by GaussianBlurDown and grads[:] by SobelGradients, all enqueued at once
     (Frame::FillPyramids, core/mapping/frame.h:80-94)."""
-    hd = _free_handle()
     n = len(imgs)
     ia = (DfkImage * n)(*[_image(t) for t in imgs])
     ga = (DfkImage * n)(*[_image(t, 2) for t in grads]) if grads is not None else None
-    check(hd.h, lib().dfk_build_image_pyramid(hd.h, ia, ga, n))
+    _free_handle().call("dfk_build_image_pyramid", ia, ga, n)
 
 
 def SquaredError(buf1, buf2) -> float:
     """df::SquaredError (cu_image_proc.cpp:208-242)."""
-    hd = _free_handle(buf1.device)
     a, b = _image(buf1), _image(buf2)
     out = C.c_float(0)
-    check(hd.h, lib().dfk_squared_error(hd.h, C.byref(a), C.byref(b), C.byref(out)))
+    _free_handle(buf1.device).call("dfk_squared_error", C.byref(a), C.byref(b), C.byref(out))
     return float(out.value)
