@@ -142,6 +142,30 @@ class DfkLevelTrace(C.Structure):
                 ("pair_steps_done", C.POINTER(C.c_int32)), ("num_switches", C.c_int32)]
 
 
+class DfkIsam2Params(C.Structure):
+    _fields_ = [("relinearize_threshold", C.c_double), ("relinearize_skip", C.c_int32),
+                ("code_prior_weight", C.c_double), ("fix_first_pose", C.c_int32)]
+
+
+class DfkIsam2Result(C.Structure):
+    _fields_ = [("variables_relinearized", C.c_int32), ("variables_reeliminated", C.c_int32),
+                ("factors_relinearised", C.c_int32), ("first_column", C.c_int32)]
+
+
+MAX_WORK_LEVELS = 8  # DFK_MAX_WORK_LEVELS
+
+
+class DfkWorkState(C.Structure):
+    _fields_ = [("active_level", C.c_int32), ("iters", C.c_int32 * MAX_WORK_LEVELS), ("first", C.c_int32),
+                ("remove", C.c_int32), ("factor", C.c_int32), ("erased", C.c_int32)]
+
+
+class DfkMapTrace(C.Structure):
+    _fields_ = [("variables_relinearized", C.POINTER(C.c_int32)), ("variables_reeliminated", C.POINTER(C.c_int32)),
+                ("factors_relinearised", C.POINTER(C.c_int32)), ("first_column", C.POINTER(C.c_int32)),
+                ("pair_levels", C.POINTER(C.c_int32)), ("num_steps", C.c_int32)]
+
+
 class DfkFeatureSet(C.Structure):
     _fields_ = [("keypoints", C.c_void_p), ("descriptors", C.c_void_p), ("num", C.c_int32),
                 ("descriptor_bytes", C.c_int32)]
@@ -317,6 +341,13 @@ SYMBOLS = {
     "dfk_window_problem_set_active": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dfk_window_lm_levels": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkLMParams), C.POINTER(DfkLevelSchedule),
                                        C.POINTER(DfkLMTrace), C.POINTER(DfkLevelTrace)]),
+    "dfk_window_problem_isam2_update": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkIsam2Params),
+                                                  C.POINTER(DfkIsam2Result)]),
+    "dfk_window_problem_get_linearization": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dfk_window_problem_grow_from": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                               C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "dfk_window_map_steps": (C.c_int, [_H, C.c_void_p, C.POINTER(DfkIsam2Params), C.POINTER(DfkLevelSchedule),
+                                       C.POINTER(DfkWorkState), C.c_int, C.POINTER(DfkMapTrace)]),
     "dfk_se3_run_step": (C.c_int, [_H, _F, _CAM, _IMG, _IMG, _IMG, _IMG, _F, _F, _F, C.POINTER(C.c_uint64)]),
     "dfk_se3_track": (C.c_int, [_H, _F, C.POINTER(DfkTrackLevel), C.c_int, _F, _F, _F, _F, C.c_int]),
     "dfk_se3_track_batch": (C.c_int, [_H, C.c_int, C.c_int, _F, C.POINTER(DfkTrackLevel), _F, _F, _F]),

@@ -1252,7 +1252,7 @@ class WindowProblem(_Owner):
         self.p = C.c_void_p()
         self._hd.call("dfk_window_problem_create", C.byref(d), C.byref(self.p))
         self.num_poses, self.num_codes = L.num_keyframes + L.num_frames, L.num_keyframes * L.code_size
-        self.num_dense, self.num_error = nd, ne
+        self.num_dense, self.num_error, self.num_reproj, self.num_geo = nd, ne, nr, ng
 
     def _free(self, p):
         lib().dfk_window_problem_destroy(self._al.handle, p)
@@ -1369,6 +1369,88 @@ class WindowProblem(_Owner):
         out.update(switch_energy=sw[:lt.num_switches].tolist(),
                    pair_levels=[lv[s * P:(s + 1) * P].tolist() for s in range(n)], pair_steps_done=done[:P].tolist())
         return out
+
+    @staticmethod
+    def _isam2_params(relinearize_threshold, relinearize_skip, code_prior_weight, fix_first_pose):
+        return _lib.DfkIsam2Params(float(relinearize_threshold), int(relinearize_skip), float(code_prior_weight),
+                                   int(bool(fix_first_pose)))
+
+    def isam2_update(self, relinearize_threshold=0.05, relinearize_skip=1, code_prior_weight=0.0,
+                     fix_first_pose=True) -> tuple:
+        """dfk_window_problem_isam2_update: one IncrementalOptimizer.update() on the device.  Returns
+        (variables_relinearized, variables_reeliminated, factors_relinearised, first_column)."""
+        prm = self._isam2_params(relinearize_threshold, relinearize_skip, code_prior_weight, fix_first_pose)
+        r = _lib.DfkIsam2Result()
+        self._hd.call("dfk_window_problem_isam2_update", self.p, C.byref(prm), C.byref(r))
+        return r.variables_relinearized, r.variables_reeliminated, r.factors_relinearised, r.first_column
+
+    def get_linearization(self):
+        """dfk_window_problem_get_linearization: (theta_lin poses [(K + F), 7], theta_lin codes [K, C], delta
+        [K B + 6 F]) float64 host arrays of the last ISAM2 update"""
+        P = np.zeros((self.num_poses, 7))
+        Q = np.zeros((self.layout.num_keyframes, self.layout.code_size))
+        D = np.zeros(self.layout.dim)
+        self._hd.call("dfk_window_problem_get_linearization", self.p, _ptr(P), _ptr(Q), _ptr(D))
+        self._hd.call("dfk_synchronize")
+        return P, Q, D
+
+    def grow_from(self, old: "WindowProblem", dense_of, rep_of, geo_of, frame_of):
+        """dfk_window_problem_grow_from: continue `old`'s ISAM2 run on this grown problem; each map gives the old item
+        of every item of this problem (-1: new)"""
+        keep = []
+        maps = []
+        for x, n, what in ((dense_of, self.num_dense, "dense_of"), (rep_of, self.num_reproj, "rep_of"),
+                           (geo_of, self.num_geo, "geo_of"), (frame_of, self.layout.num_frames, "frame_of")):
+            maps.append(_host(keep, np.asarray(list(x), dtype=np.int64).astype(np.int32), np.int32, (n,), what,
+                              null_if_empty=True))
+        self._hd.call("dfk_window_problem_grow_from", self.p, old.p, *maps)
+
+    def map_steps(self, schedule, works, max_steps: int, relinearize_threshold=0.05, relinearize_skip=1,
+                  code_prior_weight=0.0, fix_first_pose=True) -> dict:
+        """dfk_window_map_steps with a window_opt.LevelSchedule (its iters, item_level, error_pair / error_level and
+        remove_after; steps_done is ignored) and `works`: one window_opt.OptimizeWork per schedule pair, or None for
+        fresh works.  The works' states are read and rewritten in place.  Returns the trace: per step the four
+        ISAM2Result counts and every pair's factor level (-1: none)."""
+        P, L = len(schedule.remove_after), len(schedule.iters)
+        ln = lambda x: len(np.ravel(x))
+        if ln(schedule.item_level) != self.num_dense or \
+                any(x is not None and ln(x) != self.num_error for x in (schedule.error_pair, schedule.error_level)) or \
+                (works is not None and len(works) != P):
+            raise ValueError(f"a schedule of {self.num_dense} dense items, {self.num_error} error items and one work "
+                             f"per pair ({P}) expected")
+        keep = []
+        i32 = lambda x: None if x is None else _host(keep, np.ravel(x), np.int32)
+        rem = _host(keep, np.asarray(schedule.remove_after, dtype=bool).ravel(), np.uint8, null_if_empty=True)
+        sc = _lib.DfkLevelSchedule(L, i32(schedule.iters), i32(schedule.item_level), i32(schedule.error_pair),
+                                   i32(schedule.error_level), P, None, rem)
+        ws = (_lib.DfkWorkState * max(P, 1))()
+        if works is not None:
+            for q, w in enumerate(works):
+                if len(w.iters) != L or L > _lib.MAX_WORK_LEVELS:
+                    raise ValueError(f"work {q} has {len(w.iters)} levels, the schedule {L} (at most "
+                                     f"{_lib.MAX_WORK_LEVELS})")
+                ws[q].active_level, ws[q].first, ws[q].remove = w.active_level, int(w.first), int(w.remove)
+                ws[q].factor = -1 if w.factor is None else w.factor
+                ws[q].erased = int(w.erased)
+                for l in range(L):
+                    ws[q].iters[l] = w.iters[l]
+        n = max(int(max_steps), 1)
+        cols = [np.zeros(n, np.int32) for _ in range(4)]
+        lv = np.zeros(n * max(P, 1), np.int32)
+        tr = _lib.DfkMapTrace(*[_ptr(c) for c in cols], _ptr(lv), 0)
+        prm = self._isam2_params(relinearize_threshold, relinearize_skip, code_prior_weight, fix_first_pose)
+        self._hd.call("dfk_window_map_steps", self.p, C.byref(prm), C.byref(sc), ws if works is not None else None,
+                      int(max_steps), C.byref(tr))
+        if works is not None:
+            for q, w in enumerate(works):
+                w.active_level, w.first, w.remove = ws[q].active_level, bool(ws[q].first), bool(ws[q].remove)
+                w.factor = None if ws[q].factor < 0 else ws[q].factor
+                w.erased = bool(ws[q].erased)
+                w.iters = [ws[q].iters[l] for l in range(L)]
+        s = tr.num_steps
+        return dict(variables_relinearized=cols[0][:s].tolist(), variables_reeliminated=cols[1][:s].tolist(),
+                    factors_relinearised=cols[2][:s].tolist(), first_column=cols[3][:s].tolist(),
+                    pair_levels=[lv[i * P:(i + 1) * P].tolist() for i in range(s)])
 
 
 # ------------------------------------------------------------------------------------------- SE3Aligner

@@ -1,5 +1,5 @@
 // dfk_api_window.cu -- C ABI of libdfk.so (see include/dfk.h), keyframe window: the window (create, assemble, priors,
-// marginalisation, blanket), its solver, and the window problem with its Levenberg-Marquardt loops.
+// marginalisation, blanket), its solver, and the window problem with its Levenberg-Marquardt loops and ISAM2 steps.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -16,6 +16,7 @@
 #include "dfk_internal.h"
 #include "dfk_levels.h"
 #include "dfk_lm.h"
+#include "dfk_works.h"
 
 using namespace dfk;
 
@@ -113,6 +114,32 @@ struct DfkWindowProblem {
   Part<int> dp_csr, dp_level_ptr, dp_kf;
   Part<float> dp_sigma;
   DeviceBuf<float> dp_partials, dp_records, dp_err;
+  std::vector<int> dp_item_kf;       // the keyframe of every depth-prior item
+  // ISAM2 (dfk_window_problem_isam2_update): two slots [theta_lin S | Delta K B + 6 F] doubles, [ic] the committed one
+  // (an update writes the other and commits it when the solve succeeds), and the host's "linearised at theta_lin" flag
+  // of every dense item, reprojection link, geometric link and depth-prior item
+  DeviceBuf<double> isam;
+  int ic = 0;
+  bool isam_fresh = true;            // the next update starts from the state
+  long long isam_updates = 0;
+  double diag_eps = -1.0;            // fixed by the first update
+  std::vector<uint8_t> lin_dense, lin_rep, lin_geo, lin_dp;
+  std::vector<uint8_t> active;       // the dense mask of the last set_active
+  std::vector<int4> rep_slots_h, geo_slots_h;
+  std::vector<int> rep_size_h, geo_size_h;  // matches / points of every link (growth checks them)
+  DeviceBuf<int2> gather;                    // dfk_window_problem_grow_from's (new row, old row) lists
+  // the read-back block [diagonal max | moved flags 2 K + F | info] and its pinned mirror
+  DeviceBuf<unsigned char> isam_small;
+  PinnedBuf<unsigned char> isam_small_host;
+  DeviceBuf<uint8_t> stale_dev;      // reprojection | geometric | depth-prior items
+  DeviceBuf<int2> self_pairs;        // (pair, keyframe) of every pair (k, k)
+  int num_self = -1;
+  // the stale active dense items: their items, slots, tile plan and records, and every slot's source
+  SfmLaunchPlan stale_plan;
+  DeviceBuf<SfmItemDev> stale_items;
+  DeviceBuf<int4> stale_slots;
+  DeviceBuf<int> stale_src;
+  DeviceBuf<float> stale_records;
   ~DfkWindowProblem()
   {
     window_solver_destroy(solver[0]);
@@ -122,6 +149,16 @@ struct DfkWindowProblem {
   double* energy() const { return sm_energy.at(small.at(blob.ptr)); }
   int32_t* info() const { return sm_info.at(small.at(blob.ptr)); }
   double* depth_energy() const { return sm_depth_energy.at(small.at(blob.ptr)); }
+  size_t delta_size() const { return (size_t)K * B + 6 * (size_t)F; }
+  double* lin(int i) const { return isam.ptr + (size_t)i * (S + delta_size()); }
+  double* isam_delta(int i) const { return lin(i) + S; }
+  void clear_linearised()
+  {
+    std::fill(lin_dense.begin(), lin_dense.end(), 0);
+    std::fill(lin_rep.begin(), lin_rep.end(), 0);
+    std::fill(lin_geo.begin(), lin_geo.end(), 0);
+    std::fill(lin_dp.begin(), lin_dp.end(), 0);
+  }
 };
 
 namespace {
@@ -172,14 +209,17 @@ WindowReposeDev repose_args(const DfkWindowProblem* p, const double* state)
   return a;
 }
 
-// the depth priors' batch at `state`: the items' codes from the state, then the records (gram) or the error rows
-DfkStatus problem_depth_priors(DfkHandle h, DfkWindowProblem* p, const double* state, bool gram, const char* what)
+// the depth priors' batch at `state`: the items' codes from the state, then the records (gram) or the error rows;
+// stale (device, optional): only those items are written
+DfkStatus problem_depth_priors(DfkHandle h, DfkWindowProblem* p, const double* state, bool gram, const char* what,
+                               const uint8_t* stale = nullptr)
 {
   DFK_CUDA(h, launch_depth_prior_codes(state + (size_t)(p->K + p->F) * 7, p->dp_kf.at(p->dp_lists.ptr), p->ndpi, p->C,
                                        p->dp_st.codes.at(p->dp.ptr), h->stream),
            what);
   DFK_CUDA(h, launch_depth_prior_batch(p->C, p->dp_st.descs.at(p->dp.ptr), p->ndpi, p->dp_st.max_parts, p->avg_dpt,
-                                       p->dp_partials.ptr, gram ? p->dp_records.ptr : p->dp_err.ptr, gram, h->stream),
+                                       p->dp_partials.ptr, gram ? p->dp_records.ptr : p->dp_err.ptr, gram, h->stream,
+                                       stale),
            what);
   h->launches += 3;
   return DFK_OK;
@@ -195,11 +235,15 @@ DfkStatus problem_deltas(DfkHandle h, const DfkWindowProblem* p, const double* s
   return DFK_OK;
 }
 
-// the window buffer at state `state` into buf (dfk_window_problem_linearize)
+DfkStatus problem_finish(DfkHandle h, DfkWindowProblem* p, const double* state, float* buf, const uint8_t* dp_stale);
+
+// the window buffer at state `state` into buf (dfk_window_problem_linearize).  Every record is rewritten, so no item
+// is linearised at the ISAM2 theta_lin any more
 DfkStatus problem_linearize(DfkHandle h, DfkWindowProblem* p, const double* state, float* buf)
 {
   const char* what = "[WindowProblem::linearize] kernel launch failed";
   unsigned char* b = p->blob.ptr;
+  p->clear_linearised();
   DFK_CUDA(h, launch_window_repose(repose_args(p, state), h->stream), what);
   h->launches += 1;
   const float avg = p->avg_dpt;
@@ -232,6 +276,15 @@ DfkStatus problem_linearize(DfkHandle h, DfkWindowProblem* p, const double* stat
              what);
     h->launches += 1;
   }
+  return problem_finish(h, p, state, buf, nullptr);
+}
+
+// the buffer from the records: the assembly, the frame and keyframe priors at `state`, then the depth priors (only the
+// dp_stale items re-evaluated when given)
+DfkStatus problem_finish(DfkHandle h, DfkWindowProblem* p, const double* state, float* buf, const uint8_t* dp_stale)
+{
+  const char* what = "[WindowProblem::linearize] kernel launch failed";
+  unsigned char* b = p->blob.ptr;
   const DfkWindow* w = p->w;
   DFK_TRY(assemble_window(h, w, p->records, p->ng > 0 ? p->geo_records : nullptr, buf, what));
   DFK_TRY(problem_deltas(h, p, state));
@@ -248,7 +301,7 @@ DfkStatus problem_linearize(DfkHandle h, DfkWindowProblem* p, const double* stat
     h->launches += 1;
   }
   if (p->ndp > 0) {  // after the frame and keyframe priors, as SfmWindowProblem.linearise without an all-reduce
-    DFK_TRY(problem_depth_priors(h, p, state, true, what));
+    DFK_TRY(problem_depth_priors(h, p, state, true, what, dp_stale));
     unsigned char* l = p->dp_lists.ptr;
     DFK_CUDA(h, launch_window_add_depth_priors(w->dev, p->ndp, p->dp_csr.at(l), p->dp_csr.at(l) + p->K + 1,
                                                p->dp_level_ptr.at(l), p->dp_sigma.at(l), p->dp_records.ptr, buf,
@@ -338,6 +391,11 @@ DfkStatus problem_set_active(DfkHandle h, DfkWindowProblem* p, const uint8_t* dm
   const char* umsg = "[WindowProblem::set_active] upload failed";
   const int nd = p->nd, ne = p->ne;
   const bool all_d = std::all_of(dm, dm + nd, [](uint8_t v) { return v != 0; });
+  for (int i = 0; i < nd; ++i) {
+    // an item switched on or off holds another record than its last linearisation left: stale for ISAM2
+    if (p->active[i] != (dm[i] != 0)) p->lin_dense[i] = 0;
+    p->active[i] = dm[i] != 0;
+  }
   const bool all_e = std::all_of(em, em + ne, [](uint8_t v) { return v != 0; });
   if (!all_d || !all_e) {
     DFK_CUDA(h, p->sub_slots.ensure((size_t)std::max(nd + ne, 1)), amsg);
@@ -477,6 +535,260 @@ DfkStatus lm_setup(DfkHandle h, DfkWindowProblem* p, const DfkLMParams* prm, Dfk
   DFK_CUDA(h, p->bufs.ensure(2 * nf), amsg.c_str());
   DFK_CUDA(h, p->dx.ensure((size_t)p->K * p->B + 6 * (size_t)p->F), amsg.c_str());
   *ops = ProblemLMOps{h, p, prm, p->solver[fix], nf, f_off, prm->code_prior_weight};
+  return DFK_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------- ISAM2
+DfkStatus isam2_check(DfkHandle h, const DfkWindowProblem* p, const DfkIsam2Params* prm, const std::string& what)
+{
+  if (!p || !prm) return fail(h, DFK_ERR_INVALID_ARG, what + "null argument");
+  if (p->device != h->device) return fail(h, DFK_ERR_INVALID_ARG, what + "problem and handle live on different devices");
+  if (prm->relinearize_skip < 1 || std::isnan(prm->relinearize_threshold) ||
+      !(std::isfinite(prm->code_prior_weight) && prm->code_prior_weight >= 0.0))
+    return fail(h, DFK_ERR_INVALID_ARG, what + "relinearize_skip must be >= 1, relinearize_threshold a number and "
+                                               "code_prior_weight finite and >= 0");
+  return DFK_OK;
+}
+
+// the buffers of the ISAM2 state and of a partial linearisation, allocated at their full sizes so that no later update
+// reallocates what a queued launch reads; the solver of fix_first_pose; a fresh run starts from the state
+DfkStatus isam2_setup(DfkHandle h, DfkWindowProblem* p, int fix, const char* amsg)
+{
+  const int K = p->K, F = p->F, nd = p->nd;
+  DFK_CUDA(h, p->isam.ensure(2 * (p->S + p->delta_size())), amsg);
+  DFK_CUDA(h, p->isam_small.ensure(sizeof(double) + (size_t)(2 * K + F + 1) * 4), amsg);
+  DFK_CUDA(h, p->isam_small_host.ensure(sizeof(double) + (size_t)(2 * K + F + 1) * 4), amsg);
+  DFK_CUDA(h, p->stale_dev.ensure((size_t)std::max(1, p->nr + p->ng + p->ndpi)), amsg);
+  DFK_CUDA(h, p->stale_items.ensure((size_t)std::max(nd, 1)), amsg);
+  DFK_CUDA(h, p->stale_slots.ensure((size_t)std::max(nd, 1)), amsg);
+  DFK_CUDA(h, p->stale_src.ensure((size_t)std::max(nd, 1)), amsg);
+  DFK_CUDA(h, p->stale_records.ensure((size_t)std::max(nd, 1) * DFK_SFM_RECORD_FLOATS(p->C)), amsg);
+  DFK_CUDA(h, p->bufs.ensure(2 * p->w->floats), amsg);
+  if (!p->solver[fix])
+    DFK_CUDA(h, window_solver_create(K, p->C, F, p->w->pair_k0, p->w->pair_k1, p->w->link_k0, p->w->link_k1,
+                                     p->w->blk_i, p->w->blk_j, p->w->kp.block_off, std::vector<int>(), &p->solver[0]),
+             amsg);
+  if (p->num_self < 0) {
+    std::vector<int2> self;
+    for (size_t q = 0; q < p->w->pair_k0.size(); ++q)
+      if (p->w->pair_k0[q] == p->w->pair_k1[q]) self.push_back(make_int2((int)q, p->w->pair_k0[q]));
+    DFK_CUDA(h, p->self_pairs.ensure(std::max<size_t>(1, self.size())), amsg);
+    if (!self.empty())
+      DFK_CUDA(h, cudaMemcpyAsync(p->self_pairs.ptr, self.data(), sizeof(int2) * self.size(), cudaMemcpyHostToDevice,
+                                  h->stream),
+               amsg);
+    p->num_self = (int)self.size();
+  }
+  if (p->isam_fresh) {
+    DFK_CUDA(h, cudaMemcpyAsync(p->lin(p->ic), p->st(p->cur), sizeof(double) * p->S, cudaMemcpyDeviceToDevice, h->stream),
+             amsg);
+    DFK_CUDA(h, cudaMemsetAsync(p->isam_delta(p->ic), 0, sizeof(double) * p->delta_size(), h->stream), amsg);
+    p->clear_linearised();
+    p->isam_updates = 0;
+    p->diag_eps = -1.0;
+    p->isam_fresh = false;
+  }
+  return DFK_OK;
+}
+
+// one IncrementalOptimizer.update() (dfk_window_problem_isam2_update's steps 1-6)
+DfkStatus problem_isam2_update(DfkHandle h, DfkWindowProblem* p, const DfkIsam2Params* prm, DfkIsam2Result* res)
+{
+  const char* what = "[WindowProblem::isam2_update] kernel launch failed";
+  const char* amsg = "[WindowProblem::isam2_update] allocation failed";
+  const char* umsg = "[WindowProblem::isam2_update] upload failed";
+  const int K = p->K, F = p->F, C = p->C, B = p->B, nd = p->nd, nr = p->nr, ng = p->ng, ndpi = p->ndpi;
+  const int fix = prm->fix_first_pose ? 1 : 0;
+  DFK_TRY(isam2_setup(h, p, fix, amsg));
+  const int nxt = 1 - p->ic;
+  const double* lin_in = p->lin(p->ic);
+  double* lin = p->lin(nxt);
+  double* delta = p->isam_delta(nxt);
+  unsigned char* sd = p->isam_small.ptr;
+  unsigned char* sh = p->isam_small_host.ptr;
+  double* diag_dev = reinterpret_cast<double*>(sd);  // first: 8-byte aligned
+  int32_t* moved_dev = reinterpret_cast<int32_t*>(sd + sizeof(double));
+  int32_t* info_dev = moved_dev + 2 * K + F;
+  // 1. the relinearisation check
+  const bool check = (p->isam_updates + 1) % prm->relinearize_skip == 0;
+  DFK_CUDA(h, launch_window_relinearize(lin_in, lin, p->isam_delta(p->ic), K, F, C, check, prm->relinearize_threshold,
+                                        moved_dev, h->stream),
+           what);
+  h->launches += 1;
+  std::vector<int32_t> moved(2 * K + F, 0);
+  if (check) {
+    DFK_TRY(download(h, sh, moved_dev, sizeof(int32_t) * moved.size(), "[WindowProblem::isam2_update] read-back failed",
+                     "[WindowProblem::isam2_update] kernel failed"));
+    memcpy(moved.data(), sh, sizeof(int32_t) * moved.size());
+  }
+  int num_moved = 0;
+  for (int v : moved) num_moved += v;
+  // 2. the stale items
+  auto pose_moved = [&](int s) { return s >= 0 && moved[s < K ? 2 * s : 2 * K + (s - K)] != 0; };
+  auto code_moved = [&](int c) { return c >= 0 && moved[2 * c + 1] != 0; };
+  auto stale_of = [&](const int4& sl, uint8_t linearised) {
+    return !linearised || pose_moved(sl.x) || pose_moved(sl.y) || code_moved(sl.z) || code_moved(sl.w);
+  };
+  std::vector<uint8_t> sd_dense(nd), sd_sparse(nr + ng + ndpi);
+  for (int i = 0; i < nd; ++i) sd_dense[i] = stale_of(p->slots_tmpl[i], p->lin_dense[i]);
+  for (int j = 0; j < nr; ++j) sd_sparse[j] = stale_of(p->rep_slots_h[j], p->lin_rep[j]);
+  for (int j = 0; j < ng; ++j) sd_sparse[nr + j] = stale_of(p->geo_slots_h[j], p->lin_geo[j]);
+  for (int j = 0; j < ndpi; ++j) sd_sparse[nr + ng + j] = !p->lin_dp[j] || code_moved(p->dp_item_kf[j]);
+  // factors: the window pairs of the stale dense items, the stale links
+  std::vector<int> pairs;
+  for (int i = 0; i < nd; ++i)
+    if (sd_dense[i]) pairs.push_back(p->w->item_pair[i]);
+  std::sort(pairs.begin(), pairs.end());
+  int factors = (int)(std::unique(pairs.begin(), pairs.end()) - pairs.begin());
+  for (int j = 0; j < nr + ng; ++j) factors += sd_sparse[j];
+  // 3. the stale items at theta_lin: the stale active dense items in record order, every slot's record source
+  std::vector<SfmItemDev> items;
+  std::vector<int4> sl;
+  std::vector<int> src(nd);
+  bool scatter = false;
+  for (int i = 0; i < nd; ++i) {
+    if (!p->active[i]) {
+      src[i] = -1;
+      scatter = true;
+    } else if (sd_dense[i]) {
+      src[i] = (int)items.size();
+      items.push_back(p->dense_tmpl[i]);
+      sl.push_back(p->slots_tmpl[i]);
+      scatter = true;
+    } else {
+      src[i] = kKeepRecord;
+    }
+  }
+  const int ns = (int)items.size();
+  if (ns > 0) {
+    plan_tiles(items.data(), ns, p->step.max_ctas, &p->stale_plan);
+    DFK_CUDA(h, cudaMemcpyAsync(p->stale_items.ptr, items.data(), sizeof(SfmItemDev) * ns, cudaMemcpyHostToDevice,
+                                h->stream),
+             umsg);
+    DFK_CUDA(h, cudaMemcpyAsync(p->stale_slots.ptr, sl.data(), sizeof(int4) * ns, cudaMemcpyHostToDevice, h->stream),
+             umsg);
+  }
+  if (scatter)
+    DFK_CUDA(h, cudaMemcpyAsync(p->stale_src.ptr, src.data(), sizeof(int) * nd, cudaMemcpyHostToDevice, h->stream), umsg);
+  if (!sd_sparse.empty())
+    DFK_CUDA(h, cudaMemcpyAsync(p->stale_dev.ptr, sd_sparse.data(), sd_sparse.size(), cudaMemcpyHostToDevice, h->stream),
+             umsg);
+  WindowReposeDev a = repose_args(p, lin);
+  a.dense = p->stale_items.ptr; a.dense_slots = p->stale_slots.ptr; a.num_dense = ns;
+  a.num_error = 0;
+  a.num_depth = 0;
+  DFK_CUDA(h, launch_window_repose(a, h->stream), what);
+  h->launches += 1;
+  if (ns > 0) {
+    DFK_CUDA(h, h->partials_dev.ensure((size_t)p->stale_plan.num_partials * p->step.pfloats), amsg);
+    DFK_TRY(launch_step(h, p->step, C, p->stale_items.ptr, ns, p->stale_plan, h->partials_dev.ptr,
+                        p->stale_records.ptr));
+  }
+  if (scatter) {
+    DFK_CUDA(h, launch_window_scatter_records(p->stale_records.ptr, p->stale_src.ptr, nd, DFK_SFM_RECORD_FLOATS(C),
+                                              p->records, h->stream),
+             what);
+    h->launches += 1;
+  }
+  const float avg = p->avg_dpt;
+  const bool any_rep = std::any_of(sd_sparse.begin(), sd_sparse.begin() + nr, [](uint8_t v) { return v != 0; });
+  const bool any_geo = std::any_of(sd_sparse.begin() + nr, sd_sparse.begin() + nr + ng, [](uint8_t v) { return v != 0; });
+  if (any_rep) {
+    const float2* q = p->rep_st.payload.at(p->rep.ptr);
+    DFK_CUDA(h, launch_reprojection_records(C, p->rep_st.descs.at(p->rep.ptr), nr, q, q + p->rep_st.total, avg,
+                                            p->records + (size_t)nd * DFK_SFM_RECORD_FLOATS(C), h->stream,
+                                            p->stale_dev.ptr),
+             what);
+    h->launches += 1;
+  }
+  if (any_geo) {
+    DFK_CUDA(h, launch_sparse_geometric_records(C, p->geo_st.descs.at(p->geo.ptr), ng, p->geo_st.payload.at(p->geo.ptr),
+                                                avg, p->geo_records, h->stream, p->stale_dev.ptr + nr),
+             what);
+    h->launches += 1;
+  }
+  float* buf = p->bufs.ptr;
+  DFK_TRY(problem_finish(h, p, lin, buf, p->stale_dev.ptr + nr + ng));
+  // 4. diag_eps, fixed by the first update
+  if (p->diag_eps < 0.0) {
+    const size_t o_c = (size_t)K * B * (B + 1);
+    const size_t o_f = o_c + (size_t)p->w->dev.num_pairs * 6 * B + 2 + (size_t)p->w->dev.num_links * B * B;
+    DFK_CUDA(h, launch_window_diag_max(buf, K, F, C, o_c, o_f, p->self_pairs.ptr, p->num_self, prm->code_prior_weight,
+                                       fix != 0, diag_dev, h->stream),
+             what);
+    h->launches += 1;
+    double mx = 0.0;
+    DFK_TRY(download(h, &mx, diag_dev, sizeof(double), "[WindowProblem::isam2_update] read-back failed",
+                     "[WindowProblem::isam2_update] kernel failed"));
+    p->diag_eps = 1e-12 * mx;
+  }
+  // 5. the incremental solve from theta_lin
+  int j0 = 0;
+  DFK_CUDA(h, launch_window_solver_update(p->solver[fix], buf, prm->code_prior_weight, p->diag_eps,
+                                          lin + (size_t)(K + F) * 7, delta, info_dev, h->stream, &h->launches, &j0,
+                                          true),
+           "[WindowProblem::isam2_update] solve failed");
+  int32_t info = 0;
+  DFK_TRY(download(h, sh, info_dev, sizeof(int32_t), "[WindowProblem::isam2_update] read-back failed",
+                   "[WindowProblem::isam2_update] solve failed"));
+  memcpy(&info, sh, sizeof(int32_t));
+  const uint8_t now = info == 0 ? 1 : 0;  // a failed update leaves theta_lin: its records describe no linearisation
+  for (int i = 0; i < nd; ++i)
+    if (sd_dense[i]) p->lin_dense[i] = now;
+  for (int j = 0; j < nr; ++j)
+    if (sd_sparse[j]) p->lin_rep[j] = now;
+  for (int j = 0; j < ng; ++j)
+    if (sd_sparse[nr + j]) p->lin_geo[j] = now;
+  for (int j = 0; j < ndpi; ++j)
+    if (sd_sparse[nr + ng + j]) p->lin_dp[j] = now;
+  if (info != 0)
+    return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem::isam2_update] the window's system at theta_lin is not "
+                                        "positive definite (info " + std::to_string(info) + ")");
+  p->isam_updates += 1;
+  p->ic = nxt;
+  // 6. the estimate theta_lin (+) Delta
+  DFK_CUDA(h, launch_window_retract(lin, p->st(p->cur), delta, K, F, C, h->stream), what);
+  h->launches += 1;
+  res->variables_relinearized = num_moved;
+  res->variables_reeliminated = (K - j0) * B + 6 * F;
+  res->factors_relinearised = factors;
+  res->first_column = j0;
+  return DFK_OK;
+}
+
+// the schedule's pairs and levels of the dense and error items (dfk_window_lm_levels and dfk_window_map_steps)
+DfkStatus schedule_items(DfkHandle h, const DfkWindowProblem* p, const DfkLevelSchedule* sc, const std::string& what,
+                         std::vector<int>& dpair, std::vector<int>& epair, std::vector<int>& elevel)
+{
+  const int nd = p->nd, ne = p->ne, L = sc->num_levels;
+  if (L < 1 || !sc->iters || (nd > 0 && !sc->dense_level) || sc->num_pairs < 0)
+    return fail(h, DFK_ERR_INVALID_ARG, what + "num_levels < 1, or null iters / dense_level");
+  if (ne > 0 && ne != nd && (!sc->error_pair || !sc->error_level))
+    return fail(h, DFK_ERR_INVALID_ARG, what + "error_pair and error_level are required when num_error != num_dense");
+  for (int l = 0; l < L; ++l)
+    if (sc->iters[l] < 0) return fail(h, DFK_ERR_INVALID_ARG, what + "iters[" + std::to_string(l) + "] < 0");
+  // the schedule's pairs: the distinct window pairs of the dense items, in window order
+  std::vector<int> ids;
+  dpair.assign(nd, 0);
+  for (int i = 0; i < nd; ++i) ids.push_back(p->w->item_pair[i]);
+  std::sort(ids.begin(), ids.end());
+  ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
+  if ((int)ids.size() != sc->num_pairs)
+    return fail(h, DFK_ERR_INVALID_ARG, what + "num_pairs " + std::to_string(sc->num_pairs) + ", but the dense items" +
+                                            " cover " + std::to_string(ids.size()) + " pairs");
+  for (int i = 0; i < nd; ++i)
+    dpair[i] = (int)(std::lower_bound(ids.begin(), ids.end(), p->w->item_pair[i]) - ids.begin());
+  for (int i = 0; i < nd; ++i)
+    if (sc->dense_level[i] < 0 || sc->dense_level[i] >= L)
+      return fail(h, DFK_ERR_INVALID_ARG, what + "dense item " + std::to_string(i) + ": level outside [0, num_levels)");
+  epair.assign(ne, 0);
+  elevel.assign(ne, 0);
+  for (int i = 0; i < ne; ++i) {
+    epair[i] = sc->error_pair ? sc->error_pair[i] : dpair[i];
+    elevel[i] = sc->error_level ? sc->error_level[i] : sc->dense_level[i];
+    if (epair[i] < 0 || epair[i] >= sc->num_pairs || elevel[i] < 0 || elevel[i] >= L)
+      return fail(h, DFK_ERR_INVALID_ARG, what + "error item " + std::to_string(i) + ": pair or level out of range");
+  }
   return DFK_OK;
 }
 
@@ -1257,6 +1569,12 @@ DfkStatus dfk_window_problem_create(DfkHandle h, const DfkWindowProblemDesc* d, 
     put_slots(p->depth_slots, d->depth_slots, ndep);
     p->slots_tmpl.assign(p->dense_slots.at(hb), p->dense_slots.at(hb) + nd);
     p->slots_tmpl.insert(p->slots_tmpl.end(), p->err_slots.at(hb), p->err_slots.at(hb) + ne);
+    for (int j = 0; j < nr; ++j) p->rep_size_h.push_back(d->reproj[j].num_matches);
+    for (int j = 0; j < ng; ++j) p->geo_size_h.push_back(d->geo[j].num_points);
+    p->rep_slots_h.assign(p->rep_slots.at(hb), p->rep_slots.at(hb) + nr);
+    p->geo_slots_h.assign(p->geo_slots.at(hb), p->geo_slots.at(hb) + ng);
+    p->lin_dense.assign(nd, 0); p->lin_rep.assign(nr, 0); p->lin_geo.assign(ng, 0);
+    p->active.assign(nd, 1);
     // ---- priors: rows, add_priors' lists, the keyframe of every delta row and the frozen points (frame priors, then
     // keyframe-prior members)
     if (mf > 0) {
@@ -1310,6 +1628,7 @@ DfkStatus dfk_window_problem_set_state(DfkHandle h, DfkWindowProblem* p, const d
     if (p->K * p->C > 0)
       DFK_CUDA(h, cudaMemcpyAsync(p->st(p->cur) + np, codes, sizeof(double) * (p->S - np), cudaMemcpyDefault, h->stream),
                "[WindowProblem] state copy failed");
+    p->isam_fresh = true;
     return DFK_OK;
   });
 }
@@ -1397,6 +1716,8 @@ DfkStatus dfk_window_problem_set_depth_priors(DfkHandle h, DfkWindowProblem* p, 
     DeviceGuard guard(h->device);
     if (m == 0) {
       p->ndp = p->ndpi = 0;
+      p->dp_item_kf.clear();
+      p->lin_dp.clear();
       return DFK_OK;
     }
     const int n = level_ptr[m];
@@ -1425,6 +1746,8 @@ DfkStatus dfk_window_problem_set_depth_priors(DfkHandle h, DfkWindowProblem* p, 
     p->dp_level_ptr = lp;
     p->dp_sigma = sg;
     p->dp_kf = kf;
+    p->dp_item_kf.assign(kf.at(s.host()), kf.at(s.host()) + n);
+    p->lin_dp.assign(n, 0);
     return DFK_OK;
   });
 }
@@ -1475,35 +1798,10 @@ DfkStatus dfk_window_lm_levels(DfkHandle h, DfkWindowProblem* p, const DfkLMPara
   return guarded(h, [&] {
     const std::string what = "[WindowLMLevels] ";
     if (!p || !sc) return fail(h, DFK_ERR_INVALID_ARG, what + "null argument");
-    const int nd = p->nd, ne = p->ne, L = sc->num_levels;
-    if (L < 1 || !sc->iters || (nd > 0 && !sc->dense_level) || sc->num_pairs < 0 ||
-        (sc->num_pairs > 0 && !sc->pair_steps_done))
-      return fail(h, DFK_ERR_INVALID_ARG, what + "num_levels < 1, or null iters / dense_level / pair_steps_done");
-    if (ne > 0 && ne != nd && (!sc->error_pair || !sc->error_level))
-      return fail(h, DFK_ERR_INVALID_ARG, what + "error_pair and error_level are required when num_error != num_dense");
-    for (int l = 0; l < L; ++l)
-      if (sc->iters[l] < 0) return fail(h, DFK_ERR_INVALID_ARG, what + "iters[" + std::to_string(l) + "] < 0");
-    // the schedule's pairs: the distinct window pairs of the dense items, in window order
-    std::vector<int> dpair(nd), ids;
-    for (int i = 0; i < nd; ++i) ids.push_back(p->w->item_pair[i]);
-    std::sort(ids.begin(), ids.end());
-    ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
-    if ((int)ids.size() != sc->num_pairs)
-      return fail(h, DFK_ERR_INVALID_ARG, what + "num_pairs " + std::to_string(sc->num_pairs) + ", but the dense items" +
-                                              " cover " + std::to_string(ids.size()) + " pairs");
-    for (int i = 0; i < nd; ++i)
-      dpair[i] = (int)(std::lower_bound(ids.begin(), ids.end(), p->w->item_pair[i]) - ids.begin());
-    for (int i = 0; i < nd; ++i)
-      if (sc->dense_level[i] < 0 || sc->dense_level[i] >= L)
-        return fail(h, DFK_ERR_INVALID_ARG, what + "dense item " + std::to_string(i) + ": level outside [0, num_levels)");
-    std::vector<int> epair(ne), elevel(ne);
-    for (int i = 0; i < ne; ++i) {
-      epair[i] = sc->error_pair ? sc->error_pair[i] : dpair[i];
-      elevel[i] = sc->error_level ? sc->error_level[i] : sc->dense_level[i];
-      if (epair[i] < 0 || epair[i] >= sc->num_pairs || elevel[i] < 0 || elevel[i] >= L)
-        return fail(h, DFK_ERR_INVALID_ARG, what + "error item " + std::to_string(i) +
-                                                ": pair or level out of range");
-    }
+    if (sc->num_pairs > 0 && !sc->pair_steps_done) return fail(h, DFK_ERR_INVALID_ARG, what + "null pair_steps_done");
+    const int nd = p->nd, ne = p->ne;
+    std::vector<int> dpair, epair, elevel;
+    DFK_TRY(schedule_items(h, p, sc, what, dpair, epair, elevel));
     for (int q = 0; q < sc->num_pairs; ++q)
       if (sc->pair_steps_done[q] < 0)
         return fail(h, DFK_ERR_INVALID_ARG, what + "pair_steps_done[" + std::to_string(q) + "] < 0");
@@ -1529,6 +1827,268 @@ DfkStatus dfk_window_lm_levels(DfkHandle h, DfkWindowProblem* p, const DfkLMPara
     ops.dm.assign(nd, 1);
     ops.em.assign(ne, 1);
     return lm_levels_run(*prm, *sc, ops, tr, lt);
+  });
+}
+
+DfkStatus dfk_window_problem_isam2_update(DfkHandle h, DfkWindowProblem* p, const DfkIsam2Params* prm,
+                                          DfkIsam2Result* res)
+{
+  return guarded(h, [&] {
+    const std::string what = "[WindowProblem::isam2_update] ";
+    DFK_TRY(isam2_check(h, p, prm, what));
+    if (!res) return fail(h, DFK_ERR_INVALID_ARG, what + "null argument");
+    DeviceGuard guard(h->device);
+    return problem_isam2_update(h, p, prm, res);
+  });
+}
+
+DfkStatus dfk_window_problem_get_linearization(DfkHandle h, const DfkWindowProblem* p, double* lin_poses,
+                                               double* lin_codes, double* delta)
+{
+  return guarded(h, [&] {
+    const char* what = "[WindowProblem::get_linearization] copy failed";
+    if (!p) return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem::get_linearization] null argument");
+    if (p->device != h->device)
+      return fail(h, DFK_ERR_INVALID_ARG, "[WindowProblem] problem and handle live on different devices");
+    DeviceGuard guard(h->device);
+    const size_t np = (size_t)(p->K + p->F) * 7;
+    if (p->isam_fresh) {  // no update since create / set_state: the state, and zeros
+      if (delta) {
+        cudaPointerAttributes at{};
+        DFK_CUDA(h, cudaPointerGetAttributes(&at, delta), what);
+        if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) {
+          DFK_CUDA(h, cudaMemsetAsync(delta, 0, sizeof(double) * p->delta_size(), h->stream), what);
+        } else {
+          DFK_CUDA(h, cudaStreamSynchronize(h->stream), what);  // after any copy still writing it
+          std::fill(delta, delta + p->delta_size(), 0.0);
+        }
+      }
+      const double* st = p->st(p->cur);
+      if (lin_poses) DFK_CUDA(h, cudaMemcpyAsync(lin_poses, st, sizeof(double) * np, cudaMemcpyDefault, h->stream), what);
+      if (lin_codes && p->K * p->C > 0)
+        DFK_CUDA(h, cudaMemcpyAsync(lin_codes, st + np, sizeof(double) * (p->S - np), cudaMemcpyDefault, h->stream),
+                 what);
+      return DFK_OK;
+    }
+    const double* lin = p->lin(p->ic);
+    if (lin_poses)
+      DFK_CUDA(h, cudaMemcpyAsync(lin_poses, lin, sizeof(double) * np, cudaMemcpyDefault, h->stream), what);
+    if (lin_codes && p->K * p->C > 0)
+      DFK_CUDA(h, cudaMemcpyAsync(lin_codes, lin + np, sizeof(double) * (p->S - np), cudaMemcpyDefault, h->stream), what);
+    if (delta)
+      DFK_CUDA(h, cudaMemcpyAsync(delta, p->isam_delta(p->ic), sizeof(double) * p->delta_size(), cudaMemcpyDefault,
+                                  h->stream),
+               what);
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_problem_grow_from(DfkHandle h, DfkWindowProblem* pn, const DfkWindowProblem* po,
+                                       const int32_t* dense_of, const int32_t* rep_of, const int32_t* geo_of,
+                                       const int32_t* frame_of)
+{
+  return guarded(h, [&] {
+    const std::string what = "[WindowProblem::grow_from] ";
+    auto bad = [&](const std::string& m) { return fail(h, DFK_ERR_INVALID_ARG, what + m); };
+    if (!pn || !po || pn == po) return bad("null argument, or the same problem twice");
+    if ((pn->nd && !dense_of) || (pn->nr && !rep_of) || (pn->ng && !geo_of) || (pn->F && !frame_of))
+      return bad("null map");
+    if (pn->device != h->device || po->device != h->device)
+      return bad("problems and handle live on different devices");
+    if (po->isam_fresh) return bad("the old problem has no ISAM2 run to carry over");
+    const int K0 = po->K, F0 = po->F, K = pn->K, F = pn->F, C = pn->C, B = pn->B;
+    if (pn->C != po->C || K < K0)
+      return bad("the new window must keep the old keyframes first, with the same code size");
+    // frames: distinct old frames
+    std::vector<char> used(F0, 0);
+    for (int f = 0; f < F; ++f) {
+      const int o = frame_of[f];
+      if (o < -1 || o >= F0 || (o >= 0 && used[o]++)) return bad("frame_of[" + std::to_string(f) + "] is not a distinct old frame or -1");
+    }
+    // a new slot in terms of the old problem's slots: keyframes keep their index, a frame maps by frame_of, a new
+    // keyframe or frame has no old slot
+    auto pose_old = [&](int s) { return s < 0 ? -1 : s < K ? (s < K0 ? s : -2) : (frame_of[s - K] >= 0 ? K0 + frame_of[s - K] : -2); };
+    auto code_old = [&](int c) { return c < 0 ? -1 : c < K0 ? c : -2; };
+    auto same = [&](const int4& a, const int4& b) {
+      return pose_old(a.x) == b.x && pose_old(a.y) == b.y && code_old(a.z) == b.z && code_old(a.w) == b.w;
+    };
+    struct Kind {
+      const char* name;
+      const int32_t* of;
+      int n, n_old;
+    };
+    const Kind kinds[3] = {{"dense", dense_of, pn->nd, po->nd}, {"reprojection", rep_of, pn->nr, po->nr},
+                           {"geometric", geo_of, pn->ng, po->ng}};
+    std::vector<int2> rec_map, geo_map;
+    for (int k = 0; k < 3; ++k) {
+      std::vector<char> seen(kinds[k].n_old, 0);
+      for (int i = 0; i < kinds[k].n; ++i) {
+        const int o = kinds[k].of[i];
+        const std::string it = std::string(kinds[k].name) + " item " + std::to_string(i);
+        if (o == -1) continue;
+        if (o < 0 || o >= kinds[k].n_old || seen[o]++) return bad(it + ": not a distinct old item or -1");
+        bool ok;
+        if (k == 0) {
+          const SfmItemDev &a = pn->dense_tmpl[i], &b = po->dense_tmpl[o];
+          ok = same(pn->slots_tmpl[i], po->slots_tmpl[o]) && a.width == b.width && a.height == b.height &&
+               a.fx == b.fx && a.fy == b.fy && a.u0 == b.u0 && a.v0 == b.v0;
+          rec_map.push_back(make_int2(i, o));
+        } else if (k == 1) {
+          ok = same(pn->rep_slots_h[i], po->rep_slots_h[o]) && pn->rep_size_h[i] == po->rep_size_h[o];
+          rec_map.push_back(make_int2(pn->nd + i, po->nd + o));
+        } else {
+          ok = same(pn->geo_slots_h[i], po->geo_slots_h[o]) && pn->geo_size_h[i] == po->geo_size_h[o];
+          geo_map.push_back(make_int2(i, o));
+        }
+        if (!ok) return bad(it + " does not read its old item's keys, or has another level or size");
+      }
+    }
+    DeviceGuard guard(h->device);
+    const char* amsg = "[WindowProblem::grow_from] allocation failed";
+    // the solvers, grown from the old ones (dfk_window_solver_create_from's checks), before anything is written
+    WindowSolverDev* grown[2] = {nullptr, nullptr};
+    auto drop = [&] { window_solver_destroy(grown[0]); window_solver_destroy(grown[1]); };
+    for (int fix = 0; fix < 2; ++fix) {
+      if (!po->solver[fix]) continue;
+      const std::vector<int> fixed = fix ? std::vector<int>{0, 1, 2, 3, 4, 5} : std::vector<int>();
+      const cudaError_t e = window_solver_create(K, C, F, pn->w->pair_k0, pn->w->pair_k1, pn->w->link_k0,
+                                                 pn->w->link_k1, pn->w->blk_i, pn->w->blk_j, pn->w->kp.block_off,
+                                                 fixed, &grown[fix]);
+      if (e != cudaSuccess) {
+        drop();
+        return cuda_fail(h, e, amsg);
+      }
+      if (!window_solver_extends(po->solver[fix], grown[fix])) {
+        drop();
+        return bad("the new window does not extend the old one's solver (keyframes, code size or fixed variables)");
+      }
+    }
+    // the ISAM2 buffers of the new problem; its run continues the old one's
+    pn->isam_fresh = false;
+    DfkStatus st = isam2_setup(h, pn, 1, amsg);
+    if (st == DFK_OK) {
+      const cudaError_t e = pn->gather.ensure(std::max<size_t>(1, rec_map.size() + geo_map.size()));
+      if (e != cudaSuccess) st = cuda_fail(h, e, amsg);
+    }
+    if (st != DFK_OK) {
+      pn->isam_fresh = true;
+      drop();
+      return st;
+    }
+    for (int fix = 0; fix < 2; ++fix)
+      if (grown[fix]) {
+        int cols = 0;
+        DFK_CUDA(h, window_solver_adopt(grown[fix], po->solver[fix], h->stream, &cols), amsg);
+        window_solver_destroy(pn->solver[fix]);
+        pn->solver[fix] = grown[fix];
+        grown[fix] = nullptr;
+      }
+    const char* cmsg = "[WindowProblem::grow_from] copy failed";
+    // the kept records, one gather launch per record buffer
+    std::vector<int2> maps(rec_map);
+    maps.insert(maps.end(), geo_map.begin(), geo_map.end());
+    if (!maps.empty()) {
+      DFK_CUDA(h, cudaMemcpyAsync(pn->gather.ptr, maps.data(), sizeof(int2) * maps.size(), cudaMemcpyHostToDevice,
+                                  h->stream),
+               cmsg);
+      if (!rec_map.empty()) {
+        DFK_CUDA(h, launch_window_gather_records(po->records, pn->records, pn->gather.ptr, (int)rec_map.size(),
+                                                 DFK_SFM_RECORD_FLOATS(C), h->stream),
+                 cmsg);
+        h->launches += 1;
+      }
+      if (!geo_map.empty()) {
+        DFK_CUDA(h, launch_window_gather_records(po->geo_records, pn->geo_records, pn->gather.ptr + rec_map.size(),
+                                                 (int)geo_map.size(), DFK_GEO_RECORD_FLOATS(C), h->stream),
+                 cmsg);
+        h->launches += 1;
+      }
+    }
+    // theta_lin and Delta: the old keyframes' and kept frames' from the old run, the new ones' from the new state
+    const double *ol = po->lin(po->ic), *od = po->isam_delta(po->ic), *ns = pn->st(pn->cur);
+    double *nl = pn->lin(pn->ic), *nd = pn->isam_delta(pn->ic);
+    auto d2d = [&](double* dst, const double* src, size_t n) {
+      return n ? cudaMemcpyAsync(dst, src, sizeof(double) * n, cudaMemcpyDeviceToDevice, h->stream) : cudaSuccess;
+    };
+    const size_t npn = (size_t)(K + F) * 7, npo = (size_t)(K0 + F0) * 7;
+    DFK_CUDA(h, d2d(nl, ns, pn->S), cmsg);                                    // everything new from the state
+    DFK_CUDA(h, d2d(nl, ol, (size_t)K0 * 7), cmsg);                          // old keyframe poses
+    DFK_CUDA(h, d2d(nl + npn, ol + npo, (size_t)K0 * C), cmsg);              // old codes
+    DFK_CUDA(h, cudaMemsetAsync(nd, 0, sizeof(double) * pn->delta_size(), h->stream), cmsg);
+    DFK_CUDA(h, d2d(nd, od, (size_t)K0 * B), cmsg);                          // old keyframes' delta
+    for (int f = 0; f < F; ++f)
+      if (frame_of[f] >= 0) {
+        DFK_CUDA(h, d2d(nl + (size_t)(K + f) * 7, ol + (size_t)(K0 + frame_of[f]) * 7, 7), cmsg);
+        DFK_CUDA(h, d2d(nd + (size_t)K * B + 6 * f, od + (size_t)K0 * B + 6 * frame_of[f], 6), cmsg);
+      }
+    // the flags: kept items as they were, new items and the depth priors stale
+    pn->clear_linearised();
+    for (const int2& m : rec_map) {
+      if (m.x < pn->nd) pn->lin_dense[m.x] = po->lin_dense[m.y];
+      else pn->lin_rep[m.x - pn->nd] = po->lin_rep[m.y - po->nd];
+    }
+    for (const int2& m : geo_map) pn->lin_geo[m.x] = po->lin_geo[m.y];
+    pn->isam_updates = po->isam_updates;
+    pn->diag_eps = po->diag_eps;
+    return DFK_OK;
+  });
+}
+
+DfkStatus dfk_window_map_steps(DfkHandle h, DfkWindowProblem* p, const DfkIsam2Params* prm, const DfkLevelSchedule* sc,
+                               DfkWorkState* works, int max_steps, DfkMapTrace* tr)
+{
+  return guarded(h, [&] {
+    const std::string what = "[WindowMapSteps] ";
+    DFK_TRY(isam2_check(h, p, prm, what));
+    if (!sc) return fail(h, DFK_ERR_INVALID_ARG, what + "null argument");
+    if (max_steps < 0) return fail(h, DFK_ERR_INVALID_ARG, what + "max_steps < 0");
+    const int L = sc->num_levels, P = sc->num_pairs, nd = p->nd, ne = p->ne;
+    if (L > DFK_MAX_WORK_LEVELS)
+      return fail(h, DFK_ERR_INVALID_ARG, what + "more than DFK_MAX_WORK_LEVELS (" + std::to_string(DFK_MAX_WORK_LEVELS) +
+                                              ") levels");
+    std::vector<int> dpair, epair, elevel;
+    DFK_TRY(schedule_items(h, p, sc, what, dpair, epair, elevel));
+    std::vector<DfkWorkState> wk(P);
+    for (int q = 0; q < P; ++q) {
+      wk[q] = works ? works[q] : work_fresh(sc->iters, L);
+      const DfkWorkState& w = wk[q];
+      bool ok = w.active_level >= -2 && w.active_level < L && w.factor >= -1 && w.factor < L;
+      for (int l = 0; l < L; ++l) ok = ok && w.iters[l] >= -1 && w.iters[l] <= sc->iters[l];
+      if (!ok) return fail(h, DFK_ERR_INVALID_ARG, what + "work " + std::to_string(q) + " is not a state of its schedule");
+    }
+    DeviceGuard guard(h->device);
+    std::vector<int> factor(P), prev(P);
+    std::vector<uint8_t> dm(nd), em(ne);
+    int step = 0;
+    for (; step < max_steps && !works_empty(wk.data(), P); ++step) {
+      for (int q = 0; q < P; ++q) prev[q] = wk[q].factor;
+      works_step(wk.data(), P, sc->iters, sc->pair_remove_after, factor.data());
+      for (int i = 0; i < nd; ++i) dm[i] = factor[dpair[i]] == sc->dense_level[i];
+      for (int i = 0; i < ne; ++i) em[i] = factor[epair[i]] == elevel[i];
+      DFK_TRY(problem_set_active(h, p, dm.data(), em.data()));
+      // a pair whose factor changed holds a new factor: linearised at theta_lin.  Flags exist once an update ran
+      if (!p->isam_fresh)
+        for (int i = 0; i < nd; ++i)
+          if (factor[dpair[i]] != prev[dpair[i]]) p->lin_dense[i] = 0;
+      DfkIsam2Result r{};
+      const DfkStatus st = problem_isam2_update(h, p, prm, &r);
+      if (st != DFK_OK) {  // the steps before this one stand: hand back their works, so the run can continue
+        if (tr) tr->num_steps = step;
+        if (works) std::copy(wk.begin(), wk.end(), works);
+        return st;
+      }
+      if (tr) {
+        if (tr->variables_relinearized) tr->variables_relinearized[step] = r.variables_relinearized;
+        if (tr->variables_reeliminated) tr->variables_reeliminated[step] = r.variables_reeliminated;
+        if (tr->factors_relinearised) tr->factors_relinearised[step] = r.factors_relinearised;
+        if (tr->first_column) tr->first_column[step] = r.first_column;
+        if (tr->pair_levels) std::copy(factor.begin(), factor.end(), tr->pair_levels + (size_t)step * P);
+      }
+      if (r.variables_relinearized == 0) works_signal(wk.data(), P);
+    }
+    if (tr) tr->num_steps = step;
+    if (works) std::copy(wk.begin(), wk.end(), works);
+    return DFK_OK;
   });
 }
 

@@ -56,8 +56,10 @@ __device__ __forceinline__ void stage_chunk(const DepthPriorDesc& d, const float
 // Block (x, i): partial row x of item i.  kGram: the packed upper augmented Gram (NE floats), else diff^2 (1 float).
 template <int C, bool kGram>
 __global__ void __launch_bounds__(kThreads)
-depth_prior_partial_kernel(const DepthPriorDesc* __restrict__ descs, float avg_dpt, float* __restrict__ partials)
+depth_prior_partial_kernel(const DepthPriorDesc* __restrict__ descs, float avg_dpt, float* __restrict__ partials,
+                           const uint8_t* __restrict__ stale)
 {
+  if (stale && !stale[blockIdx.y]) return;  // an item that is not stale keeps its record
   constexpr int NA = C + 1;                 // augmented row: s*jc | diff
   constexpr int NE = NA * (NA + 1) / 2;     // packed upper triangle of the augmented Gram
   constexpr int EPT = (NE + kThreads - 1) / kThreads;
@@ -128,8 +130,9 @@ depth_prior_partial_kernel(const DepthPriorDesc* __restrict__ descs, float avg_d
 template <int C, bool kGram>
 __global__ void __launch_bounds__(kThreads)
 depth_prior_finalize_kernel(const DepthPriorDesc* __restrict__ descs, const float* __restrict__ partials,
-                            float* __restrict__ out)
+                            float* __restrict__ out, const uint8_t* __restrict__ stale)
 {
+  if (stale && !stale[blockIdx.x]) return;
   constexpr int NA = C + 1;
   constexpr int NE = NA * (NA + 1) / 2;
   constexpr int NH = C * (C + 1) / 2;
@@ -161,15 +164,15 @@ depth_prior_finalize_kernel(const DepthPriorDesc* __restrict__ descs, const floa
 
 template <int C>
 cudaError_t launch(const DepthPriorDesc* descs_dev, int n, int max_parts, float avg_dpt, float* partials, float* out,
-                   bool gram, cudaStream_t s)
+                   bool gram, cudaStream_t s, const uint8_t* stale)
 {
   const dim3 grid((unsigned)max_parts, (unsigned)n);
   if (gram) {
-    depth_prior_partial_kernel<C, true><<<grid, kThreads, 0, s>>>(descs_dev, avg_dpt, partials);
-    depth_prior_finalize_kernel<C, true><<<n, kThreads, 0, s>>>(descs_dev, partials, out);
+    depth_prior_partial_kernel<C, true><<<grid, kThreads, 0, s>>>(descs_dev, avg_dpt, partials, stale);
+    depth_prior_finalize_kernel<C, true><<<n, kThreads, 0, s>>>(descs_dev, partials, out, stale);
   } else {
-    depth_prior_partial_kernel<C, false><<<grid, kThreads, 0, s>>>(descs_dev, avg_dpt, partials);
-    depth_prior_finalize_kernel<C, false><<<n, kThreads, 0, s>>>(descs_dev, partials, out);
+    depth_prior_partial_kernel<C, false><<<grid, kThreads, 0, s>>>(descs_dev, avg_dpt, partials, stale);
+    depth_prior_finalize_kernel<C, false><<<n, kThreads, 0, s>>>(descs_dev, partials, out, stale);
   }
   return cudaGetLastError();
 }
@@ -261,14 +264,14 @@ size_t depth_prior_partial_floats(int code_size, bool gram)
 }
 
 cudaError_t launch_depth_prior_batch(int code_size, const DepthPriorDesc* descs_dev, int n, int max_parts, float avg_dpt,
-                                     float* partials, float* out_dev, bool gram, cudaStream_t s)
+                                     float* partials, float* out_dev, bool gram, cudaStream_t s, const uint8_t* stale)
 {
   switch (code_size) {
-    case 8: return launch<8>(descs_dev, n, max_parts, avg_dpt, partials, out_dev, gram, s);
-    case 16: return launch<16>(descs_dev, n, max_parts, avg_dpt, partials, out_dev, gram, s);
-    case 32: return launch<32>(descs_dev, n, max_parts, avg_dpt, partials, out_dev, gram, s);
-    case 64: return launch<64>(descs_dev, n, max_parts, avg_dpt, partials, out_dev, gram, s);
-    case 128: return launch<128>(descs_dev, n, max_parts, avg_dpt, partials, out_dev, gram, s);
+    case 8: return launch<8>(descs_dev, n, max_parts, avg_dpt, partials, out_dev, gram, s, stale);
+    case 16: return launch<16>(descs_dev, n, max_parts, avg_dpt, partials, out_dev, gram, s, stale);
+    case 32: return launch<32>(descs_dev, n, max_parts, avg_dpt, partials, out_dev, gram, s, stale);
+    case 64: return launch<64>(descs_dev, n, max_parts, avg_dpt, partials, out_dev, gram, s, stale);
+    case 128: return launch<128>(descs_dev, n, max_parts, avg_dpt, partials, out_dev, gram, s, stale);
     default: return cudaErrorInvalidValue;
   }
 }

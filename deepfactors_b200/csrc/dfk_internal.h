@@ -331,7 +331,8 @@ cudaError_t launch_window_solve(const WindowSolverDev* s, const float* window_de
 // workspace.
 cudaError_t launch_window_solver_update(WindowSolverDev* s, const float* window_dev, double prior, double diag_eps,
                                         const double* codes_host, double* dx_dev, int32_t* info_dev,
-                                        cudaStream_t stream, uint64_t* launches, int* first_column);
+                                        cudaStream_t stream, uint64_t* launches, int* first_column,
+                                        bool codes_on_device = false);
 // growth (dfk_window_solver_create_from): whether s's window can extend prev's (same code size, at least as many
 // keyframes, the same fixed variables among prev's), and s taking over prev's longest prefix of columns with the same
 // tile pattern (bounded by what prev holds from its last update): factor, stored loaded system and forward pass,
@@ -365,9 +366,11 @@ int depth_prior_parts(int width, int height);
 // floats per partial row: the augmented Gram (gram) or diff^2 alone
 size_t depth_prior_partial_floats(int code_size, bool gram);
 // gram: n records of DFK_DEPTH_RECORD_FLOATS(code_size) into out_dev; else n rows [residual | inliers (u32 bits)].  Two
-// launches: the partial rows (grid max_parts x n), then one block per item sums them in partial order.
+// launches: the partial rows (grid max_parts x n), then one block per item sums them in partial order.  stale (device,
+// n bytes, optional): the CTAs of an item whose byte is 0 return at once, so its output row is left as it was.
 cudaError_t launch_depth_prior_batch(int code_size, const DepthPriorDesc* descs_dev, int n, int max_parts, float avg_dpt,
-                                     float* partials, float* out_dev, bool gram, cudaStream_t s);
+                                     float* partials, float* out_dev, bool gram, cudaStream_t s,
+                                     const uint8_t* stale = nullptr);
 // m depth priors (kf_ptr[K+1] / kf_priors: the CSR of prior indices per keyframe, in list order; level_ptr[m+1]: the
 // records of each prior; sigma[m]) into an assembled window buffer, in place
 // the codes of n depth-prior items from the state's codes (K x C doubles): item i reads keyframe item_kf[i], rounded to
@@ -399,9 +402,12 @@ struct ReprojItemDev {
 // rows_dev: 2 num_matches rows of 13 + code_size floats; err2_dev: num_matches squared errors
 cudaError_t launch_reprojection_rows(int code_size, const ReprojItemDev& item, const float2* query_dev,
                                      const float2* train_dev, float avg_dpt, float* rows_dev, float* err2_dev, cudaStream_t s);
-// one CTA per item; records_dev: num_items records of DFK_SFM_RECORD_FLOATS(code_size) floats
+// one CTA per item; records_dev: num_items records of DFK_SFM_RECORD_FLOATS(code_size) floats.  stale (device,
+// num_items bytes, optional): an item whose byte is 0 keeps its record (its CTAs return before they write), as in
+// launch_sparse_geometric_records
 cudaError_t launch_reprojection_records(int code_size, const ReprojItemDev* items_dev, int num_items, const float2* query_dev,
-                                        const float2* train_dev, float avg_dpt, float* records_dev, cudaStream_t s);
+                                        const float2* train_dev, float avg_dpt, float* records_dev, cudaStream_t s,
+                                        const uint8_t* stale = nullptr);
 
 // One SparseGeometricFactor.  Its points are points[point_begin, + num_points); code0 / code1 point at its code_size
 // floats each in device scratch.
@@ -420,7 +426,8 @@ cudaError_t launch_sparse_geometric_rows(int code_size, const GeoItemDev& item, 
                                          float* rows_dev, cudaStream_t s);
 // grid (num_items, 1 or 4 entry slices); records_dev: num_items records of DFK_GEO_RECORD_FLOATS(code_size) floats
 cudaError_t launch_sparse_geometric_records(int code_size, const GeoItemDev* items_dev, int num_items, const int2* points_dev,
-                                            float avg_dpt, float* records_dev, cudaStream_t s);
+                                            float avg_dpt, float* records_dev, cudaStream_t s,
+                                            const uint8_t* stale = nullptr);
 // error() of a batch: one CTA per item; out_dev: num_items x [b^T b | valid matches / points (u32 bits)], b^T b bit for
 // bit the residual of the item's record from launch_reprojection_records / launch_sparse_geometric_records
 cudaError_t launch_reprojection_error(int code_size, const ReprojItemDev* items_dev, int num_items, const float2* query_dev,
@@ -474,9 +481,27 @@ struct WindowEnergyDev {
   double* out;  // [E | photometric | reprojection | geometric | priors | items without inliers | inliers | E + code prior]
 };
 cudaError_t launch_window_energy(const WindowEnergyDev& a, cudaStream_t stream);
-// records slot i (i < n, rf floats each) <- sub record src[i], or zeros where src[i] < 0 (an inactive item)
+// records slot i (i < n, rf floats each) <- sub record src[i]; zeros where src[i] == -1 (an inactive item); left as
+// it is where src[i] == kKeepRecord (an active item whose record is still valid: ISAM2's partial linearisation)
+constexpr int kKeepRecord = -2;
 cudaError_t launch_window_scatter_records(const float* sub, const int* src, int n, int rf, float* records,
                                           cudaStream_t stream);
+// dst record map[i].x <- src record map[i].y (rf floats each), one CTA per entry (dfk_window_problem_grow_from)
+cudaError_t launch_window_gather_records(const float* src, float* dst, const int2* map, int n, int rf,
+                                         cudaStream_t stream);
+// ISAM2's relinearisation check (dfk_window_problem_isam2_update), one CTA per key -- pose k is key 2 k, code k key
+// 2 k + 1, frame f key 2 K + f: lin_out = lin_in, except that with `check` a key whose delta (the solve's layout)
+// has max |delta_key| >= threshold (a NaN never does) moves to lin_in (+) delta_key (the retraction of
+// launch_window_retract, codes by addition); moved[key] = 1 for those keys, else 0
+cudaError_t launch_window_relinearize(const double* lin_in, double* lin_out, const double* delta, int K, int F, int C,
+                                      bool check, double threshold, int32_t* moved, cudaStream_t stream);
+// max |d| over the kept variables of the diagonal of a window buffer's dense system (WindowBlocks.to_dense: the
+// keyframe blocks, each self pair's (k, k) coupling block added twice in pair order, the frame blocks) plus w on every
+// code entry, in fp64; variables 0..5 are skipped when fix_first_pose.  self_pairs: num_self (pair, keyframe) int2.
+// One CTA, into *out
+cudaError_t launch_window_diag_max(const float* buf, int K, int F, int C, size_t coupling_off, size_t frame_off,
+                                   const int2* self_pairs, int num_self, double w, bool fix_first_pose, double* out,
+                                   cudaStream_t stream);
 
 // one factor of dfk_hamming_match_batch / dfk_reprojection_match_batch (dfk_match.cu)
 struct MatchItemDev {

@@ -231,8 +231,10 @@ __device__ __forceinline__ void gram_records(int M, float* __restrict__ records,
 template <int C>
 __global__ void __launch_bounds__(RepCfg<C>::NT)
 reprojection_records_kernel(const ReprojItemDev* __restrict__ items, const float2* __restrict__ query,
-                            const float2* __restrict__ train, float avg_dpt, float* __restrict__ records)
+                            const float2* __restrict__ train, float avg_dpt, float* __restrict__ records,
+                            const uint8_t* __restrict__ stale)
 {
+  if (stale && !stale[blockIdx.x]) return;  // a factor that is not stale keeps its record
   __shared__ ReprojItemDev it;
   load_item<RepCfg<C>::NT>(items + blockIdx.x, it);
   gram_records<RepCfg<C>>(it.num_matches, records, [&](int m, float* r0) {
@@ -356,8 +358,9 @@ sparse_geometric_rows_kernel(const __grid_constant__ GeoItemDev it, const int2* 
 template <int C>
 __global__ void __launch_bounds__(GeoCfg<C>::NT)
 sparse_geometric_records_kernel(const GeoItemDev* __restrict__ items, const int2* __restrict__ points, float avg_dpt,
-                                float* __restrict__ records)
+                                float* __restrict__ records, const uint8_t* __restrict__ stale)
 {
+  if (stale && !stale[blockIdx.x]) return;  // a factor that is not stale keeps its record
   __shared__ GeoItemDev it;
   load_item<GeoCfg<C>::NT>(items + blockIdx.x, it);
   gram_records<GeoCfg<C>>(it.num_points, records, [&](int m, float* r) {
@@ -466,7 +469,8 @@ cudaError_t launch_reprojection_rows(int code_size, const ReprojItemDev& item, c
 }
 
 cudaError_t launch_reprojection_records(int code_size, const ReprojItemDev* items_dev, int num_items, const float2* query_dev,
-                                        const float2* train_dev, float avg_dpt, float* records_dev, cudaStream_t s)
+                                        const float2* train_dev, float avg_dpt, float* records_dev, cudaStream_t s,
+                                        const uint8_t* stale)
 {
   return with_sparse_code_size(code_size, [&](auto cs) {
     using Cfg = RepCfg<cs.value>;
@@ -474,7 +478,7 @@ cudaError_t launch_reprojection_records(int code_size, const ReprojItemDev* item
                                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
     if (e != cudaSuccess) return e;
     reprojection_records_kernel<cs.value><<<num_items, Cfg::NT, Cfg::SMEM, s>>>(items_dev, query_dev, train_dev, avg_dpt,
-                                                                               records_dev);
+                                                                               records_dev, stale);
     return cudaGetLastError();
   });
 }
@@ -490,7 +494,7 @@ cudaError_t launch_sparse_geometric_rows(int code_size, const GeoItemDev& item, 
 }
 
 cudaError_t launch_sparse_geometric_records(int code_size, const GeoItemDev* items_dev, int num_items, const int2* points_dev,
-                                            float avg_dpt, float* records_dev, cudaStream_t s)
+                                            float avg_dpt, float* records_dev, cudaStream_t s, const uint8_t* stale)
 {
   return with_sparse_code_size(code_size, [&](auto cs) {
     using Cfg = GeoCfg<cs.value>;
@@ -498,7 +502,8 @@ cudaError_t launch_sparse_geometric_records(int code_size, const GeoItemDev* ite
                                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
     if (e != cudaSuccess) return e;
     sparse_geometric_records_kernel<cs.value><<<dim3(num_items, Cfg::NS), Cfg::NT, Cfg::SMEM, s>>>(items_dev, points_dev,
-                                                                                                   avg_dpt, records_dev);
+                                                                                                   avg_dpt, records_dev,
+                                                                                                   stale);
     return cudaGetLastError();
   });
 }

@@ -11,7 +11,10 @@
 //   energy    one CTA: the window energy from the error outputs (each part summed sequentially in factor order, as
 //             window_error_sum does) or from the buffer's f, plus the prior terms and the code prior
 //   scatter   with an active subset (dfk_window_problem_set_active): the subset's records into their slots, zeros
-//             into the inactive items' slots
+//             into the inactive items' slots; with ISAM2's partial linearisation also "keep" for a valid record
+//   relin     ISAM2's relinearisation check: theta_lin (+) delta_key for every key whose delta reaches the threshold
+//   gather    a grown problem's kept records from the old problem's
+//   diag max  max |d| of a buffer's diagonal over the kept variables (ISAM2's fixed diag_eps = 1e-12 of it)
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -261,6 +264,7 @@ __global__ void __launch_bounds__(256) window_scatter_records_kernel(const float
                                                                      float* __restrict__ records)
 {
   const int s = src[blockIdx.x];
+  if (s == kKeepRecord) return;
   float* o = records + (size_t)blockIdx.x * rf;
   if (s < 0) {
     for (int k = threadIdx.x; k < rf; k += blockDim.x) o[k] = 0.0f;
@@ -270,7 +274,127 @@ __global__ void __launch_bounds__(256) window_scatter_records_kernel(const float
   for (int k = threadIdx.x; k < rf; k += blockDim.x) o[k] = in[k];
 }
 
+// one CTA per key (see launch_window_relinearize)
+constexpr int kRelinThreads = 128;
+__global__ void __launch_bounds__(kRelinThreads)
+window_relinearize_kernel(const double* __restrict__ in, double* __restrict__ out, const double* __restrict__ delta,
+                          int K, int F, int C, int check, double thr, int32_t* __restrict__ moved)
+{
+  __shared__ double red[kRelinThreads];
+  __shared__ int any_nan;
+  const int key = blockIdx.x, B = 6 + C;
+  const bool is_code = key < 2 * K && (key & 1);
+  const int slot = key < 2 * K ? key >> 1 : K + (key - 2 * K);  // pose slot (a keyframe or K + frame)
+  const double* d = key < 2 * K ? delta + (size_t)(key >> 1) * B + (is_code ? 6 : 0)
+                                : delta + (size_t)K * B + 6 * (size_t)(key - 2 * K);
+  const int n = is_code ? C : 6;
+  if (threadIdx.x == 0) any_nan = 0;
+  __syncthreads();
+  double m = 0.0;
+  for (int i = threadIdx.x; i < n; i += kRelinThreads) {
+    const double a = fabs(d[i]);
+    if (a != a) any_nan = 1;
+    m = fmax(m, a);
+  }
+  red[threadIdx.x] = m;
+  __syncthreads();
+  for (int s = kRelinThreads / 2; s > 0; s >>= 1) {
+    if (threadIdx.x < s) red[threadIdx.x] = fmax(red[threadIdx.x], red[threadIdx.x + s]);
+    __syncthreads();
+  }
+  // numpy's max propagates a NaN, and NaN >= threshold is false
+  const bool mv = check && !any_nan && red[0] >= thr;
+  if (is_code) {
+    const size_t c0 = (size_t)(K + F) * 7 + (size_t)(key >> 1) * C;
+    for (int c = threadIdx.x; c < C; c += kRelinThreads) out[c0 + c] = mv ? in[c0 + c] + d[c] : in[c0 + c];
+  } else if (threadIdx.x == 0) {
+    const double* p = in + (size_t)slot * 7;
+    double* o = out + (size_t)slot * 7;
+    if (mv) {  // window_retract_kernel's arithmetic
+      double e[4], q[4];
+      so3_exp(d + 3, e);
+      quat_mul_d(e, p, q);
+      const double nrm = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+      for (int k = 0; k < 4; ++k) o[k] = q[k] / nrm;
+      for (int k = 0; k < 3; ++k) o[4 + k] = p[4 + k] + d[k];
+    } else {
+      for (int k = 0; k < 7; ++k) o[k] = p[k];
+    }
+  }
+  if (threadIdx.x == 0) moved[key] = mv ? 1 : 0;
+}
+
+// one CTA per (new row, old row)
+__global__ void __launch_bounds__(256) window_gather_records_kernel(const float* __restrict__ src, float* __restrict__ dst,
+                                                                    const int2* __restrict__ map, int rf)
+{
+  const int2 m = map[blockIdx.x];
+  for (int k = threadIdx.x; k < rf; k += blockDim.x) dst[(size_t)m.x * rf + k] = src[(size_t)m.y * rf + k];
+}
+
+// one CTA (see launch_window_diag_max)
+constexpr int kDiagThreads = 256;
+__global__ void __launch_bounds__(kDiagThreads)
+window_diag_max_kernel(const float* __restrict__ buf, int K, int F, int C, size_t o_c, size_t o_f,
+                       const int2* __restrict__ self_pairs, int num_self, double w, int fixed, double* out)
+{
+  __shared__ double red[kDiagThreads];
+  const int B = 6 + C, n = K * B + 6 * F;
+  double m = 0.0;
+  for (int i = threadIdx.x; i < n; i += kDiagThreads) {
+    if (i < fixed) continue;
+    double d;
+    if (i < K * B) {
+      const int k = i / B, r = i - k * B;
+      d = (double)buf[(size_t)k * B * B + (size_t)r * B + r];
+      if (r < 6)
+        for (int s = 0; s < num_self; ++s)
+          if (self_pairs[s].y == k) {  // H += O, then H += O^T: the diagonal gets O(r, r) twice
+            const double o = (double)buf[o_c + (size_t)self_pairs[s].x * 6 * B + (size_t)r * 6 + r];
+            d = __dadd_rn(__dadd_rn(d, o), o);
+          }
+      if (r >= 6 && w > 0.0) d = __dadd_rn(d, w);
+    } else {
+      const int f = (i - K * B) / 6, r = i - K * B - 6 * f;
+      d = (double)buf[o_f + 36 * (size_t)f + 7 * (size_t)r];
+    }
+    m = fmax(m, fabs(d));
+  }
+  red[threadIdx.x] = m;
+  __syncthreads();
+  for (int s = kDiagThreads / 2; s > 0; s >>= 1) {
+    if (threadIdx.x < s) red[threadIdx.x] = fmax(red[threadIdx.x], red[threadIdx.x + s]);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *out = red[0];
+}
+
 }  // namespace
+
+cudaError_t launch_window_relinearize(const double* lin_in, double* lin_out, const double* delta, int K, int F, int C,
+                                      bool check, double threshold, int32_t* moved, cudaStream_t stream)
+{
+  window_relinearize_kernel<<<2 * K + F, kRelinThreads, 0, stream>>>(lin_in, lin_out, delta, K, F, C, check ? 1 : 0,
+                                                                     threshold, moved);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_gather_records(const float* src, float* dst, const int2* map, int n, int rf,
+                                         cudaStream_t stream)
+{
+  if (n == 0) return cudaSuccess;
+  window_gather_records_kernel<<<n, 256, 0, stream>>>(src, dst, map, rf);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_diag_max(const float* buf, int K, int F, int C, size_t coupling_off, size_t frame_off,
+                                   const int2* self_pairs, int num_self, double w, bool fix_first_pose, double* out,
+                                   cudaStream_t stream)
+{
+  window_diag_max_kernel<<<1, kDiagThreads, 0, stream>>>(buf, K, F, C, coupling_off, frame_off, self_pairs, num_self, w,
+                                                          fix_first_pose ? 6 : 0, out);
+  return cudaGetLastError();
+}
 
 cudaError_t launch_window_scatter_records(const float* sub, const int* src, int n, int rf, float* records,
                                           cudaStream_t stream)

@@ -933,7 +933,8 @@ cudaError_t ensure_incremental(WindowSolverDev* s)
 
 cudaError_t launch_window_solver_update(WindowSolverDev* s, const float* window_dev, double prior, double diag_eps,
                                         const double* codes_host, double* dx_dev, int32_t* info_dev,
-                                        cudaStream_t stream, uint64_t* launches, int* first_column)
+                                        cudaStream_t stream, uint64_t* launches, int* first_column,
+                                        bool codes_on_device)
 {
   const int reuse = s->reuse;
   s->reuse = 0;  // until this update completes
@@ -952,7 +953,8 @@ cudaError_t launch_window_solver_update(WindowSolverDev* s, const float* window_
   fa.frame_ptr = s->frame_ptr; fa.frame_list = s->frame_list; fa.frame_pair = s->frame_pair; fa.frame_kf = s->frame_kf;
   fa.frame_L = s->frame_L; fa.frame_bad = s->frame_bad;
   if (prior > 0.0) {
-    e = cudaMemcpyAsync(s->codes, codes_host, (size_t)s->K * s->C * sizeof(double), cudaMemcpyHostToDevice, stream);
+    e = cudaMemcpyAsync(s->codes, codes_host, (size_t)s->K * s->C * sizeof(double),
+                        codes_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream);
     if (e != cudaSuccess) return e;
   }
   const LoadedSet now = s->loaded[1 - s->cur], before = s->loaded[s->cur];

@@ -40,6 +40,7 @@ The host side (cache, retraction, damping schedule) is plain Python / numpy; not
 from __future__ import annotations
 
 import ctypes
+import dataclasses
 import functools
 from dataclasses import dataclass, field
 from typing import Callable, List, Optional, Sequence, Tuple
@@ -133,6 +134,7 @@ class OptimizeWork:
         self.active_level = len(iters) - 1
         self.first, self.remove, self.remove_after = True, False, remove_after
         self.factor: Optional[int] = None  # the level of the PhotometricFactor in the graph
+        self.erased = False  # mapping_steps: the work manager dropped it (finished at an update); its factor stays
 
     def is_new_level_start(self) -> bool:
         return self.active_level >= 0 and self.iters[self.active_level] == self.orig[self.active_level]
@@ -309,8 +311,13 @@ class LinearisationCache:
             self._at[p] = (poses[k0].copy(), self._pose1(poses, frame_poses, k1).copy(), codes[k0].copy(),
                            codes[k1].copy() if geo else None)
 
-    def invalidate(self):
-        self._at = [None] * (len(self.pairs) + len(self.geometric))
+    def invalidate(self, which: Optional[Sequence[int]] = None):
+        """forget the evaluation of the factors `which` (default: all)"""
+        if which is None:
+            self._at = [None] * (len(self.pairs) + len(self.geometric))
+        else:
+            for i in which:
+                self._at[i] = None
 
 
 def apply_update(poses: np.ndarray, codes: np.ndarray, dx: np.ndarray, code_size: int,
@@ -563,6 +570,140 @@ class IncrementalOptimizer:
         factor_of, frame_of = list(factor_of), list(frame_of)
         prob.carry_records(old, factor_of, frame_of)
         self.grow(prob.layout, prob.linearise, poses, codes, frame_poses, factor_of, frame_of, window=prob.window)
+
+
+def mapping_steps(opt: IncrementalOptimizer, prob, works: Sequence[OptimizeWork], max_steps: int,
+                  schedule: Optional[LevelSchedule] = None) -> Tuple[List[ISAM2Result], List[List[int]]]:
+    """Up to max_steps of the reference's mapping steps (Mapper::MappingStep, repeated by DeepFactors::ProcessFrame while
+    the work manager has work) with one OptimizeWork per pair of prob's level schedule: the host mirror of
+    dfk_window_map_steps.  Each step, in the reference's order:
+      1. bookkeeping of every work the manager still holds (WorkManager::Bookkeeping);
+      2. their update; a work that has finished is erased from the manager, its factor stays in the graph;
+      3. prob.set_active to the pairs' factor levels; a pair whose factor changed holds a new factor, so its cache
+         entry is invalidated and it is linearised at theta_lin;
+      4. opt.update();
+      5. signal_no_relinearize of every work the manager holds when nothing was relinearised.
+    It stops early once every work is erased.  schedule (default prob.level_schedule(works[0].orig)) gives the dense
+    items' pairs and levels; prob.dense_pairs() the cache index of every schedule pair.  The works are updated in
+    place, so a later call continues the run.  Returns every step's ISAM2Result and pair factor levels (-1: none)."""
+    sched = prob.level_schedule(works[0].orig) if schedule is None else schedule
+    ids = prob.dense_pairs()
+    results, levels = [], []
+    for _ in range(int(max_steps)):
+        if all(w.erased for w in works):
+            break
+        prev = [w.factor for w in works]
+        for w in works:
+            if not w.erased:
+                w.bookkeeping()
+        for w in works:
+            if not w.erased:
+                w.update()
+                w.erased = w.finished()
+        lvl = [-1 if w.factor is None else w.factor for w in works]
+        prob.set_active(*sched.masks(lvl))
+        opt.cache.invalidate([ids[q] for q, w in enumerate(works) if w.factor != prev[q]])
+        r = opt.update()
+        results.append(r)
+        levels.append(lvl)
+        if r.variables_relinearized == 0:
+            for w in works:
+                if not w.erased:
+                    w.signal_no_relinearize()
+    return results, levels
+
+
+class DeviceIncrementalOptimizer:
+    """IncrementalOptimizer on the device (dfk_window_problem_isam2_update on SfmWindowProblem.device_problem()):
+    theta_lin, the last delta and the estimate stay on the device, the stale items are found from the keys the check
+    moved, and only those are re-linearised.  The run starts from the device problem's state: pass poses / codes /
+    frame_poses to set it (any later set_state starts a new run).  update() returns IncrementalOptimizer.update's
+    ISAM2Result; estimate() reads theta_lin (+) delta back.  grow_problem moves the run onto a grown window
+    (dfk_window_problem_grow_from).  map_steps runs mapping_steps' loop as one call (dfk_window_map_steps).  A sharded
+    window (allreduce) cannot run here."""
+
+    def __init__(self, prob: "SfmWindowProblem", relinearize_threshold: float = 0.05, relinearize_skip: int = 1,
+                 code_prior_weight: float = 0.0, fix_first_pose: bool = True, poses=None, codes=None,
+                 frame_poses=None):
+        if relinearize_skip < 1:
+            raise ValueError("relinearize_skip must be >= 1")
+        self.prob, self.layout = prob, prob.layout
+        self.dev = prob.device_problem()
+        self.params = dict(relinearize_threshold=float(relinearize_threshold), relinearize_skip=int(relinearize_skip),
+                           code_prior_weight=float(code_prior_weight), fix_first_pose=bool(fix_first_pose))
+        if poses is not None:
+            frames = np.zeros((0, 7)) if frame_poses is None else np.asarray(frame_poses, np.float64).reshape(-1, 7)
+            if len(frames) != self.layout.num_frames:
+                raise ValueError(f"the window has {self.layout.num_frames} tracked frames: pass as many frame_poses")
+            self.dev.set_state(np.concatenate([np.asarray(poses, np.float64).reshape(-1, 7), frames]),
+                               np.asarray(codes, np.float64))
+
+    def update(self) -> ISAM2Result:
+        return ISAM2Result(*self.dev.isam2_update(**self.params))
+
+    def estimate(self):
+        """theta_lin (+) delta: (poses, codes, frame_poses)"""
+        p, c = self.dev.get_state()
+        K = self.layout.num_keyframes
+        return p[:K], c, p[K:]
+
+    def linearization(self):
+        """(theta_lin poses, theta_lin codes, theta_lin frame poses, delta) of the last update"""
+        p, c, d = self.dev.get_linearization()
+        K = self.layout.num_keyframes
+        return p[:K], c, p[K:], d
+
+    def grow_problem(self, old: "SfmWindowProblem", prob: "SfmWindowProblem", poses, codes,
+                     frame_poses: Optional[np.ndarray], factor_of: Sequence[Optional[int]],
+                     frame_of: Sequence[Optional[int]]):
+        """IncrementalOptimizer.grow_problem on the device (dfk_window_problem_grow_from): the run moves onto `prob`,
+        the window `old` grew into.  poses / codes / frame_poses: the new keyframes' and frames' initial estimates (the
+        kept ones keep theta_lin and delta); factor_of / frame_of as grow_problem takes them, turned into item maps"""
+        if old is not self.prob:
+            raise ValueError("grow_problem continues the run of the optimiser's own problem")
+        if len(factor_of) != len(prob.pairs) + len(prob.geometric) or len(frame_of) != len(prob.frames):
+            raise ValueError("factor_of needs one entry per factor and frame_of one per frame")
+        L = prob.levels
+
+        def kind_of(pr, i):
+            P, PF, NP = pr._num_photometric, pr._num_photometric + len(pr.links), len(pr.pairs)
+            return ("dense", i) if i < P else ("rep", i - P) if i < PF else ("frame", i - PF) if i < NP else \
+                ("geo", i - NP)
+        dense, rep, geo = [], [], []
+        order = list(range(prob._num_photometric)) + \
+            list(range(prob._num_photometric + len(prob.links), len(prob.pairs)))
+        for i in order:  # the dense items in record order: photometric pairs, then frame pairs
+            o = factor_of[i]
+            ok, oi = kind_of(old, o) if o is not None else (None, None)
+            kn = kind_of(prob, i)[0]
+            if o is not None and ok != kn:
+                raise ValueError(f"factor {i} ({kn}) is old factor {o} of another kind ({ok})")
+            base = None if o is None else (oi if ok == "dense" else old._num_photometric + oi) * L
+            dense += [-1 if base is None else base + l for l in range(L)]
+        for i in range(len(prob.pairs) + len(prob.geometric)):
+            kn, j = kind_of(prob, i)
+            if kn not in ("rep", "geo"):
+                continue
+            o = factor_of[i]
+            if o is not None and kind_of(old, o)[0] != kn:
+                raise ValueError(f"factor {i} ({kn}) is old factor {o} of another kind")
+            (rep if kn == "rep" else geo).append(-1 if o is None else kind_of(old, o)[1])
+        dev = prob.device_problem()
+        K = prob.layout.num_keyframes
+        fr = np.zeros((0, 7)) if frame_poses is None else np.asarray(frame_poses, np.float64).reshape(-1, 7)
+        dev.set_state(np.concatenate([np.asarray(poses, np.float64).reshape(K, 7), fr]), np.asarray(codes, np.float64))
+        dev.grow_from(self.dev, dense, rep, geo, [-1 if o is None else o for o in frame_of])
+        self.prob, self.layout, self.dev = prob, prob.layout, dev
+
+    def map_steps(self, works: Sequence[OptimizeWork], max_steps: int, schedule: Optional[LevelSchedule] = None
+                  ) -> Tuple[List[ISAM2Result], List[List[int]]]:
+        """mapping_steps(opt, prob, works, max_steps, schedule) on the device: the works are updated in place"""
+        sched = self.prob.level_schedule(works[0].orig) if schedule is None else schedule
+        sched = dataclasses.replace(sched, remove_after=[w.remove_after for w in works])
+        t = self.dev.map_steps(sched, list(works), max_steps, **self.params)
+        res = [ISAM2Result(*v) for v in zip(t["variables_relinearized"], t["variables_reeliminated"],
+                                            t["factors_relinearised"], t["first_column"])]
+        return res, t["pair_levels"]
 
 
 class WindowOptimizer:
@@ -1171,6 +1312,12 @@ class SfmWindowProblem:
         if error_mask is not None and not np.array_equal(np.asarray(error_mask, dtype=bool).ravel(), m):
             raise ValueError("the error items are the dense items' twins: their mask is the dense mask")
         self._active = None if m is None or m.all() else m
+
+    def dense_pairs(self) -> List[int]:
+        """the cache index (linearise's `todo` numbering) of every pair of level_schedule: the photometric pairs, then
+        the frame pairs"""
+        P, PF = self._num_photometric, self._num_photometric + len(self.links)
+        return list(range(P)) + list(range(PF, len(self.pairs)))
 
     def level_schedule(self, iters, steps_done=None, remove_after=None) -> LevelSchedule:
         """The LevelSchedule of this window's photometric and frame pairs with pho_iters = iters: item (pair, l) has

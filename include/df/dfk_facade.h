@@ -567,6 +567,20 @@ struct LevelSchedule {
   std::vector<int32_t> iters, dense_level, error_pair, error_level, pair_steps_done;
   std::vector<uint8_t> pair_remove_after;
 };
+struct Isam2Params {  // window_opt.IncrementalOptimizer's parameters (dfk_window_problem_isam2_update)
+  double relinearize_threshold = 0.05;
+  int relinearize_skip = 1;
+  double code_prior_weight = 0.0;
+  bool fix_first_pose = true;
+};
+struct Isam2Result {  // gtsam::ISAM2Result's counts
+  int variables_relinearized = 0, variables_reeliminated = 0, factors_relinearised = 0, first_column = 0;
+  bool operator==(const Isam2Result& o) const
+  {
+    return variables_relinearized == o.variables_relinearized && variables_reeliminated == o.variables_reeliminated &&
+           factors_relinearised == o.factors_relinearised && first_column == o.first_column;
+  }
+};
 
 struct LevelTrace {  // DfkLevelTrace
   std::vector<double> switch_energy;
@@ -693,7 +707,78 @@ public:
     return r;
   }
 
+  // one ISAM2 update (dfk_window_problem_isam2_update): the state becomes theta_lin (+) delta; synchronous
+  Isam2Result UpdateIncremental(const Isam2Params& p)
+  {
+    const DfkIsam2Params c = params(p);
+    DfkIsam2Result r{};
+    detail::Check(h_, dfk_window_problem_isam2_update(h_, p_, &c, &r));
+    return Isam2Result{r.variables_relinearized, r.variables_reeliminated, r.factors_relinearised, r.first_column};
+  }
+  // theta_lin ((K + F) x 7, K x CS) and delta (K (6 + CS) + 6 F) of the last update, host
+  void GetLinearization(std::vector<double>& poses, std::vector<double>& codes, std::vector<double>& delta) const
+  {
+    poses.resize((size_t)(K_ + F_) * 7);
+    codes.resize((size_t)K_ * CS);
+    delta.resize((size_t)K_ * (6 + CS) + 6 * (size_t)F_);
+    detail::Check(h_, dfk_window_problem_get_linearization(h_, p_, poses.data(), codes.data(), delta.data()));
+    detail::Check(h_, dfk_synchronize(h_));
+  }
+  // up to max_steps mapping steps (dfk_window_map_steps) with the works of s's pairs (read and written; empty: fresh
+  // works); per step the ISAM2 counts, and in pair_levels every pair's factor level
+  std::vector<Isam2Result> MappingSteps(const Isam2Params& p, const LevelSchedule& s, std::vector<DfkWorkState>& works,
+                                        int max_steps, std::vector<std::vector<int>>* pair_levels = nullptr)
+  {
+    const size_t P = s.pair_remove_after.size();
+    if (max_steps < 0 || s.iters.empty() || s.dense_level.size() != (size_t)nd_ ||
+        (!s.error_pair.empty() && s.error_pair.size() != (size_t)ne_) ||
+        (!s.error_level.empty() && s.error_level.size() != (size_t)ne_) || (!works.empty() && works.size() != P))
+      throw std::invalid_argument("[WindowProblem::MappingSteps] schedule or works of the wrong length");
+    const DfkIsam2Params c = params(p);
+    const DfkLevelSchedule cs{(int32_t)s.iters.size(), s.iters.data(), s.dense_level.data(),
+                              s.error_pair.empty() ? nullptr : s.error_pair.data(),
+                              s.error_level.empty() ? nullptr : s.error_level.data(), (int32_t)P, nullptr,
+                              P ? s.pair_remove_after.data() : nullptr};
+    if (s.iters.size() > DFK_MAX_WORK_LEVELS)
+      throw std::invalid_argument("[WindowProblem::MappingSteps] more than DFK_MAX_WORK_LEVELS levels");
+    if (works.empty()) {  // fresh works: OptimizeWork's constructor
+      DfkWorkState f{};
+      f.active_level = (int32_t)s.iters.size() - 1;
+      for (size_t l = 0; l < s.iters.size(); ++l) f.iters[l] = s.iters[l];
+      f.first = 1;
+      f.factor = -1;
+      works.assign(P, f);
+    }
+    std::vector<DfkWorkState> w(works);
+    w.resize(std::max<size_t>(P, 1));
+    const size_t n = std::max(max_steps, 1);
+    std::vector<int32_t> a(n), b(n), f(n), j(n), lv(n * std::max<size_t>(P, 1));
+    DfkMapTrace t{a.data(), b.data(), f.data(), j.data(), lv.data(), 0};
+    detail::Check(h_, dfk_window_map_steps(h_, p_, &c, &cs, w.data(), max_steps, &t));
+    std::vector<Isam2Result> r;
+    for (int i = 0; i < t.num_steps; ++i) r.push_back(Isam2Result{a[i], b[i], f[i], j[i]});
+    if (pair_levels) {
+      pair_levels->clear();
+      for (int i = 0; i < t.num_steps; ++i) pair_levels->emplace_back(lv.begin() + i * P, lv.begin() + (i + 1) * P);
+    }
+    std::copy(w.begin(), w.begin() + P, works.begin());
+    return r;
+  }
+  // continue old's ISAM2 run on this grown problem (dfk_window_problem_grow_from); set this problem's state first
+  void GrowFrom(const WindowProblem& old, const std::vector<int32_t>& dense_of, const std::vector<int32_t>& rep_of,
+                const std::vector<int32_t>& geo_of, const std::vector<int32_t>& frame_of)
+  {
+    if (dense_of.size() != (size_t)nd_ || frame_of.size() != (size_t)F_)
+      throw std::invalid_argument("[WindowProblem::GrowFrom] one map entry per dense item and per frame");
+    detail::Check(h_, dfk_window_problem_grow_from(h_, p_, old.p_, dense_of.data(), rep_of.data(), geo_of.data(),
+                                                   frame_of.data()));
+  }
+
 private:
+  static DfkIsam2Params params(const Isam2Params& p)
+  {
+    return DfkIsam2Params{p.relinearize_threshold, p.relinearize_skip, p.code_prior_weight, p.fix_first_pose ? 1 : 0};
+  }
   DfkHandle h_;
   int K_, F_, nd_, ne_;
   DfkWindowProblem* p_ = nullptr;

@@ -1383,6 +1383,123 @@ typedef struct {
 DfkStatus dfk_window_lm_levels(DfkHandle h, DfkWindowProblem* p, const DfkLMParams* params,
                                const DfkLevelSchedule* schedule, DfkLMTrace* trace, DfkLevelTrace* level_trace);
 
+/* ------------------------------------------------------------------ ISAM2 mapping steps on the window problem */
+
+/* The mapper's back end as the reference runs it (Mapper::MappingStep: one ISAM2::update with force_relinearize, then
+ * calculateEstimate), on the window problem: window_opt.IncrementalOptimizer's rule with the state on the device.
+ * The problem holds, on the device, theta_lin (poses (K + F) x 7, codes K x C, fp64), the last full delta Delta (the
+ * solve's layout, K (6 + C) + 6 F doubles) and, on the host, one "linearised at theta_lin" flag per dense item,
+ * reprojection link, geometric link and depth-prior item.  The first update after create or set_state starts from
+ * the state: theta_lin = state, Delta = 0, nothing linearised, the update count and diag_eps reset.
+ * dfk_window_problem_linearize, dfk_window_lm and dfk_window_lm_levels rewrite the records, so they clear every flag;
+ * set_depth_priors clears the depth priors'; set_active clears the flag of every dense item it switches on or off (its
+ * record is then zeros, or a record of another linearisation), so the next update re-evaluates it. */
+typedef struct {
+  double relinearize_threshold; /* a number: a key with max |Delta_key| >= it is relinearised (the reference's 0.05f is
+                                   0.0500000007 as a double) */
+  int32_t relinearize_skip;     /* >= 1: the check runs on every relinearize_skip-th update (1 = force_relinearize) */
+  double code_prior_weight;     /* >= 0, finite: w I on every code block and -w c_lin on its gradient */
+  int32_t fix_first_pose;       /* 1: variables 0..5 (keyframe 0's pose) are held */
+} DfkIsam2Params;
+/* gtsam::ISAM2Result's counts, as IncrementalOptimizer.update returns them */
+typedef struct {
+  int32_t variables_relinearized;  /* keys moved by the check (pose and code of a keyframe count apart) */
+  int32_t variables_reeliminated;  /* (K - first_column) (6 + C) + 6 F */
+  int32_t factors_relinearised;    /* factors re-evaluated: photometric and frame pairs, reprojection and geometric links */
+  int32_t first_column;            /* the solver's first re-factorised keyframe column (K: none) */
+} DfkIsam2Result;
+/* One IncrementalOptimizer.update(), in GTSAM's order:
+ *   1. on every relinearize_skip-th update, the relinearisation check over the keys -- the pose and the code of each
+ *      keyframe, then each frame's pose -- in one launch: a key with max |Delta_key| >= threshold moves to
+ *      theta_lin (+) Delta_key (poses: dfk_window_problem_retract's fp64 arithmetic; codes: addition);
+ *   2. the stale items: an item is stale when it was never linearised at theta_lin or a key it reads (its
+ *      DfkWindowItemSlots) moved; a depth-prior item when its keyframe's code moved;
+ *   3. the stale items linearised at theta_lin: one RunStep launch over the stale active dense items in record order,
+ *      planned over exactly those (the items and order SfmWindowProblem.linearise hands RunStepBatch for the same
+ *      stale factors); an active item that is not stale keeps its record, an inactive one gets zeros.  The reprojection,
+ *      geometric and depth-prior batches run over every item and skip the ones that are not stale.  Then the assembly,
+ *      the frame and keyframe priors with their deltas Local(x0, theta_lin) and the depth priors, in
+ *      dfk_window_problem_linearize's order;
+ *   4. diag_eps: on the first update 1e-12 max |d| of that buffer's diagonal over the kept variables with the code
+ *      prior (window_opt.diag_eps_of), computed on the device and read back once; fixed after that;
+ *   5. dfk_window_solver_update of the buffer, with theta_lin's codes for the code prior: Delta;
+ *   6. the problem's state = theta_lin (+) Delta (dfk_window_problem_retract's arithmetic, on the device).
+ * Host synchronisations: the moved flags after step 1 (the host plans the dense subset from them), the solver's own
+ * read-back of first_column, and the solve's info; on the first update also the diagonal maximum.  A failed pivot
+ * returns DFK_ERR_INVALID_ARG with the info dfk_window_solve would report (1 + the variable) in the message (the
+ * system at theta_lin is not positive definite); theta_lin and
+ * Delta then stay as they were, the state is not written and the re-evaluated items count as not linearised.
+ * A problem built for sharded pairs cannot run this (the all-reduce is the caller's).  A rejected call writes
+ * nothing.  Synchronous. */
+DfkStatus dfk_window_problem_isam2_update(DfkHandle h, DfkWindowProblem* p, const DfkIsam2Params* params,
+                                          DfkIsam2Result* result);
+/* theta_lin ((K + F) x 7 poses, K x C codes) and Delta (K (6 + C) + 6 F) of the last update, host or device memory;
+ * any may be NULL.  Before the first update: the state and zeros.  Asynchronous on the handle's stream. */
+DfkStatus dfk_window_problem_get_linearization(DfkHandle h, const DfkWindowProblem* p, double* lin_poses,
+                                               double* lin_codes, double* delta);
+
+/* Growth of the map (IncrementalOptimizer.grow_problem on the device): p_new is the window p_old grew into --
+ * keyframes appended in index order, new pairs, links and frames; no slide -- and continues p_old's ISAM2 run.  Each
+ * map sends an item of p_new to its item in p_old, or -1 for a new one: dense_of [p_new's num_dense], rep_of
+ * [num_reproj], geo_of [num_geo], frame_of [F_new] (old frame or -1).  HOST arrays; NULL only where the count is 0.
+ * On the handle's stream, without a synchronisation:
+ *   - the kept items' records are copied from p_old's record buffers into p_new's (one gather launch per buffer);
+ *   - theta_lin and Delta of the old keyframes and of the kept frames are copied; the new keyframes and frames start at
+ *     p_new's state (set it first) with Delta = 0;
+ *   - a kept item keeps its "linearised" flag; new items and every depth-prior item of p_new are stale;
+ *   - p_new's solvers become dfk_window_solver_create_from(p_old's), so the next update re-factorises from the first
+ *     changed column; the update count and diag_eps carry over.
+ * Checks (a rejected call writes nothing): dfk_window_solver_create_from's (same code size, p_old's keyframes first,
+ * the same fixed variables), p_old has had an update, the maps name distinct old items, and a kept item reads the
+ * keys its old item read (keyframes keep their index, a frame maps by frame_of) and has its old item's size: the
+ * dense item's level (image size and camera), a link's number of matches or points. */
+DfkStatus dfk_window_problem_grow_from(DfkHandle h, DfkWindowProblem* p_new, const DfkWindowProblem* p_old,
+                                       const int32_t* dense_of, const int32_t* rep_of, const int32_t* geo_of,
+                                       const int32_t* frame_of);
+
+/* One pair's coarse-to-fine work (window_opt.OptimizeWork, df_work.cpp:100-190): the counters of every level
+ * (iters[l] counts down from pho_iters[l]), the active level (num_levels - 1 .. -2), first / remove, the level of the
+ * factor the pair holds in the graph (-1: none), and erased: the work manager has dropped the work (it finished at an
+ * update), so it takes no more steps, while its factor stays in the graph. */
+#define DFK_MAX_WORK_LEVELS 8
+typedef struct {
+  int32_t active_level;
+  int32_t iters[DFK_MAX_WORK_LEVELS];
+  int32_t first, remove;
+  int32_t factor;
+  int32_t erased;
+} DfkWorkState;
+/* Per mapping step, the caller's HOST arrays (any may be NULL): DfkIsam2Result's four counts [max_steps] each, and
+ * every pair's factor level [max_steps x num_pairs] (-1: none).  num_steps (out): the steps taken. */
+typedef struct {
+  int32_t* variables_relinearized;
+  int32_t* variables_reeliminated;
+  int32_t* factors_relinearised;
+  int32_t* first_column;
+  int32_t* pair_levels;
+  int32_t num_steps;
+} DfkMapTrace;
+/* Up to max_steps mapping steps (Mapper::MappingStep, repeated by DeepFactors::ProcessFrame while the work manager has
+ * work) with one OptimizeWork per pair of the schedule.  The schedule gives iters (pho_iters, at most
+ * DFK_MAX_WORK_LEVELS levels), the dense items' levels (the pairs as dfk_window_lm_levels takes them), error_pair /
+ * error_level for the error items, and pair_remove_after; pair_steps_done is ignored.  works: num_pairs entries, read
+ * and written (the end state, so that a later call -- also one on a grown problem whose pairs the caller renumbered --
+ * continues the run); NULL starts every pair fresh.  Each step, in the reference's order:
+ *   1. bookkeeping of every work not erased (a factor at the level start; removed after remove_after);
+ *   2. update of every work not erased; a work that has finished is erased;
+ *   3. the masks of the pairs' factors (dfk_window_problem_set_active); the items of a pair whose factor level changed
+ *      become stale (a new factor is linearised at theta_lin);
+ *   4. dfk_window_problem_isam2_update;
+ *   5. signal_no_relinearize of every work not erased when nothing was relinearised.
+ * The run stops early when every work is erased (WorkManager is empty).  The rule is dfk_works.h's, not dfk_levels.h's:
+ * a signal lowers the active level without resetting counters, a remove_after pair signalled at level 0 keeps its
+ * factor one more step, and bookkeeping runs before the update.  The reprojection and geometric links stay active.
+ * When a step's update fails (a failed pivot), the call returns its error after writing the works and trace of the
+ * steps before it, which stand.  Synchronous; a rejected call writes nothing. */
+DfkStatus dfk_window_map_steps(DfkHandle h, DfkWindowProblem* p, const DfkIsam2Params* params,
+                               const DfkLevelSchedule* schedule, DfkWorkState* works, int max_steps,
+                               DfkMapTrace* trace);
+
 #ifdef __cplusplus
 }
 #endif
