@@ -122,13 +122,19 @@ __device__ __forceinline__ float2 table_ray(const SfmItem<MAXCODE>& I, uint32_t 
 
 // The per-pixel row of the reduced system for pixel (x, y) with ray = table_ray(I, x, y), depth d and img0 value i0:
 // exact-order validity chain; for a valid pixel valid0 = 1 and feat = w * [e | a0..a5 | diff].  Returns the validity;
-// feat is left alone for an invalid pixel.
+// feat is left alone for an invalid pixel.  It is the two halves below: pixel_warp, which needs no gather, and
+// valid_pixel_row; a kernel may run them apart, to issue loads that depend on the validity before the gathers.
 template <int MAXCODE>
-__device__ __forceinline__ bool pixel_row(const SfmItem<MAXCODE>& I, uint32_t x, uint32_t y, float2 ray, float d,
-                                          float i0, bool grad_aligned8, float (&feat)[8])
+__device__ __forceinline__ Warped pixel_warp(const SfmItem<MAXCODE>& I, float2 ray, float d)
 {
-  const Warped w = warp_ray(ray.x, ray.y, d, I.q, I.t, I.fx, I.fy, I.u0, I.v0, I.border, I.ulim, I.vlim, I.min_dpt);
-  if (!w.valid) return false;
+  return warp_ray(ray.x, ray.y, d, I.q, I.t, I.fx, I.fy, I.u0, I.v0, I.border, I.ulim, I.vlim, I.min_dpt);
+}
+
+// the row of a pixel whose warp w = pixel_warp(I, ray, d) is valid
+template <int MAXCODE>
+__device__ __forceinline__ void valid_pixel_row(const SfmItem<MAXCODE>& I, uint32_t x, uint32_t y, const Warped& w,
+                                                float d, float i0, bool grad_aligned8, float (&feat)[8])
+{
   I.valid0[(size_t)y * I.valid0_pitch + x] = 1.0f;  // dense_sfm.h:161
   int ix, iy;
   float fu, fv, gx, gy;
@@ -148,6 +154,15 @@ __device__ __forceinline__ bool pixel_row(const SfmItem<MAXCODE>& I, uint32_t x,
 #pragma unroll
   for (int f = 0; f < 6; ++f) feat[1 + f] = hw * a[f];
   feat[7] = hw * diff;
+}
+
+template <int MAXCODE>
+__device__ __forceinline__ bool pixel_row(const SfmItem<MAXCODE>& I, uint32_t x, uint32_t y, float2 ray, float d,
+                                          float i0, bool grad_aligned8, float (&feat)[8])
+{
+  const Warped w = pixel_warp(I, ray, d);
+  if (!w.valid) return false;
+  valid_pixel_row(I, x, y, w, d, i0, grad_aligned8, feat);
   return true;
 }
 

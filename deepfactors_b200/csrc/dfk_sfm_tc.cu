@@ -22,10 +22,12 @@
 //   warpgroup, two M-tiles, 88 floats per thread, two CTAs per SM; C = 128: two warpgroups, two M-tiles each, 152
 //   floats per thread, one CTA per SM).  Warp w runs the per-pixel front-end ((optional depth decode,) exact-order
 //   validity chain, bilinear gathers, Jacobian row, Huber -> s = w*e, w*a[6], w*diff) for the PW = 32 / NWG pixels
-//   PW w .. PW w + PW - 1 (lane < PW: its own pixel), then the warp reads those pixels' code-Jacobian rows straight from
-//   global memory, coalesced (lane = 16-byte chunk lane & 7 of a 32-feature block of pixel 4i + lane / 8), scales them
-//   by the pixel's s (one shuffle), splits them into h / l and stores them K-major; each lane < PW adds its own pixel's
-//   7 pose / residual values.  Invalid pixels contribute exact zeros, and a tile with no valid pixel issues no MMA.
+//   PW w .. PW w + PW - 1 (lane < PW: its own pixel), and the warp reads the valid pixels' code-Jacobian rows straight
+//   from global memory, coalesced (lane = 16-byte chunk lane & 7 of a 32-feature block of pixel 4i + lane / 8): at
+//   C = 32 right after the validity chain and the ballot, so that they load while the gathers run; at C = 64 and 128
+//   after the Huber weight.  Then it scales them by the pixel's s (one shuffle), splits them into h / l and stores them
+//   K-major; each lane < PW adds its own pixel's 7 pose / residual values.  Invalid pixels contribute exact zeros, and
+//   a tile with no valid pixel issues no MMA.
 //   After one CTA barrier every warpgroup issues 16 k-steps x MT M-tiles of wgmma.m64nNk8 and, without waiting, goes on
 //   with the next tile's gathers; it waits for its MMAs only before the operand buffer is overwritten (with two
 //   warpgroups, a CTA barrier after the wait keeps one warpgroup from overwriting what the other still reads).
@@ -183,6 +185,9 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_tiles, float* _
   // quads whose code rows are loaded before the wait for the MMAs: all of them at C = 32 and 64; none at C = 128, where
   // the 152 accumulators leave registers for one quad at a time (each quad is loaded, then stored, after the wait)
   constexpr int PRE = C >= 128 ? 0 : NQ;
+  // C = 32 issues the code rows between the validity chain and the gathers (DESIGN §4.1); C = 64 and 128, whose 88 / 152
+  // accumulators already take them to 255 registers, issue them after the Huber weight
+  constexpr bool EARLY_ROWS = C == 32;
   constexpr int S = T::S;
   constexpr int F = T::F;
   constexpr bool kRawD = sfm_tc_writes_d(C);
@@ -331,12 +336,15 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_tiles, float* _
     }
     const float* __restrict__ jac = I.jac;
     const uint32_t joff = py * I.jac_pitch + pxx * C;  // this lane's pixel's code-Jacobian row (floats)
-    float feat[8];
+    // the per-pixel row in its two halves (dfk_sfm_frontend.cuh): the validity first, then the gathers, Jacobian and
+    // Huber of the valid pixels
+    Warped w;
+    float d = 0.0f, i0 = 0.0f;
     bool ok = false;
     if (blk_live) {
       const float2 ray = table_ray(I, pxx, py);  // issued before the decode: its latency hides behind it
-      float d = ld_stream(I.dpt0 + (size_t)py * I.dpt0_pitch + pxx);
-      const float i0 = ld_stream(I.img0 + (size_t)py * I.img0_pitch + pxx);
+      d = ld_stream(I.dpt0 + (size_t)py * I.dpt0_pitch + pxx);
+      i0 = ld_stream(I.img0 + (size_t)py * I.img0_pitch + pxx);
       if (fused) {
         // dpt0 is prx_orig: decode the depth from the pixel's code-Jacobian row with the arithmetic of
         // update_depth_kernel's vector body, here across the 8 lanes (and the NCB registers) that hold the chunks of
@@ -365,11 +373,10 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_tiles, float* _
         d = prx_to_depth(__fadd_rn(d, mine), I.avg_dpt);
         if (inb) I.dpt_out[(size_t)py * I.dpt_out_pitch + pxx] = d;
       }
-      if (inb) ok = pixel_row(I, pxx, py, ray, d, i0, true, feat);  // the API guarantees 8-byte grad1 rows here
-    }
-    if (!ok) {
-#pragma unroll
-      for (int f = 0; f < 8; ++f) feat[f] = 0.0f;
+      if (inb) {
+        w = pixel_warp(I, ray, d);
+        ok = w.valid;
+      }
     }
     const unsigned bal = __ballot_sync(0xffffffffu, ok);
     float4 v[NQ][NCB];
@@ -383,8 +390,22 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_tiles, float* _
         if (live) v[i4][cb] = load_chunk(jc + offk + 32 * cb, a16);
       }
     };
+    // EARLY_ROWS: the valid pixels' code rows are issued as soon as the ballot is known, and load while the gathers run
+    if constexpr (EARLY_ROWS) {
 #pragma unroll
-    for (int i4 = 0; i4 < PRE; ++i4) load_quad(i4);
+      for (int i4 = 0; i4 < PRE; ++i4) load_quad(i4);
+    }
+    float feat[8];
+    if (ok) {
+      valid_pixel_row(I, pxx, py, w, d, i0, true, feat);  // the API guarantees 8-byte grad1 rows here
+    } else {
+#pragma unroll
+      for (int f = 0; f < 8; ++f) feat[f] = 0.0f;
+    }
+    if constexpr (!EARLY_ROWS) {
+#pragma unroll
+      for (int i4 = 0; i4 < PRE; ++i4) load_quad(i4);
+    }
     // ---- the operand buffer is free once every warpgroup's MMAs of the previous tile have completed -------------------
     wgmma_wait_all();
     if constexpr (W::NWG > 1) __syncthreads();
