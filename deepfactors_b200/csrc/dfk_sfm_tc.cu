@@ -27,7 +27,8 @@
 //   C = 32 right after the validity chain and the ballot, so that they load while the gathers run; at C = 64 and 128
 //   after the Huber weight.  Then it scales them by the pixel's s (one shuffle), splits them into h / l and stores them
 //   K-major; each lane < PW adds its own pixel's 7 pose / residual values.  Invalid pixels contribute exact zeros, and
-//   a tile with no valid pixel issues no MMA.
+//   a tile with no valid pixel issues no MMA; at C = 32 it stops right after the validity chain (one CTA barrier that
+//   counts the tile's valid pixels), before the code rows, the gathers and the operand stores.
 //   After one CTA barrier every warpgroup issues 16 k-steps x MT M-tiles of wgmma.m64nNk8 and, without waiting, goes on
 //   with the next tile's gathers; it waits for its MMAs only before the operand buffer is overwritten (with two
 //   warpgroups, a CTA barrier after the wait keeps one warpgroup from overwriting what the other still reads).
@@ -376,6 +377,15 @@ sfm_step_tc_kernel(const SfmItemDev* __restrict__ items, int num_tiles, float* _
       if (inb) {
         w = pixel_warp(I, ray, d);
         ok = w.valid;
+      }
+    }
+    // C = 32: a tile without a valid pixel (about a third of them at the reference poses) ends here, once every warp knows
+    // its validity: no code rows, gathers, operand stores or MMAs, and no wait for the previous tile's MMAs.  Its chain
+    // bookkeeping is the same as if it had run (it counts towards the flush), so the sums are bitwise the same
+    if constexpr (C == 32) {
+      if (__syncthreads_count(ok) == 0) {
+        ++tiles_in_chain;
+        continue;
       }
     }
     const unsigned bal = __ballot_sync(0xffffffffu, ok);
